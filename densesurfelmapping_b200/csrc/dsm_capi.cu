@@ -36,99 +36,17 @@ extern "C" const char *dsm_strerror(int code)
 
 extern "C" const char *dsm_last_error(const dsm_ctx *ctx) { return ctx ? ctx->err : "null context"; }
 extern "C" const char *dsm_kernel_name(int id) { return (id >= 0 && id < DSM_NUM_KERNELS) ? kKernelNames[id] : "?"; }
-extern "C" int dsm_num_seeds(const dsm_ctx *ctx) { return ctx ? ctx->S : DSM_E_INVALID; }
-
-template <typename T>
-static cudaError_t dmalloc(T **p, size_t n)
-{
-    cudaError_t e = cudaMalloc((void **)p, n * sizeof(T));
-    if (e == cudaSuccess) e = cudaMemset(*p, 0, n * sizeof(T));
-    return e;
-}
+extern "C" int dsm_num_seeds(const dsm_ctx *ctx) { return ctx ? ctx->d.S : DSM_E_INVALID; }
 
 extern "C" void dsm_destroy(dsm_ctx *ctx)
 {
     if (!ctx) return;
     cudaSetDevice(ctx->device);
     dsm_comm_destroy(ctx);
-    // an asynchronous batch may still be in flight on any of the context's streams
-    if (ctx->s_h2d) cudaStreamSynchronize(ctx->s_h2d);
-    for (int i = 0; i < 4; i++)
-        if (ctx->s_comp[i]) cudaStreamSynchronize(ctx->s_comp[i]);
-    if (ctx->s_hi) cudaStreamSynchronize(ctx->s_hi);
-    if (ctx->s_d2h) cudaStreamSynchronize(ctx->s_d2h);
+    // an asynchronous batch may still be in flight on any of the context's streams: drain them before the buffers go
+    for (auto &s : ctx->own.streams) cudaStreamSynchronize(s.get());
     if (ctx->stream) cudaStreamSynchronize(ctx->stream);
-    for (auto &r : ctx->prof_pending)
-    {
-        cudaEventDestroy(r.e0);
-        cudaEventDestroy(r.e1);
-    }
-    for (auto &e : ctx->ev_free) cudaEventDestroy(e);
-    for (auto &g : ctx->graphs) cudaGraphExecDestroy(g.exec);
-    DsmDev &d = ctx->d;
-    cudaFree(ctx->gray);
-    cudaFree(ctx->depth);
-    cudaFree(d.labels);
-    cudaFree(d.seed);
-    cudaFree(d.inv_md);
-    cudaFree(d.invd);
-    cudaFree(d.code);
-    cudaFree(d.seed_hl);
-    cudaFree(d.done);
-    cudaFree(d.hardq);
-    cudaFree(d.nhard);
-    cudaFree(d.hrec);
-    cudaFree(d.tstable);
-    cudaFree(d.usum);
-    cudaFree(d.und);
-    cudaFree(d.dlist);
-    cudaFree(d.errflag);
-    cudaFree(d.qlist);
-    cudaFree(d.pfsum);
-    cudaFree(d.plane);
-    cudaFree(d.fused);
-    cudaFree(d.list);
-    cudaFree(d.nlist);
-    cudaFree(d.pool);
-    cudaFree(ctx->pool_snap);
-    cudaFree(ctx->poolofs);
-    cudaFree(d.newsurf);
-    cudaFree(d.nnew);
-    cudaFree(ctx->pose);
-    cudaFree(ctx->ipose);
-    cudaFree(ctx->refidx);
-    cudaFree(ctx->seed_export);
-    cudaFree(ctx->kx);
-    cudaFree(ctx->ky);
-    cudaFree(ctx->gray_packed);
-    cudaFree(ctx->blkcnt);
-    cudaFree(ctx->blkofs);
-    cudaFree(ctx->newofs);
-    cudaFree(ctx->wmat);
-    cudaFree(ctx->inact);
-    cudaFree(ctx->inact_ofs);
-    cudaFree(ctx->res_ofs);
-    cudaFree(ctx->depth_packed);
-    if (ctx->s_h2d) cudaStreamDestroy(ctx->s_h2d);
-    if (ctx->s_d2h) cudaStreamDestroy(ctx->s_d2h);
-    for (int i = 0; i < 4; i++)
-        if (ctx->s_comp[i]) cudaStreamDestroy(ctx->s_comp[i]);
-    if (ctx->s_hi) cudaStreamDestroy(ctx->s_hi);
-    if (ctx->ev_p2) cudaEventDestroy(ctx->ev_p2);
-    for (int i = 0; i < 8; i++)
-    {
-        if (ctx->ev_h2d[i]) cudaEventDestroy(ctx->ev_h2d[i]);
-        if (ctx->ev_done[i]) cudaEventDestroy(ctx->ev_done[i]);
-    }
-    if (ctx->ev_start) cudaEventDestroy(ctx->ev_start);
-    if (ctx->ev_fork) cudaEventDestroy(ctx->ev_fork);
-    for (int i = 0; i < 4; i++)
-        if (ctx->ev_join[i]) cudaEventDestroy(ctx->ev_join[i]);
-    cudaFreeHost(ctx->h_pose);
-    cudaFreeHost(ctx->h_ofs);
-    cudaFreeHost(ctx->h_ref);
-    if (ctx->own_stream && ctx->stream) cudaStreamDestroy(ctx->stream);
-    delete ctx;
+    delete ctx; // releases every buffer, stream, event and captured graph the context owns
 }
 
 // TMA descriptors for the tile kernels: each per-pixel array as a [B][H][Wp] tensor, box = one 8x4-seed tile plus
@@ -208,45 +126,14 @@ extern "C" int dsm_create(const dsm_params *params, int device, void *cuda_strea
 
     dsm_ctx *ctx = new (std::nothrow) dsm_ctx();
     if (!ctx) return DSM_E_NOMEM;
-    memset(&ctx->d, 0, sizeof(ctx->d));
     ctx->p = *params;
-    ctx->comm = nullptr;
     ctx->device = device;
-    ctx->err[0] = 0;
-    ctx->prof_mask = 0;
-    memset(ctx->prof_ms, 0, sizeof(ctx->prof_ms));
-    memset(ctx->prof_n, 0, sizeof(ctx->prof_n));
-    ctx->nb = 0;
-    ctx->n_pool = 0;
-    ctx->uploaded = ctx->ran = false;
-    ctx->in_flight = false;
-    ctx->stop_after = 0;
     {
         const char *e = getenv("DSM_GRAPHS");
         ctx->use_graphs = !(e && e[0] == '0');
     }
-    ctx->s_h2d = ctx->s_d2h = nullptr;
-    for (int i = 0; i < 4; i++) ctx->s_comp[i] = nullptr;
-    ctx->ev_start = nullptr;
-    ctx->ev_fork = nullptr;
-    ctx->s_hi = nullptr;
-    ctx->ev_p2 = nullptr;
-    for (int i = 0; i < 4; i++) ctx->ev_join[i] = nullptr;
-    ctx->run_split = 2;
-    ctx->single_pending = false;
-    for (int i = 0; i < 8; i++) ctx->ev_h2d[i] = ctx->ev_done[i] = nullptr;
-    ctx->gray_packed = nullptr;
-    ctx->res_upper = 0;
-    ctx->res_active = false;
-    ctx->res_frame = 0;
-    ctx->res_ofs = nullptr;
-    ctx->blkcnt = ctx->blkofs = ctx->newofs = nullptr;
-    ctx->wmat = nullptr;
-    ctx->inact = nullptr, ctx->inact_ofs = nullptr, ctx->inact_cap = ctx->inact_size = 0;
-    ctx->depth_packed = nullptr;
-    ctx->own_stream = (cuda_stream == nullptr);
     ctx->stream = (cudaStream_t)cuda_stream;
-    if (ctx->own_stream && cudaStreamCreateWithFlags(&ctx->stream, cudaStreamNonBlocking) != cudaSuccess)
+    if (!ctx->stream && ctx->own.stream(&ctx->stream) != cudaSuccess)
     {
         delete ctx;
         return DSM_E_CUDA;
@@ -255,9 +142,6 @@ extern "C" int dsm_create(const dsm_params *params, int device, void *cuda_strea
     const int Wp = (W + 15) / 16 * 16;
     const int spw = W / DSM_SP, sph = H / DSM_SP, S = spw * sph;
     const size_t px = (size_t)H * Wp;
-    ctx->S = S;
-    ctx->Wp = Wp;
-    ctx->px = px;
     DsmDev &d = ctx->d;
     d.W = W, d.H = H, d.Wp = Wp, d.spw = spw, d.sph = sph, d.S = S, d.B = B;
     d.Sp = (S + 31) / 32 * 32;
@@ -273,7 +157,7 @@ extern "C" int dsm_create(const dsm_params *params, int device, void *cuda_strea
     cudaError_t e = cudaSuccess;
     // +64 bytes/elements of slack so the 16-byte vector accesses on the last pitched row stay in bounds
 #define ALLOC(ptr, n)                        \
-    if (e == cudaSuccess) e = dmalloc(&(ptr), (size_t)(n))
+    if (e == cudaSuccess) e = ctx->own.device(&(ptr), (size_t)(n), true)
     ALLOC(ctx->gray, B * px + 64);
     ALLOC(ctx->depth, B * px + 64);
     ALLOC(d.labels, B * px + 64);
@@ -316,25 +200,25 @@ extern "C" int dsm_create(const dsm_params *params, int device, void *cuda_strea
     ALLOC(ctx->wmat, 16);
     ALLOC(ctx->res_ofs, 2);
 #undef ALLOC
-    d.frame0 = 0;
-    if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&ctx->s_h2d, cudaStreamNonBlocking);
-    if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&ctx->s_d2h, cudaStreamNonBlocking);
-    for (int i = 0; i < 4 && e == cudaSuccess; i++) e = cudaStreamCreateWithFlags(&ctx->s_comp[i], cudaStreamNonBlocking);
-    for (int i = 0; i < 8 && e == cudaSuccess; i++)
+    if (e == cudaSuccess) e = ctx->own.host(&ctx->h_pose, (size_t)2 * B * 32);
+    if (e == cudaSuccess) e = ctx->own.host(&ctx->h_ofs, (size_t)B + 1);
+    if (e == cudaSuccess) e = ctx->own.host(&ctx->h_ref, (size_t)2 * B);
+    int least = 0, greatest = 0;
+    if (e == cudaSuccess) e = cudaDeviceGetStreamPriorityRange(&least, &greatest);
+    if (e == cudaSuccess) e = ctx->own.stream(&ctx->s_hi, greatest);
+    if (e == cudaSuccess) e = ctx->own.stream(&ctx->s_h2d);
+    if (e == cudaSuccess) e = ctx->own.stream(&ctx->s_d2h);
+    for (cudaStream_t &s : ctx->s_comp)
+        if (e == cudaSuccess) e = ctx->own.stream(&s);
+    for (cudaEvent_t *ev : {&ctx->ev_start, &ctx->ev_fork, &ctx->ev_p2})
+        if (e == cudaSuccess) e = ctx->own.event(ev);
+    for (cudaEvent_t &ev : ctx->ev_join)
+        if (e == cudaSuccess) e = ctx->own.event(&ev);
+    for (int i = 0; i < EV_COUNT; i++)
     {
-        e = cudaEventCreateWithFlags(&ctx->ev_h2d[i], cudaEventDisableTiming);
-        if (e == cudaSuccess) e = cudaEventCreateWithFlags(&ctx->ev_done[i], cudaEventDisableTiming);
+        if (e == cudaSuccess) e = ctx->own.event(&ctx->ev_h2d[i]);
+        if (e == cudaSuccess) e = ctx->own.event(&ctx->ev_done[i]);
     }
-    if (e == cudaSuccess) e = cudaEventCreateWithFlags(&ctx->ev_start, cudaEventDisableTiming);
-    if (e == cudaSuccess) e = cudaEventCreateWithFlags(&ctx->ev_fork, cudaEventDisableTiming);
-    if (e == cudaSuccess) e = cudaEventCreateWithFlags(&ctx->ev_p2, cudaEventDisableTiming);
-    if (e == cudaSuccess)
-    {
-        int least = 0, greatest = 0;
-        e = cudaDeviceGetStreamPriorityRange(&least, &greatest);
-        if (e == cudaSuccess) e = cudaStreamCreateWithPriority(&ctx->s_hi, cudaStreamNonBlocking, greatest);
-    }
-    for (int i = 0; i < 4 && e == cudaSuccess; i++) e = cudaEventCreateWithFlags(&ctx->ev_join[i], cudaEventDisableTiming);
     if (e == cudaSuccess)
     { // back-projection factor tables: the same float ops as back_project (fusion_functions.cpp:94-95)
         std::vector<float> hx((size_t)Wp + 16), hy((size_t)H + 16);
@@ -343,9 +227,6 @@ extern "C" int dsm_create(const dsm_params *params, int device, void *cuda_strea
         e = cudaMemcpy(ctx->kx, hx.data(), hx.size() * sizeof(float), cudaMemcpyHostToDevice);
         if (e == cudaSuccess) e = cudaMemcpy(ctx->ky, hy.data(), hy.size() * sizeof(float), cudaMemcpyHostToDevice);
     }
-    if (e == cudaSuccess) e = cudaMallocHost((void **)&ctx->h_pose, (size_t)2 * B * 32 * sizeof(float)); // second half: dsm_fuse_stream_resident's own tables
-    if (e == cudaSuccess) e = cudaMallocHost((void **)&ctx->h_ofs, ((size_t)B + 1) * sizeof(int32_t));
-    if (e == cudaSuccess) e = cudaMallocHost((void **)&ctx->h_ref, (size_t)2 * B * sizeof(int32_t));
     if (e != cudaSuccess)
     {
         dsm_destroy(ctx);
@@ -359,7 +240,6 @@ extern "C" int dsm_create(const dsm_params *params, int device, void *cuda_strea
     d.refidx = ctx->refidx;
     d.kx = ctx->kx;
     d.ky = ctx->ky;
-    d.max_pool_per_frame = 0;
     if (make_tile_maps(ctx) != DSM_OK || dsm_tile_setup() != 0)
     {
         dsm_destroy(ctx);
@@ -404,8 +284,8 @@ static cudaEvent_t prof_event(dsm_ctx *ctx)
         ctx->ev_free.pop_back();
         return e;
     }
-    cudaEvent_t e;
-    cudaEventCreate(&e);
+    cudaEvent_t e = nullptr;
+    ctx->own.event(&e, cudaEventDefault); // recycled through ev_free, released with the context
     return e;
 }
 struct ProfScope
@@ -478,15 +358,29 @@ extern "C" int dsm_profile_read(dsm_ctx *ctx, float *ms_total, int32_t *launches
 }
 
 // ---- batch stages ----
+// The per-frame tables of n frames: pose, its inverse and the reference index go to the pinned rows [row, row + n) of
+// h_pose / h_ref, then to the device slots [slot, slot + n) of pose / ipose / refidx on `st` (pose and inverse are
+// interleaved on the host: two strided copies).  The caller makes sure earlier copies out of these rows have completed.
+static int stage_tables(dsm_ctx *ctx, size_t row, int slot, int n, const float *poses, const int32_t *ref, cudaStream_t st)
+{
+    float *hp = ctx->h_pose + row * 32;
+    for (int b = 0; b < n; b++)
+    {
+        memcpy(hp + (size_t)b * 32, poses + (size_t)b * 16, 16 * sizeof(float));
+        inverse4f(poses + (size_t)b * 16, hp + (size_t)b * 32 + 16);
+        ctx->h_ref[row + b] = ref[b];
+    }
+    CK(cudaMemcpy2DAsync(ctx->pose + (size_t)slot * 16, 16 * sizeof(float), hp, 32 * sizeof(float), 16 * sizeof(float), n, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpy2DAsync(ctx->ipose + (size_t)slot * 16, 16 * sizeof(float), hp + 16, 32 * sizeof(float), 16 * sizeof(float), n, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(ctx->refidx + slot, ctx->h_ref + row, (size_t)n * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+    return DSM_OK;
+}
+
+// Batch-mode tables of frames [0, n) on the main stream (first pinned half): per-frame pool offsets `ofs`, validated, or
+// (ofs == nullptr) one frame's n_local_single surfels.
 static int upload_tables(dsm_ctx *ctx, int n, const int32_t *ref, const float *poses, const int32_t *ofs, int n_local_single)
 {
     int total = 0, maxper = 0;
-    for (int b = 0; b < n; b++)
-    {
-        memcpy(ctx->h_pose + (size_t)b * 32, poses + (size_t)b * 16, 16 * sizeof(float));
-        inverse4f(poses + (size_t)b * 16, ctx->h_pose + (size_t)b * 32 + 16);
-        ctx->h_ref[b] = ref[b];
-    }
     if (ofs)
     {
         if (ofs[0] != 0) return DSM_E_INVALID;
@@ -508,12 +402,8 @@ static int upload_tables(dsm_ctx *ctx, int n, const int32_t *ref, const float *p
     if (total > ctx->p.max_local_surfels) return DSM_E_CAPACITY;
     ctx->n_pool = total;
     ctx->d.max_pool_per_frame = maxper;
-    // pose and inverse interleaved on the host: two strided copies
-    CK(cudaMemcpy2DAsync(ctx->pose, 16 * sizeof(float), ctx->h_pose, 32 * sizeof(float), 16 * sizeof(float), n, cudaMemcpyHostToDevice, ctx->stream));
-    CK(cudaMemcpy2DAsync(ctx->ipose, 16 * sizeof(float), ctx->h_pose + 16, 32 * sizeof(float), 16 * sizeof(float), n, cudaMemcpyHostToDevice, ctx->stream));
     CK(cudaMemcpyAsync(ctx->poolofs, ctx->h_ofs, ((size_t)n + 1) * sizeof(int32_t), cudaMemcpyHostToDevice, ctx->stream));
-    CK(cudaMemcpyAsync(ctx->refidx, ctx->h_ref, (size_t)n * sizeof(int32_t), cudaMemcpyHostToDevice, ctx->stream));
-    return DSM_OK;
+    return stage_tables(ctx, 0, 0, n, poses, ref, ctx->stream);
 }
 
 extern "C" int dsm_batch_upload(dsm_ctx *ctx, int n, const int32_t *ref, const uint8_t *gray, const float *depth,
@@ -559,15 +449,14 @@ extern "C" int dsm_batch_restore_pool(dsm_ctx *ctx)
     return DSM_OK;
 }
 
-// The per-frame schedule: generate_super_pixels (:960-975) then fuse (:58-71) then initialise (:79),
-// enqueued for the frame slots [f0, f0 + nf).
+// Launches of the schedule up to and including the plane fit: seed init, 3 x (assign, gather, Newton), plane gather, solve.
+static const int kPlaneFitSteps = 12;
+
+// The per-frame schedule: generate_super_pixels (:960-975) then fuse (:58-71) then initialise (:79), enqueued for the
+// frame slots [d.frame0, d.frame0 + nb) of the view `d` (its pool, poolofs and max_pool_per_frame).
 // phase bit 0: the pose- and pool-independent part (superpixels, pixel normals, plane fit); bit 1: fuse + initialise.
-static int launch_schedule(dsm_ctx *ctx, int f0, int nf, int max_pool_per_frame, cudaStream_t st, int phase = 3)
+static int launch_schedule(dsm_ctx *ctx, const DsmDev &d, int nb, cudaStream_t st, int phase)
 {
-    DsmDev d = ctx->d;
-    d.frame0 = f0;
-    d.max_pool_per_frame = max_pool_per_frame;
-    const int nb = nf;
     int budget = ctx->stop_after > 0 ? ctx->stop_after : 1 << 30;
 #define STEP(ID, CALL)                  \
     if (budget-- > 0)                   \
@@ -589,45 +478,42 @@ static int launch_schedule(dsm_ctx *ctx, int f0, int nf, int max_pool_per_frame,
     }
     if (phase & 2)
     {
-    if (max_pool_per_frame > 0)
-    {
-        STEP(DSM_K_FUSE, dsm_launch_fuse(d, nb, st));
-    }
-    STEP(DSM_K_INIT_SURFELS, dsm_launch_init_surfels(d, nb, st));
+        if (d.max_pool_per_frame > 0)
+        {
+            STEP(DSM_K_FUSE, dsm_launch_fuse(d, nb, st));
+        }
+        STEP(DSM_K_INIT_SURFELS, dsm_launch_init_surfels(d, nb, st));
     }
 #undef STEP
     CK(cudaGetLastError());
     return DSM_OK;
 }
 
-// Enqueue the schedule, optionally followed by the resident-pool post-step (compaction into `alt`).
+// Enqueue the schedule for the view `v` (frames [v.frame0, v.frame0 + nf)), followed, when `alt` is given, by the
+// resident-pool post-step: compaction of v.pool into `alt`.
 // The 17-21 launches are captured once per distinct parameter set into a CUDA graph and replayed: the
 // per-launch CPU cost and inter-kernel gaps matter for single frames and small chunks.  Profiling
 // (event pairs around kernels) and the debug kernel budget use plain launches.
-static int enqueue_schedule(dsm_ctx *ctx, int f0, int nf, int maxper, cudaStream_t st, bool compact = false, int phase = 3)
+static int enqueue_schedule(dsm_ctx *ctx, const DsmDev &v, int nf, cudaStream_t st, dsm_surfel_t *alt = nullptr, int phase = 3)
 {
-    // grids over the pool are sized from `maxper` rounded up to 4 Ki surfels (the kernels take the true
+    // grids over the pool are sized from max_pool_per_frame rounded up to 4 Ki surfels (the kernels take the true
     // ranges from poolofs on the device, surplus blocks exit at once), so that callers whose pool size
     // changes a little from call to call keep hitting the same captured graph
-    if (maxper > 0) maxper = (maxper + 4095) & ~4095;
+    DsmDev d = v;
+    if (d.max_pool_per_frame > 0) d.max_pool_per_frame = (d.max_pool_per_frame + 4095) & ~4095;
     auto plain = [&]() -> int
     {
-        int rc = launch_schedule(ctx, f0, nf, maxper, st, phase);
+        int rc = launch_schedule(ctx, d, nf, st, phase);
         if (rc != DSM_OK) return rc;
-        if (compact)
-        {
-            DsmDev d = ctx->d;
-            d.frame0 = f0;
-            dsm_launch_pool_compact(d, f0, maxper, ctx->blkcnt, ctx->blkofs, ctx->newofs, ctx->pool_snap, ctx->res_ofs, st);
-        }
+        if (alt) dsm_launch_pool_compact(d, d.frame0, d.max_pool_per_frame, ctx->blkcnt, ctx->blkofs, ctx->newofs, alt, ctx->res_ofs, st);
         return DSM_OK;
     };
     if (!ctx->use_graphs || ctx->prof_mask != 0 || ctx->stop_after > 0) return plain();
     for (auto &g : ctx->graphs)
-        if (g.f0 == f0 && g.nf == nf && g.maxper == maxper && g.compact == (int)compact && g.pool == ctx->d.pool &&
-            g.poolofs == ctx->d.poolofs && g.alt == ctx->pool_snap && g.phase == phase)
+        if (g.f0 == d.frame0 && g.nf == nf && g.maxper == d.max_pool_per_frame && g.pool == d.pool && g.poolofs == d.poolofs &&
+            g.alt == alt && g.phase == phase)
         {
-            CK(cudaGraphLaunch(g.exec, st));
+            CK(cudaGraphLaunch(g.exec.get(), st));
             return DSM_OK;
         }
     cudaGraph_t graph = nullptr;
@@ -654,12 +540,8 @@ static int enqueue_schedule(dsm_ctx *ctx, int f0, int nf, int maxper, cudaStream
         ctx->use_graphs = false;
         return plain();
     }
-    if (ctx->graphs.size() >= 64)
-    { // bounded cache
-        cudaGraphExecDestroy(ctx->graphs.front().exec);
-        ctx->graphs.erase(ctx->graphs.begin());
-    }
-    ctx->graphs.push_back(GraphEntry{f0, nf, maxper, (int)compact, ctx->d.pool, ctx->d.poolofs, ctx->pool_snap, exec, phase});
+    if (ctx->graphs.size() >= 64) ctx->graphs.erase(ctx->graphs.begin()); // bounded cache
+    ctx->graphs.push_back(GraphEntry{d.frame0, nf, d.max_pool_per_frame, phase, d.pool, d.poolofs, alt, GraphExecPtr(exec)});
     CK(cudaGraphLaunch(exec, st));
     return DSM_OK;
 }
@@ -674,24 +556,25 @@ extern "C" int dsm_batch_run(dsm_ctx *ctx)
     // contexts alternating (bench.py) the gain on an H100 at 400 W is small: 1.150 / 1.163 ms per 32-frame step with two
     // sub-batches against 1.153 / 1.168 ms with one (two runs each); three or four sub-batches were slower.
     const int parts = (ctx->stop_after > 0 || ctx->nb < 8) ? 1 : (ctx->run_split < ctx->nb ? ctx->run_split : ctx->nb);
+    DsmDev v = ctx->d; // batch view: per-frame pool slices at poolofs, frames from slot 0
+    v.frame0 = 0;
     if (parts <= 1)
     {
-        int rc = enqueue_schedule(ctx, 0, ctx->nb, ctx->d.max_pool_per_frame, ctx->stream);
+        int rc = enqueue_schedule(ctx, v, ctx->nb, ctx->stream);
         if (rc != DSM_OK) return rc;
     }
     else
     {
         CK(cudaEventRecord(ctx->ev_fork, ctx->stream));
-        int f0 = 0;
         for (int i = 0; i < parts; i++)
         {
-            const int nf = (ctx->nb - f0 + (parts - i) - 1) / (parts - i);
+            const int nf = (ctx->nb - v.frame0 + (parts - i) - 1) / (parts - i);
             CK(cudaStreamWaitEvent(ctx->s_comp[i], ctx->ev_fork, 0));
-            int rc = enqueue_schedule(ctx, f0, nf, ctx->d.max_pool_per_frame, ctx->s_comp[i]);
+            int rc = enqueue_schedule(ctx, v, nf, ctx->s_comp[i]);
             if (rc != DSM_OK) return rc;
             CK(cudaEventRecord(ctx->ev_join[i], ctx->s_comp[i]));
             CK(cudaStreamWaitEvent(ctx->stream, ctx->ev_join[i], 0));
-            f0 += nf;
+            v.frame0 += nf;
         }
     }
     ctx->ran = true;
@@ -712,8 +595,7 @@ extern "C" int dsm_set_constants(dsm_ctx *ctx, const dsm_constants *k)
     if (ctx->in_flight) return DSM_E_STATE;
     CK(cudaSetDevice(ctx->device));
     CK(cudaStreamSynchronize(ctx->stream));
-    for (auto &g : ctx->graphs) cudaGraphExecDestroy(g.exec); // captured schedules embed the kernel parameters
-    ctx->graphs.clear();
+    ctx->graphs.clear(); // captured schedules embed the kernel parameters
     apply_constants(ctx->d, *k);
     return DSM_OK;
 }
@@ -747,7 +629,7 @@ extern "C" int dsm_batch_download(dsm_ctx *ctx, dsm_surfel_t *local_out, dsm_sur
     if (local_out && ctx->n_pool > 0)
         CK(cudaMemcpyAsync(local_out, ctx->d.pool, (size_t)ctx->n_pool * sizeof(dsm_surfel_t), cudaMemcpyDeviceToHost, ctx->stream));
     if (new_out)
-        CK(cudaMemcpyAsync(new_out, ctx->d.newsurf, (size_t)ctx->nb * ctx->S * sizeof(dsm_surfel_t), cudaMemcpyDeviceToHost, ctx->stream));
+        CK(cudaMemcpyAsync(new_out, ctx->d.newsurf, (size_t)ctx->nb * ctx->d.S * sizeof(dsm_surfel_t), cudaMemcpyDeviceToHost, ctx->stream));
     if (n_new)
         CK(cudaMemcpyAsync(n_new, ctx->d.nnew, (size_t)ctx->nb * sizeof(int32_t), cudaMemcpyDeviceToHost, ctx->stream));
     return DSM_OK;
@@ -771,7 +653,7 @@ extern "C" int dsm_batch_wait(dsm_ctx *ctx)
     if (!ctx) return DSM_E_INVALID;
     CK(cudaSetDevice(ctx->device));
     CK(cudaStreamSynchronize(ctx->s_h2d));
-    for (int i = 0; i < 4; i++) CK(cudaStreamSynchronize(ctx->s_comp[i]));
+    for (cudaStream_t s : ctx->s_comp) CK(cudaStreamSynchronize(s));
     CK(cudaStreamSynchronize(ctx->stream));
     CK(cudaStreamSynchronize(ctx->s_d2h));
     CK(cudaGetLastError());
@@ -795,15 +677,10 @@ extern "C" int dsm_fuse_batch_async(dsm_ctx *ctx, int n, const int32_t *ref, con
     CK(cudaStreamSynchronize(ctx->stream));
     int rc = upload_tables(ctx, n, ref, poses, ofs, 0); // small tables, on the compute stream
     if (rc != DSM_OK) return rc;
-    const int W = ctx->p.width, H = ctx->p.height, S = ctx->S;
+    const int W = ctx->p.width, H = ctx->p.height, S = ctx->d.S;
     const size_t fpx = (size_t)H * W;
-    int nchunks = n >= 16 ? 4 : (n >= 4 ? 2 : 1);
-    if (const char *e = getenv("DSM_E2E_CHUNKS"))
-    { // tuning knob for experiments (1..8)
-        const int v = atoi(e);
-        if (v >= 1 && v <= 8 && v <= n) nchunks = v;
-    }
-    int csize[8]; // even chunks (a smaller first chunk was tried: no gain, the kernels of small chunks are less efficient)
+    const int nchunks = n >= 16 ? 4 : (n >= 4 ? 2 : 1); // at most DSM_MAX_CHUNKS: one compute stream each
+    int csize[DSM_MAX_CHUNKS]; // even chunks (a smaller first chunk was tried: no gain, the kernels of small chunks are less efficient)
     {
         int rest = n, left = nchunks;
         for (int c = 0; c < nchunks; c++)
@@ -817,7 +694,7 @@ extern "C" int dsm_fuse_batch_async(dsm_ctx *ctx, int n, const int32_t *ref, con
     CK(cudaEventRecord(ctx->ev_start, ctx->stream));
     CK(cudaStreamWaitEvent(ctx->s_h2d, ctx->ev_start, 0));
     CK(cudaStreamWaitEvent(ctx->s_d2h, ctx->ev_start, 0));
-    for (int i = 0; i < 4; i++) CK(cudaStreamWaitEvent(ctx->s_comp[i], ctx->ev_start, 0));
+    for (cudaStream_t s : ctx->s_comp) CK(cudaStreamWaitEvent(s, ctx->ev_start, 0));
     int nc = 0;
     for (int f0 = 0; f0 < n; f0 += csize[nc], nc++)
     {
@@ -831,22 +708,23 @@ extern "C" int dsm_fuse_batch_async(dsm_ctx *ctx, int n, const int32_t *ref, con
         CK(cudaMemcpyAsync(ctx->depth_packed + (size_t)f0 * fpx, depth + (size_t)f0 * fpx, (size_t)nf * fpx * sizeof(float), cudaMemcpyHostToDevice, ctx->s_h2d));
         if (p1 > p0)
             CK(cudaMemcpyAsync(ctx->d.pool + p0, local + p0, (size_t)(p1 - p0) * sizeof(dsm_surfel_t), cudaMemcpyHostToDevice, ctx->s_h2d));
-        CK(cudaEventRecord(ctx->ev_h2d[nc], ctx->s_h2d));
+        CK(cudaEventRecord(ctx->ev_h2d[EV_CHUNK + nc], ctx->s_h2d));
         // kernels: each chunk on its own compute stream, so the latency-bound per-seed kernels of one
         // chunk overlap the wide kernels of its neighbours instead of leaving SMs idle
-        cudaStream_t cs = nchunks > 1 ? ctx->s_comp[nc & 3] : ctx->stream;
-        CK(cudaStreamWaitEvent(cs, ctx->ev_h2d[nc], 0));
+        cudaStream_t cs = nchunks > 1 ? ctx->s_comp[nc] : ctx->stream;
+        CK(cudaStreamWaitEvent(cs, ctx->ev_h2d[EV_CHUNK + nc], 0));
+        DsmDev v = ctx->d; // batch view of this chunk
+        v.frame0 = f0;
+        v.max_pool_per_frame = maxper;
         {
-            DsmDev d = ctx->d;
-            d.frame0 = f0;
             ProfScope p(ctx, DSM_K_REPACK, cs);
-            dsm_launch_repack(d, nf, ctx->gray_packed + (size_t)f0 * fpx, ctx->depth_packed + (size_t)f0 * fpx, cs);
+            dsm_launch_repack(v, nf, ctx->gray_packed + (size_t)f0 * fpx, ctx->depth_packed + (size_t)f0 * fpx, cs);
         }
-        rc = enqueue_schedule(ctx, f0, nf, maxper, cs);
+        rc = enqueue_schedule(ctx, v, nf, cs);
         if (rc != DSM_OK) return rc;
-        CK(cudaEventRecord(ctx->ev_done[nc], cs));
+        CK(cudaEventRecord(ctx->ev_done[EV_CHUNK + nc], cs));
         // D2H of this chunk
-        CK(cudaStreamWaitEvent(ctx->s_d2h, ctx->ev_done[nc], 0));
+        CK(cudaStreamWaitEvent(ctx->s_d2h, ctx->ev_done[EV_CHUNK + nc], 0));
         if (p1 > p0)
             CK(cudaMemcpyAsync(local + p0, ctx->d.pool + p0, (size_t)(p1 - p0) * sizeof(dsm_surfel_t), cudaMemcpyDeviceToHost, ctx->s_d2h));
         if (new_out)
@@ -892,8 +770,8 @@ extern "C" int dsm_fuse_frame(dsm_ctx *ctx, int ref_idx, const uint8_t *gray, si
     int32_t ref = ref_idx;
     int rc = upload_tables(ctx, 1, &ref, pose, nullptr, n_local);
     if (rc != DSM_OK) return rc;
-    CK(cudaMemcpy2DAsync(ctx->gray, ctx->Wp, gray, gray_pitch, W, H, cudaMemcpyHostToDevice, ctx->stream));
-    CK(cudaMemcpy2DAsync(ctx->depth, (size_t)ctx->Wp * 4, depth, depth_pitch, (size_t)W * 4, H, cudaMemcpyHostToDevice, ctx->stream));
+    CK(cudaMemcpy2DAsync(ctx->gray, ctx->d.Wp, gray, gray_pitch, W, H, cudaMemcpyHostToDevice, ctx->stream));
+    CK(cudaMemcpy2DAsync(ctx->depth, (size_t)ctx->d.Wp * 4, depth, depth_pitch, (size_t)W * 4, H, cudaMemcpyHostToDevice, ctx->stream));
     if (n_local > 0)
         CK(cudaMemcpyAsync(ctx->d.pool, local, (size_t)n_local * sizeof(dsm_surfel_t), cudaMemcpyHostToDevice, ctx->stream));
     ctx->nb = 1;
@@ -919,12 +797,25 @@ extern "C" int dsm_fuse_frame(dsm_ctx *ctx, int ref_idx, const uint8_t *gray, si
 // ---- GPU-resident pool (stream mode) ----
 // The resident pool is described by res_ofs = {0, n} on the device.  Frames alternate between two
 // frame slots (when max_batch >= 2) so that the H2D copy of frame t+1 overlaps the kernels of frame t.
+// The view of frame slot `slot`: grids over the pool are sized from its upper bound rounded up to 64 Ki surfels and
+// clamped to the capacity, so that the captured graph stays valid while the pool grows (surplus blocks exit at once:
+// the kernels read the true range from the device).
 static DsmDev resident_view(dsm_ctx *ctx, int slot)
 {
     DsmDev d = ctx->d;
     d.frame0 = slot;
     d.poolofs = ctx->res_ofs - slot; // kernels read poolofs[b], poolofs[b+1] with b == slot
+    const int upq = (ctx->res_upper + 65535) / 65536 * 65536;
+    d.max_pool_per_frame = upq < ctx->p.max_local_surfels ? upq : ctx->p.max_local_surfels;
     return d;
+}
+
+// After a frame's compaction into the alternate buffer, that buffer holds the pool.
+static void swap_pool(dsm_ctx *ctx)
+{
+    dsm_surfel_t *t = ctx->d.pool;
+    ctx->d.pool = ctx->pool_snap;
+    ctx->pool_snap = t;
 }
 
 extern "C" int dsm_pool_upload(dsm_ctx *ctx, const dsm_surfel_t *local, int n)
@@ -1066,12 +957,12 @@ extern "C" int dsm_fuse_frame_resident(dsm_ctx *ctx, int ref_idx, const uint8_t 
     const int W = ctx->p.width, H = ctx->p.height;
     if (gray_pitch < (size_t)W || depth_pitch < (size_t)W * 4) return DSM_E_INVALID;
     CK(cudaSetDevice(ctx->device));
-    if (ctx->res_upper + ctx->S > ctx->p.max_local_surfels)
+    if (ctx->res_upper + ctx->d.S > ctx->p.max_local_surfels)
     { // the bound may be loose: fetch the exact size before giving up
         int n = 0;
         int rc = dsm_pool_size(ctx, &n);
         if (rc != DSM_OK) return rc;
-        if (n + ctx->S > ctx->p.max_local_surfels) return DSM_E_CAPACITY;
+        if (n + ctx->d.S > ctx->p.max_local_surfels) return DSM_E_CAPACITY;
     }
     const int nslots = ctx->p.max_batch >= 2 ? 2 : 1;
     const int slot = ctx->res_frame % nslots;
@@ -1079,14 +970,11 @@ extern "C" int dsm_fuse_frame_resident(dsm_ctx *ctx, int ref_idx, const uint8_t 
     const size_t fpx = (size_t)H * W;
     // this slot's pinned tables / image buffers were last used two frames ago: make sure that copy and
     // those kernels are done (normally long finished, so these do not stall)
-    CK(cudaEventSynchronize(ctx->ev_h2d[slot]));
-    CK(cudaStreamWaitEvent(ctx->s_h2d, ctx->ev_done[slot], 0));
-    memcpy(ctx->h_pose + (size_t)slot * 32, pose, 16 * sizeof(float));
-    inverse4f(pose, ctx->h_pose + (size_t)slot * 32 + 16);
-    ctx->h_ref[slot] = ref_idx;
-    CK(cudaMemcpyAsync(ctx->pose + slot * 16, ctx->h_pose + (size_t)slot * 32, 16 * sizeof(float), cudaMemcpyHostToDevice, ctx->s_h2d));
-    CK(cudaMemcpyAsync(ctx->ipose + slot * 16, ctx->h_pose + (size_t)slot * 32 + 16, 16 * sizeof(float), cudaMemcpyHostToDevice, ctx->s_h2d));
-    CK(cudaMemcpyAsync(ctx->refidx + slot, ctx->h_ref + slot, sizeof(int32_t), cudaMemcpyHostToDevice, ctx->s_h2d));
+    CK(cudaEventSynchronize(ctx->ev_h2d[EV_SLOT + slot]));
+    CK(cudaStreamWaitEvent(ctx->s_h2d, ctx->ev_done[EV_SLOT + slot], 0));
+    const int32_t ref = ref_idx;
+    int rc = stage_tables(ctx, slot, slot, 1, pose, &ref, ctx->s_h2d); // pinned row = frame slot, in the first half
+    if (rc != DSM_OK) return rc;
     const bool packed = gray_pitch == (size_t)W && depth_pitch == (size_t)W * 4;
     if (packed)
     { // one contiguous copy per image, repacked to the pitched layout on the device
@@ -1095,11 +983,11 @@ extern "C" int dsm_fuse_frame_resident(dsm_ctx *ctx, int ref_idx, const uint8_t 
     }
     else
     {
-        CK(cudaMemcpy2DAsync(ctx->gray + (size_t)slot * ctx->px, ctx->Wp, gray, gray_pitch, W, H, cudaMemcpyHostToDevice, ctx->s_h2d));
-        CK(cudaMemcpy2DAsync(ctx->depth + (size_t)slot * ctx->px, (size_t)ctx->Wp * 4, depth, depth_pitch, (size_t)W * 4, H, cudaMemcpyHostToDevice, ctx->s_h2d));
+        CK(cudaMemcpy2DAsync(ctx->gray + (size_t)slot * ctx->d.px_stride, ctx->d.Wp, gray, gray_pitch, W, H, cudaMemcpyHostToDevice, ctx->s_h2d));
+        CK(cudaMemcpy2DAsync(ctx->depth + (size_t)slot * ctx->d.px_stride, (size_t)ctx->d.Wp * 4, depth, depth_pitch, (size_t)W * 4, H, cudaMemcpyHostToDevice, ctx->s_h2d));
     }
-    CK(cudaEventRecord(ctx->ev_h2d[slot], ctx->s_h2d));
-    CK(cudaStreamWaitEvent(ctx->stream, ctx->ev_h2d[slot], 0));
+    CK(cudaEventRecord(ctx->ev_h2d[EV_SLOT + slot], ctx->s_h2d));
+    CK(cudaStreamWaitEvent(ctx->stream, ctx->ev_h2d[EV_SLOT + slot], 0));
     const DsmDev dv = resident_view(ctx, slot);
     if (packed)
     {
@@ -1108,32 +996,18 @@ extern "C" int dsm_fuse_frame_resident(dsm_ctx *ctx, int ref_idx, const uint8_t 
     }
     ctx->nb = slot + 1;
     ctx->uploaded = true;
-    {
-        // enqueue_schedule takes its view from ctx->d: temporarily present the resident pool table
-        const int32_t *saved = ctx->d.poolofs;
-        ctx->d.poolofs = dv.poolofs;
-        // + post-step of SurfelMap::fuse_map on the device: compact into the alternate buffer (then swap)
-        // grid sizes use the bound rounded up to 64 Ki surfels so that the captured graph stays valid while
-        // the pool grows (surplus blocks exit at once: the kernels read the true range from the device)
-        int upq = (ctx->res_upper + 65535) / 65536 * 65536;
-        if (upq > ctx->p.max_local_surfels) upq = ctx->p.max_local_surfels;
-        int rc = enqueue_schedule(ctx, slot, 1, upq, ctx->stream, true);
-        ctx->d.poolofs = saved;
-        if (rc != DSM_OK) return rc;
-    }
+    // + post-step of SurfelMap::fuse_map on the device: compact into the alternate buffer, then swap
+    rc = enqueue_schedule(ctx, dv, 1, ctx->stream, ctx->pool_snap);
+    if (rc != DSM_OK) return rc;
     ctx->ran = true;
-    CK(cudaEventRecord(ctx->ev_done[slot], ctx->stream)); // (the compaction's last kernel stored the new pool size in res_ofs[1])
+    CK(cudaEventRecord(ctx->ev_done[EV_SLOT + slot], ctx->stream)); // (the compaction's last kernel stored the new pool size in res_ofs[1])
     ctx->single_pending = true;
-    {
-        dsm_surfel_t *t = ctx->d.pool;
-        ctx->d.pool = ctx->pool_snap;
-        ctx->pool_snap = t;
-    }
-    ctx->res_upper += ctx->S; // every seed can add at most one surfel; dsm_pool_size() tightens it
+    swap_pool(ctx);
+    ctx->res_upper += ctx->d.S; // every seed can add at most one surfel; dsm_pool_size() tightens it
     CK(cudaGetLastError());
     // the caller may reuse its image buffers as soon as we return: wait for THIS frame's copy only
     // (the kernels keep running and overlap the next call's copy)
-    CK(cudaEventSynchronize(ctx->ev_h2d[slot]));
+    CK(cudaEventSynchronize(ctx->ev_h2d[EV_SLOT + slot]));
     if (n_new)
     {
         int32_t c = 0;
@@ -1153,7 +1027,7 @@ static DsmDev inactive_view(dsm_ctx *ctx)
 {
     DsmDev d = ctx->d;
     d.frame0 = 0;
-    d.pool = ctx->inact;
+    d.pool = ctx->inact.get();
     d.poolofs = ctx->inact_ofs; // {first, last} of the range a call works on, set in stream order by k_set2
     return d;
 }
@@ -1164,11 +1038,18 @@ extern "C" int dsm_inactive_reserve(dsm_ctx *ctx, int max_inactive_surfels)
     if (ctx->inact_size > 0) return DSM_E_STATE;
     CK(cudaSetDevice(ctx->device));
     CK(cudaStreamSynchronize(ctx->stream));
-    cudaFree(ctx->inact);
-    ctx->inact = nullptr;
+    ctx->inact.reset();
     ctx->inact_cap = 0;
-    if (!ctx->inact_ofs && dmalloc(&ctx->inact_ofs, 2) != cudaSuccess) return DSM_E_NOMEM;
-    if (dmalloc(&ctx->inact, (size_t)max_inactive_surfels) != cudaSuccess)
+    if (!ctx->inact_ofs && ctx->own.device(&ctx->inact_ofs, 2, true) != cudaSuccess) return DSM_E_NOMEM;
+    const size_t bytes = (size_t)max_inactive_surfels * sizeof(dsm_surfel_t);
+    void *p = nullptr;
+    cudaError_t e = cudaMalloc(&p, bytes);
+    if (e == cudaSuccess)
+    {
+        ctx->inact.reset(static_cast<dsm_surfel_t *>(p));
+        e = cudaMemset(p, 0, bytes);
+    }
+    if (e != cudaSuccess)
     {
         cudaGetLastError();
         return DSM_E_NOMEM;
@@ -1196,7 +1077,7 @@ extern "C" int dsm_inactive_retire(dsm_ctx *ctx, int kf, int *n_moved)
     int rc = dsm_pool_size(ctx, &cur); // exact pool size: bounds the segment
     if (rc != DSM_OK) return rc;
     if (ctx->inact_size + cur > ctx->inact_cap) return DSM_E_CAPACITY;
-    dsm_launch_pool_retire(resident_view(ctx, 0), 0, ctx->res_upper, kf, ctx->blkcnt, ctx->blkofs, ctx->newofs, ctx->inact + ctx->inact_size, ctx->stream);
+    dsm_launch_pool_retire(resident_view(ctx, 0), 0, ctx->res_upper, kf, ctx->blkcnt, ctx->blkofs, ctx->newofs, ctx->inact.get() + ctx->inact_size, ctx->stream);
     int32_t h[2] = {0, 0};
     CK(cudaMemcpyAsync(h, ctx->newofs, 2 * sizeof(int32_t), cudaMemcpyDeviceToHost, ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
@@ -1235,7 +1116,7 @@ extern "C" int dsm_inactive_reactivate(dsm_ctx *ctx, int kf, int *n_moved)
             i++;
             continue;
         }
-        CK(cudaMemcpyAsync(ctx->d.pool + cur, ctx->inact + sg.ofs, (size_t)sg.cnt * sizeof(dsm_surfel_t), cudaMemcpyDeviceToDevice, st));
+        CK(cudaMemcpyAsync(ctx->d.pool + cur, ctx->inact.get() + sg.ofs, (size_t)sg.cnt * sizeof(dsm_surfel_t), cudaMemcpyDeviceToDevice, st));
         cur += sg.cnt;
         // close the gap: move the tail down through the alternate pool buffer (free between frames), chunk by chunk
         int src = sg.ofs + sg.cnt;
@@ -1243,8 +1124,8 @@ extern "C" int dsm_inactive_reactivate(dsm_ctx *ctx, int kf, int *n_moved)
         while (src < end)
         {
             const int len = (end - src) < npool ? (end - src) : npool;
-            CK(cudaMemcpyAsync(ctx->pool_snap, ctx->inact + src, (size_t)len * sizeof(dsm_surfel_t), cudaMemcpyDeviceToDevice, st));
-            CK(cudaMemcpyAsync(ctx->inact + src - sg.cnt, ctx->pool_snap, (size_t)len * sizeof(dsm_surfel_t), cudaMemcpyDeviceToDevice, st));
+            CK(cudaMemcpyAsync(ctx->pool_snap, ctx->inact.get() + src, (size_t)len * sizeof(dsm_surfel_t), cudaMemcpyDeviceToDevice, st));
+            CK(cudaMemcpyAsync(ctx->inact.get() + src - sg.cnt, ctx->pool_snap, (size_t)len * sizeof(dsm_surfel_t), cudaMemcpyDeviceToDevice, st));
             src += len;
         }
         ctx->inact_size -= sg.cnt;
@@ -1289,7 +1170,7 @@ extern "C" int dsm_inactive_download(dsm_ctx *ctx, int kf, dsm_surfel_t *out, in
     {
         if (kf >= 0 && sg.kf != kf) continue;
         const int c = (n + sg.cnt <= cap) ? sg.cnt : (cap > n ? cap - n : 0);
-        if (c > 0) CK(cudaMemcpyAsync(out + n, ctx->inact + sg.ofs, (size_t)c * sizeof(dsm_surfel_t), cudaMemcpyDeviceToHost, ctx->stream));
+        if (c > 0) CK(cudaMemcpyAsync(out + n, ctx->inact.get() + sg.ofs, (size_t)c * sizeof(dsm_surfel_t), cudaMemcpyDeviceToHost, ctx->stream));
         n += sg.cnt;
     }
     CK(cudaStreamSynchronize(ctx->stream));
@@ -1332,12 +1213,12 @@ extern "C" int dsm_fuse_stream_resident(dsm_ctx *ctx, int n, const int32_t *ref_
     if (!ctx->res_active) return DSM_E_STATE;
     if (ctx->in_flight) return DSM_E_STATE;
     CK(cudaSetDevice(ctx->device));
-    if (ctx->res_upper + n * ctx->S > ctx->p.max_local_surfels)
+    if (ctx->res_upper + n * ctx->d.S > ctx->p.max_local_surfels)
     { // the bound may be loose: fetch the exact size before giving up
         int cur = 0;
         int rc = dsm_pool_size(ctx, &cur);
         if (rc != DSM_OK) return rc;
-        if (cur + n * ctx->S > ctx->p.max_local_surfels) return DSM_E_CAPACITY;
+        if (cur + n * ctx->d.S > ctx->p.max_local_surfels) return DSM_E_CAPACITY;
     }
     const int W = ctx->p.width, H = ctx->p.height;
     const size_t fpx = (size_t)H * W;
@@ -1345,9 +1226,9 @@ extern "C" int dsm_fuse_stream_resident(dsm_ctx *ctx, int n, const int32_t *ref_
     const bool dbl = 2 * n <= ctx->p.max_batch;
     const int par = dbl ? (ctx->res_frame & 1) : 0;
     ctx->res_frame++;
-    const int e = 6 + par; // events 6/7: this half's staging buffers and pinned tables are free again
+    const int e = EV_HALF + par; // this half's staging buffers and pinned tables are free again
     CK(cudaEventSynchronize(ctx->ev_done[e]));
-    if (!dbl) CK(cudaEventSynchronize(ctx->ev_done[6 + (1 - par)]));
+    if (!dbl) CK(cudaEventSynchronize(ctx->ev_done[EV_HALF + (1 - par)]));
     // single-frame calls (dsm_fuse_frame_resident) may still be running out of the same staging buffers and frame slots
     // 0 / 1 (only then: the events are also recorded at the end of every run of this function, and waiting for the
     // previous run here would serialise this run's copies behind it)
@@ -1355,20 +1236,10 @@ extern "C" int dsm_fuse_stream_resident(dsm_ctx *ctx, int n, const int32_t *ref_
     ctx->single_pending = false;
     if (after_single)
     {
-        CK(cudaStreamWaitEvent(ctx->s_h2d, ctx->ev_done[0], 0));
-        CK(cudaStreamWaitEvent(ctx->s_h2d, ctx->ev_done[1], 0));
+        CK(cudaStreamWaitEvent(ctx->s_h2d, ctx->ev_done[EV_SLOT + 0], 0));
+        CK(cudaStreamWaitEvent(ctx->s_h2d, ctx->ev_done[EV_SLOT + 1], 0));
     }
     const size_t so = (size_t)par * (size_t)(ctx->p.max_batch / 2); // fixed halves: runs of different length never overlap
-    // pinned tables of this mode live in the second half of h_pose / h_ref (the first half belongs to the single-frame
-    // and batch calls, which only wait for their own copies before rewriting it); this half's previous table copy ran
-    // before ev_done[e], which has been waited for above
-    const size_t ho = (size_t)ctx->p.max_batch + so;
-    for (int t = 0; t < n; t++)
-    {
-        memcpy(ctx->h_pose + (ho + t) * 32, poses + (size_t)t * 16, 16 * sizeof(float));
-        inverse4f(poses + (size_t)t * 16, ctx->h_pose + (ho + t) * 32 + 16);
-        ctx->h_ref[ho + t] = ref_idx[t];
-    }
     uint8_t *gp = ctx->gray_packed + so * fpx;
     float *dp = ctx->depth_packed + so * fpx;
     CK(cudaMemcpyAsync(gp, gray, (size_t)n * fpx, cudaMemcpyHostToDevice, ctx->s_h2d));
@@ -1390,41 +1261,37 @@ extern "C" int dsm_fuse_stream_resident(dsm_ctx *ctx, int n, const int32_t *ref_
         CK(cudaStreamWaitEvent(s2, ctx->ev_fork, 0));
         CK(cudaStreamWaitEvent(s1, ctx->ev_done[e], 0));
     }
-    CK(cudaMemcpy2DAsync(ctx->pose + (size_t)slot0 * 16, 16 * sizeof(float), ctx->h_pose + ho * 32, 32 * sizeof(float), 16 * sizeof(float), n, cudaMemcpyHostToDevice, s1));
-    CK(cudaMemcpy2DAsync(ctx->ipose + (size_t)slot0 * 16, 16 * sizeof(float), ctx->h_pose + ho * 32 + 16, 32 * sizeof(float), 16 * sizeof(float), n, cudaMemcpyHostToDevice, s1));
-    CK(cudaMemcpyAsync(ctx->refidx + slot0, ctx->h_ref + ho, (size_t)n * sizeof(int32_t), cudaMemcpyHostToDevice, s1));
+    // pinned tables of this mode live in the second half of h_pose / h_ref (the first half belongs to the single-frame
+    // and batch calls, which only wait for their own copies before rewriting it); this half's previous table copy ran
+    // before ev_done[e], which has been waited for above
+    int rc = stage_tables(ctx, (size_t)ctx->p.max_batch + so, slot0, n, poses, ref_idx, s1);
+    if (rc != DSM_OK) return rc;
     CK(cudaStreamWaitEvent(s1, ctx->ev_h2d[e], 0));
+    // phase 1: all n frames at once, in the batch view (never touches the pool)
+    DsmDev v = ctx->d;
+    v.frame0 = slot0;
+    v.max_pool_per_frame = 0;
     {
-        DsmDev d = ctx->d;
-        d.frame0 = slot0;
         ProfScope p(ctx, DSM_K_REPACK, s1);
-        dsm_launch_repack(d, n, gp, dp, s1);
+        dsm_launch_repack(v, n, gp, dp, s1);
     }
     ctx->nb = slot0 + n;
     ctx->uploaded = true;
-    const int32_t *saved = ctx->d.poolofs;
-    // phase 1: all n frames at once
-    int rc = enqueue_schedule(ctx, slot0, n, 0, s1, false, 1);
-    if (dbl && rc == DSM_OK)
+    rc = enqueue_schedule(ctx, v, n, s1, nullptr, 1);
+    if (rc != DSM_OK) return rc;
+    if (dbl)
     {
         CK(cudaEventRecord(ctx->ev_join[par], s1));
         CK(cudaStreamWaitEvent(s2, ctx->ev_join[par], 0));
     }
     // phase 2: frame by frame on the resident pool, compaction into the alternate buffer, swap
-    for (int t = 0; t < n && rc == DSM_OK; t++)
+    for (int t = 0; t < n; t++)
     {
-        ctx->d.poolofs = ctx->res_ofs - (slot0 + t); // kernels read poolofs[b], poolofs[b+1] with b == slot0 + t
-        int upq = (ctx->res_upper + 65535) / 65536 * 65536;
-        if (upq > ctx->p.max_local_surfels) upq = ctx->p.max_local_surfels;
-        rc = enqueue_schedule(ctx, slot0 + t, 1, upq, s2, true, 2);
-        if (rc != DSM_OK) break;
-        dsm_surfel_t *tmp = ctx->d.pool;
-        ctx->d.pool = ctx->pool_snap;
-        ctx->pool_snap = tmp;
-        ctx->res_upper += ctx->S;
+        rc = enqueue_schedule(ctx, resident_view(ctx, slot0 + t), 1, s2, ctx->pool_snap, 2);
+        if (rc != DSM_OK) return rc;
+        swap_pool(ctx);
+        ctx->res_upper += ctx->d.S;
     }
-    ctx->d.poolofs = saved;
-    if (rc != DSM_OK) return rc;
     ctx->ran = true;
     if (dbl)
     {
@@ -1432,8 +1299,8 @@ extern "C" int dsm_fuse_stream_resident(dsm_ctx *ctx, int n, const int32_t *ref_
         CK(cudaStreamWaitEvent(st, ctx->ev_p2, 0));
     }
     CK(cudaEventRecord(ctx->ev_done[e], st));
-    CK(cudaEventRecord(ctx->ev_done[0], st)); // dsm_fuse_frame_resident waits on these before reusing slot 0 / 1
-    CK(cudaEventRecord(ctx->ev_done[1], st));
+    CK(cudaEventRecord(ctx->ev_done[EV_SLOT + 0], st)); // dsm_fuse_frame_resident waits on these before reusing slot 0 / 1
+    CK(cudaEventRecord(ctx->ev_done[EV_SLOT + 1], st));
     CK(cudaGetLastError());
     // the caller may reuse its image buffers as soon as we return
     CK(cudaEventSynchronize(ctx->ev_h2d[e]));
@@ -1452,7 +1319,7 @@ extern "C" int dsm_get_labels(dsm_ctx *ctx, int frame, int32_t *labels_hw)
     if (!ctx->ran) return DSM_E_STATE;
     CK(cudaSetDevice(ctx->device));
     const int W = ctx->p.width, H = ctx->p.height;
-    CK(cudaMemcpy2DAsync(labels_hw, (size_t)W * 4, ctx->d.labels + (size_t)frame * ctx->px, (size_t)ctx->Wp * 4,
+    CK(cudaMemcpy2DAsync(labels_hw, (size_t)W * 4, ctx->d.labels + (size_t)frame * ctx->d.px_stride, (size_t)ctx->d.Wp * 4,
                          (size_t)W * 4, H, cudaMemcpyDeviceToHost, ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
     return DSM_OK;
@@ -1463,9 +1330,8 @@ extern "C" int dsm_get_seeds(dsm_ctx *ctx, int frame, dsm_seed_t *seeds)
     if (!ctx || !seeds || frame < 0 || frame >= ctx->p.max_batch) return DSM_E_INVALID;
     if (!ctx->ran) return DSM_E_STATE;
     CK(cudaSetDevice(ctx->device));
-    const int plane_done = 12; // kernels of the schedule up to and including the plane fit
-    dsm_launch_seeds_export(ctx->d, frame, ctx->seed_export, (ctx->stop_after > 0 && ctx->stop_after < plane_done) ? 1 : 0, ctx->stream);
-    CK(cudaMemcpyAsync(seeds, ctx->seed_export, (size_t)ctx->S * sizeof(dsm_seed_t), cudaMemcpyDeviceToHost, ctx->stream));
+    dsm_launch_seeds_export(ctx->d, frame, ctx->seed_export, (ctx->stop_after > 0 && ctx->stop_after < kPlaneFitSteps) ? 1 : 0, ctx->stream);
+    CK(cudaMemcpyAsync(seeds, ctx->seed_export, (size_t)ctx->d.S * sizeof(dsm_seed_t), cudaMemcpyDeviceToHost, ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
     CK(cudaGetLastError());
     return DSM_OK;
@@ -1478,7 +1344,7 @@ extern "C" int dsm_device_buffer(dsm_ctx *ctx, int which, void **dev_ptr, size_t
     {
     case DSM_BUF_NEW_SURFELS:
         *dev_ptr = ctx->d.newsurf;
-        *bytes = (size_t)ctx->p.max_batch * ctx->S * sizeof(dsm_surfel_t);
+        *bytes = (size_t)ctx->p.max_batch * ctx->d.S * sizeof(dsm_surfel_t);
         return DSM_OK;
     case DSM_BUF_NEW_COUNTS:
         *dev_ptr = ctx->d.nnew;

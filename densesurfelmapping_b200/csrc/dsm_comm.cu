@@ -80,6 +80,7 @@ static DsmNccl *nccl_api()
 
 struct DsmComm
 {
+    CudaOwner own; // the buffers, streams and events below, except recv
     ncclComm_t comm = nullptr;
     int rank = 0, nranks = 1;
     cudaStream_t stream = nullptr;       // pack + collectives
@@ -87,7 +88,7 @@ struct DsmComm
     cudaEvent_t ev_packed = nullptr;     // the pack has read newsurf / pool: the next batch may overwrite them
     unsigned char *pack = nullptr;       // device: this rank's payload
     size_t pack_cap = 0;
-    unsigned char *recv = nullptr;       // device, root only: all payloads back to back
+    DevPtr<unsigned char> recv;          // device, root only: all payloads back to back (grown on demand)
     size_t recv_cap = 0;
     int64_t *d_bytes = nullptr;          // device [nranks]
     int64_t *h_bytes = nullptr;          // pinned [nranks]
@@ -104,7 +105,7 @@ struct DsmComm
     struct DsmPeerCtrl *ctrl = nullptr;  // local allocation: control block (used when this rank is the root)
     unsigned char *r_slots = nullptr;    // the ROOT's slots as seen from this rank (== slots on the root)
     struct DsmPeerCtrl *r_ctrl = nullptr;
-    bool r_mapped = false;               // r_slots / r_ctrl come from cudaIpcOpenMemHandle
+    std::unique_ptr<void, Release<void *, cudaIpcCloseMemHandle>> ipc_slots, ipc_ctrl; // other ranks: what r_slots / r_ctrl map
     unsigned long long seq = 0;          // gathers done on this mapping
     unsigned char *d_handles = nullptr;  // device staging for the handle exchange [nranks][128]
     bool last_peer = false;              // the last gather used the peer transport
@@ -135,7 +136,7 @@ struct DsmPeerCtrl
 static size_t header_bytes(int n_frames) { return ((size_t)(4 + n_frames + n_frames + 1) * 4 + 15) / 16 * 16; }
 static size_t payload_cap(const dsm_ctx *ctx)
 {
-    return header_bytes(ctx->p.max_batch) + ((size_t)ctx->p.max_batch * ctx->S + (size_t)(ctx->p.max_local_surfels > 0 ? ctx->p.max_local_surfels : 1)) * sizeof(dsm_surfel_t);
+    return header_bytes(ctx->p.max_batch) + ((size_t)ctx->p.max_batch * ctx->d.S + (size_t)(ctx->p.max_local_surfels > 0 ? ctx->p.max_local_surfels : 1)) * sizeof(dsm_surfel_t);
 }
 
 // valid new surfels of frame (frame0 + blockIdx.y) -> packed[offset of the frame .. ), one thread per 4-byte word
@@ -254,25 +255,7 @@ extern "C" int dsm_comm_destroy(dsm_ctx *ctx)
     if (c->stream) cudaStreamSynchronize(c->stream);
     DsmNccl *api = nccl_api();
     if (c->comm && api) api->CommDestroy(c->comm);
-    if (c->r_mapped)
-    {
-        cudaIpcCloseMemHandle(c->r_slots);
-        cudaIpcCloseMemHandle(c->r_ctrl);
-    }
-    if (c->poll) cudaStreamDestroy(c->poll);
-    cudaFreeHost(c->h_arrived);
-    cudaFree(c->slots);
-    cudaFree(c->ctrl);
-    cudaFree(c->d_handles);
-    cudaFree(c->pack);
-    cudaFree(c->recv);
-    cudaFree(c->d_bytes);
-    cudaFreeHost(c->h_bytes);
-    cudaFreeHost(c->h_hdr);
-    if (c->ev_kernels) cudaEventDestroy(c->ev_kernels);
-    if (c->ev_packed) cudaEventDestroy(c->ev_packed);
-    if (c->stream) cudaStreamDestroy(c->stream);
-    delete c;
+    delete c; // unmaps the root's buffers, releases every buffer, stream and event
     ctx->comm = nullptr;
     return DSM_OK;
 }
@@ -299,20 +282,27 @@ extern "C" int dsm_comm_init(dsm_ctx *ctx, const void *id, int rank, int nranks)
     ncclUniqueId uid;
     memcpy(&uid, id, DSM_COMM_ID_BYTES);
     NK(api->CommInitRank(&c->comm, nranks, uid, rank));
-    CK(cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking));
-    CK(cudaEventCreateWithFlags(&c->ev_kernels, cudaEventDisableTiming));
-    CK(cudaEventCreateWithFlags(&c->ev_packed, cudaEventDisableTiming));
+    CK(c->own.stream(&c->stream));
+    CK(c->own.event(&c->ev_kernels));
+    CK(c->own.event(&c->ev_packed));
     c->pack_cap = payload_cap(ctx);
-    CK(cudaMalloc((void **)&c->pack, c->pack_cap));
-    CK(cudaMalloc((void **)&c->d_bytes, (size_t)nranks * sizeof(int64_t)));
-    CK(cudaMallocHost((void **)&c->h_bytes, (size_t)nranks * sizeof(int64_t)));
+    CK(c->own.device(&c->pack, c->pack_cap));
+    CK(c->own.device(&c->d_bytes, (size_t)nranks));
+    CK(c->own.host(&c->h_bytes, (size_t)nranks));
     c->hdr_cap = header_bytes(ctx->p.max_batch) + (size_t)ctx->p.max_batch * 4;
-    CK(cudaMallocHost((void **)&c->h_hdr, c->hdr_cap));
+    CK(c->own.host(&c->h_hdr, c->hdr_cap / sizeof(int32_t)));
     c->ofs.assign((size_t)nranks + 1, 0);
     return DSM_OK;
 }
 
 // ---- peer-memory transport: host side ----
+static void unmap_root(DsmComm *c)
+{
+    c->ipc_slots.reset();
+    c->ipc_ctrl.reset();
+    c->r_slots = nullptr, c->r_ctrl = nullptr;
+}
+
 // Collective over the communicator (every rank calls dsm_gather_deltas with the same root): maps the root's slots and
 // control block into this process.  Leaves peer_ok false (-> NCCL transport) when any rank cannot map them.
 static int peer_setup(dsm_ctx *ctx, int root)
@@ -321,24 +311,18 @@ static int peer_setup(dsm_ctx *ctx, int root)
     DsmNccl *api = nccl_api();
     cudaStream_t cs = c->stream;
     CK(cudaStreamSynchronize(cs));
-    if (c->r_mapped)
-    {
-        cudaIpcCloseMemHandle(c->r_slots);
-        cudaIpcCloseMemHandle(c->r_ctrl);
-        c->r_mapped = false;
-    }
+    unmap_root(c);
     c->peer_root = root, c->peer_ok = false, c->seq = 0;
-    c->r_slots = nullptr, c->r_ctrl = nullptr;
     c->slot_bytes = (c->pack_cap + 255) / 256 * 256;
     if (!c->slots)
     {
-        CK(cudaMalloc((void **)&c->slots, (size_t)c->nranks * c->slot_bytes));
-        CK(cudaMalloc((void **)&c->ctrl, sizeof(DsmPeerCtrl)));
+        CK(c->own.device(&c->slots, (size_t)c->nranks * c->slot_bytes));
+        CK(c->own.device(&c->ctrl, 1));
     }
     if (!c->poll)
     {
-        CK(cudaStreamCreateWithFlags(&c->poll, cudaStreamNonBlocking));
-        CK(cudaMallocHost((void **)&c->h_arrived, DSM_MAX_RANKS * sizeof(unsigned long long)));
+        CK(c->own.stream(&c->poll));
+        CK(c->own.host(&c->h_arrived, DSM_MAX_RANKS));
     }
     c->done_seq = 0;
     CK(cudaMemsetAsync(c->ctrl, 0, sizeof(DsmPeerCtrl), cs));
@@ -356,7 +340,7 @@ static int peer_setup(dsm_ctx *ctx, int root)
     cudaGetLastError();
     memcpy(mine, &h_slots, 64);
     memcpy(mine + 64, &h_ctrl, 64);
-    if (!c->d_handles) CK(cudaMalloc((void **)&c->d_handles, (size_t)c->nranks * 128));
+    if (!c->d_handles) CK(c->own.device(&c->d_handles, (size_t)c->nranks * 128));
     CK(cudaMemcpyAsync(c->d_handles + (size_t)c->rank * 128, mine, 128, cudaMemcpyHostToDevice, cs));
     NK(api->AllGather(c->d_handles + (size_t)c->rank * 128, c->d_handles, 128, ncclInt8, c->comm, cs));
     std::vector<unsigned char> all((size_t)c->nranks * 128);
@@ -368,17 +352,17 @@ static int peer_setup(dsm_ctx *ctx, int root)
     {
         memcpy(&h_slots, all.data() + (size_t)root * 128, 64);
         memcpy(&h_ctrl, all.data() + (size_t)root * 128 + 64, 64);
-        void *p1 = nullptr, *p2 = nullptr;
-        const cudaError_t e1 = cudaIpcOpenMemHandle(&p1, h_slots, cudaIpcMemLazyEnablePeerAccess);
-        const cudaError_t e2 = e1 == cudaSuccess ? cudaIpcOpenMemHandle(&p2, h_ctrl, cudaIpcMemLazyEnablePeerAccess) : cudaErrorUnknown;
-        if (e1 == cudaSuccess && e2 == cudaSuccess)
+        void *p = nullptr;
+        if (cudaIpcOpenMemHandle(&p, h_slots, cudaIpcMemLazyEnablePeerAccess) == cudaSuccess) c->ipc_slots.reset(p);
+        if (c->ipc_slots && cudaIpcOpenMemHandle(&p, h_ctrl, cudaIpcMemLazyEnablePeerAccess) == cudaSuccess) c->ipc_ctrl.reset(p);
+        if (c->ipc_ctrl)
         {
-            c->r_slots = static_cast<unsigned char *>(p1), c->r_ctrl = static_cast<DsmPeerCtrl *>(p2);
-            c->r_mapped = true;
+            c->r_slots = static_cast<unsigned char *>(c->ipc_slots.get());
+            c->r_ctrl = static_cast<DsmPeerCtrl *>(c->ipc_ctrl.get());
         }
         else
         {
-            if (e1 == cudaSuccess) cudaIpcCloseMemHandle(p1);
+            unmap_root(c);
             cudaGetLastError();
             good = false;
         }
@@ -391,12 +375,7 @@ static int peer_setup(dsm_ctx *ctx, int root)
     CK(cudaStreamSynchronize(cs));
     bool all_good = true;
     for (int r = 0; r < c->nranks; r++) all_good &= c->h_bytes[r] == 1;
-    if (!all_good && c->r_mapped)
-    {
-        cudaIpcCloseMemHandle(c->r_slots);
-        cudaIpcCloseMemHandle(c->r_ctrl);
-        c->r_mapped = false;
-    }
+    if (!all_good && c->ipc_slots) unmap_root(c);
     c->peer_ok = all_good;
     return DSM_OK;
 }
@@ -433,7 +412,7 @@ static int gather_peer(dsm_ctx *ctx, int root)
 {
     DsmComm *c = ctx->comm;
     cudaStream_t cs = c->stream;
-    const int nb = ctx->nb, S = ctx->S;
+    const int nb = ctx->nb, S = ctx->d.S;
     const unsigned long long seq = ++c->seq;
     const unsigned hb = (unsigned)header_bytes(nb);
     CK(cudaEventRecord(c->ev_kernels, ctx->stream)); // the batch's kernels (all sub-batch streams are joined into it)
@@ -478,7 +457,7 @@ static int gather_nccl(dsm_ctx *ctx, int root)
 {
     DsmComm *c = ctx->comm;
     DsmNccl *api = nccl_api();
-    const int nb = ctx->nb, S = ctx->S;
+    const int nb = ctx->nb, S = ctx->d.S;
     // (1) new-surfel counts of the batch -> pinned memory; this waits for the batch's kernels
     int32_t *h_cnt = c->h_hdr + header_bytes(ctx->p.max_batch) / 4;
     CK(cudaStreamSynchronize(c->stream)); // the previous gather has consumed the staging buffers
@@ -532,14 +511,16 @@ static int gather_nccl(dsm_ctx *ctx, int root)
         if (total > c->recv_cap)
         { // grown on demand (first call: nranks payloads of this context's capacity)
             CK(cudaStreamSynchronize(cs));
-            cudaFree(c->recv);
-            c->recv = nullptr;
+            c->recv.reset();
+            c->recv_cap = 0;
             size_t want = (size_t)c->nranks * ((c->pack_cap + 255) / 256 * 256);
             if (want < total) want = total;
-            CK(cudaMalloc((void **)&c->recv, want));
+            void *p = nullptr;
+            CK(cudaMalloc(&p, want));
+            c->recv.reset(static_cast<unsigned char *>(p));
             c->recv_cap = want;
         }
-        CK(cudaMemcpyAsync(c->recv + c->ofs[root], c->pack, my_bytes, cudaMemcpyDeviceToDevice, cs));
+        CK(cudaMemcpyAsync(c->recv.get() + c->ofs[root], c->pack, my_bytes, cudaMemcpyDeviceToDevice, cs));
     }
     if (c->nranks > 1)
     {
@@ -547,7 +528,7 @@ static int gather_nccl(dsm_ctx *ctx, int root)
         if (c->rank == root)
         {
             for (int r = 0; r < c->nranks; r++)
-                if (r != root) NK(api->Recv(c->recv + c->ofs[r], (size_t)c->h_bytes[r], ncclInt8, r, c->comm, cs));
+                if (r != root) NK(api->Recv(c->recv.get() + c->ofs[r], (size_t)c->h_bytes[r], ncclInt8, r, c->comm, cs));
         }
         else
             NK(api->Send(c->pack, my_bytes, ncclInt8, root, c->comm, cs));
@@ -572,7 +553,7 @@ extern "C" int dsm_gathered_device(dsm_ctx *ctx, void **dev_ptr, size_t *rank_of
     if (!ctx || !dev_ptr || !rank_offsets) return DSM_E_INVALID;
     DsmComm *c = ctx->comm;
     if (!c || c->last_root != c->rank) return DSM_E_STATE;
-    *dev_ptr = c->last_peer ? c->slots : c->recv;
+    *dev_ptr = c->last_peer ? c->slots : c->recv.get();
     for (int r = 0; r <= c->nranks; r++) rank_offsets[r] = c->ofs[r];
     return DSM_OK;
 }
@@ -601,6 +582,6 @@ extern "C" int dsm_gathered_download(dsm_ctx *ctx, int rank, void *host_out, siz
     if (rcw != DSM_OK) return rcw;
     const size_t nbytes = (size_t)c->h_bytes[rank];
     if (nbytes > cap) return DSM_E_CAPACITY;
-    CK(cudaMemcpy(host_out, (c->last_peer ? c->slots : c->recv) + c->ofs[rank], nbytes, cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(host_out, (c->last_peer ? c->slots : c->recv.get()) + c->ofs[rank], nbytes, cudaMemcpyDeviceToHost));
     return DSM_OK;
 }

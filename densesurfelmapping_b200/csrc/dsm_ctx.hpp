@@ -3,9 +3,68 @@
 #pragma once
 #include "dsm_device.cuh"
 #include <cstdio>
+#include <memory>
 #include <vector>
 
 struct DsmComm; // multi-GPU state (dsm_comm.cu), nullptr until dsm_comm_init
+
+// Owning handles: each releases its resource exactly once, when it is reset or destroyed.  Internal to the library:
+// hidden, so that their template instantiations stay out of its exported symbols.
+#pragma GCC visibility push(hidden)
+template <typename H, cudaError_t (*release)(H)>
+struct Release
+{
+    void operator()(H h) const { release(h); }
+};
+template <typename T>
+using DevPtr = std::unique_ptr<T, Release<void *, cudaFree>>;
+using HostPtr = std::unique_ptr<void, Release<void *, cudaFreeHost>>;
+using StreamPtr = std::unique_ptr<CUstream_st, Release<cudaStream_t, cudaStreamDestroy>>;
+using EventPtr = std::unique_ptr<CUevent_st, Release<cudaEvent_t, cudaEventDestroy>>;
+using GraphExecPtr = std::unique_ptr<CUgraphExec_st, Release<cudaGraphExec_t, cudaGraphExecDestroy>>;
+
+// Every allocation, stream and event a context or communicator makes once and keeps for its lifetime.  The raw pointers
+// and handles the code works with (and the DsmDev the kernels receive) are views; the owner releases them when its
+// holder is deleted.  The holder's streams must be drained before that.
+struct CudaOwner
+{
+    std::vector<DevPtr<void>> dev;
+    std::vector<HostPtr> pinned;
+    std::vector<StreamPtr> streams;
+    std::vector<EventPtr> events;
+
+    template <typename T>
+    cudaError_t device(T **p, size_t n, bool zero = false)
+    {
+        cudaError_t e = cudaMalloc((void **)p, n * sizeof(T));
+        if (e == cudaSuccess) dev.emplace_back(*p);
+        if (e == cudaSuccess && zero) e = cudaMemset(*p, 0, n * sizeof(T));
+        return e;
+    }
+    template <typename T>
+    cudaError_t host(T **p, size_t n)
+    {
+        cudaError_t e = cudaMallocHost((void **)p, n * sizeof(T));
+        if (e == cudaSuccess) pinned.emplace_back(*p);
+        return e;
+    }
+    cudaError_t stream(cudaStream_t *s, int priority = 0)
+    {
+        cudaError_t e = cudaStreamCreateWithPriority(s, cudaStreamNonBlocking, priority);
+        if (e == cudaSuccess) streams.emplace_back(*s);
+        return e;
+    }
+    cudaError_t event(cudaEvent_t *ev, unsigned flags = cudaEventDisableTiming)
+    {
+        cudaError_t e = cudaEventCreateWithFlags(ev, flags);
+        if (e == cudaSuccess) events.emplace_back(*ev);
+        return e;
+    }
+};
+#pragma GCC visibility pop
+// The context types below hold these handles but keep default visibility (their own template instantiations stay
+// exported as they are); GCC's warning about that mix does not matter for types that never cross the library boundary.
+#pragma GCC diagnostic ignored "-Wattributes"
 
 struct ProfRec
 {
@@ -16,76 +75,86 @@ struct ProfRec
 // A captured kernel schedule, replayable while every launch parameter is unchanged.
 struct GraphEntry
 {
-    int f0, nf, maxper, compact;
+    int f0, nf, maxper, phase;
     const void *pool, *poolofs, *alt;
-    cudaGraphExec_t exec;
-    int phase;
+    GraphExecPtr exec;
+};
+
+// Input copy / kernel completion events (ev_h2d / ev_done) per staging area.  The index ranges overlap on purpose, and
+// waits across entry points rely on it: dsm_fuse_batch_async's chunks use EV_CHUNK + c (c < DSM_MAX_CHUNKS),
+// dsm_fuse_frame_resident's frame slots use EV_SLOT + s (s < 2) and wait for the EV_SLOT events that
+// dsm_fuse_stream_resident records at the end of every run, whose staging halves use EV_HALF + h (h < 2).
+#define DSM_MAX_CHUNKS 4
+enum
+{
+    EV_CHUNK = 0,
+    EV_SLOT = 0,
+    EV_HALF = 6,
+    EV_COUNT = 8
 };
 
 struct dsm_ctx
 {
-    dsm_params p;
-    int device;
-    cudaStream_t stream;
-    bool own_stream;
-    DsmComm *comm;
-    DsmDev d;
-    DsmMaps maps;  // TMA descriptors of labels / depth / gray for the tile kernels
-    int S, Wp;
-    size_t px;    // pitched pixels per frame
-    int nb;       // frames in the current batch
-    int n_pool;   // local surfels in the current batch
-    bool uploaded, ran;
-    bool in_flight; // a dsm_fuse_batch_async batch has been enqueued and not yet waited for
-    int stop_after; // debug: number of kernels to enqueue (<= 0: all)
+    CudaOwner own; // the buffers, streams and events below (the caller's stream excepted)
+    dsm_params p{};
+    int device = 0;
+    cudaStream_t stream = nullptr; // the caller's stream, or one of own.streams
+    DsmComm *comm = nullptr;
+    DsmDev d{};                    // geometry, constants and the batch-mode views of the buffers
+    DsmMaps maps{};                // TMA descriptors of labels / depth / gray for the tile kernels
+    int nb = 0;                    // frames in the current batch
+    int n_pool = 0;                // local surfels in the current batch
+    bool uploaded = false, ran = false;
+    bool in_flight = false; // a dsm_fuse_batch_async batch has been enqueued and not yet waited for
+    int stop_after = 0;     // debug: number of kernels to enqueue (<= 0: all)
     std::vector<GraphEntry> graphs; // CUDA-graph cache of the kernel schedule (launch-bound single-frame / small-chunk runs)
-    bool use_graphs;
-    // raw allocations (non-const views of what DsmDev holds)
-    uint8_t *gray;
-    float *depth;
-    dsm_surfel_t *pool_snap;
-    int32_t *poolofs, *refidx;
-    float *pose, *ipose;
-    dsm_seed_t *seed_export;
-    float *kx, *ky;
+    bool use_graphs = true;
+    // non-const views of what DsmDev holds, and buffers the kernels take as arguments
+    uint8_t *gray = nullptr;
+    float *depth = nullptr;
+    dsm_surfel_t *pool_snap = nullptr; // alternate pool buffer (batch snapshot / resident compaction target)
+    int32_t *poolofs = nullptr, *refidx = nullptr;
+    float *pose = nullptr, *ipose = nullptr;
+    dsm_seed_t *seed_export = nullptr;
+    float *kx = nullptr, *ky = nullptr;
     // end-to-end pipeline (dsm_fuse_batch): packed staging + copy streams + per-chunk events
-    uint8_t *gray_packed; // [B][H][W]
-    float *depth_packed;  // [B][H][W]
-    cudaStream_t s_h2d, s_d2h, s_comp[4];
-    cudaStream_t s_hi;   // highest priority: the frame-by-frame (latency-bound) phase of dsm_fuse_stream_resident
-    cudaEvent_t ev_p2;   // end of that phase, joined into the main stream
+    uint8_t *gray_packed = nullptr; // [B][H][W]
+    float *depth_packed = nullptr;  // [B][H][W]
+    cudaStream_t s_h2d = nullptr, s_d2h = nullptr, s_comp[DSM_MAX_CHUNKS] = {};
+    cudaStream_t s_hi = nullptr; // highest priority: the frame-by-frame (latency-bound) phase of dsm_fuse_stream_resident
+    cudaEvent_t ev_p2 = nullptr; // end of that phase, joined into the main stream
     // resident pool (stream mode)
-    int res_upper;      // host-side upper bound of the resident pool size (exact after a sync)
-    bool res_active;
-    int res_frame;      // frames fused in resident mode so far (selects the frame slot)
-    int32_t *res_ofs;   // device [2]: {0, resident pool size}
-    int *blkcnt, *blkofs, *newofs;
-    float *wmat;        // device copy of the 4x4 of dsm_pool_transform
+    int res_upper = 0;   // host-side upper bound of the resident pool size (exact after a sync)
+    bool res_active = false;
+    int res_frame = 0;   // frames fused in resident mode so far (selects the frame slot)
+    int32_t *res_ofs = nullptr; // device [2]: {0, resident pool size}
+    int *blkcnt = nullptr, *blkofs = nullptr, *newofs = nullptr;
+    float *wmat = nullptr; // device copy of the 4x4 of dsm_pool_transform
     // inactive store (EXPERIMENTAL, dsm_inactive_*): the attached_surfels of every pose outside the drift-free window,
     // dense on the device in retirement order; the (keyframe, offset, count) segment list lives on the host
-    dsm_surfel_t *inact;
-    int inact_cap, inact_size;
-    int32_t *inact_ofs; // device [2]
+    DevPtr<dsm_surfel_t> inact; // reallocated by dsm_inactive_reserve
+    int inact_cap = 0, inact_size = 0;
+    int32_t *inact_ofs = nullptr; // device [2]
     struct InactSeg
     {
         int kf, ofs, cnt;
     };
     std::vector<InactSeg> inact_segs;
-    cudaEvent_t ev_h2d[8], ev_done[8], ev_start;
-    cudaEvent_t ev_fork, ev_join[4]; // dsm_batch_run: fork / join of the concurrent sub-batches
-    bool single_pending;             // a dsm_fuse_frame_resident call since the last dsm_fuse_stream_resident (they share frame slots 0 / 1)
-    int run_split;                   // sub-batches per dsm_batch_run (dsm_set_concurrency)
+    cudaEvent_t ev_h2d[EV_COUNT] = {}, ev_done[EV_COUNT] = {}, ev_start = nullptr;
+    cudaEvent_t ev_fork = nullptr, ev_join[4] = {}; // dsm_batch_run: fork / join of the concurrent sub-batches
+    bool single_pending = false; // a dsm_fuse_frame_resident call since the last dsm_fuse_stream_resident (they share frame slots 0 / 1)
+    int run_split = 2;           // sub-batches per dsm_batch_run (dsm_set_concurrency)
     // pinned host staging for the small per-batch tables
-    float *h_pose; // [B][32]: pose then inverse
-    int32_t *h_ofs;
-    int32_t *h_ref;
+    float *h_pose = nullptr; // [2B][32]: pose then inverse; second half: dsm_fuse_stream_resident's own tables
+    int32_t *h_ofs = nullptr;
+    int32_t *h_ref = nullptr; // [2B], halves as h_pose
     // profiling
-    uint32_t prof_mask;
+    uint32_t prof_mask = 0;
     std::vector<ProfRec> prof_pending;
     std::vector<cudaEvent_t> ev_free;
-    float prof_ms[DSM_NUM_KERNELS];
-    int32_t prof_n[DSM_NUM_KERNELS];
-    char err[512];
+    float prof_ms[DSM_NUM_KERNELS] = {};
+    int32_t prof_n[DSM_NUM_KERNELS] = {};
+    char err[512] = {};
 };
 
 #define CK(call)                                                                                         \
