@@ -1319,6 +1319,8 @@ extern "C" int dsm_get_labels(dsm_ctx *ctx, int frame, int32_t *labels_hw)
     if (!ctx->ran) return DSM_E_STATE;
     CK(cudaSetDevice(ctx->device));
     const int W = ctx->p.width, H = ctx->p.height;
+    dsm_launch_labels_export(ctx->d, frame, ctx->stream); // the schedule keeps the labels as the u8 code plane only
+    CK(cudaGetLastError());
     CK(cudaMemcpy2DAsync(labels_hw, (size_t)W * 4, ctx->d.labels + (size_t)frame * ctx->d.px_stride, (size_t)ctx->d.Wp * 4,
                          (size_t)W * 4, H, cudaMemcpyDeviceToHost, ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));

@@ -4,9 +4,10 @@
 //   gray    u8  [B][H][Wp]      Wp = W rounded up to 16 so every row starts 16-byte aligned
 //   depth   f32 [B][H][Wp]      (vector loads, TMA boxes; SURVEY.md section 7 H8)
 //   invd    f32 [B][H][Wp]      (float)(1.0 / (double)depth) for depth > 0.01, else 0 (:404-405): what the assign passes read
-//   labels  i32 [B][H][Wp]      superpixel_index of the reference (fusion_functions.h:37)
-//   code    u8  [B][H][Wp]      the same label as the index of the winning candidate among the pixel's 2x2 candidate seeds:
-//                               what the window gathers test (1 B/px, a byte compare against a position-only pattern)
+//   code    u8  [B][H][Wp]      superpixel_index of the reference (fusion_functions.h:37) as the index of the winning
+//                               candidate among the pixel's 2x2 candidate seeds (dsm_code_seed): the only label state of
+//                               the schedule (1 B/px; the window gathers test it with a byte compare against a position-only pattern)
+//   labels  i32 [B][H][Wp]      download buffer: filled from the code plane by dsm_get_labels only
 //   seed    float4 [B][S]       (x, y, mean_intensity, mean_depth)  -- the clustering state
 //   seed_hl float2 [B][S]       1.0 / (double)mean_depth as hi + lo floats (fp32 cost filter of the assign pass)
 //   inv_md  f64 [B][S]          1.0 / (double)mean_depth (exact path of the assign pass, :380)
@@ -78,7 +79,7 @@ struct DsmDev
     const int32_t *refidx;
     int max_pool_per_frame; // largest per-frame pool slice in this batch (grid sizing)
     // tile path (dsm_tile.cu)
-    uint8_t *code;      // [B][H][Wp] label of every pixel as the index (0..3) of the winning candidate among its 2x2 candidate seeds (mirror of labels)
+    uint8_t *code;      // [B][H][Wp] label of every pixel as the index (0..3) of the winning candidate among its 2x2 candidate seeds, or DSM_CODE_NONE
     float *invd;        // [B][H][Wp] (float)(1.0 / (double)depth) for depth > 0.01, else 0 (:404-405), written by the first assign pass
     float2 *seed_hl;    // [B][S] 1.0 / (double)mean_depth split into two floats (hi, lo) for the filtered assign pass
     int32_t *hardq;     // [B][S] seeds whose Huber-Newton needs the entry-by-entry classification (k_newton2 -> k_newton_hard)
@@ -86,6 +87,16 @@ struct DsmDev
     int32_t *done;      // [B] frame-completion tickets of the assign pass (the last CTA of a frame runs the stable relaxation)
     double *hrec;       // [B][24][S] plane fit, first residual pass: H = sum 2 q q^T (9), the same over out-of-range points (10), their clamped gradient (4), packed (margin, qmax2)
 };
+
+// Label code of a pixel: which of its (at most) 2x2 candidate seeds it is labelled with, c = 2*ix + iy over the seed
+// columns {xa, xa+1} and rows {ya, ya+1}, xa = floor((x - 4) / 8), ya = floor((y - 4) / 8) (the candidate set depends on
+// the pixel position only, :413-422), or DSM_CODE_NONE for a pixel the reference would have left without any label
+// (input domain, DESIGN.md 1.3), which is labelled 0.
+#define DSM_CODE_NONE 4
+__device__ __forceinline__ int dsm_code_seed(int c, int x, int y, int spw)
+{
+    return c == DSM_CODE_NONE ? 0 : (((y - 4) >> 3) + (c & 1)) * spw + ((x - 4) >> 3) + (c >> 1);
+}
 
 // TMA descriptors (cuTensorMapEncodeTiled) of the three per-pixel arrays as [B][H][Wp] tensors; box = one seed tile plus halo
 struct DsmMaps
@@ -123,6 +134,7 @@ void dsm_launch_seed_init(const DsmDev &d, int nb, cudaStream_t s);
 void dsm_launch_fuse(const DsmDev &d, int nb, cudaStream_t s);
 void dsm_launch_init_surfels(const DsmDev &d, int nb, cudaStream_t s);
 void dsm_launch_seeds_export(const DsmDev &d, int frame, dsm_seed_t *out_dev, int raw_md, cudaStream_t s);
+void dsm_launch_labels_export(const DsmDev &d, int frame, cudaStream_t s);
 void dsm_launch_pool_compact(const DsmDev &d, int frame, int upper, int *blkcnt, int *blkofs, int *newofs, dsm_surfel_t *dst, int32_t *ofs_out, cudaStream_t s);
 void dsm_launch_pool_transform(const DsmDev &d, int frame, int upper, const float *Wm_dev, cudaStream_t s);
 void dsm_launch_pool_export(const DsmDev &d, int frame, int upper, int mode, int key, bool as_cloud, int *blkcnt, int *blkofs, int *newofs, void *dst, cudaStream_t s);

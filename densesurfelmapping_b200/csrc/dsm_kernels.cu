@@ -237,7 +237,7 @@ __global__ void __launch_bounds__(FUSE_BLOCK) k_fuse(const __grid_constant__ Dsm
                 e[9] = __int_as_float(0);
                 break;
             }
-            const int sp = d.labels[fo + (size_t)vi * Wp + ui];
+            const int sp = dsm_code_seed(d.code[fo + (size_t)vi * Wp + ui], ui, vi, d.spw);
             const float4 *pl = d.plane + (so + sp) * 3;
             const float4 r0 = pl[0]; // n, view_cos
             if (r0.x == 0 && r0.y == 0 && r0.z == 0) break;
@@ -543,6 +543,15 @@ __global__ void k_seeds_export(const __grid_constant__ DsmDev d, int b, dsm_seed
     out[s] = e;
 }
 
+// parity readback: the reference's int32 superpixel_index of one frame, from the label codes
+__global__ void k_labels_export(const __grid_constant__ DsmDev d, int b)
+{
+    const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y;
+    if (x >= d.W) return;
+    const size_t o = (size_t)b * d.px_stride + (size_t)y * d.Wp + x;
+    d.labels[o] = dsm_code_seed(d.code[o], x, y, d.spw);
+}
+
 // -------------------------------------------------------------------------------------------
 // launchers
 // -------------------------------------------------------------------------------------------
@@ -571,6 +580,10 @@ void dsm_launch_init_surfels(const DsmDev &d, int nb, cudaStream_t s)
 void dsm_launch_seeds_export(const DsmDev &d, int frame, dsm_seed_t *out_dev, int raw_md, cudaStream_t s)
 {
     k_seeds_export<<<(d.S + 255) / 256, 256, 0, s>>>(d, frame, out_dev, raw_md);
+}
+void dsm_launch_labels_export(const DsmDev &d, int frame, cudaStream_t s)
+{
+    k_labels_export<<<dim3((d.W + 255) / 256, d.H), 256, 0, s>>>(d, frame);
 }
 
 // ofs_out (may be null): the resident pool's offset table {0, n}; the last kernel of the chain stores the new size there

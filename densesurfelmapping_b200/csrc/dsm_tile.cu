@@ -53,9 +53,9 @@ __device__ __forceinline__ void tma_load_3d(unsigned dst, const CUtensorMap *map
 // -------------------------------------------------------------------------------------------
 // K1  slic_assign (filtered) — update_pixels_kernel (:389-453) + calculate_cost (:364-387)
 //
-// A thread owns 4 consecutive pixels of one row (CTA = 64 x 2 threads = 256 x 2 pixels); the at most 2 x 2 candidate
-// seeds are shared by the four pixels.  The reference walks the image in raster order and skips a pixel whose current
-// seed is `stable` at that moment (:400); `stable` flips during the walk (:445/:450).  Here every seed carries a time
+// A thread owns 4 consecutive pixels of one row at a time (CTA = 64 x 2 threads, walking the 256 x 8 pixels of one seed
+// row band in four steps of two rows); the at most 2 x 2 candidate seeds are shared by the four pixels.  The reference
+// walks the image in raster order and skips a pixel whose current seed is `stable` at that moment (:400); `stable` flips during the walk (:445/:450).  Here every seed carries a time
 // stamp (tstable: -1 = unstable since the start of the pass, DSM_STABLE, or the raster index at which it became
 // unstable); pixels of seeds unstable from the start commit at once, the others are deferred to the frame's relaxation
 // (SURVEY.md H1).  How the winner of a pixel is found:
@@ -69,13 +69,24 @@ __device__ __forceinline__ void tma_load_3d(unsigned dst, const CUtensorMap *map
 //               same candidate whatever the visiting order, and it is below the 1e6 start value (m1 < 9e5).
 //   exact path  everything else (ties -- common on synthetic constant images --, near ties, all costs >= 9e5):
 //               calc_cost, expression by expression as the reference.
+// The labels live in the u8 code plane only (dsm_code_seed turns a code and the pixel position into the seed index).
 // The first pass also writes the inverse-depth plane the later passes read instead of the depth image.
+// The fast-path operands and time stamps of the CTA's candidate seeds are staged once in shared memory: its pixel rows
+// 8 blockIdx.y ... + 7 see the seed rows blockIdx.y - 1 ... blockIdx.y + 1 and its 256 pixel columns the 34 seed columns
+// 32 blockIdx.x - 1 ... 32 blockIdx.x + 32, so a thread reads its four candidates at fixed shared-memory offsets, and a
+// seed outside the image is a record 1e18 away: its cost (~1e36, finite) is never the minimum and the filter arithmetic
+// stays NaN-free.  Stamps read at the start of the pass are good enough for both uses: "unstable since the start"
+// (t < 0) does not change during the pass, and the others only decrease, so t_start <= idx implies t <= idx.
 // The last CTA of a frame to finish (ticket counter) runs the raster-order `stable` relaxation (relax_frame) for
-// that frame, so the pass needs no separate one-CTA-per-frame launch.
+// that frame, so the pass needs no separate one-CTA-per-frame launch.  A CTA covers 8 pixel rows so that the staging
+// barrier and the ticket (a fence and an L2 round trip while the CTA holds its slot) are paid once per 2048 pixels.
 // -------------------------------------------------------------------------------------------
 #define A_EPS 3.814697265625e-06f // 2^-18
 #define A_ALPHA 1e-10f
 #define A_BIG 1e30f
+#define A_REC 34 // staged seed columns per candidate row
+#define A_STEPS 4 // pixel row pairs per CTA: rows 8 blockIdx.y ... + 7
+#define A_NR 3    // staged seed rows: blockIdx.y - 1 ... blockIdx.y + 1
 
 __device__ __forceinline__ void relax_frame(const DsmDev &d, int b, int tid, int nthreads)
 {
@@ -84,9 +95,9 @@ __device__ __forceinline__ void relax_frame(const DsmDev &d, int b, int tid, int
     {
         const size_t fo = (size_t)b * d.px_stride;
         int2 *list = d.list + fo;
-        int32_t *labels = d.labels + fo;
         uint8_t *codes = d.code + fo;
         int32_t *t = d.tstable + (size_t)b * d.S;
+        const int Wp = d.Wp;
         for (;;)
         {
             int changed = 0;
@@ -94,11 +105,11 @@ __device__ __forceinline__ void relax_frame(const DsmDev &d, int b, int tid, int
             {
                 const int2 en = __ldcg(&list[e]);
                 if (en.x < 0) continue; // already evaluated
-                const int owner = __ldcg(&labels[en.x]);
+                const int py = en.x / Wp;
+                const int owner = dsm_code_seed(__ldcg(&codes[en.x]), en.x - py * Wp, py, d.spw);
                 if (__ldcg(&t[owner]) < en.x)
                 {
                     const int win = en.y & 0x0fffffff; // entry: winner seed | winner's candidate code << 28
-                    labels[en.x] = win;
                     codes[en.x] = (uint8_t)(en.y >> 28);
                     list[e].x = -1;
                     if (__ldcg(&t[win]) > en.x) atomicMin(&t[win], en.x);
@@ -120,226 +131,243 @@ __device__ __forceinline__ float pick4(float a0, float a1, float a2, float a3, i
     return i == 0 ? a0 : (i == 1 ? a1 : (i == 2 ? a2 : a3));
 }
 
-// label code of a pixel: which of its (at most) 2x2 candidate seeds it is labelled with, c = 2*ix + iy over the columns
-// {xa, xa+1} and rows {ya, ya+1} defined below (the candidate set depends on the pixel position only, :413-422), or
-// DSM_CODE_NONE for a pixel the reference would have left without any label (input domain, DESIGN.md 1.3).  The u8 code
-// plane mirrors the int32 labels; the passes that only need "is this pixel a member of seed s" read it instead
-// (1 byte per pixel, and the test is a byte compare with a pattern that depends on the window position only).
-#define DSM_CODE_NONE 4
-
 template <bool FIRST>
 __global__ void __launch_bounds__(128, 8) k_assign2(const __grid_constant__ DsmDev d)
 {
     pdl_enter();
+    __shared__ float4 s_rec[A_NR * A_REC + 1]; // (x/4, y/4, mean_intensity, hi) of seed rows blockIdx.y - 1 .. + 1, then the no-seed record
+    __shared__ float s_lo[A_NR * A_REC + 1];   // lo of 1.0 / (double)mean_depth = hi + lo
+    __shared__ int s_ts[A_NR * A_REC + 1];     // time stamps at the start of the pass
     __shared__ int s_last;
     const int b = d.frame0 + blockIdx.z;
+    const int tid = threadIdx.y * 64 + threadIdx.x;
     const int x4 = (blockIdx.x * 64 + threadIdx.x) * 4;
-    const int y = blockIdx.y * blockDim.y + threadIdx.y; // 128-thread CTAs (64 x 2): finer scheduling granularity than 256
     const int lane = threadIdx.x & 31;
-    const bool active = (x4 < d.W) && (y < d.H);
-
+    const bool half = threadIdx.x & 1; // x4 % 8 == 4: pixel 0 sees only its own seed column (:418-420)
+    const int ia = (threadIdx.x + 1) >> 1; // staged column of the thread's candidate column xa = floor((x4 - 4) / 8)
     const size_t fo = (size_t)b * d.px_stride;
     const size_t so = (size_t)b * d.S;
-    int wc[4] = {DSM_CODE_NONE, DSM_CODE_NONE, DSM_CODE_NONE, DSM_CODE_NONE}; // winner of every pixel as a candidate code
-    int oc[4] = {0, 0, 0, 0};                                                 // current label as a candidate code
-    int sidx0 = 0;                                                            // seed index of candidate 0; candidate c = sidx0 + (c & 1) * spw + (c >> 1)
-    if (active)
-    {
-        const size_t po = fo + (size_t)y * d.Wp + x4;
-        const uchar4 g4 = *reinterpret_cast<const uchar4 *>(d.gray + po);
-        float iv[4];
-        if (FIRST)
-        { // (:404-405) my_inv = (float)(1.0 / (double)depth) for depth > 0.01: 53 >= 2*24+2 bits, so the double rounding is
-          // innocuous and the correctly rounded float reciprocal is the same value (-ftz=false: subnormals included)
-            const float4 z4 = *reinterpret_cast<const float4 *>(d.depth + po);
-            iv[0] = (z4.x > F_0p01_LO) ? __frcp_rn(z4.x) : 0.0f;
-            iv[1] = (z4.y > F_0p01_LO) ? __frcp_rn(z4.y) : 0.0f;
-            iv[2] = (z4.z > F_0p01_LO) ? __frcp_rn(z4.z) : 0.0f;
-            iv[3] = (z4.w > F_0p01_LO) ? __frcp_rn(z4.w) : 0.0f;
-            *reinterpret_cast<float4 *>(d.invd + po) = make_float4(iv[0], iv[1], iv[2], iv[3]);
-        }
-        else
-        {
-            const float4 i4 = *reinterpret_cast<const float4 *>(d.invd + po);
-            iv[0] = i4.x, iv[1] = i4.y, iv[2] = i4.z, iv[3] = i4.w;
-            const uchar4 c4 = *reinterpret_cast<const uchar4 *>(d.code + po);
-            oc[0] = c4.x, oc[1] = c4.y, oc[2] = c4.z, oc[3] = c4.w;
-        }
-        const float gi[4] = {(float)g4.x, (float)g4.y, (float)g4.z, (float)g4.w};
-        const int bx = x4 >> 3, by = y >> 3, rx0 = x4 & 7, ry = y & 7;
-        const int xa = (rx0 == 0) ? bx - 1 : bx, xb = xa + 1;
-        const int ya = (ry < 4) ? by - 1 : by, yb = ya + 1;
-        const bool vxa = xa >= 0 && xa < d.spw, vxb = xb >= 0 && xb < d.spw;
-        const bool vya = ya >= 0 && ya < d.sph, vyb = (ry != 4) && yb >= 0 && yb < d.sph;
-        sidx0 = ya * d.spw + xa;
-        // candidate c = 2*ix + iy  -> (xa,ya) (xa,yb) (xb,ya) (xb,yb): dx outer, dy inner (:413-414)
-        // fast-path operands, shared by the thread's 4 pixels.  Coordinates are pre-scaled by 1/4 (exact), so that
-        // dist/16 (:374) is ax'^2 + ay'^2; an invalid candidate sits 1e18 away: its cost (~1e36, finite) is never the minimum
-        // and the filter arithmetic stays NaN-free.  When the pixel at x%8 == 4 sees only its own seed column (:418-420)
-        // the candidates of column xb get the same treatment for that pixel only (sxq0).
-        float sxq[4], sxq0[4], ayy[4], sI[4], shi[4], slo[4];
-        bool sv[4];
-        bool allmd = true, allmd0 = true; // every valid candidate seed has mean_depth > 0 (:378), over 4 / over column xa only
-        const float fyq = (float)y * 0.25f;
-#pragma unroll
-        for (int c = 0; c < 4; c++)
-        {
-            sv[c] = ((c >> 1) ? vxb : vxa) && ((c & 1) ? vyb : vya);
-            const int li = sv[c] ? sidx0 + (c & 1) * d.spw + (c >> 1) : 0; // invalid candidates read seed 0 and are pushed away below
-            const float4 s4 = d.seed[so + li];
-            const float2 hl = d.seed_hl[so + li];
-            sxq[c] = sv[c] ? s4.x * 0.25f : 1e18f;
-            sxq0[c] = ((c >> 1) && rx0 == 4) ? 1e18f : sxq[c];
-            const float ay = s4.y * 0.25f - fyq;
-            ayy[c] = ay * ay;
-            sI[c] = s4.z, shi[c] = hl.x, slo[c] = hl.y;
-            const bool mdpos = s4.w > 0.f || !sv[c];
-            allmd &= mdpos;
-            if (!(c >> 1)) allmd0 &= mdpos;
-        }
-        if (rx0 != 4) allmd0 = allmd;
-        unsigned uncertain = 0;
-#pragma unroll
-        for (int i = 0; i < 4; i++)
-        {
-            const float fxq = (float)(x4 + i) * 0.25f;
-            const float pi = gi[i], pv = iv[i];
-            // all_has_depth (:443): every valid candidate has a depth and so has the pixel -> costs with the depth term, else without
-            const float w = (pv > 0.f && (i == 0 ? allmd0 : allmd)) ? 400.f : 0.f;
-            float cost[4];
-#pragma unroll
-            for (int c = 0; c < 4; c++)
-            {
-                const float ax = (i == 0 ? sxq0[c] : sxq[c]) - fxq;
-                const float n = fmaf(ax, ax, ayy[c]);
-                const float idf = sI[c] - pi;
-                const float cn = fmaf(idf * idf, 0.01f, n);
-                const float t = (shi[c] - pv) + slo[c];
-                cost[c] = fmaf(t * t, w, cn);
-            }
-            const float lo01 = fminf(cost[0], cost[1]), hi01 = fmaxf(cost[0], cost[1]);
-            const float lo23 = fminf(cost[2], cost[3]), hi23 = fmaxf(cost[2], cost[3]);
-            const float m1 = fminf(lo01, lo23);
-            const float m2 = fminf(fminf(fmaxf(lo01, lo23), fminf(hi01, hi23)), A_BIG); // second smallest, kept finite
-            wc[i] = cost[0] == m1 ? 0 : (cost[1] == m1 ? 1 : (cost[2] == m1 ? 2 : 3));
-            const bool certain = (m2 - m1 > A_EPS * (m2 + m1) + A_ALPHA) && (m1 < 9e5f);
-            if (!certain) uncertain |= 1u << i;
-        }
-        if (uncertain)
-        { // exact path: the reference's expression, candidate order and strict '<' (first wins).  Each lane walks its OWN
-          // flagged pixels, so a warp pays max-per-lane (usually one) exact evaluations, not one per pixel slot.
-            SeedC sc[4];
-#pragma unroll
-            for (int c = 0; c < 4; c++)
-            {
-                const int li = sv[c] ? sidx0 + (c & 1) * d.spw + (c >> 1) : 0;
-                const float4 s4 = d.seed[so + li];
-                sc[c].x = s4.x, sc[c].y = s4.y, sc[c].I = s4.z, sc[c].md = s4.w;
-                sc[c].inv = d.inv_md[so + li]; // 1.0 / (double)mean_depth, only consumed when mean_depth > 0 (:378)
-            }
-            const float fy = (float)y;
-            while (uncertain)
-            {
-                const int i = __ffs(uncertain) - 1;
-                uncertain &= uncertain - 1;
-                const float fx = (float)(x4 + i);
-                const float my_i = pick4(gi[0], gi[1], gi[2], gi[3], i);
-                const float my_inv = pick4(iv[0], iv[1], iv[2], iv[3], i);
-                const double my_inv_d = (double)my_inv;
-                float min_d = 1e6f, min_nd = 1e6f;
-                int idx_d = DSM_CODE_NONE, idx_nd = DSM_CODE_NONE; // the reference's -1 (:409-411)
-                bool all_has_depth = true;
-#pragma unroll
-                for (int c = 0; c < 4; c++)
-                {
-                    const bool valid = sv[c] && ((c >> 1) ? !(rx0 == 4 && i == 0) : true);
-                    float cnd, cdd;
-                    const bool has = calc_cost(sc[c], my_i, my_inv, my_inv_d, fx, fy, cnd, cdd);
-                    cdd = valid ? cdd : __int_as_float(0x7f800000);
-                    cnd = valid ? cnd : __int_as_float(0x7f800000);
-                    all_has_depth &= has || !valid;
-                    const bool bd = cdd < min_d, bn = cnd < min_nd;
-                    min_d = bd ? cdd : min_d;
-                    idx_d = bd ? c : idx_d;
-                    min_nd = bn ? cnd : min_nd;
-                    idx_nd = bn ? c : idx_nd;
-                }
-                const int wv = all_has_depth ? idx_d : idx_nd;
-                wc[0] = i == 0 ? wv : wc[0];
-                wc[1] = i == 1 ? wv : wc[1];
-                wc[2] = i == 2 ? wv : wc[2];
-                wc[3] = i == 3 ? wv : wc[3];
-            }
-        }
-#pragma unroll
-        for (int i = 0; i < 4; i++)
-            if (x4 + i >= d.W) wc[i] = DSM_CODE_NONE;
-    }
-    const int spw = d.spw;
-    auto seed_of = [&](int c) { return c == DSM_CODE_NONE ? 0 : sidx0 + (c & 1) * spw + (c >> 1); }; // a pixel without winner is labelled 0
+    const uint8_t *const gray = d.gray + fo; // the frame's planes, indexed with 32-bit in-frame offsets
+    float *const invd = d.invd + fo;
+    uint8_t *const codes = d.code + fo;
 
-    if (FIRST)
-    { // every label is 0 and seed 0 is unstable: everything commits (:400)
+    // stage the fast-path operands of the CTA's candidate seeds.  Coordinates are pre-scaled by 1/4 (exact), so that
+    // dist/16 (:374) is ax'^2 + ay'^2.  hi > 0 iff mean_depth > 0 (split_inverse); a seed outside the image, and the
+    // no-seed record, have hi = 1: they never clear all_has_depth (:443), like the reference's skipped candidates.
+    const int ya0 = (int)blockIdx.y - 1; // first candidate seed row of the CTA: floor((8 blockIdx.y - 4) / 8)
+    if (tid <= A_NR * A_REC)
+    {
+        const int row = tid / A_REC;
+        const int sx = (int)blockIdx.x * 32 - 1 + tid - row * A_REC, sy = ya0 + row;
+        float4 r = make_float4(1e18f, 0.f, 0.f, 1.f);
+        float lo = 0.f;
+        int ts = DSM_STABLE;
+        if (tid < A_NR * A_REC && sx >= 0 && sx < d.spw && sy >= 0 && sy < d.sph)
+        {
+            const int s = sy * d.spw + sx;
+            const float4 s4 = d.seed[so + s];
+            const float2 hl = d.seed_hl[so + s];
+            if (!FIRST) ts = d.tstable[so + s];
+            r = make_float4(s4.x * 0.25f, s4.y * 0.25f, s4.z, hl.x);
+            lo = hl.y;
+        }
+        s_rec[tid] = r;
+        s_lo[tid] = lo;
+        s_ts[tid] = ts;
+    }
+    __syncthreads();
+
+#pragma unroll 1
+    for (int step = 0; step < A_STEPS; step++)
+    {
+        const int y = blockIdx.y * 2 * A_STEPS + step * 2 + threadIdx.y;
+        const bool active = (x4 < d.W) && (y < d.H);
+        const int ra = (((y - 4) >> 3) - ya0) * A_REC; // staged row of the candidate row ya = floor((y - 4) / 8)
+        const int po = y * d.Wp + x4;        // in-frame pixel offset, a multiple of 4 (the code stores index uchar4 by po / 4,
+                                             // which keeps a 64-bit address out of the registers live across the exact path)
+        int wc[4] = {DSM_CODE_NONE, DSM_CODE_NONE, DSM_CODE_NONE, DSM_CODE_NONE}; // winner of every pixel as a candidate code
+        int oc[4] = {0, 0, 0, 0};                                                 // current label as a candidate code
         if (active)
         {
-            const size_t po = fo + (size_t)y * d.Wp + x4;
-            *reinterpret_cast<int4 *>(d.labels + po) = make_int4(seed_of(wc[0]), seed_of(wc[1]), seed_of(wc[2]), seed_of(wc[3]));
-            *reinterpret_cast<uchar4 *>(d.code + po) = make_uchar4(wc[0], wc[1], wc[2], wc[3]);
-        }
-        return;
-    }
-
-    // ---- iterations 2..: commit / defer (SURVEY.md H1).  A deferred pixel whose winner IS its current label is dropped:
-    // if the raster scan evaluates it (t[label] < idx) the label does not change and the stamp t[winner] = t[label] is
-    // already below idx, so it can change nothing -- the relaxation only ever needs the pixels that would switch seeds.
-    int2 ent[4];
-    int nent = 0;
-    if (active)
-    {
-        bool changed = false;
-        const int32_t *ts = d.tstable + so;
-        // Only a pixel whose winner differs from its label has anything to do: with winner == label an evaluated pixel
-        // keeps its label and its stamp update min(t[label], idx) is a no-op (the owner is unstable, t[label] < 0 <= idx),
-        // and a pixel of a stable owner would be deferred only to be dropped again (see above).  So the stamps are read
-        // for the few switching pixels only.
-#pragma unroll
-        for (int i = 0; i < 4; i++)
-        {
-            if (x4 + i >= d.W || wc[i] == DSM_CODE_NONE || wc[i] == oc[i]) continue;
-            const int pidx = y * d.Wp + x4 + i;
-            const int win = seed_of(wc[i]);
-            if (ts[seed_of(oc[i])] < 0)
-            { // owner unstable since the start of the pass: the reference evaluates this pixel
-                oc[i] = wc[i];
-                changed = true;
-                if (ts[win] > pidx) atomicMin(&d.tstable[so + win], pidx); // stable = false at time pidx (:445/:450)
+            const uchar4 g4 = *reinterpret_cast<const uchar4 *>(gray + po);
+            float iv[4];
+            if (FIRST)
+            { // (:404-405) my_inv = (float)(1.0 / (double)depth) for depth > 0.01: 53 >= 2*24+2 bits, so the double rounding is
+              // innocuous and the correctly rounded float reciprocal is the same value (-ftz=false: subnormals included)
+                const float4 z4 = *reinterpret_cast<const float4 *>(d.depth + fo + po);
+                iv[0] = (z4.x > F_0p01_LO) ? __frcp_rn(z4.x) : 0.0f;
+                iv[1] = (z4.y > F_0p01_LO) ? __frcp_rn(z4.y) : 0.0f;
+                iv[2] = (z4.z > F_0p01_LO) ? __frcp_rn(z4.z) : 0.0f;
+                iv[3] = (z4.w > F_0p01_LO) ? __frcp_rn(z4.w) : 0.0f;
+                *reinterpret_cast<float4 *>(invd + po) = make_float4(iv[0], iv[1], iv[2], iv[3]);
             }
             else
             {
-                ent[nent++] = make_int2(pidx, win | (wc[i] << 28));
+                const float4 i4 = *reinterpret_cast<const float4 *>(invd + po);
+                iv[0] = i4.x, iv[1] = i4.y, iv[2] = i4.z, iv[3] = i4.w;
+                const uchar4 c4 = *reinterpret_cast<const uchar4 *>(codes + po);
+                oc[0] = c4.x, oc[1] = c4.y, oc[2] = c4.z, oc[3] = c4.w;
             }
+            const float gi[4] = {(float)g4.x, (float)g4.y, (float)g4.z, (float)g4.w};
+            // candidate c = 2*ix + iy  -> (xa,ya) (xa,yb) (xb,ya) (xb,yb): dx outer, dy inner (:413-414), staged at
+            // ra + (c & 1) * A_REC + ia + (c >> 1).  The pixel row y % 8 == 4 has no candidate row yb: it reads the no-seed
+            // record instead.  When the pixel at x%8 == 4 sees only its own seed column (:418-420) the candidates of column xb
+            // are pushed away for that pixel only (sxq0).
+            const bool rowb = (y & 7) != 4;
+            const int ri[4] = {ra + ia, rowb ? ra + A_REC + ia : A_NR * A_REC, ra + ia + 1, rowb ? ra + A_REC + ia + 1 : A_NR * A_REC};
+            float sxq[4], sxq0[4], ayy[4], sI[4], shi[4], slo[4];
+            bool allmd = true, allmd0 = true; // every valid candidate seed has mean_depth > 0 (:378), over 4 / over column xa only
+            const float fyq = (float)y * 0.25f;
+#pragma unroll
+            for (int c = 0; c < 4; c++)
+            {
+                const float4 r = s_rec[ri[c]];
+                slo[c] = s_lo[ri[c]];
+                sxq[c] = r.x;
+                sxq0[c] = ((c >> 1) && half) ? 1e18f : r.x;
+                const float ay = r.y - fyq;
+                ayy[c] = ay * ay;
+                sI[c] = r.z, shi[c] = r.w;
+                const bool mdpos = r.w > 0.f;
+                allmd &= mdpos;
+                if (!(c >> 1)) allmd0 &= mdpos;
+            }
+            if (!half) allmd0 = allmd;
+            unsigned uncertain = 0;
+#pragma unroll
+            for (int i = 0; i < 4; i++)
+            {
+                const float fxq = (float)(x4 + i) * 0.25f;
+                const float pi = gi[i], pv = iv[i];
+                // all_has_depth (:443): every valid candidate has a depth and so has the pixel -> costs with the depth term, else without
+                const float w = (pv > 0.f && (i == 0 ? allmd0 : allmd)) ? 400.f : 0.f;
+                float cost[4];
+#pragma unroll
+                for (int c = 0; c < 4; c++)
+                {
+                    const float ax = (i == 0 ? sxq0[c] : sxq[c]) - fxq;
+                    const float n = fmaf(ax, ax, ayy[c]);
+                    const float idf = sI[c] - pi;
+                    const float cn = fmaf(idf * idf, 0.01f, n);
+                    const float t = (shi[c] - pv) + slo[c];
+                    cost[c] = fmaf(t * t, w, cn);
+                }
+                const float lo01 = fminf(cost[0], cost[1]), hi01 = fmaxf(cost[0], cost[1]);
+                const float lo23 = fminf(cost[2], cost[3]), hi23 = fmaxf(cost[2], cost[3]);
+                const float m1 = fminf(lo01, lo23);
+                const float m2 = fminf(fminf(fmaxf(lo01, lo23), fminf(hi01, hi23)), A_BIG); // second smallest, kept finite
+                wc[i] = cost[0] == m1 ? 0 : (cost[1] == m1 ? 1 : (cost[2] == m1 ? 2 : 3));
+                const bool certain = (m2 - m1 > A_EPS * (m2 + m1) + A_ALPHA) && (m1 < 9e5f);
+                if (!certain) uncertain |= 1u << i;
+            }
+            if (uncertain)
+            { // exact path: the reference's expression, candidate order and strict '<' (first wins).  Each lane walks its OWN
+              // flagged pixels, so a warp pays max-per-lane (usually one) exact evaluations, not one per pixel slot.
+                const int xa = (x4 - 4) >> 3, ya = (y - 4) >> 3;
+                const bool vx[2] = {xa >= 0 && xa < d.spw, xa + 1 >= 0 && xa + 1 < d.spw};
+                const bool vy[2] = {ya >= 0 && ya < d.sph, rowb && ya + 1 >= 0 && ya + 1 < d.sph};
+                SeedC sc[4];
+                bool sv[4];
+#pragma unroll
+                for (int c = 0; c < 4; c++)
+                {
+                    sv[c] = vx[c >> 1] && vy[c & 1];
+                    const int li = sv[c] ? dsm_code_seed(c, x4, y, d.spw) : 0;
+                    const float4 s4 = d.seed[so + li];
+                    sc[c].x = s4.x, sc[c].y = s4.y, sc[c].I = s4.z, sc[c].md = s4.w;
+                    sc[c].inv = d.inv_md[so + li]; // 1.0 / (double)mean_depth, only consumed when mean_depth > 0 (:378)
+                }
+                const float fy = (float)y;
+                while (uncertain)
+                {
+                    const int i = __ffs(uncertain) - 1;
+                    uncertain &= uncertain - 1;
+                    const float fx = (float)(x4 + i);
+                    const float my_i = pick4(gi[0], gi[1], gi[2], gi[3], i);
+                    const float my_inv = pick4(iv[0], iv[1], iv[2], iv[3], i);
+                    const double my_inv_d = (double)my_inv;
+                    float min_d = 1e6f, min_nd = 1e6f;
+                    int idx_d = DSM_CODE_NONE, idx_nd = DSM_CODE_NONE; // the reference's -1 (:409-411)
+                    bool all_has_depth = true;
+#pragma unroll
+                    for (int c = 0; c < 4; c++)
+                    {
+                        const bool valid = sv[c] && ((c >> 1) ? !(half && i == 0) : true);
+                        float cnd, cdd;
+                        const bool has = calc_cost(sc[c], my_i, my_inv, my_inv_d, fx, fy, cnd, cdd);
+                        cdd = valid ? cdd : __int_as_float(0x7f800000);
+                        cnd = valid ? cnd : __int_as_float(0x7f800000);
+                        all_has_depth &= has || !valid;
+                        const bool bd = cdd < min_d, bn = cnd < min_nd;
+                        min_d = bd ? cdd : min_d;
+                        idx_d = bd ? c : idx_d;
+                        min_nd = bn ? cnd : min_nd;
+                        idx_nd = bn ? c : idx_nd;
+                    }
+                    const int wv = all_has_depth ? idx_d : idx_nd;
+                    wc[0] = i == 0 ? wv : wc[0];
+                    wc[1] = i == 1 ? wv : wc[1];
+                    wc[2] = i == 2 ? wv : wc[2];
+                    wc[3] = i == 3 ? wv : wc[3];
+                }
+            }
+#pragma unroll
+            for (int i = 0; i < 4; i++)
+                if (x4 + i >= d.W) wc[i] = DSM_CODE_NONE;
         }
-        if (changed)
+        // the 4 pixels share the candidate seeds: dsm_code_seed(c, x4, y) is the seed of code c for each of them
+        if (FIRST)
+        { // every label is 0 and seed 0 is unstable: everything commits (:400)
+            if (active) reinterpret_cast<uchar4 *>(codes)[po >> 2] = make_uchar4(wc[0], wc[1], wc[2], wc[3]);
+            continue;
+        }
+
+        // ---- iterations 2..: commit / defer (SURVEY.md H1).  A deferred pixel whose winner IS its current label is dropped:
+        // if the raster scan evaluates it (t[label] < idx) the label does not change and the stamp t[winner] = t[label] is
+        // already below idx, so it can change nothing -- the relaxation only ever needs the pixels that would switch seeds.
+        unsigned defer = 0; // bit i: pixel i is appended to the frame's deferred-pixel list
+        if (active)
         {
-            const size_t po = fo + (size_t)y * d.Wp + x4;
-            *reinterpret_cast<int4 *>(d.labels + po) = make_int4(seed_of(oc[0]), seed_of(oc[1]), seed_of(oc[2]), seed_of(oc[3]));
-            *reinterpret_cast<uchar4 *>(d.code + po) = make_uchar4(oc[0], oc[1], oc[2], oc[3]);
+            bool changed = false;
+            // Only a pixel whose winner differs from its label has anything to do: with winner == label an evaluated pixel
+            // keeps its label and its stamp update min(t[label], idx) is a no-op (the owner is unstable, t[label] < 0 <= idx),
+            // and a pixel of a stable owner would be deferred only to be dropped again (see above).
+            auto staged_ts = [&](int c) { return s_ts[ra + (c & 1) * A_REC + ia + (c >> 1)]; };
+#pragma unroll
+            for (int i = 0; i < 4; i++)
+            {
+                if (wc[i] == DSM_CODE_NONE || wc[i] == oc[i]) continue; // (also every pixel x >= W)
+                const int pidx = po + i;
+                const int t_own = oc[i] == DSM_CODE_NONE ? d.tstable[so] : staged_ts(oc[i]); // a pixel without label is labelled 0
+                if (t_own < 0)
+                { // owner unstable since the start of the pass: the reference evaluates this pixel
+                    if (staged_ts(wc[i]) > pidx) atomicMin(&d.tstable[so + dsm_code_seed(wc[i], x4, y, d.spw)], pidx); // stable = false at time pidx (:445/:450)
+                    oc[i] = wc[i];
+                    changed = true;
+                }
+                else
+                    defer |= 1u << i;
+            }
+            if (changed) reinterpret_cast<uchar4 *>(codes)[po >> 2] = make_uchar4(oc[0], oc[1], oc[2], oc[3]);
+        }
+        // warp-aggregated append of the deferred pixels (rare: most warps have none); entry = (raster index, winner seed |
+        // winner's candidate code << 28)
+        if (__any_sync(FULL, defer != 0))
+        {
+            int total;
+            const int excl = warp_excl_scan(__popc(defer), lane, total);
+            int base = 0;
+            if (lane == 31) base = atomicAdd(&d.nlist[b], total);
+            base = __shfl_sync(FULL, base, 31);
+            int2 *list = d.list + fo + base + excl;
+#pragma unroll
+            for (int i = 0; i < 4; i++)
+                if ((defer >> i) & 1u) *list++ = make_int2(po + i, dsm_code_seed(wc[i], x4, y, d.spw) | (wc[i] << 28));
         }
     }
-    // warp-aggregated append of the deferred pixels (rare: most warps have none)
-    if (__any_sync(FULL, nent > 0))
-    {
-        int total;
-        const int excl = warp_excl_scan(nent, lane, total);
-        int base = 0;
-        if (lane == 31) base = atomicAdd(&d.nlist[b], total);
-        base = __shfl_sync(FULL, base, 31);
-        int2 *list = d.list + fo;
-        for (int j = 0; j < nent; j++) list[base + excl + j] = ent[j];
-    }
-    // frame-completion ticket: the CTA that takes the last ticket of frame b sees every other CTA's labels, list
+    if (FIRST) return;
+    // frame-completion ticket: the CTA that takes the last ticket of frame b sees every other CTA's label codes, list
     // entries and time stamps (release: fence before the ticket; acquire: fence after it) and resolves the frame
-    const int tid = threadIdx.y * 64 + threadIdx.x;
     __syncthreads(); // the CTA's writes happen-before thread 0's fence (fences are cumulative): one fence per CTA, as in a grid barrier
     if (tid == 0)
     {
@@ -1356,7 +1384,7 @@ int dsm_tile_setup()
 void dsm_launch_assign2(const DsmDev &d, int nb, bool first, cudaStream_t s)
 {
     dim3 block(64, 2);
-    dim3 grid((d.W + 255) / 256, (d.H + 1) / 2, nb);
+    dim3 grid((d.W + 255) / 256, (d.H + 2 * A_STEPS - 1) / (2 * A_STEPS), nb);
     if (first)
         pdl_launch(k_assign2<true>, grid, block, 0, s, d);
     else
