@@ -1022,7 +1022,7 @@ extern "C" int dsm_fuse_frame_resident(dsm_ctx *ctx, int ref_idx, const uint8_t 
 // What SurfelMap keeps per pose in attached_surfels / inactive_pointcloud (surfel_map.cpp:1479-1497, :1583-1587,
 // :681-748), resident on the device.  Only host orchestration over the pool kernels: retirement is the ordered
 // compaction of dsm_pool_retire writing straight into the store, the per-pose warp is k_pool_transform over one
-// segment, the inactive cloud is k_pool_scatter_cloud over the store.
+// segment, the inactive cloud is k_pool_scatter<float4> over the store.
 static DsmDev inactive_view(dsm_ctx *ctx)
 {
     DsmDev d = ctx->d;

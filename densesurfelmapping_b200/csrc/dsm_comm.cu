@@ -92,8 +92,7 @@ struct DsmComm
     size_t recv_cap = 0;
     int64_t *d_bytes = nullptr;          // device [nranks]
     int64_t *h_bytes = nullptr;          // pinned [nranks]
-    int32_t *h_hdr = nullptr;            // pinned header staging + new-surfel counts
-    size_t hdr_cap = 0;
+    int32_t *h_cnt = nullptr;            // pinned [max_batch]: new-surfel counts of the batch (NCCL transport)
     std::vector<size_t> ofs;             // root: byte offset of every rank's payload in recv (nranks + 1)
     int last_root = -1;
     // ---- peer-memory transport
@@ -139,19 +138,6 @@ static size_t payload_cap(const dsm_ctx *ctx)
     return header_bytes(ctx->p.max_batch) + ((size_t)ctx->p.max_batch * ctx->d.S + (size_t)(ctx->p.max_local_surfels > 0 ? ctx->p.max_local_surfels : 1)) * sizeof(dsm_surfel_t);
 }
 
-// valid new surfels of frame (frame0 + blockIdx.y) -> packed[offset of the frame .. ), one thread per 4-byte word
-__global__ void k_pack_new(const dsm_surfel_t *newsurf, const int32_t *nnew, int S, int nb, dsm_surfel_t *packed)
-{
-    const int f = blockIdx.y;
-    int before = 0;
-    for (int i = 0; i < f; i++) before += nnew[i]; // nb <= max_batch: a few hundred adds at most
-    const int n = nnew[f];
-    const uint32_t *src = reinterpret_cast<const uint32_t *>(newsurf + (size_t)f * S);
-    uint32_t *dst = reinterpret_cast<uint32_t *>(packed + before);
-    for (int w = blockIdx.x * blockDim.x + threadIdx.x; w < n * 11; w += gridDim.x * blockDim.x) dst[w] = src[w];
-    (void)nb;
-}
-
 // ---- peer-memory transport: device side ----
 __device__ __forceinline__ unsigned long long ld_acquire_sys(const unsigned long long *p)
 {
@@ -178,8 +164,9 @@ __global__ void k_peer_wait_credit(const DsmPeerCtrl *ctrl, unsigned long long s
     }
 }
 
-// One rank's payload written straight into its slot (in the root's memory): blockIdx.y < nb -> the valid new surfels of
-// frame blockIdx.y, blockIdx.y == nb -> the pool and (block 0) the header.  4-byte words, coalesced.
+// One rank's payload, the only writer of the wire format: straight into its slot in the root's memory (peer transport) or
+// into the local send buffer (NCCL).  blockIdx.y < nb -> the valid new surfels of frame blockIdx.y, blockIdx.y == nb ->
+// the pool and (block 0) the header.  4-byte words, coalesced.
 __global__ void __launch_bounds__(256) k_peer_pack(const dsm_surfel_t *newsurf, const int32_t *nnew, const dsm_surfel_t *pool,
                                                    const int32_t *poolofs, int S, int nb, unsigned char *slot, unsigned hb)
 {
@@ -289,8 +276,7 @@ extern "C" int dsm_comm_init(dsm_ctx *ctx, const void *id, int rank, int nranks)
     CK(c->own.device(&c->pack, c->pack_cap));
     CK(c->own.device(&c->d_bytes, (size_t)nranks));
     CK(c->own.host(&c->h_bytes, (size_t)nranks));
-    c->hdr_cap = header_bytes(ctx->p.max_batch) + (size_t)ctx->p.max_batch * 4;
-    CK(c->own.host(&c->h_hdr, c->hdr_cap / sizeof(int32_t)));
+    CK(c->own.host(&c->h_cnt, (size_t)ctx->p.max_batch));
     c->ofs.assign((size_t)nranks + 1, 0);
     return DSM_OK;
 }
@@ -458,38 +444,23 @@ static int gather_nccl(dsm_ctx *ctx, int root)
     DsmComm *c = ctx->comm;
     DsmNccl *api = nccl_api();
     const int nb = ctx->nb, S = ctx->d.S;
-    // (1) new-surfel counts of the batch -> pinned memory; this waits for the batch's kernels
-    int32_t *h_cnt = c->h_hdr + header_bytes(ctx->p.max_batch) / 4;
+    // (1) new-surfel counts of the batch -> pinned memory (NCCL needs the payload's size on the host); this waits for the
+    // batch's kernels
     CK(cudaStreamSynchronize(c->stream)); // the previous gather has consumed the staging buffers
-    CK(cudaMemcpyAsync(h_cnt, ctx->d.nnew, (size_t)nb * sizeof(int32_t), cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaMemcpyAsync(c->h_cnt, ctx->d.nnew, (size_t)nb * sizeof(int32_t), cudaMemcpyDeviceToHost, ctx->stream));
     CK(cudaEventRecord(c->ev_kernels, ctx->stream));
     CK(cudaEventSynchronize(c->ev_kernels));
-    // (2) header on the host
-    int n_new_total = 0;
-    for (int f = 0; f < nb; f++) n_new_total += h_cnt[f];
-    const int n_pool = ctx->n_pool;
-    int32_t *h = c->h_hdr;
-    h[0] = 0x444d5344; // 'DSMD'
-    h[1] = nb, h[2] = n_new_total, h[3] = n_pool;
-    for (int f = 0; f < nb; f++) h[4 + f] = h_cnt[f];
-    for (int f = 0; f <= nb; f++) h[4 + nb + f] = ctx->h_ofs[f];
-    const size_t hb = header_bytes(nb);
-    const size_t my_bytes = hb + ((size_t)n_new_total + (size_t)n_pool) * sizeof(dsm_surfel_t);
+    size_t n_rec = (size_t)ctx->n_pool;
+    for (int f = 0; f < nb; f++) n_rec += c->h_cnt[f];
+    const unsigned hb = (unsigned)header_bytes(nb);
+    const size_t my_bytes = hb + n_rec * sizeof(dsm_surfel_t);
     if (my_bytes > c->pack_cap) return DSM_E_CAPACITY;
-    // (3) pack on the side stream
+    // (2) pack on the side stream: the payload a peer writes into its slot, here into the local send buffer
     cudaStream_t cs = c->stream;
-    CK(cudaMemcpyAsync(c->pack, h, hb, cudaMemcpyHostToDevice, cs));
-    dsm_surfel_t *body = reinterpret_cast<dsm_surfel_t *>(c->pack + hb);
-    if (n_new_total > 0)
-    {
-        dim3 grid(16, nb);
-        k_pack_new<<<grid, 256, 0, cs>>>(ctx->d.newsurf, ctx->d.nnew, S, nb, body);
-    }
-    if (n_pool > 0)
-        CK(cudaMemcpyAsync(body + n_new_total, ctx->d.pool, (size_t)n_pool * sizeof(dsm_surfel_t), cudaMemcpyDeviceToDevice, cs));
+    k_peer_pack<<<dim3(64, nb + 1), 256, 0, cs>>>(ctx->d.newsurf, ctx->d.nnew, ctx->d.pool, ctx->d.poolofs, S, nb, c->pack, hb);
     CK(cudaEventRecord(c->ev_packed, cs));
     CK(cudaStreamWaitEvent(ctx->stream, c->ev_packed, 0)); // later work on the compute stream may overwrite newsurf / pool
-    // (4) byte counts of every rank
+    // (3) byte counts of every rank
     c->h_bytes[c->rank] = (int64_t)my_bytes;
     CK(cudaMemcpyAsync(c->d_bytes + c->rank, c->h_bytes + c->rank, sizeof(int64_t), cudaMemcpyHostToDevice, cs));
     if (c->nranks > 1)
@@ -498,7 +469,7 @@ static int gather_nccl(dsm_ctx *ctx, int root)
         CK(cudaMemcpyAsync(c->h_bytes, c->d_bytes, (size_t)c->nranks * sizeof(int64_t), cudaMemcpyDeviceToHost, cs));
         CK(cudaStreamSynchronize(cs));
     }
-    // (5) payloads
+    // (4) payloads
     if (c->rank == root)
     {
         size_t total = 0;

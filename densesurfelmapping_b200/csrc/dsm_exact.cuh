@@ -1,16 +1,11 @@
-// Exactness helpers shared by the kernel files: the float-vs-double-literal compare constants, warp helpers and the
-// expression-by-expression restatement of calculate_cost (fusion_functions.cpp:364-387).
+// Exactness helpers shared by the kernel files: the float-vs-double-literal compare constants, warp helpers, the
+// mbarrier / bulk-copy primitives and the expression-by-expression restatement of calculate_cost
+// (fusion_functions.cpp:364-387).
 #pragma once
 #include "dsm_device.cuh"
 #include <climits>
-#include <cuda/barrier>
-#include <cuda/ptx>
 
-#define HUBER_RANGE 0.4       // fusion_functions.h:13
 #define MAX_ANGLE_COS 0.1     // fusion_functions.h:11
-#define BASELINE 0.5          // fusion_functions.h:14
-#define DISPARITY_ERROR 4.0   // fusion_functions.h:15
-#define MIN_TOLERATE_DIFF 0.1 // fusion_functions.h:16
 
 #define FULL 0xffffffffu
 
@@ -54,8 +49,6 @@ static inline void pdl_launch(void (*kern)(KArgs...), dim3 grid, dim3 block, siz
 //   (double)x >= c  <=>  x >= c_hi        (double)x <= c  <=>  x <= c_lo
 // and for -c by symmetry (x > -c <=> x > -c_hi).  Used in the hot loops to keep the FP64 pipe for
 // the arithmetic that really needs it; tests/test_abi.py re-derives every constant.
-#define F_0p4_HI __uint_as_float(0x3ecccccdu)
-#define F_0p4_LO __uint_as_float(0x3eccccccu)
 #define F_0p1_HI __uint_as_float(0x3dcccccdu)
 #define F_0p1_LO __uint_as_float(0x3dccccccu)
 #define F_0p01_HI __uint_as_float(0x3c23d70bu)
@@ -67,30 +60,6 @@ static inline void pdl_launch(void (*kern)(KArgs...), dim3 grid, dim3 block, siz
 // -------------------------------------------------------------------------------------------
 // small helpers
 // -------------------------------------------------------------------------------------------
-using dsm_barrier = cuda::barrier<cuda::thread_scope_block>; // mbarrier for the TMA (cp.async.bulk) stagings
-// Wait for phase 0 of a tile barrier.  Experimental kernels only: a byte-count mistake would otherwise spin forever and
-// take the GPU with it, so the wait is bounded (each try_wait already blocks for a hardware time slice) and traps.
-__device__ __forceinline__ void tile_wait(dsm_barrier &bar)
-{
-    for (unsigned spin = 0; !cuda::ptx::mbarrier_try_wait_parity(cuda::device::barrier_native_handle(bar), 0); spin++)
-        if (spin > (1u << 22)) __trap();
-}
-__device__ __forceinline__ void sts_f32(unsigned addr, float v)
-{ // st.shared with a precomputed 32-bit shared-window address (keeps the address math out of the hot loops)
-    asm volatile("st.shared.f32 [%0], %1;" ::"r"(addr), "f"(v));
-}
-__device__ __forceinline__ float warp_sum_f(float v)
-{
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(FULL, v, o);
-    return v;
-}
-__device__ __forceinline__ float warp_max_f(float v)
-{
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(FULL, v, o));
-    return v;
-}
 __device__ __forceinline__ int warp_excl_scan(int v, int lane, int &total)
 {
     int incl = v;
@@ -104,6 +73,57 @@ __device__ __forceinline__ int warp_excl_scan(int v, int lane, int &total)
     return incl - v;
 }
 
+// -------------------------------------------------------------------------------------------
+// mbarrier / TMA primitives (raw PTX).  One elected thread initialises a CTA's barrier, arms it with the byte count and
+// issues the copies (3-D tensor boxes for the seed tiles, 1-D bulk runs for the pool records); the CTA waits for phase 0.
+// -------------------------------------------------------------------------------------------
+__device__ __forceinline__ unsigned smem_u32(const void *p) { return (unsigned)__cvta_generic_to_shared(p); }
+__device__ __forceinline__ void mbar_init(unsigned bar, unsigned count)
+{
+    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count) : "memory");
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); // visible to the async proxy before the first copy
+}
+__device__ __forceinline__ void mbar_expect_tx(unsigned bar, unsigned bytes)
+{
+    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
+}
+// Bounded wait: a descriptor or byte-count mistake must trap, not hang the GPU (each try_wait blocks for a hardware time slice).
+__device__ __forceinline__ void mbar_wait(unsigned bar, unsigned parity)
+{
+    unsigned ok = 0;
+    for (unsigned spin = 0; !ok; spin++)
+    {
+        asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
+                     : "=r"(ok)
+                     : "r"(bar), "r"(parity)
+                     : "memory");
+        if (!ok && spin > (1u << 20)) __trap();
+    }
+}
+__device__ __forceinline__ void tma_load_3d(unsigned dst, const CUtensorMap *map, int x, int y, int z, unsigned bar)
+{
+    asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];" ::"r"(dst),
+                 "l"(reinterpret_cast<unsigned long long>(map)), "r"(bar), "r"(x), "r"(y), "r"(z)
+                 : "memory");
+}
+// 1-D bulk copies: global and shared addresses 16-byte aligned, size a multiple of 16 bytes
+__device__ __forceinline__ void bulk_load(unsigned dst, const void *src, unsigned bytes, unsigned bar)
+{
+    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst), "l"(src), "r"(bytes),
+                 "r"(bar)
+                 : "memory");
+}
+// returns once the shared-memory source has been read (it may be overwritten, or the CTA exit); the global writes complete
+// asynchronously
+__device__ __forceinline__ void bulk_store(void *dst, unsigned src, unsigned bytes)
+{
+    asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(dst), "r"(src), "r"(bytes) : "memory");
+    asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+    asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
+}
+// this thread's generic-proxy shared-memory writes -> visible to the async proxy (a bulk store that follows)
+__device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+
 // (hi, lo) split of 1.0 / (double)mean_depth for the fp32 cost filter.  mean_depth <= 0 (or NaN): the candidate has no
 // depth term (:378), the pair is unused.  mean_depth < 2^-10: hi = 1e18 (its square is still finite, so a zero depth weight cannot produce a NaN) -- the depth term of such a seed exceeds 1e6 for
 // every valid pixel depth (> 0.01 m, i.e. inverse < 100), so it can never be the minimum (:408, :427) and the filter
@@ -115,6 +135,16 @@ __device__ __forceinline__ float2 split_inverse(float md)
     const double inv = 1.0 / (double)md;
     const float hi = (float)inv;
     return make_float2(hi, (float)(inv - (double)hi));
+}
+
+// A seed's state as the assign pass reads it: (x, y, mean_intensity, mean_depth), the fast-path and exact-path forms of
+// 1 / mean_depth (only consumed when mean_depth > 0, :378) and the stable flag
+__device__ __forceinline__ void store_seed(const DsmDev &d, size_t o, float x, float y, float I, float md, bool stable)
+{
+    d.seed[o] = make_float4(x, y, I, md);
+    d.inv_md[o] = 1.0 / (double)md;
+    d.seed_hl[o] = split_inverse(md);
+    d.tstable[o] = stable ? DSM_STABLE : -1;
 }
 
 struct SeedC

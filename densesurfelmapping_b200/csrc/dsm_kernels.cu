@@ -12,6 +12,7 @@
 // ":NNN" refer to the reference's surfel_fusion/src/fusion_functions.cpp.
 #include "dsm_exact.cuh"
 #include <cuda_pipeline.h>
+#include <type_traits>
 
 // -------------------------------------------------------------------------------------------
 // Kin  repack — the caller's tightly packed [n][H][W] gray / depth arrive by ONE contiguous H2D copy
@@ -103,11 +104,8 @@ __global__ void __launch_bounds__(256) k_seed_init(const __grid_constant__ DsmDe
     }
     if (!live) return;
     const size_t o = (size_t)b * d.S + s;
-    d.seed[o] = make_float4((float)ix, (float)iy, (float)gray[iy * Wp + ix], md);
-    d.inv_md[o] = 1.0 / (double)md; // only consumed when md > 0 (:378)
-    d.seed_hl[o] = split_inverse(md);
-    d.tstable[o] = -1;              // stable = false
-    d.fused[o] = 0;                 // fused = false
+    store_seed(d, o, (float)ix, (float)iy, (float)gray[iy * Wp + ix], md, false); // stable = false
+    d.fused[o] = 0;                                                                 // fused = false
 }
 
 // -------------------------------------------------------------------------------------------
@@ -117,27 +115,21 @@ __global__ void __launch_bounds__(256) k_seed_init(const __grid_constant__ DsmDe
 // the load, a bulk async-group for the store) issued by a single thread -- no per-thread address math,
 // no register staging; otherwise (unaligned slice start, ragged tail) coalesced 4-byte accesses.
 // -------------------------------------------------------------------------------------------
-__device__ __forceinline__ bool stage_in(float *sm, const float *g, int cnt, dsm_barrier *bar, int nthreads)
+__device__ __forceinline__ bool stage_in(float *sm, const float *g, int cnt, uint64_t *bar, int nthreads)
 {
     const unsigned bytes = (unsigned)cnt * 44u;
     const bool bulk = (bytes % 16u == 0u) && ((reinterpret_cast<uintptr_t>(g) & 15u) == 0u);
     if (bulk)
     {
+        const unsigned b = smem_u32(bar);
         if (threadIdx.x == 0)
         {
-            init(bar, 1);
-            cuda::ptx::fence_proxy_async(cuda::ptx::space_shared); // make the initialised barrier visible to the async proxy
+            mbar_init(b, 1);
+            mbar_expect_tx(b, bytes);
+            bulk_load(smem_u32(sm), g, bytes, b);
         }
-        __syncthreads();
-        if (threadIdx.x == 0)
-        {
-            cuda::device::memcpy_async_tx(sm, g, cuda::aligned_size_t<16>(bytes), *bar);
-            (void)cuda::device::barrier_arrive_tx(*bar, 1, bytes);
-        }
-        // bounded wait: a bulk copy that never completes (a bad pointer would fault first) traps instead of hanging the GPU
-        unsigned spin = 0;
-        while (!cuda::ptx::mbarrier_try_wait_parity(cuda::device::barrier_native_handle(*bar), 0))
-            if (++spin > (1u << 22)) __trap();
+        __syncthreads(); // barrier initialised before anybody polls it
+        mbar_wait(b, 0);
     }
     else
     {
@@ -151,14 +143,9 @@ __device__ __forceinline__ void stage_out(float *g, const float *sm, int cnt, bo
 {
     if (bulk)
     {
-        cuda::ptx::fence_proxy_async(cuda::ptx::space_shared); // this thread's smem writes -> async proxy
+        fence_proxy_async_smem();
         __syncthreads();
-        if (threadIdx.x == 0)
-        {
-            cuda::ptx::cp_async_bulk(cuda::ptx::space_global, cuda::ptx::space_shared, g, sm, (unsigned)cnt * 44u);
-            cuda::ptx::cp_async_bulk_commit_group();
-            cuda::ptx::cp_async_bulk_wait_group_read(cuda::ptx::n32_t<0>()); // smem must stay alive until it has been read
-        }
+        if (threadIdx.x == 0) bulk_store(g, smem_u32(sm), (unsigned)cnt * 44u);
     }
     else
     {
@@ -194,8 +181,7 @@ __global__ void __launch_bounds__(FUSE_BLOCK) k_fuse(const __grid_constant__ Dsm
     pdl_enter();
     __shared__ alignas(128) float sm[FUSE_BLOCK * 11];
     __shared__ float s_pose[32];
-#pragma nv_diag_suppress static_var_with_dynamic_init
-    __shared__ dsm_barrier bar;
+    __shared__ uint64_t bar;
     const int b = d.frame0 + blockIdx.y;
     const int begin = d.poolofs[b], end = d.poolofs[b + 1];
     const int first = begin + blockIdx.x * FUSE_BLOCK;
@@ -285,6 +271,19 @@ __global__ void __launch_bounds__(FUSE_BLOCK) k_fuse(const __grid_constant__ Dsm
     stage_out(g, sm, cnt, bulk, FUSE_BLOCK);
 }
 
+// Block rank (ballot -> per-warp count -> prefix over the warps): the position of this thread among the CTA's threads
+// with `live` set, in thread order.  s_warp (shared, one int per warp) holds every warp's count when it returns.
+__device__ __forceinline__ int block_rank(bool live, int *s_warp)
+{
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const unsigned bal = __ballot_sync(FULL, live);
+    if (lane == 0) s_warp[warp] = __popc(bal);
+    __syncthreads();
+    int pos = 0;
+    for (int w = 0; w < warp; w++) pos += s_warp[w];
+    return pos + __popc(bal & ((1u << lane) - 1));
+}
+
 // -------------------------------------------------------------------------------------------
 // K6  surfel_init — initialize_surfels (:315-361).  new_surfels come out in seed-index order exactly like the
 // reference's serial push_back loop, with several CTAs per frame and no inter-CTA communication: CTA j owns
@@ -305,7 +304,6 @@ __global__ void __launch_bounds__(1024) k_init_surfels(const __grid_constant__ D
     __shared__ int s_before[32];
     __shared__ float s_pose[16];
     const int b = d.frame0 + blockIdx.y;
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const size_t so = (size_t)b * d.S;
     if (threadIdx.x < 16) s_pose[threadIdx.x] = d.pose[b * 16 + threadIdx.x];
     const int first = blockIdx.x * 1024;
@@ -315,23 +313,15 @@ __global__ void __launch_bounds__(1024) k_init_surfels(const __grid_constant__ D
     before = __reduce_add_sync(FULL, before);
     const int s = first + threadIdx.x;
     const bool e = s < d.S && init_emits(d, so, s);
-    const unsigned bal = __ballot_sync(FULL, e);
-    if (lane == 0)
-    {
-        s_warp[warp] = __popc(bal);
-        s_before[warp] = before;
-    }
-    __syncthreads();
-    int pos = 0, total = 0;
+    if ((threadIdx.x & 31) == 0) s_before[threadIdx.x >> 5] = before; // read after block_rank's barrier
+    int pos = block_rank(e, s_warp), total = 0;
     for (int w = 0; w < 32; w++)
     {
-        const int c = s_warp[w];
-        pos += s_before[w] + (w < warp ? c : 0);
-        total += s_before[w] + c;
+        pos += s_before[w];
+        total += s_before[w] + s_warp[w];
     }
     if (e)
     {
-        pos += __popc(bal & ((1u << lane) - 1));
         const float4 *pl = d.plane + (so + s) * 3;
         const float4 r0 = pl[0], r1 = pl[1], r2 = pl[2];
         float pw[4], nw[3];
@@ -421,14 +411,18 @@ __global__ void __launch_bounds__(1024) k_pool_scan(const __grid_constant__ DsmD
     }
 }
 
-__global__ void __launch_bounds__(256) k_pool_scatter(const __grid_constant__ DsmDev d, int b, const int *blkofs, dsm_surfel_t *dst, int mode, int key)
+// The selected surfels of the CTA's 256 pool entries, in pool order, to dst + blkofs[CTA].  Rec is the output record:
+// the whole 44-byte surfel (compaction, retire, surfel export) or, for the point-cloud builders of SurfelMap
+// (publish_active_pointcloud surfel_map.cpp:1398-1417, publish_all_pointcloud :1419-1454, publish_neighbor_pointcloud
+// :1284-1300, save_cloud :1153-1173), one PointXYZI float4 {px, py, pz, intensity = color} like the serial push_back loops.
+template <typename Rec>
+__global__ void __launch_bounds__(256) k_pool_scatter(const __grid_constant__ DsmDev d, int b, const int *blkofs, Rec *dst, int mode, int key)
 {
     pdl_enter();
     __shared__ int s_warp[8];
     const int begin = d.poolofs[b], end = d.poolofs[b + 1];
     const int i = begin + blockIdx.x * 256 + threadIdx.x;
     if (begin + blockIdx.x * 256 >= end) return;
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     dsm_surfel_t e;
     bool live = false;
     if (i < end)
@@ -437,39 +431,13 @@ __global__ void __launch_bounds__(256) k_pool_scatter(const __grid_constant__ Ds
         live = pool_pred(e, mode, key);
         if (live && mode == 1) d.pool[i].update_times = 0; // "delete the surfel from the local point" (surfel_map.cpp:1496)
     }
-    const unsigned bal = __ballot_sync(FULL, live);
-    if (lane == 0) s_warp[warp] = __popc(bal);
-    __syncthreads();
-    int wofs = 0;
-    for (int w = 0; w < warp; w++) wofs += s_warp[w];
-    if (live) dst[blkofs[blockIdx.x] + wofs + __popc(bal & ((1u << lane) - 1))] = e;
-}
-
-// k_pool_scatter_cloud — the point-cloud builders of SurfelMap (publish_active_pointcloud surfel_map.cpp:1398-1417,
-//   publish_all_pointcloud :1419-1454, publish_neighbor_pointcloud :1284-1300, save_cloud :1153-1173): every
-//   selected surfel becomes one PointXYZI {px, py, pz, intensity = color}, in pool order like the serial
-//   push_back loops.  Same count/scan as the compaction; 44 B read and 16 B written per surfel.
-__global__ void __launch_bounds__(256) k_pool_scatter_cloud(const __grid_constant__ DsmDev d, int b, const int *blkofs, float4 *dst, int mode, int key)
-{
-    __shared__ int s_warp[8];
-    const int begin = d.poolofs[b], end = d.poolofs[b + 1];
-    const int i = begin + blockIdx.x * 256 + threadIdx.x;
-    if (begin + blockIdx.x * 256 >= end) return;
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    float4 pt = make_float4(0.f, 0.f, 0.f, 0.f);
-    bool live = false;
-    if (i < end)
-    {
-        const dsm_surfel_t e = d.pool[i];
-        live = pool_pred(e, mode, key);
-        pt = make_float4(e.px, e.py, e.pz, e.color);
-    }
-    const unsigned bal = __ballot_sync(FULL, live);
-    if (lane == 0) s_warp[warp] = __popc(bal);
-    __syncthreads();
-    int wofs = 0;
-    for (int w = 0; w < warp; w++) wofs += s_warp[w];
-    if (live) dst[blkofs[blockIdx.x] + wofs + __popc(bal & ((1u << lane) - 1))] = pt;
+    const int rank = block_rank(live, s_warp);
+    if (!live) return;
+    const int pos = blkofs[blockIdx.x] + rank;
+    if constexpr (std::is_same<Rec, float4>::value)
+        dst[pos] = make_float4(e.px, e.py, e.pz, e.color);
+    else
+        dst[pos] = e;
 }
 
 __global__ void __launch_bounds__(256) k_pool_append(const __grid_constant__ DsmDev d, int b, const int *newofs, dsm_surfel_t *dst, int32_t *ofs_out)
@@ -486,8 +454,7 @@ __global__ void __launch_bounds__(XF_BLOCK) k_pool_transform(const __grid_consta
 {
     __shared__ alignas(128) float sm[XF_BLOCK * 11];
     __shared__ float s_w[16];
-#pragma nv_diag_suppress static_var_with_dynamic_init
-    __shared__ dsm_barrier bar;
+    __shared__ uint64_t bar;
     const int begin = d.poolofs[b], end = d.poolofs[b + 1];
     const int first = begin + blockIdx.x * XF_BLOCK;
     if (first >= end) return;
@@ -592,7 +559,7 @@ void dsm_launch_pool_compact(const DsmDev &d, int frame, int upper, int *blkcnt,
     const int nblk = (upper + 255) / 256;
     if (nblk > 0) pdl_launch(k_pool_count, dim3(nblk), dim3(256), 0, s, d, frame, blkcnt, 0, 0);
     pdl_launch(k_pool_scan, dim3(1), dim3(1024), 0, s, d, frame, (const int *)blkcnt, blkofs, newofs);
-    if (nblk > 0) pdl_launch(k_pool_scatter, dim3(nblk), dim3(256), 0, s, d, frame, (const int *)blkofs, dst, 0, 0);
+    if (nblk > 0) pdl_launch(k_pool_scatter<dsm_surfel_t>, dim3(nblk), dim3(256), 0, s, d, frame, (const int *)blkofs, dst, 0, 0);
     pdl_launch(k_pool_append, dim3((d.S + 255) / 256), dim3(256), 0, s, d, frame, (const int *)newofs, dst, ofs_out);
 }
 // move_add_surfels, removal half (surfel_map.cpp:1479-1497): the live surfels whose last_update == key are
@@ -602,7 +569,7 @@ void dsm_launch_pool_retire(const DsmDev &d, int frame, int upper, int key, int 
     const int nblk = (upper + 255) / 256;
     if (nblk > 0) k_pool_count<<<nblk, 256, 0, s>>>(d, frame, blkcnt, 1, key);
     k_pool_scan<<<1, 1024, 0, s>>>(d, frame, blkcnt, blkofs, newofs);
-    if (nblk > 0 && dst) k_pool_scatter<<<nblk, 256, 0, s>>>(d, frame, blkofs, dst, 1, key); // dst == nullptr: count only
+    if (nblk > 0 && dst) k_pool_scatter<dsm_surfel_t><<<nblk, 256, 0, s>>>(d, frame, blkofs, dst, 1, key); // dst == nullptr: count only
 }
 // publish/save filters (mode/key as pool_pred): as_cloud ? PointXYZI float4 records : whole 44-byte surfels, in pool
 // order to dst (count in newofs[0]); the pool itself is not modified
@@ -613,9 +580,9 @@ void dsm_launch_pool_export(const DsmDev &d, int frame, int upper, int mode, int
     k_pool_scan<<<1, 1024, 0, s>>>(d, frame, blkcnt, blkofs, newofs);
     if (nblk == 0) return;
     if (as_cloud)
-        k_pool_scatter_cloud<<<nblk, 256, 0, s>>>(d, frame, blkofs, static_cast<float4 *>(dst), mode, key);
+        k_pool_scatter<float4><<<nblk, 256, 0, s>>>(d, frame, blkofs, static_cast<float4 *>(dst), mode, key);
     else
-        k_pool_scatter<<<nblk, 256, 0, s>>>(d, frame, blkofs, static_cast<dsm_surfel_t *>(dst), mode, key);
+        k_pool_scatter<dsm_surfel_t><<<nblk, 256, 0, s>>>(d, frame, blkofs, static_cast<dsm_surfel_t *>(dst), mode, key);
 }
 void dsm_launch_pool_transform(const DsmDev &d, int frame, int upper, const float *Wm_dev, cudaStream_t s)
 {

@@ -18,39 +18,6 @@
 #include <cuda_pipeline.h>
 
 // -------------------------------------------------------------------------------------------
-// mbarrier / TMA helpers (raw PTX; one elected thread arms the barrier and issues the tensor copies)
-// -------------------------------------------------------------------------------------------
-__device__ __forceinline__ unsigned smem_u32(const void *p) { return (unsigned)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(unsigned bar, unsigned count)
-{
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count) : "memory");
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); // visible to the async proxy before the first copy
-}
-__device__ __forceinline__ void mbar_expect_tx(unsigned bar, unsigned bytes)
-{
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-// Bounded wait: a descriptor or byte-count mistake must trap, not hang the GPU (each try_wait blocks for a hardware time slice).
-__device__ __forceinline__ void mbar_wait(unsigned bar, unsigned parity)
-{
-    unsigned ok = 0;
-    for (unsigned spin = 0; !ok; spin++)
-    {
-        asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
-                     : "=r"(ok)
-                     : "r"(bar), "r"(parity)
-                     : "memory");
-        if (!ok && spin > (1u << 20)) __trap();
-    }
-}
-__device__ __forceinline__ void tma_load_3d(unsigned dst, const CUtensorMap *map, int x, int y, int z, unsigned bar)
-{
-    asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];" ::"r"(dst),
-                 "l"(reinterpret_cast<unsigned long long>(map)), "r"(bar), "r"(x), "r"(y), "r"(z)
-                 : "memory");
-}
-
-// -------------------------------------------------------------------------------------------
 // K1  slic_assign (filtered) — update_pixels_kernel (:389-453) + calculate_cost (:364-387)
 //
 // A thread owns 4 consecutive pixels of one row at a time (CTA = 64 x 2 threads, walking the 256 x 8 pixels of one seed
@@ -403,16 +370,19 @@ __global__ void __launch_bounds__(128, 8) k_assign2(const __grid_constant__ DsmD
 //   sum_a = fmaf(2, md - z, sum_a) (2 r is exact: the same single rounding as `sum_a += 2 * residual`).
 // -------------------------------------------------------------------------------------------
 #define DL_STRIDE 232 // floats per seed list: >= 15*15 possible members, multiple of 8 (32-byte sectors)
+// Shared memory of the two seed-tile kernels (k_gather, k_plane_gather): the tile's depth and label-code boxes, then
+// each kernel's own planes from TILE_SMEM_OWN on
 #define TILE_PLANE_BYTES 12544 // 76 * 41 * 4 = 12464 rounded up to 128: TMA destinations are 128-byte aligned
 #define TILE_BYTE_PLANE 4608 // 112 * 41 = 4592 rounded up to 128
-#define GAT_SMEM_DEP 0
-#define GAT_SMEM_COD TILE_PLANE_BYTES
-#define GAT_SMEM_GRY (TILE_PLANE_BYTES + TILE_BYTE_PLANE)
-#define GAT_SMEM_LIST (TILE_PLANE_BYTES + 2 * TILE_BYTE_PLANE) // float [16][DL_STRIDE]: the 16 seeds of one round
+#define TILE_SMEM_DEP 0                // float [41][76] depth box
+#define TILE_SMEM_COD TILE_PLANE_BYTES // u8 [41][112] label-code box
+#define TILE_SMEM_OWN (TILE_PLANE_BYTES + TILE_BYTE_PLANE)
+#define TILE_TX_BYTES (DSM_TILE_W * DSM_TILE_H * 4u + (unsigned)DSM_TILE_GW * DSM_TILE_H) // the depth and code boxes
+#define GAT_SMEM_GRY TILE_SMEM_OWN                               // u8 [41][112] gray box
+#define GAT_SMEM_LIST (TILE_SMEM_OWN + TILE_BYTE_PLANE)          // float [16][DL_STRIDE]: the 16 seeds of one round
 #define GAT_SMEM_ND (GAT_SMEM_LIST + 16 * DL_STRIDE * 4)        // int [16] list lengths of the round
 #define GAT_SMEM_BAR (GAT_SMEM_ND + 16 * 4)
 #define GAT_SMEM_BYTES (GAT_SMEM_BAR + 16)
-#define TILE_TX_BYTES (DSM_TILE_W * DSM_TILE_H * 4u + 2u * DSM_TILE_GW * DSM_TILE_H)
 
 // 16-bit membership mask of one window row from the label-code tile: bit k set iff the pixel at window column k is labelled
 // with the seed whose window this is.  Inside the 16 x 16 window of seed (sx, sy) the pixel at column k, row r sees that
@@ -440,12 +410,68 @@ __device__ __forceinline__ int mask_index_sum(unsigned m)
 // 4-bit mask -> 0xff per set bit
 __device__ __forceinline__ unsigned nibble_to_bytes(unsigned n) { return (((n & 0xfu) * 0x00204081u) & 0x01010101u) * 0xffu; }
 
+// Seed slot sl of the CTA's 8 x 4 seed tile (row-major) -> the superpixel it holds; live: inside the frame's seed grid
+struct TileSeed
+{
+    int tx, ty;     // slot column / row in the tile
+    int sp_x, sp_y; // superpixel
+    bool live;
+};
+__device__ __forceinline__ TileSeed tile_seed(const DsmDev &d, int sl)
+{
+    TileSeed t;
+    t.tx = sl & 7, t.ty = sl >> 3;
+    t.sp_x = blockIdx.x * DSM_TILE_SX + t.tx, t.sp_y = blockIdx.y * DSM_TILE_SY + t.ty;
+    t.live = t.sp_x < d.spw && t.sp_y < d.sph;
+    return t;
+}
+
+// Thread 0 of a seed-tile kernel: initialise the tile barrier, arm it with `bytes` and issue the depth and label-code
+// boxes of frame b for the tile at pixel (X0, Y0).  The code box starts DSM_TILE_GX pixels further left (16-byte rule).
+__device__ __forceinline__ void tile_issue(unsigned char *smem, unsigned bar, unsigned bytes, const DsmMaps &mp, int X0, int Y0, int b)
+{
+    mbar_init(bar, 1);
+    mbar_expect_tx(bar, bytes);
+    tma_load_3d(smem_u32(smem + TILE_SMEM_DEP), &mp.dep, X0, Y0, b, bar);
+    tma_load_3d(smem_u32(smem + TILE_SMEM_COD), &mp.cod, X0 - DSM_TILE_GX, Y0, b, bar);
+}
+
+// One window row from the staged tile (tile row trow, columns tcol .. tcol + 15; lane = window row r): the 16-bit
+// membership mask, and the 16 depths into zk
+__device__ __forceinline__ unsigned window_row(const unsigned char *smem, int trow, int tcol, int r, float zk[16])
+{
+    const unsigned *pc = reinterpret_cast<const unsigned *>(smem + TILE_SMEM_COD + trow * DSM_TILE_GW + DSM_TILE_GX + tcol); // 4-byte aligned
+    const unsigned cw[4] = {pc[0], pc[1], pc[2], pc[3]};
+    const unsigned mm = member_mask16(cw, r);
+    const float4 *pz = reinterpret_cast<const float4 *>(reinterpret_cast<const float *>(smem + TILE_SMEM_DEP) + trow * DSM_TILE_W + tcol);
+#pragma unroll
+    for (int qd = 0; qd < 4; qd++)
+    {
+        const float4 z = pz[qd];
+        zk[4 * qd] = z.x, zk[4 * qd + 1] = z.y, zk[4 * qd + 2] = z.z, zk[4 * qd + 3] = z.w;
+    }
+    return mm;
+}
+
+// Scan of c over the 16 lanes of a half-warp (lane r = window row): the sum over the lanes before r, and (total) over all 16
+__device__ __forceinline__ int half_warp_scan(int c, int r, int &total)
+{
+    int incl = c;
+#pragma unroll
+    for (int o = 1; o < 16; o <<= 1)
+    {
+        const int nb = __shfl_up_sync(FULL, incl, o, 16);
+        if (r >= o) incl += nb;
+    }
+    total = __shfl_sync(FULL, incl, 15, 16);
+    return incl - c;
+}
+
 __global__ void __launch_bounds__(256, 6) k_gather(const __grid_constant__ DsmDev d, const __grid_constant__ DsmMaps mp)
 {
     pdl_enter();
     extern __shared__ __align__(128) unsigned char smem[];
-    const float *t_dep = reinterpret_cast<const float *>(smem + GAT_SMEM_DEP);
-    const uint8_t *t_cod = smem + GAT_SMEM_COD, *t_gry = smem + GAT_SMEM_GRY;
+    const uint8_t *t_gry = smem + GAT_SMEM_GRY;
     float *lists = reinterpret_cast<float *>(smem + GAT_SMEM_LIST);
     int *s_nd = reinterpret_cast<int *>(smem + GAT_SMEM_ND);
     const unsigned bar = smem_u32(smem + GAT_SMEM_BAR);
@@ -455,10 +481,7 @@ __global__ void __launch_bounds__(256, 6) k_gather(const __grid_constant__ DsmDe
     const int X0 = blockIdx.x * (DSM_TILE_SX * DSM_SP) - DSM_SP / 2, Y0 = blockIdx.y * (DSM_TILE_SY * DSM_SP) - DSM_SP / 2;
     if (threadIdx.x == 0)
     {
-        mbar_init(bar, 1);
-        mbar_expect_tx(bar, TILE_TX_BYTES);
-        tma_load_3d(smem_u32(smem + GAT_SMEM_DEP), &mp.dep, X0, Y0, b, bar);
-        tma_load_3d(smem_u32(smem + GAT_SMEM_COD), &mp.cod, X0 - DSM_TILE_GX, Y0, b, bar);
+        tile_issue(smem, bar, TILE_TX_BYTES + DSM_TILE_GW * DSM_TILE_H, mp, X0, Y0, b);
         tma_load_3d(smem_u32(smem + GAT_SMEM_GRY), &mp.gry, X0 - DSM_TILE_GX, Y0, b, bar);
     }
     if (threadIdx.x == 1 && blockIdx.x == 0 && blockIdx.y == 0) d.nhard[b] = 0; // this pass's queue of hard Newton seeds
@@ -470,10 +493,8 @@ __global__ void __launch_bounds__(256, 6) k_gather(const __grid_constant__ DsmDe
 #pragma unroll
     for (int rd = 0; rd < 2; rd++)
     {
-        const int sl = rd * 16 + warp * 2 + half;
-        const int sp_x = blockIdx.x * DSM_TILE_SX + (sl & 7), sp_y = blockIdx.y * DSM_TILE_SY + (sl >> 3);
-        const bool live = sp_x < d.spw && sp_y < d.sph;
-        tflag[rd] = live ? d.tstable[so + sp_y * d.spw + sp_x] : DSM_STABLE;
+        const TileSeed t = tile_seed(d, rd * 16 + warp * 2 + half);
+        tflag[rd] = t.live ? d.tstable[so + t.sp_y * d.spw + t.sp_x] : DSM_STABLE;
     }
     __syncthreads(); // barrier initialised before anybody polls it
     mbar_wait(bar, 0);
@@ -481,12 +502,10 @@ __global__ void __launch_bounds__(256, 6) k_gather(const __grid_constant__ DsmDe
     for (int rd = 0; rd < 2; rd++)
     {
         const int q = warp * 2 + half; // seed slot of this round
-        const int sl = rd * 16 + q;
-        const int tx = sl & 7, ty = sl >> 3;
-        const int sp_x = blockIdx.x * DSM_TILE_SX + tx, sp_y = blockIdx.y * DSM_TILE_SY + ty;
-        const int s = sp_y * d.spw + sp_x;
+        const TileSeed t = tile_seed(d, rd * 16 + q);
+        const int s = t.sp_y * d.spw + t.sp_x;
         const bool act = tflag[rd] != DSM_STABLE;
-        const int x0 = sp_x * DSM_SP - DSM_SP / 2, y0 = sp_y * DSM_SP - DSM_SP / 2;
+        const int x0 = t.sp_x * DSM_SP - DSM_SP / 2, y0 = t.sp_y * DSM_SP - DSM_SP / 2;
         const int xb = x0 > 0 ? x0 : 0, yb = y0 > 0 ? y0 : 0;
         const int xe = (x0 + 16) < W - 1 ? (x0 + 16) : W - 1; // end-exclusive: last row/col never visited (:488-489)
         const int ye = (y0 + 16) < H - 1 ? (y0 + 16) : H - 1;
@@ -494,23 +513,11 @@ __global__ void __launch_bounds__(256, 6) k_gather(const __grid_constant__ DsmDe
         const bool rowin = act && y >= yb && y < ye;
         // member columns of the window: xb - x0 <= k < xe - x0; nothing if the row is outside
         const unsigned kmask = rowin ? (((1u << (xe - x0)) - 1u) & ~((1u << (xb - x0)) - 1u)) : 0u;
-        const int trow = ty * DSM_SP + r, tcol = tx * DSM_SP;
+        const int trow = t.ty * DSM_SP + r, tcol = t.tx * DSM_SP;
         float zk[16];
-        unsigned mm, zm = 0; // bit k: labelled with this seed / depth > 0.1
-        {
-            const unsigned *pc = reinterpret_cast<const unsigned *>(t_cod + trow * DSM_TILE_GW + DSM_TILE_GX + tcol); // 4-byte aligned
-            const unsigned cw[4] = {pc[0], pc[1], pc[2], pc[3]};
-            mm = member_mask16(cw, r);
-            const float4 *pz = reinterpret_cast<const float4 *>(t_dep + trow * DSM_TILE_W + tcol);
+        unsigned mm = window_row(smem, trow, tcol, r, zk), zm = 0; // bit k: labelled with this seed / depth > 0.1
 #pragma unroll
-            for (int qd = 0; qd < 4; qd++)
-            {
-                const float4 z = pz[qd];
-                zk[4 * qd] = z.x, zk[4 * qd + 1] = z.y, zk[4 * qd + 2] = z.z, zk[4 * qd + 3] = z.w;
-            }
-#pragma unroll
-            for (int k = 0; k < 16; k++) zm |= (zk[k] > F_0p1_LO ? 1u : 0u) << k; // (double)depth > 0.1 (:508)
-        }
+        for (int k = 0; k < 16; k++) zm |= (zk[k] > F_0p1_LO ? 1u : 0u) << k; // (double)depth > 0.1 (:508)
         mm &= kmask;
         const unsigned dm = mm & zm; // member with depth > 0.1
         const int cnt = __popc(mm);
@@ -530,17 +537,10 @@ __global__ void __launch_bounds__(256, 6) k_gather(const __grid_constant__ DsmDe
             pa += __shfl_xor_sync(FULL, pa, o);
             pb += __shfl_xor_sync(FULL, pb, o);
         }
-        const int c = __popc(dm);
-        int incl = c;
-#pragma unroll
-        for (int o = 1; o < 16; o <<= 1)
-        {
-            const int nb = __shfl_up_sync(FULL, incl, o, 16);
-            if (r >= o) incl += nb;
-        }
-        const int ndt = __shfl_sync(FULL, incl, 15, 16);
+        int ndt;
+        const int excl = half_warp_scan(__popc(dm), r, ndt);
         if (rd) __syncthreads(); // the previous round's lists have been copied out
-        float *lp = lists + q * DL_STRIDE + (incl - c);
+        float *lp = lists + q * DL_STRIDE + excl;
 #pragma unroll
         for (int k = 0; k < 16; k++)
             if ((dm >> k) & 1u) *lp++ = zk[k];
@@ -561,8 +561,8 @@ __global__ void __launch_bounds__(256, 6) k_gather(const __grid_constant__ DsmDe
         {
             const int q2 = warp + 8 * h2, n2 = s_nd[q2];
             if (n2 == 0) continue; // warp-uniform
-            const int sl2 = rd * 16 + q2;
-            const int s2 = (blockIdx.y * DSM_TILE_SY + (sl2 >> 3)) * d.spw + blockIdx.x * DSM_TILE_SX + (sl2 & 7);
+            const TileSeed t2 = tile_seed(d, rd * 16 + q2);
+            const int s2 = t2.sp_y * d.spw + t2.sp_x;
             float4 *dst = reinterpret_cast<float4 *>(d.dlist + (so + s2) * DL_STRIDE);
             const float4 *src = reinterpret_cast<const float4 *>(lists + q2 * DL_STRIDE);
             if (4 * lane < n2) dst[lane] = src[lane];
@@ -573,25 +573,15 @@ __global__ void __launch_bounds__(256, 6) k_gather(const __grid_constant__ DsmDe
 
 #define NW_T 64       // seeds (threads) per CTA of the two Newton kernels
 #define NW_CAP 5632   // floats of list staging per CTA (22 KB): 88 entries per seed on average, 225 possible; 8 CTAs per SM
-__global__ void __launch_bounds__(NW_T, 8) k_newton2(const __grid_constant__ DsmDev d)
+
+// Every thread of a Newton CTA stages its seed's list src[0 .. nd) (a contiguous run in global memory) into buf with 16-byte
+// cp.async: all copies of the CTA are in flight at once, no register staging, and a thread waits for its own copies only
+// (it never reads another list).  Lists that do not fit (rare: NW_CAP covers 88 entries per seed) stay in global memory.
+// Issues and commits the copies and returns where the list will be (generic: shared or global); the caller waits with
+// __pipeline_wait_prior(0).
+__device__ __forceinline__ const float *stage_list(float *buf, int *s_off, int *s_wsum, const float *src, int nd)
 {
-    pdl_enter();
-    // Every thread stages its seed's list (a contiguous run in global memory) into shared memory with 16-byte cp.async and
-    // then walks it there up to six times.  Lists that do not fit (rare: NW_CAP covers 88 entries per seed) stay in global memory.
-    __shared__ __align__(16) float buf[NW_CAP];
-    __shared__ int s_off[NW_T], s_wsum[NW_T / 32];
-    const int b = d.frame0 + blockIdx.y;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const int s = blockIdx.x * NW_T + tid;
-    const size_t so = (size_t)b * d.S;
-    // the four per-seed loads are independent and issued together (one memory round trip), before the list staging
-    const bool inr = s < d.S;
-    const int tflag = inr ? d.tstable[so + s] : DSM_STABLE;
-    const int nd_raw = inr ? d.und[so + s] : 0;
-    const int4 su = inr ? d.usum[so + s] : make_int4(0, 0, 0, 0);
-    const float4 pre = inr ? d.seed[so + s] : make_float4(0.f, 0.f, 0.f, 0.f);
-    const bool act = tflag != DSM_STABLE; // stable seeds are untouched by update_seeds (:478-479)
-    const int nd = act ? nd_raw : 0;
     {
         const int len4 = (nd + 3) & ~3;
         int wtot;
@@ -603,15 +593,51 @@ __global__ void __launch_bounds__(NW_T, 8) k_newton2(const __grid_constant__ Dsm
         const int off = base + wex;
         s_off[tid] = (off + len4 <= NW_CAP) ? off : -1;
     }
-    // every thread copies its own list (a contiguous run in global memory) with 16-byte cp.async: all copies of the CTA are in
-    // flight at once, no register staging, and a thread waits for its own copies only (it never reads another list)
     if (s_off[tid] >= 0)
     {
-        const float4 *src = reinterpret_cast<const float4 *>(d.dlist + (so + s) * DL_STRIDE);
+        const float4 *src4 = reinterpret_cast<const float4 *>(src);
         float4 *dst = reinterpret_cast<float4 *>(buf + s_off[tid]);
-        for (int j4 = 0; 4 * j4 < nd; j4++) __pipeline_memcpy_async(dst + j4, src + j4, 16);
+        for (int j4 = 0; 4 * j4 < nd; j4++) __pipeline_memcpy_async(dst + j4, src4 + j4, 16);
     }
     __pipeline_commit();
+    return s_off[tid] >= 0 ? buf + s_off[tid] : src;
+}
+
+// One Newton pass over a list whose entries are ALL inside the Huber range: sum_a += 2 * residual, i.e.
+// fmaf(2, md - z, sum_a) (2 r is exact: the same single rounding per add), eight entries (two 16-byte loads) per step.
+__device__ __forceinline__ float huber_sum_in_range(const float *dl, int nd, float md)
+{
+    const float4 *dl4 = reinterpret_cast<const float4 *>(dl);
+    float sa = 0.0f;
+    int k = 0;
+    for (; k + 8 <= nd; k += 8)
+    {
+        const float4 a = dl4[k >> 2], c = dl4[(k >> 2) + 1];
+        sa = fmaf(2.0f, md - a.x, sa), sa = fmaf(2.0f, md - a.y, sa), sa = fmaf(2.0f, md - a.z, sa), sa = fmaf(2.0f, md - a.w, sa);
+        sa = fmaf(2.0f, md - c.x, sa), sa = fmaf(2.0f, md - c.y, sa), sa = fmaf(2.0f, md - c.z, sa), sa = fmaf(2.0f, md - c.w, sa);
+    }
+    for (; k < nd; k++) sa = fmaf(2.0f, md - dl[k], sa);
+    return sa;
+}
+
+__global__ void __launch_bounds__(NW_T, 8) k_newton2(const __grid_constant__ DsmDev d)
+{
+    pdl_enter();
+    // Every thread stages its seed's list into shared memory and then walks it there up to six times.
+    __shared__ __align__(16) float buf[NW_CAP];
+    __shared__ int s_off[NW_T], s_wsum[NW_T / 32];
+    const int b = d.frame0 + blockIdx.y;
+    const int s = blockIdx.x * NW_T + threadIdx.x;
+    const size_t so = (size_t)b * d.S;
+    // the four per-seed loads are independent and issued together (one memory round trip), before the list staging
+    const bool inr = s < d.S;
+    const int tflag = inr ? d.tstable[so + s] : DSM_STABLE;
+    const int nd_raw = inr ? d.und[so + s] : 0;
+    const int4 su = inr ? d.usum[so + s] : make_int4(0, 0, 0, 0);
+    const float4 pre = inr ? d.seed[so + s] : make_float4(0.f, 0.f, 0.f, 0.f);
+    const bool act = tflag != DSM_STABLE; // stable seeds are untouched by update_seeds (:478-479)
+    const int nd = act ? nd_raw : 0;
+    const float *dl = stage_list(buf, s_off, s_wsum, d.dlist + (so + s) * DL_STRIDE, nd);
     __pipeline_wait_prior(0);
     if (!act) return;
     // Every seed runs its mean pass and its Newton passes as long as every entry is inside the Huber range (a pure
@@ -639,7 +665,6 @@ __global__ void __launch_bounds__(NW_T, 8) k_newton2(const __grid_constant__ Dsm
             bool queued = false;
             if (nd > 0)
             {
-                const float *dl = s_off[tid] >= 0 ? buf + s_off[tid] : d.dlist + (so + s) * DL_STRIDE; // generic: shared or global
                 const float4 *dl4 = reinterpret_cast<const float4 *>(dl);
                 float sum_d = 0.0f, zmn = __int_as_float(0x7f800000), zmx = 0.f;
                 {
@@ -672,17 +697,8 @@ __global__ void __launch_bounds__(NW_T, 8) k_newton2(const __grid_constant__ Dsm
                         d.pfsum[(so + s) * 2] = make_float4(md, __int_as_float(it), zmn, zmx); // the plane-fit scratch is free during the clustering
                         break;
                     }
-                    // every entry in range: sum_a += 2 * residual (2 r is exact, one rounding per add = fmaf(2, r, sum_a)),
-                    // sum_b = nd exact additions of 2
-                    float sa = 0.0f;
-                    int k = 0;
-                    for (; k + 8 <= nd; k += 8)
-                    {
-                        const float4 a = dl4[k >> 2], c = dl4[(k >> 2) + 1];
-                        sa = fmaf(2.0f, md - a.x, sa), sa = fmaf(2.0f, md - a.y, sa), sa = fmaf(2.0f, md - a.z, sa), sa = fmaf(2.0f, md - a.w, sa);
-                        sa = fmaf(2.0f, md - c.x, sa), sa = fmaf(2.0f, md - c.y, sa), sa = fmaf(2.0f, md - c.z, sa), sa = fmaf(2.0f, md - c.w, sa);
-                    }
-                    for (; k < nd; k++) sa = fmaf(2.0f, md - dl[k], sa);
+                    // every entry in range; sum_b = nd exact additions of 2
+                    const float sa = huber_sum_in_range(dl, nd, md);
                     const float delta = (float)((double)(-sa) / ((double)(float)(2 * nd) + 10.0));
                     md = md + delta;
                     if (delta < F_0p01_HI && delta > -F_0p01_HI) break; // |delta| < 0.01 in double (:552)
@@ -694,12 +710,7 @@ __global__ void __launch_bounds__(NW_T, 8) k_newton2(const __grid_constant__ Dsm
                 d.hardq[so + atomicAdd(&d.nhard[b], 1)] = s;
             }
             else
-            {
-                d.seed[so + s] = make_float4(mx, my, mi, md);
-                d.seed_hl[so + s] = split_inverse(md);
-                d.inv_md[so + s] = 1.0 / (double)md; // exact-path operand of the assign pass, only consumed when md > 0 (:378)
-                d.tstable[so + s] = newstable ? DSM_STABLE : -1;
-            }
+                store_seed(d, so + s, mx, my, mi, md, newstable);
         }
     }
 }
@@ -714,36 +725,17 @@ __global__ void __launch_bounds__(NW_T, 8) k_newton_hard(const __grid_constant__
     __shared__ __align__(16) float buf[NW_CAP];
     __shared__ int s_off[NW_T], s_wsum[NW_T / 32];
     const int b = d.frame0 + blockIdx.y;
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int nq = d.nhard[b];
     if (blockIdx.x * NW_T >= nq) return; // whole CTA beyond the queue
-    const int q = blockIdx.x * NW_T + tid;
+    const int q = blockIdx.x * NW_T + threadIdx.x;
     const size_t so = (size_t)b * d.S;
     const bool act = q < nq;
     const int s = act ? d.hardq[so + q] : 0;
     const int nd = act ? d.und[so + s] : 0;
-    { // stage the CTA's lists into shared memory exactly like k_newton2 (coalesced cp.async, all in flight at once)
-        const int len4 = (nd + 3) & ~3;
-        int wtot;
-        const int wex = warp_excl_scan(len4, lane, wtot);
-        if (lane == 31) s_wsum[warp] = wtot;
-        __syncthreads();
-        int base = 0;
-        for (int w = 0; w < warp; w++) base += s_wsum[w];
-        const int off = base + wex;
-        s_off[tid] = (off + len4 <= NW_CAP) ? off : -1;
-    }
-    if (s_off[tid] >= 0)
-    {
-        const float4 *src = reinterpret_cast<const float4 *>(d.dlist + (so + s) * DL_STRIDE);
-        float4 *dst = reinterpret_cast<float4 *>(buf + s_off[tid]);
-        for (int j4 = 0; 4 * j4 < nd; j4++) __pipeline_memcpy_async(dst + j4, src + j4, 16);
-    }
-    __pipeline_commit();
+    const float *dl = stage_list(buf, s_off, s_wsum, d.dlist + (so + s) * DL_STRIDE, nd);
     const float4 st = d.pfsum[(so + s) * 2], mn = d.pfsum[(so + s) * 2 + 1]; // in flight together with the list copies
     __pipeline_wait_prior(0);
     if (!act) return;
-    const float *dl = s_off[tid] >= 0 ? buf + s_off[tid] : d.dlist + (so + s) * DL_STRIDE; // generic: shared or global
     const float4 *dl4 = reinterpret_cast<const float4 *>(dl);
     float md = st.x;
     const float zmn = st.z, zmx = st.w;
@@ -753,14 +745,7 @@ __global__ void __launch_bounds__(NW_T, 8) k_newton_hard(const __grid_constant__
         float sa = 0.0f, sb = 0.0f;
         if ((md - zmn) < d.huber_hi && (md - zmx) > -d.huber_hi)
         { // back inside the range with every entry: the pure chain
-            int k = 0;
-            for (; k + 8 <= nd; k += 8)
-            {
-                const float4 a = dl4[k >> 2], c = dl4[(k >> 2) + 1];
-                sa = fmaf(2.0f, md - a.x, sa), sa = fmaf(2.0f, md - a.y, sa), sa = fmaf(2.0f, md - a.z, sa), sa = fmaf(2.0f, md - a.w, sa);
-                sa = fmaf(2.0f, md - c.x, sa), sa = fmaf(2.0f, md - c.y, sa), sa = fmaf(2.0f, md - c.z, sa), sa = fmaf(2.0f, md - c.w, sa);
-            }
-            for (; k < nd; k++) sa = fmaf(2.0f, md - dl[k], sa);
+            sa = huber_sum_in_range(dl, nd, md);
             sb = (float)(2 * nd);
         }
         else
@@ -791,10 +776,7 @@ __global__ void __launch_bounds__(NW_T, 8) k_newton_hard(const __grid_constant__
         md = md + delta;
         if (delta < F_0p01_HI && delta > -F_0p01_HI) break; // |delta| < 0.01 in double (:552)
     }
-    d.seed[so + s] = make_float4(mn.x, mn.y, mn.z, md);
-    d.seed_hl[so + s] = split_inverse(md);
-    d.inv_md[so + s] = 1.0 / (double)md;
-    d.tstable[so + s] = mn.w != 0.f ? DSM_STABLE : -1;
+    store_seed(d, so + s, mn.x, mn.y, mn.z, md, mn.w != 0.f);
 }
 
 // -------------------------------------------------------------------------------------------
@@ -820,15 +802,15 @@ __global__ void __launch_bounds__(NW_T, 8) k_newton_hard(const __grid_constant__
 // -------------------------------------------------------------------------------------------
 #define PL_STRIDE 232 // floats per plane of a seed's centred-point list (>= 225, multiple of 8)
 #define HREC 24       // doubles per seed: H (9), ho (10), jo (4), packed (margin, qmax2)
-#define PG_SMEM_DEP 0
-#define PG_SMEM_COD TILE_PLANE_BYTES
-#define PG_SMEM_POS (TILE_PLANE_BYTES + TILE_BYTE_PLANE)         // u16 [32][PG_POS_STRIDE]
+#define PG_SMEM_POS TILE_SMEM_OWN                                // u16 [32][PG_POS_STRIDE]
 #define PG_POS_STRIDE 232
 #define PG_SMEM_KX (PG_SMEM_POS + 32 * PG_POS_STRIDE * 2)        // float [80] kx, float [48] ky
 #define PG_SMEM_REC (PG_SMEM_KX + 128 * 4)                       // float maxd[32], int nvalid[32], int ninl[32]
 #define PG_SMEM_BAR (PG_SMEM_REC + 96 * 4)
 #define PG_SMEM_BYTES (PG_SMEM_BAR + 16)
-#define PG_TX_BYTES (DSM_TILE_W * DSM_TILE_H * 4u + (unsigned)DSM_TILE_GW * DSM_TILE_H)
+
+// the seed's record of the plane-fit sums, field i at hr[i * S]: [b][field][seed], so the solver's thread-per-seed reads coalesce
+__device__ __forceinline__ double *hrec_of(const DsmDev &d, int b, int s) { return d.hrec + (size_t)b * HREC * d.S + s; }
 
 __device__ __forceinline__ float group8_sum_f(float v)
 {
@@ -847,8 +829,7 @@ __global__ void __launch_bounds__(256, 4) k_plane_gather(const __grid_constant__
 {
     pdl_enter();
     extern __shared__ __align__(128) unsigned char smem[];
-    const float *t_dep = reinterpret_cast<const float *>(smem + PG_SMEM_DEP);
-    const uint8_t *t_cod = smem + PG_SMEM_COD;
+    const float *t_dep = reinterpret_cast<const float *>(smem + TILE_SMEM_DEP);
     uint16_t *s_pos = reinterpret_cast<uint16_t *>(smem + PG_SMEM_POS);
     float *s_kx = reinterpret_cast<float *>(smem + PG_SMEM_KX), *s_ky = s_kx + 80;
     float *s_maxd = reinterpret_cast<float *>(smem + PG_SMEM_REC);
@@ -858,13 +839,7 @@ __global__ void __launch_bounds__(256, 4) k_plane_gather(const __grid_constant__
     const int b = d.frame0 + blockIdx.z;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int X0 = blockIdx.x * (DSM_TILE_SX * DSM_SP) - DSM_SP / 2, Y0 = blockIdx.y * (DSM_TILE_SY * DSM_SP) - DSM_SP / 2;
-    if (threadIdx.x == 0)
-    {
-        mbar_init(bar, 1);
-        mbar_expect_tx(bar, PG_TX_BYTES);
-        tma_load_3d(smem_u32(smem + PG_SMEM_DEP), &mp.dep, X0, Y0, b, bar);
-        tma_load_3d(smem_u32(smem + PG_SMEM_COD), &mp.cod, X0 - DSM_TILE_GX, Y0, b, bar);
-    }
+    if (threadIdx.x == 0) tile_issue(smem, bar, TILE_TX_BYTES, mp, X0, Y0, b);
     const int W = d.W, H = d.H;
     const size_t so = (size_t)b * d.S;
     // back-projection factors of the tile's columns / rows (tables hold Wp+16 / H+16 entries; clamp the halo)
@@ -885,10 +860,8 @@ __global__ void __launch_bounds__(256, 4) k_plane_gather(const __grid_constant__
 #pragma unroll
     for (int rd = 0; rd < 2; rd++)
     {
-        const int sl = rd * 16 + warp * 2 + half;
-        const int sp_x = blockIdx.x * DSM_TILE_SX + (sl & 7), sp_y = blockIdx.y * DSM_TILE_SY + (sl >> 3);
-        const bool live = sp_x < d.spw && sp_y < d.sph;
-        sdv[rd] = d.seed[so + (live ? sp_y * d.spw + sp_x : 0)]; // x, y, I, mean_depth (Huber mean after the 3 iterations)
+        const TileSeed t = tile_seed(d, rd * 16 + warp * 2 + half);
+        sdv[rd] = d.seed[so + (t.live ? t.sp_y * d.spw + t.sp_x : 0)]; // x, y, I, mean_depth (Huber mean after the 3 iterations)
     }
     __syncthreads();
     mbar_wait(bar, 0);
@@ -897,35 +870,22 @@ __global__ void __launch_bounds__(256, 4) k_plane_gather(const __grid_constant__
     for (int rd = 0; rd < 2; rd++)
     {
         const int sl = rd * 16 + warp * 2 + half;
-        const int tx = sl & 7, ty = sl >> 3;
-        const int sp_x = blockIdx.x * DSM_TILE_SX + tx, sp_y = blockIdx.y * DSM_TILE_SY + ty;
-        const bool live = sp_x < d.spw && sp_y < d.sph;
+        const TileSeed t = tile_seed(d, sl);
         const float4 sd = sdv[rd];
-        const int x0 = sp_x * DSM_SP - DSM_SP / 2, y0 = sp_y * DSM_SP - DSM_SP / 2;
+        const int x0 = t.sp_x * DSM_SP - DSM_SP / 2, y0 = t.sp_y * DSM_SP - DSM_SP / 2;
         const int y = y0 + r;
-        const bool rowin = live && y >= 0 && y < H; // window bounded by the flat index only (:816)
+        const bool rowin = t.live && y >= 0 && y < H; // window bounded by the flat index only (:816)
         const int kb = x0 < 0 ? -x0 : 0, ke = (W - x0) < 16 ? (W - x0) : 16;
         const unsigned kmask = rowin ? (((1u << ke) - 1u) & ~((1u << kb) - 1u)) : 0u;
-        const int trow = ty * DSM_SP + r, tcol = tx * DSM_SP;
-        unsigned mm, vm = 0, im = 0; // bit k: labelled with this seed / depth > 0.05 / |mean_depth - depth| < HUBER_RANGE
+        const int trow = t.ty * DSM_SP + r, tcol = t.tx * DSM_SP;
+        float zk[16];
+        unsigned mm = window_row(smem, trow, tcol, r, zk), vm = 0, im = 0; // bit k: labelled with this seed / depth > 0.05 / |mean_depth - depth| < HUBER_RANGE
+#pragma unroll
+        for (int k = 0; k < 16; k++)
         {
-            const unsigned *pc = reinterpret_cast<const unsigned *>(t_cod + trow * DSM_TILE_GW + DSM_TILE_GX + tcol); // 4-byte aligned
-            const unsigned cw[4] = {pc[0], pc[1], pc[2], pc[3]};
-            mm = member_mask16(cw, r);
-            const float4 *pz = reinterpret_cast<const float4 *>(t_dep + trow * DSM_TILE_W + tcol);
-#pragma unroll
-            for (int qd = 0; qd < 4; qd++)
-            {
-                const float4 z = pz[qd];
-                const float zz[4] = {z.x, z.y, z.z, z.w};
-#pragma unroll
-                for (int j = 0; j < 4; j++)
-                {
-                    vm |= (zz[j] > F_0p05_LO ? 1u : 0u) << (4 * qd + j); // (double)depth > 0.05 (:827)
-                    const float rr = sd.w - zz[j];
-                    im |= ((rr < d.huber_hi && rr > -d.huber_hi) ? 1u : 0u) << (4 * qd + j); // inlier (:849-860)
-                }
-            }
+            vm |= (zk[k] > F_0p05_LO ? 1u : 0u) << k; // (double)depth > 0.05 (:827)
+            const float rr = sd.w - zk[k];
+            im |= ((rr < d.huber_hi && rr > -d.huber_hi) ? 1u : 0u) << k; // inlier (:849-860)
         }
         mm &= kmask;
         vm &= mm;
@@ -947,16 +907,8 @@ __global__ void __launch_bounds__(256, 4) k_plane_gather(const __grid_constant__
             maxd = fmaxf(maxd, __shfl_xor_sync(FULL, maxd, o));
             nvalid += __shfl_xor_sync(FULL, nvalid, o);
         }
-        const int c = __popc(im);
-        int incl = c;
-#pragma unroll
-        for (int o = 1; o < 16; o <<= 1)
-        {
-            const int nb = __shfl_up_sync(FULL, incl, o, 16);
-            if (r >= o) incl += nb;
-        }
-        const int ninl = __shfl_sync(FULL, incl, 15, 16);
-        uint16_t *pp = s_pos + sl * PG_POS_STRIDE + (incl - c);
+        int ninl;
+        uint16_t *pp = s_pos + sl * PG_POS_STRIDE + half_warp_scan(__popc(im), r, ninl);
         const int pbase = (trow << 7) | tcol; // (tile row, tile column) packed: no division when unpacking
 #pragma unroll
         for (int k = 0; k < 16; k++)
@@ -972,9 +924,9 @@ __global__ void __launch_bounds__(256, 4) k_plane_gather(const __grid_constant__
     // ---- phase 2: 8 lanes per seed, 4 seeds per warp; lane gl of a group walks the inliers gl, gl + 8, ...
     const int gl = lane & 7;
     const int sl = warp * 4 + (lane >> 3);
-    const int sp_x = blockIdx.x * DSM_TILE_SX + (sl & 7), sp_y = blockIdx.y * DSM_TILE_SY + (sl >> 3);
-    const bool live = sp_x < d.spw && sp_y < d.sph;
-    const int s = sp_y * d.spw + sp_x;
+    const TileSeed t = tile_seed(d, sl);
+    const bool live = t.live;
+    const int s = t.sp_y * d.spw + t.sp_x;
     const int nvalid = s_nvalid[sl], ninl_raw = s_ninl[sl];
     const float maxd = s_maxd[sl];
     const bool ok = live && nvalid >= 16 && !((float)ninl_raw / (float)nvalid < F_0p8_HI); // (:841), (double)ratio < 0.8 (:862)
@@ -1059,7 +1011,7 @@ __global__ void __launch_bounds__(256, 4) k_plane_gather(const __grid_constant__
         rnan |= __shfl_xor_sync(FULL, rnan ? 1 : 0, o) != 0;
     }
     if (rnan) margin = __int_as_float(0x7fc00000); // a NaN residual: no pass may ever be skipped
-    double *hr = d.hrec + (size_t)b * HREC * d.S + s; // [b][field][seed]: the solver's thread-per-seed reads coalesce
+    double *hr = hrec_of(d, b, s);
     const size_t hs = (size_t)d.S;
     if (ok)
     { // the group's lanes write the 9 sums and the packed (margin, qmax2)
@@ -1206,6 +1158,14 @@ __device__ __forceinline__ float gn_step(const double *hh0, const double *jo, fl
     return qmax * sqrtf(dx * dx + dy * dy + dz * dz) * 1.0001f + fabsf(nb - ob) + 1e-4f;
 }
 
+// H over all n points of a seed: the 9 sums k_plane_gather recorded and ww = 2 n
+__device__ __forceinline__ void load_h_all(const double *hr, size_t hs, int n, double *hh0)
+{
+#pragma unroll
+    for (int i = 0; i < 9; i++) hh0[i] = hr[i * hs];
+    hh0[9] = 2.0 * (double)n;
+}
+
 #define GS_CAP 9216 // floats of point staging per 128-seed CTA (36 KB): three planes of the queued seeds' centred points
 __global__ void __launch_bounds__(128, 4) k_gn_solve(const __grid_constant__ DsmDev d)
 {
@@ -1240,12 +1200,10 @@ __global__ void __launch_bounds__(128, 4) k_gn_solve(const __grid_constant__ Dsm
         {
             const float len0 = sqrtf(P0.x * P0.x + P0.y * P0.y + P0.z * P0.z);
             float nx = P0.x / len0, ny = P0.y / len0, nz = P0.z / len0, nb = 0.f; // len0 == 0 -> NaN, propagated (H6-iii)
-            const double *hr = d.hrec + (size_t)b * HREC * d.S + s; // [b][field][seed]
+            const double *hr = hrec_of(d, b, s);
             // hh0 = H over the in-range points = H_all - ho; jo = clamped gradient of the out-of-range points
             double hh0[10], jo[4] = {0, 0, 0, 0};
-#pragma unroll
-            for (int i = 0; i < 9; i++) hh0[i] = hr[i * hs];
-            hh0[9] = 2.0 * (double)n;
+            load_h_all(hr, hs, n, hh0);
             if (hr[18 * hs] != 0.0)
             { // the first pass found points outside the Huber range
 #pragma unroll
@@ -1301,7 +1259,7 @@ __global__ void __launch_bounds__(128, 4) k_gn_solve(const __grid_constant__ Dsm
         const float4 sd = d.seed[o2];
         const float4 P0 = d.pfsum[o2 * 2], P1 = d.pfsum[o2 * 2 + 1];
         const int n = __float_as_int(P1.w), l4 = ((n + 3) & ~3) >> 2;
-        const double *hr = d.hrec + (size_t)b * HREC * d.S + (blockIdx.x * 128 + t2);
+        const double *hr = hrec_of(d, b, blockIdx.x * 128 + t2);
         const float qmax = sqrtf(__int_as_float(__double2hiint(hr[23 * hs])));
         const float4 th = s_theta[t2];
         float nx = th.x, ny = th.y, nz = th.z, nb = th.w;
@@ -1314,9 +1272,7 @@ __global__ void __launch_bounds__(128, 4) k_gn_solve(const __grid_constant__ Dsm
         {
             if (!(moved + 2e-3f < margin))
             { // classify the points again (:131-171)
-#pragma unroll
-                for (int i = 0; i < 9; i++) hh0[i] = hr[i * hs];
-                hh0[9] = 2.0 * (double)n;
+                load_h_all(hr, hs, n, hh0);
 #pragma unroll
                 for (int i = 0; i < 4; i++) jo[i] = 0.0;
                 float mg = __int_as_float(0x7f800000);
@@ -1390,10 +1346,11 @@ void dsm_launch_assign2(const DsmDev &d, int nb, bool first, cudaStream_t s)
     else
         pdl_launch(k_assign2<false>, grid, block, 0, s, d);
 }
+// one CTA per 8 x 4 seed tile of every frame (k_gather, k_plane_gather)
+static dim3 tile_grid(const DsmDev &d, int nb) { return dim3((d.spw + DSM_TILE_SX - 1) / DSM_TILE_SX, (d.sph + DSM_TILE_SY - 1) / DSM_TILE_SY, nb); }
 void dsm_launch_gather(const DsmDev &d, const DsmMaps &m, int nb, cudaStream_t s)
 {
-    dim3 grid((d.spw + DSM_TILE_SX - 1) / DSM_TILE_SX, (d.sph + DSM_TILE_SY - 1) / DSM_TILE_SY, nb);
-    pdl_launch(k_gather, grid, dim3(256), GAT_SMEM_BYTES, s, d, m);
+    pdl_launch(k_gather, tile_grid(d, nb), dim3(256), GAT_SMEM_BYTES, s, d, m);
 }
 void dsm_launch_newton2(const DsmDev &d, int nb, cudaStream_t s)
 {
@@ -1403,8 +1360,7 @@ void dsm_launch_newton2(const DsmDev &d, int nb, cudaStream_t s)
 }
 void dsm_launch_plane_gather(const DsmDev &d, const DsmMaps &m, int nb, cudaStream_t s)
 {
-    dim3 grid((d.spw + DSM_TILE_SX - 1) / DSM_TILE_SX, (d.sph + DSM_TILE_SY - 1) / DSM_TILE_SY, nb);
-    pdl_launch(k_plane_gather, grid, dim3(256), PG_SMEM_BYTES, s, d, m);
+    pdl_launch(k_plane_gather, tile_grid(d, nb), dim3(256), PG_SMEM_BYTES, s, d, m);
 }
 void dsm_launch_gn_solve(const DsmDev &d, int nb, cudaStream_t s)
 {

@@ -67,10 +67,18 @@ def test_synthetic_generator_is_deterministic():
 
 def test_float_bounds_for_double_literal_compares():
     """csrc/dsm_exact.cuh (used by every kernel file) replaces `(double)x < c` by `x < c_hi` (and `> c` by `> c_lo`) in hot loops;
-    every F_<c>_HI / _LO constant must be the float neighbour of the double literal c."""
-    src = open(os.path.join(ROOT, "densesurfelmapping_b200", "csrc", "dsm_exact.cuh")).read()
+    every F_<c>_HI / _LO constant must be the float neighbour of the double literal c, and the kernel files use exactly
+    the constants the header defines."""
+    csrc = os.path.join(ROOT, "densesurfelmapping_b200", "csrc")
+    src = open(os.path.join(csrc, "dsm_exact.cuh")).read()
     found = re.findall(r"#define F_(\d+)p(\d+)_(HI|LO) __uint_as_float\(0x([0-9a-f]+)u\)", src)
-    assert len(found) >= 8
+    defined = {f"F_{ip}p{fp}_{kind}" for ip, fp, kind, _ in found}
+    assert len(defined) == len(found) == len(re.findall(r"#define F_", src))  # every F_ macro parsed, none twice
+    used = set()
+    for name in os.listdir(csrc):
+        if name.endswith(".cu"):
+            used |= set(re.findall(r"\bF_\d+p\d+_(?:HI|LO)\b", open(os.path.join(csrc, name)).read()))
+    assert used == defined, (sorted(used - defined), sorted(defined - used))
     for ip, fp, kind, hexv in found:
         c = float(f"{ip}.{fp}")
         f = np.array([int(hexv, 16)], dtype=np.uint32).view(np.float32)[0]

@@ -1,9 +1,13 @@
 """The C++ drop-in: include/dsm_fusion_functions.hpp mirrors the reference's FusionFunctions class.
 CPU: it compiles against cv::Mat / Eigen-like caller types and links to the C ABI; without a GPU it
 fails loudly (exit code 3, no fallback).  GPU: its results match the oracle."""
+import atexit
+import functools
 import os
+import shutil
 import struct
 import subprocess
+import tempfile
 
 import numpy as np
 import pytest
@@ -13,15 +17,20 @@ from densesurfelmapping_b200.elements import SURFEL_DTYPE
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 PKG = os.path.join(ROOT, "densesurfelmapping_b200")
-BIN = os.path.join(ROOT, "tests", "cpp", "adapter_main")
 
 
-def build_adapter(name="adapter_main", header="dsm_fusion_functions.hpp"):
+@functools.lru_cache(maxsize=None)
+def _bin_dir():
+    d = tempfile.mkdtemp(prefix="dsm_cpp_adapter_")
+    atexit.register(shutil.rmtree, d, True)
+    return d
+
+
+@functools.lru_cache(maxsize=None)
+def build_adapter(name="adapter_main"):
+    """tests/cpp/<name>.cpp compiled once per session, outside the tree (the checkout may be read-only)."""
     src = os.path.join(ROOT, "tests", "cpp", name + ".cpp")
-    out = os.path.join(ROOT, "tests", "cpp", name)
-    deps = [src, os.path.join(ROOT, "include", header), os.path.join(ROOT, "include", "dsm.h")]
-    if os.path.exists(out) and os.path.getmtime(out) > max(os.path.getmtime(p) for p in deps):
-        return out
+    out = os.path.join(_bin_dir(), name)
     cmd = ["g++", "-std=c++11", "-O2", "-Wall", "-I", os.path.join(ROOT, "include"), "-I", os.path.join(ROOT, "oracle", "shim"), src,
            "-o", out, "-L", PKG, "-ldsm_b200", f"-Wl,-rpath,{PKG}"]
     r = subprocess.run(cmd, capture_output=True, text=True)
@@ -34,7 +43,7 @@ def run_adapter(tmp, cam, ref, pose, gray, depth, local):
     with open(fin, "wb") as f:
         f.write(struct.pack("<i", ref) + np.asarray(pose, np.float32).tobytes() + struct.pack("<i", len(local)))
         f.write(gray.tobytes() + depth.tobytes() + local.tobytes())
-    args = [BIN, str(cam.width), str(cam.height)] + [repr(float(v)) for v in (cam.fx, cam.fy, cam.cx, cam.cy, cam.far, cam.near)] + [fin, fout]
+    args = [build_adapter(), str(cam.width), str(cam.height)] + [repr(float(v)) for v in (cam.fx, cam.fy, cam.cx, cam.cy, cam.far, cam.near)] + [fin, fout]
     r = subprocess.run(args, capture_output=True, text=True)
     return r, fout
 
@@ -81,7 +90,7 @@ def write_stream(path, cam, frames, warp, retire_kf):
 
 
 def run_resident(tmp, cam, frames, warp, retire_kf):
-    exe = build_adapter("resident_main", "dsm_surfel_map.hpp")
+    exe = build_adapter("resident_main")
     fin = os.path.join(tmp, "stream.bin")
     outs = [os.path.join(tmp, n) for n in ("out.bin", "cloud.pcd", "mesh.ply")]
     write_stream(fin, cam, frames, warp, retire_kf)
@@ -91,7 +100,7 @@ def run_resident(tmp, cam, frames, warp, retire_kf):
 
 def test_resident_helper_compiles_and_fails_loudly_without_gpu(tmp_path):
     import torch
-    build_adapter("resident_main", "dsm_surfel_map.hpp")
+    build_adapter("resident_main")
     if torch.cuda.is_available():
         pytest.skip("GPU present")
     cam = synth.VGA

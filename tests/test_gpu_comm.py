@@ -29,7 +29,7 @@ def _run_batch(capi, device, rank):
     return ctx, gather.pack_payload(news, local, ofs)
 
 
-def test_single_rank_gather_equals_batch_download():
+def _single_rank_gather():
     from densesurfelmapping_b200 import capi
     ctx, want = _run_batch(capi, 0, 0)
     ctx.comm_init(capi.comm_unique_id(), 0, 1)
@@ -41,6 +41,18 @@ def test_single_rank_gather_equals_batch_download():
     news, pool, ofs = gather.unpack_payload(got)
     assert len(news) == B and sum(len(a) for a in news) > 0 and len(pool) == ofs[-1] > 0
     ctx.close()
+
+
+def test_single_rank_gather_equals_batch_download():
+    """Peer transport: the pack kernel writes into the context's own slot."""
+    _single_rank_gather()
+
+
+def test_single_rank_nccl_gather_equals_batch_download(monkeypatch):
+    """NCCL transport: the same pack kernel writes into the send buffer; the root copies its own payload into the receive
+    buffer."""
+    monkeypatch.setenv("DSM_GATHER_NCCL", "1")  # read by dsm_comm_init
+    _single_rank_gather()
 
 
 def _worker(rank, world, uid_q, res_q, transport="peer"):

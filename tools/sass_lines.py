@@ -6,9 +6,11 @@ lib = os.path.join(ROOT, "densesurfelmapping_b200", "libdsm_b200.so")
 pat, top = sys.argv[1], int(sys.argv[2]) if len(sys.argv) > 2 else 30
 tmp = tempfile.mkdtemp()
 subprocess.run(["cuobjdump", "-xelf", "all", lib], cwd=tmp, capture_output=True)
-cub = [f for f in os.listdir(tmp) if f.startswith("dsm_kernels.") and f.endswith(".cubin")][0]
-txt = subprocess.run(["nvdisasm", "-g", "-c", os.path.join(tmp, cub)], capture_output=True, text=True).stdout.splitlines()
-src = open(os.path.join(ROOT, "densesurfelmapping_b200", "csrc", "dsm_kernels.cu")).read().splitlines()
+for cub in sorted(f for f in os.listdir(tmp) if f.endswith(".cubin")):  # the cubin that holds the kernel
+    txt = subprocess.run(["nvdisasm", "-g", "-c", os.path.join(tmp, cub)], capture_output=True, text=True).stdout.splitlines()
+    if any(l.startswith(".text.") and pat in l for l in txt):
+        break
+src = {}  # source file named in the line info -> its lines
 fn = cur = None
 cnts = {}
 for l in txt:
@@ -31,4 +33,7 @@ for f, c in cnts.items():
                 print(f"{n:5d}  ?")
                 continue
             fl, ln = k
-            print(f"{n:5d}  {fl}:{ln}: {src[ln - 1].strip()[:105] if fl.startswith('dsm_kernels') else ''}")
+            if fl not in src:
+                path = os.path.join(ROOT, "densesurfelmapping_b200", "csrc", fl)
+                src[fl] = open(path).read().splitlines() if os.path.exists(path) else []
+            print(f"{n:5d}  {fl}:{ln}: {src[fl][ln - 1].strip()[:105] if ln <= len(src[fl]) else ''}")
