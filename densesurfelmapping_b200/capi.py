@@ -28,7 +28,7 @@ EXPORTS = [
     "dsm_debug_stop_after", "dsm_debug_invariant_violations", "dsm_profile_enable", "dsm_profile_reset", "dsm_profile_read", "dsm_kernel_name", "dsm_device_buffer",
     "dsm_pool_export_cloud", "dsm_pool_export_surfels", "dsm_write_pcd", "dsm_write_ply_mesh", "dsm_mesh_vertices", "dsm_fuse_stream_resident",
     "dsm_inactive_reserve", "dsm_inactive_retire", "dsm_inactive_reactivate", "dsm_inactive_transform", "dsm_inactive_export_cloud",
-    "dsm_inactive_download", "dsm_inactive_size",
+    "dsm_inactive_download", "dsm_inactive_size", "dsm_frame_raw_cloud", "dsm_inactive_export_poses",
     "dsm_comm_unique_id", "dsm_comm_init", "dsm_comm_destroy", "dsm_gather_deltas", "dsm_gather_wait", "dsm_gathered_device",
     "dsm_gathered_rank_bytes", "dsm_gathered_download", "dsm_set_constants", "dsm_set_concurrency",
 ]
@@ -98,6 +98,8 @@ def load_library():
     L.dsm_inactive_reactivate.argtypes = [vp, ci, ctypes.POINTER(ci)]
     L.dsm_inactive_transform.argtypes = [vp, ci, vp]
     L.dsm_inactive_export_cloud.argtypes = [vp, vp, ci, ctypes.POINTER(ci)]
+    L.dsm_inactive_export_poses.argtypes = [vp, vp, ci, vp, ci, ctypes.POINTER(ci)]
+    L.dsm_frame_raw_cloud.argtypes = [vp, ci, vp, vp, ci, ctypes.POINTER(ci)]
     L.dsm_inactive_download.argtypes = [vp, ci, vp, ci, ctypes.POINTER(ci)]
     L.dsm_inactive_size.argtypes = [vp, ctypes.POINTER(ci), ctypes.POINTER(ci)]
     L.dsm_pool_retire.argtypes = [vp, ci, vp, ci, ctypes.POINTER(ci)]
@@ -372,6 +374,28 @@ class Context:
         out = np.zeros(max(cap, 1), dtype=POINT_DTYPE)
         n = ctypes.c_int(0)
         self._ck(self.lib.dsm_inactive_export_cloud(self.h, _ptr(out), cap, ctypes.byref(n)))
+        return out[:min(n.value, cap)].copy()
+
+    def inactive_export_poses(self, keyframes, cap=None):
+        """The inactive half of publish_neighbor_pointcloud (surfel_map.cpp:1306-1321): the stored points of each listed
+        keyframe, list order; keyframes with nothing stored contribute nothing.  POINT_DTYPE array."""
+        kf = np.ascontiguousarray(keyframes, dtype=np.int32).reshape(-1)
+        cap = self.inactive_size()[0] if cap is None else cap
+        out = np.zeros(max(cap, 1), dtype=POINT_DTYPE)
+        n = ctypes.c_int(0)
+        self._ck(self.lib.dsm_inactive_export_poses(self.h, _ptr(kf) if len(kf) else None, len(kf), _ptr(out), cap, ctypes.byref(n)))
+        return out[:min(n.value, cap)].copy()
+
+    # ---- raw cloud of a frame ----
+    def frame_raw_cloud(self, frame, pose7, cap=None):
+        """publish_raw_pointcloud (surfel_map.cpp:1115-1151) on frame `frame` of the most recent call that took images:
+        W*H POINT_DTYPE points, column-major (point i*H + j = column i, row j).  pose7 = (px, py, pz, qx, qy, qz, qw)."""
+        p = np.ascontiguousarray(pose7, dtype=np.float64).reshape(7)
+        npx = self.cam.width * self.cam.height
+        cap = npx if cap is None else cap
+        out = np.zeros(max(cap, 1), dtype=POINT_DTYPE)
+        n = ctypes.c_int(0)
+        self._ck(self.lib.dsm_frame_raw_cloud(self.h, int(frame), _ptr(p), _ptr(out), cap, ctypes.byref(n)))
         return out[:min(n.value, cap)].copy()
 
     # ---- parity readback ----

@@ -427,6 +427,7 @@ extern "C" int dsm_batch_upload(dsm_ctx *ctx, int n, const int32_t *ref, const u
         ProfScope p(ctx, DSM_K_REPACK);
         dsm_launch_repack(d, n, ctx->gray_packed, ctx->depth_packed, ctx->stream);
     }
+    ctx->img_slot0 = 0, ctx->img_n = n;
     if (ctx->n_pool > 0)
     {
         CK(cudaMemcpyAsync(ctx->d.pool, local, (size_t)ctx->n_pool * sizeof(dsm_surfel_t), cudaMemcpyHostToDevice, ctx->stream));
@@ -736,6 +737,7 @@ extern "C" int dsm_fuse_batch_async(dsm_ctx *ctx, int n, const int32_t *ref, con
     ctx->uploaded = true;
     ctx->ran = true;
     ctx->in_flight = true;
+    ctx->img_slot0 = 0, ctx->img_n = n;
     ctx->res_active = false; // the pool buffer now holds this batch's slices: a resident pool (if any) is gone
     CK(cudaGetLastError());
     return DSM_OK;
@@ -776,6 +778,7 @@ extern "C" int dsm_fuse_frame(dsm_ctx *ctx, int ref_idx, const uint8_t *gray, si
         CK(cudaMemcpyAsync(ctx->d.pool, local, (size_t)n_local * sizeof(dsm_surfel_t), cudaMemcpyHostToDevice, ctx->stream));
     ctx->nb = 1;
     ctx->uploaded = true;
+    ctx->img_slot0 = 0, ctx->img_n = 1;
     rc = dsm_batch_run(ctx);
     if (rc != DSM_OK) return rc;
     if (n_local > 0)
@@ -996,6 +999,7 @@ extern "C" int dsm_fuse_frame_resident(dsm_ctx *ctx, int ref_idx, const uint8_t 
     }
     ctx->nb = slot + 1;
     ctx->uploaded = true;
+    ctx->img_slot0 = slot, ctx->img_n = 1;
     // + post-step of SurfelMap::fuse_map on the device: compact into the alternate buffer, then swap
     rc = enqueue_schedule(ctx, dv, 1, ctx->stream, ctx->pool_snap);
     if (rc != DSM_OK) return rc;
@@ -1178,27 +1182,55 @@ extern "C" int dsm_inactive_download(dsm_ctx *ctx, int kf, dsm_surfel_t *out, in
     return DSM_OK;
 }
 
+// The store ranges [ofs, ofs + cnt) as one PointXYZI per stored surfel, concatenated in list order: *n_out = their total,
+// the first min(cap, total) points are written
+static int inactive_export_ranges(dsm_ctx *ctx, const std::vector<dsm_ctx::InactSeg> &ranges, dsm_point_t *out, int cap, int *n_out)
+{
+    CK(cudaSetDevice(ctx->device));
+    int total = 0;
+    for (const auto &r : ranges) total += r.cnt;
+    *n_out = total;
+    const int npool = ctx->p.max_local_surfels > 0 ? ctx->p.max_local_surfels : 1;
+    const DsmDev d = inactive_view(ctx);
+    int n = 0;
+    for (const auto &r : ranges)
+        for (int c0 = 0; c0 < r.cnt && n < cap;)
+        { // chunks sized for the block tables and the alternate pool buffer (16-byte points into 44-byte slots)
+            int len = r.cnt - c0;
+            if (len > npool) len = npool;
+            if (len > cap - n) len = cap - n;
+            dsm_launch_set2(ctx->inact_ofs, r.ofs + c0, r.ofs + c0 + len, ctx->stream);
+            dsm_launch_pool_export(d, 0, len, 2, INT32_MIN, true, ctx->blkcnt, ctx->blkofs, ctx->newofs, ctx->pool_snap, ctx->stream);
+            CK(cudaMemcpyAsync(out + n, ctx->pool_snap, (size_t)len * sizeof(dsm_point_t), cudaMemcpyDeviceToHost, ctx->stream));
+            c0 += len;
+            n += len;
+        }
+    CK(cudaStreamSynchronize(ctx->stream));
+    CK(cudaGetLastError());
+    return DSM_OK;
+}
+
 // inactive_pointcloud (publish_inactive_pointcloud surfel_map.cpp:1385-1396, the tail of publish_all_pointcloud and
 // save_cloud): one PointXYZI per stored surfel, store order
 extern "C" int dsm_inactive_export_cloud(dsm_ctx *ctx, dsm_point_t *out, int cap, int *n_out)
 {
     if (!ctx || !n_out || cap < 0 || (cap > 0 && !out)) return DSM_E_INVALID;
     if (!ctx->inact) return DSM_E_STATE;
-    CK(cudaSetDevice(ctx->device));
-    *n_out = ctx->inact_size;
-    const int want = ctx->inact_size < cap ? ctx->inact_size : cap;
-    const int npool = ctx->p.max_local_surfels > 0 ? ctx->p.max_local_surfels : 1;
-    const DsmDev d = inactive_view(ctx);
-    for (int c0 = 0; c0 < want; c0 += npool)
-    { // chunks sized for the block tables and the alternate pool buffer (16-byte points into 44-byte slots)
-        const int len = (want - c0) < npool ? (want - c0) : npool;
-        dsm_launch_set2(ctx->inact_ofs, c0, c0 + len, ctx->stream);
-        dsm_launch_pool_export(d, 0, len, 2, INT32_MIN, true, ctx->blkcnt, ctx->blkofs, ctx->newofs, ctx->pool_snap, ctx->stream);
-        CK(cudaMemcpyAsync(out + c0, ctx->pool_snap, (size_t)len * sizeof(dsm_point_t), cudaMemcpyDeviceToHost, ctx->stream));
-    }
-    CK(cudaStreamSynchronize(ctx->stream));
-    CK(cudaGetLastError());
-    return DSM_OK;
+    return inactive_export_ranges(ctx, {dsm_ctx::InactSeg{-1, 0, ctx->inact_size}}, out, cap, n_out);
+}
+
+// the inactive half of publish_neighbor_pointcloud (surfel_map.cpp:1306-1321): the stored points of each listed
+// keyframe, list order, store order within a keyframe.  A keyframe without stored points (a local pose, or one with
+// empty attached_surfels) contributes nothing, which is the reference's skip of both (:1311-1316).
+extern "C" int dsm_inactive_export_poses(dsm_ctx *ctx, const int32_t *keyframes, int n_keyframes, dsm_point_t *out, int cap, int *n_out)
+{
+    if (!ctx || !n_out || n_keyframes < 0 || (n_keyframes > 0 && !keyframes) || cap < 0 || (cap > 0 && !out)) return DSM_E_INVALID;
+    if (!ctx->inact) return DSM_E_STATE;
+    std::vector<dsm_ctx::InactSeg> ranges;
+    for (int k = 0; k < n_keyframes; k++)
+        for (const auto &sg : ctx->inact_segs)
+            if (sg.kf == keyframes[k]) ranges.push_back(sg);
+    return inactive_export_ranges(ctx, ranges, out, cap, n_out);
 }
 
 // A run of n consecutive frames of ONE sequential stream on the resident pool.  Results are identical to n calls of
@@ -1277,6 +1309,7 @@ extern "C" int dsm_fuse_stream_resident(dsm_ctx *ctx, int n, const int32_t *ref_
     }
     ctx->nb = slot0 + n;
     ctx->uploaded = true;
+    ctx->img_slot0 = slot0, ctx->img_n = n; // ordered before the main stream through phase 2 (ev_join / ev_p2) below
     rc = enqueue_schedule(ctx, v, n, s1, nullptr, 1);
     if (rc != DSM_OK) return rc;
     if (dbl)
@@ -1309,6 +1342,50 @@ extern "C" int dsm_fuse_stream_resident(dsm_ctx *ctx, int n, const int32_t *ref_
         CK(cudaMemcpyAsync(n_new, ctx->d.nnew + slot0, (size_t)n * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
         CK(cudaStreamSynchronize(st));
     }
+    return DSM_OK;
+}
+
+// ---- raw cloud of a frame (publish_raw_pointcloud, surfel_map.cpp:1115-1151) ----
+// R = Quaternionf(qw, qx, qy, qz).toRotationMatrix() (not normalised) and T = position, in float like the reference
+static DsmRawPose raw_pose(const double p7[7])
+{
+    const float qx = (float)p7[3], qy = (float)p7[4], qz = (float)p7[5], qw = (float)p7[6];
+    const float tx = 2.f * qx, ty = 2.f * qy, tz = 2.f * qz;
+    const float twx = tx * qw, twy = ty * qw, twz = tz * qw;
+    const float txx = tx * qx, txy = ty * qx, txz = tz * qx;
+    const float tyy = ty * qy, tyz = tz * qy, tzz = tz * qz;
+    return DsmRawPose{{1.f - (tyy + tzz), txy - twz, txz + twy,
+                       txy + twz, 1.f - (txx + tzz), tyz - twx,
+                       txz - twy, tyz + twx, 1.f - (txx + tyy)},
+                      {(float)p7[0], (float)p7[1], (float)p7[2]}};
+}
+
+extern "C" int dsm_frame_raw_cloud(dsm_ctx *ctx, int frame, const double pose7[7], dsm_point_t *out, int cap, int *n_out)
+{
+    if (!ctx || !pose7 || !n_out || cap < 0 || (cap > 0 && !out)) return DSM_E_INVALID;
+    if (ctx->img_n == 0) return DSM_E_STATE;
+    if (frame < 0 || frame >= ctx->img_n) return DSM_E_INVALID;
+    CK(cudaSetDevice(ctx->device));
+    if (ctx->in_flight)
+    { // the chunks of dsm_fuse_batch_async copy and repack on their own streams: finish the batch first
+        int rcw = dsm_batch_wait(ctx);
+        if (rcw != DSM_OK) return rcw;
+    }
+    const int W = ctx->p.width, H = ctx->p.height;
+    const size_t npx = (size_t)W * H;
+    if (!ctx->raw_out && ctx->own.device(&ctx->raw_out, npx) != cudaSuccess)
+    {
+        cudaGetLastError();
+        ctx->raw_out = nullptr;
+        return DSM_E_NOMEM;
+    }
+    // every entry point leaves the frame's copy and repack ordered before later work on the main stream
+    dsm_launch_raw_cloud(ctx->d, ctx->img_slot0 + frame, raw_pose(pose7), ctx->raw_out, ctx->stream);
+    CK(cudaGetLastError());
+    *n_out = (int)npx;
+    const size_t c = npx < (size_t)cap ? npx : (size_t)cap;
+    if (c > 0) CK(cudaMemcpyAsync(out, ctx->raw_out, c * sizeof(dsm_point_t), cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
     return DSM_OK;
 }
 

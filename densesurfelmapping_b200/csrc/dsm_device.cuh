@@ -139,6 +139,12 @@ void dsm_launch_pool_compact(const DsmDev &d, int frame, int upper, int *blkcnt,
 void dsm_launch_pool_transform(const DsmDev &d, int frame, int upper, const float *Wm_dev, cudaStream_t s);
 void dsm_launch_pool_export(const DsmDev &d, int frame, int upper, int mode, int key, bool as_cloud, int *blkcnt, int *blkofs, int *newofs, void *dst, cudaStream_t s);
 void dsm_launch_set2(int32_t *p, int a, int b, cudaStream_t s);
+// camera -> world of dsm_frame_raw_cloud: R row-major (R[3r + c] = R(r, c)) and T, formed on the host
+struct DsmRawPose
+{
+    float R[9], T[3];
+};
+void dsm_launch_raw_cloud(const DsmDev &d, int frame, const DsmRawPose &pose, float4 *out, cudaStream_t s);
 // tile path (dsm_tile.cu)
 int dsm_tile_setup(); // raises the dynamic shared-memory limits of the tile kernels (once per process and device)
 void dsm_launch_assign2(const DsmDev &d, int nb, bool first, cudaStream_t s);

@@ -520,6 +520,47 @@ __global__ void k_labels_export(const __grid_constant__ DsmDev d, int b)
 }
 
 // -------------------------------------------------------------------------------------------
+// raw cloud — publish_raw_pointcloud (surfel_map.cpp:1115-1151): every pixel of one frame back-projected into the world,
+// intensity = gray.  The reference loops column-outer (point k = i*H + j) while the planes are row-major, so a CTA
+// transposes a 32-column x 32-row tile through shared memory: coalesced row reads, points computed in registers and
+// staged as float4 (row pitch 33: conflict-free both ways), then each column's run of up to 32 points is stored as
+// contiguous 16-byte points (512 B per warp and column).  Float operations in the reference's order; with -fmad=false
+// and IEEE division the points are bit-identical to the serial loop (holes included: depth 0 maps to T).
+// -------------------------------------------------------------------------------------------
+#define RAW_TILE 32
+__global__ void __launch_bounds__(256) k_raw_cloud(const __grid_constant__ DsmDev d, int b, const DsmRawPose P, float4 *out)
+{
+    __shared__ float4 tile[RAW_TILE][RAW_TILE + 1]; // [column][row]
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int i0 = blockIdx.x * RAW_TILE, j0 = blockIdx.y * RAW_TILE;
+    const int i = i0 + lane;
+    const float ci = (float)i - d.cx; // (i - cam_cx): int promoted to float
+    const size_t base = (size_t)b * d.px_stride;
+#pragma unroll
+    for (int r = warp; r < RAW_TILE; r += 8)
+    {
+        const int j = j0 + r;
+        if (i >= d.W || j >= d.H) continue;
+        const size_t o = base + (size_t)j * d.Wp + i;
+        const float z = d.depth[o];
+        const float c0 = ci * z / d.fx;
+        const float c1 = ((float)j - d.cy) * z / d.fy;
+        float4 p;
+        p.x = ((P.R[0] * c0 + P.R[1] * c1) + P.R[2] * z) + P.T[0];
+        p.y = ((P.R[3] * c0 + P.R[4] * c1) + P.R[5] * z) + P.T[1];
+        p.z = ((P.R[6] * c0 + P.R[7] * c1) + P.R[8] * z) + P.T[2];
+        p.w = (float)d.gray[o];
+        tile[lane][r] = p;
+    }
+    __syncthreads();
+    const int rows = min(RAW_TILE, d.H - j0);
+    if (lane >= rows) return;
+#pragma unroll
+    for (int c = warp; c < RAW_TILE; c += 8)
+        if (i0 + c < d.W) out[(size_t)(i0 + c) * d.H + j0 + lane] = tile[c][lane];
+}
+
+// -------------------------------------------------------------------------------------------
 // launchers
 // -------------------------------------------------------------------------------------------
 void dsm_launch_repack(const DsmDev &d, int nb, const uint8_t *gray_packed, const float *depth_packed, cudaStream_t s)
@@ -583,6 +624,11 @@ void dsm_launch_pool_export(const DsmDev &d, int frame, int upper, int mode, int
         k_pool_scatter<float4><<<nblk, 256, 0, s>>>(d, frame, blkofs, static_cast<float4 *>(dst), mode, key);
     else
         k_pool_scatter<dsm_surfel_t><<<nblk, 256, 0, s>>>(d, frame, blkofs, static_cast<dsm_surfel_t *>(dst), mode, key);
+}
+void dsm_launch_raw_cloud(const DsmDev &d, int frame, const DsmRawPose &pose, float4 *out, cudaStream_t s)
+{
+    dim3 grid((d.W + RAW_TILE - 1) / RAW_TILE, (d.H + RAW_TILE - 1) / RAW_TILE);
+    k_raw_cloud<<<grid, 256, 0, s>>>(d, frame, pose, out);
 }
 void dsm_launch_pool_transform(const DsmDev &d, int frame, int upper, const float *Wm_dev, cudaStream_t s)
 {

@@ -241,12 +241,27 @@ typedef struct dsm_point_t
  *   dsm_write_ply_mesh         SurfelMap::save_mesh (:1229-1280): one hexagon (6 vertices, 4 triangles) per
  *                              surfel via push_a_surfel (:1175-1226), ASCII PLY.  The caller passes the attached
  *                              surfels of every pose followed by dsm_pool_export_surfels(ctx, 5, ...).  Host only.
- *   dsm_mesh_vertices          push_a_surfel alone: 36 floats (6 x {x, y, z, c, c, c}) per surfel. */
+ *   dsm_mesh_vertices          push_a_surfel alone: 36 floats (6 x {x, y, z, c, c, c}) per surfel.
+ *   dsm_frame_raw_cloud        publish_raw_pointcloud (:1115-1151) on the context's copy of a frame: every pixel
+ *                              back-projected into the world, holes included (depth 0 -> T), W*H points in the
+ *                              reference's column-major loop order (point k = i*H + j for column i, row j), intensity =
+ *                              gray.  pose7 = geometry_msgs::Pose {px, py, pz, qx, qy, qz, qw}: R =
+ *                              Quaternionf((float)qw, (float)qx, (float)qy, (float)qz).toRotationMatrix() (not
+ *                              normalised), T = (float)position; the points are bit-identical to the reference's float
+ *                              loop.  `frame` indexes the frames of the context's most recent call that took images:
+ *                              dsm_fuse_frame / dsm_fuse_frame_resident -> 0, dsm_fuse_stream_resident -> 0..n-1,
+ *                              dsm_batch_upload / dsm_fuse_batch[_async] -> 0..n_frames-1 (an asynchronous batch is
+ *                              waited for).  DSM_E_STATE before any such call, DSM_E_INVALID for a frame outside it.
+ *                              *n_out = W*H, min(cap, W*H) points are written.  Synchronises; touches no pool, label or
+ *                              seed state.  The first call allocates W*H*16 bytes of device memory, kept with the context.
+ *   The neighbourhood cloud of publish_neighbor_pointcloud (:1283-1383) is dsm_pool_export_cloud(ctx, 1, ...) followed by
+ *   dsm_inactive_export_poses(ctx, get_driftfree_poses(reference_index, 2*drift_free_poses), ...) (inactive store below). */
 int dsm_pool_export_cloud(dsm_ctx *ctx, int min_update_times, dsm_point_t *out, int cap, int *n_out);
 int dsm_pool_export_surfels(dsm_ctx *ctx, int min_update_times, dsm_surfel_t *out, int cap, int *n_out);
 int dsm_write_pcd(const char *path, const dsm_point_t *points, size_t n, int binary);
 int dsm_write_ply_mesh(const char *path, const dsm_surfel_t *surfels, size_t n);
 int dsm_mesh_vertices(const dsm_surfel_t *surfels, size_t n, float *vertices36);
+int dsm_frame_raw_cloud(dsm_ctx *ctx, int frame, const double pose7[7], dsm_point_t *out, int cap, int *n_out);
 
 /* ---- inactive store ----
  * What SurfelMap keeps per pose outside the drift-free window -- PoseElement::attached_surfels and the mirror
@@ -260,6 +275,14 @@ int dsm_mesh_vertices(const dsm_surfel_t *surfels, size_t n, float *vertices36);
  *   dsm_inactive_reactivate   insertion (surfel_map.cpp:1583-1587): the pose's segment returns to the end of the pool
  *   dsm_inactive_transform    warp_inactive_surfels_cpu_kernel for one pose (surfel_map.cpp:704-733), asynchronous
  *   dsm_inactive_export_cloud inactive_pointcloud as the node publishes / saves it (store order)
+ *   dsm_inactive_export_poses the inactive half of publish_neighbor_pointcloud (surfel_map.cpp:1306-1321): the stored
+ *                             points of each listed keyframe, concatenated in list order (store order within a keyframe).
+ *                             A keyframe with nothing stored contributes nothing -- the reference's skip of local poses
+ *                             and of empty attached_surfels (:1311-1316) -- so the caller passes the drift-free BFS list
+ *                             of 2*drift_free_poses unchanged.  cap / *n_out as dsm_inactive_export_cloud.
+ *                             Both exports return the points as the store holds them, i.e. after dsm_inactive_transform
+ *                             every point of a pose is warped; the reference's slice of inactive_pointcloud keeps its last
+ *                             point stale (the std::copy(&front, &back) off-by-one of surfel_map.cpp:742, SURVEY.md §8f row 1).
  *   dsm_inactive_download     attached_surfels of one pose (keyframe_index >= 0) or of all poses (< 0; save_mesh)
  *   dsm_inactive_size         surfels / segments currently stored */
 int dsm_inactive_reserve(dsm_ctx *ctx, int max_inactive_surfels);
@@ -267,6 +290,7 @@ int dsm_inactive_retire(dsm_ctx *ctx, int keyframe_index, int *n_moved);
 int dsm_inactive_reactivate(dsm_ctx *ctx, int keyframe_index, int *n_moved);
 int dsm_inactive_transform(dsm_ctx *ctx, int keyframe_index, const float W_colmajor[16]);
 int dsm_inactive_export_cloud(dsm_ctx *ctx, dsm_point_t *out, int cap, int *n_out);
+int dsm_inactive_export_poses(dsm_ctx *ctx, const int32_t *keyframes, int n_keyframes, dsm_point_t *out, int cap, int *n_out);
 int dsm_inactive_download(dsm_ctx *ctx, int keyframe_index, dsm_surfel_t *out, int cap, int *n_out);
 int dsm_inactive_size(dsm_ctx *ctx, int *n_surfels, int *n_segments);
 

@@ -1,10 +1,11 @@
 // dsm_surfel_map.hpp — header-only C++ helper for the SECOND integration step of INTEGRATION.md §4: the
 // `local_surfels` of the reference's SurfelMap kept on the GPU between frames.  Each method has the name and
 // the role of the SurfelMap member whose `local_surfels` part it replaces (surfel_fusion/src/surfel_map.cpp);
-// everything else in those members (pose graph, drift-free BFS, inactive cloud, ROS publishing) stays in
-// SurfelMap unchanged.  Like dsm_fusion_functions.hpp it needs neither OpenCV, Eigen, PCL nor ROS: images are
-// any type with .data / .step (cv::Mat), matrices any type with a column-major .data() (Eigen::Matrix4f),
-// points any 16-byte {x, y, z, intensity} POD or pcl::PointXYZI (converted field by field).
+// everything else in those members (pose graph, drift-free BFS, ROS publishing, and the inactive cloud unless the
+// device-resident store below is used) stays in SurfelMap unchanged.  Like dsm_fusion_functions.hpp it needs neither
+// OpenCV, Eigen, PCL nor ROS: images are any type with .data / .step (cv::Mat), matrices any type with a column-major
+// .data() (Eigen::Matrix4f), poses any type with position.{x,y,z} / orientation.{x,y,z,w} (geometry_msgs::Pose), points
+// any 16-byte {x, y, z, intensity} POD or pcl::PointXYZI (converted field by field).
 //
 //   SurfelMap member (file:line)                          here
 //   ----------------------------------------------------  -----------------------------------------------
@@ -14,7 +15,8 @@
 //   move_add_surfels(), removal loop      (:1479-1497)    retire_surfels(inactive_index, attached_surfels)
 //   move_add_surfels(), insertion         (:1583-1587)    add_surfels(attached_surfels)
 //   publish_active/all_pointcloud, local  (:1398-1454)    active_points(points, 5)
-//   publish_neighbor_pointcloud, local    (:1284-1300)    active_points(points, 1)
+//   publish_neighbor_pointcloud           (:1283-1383)    neighbor_points(points, neighbor_indexs)
+//   publish_raw_pointcloud                (:1115-1151)    raw_points(points, pose)
 //   save_cloud                            (:1153-1173)    save_cloud(name, inactive_points)
 //   save_mesh                             (:1229-1280)    save_mesh(name, attached_surfels_of_all_poses)
 //   local_surfels.size()                                  size()
@@ -33,7 +35,7 @@ namespace dsm
 class ResidentSurfelPool
 {
   public:
-    ResidentSurfelPool() : ctx_(nullptr), err_(0), device_(0), capacity_(1 << 21) {}
+    ResidentSurfelPool() : ctx_(nullptr), err_(0), device_(0), capacity_(1 << 21), width_(0), height_(0) {}
     ~ResidentSurfelPool() { dsm_destroy(ctx_); }
     ResidentSurfelPool(const ResidentSurfelPool &) = delete;
     ResidentSurfelPool &operator=(const ResidentSurfelPool &) = delete;
@@ -55,6 +57,7 @@ class ResidentSurfelPool
         p.fuse_far = fuse_far, p.fuse_near = fuse_near;
         p.max_batch = 2; // two frame slots: the copy of frame t+1 overlaps the kernels of frame t
         p.max_local_surfels = capacity_;
+        width_ = width, height_ = height;
         err_ = dsm_create(&p, device_, nullptr, &ctx_);
         if (err_ == DSM_OK) err_ = dsm_pool_upload(ctx_, nullptr, 0); // local_surfels starts empty
         return report("initialize");
@@ -123,14 +126,7 @@ class ResidentSurfelPool
         int got = 0;
         err_ = dsm_pool_export_cloud(ctx_, min_update_times, scratch_.data(), n, &got);
         if (err_ != DSM_OK) return report("active_points");
-        points.reserve(points.size() + (size_t)got);
-        for (int i = 0; i < got; i++)
-        {
-            Point p;
-            p.x = scratch_[(size_t)i].x, p.y = scratch_[(size_t)i].y, p.z = scratch_[(size_t)i].z;
-            p.intensity = scratch_[(size_t)i].intensity;
-            points.push_back(p);
-        }
+        append(points, got);
         return DSM_OK;
     }
 
@@ -216,14 +212,43 @@ class ResidentSurfelPool
         int got = 0;
         err_ = dsm_inactive_export_cloud(ctx_, scratch_.data(), n, &got);
         if (err_ != DSM_OK) return report("inactive_points");
-        points.reserve(points.size() + (size_t)got);
-        for (int i = 0; i < got; i++)
-        {
-            Point p;
-            p.x = scratch_[(size_t)i].x, p.y = scratch_[(size_t)i].y, p.z = scratch_[(size_t)i].z;
-            p.intensity = scratch_[(size_t)i].intensity;
-            points.push_back(p);
-        }
+        append(points, got);
+        return DSM_OK;
+    }
+
+    // publish_neighbor_pointcloud (surfel_map.cpp:1283-1383): the live local points (update_times != 0) followed by the
+    // stored points of the poses in neighbor_indexs, in list order -- pass get_driftfree_poses(reference_index, ...,
+    // 2*drift_free_poses) unchanged (local poses and poses with nothing stored contribute nothing).  Appended to `points`.
+    template <class Point>
+    int neighbor_points(std::vector<Point> &points, const std::vector<int> &neighbor_indexs)
+    {
+        if (active_points(points, 1) != DSM_OK) return err_;
+        int n = 0;
+        err_ = dsm_inactive_size(ctx_, &n, nullptr);
+        if (err_ != DSM_OK) return report("neighbor_points");
+        scratch_.resize((size_t)(n > 0 ? n : 1));
+        std::vector<int32_t> kf(neighbor_indexs.begin(), neighbor_indexs.end());
+        int got = 0;
+        err_ = dsm_inactive_export_poses(ctx_, kf.data(), (int)kf.size(), scratch_.data(), n, &got);
+        if (err_ != DSM_OK) return report("neighbor_points");
+        append(points, got);
+        return DSM_OK;
+    }
+
+    // publish_raw_pointcloud (surfel_map.cpp:1115-1151) of the frame of the last fuse_map: every pixel in the world frame,
+    // column-major, holes included.  Pose: any type with position.{x,y,z} and orientation.{x,y,z,w}
+    // (geometry_msgs::Pose).  Appended to `points`.
+    template <class Point, class Pose>
+    int raw_points(std::vector<Point> &points, const Pose &pose)
+    {
+        if (!ready("raw_points")) return err_;
+        const double p7[7] = {pose.position.x, pose.position.y, pose.position.z, pose.orientation.x, pose.orientation.y,
+                              pose.orientation.z, pose.orientation.w};
+        scratch_.resize((size_t)width_ * (size_t)height_);
+        int got = 0;
+        err_ = dsm_frame_raw_cloud(ctx_, 0, p7, scratch_.data(), (int)scratch_.size(), &got);
+        if (err_ != DSM_OK) return report("raw_points");
+        append(points, got);
         return DSM_OK;
     }
 
@@ -262,6 +287,19 @@ class ResidentSurfelPool
         std::fprintf(stderr, "dsm::ResidentSurfelPool::%s: initialize() has not succeeded\n", what);
         return false;
     }
+    // the first `got` points of scratch_, converted field by field, appended to `points`
+    template <class Point>
+    void append(std::vector<Point> &points, int got)
+    {
+        points.reserve(points.size() + (size_t)got);
+        for (int i = 0; i < got; i++)
+        {
+            Point p;
+            p.x = scratch_[(size_t)i].x, p.y = scratch_[(size_t)i].y, p.z = scratch_[(size_t)i].z;
+            p.intensity = scratch_[(size_t)i].intensity;
+            points.push_back(p);
+        }
+    }
     int report(const char *what)
     {
         if (err_ != DSM_OK)
@@ -272,6 +310,7 @@ class ResidentSurfelPool
     int err_;
     int device_;
     int capacity_;
+    int width_, height_;
     std::vector<dsm_point_t> scratch_;
 };
 } // namespace dsm
