@@ -29,6 +29,7 @@ EXPORTS = [
     "dsm_pool_export_cloud", "dsm_pool_export_surfels", "dsm_write_pcd", "dsm_write_ply_mesh", "dsm_mesh_vertices", "dsm_fuse_stream_resident",
     "dsm_inactive_reserve", "dsm_inactive_retire", "dsm_inactive_reactivate", "dsm_inactive_transform", "dsm_inactive_export_cloud",
     "dsm_inactive_download", "dsm_inactive_size", "dsm_frame_raw_cloud", "dsm_inactive_export_poses",
+    "dsm_frame_superpixel_image",
     "dsm_comm_unique_id", "dsm_comm_init", "dsm_comm_destroy", "dsm_gather_deltas", "dsm_gather_wait", "dsm_gathered_device",
     "dsm_gathered_rank_bytes", "dsm_gathered_download", "dsm_set_constants", "dsm_set_concurrency",
 ]
@@ -99,6 +100,7 @@ def load_library():
     L.dsm_inactive_transform.argtypes = [vp, ci, vp]
     L.dsm_inactive_export_cloud.argtypes = [vp, vp, ci, ctypes.POINTER(ci)]
     L.dsm_inactive_export_poses.argtypes = [vp, vp, ci, vp, ci, ctypes.POINTER(ci)]
+    L.dsm_frame_superpixel_image.argtypes = [vp, ci, vp, ctypes.c_size_t]
     L.dsm_frame_raw_cloud.argtypes = [vp, ci, vp, vp, ci, ctypes.POINTER(ci)]
     L.dsm_inactive_download.argtypes = [vp, ci, vp, ci, ctypes.POINTER(ci)]
     L.dsm_inactive_size.argtypes = [vp, ctypes.POINTER(ci), ctypes.POINTER(ci)]
@@ -397,6 +399,17 @@ class Context:
         n = ctypes.c_int(0)
         self._ck(self.lib.dsm_frame_raw_cloud(self.h, int(frame), _ptr(p), _ptr(out), cap, ctypes.byref(n)))
         return out[:min(n.value, cap)].copy()
+
+    # ---- superpixel normal image of a frame ----
+    def superpixel_image(self, frame=0, pitch=None):
+        """FusionFunctions::debug_show (fusion_functions.cpp:977-1006) on frame `frame` of the most recent call that took
+        images: [H][W][3] uint8, {|nx|, |ny|, |nz|} * 255 of each pixel's superpixel, black on label boundaries.
+        `pitch` (bytes per row, >= 3*W) only sets the row pitch of the buffer the library writes into."""
+        W, H = self.cam.width, self.cam.height
+        pitch = 3 * W if pitch is None else int(pitch)
+        buf = np.zeros((H, max(pitch, 1)), dtype=np.uint8)
+        self._ck(self.lib.dsm_frame_superpixel_image(self.h, int(frame), _ptr(buf), pitch))
+        return buf[:, :3 * W].reshape(H, W, 3).copy()
 
     # ---- parity readback ----
     def labels(self, frame=0):

@@ -427,7 +427,7 @@ extern "C" int dsm_batch_upload(dsm_ctx *ctx, int n, const int32_t *ref, const u
         ProfScope p(ctx, DSM_K_REPACK);
         dsm_launch_repack(d, n, ctx->gray_packed, ctx->depth_packed, ctx->stream);
     }
-    ctx->img_slot0 = 0, ctx->img_n = n;
+    ctx->img_slot0 = 0, ctx->img_n = n, ctx->img_fit = false;
     if (ctx->n_pool > 0)
     {
         CK(cudaMemcpyAsync(ctx->d.pool, local, (size_t)ctx->n_pool * sizeof(dsm_surfel_t), cudaMemcpyHostToDevice, ctx->stream));
@@ -452,6 +452,8 @@ extern "C" int dsm_batch_restore_pool(dsm_ctx *ctx)
 
 // Launches of the schedule up to and including the plane fit: seed init, 3 x (assign, gather, Newton), plane gather, solve.
 static const int kPlaneFitSteps = 12;
+// the schedule enqueued now runs at least through the plane fit (dsm_debug_stop_after does not cut it short before)
+static bool schedule_fits(const dsm_ctx *ctx) { return ctx->stop_after <= 0 || ctx->stop_after >= kPlaneFitSteps; }
 
 // The per-frame schedule: generate_super_pixels (:960-975) then fuse (:58-71) then initialise (:79), enqueued for the
 // frame slots [d.frame0, d.frame0 + nb) of the view `d` (its pool, poolofs and max_pool_per_frame).
@@ -579,6 +581,7 @@ extern "C" int dsm_batch_run(dsm_ctx *ctx)
         }
     }
     ctx->ran = true;
+    ctx->img_fit = schedule_fits(ctx);
     return DSM_OK;
 }
 
@@ -737,7 +740,7 @@ extern "C" int dsm_fuse_batch_async(dsm_ctx *ctx, int n, const int32_t *ref, con
     ctx->uploaded = true;
     ctx->ran = true;
     ctx->in_flight = true;
-    ctx->img_slot0 = 0, ctx->img_n = n;
+    ctx->img_slot0 = 0, ctx->img_n = n, ctx->img_fit = schedule_fits(ctx);
     ctx->res_active = false; // the pool buffer now holds this batch's slices: a resident pool (if any) is gone
     CK(cudaGetLastError());
     return DSM_OK;
@@ -778,7 +781,7 @@ extern "C" int dsm_fuse_frame(dsm_ctx *ctx, int ref_idx, const uint8_t *gray, si
         CK(cudaMemcpyAsync(ctx->d.pool, local, (size_t)n_local * sizeof(dsm_surfel_t), cudaMemcpyHostToDevice, ctx->stream));
     ctx->nb = 1;
     ctx->uploaded = true;
-    ctx->img_slot0 = 0, ctx->img_n = 1;
+    ctx->img_slot0 = 0, ctx->img_n = 1, ctx->img_fit = false; // dsm_batch_run sets img_fit
     rc = dsm_batch_run(ctx);
     if (rc != DSM_OK) return rc;
     if (n_local > 0)
@@ -999,11 +1002,12 @@ extern "C" int dsm_fuse_frame_resident(dsm_ctx *ctx, int ref_idx, const uint8_t 
     }
     ctx->nb = slot + 1;
     ctx->uploaded = true;
-    ctx->img_slot0 = slot, ctx->img_n = 1;
+    ctx->img_slot0 = slot, ctx->img_n = 1, ctx->img_fit = false;
     // + post-step of SurfelMap::fuse_map on the device: compact into the alternate buffer, then swap
     rc = enqueue_schedule(ctx, dv, 1, ctx->stream, ctx->pool_snap);
     if (rc != DSM_OK) return rc;
     ctx->ran = true;
+    ctx->img_fit = schedule_fits(ctx);
     CK(cudaEventRecord(ctx->ev_done[EV_SLOT + slot], ctx->stream)); // (the compaction's last kernel stored the new pool size in res_ofs[1])
     ctx->single_pending = true;
     swap_pool(ctx);
@@ -1310,8 +1314,10 @@ extern "C" int dsm_fuse_stream_resident(dsm_ctx *ctx, int n, const int32_t *ref_
     ctx->nb = slot0 + n;
     ctx->uploaded = true;
     ctx->img_slot0 = slot0, ctx->img_n = n; // ordered before the main stream through phase 2 (ev_join / ev_p2) below
+    ctx->img_fit = false;
     rc = enqueue_schedule(ctx, v, n, s1, nullptr, 1);
     if (rc != DSM_OK) return rc;
+    ctx->img_fit = schedule_fits(ctx);
     if (dbl)
     {
         CK(cudaEventRecord(ctx->ev_join[par], s1));
@@ -1385,6 +1391,35 @@ extern "C" int dsm_frame_raw_cloud(dsm_ctx *ctx, int frame, const double pose7[7
     *n_out = (int)npx;
     const size_t c = npx < (size_t)cap ? npx : (size_t)cap;
     if (c > 0) CK(cudaMemcpyAsync(out, ctx->raw_out, c * sizeof(dsm_point_t), cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    return DSM_OK;
+}
+
+// ---- superpixel normal image of a frame (FusionFunctions::debug_show, fusion_functions.cpp:977-1006) ----
+extern "C" int dsm_frame_superpixel_image(dsm_ctx *ctx, int frame, uint8_t *bgr, size_t pitch)
+{
+    if (!ctx || !bgr || pitch < (size_t)3 * ctx->p.width) return DSM_E_INVALID;
+    if (ctx->img_n == 0) return DSM_E_STATE;
+    if (frame < 0 || frame >= ctx->img_n) return DSM_E_INVALID;
+    if (!ctx->img_fit) return DSM_E_STATE; // uploaded but not run, or run with the plane fit cut off
+    CK(cudaSetDevice(ctx->device));
+    if (ctx->in_flight)
+    { // the chunks of dsm_fuse_batch_async run on their own streams: finish the batch first
+        int rcw = dsm_batch_wait(ctx);
+        if (rcw != DSM_OK) return rcw;
+    }
+    const int W = ctx->p.width, H = ctx->p.height;
+    const size_t row = (size_t)3 * ctx->d.Wp; // staging row pitch: a multiple of 48 bytes, so every row is word-aligned
+    if (!ctx->spimg_out && ctx->own.device(&ctx->spimg_out, row * H) != cudaSuccess)
+    {
+        cudaGetLastError();
+        ctx->spimg_out = nullptr;
+        return DSM_E_NOMEM;
+    }
+    // every entry point leaves the frame's schedule ordered before later work on the main stream
+    dsm_launch_superpixel_image(ctx->d, ctx->img_slot0 + frame, ctx->spimg_out, ctx->stream);
+    CK(cudaGetLastError());
+    CK(cudaMemcpy2DAsync(bgr, pitch, ctx->spimg_out, row, (size_t)3 * W, H, cudaMemcpyDeviceToHost, ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
     return DSM_OK;
 }

@@ -144,9 +144,13 @@ struct dsm_ctx
     cudaEvent_t ev_fork = nullptr, ev_join[4] = {}; // dsm_batch_run: fork / join of the concurrent sub-batches
     bool single_pending = false; // a dsm_fuse_frame_resident call since the last dsm_fuse_stream_resident (they share frame slots 0 / 1)
     // frame slots [img_slot0, img_slot0 + img_n) hold the images of the most recent call that took images (img_n == 0: none
-    // yet); dsm_frame_raw_cloud reads them, into raw_out (W*H points, allocated at its first call)
+    // yet); dsm_frame_raw_cloud reads them, into raw_out (W*H points, allocated at its first call).  img_fit: that call's
+    // schedule has run through the plane fit, so the slots' label codes and plane normals are complete;
+    // dsm_frame_superpixel_image reads them, into spimg_out ([H][3*Wp] bytes, allocated at its first call)
     int img_slot0 = 0, img_n = 0;
+    bool img_fit = false;
     float4 *raw_out = nullptr;
+    uint8_t *spimg_out = nullptr;
     int run_split = 2;           // sub-batches per dsm_batch_run (dsm_set_concurrency)
     // pinned host staging for the small per-batch tables
     float *h_pose = nullptr; // [2B][32]: pose then inverse; second half: dsm_fuse_stream_resident's own tables

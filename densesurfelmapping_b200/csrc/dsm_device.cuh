@@ -145,6 +145,8 @@ struct DsmRawPose
     float R[9], T[3];
 };
 void dsm_launch_raw_cloud(const DsmDev &d, int frame, const DsmRawPose &pose, float4 *out, cudaStream_t s);
+// debug_show of dsm_frame_superpixel_image: out = [H][3*Wp] bytes (16-byte aligned), pixels >= W written as 0
+void dsm_launch_superpixel_image(const DsmDev &d, int frame, uint8_t *out, cudaStream_t s);
 // tile path (dsm_tile.cu)
 int dsm_tile_setup(); // raises the dynamic shared-memory limits of the tile kernels (once per process and device)
 void dsm_launch_assign2(const DsmDev &d, int nb, bool first, cudaStream_t s);

@@ -561,6 +561,69 @@ __global__ void __launch_bounds__(256) k_raw_cloud(const __grid_constant__ DsmDe
 }
 
 // -------------------------------------------------------------------------------------------
+// superpixel image — FusionFunctions::debug_show (fusion_functions.cpp:977-1006) of one frame: every pixel painted with
+// |normal| * 255 of its superpixel (cv::Vec3b order {|nx|, |ny|, |nz|}), black where the right or the lower neighbour has
+// another label.  A thread covers 4 consecutive pixels of a row: one u32 of codes, the u32 below it and the code right of
+// its last pixel (both L1/L2 hits of neighbouring threads' rows); its 12 output bytes go through a per-warp staging row
+// so that the warp stores 96 consecutive 32-bit words.  Output rows have a pitch of 3*Wp bytes; pixels >= W are 0.
+// -------------------------------------------------------------------------------------------
+// `uchar = fabs(n) * 255` (:986-988) as the reference's x86-64 build computes it: fabs of the float promoted to double,
+// the product exact in double (24-bit mantissa x 255 < 2^32), then a truncating conversion through int32 whose low byte
+// is kept; NaN (and anything >= 2^31) converts to INT_MIN, i.e. byte 0
+__device__ __forceinline__ uint32_t sp_channel(float n)
+{
+    const double v = fabs((double)n) * 255.0;
+    return v < 2147483648.0 ? (uint32_t)(int)v & 0xffu : 0u;
+}
+
+#define SPI_PX 4                    // pixels per thread
+#define SPI_WARPS 4                 // rows per CTA (one warp each)
+#define SPI_SPAN (32 * SPI_PX)      // pixels per warp
+__global__ void __launch_bounds__(32 * SPI_WARPS) k_superpixel_image(const __grid_constant__ DsmDev d, int b, uint32_t *out)
+{
+    __shared__ uint32_t stage[SPI_WARPS][3 * 32]; // a warp's 384 output bytes; lane l writes words 3l..3l+2 (conflict-free)
+    const int lane = threadIdx.x, y = blockIdx.y * SPI_WARPS + threadIdx.y;
+    if (y >= d.H) return; // whole warps: the rows of a CTA are its warps
+    const int x0 = blockIdx.x * SPI_SPAN, x = x0 + lane * SPI_PX;
+    uint32_t px[SPI_PX] = {0u, 0u, 0u, 0u}; // 24-bit {b0, b1, b2} per pixel
+    if (x < d.W)
+    { // x + 3 < Wp (Wp is a multiple of 16): the u32 reads stay inside the pitched row
+        const size_t o = (size_t)b * d.px_stride + (size_t)y * d.Wp + x;
+        const uint32_t c = *reinterpret_cast<const uint32_t *>(d.code + o);
+        const uint32_t cd = y + 1 < d.H ? *reinterpret_cast<const uint32_t *>(d.code + o + d.Wp) : 0u;
+        const int right = x + SPI_PX < d.W ? dsm_code_seed(d.code[o + SPI_PX], x + SPI_PX, y, d.spw) : -1;
+        const float4 *pl = d.plane + (size_t)b * d.S * 3;
+        int s = dsm_code_seed(c & 0xff, x, y, d.spw);
+#pragma unroll
+        for (int i = 0; i < SPI_PX; i++)
+        {
+            const int xi = x + i;
+            if (xi >= d.W) break;
+            // right neighbour: the next pixel of this thread, or the first pixel of the next group
+            const int sr = i + 1 < SPI_PX ? dsm_code_seed((c >> (8 * (i + 1))) & 0xff, xi + 1, y, d.spw) : right;
+            const bool edge = (xi + 1 < d.W && sr != s) || (y + 1 < d.H && dsm_code_seed((cd >> (8 * i)) & 0xff, xi, y + 1, d.spw) != s);
+            if (!edge)
+            {
+                const float4 n = pl[(size_t)s * 3];
+                px[i] = sp_channel(n.x) | sp_channel(n.y) << 8 | sp_channel(n.z) << 16;
+            }
+            s = sr;
+        }
+    }
+    uint32_t *st = stage[threadIdx.y];
+    st[3 * lane + 0] = px[0] | px[1] << 24;
+    st[3 * lane + 1] = px[1] >> 8 | px[2] << 16;
+    st[3 * lane + 2] = px[2] >> 16 | px[3] << 8;
+    __syncwarp();
+    // the row holds 3*Wp/4 words (Wp is a multiple of 16); this warp's run starts at word 3*x0/4
+    const int row_words = 3 * d.Wp / 4, w0 = 3 * x0 / 4;
+    uint32_t *dst = out + (size_t)y * row_words + w0;
+#pragma unroll
+    for (int k = 0; k < 3; k++)
+        if (w0 + 32 * k + lane < row_words) dst[32 * k + lane] = st[32 * k + lane];
+}
+
+// -------------------------------------------------------------------------------------------
 // launchers
 // -------------------------------------------------------------------------------------------
 void dsm_launch_repack(const DsmDev &d, int nb, const uint8_t *gray_packed, const float *depth_packed, cudaStream_t s)
@@ -629,6 +692,11 @@ void dsm_launch_raw_cloud(const DsmDev &d, int frame, const DsmRawPose &pose, fl
 {
     dim3 grid((d.W + RAW_TILE - 1) / RAW_TILE, (d.H + RAW_TILE - 1) / RAW_TILE);
     k_raw_cloud<<<grid, 256, 0, s>>>(d, frame, pose, out);
+}
+void dsm_launch_superpixel_image(const DsmDev &d, int frame, uint8_t *out, cudaStream_t s)
+{
+    dim3 grid((d.W + SPI_SPAN - 1) / SPI_SPAN, (d.H + SPI_WARPS - 1) / SPI_WARPS);
+    k_superpixel_image<<<grid, dim3(32, SPI_WARPS), 0, s>>>(d, frame, reinterpret_cast<uint32_t *>(out));
 }
 void dsm_launch_pool_transform(const DsmDev &d, int frame, int upper, const float *Wm_dev, cudaStream_t s)
 {

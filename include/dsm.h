@@ -263,6 +263,28 @@ int dsm_write_ply_mesh(const char *path, const dsm_surfel_t *surfels, size_t n);
 int dsm_mesh_vertices(const dsm_surfel_t *surfels, size_t n, float *vertices36);
 int dsm_frame_raw_cloud(dsm_ctx *ctx, int frame, const double pose7[7], dsm_point_t *out, int cap, int *n_out);
 
+/* ---- superpixel normal image of a frame: FusionFunctions::debug_show (fusion_functions.cpp:977-1006) ----
+ * The reference's one view of what the superpixel stage did, built on the device from the labels and plane fits the
+ * context already holds (3 B/px cross PCIe instead of the 4 B/px labels plus 60 B per seed of dsm_get_labels /
+ * dsm_get_seeds).  bgr receives H rows of 3*W bytes at a row pitch of `pitch` bytes (a cv::Mat of CV_8UC3):
+ *   pixel (x, y) = {b0, b1, b2} = {|norm_x|, |norm_y|, |norm_z|} * 255 of the seed that labels it (cv::Vec3b order,
+ *   :986-988); {0, 0, 0} when x + 1 < W and the label of (x+1, y) differs, or y + 1 < H and the label of (x, y+1)
+ *   differs (:991-1000).  A seed whose plane fit was rejected has a zero normal, so its superpixel is black.
+ * Each channel is the reference's arithmetic: (double)fabs(n) * 255 (exact in double), converted to uchar the way its
+ * x86-64 build does, through a truncating 32-bit conversion whose low byte is kept.  A NaN normal (DESIGN.md 1.3:
+ * a superpixel whose pixel normals are all zero) gives 0; for |n| <= 1 the byte is floor(|n| * 255).
+ * Exactness: given the context's own labels and seeds (dsm_get_labels / dsm_get_seeds of the same frame slot), the image
+ * equals the reference's debug_show byte for byte.  Against the reference's whole pipeline the black boundary pixels
+ * are exact (labels are bit-identical) and a colour differs by at most 1 per channel, in the rare superpixel whose
+ * |n| * 255 lies within the 1e-4 plane-normal budget of an integer.
+ * `frame` as in dsm_frame_raw_cloud: the frame-th frame of the most recent call that took images (an asynchronous
+ * batch is waited for).  DSM_E_STATE before any such call, or when that call's schedule has not run through the plane
+ * fit (dsm_batch_upload without dsm_batch_run, or a run cut short by dsm_debug_stop_after before the plane fit);
+ * DSM_E_INVALID for a frame outside the call, a null bgr or pitch < 3*W.  Bytes between 3*W and pitch are left
+ * untouched.  Synchronises; touches no pool, label, seed or inactive-store state.  The first call allocates
+ * H * 3*Wp bytes (Wp = W rounded up to 16) of device memory, kept with the context. */
+int dsm_frame_superpixel_image(dsm_ctx *ctx, int frame, uint8_t *bgr, size_t pitch);
+
 /* ---- inactive store ----
  * What SurfelMap keeps per pose outside the drift-free window -- PoseElement::attached_surfels and the mirror
  * inactive_pointcloud (surfel_map.h:36-46) -- resident on the device next to the local pool, so that

@@ -85,6 +85,24 @@ class FusionFunctions
         new_surfels.resize((size_t)n_new);
     }
 
+    // reference: FusionFunctions::debug_show (fusion_functions.cpp:977-1006) of the frame of the last
+    // fuse_initialize_map, written into `image` instead of cv::imshow: height rows of width x 3 bytes at the
+    // image's row pitch.  Mat: any type with .data and .step, allocated by the caller (cv::Mat of CV_8UC3).
+    // Returns the C ABI code (also kept in last_error()).
+    template <class Mat>
+    int superpixel_image(Mat &image)
+    {
+        if (!ctx_)
+        {
+            err_ = DSM_E_STATE;
+            std::fprintf(stderr, "dsm::FusionFunctions::superpixel_image: initialize() has not succeeded\n");
+            return err_;
+        }
+        err_ = dsm_frame_superpixel_image(ctx_, 0, reinterpret_cast<uint8_t *>(image.data), (size_t)image.step);
+        if (err_ != DSM_OK) std::fprintf(stderr, "dsm::FusionFunctions::superpixel_image failed: %s (%s)\n", dsm_strerror(err_), dsm_last_error(ctx_));
+        return err_;
+    }
+
     int last_error() const { return err_; }
     dsm_ctx *context() { return ctx_; }
 

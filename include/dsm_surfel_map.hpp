@@ -17,6 +17,7 @@
 //   publish_active/all_pointcloud, local  (:1398-1454)    active_points(points, 5)
 //   publish_neighbor_pointcloud           (:1283-1383)    neighbor_points(points, neighbor_indexs)
 //   publish_raw_pointcloud                (:1115-1151)    raw_points(points, pose)
+//   FusionFunctions::debug_show (fusion_functions.cpp:977-1006)   superpixel_image(image)
 //   save_cloud                            (:1153-1173)    save_cloud(name, inactive_points)
 //   save_mesh                             (:1229-1280)    save_mesh(name, attached_surfels_of_all_poses)
 //   local_surfels.size()                                  size()
@@ -250,6 +251,17 @@ class ResidentSurfelPool
         if (err_ != DSM_OK) return report("raw_points");
         append(points, got);
         return DSM_OK;
+    }
+
+    // FusionFunctions::debug_show (fusion_functions.cpp:977-1006) of the frame of the last fuse_map: the superpixel normal
+    // image, height rows of width x 3 bytes written at the image's row pitch (bytes past 3*width untouched).  Mat: any
+    // type with .data and .step, allocated by the caller (a cv::Mat(height, width, CV_8UC3)).
+    template <class Mat>
+    int superpixel_image(Mat &image)
+    {
+        if (!ready("superpixel_image")) return err_;
+        err_ = dsm_frame_superpixel_image(ctx_, 0, reinterpret_cast<uint8_t *>(image.data), (size_t)image.step);
+        return report("superpixel_image");
     }
 
     // local_surfels as a host vector (debugging, or a caller that still wants the whole pool)
