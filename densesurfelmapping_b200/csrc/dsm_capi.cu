@@ -196,7 +196,10 @@ extern "C" int dsm_create(const dsm_params *params, int device, void *cuda_strea
     ALLOC(ctx->depth_packed, (size_t)B * H * W + 64);
     ALLOC(ctx->blkcnt, npool / 256 + 64);
     ALLOC(ctx->blkofs, npool / 256 + 64);
-    ALLOC(ctx->newofs, 2);
+    ALLOC(ctx->nsel, 1);
+    ALLOC(ctx->holes, npool);
+    ALLOC(ctx->rc_src, npool);
+    ALLOC(ctx->rc_sync, dsm_recycle_sync_len((int)npool));
     ALLOC(ctx->wmat, 16);
     ALLOC(ctx->res_ofs, 2);
 #undef ALLOC
@@ -492,12 +495,12 @@ static int launch_schedule(dsm_ctx *ctx, const DsmDev &d, int nb, cudaStream_t s
     return DSM_OK;
 }
 
-// Enqueue the schedule for the view `v` (frames [v.frame0, v.frame0 + nf)), followed, when `alt` is given, by the
-// resident-pool post-step: compaction of v.pool into `alt`.
+// Enqueue the schedule for the view `v` (frames [v.frame0, v.frame0 + nf)), followed, when `post` is set, by the
+// resident pool's fuse_map post-step (in place, slot for slot as the reference).
 // The 17-21 launches are captured once per distinct parameter set into a CUDA graph and replayed: the
 // per-launch CPU cost and inter-kernel gaps matter for single frames and small chunks.  Profiling
 // (event pairs around kernels) and the debug kernel budget use plain launches.
-static int enqueue_schedule(dsm_ctx *ctx, const DsmDev &v, int nf, cudaStream_t st, dsm_surfel_t *alt = nullptr, int phase = 3)
+static int enqueue_schedule(dsm_ctx *ctx, const DsmDev &v, int nf, cudaStream_t st, bool post = false, int phase = 3)
 {
     // grids over the pool are sized from max_pool_per_frame rounded up to 4 Ki surfels (the kernels take the true
     // ranges from poolofs on the device, surplus blocks exit at once), so that callers whose pool size
@@ -508,13 +511,15 @@ static int enqueue_schedule(dsm_ctx *ctx, const DsmDev &v, int nf, cudaStream_t 
     {
         int rc = launch_schedule(ctx, d, nf, st, phase);
         if (rc != DSM_OK) return rc;
-        if (alt) dsm_launch_pool_compact(d, d.frame0, d.max_pool_per_frame, ctx->blkcnt, ctx->blkofs, ctx->newofs, alt, ctx->res_ofs, st);
+        if (post)
+            dsm_launch_pool_recycle(d, d.frame0, d.max_pool_per_frame, ctx->blkcnt, ctx->blkofs, ctx->nsel, ctx->holes, ctx->rc_src,
+                                    ctx->rc_sync, ctx->res_ofs, st);
         return DSM_OK;
     };
     if (!ctx->use_graphs || ctx->prof_mask != 0 || ctx->stop_after > 0) return plain();
     for (auto &g : ctx->graphs)
         if (g.f0 == d.frame0 && g.nf == nf && g.maxper == d.max_pool_per_frame && g.pool == d.pool && g.poolofs == d.poolofs &&
-            g.alt == alt && g.phase == phase)
+            g.post == post && g.phase == phase)
         {
             CK(cudaGraphLaunch(g.exec.get(), st));
             return DSM_OK;
@@ -544,7 +549,7 @@ static int enqueue_schedule(dsm_ctx *ctx, const DsmDev &v, int nf, cudaStream_t 
         return plain();
     }
     if (ctx->graphs.size() >= 64) ctx->graphs.erase(ctx->graphs.begin()); // bounded cache
-    ctx->graphs.push_back(GraphEntry{d.frame0, nf, d.max_pool_per_frame, phase, d.pool, d.poolofs, alt, GraphExecPtr(exec)});
+    ctx->graphs.push_back(GraphEntry{d.frame0, nf, d.max_pool_per_frame, phase, d.pool, d.poolofs, post, GraphExecPtr(exec)});
     CK(cudaGraphLaunch(exec, st));
     return DSM_OK;
 }
@@ -816,14 +821,6 @@ static DsmDev resident_view(dsm_ctx *ctx, int slot)
     return d;
 }
 
-// After a frame's compaction into the alternate buffer, that buffer holds the pool.
-static void swap_pool(dsm_ctx *ctx)
-{
-    dsm_surfel_t *t = ctx->d.pool;
-    ctx->d.pool = ctx->pool_snap;
-    ctx->pool_snap = t;
-}
-
 extern "C" int dsm_pool_upload(dsm_ctx *ctx, const dsm_surfel_t *local, int n)
 {
     if (!ctx || n < 0 || (n > 0 && !local)) return DSM_E_INVALID;
@@ -875,15 +872,15 @@ extern "C" int dsm_pool_retire(dsm_ctx *ctx, int kf, dsm_surfel_t *out, int cap,
     if (!ctx->res_active) return DSM_E_STATE;
     CK(cudaSetDevice(ctx->device));
     // count first: nothing is flagged dead unless every retired surfel fits the caller's buffer
-    int32_t h[2] = {0, 0};
-    dsm_launch_pool_retire(resident_view(ctx, 0), 0, ctx->res_upper, kf, ctx->blkcnt, ctx->blkofs, ctx->newofs, nullptr, ctx->stream);
-    CK(cudaMemcpyAsync(h, ctx->newofs, 2 * sizeof(int32_t), cudaMemcpyDeviceToHost, ctx->stream));
+    int32_t h[1] = {0};
+    dsm_launch_pool_retire(resident_view(ctx, 0), 0, ctx->res_upper, kf, ctx->blkcnt, ctx->blkofs, ctx->nsel, nullptr, ctx->stream);
+    CK(cudaMemcpyAsync(h, ctx->nsel, sizeof(int32_t), cudaMemcpyDeviceToHost, ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
     CK(cudaGetLastError());
     *n_out = h[0];
     if (h[0] > cap) return DSM_E_CAPACITY; // pool untouched; call again with cap >= *n_out
-    // the alternate pool buffer is free between frames: use it as the ordered output
-    dsm_launch_pool_retire(resident_view(ctx, 0), 0, ctx->res_upper, kf, ctx->blkcnt, ctx->blkofs, ctx->newofs, ctx->pool_snap, ctx->stream);
+    // the second pool buffer (pool_snap) is the ordered output
+    dsm_launch_pool_retire(resident_view(ctx, 0), 0, ctx->res_upper, kf, ctx->blkcnt, ctx->blkofs, ctx->nsel, ctx->pool_snap, ctx->stream);
     CK(cudaGetLastError());
     const int c = h[0] < cap ? h[0] : cap;
     if (c > 0)
@@ -900,11 +897,11 @@ static int pool_export(dsm_ctx *ctx, int min_ut, bool as_cloud, void *out, int c
     if (!ctx || !n_out || cap < 0 || (cap > 0 && !out)) return DSM_E_INVALID;
     if (!ctx->res_active) return DSM_E_STATE;
     CK(cudaSetDevice(ctx->device));
-    // the alternate pool buffer is free between frames: ordered output (16 or 44 bytes per selected surfel)
-    dsm_launch_pool_export(resident_view(ctx, 0), 0, ctx->res_upper, 2, min_ut, as_cloud, ctx->blkcnt, ctx->blkofs, ctx->newofs,
+    // the second pool buffer (pool_snap) is the ordered output (16 or 44 bytes per selected surfel)
+    dsm_launch_pool_export(resident_view(ctx, 0), 0, ctx->res_upper, 2, min_ut, as_cloud, ctx->blkcnt, ctx->blkofs, ctx->nsel,
                            ctx->pool_snap, ctx->stream);
-    int32_t h[2] = {0, 0};
-    CK(cudaMemcpyAsync(h, ctx->newofs, 2 * sizeof(int32_t), cudaMemcpyDeviceToHost, ctx->stream));
+    int32_t h[1] = {0};
+    CK(cudaMemcpyAsync(h, ctx->nsel, sizeof(int32_t), cudaMemcpyDeviceToHost, ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
     CK(cudaGetLastError());
     *n_out = h[0];
@@ -1003,14 +1000,13 @@ extern "C" int dsm_fuse_frame_resident(dsm_ctx *ctx, int ref_idx, const uint8_t 
     ctx->nb = slot + 1;
     ctx->uploaded = true;
     ctx->img_slot0 = slot, ctx->img_n = 1, ctx->img_fit = false;
-    // + post-step of SurfelMap::fuse_map on the device: compact into the alternate buffer, then swap
-    rc = enqueue_schedule(ctx, dv, 1, ctx->stream, ctx->pool_snap);
+    // + post-step of SurfelMap::fuse_map on the device, in place
+    rc = enqueue_schedule(ctx, dv, 1, ctx->stream, true);
     if (rc != DSM_OK) return rc;
     ctx->ran = true;
     ctx->img_fit = schedule_fits(ctx);
-    CK(cudaEventRecord(ctx->ev_done[EV_SLOT + slot], ctx->stream)); // (the compaction's last kernel stored the new pool size in res_ofs[1])
+    CK(cudaEventRecord(ctx->ev_done[EV_SLOT + slot], ctx->stream)); // (the post-step's last kernel stored the new pool size in res_ofs[1])
     ctx->single_pending = true;
-    swap_pool(ctx);
     ctx->res_upper += ctx->d.S; // every seed can add at most one surfel; dsm_pool_size() tightens it
     CK(cudaGetLastError());
     // the caller may reuse its image buffers as soon as we return: wait for THIS frame's copy only
@@ -1085,9 +1081,9 @@ extern "C" int dsm_inactive_retire(dsm_ctx *ctx, int kf, int *n_moved)
     int rc = dsm_pool_size(ctx, &cur); // exact pool size: bounds the segment
     if (rc != DSM_OK) return rc;
     if (ctx->inact_size + cur > ctx->inact_cap) return DSM_E_CAPACITY;
-    dsm_launch_pool_retire(resident_view(ctx, 0), 0, ctx->res_upper, kf, ctx->blkcnt, ctx->blkofs, ctx->newofs, ctx->inact.get() + ctx->inact_size, ctx->stream);
-    int32_t h[2] = {0, 0};
-    CK(cudaMemcpyAsync(h, ctx->newofs, 2 * sizeof(int32_t), cudaMemcpyDeviceToHost, ctx->stream));
+    dsm_launch_pool_retire(resident_view(ctx, 0), 0, ctx->res_upper, kf, ctx->blkcnt, ctx->blkofs, ctx->nsel, ctx->inact.get() + ctx->inact_size, ctx->stream);
+    int32_t h[1] = {0};
+    CK(cudaMemcpyAsync(h, ctx->nsel, sizeof(int32_t), cudaMemcpyDeviceToHost, ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
     CK(cudaGetLastError());
     if (h[0] > 0)
@@ -1126,7 +1122,7 @@ extern "C" int dsm_inactive_reactivate(dsm_ctx *ctx, int kf, int *n_moved)
         }
         CK(cudaMemcpyAsync(ctx->d.pool + cur, ctx->inact.get() + sg.ofs, (size_t)sg.cnt * sizeof(dsm_surfel_t), cudaMemcpyDeviceToDevice, st));
         cur += sg.cnt;
-        // close the gap: move the tail down through the alternate pool buffer (free between frames), chunk by chunk
+        // close the gap: move the tail down through the second pool buffer, chunk by chunk
         int src = sg.ofs + sg.cnt;
         const int end = ctx->inact_size;
         while (src < end)
@@ -1199,12 +1195,12 @@ static int inactive_export_ranges(dsm_ctx *ctx, const std::vector<dsm_ctx::Inact
     int n = 0;
     for (const auto &r : ranges)
         for (int c0 = 0; c0 < r.cnt && n < cap;)
-        { // chunks sized for the block tables and the alternate pool buffer (16-byte points into 44-byte slots)
+        { // chunks sized for the block tables and the second pool buffer (16-byte points into 44-byte slots)
             int len = r.cnt - c0;
             if (len > npool) len = npool;
             if (len > cap - n) len = cap - n;
             dsm_launch_set2(ctx->inact_ofs, r.ofs + c0, r.ofs + c0 + len, ctx->stream);
-            dsm_launch_pool_export(d, 0, len, 2, INT32_MIN, true, ctx->blkcnt, ctx->blkofs, ctx->newofs, ctx->pool_snap, ctx->stream);
+            dsm_launch_pool_export(d, 0, len, 2, INT32_MIN, true, ctx->blkcnt, ctx->blkofs, ctx->nsel, ctx->pool_snap, ctx->stream);
             CK(cudaMemcpyAsync(out + n, ctx->pool_snap, (size_t)len * sizeof(dsm_point_t), cudaMemcpyDeviceToHost, ctx->stream));
             c0 += len;
             n += len;
@@ -1240,7 +1236,7 @@ extern "C" int dsm_inactive_export_poses(dsm_ctx *ctx, const int32_t *keyframes,
 // A run of n consecutive frames of ONE sequential stream on the resident pool.  Results are identical to n calls of
 // dsm_fuse_frame_resident: superpixels, normals and plane fits do not depend on the pose or the pool, so they run
 // for all n frames as one batch (full-width launches instead of n latency-bound single-frame ones); only the fuse /
-// initialise / compaction steps, which carry the pool from frame t to frame t+1, run frame by frame.
+// initialise / post-step, which carry the pool from frame t to frame t+1, run frame by frame.
 extern "C" int dsm_fuse_stream_resident(dsm_ctx *ctx, int n, const int32_t *ref_idx, const uint8_t *gray, const float *depth,
                                         const float *poses, int32_t *n_new)
 {
@@ -1315,7 +1311,7 @@ extern "C" int dsm_fuse_stream_resident(dsm_ctx *ctx, int n, const int32_t *ref_
     ctx->uploaded = true;
     ctx->img_slot0 = slot0, ctx->img_n = n; // ordered before the main stream through phase 2 (ev_join / ev_p2) below
     ctx->img_fit = false;
-    rc = enqueue_schedule(ctx, v, n, s1, nullptr, 1);
+    rc = enqueue_schedule(ctx, v, n, s1, false, 1);
     if (rc != DSM_OK) return rc;
     ctx->img_fit = schedule_fits(ctx);
     if (dbl)
@@ -1323,12 +1319,11 @@ extern "C" int dsm_fuse_stream_resident(dsm_ctx *ctx, int n, const int32_t *ref_
         CK(cudaEventRecord(ctx->ev_join[par], s1));
         CK(cudaStreamWaitEvent(s2, ctx->ev_join[par], 0));
     }
-    // phase 2: frame by frame on the resident pool, compaction into the alternate buffer, swap
+    // phase 2: frame by frame on the resident pool, each frame ending with the in-place post-step
     for (int t = 0; t < n; t++)
     {
-        rc = enqueue_schedule(ctx, resident_view(ctx, slot0 + t), 1, s2, ctx->pool_snap, 2);
+        rc = enqueue_schedule(ctx, resident_view(ctx, slot0 + t), 1, s2, true, 2);
         if (rc != DSM_OK) return rc;
-        swap_pool(ctx);
         ctx->res_upper += ctx->d.S;
     }
     ctx->ran = true;

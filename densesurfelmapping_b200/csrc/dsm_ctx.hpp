@@ -76,7 +76,8 @@ struct ProfRec
 struct GraphEntry
 {
     int f0, nf, maxper, phase;
-    const void *pool, *poolofs, *alt;
+    const void *pool, *poolofs;
+    bool post; // ends with the resident pool's post-step
     GraphExecPtr exec;
 };
 
@@ -112,7 +113,7 @@ struct dsm_ctx
     // non-const views of what DsmDev holds, and buffers the kernels take as arguments
     uint8_t *gray = nullptr;
     float *depth = nullptr;
-    dsm_surfel_t *pool_snap = nullptr; // alternate pool buffer (batch snapshot / resident compaction target)
+    dsm_surfel_t *pool_snap = nullptr; // second pool-sized buffer: batch snapshot, ordered output of the resident-pool exports
     int32_t *poolofs = nullptr, *refidx = nullptr;
     float *pose = nullptr, *ipose = nullptr;
     dsm_seed_t *seed_export = nullptr;
@@ -128,7 +129,8 @@ struct dsm_ctx
     bool res_active = false;
     int res_frame = 0;   // frames fused in resident mode so far (selects the frame slot)
     int32_t *res_ofs = nullptr; // device [2]: {0, resident pool size}
-    int *blkcnt = nullptr, *blkofs = nullptr, *newofs = nullptr;
+    int *blkcnt = nullptr, *blkofs = nullptr, *nsel = nullptr; // ordered selection: per-block counts / offsets, total
+    int32_t *holes = nullptr, *rc_src = nullptr, *rc_sync = nullptr; // fuse_map post-step (dsm_launch_pool_recycle)
     float *wmat = nullptr; // device copy of the 4x4 of dsm_pool_transform
     // inactive store (EXPERIMENTAL, dsm_inactive_*): the attached_surfels of every pose outside the drift-free window,
     // dense on the device in retirement order; the (keyframe, offset, count) segment list lives on the host

@@ -135,9 +135,13 @@ void dsm_launch_fuse(const DsmDev &d, int nb, cudaStream_t s);
 void dsm_launch_init_surfels(const DsmDev &d, int nb, cudaStream_t s);
 void dsm_launch_seeds_export(const DsmDev &d, int frame, dsm_seed_t *out_dev, int raw_md, cudaStream_t s);
 void dsm_launch_labels_export(const DsmDev &d, int frame, cudaStream_t s);
-void dsm_launch_pool_compact(const DsmDev &d, int frame, int upper, int *blkcnt, int *blkofs, int *newofs, dsm_surfel_t *dst, int32_t *ofs_out, cudaStream_t s);
+// fuse_map post-step, in place: holes [capacity], src [capacity], sync [dsm_recycle_sync_len(capacity)] (zeroed once)
+void dsm_launch_pool_recycle(const DsmDev &d, int frame, int upper, int *blkcnt, int *blkofs, int *nsel, int32_t *holes, int32_t *src,
+                             int32_t *sync, int32_t *ofs_out, cudaStream_t s);
+#define DSM_RECYCLE_SEG 1024 // tail slots per segment of k_pool_recycle (one CTA works on a segment at a time)
+inline size_t dsm_recycle_sync_len(int capacity) { return 2 + (size_t)capacity / DSM_RECYCLE_SEG + 1; } // {ticket, done, segment flags}
 void dsm_launch_pool_transform(const DsmDev &d, int frame, int upper, const float *Wm_dev, cudaStream_t s);
-void dsm_launch_pool_export(const DsmDev &d, int frame, int upper, int mode, int key, bool as_cloud, int *blkcnt, int *blkofs, int *newofs, void *dst, cudaStream_t s);
+void dsm_launch_pool_export(const DsmDev &d, int frame, int upper, int mode, int key, bool as_cloud, int *blkcnt, int *blkofs, int *nsel, void *dst, cudaStream_t s);
 void dsm_launch_set2(int32_t *p, int a, int b, cudaStream_t s);
 // camera -> world of dsm_frame_raw_cloud: R row-major (R[3r + c] = R(r, c)) and T, formed on the host
 struct DsmRawPose
@@ -154,4 +158,4 @@ void dsm_launch_gather(const DsmDev &d, const DsmMaps &m, int nb, cudaStream_t s
 void dsm_launch_newton2(const DsmDev &d, int nb, cudaStream_t s);
 void dsm_launch_plane_gather(const DsmDev &d, const DsmMaps &m, int nb, cudaStream_t s);
 void dsm_launch_gn_solve(const DsmDev &d, int nb, cudaStream_t s);
-void dsm_launch_pool_retire(const DsmDev &d, int frame, int upper, int key, int *blkcnt, int *blkofs, int *newofs, dsm_surfel_t *dst, cudaStream_t s);
+void dsm_launch_pool_retire(const DsmDev &d, int frame, int upper, int key, int *blkcnt, int *blkofs, int *nsel, dsm_surfel_t *dst, cudaStream_t s);

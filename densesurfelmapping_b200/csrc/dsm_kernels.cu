@@ -344,23 +344,22 @@ __global__ void __launch_bounds__(1024) k_init_surfels(const __grid_constant__ D
 // GPU-resident pool (SURVEY.md §8f rows 1-2): what SurfelMap does to `local_surfels` between and
 // after the hot-path calls, kept on the device so a stream never round-trips its pool.
 //
-// k_pool_count / k_pool_scan / k_pool_scatter / k_pool_append — the post-fusion step of
-//   SurfelMap::fuse_map (surfel_map.cpp:1077-1109): drop surfels with update_times == 0, add the
-//   newly initialised ones.  The reference recycles freed slots from the highest index and swaps
-//   the rest with the back, which is inherently sequential; here it is a deterministic ordered
-//   compaction (live surfels keep their order, new ones follow), so the resulting pool equals the
-//   reference's AS A SET (nothing on the path depends on pool order).
+// k_pool_count / k_pool_scan / k_pool_scatter — ordered selection over a pool range (retire, exports, and the hole list of
+//   the post-step below).
+// k_pool_recycle — the post-fusion step of SurfelMap::fuse_map (surfel_map.cpp:1077-1109) in place, slot for slot: new
+//   surfels fill the dead slots from the highest index down, the rest are appended; leftover holes are filled from the
+//   back (see the kernel).
 // k_pool_transform — warp_active_surfels_cpu_kernel (surfel_map.cpp:750-789): p <- W p, n <- R_W n
 //   for every surfel of the pool after a loop closure.  Pure streaming over the 44-byte records,
 //   staged through shared memory like k_fuse.
 // -------------------------------------------------------------------------------------------
-// selection predicate of the pool kernels: mode 0 = live surfels (update_times != 0, fuse_map post-step);
+// selection predicate of the pool kernels: mode 0 = dead slots (update_times == 0, fuse_map post-step, surfel_map.cpp:1081);
 // mode 1 = live surfels last updated by keyframe `key` (move_add_surfels, surfel_map.cpp:1479-1497);
 // mode 2 = surfels with update_times >= key (the publish/save filters, surfel_map.cpp:1158, :1243, :1406, :1429)
 __device__ __forceinline__ bool pool_pred(const dsm_surfel_t &e, int mode, int key)
 {
     if (mode == 2) return e.update_times >= key;
-    return mode == 0 ? (e.update_times != 0) : (e.update_times > 0 && e.last_update == key);
+    return mode == 0 ? (e.update_times == 0) : (e.update_times > 0 && e.last_update == key);
 }
 
 __global__ void __launch_bounds__(256) k_pool_count(const __grid_constant__ DsmDev d, int b, int *blkcnt, int mode, int key)
@@ -373,7 +372,7 @@ __global__ void __launch_bounds__(256) k_pool_count(const __grid_constant__ DsmD
     if (threadIdx.x == 0) blkcnt[blockIdx.x] = (begin + blockIdx.x * 256 < end) ? c : 0;
 }
 
-__global__ void __launch_bounds__(1024) k_pool_scan(const __grid_constant__ DsmDev d, int b, const int *blkcnt, int *blkofs, int *newofs)
+__global__ void __launch_bounds__(1024) k_pool_scan(const __grid_constant__ DsmDev d, int b, const int *blkcnt, int *blkofs, int *nsel)
 {
     pdl_enter();
     __shared__ int s_warp[32];
@@ -404,17 +403,14 @@ __global__ void __launch_bounds__(1024) k_pool_scan(const __grid_constant__ DsmD
         if (threadIdx.x == 0) s_run = run + tot;
         __syncthreads();
     }
-    if (threadIdx.x == 0)
-    {
-        newofs[0] = s_run;                // live surfels kept
-        newofs[1] = s_run + d.nnew[b];    // new pool size
-    }
+    if (threadIdx.x == 0) *nsel = s_run; // selected surfels in the range
 }
 
 // The selected surfels of the CTA's 256 pool entries, in pool order, to dst + blkofs[CTA].  Rec is the output record:
-// the whole 44-byte surfel (compaction, retire, surfel export) or, for the point-cloud builders of SurfelMap
-// (publish_active_pointcloud surfel_map.cpp:1398-1417, publish_all_pointcloud :1419-1454, publish_neighbor_pointcloud
-// :1284-1300, save_cloud :1153-1173), one PointXYZI float4 {px, py, pz, intensity = color} like the serial push_back loops.
+// the whole 44-byte surfel (retire, surfel export), its pool index (the hole list of k_pool_recycle) or, for the
+// point-cloud builders of SurfelMap (publish_active_pointcloud surfel_map.cpp:1398-1417, publish_all_pointcloud :1419-1454,
+// publish_neighbor_pointcloud :1284-1300, save_cloud :1153-1173), one PointXYZI float4 {px, py, pz, intensity = color}
+// like the serial push_back loops.
 template <typename Rec>
 __global__ void __launch_bounds__(256) k_pool_scatter(const __grid_constant__ DsmDev d, int b, const int *blkofs, Rec *dst, int mode, int key)
 {
@@ -436,17 +432,141 @@ __global__ void __launch_bounds__(256) k_pool_scatter(const __grid_constant__ Ds
     const int pos = blkofs[blockIdx.x] + rank;
     if constexpr (std::is_same<Rec, float4>::value)
         dst[pos] = make_float4(e.px, e.py, e.pz, e.color);
+    else if constexpr (std::is_same<Rec, int32_t>::value)
+        dst[pos] = i;
     else
         dst[pos] = e;
 }
 
-__global__ void __launch_bounds__(256) k_pool_append(const __grid_constant__ DsmDev d, int b, const int *newofs, dsm_surfel_t *dst, int32_t *ofs_out)
+// -------------------------------------------------------------------------------------------
+// k_pool_recycle — the post-step of SurfelMap::fuse_map (surfel_map.cpp:1077-1109) on the resident pool [0, N), in place.
+// The reference, with D = d_0 < ... < d_{m-1} the slots with update_times == 0 and K new surfels:
+//   for k < K:  if D is not empty: local[D.back()] = new[k], D.pop_back()   else push_back(new[k])
+//   while D is not empty: local[D.back()] = local.back(), D.pop_back(), local.pop_back()
+// so the new size is N' = N - m + K and
+//   fill:  new[k] -> slot d_{m-1-k} for k < min(K, m); new[k] -> slot N + k - m for k >= m (then there is no tail).
+//   tail:  (K < m) the q = m - K lowest holes d_0..d_{q-1} remain.  Iteration j of the while loop reads the back,
+//          position N-1-j, and writes hole d_{q-1-j}: hole d_t reads position N' + t ("tail offset" t, t < q).  A hole d_t
+//          >= N' lies inside the tail and is popped later; one below N' is a final slot.  What tail offset t holds when
+//          it is read: position N'+t itself if it was occupied after the fill (a live surfel, or new[m-1-i] when it is
+//          the filled hole d_i, i >= q); otherwise N'+t is a leftover hole d_s, which an earlier iteration wrote with
+//          what tail offset s held (s > t: that iteration read position N'+s = p + u(p), u(p) = occupied positions in
+//          (p, N) = (N-1-p) - (q-1-s) >= 0, and s == t only for a hole that is the back when it is read, whose own read
+//          no final slot ever follows).
+// So src(t) = t's own surfel if occupied, else src(s): pointer chains over the tail that only go up, of any length up to
+// q.  They are resolved by pointer doubling in shared memory within segments of RC_SEG tail offsets, and across segments
+// by taking the segments from the top down: a CTA draws a ticket (atomic) for each segment it takes, so every segment
+// above it belongs to a CTA that is already running; it waits for the completion flags of the segments its remaining
+// pointers leave to and reads their resolved sources.  No CTA waits for one that may not have started: no co-residency assumption.
+// Every destination (fill, final slot) lies below N' or at an append slot >= N, every source at or above N' (or in
+// newsurf): nothing is read after another thread of the grid wrote it.  The last CTA to finish stores N' in ofs_out[1]
+// (every CTA has read N from it before) and clears the tickets and flags for the next call.
+// holes: d_0..d_{m-1} ascending, *nhole = m (k_pool_scatter<int32_t> over mode 0); src: [capacity] resolved sources;
+// sync: [2 + capacity / RC_SEG + 1] = {ticket, done, segment flags}, zero between calls.
+// -------------------------------------------------------------------------------------------
+#define RC_SEG DSM_RECYCLE_SEG
+#define RC_LOG 10 // log2(RC_SEG): doubling rounds that collapse any chain inside a segment
+static_assert(RC_SEG == 1 << RC_LOG, "RC_LOG");
+#define RC_MIN_GRID 16 // CTAs beyond the fill's: tail segments are taken by ticket, so any grid resolves any tail
+__global__ void __launch_bounds__(RC_SEG) k_pool_recycle(const __grid_constant__ DsmDev d, int b, const int *nhole, const int32_t *holes,
+                                                         int32_t *src, int32_t *sync, int32_t *ofs_out)
 {
     pdl_enter();
-    const int n = d.nnew[b];
-    const int j = blockIdx.x * 256 + threadIdx.x;
-    if (j < n) dst[newofs[0] + j] = d.newsurf[(size_t)b * d.S + j];
-    if (j == 0 && ofs_out) ofs_out[1] = newofs[1]; // nothing in this grid reads the pool's offset table
+    __shared__ int s_val[RC_SEG];
+    __shared__ int s_ticket;
+    const int N = d.poolofs[b + 1]; // the resident pool starts at 0
+    const int m = *nhole, K = d.nnew[b];
+    const int Np = N - m + K;
+    const dsm_surfel_t *newsurf = d.newsurf + (size_t)b * d.S;
+    for (int k = blockIdx.x * RC_SEG + threadIdx.x; k < K; k += gridDim.x * RC_SEG)
+    { // fill: a hole at or above N' is popped, its new surfel is read from newsurf by the tail
+        if (k < m)
+        {
+            const int h = holes[m - 1 - k];
+            if (h < Np) d.pool[h] = newsurf[k];
+        }
+        else
+            d.pool[N + k - m] = newsurf[k];
+    }
+    const int q = m - K;
+    const int nseg = q > 0 ? (q + RC_SEG - 1) / RC_SEG : 0;
+    while (nseg > 0)
+    {
+        if (threadIdx.x == 0) s_ticket = atomicAdd(&sync[0], 1);
+        __syncthreads();
+        const int ticket = s_ticket;
+        __syncthreads();
+        if (ticket >= nseg) break;
+        const int seg = nseg - 1 - ticket, t0 = seg * RC_SEG, t = t0 + threadIdx.x;
+        const bool mine = t < q;
+        // v >= 0: pointer to tail offset v; v < 0: resolved, source -1 - v (a pool position in [N', N), or N + k for new[k])
+        int v = 0;
+        if (mine)
+        {
+            const int p = Np + t;
+            if (d.pool[p].update_times != 0)
+                v = -1 - p;
+            else
+            { // p is a hole d_i; the holes >= N' are the last entries of D, at most q of them: i is in [K, m)
+                int lo = K, hi = m - 1;
+                while (lo < hi)
+                {
+                    const int mid = (lo + hi) >> 1;
+                    if (holes[mid] < p) lo = mid + 1;
+                    else hi = mid;
+                }
+                if (lo >= q) v = -1 - (N + m - 1 - lo); // filled with new[m-1-i]
+                else v = lo == t ? -1 - p : lo;         // leftover hole: what tail offset i held (i == t: never read)
+            }
+        }
+        s_val[threadIdx.x] = v;
+        if (__syncthreads_or(mine && v >= 0))
+        {
+#pragma unroll 1
+            for (int r = 0; r < RC_LOG; r++)
+            {
+                const int nv = (mine && v >= 0 && v < t0 + RC_SEG) ? s_val[v - t0] : v;
+                __syncthreads();
+                s_val[threadIdx.x] = v = nv;
+                __syncthreads();
+            }
+        }
+        if (mine && v >= 0)
+        { // leaves the segment upwards: that segment's CTA holds an earlier ticket
+            const volatile int32_t *flag = sync + 2 + v / RC_SEG;
+            while (*flag == 0) __nanosleep(32);
+            __threadfence();
+            v = __ldcg(src + v);
+        }
+        if (mine)
+        {
+            src[t] = v;
+            const int h = holes[t];
+            if (h < Np)
+            {
+                const int s = -1 - v;
+                d.pool[h] = s >= N ? newsurf[s - N] : d.pool[s];
+            }
+        }
+        __threadfence();
+        __syncthreads();
+        if (threadIdx.x == 0) atomicExch(&sync[2 + seg], 1);
+    }
+    __shared__ bool s_last;
+    if (threadIdx.x == 0)
+    {
+        __threadfence();
+        s_last = atomicAdd(&sync[1], 1) == (int)gridDim.x - 1;
+    }
+    __syncthreads();
+    if (!s_last) return;
+    for (int i = threadIdx.x; i < nseg; i += RC_SEG) sync[2 + i] = 0;
+    if (threadIdx.x == 0)
+    {
+        sync[0] = 0;
+        sync[1] = 0;
+        ofs_out[1] = Np;
+    }
 }
 
 #define XF_BLOCK 256
@@ -657,31 +777,38 @@ void dsm_launch_labels_export(const DsmDev &d, int frame, cudaStream_t s)
     k_labels_export<<<dim3((d.W + 255) / 256, d.H), 256, 0, s>>>(d, frame);
 }
 
-// ofs_out (may be null): the resident pool's offset table {0, n}; the last kernel of the chain stores the new size there
-void dsm_launch_pool_compact(const DsmDev &d, int frame, int upper, int *blkcnt, int *blkofs, int *newofs, dsm_surfel_t *dst, int32_t *ofs_out, cudaStream_t s)
+// the fuse_map post-step on the resident pool of frame slot `frame` (whose offset table is ofs_out = {0, N}): hole list,
+// then k_pool_recycle, whose last CTA stores the new size in ofs_out[1].  upper >= N bounds the grids.
+void dsm_launch_pool_recycle(const DsmDev &d, int frame, int upper, int *blkcnt, int *blkofs, int *nsel, int32_t *holes, int32_t *src,
+                             int32_t *sync, int32_t *ofs_out, cudaStream_t s)
 {
     const int nblk = (upper + 255) / 256;
     if (nblk > 0) pdl_launch(k_pool_count, dim3(nblk), dim3(256), 0, s, d, frame, blkcnt, 0, 0);
-    pdl_launch(k_pool_scan, dim3(1), dim3(1024), 0, s, d, frame, (const int *)blkcnt, blkofs, newofs);
-    if (nblk > 0) pdl_launch(k_pool_scatter<dsm_surfel_t>, dim3(nblk), dim3(256), 0, s, d, frame, (const int *)blkofs, dst, 0, 0);
-    pdl_launch(k_pool_append, dim3((d.S + 255) / 256), dim3(256), 0, s, d, frame, (const int *)newofs, dst, ofs_out);
+    pdl_launch(k_pool_scan, dim3(1), dim3(1024), 0, s, d, frame, (const int *)blkcnt, blkofs, nsel);
+    if (nblk > 0) pdl_launch(k_pool_scatter<int32_t>, dim3(nblk), dim3(256), 0, s, d, frame, (const int *)blkofs, holes, 0, 0);
+    // Sized by the fill (K <= S), not by `upper`, which can be far above the pool size: in the common frame there is no
+    // tail and every further 1024-thread CTA only waits for a free SM next to the other stream's kernels.  A long tail
+    // (after a large retire) is worked through by these CTAs segment after segment.
+    const int grid = (d.S + RC_SEG - 1) / RC_SEG;
+    pdl_launch(k_pool_recycle, dim3(grid > RC_MIN_GRID ? grid : RC_MIN_GRID), dim3(RC_SEG), 0, s, d, frame, (const int *)nsel,
+               (const int32_t *)holes, src, sync, ofs_out);
 }
 // move_add_surfels, removal half (surfel_map.cpp:1479-1497): the live surfels whose last_update == key are
-// copied in pool order to dst (count in newofs[0]) and flagged dead in the pool
-void dsm_launch_pool_retire(const DsmDev &d, int frame, int upper, int key, int *blkcnt, int *blkofs, int *newofs, dsm_surfel_t *dst, cudaStream_t s)
+// copied in pool order to dst (count in *nsel) and flagged dead in the pool
+void dsm_launch_pool_retire(const DsmDev &d, int frame, int upper, int key, int *blkcnt, int *blkofs, int *nsel, dsm_surfel_t *dst, cudaStream_t s)
 {
     const int nblk = (upper + 255) / 256;
     if (nblk > 0) k_pool_count<<<nblk, 256, 0, s>>>(d, frame, blkcnt, 1, key);
-    k_pool_scan<<<1, 1024, 0, s>>>(d, frame, blkcnt, blkofs, newofs);
+    k_pool_scan<<<1, 1024, 0, s>>>(d, frame, blkcnt, blkofs, nsel);
     if (nblk > 0 && dst) k_pool_scatter<dsm_surfel_t><<<nblk, 256, 0, s>>>(d, frame, blkofs, dst, 1, key); // dst == nullptr: count only
 }
 // publish/save filters (mode/key as pool_pred): as_cloud ? PointXYZI float4 records : whole 44-byte surfels, in pool
-// order to dst (count in newofs[0]); the pool itself is not modified
-void dsm_launch_pool_export(const DsmDev &d, int frame, int upper, int mode, int key, bool as_cloud, int *blkcnt, int *blkofs, int *newofs, void *dst, cudaStream_t s)
+// order to dst (count in *nsel); the pool itself is not modified
+void dsm_launch_pool_export(const DsmDev &d, int frame, int upper, int mode, int key, bool as_cloud, int *blkcnt, int *blkofs, int *nsel, void *dst, cudaStream_t s)
 {
     const int nblk = (upper + 255) / 256;
     if (nblk > 0) k_pool_count<<<nblk, 256, 0, s>>>(d, frame, blkcnt, mode, key);
-    k_pool_scan<<<1, 1024, 0, s>>>(d, frame, blkcnt, blkofs, newofs);
+    k_pool_scan<<<1, 1024, 0, s>>>(d, frame, blkcnt, blkofs, nsel);
     if (nblk == 0) return;
     if (as_cloud)
         k_pool_scatter<float4><<<nblk, 256, 0, s>>>(d, frame, blkofs, static_cast<float4 *>(dst), mode, key);

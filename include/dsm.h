@@ -184,9 +184,11 @@ int dsm_batch_restore_pool(dsm_ctx *ctx);
  * the hot-path call:
  *   dsm_pool_upload            local_surfels := given array
  *   dsm_fuse_frame_resident    fuse_initialize_map on the resident pool, THEN the post-step of
- *                              SurfelMap::fuse_map (surfel_map.cpp:1077-1109): dead surfels dropped,
- *                              new surfels added.  The resulting pool equals the reference's as a
- *                              SET (the reference's slot recycling order is not reproduced).
+ *                              SurfelMap::fuse_map (surfel_map.cpp:1077-1109), in place: new surfels fill the
+ *                              dead slots from the highest index down, the rest are appended, leftover dead slots
+ *                              take the back element.  The pool equals the reference's local_surfels element for
+ *                              element (byte for byte given the same fuse results), and slots are stable: a
+ *                              surfel keeps its index until it dies or is the back element moved into a hole.
  *                              *n_new (optional) = number of new surfels; passing it synchronises.
  *   dsm_pool_transform         warp_active_surfels_cpu_kernel (surfel_map.cpp:750-789):
  *                              p <- W p, n <- R_W n for every pool surfel after a loop closure
@@ -194,7 +196,7 @@ int dsm_batch_restore_pool(dsm_ctx *ctx);
  *   dsm_pool_retire            the removal half of SurfelMap::move_add_surfels (surfel_map.cpp:1479-1497):
  *                              the live surfels whose last_update == keyframe_index are copied out in
  *                              pool order (they become that pose's attached_surfels) and flagged dead
- *                              (update_times = 0; the next fuse post-step drops them).  Counts first: if more than
+ *                              (update_times = 0; the next fuse post-step recycles their slots, as the reference does).  Counts first: if more than
  *                              `cap` surfels match, nothing is flagged, *n_out is the number needed and the call
  *                              returns DSM_E_CAPACITY.  Synchronises.
  *   dsm_pool_append            the insertion half (surfel_map.cpp:1583-1587): surfels of poses that
@@ -206,7 +208,7 @@ int dsm_fuse_frame_resident(dsm_ctx *ctx, int reference_frame_index,
                             const float pose_colmajor[16], int *n_new);
 /* n consecutive frames of the SAME stream in one call (tightly packed [n][H][W] images, [n][16] poses): results are
  * those of n calls of dsm_fuse_frame_resident (same kernels, same order on the pool), but the pose- and pool-independent stages (superpixels, normals, plane fit) of all n frames run as one
- * batch; only fuse / initialise / compaction run frame by frame.  Trades
+ * batch; only fuse / initialise / post-step run frame by frame.  Trades
  * n-1 frames of latency for throughput (offline sequences, or a node that lags behind its camera).  n <= max_batch;
  * with 2n <= max_batch consecutive runs use alternate halves of the frame slots: the copy and the batched stages of one
  * run overlap the frame-by-frame stages of the previous one.  n_new (optional, [n]) = new surfels per frame; passing it

@@ -64,7 +64,7 @@ class ResidentSurfelPool
         return report("initialize");
     }
 
-    // SurfelMap::fuse_map: the hot-path call plus the compaction / append post-step, all on the device.
+    // SurfelMap::fuse_map: the hot-path call plus the post-step (slot recycling as the reference), all on the device.
     // Returns as soon as the images have been copied; the kernels overlap the caller's next steps.
     template <class Mat, class Mat4f>
     int fuse_map(Mat &image, Mat &depth, Mat4f &pose, int reference_index)
