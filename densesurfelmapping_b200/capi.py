@@ -18,6 +18,7 @@ DSM_OK = 0
 ERRORS = {-1: "DSM_E_INVALID", -2: "DSM_E_SHAPE", -3: "DSM_E_NODEVICE", -4: "DSM_E_CUDA",
           -5: "DSM_E_NOMEM", -6: "DSM_E_CAPACITY", -7: "DSM_E_STATE", -8: "DSM_E_NCCL", -9: "DSM_E_IO"}
 NUM_KERNELS = 10
+WINDOW_MAX_KEYS = 128  # DSM_WINDOW_MAX_KEYS: keys per frame and list of dsm_fuse_stream_window
 
 # every symbol include/dsm.h declares (tests/test_abi.py checks the library exports all of them)
 EXPORTS = [
@@ -29,7 +30,7 @@ EXPORTS = [
     "dsm_pool_export_cloud", "dsm_pool_export_surfels", "dsm_write_pcd", "dsm_write_ply_mesh", "dsm_mesh_vertices", "dsm_fuse_stream_resident",
     "dsm_inactive_reserve", "dsm_inactive_retire", "dsm_inactive_reactivate", "dsm_inactive_transform", "dsm_inactive_export_cloud",
     "dsm_inactive_download", "dsm_inactive_size", "dsm_frame_raw_cloud", "dsm_inactive_export_poses",
-    "dsm_frame_superpixel_image",
+    "dsm_frame_superpixel_image", "dsm_fuse_stream_window",
     "dsm_comm_unique_id", "dsm_comm_init", "dsm_comm_destroy", "dsm_gather_deltas", "dsm_gather_wait", "dsm_gathered_device",
     "dsm_gathered_rank_bytes", "dsm_gathered_download", "dsm_set_constants", "dsm_set_concurrency",
 ]
@@ -94,6 +95,7 @@ def load_library():
     L.dsm_fuse_frame_resident.argtypes = [vp, ci, vp, cs, vp, cs, vp, ctypes.POINTER(ci)]
     L.dsm_pool_transform.argtypes = [vp, vp]
     L.dsm_fuse_stream_resident.argtypes = [vp, ci, vp, vp, vp, vp, vp]
+    L.dsm_fuse_stream_window.argtypes = [vp, ci, vp, vp, vp, vp, vp, vp, vp, vp, vp]
     L.dsm_inactive_reserve.argtypes = [vp, ci]
     L.dsm_inactive_retire.argtypes = [vp, ci, ctypes.POINTER(ci)]
     L.dsm_inactive_reactivate.argtypes = [vp, ci, ctypes.POINTER(ci)]
@@ -152,6 +154,15 @@ def kernel_names():
 
 def _ptr(a):
     return None if a is None else a.ctypes.data
+
+
+def window_lists(per_frame):
+    """One list of keyframes per frame -> (keys, offsets[n + 1]) as dsm_fuse_stream_window takes them."""
+    lens = [len(x) for x in per_frame]
+    ofs = np.zeros(len(lens) + 1, dtype=np.int32)
+    ofs[1:] = np.cumsum(lens)
+    keys = np.concatenate([np.asarray(x, dtype=np.int32).reshape(-1) for x in per_frame] + [np.zeros(1, np.int32)])
+    return np.ascontiguousarray(keys, dtype=np.int32), ofs
 
 
 def pose16(pose):
@@ -298,6 +309,29 @@ class Context:
         cnt = np.zeros(len(ref), dtype=np.int32)
         self._ck(self.lib.dsm_fuse_stream_resident(self.h, len(ref), _ptr(ref), _ptr(gray), _ptr(depth), _ptr(poses),
                                                    _ptr(cnt) if want_counts else None))
+        return cnt if want_counts else None
+
+    def fuse_stream_window(self, ref_idx, gray, depth, poses, retire, reactivate, want_counts=False):
+        """fuse_stream_resident with each frame's move_add_surfels in front of its fuse (see include/dsm.h).
+        retire / reactivate: one list of keyframe indices per frame (poses_to_remove / poses_to_add of the node).
+        want_counts: synchronise and return the new surfels per frame (-1: frame not applied); a rejected frame then
+        raises DsmError(DSM_E_CAPACITY) with the counts in .counts."""
+        ref = np.ascontiguousarray(ref_idx, dtype=np.int32)
+        n = len(ref)
+        gray = np.ascontiguousarray(gray, dtype=np.uint8)
+        depth = np.ascontiguousarray(depth, dtype=np.float32)
+        poses = np.ascontiguousarray(poses, dtype=np.float32).reshape(n, 16)
+        assert gray.shape == (n, self.cam.height, self.cam.width) and depth.shape == gray.shape
+        assert len(retire) == n and len(reactivate) == n
+        rk, ro = window_lists(retire)
+        ak, ao = window_lists(reactivate)
+        cnt = np.zeros(n, dtype=np.int32)
+        rc = self.lib.dsm_fuse_stream_window(self.h, n, _ptr(ref), _ptr(gray), _ptr(depth), _ptr(poses), _ptr(rk), _ptr(ro),
+                                             _ptr(ak), _ptr(ao), _ptr(cnt) if want_counts else None)
+        if rc != DSM_OK:
+            err = DsmError(rc, self.lib.dsm_last_error(self.h).decode() or self.lib.dsm_strerror(rc).decode())
+            err.counts = cnt if want_counts else None
+            raise err
         return cnt if want_counts else None
 
     def pool_transform(self, W_colmajor):

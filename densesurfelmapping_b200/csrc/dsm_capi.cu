@@ -8,6 +8,7 @@
 #include <cstring>
 #include <cstdlib>
 #include <cstdint>
+#include <algorithm>
 #include <new>
 #include <vector>
 
@@ -201,11 +202,15 @@ extern "C" int dsm_create(const dsm_params *params, int device, void *cuda_strea
     ALLOC(ctx->rc_src, npool);
     ALLOC(ctx->rc_sync, dsm_recycle_sync_len((int)npool));
     ALLOC(ctx->wmat, 16);
-    ALLOC(ctx->res_ofs, 2);
+    ALLOC(ctx->res_ofs, 4);
+    ALLOC(ctx->win_hdr, 4);
+    ctx->win_len = (size_t)DSM_WIN_KEYS(B) + (size_t)2 * B * DSM_WINDOW_MAX_KEYS;
+    ALLOC(ctx->d_win, 2 * ctx->win_len);
 #undef ALLOC
     if (e == cudaSuccess) e = ctx->own.host(&ctx->h_pose, (size_t)2 * B * 32);
     if (e == cudaSuccess) e = ctx->own.host(&ctx->h_ofs, (size_t)B + 1);
     if (e == cudaSuccess) e = ctx->own.host(&ctx->h_ref, (size_t)2 * B);
+    if (e == cudaSuccess) e = ctx->own.host(&ctx->h_win, 2 * ctx->win_len);
     int least = 0, greatest = 0;
     if (e == cudaSuccess) e = cudaDeviceGetStreamPriorityRange(&least, &greatest);
     if (e == cudaSuccess) e = ctx->own.stream(&ctx->s_hi, greatest);
@@ -519,7 +524,7 @@ static int enqueue_schedule(dsm_ctx *ctx, const DsmDev &v, int nf, cudaStream_t 
     if (!ctx->use_graphs || ctx->prof_mask != 0 || ctx->stop_after > 0) return plain();
     for (auto &g : ctx->graphs)
         if (g.f0 == d.frame0 && g.nf == nf && g.maxper == d.max_pool_per_frame && g.pool == d.pool && g.poolofs == d.poolofs &&
-            g.post == post && g.phase == phase)
+            g.gate == d.gate && g.post == post && g.phase == phase)
         {
             CK(cudaGraphLaunch(g.exec.get(), st));
             return DSM_OK;
@@ -549,7 +554,7 @@ static int enqueue_schedule(dsm_ctx *ctx, const DsmDev &v, int nf, cudaStream_t 
         return plain();
     }
     if (ctx->graphs.size() >= 64) ctx->graphs.erase(ctx->graphs.begin()); // bounded cache
-    ctx->graphs.push_back(GraphEntry{d.frame0, nf, d.max_pool_per_frame, phase, d.pool, d.poolofs, post, GraphExecPtr(exec)});
+    ctx->graphs.push_back(GraphEntry{d.frame0, nf, d.max_pool_per_frame, phase, d.pool, d.poolofs, d.gate, post, GraphExecPtr(exec)});
     CK(cudaGraphLaunch(exec, st));
     return DSM_OK;
 }
@@ -818,7 +823,77 @@ static DsmDev resident_view(dsm_ctx *ctx, int slot)
     d.poolofs = ctx->res_ofs - slot; // kernels read poolofs[b], poolofs[b+1] with b == slot
     const int upq = (ctx->res_upper + 65535) / 65536 * 65536;
     d.max_pool_per_frame = upq < ctx->p.max_local_surfels ? upq : ctx->p.max_local_surfels;
+    // the error word exists for dsm_fuse_stream_window only: a context that has never run it reads no gate
+    d.gate = ctx->win_tag > 0 ? ctx->res_ofs + 2 : nullptr;
     return d;
+}
+
+// The synchronisation point of dsm_fuse_stream_window's device-side state: after a windowed call, the pool size, the
+// store size, the segment table and the error word are known only on the device.  Waits for the stream, refreshes the
+// host bounds and the segment mirror, and reports (and clears) a rejected frame as DSM_E_CAPACITY.  A no-op when no
+// windowed call has run since the last one.
+static int res_sync(dsm_ctx *ctx)
+{
+    if (!ctx->win_pending) return DSM_OK;
+    CK(cudaSetDevice(ctx->device));
+    int32_t h[4] = {0, 0, 0, 0}, hdr[4] = {0, 0, 0, 0};
+    CK(cudaMemcpyAsync(h, ctx->res_ofs, sizeof(h), cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaMemcpyAsync(hdr, ctx->win_hdr, sizeof(hdr), cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    CK(cudaGetLastError());
+    if (ctx->inact)
+    {
+        std::vector<int4> t((size_t)hdr[1]);
+        if (hdr[1] > 0)
+        {
+            CK(cudaMemcpyAsync(t.data(), ctx->inact_seg.get(), t.size() * sizeof(int4), cudaMemcpyDeviceToHost, ctx->stream));
+            CK(cudaStreamSynchronize(ctx->stream));
+        }
+        ctx->inact_segs.clear();
+        for (const int4 &g : t) ctx->inact_segs.push_back(dsm_ctx::InactSeg{g.x, g.y, g.z});
+        ctx->inact_size = ctx->inact_upper = hdr[0];
+    }
+    ctx->res_upper = h[1];
+    ctx->win_pending = false;
+    if (h[2] == 0) return DSM_OK;
+    CK(cudaMemsetAsync(ctx->res_ofs + 2, 0, 2 * sizeof(int32_t), ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    snprintf(ctx->err, sizeof(ctx->err), "dsm_fuse_stream_window: frame %d of a call did not fit the pool or the store; "
+             "the map holds the frames before it", h[3]);
+    return DSM_E_CAPACITY;
+}
+
+// After host-side changes of the store (dsm_inactive_retire / _reactivate): the device table and header follow the
+// mirror, before the first windowed call that reads them.  Synchronises.
+static int inact_push(dsm_ctx *ctx)
+{
+    std::vector<int4> t;
+    for (const auto &g : ctx->inact_segs) t.push_back(make_int4(g.kf, g.ofs, g.cnt, 0));
+    const int32_t hdr[4] = {ctx->inact_size, (int32_t)t.size(), 0, 0};
+    if (!t.empty()) CK(cudaMemcpyAsync(ctx->inact_seg.get(), t.data(), t.size() * sizeof(int4), cudaMemcpyHostToDevice, ctx->stream));
+    CK(cudaMemcpyAsync(ctx->win_hdr, hdr, sizeof(hdr), cudaMemcpyHostToDevice, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    ctx->inact_dev_stale = false;
+    return DSM_OK;
+}
+
+// the device-side view of the store and the window tables; `half` selects the staging half of the window lists
+static DsmWin window_view(dsm_ctx *ctx, int half, int t)
+{
+    DsmWin w{};
+    w.tab = ctx->d_win + (size_t)half * ctx->win_len;
+    w.t = t, w.B = ctx->p.max_batch;
+    w.store = ctx->inact.get();
+    w.seg = reinterpret_cast<int4 *>(ctx->inact_seg.get());
+    w.hdr = ctx->win_hdr;
+    w.res = ctx->res_ofs;
+    w.blk = ctx->win_blk.get();
+    w.sync = ctx->win_sync.get();
+    w.blk_stride = ctx->win_blk_stride;
+    w.pool_cap = ctx->p.max_local_surfels;
+    w.store_cap = ctx->inact_cap;
+    w.S = ctx->d.S;
+    return w;
 }
 
 extern "C" int dsm_pool_upload(dsm_ctx *ctx, const dsm_surfel_t *local, int n)
@@ -827,6 +902,8 @@ extern "C" int dsm_pool_upload(dsm_ctx *ctx, const dsm_surfel_t *local, int n)
     if (n > ctx->p.max_local_surfels) return DSM_E_CAPACITY;
     CK(cudaSetDevice(ctx->device));
     CK(cudaStreamSynchronize(ctx->s_h2d));
+    const int rs = res_sync(ctx); // the new pool replaces whatever a rejected windowed frame left: its error is dropped
+    if (rs != DSM_OK && rs != DSM_E_CAPACITY) return rs;
     CK(cudaStreamSynchronize(ctx->stream));
     if (n > 0) CK(cudaMemcpyAsync(ctx->d.pool, local, (size_t)n * sizeof(dsm_surfel_t), cudaMemcpyHostToDevice, ctx->stream));
     ctx->h_ofs[0] = 0;
@@ -843,6 +920,8 @@ extern "C" int dsm_pool_size(dsm_ctx *ctx, int *n)
 {
     if (!ctx || !n) return DSM_E_INVALID;
     if (!ctx->res_active) return DSM_E_STATE;
+    int rs = res_sync(ctx);
+    if (rs != DSM_OK) return rs;
     CK(cudaSetDevice(ctx->device));
     int32_t h[2] = {0, 0};
     CK(cudaMemcpyAsync(h, ctx->res_ofs, 2 * sizeof(int32_t), cudaMemcpyDeviceToHost, ctx->stream));
@@ -870,6 +949,8 @@ extern "C" int dsm_pool_retire(dsm_ctx *ctx, int kf, dsm_surfel_t *out, int cap,
 {
     if (!ctx || !n_out || cap < 0 || (cap > 0 && !out)) return DSM_E_INVALID;
     if (!ctx->res_active) return DSM_E_STATE;
+    int rs = res_sync(ctx);
+    if (rs != DSM_OK) return rs;
     CK(cudaSetDevice(ctx->device));
     // count first: nothing is flagged dead unless every retired surfel fits the caller's buffer
     int32_t h[1] = {0};
@@ -896,6 +977,8 @@ static int pool_export(dsm_ctx *ctx, int min_ut, bool as_cloud, void *out, int c
 {
     if (!ctx || !n_out || cap < 0 || (cap > 0 && !out)) return DSM_E_INVALID;
     if (!ctx->res_active) return DSM_E_STATE;
+    int rs = res_sync(ctx);
+    if (rs != DSM_OK) return rs;
     CK(cudaSetDevice(ctx->device));
     // the second pool buffer (pool_snap) is the ordered output (16 or 44 bytes per selected surfel)
     dsm_launch_pool_export(resident_view(ctx, 0), 0, ctx->res_upper, 2, min_ut, as_cloud, ctx->blkcnt, ctx->blkofs, ctx->nsel,
@@ -1018,15 +1101,17 @@ extern "C" int dsm_fuse_frame_resident(dsm_ctx *ctx, int ref_idx, const uint8_t 
         CK(cudaMemcpyAsync(&c, ctx->d.nnew + slot, sizeof(int32_t), cudaMemcpyDeviceToHost, ctx->stream));
         CK(cudaStreamSynchronize(ctx->stream));
         *n_new = c;
+        return res_sync(ctx); // a windowed frame rejected before this one: this frame was not applied either
     }
     return DSM_OK;
 }
 
-// ---- inactive store (EXPERIMENTAL; DESIGN.md section 9) ----
+// ---- inactive store (DESIGN.md section 8.2) ----
 // What SurfelMap keeps per pose in attached_surfels / inactive_pointcloud (surfel_map.cpp:1479-1497, :1583-1587,
-// :681-748), resident on the device.  Only host orchestration over the pool kernels: retirement is the ordered
-// compaction of dsm_pool_retire writing straight into the store, the per-pose warp is k_pool_transform over one
-// segment, the inactive cloud is k_pool_scatter<float4> over the store.
+// :681-748), resident on the device.  The calls below orchestrate the pool kernels from the host, on the segment mirror:
+// retirement is the ordered compaction of dsm_pool_retire writing straight into the store, the per-pose warp is
+// k_pool_transform over one segment, the inactive cloud is k_pool_scatter<float4> over the store.  The window step of
+// dsm_fuse_stream_window does the same on the device-side table (dsm_launch_window_step).
 static DsmDev inactive_view(dsm_ctx *ctx)
 {
     DsmDev d = ctx->d;
@@ -1039,10 +1124,15 @@ static DsmDev inactive_view(dsm_ctx *ctx)
 extern "C" int dsm_inactive_reserve(dsm_ctx *ctx, int max_inactive_surfels)
 {
     if (!ctx || max_inactive_surfels < 1) return DSM_E_INVALID;
+    int rs = res_sync(ctx);
+    if (rs != DSM_OK) return rs;
     if (ctx->inact_size > 0) return DSM_E_STATE;
     CK(cudaSetDevice(ctx->device));
     CK(cudaStreamSynchronize(ctx->stream));
     ctx->inact.reset();
+    ctx->inact_seg.reset();
+    ctx->win_blk.reset();
+    ctx->win_sync.reset();
     ctx->inact_cap = 0;
     if (!ctx->inact_ofs && ctx->own.device(&ctx->inact_ofs, 2, true) != cudaSuccess) return DSM_E_NOMEM;
     const size_t bytes = (size_t)max_inactive_surfels * sizeof(dsm_surfel_t);
@@ -1053,19 +1143,44 @@ extern "C" int dsm_inactive_reserve(dsm_ctx *ctx, int max_inactive_surfels)
         ctx->inact.reset(static_cast<dsm_surfel_t *>(p));
         e = cudaMemset(p, 0, bytes);
     }
+    // the device side of the window step: segment table, per-key block counts over the pool, compaction flags (zero)
+    const int npool = ctx->p.max_local_surfels > 0 ? ctx->p.max_local_surfels : 1;
+    const size_t lens[3] = {(size_t)max_inactive_surfels * 4, (size_t)DSM_WINDOW_MAX_KEYS * (npool / 256 + 1),
+                            dsm_win_sync_len(max_inactive_surfels)};
+    DevPtr<int32_t> *bufs[3] = {&ctx->inact_seg, &ctx->win_blk, &ctx->win_sync};
+    for (int i = 0; i < 3 && e == cudaSuccess; i++)
+    {
+        p = nullptr;
+        e = cudaMalloc(&p, lens[i] * sizeof(int32_t));
+        if (e == cudaSuccess)
+        {
+            bufs[i]->reset(static_cast<int32_t *>(p));
+            e = cudaMemset(p, 0, lens[i] * sizeof(int32_t));
+        }
+    }
+    if (e == cudaSuccess) e = cudaMemset(ctx->win_hdr, 0, 4 * sizeof(int32_t));
     if (e != cudaSuccess)
     {
         cudaGetLastError();
+        ctx->inact.reset();
+        ctx->inact_seg.reset();
+        ctx->win_blk.reset();
+        ctx->win_sync.reset();
         return DSM_E_NOMEM;
     }
+    ctx->win_blk_stride = npool / 256 + 1;
     ctx->inact_cap = max_inactive_surfels;
+    ctx->inact_upper = 0;
     ctx->inact_segs.clear();
+    ctx->inact_dev_stale = false; // header zeroed above
     return DSM_OK;
 }
 
 extern "C" int dsm_inactive_size(dsm_ctx *ctx, int *n_surfels, int *n_segments)
 {
     if (!ctx) return DSM_E_INVALID;
+    int rs = res_sync(ctx);
+    if (rs != DSM_OK) return rs;
     if (n_surfels) *n_surfels = ctx->inact_size;
     if (n_segments) *n_segments = (int)ctx->inact_segs.size();
     return DSM_OK;
@@ -1092,6 +1207,8 @@ extern "C" int dsm_inactive_retire(dsm_ctx *ctx, int kf, int *n_moved)
         ctx->inact_size += h[0];
     }
     if (n_moved) *n_moved = h[0];
+    ctx->inact_upper = ctx->inact_size;
+    ctx->inact_dev_stale = true;
     return DSM_OK;
 }
 
@@ -1100,6 +1217,8 @@ extern "C" int dsm_inactive_reactivate(dsm_ctx *ctx, int kf, int *n_moved)
 {
     if (!ctx) return DSM_E_INVALID;
     if (!ctx->res_active || !ctx->inact) return DSM_E_STATE;
+    int rs = res_sync(ctx);
+    if (rs != DSM_OK) return rs;
     CK(cudaSetDevice(ctx->device));
     int total = 0;
     for (const auto &sg : ctx->inact_segs)
@@ -1140,6 +1259,8 @@ extern "C" int dsm_inactive_reactivate(dsm_ctx *ctx, int kf, int *n_moved)
     CK(cudaStreamSynchronize(st));
     CK(cudaGetLastError());
     ctx->res_upper = cur;
+    ctx->inact_upper = ctx->inact_size;
+    ctx->inact_dev_stale = true;
     return DSM_OK;
 }
 
@@ -1150,6 +1271,13 @@ extern "C" int dsm_inactive_transform(dsm_ctx *ctx, int kf, const float Wm[16])
     if (!ctx || !Wm) return DSM_E_INVALID;
     if (!ctx->inact) return DSM_E_STATE;
     CK(cudaSetDevice(ctx->device));
+    if (ctx->win_pending)
+    { // the mirror may be stale: the keyframe's segments are found on the device, in stream order
+        CK(cudaMemcpyAsync(ctx->wmat, Wm, 16 * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
+        dsm_launch_inactive_transform(window_view(ctx, 0, 0), kf, ctx->wmat, ctx->stream);
+        CK(cudaGetLastError());
+        return DSM_OK;
+    }
     bool first = true;
     for (const auto &sg : ctx->inact_segs)
     {
@@ -1168,6 +1296,8 @@ extern "C" int dsm_inactive_download(dsm_ctx *ctx, int kf, dsm_surfel_t *out, in
 {
     if (!ctx || !n_out || cap < 0 || (cap > 0 && !out)) return DSM_E_INVALID;
     if (!ctx->inact) return DSM_E_STATE;
+    int rs = res_sync(ctx);
+    if (rs != DSM_OK) return rs;
     CK(cudaSetDevice(ctx->device));
     int n = 0;
     for (const auto &sg : ctx->inact_segs)
@@ -1216,6 +1346,8 @@ extern "C" int dsm_inactive_export_cloud(dsm_ctx *ctx, dsm_point_t *out, int cap
 {
     if (!ctx || !n_out || cap < 0 || (cap > 0 && !out)) return DSM_E_INVALID;
     if (!ctx->inact) return DSM_E_STATE;
+    int rs = res_sync(ctx);
+    if (rs != DSM_OK) return rs;
     return inactive_export_ranges(ctx, {dsm_ctx::InactSeg{-1, 0, ctx->inact_size}}, out, cap, n_out);
 }
 
@@ -1226,6 +1358,8 @@ extern "C" int dsm_inactive_export_poses(dsm_ctx *ctx, const int32_t *keyframes,
 {
     if (!ctx || !n_out || n_keyframes < 0 || (n_keyframes > 0 && !keyframes) || cap < 0 || (cap > 0 && !out)) return DSM_E_INVALID;
     if (!ctx->inact) return DSM_E_STATE;
+    int rs = res_sync(ctx);
+    if (rs != DSM_OK) return rs;
     std::vector<dsm_ctx::InactSeg> ranges;
     for (int k = 0; k < n_keyframes; k++)
         for (const auto &sg : ctx->inact_segs)
@@ -1237,15 +1371,89 @@ extern "C" int dsm_inactive_export_poses(dsm_ctx *ctx, const int32_t *keyframes,
 // dsm_fuse_frame_resident: superpixels, normals and plane fits do not depend on the pose or the pool, so they run
 // for all n frames as one batch (full-width launches instead of n latency-bound single-frame ones); only the fuse /
 // initialise / post-step, which carry the pool from frame t to frame t+1, run frame by frame.
-extern "C" int dsm_fuse_stream_resident(dsm_ctx *ctx, int n, const int32_t *ref_idx, const uint8_t *gray, const float *depth,
-                                        const float *poses, int32_t *n_new)
+// The per-frame window lists of dsm_fuse_stream_window (a null offset array: empty lists)
+struct WinLists
+{
+    const int32_t *rk, *ro, *ak, *ao;
+};
+static int list_len(const int32_t *o, int t) { return o ? o[t + 1] - o[t] : 0; }
+
+// Host-side validation of the lists (include/dsm.h); *any: some frame has a non-empty list
+static int window_validate(const dsm_ctx *ctx, int n, const WinLists &w, bool *any)
+{
+    *any = false;
+    const int32_t *k[2] = {w.rk, w.ak}, *o[2] = {w.ro, w.ao};
+    for (int l = 0; l < 2; l++)
+    {
+        if (!o[l]) continue;
+        if (o[l][0] < 0) return DSM_E_INVALID;
+        for (int t = 0; t < n; t++)
+            if (o[l][t + 1] < o[l][t] || o[l][t + 1] - o[l][t] > DSM_WINDOW_MAX_KEYS) return DSM_E_INVALID;
+        if (o[l][n] > o[l][0])
+        {
+            if (!k[l]) return DSM_E_INVALID;
+            *any = true;
+        }
+    }
+    std::vector<int32_t> f;
+    for (int t = 0; t < n; t++)
+    { // no keyframe twice in one frame's lists, nor in both
+        f.clear();
+        for (int l = 0; l < 2; l++)
+            for (int i = o[l] ? o[l][t] : 0; o[l] && i < o[l][t + 1]; i++)
+            {
+                if (k[l][i] < 0) return DSM_E_INVALID;
+                f.push_back(k[l][i]);
+            }
+        std::sort(f.begin(), f.end());
+        if (std::adjacent_find(f.begin(), f.end()) != f.end()) return DSM_E_INVALID;
+    }
+    if (*any && !ctx->inact) return DSM_E_STATE;
+    return DSM_OK;
+}
+
+// The lists of n frames into staging half `half` (table layout: DsmWin), copied on `st` like the pose tables: the
+// device reads them when the window step runs, so a captured schedule never depends on their contents
+static int stage_window(dsm_ctx *ctx, int half, int n, const WinLists &w, int tag, cudaStream_t st)
+{
+    const int B = ctx->p.max_batch, KR = DSM_WIN_KEYS(B);
+    int32_t *h = ctx->h_win + (size_t)half * ctx->win_len;
+    for (int t = 0; t <= n; t++)
+    {
+        h[t] = w.ro ? w.ro[t] - w.ro[0] : 0;
+        h[B + 1 + t] = w.ao ? w.ao[t] - w.ao[0] : 0;
+    }
+    const int nr = h[n], na = h[B + 1 + n];
+    if (nr > 0) memcpy(h + KR, w.rk + w.ro[0], (size_t)nr * sizeof(int32_t));
+    if (na > 0) memcpy(h + KR + nr, w.ak + w.ao[0], (size_t)na * sizeof(int32_t));
+    h[2 * B + 2] = tag;
+    h[2 * B + 3] = KR + nr;
+    CK(cudaMemcpyAsync(ctx->d_win + (size_t)half * ctx->win_len, h, (size_t)(KR + nr + na) * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+    return DSM_OK;
+}
+
+// dsm_fuse_stream_resident, and with `win` dsm_fuse_stream_window: each frame's window step runs right before its fuse
+static int stream_run(dsm_ctx *ctx, int n, const int32_t *ref_idx, const uint8_t *gray, const float *depth,
+                      const float *poses, int32_t *n_new, const WinLists *win)
 {
     if (!ctx || !ref_idx || !gray || !depth || !poses) return DSM_E_INVALID;
     if (n < 1 || n > ctx->p.max_batch) return DSM_E_INVALID;
+    bool any = false;
+    if (win)
+    {
+        const int rv = window_validate(ctx, n, *win, &any);
+        if (rv != DSM_OK) return rv;
+    }
     if (!ctx->res_active) return DSM_E_STATE;
     if (ctx->in_flight) return DSM_E_STATE;
     CK(cudaSetDevice(ctx->device));
-    if (ctx->res_upper + n * ctx->d.S > ctx->p.max_local_surfels)
+    if (win && ctx->inact && ctx->inact_dev_stale)
+    {
+        const int rp = inact_push(ctx);
+        if (rp != DSM_OK) return rp;
+    }
+    // (the windowed call checks every frame on the device, with the counts only the device has)
+    if (!win && ctx->res_upper + n * ctx->d.S > ctx->p.max_local_surfels)
     { // the bound may be loose: fetch the exact size before giving up
         int cur = 0;
         int rc = dsm_pool_size(ctx, &cur);
@@ -1298,6 +1506,12 @@ extern "C" int dsm_fuse_stream_resident(dsm_ctx *ctx, int n, const int32_t *ref_
     // before ev_done[e], which has been waited for above
     int rc = stage_tables(ctx, (size_t)ctx->p.max_batch + so, slot0, n, poses, ref_idx, s1);
     if (rc != DSM_OK) return rc;
+    const int tag = win ? (ctx->win_tag = ctx->win_tag % 0x3fffffff + 1) : 0;
+    if (win)
+    {
+        rc = stage_window(ctx, par, n, *win, tag, s1);
+        if (rc != DSM_OK) return rc;
+    }
     CK(cudaStreamWaitEvent(s1, ctx->ev_h2d[e], 0));
     // phase 1: all n frames at once, in the batch view (never touches the pool)
     DsmDev v = ctx->d;
@@ -1320,12 +1534,26 @@ extern "C" int dsm_fuse_stream_resident(dsm_ctx *ctx, int n, const int32_t *ref_
         CK(cudaStreamWaitEvent(s2, ctx->ev_join[par], 0));
     }
     // phase 2: frame by frame on the resident pool, each frame ending with the in-place post-step
+    const int cap = ctx->p.max_local_surfels;
     for (int t = 0; t < n; t++)
     {
+        if (win)
+        { // host bounds without readback: a retire can move at most the pool, a reactivation at most the store
+            const int nr = list_len(win->ro, t), na = list_len(win->ao, t);
+            if (nr > 0) ctx->inact_upper = (int)std::min<long long>((long long)ctx->inact_upper + ctx->res_upper, ctx->inact_cap);
+            if (na > 0) ctx->res_upper = (int)std::min<long long>((long long)ctx->res_upper + ctx->inact_upper, cap);
+            // with empty lists the step is only the capacity check, needed once the bound no longer proves the frame fits
+            if (nr > 0 || na > 0 || ctx->res_upper + ctx->d.S > cap)
+            {
+                const DsmDev dv = resident_view(ctx, slot0 + t);
+                dsm_launch_window_step(dv, window_view(ctx, par, t), dv.max_pool_per_frame, nr, na, s2);
+            }
+        }
         rc = enqueue_schedule(ctx, resident_view(ctx, slot0 + t), 1, s2, true, 2);
         if (rc != DSM_OK) return rc;
         ctx->res_upper += ctx->d.S;
     }
+    if (win) ctx->win_pending = true;
     ctx->ran = true;
     if (dbl)
     {
@@ -1340,10 +1568,31 @@ extern "C" int dsm_fuse_stream_resident(dsm_ctx *ctx, int n, const int32_t *ref_
     CK(cudaEventSynchronize(ctx->ev_h2d[e]));
     if (n_new)
     {
+        int32_t h[4] = {0, 0, 0, 0};
         CK(cudaMemcpyAsync(n_new, ctx->d.nnew + slot0, (size_t)n * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+        if (ctx->win_pending) CK(cudaMemcpyAsync(h, ctx->res_ofs, sizeof(h), cudaMemcpyDeviceToHost, st)); // (only set by a windowed call)
         CK(cudaStreamSynchronize(st));
+        if (h[2] != 0)
+        { // frames from the rejected one on (all of them when an earlier call's frame was rejected) were not applied
+            for (int t = h[2] == tag ? h[3] : 0; t < n; t++) n_new[t] = -1;
+        }
+        return res_sync(ctx);
     }
     return DSM_OK;
+}
+
+extern "C" int dsm_fuse_stream_resident(dsm_ctx *ctx, int n, const int32_t *ref_idx, const uint8_t *gray, const float *depth,
+                                        const float *poses, int32_t *n_new)
+{
+    return stream_run(ctx, n, ref_idx, gray, depth, poses, n_new, nullptr);
+}
+
+extern "C" int dsm_fuse_stream_window(dsm_ctx *ctx, int n, const int32_t *ref_idx, const uint8_t *gray, const float *depth,
+                                      const float *poses, const int32_t *retire_kf, const int32_t *retire_ofs,
+                                      const int32_t *reactivate_kf, const int32_t *reactivate_ofs, int32_t *n_new)
+{
+    const WinLists w{retire_kf, retire_ofs, reactivate_kf, reactivate_ofs};
+    return stream_run(ctx, n, ref_idx, gray, depth, poses, n_new, &w);
 }
 
 // ---- raw cloud of a frame (publish_raw_pointcloud, surfel_map.cpp:1115-1151) ----

@@ -76,7 +76,7 @@ struct ProfRec
 struct GraphEntry
 {
     int f0, nf, maxper, phase;
-    const void *pool, *poolofs;
+    const void *pool, *poolofs, *gate;
     bool post; // ends with the resident pool's post-step
     GraphExecPtr exec;
 };
@@ -128,20 +128,32 @@ struct dsm_ctx
     int res_upper = 0;   // host-side upper bound of the resident pool size (exact after a sync)
     bool res_active = false;
     int res_frame = 0;   // frames fused in resident mode so far (selects the frame slot)
-    int32_t *res_ofs = nullptr; // device [2]: {0, resident pool size}
+    int32_t *res_ofs = nullptr; // device [4]: {0, resident pool size, error tag of dsm_fuse_stream_window, rejected frame}
     int *blkcnt = nullptr, *blkofs = nullptr, *nsel = nullptr; // ordered selection: per-block counts / offsets, total
     int32_t *holes = nullptr, *rc_src = nullptr, *rc_sync = nullptr; // fuse_map post-step (dsm_launch_pool_recycle)
     float *wmat = nullptr; // device copy of the 4x4 of dsm_pool_transform
-    // inactive store (EXPERIMENTAL, dsm_inactive_*): the attached_surfels of every pose outside the drift-free window,
-    // dense on the device in retirement order; the (keyframe, offset, count) segment list lives on the host
+    // inactive store (dsm_inactive_*): the attached_surfels of every pose outside the drift-free window, dense on the
+    // device in retirement order.  The (keyframe, offset, count) segment table and the store size live on the device
+    // (inact_seg, win_hdr); inact_segs / inact_size mirror them, exactly unless win_pending
     DevPtr<dsm_surfel_t> inact; // reallocated by dsm_inactive_reserve
+    DevPtr<int32_t> inact_seg;  // int4 [inact_cap] (keyframe, offset, count, scratch): a stored segment holds >= 1 surfel
     int inact_cap = 0, inact_size = 0;
+    int inact_upper = 0;          // host-side upper bound of the store size (exact after a sync)
     int32_t *inact_ofs = nullptr; // device [2]
     struct InactSeg
     {
         int kf, ofs, cnt;
     };
     std::vector<InactSeg> inact_segs;
+    // dsm_fuse_stream_window: staged window lists (pinned h_win -> d_win, one table of win_len ints per staging half),
+    // device header {store size, segments, per-frame scratch x2}, per-key block counts and the compaction flags
+    int32_t *h_win = nullptr, *d_win = nullptr, *win_hdr = nullptr;
+    size_t win_len = 0;
+    DevPtr<int32_t> win_blk, win_sync;
+    int win_blk_stride = 0;
+    int win_tag = 0;          // tag of the latest windowed call (what a rejected frame writes into the error word)
+    bool win_pending = false; // a windowed call since the last synchronisation: mirrors stale, error word unread
+    bool inact_dev_stale = false; // dsm_inactive_retire / _reactivate changed the mirror: the device table follows it lazily
     cudaEvent_t ev_h2d[EV_COUNT] = {}, ev_done[EV_COUNT] = {}, ev_start = nullptr;
     cudaEvent_t ev_fork = nullptr, ev_join[4] = {}; // dsm_batch_run: fork / join of the concurrent sub-batches
     bool single_pending = false; // a dsm_fuse_frame_resident call since the last dsm_fuse_stream_resident (they share frame slots 0 / 1)

@@ -78,6 +78,9 @@ struct DsmDev
     const float *ipose;
     const int32_t *refidx;
     int max_pool_per_frame; // largest per-frame pool slice in this batch (grid sizing)
+    // resident views only (nullptr in batch views): the sticky error word of dsm_fuse_stream_window.  While it is set,
+    // the fuse / initialise / post-step kernels exit at once, so no frame after a rejected one touches the pool.
+    const int32_t *gate;
     // tile path (dsm_tile.cu)
     uint8_t *code;      // [B][H][Wp] label of every pixel as the index (0..3) of the winning candidate among its 2x2 candidate seeds, or DSM_CODE_NONE
     float *invd;        // [B][H][Wp] (float)(1.0 / (double)depth) for depth > 0.01, else 0 (:404-405), written by the first assign pass
@@ -159,3 +162,26 @@ void dsm_launch_newton2(const DsmDev &d, int nb, cudaStream_t s);
 void dsm_launch_plane_gather(const DsmDev &d, const DsmMaps &m, int nb, cudaStream_t s);
 void dsm_launch_gn_solve(const DsmDev &d, int nb, cudaStream_t s);
 void dsm_launch_pool_retire(const DsmDev &d, int frame, int upper, int key, int *blkcnt, int *blkofs, int *nsel, dsm_surfel_t *dst, cudaStream_t s);
+
+// Window step of dsm_fuse_stream_window (move_add_surfels on the device) and the device side of the inactive store.
+// tab: the call's staged lists, [0, B] retire offsets and [B+1, 2B+1] reactivation offsets (relative to the key
+// arrays), [2B+2] the call's tag, [2B+3] index of the first reactivation key, retire keys from 2B+4.
+#define DSM_WIN_KEYS(B) (2 * (B) + 4)
+#define DSM_WIN_CHUNK 1024 // store surfels per CTA step of the compaction
+struct DsmWin
+{
+    const int32_t *tab;
+    int t, B;             // frame of the call, table stride
+    dsm_surfel_t *store;  // inactive store
+    int4 *seg;            // segment table: (keyframe, offset, count, scratch) in retirement order
+    int32_t *hdr;         // {store size, segments, surfels the frame reactivates, lowest offset they leave}
+    int32_t *res;         // resident offsets {0, pool size, error tag, rejected frame}
+    int32_t *blk;         // [DSM_WINDOW_MAX_KEYS][blk_stride] per-key block counts, then store offsets
+    int32_t *sync;        // compaction: {ticket, unused, per-chunk "read" flags}, zero between steps
+    int blk_stride, pool_cap, store_cap, S;
+};
+inline size_t dsm_win_sync_len(int store_cap) { return 2 + (size_t)store_cap / DSM_WIN_CHUNK + 2; }
+// nr / na: lengths of the frame's retire / reactivation lists (which kernels are needed); `upper` bounds the pool size
+void dsm_launch_window_step(const DsmDev &d, const DsmWin &w, int upper, int nr, int na, cudaStream_t s);
+// warp_inactive_surfels_cpu_kernel for the segments of keyframe kf, located on the device (w.seg / w.hdr)
+void dsm_launch_inactive_transform(const DsmWin &w, int kf, const float *Wm_dev, cudaStream_t s);

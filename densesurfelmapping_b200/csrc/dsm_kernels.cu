@@ -12,6 +12,7 @@
 // ":NNN" refer to the reference's surfel_fusion/src/fusion_functions.cpp.
 #include "dsm_exact.cuh"
 #include <cuda_pipeline.h>
+#include <climits>
 #include <type_traits>
 
 // -------------------------------------------------------------------------------------------
@@ -154,6 +155,10 @@ __device__ __forceinline__ void stage_out(float *g, const float *sm, int cnt, bo
     }
 }
 
+// A resident view whose error word is set (a frame of dsm_fuse_stream_window was rejected): the pool stays as it is.
+// Read after pdl_enter, i.e. after the kernel that may have set it has completed.
+__device__ __forceinline__ bool gated(const DsmDev &d) { return d.gate && *(volatile const int32_t *)d.gate != 0; }
+
 // -------------------------------------------------------------------------------------------
 // K5  surfel_fuse — fuse_surfels_kernel (:190-313).  Pure map over the frame's pool slice.
 // The AoS pool (44 B/element, ABI layout) is staged through shared memory with fully coalesced
@@ -179,6 +184,7 @@ __device__ __forceinline__ float get_weight(float depth)
 __global__ void __launch_bounds__(FUSE_BLOCK) k_fuse(const __grid_constant__ DsmDev d)
 {
     pdl_enter();
+    if (gated(d)) return;
     __shared__ alignas(128) float sm[FUSE_BLOCK * 11];
     __shared__ float s_pose[32];
     __shared__ uint64_t bar;
@@ -300,6 +306,7 @@ __device__ __forceinline__ bool init_emits(const DsmDev &d, size_t so, int s)
 __global__ void __launch_bounds__(1024) k_init_surfels(const __grid_constant__ DsmDev d)
 {
     pdl_enter();
+    if (gated(d)) return;
     __shared__ int s_warp[32];
     __shared__ int s_before[32];
     __shared__ float s_pose[16];
@@ -365,6 +372,7 @@ __device__ __forceinline__ bool pool_pred(const dsm_surfel_t &e, int mode, int k
 __global__ void __launch_bounds__(256) k_pool_count(const __grid_constant__ DsmDev d, int b, int *blkcnt, int mode, int key)
 {
     pdl_enter();
+    if (gated(d)) return;
     const int begin = d.poolofs[b], end = d.poolofs[b + 1];
     const int i = begin + blockIdx.x * 256 + threadIdx.x;
     const bool live = i < end && pool_pred(d.pool[i], mode, key);
@@ -375,6 +383,7 @@ __global__ void __launch_bounds__(256) k_pool_count(const __grid_constant__ DsmD
 __global__ void __launch_bounds__(1024) k_pool_scan(const __grid_constant__ DsmDev d, int b, const int *blkcnt, int *blkofs, int *nsel)
 {
     pdl_enter();
+    if (gated(d)) return;
     __shared__ int s_warp[32];
     __shared__ int s_run;
     const int begin = d.poolofs[b], end = d.poolofs[b + 1];
@@ -415,6 +424,7 @@ template <typename Rec>
 __global__ void __launch_bounds__(256) k_pool_scatter(const __grid_constant__ DsmDev d, int b, const int *blkofs, Rec *dst, int mode, int key)
 {
     pdl_enter();
+    if (gated(d)) return;
     __shared__ int s_warp[8];
     const int begin = d.poolofs[b], end = d.poolofs[b + 1];
     const int i = begin + blockIdx.x * 256 + threadIdx.x;
@@ -472,6 +482,7 @@ __global__ void __launch_bounds__(RC_SEG) k_pool_recycle(const __grid_constant__
                                                          int32_t *src, int32_t *sync, int32_t *ofs_out)
 {
     pdl_enter();
+    if (gated(d)) return; // uniform over the grid: no ticket is drawn, nothing to reset
     __shared__ int s_val[RC_SEG];
     __shared__ int s_ticket;
     const int N = d.poolofs[b + 1]; // the resident pool starts at 0
@@ -602,6 +613,385 @@ __global__ void k_set2(int32_t *p, int a, int b)
     p[1] = b;
 }
 void dsm_launch_set2(int32_t *p, int a, int b, cudaStream_t s) { k_set2<<<1, 1, 0, s>>>(p, a, b); }
+
+// -------------------------------------------------------------------------------------------
+// Window step of dsm_fuse_stream_window: SurfelMap::move_add_surfels (surfel_map.cpp:1473-1594) for one frame, on the
+// resident pool and the inactive store, with every count on the device.  The store is dense in retirement order and
+// described by the segment table (keyframe, offset, count) in the same order; hdr holds its size and length.
+//   k_win_plan     (reactivation) the listed keyframes' segments: their total, the pool slot each one goes to (list
+//                  order, store order within a keyframe) and the offset every other segment will have after the holes
+//                  close, kept in the segments' scratch field (< 0: -1 - pool slot; >= 0: new offset)
+//   k_win_count    (retire) per 256-slot block of the pool, how many live surfels each listed keyframe owns
+//   k_win_commit   capacity check of the whole frame (store after the retire, pool after the reactivation plus one
+//                  frame of new surfels); a frame that does not fit sets the error word and nothing of it is applied.
+//                  Otherwise: the block counts become store offsets (key-major scan), one segment per non-empty key is
+//                  appended
+//   k_win_scatter  (retire) the selected surfels to their store slots, flagged dead in the pool
+//   k_win_copy     (reactivation) the listed segments to their pool slots
+//   k_win_compact  (reactivation) the store's remaining surfels move down over the holes, order kept
+//   k_win_finish   (reactivation) segment table compacted, store and pool sizes updated, compaction flags cleared
+// Every kernel exits at once while the error word is set.  Surfels of a keyframe are selected by last_update: a
+// surfel matches at most one listed keyframe, so one pass over the pool equals the reference's loop over the list.
+// -------------------------------------------------------------------------------------------
+#define WIN_MAX DSM_WINDOW_MAX_KEYS
+__device__ __forceinline__ int win_list(const DsmWin &w, bool react, const int32_t **keys)
+{
+    const int32_t *o = w.tab + (react ? w.B + 1 : 0);
+    const int a = o[w.t];
+    *keys = w.tab + (react ? w.tab[2 * w.B + 3] : DSM_WIN_KEYS(w.B)) + a;
+    return o[w.t + 1] - a;
+}
+__device__ __forceinline__ int win_rank(const int *s_key, int n, int kf)
+{
+    for (int r = 0; r < n; r++)
+        if (s_key[r] == kf) return r;
+    return -1;
+}
+__device__ __forceinline__ bool win_failed(const DsmWin &w) { return *(volatile const int32_t *)(w.res + 2) != 0; }
+// exclusive prefix of v over a CTA of 32 * nwarp threads; total over the CTA in *tot (s_warp: 32 ints, reused)
+__device__ __forceinline__ int cta_excl_scan(int v, int *s_warp, int &tot)
+{
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
+    int wtot;
+    const int ex = warp_excl_scan(v, lane, wtot);
+    __syncthreads();
+    if (lane == 31) s_warp[warp] = wtot;
+    __syncthreads();
+    int before = 0;
+    tot = 0;
+    for (int k = 0; k < nw; k++)
+    {
+        const int c = s_warp[k];
+        before += k < warp ? c : 0;
+        tot += c;
+    }
+    return before + ex;
+}
+
+__global__ void __launch_bounds__(1024) k_win_plan(const DsmWin w)
+{
+    pdl_enter();
+    if (win_failed(w)) return;
+    __shared__ int s_key[WIN_MAX], s_run[WIN_MAX], s_warp[32];
+    __shared__ int s_lo, s_carry, s_sel[1024];
+    const int32_t *keys;
+    const int na = win_list(w, true, &keys);
+    for (int r = threadIdx.x; r < na; r += blockDim.x) s_key[r] = keys[r], s_run[r] = 0;
+    if (threadIdx.x == 0) s_lo = INT_MAX, s_carry = 0;
+    __syncthreads();
+    const int nseg = w.hdr[1], N = w.res[1];
+    for (int j = threadIdx.x; j < nseg; j += blockDim.x)
+    {
+        const int4 s = w.seg[j];
+        const int r = win_rank(s_key, na, s.x);
+        if (r >= 0)
+        {
+            atomicAdd(&s_run[r], s.z);
+            atomicMin(&s_lo, s.y);
+        }
+    }
+    __syncthreads();
+    if (threadIdx.x == 0)
+    { // s_run: first pool slot of each listed keyframe (list order)
+        int run = 0;
+        for (int r = 0; r < na; r++)
+        {
+            const int c = s_run[r];
+            s_run[r] = N + run;
+            run += c;
+        }
+        w.hdr[2] = run;
+        w.hdr[3] = s_lo;
+    }
+    __syncthreads();
+    for (int base = 0; base < nseg; base += blockDim.x)
+    {
+        const int j = base + threadIdx.x;
+        int4 s = make_int4(0, 0, 0, 0);
+        int r = -1;
+        if (j < nseg)
+        {
+            s = w.seg[j];
+            r = win_rank(s_key, na, s.x);
+        }
+        int tot;
+        const int gone = s_carry + cta_excl_scan(r >= 0 ? s.z : 0, s_warp, tot); // reactivated surfels below this segment
+        if (j < nseg && r < 0) w.seg[j].w = s.y - gone;
+        int nsel;
+        const int k = cta_excl_scan(r >= 0 ? 1 : 0, s_warp, nsel);
+        if (r >= 0) s_sel[k] = j;
+        __syncthreads();
+        if (threadIdx.x == 0)
+        { // the chunk's listed segments in store order: pool slots in order within each keyframe
+            for (int q = 0; q < nsel; q++)
+            {
+                const int4 t = w.seg[s_sel[q]];
+                const int rr = win_rank(s_key, na, t.x);
+                w.seg[s_sel[q]].w = -1 - s_run[rr];
+                s_run[rr] += t.z;
+            }
+            s_carry += tot;
+        }
+        __syncthreads();
+    }
+}
+
+__global__ void __launch_bounds__(256) k_win_count(const __grid_constant__ DsmDev d, const DsmWin w)
+{
+    pdl_enter();
+    if (win_failed(w)) return;
+    __shared__ int s_key[WIN_MAX], s_cnt[WIN_MAX];
+    const int32_t *keys;
+    const int nr = win_list(w, false, &keys);
+    const int N = w.res[1];
+    if (blockIdx.x * 256 >= N) return; // the commit scans the blocks below N only
+    for (int r = threadIdx.x; r < nr; r += 256) s_key[r] = keys[r], s_cnt[r] = 0;
+    __syncthreads();
+    const int i = blockIdx.x * 256 + threadIdx.x;
+    if (i < N && d.pool[i].update_times > 0)
+    {
+        const int r = win_rank(s_key, nr, d.pool[i].last_update);
+        if (r >= 0) atomicAdd(&s_cnt[r], 1);
+    }
+    __syncthreads();
+    for (int r = threadIdx.x; r < nr; r += 256) w.blk[(size_t)r * w.blk_stride + blockIdx.x] = s_cnt[r];
+}
+
+__global__ void __launch_bounds__(1024) k_win_commit(const DsmWin w, int nr, int na)
+{
+    pdl_enter();
+    if (win_failed(w)) return;
+    __shared__ int s_start[WIN_MAX + 1], s_warp[32], s_carry;
+    const int32_t *keys;
+    win_list(w, false, &keys);
+    const int N = w.res[1], nblk = (N + 255) / 256, size = w.hdr[0];
+    for (int r = threadIdx.x; r <= nr; r += blockDim.x) s_start[r] = 0;
+    if (threadIdx.x == 0) s_carry = 0;
+    __syncthreads();
+    const int E = nr * nblk; // key-major: the surfels of key 0 in pool order, then key 1, ...
+    for (int base = 0; base < E; base += blockDim.x)
+    {
+        const int e = base + threadIdx.x;
+        const int r = nblk ? e / nblk : 0, b = nblk ? e - r * nblk : 0;
+        int32_t *c = w.blk + (size_t)r * w.blk_stride + b;
+        const int v = e < E ? *c : 0;
+        int tot;
+        const int ex = s_carry + cta_excl_scan(v, s_warp, tot);
+        if (e < E)
+        {
+            *c = size + ex;
+            if (b == 0) s_start[r] = ex;
+        }
+        __syncthreads();
+        if (threadIdx.x == 0) s_carry += tot;
+        __syncthreads();
+    }
+    if (threadIdx.x != 0) return;
+    const int moved = s_carry, react = na > 0 ? w.hdr[2] : 0;
+    s_start[nr] = moved;
+    if ((long long)size + moved > w.store_cap || (long long)N + react + w.S > w.pool_cap)
+    { // the frame does not fit: it and every later one are not applied
+        w.res[3] = w.t;
+        __threadfence();
+        w.res[2] = w.tab[2 * w.B + 2];
+        return;
+    }
+    int nseg = w.hdr[1];
+    for (int r = 0; r < nr; r++)
+    {
+        const int c = s_start[r + 1] - s_start[r];
+        if (c > 0) w.seg[nseg++] = make_int4(keys[r], size + s_start[r], c, size + s_start[r] - react);
+    }
+    w.hdr[0] = size + moved;
+    w.hdr[1] = nseg;
+}
+
+__global__ void __launch_bounds__(256) k_win_scatter(const __grid_constant__ DsmDev d, const DsmWin w)
+{
+    pdl_enter();
+    if (win_failed(w)) return;
+    __shared__ int s_key[WIN_MAX], s_wc[8][WIN_MAX];
+    const int32_t *keys;
+    const int nr = win_list(w, false, &keys);
+    const int N = w.res[1];
+    if (blockIdx.x * 256 >= N) return;
+    for (int r = threadIdx.x; r < nr; r += 256) s_key[r] = keys[r];
+    for (int q = threadIdx.x; q < 8 * nr; q += 256) s_wc[q / nr][q % nr] = 0;
+    __syncthreads();
+    const int i = blockIdx.x * 256 + threadIdx.x, lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    dsm_surfel_t e;
+    int r = -1;
+    if (i < N)
+    {
+        e = d.pool[i];
+        if (e.update_times > 0) r = win_rank(s_key, nr, e.last_update);
+    }
+    // position among the block's surfels of the same key, in pool order: within the warp, then over the warps before
+    const unsigned peers = __match_any_sync(FULL, r);
+    if (r >= 0 && lane == __ffs(peers) - 1) s_wc[warp][r] = __popc(peers);
+    __syncthreads();
+    if (r < 0) return;
+    int pos = w.blk[(size_t)r * w.blk_stride + blockIdx.x] + __popc(peers & ((1u << lane) - 1));
+    for (int q = 0; q < warp; q++) pos += s_wc[q][r];
+    w.store[pos] = e;
+    d.pool[i].update_times = 0; // "delete the surfel from the local point" (surfel_map.cpp:1496)
+}
+
+__global__ void __launch_bounds__(256) k_win_copy(const __grid_constant__ DsmDev d, const DsmWin w)
+{
+    pdl_enter();
+    if (win_failed(w) || w.hdr[2] == 0) return;
+    __shared__ int4 s_list[256];
+    __shared__ int s_n;
+    const int nseg = w.hdr[1];
+    for (int base = 0; base < nseg; base += 256)
+    {
+        __syncthreads();
+        if (threadIdx.x == 0) s_n = 0;
+        __syncthreads();
+        const int j = base + threadIdx.x;
+        if (j < nseg)
+        {
+            const int4 s = w.seg[j];
+            if (s.w < 0) s_list[atomicAdd(&s_n, 1)] = s;
+        }
+        __syncthreads();
+        for (int q = 0; q < s_n; q++)
+        {
+            const int4 s = s_list[q];
+            dsm_surfel_t *dst = d.pool + (-1 - s.w);
+            for (int k = blockIdx.x * 256 + threadIdx.x; k < s.z; k += gridDim.x * 256) dst[k] = w.store[s.y + k];
+        }
+    }
+}
+
+// In place, downwards, order kept.  The range [lo, size) is cut into chunks of DSM_WIN_CHUNK surfels that CTAs take by
+// ticket in ascending order.  A CTA reads its chunk into shared memory, raises the chunk's flag, then waits for the
+// flags of the chunks its destinations fall into (all of them below or at its own: every destination is below its
+// source) before it writes.  It only ever waits for chunks with earlier tickets, whose CTAs are running and raise
+// their flags without waiting for anything: no co-residency is assumed and no store-sized scratch is used.
+__global__ void __launch_bounds__(DSM_WIN_CHUNK) k_win_compact(const DsmWin w)
+{
+    pdl_enter();
+    if (win_failed(w) || w.hdr[2] == 0) return;
+    __shared__ dsm_surfel_t s_e[DSM_WIN_CHUNK];
+    __shared__ int s_ticket, s_dmin;
+    const int size = w.hdr[0], lo = w.hdr[3], nseg = w.hdr[1];
+    const int nchunk = (size - lo + DSM_WIN_CHUNK - 1) / DSM_WIN_CHUNK;
+    for (;;)
+    {
+        __syncthreads();
+        if (threadIdx.x == 0)
+        {
+            s_ticket = atomicAdd(&w.sync[0], 1);
+            s_dmin = INT_MAX;
+        }
+        __syncthreads();
+        const int k = s_ticket;
+        if (k >= nchunk) break;
+        const int p = lo + k * DSM_WIN_CHUNK + threadIdx.x;
+        int dst = -1;
+        if (p < size)
+        { // the segment holding p: the last one starting at or below it
+            int a = 0, b = nseg - 1;
+            while (a < b)
+            {
+                const int m = (a + b + 1) >> 1;
+                if (w.seg[m].y <= p) a = m;
+                else b = m - 1;
+            }
+            const int4 s = w.seg[a];
+            if (s.w >= 0)
+            {
+                dst = s.w + (p - s.y);
+                s_e[threadIdx.x] = w.store[p];
+                atomicMin(&s_dmin, dst);
+            }
+        }
+        __syncthreads();
+        if (threadIdx.x == 0)
+        {
+            __threadfence();
+            atomicExch(&w.sync[2 + k], 1);
+            if (s_dmin != INT_MAX)
+                for (int j = (s_dmin - lo) / DSM_WIN_CHUNK; j < k; j++)
+                {
+                    const volatile int32_t *flag = w.sync + 2 + j;
+                    while (*flag == 0) __nanosleep(32);
+                }
+            __threadfence();
+        }
+        __syncthreads();
+        if (dst >= 0) w.store[dst] = s_e[threadIdx.x];
+    }
+}
+
+__global__ void __launch_bounds__(1024) k_win_finish(const DsmWin w)
+{
+    pdl_enter();
+    if (win_failed(w)) return;
+    __shared__ int s_warp[32], s_carry;
+    const int react = w.hdr[2], size = w.hdr[0], lo = w.hdr[3], nseg = w.hdr[1];
+    if (react == 0) return; // nothing was stored for the listed keyframes: no compaction ran
+    const int nchunk = (size - lo + DSM_WIN_CHUNK - 1) / DSM_WIN_CHUNK;
+    for (int i = threadIdx.x; i < nchunk; i += blockDim.x) w.sync[2 + i] = 0;
+    if (threadIdx.x == 0) w.sync[0] = 0, s_carry = 0;
+    __syncthreads();
+    for (int base = 0; base < nseg; base += blockDim.x)
+    { // entries only move down, and a chunk is read before any of it is written
+        const int j = base + threadIdx.x;
+        int4 s = make_int4(0, 0, 0, -1);
+        if (j < nseg) s = w.seg[j];
+        int tot;
+        const int k = s_carry + cta_excl_scan(s.w >= 0 ? 1 : 0, s_warp, tot);
+        __syncthreads();
+        if (j < nseg && s.w >= 0) w.seg[k] = make_int4(s.x, s.w, s.z, 0);
+        __syncthreads();
+        if (threadIdx.x == 0) s_carry += tot;
+        __syncthreads();
+    }
+    __syncthreads();
+    if (threadIdx.x == 0)
+    {
+        w.hdr[0] = size - react;
+        w.hdr[1] = s_carry;
+        w.res[1] += react;
+    }
+}
+
+// warp_inactive_surfels_cpu_kernel (surfel_map.cpp:704-733) on the segments of keyframe kf, found in the device table:
+// the same arithmetic as k_pool_transform, one surfel per thread
+__global__ void __launch_bounds__(256) k_inactive_transform(const DsmWin w, int kf, const float *Wm)
+{
+    __shared__ float s_w[16];
+    __shared__ int2 s_list[256];
+    __shared__ int s_n;
+    if (threadIdx.x < 16) s_w[threadIdx.x] = Wm[threadIdx.x];
+    const int nseg = w.hdr[1];
+    for (int base = 0; base < nseg; base += 256)
+    {
+        __syncthreads();
+        if (threadIdx.x == 0) s_n = 0;
+        __syncthreads();
+        const int j = base + threadIdx.x;
+        if (j < nseg)
+        {
+            const int4 s = w.seg[j];
+            if (s.x == kf) s_list[atomicAdd(&s_n, 1)] = make_int2(s.y, s.z);
+        }
+        __syncthreads();
+        for (int q = 0; q < s_n; q++)
+            for (int k = blockIdx.x * 256 + threadIdx.x; k < s_list[q].y; k += gridDim.x * 256)
+            {
+                float *e = reinterpret_cast<float *>(w.store + s_list[q].x + k);
+                float pw[4], nw[3];
+                mat4_mul(s_w, e[0], e[1], e[2], 1.0f, pw);
+                mat3_mul(s_w, e[3], e[4], e[5], nw);
+                e[0] = pw[0], e[1] = pw[1], e[2] = pw[2];
+                e[3] = nw[0], e[4] = nw[1], e[5] = nw[2];
+            }
+    }
+}
 
 // -------------------------------------------------------------------------------------------
 // parity readback: rebuild the reference's 60-byte Superpixel_seed records for one frame
@@ -829,4 +1219,24 @@ void dsm_launch_pool_transform(const DsmDev &d, int frame, int upper, const floa
 {
     if (upper <= 0) return;
     k_pool_transform<<<(upper + XF_BLOCK - 1) / XF_BLOCK, XF_BLOCK, 0, s>>>(d, frame, Wm_dev);
+}
+
+// one frame's window step (see k_win_plan): `upper` >= pool size sizes the two pool passes; the compaction and the copy
+// run on a fixed grid and take their sizes from the device
+#define WIN_GRID 264
+void dsm_launch_window_step(const DsmDev &d, const DsmWin &w, int upper, int nr, int na, cudaStream_t s)
+{
+    const int nblk = (upper + 255) / 256;
+    if (na > 0) pdl_launch(k_win_plan, dim3(1), dim3(1024), 0, s, w);
+    if (nr > 0 && nblk > 0) pdl_launch(k_win_count, dim3(nblk), dim3(256), 0, s, d, w);
+    pdl_launch(k_win_commit, dim3(1), dim3(1024), 0, s, w, nr, na);
+    if (nr > 0 && nblk > 0) pdl_launch(k_win_scatter, dim3(nblk), dim3(256), 0, s, d, w);
+    if (na == 0) return;
+    pdl_launch(k_win_copy, dim3(WIN_GRID), dim3(256), 0, s, d, w);
+    pdl_launch(k_win_compact, dim3(WIN_GRID), dim3(DSM_WIN_CHUNK), 0, s, w);
+    pdl_launch(k_win_finish, dim3(1), dim3(1024), 0, s, w);
+}
+void dsm_launch_inactive_transform(const DsmWin &w, int kf, const float *Wm_dev, cudaStream_t s)
+{
+    k_inactive_transform<<<WIN_GRID, 256, 0, s>>>(w, kf, Wm_dev);
 }

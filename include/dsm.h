@@ -290,8 +290,9 @@ int dsm_frame_superpixel_image(dsm_ctx *ctx, int frame, uint8_t *bgr, size_t pit
 /* ---- inactive store ----
  * What SurfelMap keeps per pose outside the drift-free window -- PoseElement::attached_surfels and the mirror
  * inactive_pointcloud (surfel_map.h:36-46) -- resident on the device next to the local pool, so that
- * move_add_surfels and the loop-closure warp of the inactive surfels never cross PCIe.  Host orchestration over the
- * pool kernels; segments are kept dense in retirement order.
+ * move_add_surfels and the loop-closure warp of the inactive surfels never cross PCIe.  Segments are kept dense in
+ * retirement order; the segment table lives on the device (dsm_fuse_stream_window updates it there), and the calls below
+ * that synchronise refresh a host mirror of it.
  *   dsm_inactive_reserve      capacity in surfels (once, while the store is empty)
  *   dsm_inactive_retire       move_add_surfels removal loop (surfel_map.cpp:1479-1497): local surfels with
  *                             update_times > 0 and last_update == keyframe_index become that pose's segment (pool
@@ -317,6 +318,42 @@ int dsm_inactive_export_cloud(dsm_ctx *ctx, dsm_point_t *out, int cap, int *n_ou
 int dsm_inactive_export_poses(dsm_ctx *ctx, const int32_t *keyframes, int n_keyframes, dsm_point_t *out, int cap, int *n_out);
 int dsm_inactive_download(dsm_ctx *ctx, int keyframe_index, dsm_surfel_t *out, int cap, int *n_out);
 int dsm_inactive_size(dsm_ctx *ctx, int *n_surfels, int *n_segments);
+
+/* ---- the node's whole per-frame sequence on the device: move_add_surfels + fuse_map (surfel_map.cpp:154-161) ----
+ * dsm_fuse_stream_window is dsm_fuse_stream_resident with each frame's drift-free window step in front of its fuse.
+ * For frame t, in order:
+ *   1. every keyframe of retire_kf[retire_ofs[t] .. retire_ofs[t+1]) is retired, in list order (= dsm_inactive_retire)
+ *   2. every keyframe of reactivate_kf[reactivate_ofs[t] .. reactivate_ofs[t+1]) is reactivated, in list order
+ *      (= dsm_inactive_reactivate)
+ *   3. frame t is fused on the resident pool, post-step included (= dsm_fuse_frame_resident)
+ * The lists are the node's poses_to_remove / poses_to_add of get_add_remove_poses (surfel_map.cpp:1597-1641), which the
+ * caller knows before any kernel runs.  Afterwards the pool, the store (contents and order) and its segment list are
+ * byte-identical to what that sequence of calls leaves.  Phase 1 (superpixels, plane fits) runs batched and overlaps the
+ * previous call exactly as in dsm_fuse_stream_resident; the window step of a frame runs right before its fuse on the
+ * same high-priority stream.  All lists empty: the result of dsm_fuse_stream_resident.  n_frames = 1: the single-frame
+ * node.  A NULL offset array means empty lists for every frame.
+ * Nothing waits for the device unless n_new ([n_frames], optional) is passed: the surfel counts stay on the device.
+ * Checked on the host before anything is enqueued:
+ *   DSM_E_INVALID  offsets that decrease, more than DSM_WINDOW_MAX_KEYS keys in one frame's list, a negative keyframe,
+ *                  a keyframe listed twice in one frame's lists or in both lists of one frame
+ *   DSM_E_STATE    a non-empty list without dsm_inactive_reserve, and the errors of dsm_fuse_stream_resident
+ * Capacity is checked on the device, with the exact counts, for each frame before any of it is applied: the store after
+ * its retirements must fit the reservation, and the pool after its reactivations plus one frame of new surfels (S =
+ * dsm_num_seeds) must fit max_local_surfels (the test of dsm_fuse_frame_resident).  A frame that does not fit is not
+ * applied, and neither is any later frame, of this call or of later calls: it sets a sticky error word on the device,
+ * every resident kernel exits at once while the word is set, and the pool and store stay exactly as after the last
+ * applied frame.  The error is returned as DSM_E_CAPACITY by this call when n_new is passed (n_new[t] = -1 for every
+ * frame not applied), otherwise by the next call that synchronises with the resident state (dsm_pool_size,
+ * dsm_pool_download, dsm_pool_retire, dsm_pool_export_*, dsm_pool_append, dsm_inactive_* except _transform, and the
+ * fuse calls that return n_new).  That call clears the word and does nothing else; the map can be read and the stream
+ * resumed from the last applied frame.  The segment table has one entry per surfel of the reservation, so it cannot
+ * overflow on its own. */
+#define DSM_WINDOW_MAX_KEYS 128
+int dsm_fuse_stream_window(dsm_ctx *ctx, int n_frames, const int32_t *reference_frame_index,
+                           const uint8_t *gray, const float *depth, const float *poses_colmajor,
+                           const int32_t *retire_kf, const int32_t *retire_ofs,         /* [n_frames + 1] */
+                           const int32_t *reactivate_kf, const int32_t *reactivate_ofs, /* [n_frames + 1] */
+                           int32_t *n_new);
 
 /* ---- multi-GPU: frames of a batch sharded across GPUs, ONE gather of the surfel deltas at the end (SURVEY.md 8e) ----
  * One context per GPU (one process or thread each).  The reference has no counterpart (fuse_initialize_map is

@@ -75,6 +75,36 @@ class ResidentSurfelPool
         return report("fuse_map");
     }
 
+    // synchronize_msgs (surfel_map.cpp:154-161) in one call: move_add_surfels with the lists get_add_remove_poses hands
+    // it (poses_to_remove, then poses_to_add), then fuse_map -- all on the device, and the call never synchronises (a
+    // frame that does not fit the pool or the inactive store is reported by the next call that reads the map, see
+    // dsm_fuse_stream_window).  Non-empty lists need reserve_inactive().
+    template <class Mat, class Mat4f>
+    int fuse_map(Mat &image, Mat &depth, Mat4f &pose, int reference_index, const std::vector<int> &poses_to_remove,
+                 const std::vector<int> &poses_to_add)
+    {
+        if (!ready("fuse_map")) return err_;
+        const uint8_t *g = reinterpret_cast<const uint8_t *>(image.data);
+        const float *d = reinterpret_cast<const float *>(depth.data);
+        if ((size_t)image.step != (size_t)width_ || (size_t)depth.step != (size_t)width_ * 4)
+        { // the stream entry point takes tightly packed images
+            packed_gray_.resize((size_t)width_ * height_);
+            packed_depth_.resize((size_t)width_ * height_);
+            for (int y = 0; y < height_; y++)
+            {
+                std::memcpy(&packed_gray_[(size_t)y * width_], g + (size_t)y * image.step, (size_t)width_);
+                std::memcpy(&packed_depth_[(size_t)y * width_], reinterpret_cast<const uint8_t *>(d) + (size_t)y * depth.step,
+                            (size_t)width_ * 4);
+            }
+            g = packed_gray_.data(), d = packed_depth_.data();
+        }
+        const std::vector<int32_t> rk(poses_to_remove.begin(), poses_to_remove.end()), ak(poses_to_add.begin(), poses_to_add.end());
+        const int32_t ro[2] = {0, (int32_t)rk.size()}, ao[2] = {0, (int32_t)ak.size()};
+        const int32_t ref = reference_index;
+        err_ = dsm_fuse_stream_window(ctx_, 1, &ref, g, d, pose.data(), rk.data(), ro, ak.data(), ao, nullptr);
+        return report("fuse_map");
+    }
+
     // warp_surfels(): p <- W p, n <- R_W n for every local surfel; W = T_loop * T_cam^-1 as float, column-major
     template <class Mat4f>
     int warp_active_surfels(Mat4f &warp_pose)
@@ -324,5 +354,7 @@ class ResidentSurfelPool
     int capacity_;
     int width_, height_;
     std::vector<dsm_point_t> scratch_;
+    std::vector<uint8_t> packed_gray_;
+    std::vector<float> packed_depth_;
 };
 } // namespace dsm
