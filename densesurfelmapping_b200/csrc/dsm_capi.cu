@@ -172,7 +172,6 @@ extern "C" int dsm_create(const dsm_params *params, int device, void *cuda_strea
     ALLOC(d.nhard, (size_t)B);
     ALLOC(d.hrec, (size_t)B * S * 24);
     ALLOC(d.tstable, (size_t)B * S);
-    ALLOC(d.usum, (size_t)B * S);
     ALLOC(d.und, (size_t)B * S);
     ALLOC(d.dlist, (size_t)B * S * 232);
     ALLOC(d.errflag, (size_t)B);
@@ -502,7 +501,7 @@ static int launch_schedule(dsm_ctx *ctx, const DsmDev &d, int nb, cudaStream_t s
 
 // Enqueue the schedule for the view `v` (frames [v.frame0, v.frame0 + nf)), followed, when `post` is set, by the
 // resident pool's fuse_map post-step (in place, slot for slot as the reference).
-// The 17-21 launches are captured once per distinct parameter set into a CUDA graph and replayed: the
+// The 14-18 launches are captured once per distinct parameter set into a CUDA graph and replayed: the
 // per-launch CPU cost and inter-kernel gaps matter for single frames and small chunks.  Profiling
 // (event pairs around kernels) and the debug kernel budget use plain launches.
 static int enqueue_schedule(dsm_ctx *ctx, const DsmDev &v, int nf, cudaStream_t st, bool post = false, int phase = 3)

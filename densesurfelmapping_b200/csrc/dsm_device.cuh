@@ -13,8 +13,10 @@
 //   inv_md  f64 [B][S]          1.0 / (double)mean_depth (exact path of the assign pass, :380)
 //   tstable i32 [B][S]          stable flag + raster time stamp: INT_MAX = stable,
 //                               -1 = unstable, k >= 0 = un-stabled when raster scan reached k
-//   usum    int4 [B][S], und i32 [B][S]   update_seeds integer sums / depth-list lengths
-//   dlist   f32 [B][S][232]     member depths in raster order (k_gather -> k_newton2), one contiguous list per seed
+//   und     i32 [B][S]          depth-list lengths of the queued hard Newton seeds (k_gather -> k_newton_hard)
+//   dlist   f32 [B][S][232]     member depths in raster order of the queued hard Newton seeds, one contiguous list per
+//                               seed (the lists of the other seeds never leave k_gather's shared memory)
+//   hardq   i32 [B][S], nhard i32 [B]   queue of the hard Newton seeds (reset by k_assign2, appended by k_gather)
 //   done    i32 [B]             frame-completion tickets of the assign pass
 //   errflag i32 [B]             invariant violations (must stay 0)
 //   kx, ky  f32 [Wp+16], [H+16] back-projection factors, computed once per context
@@ -58,9 +60,8 @@ struct DsmDev
     float4 *seed;
     double *inv_md;
     int32_t *tstable;
-    int4 *usum;         // update_seeds integer sums per seed: (count, sum x, sum y, sum intensity)
-    int32_t *und;       // number of member depths > 0.1
-    float *dlist;       // [B][S][232] member depths in raster order, one contiguous list per seed
+    int32_t *und;       // number of member depths > 0.1 (written for the queued hard Newton seeds only)
+    float *dlist;       // [B][S][232] member depths in raster order, one contiguous list per queued hard Newton seed
     int32_t *errflag;   // [B] count of "impossible" events (non-stable seed without members, SURVEY H3)
     float4 *plane;
     const float *kx;    // [Wp+16]: ((float)u - cx) / fx, the per-column factor of back_project (:94)
@@ -85,8 +86,8 @@ struct DsmDev
     uint8_t *code;      // [B][H][Wp] label of every pixel as the index (0..3) of the winning candidate among its 2x2 candidate seeds, or DSM_CODE_NONE
     float *invd;        // [B][H][Wp] (float)(1.0 / (double)depth) for depth > 0.01, else 0 (:404-405), written by the first assign pass
     float2 *seed_hl;    // [B][S] 1.0 / (double)mean_depth split into two floats (hi, lo) for the filtered assign pass
-    int32_t *hardq;     // [B][S] seeds whose Huber-Newton needs the entry-by-entry classification (k_newton2 -> k_newton_hard)
-    int32_t *nhard;     // [B] queue lengths
+    int32_t *hardq;     // [B][S] seeds whose Huber-Newton needs the entry-by-entry classification (k_gather -> k_newton_hard)
+    int32_t *nhard;     // [B] queue lengths (reset by k_assign2)
     int32_t *done;      // [B] frame-completion tickets of the assign pass (the last CTA of a frame runs the stable relaxation)
     double *hrec;       // [B][24][S] plane fit, first residual pass: H = sum 2 q q^T (9), the same over out-of-range points (10), their clamped gradient (4), packed (margin, qmax2)
 };
@@ -122,8 +123,8 @@ enum DsmKernelId
     DSM_K_SEED_INIT = 0,
     DSM_K_ASSIGN_FIRST = 1,
     DSM_K_ASSIGN = 2,
-    DSM_K_GATHER = 3,       // window gather of update_seeds_kernel
-    DSM_K_NEWTON = 4,       // Huber-Newton solve of update_seeds_kernel
+    DSM_K_GATHER = 3,       // window gather of update_seeds_kernel + the Huber-Newton passes inside the Huber range
+    DSM_K_NEWTON = 4,       // Huber-Newton of the seeds with out-of-range entries (k_newton_hard)
     DSM_K_PLANE_GATHER = 5, // pixel normals + plane-fit gather
     DSM_K_PLANE_SOLVE = 6,  // plane-fit solver
     DSM_K_FUSE = 7,

@@ -122,6 +122,9 @@ __global__ void __launch_bounds__(128, 8) k_assign2(const __grid_constant__ DsmD
     // dist/16 (:374) is ax'^2 + ay'^2.  hi > 0 iff mean_depth > 0 (split_inverse); a seed outside the image, and the
     // no-seed record, have hi = 1: they never clear all_has_depth (:443), like the reference's skipped candidates.
     const int ya0 = (int)blockIdx.y - 1; // first candidate seed row of the CTA: floor((8 blockIdx.y - 4) / 8)
+    // this iteration's queue of hard Newton seeds (k_gather appends, k_newton_hard reads): emptied here, after the previous
+    // iteration's k_newton_hard has completed and before the k_gather that follows starts its work
+    if (tid == 0 && blockIdx.x == 0 && blockIdx.y == 0) d.nhard[b] = 0;
     if (tid <= A_NR * A_REC)
     {
         const int row = tid / A_REC;
@@ -350,7 +353,7 @@ __global__ void __launch_bounds__(128, 8) k_assign2(const __grid_constant__ DsmD
 }
 
 // -------------------------------------------------------------------------------------------
-// K2  slic_update — update_seeds_kernel (:468-562), as a tile gather and a per-seed solve
+// K2  slic_update — update_seeds_kernel (:468-562), as a tile gather with the per-seed solve at its end
 //
 // K2a k_gather (CTA = DSM_TILE_SX x DSM_TILE_SY = 32 seeds).  One thread arms an mbarrier and issues three TMA tensor
 //   copies (labels, depth boxes of 76x41 elements at pixel (64 bx - 4, 32 by - 4), gray box of 112x41 at (64 bx - 16,
@@ -360,16 +363,19 @@ __global__ void __launch_bounds__(128, 8) k_assign2(const __grid_constant__ DsmD
 //   intensity (exactly representable integers < 2^24, so the reference's float accumulation is exact and order-free)
 //   come from population counts and byte dot products of the mask and are combined over the 16 lanes by packed
 //   xor-butterflies.  Member depths > 0.1 are compacted IN RASTER ORDER (row-major = lane order, then column order
-//   inside the lane) into a per-seed list staged in shared memory and copied out as contiguous 16-byte runs:
-//   dlist[b][seed][DL_STRIDE].
-// K2b k_newton2 (thread per seed, every seed of the batch in flight): the float sums sum_depth (:511) and sum_a
-//   (:536-549) feed the next pass's costs and are order-sensitive (SURVEY.md H2), so one thread walks its seed's list
-//   sequentially, 8 entries (two 16-byte loads = one 32-byte sector) per step.  residual = fl(md - z) is monotone
-//   in z, so the list's extremes (found during the mean pass) decide for ALL entries whether they are inside the
-//   Huber range; in that -- by far most common -- case a Newton pass is a pure dependent chain
-//   sum_a = fmaf(2, md - z, sum_a) (2 r is exact: the same single rounding as `sum_a += 2 * residual`).
+//   inside the lane) into the seed's list in shared memory.  A pixel has one label, so the lists of the tile's 32
+//   seeds are disjoint subsets of the tile's footprint: packed back to back they fit one small buffer, and the lists
+//   never leave the SM.
+//   Then warp 0 runs the Newton of the tile's seeds, one lane per seed (update_seed_newton): the float sums sum_depth
+//   (:511) and sum_a (:536-549) feed the next pass's costs and are order-sensitive (SURVEY.md H2), so one thread walks
+//   its seed's list sequentially, 8 entries (two 16-byte loads) per step.  residual = fl(md - z) is monotone in z, so
+//   the list's extremes (found during the mean pass) decide for ALL entries whether they are inside the Huber range;
+//   in that -- by far most common -- case a Newton pass is a pure dependent chain sum_a = fmaf(2, md - z, sum_a)
+//   (2 r is exact: the same single rounding as `sum_a += 2 * residual`).  The other warps exit; the serial tail of
+//   one CTA overlaps the gathers of the other CTAs on the SM.  A seed that meets an out-of-range entry is queued for
+//   k_newton_hard with its state, and only its list goes to HBM (dlist[b][seed][DL_STRIDE]).
 // -------------------------------------------------------------------------------------------
-#define DL_STRIDE 232 // floats per seed list: >= 15*15 possible members, multiple of 8 (32-byte sectors)
+#define DL_STRIDE 232 // floats per queued seed list in dlist: >= 15*15 possible members, multiple of 8 (32-byte sectors)
 // Shared memory of the two seed-tile kernels (k_gather, k_plane_gather): the tile's depth and label-code boxes, then
 // each kernel's own planes from TILE_SMEM_OWN on
 #define TILE_PLANE_BYTES 12544 // 76 * 41 * 4 = 12464 rounded up to 128: TMA destinations are 128-byte aligned
@@ -378,10 +384,18 @@ __global__ void __launch_bounds__(128, 8) k_assign2(const __grid_constant__ DsmD
 #define TILE_SMEM_COD TILE_PLANE_BYTES // u8 [41][112] label-code box
 #define TILE_SMEM_OWN (TILE_PLANE_BYTES + TILE_BYTE_PLANE)
 #define TILE_TX_BYTES (DSM_TILE_W * DSM_TILE_H * 4u + (unsigned)DSM_TILE_GW * DSM_TILE_H) // the depth and code boxes
+// Packed member-depth lists of one tile: the windows of the tile's seeds cover (DSM_TILE_SX + 1) x (DSM_TILE_SY + 1)
+// superpixels of pixels (72 x 40), every pixel is in at most one seed's list, and each list starts 16-byte aligned
+// (at most 3 floats of padding per seed).
+#define GAT_NSEED (DSM_TILE_SX * DSM_TILE_SY)
+#define GAT_LIST_CAP ((DSM_TILE_SX + 1) * DSM_SP * (DSM_TILE_SY + 1) * DSM_SP + 3 * GAT_NSEED)
+static_assert(GAT_NSEED == 32, "warp 0 of k_gather runs the Newton with one lane per seed of the tile");
+static_assert(GAT_LIST_CAP == 72 * 40 + 96 && GAT_LIST_CAP % 4 == 0, "2880 member depths + 16-byte padding of 32 lists");
 #define GAT_SMEM_GRY TILE_SMEM_OWN                               // u8 [41][112] gray box
-#define GAT_SMEM_LIST (TILE_SMEM_OWN + TILE_BYTE_PLANE)          // float [16][DL_STRIDE]: the 16 seeds of one round
-#define GAT_SMEM_ND (GAT_SMEM_LIST + 16 * DL_STRIDE * 4)        // int [16] list lengths of the round
-#define GAT_SMEM_BAR (GAT_SMEM_ND + 16 * 4)
+#define GAT_SMEM_LIST (TILE_SMEM_OWN + TILE_BYTE_PLANE)          // float [GAT_LIST_CAP]: the 32 lists, in seed-slot order
+#define GAT_SMEM_SUM (GAT_SMEM_LIST + GAT_LIST_CAP * 4)          // int4 [32] integer sums (count, sum x, sum y, sum intensity)
+#define GAT_SMEM_ND (GAT_SMEM_SUM + GAT_NSEED * 16)              // int [32] list lengths, -1 for a seed update_seeds skips
+#define GAT_SMEM_BAR (GAT_SMEM_ND + GAT_NSEED * 4)
 #define GAT_SMEM_BYTES (GAT_SMEM_BAR + 16)
 
 // 16-bit membership mask of one window row from the label-code tile: bit k set iff the pixel at window column k is labelled
@@ -467,12 +481,104 @@ __device__ __forceinline__ int half_warp_scan(int c, int r, int &total)
     return incl - c;
 }
 
+// One Newton pass over a list whose entries are ALL inside the Huber range: sum_a += 2 * residual, i.e.
+// fmaf(2, md - z, sum_a) (2 r is exact: the same single rounding per add), eight entries (two 16-byte loads) per step.
+__device__ __forceinline__ float huber_sum_in_range(const float *dl, int nd, float md)
+{
+    const float4 *dl4 = reinterpret_cast<const float4 *>(dl);
+    float sa = 0.0f;
+    int k = 0;
+    for (; k + 8 <= nd; k += 8)
+    {
+        const float4 a = dl4[k >> 2], c = dl4[(k >> 2) + 1];
+        sa = fmaf(2.0f, md - a.x, sa), sa = fmaf(2.0f, md - a.y, sa), sa = fmaf(2.0f, md - a.z, sa), sa = fmaf(2.0f, md - a.w, sa);
+        sa = fmaf(2.0f, md - c.x, sa), sa = fmaf(2.0f, md - c.y, sa), sa = fmaf(2.0f, md - c.z, sa), sa = fmaf(2.0f, md - c.w, sa);
+    }
+    for (; k < nd; k++) sa = fmaf(2.0f, md - dl[k], sa);
+    return sa;
+}
+
+// The per-seed part of update_seeds (:496-556) for seed o that is not stable: the mean depth of its member list
+// dl[0 .. nd) (16-byte aligned, raster order) and its Newton passes as long as every entry is inside the Huber range (a
+// pure dependent chain), then the means and `stable` from its integer sums *su = (count, sum x, sum y, sum intensity)
+// (computed last: independent of the depths, and nothing of them is live across the chain).  A seed that meets an
+// out-of-range entry is left to k_newton_hard, one thread each at full occupancy, so that the entry-by-entry
+// classification loop is never executed by a warp in which one lane needs it and 31 wait: its state goes to pfsum and
+// the function returns true; the caller queues it and copies its list to dlist.  Otherwise the seed is stored.
+__device__ __forceinline__ bool update_seed_newton(const DsmDev &d, int b, size_t o, const int4 *su, const float *dl, int nd)
+{
+    if (su->x == 0)
+    { // unreachable for supported shapes (every seed keeps its centre pixel, SURVEY H3); recorded, never silently ignored
+        atomicAdd(&d.errflag[b], 1);
+        d.tstable[o] = -1;
+        return false;
+    }
+    float md = 0.0f;
+    bool queued = false;
+    if (nd > 0)
+    {
+        const float4 *dl4 = reinterpret_cast<const float4 *>(dl);
+        float sum_d = 0.0f, zmn = __int_as_float(0x7f800000), zmx = 0.f;
+        {
+            int k = 0;
+            for (; k + 8 <= nd; k += 8)
+            {
+                const float4 a = dl4[k >> 2], c = dl4[(k >> 2) + 1];
+                const float v[8] = {a.x, a.y, a.z, a.w, c.x, c.y, c.z, c.w};
+#pragma unroll
+                for (int j = 0; j < 8; j++) sum_d += v[j]; // raster order (:511)
+                zmn = fminf(zmn, fminf(fminf(fminf(v[0], v[1]), fminf(v[2], v[3])), fminf(fminf(v[4], v[5]), fminf(v[6], v[7]))));
+                zmx = fmaxf(zmx, fmaxf(fmaxf(fmaxf(v[0], v[1]), fmaxf(v[2], v[3])), fmaxf(fmaxf(v[4], v[5]), fmaxf(v[6], v[7]))));
+            }
+            for (; k < nd; k++)
+            {
+                const float v = dl[k];
+                sum_d += v;
+                zmn = fminf(zmn, v);
+                zmx = fmaxf(zmx, v);
+            }
+        }
+        md = sum_d / (float)nd;
+        for (int it = 0; it < 5; it++)
+        { // damped Huber-Newton (:534-554)
+            // residual = fl(md - z) is monotone in z: the list's extremes decide for ALL entries whether they are inside
+            // the Huber range ((double)r < HUBER_RANGE && (double)r > -HUBER_RANGE, :540)
+            if (!((md - zmn) < d.huber_hi && (md - zmx) > -d.huber_hi))
+            {
+                queued = true;
+                d.pfsum[o * 2] = make_float4(md, __int_as_float(it), zmn, zmx); // the plane-fit scratch is free during the clustering
+                break;
+            }
+            // every entry in range; sum_b = nd exact additions of 2
+            const float sa = huber_sum_in_range(dl, nd, md);
+            const float delta = (float)((double)(-sa) / ((double)(float)(2 * nd) + 10.0));
+            md = md + delta;
+            if (delta < F_0p01_HI && delta > -F_0p01_HI) break; // |delta| < 0.01 in double (:552)
+        }
+    }
+    const int4 sm = *su;
+    const float4 pre = d.seed[o];
+    const float fn = (float)sm.x; // sums below are < 2^24 so the reference's float accumulation is exact
+    const float mi = (float)sm.w / fn;
+    const float mx = (float)sm.y / fn;
+    const float my = (float)sm.z / fn;
+    // ::fabs(double): float differences, summed in double, rounded once (:527)
+    const float diff = (float)(fabs((double)(pre.z - mi)) + fabs((double)(pre.x - mx)) + fabs((double)(pre.y - my)));
+    const bool newstable = diff < F_0p2_HI; // (double)diff < 0.2 (:528)
+    if (queued)
+        d.pfsum[o * 2 + 1] = make_float4(mx, my, mi, newstable ? 1.f : 0.f);
+    else
+        store_seed(d, o, mx, my, mi, md, newstable);
+    return queued;
+}
+
 __global__ void __launch_bounds__(256, 6) k_gather(const __grid_constant__ DsmDev d, const __grid_constant__ DsmMaps mp)
 {
     pdl_enter();
     extern __shared__ __align__(128) unsigned char smem[];
     const uint8_t *t_gry = smem + GAT_SMEM_GRY;
     float *lists = reinterpret_cast<float *>(smem + GAT_SMEM_LIST);
+    int4 *s_sum = reinterpret_cast<int4 *>(smem + GAT_SMEM_SUM);
     int *s_nd = reinterpret_cast<int *>(smem + GAT_SMEM_ND);
     const unsigned bar = smem_u32(smem + GAT_SMEM_BAR);
 
@@ -484,7 +590,6 @@ __global__ void __launch_bounds__(256, 6) k_gather(const __grid_constant__ DsmDe
         tile_issue(smem, bar, TILE_TX_BYTES + DSM_TILE_GW * DSM_TILE_H, mp, X0, Y0, b);
         tma_load_3d(smem_u32(smem + GAT_SMEM_GRY), &mp.gry, X0 - DSM_TILE_GX, Y0, b, bar);
     }
-    if (threadIdx.x == 1 && blockIdx.x == 0 && blockIdx.y == 0) d.nhard[b] = 0; // this pass's queue of hard Newton seeds
     const int W = d.W, H = d.H;
     const size_t so = (size_t)b * d.S;
     const int half = lane >> 4, r = lane & 15;
@@ -498,12 +603,12 @@ __global__ void __launch_bounds__(256, 6) k_gather(const __grid_constant__ DsmDe
     }
     __syncthreads(); // barrier initialised before anybody polls it
     mbar_wait(bar, 0);
+    int lbase = 0; // start of this round's lists in the packed buffer: round 1 follows round 0's
 #pragma unroll
     for (int rd = 0; rd < 2; rd++)
     {
         const int q = warp * 2 + half; // seed slot of this round
         const TileSeed t = tile_seed(d, rd * 16 + q);
-        const int s = t.sp_y * d.spw + t.sp_x;
         const bool act = tflag[rd] != DSM_STABLE;
         const int x0 = t.sp_x * DSM_SP - DSM_SP / 2, y0 = t.sp_y * DSM_SP - DSM_SP / 2;
         const int xb = x0 > 0 ? x0 : 0, yb = y0 > 0 ? y0 : 0;
@@ -514,64 +619,89 @@ __global__ void __launch_bounds__(256, 6) k_gather(const __grid_constant__ DsmDe
         // member columns of the window: xb - x0 <= k < xe - x0; nothing if the row is outside
         const unsigned kmask = rowin ? (((1u << (xe - x0)) - 1u) & ~((1u << (xb - x0)) - 1u)) : 0u;
         const int trow = t.ty * DSM_SP + r, tcol = t.tx * DSM_SP;
-        float zk[16];
-        unsigned mm = window_row(smem, trow, tcol, r, zk), zm = 0; // bit k: labelled with this seed / depth > 0.1
-#pragma unroll
-        for (int k = 0; k < 16; k++) zm |= (zk[k] > F_0p1_LO ? 1u : 0u) << k; // (double)depth > 0.1 (:508)
-        mm &= kmask;
-        const unsigned dm = mm & zm; // member with depth > 0.1
-        const int cnt = __popc(mm);
-        const int sdx = mask_index_sum(mm);
-        int si = 0;
+        unsigned dm; // bit k: member with depth > 0.1
+        int excl, ndt;
         {
-            const unsigned *pg = reinterpret_cast<const unsigned *>(t_gry + trow * DSM_TILE_GW + DSM_TILE_GX + tcol); // 4-byte aligned
+            float zk[16];
+            unsigned mm = window_row(smem, trow, tcol, r, zk), zm = 0; // bit k: labelled with this seed / depth > 0.1
 #pragma unroll
-            for (int qd = 0; qd < 4; qd++) si = (int)__dp4a(pg[qd] & nibble_to_bytes(mm >> (4 * qd)), 0x01010101u, (unsigned)si);
-        }
-        // packed 16-lane butterflies: count <= 225 (8 bits) | sum intensity <= 57375 (16 bits);
-        // sum (x - x0) <= 3375 (12 bits) | sum (y - y0) <= 3375
-        int pa = cnt | (si << 8), pb = sdx | ((cnt * r) << 12);
+            for (int k = 0; k < 16; k++) zm |= (zk[k] > F_0p1_LO ? 1u : 0u) << k; // (double)depth > 0.1 (:508)
+            mm &= kmask;
+            dm = mm & zm;
+            const int cnt = __popc(mm);
+            const int sdx = mask_index_sum(mm);
+            int si = 0;
+            {
+                const unsigned *pg = reinterpret_cast<const unsigned *>(t_gry + trow * DSM_TILE_GW + DSM_TILE_GX + tcol); // 4-byte aligned
 #pragma unroll
-        for (int o = 8; o > 0; o >>= 1)
-        {
-            pa += __shfl_xor_sync(FULL, pa, o);
-            pb += __shfl_xor_sync(FULL, pb, o);
-        }
-        int ndt;
-        const int excl = half_warp_scan(__popc(dm), r, ndt);
-        if (rd) __syncthreads(); // the previous round's lists have been copied out
-        float *lp = lists + q * DL_STRIDE + excl;
+                for (int qd = 0; qd < 4; qd++) si = (int)__dp4a(pg[qd] & nibble_to_bytes(mm >> (4 * qd)), 0x01010101u, (unsigned)si);
+            }
+            // packed 16-lane butterflies: count <= 225 (8 bits) | sum intensity <= 57375 (16 bits);
+            // sum (x - x0) <= 3375 (12 bits) | sum (y - y0) <= 3375
+            int pa = cnt | (si << 8), pb = sdx | ((cnt * r) << 12);
 #pragma unroll
-        for (int k = 0; k < 16; k++)
-            if ((dm >> k) & 1u) *lp++ = zk[k];
-        if (r == 0)
-        {
-            s_nd[q] = act ? ndt : 0;
-            if (act)
+            for (int o = 8; o > 0; o >>= 1)
+            {
+                pa += __shfl_xor_sync(FULL, pa, o);
+                pb += __shfl_xor_sync(FULL, pb, o);
+            }
+            excl = half_warp_scan(__popc(dm), r, ndt);
+            if (r == 0)
             {
                 const int n = pa & 0xff;
-                d.usum[so + s] = make_int4(n, n * x0 + (pb & 0xfff), n * y0 + (pb >> 12), pa >> 8);
-                d.und[so + s] = ndt;
+                s_nd[rd * 16 + q] = act ? ndt : -1;
+                s_sum[rd * 16 + q] = make_int4(n, n * x0 + (pb & 0xfff), n * y0 + (pb >> 12), pa >> 8);
             }
         }
-        __syncthreads();
-        // copy-out: warp w moves the lists of seed slots w and w + 8 of this round -> dlist[b][seed][0 .. nd), 16 bytes per lane
+        __syncthreads(); // the round's list lengths are known
+        // offset of the seed's list: the lists are packed in seed-slot order, each padded to 16 bytes (a skipped seed has
+        // none); every half-warp scans the round's 16 lengths, lane r holds the start of slot r's list
+        int rtot;
+        const int nr = s_nd[rd * 16 + r];
+        const int lofs = lbase + half_warp_scan(nr > 0 ? (nr + 3) & ~3 : 0, r, rtot);
+        float *lp = lists + __shfl_sync(FULL, lofs, q & 15, 16) + excl;
+        lbase += rtot;
+        // the depths are read again from the staged tile rather than kept in registers across the barrier
+        const float4 *pz = reinterpret_cast<const float4 *>(reinterpret_cast<const float *>(smem + TILE_SMEM_DEP) + trow * DSM_TILE_W + tcol);
 #pragma unroll
-        for (int h2 = 0; h2 < 2; h2++)
+        for (int qd = 0; qd < 4; qd++)
         {
-            const int q2 = warp + 8 * h2, n2 = s_nd[q2];
-            if (n2 == 0) continue; // warp-uniform
-            const TileSeed t2 = tile_seed(d, rd * 16 + q2);
-            const int s2 = t2.sp_y * d.spw + t2.sp_x;
-            float4 *dst = reinterpret_cast<float4 *>(d.dlist + (so + s2) * DL_STRIDE);
-            const float4 *src = reinterpret_cast<const float4 *>(lists + q2 * DL_STRIDE);
-            if (4 * lane < n2) dst[lane] = src[lane];
-            if (4 * (lane + 32) < n2) dst[lane + 32] = src[lane + 32];
+            if (!((dm >> (4 * qd)) & 0xfu)) continue;
+            const float4 z = pz[qd];
+            const float zq[4] = {z.x, z.y, z.z, z.w};
+#pragma unroll
+            for (int k = 0; k < 4; k++)
+                if ((dm >> (4 * qd + k)) & 1u) *lp++ = zq[k];
         }
+    }
+    __syncthreads(); // every list of the tile is written
+    if (warp != 0) return;
+
+    // Newton of the tile's seeds: lane = seed slot
+    const int nd = s_nd[lane];
+    int ltot;
+    const int lofs = warp_excl_scan(nd > 0 ? (nd + 3) & ~3 : 0, lane, ltot); // the same packing as the list writes
+    const TileSeed t = tile_seed(d, lane);
+    const int s = t.sp_y * d.spw + t.sp_x;
+    const float *dl = lists + lofs;
+    const bool queued = nd >= 0 && update_seed_newton(d, b, so + s, s_sum + lane, dl, nd);
+    if (queued)
+    {
+        d.und[so + s] = nd;
+        d.hardq[so + atomicAdd(&d.nhard[b], 1)] = s;
+    }
+    // the lists of the queued seeds go to dlist[b][seed][0 .. nd), one list at a time over the warp, 16 bytes per lane
+    for (unsigned hq = __ballot_sync(FULL, queued); hq; hq &= hq - 1)
+    {
+        const int j = __ffs(hq) - 1;
+        const int nj = __shfl_sync(FULL, nd, j), oj = __shfl_sync(FULL, lofs, j), sj = __shfl_sync(FULL, s, j);
+        float4 *dst = reinterpret_cast<float4 *>(d.dlist + (so + sj) * DL_STRIDE);
+        const float4 *src = reinterpret_cast<const float4 *>(lists + oj);
+        for (int i = lane; 4 * i < nj; i += 32) dst[i] = src[i];
     }
 }
 
-#define NW_T 64       // seeds (threads) per CTA of the two Newton kernels
+#define NW_T 64       // seeds (threads) per CTA of k_newton_hard
 #define NW_CAP 5632   // floats of list staging per CTA (22 KB): 88 entries per seed on average, 225 possible; 8 CTAs per SM
 
 // Every thread of a Newton CTA stages its seed's list src[0 .. nd) (a contiguous run in global memory) into buf with 16-byte
@@ -603,120 +733,8 @@ __device__ __forceinline__ const float *stage_list(float *buf, int *s_off, int *
     return s_off[tid] >= 0 ? buf + s_off[tid] : src;
 }
 
-// One Newton pass over a list whose entries are ALL inside the Huber range: sum_a += 2 * residual, i.e.
-// fmaf(2, md - z, sum_a) (2 r is exact: the same single rounding per add), eight entries (two 16-byte loads) per step.
-__device__ __forceinline__ float huber_sum_in_range(const float *dl, int nd, float md)
-{
-    const float4 *dl4 = reinterpret_cast<const float4 *>(dl);
-    float sa = 0.0f;
-    int k = 0;
-    for (; k + 8 <= nd; k += 8)
-    {
-        const float4 a = dl4[k >> 2], c = dl4[(k >> 2) + 1];
-        sa = fmaf(2.0f, md - a.x, sa), sa = fmaf(2.0f, md - a.y, sa), sa = fmaf(2.0f, md - a.z, sa), sa = fmaf(2.0f, md - a.w, sa);
-        sa = fmaf(2.0f, md - c.x, sa), sa = fmaf(2.0f, md - c.y, sa), sa = fmaf(2.0f, md - c.z, sa), sa = fmaf(2.0f, md - c.w, sa);
-    }
-    for (; k < nd; k++) sa = fmaf(2.0f, md - dl[k], sa);
-    return sa;
-}
-
-__global__ void __launch_bounds__(NW_T, 8) k_newton2(const __grid_constant__ DsmDev d)
-{
-    pdl_enter();
-    // Every thread stages its seed's list into shared memory and then walks it there up to six times.
-    __shared__ __align__(16) float buf[NW_CAP];
-    __shared__ int s_off[NW_T], s_wsum[NW_T / 32];
-    const int b = d.frame0 + blockIdx.y;
-    const int s = blockIdx.x * NW_T + threadIdx.x;
-    const size_t so = (size_t)b * d.S;
-    // the four per-seed loads are independent and issued together (one memory round trip), before the list staging
-    const bool inr = s < d.S;
-    const int tflag = inr ? d.tstable[so + s] : DSM_STABLE;
-    const int nd_raw = inr ? d.und[so + s] : 0;
-    const int4 su = inr ? d.usum[so + s] : make_int4(0, 0, 0, 0);
-    const float4 pre = inr ? d.seed[so + s] : make_float4(0.f, 0.f, 0.f, 0.f);
-    const bool act = tflag != DSM_STABLE; // stable seeds are untouched by update_seeds (:478-479)
-    const int nd = act ? nd_raw : 0;
-    const float *dl = stage_list(buf, s_off, s_wsum, d.dlist + (so + s) * DL_STRIDE, nd);
-    __pipeline_wait_prior(0);
-    if (!act) return;
-    // Every seed runs its mean pass and its Newton passes as long as every entry is inside the Huber range (a pure
-    // dependent chain).  A seed that meets an out-of-range entry is appended to the frame's queue of hard seeds with its
-    // state; k_newton_hard continues those, one thread each at full occupancy, so that the entry-by-entry
-    // classification loop is never executed by a warp in which one lane needs it and 31 wait.
-    if (act)
-    {
-        const int n = su.x;
-        if (n == 0)
-        { // unreachable for supported shapes (every seed keeps its centre pixel, SURVEY H3); recorded, never silently ignored
-            atomicAdd(&d.errflag[b], 1);
-            d.tstable[so + s] = -1;
-        }
-        else
-        {
-            const float fn = (float)n; // sums below are < 2^24 so the reference's float accumulation is exact
-            const float mi = (float)su.w / fn;
-            const float mx = (float)su.y / fn;
-            const float my = (float)su.z / fn;
-            // ::fabs(double): float differences, summed in double, rounded once (:527)
-            const float diff = (float)(fabs((double)(pre.z - mi)) + fabs((double)(pre.x - mx)) + fabs((double)(pre.y - my)));
-            const bool newstable = diff < F_0p2_HI; // (double)diff < 0.2 (:528)
-            float md = 0.0f;
-            bool queued = false;
-            if (nd > 0)
-            {
-                const float4 *dl4 = reinterpret_cast<const float4 *>(dl);
-                float sum_d = 0.0f, zmn = __int_as_float(0x7f800000), zmx = 0.f;
-                {
-                    int k = 0;
-                    for (; k + 8 <= nd; k += 8)
-                    {
-                        const float4 a = dl4[k >> 2], c = dl4[(k >> 2) + 1];
-                        const float v[8] = {a.x, a.y, a.z, a.w, c.x, c.y, c.z, c.w};
-#pragma unroll
-                        for (int j = 0; j < 8; j++) sum_d += v[j]; // raster order (:511)
-                        zmn = fminf(zmn, fminf(fminf(fminf(v[0], v[1]), fminf(v[2], v[3])), fminf(fminf(v[4], v[5]), fminf(v[6], v[7]))));
-                        zmx = fmaxf(zmx, fmaxf(fmaxf(fmaxf(v[0], v[1]), fmaxf(v[2], v[3])), fmaxf(fmaxf(v[4], v[5]), fmaxf(v[6], v[7]))));
-                    }
-                    for (; k < nd; k++)
-                    {
-                        const float v = dl[k];
-                        sum_d += v;
-                        zmn = fminf(zmn, v);
-                        zmx = fmaxf(zmx, v);
-                    }
-                }
-                md = sum_d / (float)nd;
-                for (int it = 0; it < 5; it++)
-                { // damped Huber-Newton (:534-554)
-                    // residual = fl(md - z) is monotone in z: the list's extremes decide for ALL entries whether they are inside
-                    // the Huber range ((double)r < HUBER_RANGE && (double)r > -HUBER_RANGE, :540)
-                    if (!((md - zmn) < d.huber_hi && (md - zmx) > -d.huber_hi))
-                    {
-                        queued = true;
-                        d.pfsum[(so + s) * 2] = make_float4(md, __int_as_float(it), zmn, zmx); // the plane-fit scratch is free during the clustering
-                        break;
-                    }
-                    // every entry in range; sum_b = nd exact additions of 2
-                    const float sa = huber_sum_in_range(dl, nd, md);
-                    const float delta = (float)((double)(-sa) / ((double)(float)(2 * nd) + 10.0));
-                    md = md + delta;
-                    if (delta < F_0p01_HI && delta > -F_0p01_HI) break; // |delta| < 0.01 in double (:552)
-                }
-            }
-            if (queued)
-            {
-                d.pfsum[(so + s) * 2 + 1] = make_float4(mx, my, mi, newstable ? 1.f : 0.f);
-                d.hardq[so + atomicAdd(&d.nhard[b], 1)] = s;
-            }
-            else
-                store_seed(d, so + s, mx, my, mi, md, newstable);
-        }
-    }
-}
-
 // K2c k_newton_hard (thread per queued seed): the Newton passes of the seeds that have entries outside the Huber range
-// (:540-547), continued from the state k_newton2 left.  Eight entries per step: their residuals and in-range flags are
+// (:540-547), continued from the state k_gather left.  Eight entries per step: their residuals and in-range flags are
 // independent and computed first; what remains serial is the reference's running sum -- fmaf(2, r, sum_a) for an entry
 // in range, (float)((double)sum_a + -+HUBER_RANGE) for one outside (:547).
 __global__ void __launch_bounds__(NW_T, 8) k_newton_hard(const __grid_constant__ DsmDev d)
@@ -1331,8 +1349,9 @@ int dsm_tile_setup()
 {
     cudaError_t e = cudaFuncSetAttribute(k_gather, cudaFuncAttributeMaxDynamicSharedMemorySize, GAT_SMEM_BYTES);
     if (e == cudaSuccess) e = cudaFuncSetAttribute(k_plane_gather, cudaFuncAttributeMaxDynamicSharedMemorySize, PG_SMEM_BYTES);
-    // shared memory is what limits the residency of the two tile kernels (36.6 KB / 33 KB per CTA): ask for the largest carve-out;
-    // k_gather then runs 6 CTAs per SM (6 x (36,688 B + the 1 KB per-CTA reserve) fits the 228 KB of an H100 SM)
+    // shared memory is what limits the residency of the two tile kernels (34.3 KB / 33 KB per CTA): ask for the largest carve-out;
+    // k_gather then runs 6 CTAs per SM (6 x (34,320 B + the 1 KB per-CTA reserve) fits the 228 KB of an H100 SM; its 40
+    // registers per thread allow 6 as well)
     if (e == cudaSuccess) e = cudaFuncSetAttribute(k_gather, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
     if (e == cudaSuccess) e = cudaFuncSetAttribute(k_plane_gather, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
     return e == cudaSuccess ? 0 : -1;
@@ -1353,9 +1372,8 @@ void dsm_launch_gather(const DsmDev &d, const DsmMaps &m, int nb, cudaStream_t s
     pdl_launch(k_gather, tile_grid(d, nb), dim3(256), GAT_SMEM_BYTES, s, d, m);
 }
 void dsm_launch_newton2(const DsmDev &d, int nb, cudaStream_t s)
-{
+{ // the in-range Newton passes run at the end of k_gather; this continues the seeds it queued
     dim3 grid((d.S + NW_T - 1) / NW_T, nb);
-    pdl_launch(k_newton2, grid, dim3(NW_T), 0, s, d);
     pdl_launch(k_newton_hard, grid, dim3(NW_T), 0, s, d); // surplus CTAs exit at once: the queue length is on the device
 }
 void dsm_launch_plane_gather(const DsmDev &d, const DsmMaps &m, int nb, cudaStream_t s)

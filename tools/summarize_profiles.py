@@ -16,9 +16,9 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 out = os.path.join(ROOT, "profiles")
 os.makedirs(out, exist_ok=True)
 BENCH = {"k_seed_init": "seed_init", "k_assign2<1>": "slic_assign_first", "k_assign2<0>": "slic_assign", "k_gather": "slic_gather",
-         "k_newton2": "slic_newton", "k_newton_hard": "slic_newton", "k_plane_gather": "plane_gather", "k_gn_solve": "plane_solve",
+         "k_newton_hard": "slic_newton", "k_plane_gather": "plane_gather", "k_gn_solve": "plane_solve",
          "k_fuse": "surfel_fuse", "k_init_surfels": "surfel_init", "k_repack": "repack"}
-PER_STEP = {"k_seed_init": 1, "k_assign2<1>": 1, "k_assign2<0>": 2, "k_gather": 3, "k_newton2": 3, "k_newton_hard": 3, "k_plane_gather": 1,
+PER_STEP = {"k_seed_init": 1, "k_assign2<1>": 1, "k_assign2<0>": 2, "k_gather": 3, "k_newton_hard": 3, "k_plane_gather": 1,
             "k_gn_solve": 1, "k_fuse": 1, "k_init_surfels": 1}
 PHASE = {"slic_assign_first": "slic_assign"}
 
