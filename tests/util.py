@@ -56,7 +56,8 @@ def check_surfels(got, want, what="surfels", tol=TOL):
 
 
 def check_seeds(got, want, tol=TOL, cluster_exact=True):
-    """Clustering state (x, y, mean_intensity, stable) must be bit-exact; plane-fit outputs within tol."""
+    """Clustering state (x, y, mean_intensity, stable, and mean_depth where the plane fit rejected the seed) must be
+    bit-exact; plane-fit outputs within tol."""
     assert len(got) == len(want)
     if cluster_exact:
         for f in ("x", "y", "mean_intensity"):
@@ -77,6 +78,12 @@ def check_seeds(got, want, tol=TOL, cluster_exact=True):
     zero_w = (nw == 0).all(1)
     zero_g = (ng == 0).all(1)
     assert (zero_w[ok] == zero_g[ok]).all(), f"plane-fit accept/reject differs at {np.nonzero(ok & (zero_w != zero_g))[0][:8]}"
+    # a seed the plane fit rejected keeps the mean_depth of the last Huber-Newton pass: clustering state, bit-exact
+    if cluster_exact:
+        rej = np.nonzero(ok & zero_w)[0]
+        bad = rej[~bits_equal_nan(got["mean_depth"][rej], want["mean_depth"][rej])]
+        assert len(bad) == 0, (f"seed.mean_depth of rejected seeds differs at {bad[:8]}: "
+                               f"got {got['mean_depth'][bad[:8]]} want {want['mean_depth'][bad[:8]]}")
     assert np.linalg.norm(ng[ok] - nw[ok], axis=1).max() <= tol, "seed normal error"
     pe = np.linalg.norm(pg[ok] - pw[ok], axis=1) / np.maximum(np.linalg.norm(pw[ok], axis=1), 1e-12)
     assert pe.max() <= tol, f"seed position error {pe.max():.3e}"
