@@ -210,6 +210,7 @@ extern "C" int dsm_create(const dsm_params *params, int device, void *cuda_strea
     if (e == cudaSuccess) e = ctx->own.host(&ctx->h_ofs, (size_t)B + 1);
     if (e == cudaSuccess) e = ctx->own.host(&ctx->h_ref, (size_t)2 * B);
     if (e == cudaSuccess) e = ctx->own.host(&ctx->h_win, 2 * ctx->win_len);
+    if (e == cudaSuccess) e = ctx->own.host(&ctx->h_sync, 8);
     int least = 0, greatest = 0;
     if (e == cudaSuccess) e = cudaDeviceGetStreamPriorityRange(&least, &greatest);
     if (e == cudaSuccess) e = ctx->own.stream(&ctx->s_hi, greatest);
@@ -827,25 +828,30 @@ static DsmDev resident_view(dsm_ctx *ctx, int slot)
     return d;
 }
 
-// The synchronisation point of dsm_fuse_stream_window's device-side state: after a windowed call, the pool size, the
-// store size, the segment table and the error word are known only on the device.  Waits for the stream, refreshes the
-// host bounds and the segment mirror, and reports (and clears) a rejected frame as DSM_E_CAPACITY.  A no-op when no
-// windowed call has run since the last one.
-static int res_sync(dsm_ctx *ctx)
+// The synchronisation point of the device-side state: after a window step, the pool size, the store size, the segment
+// table and the error word are known only on the device.  Waits for the stream, refreshes the host bounds and the
+// segment mirror, and reports (and clears) a rejected frame as DSM_E_CAPACITY.  A no-op when no window step has run
+// since the last one.  The first nseg_hint table entries are read with the header; only a longer table takes a second
+// round trip.
+static int res_sync(dsm_ctx *ctx, int nseg_hint = 0)
 {
     if (!ctx->win_pending) return DSM_OK;
     CK(cudaSetDevice(ctx->device));
-    int32_t h[4] = {0, 0, 0, 0}, hdr[4] = {0, 0, 0, 0};
-    CK(cudaMemcpyAsync(h, ctx->res_ofs, sizeof(h), cudaMemcpyDeviceToHost, ctx->stream));
-    CK(cudaMemcpyAsync(hdr, ctx->win_hdr, sizeof(hdr), cudaMemcpyDeviceToHost, ctx->stream));
+    int32_t *h = ctx->h_sync, *hdr = ctx->h_sync + 4; // pinned, so these copies do not wait for the stream one by one
+    std::vector<int4> t(ctx->inact ? (size_t)std::min(nseg_hint, ctx->inact_cap) : 0);
+    CK(cudaMemcpyAsync(h, ctx->res_ofs, 4 * sizeof(int32_t), cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaMemcpyAsync(hdr, ctx->win_hdr, 4 * sizeof(int32_t), cudaMemcpyDeviceToHost, ctx->stream));
+    if (!t.empty()) CK(cudaMemcpyAsync(t.data(), ctx->inact_seg.get(), t.size() * sizeof(int4), cudaMemcpyDeviceToHost, ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
     CK(cudaGetLastError());
     if (ctx->inact)
     {
-        std::vector<int4> t((size_t)hdr[1]);
-        if (hdr[1] > 0)
+        const size_t read = t.size();
+        t.resize((size_t)hdr[1]);
+        if (t.size() > read)
         {
-            CK(cudaMemcpyAsync(t.data(), ctx->inact_seg.get(), t.size() * sizeof(int4), cudaMemcpyDeviceToHost, ctx->stream));
+            CK(cudaMemcpyAsync(t.data() + read, ctx->inact_seg.get() + 4 * read, (t.size() - read) * sizeof(int4),
+                               cudaMemcpyDeviceToHost, ctx->stream));
             CK(cudaStreamSynchronize(ctx->stream));
         }
         ctx->inact_segs.clear();
@@ -862,22 +868,9 @@ static int res_sync(dsm_ctx *ctx)
     return DSM_E_CAPACITY;
 }
 
-// After host-side changes of the store (dsm_inactive_retire / _reactivate): the device table and header follow the
-// mirror, before the first windowed call that reads them.  Synchronises.
-static int inact_push(dsm_ctx *ctx)
-{
-    std::vector<int4> t;
-    for (const auto &g : ctx->inact_segs) t.push_back(make_int4(g.kf, g.ofs, g.cnt, 0));
-    const int32_t hdr[4] = {ctx->inact_size, (int32_t)t.size(), 0, 0};
-    if (!t.empty()) CK(cudaMemcpyAsync(ctx->inact_seg.get(), t.data(), t.size() * sizeof(int4), cudaMemcpyHostToDevice, ctx->stream));
-    CK(cudaMemcpyAsync(ctx->win_hdr, hdr, sizeof(hdr), cudaMemcpyHostToDevice, ctx->stream));
-    CK(cudaStreamSynchronize(ctx->stream));
-    ctx->inact_dev_stale = false;
-    return DSM_OK;
-}
-
-// the device-side view of the store and the window tables; `half` selects the staging half of the window lists
-static DsmWin window_view(dsm_ctx *ctx, int half, int t)
+// the device-side view of the store and the window tables; `half` selects the staging half of the window lists, S is
+// the room for new surfels the capacity check keeps in the pool (a fused frame's seeds; 0 for a step without a fuse)
+static DsmWin window_view(dsm_ctx *ctx, int half, int t, int S)
 {
     DsmWin w{};
     w.tab = ctx->d_win + (size_t)half * ctx->win_len;
@@ -891,8 +884,34 @@ static DsmWin window_view(dsm_ctx *ctx, int half, int t)
     w.blk_stride = ctx->win_blk_stride;
     w.pool_cap = ctx->p.max_local_surfels;
     w.store_cap = ctx->inact_cap;
-    w.S = ctx->d.S;
+    w.S = S;
     return w;
+}
+
+// The per-frame window lists of dsm_fuse_stream_window (a null offset array: empty lists)
+struct WinLists
+{
+    const int32_t *rk, *ro, *ak, *ao;
+};
+
+// The lists of n frames into staging half `half` (table layout: DsmWin), copied on `st` like the pose tables: the
+// device reads them when the window step runs, so a captured schedule never depends on their contents
+static int stage_window(dsm_ctx *ctx, int half, int n, const WinLists &w, int tag, cudaStream_t st)
+{
+    const int B = ctx->p.max_batch, KR = DSM_WIN_KEYS(B);
+    int32_t *h = ctx->h_win + (size_t)half * ctx->win_len;
+    for (int t = 0; t <= n; t++)
+    {
+        h[t] = w.ro ? w.ro[t] - w.ro[0] : 0;
+        h[B + 1 + t] = w.ao ? w.ao[t] - w.ao[0] : 0;
+    }
+    const int nr = h[n], na = h[B + 1 + n];
+    if (nr > 0) memcpy(h + KR, w.rk + w.ro[0], (size_t)nr * sizeof(int32_t));
+    if (na > 0) memcpy(h + KR + nr, w.ak + w.ao[0], (size_t)na * sizeof(int32_t));
+    h[2 * B + 2] = tag;
+    h[2 * B + 3] = KR + nr;
+    CK(cudaMemcpyAsync(ctx->d_win + (size_t)half * ctx->win_len, h, (size_t)(KR + nr + na) * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+    return DSM_OK;
 }
 
 extern "C" int dsm_pool_upload(dsm_ctx *ctx, const dsm_surfel_t *local, int n)
@@ -1106,11 +1125,6 @@ extern "C" int dsm_fuse_frame_resident(dsm_ctx *ctx, int ref_idx, const uint8_t 
 }
 
 // ---- inactive store (DESIGN.md section 8.2) ----
-// What SurfelMap keeps per pose in attached_surfels / inactive_pointcloud (surfel_map.cpp:1479-1497, :1583-1587,
-// :681-748), resident on the device.  The calls below orchestrate the pool kernels from the host, on the segment mirror:
-// retirement is the ordered compaction of dsm_pool_retire writing straight into the store, the per-pose warp is
-// k_pool_transform over one segment, the inactive cloud is k_pool_scatter<float4> over the store.  The window step of
-// dsm_fuse_stream_window does the same on the device-side table (dsm_launch_window_step).
 static DsmDev inactive_view(dsm_ctx *ctx)
 {
     DsmDev d = ctx->d;
@@ -1171,7 +1185,6 @@ extern "C" int dsm_inactive_reserve(dsm_ctx *ctx, int max_inactive_surfels)
     ctx->inact_cap = max_inactive_surfels;
     ctx->inact_upper = 0;
     ctx->inact_segs.clear();
-    ctx->inact_dev_stale = false; // header zeroed above
     return DSM_OK;
 }
 
@@ -1185,6 +1198,24 @@ extern "C" int dsm_inactive_size(dsm_ctx *ctx, int *n_surfels, int *n_segments)
     return DSM_OK;
 }
 
+// dsm_inactive_retire / _reactivate: the window step of one frame whose retire (or reactivation) list is {kf}, staged in
+// half 0.  The caller has synchronised the stream, into which both phases of stream_run are joined, so the half is free.
+// It has also checked capacity with exact sizes, so the step's own check cannot fail; S = 0, as no fuse follows.  No
+// window tag is drawn: the step leaves the error gate of the resident kernels as it is.  Waits for the step and
+// refreshes the mirror in the same round trip.
+static int inactive_step(dsm_ctx *ctx, int kf, bool react)
+{
+    const int32_t ofs[2] = {0, 1};
+    const WinLists w = react ? WinLists{nullptr, nullptr, &kf, ofs} : WinLists{&kf, ofs, nullptr, nullptr};
+    const int rc = stage_window(ctx, 0, 1, w, 0, ctx->stream);
+    if (rc != DSM_OK) return rc;
+    const int nseg = (int)ctx->inact_segs.size();
+    dsm_launch_window_step(resident_view(ctx, 0), window_view(ctx, 0, 0, 0), ctx->res_upper, react ? 0 : 1, react ? 1 : 0, ctx->stream);
+    CK(cudaGetLastError());
+    ctx->win_pending = true;
+    return res_sync(ctx, react ? nseg : nseg + 1);
+}
+
 // move_add_surfels, removal loop: local surfels last updated by keyframe kf -> a new segment of the store
 extern "C" int dsm_inactive_retire(dsm_ctx *ctx, int kf, int *n_moved)
 {
@@ -1195,19 +1226,10 @@ extern "C" int dsm_inactive_retire(dsm_ctx *ctx, int kf, int *n_moved)
     int rc = dsm_pool_size(ctx, &cur); // exact pool size: bounds the segment
     if (rc != DSM_OK) return rc;
     if (ctx->inact_size + cur > ctx->inact_cap) return DSM_E_CAPACITY;
-    dsm_launch_pool_retire(resident_view(ctx, 0), 0, ctx->res_upper, kf, ctx->blkcnt, ctx->blkofs, ctx->nsel, ctx->inact.get() + ctx->inact_size, ctx->stream);
-    int32_t h[1] = {0};
-    CK(cudaMemcpyAsync(h, ctx->nsel, sizeof(int32_t), cudaMemcpyDeviceToHost, ctx->stream));
-    CK(cudaStreamSynchronize(ctx->stream));
-    CK(cudaGetLastError());
-    if (h[0] > 0)
-    {
-        ctx->inact_segs.push_back(dsm_ctx::InactSeg{kf, ctx->inact_size, h[0]});
-        ctx->inact_size += h[0];
-    }
-    if (n_moved) *n_moved = h[0];
-    ctx->inact_upper = ctx->inact_size;
-    ctx->inact_dev_stale = true;
+    const int before = ctx->inact_size;
+    rc = inactive_step(ctx, kf, false);
+    if (rc != DSM_OK) return rc;
+    if (n_moved) *n_moved = ctx->inact_size - before;
     return DSM_OK;
 }
 
@@ -1228,64 +1250,19 @@ extern "C" int dsm_inactive_reactivate(dsm_ctx *ctx, int kf, int *n_moved)
     int rc = dsm_pool_size(ctx, &cur);
     if (rc != DSM_OK) return rc;
     if (cur + total > ctx->p.max_local_surfels) return DSM_E_CAPACITY;
-    cudaStream_t st = ctx->stream;
-    const int npool = ctx->p.max_local_surfels > 0 ? ctx->p.max_local_surfels : 1;
-    for (size_t i = 0; i < ctx->inact_segs.size();)
-    {
-        const dsm_ctx::InactSeg sg = ctx->inact_segs[i];
-        if (sg.kf != kf)
-        {
-            i++;
-            continue;
-        }
-        CK(cudaMemcpyAsync(ctx->d.pool + cur, ctx->inact.get() + sg.ofs, (size_t)sg.cnt * sizeof(dsm_surfel_t), cudaMemcpyDeviceToDevice, st));
-        cur += sg.cnt;
-        // close the gap: move the tail down through the second pool buffer, chunk by chunk
-        int src = sg.ofs + sg.cnt;
-        const int end = ctx->inact_size;
-        while (src < end)
-        {
-            const int len = (end - src) < npool ? (end - src) : npool;
-            CK(cudaMemcpyAsync(ctx->pool_snap, ctx->inact.get() + src, (size_t)len * sizeof(dsm_surfel_t), cudaMemcpyDeviceToDevice, st));
-            CK(cudaMemcpyAsync(ctx->inact.get() + src - sg.cnt, ctx->pool_snap, (size_t)len * sizeof(dsm_surfel_t), cudaMemcpyDeviceToDevice, st));
-            src += len;
-        }
-        ctx->inact_size -= sg.cnt;
-        ctx->inact_segs.erase(ctx->inact_segs.begin() + (long)i);
-        for (size_t j = i; j < ctx->inact_segs.size(); j++) ctx->inact_segs[j].ofs -= sg.cnt;
-    }
-    dsm_launch_set2(ctx->res_ofs, 0, cur, st);
-    CK(cudaStreamSynchronize(st));
-    CK(cudaGetLastError());
-    ctx->res_upper = cur;
-    ctx->inact_upper = ctx->inact_size;
-    ctx->inact_dev_stale = true;
-    return DSM_OK;
+    return inactive_step(ctx, kf, true);
 }
 
 // warp_inactive_surfels_cpu_kernel for ONE pose (surfel_map.cpp:704-733): p <- W p, n <- R_W n over its segment(s),
-// W = (T_loop * T_cam^-1) computed by the caller in fp64 and cast to float, column-major.  Asynchronous.
+// W = (T_loop * T_cam^-1) computed by the caller in fp64 and cast to float, column-major.  Asynchronous: the keyframe's
+// segments are found in the device table, in stream order.
 extern "C" int dsm_inactive_transform(dsm_ctx *ctx, int kf, const float Wm[16])
 {
     if (!ctx || !Wm) return DSM_E_INVALID;
     if (!ctx->inact) return DSM_E_STATE;
     CK(cudaSetDevice(ctx->device));
-    if (ctx->win_pending)
-    { // the mirror may be stale: the keyframe's segments are found on the device, in stream order
-        CK(cudaMemcpyAsync(ctx->wmat, Wm, 16 * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
-        dsm_launch_inactive_transform(window_view(ctx, 0, 0), kf, ctx->wmat, ctx->stream);
-        CK(cudaGetLastError());
-        return DSM_OK;
-    }
-    bool first = true;
-    for (const auto &sg : ctx->inact_segs)
-    {
-        if (sg.kf != kf) continue;
-        if (first) CK(cudaMemcpyAsync(ctx->wmat, Wm, 16 * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
-        first = false;
-        dsm_launch_set2(ctx->inact_ofs, sg.ofs, sg.ofs + sg.cnt, ctx->stream);
-        dsm_launch_pool_transform(inactive_view(ctx), 0, sg.cnt, ctx->wmat, ctx->stream);
-    }
+    CK(cudaMemcpyAsync(ctx->wmat, Wm, 16 * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
+    dsm_launch_inactive_transform(window_view(ctx, 0, 0, 0), kf, ctx->wmat, ctx->stream);
     CK(cudaGetLastError());
     return DSM_OK;
 }
@@ -1370,11 +1347,6 @@ extern "C" int dsm_inactive_export_poses(dsm_ctx *ctx, const int32_t *keyframes,
 // dsm_fuse_frame_resident: superpixels, normals and plane fits do not depend on the pose or the pool, so they run
 // for all n frames as one batch (full-width launches instead of n latency-bound single-frame ones); only the fuse /
 // initialise / post-step, which carry the pool from frame t to frame t+1, run frame by frame.
-// The per-frame window lists of dsm_fuse_stream_window (a null offset array: empty lists)
-struct WinLists
-{
-    const int32_t *rk, *ro, *ak, *ao;
-};
 static int list_len(const int32_t *o, int t) { return o ? o[t + 1] - o[t] : 0; }
 
 // Host-side validation of the lists (include/dsm.h); *any: some frame has a non-empty list
@@ -1411,26 +1383,6 @@ static int window_validate(const dsm_ctx *ctx, int n, const WinLists &w, bool *a
     return DSM_OK;
 }
 
-// The lists of n frames into staging half `half` (table layout: DsmWin), copied on `st` like the pose tables: the
-// device reads them when the window step runs, so a captured schedule never depends on their contents
-static int stage_window(dsm_ctx *ctx, int half, int n, const WinLists &w, int tag, cudaStream_t st)
-{
-    const int B = ctx->p.max_batch, KR = DSM_WIN_KEYS(B);
-    int32_t *h = ctx->h_win + (size_t)half * ctx->win_len;
-    for (int t = 0; t <= n; t++)
-    {
-        h[t] = w.ro ? w.ro[t] - w.ro[0] : 0;
-        h[B + 1 + t] = w.ao ? w.ao[t] - w.ao[0] : 0;
-    }
-    const int nr = h[n], na = h[B + 1 + n];
-    if (nr > 0) memcpy(h + KR, w.rk + w.ro[0], (size_t)nr * sizeof(int32_t));
-    if (na > 0) memcpy(h + KR + nr, w.ak + w.ao[0], (size_t)na * sizeof(int32_t));
-    h[2 * B + 2] = tag;
-    h[2 * B + 3] = KR + nr;
-    CK(cudaMemcpyAsync(ctx->d_win + (size_t)half * ctx->win_len, h, (size_t)(KR + nr + na) * sizeof(int32_t), cudaMemcpyHostToDevice, st));
-    return DSM_OK;
-}
-
 // dsm_fuse_stream_resident, and with `win` dsm_fuse_stream_window: each frame's window step runs right before its fuse
 static int stream_run(dsm_ctx *ctx, int n, const int32_t *ref_idx, const uint8_t *gray, const float *depth,
                       const float *poses, int32_t *n_new, const WinLists *win)
@@ -1446,11 +1398,6 @@ static int stream_run(dsm_ctx *ctx, int n, const int32_t *ref_idx, const uint8_t
     if (!ctx->res_active) return DSM_E_STATE;
     if (ctx->in_flight) return DSM_E_STATE;
     CK(cudaSetDevice(ctx->device));
-    if (win && ctx->inact && ctx->inact_dev_stale)
-    {
-        const int rp = inact_push(ctx);
-        if (rp != DSM_OK) return rp;
-    }
     // (the windowed call checks every frame on the device, with the counts only the device has)
     if (!win && ctx->res_upper + n * ctx->d.S > ctx->p.max_local_surfels)
     { // the bound may be loose: fetch the exact size before giving up
@@ -1545,7 +1492,7 @@ static int stream_run(dsm_ctx *ctx, int n, const int32_t *ref_idx, const uint8_t
             if (nr > 0 || na > 0 || ctx->res_upper + ctx->d.S > cap)
             {
                 const DsmDev dv = resident_view(ctx, slot0 + t);
-                dsm_launch_window_step(dv, window_view(ctx, par, t), dv.max_pool_per_frame, nr, na, s2);
+                dsm_launch_window_step(dv, window_view(ctx, par, t, ctx->d.S), dv.max_pool_per_frame, nr, na, s2);
             }
         }
         rc = enqueue_schedule(ctx, resident_view(ctx, slot0 + t), 1, s2, true, 2);

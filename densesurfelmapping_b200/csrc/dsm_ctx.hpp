@@ -134,7 +134,8 @@ struct dsm_ctx
     float *wmat = nullptr; // device copy of the 4x4 of dsm_pool_transform
     // inactive store (dsm_inactive_*): the attached_surfels of every pose outside the drift-free window, dense on the
     // device in retirement order.  The (keyframe, offset, count) segment table and the store size live on the device
-    // (inact_seg, win_hdr); inact_segs / inact_size mirror them, exactly unless win_pending
+    // (inact_seg, win_hdr), and only the window step changes them; inact_segs / inact_size mirror them, exactly unless
+    // win_pending, and only res_sync refreshes the mirror
     DevPtr<dsm_surfel_t> inact; // reallocated by dsm_inactive_reserve
     DevPtr<int32_t> inact_seg;  // int4 [inact_cap] (keyframe, offset, count, scratch): a stored segment holds >= 1 surfel
     int inact_cap = 0, inact_size = 0;
@@ -152,8 +153,7 @@ struct dsm_ctx
     DevPtr<int32_t> win_blk, win_sync;
     int win_blk_stride = 0;
     int win_tag = 0;          // tag of the latest windowed call (what a rejected frame writes into the error word)
-    bool win_pending = false; // a windowed call since the last synchronisation: mirrors stale, error word unread
-    bool inact_dev_stale = false; // dsm_inactive_retire / _reactivate changed the mirror: the device table follows it lazily
+    bool win_pending = false; // a window step since the last synchronisation: mirrors stale, error word unread
     cudaEvent_t ev_h2d[EV_COUNT] = {}, ev_done[EV_COUNT] = {}, ev_start = nullptr;
     cudaEvent_t ev_fork = nullptr, ev_join[4] = {}; // dsm_batch_run: fork / join of the concurrent sub-batches
     bool single_pending = false; // a dsm_fuse_frame_resident call since the last dsm_fuse_stream_resident (they share frame slots 0 / 1)
@@ -170,6 +170,7 @@ struct dsm_ctx
     float *h_pose = nullptr; // [2B][32]: pose then inverse; second half: dsm_fuse_stream_resident's own tables
     int32_t *h_ofs = nullptr;
     int32_t *h_ref = nullptr; // [2B], halves as h_pose
+    int32_t *h_sync = nullptr; // [8]: res_sync's readback of res_ofs and win_hdr
     // profiling
     uint32_t prof_mask = 0;
     std::vector<ProfRec> prof_pending;

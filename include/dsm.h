@@ -291,8 +291,8 @@ int dsm_frame_superpixel_image(dsm_ctx *ctx, int frame, uint8_t *bgr, size_t pit
  * What SurfelMap keeps per pose outside the drift-free window -- PoseElement::attached_surfels and the mirror
  * inactive_pointcloud (surfel_map.h:36-46) -- resident on the device next to the local pool, so that
  * move_add_surfels and the loop-closure warp of the inactive surfels never cross PCIe.  Segments are kept dense in
- * retirement order; the segment table lives on the device (dsm_fuse_stream_window updates it there), and the calls below
- * that synchronise refresh a host mirror of it.
+ * retirement order; the segment table lives on the device, where retirements and reactivations update it (the calls
+ * below and dsm_fuse_stream_window), and the calls below that synchronise refresh a host mirror of it.
  *   dsm_inactive_reserve      capacity in surfels (once, while the store is empty)
  *   dsm_inactive_retire       move_add_surfels removal loop (surfel_map.cpp:1479-1497): local surfels with
  *                             update_times > 0 and last_update == keyframe_index become that pose's segment (pool

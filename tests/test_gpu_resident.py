@@ -247,3 +247,46 @@ def test_inactive_store_round_trip():
     after = ctx.pool_download()
     assert len(after) == len(loc0) + len(seg1) and after[len(loc0):].tobytes() == seg1.tobytes()
     ctx.close()
+
+
+def test_inactive_capacity_errors_change_nothing():
+    """dsm_inactive_retire fails with DSM_E_CAPACITY when the store size plus the exact pool size exceeds the
+    reservation, dsm_inactive_reactivate when the pool size plus the keyframe's stored surfels exceeds max_local_surfels.
+    A rejected call leaves the pool, the store and both exports byte-identical, and the next call that fits succeeds."""
+    from densesurfelmapping_b200 import capi
+    rng = np.random.default_rng(11)
+    pool = np.zeros(300, SURFEL_DTYPE)
+    for f in ("px", "py", "pz", "nx", "ny", "nz", "size", "color", "weight"):
+        pool[f] = rng.standard_normal(len(pool))
+    pool["update_times"] = 3
+    pool["last_update"] = np.arange(len(pool)) % 3  # 100 surfels each of keyframes 0, 1, 2, interleaved
+
+    def state(ctx):
+        return (ctx.pool_download().tobytes(), ctx.inactive_download().tobytes(), ctx.inactive_size(),
+                ctx.inactive_export_cloud().tobytes(), ctx.inactive_export_poses([0, 1, 2]).tobytes())
+
+    def rejected(ctx, call, kf):
+        before = state(ctx)
+        with pytest.raises(capi.DsmError) as e:
+            call(kf)
+        assert e.value.code == -6
+        assert state(ctx) == before
+
+    def new_ctx(cap, store):
+        ctx = capi.Context(synth.VGA, max_batch=2, max_local_surfels=cap)
+        ctx.pool_upload(pool)
+        ctx.inactive_reserve(store)
+        assert ctx.inactive_retire(1) == 100
+        return ctx
+
+    ctx = new_ctx(400, 350)
+    rejected(ctx, ctx.inactive_retire, 0)          # 100 stored + 300 in the pool > 350
+    assert ctx.inactive_reactivate(1) == 100       # 300 + 100 <= 400
+    assert ctx.inactive_size() == (0, 0) and ctx.pool_size() == 400
+    ctx.close()
+    ctx = new_ctx(399, 400)
+    rejected(ctx, ctx.inactive_reactivate, 1)      # 300 in the pool + 100 stored > 399
+    assert ctx.inactive_retire(0) == 100           # 100 + 300 <= 400
+    assert ctx.inactive_size() == (200, 2)
+    assert ctx.inactive_download().tobytes() == np.concatenate([pool[pool["last_update"] == k] for k in (1, 0)]).tobytes()
+    ctx.close()

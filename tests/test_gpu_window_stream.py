@@ -264,11 +264,12 @@ def ros7_to_matrix(p7):
 
 
 @pytest.mark.skipif(not pyoracle_window.have_refmap_window(b200=True), reason="libdsm_refmap_window_b200.so not built")
-@pytest.mark.parametrize("chunk", [1, 4])
+@pytest.mark.parametrize("chunk", [1, 4, "per_call"])
 def test_product_equals_the_reference_node(chunk):
     """The reference node over the product (its own move_add_surfels and host post-step, the product's fuse kernels)
     against dsm_fuse_stream_window fed with the fuse poses and window lists that node used: local_surfels slot for slot,
-    attached_surfels and inactive_pointcloud byte for byte."""
+    attached_surfels and inactive_pointcloud byte for byte.  "per_call": the same frames through dsm_inactive_retire /
+    dsm_inactive_reactivate / dsm_fuse_frame_resident, one call each."""
     m = pyoracle_window.RefMapWindow(CAM, drift_free_poses=2, b200=True)
     path, last_kf, rec = [], 0, []
     for t in range(T):
@@ -286,11 +287,19 @@ def test_product_equals_the_reference_node(chunk):
         rec.append(pending)
     assert any(r for _, _, r, _ in rec) and any(a for _, _, _, a in rec)
     ctx = new_ctx()
-    for t0 in range(0, T, chunk):
-        part = rec[t0:t0 + chunk]
-        fr = frames()[t0:t0 + chunk]
-        ctx.fuse_stream_window([r[0] for r in part], np.stack([f[1] for f in fr]), np.stack([f[2] for f in fr]),
-                               np.stack([r[1] for r in part]), [r[2] for r in part], [r[3] for r in part])
+    if chunk == "per_call":
+        for (ref, pose, rem, add), (_, gray, depth) in zip(rec, frames()):
+            for kf in rem:
+                ctx.inactive_retire(kf)
+            for kf in add:
+                ctx.inactive_reactivate(kf)
+            ctx.fuse_frame_resident(ref, gray, depth, pose)
+    else:
+        for t0 in range(0, T, chunk):
+            part = rec[t0:t0 + chunk]
+            fr = frames()[t0:t0 + chunk]
+            ctx.fuse_stream_window([r[0] for r in part], np.stack([f[1] for f in fr]), np.stack([f[2] for f in fr]),
+                                   np.stack([r[1] for r in part]), [r[2] for r in part], [r[3] for r in part])
     assert ctx.pool_download().tobytes() == m.local().tobytes()
     for p in range(m.num_poses()):
         assert ctx.inactive_download(p).tobytes() == m.attached(p).tobytes(), f"attached_surfels of pose {p}"
