@@ -22,18 +22,24 @@ sys.path.insert(0, os.path.dirname(HERE))
 from densesurfelmapping_b200.elements import SEED_DTYPE, SURFEL_DTYPE, num_seeds  # noqa: E402
 
 
-def build(verbose=False):
-    """Build the restatement (always) and the reference variants (when the reference sources exist, see oracle/Makefile)."""
-    r = subprocess.run(["make", "-C", HERE, "all"], capture_output=True, text=True)
+def build(force=False, verbose=False):
+    """Build every oracle library that is out of date, or all of them with force=True: the restatement always, the
+    reference variants when the reference sources exist (see oracle/Makefile)."""
+    r = subprocess.run(["make", "-C", HERE, "all"] + (["-B"] if force else []), capture_output=True, text=True)
     if verbose or r.returncode != 0:
         print(r.stdout, r.stderr)
     if r.returncode != 0:
         raise RuntimeError("oracle build failed")
 
 
+def have(libname):
+    """Whether oracle/_ref/<libname> is built."""
+    return os.path.exists(os.path.join(REFDIR, libname))
+
+
 def _lib(name):
     path = os.path.join(REFDIR, name)
-    if not os.path.exists(path):
+    if not have(name):
         build()
     if not os.path.exists(path):
         raise FileNotFoundError(path)
@@ -269,7 +275,7 @@ def pcd_text(points):
 
 # ---- the reference's whole SurfelMap, compiled in place (oracle/ref_map_driver.cpp) ----
 def have_refmap(b200=False):
-    return os.path.exists(os.path.join(REFDIR, "libdsm_refmap_b200.so" if b200 else "libdsm_refmap.so"))
+    return have(RefMap.libname_b200 if b200 else RefMap.libname)
 
 
 def pose_to_ros7(pose_colmajor16):
@@ -285,10 +291,12 @@ class RefMap:
     """SurfelMap of the reference (surfel_fusion/src/surfel_map.cpp) behind oracle/ref_map_driver.cpp.
     b200=False: with the reference's own FusionFunctions (threads inlined: deterministic) -- the system-level oracle.
     b200=True : the same SurfelMap holding the product's dsm::FusionFunctions (INTEGRATION.md's patch); needs a GPU."""
+    libname = "libdsm_refmap.so"
+    libname_b200 = "libdsm_refmap_b200.so"
 
     def __init__(self, cam, drift_free_poses=10, b200=False):
         vp, ci, cf, cd = ctypes.c_void_p, ctypes.c_int, ctypes.c_float, ctypes.c_double
-        self.lib = L = _lib("libdsm_refmap_b200.so" if b200 else "libdsm_refmap.so")
+        self.lib = L = _lib(self.libname_b200 if b200 else self.libname)
         self.cam = cam
         L.dsmmap_create.restype = vp
         L.dsmmap_create.argtypes = [ci, ci, cf, cf, cf, cf, cf, cf, ci]
@@ -404,7 +412,7 @@ class RefMap:
 
 
 def have_reference():
-    return os.path.exists(os.path.join(REFDIR, "libdsm_ref_serial.so"))
+    return have(RefSerial.libname)
 
 
 # ---- comparison metrics (SURVEY.md §7 H5: norm-based, not per-component relative) ----

@@ -2,31 +2,18 @@
 tests/test_gpu_node_clouds.py.
 
   raw_cloud       publish_raw_pointcloud (surfel_map.cpp:1115-1151) restated in numpy float32, operation by operation
-  RefMapClouds    pyoracle.RefMap over oracle/_ref/libdsm_refmap_clouds.so (oracle/clouds.mk, ref_map_clouds.cpp): the
+  RefMapClouds    pyoracle.RefMap over oracle/_ref/libdsm_refmap_clouds.so (oracle/Makefile, ref_map_clouds.cpp): the
                   reference's SurfelMap with two more hooks, publish_raw() and driftfree_poses()
 """
 import ctypes
-import os
-import subprocess
 
 import numpy as np
 
 import pyoracle
 
-LIBNAME = "libdsm_refmap_clouds.so"
-
-
-def build(verbose=False):
-    """Build libdsm_refmap_clouds.so where the reference sources exist (see oracle/clouds.mk)."""
-    r = subprocess.run(["make", "-C", pyoracle.HERE, "-f", "clouds.mk", "clouds"], capture_output=True, text=True)
-    if verbose or r.returncode != 0:
-        print(r.stdout, r.stderr)
-    if r.returncode != 0:
-        raise RuntimeError("oracle build failed (clouds.mk)")
-
 
 def have_refmap_clouds():
-    return os.path.exists(os.path.join(pyoracle.REFDIR, LIBNAME))
+    return pyoracle.have(RefMapClouds.libname)
 
 
 def raw_rotation(pose7):
@@ -65,19 +52,11 @@ def raw_cloud(cam, gray, depth, pose7):
 class RefMapClouds(pyoracle.RefMap):
     """pyoracle.RefMap (the reference's SurfelMap, its own CPU FusionFunctions) loaded from libdsm_refmap_clouds.so,
     which adds publish_raw() and driftfree_poses()."""
+    libname = "libdsm_refmap_clouds.so"
 
     def __init__(self, cam, drift_free_poses=10):
-        path = os.path.join(pyoracle.REFDIR, LIBNAME)
-        if not os.path.exists(path):
-            build()
-        lib = ctypes.CDLL(path)
-        # RefMap.__init__ resolves its library through pyoracle._lib: hand it this one
-        load = pyoracle._lib
-        pyoracle._lib = lambda name: lib
-        try:
-            super().__init__(cam, drift_free_poses)
-        finally:
-            pyoracle._lib = load
+        super().__init__(cam, drift_free_poses)
+        lib = self.lib
         vp, ci = ctypes.c_void_p, ctypes.c_int
         lib.dsmmap_publish_raw.argtypes = [vp, vp, vp, vp]
         lib.dsmmap_driftfree_poses.argtypes = [vp, ci, ci, vp, ci]

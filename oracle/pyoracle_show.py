@@ -2,32 +2,19 @@
 for tests/test_superpixel_image.py and tests/test_gpu_superpixel_image.py.
 
   superpixel_image  debug_show restated in numpy: the exact double product and the reference build's uchar conversion
-  RefShow           the serial reference (pyoracle.RefSerial) loaded from oracle/_ref/libdsm_ref_show.so (oracle/show.mk,
+  RefShow           the serial reference (pyoracle.RefSerial) loaded from oracle/_ref/libdsm_ref_show.so (oracle/Makefile,
                     ref_debug_show.cpp), which adds debug_show(): the image the reference hands to cv::imshow
 """
 import ctypes
-import os
-import subprocess
 
 import numpy as np
 
 import pyoracle
 from densesurfelmapping_b200.elements import SEED_DTYPE
 
-LIBNAME = "libdsm_ref_show.so"
-
-
-def build(verbose=False):
-    """Build libdsm_ref_show.so where the reference sources exist (see oracle/show.mk)."""
-    r = subprocess.run(["make", "-C", pyoracle.HERE, "-f", "show.mk", "show"], capture_output=True, text=True)
-    if verbose or r.returncode != 0:
-        print(r.stdout, r.stderr)
-    if r.returncode != 0:
-        raise RuntimeError("oracle build failed (show.mk)")
-
 
 def have_ref_show():
-    return os.path.exists(os.path.join(pyoracle.REFDIR, LIBNAME))
+    return pyoracle.have(RefShow.libname)
 
 
 def channel(n):
@@ -58,11 +45,9 @@ def superpixel_image(labels, seeds):
 class RefShow(pyoracle._Base):
     """The serial reference with a debug_show hook: superpixels() / fuse() as pyoracle.RefSerial, then debug_show()."""
     prefix = "dsmref_"
-    libname = LIBNAME
+    libname = "libdsm_ref_show.so"
 
     def __init__(self, cam):
-        if not have_ref_show():
-            build()
         super().__init__(cam)
         self.lib.dsmref_debug_show.argtypes = [ctypes.c_void_p] * 4
         self.lib.dsmref_debug_show.restype = ctypes.c_int

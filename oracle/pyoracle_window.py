@@ -3,12 +3,10 @@ for tests/test_window_step.py and tests/test_gpu_window_stream.py.
 
   WindowModel     the window step restated in numpy on the three things the device keeps: the pool (local_surfels), the
                   inactive store (every pose's attached_surfels, dense in retirement order) and its segment list
-  RefMapWindow    pyoracle.RefMap over oracle/_ref/libdsm_refmap_window[_b200].so (oracle/window.mk, ref_map_window.cpp):
+  RefMapWindow    pyoracle.RefMap over oracle/_ref/libdsm_refmap_window[_b200].so (oracle/Makefile, ref_map_window.cpp):
                   the reference's SurfelMap with three more hooks, window_lists(), pending_frame() and images()
 """
 import ctypes
-import os
-import subprocess
 
 import numpy as np
 
@@ -16,21 +14,8 @@ import pyoracle
 from pyoracle import SURFEL_DTYPE
 
 
-def build(verbose=False):
-    """Build libdsm_refmap_window[_b200].so where the reference sources exist (see oracle/window.mk)."""
-    r = subprocess.run(["make", "-C", pyoracle.HERE, "-f", "window.mk", "window"], capture_output=True, text=True)
-    if verbose or r.returncode != 0:
-        print(r.stdout, r.stderr)
-    if r.returncode != 0:
-        raise RuntimeError("oracle build failed (window.mk)")
-
-
-def libname(b200=False):
-    return "libdsm_refmap_window_b200.so" if b200 else "libdsm_refmap_window.so"
-
-
 def have_refmap_window(b200=False):
-    return os.path.exists(os.path.join(pyoracle.REFDIR, libname(b200)))
+    return pyoracle.have(RefMapWindow.libname_b200 if b200 else RefMapWindow.libname)
 
 
 def cloud(surfels):
@@ -81,18 +66,12 @@ class WindowModel:
 class RefMapWindow(pyoracle.RefMap):
     """pyoracle.RefMap loaded from libdsm_refmap_window[_b200].so, which adds window_lists(), pending_frame() and
     images().  b200=True: the node over the product adapter (needs a GPU)."""
+    libname = "libdsm_refmap_window.so"
+    libname_b200 = "libdsm_refmap_window_b200.so"
 
     def __init__(self, cam, drift_free_poses=10, b200=False):
-        path = os.path.join(pyoracle.REFDIR, libname(b200))
-        if not os.path.exists(path):
-            build()
-        lib = ctypes.CDLL(path)
-        load = pyoracle._lib
-        pyoracle._lib = lambda name: lib  # RefMap.__init__ resolves its library through pyoracle._lib
-        try:
-            super().__init__(cam, drift_free_poses)
-        finally:
-            pyoracle._lib = load
+        super().__init__(cam, drift_free_poses, b200)
+        lib = self.lib
         vp, ci = ctypes.c_void_p, ctypes.c_int
         lib.dsmmap_window_lists.argtypes = [vp, ci, vp, vp, vp, vp, ci]
         lib.dsmmap_window_lists.restype = None

@@ -1,7 +1,7 @@
 // TEST INFRASTRUCTURE ONLY.  The serial reference oracle of ref_driver.cpp (the reference's own fusion_functions.cpp
 // compiled in place, thread bodies inline) with one more hook, for FusionFunctions::debug_show (fusion_functions.cpp:
 // 977-1006), the superpixel normal image the reference draws and hands to cv::imshow.  Built into
-// oracle/_ref/libdsm_ref_show.so by oracle/show.mk against oracle/shim_show, whose imshow keeps the last image shown;
+// oracle/_ref/libdsm_ref_show.so by oracle/Makefile against oracle/shim_show, whose imshow keeps the last image shown;
 // every entry point of libdsm_ref_serial.so is exported too.
 #include "ref_driver.cpp"
 

@@ -1,7 +1,7 @@
 // TEST INFRASTRUCTURE ONLY.  The SurfelMap oracle of ref_map_driver.cpp (the reference's own surfel_map.cpp compiled in
 // place) with two more hooks, for the node's two remaining cloud publishers: publish_raw_pointcloud itself, and the
 // drift-free BFS (get_driftfree_poses) that publish_neighbor_pointcloud walks.  Built into
-// oracle/_ref/libdsm_refmap_clouds.so by oracle/clouds.mk; every entry point of libdsm_refmap.so is exported too.
+// oracle/_ref/libdsm_refmap_clouds.so by oracle/Makefile; every entry point of libdsm_refmap.so is exported too.
 #include "ref_map_driver.cpp"
 
 extern "C"

@@ -1,7 +1,7 @@
 // TEST INFRASTRUCTURE ONLY.  The SurfelMap oracle of ref_map_driver.cpp (the reference's own surfel_map.cpp compiled in
 // place) with three more hooks for the node's per-frame window step (move_add_surfels, surfel_map.cpp:1458-1595): the
 // lists get_add_remove_poses hands it, the fuse pose synchronize_msgs hands fuse_map, and the image callbacks alone.  Built into
-// oracle/_ref/libdsm_refmap_window[_b200].so by oracle/window.mk; every entry point of libdsm_refmap.so is exported too.
+// oracle/_ref/libdsm_refmap_window[_b200].so by oracle/Makefile; every entry point of libdsm_refmap.so is exported too.
 #include "ref_map_driver.cpp"
 
 static int copy_list(const std::vector<int> &v, int *out, int cap)

@@ -1,5 +1,5 @@
 // TEST INFRASTRUCTURE ONLY (oracle build).  oracle/shim/opencv2/opencv.hpp with an observable cv::imshow: placed before
-// oracle/shim on the include path (oracle/show.mk), it includes that stand-in with its no-op imshow renamed away and
+// oracle/shim on the include path (oracle/Makefile), it includes that stand-in with its no-op imshow renamed away and
 // defines an imshow that keeps a deep copy of the last image shown, so that a driver can read what the reference's
 // debug_show() (fusion_functions.cpp:977-1006) displays.  No other oracle library is built with this directory.
 #pragma once

@@ -62,7 +62,7 @@ def stream_checksums(cam, n, flat):
 
 
 def main():
-    assert pyoracle.have_reference(), "needs oracle/_ref/libdsm_ref_serial.so (make -C oracle ref)"
+    assert pyoracle.have_reference(), "needs oracle/_ref/libdsm_ref_serial.so (make -C oracle)"
     cam = synth.VGA
     g, d = synth.make_frame(cam, 0)
     pose = synth.identity_pose()

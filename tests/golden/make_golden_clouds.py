@@ -1,5 +1,5 @@
 """Mints tests/golden/raw_cloud_checksums.json: the CRC32 of what the reference's own publish_raw_pointcloud
-(surfel_map.cpp:1115-1151, compiled in place: oracle/_ref/libdsm_refmap_clouds.so, see oracle/clouds.mk) publishes for
+(surfel_map.cpp:1115-1151, compiled in place: oracle/_ref/libdsm_refmap_clouds.so, see oracle/Makefile) publishes for
 the cases of tests/test_node_clouds.py::raw_cases, so that the numpy restatement is pinned on a checkout without it.
 Run where oracle/_ref/ holds that build:  python tests/golden/make_golden_clouds.py
 """
@@ -18,7 +18,7 @@ from test_oracle import crc  # noqa: E402
 
 
 def main():
-    assert pyoracle_clouds.have_refmap_clouds(), "needs oracle/_ref/libdsm_refmap_clouds.so (make -C oracle -f clouds.mk clouds)"
+    assert pyoracle_clouds.have_refmap_clouds(), "needs oracle/_ref/libdsm_refmap_clouds.so (make -C oracle)"
     sums = {}
     for name, (cam, gray, depth, p7) in test_node_clouds.raw_cases().items():
         m = pyoracle_clouds.RefMapClouds(cam)

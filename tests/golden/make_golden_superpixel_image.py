@@ -1,5 +1,5 @@
 """Mints tests/golden/superpixel_image_checksums.json: the CRC32 of the image the reference's own debug_show
-(fusion_functions.cpp:977-1006, compiled in place: oracle/_ref/libdsm_ref_show.so, see oracle/show.mk) draws for the
+(fusion_functions.cpp:977-1006, compiled in place: oracle/_ref/libdsm_ref_show.so, see oracle/Makefile) draws for the
 cases of tests/test_superpixel_image.py::image_cases, so that the numpy restatement is pinned on a checkout without it.
 Run where oracle/_ref/ holds that build:  python tests/golden/make_golden_superpixel_image.py
 """
@@ -18,7 +18,7 @@ from test_oracle import crc  # noqa: E402
 
 
 def main():
-    assert pyoracle_show.have_ref_show(), "needs oracle/_ref/libdsm_ref_show.so (make -C oracle -f show.mk show)"
+    assert pyoracle_show.have_ref_show(), "needs oracle/_ref/libdsm_ref_show.so (make -C oracle)"
     sums = {}
     for name, (cam, gray, depth) in test_superpixel_image.image_cases().items():
         m = pyoracle_show.RefShow(cam)
