@@ -220,13 +220,12 @@ extern "C" int dsm_create(const dsm_params *params, int device, void *cuda_strea
         if (e == cudaSuccess) e = ctx->own.stream(&s);
     for (cudaEvent_t *ev : {&ctx->ev_start, &ctx->ev_fork, &ctx->ev_p2})
         if (e == cudaSuccess) e = ctx->own.event(ev);
-    for (cudaEvent_t &ev : ctx->ev_join)
-        if (e == cudaSuccess) e = ctx->own.event(&ev);
-    for (int i = 0; i < EV_COUNT; i++)
-    {
-        if (e == cudaSuccess) e = ctx->own.event(&ctx->ev_h2d[i]);
-        if (e == cudaSuccess) e = ctx->own.event(&ctx->ev_done[i]);
-    }
+    for (int i = 0; i < DSM_MAX_CHUNKS; i++)
+        for (cudaEvent_t *ev : {&ctx->ev_join[i], &ctx->ev_h2d[i], &ctx->ev_done[i]})
+            if (e == cudaSuccess) e = ctx->own.event(ev);
+    for (int h = 0; h < 2; h++)
+        for (cudaEvent_t *ev : {&ctx->half_h2d[h], &ctx->half_free[h]})
+            if (e == cudaSuccess) e = ctx->own.event(ev);
     if (e == cudaSuccess)
     { // back-projection factor tables: the same float ops as back_project (fusion_functions.cpp:94-95)
         std::vector<float> hx((size_t)Wp + 16), hy((size_t)H + 16);
@@ -500,12 +499,13 @@ static int launch_schedule(dsm_ctx *ctx, const DsmDev &d, int nb, cudaStream_t s
     return DSM_OK;
 }
 
-// Enqueue the schedule for the view `v` (frames [v.frame0, v.frame0 + nf)), followed, when `post` is set, by the
-// resident pool's fuse_map post-step (in place, slot for slot as the reference).
+// Enqueue the schedule for the view `v` (frames [v.frame0, v.frame0 + nf)).  Phase 2 (the resident stream's fuse /
+// initialise on its pool) ends with the pool's fuse_map post-step (in place, slot for slot as the reference); phase 3
+// (the batch calls) and phase 1 have none.
 // The 14-18 launches are captured once per distinct parameter set into a CUDA graph and replayed: the
 // per-launch CPU cost and inter-kernel gaps matter for single frames and small chunks.  Profiling
 // (event pairs around kernels) and the debug kernel budget use plain launches.
-static int enqueue_schedule(dsm_ctx *ctx, const DsmDev &v, int nf, cudaStream_t st, bool post = false, int phase = 3)
+static int enqueue_schedule(dsm_ctx *ctx, const DsmDev &v, int nf, cudaStream_t st, int phase = 3)
 {
     // grids over the pool are sized from max_pool_per_frame rounded up to 4 Ki surfels (the kernels take the true
     // ranges from poolofs on the device, surplus blocks exit at once), so that callers whose pool size
@@ -516,7 +516,7 @@ static int enqueue_schedule(dsm_ctx *ctx, const DsmDev &v, int nf, cudaStream_t 
     {
         int rc = launch_schedule(ctx, d, nf, st, phase);
         if (rc != DSM_OK) return rc;
-        if (post)
+        if (phase == 2)
             dsm_launch_pool_recycle(d, d.frame0, d.max_pool_per_frame, ctx->blkcnt, ctx->blkofs, ctx->nsel, ctx->holes, ctx->rc_src,
                                     ctx->rc_sync, ctx->res_ofs, st);
         return DSM_OK;
@@ -524,7 +524,7 @@ static int enqueue_schedule(dsm_ctx *ctx, const DsmDev &v, int nf, cudaStream_t 
     if (!ctx->use_graphs || ctx->prof_mask != 0 || ctx->stop_after > 0) return plain();
     for (auto &g : ctx->graphs)
         if (g.f0 == d.frame0 && g.nf == nf && g.maxper == d.max_pool_per_frame && g.pool == d.pool && g.poolofs == d.poolofs &&
-            g.gate == d.gate && g.post == post && g.phase == phase)
+            g.gate == d.gate && g.phase == phase)
         {
             CK(cudaGraphLaunch(g.exec.get(), st));
             return DSM_OK;
@@ -554,7 +554,7 @@ static int enqueue_schedule(dsm_ctx *ctx, const DsmDev &v, int nf, cudaStream_t 
         return plain();
     }
     if (ctx->graphs.size() >= 64) ctx->graphs.erase(ctx->graphs.begin()); // bounded cache
-    ctx->graphs.push_back(GraphEntry{d.frame0, nf, d.max_pool_per_frame, phase, d.pool, d.poolofs, d.gate, post, GraphExecPtr(exec)});
+    ctx->graphs.push_back(GraphEntry{d.frame0, nf, d.max_pool_per_frame, phase, d.pool, d.poolofs, d.gate, GraphExecPtr(exec)});
     CK(cudaGraphLaunch(exec, st));
     return DSM_OK;
 }
@@ -722,11 +722,11 @@ extern "C" int dsm_fuse_batch_async(dsm_ctx *ctx, int n, const int32_t *ref, con
         CK(cudaMemcpyAsync(ctx->depth_packed + (size_t)f0 * fpx, depth + (size_t)f0 * fpx, (size_t)nf * fpx * sizeof(float), cudaMemcpyHostToDevice, ctx->s_h2d));
         if (p1 > p0)
             CK(cudaMemcpyAsync(ctx->d.pool + p0, local + p0, (size_t)(p1 - p0) * sizeof(dsm_surfel_t), cudaMemcpyHostToDevice, ctx->s_h2d));
-        CK(cudaEventRecord(ctx->ev_h2d[EV_CHUNK + nc], ctx->s_h2d));
+        CK(cudaEventRecord(ctx->ev_h2d[nc], ctx->s_h2d));
         // kernels: each chunk on its own compute stream, so the latency-bound per-seed kernels of one
         // chunk overlap the wide kernels of its neighbours instead of leaving SMs idle
         cudaStream_t cs = nchunks > 1 ? ctx->s_comp[nc] : ctx->stream;
-        CK(cudaStreamWaitEvent(cs, ctx->ev_h2d[EV_CHUNK + nc], 0));
+        CK(cudaStreamWaitEvent(cs, ctx->ev_h2d[nc], 0));
         DsmDev v = ctx->d; // batch view of this chunk
         v.frame0 = f0;
         v.max_pool_per_frame = maxper;
@@ -736,9 +736,9 @@ extern "C" int dsm_fuse_batch_async(dsm_ctx *ctx, int n, const int32_t *ref, con
         }
         rc = enqueue_schedule(ctx, v, nf, cs);
         if (rc != DSM_OK) return rc;
-        CK(cudaEventRecord(ctx->ev_done[EV_CHUNK + nc], cs));
+        CK(cudaEventRecord(ctx->ev_done[nc], cs));
         // D2H of this chunk
-        CK(cudaStreamWaitEvent(ctx->s_d2h, ctx->ev_done[EV_CHUNK + nc], 0));
+        CK(cudaStreamWaitEvent(ctx->s_d2h, ctx->ev_done[nc], 0));
         if (p1 > p0)
             CK(cudaMemcpyAsync(local + p0, ctx->d.pool + p0, (size_t)(p1 - p0) * sizeof(dsm_surfel_t), cudaMemcpyDeviceToHost, ctx->s_d2h));
         if (new_out)
@@ -811,8 +811,8 @@ extern "C" int dsm_fuse_frame(dsm_ctx *ctx, int ref_idx, const uint8_t *gray, si
 }
 
 // ---- GPU-resident pool (stream mode) ----
-// The resident pool is described by res_ofs = {0, n} on the device.  Frames alternate between two
-// frame slots (when max_batch >= 2) so that the H2D copy of frame t+1 overlaps the kernels of frame t.
+// The resident pool is described by res_ofs = {0, n} on the device; its frames run in the frame slots of the staging
+// half their call uses (stream_run).
 // The view of frame slot `slot`: grids over the pool are sized from its upper bound rounded up to 64 Ki surfels and
 // clamped to the capacity, so that the captured graph stays valid while the pool grows (surplus blocks exit at once:
 // the kernels read the true range from the device).
@@ -1053,77 +1053,6 @@ extern "C" int dsm_pool_transform(dsm_ctx *ctx, const float Wm[16])
     return DSM_OK;
 }
 
-extern "C" int dsm_fuse_frame_resident(dsm_ctx *ctx, int ref_idx, const uint8_t *gray, size_t gray_pitch,
-                                       const float *depth, size_t depth_pitch, const float pose[16], int *n_new)
-{
-    if (!ctx || !gray || !depth || !pose) return DSM_E_INVALID;
-    if (!ctx->res_active) return DSM_E_STATE;
-    const int W = ctx->p.width, H = ctx->p.height;
-    if (gray_pitch < (size_t)W || depth_pitch < (size_t)W * 4) return DSM_E_INVALID;
-    CK(cudaSetDevice(ctx->device));
-    if (ctx->res_upper + ctx->d.S > ctx->p.max_local_surfels)
-    { // the bound may be loose: fetch the exact size before giving up
-        int n = 0;
-        int rc = dsm_pool_size(ctx, &n);
-        if (rc != DSM_OK) return rc;
-        if (n + ctx->d.S > ctx->p.max_local_surfels) return DSM_E_CAPACITY;
-    }
-    const int nslots = ctx->p.max_batch >= 2 ? 2 : 1;
-    const int slot = ctx->res_frame % nslots;
-    ctx->res_frame++;
-    const size_t fpx = (size_t)H * W;
-    // this slot's pinned tables / image buffers were last used two frames ago: make sure that copy and
-    // those kernels are done (normally long finished, so these do not stall)
-    CK(cudaEventSynchronize(ctx->ev_h2d[EV_SLOT + slot]));
-    CK(cudaStreamWaitEvent(ctx->s_h2d, ctx->ev_done[EV_SLOT + slot], 0));
-    const int32_t ref = ref_idx;
-    int rc = stage_tables(ctx, slot, slot, 1, pose, &ref, ctx->s_h2d); // pinned row = frame slot, in the first half
-    if (rc != DSM_OK) return rc;
-    const bool packed = gray_pitch == (size_t)W && depth_pitch == (size_t)W * 4;
-    if (packed)
-    { // one contiguous copy per image, repacked to the pitched layout on the device
-        CK(cudaMemcpyAsync(ctx->gray_packed + (size_t)slot * fpx, gray, fpx, cudaMemcpyHostToDevice, ctx->s_h2d));
-        CK(cudaMemcpyAsync(ctx->depth_packed + (size_t)slot * fpx, depth, fpx * sizeof(float), cudaMemcpyHostToDevice, ctx->s_h2d));
-    }
-    else
-    {
-        CK(cudaMemcpy2DAsync(ctx->gray + (size_t)slot * ctx->d.px_stride, ctx->d.Wp, gray, gray_pitch, W, H, cudaMemcpyHostToDevice, ctx->s_h2d));
-        CK(cudaMemcpy2DAsync(ctx->depth + (size_t)slot * ctx->d.px_stride, (size_t)ctx->d.Wp * 4, depth, depth_pitch, (size_t)W * 4, H, cudaMemcpyHostToDevice, ctx->s_h2d));
-    }
-    CK(cudaEventRecord(ctx->ev_h2d[EV_SLOT + slot], ctx->s_h2d));
-    CK(cudaStreamWaitEvent(ctx->stream, ctx->ev_h2d[EV_SLOT + slot], 0));
-    const DsmDev dv = resident_view(ctx, slot);
-    if (packed)
-    {
-        ProfScope p(ctx, DSM_K_REPACK);
-        dsm_launch_repack(dv, 1, ctx->gray_packed + (size_t)slot * fpx, ctx->depth_packed + (size_t)slot * fpx, ctx->stream);
-    }
-    ctx->nb = slot + 1;
-    ctx->uploaded = true;
-    ctx->img_slot0 = slot, ctx->img_n = 1, ctx->img_fit = false;
-    // + post-step of SurfelMap::fuse_map on the device, in place
-    rc = enqueue_schedule(ctx, dv, 1, ctx->stream, true);
-    if (rc != DSM_OK) return rc;
-    ctx->ran = true;
-    ctx->img_fit = schedule_fits(ctx);
-    CK(cudaEventRecord(ctx->ev_done[EV_SLOT + slot], ctx->stream)); // (the post-step's last kernel stored the new pool size in res_ofs[1])
-    ctx->single_pending = true;
-    ctx->res_upper += ctx->d.S; // every seed can add at most one surfel; dsm_pool_size() tightens it
-    CK(cudaGetLastError());
-    // the caller may reuse its image buffers as soon as we return: wait for THIS frame's copy only
-    // (the kernels keep running and overlap the next call's copy)
-    CK(cudaEventSynchronize(ctx->ev_h2d[EV_SLOT + slot]));
-    if (n_new)
-    {
-        int32_t c = 0;
-        CK(cudaMemcpyAsync(&c, ctx->d.nnew + slot, sizeof(int32_t), cudaMemcpyDeviceToHost, ctx->stream));
-        CK(cudaStreamSynchronize(ctx->stream));
-        *n_new = c;
-        return res_sync(ctx); // a windowed frame rejected before this one: this frame was not applied either
-    }
-    return DSM_OK;
-}
-
 // ---- inactive store (DESIGN.md section 8.2) ----
 static DsmDev inactive_view(dsm_ctx *ctx)
 {
@@ -1343,8 +1272,8 @@ extern "C" int dsm_inactive_export_poses(dsm_ctx *ctx, const int32_t *keyframes,
     return inactive_export_ranges(ctx, ranges, out, cap, n_out);
 }
 
-// A run of n consecutive frames of ONE sequential stream on the resident pool.  Results are identical to n calls of
-// dsm_fuse_frame_resident: superpixels, normals and plane fits do not depend on the pose or the pool, so they run
+// A run of n consecutive frames of ONE sequential stream on the resident pool.  Results are identical to n runs of one
+// frame each (dsm_fuse_frame_resident): superpixels, normals and plane fits do not depend on the pose or the pool, so they run
 // for all n frames as one batch (full-width launches instead of n latency-bound single-frame ones); only the fuse /
 // initialise / post-step, which carry the pool from frame t to frame t+1, run frame by frame.
 static int list_len(const int32_t *o, int t) { return o ? o[t + 1] - o[t] : 0; }
@@ -1383,9 +1312,10 @@ static int window_validate(const dsm_ctx *ctx, int n, const WinLists &w, bool *a
     return DSM_OK;
 }
 
-// dsm_fuse_stream_resident, and with `win` dsm_fuse_stream_window: each frame's window step runs right before its fuse
-static int stream_run(dsm_ctx *ctx, int n, const int32_t *ref_idx, const uint8_t *gray, const float *depth,
-                      const float *poses, int32_t *n_new, const WinLists *win)
+// dsm_fuse_stream_resident and dsm_fuse_frame_resident, and with `win` dsm_fuse_stream_window: each frame's window step
+// runs right before its fuse.  Rows of the n images lie gray_pitch / depth_pitch bytes apart.
+static int stream_run(dsm_ctx *ctx, int n, const int32_t *ref_idx, const uint8_t *gray, size_t gray_pitch, const float *depth,
+                      size_t depth_pitch, const float *poses, int32_t *n_new, const WinLists *win)
 {
     if (!ctx || !ref_idx || !gray || !depth || !poses) return DSM_E_INVALID;
     if (n < 1 || n > ctx->p.max_batch) return DSM_E_INVALID;
@@ -1412,26 +1342,29 @@ static int stream_run(dsm_ctx *ctx, int n, const int32_t *ref_idx, const uint8_t
     const bool dbl = 2 * n <= ctx->p.max_batch;
     const int par = dbl ? (ctx->res_frame & 1) : 0;
     ctx->res_frame++;
-    const int e = EV_HALF + par; // this half's staging buffers and pinned tables are free again
-    CK(cudaEventSynchronize(ctx->ev_done[e]));
-    if (!dbl) CK(cudaEventSynchronize(ctx->ev_done[EV_HALF + (1 - par)]));
-    // single-frame calls (dsm_fuse_frame_resident) may still be running out of the same staging buffers and frame slots
-    // 0 / 1 (only then: the events are also recorded at the end of every run of this function, and waiting for the
-    // previous run here would serialise this run's copies behind it)
-    const bool after_single = ctx->single_pending;
-    ctx->single_pending = false;
-    if (after_single)
-    {
-        CK(cudaStreamWaitEvent(ctx->s_h2d, ctx->ev_done[EV_SLOT + 0], 0));
-        CK(cudaStreamWaitEvent(ctx->s_h2d, ctx->ev_done[EV_SLOT + 1], 0));
-    }
+    cudaStream_t st = ctx->stream;
+    // The ordering rule of include/dsm.h (dsm_fuse_stream_resident).  Each call records half_free of the OTHER half on the
+    // main stream at its entry: the next run uses that half, and everything enqueued before this call (that half's
+    // previous run and any later reads of its slots included) comes before that point, but this run does not, so the
+    // next run's phase 1 overlaps this run's phase 2.  The host waits for the same point before it rewrites the half's
+    // pinned tables and staging buffers.  A run over both halves (!dbl) is ordered on the main stream and frees both
+    // halves at its end.
+    CK(cudaEventRecord(ctx->half_free[1 - par], st));
+    CK(cudaEventSynchronize(ctx->half_free[par]));
+    if (!dbl) CK(cudaEventSynchronize(ctx->half_free[1 - par]));
     const size_t so = (size_t)par * (size_t)(ctx->p.max_batch / 2); // fixed halves: runs of different length never overlap
     uint8_t *gp = ctx->gray_packed + so * fpx;
     float *dp = ctx->depth_packed + so * fpx;
-    CK(cudaMemcpyAsync(gp, gray, (size_t)n * fpx, cudaMemcpyHostToDevice, ctx->s_h2d));
-    CK(cudaMemcpyAsync(dp, depth, (size_t)n * fpx * sizeof(float), cudaMemcpyHostToDevice, ctx->s_h2d));
-    CK(cudaEventRecord(ctx->ev_h2d[e], ctx->s_h2d));
-    cudaStream_t st = ctx->stream;
+    // packed rows: one contiguous copy per image; padded rows: one 2-D copy into the same packed staging
+    if (gray_pitch == (size_t)W)
+        CK(cudaMemcpyAsync(gp, gray, (size_t)n * fpx, cudaMemcpyHostToDevice, ctx->s_h2d));
+    else
+        CK(cudaMemcpy2DAsync(gp, W, gray, gray_pitch, W, (size_t)n * H, cudaMemcpyHostToDevice, ctx->s_h2d));
+    if (depth_pitch == (size_t)W * 4)
+        CK(cudaMemcpyAsync(dp, depth, (size_t)n * fpx * sizeof(float), cudaMemcpyHostToDevice, ctx->s_h2d));
+    else
+        CK(cudaMemcpy2DAsync(dp, (size_t)W * 4, depth, depth_pitch, (size_t)W * 4, (size_t)n * H, cudaMemcpyHostToDevice, ctx->s_h2d));
+    CK(cudaEventRecord(ctx->half_h2d[par], ctx->s_h2d));
     // Phase 1 (superpixels, normals, plane fits of all n frames; never touches the pool) runs on a side stream and in this
     // half's own frame slots [so, so + n): it overlaps the frame-by-frame phase 2 of the PREVIOUS run, which owns the
     // other half's slots and the main stream.  (With a single half, so == 0 and everything is ordered on the main stream.)
@@ -1445,11 +1378,11 @@ static int stream_run(dsm_ctx *ctx, int n, const int32_t *ref_idx, const uint8_t
     { // this half's slots and device tables were last read by the phase 2 of the run before the previous one
         CK(cudaEventRecord(ctx->ev_fork, st));
         CK(cudaStreamWaitEvent(s2, ctx->ev_fork, 0));
-        CK(cudaStreamWaitEvent(s1, ctx->ev_done[e], 0));
+        CK(cudaStreamWaitEvent(s1, ctx->half_free[par], 0));
     }
-    // pinned tables of this mode live in the second half of h_pose / h_ref (the first half belongs to the single-frame
-    // and batch calls, which only wait for their own copies before rewriting it); this half's previous table copy ran
-    // before ev_done[e], which has been waited for above
+    // pinned tables of this mode live in the second half of h_pose / h_ref (the first half belongs to the batch calls,
+    // which only wait for their own copies before rewriting it); this half's previous table copy ran before
+    // half_free[par], which has been waited for above
     int rc = stage_tables(ctx, (size_t)ctx->p.max_batch + so, slot0, n, poses, ref_idx, s1);
     if (rc != DSM_OK) return rc;
     const int tag = win ? (ctx->win_tag = ctx->win_tag % 0x3fffffff + 1) : 0;
@@ -1458,7 +1391,7 @@ static int stream_run(dsm_ctx *ctx, int n, const int32_t *ref_idx, const uint8_t
         rc = stage_window(ctx, par, n, *win, tag, s1);
         if (rc != DSM_OK) return rc;
     }
-    CK(cudaStreamWaitEvent(s1, ctx->ev_h2d[e], 0));
+    CK(cudaStreamWaitEvent(s1, ctx->half_h2d[par], 0));
     // phase 1: all n frames at once, in the batch view (never touches the pool)
     DsmDev v = ctx->d;
     v.frame0 = slot0;
@@ -1471,7 +1404,7 @@ static int stream_run(dsm_ctx *ctx, int n, const int32_t *ref_idx, const uint8_t
     ctx->uploaded = true;
     ctx->img_slot0 = slot0, ctx->img_n = n; // ordered before the main stream through phase 2 (ev_join / ev_p2) below
     ctx->img_fit = false;
-    rc = enqueue_schedule(ctx, v, n, s1, false, 1);
+    rc = enqueue_schedule(ctx, v, n, s1, 1);
     if (rc != DSM_OK) return rc;
     ctx->img_fit = schedule_fits(ctx);
     if (dbl)
@@ -1495,7 +1428,7 @@ static int stream_run(dsm_ctx *ctx, int n, const int32_t *ref_idx, const uint8_t
                 dsm_launch_window_step(dv, window_view(ctx, par, t, ctx->d.S), dv.max_pool_per_frame, nr, na, s2);
             }
         }
-        rc = enqueue_schedule(ctx, resident_view(ctx, slot0 + t), 1, s2, true, 2);
+        rc = enqueue_schedule(ctx, resident_view(ctx, slot0 + t), 1, s2, 2);
         if (rc != DSM_OK) return rc;
         ctx->res_upper += ctx->d.S;
     }
@@ -1506,12 +1439,13 @@ static int stream_run(dsm_ctx *ctx, int n, const int32_t *ref_idx, const uint8_t
         CK(cudaEventRecord(ctx->ev_p2, s2));
         CK(cudaStreamWaitEvent(st, ctx->ev_p2, 0));
     }
-    CK(cudaEventRecord(ctx->ev_done[e], st));
-    CK(cudaEventRecord(ctx->ev_done[EV_SLOT + 0], st)); // dsm_fuse_frame_resident waits on these before reusing slot 0 / 1
-    CK(cudaEventRecord(ctx->ev_done[EV_SLOT + 1], st));
+    else
+    {
+        for (cudaEvent_t ev : ctx->half_free) CK(cudaEventRecord(ev, st));
+    }
     CK(cudaGetLastError());
     // the caller may reuse its image buffers as soon as we return
-    CK(cudaEventSynchronize(ctx->ev_h2d[e]));
+    CK(cudaEventSynchronize(ctx->half_h2d[par]));
     if (n_new)
     {
         int32_t h[4] = {0, 0, 0, 0};
@@ -1527,18 +1461,30 @@ static int stream_run(dsm_ctx *ctx, int n, const int32_t *ref_idx, const uint8_t
     return DSM_OK;
 }
 
+extern "C" int dsm_fuse_frame_resident(dsm_ctx *ctx, int ref_idx, const uint8_t *gray, size_t gray_pitch,
+                                       const float *depth, size_t depth_pitch, const float pose[16], int *n_new)
+{
+    if (!ctx || !gray || !depth || !pose) return DSM_E_INVALID;
+    if (!ctx->res_active) return DSM_E_STATE;
+    if (gray_pitch < (size_t)ctx->p.width || depth_pitch < (size_t)ctx->p.width * 4) return DSM_E_INVALID;
+    const int32_t ref = ref_idx;
+    return stream_run(ctx, 1, &ref, gray, gray_pitch, depth, depth_pitch, pose, n_new, nullptr);
+}
+
 extern "C" int dsm_fuse_stream_resident(dsm_ctx *ctx, int n, const int32_t *ref_idx, const uint8_t *gray, const float *depth,
                                         const float *poses, int32_t *n_new)
 {
-    return stream_run(ctx, n, ref_idx, gray, depth, poses, n_new, nullptr);
+    if (!ctx) return DSM_E_INVALID;
+    return stream_run(ctx, n, ref_idx, gray, (size_t)ctx->p.width, depth, (size_t)ctx->p.width * 4, poses, n_new, nullptr);
 }
 
 extern "C" int dsm_fuse_stream_window(dsm_ctx *ctx, int n, const int32_t *ref_idx, const uint8_t *gray, const float *depth,
                                       const float *poses, const int32_t *retire_kf, const int32_t *retire_ofs,
                                       const int32_t *reactivate_kf, const int32_t *reactivate_ofs, int32_t *n_new)
 {
+    if (!ctx) return DSM_E_INVALID;
     const WinLists w{retire_kf, retire_ofs, reactivate_kf, reactivate_ofs};
-    return stream_run(ctx, n, ref_idx, gray, depth, poses, n_new, &w);
+    return stream_run(ctx, n, ref_idx, gray, (size_t)ctx->p.width, depth, (size_t)ctx->p.width * 4, poses, n_new, &w);
 }
 
 // ---- raw cloud of a frame (publish_raw_pointcloud, surfel_map.cpp:1115-1151) ----

@@ -77,22 +77,10 @@ struct GraphEntry
 {
     int f0, nf, maxper, phase;
     const void *pool, *poolofs, *gate;
-    bool post; // ends with the resident pool's post-step
     GraphExecPtr exec;
 };
 
-// Input copy / kernel completion events (ev_h2d / ev_done) per staging area.  The index ranges overlap on purpose, and
-// waits across entry points rely on it: dsm_fuse_batch_async's chunks use EV_CHUNK + c (c < DSM_MAX_CHUNKS),
-// dsm_fuse_frame_resident's frame slots use EV_SLOT + s (s < 2) and wait for the EV_SLOT events that
-// dsm_fuse_stream_resident records at the end of every run, whose staging halves use EV_HALF + h (h < 2).
 #define DSM_MAX_CHUNKS 4
-enum
-{
-    EV_CHUNK = 0,
-    EV_SLOT = 0,
-    EV_HALF = 6,
-    EV_COUNT = 8
-};
 
 struct dsm_ctx
 {
@@ -127,7 +115,7 @@ struct dsm_ctx
     // resident pool (stream mode)
     int res_upper = 0;   // host-side upper bound of the resident pool size (exact after a sync)
     bool res_active = false;
-    int res_frame = 0;   // frames fused in resident mode so far (selects the frame slot)
+    int res_frame = 0;   // resident stream runs so far (alternates the staging halves)
     int32_t *res_ofs = nullptr; // device [4]: {0, resident pool size, error tag of dsm_fuse_stream_window, rejected frame}
     int *blkcnt = nullptr, *blkofs = nullptr, *nsel = nullptr; // ordered selection: per-block counts / offsets, total
     int32_t *holes = nullptr, *rc_src = nullptr, *rc_sync = nullptr; // fuse_map post-step (dsm_launch_pool_recycle)
@@ -154,9 +142,11 @@ struct dsm_ctx
     int win_blk_stride = 0;
     int win_tag = 0;          // tag of the latest windowed call (what a rejected frame writes into the error word)
     bool win_pending = false; // a window step since the last synchronisation: mirrors stale, error word unread
-    cudaEvent_t ev_h2d[EV_COUNT] = {}, ev_done[EV_COUNT] = {}, ev_start = nullptr;
-    cudaEvent_t ev_fork = nullptr, ev_join[4] = {}; // dsm_batch_run: fork / join of the concurrent sub-batches
-    bool single_pending = false; // a dsm_fuse_frame_resident call since the last dsm_fuse_stream_resident (they share frame slots 0 / 1)
+    cudaEvent_t ev_h2d[DSM_MAX_CHUNKS] = {}, ev_done[DSM_MAX_CHUNKS] = {}, ev_start = nullptr; // dsm_fuse_batch_async's chunks
+    // the resident stream's staging halves: half_h2d[h] ends a run's input copy into half h; half_free[h] lies on the main
+    // stream after every earlier use of half h (stream_run records it, see there)
+    cudaEvent_t half_h2d[2] = {}, half_free[2] = {};
+    cudaEvent_t ev_fork = nullptr, ev_join[DSM_MAX_CHUNKS] = {}; // dsm_batch_run: fork / join of the concurrent sub-batches
     // frame slots [img_slot0, img_slot0 + img_n) hold the images of the most recent call that took images (img_n == 0: none
     // yet); dsm_frame_raw_cloud reads them, into raw_out (W*H points, allocated at its first call).  img_fit: that call's
     // schedule has run through the plane fit, so the slots' label codes and plane normals are complete;
@@ -167,7 +157,7 @@ struct dsm_ctx
     uint8_t *spimg_out = nullptr;
     int run_split = 2;           // sub-batches per dsm_batch_run (dsm_set_concurrency)
     // pinned host staging for the small per-batch tables
-    float *h_pose = nullptr; // [2B][32]: pose then inverse; second half: dsm_fuse_stream_resident's own tables
+    float *h_pose = nullptr; // [2B][32]: pose then inverse; first half: the batch calls, second half: the resident stream
     int32_t *h_ofs = nullptr;
     int32_t *h_ref = nullptr; // [2B], halves as h_pose
     int32_t *h_sync = nullptr; // [8]: res_sync's readback of res_ofs and win_hdr

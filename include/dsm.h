@@ -179,7 +179,7 @@ int dsm_batch_wait(dsm_ctx *ctx);
 int dsm_batch_restore_pool(dsm_ctx *ctx);
 
 /* ---- GPU-resident pool for a sequential stream (SURVEY.md §8f rows 1-2) ----
- * The pool of ONE stream lives on the device between frames (frame slot 0 of the context), so per
+ * The pool of ONE stream lives on the device between frames, so per
  * frame only the image pair and the pose cross PCIe.  Semantics mirror what SurfelMap does around
  * the hot-path call:
  *   dsm_pool_upload            local_surfels := given array
@@ -189,7 +189,9 @@ int dsm_batch_restore_pool(dsm_ctx *ctx);
  *                              take the back element.  The pool equals the reference's local_surfels element for
  *                              element (byte for byte given the same fuse results), and slots are stable: a
  *                              surfel keeps its index until it dies or is the back element moved into a hole.
- *                              *n_new (optional) = number of new surfels; passing it synchronises.
+ *                              *n_new (optional) = number of new surfels; passing it synchronises.  The call is
+ *                              dsm_fuse_stream_resident with n_frames = 1, except that image rows lie gray_pitch /
+ *                              depth_pitch bytes apart; it is ordered as stated there.
  *   dsm_pool_transform         warp_active_surfels_cpu_kernel (surfel_map.cpp:750-789):
  *                              p <- W p, n <- R_W n for every pool surfel after a loop closure
  *                              (W = T_loop * T_cam^-1 computed by the caller in fp64, cast to f32).
@@ -212,7 +214,19 @@ int dsm_fuse_frame_resident(dsm_ctx *ctx, int reference_frame_index,
  * n-1 frames of latency for throughput (offline sequences, or a node that lags behind its camera).  n <= max_batch;
  * with 2n <= max_batch consecutive runs use alternate halves of the frame slots: the copy and the batched stages of one
  * run overlap the frame-by-frame stages of the previous one.  n_new (optional, [n]) = new surfels per frame; passing it
- * synchronises. */
+ * synchronises.
+ * Ordering of the resident stream calls (this one, dsm_fuse_frame_resident and dsm_fuse_stream_window): a run's
+ * frame-by-frame stages follow everything enqueued on the context's stream before the call, and work enqueued on that
+ * stream after the call follows them.  Its batched stages rewrite the frame slots of the run's staging half, new surfels
+ * and counts included (DSM_BUF_NEW_SURFELS / DSM_BUF_NEW_COUNTS), and wait only for what was enqueued on the context's
+ * stream before the PREVIOUS call began.  With alternating halves that is the last run on the same half and every read
+ * of its slots enqueued before the next call; a read enqueued later may see the slots rewritten.  The same holds for
+ * batch calls (dsm_batch_upload / _run / _download) enqueued between two resident calls: they use frame slots from 0
+ * and are not ordered before the batched stages of the call after the next.  The host waits for the same point before
+ * it reuses a half's staging buffers, so it blocks when it gets more than two calls ahead.  With a single half
+ * (2n > max_batch, e.g. every single-frame call at max_batch = 1) the run is ordered on the context's stream like
+ * every other call, and the host waits at its entry for everything enqueued on that stream before it.  The resident
+ * stream calls return DSM_E_STATE while a dsm_fuse_batch_async batch is in flight. */
 int dsm_fuse_stream_resident(dsm_ctx *ctx, int n_frames, const int32_t *reference_frame_index,
                              const uint8_t *gray, const float *depth, const float *poses_colmajor, int32_t *n_new);
 int dsm_pool_transform(dsm_ctx *ctx, const float W_colmajor[16]);

@@ -73,7 +73,7 @@ def pool(ctx):
 
 
 def test_byte_exact_on_both_frame_slots(ctx, pool):
-    for t in range(3, 7):                  # alternating frame slots 0 / 1
+    for t in range(3, 7):                  # alternating frame slots 0 / 4 (the first slot of each staging half)
         gray, depth, pose = frame(t)
         lo, no, want = expect(ctx, t, gray, depth, pose, pool)
         n_new, got = resident(ctx, pool, t, gray, depth, pose)

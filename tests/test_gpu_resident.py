@@ -204,6 +204,46 @@ def test_stream_chunks_equal_frame_by_frame(chunk):
     b.close()
 
 
+@pytest.mark.parametrize("max_batch", [1, 2, 8])
+def test_frame_resident_padded_rows_equal_packed_rows(max_batch):
+    """dsm_fuse_frame_resident with padded rows (gray rows of W+24 bytes, depth rows of W+8 floats, the padding holding
+    values no frame has), for gray, depth or both, must leave the pool byte-identical to the same stream with packed rows,
+    with the same counts.  The C function is called directly: Context.fuse_frame_resident makes its inputs contiguous."""
+    import ctypes
+    from densesurfelmapping_b200 import capi
+    cam = synth.VGA
+    W, H = cam.width, cam.height
+    frames = []
+    for t in range(5):
+        pose = synth.pose_stream(t)
+        gray, depth = synth.make_frame(cam, 700 + t, pose)
+        frames.append((t // 2, gray, depth, capi.pose16(pose)))
+    pools, counts = [], []
+    for padded in ((), ("gray",), ("depth",), ("gray", "depth")):
+        ctx = capi.Context(cam, max_batch=max_batch, max_local_surfels=100000)
+        ctx.pool_upload(np.zeros(0, SURFEL_DTYPE))
+        cnt = []
+        for ref, gray, depth, pose in frames:
+            g, d = np.ascontiguousarray(gray), np.ascontiguousarray(depth)
+            if "gray" in padded:
+                g = np.full((H, W + 24), 255, np.uint8)
+                g[:, :W] = gray
+            if "depth" in padded:
+                d = np.full((H, W + 8), 7.5, np.float32)
+                d[:, :W] = depth
+            n = ctypes.c_int(0)
+            ctx._ck(ctx.lib.dsm_fuse_frame_resident(ctx.h, ref, g.ctypes.data, g.strides[0], d.ctypes.data, d.strides[0],
+                                                    pose.ctypes.data, ctypes.byref(n)))
+            cnt.append(n.value)
+        pools.append(ctx.pool_download().tobytes())
+        counts.append(cnt)
+        ctx.close()
+    assert min(counts[0]) > 0
+    for k in range(1, len(pools)):
+        assert counts[k] == counts[0], f"padded variant {k}"
+        assert pools[k] == pools[0], f"padded variant {k}"
+
+
 def test_inactive_store_round_trip():
     """Device-resident attached_surfels: retire two keyframes into the store, warp one of them, publish the inactive
     cloud, bring one back -- against the restated (and reference-pinned, tests/test_refmap.py) SurfelMap members."""

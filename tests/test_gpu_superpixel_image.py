@@ -187,7 +187,7 @@ def test_no_side_effects_on_the_stream():
             ctx.superpixel_image(0), ctx.superpixel_image(1)
     a, b = ctxs
     assert a.pool_download().tobytes() == b.pool_download().tobytes()
-    for slot in (0, 1, 4, 5):   # the single-frame slots, and the stream's half (res_frame 3 -> the second half)
+    for slot in (0, 1, 4, 5):   # the single-frame slots 0 / 4, and the stream's half (its 4th run -> the second half)
         assert a.labels(slot).tobytes() == b.labels(slot).tobytes() and a.seeds(slot).tobytes() == b.seeds(slot).tobytes()
     for c in ctxs:
         c.close()

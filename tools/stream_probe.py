@@ -1,5 +1,6 @@
 """Where does a resident single-frame stream spend its time?  Per-call host time and device time of dsm_fuse_frame_resident
-with and without CUDA graphs.   python tools/stream_probe.py"""
+(a one-frame dsm_fuse_stream_resident: phase 1 and phase 2 are two graphs per frame, on two streams) with and without
+CUDA graphs.   python tools/stream_probe.py"""
 import os
 import sys
 import time
