@@ -383,34 +383,60 @@ static int stage_tables(dsm_ctx *ctx, size_t row, int slot, int n, const float *
     return DSM_OK;
 }
 
-// Batch-mode tables of frames [0, n) on the main stream (first pinned half): per-frame pool offsets `ofs`, validated, or
-// (ofs == nullptr) one frame's n_local_single surfels.
-static int upload_tables(dsm_ctx *ctx, int n, const int32_t *ref, const float *poses, const int32_t *ofs, int n_local_single)
+// Batch-mode tables of frames [0, n) on the main stream (first pinned half): per-frame pool offsets `ofs`, validated.
+static int upload_tables(dsm_ctx *ctx, int n, const int32_t *ref, const float *poses, const int32_t *ofs)
 {
-    int total = 0, maxper = 0;
-    if (ofs)
+    if (ofs[0] != 0) return DSM_E_INVALID;
+    int maxper = 0;
+    for (int b = 0; b <= n; b++) ctx->h_ofs[b] = ofs[b];
+    for (int b = 0; b < n; b++)
     {
-        if (ofs[0] != 0) return DSM_E_INVALID;
-        for (int b = 0; b <= n; b++) ctx->h_ofs[b] = ofs[b];
-        for (int b = 0; b < n; b++)
-        {
-            int c = ofs[b + 1] - ofs[b];
-            if (c < 0) return DSM_E_INVALID;
-            if (c > maxper) maxper = c;
-        }
-        total = ofs[n];
+        int c = ofs[b + 1] - ofs[b];
+        if (c < 0) return DSM_E_INVALID;
+        if (c > maxper) maxper = c;
     }
-    else
-    {
-        ctx->h_ofs[0] = 0;
-        for (int b = 1; b <= n; b++) ctx->h_ofs[b] = n_local_single;
-        total = maxper = n_local_single;
-    }
-    if (total > ctx->p.max_local_surfels) return DSM_E_CAPACITY;
-    ctx->n_pool = total;
+    if (ofs[n] > ctx->p.max_local_surfels) return DSM_E_CAPACITY;
+    ctx->n_pool = ofs[n];
     ctx->d.max_pool_per_frame = maxper;
     CK(cudaMemcpyAsync(ctx->poolofs, ctx->h_ofs, ((size_t)n + 1) * sizeof(int32_t), cudaMemcpyHostToDevice, ctx->stream));
     return stage_tables(ctx, 0, 0, n, poses, ref, ctx->stream);
+}
+
+// The images of n frames, rows gray_pitch / depth_pitch bytes apart, into the packed staging from frame slot `slot` on
+// `st`: packed rows in one contiguous copy per array, padded rows in one 2-D copy.  k_repack then lays them out in the
+// pitched planes, the same for both.
+static int stage_images(dsm_ctx *ctx, int slot, int n, const uint8_t *gray, size_t gray_pitch, const float *depth,
+                        size_t depth_pitch, cudaStream_t st)
+{
+    const size_t W = ctx->p.width, rows = (size_t)n * ctx->p.height, row0 = (size_t)slot * ctx->p.height;
+    uint8_t *gp = ctx->gray_packed + row0 * W;
+    float *dp = ctx->depth_packed + row0 * W;
+    if (gray_pitch == W)
+        CK(cudaMemcpyAsync(gp, gray, rows * W, cudaMemcpyHostToDevice, st));
+    else
+        CK(cudaMemcpy2DAsync(gp, W, gray, gray_pitch, W, rows, cudaMemcpyHostToDevice, st));
+    if (depth_pitch == W * 4)
+        CK(cudaMemcpyAsync(dp, depth, rows * W * 4, cudaMemcpyHostToDevice, st));
+    else
+        CK(cudaMemcpy2DAsync(dp, W * 4, depth, depth_pitch, W * 4, rows, cudaMemcpyHostToDevice, st));
+    return DSM_OK;
+}
+
+// Launches of the schedule up to and including the plane fit: seed init, 3 x (assign, gather, Newton), plane gather, solve.
+static const int kPlaneFitSteps = 12;
+// the schedule enqueued now runs at least through the plane fit (dsm_debug_stop_after does not cut it short before)
+static bool schedule_fits(const dsm_ctx *ctx) { return ctx->stop_after <= 0 || ctx->stop_after >= kPlaneFitSteps; }
+
+// The frames the context holds: slots [slot0, slot0 + n) hold the images of the latest call that took images, and the
+// batch calls' frames are [0, nb).  `ran`: their schedule has been enqueued (through the plane fit unless
+// dsm_debug_stop_after cuts it).
+static void hold_frames(dsm_ctx *ctx, int slot0, int n, bool ran)
+{
+    ctx->nb = slot0 + n;
+    ctx->uploaded = true;
+    ctx->ran = ran;
+    ctx->img_slot0 = slot0, ctx->img_n = n;
+    ctx->img_fit = ran && schedule_fits(ctx);
 }
 
 extern "C" int dsm_batch_upload(dsm_ctx *ctx, int n, const int32_t *ref, const uint8_t *gray, const float *depth,
@@ -422,27 +448,22 @@ extern "C" int dsm_batch_upload(dsm_ctx *ctx, int n, const int32_t *ref, const u
     CK(cudaSetDevice(ctx->device));
     // the pinned tables are reused: make sure the previous batch's copies have drained
     CK(cudaStreamSynchronize(ctx->stream));
-    int rc = upload_tables(ctx, n, ref, poses, ofs, 0);
+    int rc = upload_tables(ctx, n, ref, poses, ofs);
     if (rc != DSM_OK) return rc;
-    const int W = ctx->p.width, H = ctx->p.height;
-    // [n][H][W] packed: one contiguous copy each, then the repack kernel lays out the pitched format
-    CK(cudaMemcpyAsync(ctx->gray_packed, gray, (size_t)n * H * W, cudaMemcpyHostToDevice, ctx->stream));
-    CK(cudaMemcpyAsync(ctx->depth_packed, depth, (size_t)n * H * W * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
+    rc = stage_images(ctx, 0, n, gray, (size_t)ctx->p.width, depth, (size_t)ctx->p.width * 4, ctx->stream);
+    if (rc != DSM_OK) return rc;
     {
         DsmDev d = ctx->d;
         d.frame0 = 0;
         ProfScope p(ctx, DSM_K_REPACK);
         dsm_launch_repack(d, n, ctx->gray_packed, ctx->depth_packed, ctx->stream);
     }
-    ctx->img_slot0 = 0, ctx->img_n = n, ctx->img_fit = false;
     if (ctx->n_pool > 0)
     {
         CK(cudaMemcpyAsync(ctx->d.pool, local, (size_t)ctx->n_pool * sizeof(dsm_surfel_t), cudaMemcpyHostToDevice, ctx->stream));
         CK(cudaMemcpyAsync(ctx->pool_snap, ctx->d.pool, (size_t)ctx->n_pool * sizeof(dsm_surfel_t), cudaMemcpyDeviceToDevice, ctx->stream));
     }
-    ctx->nb = n;
-    ctx->uploaded = true;
-    ctx->ran = false;
+    hold_frames(ctx, 0, n, false);
     ctx->res_active = false;
     return DSM_OK;
 }
@@ -456,11 +477,6 @@ extern "C" int dsm_batch_restore_pool(dsm_ctx *ctx)
         CK(cudaMemcpyAsync(ctx->d.pool, ctx->pool_snap, (size_t)ctx->n_pool * sizeof(dsm_surfel_t), cudaMemcpyDeviceToDevice, ctx->stream));
     return DSM_OK;
 }
-
-// Launches of the schedule up to and including the plane fit: seed init, 3 x (assign, gather, Newton), plane gather, solve.
-static const int kPlaneFitSteps = 12;
-// the schedule enqueued now runs at least through the plane fit (dsm_debug_stop_after does not cut it short before)
-static bool schedule_fits(const dsm_ctx *ctx) { return ctx->stop_after <= 0 || ctx->stop_after >= kPlaneFitSteps; }
 
 // The per-frame schedule: generate_super_pixels (:960-975) then fuse (:58-71) then initialise (:79), enqueued for the
 // frame slots [d.frame0, d.frame0 + nb) of the view `d` (its pool, poolofs and max_pool_per_frame).
@@ -559,6 +575,26 @@ static int enqueue_schedule(dsm_ctx *ctx, const DsmDev &v, int nf, cudaStream_t 
     return DSM_OK;
 }
 
+// Frames [0, n) in `parts` even parts, part i on s_comp[i], forked from the main stream and joined back into it (a
+// single part runs on the main stream itself).  part(i, f0, nf, st) enqueues part i, frames [f0, f0 + nf), on st.
+template <typename Part>
+static int run_parts(dsm_ctx *ctx, int n, int parts, Part part)
+{
+    if (parts <= 1) return part(0, 0, n, ctx->stream);
+    CK(cudaEventRecord(ctx->ev_fork, ctx->stream));
+    for (int i = 0, f0 = 0; i < parts; i++)
+    {
+        const int nf = (n - f0 + (parts - i) - 1) / (parts - i);
+        CK(cudaStreamWaitEvent(ctx->s_comp[i], ctx->ev_fork, 0));
+        const int rc = part(i, f0, nf, ctx->s_comp[i]);
+        if (rc != DSM_OK) return rc;
+        CK(cudaEventRecord(ctx->ev_join[i], ctx->s_comp[i]));
+        CK(cudaStreamWaitEvent(ctx->stream, ctx->ev_join[i], 0));
+        f0 += nf;
+    }
+    return DSM_OK;
+}
+
 extern "C" int dsm_batch_run(dsm_ctx *ctx)
 {
     if (!ctx) return DSM_E_INVALID;
@@ -569,29 +605,13 @@ extern "C" int dsm_batch_run(dsm_ctx *ctx)
     // contexts alternating (bench.py) the gain on an H100 at 400 W is small: 1.150 / 1.163 ms per 32-frame step with two
     // sub-batches against 1.153 / 1.168 ms with one (two runs each); three or four sub-batches were slower.
     const int parts = (ctx->stop_after > 0 || ctx->nb < 8) ? 1 : (ctx->run_split < ctx->nb ? ctx->run_split : ctx->nb);
-    DsmDev v = ctx->d; // batch view: per-frame pool slices at poolofs, frames from slot 0
-    v.frame0 = 0;
-    if (parts <= 1)
-    {
-        int rc = enqueue_schedule(ctx, v, ctx->nb, ctx->stream);
-        if (rc != DSM_OK) return rc;
-    }
-    else
-    {
-        CK(cudaEventRecord(ctx->ev_fork, ctx->stream));
-        for (int i = 0; i < parts; i++)
-        {
-            const int nf = (ctx->nb - v.frame0 + (parts - i) - 1) / (parts - i);
-            CK(cudaStreamWaitEvent(ctx->s_comp[i], ctx->ev_fork, 0));
-            int rc = enqueue_schedule(ctx, v, nf, ctx->s_comp[i]);
-            if (rc != DSM_OK) return rc;
-            CK(cudaEventRecord(ctx->ev_join[i], ctx->s_comp[i]));
-            CK(cudaStreamWaitEvent(ctx->stream, ctx->ev_join[i], 0));
-            v.frame0 += nf;
-        }
-    }
-    ctx->ran = true;
-    ctx->img_fit = schedule_fits(ctx);
+    const int rc = run_parts(ctx, ctx->nb, parts, [&](int, int f0, int nf, cudaStream_t st) {
+        DsmDev v = ctx->d; // batch view: per-frame pool slices at poolofs, frames from slot 0
+        v.frame0 = f0;
+        return enqueue_schedule(ctx, v, nf, st);
+    });
+    if (rc != DSM_OK) return rc;
+    hold_frames(ctx, ctx->img_slot0, ctx->img_n, true); // the same frames (nb == img_slot0 + img_n), now run
     return DSM_OK;
 }
 
@@ -675,58 +695,45 @@ extern "C" int dsm_batch_wait(dsm_ctx *ctx)
     return DSM_OK;
 }
 
-extern "C" int dsm_fuse_batch_async(dsm_ctx *ctx, int n, const int32_t *ref, const uint8_t *gray, const float *depth,
-                                    const float *poses, dsm_surfel_t *local, const int32_t *ofs,
-                                    dsm_surfel_t *new_out, int32_t *n_new)
+// an in-flight dsm_fuse_batch_async batch copies and runs on the context's side streams: finish it first
+static int finish_batch(dsm_ctx *ctx) { return ctx->in_flight ? dsm_batch_wait(ctx) : DSM_OK; }
+
+// dsm_fuse_batch_async, with rows of the n images gray_pitch / depth_pitch bytes apart
+static int fuse_batch_async(dsm_ctx *ctx, int n, const int32_t *ref, const uint8_t *gray, size_t gray_pitch, const float *depth,
+                            size_t depth_pitch, const float *poses, dsm_surfel_t *local, const int32_t *ofs,
+                            dsm_surfel_t *new_out, int32_t *n_new)
 {
     if (!ctx || !ref || !gray || !depth || !poses || !ofs) return DSM_E_INVALID;
     if (n < 1 || n > ctx->p.max_batch) return DSM_E_INVALID;
     if (ofs[n] > 0 && !local) return DSM_E_INVALID;
     CK(cudaSetDevice(ctx->device));
-    if (ctx->in_flight)
-    { // one batch per context at a time: finish the previous one first
-        int rcw = dsm_batch_wait(ctx);
-        if (rcw != DSM_OK) return rcw;
-    }
-    CK(cudaStreamSynchronize(ctx->stream));
-    int rc = upload_tables(ctx, n, ref, poses, ofs, 0); // small tables, on the compute stream
+    int rc = finish_batch(ctx); // one batch per context at a time
     if (rc != DSM_OK) return rc;
-    const int W = ctx->p.width, H = ctx->p.height, S = ctx->d.S;
-    const size_t fpx = (size_t)H * W;
-    const int nchunks = n >= 16 ? 4 : (n >= 4 ? 2 : 1); // at most DSM_MAX_CHUNKS: one compute stream each
-    int csize[DSM_MAX_CHUNKS]; // even chunks (a smaller first chunk was tried: no gain, the kernels of small chunks are less efficient)
-    {
-        int rest = n, left = nchunks;
-        for (int c = 0; c < nchunks; c++)
-        {
-            csize[c] = (rest + left - 1) / left;
-            rest -= csize[c];
-            left--;
-        }
-    }
-    // copies must not start before earlier work on the compute stream (previous users of the buffers) is done
+    CK(cudaStreamSynchronize(ctx->stream));
+    rc = upload_tables(ctx, n, ref, poses, ofs); // small tables, on the main stream
+    if (rc != DSM_OK) return rc;
+    const int H = ctx->p.height, S = ctx->d.S;
+    const size_t fpx = (size_t)H * ctx->p.width;
+    // copies must not start before earlier work on the main stream (previous users of the buffers) is done
     CK(cudaEventRecord(ctx->ev_start, ctx->stream));
     CK(cudaStreamWaitEvent(ctx->s_h2d, ctx->ev_start, 0));
     CK(cudaStreamWaitEvent(ctx->s_d2h, ctx->ev_start, 0));
-    for (cudaStream_t s : ctx->s_comp) CK(cudaStreamWaitEvent(s, ctx->ev_start, 0));
-    int nc = 0;
-    for (int f0 = 0; f0 < n; f0 += csize[nc], nc++)
-    {
-        const int nf = csize[nc];
-        if (nf <= 0) break;
+    // even chunks (a smaller first chunk was tried: no gain, the kernels of small chunks are less efficient); the kernels
+    // of each chunk run on their own compute stream, so the latency-bound per-seed kernels of one chunk overlap the wide
+    // kernels of its neighbours instead of leaving SMs idle
+    const int nchunks = n >= 16 ? 4 : (n >= 4 ? 2 : 1);
+    rc = run_parts(ctx, n, nchunks, [&](int c, int f0, int nf, cudaStream_t cs) {
         const int p0 = ofs[f0], p1 = ofs[f0 + nf];
         int maxper = 0;
         for (int b = f0; b < f0 + nf; b++) maxper = (ofs[b + 1] - ofs[b] > maxper) ? ofs[b + 1] - ofs[b] : maxper;
         // H2D of this chunk
-        CK(cudaMemcpyAsync(ctx->gray_packed + (size_t)f0 * fpx, gray + (size_t)f0 * fpx, (size_t)nf * fpx, cudaMemcpyHostToDevice, ctx->s_h2d));
-        CK(cudaMemcpyAsync(ctx->depth_packed + (size_t)f0 * fpx, depth + (size_t)f0 * fpx, (size_t)nf * fpx * sizeof(float), cudaMemcpyHostToDevice, ctx->s_h2d));
+        int r = stage_images(ctx, f0, nf, gray + (size_t)f0 * H * gray_pitch, gray_pitch,
+                             (const float *)((const char *)depth + (size_t)f0 * H * depth_pitch), depth_pitch, ctx->s_h2d);
+        if (r != DSM_OK) return r;
         if (p1 > p0)
             CK(cudaMemcpyAsync(ctx->d.pool + p0, local + p0, (size_t)(p1 - p0) * sizeof(dsm_surfel_t), cudaMemcpyHostToDevice, ctx->s_h2d));
-        CK(cudaEventRecord(ctx->ev_h2d[nc], ctx->s_h2d));
-        // kernels: each chunk on its own compute stream, so the latency-bound per-seed kernels of one
-        // chunk overlap the wide kernels of its neighbours instead of leaving SMs idle
-        cudaStream_t cs = nchunks > 1 ? ctx->s_comp[nc] : ctx->stream;
-        CK(cudaStreamWaitEvent(cs, ctx->ev_h2d[nc], 0));
+        CK(cudaEventRecord(ctx->ev_h2d[c], ctx->s_h2d));
+        CK(cudaStreamWaitEvent(cs, ctx->ev_h2d[c], 0));
         DsmDev v = ctx->d; // batch view of this chunk
         v.frame0 = f0;
         v.max_pool_per_frame = maxper;
@@ -734,26 +741,34 @@ extern "C" int dsm_fuse_batch_async(dsm_ctx *ctx, int n, const int32_t *ref, con
             ProfScope p(ctx, DSM_K_REPACK, cs);
             dsm_launch_repack(v, nf, ctx->gray_packed + (size_t)f0 * fpx, ctx->depth_packed + (size_t)f0 * fpx, cs);
         }
-        rc = enqueue_schedule(ctx, v, nf, cs);
-        if (rc != DSM_OK) return rc;
-        CK(cudaEventRecord(ctx->ev_done[nc], cs));
+        r = enqueue_schedule(ctx, v, nf, cs);
+        if (r != DSM_OK) return r;
+        CK(cudaEventRecord(ctx->ev_done[c], cs));
         // D2H of this chunk
-        CK(cudaStreamWaitEvent(ctx->s_d2h, ctx->ev_done[nc], 0));
+        CK(cudaStreamWaitEvent(ctx->s_d2h, ctx->ev_done[c], 0));
         if (p1 > p0)
             CK(cudaMemcpyAsync(local + p0, ctx->d.pool + p0, (size_t)(p1 - p0) * sizeof(dsm_surfel_t), cudaMemcpyDeviceToHost, ctx->s_d2h));
         if (new_out)
             CK(cudaMemcpyAsync(new_out + (size_t)f0 * S, ctx->d.newsurf + (size_t)f0 * S, (size_t)nf * S * sizeof(dsm_surfel_t), cudaMemcpyDeviceToHost, ctx->s_d2h));
         if (n_new)
             CK(cudaMemcpyAsync(n_new + f0, ctx->d.nnew + f0, (size_t)nf * sizeof(int32_t), cudaMemcpyDeviceToHost, ctx->s_d2h));
-    }
-    ctx->nb = n;
-    ctx->uploaded = true;
-    ctx->ran = true;
+        return DSM_OK;
+    });
+    if (rc != DSM_OK) return rc;
+    hold_frames(ctx, 0, n, true);
     ctx->in_flight = true;
-    ctx->img_slot0 = 0, ctx->img_n = n, ctx->img_fit = schedule_fits(ctx);
     ctx->res_active = false; // the pool buffer now holds this batch's slices: a resident pool (if any) is gone
     CK(cudaGetLastError());
     return DSM_OK;
+}
+
+extern "C" int dsm_fuse_batch_async(dsm_ctx *ctx, int n, const int32_t *ref, const uint8_t *gray, const float *depth,
+                                    const float *poses, dsm_surfel_t *local, const int32_t *ofs,
+                                    dsm_surfel_t *new_out, int32_t *n_new)
+{
+    if (!ctx) return DSM_E_INVALID;
+    return fuse_batch_async(ctx, n, ref, gray, (size_t)ctx->p.width, depth, (size_t)ctx->p.width * 4, poses, local, ofs,
+                            new_out, n_new);
 }
 
 extern "C" int dsm_fuse_batch(dsm_ctx *ctx, int n, const int32_t *ref, const uint8_t *gray, const float *depth,
@@ -765,40 +780,19 @@ extern "C" int dsm_fuse_batch(dsm_ctx *ctx, int n, const int32_t *ref, const uin
     return dsm_batch_wait(ctx);
 }
 
+// one frame of fuse_batch_async with the caller's row pitches, then its wait
 extern "C" int dsm_fuse_frame(dsm_ctx *ctx, int ref_idx, const uint8_t *gray, size_t gray_pitch,
                               const float *depth, size_t depth_pitch, const float pose[16],
                               dsm_surfel_t *local, int n_local, dsm_surfel_t *new_out, int new_cap, int *n_new)
 {
     if (!ctx || !gray || !depth || !pose || n_local < 0 || new_cap < 0 || !n_new) return DSM_E_INVALID;
-    if (n_local > 0 && !local) return DSM_E_INVALID;
     if (new_cap > 0 && !new_out) return DSM_E_INVALID;
-    const int W = ctx->p.width, H = ctx->p.height;
-    if (gray_pitch < (size_t)W || depth_pitch < (size_t)W * 4) return DSM_E_INVALID;
-    CK(cudaSetDevice(ctx->device));
-    if (ctx->in_flight)
-    { // an asynchronous batch still owns the buffers: finish it first
-        int rcw = dsm_batch_wait(ctx);
-        if (rcw != DSM_OK) return rcw;
-    }
-    CK(cudaStreamSynchronize(ctx->stream));
-    ctx->res_active = false; // the caller's surfels replace whatever the pool buffer held (a resident pool included)
-    int32_t ref = ref_idx;
-    int rc = upload_tables(ctx, 1, &ref, pose, nullptr, n_local);
-    if (rc != DSM_OK) return rc;
-    CK(cudaMemcpy2DAsync(ctx->gray, ctx->d.Wp, gray, gray_pitch, W, H, cudaMemcpyHostToDevice, ctx->stream));
-    CK(cudaMemcpy2DAsync(ctx->depth, (size_t)ctx->d.Wp * 4, depth, depth_pitch, (size_t)W * 4, H, cudaMemcpyHostToDevice, ctx->stream));
-    if (n_local > 0)
-        CK(cudaMemcpyAsync(ctx->d.pool, local, (size_t)n_local * sizeof(dsm_surfel_t), cudaMemcpyHostToDevice, ctx->stream));
-    ctx->nb = 1;
-    ctx->uploaded = true;
-    ctx->img_slot0 = 0, ctx->img_n = 1, ctx->img_fit = false; // dsm_batch_run sets img_fit
-    rc = dsm_batch_run(ctx);
-    if (rc != DSM_OK) return rc;
-    if (n_local > 0)
-        CK(cudaMemcpyAsync(local, ctx->d.pool, (size_t)n_local * sizeof(dsm_surfel_t), cudaMemcpyDeviceToHost, ctx->stream));
+    if (gray_pitch < (size_t)ctx->p.width || depth_pitch < (size_t)ctx->p.width * 4) return DSM_E_INVALID;
+    const int32_t ref = ref_idx, ofs[2] = {0, n_local};
     int32_t cnt = 0;
-    CK(cudaMemcpyAsync(&cnt, ctx->d.nnew, sizeof(int32_t), cudaMemcpyDeviceToHost, ctx->stream));
-    CK(cudaStreamSynchronize(ctx->stream));
+    int rc = fuse_batch_async(ctx, 1, &ref, gray, gray_pitch, depth, depth_pitch, pose, local, ofs, nullptr, &cnt);
+    if (rc == DSM_OK) rc = dsm_batch_wait(ctx);
+    if (rc != DSM_OK) return rc;
     *n_new = cnt;
     const int ncopy = cnt < new_cap ? cnt : new_cap;
     if (ncopy > 0)
@@ -806,7 +800,6 @@ extern "C" int dsm_fuse_frame(dsm_ctx *ctx, int ref_idx, const uint8_t *gray, si
         CK(cudaMemcpyAsync(new_out, ctx->d.newsurf, (size_t)ncopy * sizeof(dsm_surfel_t), cudaMemcpyDeviceToHost, ctx->stream));
         CK(cudaStreamSynchronize(ctx->stream));
     }
-    CK(cudaGetLastError());
     return DSM_OK;
 }
 
@@ -1336,8 +1329,7 @@ static int stream_run(dsm_ctx *ctx, int n, const int32_t *ref_idx, const uint8_t
         if (rc != DSM_OK) return rc;
         if (cur + n * ctx->d.S > ctx->p.max_local_surfels) return DSM_E_CAPACITY;
     }
-    const int W = ctx->p.width, H = ctx->p.height;
-    const size_t fpx = (size_t)H * W;
+    const size_t fpx = (size_t)ctx->p.height * ctx->p.width;
     // two staging halves when they fit: the H2D copy of this run overlaps the kernels of the previous one
     const bool dbl = 2 * n <= ctx->p.max_batch;
     const int par = dbl ? (ctx->res_frame & 1) : 0;
@@ -1353,17 +1345,9 @@ static int stream_run(dsm_ctx *ctx, int n, const int32_t *ref_idx, const uint8_t
     CK(cudaEventSynchronize(ctx->half_free[par]));
     if (!dbl) CK(cudaEventSynchronize(ctx->half_free[1 - par]));
     const size_t so = (size_t)par * (size_t)(ctx->p.max_batch / 2); // fixed halves: runs of different length never overlap
-    uint8_t *gp = ctx->gray_packed + so * fpx;
-    float *dp = ctx->depth_packed + so * fpx;
-    // packed rows: one contiguous copy per image; padded rows: one 2-D copy into the same packed staging
-    if (gray_pitch == (size_t)W)
-        CK(cudaMemcpyAsync(gp, gray, (size_t)n * fpx, cudaMemcpyHostToDevice, ctx->s_h2d));
-    else
-        CK(cudaMemcpy2DAsync(gp, W, gray, gray_pitch, W, (size_t)n * H, cudaMemcpyHostToDevice, ctx->s_h2d));
-    if (depth_pitch == (size_t)W * 4)
-        CK(cudaMemcpyAsync(dp, depth, (size_t)n * fpx * sizeof(float), cudaMemcpyHostToDevice, ctx->s_h2d));
-    else
-        CK(cudaMemcpy2DAsync(dp, (size_t)W * 4, depth, depth_pitch, (size_t)W * 4, (size_t)n * H, cudaMemcpyHostToDevice, ctx->s_h2d));
+    const int slot0 = (int)so;
+    int rc = stage_images(ctx, slot0, n, gray, gray_pitch, depth, depth_pitch, ctx->s_h2d);
+    if (rc != DSM_OK) return rc;
     CK(cudaEventRecord(ctx->half_h2d[par], ctx->s_h2d));
     // Phase 1 (superpixels, normals, plane fits of all n frames; never touches the pool) runs on a side stream and in this
     // half's own frame slots [so, so + n): it overlaps the frame-by-frame phase 2 of the PREVIOUS run, which owns the
@@ -1373,7 +1357,6 @@ static int stream_run(dsm_ctx *ctx, int n, const int32_t *ref_idx, const uint8_t
     // main stream, which keeps the order with every other call on the context).
     cudaStream_t s1 = dbl ? ctx->s_comp[par] : st;
     cudaStream_t s2 = dbl ? ctx->s_hi : st;
-    const int slot0 = (int)so;
     if (dbl)
     { // this half's slots and device tables were last read by the phase 2 of the run before the previous one
         CK(cudaEventRecord(ctx->ev_fork, st));
@@ -1383,7 +1366,7 @@ static int stream_run(dsm_ctx *ctx, int n, const int32_t *ref_idx, const uint8_t
     // pinned tables of this mode live in the second half of h_pose / h_ref (the first half belongs to the batch calls,
     // which only wait for their own copies before rewriting it); this half's previous table copy ran before
     // half_free[par], which has been waited for above
-    int rc = stage_tables(ctx, (size_t)ctx->p.max_batch + so, slot0, n, poses, ref_idx, s1);
+    rc = stage_tables(ctx, (size_t)ctx->p.max_batch + so, slot0, n, poses, ref_idx, s1);
     if (rc != DSM_OK) return rc;
     const int tag = win ? (ctx->win_tag = ctx->win_tag % 0x3fffffff + 1) : 0;
     if (win)
@@ -1398,15 +1381,10 @@ static int stream_run(dsm_ctx *ctx, int n, const int32_t *ref_idx, const uint8_t
     v.max_pool_per_frame = 0;
     {
         ProfScope p(ctx, DSM_K_REPACK, s1);
-        dsm_launch_repack(v, n, gp, dp, s1);
+        dsm_launch_repack(v, n, ctx->gray_packed + so * fpx, ctx->depth_packed + so * fpx, s1);
     }
-    ctx->nb = slot0 + n;
-    ctx->uploaded = true;
-    ctx->img_slot0 = slot0, ctx->img_n = n; // ordered before the main stream through phase 2 (ev_join / ev_p2) below
-    ctx->img_fit = false;
     rc = enqueue_schedule(ctx, v, n, s1, 1);
     if (rc != DSM_OK) return rc;
-    ctx->img_fit = schedule_fits(ctx);
     if (dbl)
     {
         CK(cudaEventRecord(ctx->ev_join[par], s1));
@@ -1433,7 +1411,7 @@ static int stream_run(dsm_ctx *ctx, int n, const int32_t *ref_idx, const uint8_t
         ctx->res_upper += ctx->d.S;
     }
     if (win) ctx->win_pending = true;
-    ctx->ran = true;
+    hold_frames(ctx, slot0, n, true); // the slots are ordered before the main stream through phase 2 (ev_join / ev_p2)
     if (dbl)
     {
         CK(cudaEventRecord(ctx->ev_p2, s2));
@@ -1508,11 +1486,8 @@ extern "C" int dsm_frame_raw_cloud(dsm_ctx *ctx, int frame, const double pose7[7
     if (ctx->img_n == 0) return DSM_E_STATE;
     if (frame < 0 || frame >= ctx->img_n) return DSM_E_INVALID;
     CK(cudaSetDevice(ctx->device));
-    if (ctx->in_flight)
-    { // the chunks of dsm_fuse_batch_async copy and repack on their own streams: finish the batch first
-        int rcw = dsm_batch_wait(ctx);
-        if (rcw != DSM_OK) return rcw;
-    }
+    const int rc = finish_batch(ctx);
+    if (rc != DSM_OK) return rc;
     const int W = ctx->p.width, H = ctx->p.height;
     const size_t npx = (size_t)W * H;
     if (!ctx->raw_out && ctx->own.device(&ctx->raw_out, npx) != cudaSuccess)
@@ -1539,11 +1514,8 @@ extern "C" int dsm_frame_superpixel_image(dsm_ctx *ctx, int frame, uint8_t *bgr,
     if (frame < 0 || frame >= ctx->img_n) return DSM_E_INVALID;
     if (!ctx->img_fit) return DSM_E_STATE; // uploaded but not run, or run with the plane fit cut off
     CK(cudaSetDevice(ctx->device));
-    if (ctx->in_flight)
-    { // the chunks of dsm_fuse_batch_async run on their own streams: finish the batch first
-        int rcw = dsm_batch_wait(ctx);
-        if (rcw != DSM_OK) return rcw;
-    }
+    const int rc = finish_batch(ctx);
+    if (rc != DSM_OK) return rc;
     const int W = ctx->p.width, H = ctx->p.height;
     const size_t row = (size_t)3 * ctx->d.Wp; // staging row pitch: a multiple of 48 bytes, so every row is word-aligned
     if (!ctx->spimg_out && ctx->own.device(&ctx->spimg_out, row * H) != cudaSuccess)

@@ -106,7 +106,7 @@ struct dsm_ctx
     float *pose = nullptr, *ipose = nullptr;
     dsm_seed_t *seed_export = nullptr;
     float *kx = nullptr, *ky = nullptr;
-    // end-to-end pipeline (dsm_fuse_batch): packed staging + copy streams + per-chunk events
+    // packed staging of every call that takes images (stage_images; k_repack lays it out in gray / depth), copy streams
     uint8_t *gray_packed = nullptr; // [B][H][W]
     float *depth_packed = nullptr;  // [B][H][W]
     cudaStream_t s_h2d = nullptr, s_d2h = nullptr, s_comp[DSM_MAX_CHUNKS] = {};
@@ -146,9 +146,9 @@ struct dsm_ctx
     // the resident stream's staging halves: half_h2d[h] ends a run's input copy into half h; half_free[h] lies on the main
     // stream after every earlier use of half h (stream_run records it, see there)
     cudaEvent_t half_h2d[2] = {}, half_free[2] = {};
-    cudaEvent_t ev_fork = nullptr, ev_join[DSM_MAX_CHUNKS] = {}; // dsm_batch_run: fork / join of the concurrent sub-batches
+    cudaEvent_t ev_fork = nullptr, ev_join[DSM_MAX_CHUNKS] = {}; // run_parts: fork / join of the parts on s_comp
     // frame slots [img_slot0, img_slot0 + img_n) hold the images of the most recent call that took images (img_n == 0: none
-    // yet); dsm_frame_raw_cloud reads them, into raw_out (W*H points, allocated at its first call).  img_fit: that call's
+    // yet; hold_frames writes these with nb, uploaded and ran); dsm_frame_raw_cloud reads them, into raw_out (W*H points, allocated at its first call).  img_fit: that call's
     // schedule has run through the plane fit, so the slots' label codes and plane normals are complete;
     // dsm_frame_superpixel_image reads them, into spimg_out ([H][3*Wp] bytes, allocated at its first call)
     int img_slot0 = 0, img_n = 0;

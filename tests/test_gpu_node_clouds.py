@@ -99,7 +99,7 @@ def test_raw_cloud_after_fuse_frame_with_padded_pitches_and_errors():
     out = np.zeros(cam.width * cam.height, POINT_DTYPE)
     assert L.dsm_frame_raw_cloud(ctx.h, 0, p7.ctypes.data, out.ctypes.data, len(out), ctypes.byref(n)) == -7  # DSM_E_STATE
     pose, g, d = frames(cam, 1, 120)[0]
-    gp = np.zeros((cam.height, cam.width + 29), np.uint8)       # padded rows: the 2-D copy path, no repack
+    gp = np.zeros((cam.height, cam.width + 29), np.uint8)       # padded rows: a 2-D copy into the packed staging
     dp = np.zeros((cam.height, cam.width + 19), np.float32)
     gp[:, :cam.width], dp[:, :cam.width] = g, d
     new = np.zeros(ctx.S, SURFEL_DTYPE)

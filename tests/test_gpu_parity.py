@@ -175,27 +175,51 @@ def test_concurrent_sub_batches_do_not_change_results(capi):
 
 
 def test_pitched_input_and_errors(capi):
+    import ctypes
     cam = synth.VGA
     gray, depth = synth.make_frame(cam, 7)
-    gp = np.zeros((cam.height, cam.width + 24), np.uint8)
-    dp = np.zeros((cam.height, cam.width + 8), np.float32)
+    gp = np.full((cam.height, cam.width + 24), 0xEE, np.uint8)  # pad columns hold garbage the call must not read
+    dp = np.full((cam.height, cam.width + 8), 99.0, np.float32)
     gp[:, :cam.width] = gray
     dp[:, :cam.width] = depth
-    ctx = capi.Context(cam, max_batch=1, max_local_surfels=16)
-    import ctypes
-    new = np.zeros(ctx.S, SURFEL_DTYPE)
-    n = ctypes.c_int(0)
     pose = synth.identity_pose()
-    rc = ctx.lib.dsm_fuse_frame(ctx.h, 0, gp.ctypes.data, gp.strides[0], dp.ctypes.data, dp.strides[0],
-                                pose.ctypes.data, None, 0, new.ctypes.data, ctx.S, ctypes.byref(n))
-    assert rc == 0
+
+    def fuse_padded(ctx, local, new, cap):
+        n = ctypes.c_int(-1)
+        rc = ctx.lib.dsm_fuse_frame(ctx.h, 0, gp.ctypes.data, gp.strides[0], dp.ctypes.data, dp.strides[0], pose.ctypes.data,
+                                    local.ctypes.data if len(local) else None, len(local), new.ctypes.data, cap, ctypes.byref(n))
+        assert rc == 0
+        return n.value
+
+    ctx = capi.Context(cam, max_batch=1, max_local_surfels=16)
+    new = np.zeros(ctx.S, SURFEL_DTYPE)
+    n = fuse_padded(ctx, np.zeros(0, SURFEL_DTYPE), new, ctx.S)
     _, want = oracle_for(cam).fuse(0, gray, depth, pose, np.zeros(0, SURFEL_DTYPE))
-    check_surfels(new[:n.value], want, "pitched")
+    check_surfels(new[:n], want, "pitched")
+    pool = new[:n // 2].copy()  # covers part of the frame: the next fuse both fuses and initialises
     # capacity error: more local surfels than the context was created for
     with pytest.raises(capi.DsmError) as ei:
         ctx.fuse_frame(0, gray, depth, pose, np.zeros(17, SURFEL_DTYPE))
     assert ei.value.code == -6
     ctx.close()
+    # on a non-empty pool, padded rows give byte for byte what packed rows give; with new_cap below the count exactly
+    # new_cap surfels are written, the rest of the buffer is untouched and *n_new is the full count
+    for max_batch in (1, 8):
+        ctx = capi.Context(cam, max_batch=max_batch, max_local_surfels=1 << 16)
+        want_local, want_new = ctx.fuse_frame(0, gray, depth, pose, pool)
+        assert (want_local["update_times"] > 1).any() and len(want_new) > 1
+        want_labels, want_seeds = ctx.labels().tobytes(), ctx.seeds().tobytes()
+        local, new = pool.copy(), np.zeros(ctx.S, SURFEL_DTYPE)
+        assert fuse_padded(ctx, local, new, ctx.S) == len(want_new)
+        assert local.tobytes() == want_local.tobytes() and new[:len(want_new)].tobytes() == want_new.tobytes()
+        assert ctx.labels().tobytes() == want_labels and ctx.seeds().tobytes() == want_seeds
+        cap = len(want_new) // 2
+        local = pool.copy()
+        new = np.frombuffer(b"\xa5" * (ctx.S * SURFEL_DTYPE.itemsize), SURFEL_DTYPE).copy()
+        assert fuse_padded(ctx, local, new, cap) == len(want_new)
+        assert local.tobytes() == want_local.tobytes() and new[:cap].tobytes() == want_new[:cap].tobytes()
+        assert new[cap:].tobytes() == b"\xa5" * ((ctx.S - cap) * SURFEL_DTYPE.itemsize)
+        ctx.close()
     # shape error: W%8 > 4 is undefined behaviour in the reference (fusion_functions.cpp:408-451)
     bad = synth.Camera(645, 480, 525.0, 525.0, 319.5, 239.5, 0.5, 30.0)
     with pytest.raises(capi.DsmError) as ei:
