@@ -338,12 +338,16 @@ class Context:
         w = pose16(W_colmajor)
         self._ck(self.lib.dsm_pool_transform(self.h, _ptr(w)))
 
+    def _read(self, fn, dtype, cap, *args):
+        """fn(h, *args, out, cap, &n): the first min(n, cap) records the library wrote."""
+        out = np.zeros(max(cap, 1), dtype=dtype)
+        n = ctypes.c_int(0)
+        self._ck(fn(self.h, *args, _ptr(out), cap, ctypes.byref(n)))
+        return out[:min(n.value, cap)].copy()
+
     def pool_retire(self, keyframe_index, cap=None):
         cap = self.pool_size() if cap is None else cap
-        out = np.zeros(max(cap, 1), dtype=SURFEL_DTYPE)
-        n = ctypes.c_int(0)
-        self._ck(self.lib.dsm_pool_retire(self.h, int(keyframe_index), _ptr(out), cap, ctypes.byref(n)))
-        return out[:min(n.value, cap)].copy()
+        return self._read(self.lib.dsm_pool_retire, SURFEL_DTYPE, cap, int(keyframe_index))
 
     def pool_append(self, surfels):
         surfels = np.ascontiguousarray(surfels, dtype=SURFEL_DTYPE)
@@ -363,17 +367,12 @@ class Context:
 
     def pool_export_cloud(self, min_update_times=5, cap=None):
         """publish_active_pointcloud & co. (surfel_map.cpp:1398-1417): POINT_DTYPE array in pool order."""
-        return self._pool_export(self.lib.dsm_pool_export_cloud, POINT_DTYPE, min_update_times, cap)
+        cap = self.pool_size() if cap is None else cap
+        return self._read(self.lib.dsm_pool_export_cloud, POINT_DTYPE, cap, int(min_update_times))
 
     def pool_export_surfels(self, min_update_times=5, cap=None):
-        return self._pool_export(self.lib.dsm_pool_export_surfels, SURFEL_DTYPE, min_update_times, cap)
-
-    def _pool_export(self, fn, dtype, min_update_times, cap):
         cap = self.pool_size() if cap is None else cap
-        out = np.zeros(max(cap, 1), dtype=dtype)
-        n = ctypes.c_int(0)
-        self._ck(fn(self.h, int(min_update_times), _ptr(out), cap, ctypes.byref(n)))
-        return out[:min(n.value, cap)].copy()
+        return self._read(self.lib.dsm_pool_export_surfels, SURFEL_DTYPE, cap, int(min_update_times))
 
     # ---- inactive store ----
     def inactive_reserve(self, n):
@@ -399,28 +398,17 @@ class Context:
         return a.value, b.value
 
     def inactive_download(self, keyframe_index=-1):
-        cap = self.inactive_size()[0]
-        out = np.zeros(max(cap, 1), dtype=SURFEL_DTYPE)
-        n = ctypes.c_int(0)
-        self._ck(self.lib.dsm_inactive_download(self.h, int(keyframe_index), _ptr(out), cap, ctypes.byref(n)))
-        return out[:min(n.value, cap)].copy()
+        return self._read(self.lib.dsm_inactive_download, SURFEL_DTYPE, self.inactive_size()[0], int(keyframe_index))
 
     def inactive_export_cloud(self):
-        cap = self.inactive_size()[0]
-        out = np.zeros(max(cap, 1), dtype=POINT_DTYPE)
-        n = ctypes.c_int(0)
-        self._ck(self.lib.dsm_inactive_export_cloud(self.h, _ptr(out), cap, ctypes.byref(n)))
-        return out[:min(n.value, cap)].copy()
+        return self._read(self.lib.dsm_inactive_export_cloud, POINT_DTYPE, self.inactive_size()[0])
 
     def inactive_export_poses(self, keyframes, cap=None):
         """The inactive half of publish_neighbor_pointcloud (surfel_map.cpp:1306-1321): the stored points of each listed
         keyframe, list order; keyframes with nothing stored contribute nothing.  POINT_DTYPE array."""
         kf = np.ascontiguousarray(keyframes, dtype=np.int32).reshape(-1)
         cap = self.inactive_size()[0] if cap is None else cap
-        out = np.zeros(max(cap, 1), dtype=POINT_DTYPE)
-        n = ctypes.c_int(0)
-        self._ck(self.lib.dsm_inactive_export_poses(self.h, _ptr(kf) if len(kf) else None, len(kf), _ptr(out), cap, ctypes.byref(n)))
-        return out[:min(n.value, cap)].copy()
+        return self._read(self.lib.dsm_inactive_export_poses, POINT_DTYPE, cap, _ptr(kf) if len(kf) else None, len(kf))
 
     # ---- raw cloud of a frame ----
     def frame_raw_cloud(self, frame, pose7, cap=None):
@@ -429,10 +417,7 @@ class Context:
         p = np.ascontiguousarray(pose7, dtype=np.float64).reshape(7)
         npx = self.cam.width * self.cam.height
         cap = npx if cap is None else cap
-        out = np.zeros(max(cap, 1), dtype=POINT_DTYPE)
-        n = ctypes.c_int(0)
-        self._ck(self.lib.dsm_frame_raw_cloud(self.h, int(frame), _ptr(p), _ptr(out), cap, ctypes.byref(n)))
-        return out[:min(n.value, cap)].copy()
+        return self._read(self.lib.dsm_frame_raw_cloud, POINT_DTYPE, cap, int(frame), _ptr(p))
 
     # ---- superpixel normal image of a frame ----
     def superpixel_image(self, frame=0, pitch=None):

@@ -831,25 +831,25 @@ static int res_sync(dsm_ctx *ctx, int nseg_hint = 0)
     if (!ctx->win_pending) return DSM_OK;
     CK(cudaSetDevice(ctx->device));
     int32_t *h = ctx->h_sync, *hdr = ctx->h_sync + 4; // pinned, so these copies do not wait for the stream one by one
-    std::vector<int4> t(ctx->inact ? (size_t)std::min(nseg_hint, ctx->inact_cap) : 0);
+    InactStore *store = ctx->inact.get();
+    std::vector<int4> t(store ? (size_t)std::min(nseg_hint, store->cap) : 0);
     CK(cudaMemcpyAsync(h, ctx->res_ofs, 4 * sizeof(int32_t), cudaMemcpyDeviceToHost, ctx->stream));
     CK(cudaMemcpyAsync(hdr, ctx->win_hdr, 4 * sizeof(int32_t), cudaMemcpyDeviceToHost, ctx->stream));
-    if (!t.empty()) CK(cudaMemcpyAsync(t.data(), ctx->inact_seg.get(), t.size() * sizeof(int4), cudaMemcpyDeviceToHost, ctx->stream));
+    if (!t.empty()) CK(cudaMemcpyAsync(t.data(), store->seg, t.size() * sizeof(int4), cudaMemcpyDeviceToHost, ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
     CK(cudaGetLastError());
-    if (ctx->inact)
+    if (store)
     {
         const size_t read = t.size();
         t.resize((size_t)hdr[1]);
         if (t.size() > read)
         {
-            CK(cudaMemcpyAsync(t.data() + read, ctx->inact_seg.get() + 4 * read, (t.size() - read) * sizeof(int4),
-                               cudaMemcpyDeviceToHost, ctx->stream));
+            CK(cudaMemcpyAsync(t.data() + read, store->seg + read, (t.size() - read) * sizeof(int4), cudaMemcpyDeviceToHost, ctx->stream));
             CK(cudaStreamSynchronize(ctx->stream));
         }
-        ctx->inact_segs.clear();
-        for (const int4 &g : t) ctx->inact_segs.push_back(dsm_ctx::InactSeg{g.x, g.y, g.z});
-        ctx->inact_size = ctx->inact_upper = hdr[0];
+        store->segs.clear();
+        for (const int4 &g : t) store->segs.push_back(InactStore::Seg{g.x, g.y, g.z});
+        store->size = store->upper = hdr[0];
     }
     ctx->res_upper = h[1];
     ctx->win_pending = false;
@@ -868,16 +868,15 @@ static DsmWin window_view(dsm_ctx *ctx, int half, int t, int S)
     DsmWin w{};
     w.tab = ctx->d_win + (size_t)half * ctx->win_len;
     w.t = t, w.B = ctx->p.max_batch;
-    w.store = ctx->inact.get();
-    w.seg = reinterpret_cast<int4 *>(ctx->inact_seg.get());
     w.hdr = ctx->win_hdr;
     w.res = ctx->res_ofs;
-    w.blk = ctx->win_blk.get();
-    w.sync = ctx->win_sync.get();
-    w.blk_stride = ctx->win_blk_stride;
     w.pool_cap = ctx->p.max_local_surfels;
-    w.store_cap = ctx->inact_cap;
     w.S = S;
+    if (const InactStore *s = ctx->inact.get())
+    {
+        w.store = s->surfels, w.seg = s->seg, w.blk = s->blk, w.sync = s->sync;
+        w.blk_stride = s->blk_stride, w.store_cap = s->cap;
+    }
     return w;
 }
 
@@ -907,6 +906,61 @@ static int stage_window(dsm_ctx *ctx, int half, int n, const WinLists &w, int ta
     return DSM_OK;
 }
 
+// The entry of the calls on the resident pool and the inactive store, after their own argument checks: the state they
+// need (`need`: NEED_POOL, NEED_STORE), then res_sync, then the device
+enum { NEED_POOL = 1, NEED_STORE = 2 };
+static int res_enter(dsm_ctx *ctx, int need)
+{
+    if (((need & NEED_POOL) && !ctx->res_active) || ((need & NEED_STORE) && !ctx->inact)) return DSM_E_STATE;
+    const int rs = res_sync(ctx);
+    if (rs != DSM_OK) return rs;
+    CK(cudaSetDevice(ctx->device));
+    return DSM_OK;
+}
+
+// res_ofs = {0, n} after the copies already on the stream; waits, so the caller's source buffers are free on return
+static int set_pool_size(dsm_ctx *ctx, int n)
+{
+    ctx->h_ofs[0] = 0;
+    ctx->h_ofs[1] = n;
+    CK(cudaMemcpyAsync(ctx->res_ofs, ctx->h_ofs, 2 * sizeof(int32_t), cudaMemcpyHostToDevice, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    ctx->res_upper = n;
+    return DSM_OK;
+}
+
+// The ordered selection (mode / key as pool_pred) over the range of view d into pool_snap, and its first min(cap, n)
+// records to `out`, n being its count.  With n_out, n is read back into *n_out and the call waits for the copy.  Without
+// it, the caller knows that all `cap` records of the range are selected, and nothing waits.  Mode 1 (retire) flags what
+// it selects dead, so it scatters only after the count has been checked against cap: DSM_E_CAPACITY leaves the pool as
+// it was.
+static int select_out(dsm_ctx *ctx, const DsmDev &d, int upper, int mode, int key, DsmRec rec, void *out, int cap, int *n_out)
+{
+    const bool retire = mode == 1;
+    dsm_launch_pool_select(d, 0, upper, mode, key, rec, retire ? nullptr : ctx->pool_snap, ctx->blkcnt, ctx->blkofs, ctx->nsel, ctx->stream);
+    int n = cap;
+    if (n_out)
+    {
+        CK(cudaMemcpyAsync(&n, ctx->nsel, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+        CK(cudaStreamSynchronize(ctx->stream));
+        CK(cudaGetLastError());
+        *n_out = n;
+    }
+    if (retire)
+    {
+        if (n > cap) return DSM_E_CAPACITY; // call again with cap >= *n_out
+        dsm_launch_pool_select(d, 0, upper, mode, key, rec, ctx->pool_snap, ctx->blkcnt, ctx->blkofs, ctx->nsel, ctx->stream,
+                               DSM_SEL_SCATTER_ONLY);
+        CK(cudaGetLastError());
+    }
+    const int c = std::min(n, cap);
+    if (c <= 0) return DSM_OK;
+    const size_t bytes = (size_t)c * (rec == DSM_REC_POINT ? sizeof(dsm_point_t) : sizeof(dsm_surfel_t));
+    CK(cudaMemcpyAsync(out, ctx->pool_snap, bytes, cudaMemcpyDeviceToHost, ctx->stream));
+    if (n_out) CK(cudaStreamSynchronize(ctx->stream));
+    return DSM_OK;
+}
+
 extern "C" int dsm_pool_upload(dsm_ctx *ctx, const dsm_surfel_t *local, int n)
 {
     if (!ctx || n < 0 || (n > 0 && !local)) return DSM_E_INVALID;
@@ -917,11 +971,8 @@ extern "C" int dsm_pool_upload(dsm_ctx *ctx, const dsm_surfel_t *local, int n)
     if (rs != DSM_OK && rs != DSM_E_CAPACITY) return rs;
     CK(cudaStreamSynchronize(ctx->stream));
     if (n > 0) CK(cudaMemcpyAsync(ctx->d.pool, local, (size_t)n * sizeof(dsm_surfel_t), cudaMemcpyHostToDevice, ctx->stream));
-    ctx->h_ofs[0] = 0;
-    ctx->h_ofs[1] = n;
-    CK(cudaMemcpyAsync(ctx->res_ofs, ctx->h_ofs, 2 * sizeof(int32_t), cudaMemcpyHostToDevice, ctx->stream));
-    CK(cudaStreamSynchronize(ctx->stream)); // `local` may be pageable / reused by the caller
-    ctx->res_upper = n;
+    const int rc = set_pool_size(ctx, n); // `local` may be pageable / reused by the caller
+    if (rc != DSM_OK) return rc;
     ctx->res_active = true;
     ctx->n_pool = n;
     return DSM_OK;
@@ -930,10 +981,8 @@ extern "C" int dsm_pool_upload(dsm_ctx *ctx, const dsm_surfel_t *local, int n)
 extern "C" int dsm_pool_size(dsm_ctx *ctx, int *n)
 {
     if (!ctx || !n) return DSM_E_INVALID;
-    if (!ctx->res_active) return DSM_E_STATE;
-    int rs = res_sync(ctx);
-    if (rs != DSM_OK) return rs;
-    CK(cudaSetDevice(ctx->device));
+    const int rc = res_enter(ctx, NEED_POOL);
+    if (rc != DSM_OK) return rc;
     int32_t h[2] = {0, 0};
     CK(cudaMemcpyAsync(h, ctx->res_ofs, 2 * sizeof(int32_t), cudaMemcpyDeviceToHost, ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
@@ -956,83 +1005,37 @@ extern "C" int dsm_pool_download(dsm_ctx *ctx, dsm_surfel_t *out, int cap, int *
     return DSM_OK;
 }
 
+// retire (mode 1) and the publish_*_pointcloud / save_cloud / save_mesh filters (mode 2) on the resident pool (see
+// include/dsm.h), ordered through select_out
+static int pool_select(dsm_ctx *ctx, int mode, int key, DsmRec rec, void *out, int cap, int *n_out)
+{
+    if (!ctx || !n_out || cap < 0 || (cap > 0 && !out)) return DSM_E_INVALID;
+    const int rc = res_enter(ctx, NEED_POOL);
+    return rc != DSM_OK ? rc : select_out(ctx, resident_view(ctx, 0), ctx->res_upper, mode, key, rec, out, cap, n_out);
+}
 extern "C" int dsm_pool_retire(dsm_ctx *ctx, int kf, dsm_surfel_t *out, int cap, int *n_out)
 {
-    if (!ctx || !n_out || cap < 0 || (cap > 0 && !out)) return DSM_E_INVALID;
-    if (!ctx->res_active) return DSM_E_STATE;
-    int rs = res_sync(ctx);
-    if (rs != DSM_OK) return rs;
-    CK(cudaSetDevice(ctx->device));
-    // count first: nothing is flagged dead unless every retired surfel fits the caller's buffer
-    int32_t h[1] = {0};
-    dsm_launch_pool_retire(resident_view(ctx, 0), 0, ctx->res_upper, kf, ctx->blkcnt, ctx->blkofs, ctx->nsel, nullptr, ctx->stream);
-    CK(cudaMemcpyAsync(h, ctx->nsel, sizeof(int32_t), cudaMemcpyDeviceToHost, ctx->stream));
-    CK(cudaStreamSynchronize(ctx->stream));
-    CK(cudaGetLastError());
-    *n_out = h[0];
-    if (h[0] > cap) return DSM_E_CAPACITY; // pool untouched; call again with cap >= *n_out
-    // the second pool buffer (pool_snap) is the ordered output
-    dsm_launch_pool_retire(resident_view(ctx, 0), 0, ctx->res_upper, kf, ctx->blkcnt, ctx->blkofs, ctx->nsel, ctx->pool_snap, ctx->stream);
-    CK(cudaGetLastError());
-    const int c = h[0] < cap ? h[0] : cap;
-    if (c > 0)
-    {
-        CK(cudaMemcpyAsync(out, ctx->pool_snap, (size_t)c * sizeof(dsm_surfel_t), cudaMemcpyDeviceToHost, ctx->stream));
-        CK(cudaStreamSynchronize(ctx->stream));
-    }
-    return DSM_OK;
-}
-
-// publish_*_pointcloud / save_cloud / save_mesh filters on the resident pool (see include/dsm.h)
-static int pool_export(dsm_ctx *ctx, int min_ut, bool as_cloud, void *out, int cap, int *n_out)
-{
-    if (!ctx || !n_out || cap < 0 || (cap > 0 && !out)) return DSM_E_INVALID;
-    if (!ctx->res_active) return DSM_E_STATE;
-    int rs = res_sync(ctx);
-    if (rs != DSM_OK) return rs;
-    CK(cudaSetDevice(ctx->device));
-    // the second pool buffer (pool_snap) is the ordered output (16 or 44 bytes per selected surfel)
-    dsm_launch_pool_export(resident_view(ctx, 0), 0, ctx->res_upper, 2, min_ut, as_cloud, ctx->blkcnt, ctx->blkofs, ctx->nsel,
-                           ctx->pool_snap, ctx->stream);
-    int32_t h[1] = {0};
-    CK(cudaMemcpyAsync(h, ctx->nsel, sizeof(int32_t), cudaMemcpyDeviceToHost, ctx->stream));
-    CK(cudaStreamSynchronize(ctx->stream));
-    CK(cudaGetLastError());
-    *n_out = h[0];
-    const int c = h[0] < cap ? h[0] : cap;
-    if (c > 0)
-    {
-        const size_t rec = as_cloud ? sizeof(dsm_point_t) : sizeof(dsm_surfel_t);
-        CK(cudaMemcpyAsync(out, ctx->pool_snap, (size_t)c * rec, cudaMemcpyDeviceToHost, ctx->stream));
-        CK(cudaStreamSynchronize(ctx->stream));
-    }
-    return DSM_OK;
+    return pool_select(ctx, 1, kf, DSM_REC_SURFEL, out, cap, n_out);
 }
 extern "C" int dsm_pool_export_cloud(dsm_ctx *ctx, int min_update_times, dsm_point_t *out, int cap, int *n_out)
 {
-    return pool_export(ctx, min_update_times, true, out, cap, n_out);
+    return pool_select(ctx, 2, min_update_times, DSM_REC_POINT, out, cap, n_out);
 }
 extern "C" int dsm_pool_export_surfels(dsm_ctx *ctx, int min_update_times, dsm_surfel_t *out, int cap, int *n_out)
 {
-    return pool_export(ctx, min_update_times, false, out, cap, n_out);
+    return pool_select(ctx, 2, min_update_times, DSM_REC_SURFEL, out, cap, n_out);
 }
 
 extern "C" int dsm_pool_append(dsm_ctx *ctx, const dsm_surfel_t *surfels, int n)
 {
     if (!ctx || n < 0 || (n > 0 && !surfels)) return DSM_E_INVALID;
-    if (!ctx->res_active) return DSM_E_STATE;
     int cur = 0;
     int rc = dsm_pool_size(ctx, &cur);
     if (rc != DSM_OK) return rc;
     if (cur + n > ctx->p.max_local_surfels) return DSM_E_CAPACITY;
     if (n == 0) return DSM_OK;
     CK(cudaMemcpyAsync(ctx->d.pool + cur, surfels, (size_t)n * sizeof(dsm_surfel_t), cudaMemcpyHostToDevice, ctx->stream));
-    ctx->h_ofs[0] = 0;
-    ctx->h_ofs[1] = cur + n;
-    CK(cudaMemcpyAsync(ctx->res_ofs, ctx->h_ofs, 2 * sizeof(int32_t), cudaMemcpyHostToDevice, ctx->stream));
-    CK(cudaStreamSynchronize(ctx->stream));
-    ctx->res_upper = cur + n;
-    return DSM_OK;
+    return set_pool_size(ctx, cur + n);
 }
 
 extern "C" int dsm_pool_transform(dsm_ctx *ctx, const float Wm[16])
@@ -1051,8 +1054,8 @@ static DsmDev inactive_view(dsm_ctx *ctx)
 {
     DsmDev d = ctx->d;
     d.frame0 = 0;
-    d.pool = ctx->inact.get();
-    d.poolofs = ctx->inact_ofs; // {first, last} of the range a call works on, set in stream order by k_set2
+    d.pool = ctx->inact->surfels;
+    d.poolofs = ctx->inact->range;
     return d;
 }
 
@@ -1061,52 +1064,26 @@ extern "C" int dsm_inactive_reserve(dsm_ctx *ctx, int max_inactive_surfels)
     if (!ctx || max_inactive_surfels < 1) return DSM_E_INVALID;
     int rs = res_sync(ctx);
     if (rs != DSM_OK) return rs;
-    if (ctx->inact_size > 0) return DSM_E_STATE;
+    if (ctx->inact && ctx->inact->size > 0) return DSM_E_STATE;
     CK(cudaSetDevice(ctx->device));
     CK(cudaStreamSynchronize(ctx->stream));
-    ctx->inact.reset();
-    ctx->inact_seg.reset();
-    ctx->win_blk.reset();
-    ctx->win_sync.reset();
-    ctx->inact_cap = 0;
-    if (!ctx->inact_ofs && ctx->own.device(&ctx->inact_ofs, 2, true) != cudaSuccess) return DSM_E_NOMEM;
-    const size_t bytes = (size_t)max_inactive_surfels * sizeof(dsm_surfel_t);
-    void *p = nullptr;
-    cudaError_t e = cudaMalloc(&p, bytes);
-    if (e == cudaSuccess)
-    {
-        ctx->inact.reset(static_cast<dsm_surfel_t *>(p));
-        e = cudaMemset(p, 0, bytes);
-    }
-    // the device side of the window step: segment table, per-key block counts over the pool, compaction flags (zero)
-    const int npool = ctx->p.max_local_surfels > 0 ? ctx->p.max_local_surfels : 1;
-    const size_t lens[3] = {(size_t)max_inactive_surfels * 4, (size_t)DSM_WINDOW_MAX_KEYS * (npool / 256 + 1),
-                            dsm_win_sync_len(max_inactive_surfels)};
-    DevPtr<int32_t> *bufs[3] = {&ctx->inact_seg, &ctx->win_blk, &ctx->win_sync};
-    for (int i = 0; i < 3 && e == cudaSuccess; i++)
-    {
-        p = nullptr;
-        e = cudaMalloc(&p, lens[i] * sizeof(int32_t));
-        if (e == cudaSuccess)
-        {
-            bufs[i]->reset(static_cast<int32_t *>(p));
-            e = cudaMemset(p, 0, lens[i] * sizeof(int32_t));
-        }
-    }
+    ctx->inact.reset(); // before the new store is allocated: the two need not fit at once
+    auto s = std::make_unique<InactStore>();
+    const int cap = max_inactive_surfels, npool = std::max(ctx->p.max_local_surfels, 1);
+    s->cap = cap;
+    s->blk_stride = npool / 256 + 1;
+    cudaError_t e = s->own.device(&s->surfels, cap, true);
+    if (e == cudaSuccess) e = s->own.device(&s->seg, cap, true);
+    if (e == cudaSuccess) e = s->own.device(&s->blk, (size_t)DSM_WINDOW_MAX_KEYS * s->blk_stride, true);
+    if (e == cudaSuccess) e = s->own.device(&s->sync, dsm_win_sync_len(cap), true);
+    if (e == cudaSuccess) e = s->own.device(&s->range, 2, true);
     if (e == cudaSuccess) e = cudaMemset(ctx->win_hdr, 0, 4 * sizeof(int32_t));
     if (e != cudaSuccess)
     {
         cudaGetLastError();
-        ctx->inact.reset();
-        ctx->inact_seg.reset();
-        ctx->win_blk.reset();
-        ctx->win_sync.reset();
         return DSM_E_NOMEM;
     }
-    ctx->win_blk_stride = npool / 256 + 1;
-    ctx->inact_cap = max_inactive_surfels;
-    ctx->inact_upper = 0;
-    ctx->inact_segs.clear();
+    ctx->inact = std::move(s);
     return DSM_OK;
 }
 
@@ -1115,8 +1092,9 @@ extern "C" int dsm_inactive_size(dsm_ctx *ctx, int *n_surfels, int *n_segments)
     if (!ctx) return DSM_E_INVALID;
     int rs = res_sync(ctx);
     if (rs != DSM_OK) return rs;
-    if (n_surfels) *n_surfels = ctx->inact_size;
-    if (n_segments) *n_segments = (int)ctx->inact_segs.size();
+    const InactStore *s = ctx->inact.get();
+    if (n_surfels) *n_surfels = s ? s->size : 0;
+    if (n_segments) *n_segments = s ? (int)s->segs.size() : 0;
     return DSM_OK;
 }
 
@@ -1131,7 +1109,7 @@ static int inactive_step(dsm_ctx *ctx, int kf, bool react)
     const WinLists w = react ? WinLists{nullptr, nullptr, &kf, ofs} : WinLists{&kf, ofs, nullptr, nullptr};
     const int rc = stage_window(ctx, 0, 1, w, 0, ctx->stream);
     if (rc != DSM_OK) return rc;
-    const int nseg = (int)ctx->inact_segs.size();
+    const int nseg = (int)ctx->inact->segs.size();
     dsm_launch_window_step(resident_view(ctx, 0), window_view(ctx, 0, 0, 0), ctx->res_upper, react ? 0 : 1, react ? 1 : 0, ctx->stream);
     CK(cudaGetLastError());
     ctx->win_pending = true;
@@ -1142,16 +1120,17 @@ static int inactive_step(dsm_ctx *ctx, int kf, bool react)
 extern "C" int dsm_inactive_retire(dsm_ctx *ctx, int kf, int *n_moved)
 {
     if (!ctx) return DSM_E_INVALID;
-    if (!ctx->res_active || !ctx->inact) return DSM_E_STATE;
-    CK(cudaSetDevice(ctx->device));
-    int cur = 0;
-    int rc = dsm_pool_size(ctx, &cur); // exact pool size: bounds the segment
+    int rc = res_enter(ctx, NEED_POOL | NEED_STORE);
     if (rc != DSM_OK) return rc;
-    if (ctx->inact_size + cur > ctx->inact_cap) return DSM_E_CAPACITY;
-    const int before = ctx->inact_size;
+    int cur = 0;
+    rc = dsm_pool_size(ctx, &cur); // exact pool size: bounds the segment
+    if (rc != DSM_OK) return rc;
+    const InactStore &s = *ctx->inact;
+    if (s.size + cur > s.cap) return DSM_E_CAPACITY;
+    const int before = s.size;
     rc = inactive_step(ctx, kf, false);
     if (rc != DSM_OK) return rc;
-    if (n_moved) *n_moved = ctx->inact_size - before;
+    if (n_moved) *n_moved = s.size - before;
     return DSM_OK;
 }
 
@@ -1159,17 +1138,15 @@ extern "C" int dsm_inactive_retire(dsm_ctx *ctx, int kf, int *n_moved)
 extern "C" int dsm_inactive_reactivate(dsm_ctx *ctx, int kf, int *n_moved)
 {
     if (!ctx) return DSM_E_INVALID;
-    if (!ctx->res_active || !ctx->inact) return DSM_E_STATE;
-    int rs = res_sync(ctx);
-    if (rs != DSM_OK) return rs;
-    CK(cudaSetDevice(ctx->device));
+    int rc = res_enter(ctx, NEED_POOL | NEED_STORE);
+    if (rc != DSM_OK) return rc;
     int total = 0;
-    for (const auto &sg : ctx->inact_segs)
+    for (const auto &sg : ctx->inact->segs)
         if (sg.kf == kf) total += sg.cnt;
     if (n_moved) *n_moved = total;
     if (total == 0) return DSM_OK;
     int cur = 0;
-    int rc = dsm_pool_size(ctx, &cur);
+    rc = dsm_pool_size(ctx, &cur);
     if (rc != DSM_OK) return rc;
     if (cur + total > ctx->p.max_local_surfels) return DSM_E_CAPACITY;
     return inactive_step(ctx, kf, true);
@@ -1193,16 +1170,14 @@ extern "C" int dsm_inactive_transform(dsm_ctx *ctx, int kf, const float Wm[16])
 extern "C" int dsm_inactive_download(dsm_ctx *ctx, int kf, dsm_surfel_t *out, int cap, int *n_out)
 {
     if (!ctx || !n_out || cap < 0 || (cap > 0 && !out)) return DSM_E_INVALID;
-    if (!ctx->inact) return DSM_E_STATE;
-    int rs = res_sync(ctx);
-    if (rs != DSM_OK) return rs;
-    CK(cudaSetDevice(ctx->device));
+    const int rc = res_enter(ctx, NEED_STORE);
+    if (rc != DSM_OK) return rc;
     int n = 0;
-    for (const auto &sg : ctx->inact_segs)
+    for (const auto &sg : ctx->inact->segs)
     {
         if (kf >= 0 && sg.kf != kf) continue;
         const int c = (n + sg.cnt <= cap) ? sg.cnt : (cap > n ? cap - n : 0);
-        if (c > 0) CK(cudaMemcpyAsync(out + n, ctx->inact.get() + sg.ofs, (size_t)c * sizeof(dsm_surfel_t), cudaMemcpyDeviceToHost, ctx->stream));
+        if (c > 0) CK(cudaMemcpyAsync(out + n, ctx->inact->surfels + sg.ofs, (size_t)c * sizeof(dsm_surfel_t), cudaMemcpyDeviceToHost, ctx->stream));
         n += sg.cnt;
     }
     CK(cudaStreamSynchronize(ctx->stream));
@@ -1212,24 +1187,22 @@ extern "C" int dsm_inactive_download(dsm_ctx *ctx, int kf, dsm_surfel_t *out, in
 
 // The store ranges [ofs, ofs + cnt) as one PointXYZI per stored surfel, concatenated in list order: *n_out = their total,
 // the first min(cap, total) points are written
-static int inactive_export_ranges(dsm_ctx *ctx, const std::vector<dsm_ctx::InactSeg> &ranges, dsm_point_t *out, int cap, int *n_out)
+static int inactive_export_ranges(dsm_ctx *ctx, const std::vector<InactStore::Seg> &ranges, dsm_point_t *out, int cap, int *n_out)
 {
-    CK(cudaSetDevice(ctx->device));
     int total = 0;
     for (const auto &r : ranges) total += r.cnt;
     *n_out = total;
-    const int npool = ctx->p.max_local_surfels > 0 ? ctx->p.max_local_surfels : 1;
+    const int npool = std::max(ctx->p.max_local_surfels, 1);
     const DsmDev d = inactive_view(ctx);
     int n = 0;
     for (const auto &r : ranges)
         for (int c0 = 0; c0 < r.cnt && n < cap;)
         { // chunks sized for the block tables and the second pool buffer (16-byte points into 44-byte slots)
-            int len = r.cnt - c0;
-            if (len > npool) len = npool;
-            if (len > cap - n) len = cap - n;
-            dsm_launch_set2(ctx->inact_ofs, r.ofs + c0, r.ofs + c0 + len, ctx->stream);
-            dsm_launch_pool_export(d, 0, len, 2, INT32_MIN, true, ctx->blkcnt, ctx->blkofs, ctx->nsel, ctx->pool_snap, ctx->stream);
-            CK(cudaMemcpyAsync(out + n, ctx->pool_snap, (size_t)len * sizeof(dsm_point_t), cudaMemcpyDeviceToHost, ctx->stream));
+            const int len = std::min({r.cnt - c0, npool, cap - n});
+            dsm_launch_set2(ctx->inact->range, r.ofs + c0, r.ofs + c0 + len, ctx->stream);
+            // every stored surfel passes update_times >= INT32_MIN: all len points are selected
+            const int rc = select_out(ctx, d, len, 2, INT32_MIN, DSM_REC_POINT, out + n, len, nullptr);
+            if (rc != DSM_OK) return rc;
             c0 += len;
             n += len;
         }
@@ -1243,10 +1216,8 @@ static int inactive_export_ranges(dsm_ctx *ctx, const std::vector<dsm_ctx::Inact
 extern "C" int dsm_inactive_export_cloud(dsm_ctx *ctx, dsm_point_t *out, int cap, int *n_out)
 {
     if (!ctx || !n_out || cap < 0 || (cap > 0 && !out)) return DSM_E_INVALID;
-    if (!ctx->inact) return DSM_E_STATE;
-    int rs = res_sync(ctx);
-    if (rs != DSM_OK) return rs;
-    return inactive_export_ranges(ctx, {dsm_ctx::InactSeg{-1, 0, ctx->inact_size}}, out, cap, n_out);
+    const int rc = res_enter(ctx, NEED_STORE);
+    return rc != DSM_OK ? rc : inactive_export_ranges(ctx, {InactStore::Seg{-1, 0, ctx->inact->size}}, out, cap, n_out);
 }
 
 // the inactive half of publish_neighbor_pointcloud (surfel_map.cpp:1306-1321): the stored points of each listed
@@ -1255,12 +1226,11 @@ extern "C" int dsm_inactive_export_cloud(dsm_ctx *ctx, dsm_point_t *out, int cap
 extern "C" int dsm_inactive_export_poses(dsm_ctx *ctx, const int32_t *keyframes, int n_keyframes, dsm_point_t *out, int cap, int *n_out)
 {
     if (!ctx || !n_out || n_keyframes < 0 || (n_keyframes > 0 && !keyframes) || cap < 0 || (cap > 0 && !out)) return DSM_E_INVALID;
-    if (!ctx->inact) return DSM_E_STATE;
-    int rs = res_sync(ctx);
-    if (rs != DSM_OK) return rs;
-    std::vector<dsm_ctx::InactSeg> ranges;
+    const int rc = res_enter(ctx, NEED_STORE);
+    if (rc != DSM_OK) return rc;
+    std::vector<InactStore::Seg> ranges;
     for (int k = 0; k < n_keyframes; k++)
-        for (const auto &sg : ctx->inact_segs)
+        for (const auto &sg : ctx->inact->segs)
             if (sg.kf == keyframes[k]) ranges.push_back(sg);
     return inactive_export_ranges(ctx, ranges, out, cap, n_out);
 }
@@ -1397,8 +1367,9 @@ static int stream_run(dsm_ctx *ctx, int n, const int32_t *ref_idx, const uint8_t
         if (win)
         { // host bounds without readback: a retire can move at most the pool, a reactivation at most the store
             const int nr = list_len(win->ro, t), na = list_len(win->ao, t);
-            if (nr > 0) ctx->inact_upper = (int)std::min<long long>((long long)ctx->inact_upper + ctx->res_upper, ctx->inact_cap);
-            if (na > 0) ctx->res_upper = (int)std::min<long long>((long long)ctx->res_upper + ctx->inact_upper, cap);
+            InactStore *s = ctx->inact.get(); // present whenever a list is not empty (window_validate)
+            if (nr > 0) s->upper = (int)std::min<long long>((long long)s->upper + ctx->res_upper, s->cap);
+            if (na > 0) ctx->res_upper = (int)std::min<long long>((long long)ctx->res_upper + s->upper, cap);
             // with empty lists the step is only the capacity check, needed once the bound no longer proves the frame fits
             if (nr > 0 || na > 0 || ctx->res_upper + ctx->d.S > cap)
             {

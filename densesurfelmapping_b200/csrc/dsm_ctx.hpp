@@ -80,6 +80,28 @@ struct GraphEntry
     GraphExecPtr exec;
 };
 
+// The inactive store (dsm_inactive_*): the attached_surfels of every pose outside the drift-free window, dense on the
+// device in retirement order, with what the window step needs next to it.  dsm_inactive_reserve replaces it whole.  The
+// (keyframe, offset, count) segment table and the store size live on the device (seg, win_hdr), and only the window step
+// changes them; segs / size mirror them, exactly unless win_pending, and only res_sync refreshes the mirror.
+struct InactStore
+{
+    CudaOwner own;                  // the device buffers below
+    dsm_surfel_t *surfels = nullptr; // [cap]
+    int4 *seg = nullptr;            // [cap] (keyframe, offset, count, scratch): a stored segment holds >= 1 surfel
+    int32_t *blk = nullptr;         // [DSM_WINDOW_MAX_KEYS][blk_stride] per-key block counts over the pool
+    int32_t *sync = nullptr;        // [dsm_win_sync_len(cap)] compaction flags
+    int32_t *range = nullptr;       // [2] {first, last} of the range an export works on, set in stream order by k_set2
+    int cap = 0, blk_stride = 0;
+    int size = 0;
+    int upper = 0; // host-side upper bound of the store size (exact after a sync)
+    struct Seg
+    {
+        int kf, ofs, cnt;
+    };
+    std::vector<Seg> segs;
+};
+
 #define DSM_MAX_CHUNKS 4
 
 struct dsm_ctx
@@ -120,26 +142,11 @@ struct dsm_ctx
     int *blkcnt = nullptr, *blkofs = nullptr, *nsel = nullptr; // ordered selection: per-block counts / offsets, total
     int32_t *holes = nullptr, *rc_src = nullptr, *rc_sync = nullptr; // fuse_map post-step (dsm_launch_pool_recycle)
     float *wmat = nullptr; // device copy of the 4x4 of dsm_pool_transform
-    // inactive store (dsm_inactive_*): the attached_surfels of every pose outside the drift-free window, dense on the
-    // device in retirement order.  The (keyframe, offset, count) segment table and the store size live on the device
-    // (inact_seg, win_hdr), and only the window step changes them; inact_segs / inact_size mirror them, exactly unless
-    // win_pending, and only res_sync refreshes the mirror
-    DevPtr<dsm_surfel_t> inact; // reallocated by dsm_inactive_reserve
-    DevPtr<int32_t> inact_seg;  // int4 [inact_cap] (keyframe, offset, count, scratch): a stored segment holds >= 1 surfel
-    int inact_cap = 0, inact_size = 0;
-    int inact_upper = 0;          // host-side upper bound of the store size (exact after a sync)
-    int32_t *inact_ofs = nullptr; // device [2]
-    struct InactSeg
-    {
-        int kf, ofs, cnt;
-    };
-    std::vector<InactSeg> inact_segs;
-    // dsm_fuse_stream_window: staged window lists (pinned h_win -> d_win, one table of win_len ints per staging half),
-    // device header {store size, segments, per-frame scratch x2}, per-key block counts and the compaction flags
+    std::unique_ptr<InactStore> inact; // nullptr until dsm_inactive_reserve
+    // dsm_fuse_stream_window: staged window lists (pinned h_win -> d_win, one table of win_len ints per staging half) and
+    // the store's device header {size, segments, per-frame scratch x2}
     int32_t *h_win = nullptr, *d_win = nullptr, *win_hdr = nullptr;
     size_t win_len = 0;
-    DevPtr<int32_t> win_blk, win_sync;
-    int win_blk_stride = 0;
     int win_tag = 0;          // tag of the latest windowed call (what a rejected frame writes into the error word)
     bool win_pending = false; // a window step since the last synchronisation: mirrors stale, error word unread
     cudaEvent_t ev_h2d[DSM_MAX_CHUNKS] = {}, ev_done[DSM_MAX_CHUNKS] = {}, ev_start = nullptr; // dsm_fuse_batch_async's chunks

@@ -139,13 +139,22 @@ void dsm_launch_fuse(const DsmDev &d, int nb, cudaStream_t s);
 void dsm_launch_init_surfels(const DsmDev &d, int nb, cudaStream_t s);
 void dsm_launch_seeds_export(const DsmDev &d, int frame, dsm_seed_t *out_dev, int raw_md, cudaStream_t s);
 void dsm_launch_labels_export(const DsmDev &d, int frame, cudaStream_t s);
+// Ordered selection over the pool range of frame slot `frame` (mode / key: pool_pred of dsm_kernels.cu; mode 1 flags the
+// selected surfels dead): k_pool_count and k_pool_scan leave the per-block offsets in blkofs and the total in *nsel, then
+// k_pool_scatter writes the selected records in pool order to dst.  dst == nullptr: count and scan only.
+// DSM_SEL_SCATTER_ONLY: the scatter alone, on the blkofs of a count over the same, unchanged range.  DSM_SEL_PDL:
+// PDL-linked launches (a chain whose kernels all begin with pdl_enter).  `upper` >= the range's length sizes the grids.
+// Records: int32 pool index, the whole 44-byte surfel, PointXYZI float4 {px, py, pz, color}.
+enum DsmRec { DSM_REC_INDEX, DSM_REC_SURFEL, DSM_REC_POINT };
+enum { DSM_SEL_PDL = 1, DSM_SEL_SCATTER_ONLY = 2 };
+void dsm_launch_pool_select(const DsmDev &d, int frame, int upper, int mode, int key, DsmRec rec, void *dst, int *blkcnt,
+                            int *blkofs, int *nsel, cudaStream_t s, int flags = 0);
 // fuse_map post-step, in place: holes [capacity], src [capacity], sync [dsm_recycle_sync_len(capacity)] (zeroed once)
 void dsm_launch_pool_recycle(const DsmDev &d, int frame, int upper, int *blkcnt, int *blkofs, int *nsel, int32_t *holes, int32_t *src,
                              int32_t *sync, int32_t *ofs_out, cudaStream_t s);
 #define DSM_RECYCLE_SEG 1024 // tail slots per segment of k_pool_recycle (one CTA works on a segment at a time)
 inline size_t dsm_recycle_sync_len(int capacity) { return 2 + (size_t)capacity / DSM_RECYCLE_SEG + 1; } // {ticket, done, segment flags}
 void dsm_launch_pool_transform(const DsmDev &d, int frame, int upper, const float *Wm_dev, cudaStream_t s);
-void dsm_launch_pool_export(const DsmDev &d, int frame, int upper, int mode, int key, bool as_cloud, int *blkcnt, int *blkofs, int *nsel, void *dst, cudaStream_t s);
 void dsm_launch_set2(int32_t *p, int a, int b, cudaStream_t s);
 // camera -> world of dsm_frame_raw_cloud: R row-major (R[3r + c] = R(r, c)) and T, formed on the host
 struct DsmRawPose
@@ -162,7 +171,6 @@ void dsm_launch_gather(const DsmDev &d, const DsmMaps &m, int nb, cudaStream_t s
 void dsm_launch_newton2(const DsmDev &d, int nb, cudaStream_t s);
 void dsm_launch_plane_gather(const DsmDev &d, const DsmMaps &m, int nb, cudaStream_t s);
 void dsm_launch_gn_solve(const DsmDev &d, int nb, cudaStream_t s);
-void dsm_launch_pool_retire(const DsmDev &d, int frame, int upper, int key, int *blkcnt, int *blkofs, int *nsel, dsm_surfel_t *dst, cudaStream_t s);
 
 // Window step of dsm_fuse_stream_window (move_add_surfels on the device) and the device side of the inactive store.
 // tab: the call's staged lists, [0, B] retire offsets and [B+1, 2B+1] reactivation offsets (relative to the key

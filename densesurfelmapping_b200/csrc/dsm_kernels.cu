@@ -580,6 +580,16 @@ __global__ void __launch_bounds__(RC_SEG) k_pool_recycle(const __grid_constant__
     }
 }
 
+// p <- W p, n <- R_W n of one surfel record e, in place (the per-surfel body of both warp kernels of the reference)
+__device__ __forceinline__ void transform_surfel(const float *W, float *e)
+{
+    float pw[4], nw[3];
+    mat4_mul(W, e[0], e[1], e[2], 1.0f, pw);
+    mat3_mul(W, e[3], e[4], e[5], nw);
+    e[0] = pw[0], e[1] = pw[1], e[2] = pw[2];
+    e[3] = nw[0], e[4] = nw[1], e[5] = nw[2];
+}
+
 #define XF_BLOCK 256
 __global__ void __launch_bounds__(XF_BLOCK) k_pool_transform(const __grid_constant__ DsmDev d, int b, const float *Wm)
 {
@@ -594,15 +604,7 @@ __global__ void __launch_bounds__(XF_BLOCK) k_pool_transform(const __grid_consta
     if (threadIdx.x < 16) s_w[threadIdx.x] = Wm[threadIdx.x];
     const bool bulk = stage_in(sm, g, cnt, &bar, XF_BLOCK);
     __syncthreads(); // s_w
-    if (threadIdx.x < cnt)
-    {
-        float *e = sm + threadIdx.x * 11;
-        float pw[4], nw[3];
-        mat4_mul(s_w, e[0], e[1], e[2], 1.0f, pw);
-        mat3_mul(s_w, e[3], e[4], e[5], nw);
-        e[0] = pw[0], e[1] = pw[1], e[2] = pw[2];
-        e[3] = nw[0], e[4] = nw[1], e[5] = nw[2];
-    }
+    if (threadIdx.x < cnt) transform_surfel(s_w, sm + threadIdx.x * 11);
     stage_out(g, sm, cnt, bulk, XF_BLOCK);
 }
 
@@ -959,8 +961,8 @@ __global__ void __launch_bounds__(1024) k_win_finish(const DsmWin w)
     }
 }
 
-// warp_inactive_surfels_cpu_kernel (surfel_map.cpp:704-733) on the segments of keyframe kf, found in the device table:
-// the same arithmetic as k_pool_transform, one surfel per thread
+// warp_inactive_surfels_cpu_kernel (surfel_map.cpp:704-733) on the segments of keyframe kf, found in the device table,
+// one surfel per thread
 __global__ void __launch_bounds__(256) k_inactive_transform(const DsmWin w, int kf, const float *Wm)
 {
     __shared__ float s_w[16];
@@ -982,14 +984,7 @@ __global__ void __launch_bounds__(256) k_inactive_transform(const DsmWin w, int 
         __syncthreads();
         for (int q = 0; q < s_n; q++)
             for (int k = blockIdx.x * 256 + threadIdx.x; k < s_list[q].y; k += gridDim.x * 256)
-            {
-                float *e = reinterpret_cast<float *>(w.store + s_list[q].x + k);
-                float pw[4], nw[3];
-                mat4_mul(s_w, e[0], e[1], e[2], 1.0f, pw);
-                mat3_mul(s_w, e[3], e[4], e[5], nw);
-                e[0] = pw[0], e[1] = pw[1], e[2] = pw[2];
-                e[3] = nw[0], e[4] = nw[1], e[5] = nw[2];
-            }
+                transform_surfel(s_w, reinterpret_cast<float *>(w.store + s_list[q].x + k));
     }
 }
 
@@ -1167,43 +1162,41 @@ void dsm_launch_labels_export(const DsmDev &d, int frame, cudaStream_t s)
     k_labels_export<<<dim3((d.W + 255) / 256, d.H), 256, 0, s>>>(d, frame);
 }
 
+template <typename... KArgs, typename... Args>
+static void sel_launch(bool pdl, void (*kern)(KArgs...), int grid, int block, cudaStream_t s, Args &&...args)
+{
+    if (pdl) pdl_launch(kern, dim3(grid), dim3(block), 0, s, args...);
+    else kern<<<grid, block, 0, s>>>(args...);
+}
+void dsm_launch_pool_select(const DsmDev &d, int frame, int upper, int mode, int key, DsmRec rec, void *dst, int *blkcnt,
+                            int *blkofs, int *nsel, cudaStream_t s, int flags)
+{
+    const int nblk = (upper + 255) / 256;
+    const bool pdl = flags & DSM_SEL_PDL;
+    if (!(flags & DSM_SEL_SCATTER_ONLY))
+    {
+        if (nblk > 0) sel_launch(pdl, k_pool_count, nblk, 256, s, d, frame, blkcnt, mode, key);
+        sel_launch(pdl, k_pool_scan, 1, 1024, s, d, frame, (const int *)blkcnt, blkofs, nsel);
+    }
+    if (nblk == 0 || !dst) return;
+    const int *ofs = blkofs;
+    if (rec == DSM_REC_INDEX) sel_launch(pdl, k_pool_scatter<int32_t>, nblk, 256, s, d, frame, ofs, static_cast<int32_t *>(dst), mode, key);
+    else if (rec == DSM_REC_POINT) sel_launch(pdl, k_pool_scatter<float4>, nblk, 256, s, d, frame, ofs, static_cast<float4 *>(dst), mode, key);
+    else sel_launch(pdl, k_pool_scatter<dsm_surfel_t>, nblk, 256, s, d, frame, ofs, static_cast<dsm_surfel_t *>(dst), mode, key);
+}
+
 // the fuse_map post-step on the resident pool of frame slot `frame` (whose offset table is ofs_out = {0, N}): hole list,
 // then k_pool_recycle, whose last CTA stores the new size in ofs_out[1].  upper >= N bounds the grids.
 void dsm_launch_pool_recycle(const DsmDev &d, int frame, int upper, int *blkcnt, int *blkofs, int *nsel, int32_t *holes, int32_t *src,
                              int32_t *sync, int32_t *ofs_out, cudaStream_t s)
 {
-    const int nblk = (upper + 255) / 256;
-    if (nblk > 0) pdl_launch(k_pool_count, dim3(nblk), dim3(256), 0, s, d, frame, blkcnt, 0, 0);
-    pdl_launch(k_pool_scan, dim3(1), dim3(1024), 0, s, d, frame, (const int *)blkcnt, blkofs, nsel);
-    if (nblk > 0) pdl_launch(k_pool_scatter<int32_t>, dim3(nblk), dim3(256), 0, s, d, frame, (const int *)blkofs, holes, 0, 0);
+    dsm_launch_pool_select(d, frame, upper, 0, 0, DSM_REC_INDEX, holes, blkcnt, blkofs, nsel, s, DSM_SEL_PDL);
     // Sized by the fill (K <= S), not by `upper`, which can be far above the pool size: in the common frame there is no
     // tail and every further 1024-thread CTA only waits for a free SM next to the other stream's kernels.  A long tail
     // (after a large retire) is worked through by these CTAs segment after segment.
     const int grid = (d.S + RC_SEG - 1) / RC_SEG;
     pdl_launch(k_pool_recycle, dim3(grid > RC_MIN_GRID ? grid : RC_MIN_GRID), dim3(RC_SEG), 0, s, d, frame, (const int *)nsel,
                (const int32_t *)holes, src, sync, ofs_out);
-}
-// move_add_surfels, removal half (surfel_map.cpp:1479-1497): the live surfels whose last_update == key are
-// copied in pool order to dst (count in *nsel) and flagged dead in the pool
-void dsm_launch_pool_retire(const DsmDev &d, int frame, int upper, int key, int *blkcnt, int *blkofs, int *nsel, dsm_surfel_t *dst, cudaStream_t s)
-{
-    const int nblk = (upper + 255) / 256;
-    if (nblk > 0) k_pool_count<<<nblk, 256, 0, s>>>(d, frame, blkcnt, 1, key);
-    k_pool_scan<<<1, 1024, 0, s>>>(d, frame, blkcnt, blkofs, nsel);
-    if (nblk > 0 && dst) k_pool_scatter<dsm_surfel_t><<<nblk, 256, 0, s>>>(d, frame, blkofs, dst, 1, key); // dst == nullptr: count only
-}
-// publish/save filters (mode/key as pool_pred): as_cloud ? PointXYZI float4 records : whole 44-byte surfels, in pool
-// order to dst (count in *nsel); the pool itself is not modified
-void dsm_launch_pool_export(const DsmDev &d, int frame, int upper, int mode, int key, bool as_cloud, int *blkcnt, int *blkofs, int *nsel, void *dst, cudaStream_t s)
-{
-    const int nblk = (upper + 255) / 256;
-    if (nblk > 0) k_pool_count<<<nblk, 256, 0, s>>>(d, frame, blkcnt, mode, key);
-    k_pool_scan<<<1, 1024, 0, s>>>(d, frame, blkcnt, blkofs, nsel);
-    if (nblk == 0) return;
-    if (as_cloud)
-        k_pool_scatter<float4><<<nblk, 256, 0, s>>>(d, frame, blkofs, static_cast<float4 *>(dst), mode, key);
-    else
-        k_pool_scatter<dsm_surfel_t><<<nblk, 256, 0, s>>>(d, frame, blkofs, static_cast<dsm_surfel_t *>(dst), mode, key);
 }
 void dsm_launch_raw_cloud(const DsmDev &d, int frame, const DsmRawPose &pose, float4 *out, cudaStream_t s)
 {

@@ -154,15 +154,25 @@ def test_host_pointer_calls_invalidate_the_resident_pool():
     pose = synth.pose_stream(0)
     gray, depth = synth.make_frame(cam, 511, pose)
     ctx = capi.Context(cam, max_batch=2, max_local_surfels=1 << 16)
+    # every pool call, each with its own cap so that none reaches the library through dsm_pool_size
+    pool_calls = (ctx.pool_size, ctx.pool_download, lambda: ctx.fuse_frame_resident(1, gray, depth, pose),
+                  lambda: ctx.pool_retire(0, cap=4), lambda: ctx.pool_export_cloud(1, cap=4),
+                  lambda: ctx.pool_export_surfels(1, cap=4), lambda: ctx.pool_append(np.zeros(1, SURFEL_DTYPE)),
+                  lambda: ctx.pool_transform(np.eye(4, dtype=np.float32)))
+
+    def refused(calls):
+        for call in calls:
+            with pytest.raises(capi.DsmError) as e:
+                call()
+            assert e.value.code == -7  # DSM_E_STATE
+
+    refused(pool_calls)  # before the first dsm_pool_upload
     ctx.pool_upload(np.zeros(0, SURFEL_DTYPE))
     ctx.fuse_frame_resident(0, gray, depth, pose)
     assert ctx.pool_size() > 0
     _, new = ctx.fuse_frame(0, gray, depth, pose, np.zeros(0, SURFEL_DTYPE))   # host-pointer call on the same context
     assert len(new) > 0
-    for call in (ctx.pool_size, ctx.pool_download, lambda: ctx.fuse_frame_resident(1, gray, depth, pose), lambda: ctx.pool_retire(0)):
-        with pytest.raises(capi.DsmError) as e:
-            call()
-        assert e.value.code == -7  # DSM_E_STATE
+    refused(pool_calls)
     ctx.pool_upload(new)           # a fresh upload makes the resident mode usable again
     assert ctx.pool_size() == len(new)
     ctx.close()
@@ -247,6 +257,7 @@ def test_frame_resident_padded_rows_equal_packed_rows(max_batch):
 def test_inactive_store_round_trip():
     """Device-resident attached_surfels: retire two keyframes into the store, warp one of them, publish the inactive
     cloud, bring one back -- against the restated (and reference-pinned, tests/test_refmap.py) SurfelMap members."""
+    import ctypes
     from densesurfelmapping_b200 import capi
     cam = synth.VGA
     orc = oracle_for(cam)
@@ -258,6 +269,23 @@ def test_inactive_store_round_trip():
         pool = pyoracle.fuse_map_poststep(lo, no)
     ctx = capi.Context(cam, max_batch=2, max_local_surfels=len(pool) + 5000)
     ctx.pool_upload(pool)
+    store_calls = (lambda: ctx.inactive_retire(1), lambda: ctx.inactive_reactivate(1),
+                   lambda: ctx.inactive_transform(1, np.eye(4, dtype=np.float32)), ctx.inactive_download,
+                   ctx.inactive_export_cloud, lambda: ctx.inactive_export_poses([1]))
+
+    def no_store():
+        assert ctx.inactive_size() == (0, 0)
+        for call in store_calls:
+            with pytest.raises(capi.DsmError) as e:
+                call()
+            assert e.value.code == -7  # DSM_E_STATE
+
+    no_store()
+    ctx.inactive_reserve(16)
+    with pytest.raises(capi.DsmError) as e:
+        ctx.inactive_reserve(2 ** 31 - 1)  # 94 GB of surfels: more than the device holds
+    assert e.value.code == -5  # DSM_E_NOMEM, and the store reserved before is gone
+    no_store()
     ctx.inactive_reserve(3 * len(pool))
     loc1, out1 = pyoracle.retire(pool, 1)
     loc0, out0 = pyoracle.retire(loc1, 0)
@@ -268,6 +296,14 @@ def test_inactive_store_round_trip():
     assert ctx.pool_download().tobytes() == loc0.tobytes()
     assert ctx.inactive_download(1).tobytes() == out1.tobytes() and ctx.inactive_download(0).tobytes() == out0.tobytes()
     assert ctx.inactive_download().tobytes() == np.concatenate([out1, out0]).tobytes()
+    # a cap below the count: the first cap surfels are written, nothing past them, and *n_out is the full count
+    for kf, want in ((-1, np.concatenate([out1, out0])), (0, out0)):
+        cap = len(want) - len(out0) // 2
+        buf = np.frombuffer(b"\xab" * (len(want) * SURFEL_DTYPE.itemsize), SURFEL_DTYPE).copy()
+        n = ctypes.c_int(0)
+        assert ctx.lib.dsm_inactive_download(ctx.h, kf, buf.ctypes.data, cap, ctypes.byref(n)) == 0
+        assert n.value == len(want) and buf[:cap].tobytes() == want[:cap].tobytes()
+        assert buf[cap:].tobytes() == b"\xab" * ((len(want) - cap) * SURFEL_DTYPE.itemsize)
     a = np.deg2rad(2.0)
     Wm = np.eye(4)
     Wm[:3, :3] = [[np.cos(a), 0, np.sin(a)], [0, 1, 0], [-np.sin(a), 0, np.cos(a)]]

@@ -136,13 +136,16 @@ def test_pool_export_cloud_on_device(tmp_path):
         assert got.dtype == POINT_DTYPE and got.tobytes() == want.tobytes(), f"min_update_times={min_ut}"
         sel = ctx.pool_export_surfels(min_ut)
         assert sel.tobytes() == pool[ut >= min_ut].tobytes()
-    # truncated output: count reported in full, first `cap` points written
+    # truncated output: count reported in full, the first `cap` records written and nothing past them
     L = capi.load_library()
     import ctypes
-    small = np.zeros(10, POINT_DTYPE)
-    n = ctypes.c_int(0)
-    assert L.dsm_pool_export_cloud(ctx.h, 5, small.ctypes.data, 10, ctypes.byref(n)) == 0
-    assert n.value == int((ut >= 5).sum()) and small.tobytes() == pyoracle.cloud_points(pool, 5)[:10].tobytes()
+    for fn, dtype, want in ((L.dsm_pool_export_cloud, POINT_DTYPE, pyoracle.cloud_points(pool, 5)),
+                            (L.dsm_pool_export_surfels, SURFEL_DTYPE, pool[ut >= 5])):
+        buf = np.frombuffer(b"\xab" * (12 * dtype.itemsize), dtype).copy()
+        n = ctypes.c_int(0)
+        assert fn(ctx.h, 5, buf.ctypes.data, 10, ctypes.byref(n)) == 0
+        assert n.value == int((ut >= 5).sum()) and buf[:10].tobytes() == want[:10].tobytes()
+        assert buf[10:].tobytes() == b"\xab" * (2 * dtype.itemsize)
     assert ctx.pool_download().tobytes() == pool.tobytes()
     # and straight into the reference's file: save_cloud == export(5) -> PCD
     path = tmp_path / "active.pcd"
