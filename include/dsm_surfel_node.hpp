@@ -1,0 +1,683 @@
+// dsm_surfel_node.hpp — header-only dsm::SurfelMapNode: the reference's whole SurfelMap node (surfel_fusion/src/
+// surfel_map.cpp) with the map resident on the GPU, callback for callback, built on the C ABI of dsm.h alone.  Like
+// dsm_surfel_map.hpp it needs neither ROS, Eigen, OpenCV nor PCL: poses are 7 doubles in geometry_msgs::Pose order
+// {px, py, pz, qx, qy, qz, qw}, images are a pointer and a row pitch, clouds are vectors of dsm_point_t.  A ROS node on
+// top of it is topic glue only (INTEGRATION.md §4).
+//
+//   SurfelMap member (surfel_map.cpp)                     here
+//   ---------------------------------------------------   ---------------------------------------------------------
+//   ctor (:14-29, :53)                                    SurfelMapNode(width, ..., drift_free_poses, device, ...)
+//   orb_results_input (:205-365)                          orb_results_input(stamp, loop pairs, path, pose, kf, ref)
+//   image_input / depth_input (:83-101)                   image_input(stamp, gray, pitch) / depth_input(...)
+//   synchronize_msgs (:103-163) + move_add_surfels        one dsm_fuse_stream_window call per fused frame (n = 1)
+//     + fuse_map
+//   warp_surfels (:681-824)                               dsm_pool_transform + dsm_inactive_transform per moved pose
+//   get_driftfree_poses / get_add_remove_poses            driftfree_poses(root, range) / window_lists(root, ...)
+//   publish_active/inactive/all/neighbor/raw_pointcloud   active_points / inactive_points / all_points /
+//                                                         neighbor_points(reference_index) / raw_points
+//   publish_pose_graph / publish_camera_position          pose_graph()
+//   save_map / save_mesh / save_cloud (:75-81, :1153-1280) save_map / save_mesh / save_cloud
+//
+// Pose arithmetic: every fp64 step of the node (pose_ros2eigen, pose_eigen2ros, 4x4 products, inverse, cast to float)
+// is restated operation for operation from the Eigen stand-in the repository's reference build uses (DESIGN.md §1.1:
+// Quaterniond(Matrix3d) by the trace / largest-diagonal branches, toRotationMatrix, products accumulated left to right
+// over the inner index, inverse as adjugate over determinant).  Compiled without floating-point contraction
+// (-ffp-contract=off, or any x86-64 build without -mfma), fuse poses, warp matrices and the stored poses equal that
+// build bit for bit; against real Eigen they agree to about 1e-7.
+//
+// The loop-closure warp follows the schedule of that build: the active warp W = (T_loop * T_cam^-1).cast<float>() of
+// the first local pose is taken before any cam_pose is overwritten and applied to the pool; then every pose whose
+// position moved gets its own W_i on the inactive store (a pose in the drift-free window has nothing stored and is
+// skipped) and takes cam_pose = loop_pose.
+//
+// Deviations from the reference, each deliberate:
+//   * inactive_points / all_points / save_cloud hold every stored point of a warped pose warped; the reference's
+//     inactive_pointcloud keeps the last point of each warped slice stale (std::copy(&front, &back), :742).
+//   * synchronize_msgs spins forever when the oldest image or depth is newer than the oldest pose (:114-139 have no
+//     `>` branch); here that pose is dropped without a fuse and the next one is tried.
+//   * Input the reference would index out of bounds with (a reference index or loop pair outside the pose database,
+//     a loop path that is empty while poses exist) is rejected with DSM_E_INVALID, or skipped for the empty path.
+//   * A frame that does not fit the pool or the inactive store is not applied (nor any later one); DSM_E_CAPACITY
+//     comes back from the next call that reads the map, as dsm_fuse_stream_window specifies.
+//
+// A fused frame never waits for the GPU: the callbacks only enqueue.  The readers (clouds, save_*) synchronise.
+// device < 0 builds the node without a context: the callbacks run the whole pose logic (pose database, sync, window
+// bookkeeping) and fuse nothing; any call that reads the map returns DSM_E_STATE.
+#pragma once
+#include <algorithm>
+#include <cmath>
+#include <cstdio>
+#include <cstring>
+#include <deque>
+#include <set>
+#include <string>
+#include <utility>
+#include <vector>
+#include "dsm.h"
+
+namespace dsm
+{
+// geometry_msgs::Pose: position, then orientation x, y, z, w
+struct Pose
+{
+    double x, y, z, qx, qy, qz, qw;
+};
+struct Point3
+{
+    double x, y, z;
+};
+
+namespace node_math
+{
+// a column-major 4x4 fp64 matrix (Eigen::Matrix4d memory order)
+struct M4
+{
+    double d[16];
+    double &operator()(int i, int j) { return d[j * 4 + i]; }
+    double operator()(int i, int j) const { return d[j * 4 + i]; }
+};
+inline M4 identity()
+{
+    M4 m;
+    for (int i = 0; i < 16; i++) m.d[i] = (i % 5 == 0) ? 1.0 : 0.0;
+    return m;
+}
+inline M4 mul(const M4 &a, const M4 &b)
+{
+    M4 r;
+    for (int k = 0; k < 4; k++)
+        for (int i = 0; i < 4; i++)
+        {
+            double acc = a(i, 0) * b(0, k);
+            for (int j = 1; j < 4; j++) acc = acc + a(i, j) * b(j, k);
+            r(i, k) = acc;
+        }
+    return r;
+}
+inline M4 inverse(const M4 &a)
+{
+    const double *m = a.d;
+    double v[16];
+    v[0] = m[5] * m[10] * m[15] - m[5] * m[11] * m[14] - m[9] * m[6] * m[15] + m[9] * m[7] * m[14] + m[13] * m[6] * m[11] - m[13] * m[7] * m[10];
+    v[4] = -m[4] * m[10] * m[15] + m[4] * m[11] * m[14] + m[8] * m[6] * m[15] - m[8] * m[7] * m[14] - m[12] * m[6] * m[11] + m[12] * m[7] * m[10];
+    v[8] = m[4] * m[9] * m[15] - m[4] * m[11] * m[13] - m[8] * m[5] * m[15] + m[8] * m[7] * m[13] + m[12] * m[5] * m[11] - m[12] * m[7] * m[9];
+    v[12] = -m[4] * m[9] * m[14] + m[4] * m[10] * m[13] + m[8] * m[5] * m[14] - m[8] * m[6] * m[13] - m[12] * m[5] * m[10] + m[12] * m[6] * m[9];
+    v[1] = -m[1] * m[10] * m[15] + m[1] * m[11] * m[14] + m[9] * m[2] * m[15] - m[9] * m[3] * m[14] - m[13] * m[2] * m[11] + m[13] * m[3] * m[10];
+    v[5] = m[0] * m[10] * m[15] - m[0] * m[11] * m[14] - m[8] * m[2] * m[15] + m[8] * m[3] * m[14] + m[12] * m[2] * m[11] - m[12] * m[3] * m[10];
+    v[9] = -m[0] * m[9] * m[15] + m[0] * m[11] * m[13] + m[8] * m[1] * m[15] - m[8] * m[3] * m[13] - m[12] * m[1] * m[11] + m[12] * m[3] * m[9];
+    v[13] = m[0] * m[9] * m[14] - m[0] * m[10] * m[13] - m[8] * m[1] * m[14] + m[8] * m[2] * m[13] + m[12] * m[1] * m[10] - m[12] * m[2] * m[9];
+    v[2] = m[1] * m[6] * m[15] - m[1] * m[7] * m[14] - m[5] * m[2] * m[15] + m[5] * m[3] * m[14] + m[13] * m[2] * m[7] - m[13] * m[3] * m[6];
+    v[6] = -m[0] * m[6] * m[15] + m[0] * m[7] * m[14] + m[4] * m[2] * m[15] - m[4] * m[3] * m[14] - m[12] * m[2] * m[7] + m[12] * m[3] * m[6];
+    v[10] = m[0] * m[5] * m[15] - m[0] * m[7] * m[13] - m[4] * m[1] * m[15] + m[4] * m[3] * m[13] + m[12] * m[1] * m[7] - m[12] * m[3] * m[5];
+    v[14] = -m[0] * m[5] * m[14] + m[0] * m[6] * m[13] + m[4] * m[1] * m[14] - m[4] * m[2] * m[13] - m[12] * m[1] * m[6] + m[12] * m[2] * m[5];
+    v[3] = -m[1] * m[6] * m[11] + m[1] * m[7] * m[10] + m[5] * m[2] * m[11] - m[5] * m[3] * m[10] - m[9] * m[2] * m[7] + m[9] * m[3] * m[6];
+    v[7] = m[0] * m[6] * m[11] - m[0] * m[7] * m[10] - m[4] * m[2] * m[11] + m[4] * m[3] * m[10] + m[8] * m[2] * m[7] - m[8] * m[3] * m[6];
+    v[11] = -m[0] * m[5] * m[11] + m[0] * m[7] * m[9] + m[4] * m[1] * m[11] - m[4] * m[3] * m[9] - m[8] * m[1] * m[7] + m[8] * m[3] * m[5];
+    v[15] = m[0] * m[5] * m[10] - m[0] * m[6] * m[9] - m[4] * m[1] * m[10] + m[4] * m[2] * m[9] + m[8] * m[1] * m[6] - m[8] * m[2] * m[5];
+    const double det = m[0] * v[0] + m[1] * v[4] + m[2] * v[8] + m[3] * v[12];
+    const double inv_det = 1.0 / det;
+    M4 out;
+    for (int i = 0; i < 16; i++) out.d[i] = v[i] * inv_det;
+    return out;
+}
+// pose_ros2eigen (surfel_map.cpp:367-379): T = I, T.block<3,3>(0,0) = Quaterniond(w, x, y, z).toRotationMatrix(), T(:3,3) = p
+inline M4 from_pose(const Pose &p)
+{
+    M4 r = identity();
+    const double tx = 2.0 * p.qx, ty = 2.0 * p.qy, tz = 2.0 * p.qz;
+    const double twx = tx * p.qw, twy = ty * p.qw, twz = tz * p.qw;
+    const double txx = tx * p.qx, txy = ty * p.qx, txz = tz * p.qx;
+    const double tyy = ty * p.qy, tyz = tz * p.qy, tzz = tz * p.qz;
+    r(0, 0) = 1.0 - (tyy + tzz), r(0, 1) = txy - twz, r(0, 2) = txz + twy;
+    r(1, 0) = txy + twz, r(1, 1) = 1.0 - (txx + tzz), r(1, 2) = tyz - twx;
+    r(2, 0) = txz - twy, r(2, 1) = tyz + twx, r(2, 2) = 1.0 - (txx + tyy);
+    r(0, 3) = p.x, r(1, 3) = p.y, r(2, 3) = p.z;
+    return r;
+}
+// pose_eigen2ros (surfel_map.cpp:381-391): Quaterniond(T.block<3,3>(0,0)) and T(:3,3)
+inline Pose to_pose(const M4 &m)
+{
+    Pose p;
+    double q[3], qw;
+    double t = m(0, 0) + m(1, 1) + m(2, 2);
+    if (t > 0.0)
+    {
+        t = std::sqrt(t + 1.0);
+        qw = 0.5 * t;
+        t = 0.5 / t;
+        q[0] = (m(2, 1) - m(1, 2)) * t;
+        q[1] = (m(0, 2) - m(2, 0)) * t;
+        q[2] = (m(1, 0) - m(0, 1)) * t;
+    }
+    else
+    {
+        int i = 0;
+        if (m(1, 1) > m(0, 0)) i = 1;
+        if (m(2, 2) > m(i, i)) i = 2;
+        const int j = (i + 1) % 3, k = (j + 1) % 3;
+        t = std::sqrt(m(i, i) - m(j, j) - m(k, k) + 1.0);
+        q[i] = 0.5 * t;
+        t = 0.5 / t;
+        qw = (m(k, j) - m(j, k)) * t;
+        q[j] = (m(j, i) + m(i, j)) * t;
+        q[k] = (m(k, i) + m(i, k)) * t;
+    }
+    p.qx = q[0], p.qy = q[1], p.qz = q[2], p.qw = qw;
+    p.x = m(0, 3), p.y = m(1, 3), p.z = m(2, 3);
+    return p;
+}
+// Matrix4d::cast<float>(), column-major
+inline void to_float(const M4 &m, float out[16])
+{
+    for (int i = 0; i < 16; i++) out[i] = (float)m.d[i];
+}
+inline Pose read_pose(const double *p7)
+{
+    Pose p;
+    p.x = p7[0], p.y = p7[1], p.z = p7[2], p.qx = p7[3], p.qy = p7[4], p.qz = p7[5], p.qw = p7[6];
+    return p;
+}
+inline bool same_position(const Pose &a, const Pose &b) { return a.x == b.x && a.y == b.y && a.z == b.z; }
+} // namespace node_math
+
+// PoseElement (surfel_map.h): what the node keeps per keyframe; the attached surfels live in the device store
+struct NodePose
+{
+    Pose cam_pose, loop_pose;
+    double cam_stamp;
+    std::vector<int> linked_pose_index;
+};
+
+// one transform issued by a loop closure: pose -1 is the active pool, else the keyframe whose stored surfels moved
+struct NodeWarp
+{
+    int pose;
+    float W[16];
+};
+
+// publish_pose_graph / publish_camera_position (surfel_map.cpp:906-1026) of the last fused frame
+struct NodePoseGraph
+{
+    std::vector<Pose> path;         // fusion_loop_path: every cam_pose, index order
+    std::vector<Point3> loop_edges; // loop_marker: loop_pose positions, two per non-consecutive link j > i
+    std::vector<Point3> driftfree;  // driftfree_loop_path, "driftfree": cam_pose positions of get_driftfree_poses(ref)
+    std::vector<Point3> drift;      // "drift": every other pose, index order
+    Pose camera;                    // camera_marker: the fuse pose
+};
+
+class SurfelMapNode
+{
+  public:
+    // The surfel_map.cpp:14-29 parameters (cam_*, fuse_far_distence, fuse_near_distence, drift_free_poses); the CUDA
+    // device (< 0: pose logic only, no context), the pool capacity, the inactive-store reservation in surfels and
+    // optionally a constant set (DSM_CONSTANTS_DRIVE when null).  Check last_error() after construction.
+    SurfelMapNode(int cam_width, int cam_height, double cam_fx, double cam_fy, double cam_cx, double cam_cy, double far_dist,
+                  double near_dist, int drift_free_poses, int device = 0, int max_local_surfels = 1 << 21,
+                  int max_inactive_surfels = 1 << 22, const dsm_constants *constants = nullptr)
+        : ctx_(nullptr), err_(DSM_OK), width_(cam_width), height_(cam_height), drift_free_poses_(drift_free_poses),
+          last_ref_(-1), fused_(false)
+    {
+        std::memset(transform_kitti_.d, 0, sizeof(transform_kitti_.d));
+        std::memset(&last_fuse_pose_, 0, sizeof(last_fuse_pose_));
+        if (device < 0) return;
+        dsm_params p;
+        std::memset(&p, 0, sizeof(p));
+        p.width = cam_width, p.height = cam_height;
+        p.fx = (float)cam_fx, p.fy = (float)cam_fy, p.cx = (float)cam_cx, p.cy = (float)cam_cy;
+        p.fuse_far = (float)far_dist, p.fuse_near = (float)near_dist;
+        p.max_batch = 2; // two frame slots: the copy of frame t+1 overlaps the kernels of frame t
+        p.max_local_surfels = max_local_surfels;
+        err_ = dsm_create(&p, device, nullptr, &ctx_);
+        if (err_ == DSM_OK) err_ = dsm_pool_upload(ctx_, nullptr, 0);
+        if (err_ == DSM_OK) err_ = dsm_inactive_reserve(ctx_, max_inactive_surfels);
+        if (err_ == DSM_OK && constants) err_ = dsm_set_constants(ctx_, constants);
+        if (err_ != DSM_OK)
+        {
+            report("SurfelMapNode");
+            dsm_destroy(ctx_);
+            ctx_ = nullptr;
+        }
+    }
+    ~SurfelMapNode() { dsm_destroy(ctx_); }
+    SurfelMapNode(const SurfelMapNode &) = delete;
+    SurfelMapNode &operator=(const SurfelMapNode &) = delete;
+
+    // ---- the three callbacks of ros_node.cpp ----
+
+    // orb_results_input (surfel_map.cpp:205-365).  loop_pairs: n_loops pairs of keyframe indices (the loop_stamps
+    // channel); loop_path7: n_path poses of 7 doubles (the loop path, ORB's frame); this_pose7: the frame's pose;
+    // is_keyframe / reference_index: pose.covariance[0] > 0 / pose.covariance[1].  Queues the frame and runs the sync.
+    int orb_results_input(double stamp, const int *loop_pairs, int n_loops, const double *loop_path7, int n_path, const double *this_pose7,
+                          bool is_keyframe, int reference_index)
+    {
+        using namespace node_math;
+        const int n_poses = (int)poses_.size();
+        if (!this_pose7 || n_loops < 0 || n_path < 0 || (n_loops && !loop_pairs) || (n_path && !loop_path7)) return fail(DSM_E_INVALID, "orb_results_input");
+        const bool new_kf = is_keyframe || n_poses == 0;
+        // a new keyframe links to its reference, which must exist already; any other frame refers to an existing pose
+        const int n_after = n_poses + (new_kf ? 1 : 0);
+        if (reference_index < 0 || reference_index >= (new_kf && n_poses > 0 ? n_poses : n_after)) return fail(DSM_E_INVALID, "orb_results_input");
+        for (int i = 0; i < 2 * n_loops; i++)
+            if (loop_pairs[i] < 0) return fail(DSM_E_INVALID, "orb_results_input");
+
+        last_warp_.clear();
+        // the KITTI axis fix-up, fixed by the first pose (:214-232)
+        const M4 received = from_pose(read_pose(this_pose7));
+        if (n_poses == 0)
+        {
+            M4 idea;
+            std::memset(idea.d, 0, sizeof(idea.d));
+            idea(0, 0) = 1.0, idea(1, 2) = 1.0, idea(2, 1) = -1.0, idea(3, 3) = 1.0;
+            transform_kitti_ = mul(idea, inverse(received));
+        }
+        const Pose input_pose = to_pose(mul(transform_kitti_, received));
+
+        // loop_pose of every pose the path covers (:237-253)
+        bool loop_changed = false;
+        for (int i = 0; i < n_poses && i < n_path; i++)
+        {
+            poses_[i].loop_pose = to_pose(mul(transform_kitti_, from_pose(read_pose(loop_path7 + 7 * i))));
+            if (!same_position(poses_[i].loop_pose, poses_[i].cam_pose)) loop_changed = true;
+        }
+        // the last correction carried to the poses the path does not cover yet (:255-272); an empty path has no last
+        // correction (the reference reads pose -1)
+        if (n_poses > n_path && n_path > 0)
+        {
+            const int last = n_path - 1;
+            const M4 warp = mul(from_pose(poses_[last].loop_pose), inverse(from_pose(poses_[last].cam_pose)));
+            for (int i = n_path; i < n_poses; i++) poses_[i].loop_pose = to_pose(mul(warp, from_pose(poses_[i].cam_pose)));
+        }
+        if (loop_changed) warp_surfels();
+
+        // covisibility links without duplicates (:290-316)
+        for (int i = 0; i < n_loops; i++)
+        {
+            const int a = loop_pairs[2 * i], b = loop_pairs[2 * i + 1];
+            if (a >= n_poses || b >= n_poses) continue;
+            std::vector<int> &la = poses_[a].linked_pose_index, &lb = poses_[b].linked_pose_index;
+            if (std::find(la.begin(), la.end(), b) != la.end()) continue;
+            la.push_back(b);
+            if (std::find(lb.begin(), lb.end(), a) == lb.end()) lb.push_back(a);
+        }
+
+        // a new keyframe (:319-353)
+        if (new_kf)
+        {
+            NodePose e;
+            const int index = n_poses;
+            e.cam_pose = input_pose, e.loop_pose = input_pose, e.cam_stamp = stamp;
+            if (n_poses > 0)
+            {
+                e.linked_pose_index.push_back(reference_index);
+                poses_[reference_index].linked_pose_index.push_back(index);
+            }
+            poses_.push_back(e);
+            local_.insert(index);
+        }
+
+        // the pose relative to its reference, after its round trip through geometry_msgs::Pose (:356-363)
+        PendingPose q;
+        q.stamp = stamp;
+        q.reference_index = reference_index;
+        q.relative = to_pose(mul(inverse(from_pose(poses_[reference_index].cam_pose)), from_pose(input_pose)));
+        pose_buffer_.push_back(q);
+        return synchronize();
+    }
+
+    // image_input / depth_input (surfel_map.cpp:83-101): the frame is copied (row pitch in bytes), then the sync runs
+    int image_input(double stamp, const uint8_t *gray, size_t pitch)
+    {
+        if (!gray || pitch < (size_t)width_) return fail(DSM_E_INVALID, "image_input");
+        image_buffer_.push_back(std::make_pair(stamp, std::vector<uint8_t>((size_t)width_ * height_)));
+        for (int y = 0; y < height_; y++) std::memcpy(&image_buffer_.back().second[(size_t)y * width_], gray + (size_t)y * pitch, (size_t)width_);
+        return synchronize();
+    }
+    int depth_input(double stamp, const float *depth, size_t pitch)
+    {
+        if (!depth || pitch < (size_t)width_ * 4) return fail(DSM_E_INVALID, "depth_input");
+        depth_buffer_.push_back(std::make_pair(stamp, std::vector<float>((size_t)width_ * height_)));
+        const uint8_t *src = reinterpret_cast<const uint8_t *>(depth);
+        for (int y = 0; y < height_; y++)
+            std::memcpy(&depth_buffer_.back().second[(size_t)y * width_], src + (size_t)y * pitch, (size_t)width_ * 4);
+        return synchronize();
+    }
+
+    // ---- the pose graph ----
+    const std::vector<NodePose> &poses() const { return poses_; }
+    const std::set<int> &local_surfels_indexs() const { return local_; }
+    // get_driftfree_poses (surfel_map.cpp:1643-1674): breadth-first over the links, `range` levels including the root
+    std::vector<int> driftfree_poses(int root_index, int range) const
+    {
+        std::vector<int> out;
+        if (root_index < 0 || (int)poses_.size() < root_index + 1) return out;
+        std::vector<int> this_level(1, root_index), next_level;
+        out.push_back(root_index);
+        for (int i = 1; i < range; i++)
+        {
+            for (size_t a = 0; a < this_level.size(); a++)
+            {
+                const std::vector<int> &links = poses_[(size_t)this_level[a]].linked_pose_index;
+                for (size_t b = 0; b < links.size(); b++)
+                    if (std::find(out.begin(), out.end(), links[b]) == out.end())
+                    {
+                        next_level.push_back(links[b]);
+                        out.push_back(links[b]);
+                    }
+            }
+            this_level.swap(next_level);
+            next_level.clear();
+        }
+        return out;
+    }
+    // get_add_remove_poses (surfel_map.cpp:1597-1641): the lists move_add_surfels(root) would use now
+    void window_lists(int root_index, std::vector<int> &poses_to_remove, std::vector<int> &poses_to_add) const
+    {
+        const std::vector<int> df = driftfree_poses(root_index, drift_free_poses_);
+        poses_to_add.clear(), poses_to_remove.clear();
+        for (size_t i = 0; i < df.size(); i++)
+            if (!local_.count(df[i])) poses_to_add.push_back(df[i]);
+        for (std::set<int>::const_iterator it = local_.begin(); it != local_.end(); ++it)
+            if (std::find(df.begin(), df.end(), *it) == df.end()) poses_to_remove.push_back(*it);
+    }
+    // the oldest queued frame that has not been fused: its reference index (returned, -1 when none), the pose
+    // fuse_map will receive (column-major float) and its window lists, all as of now
+    int pending_frame(float pose16[16], std::vector<int> &poses_to_remove, std::vector<int> &poses_to_add) const
+    {
+        if (pose_buffer_.empty()) return -1;
+        const PendingPose &q = pose_buffer_.front();
+        node_math::to_float(fuse_pose(q), pose16);
+        window_lists(q.reference_index, poses_to_remove, poses_to_add);
+        return q.reference_index;
+    }
+    // the transforms the last orb_results_input issued, the active pool first (pose -1); empty when its path moved no pose
+    const std::vector<NodeWarp> &last_warp() const { return last_warp_; }
+    NodePoseGraph pose_graph() const
+    {
+        NodePoseGraph g;
+        for (size_t i = 0; i < poses_.size(); i++)
+        {
+            g.path.push_back(poses_[i].cam_pose);
+            const std::vector<int> &l = poses_[i].linked_pose_index;
+            for (size_t j = 0; j < l.size(); j++)
+                if (l[j] != (int)i - 1 && l[j] != (int)i + 1 && l[j] > (int)i)
+                {
+                    g.loop_edges.push_back(position(poses_[i].loop_pose));
+                    g.loop_edges.push_back(position(poses_[(size_t)l[j]].loop_pose));
+                }
+        }
+        const std::vector<int> df = driftfree_poses(last_ref_, drift_free_poses_);
+        for (size_t i = 0; i < df.size(); i++) g.driftfree.push_back(position(poses_[(size_t)df[i]].cam_pose));
+        for (size_t i = 0; i < poses_.size(); i++)
+            if (std::find(df.begin(), df.end(), (int)i) == df.end()) g.drift.push_back(position(poses_[i].cam_pose));
+        g.camera = last_fuse_pose_;
+        return g;
+    }
+
+    // ---- the clouds the node publishes; each replaces `points` ----
+    // publish_active_pointcloud (:1398-1417): local surfels with update_times >= 5, pool order
+    int active_points(std::vector<dsm_point_t> &points) { return read_pool_cloud(points, 5, "active_points"); }
+    // publish_inactive_pointcloud (:1385-1396): the inactive store, store order, every warped point warped
+    int inactive_points(std::vector<dsm_point_t> &points)
+    {
+        points.clear();
+        return append_inactive(points, "inactive_points");
+    }
+    // publish_all_pointcloud (:1419-1454)
+    int all_points(std::vector<dsm_point_t> &points)
+    {
+        if (active_points(points) != DSM_OK) return err_;
+        return append_inactive(points, "all_points");
+    }
+    // publish_neighbor_pointcloud (:1283-1383): live local points, then the stored points of get_driftfree_poses(ref,
+    // 2 * drift_free_poses) in list order
+    int neighbor_points(int reference_index, std::vector<dsm_point_t> &points)
+    {
+        if (read_pool_cloud(points, 1, "neighbor_points") != DSM_OK) return err_;
+        const std::vector<int> df = driftfree_poses(reference_index, 2 * drift_free_poses_);
+        const std::vector<int32_t> kf(df.begin(), df.end());
+        int n = 0;
+        if ((err_ = dsm_inactive_size(ctx_, &n, nullptr)) != DSM_OK) return report("neighbor_points");
+        const size_t base = points.size();
+        points.resize(base + (size_t)n + 1);
+        int got = 0;
+        err_ = dsm_inactive_export_poses(ctx_, kf.data(), (int)kf.size(), points.data() + base, n, &got);
+        points.resize(err_ == DSM_OK ? base + (size_t)got : base);
+        return report("neighbor_points");
+    }
+    // publish_raw_pointcloud (:1115-1151) of the last fused frame at its fuse pose
+    int raw_points(std::vector<dsm_point_t> &points)
+    {
+        points.clear();
+        if (!ready("raw_points")) return err_;
+        if (!fused_) return fail(DSM_E_STATE, "raw_points");
+        const double p7[7] = {last_fuse_pose_.x, last_fuse_pose_.y, last_fuse_pose_.z, last_fuse_pose_.qx,
+                              last_fuse_pose_.qy, last_fuse_pose_.qz, last_fuse_pose_.qw};
+        points.resize((size_t)width_ * height_);
+        int got = 0;
+        err_ = dsm_frame_raw_cloud(ctx_, 0, p7, points.data(), (int)points.size(), &got);
+        points.resize(err_ == DSM_OK ? (size_t)got : 0);
+        return report("raw_points");
+    }
+    // local_surfels, pool order
+    int local_surfels(std::vector<dsm_surfel_t> &out)
+    {
+        out.clear();
+        if (!ready("local_surfels")) return err_;
+        int n = 0;
+        if ((err_ = dsm_pool_size(ctx_, &n)) != DSM_OK) return report("local_surfels");
+        out.resize((size_t)n + 1);
+        int got = 0;
+        err_ = dsm_pool_download(ctx_, out.data(), n, &got);
+        out.resize(err_ == DSM_OK ? (size_t)got : 0);
+        return report("local_surfels");
+    }
+    // PoseElement::attached_surfels of one keyframe
+    int attached_surfels(int pose_index, std::vector<dsm_surfel_t> &out)
+    {
+        out.clear();
+        if (!ready("attached_surfels")) return err_;
+        int n = 0;
+        if ((err_ = dsm_inactive_download(ctx_, pose_index, nullptr, 0, &n)) != DSM_OK) return report("attached_surfels");
+        out.resize((size_t)n + 1);
+        err_ = dsm_inactive_download(ctx_, pose_index, out.data(), n, &n);
+        out.resize(err_ == DSM_OK ? (size_t)n : 0);
+        return report("attached_surfels");
+    }
+
+    // ---- files ----
+    // save_map (:75-81)
+    int save_map(const std::string &save_name) { return save_mesh(save_name); }
+    // save_mesh (:1219-1280): the attached surfels of every pose in index order, then the local surfels with
+    // update_times >= 5; one hexagon each, ASCII PLY
+    int save_mesh(const std::string &save_path_name)
+    {
+        std::vector<dsm_surfel_t> all, part;
+        for (size_t i = 0; i < poses_.size(); i++)
+        {
+            if (local_.count((int)i)) continue; // a pose in the window has nothing stored
+            if (attached_surfels((int)i, part) != DSM_OK) return err_;
+            all.insert(all.end(), part.begin(), part.end());
+        }
+        if (!ready("save_mesh")) return err_;
+        int n = 0;
+        if ((err_ = dsm_pool_size(ctx_, &n)) != DSM_OK) return report("save_mesh");
+        const size_t base = all.size();
+        all.resize(base + (size_t)n + 1);
+        int got = 0;
+        err_ = dsm_pool_export_surfels(ctx_, 5, all.data() + base, n, &got);
+        if (err_ == DSM_OK) err_ = dsm_write_ply_mesh(save_path_name.c_str(), all.data(), base + (size_t)got);
+        return report("save_mesh");
+    }
+    // save_cloud (:1153-1173): local points with update_times >= 5, then the inactive cloud; PCD v0.7 ASCII
+    int save_cloud(const std::string &save_path_name)
+    {
+        std::vector<dsm_point_t> points;
+        if (all_points(points) != DSM_OK) return err_;
+        err_ = dsm_write_pcd(save_path_name.c_str(), points.data(), points.size(), 0);
+        return report("save_cloud");
+    }
+
+    int last_error() const { return err_; }
+    dsm_ctx *context() { return ctx_; }
+
+  private:
+    struct PendingPose
+    {
+        double stamp;
+        Pose relative;
+        int reference_index;
+    };
+
+    static Point3 position(const Pose &p)
+    {
+        Point3 q;
+        q.x = p.x, q.y = p.y, q.z = p.z;
+        return q;
+    }
+    // synchronize_msgs (:147-150): cam_pose of the reference now, times the queued relative pose
+    node_math::M4 fuse_pose(const PendingPose &q) const
+    {
+        return node_math::mul(node_math::from_pose(poses_[(size_t)q.reference_index].cam_pose), node_math::from_pose(q.relative));
+    }
+
+    // synchronize_msgs (:103-163): the oldest pose is fused once an image and a depth with exactly its stamp are there
+    int synchronize()
+    {
+        while (!pose_buffer_.empty())
+        {
+            const double t = pose_buffer_.front().stamp;
+            bool find_image = false, find_depth = false, newer = false;
+            while (!image_buffer_.empty() && image_buffer_.front().first < t) image_buffer_.pop_front();
+            if (!image_buffer_.empty()) (image_buffer_.front().first == t ? find_image : newer) = true;
+            while (!depth_buffer_.empty() && depth_buffer_.front().first < t) depth_buffer_.pop_front();
+            if (!depth_buffer_.empty()) (depth_buffer_.front().first == t ? find_depth : newer) = true;
+            if (newer)
+            { // this pose's image or depth never came: drop it, try the next
+                pose_buffer_.pop_front();
+                continue;
+            }
+            if (!find_image || !find_depth) return DSM_OK;
+            return fuse_front();
+        }
+        return DSM_OK;
+    }
+
+    // the fuse of synchronize_msgs (:144-163): move_add_surfels and fuse_map as one dsm_fuse_stream_window call
+    int fuse_front()
+    {
+        const PendingPose q = pose_buffer_.front();
+        const node_math::M4 fuse = fuse_pose(q);
+        float pose16[16];
+        node_math::to_float(fuse, pose16);
+        std::vector<int> remove, add;
+        window_lists(q.reference_index, remove, add);
+        const std::vector<int32_t> rk(remove.begin(), remove.end()), ak(add.begin(), add.end());
+        const int32_t ro[2] = {0, (int32_t)rk.size()}, ao[2] = {0, (int32_t)ak.size()};
+        const int32_t ref = q.reference_index;
+        if (ctx_)
+        {
+            err_ = dsm_fuse_stream_window(ctx_, 1, &ref, image_buffer_.front().second.data(), depth_buffer_.front().second.data(), pose16,
+                                          rk.data(), ro, ak.data(), ao, nullptr);
+            if (err_ != DSM_OK) return report("fuse");
+        }
+        for (size_t i = 0; i < remove.size(); i++) local_.erase(remove[i]);
+        local_.insert(add.begin(), add.end());
+        last_fuse_pose_ = node_math::to_pose(fuse);
+        last_ref_ = q.reference_index;
+        fused_ = true;
+        pose_buffer_.pop_front();
+        return DSM_OK;
+    }
+
+    // warp_surfels (:681-824) in the schedule described at the top of this file
+    void warp_surfels()
+    {
+        using namespace node_math;
+        if (local_.empty()) return;
+        NodeWarp w;
+        const NodePose &lp = poses_[(size_t)*local_.begin()];
+        w.pose = -1;
+        to_float(mul(from_pose(lp.loop_pose), inverse(from_pose(lp.cam_pose))), w.W);
+        last_warp_.push_back(w);
+        for (size_t i = 0; i < poses_.size(); i++)
+        {
+            NodePose &p = poses_[i];
+            if (same_position(p.cam_pose, p.loop_pose)) continue;
+            if (!local_.count((int)i))
+            {
+                w.pose = (int)i;
+                to_float(mul(from_pose(p.loop_pose), inverse(from_pose(p.cam_pose))), w.W);
+                last_warp_.push_back(w);
+            }
+            p.cam_pose = p.loop_pose;
+        }
+        if (!ctx_) return;
+        for (size_t i = 0; i < last_warp_.size(); i++)
+        {
+            const NodeWarp &x = last_warp_[i];
+            const int rc = x.pose < 0 ? dsm_pool_transform(ctx_, x.W) : dsm_inactive_transform(ctx_, x.pose, x.W);
+            if (rc != DSM_OK && err_ == DSM_OK)
+            {
+                err_ = rc;
+                report("warp_surfels");
+            }
+        }
+    }
+
+    int read_pool_cloud(std::vector<dsm_point_t> &points, int min_update_times, const char *what)
+    {
+        points.clear();
+        if (!ready(what)) return err_;
+        int n = 0;
+        if ((err_ = dsm_pool_size(ctx_, &n)) != DSM_OK) return report(what);
+        points.resize((size_t)n + 1);
+        int got = 0;
+        err_ = dsm_pool_export_cloud(ctx_, min_update_times, points.data(), n, &got);
+        points.resize(err_ == DSM_OK ? (size_t)got : 0);
+        return report(what);
+    }
+    int append_inactive(std::vector<dsm_point_t> &points, const char *what)
+    {
+        if (!ready(what)) return err_;
+        int n = 0;
+        if ((err_ = dsm_inactive_size(ctx_, &n, nullptr)) != DSM_OK) return report(what);
+        const size_t base = points.size();
+        points.resize(base + (size_t)n + 1);
+        int got = 0;
+        err_ = dsm_inactive_export_cloud(ctx_, points.data() + base, n, &got);
+        points.resize(err_ == DSM_OK ? base + (size_t)got : base);
+        return report(what);
+    }
+    bool ready(const char *what)
+    {
+        if (ctx_) return true;
+        fail(DSM_E_STATE, what);
+        return false;
+    }
+    int fail(int code, const char *what)
+    {
+        err_ = code;
+        return report(what);
+    }
+    int report(const char *what)
+    {
+        if (err_ != DSM_OK)
+            std::fprintf(stderr, "dsm::SurfelMapNode::%s failed: %s (%s)\n", what, dsm_strerror(err_), ctx_ ? dsm_last_error(ctx_) : "no context");
+        return err_;
+    }
+
+    dsm_ctx *ctx_;
+    int err_;
+    int width_, height_, drift_free_poses_;
+    node_math::M4 transform_kitti_;
+    std::vector<NodePose> poses_;
+    std::set<int> local_;
+    std::deque<PendingPose> pose_buffer_;
+    std::deque<std::pair<double, std::vector<uint8_t> > > image_buffer_;
+    std::deque<std::pair<double, std::vector<float> > > depth_buffer_;
+    std::vector<NodeWarp> last_warp_;
+    Pose last_fuse_pose_;
+    int last_ref_;
+    bool fused_;
+};
+} // namespace dsm
