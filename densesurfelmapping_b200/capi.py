@@ -31,6 +31,7 @@ EXPORTS = [
     "dsm_inactive_reserve", "dsm_inactive_retire", "dsm_inactive_reactivate", "dsm_inactive_transform", "dsm_inactive_export_cloud",
     "dsm_inactive_download", "dsm_inactive_size", "dsm_frame_raw_cloud", "dsm_inactive_export_poses",
     "dsm_frame_superpixel_image", "dsm_fuse_stream_window",
+    "dsm_publish_enable", "dsm_publish_enqueue", "dsm_publish_wait", "dsm_debug_publish_chunks",
     "dsm_comm_unique_id", "dsm_comm_init", "dsm_comm_destroy", "dsm_gather_deltas", "dsm_gather_wait", "dsm_gathered_device",
     "dsm_gathered_rank_bytes", "dsm_gathered_download", "dsm_set_constants", "dsm_set_concurrency",
 ]
@@ -96,6 +97,10 @@ def load_library():
     L.dsm_pool_transform.argtypes = [vp, vp]
     L.dsm_fuse_stream_resident.argtypes = [vp, ci, vp, vp, vp, vp, vp]
     L.dsm_fuse_stream_window.argtypes = [vp, ci, vp, vp, vp, vp, vp, vp, vp, vp, vp]
+    L.dsm_publish_enable.argtypes = [vp]
+    L.dsm_publish_enqueue.argtypes = [vp, ci]
+    L.dsm_publish_wait.argtypes = [vp, ctypes.POINTER(vp), ctypes.POINTER(ci), ctypes.POINTER(vp), ctypes.POINTER(ci), ctypes.POINTER(ci)]
+    L.dsm_debug_publish_chunks.argtypes = [vp, ctypes.POINTER(ci)]
     L.dsm_inactive_reserve.argtypes = [vp, ci]
     L.dsm_inactive_retire.argtypes = [vp, ci, ctypes.POINTER(ci)]
     L.dsm_inactive_reactivate.argtypes = [vp, ci, ctypes.POINTER(ci)]
@@ -409,6 +414,42 @@ class Context:
         kf = np.ascontiguousarray(keyframes, dtype=np.int32).reshape(-1)
         cap = self.inactive_size()[0] if cap is None else cap
         return self._read(self.lib.dsm_inactive_export_poses, POINT_DTYPE, cap, _ptr(kf) if len(kf) else None, len(kf))
+
+    # ---- publishing from inside the stream ----
+    def publish_enable(self):
+        self._ck(self.lib.dsm_publish_enable(self.h))
+
+    def publish_enqueue(self, min_update_times=5):
+        self._ck(self.lib.dsm_publish_enqueue(self.h, int(min_update_times)))
+
+    def publish_wait(self):
+        """(active, inactive, inactive_changed_from) of the enqueued snapshot: POINT_DTYPE copies of the context's pinned
+        buffers.  A snapshot taken after a rejected frame raises DsmError(DSM_E_CAPACITY) carrying the same tuple as
+        `.clouds` (the map of the last applied frame)."""
+        pa, pi = ctypes.c_void_p(), ctypes.c_void_p()
+        na, ni, cf = ctypes.c_int(0), ctypes.c_int(0), ctypes.c_int(0)
+        rc = self.lib.dsm_publish_wait(self.h, ctypes.byref(pa), ctypes.byref(na), ctypes.byref(pi), ctypes.byref(ni), ctypes.byref(cf))
+        if rc not in (DSM_OK, -6):  # DSM_E_CAPACITY still carries the clouds
+            self._ck(rc)
+
+        def cloud(ptr, n):
+            if n == 0:
+                return np.zeros(0, dtype=POINT_DTYPE)
+            buf = (ctypes.c_char * (n * POINT_DTYPE.itemsize)).from_address(ptr.value)
+            return np.frombuffer(buf, dtype=POINT_DTYPE).copy()
+
+        clouds = (cloud(pa, na.value), cloud(pi, ni.value), cf.value)
+        if rc != DSM_OK:
+            err = DsmError(rc, self.lib.dsm_last_error(self.h).decode())
+            err.clouds = clouds
+            raise err
+        return clouds
+
+    def publish_chunks(self):
+        """256-point chunks of the inactive cloud the last waited snapshot forwarded to the host."""
+        n = ctypes.c_int(0)
+        self._ck(self.lib.dsm_debug_publish_chunks(self.h, ctypes.byref(n)))
+        return n.value
 
     # ---- raw cloud of a frame ----
     def frame_raw_cloud(self, frame, pose7, cap=None):

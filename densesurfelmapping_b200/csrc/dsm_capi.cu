@@ -1059,9 +1059,27 @@ static DsmDev inactive_view(dsm_ctx *ctx)
     return d;
 }
 
+// dsm_publish_*: the store's part of a publishing context, the shadow of the inactive cloud and its pinned host mirror
+// (what an earlier, failed attempt allocated is kept and used)
+static cudaError_t store_publish_alloc(InactStore &s)
+{
+    cudaError_t e = s.shadow ? cudaSuccess : s.own.device(&s.shadow, (size_t)s.cap);
+    if (e == cudaSuccess && !s.mirror) e = s.own.mapped(&s.mirror, &s.mirror_dev, (size_t)s.cap);
+    return e;
+}
+// k_cloud_mirror's state for a shadow that holds nothing: the next snapshot forwards the whole cloud.  Ordered on the
+// context's stream, like the kernels that read it, and waited for (the source is on the stack).
+static cudaError_t publish_state_reset(dsm_ctx *ctx)
+{
+    const int32_t fresh[4] = {0, INT32_MAX, 0, 0};
+    const cudaError_t e = cudaMemcpyAsync(ctx->pub_state, fresh, sizeof(fresh), cudaMemcpyHostToDevice, ctx->stream);
+    return e != cudaSuccess ? e : cudaStreamSynchronize(ctx->stream);
+}
+
 extern "C" int dsm_inactive_reserve(dsm_ctx *ctx, int max_inactive_surfels)
 {
     if (!ctx || max_inactive_surfels < 1) return DSM_E_INVALID;
+    if (ctx->pub_in_flight) return DSM_E_STATE; // the snapshot's inactive buffer goes with the old store
     int rs = res_sync(ctx);
     if (rs != DSM_OK) return rs;
     if (ctx->inact && ctx->inact->size > 0) return DSM_E_STATE;
@@ -1078,6 +1096,8 @@ extern "C" int dsm_inactive_reserve(dsm_ctx *ctx, int max_inactive_surfels)
     if (e == cudaSuccess) e = s->own.device(&s->sync, dsm_win_sync_len(cap), true);
     if (e == cudaSuccess) e = s->own.device(&s->range, 2, true);
     if (e == cudaSuccess) e = cudaMemset(ctx->win_hdr, 0, 4 * sizeof(int32_t));
+    if (e == cudaSuccess && ctx->pub_on) e = store_publish_alloc(*s);
+    if (e == cudaSuccess && ctx->pub_on) e = publish_state_reset(ctx);
     if (e != cudaSuccess)
     {
         cudaGetLastError();
@@ -1235,6 +1255,81 @@ extern "C" int dsm_inactive_export_poses(dsm_ctx *ctx, const int32_t *keyframes,
     return inactive_export_ranges(ctx, ranges, out, cap, n_out);
 }
 
+// ---- publishing from inside the stream (include/dsm.h) ----
+extern "C" int dsm_publish_enable(dsm_ctx *ctx)
+{
+    if (!ctx) return DSM_E_INVALID;
+    if (!ctx->res_active || ctx->pub_on) return DSM_E_STATE;
+    CK(cudaSetDevice(ctx->device));
+    // a call that failed half-way keeps what it allocated; the next one allocates only what is missing
+    cudaError_t e = cudaSuccess;
+    if (!ctx->pub_active) e = ctx->own.mapped(&ctx->pub_active, &ctx->pub_active_dev, (size_t)std::max(ctx->p.max_local_surfels, 1));
+    if (e == cudaSuccess && !ctx->pub_hdr) e = ctx->own.mapped(&ctx->pub_hdr, &ctx->pub_hdr_dev, DSM_PUB_WORDS);
+    if (e == cudaSuccess && !ctx->pub_state) e = ctx->own.device(&ctx->pub_state, 4);
+    if (e == cudaSuccess && !ctx->pub_ev) e = ctx->own.event(&ctx->pub_ev);
+    if (e == cudaSuccess) e = publish_state_reset(ctx);
+    if (e == cudaSuccess && ctx->inact) e = store_publish_alloc(*ctx->inact);
+    if (e != cudaSuccess)
+    {
+        cudaGetLastError();
+        return DSM_E_NOMEM;
+    }
+    memset(ctx->pub_hdr, 0, DSM_PUB_WORDS * sizeof(int32_t));
+    ctx->pub_on = true;
+    return DSM_OK;
+}
+
+// Enqueue only: the selection writes the active points and their count, k_cloud_mirror the changed chunks of the
+// inactive cloud and the rest of the header, all through device aliases of pinned host memory.  The view has no gate:
+// after a rejected frame the pool is the one of the last applied frame, which is what the snapshot reports.
+extern "C" int dsm_publish_enqueue(dsm_ctx *ctx, int min_update_times)
+{
+    if (!ctx) return DSM_E_INVALID;
+    if (!ctx->pub_on || ctx->pub_in_flight) return DSM_E_STATE;
+    CK(cudaSetDevice(ctx->device));
+    DsmDev d = resident_view(ctx, 0);
+    d.gate = nullptr;
+    // A publisher may never synchronise, so the host bound of the pool only grows: the grids are sized from the view's
+    // bound, which is clamped to the capacity (the block tables hold no more), as the schedule's own launches are.
+    dsm_launch_pool_select(d, 0, d.max_pool_per_frame, 2, min_update_times, DSM_REC_POINT, ctx->pub_active_dev, ctx->blkcnt, ctx->blkofs,
+                           ctx->pub_hdr_dev + DSM_PUB_N_ACTIVE, ctx->stream);
+    const InactStore *s = ctx->inact.get();
+    dsm_launch_cloud_mirror(s ? s->surfels : nullptr, ctx->win_hdr, ctx->res_ofs, s ? s->upper : 0, s ? s->shadow : nullptr,
+                            s ? s->mirror_dev : nullptr, ctx->pub_state, ctx->pub_hdr_dev, ctx->stream);
+    CK(cudaGetLastError());
+    CK(cudaEventRecord(ctx->pub_ev, ctx->stream));
+    ctx->pub_in_flight = true;
+    return DSM_OK;
+}
+
+extern "C" int dsm_publish_wait(dsm_ctx *ctx, const dsm_point_t **active, int *n_active, const dsm_point_t **inactive, int *n_inactive,
+                                int *inactive_changed_from)
+{
+    if (!ctx) return DSM_E_INVALID;
+    if (!ctx->pub_in_flight) return DSM_E_STATE;
+    CK(cudaSetDevice(ctx->device));
+    CK(cudaEventSynchronize(ctx->pub_ev));
+    ctx->pub_in_flight = false;
+    const int32_t *h = ctx->pub_hdr;
+    if (active) *active = ctx->pub_active;
+    if (n_active) *n_active = h[DSM_PUB_N_ACTIVE];
+    if (inactive) *inactive = ctx->inact ? ctx->inact->mirror : nullptr;
+    if (n_inactive) *n_inactive = h[DSM_PUB_N_INACTIVE];
+    if (inactive_changed_from) *inactive_changed_from = h[DSM_PUB_CHANGED_FROM];
+    if (h[DSM_PUB_ERR_TAG] == 0) return DSM_OK;
+    snprintf(ctx->err, sizeof(ctx->err), "dsm_publish_wait: frame %d of a dsm_fuse_stream_window call did not fit the pool or the "
+             "store; the snapshot holds the frames before it", h[DSM_PUB_ERR_FRAME]);
+    return DSM_E_CAPACITY;
+}
+
+extern "C" int dsm_debug_publish_chunks(dsm_ctx *ctx, int *count)
+{
+    if (!ctx || !count) return DSM_E_INVALID;
+    if (!ctx->pub_on || ctx->pub_in_flight) return DSM_E_STATE;
+    *count = ctx->pub_hdr[DSM_PUB_CHUNKS];
+    return DSM_OK;
+}
+
 // A run of n consecutive frames of ONE sequential stream on the resident pool.  Results are identical to n runs of one
 // frame each (dsm_fuse_frame_resident): superpixels, normals and plane fits do not depend on the pose or the pool, so they run
 // for all n frames as one batch (full-width launches instead of n latency-bound single-frame ones); only the fuse /
@@ -1379,7 +1474,9 @@ static int stream_run(dsm_ctx *ctx, int n, const int32_t *ref_idx, const uint8_t
         }
         rc = enqueue_schedule(ctx, resident_view(ctx, slot0 + t), 1, s2, 2);
         if (rc != DSM_OK) return rc;
-        ctx->res_upper += ctx->d.S;
+        // the device applies no frame that would pass the capacity, so the capacity bounds the pool as well: a caller
+        // that never synchronises (a publishing node) keeps a bound that stays finite
+        ctx->res_upper = std::min(ctx->res_upper + ctx->d.S, cap);
     }
     if (win) ctx->win_pending = true;
     hold_frames(ctx, slot0, n, true); // the slots are ordered before the main stream through phase 2 (ev_join / ev_p2)

@@ -48,6 +48,15 @@ struct CudaOwner
         if (e == cudaSuccess) pinned.emplace_back(*p);
         return e;
     }
+    // pinned host memory the device writes directly: *dev is its device alias
+    template <typename T, typename D>
+    cudaError_t mapped(T **p, D **dev, size_t n)
+    {
+        cudaError_t e = cudaHostAlloc((void **)p, n * sizeof(T), cudaHostAllocMapped);
+        if (e != cudaSuccess) return e;
+        pinned.emplace_back(*p);
+        return cudaHostGetDevicePointer((void **)dev, *p, 0);
+    }
     cudaError_t stream(cudaStream_t *s, int priority = 0)
     {
         cudaError_t e = cudaStreamCreateWithPriority(s, cudaStreamNonBlocking, priority);
@@ -92,6 +101,10 @@ struct InactStore
     int32_t *blk = nullptr;         // [DSM_WINDOW_MAX_KEYS][blk_stride] per-key block counts over the pool
     int32_t *sync = nullptr;        // [dsm_win_sync_len(cap)] compaction flags
     int32_t *range = nullptr;       // [2] {first, last} of the range an export works on, set in stream order by k_set2
+    // dsm_publish_*, allocated with the store once publishing is enabled: the inactive cloud as the host last received
+    // it (device shadow, 16 B per reserved surfel) and its pinned host mirror with the device alias the kernel writes
+    float4 *shadow = nullptr, *mirror_dev = nullptr; // [cap]
+    dsm_point_t *mirror = nullptr;                   // [cap], host
     int cap = 0, blk_stride = 0;
     int size = 0;
     int upper = 0; // host-side upper bound of the store size (exact after a sync)
@@ -162,6 +175,13 @@ struct dsm_ctx
     bool img_fit = false;
     float4 *raw_out = nullptr;
     uint8_t *spimg_out = nullptr;
+    // dsm_publish_*: pinned, mapped active cloud [max_local_surfels] and snapshot header [DSM_PUB_WORDS] with their device
+    // aliases, k_cloud_mirror's device state, the event that ends a snapshot.  The inactive side lives with the store.
+    bool pub_on = false, pub_in_flight = false;
+    dsm_point_t *pub_active = nullptr;
+    float4 *pub_active_dev = nullptr;
+    int32_t *pub_hdr = nullptr, *pub_hdr_dev = nullptr, *pub_state = nullptr;
+    cudaEvent_t pub_ev = nullptr;
     int run_split = 2;           // sub-batches per dsm_batch_run (dsm_set_concurrency)
     // pinned host staging for the small per-batch tables
     float *h_pose = nullptr; // [2B][32]: pose then inverse; first half: the batch calls, second half: the resident stream

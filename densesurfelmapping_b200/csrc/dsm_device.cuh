@@ -194,3 +194,23 @@ inline size_t dsm_win_sync_len(int store_cap) { return 2 + (size_t)store_cap / D
 void dsm_launch_window_step(const DsmDev &d, const DsmWin &w, int upper, int nr, int na, cudaStream_t s);
 // warp_inactive_surfels_cpu_kernel for the segments of keyframe kf, located on the device (w.seg / w.hdr)
 void dsm_launch_inactive_transform(const DsmWin &w, int kf, const float *Wm_dev, cudaStream_t s);
+
+// Snapshot header of dsm_publish_enqueue, in pinned host memory the kernels write through its device alias: the active
+// count by the ordered selection (its count word), the rest by k_cloud_mirror
+enum
+{
+    DSM_PUB_N_ACTIVE,     // points the ordered selection wrote to the active buffer
+    DSM_PUB_N_INACTIVE,   // store size at the snapshot
+    DSM_PUB_PREV,         // store size at the previous snapshot
+    DSM_PUB_CHANGED_FROM, // lowest index below the size whose point differs from the previous snapshot, else the size
+    DSM_PUB_CHUNKS,       // chunks forwarded to the host mirror
+    DSM_PUB_ERR_TAG,      // the sticky error word of dsm_fuse_stream_window at the snapshot, and
+    DSM_PUB_ERR_FRAME,    // the frame it rejected
+    DSM_PUB_WORDS
+};
+#define DSM_PUB_CHUNK 256 // points per CTA of k_cloud_mirror: the unit compared with the shadow and forwarded
+// The inactive cloud into its host mirror, changed chunks only (k_cloud_mirror).  store == nullptr: no store, size 0.
+// size_word: the store size on the device; res: the resident offsets with the error word; `upper` >= size sizes the
+// grid; state: device [4], {0, INT_MAX, 0, 0} when the shadow is new
+void dsm_launch_cloud_mirror(const dsm_surfel_t *store, const int32_t *size_word, const int32_t *res, int upper, float4 *shadow,
+                             float4 *mirror, int32_t *state, int32_t *header, cudaStream_t s);

@@ -989,6 +989,85 @@ __global__ void __launch_bounds__(256) k_inactive_transform(const DsmWin w, int 
 }
 
 // -------------------------------------------------------------------------------------------
+// k_cloud_mirror — the inactive cloud of dsm_publish_enqueue, incrementally.  `shadow` holds the cloud as the host
+// mirror last received it, [0, state[0]) of it being published.  CTA c forms the points {px, py, pz, color} of the
+// stored surfels [256 c, 256 c + 256) below the store size (device header), compares them bit for bit with the shadow,
+// and if one differs, or the chunk reaches beyond the previously published size, writes the chunk to the shadow and,
+// through the device alias of the pinned host buffer, to the mirror at the same offset: 16 bytes per thread, whole
+// 128-byte lines per quarter-warp, and only changed chunks cross PCIe.  Nothing upstream marks what it changed: the
+// compare finds it whatever kernel wrote the store.  The surfels are staged like k_pool_transform's (one TMA bulk copy
+// per chunk, stride-11 words); the pass reads 44 + 16 bytes per stored surfel and writes 32 per forwarded point.
+// The last CTA to finish writes the header (PUB_* words) and prepares `state` {published size, lowest changed index,
+// chunks forwarded, CTAs done} for the next snapshot.  A context without a store runs one CTA on size 0.
+// -------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(DSM_PUB_CHUNK) k_cloud_mirror(const dsm_surfel_t *store, const int32_t *size_word, const int32_t *res,
+                                                                float4 *shadow, float4 *mirror, int32_t *state, int32_t *header)
+{
+    __shared__ alignas(128) float sm[DSM_PUB_CHUNK * 11];
+    __shared__ uint64_t bar;
+    __shared__ int s_low;
+    __shared__ bool s_last;
+    const int size = store ? *size_word : 0, prev = state[0];
+    const int nchunk = max(1, (size + DSM_PUB_CHUNK - 1) / DSM_PUB_CHUNK);
+    if ((int)blockIdx.x >= nchunk) return; // the grid is sized from the host's upper bound of the store
+    const int first = blockIdx.x * DSM_PUB_CHUNK, cnt = min(DSM_PUB_CHUNK, size - first);
+    if (threadIdx.x == 0) s_low = INT_MAX;
+    if (cnt > 0)
+    {
+        stage_in(sm, reinterpret_cast<const float *>(store + first), cnt, &bar, DSM_PUB_CHUNK);
+        const int i = first + threadIdx.x;
+        float4 p = make_float4(0.f, 0.f, 0.f, 0.f);
+        bool differs = false;
+        if (threadIdx.x < cnt)
+        {
+            const float *e = sm + threadIdx.x * 11;
+            p = make_float4(e[0], e[1], e[2], e[7]);
+            differs = i >= prev;
+            if (!differs)
+            {
+                const float4 o = shadow[i];
+                differs = __float_as_uint(o.x) != __float_as_uint(p.x) || __float_as_uint(o.y) != __float_as_uint(p.y) ||
+                          __float_as_uint(o.z) != __float_as_uint(p.z) || __float_as_uint(o.w) != __float_as_uint(p.w);
+            }
+            if (differs) atomicMin(&s_low, i);
+        }
+        if (__syncthreads_or(differs))
+        {
+            if (threadIdx.x < cnt)
+            {
+                shadow[i] = p;
+                mirror[i] = p;
+            }
+            if (threadIdx.x == 0)
+            {
+                atomicMin(&state[1], s_low);
+                atomicAdd(&state[2], 1);
+            }
+        }
+    }
+    __syncthreads(); // the chunk's stores come before the count of finished CTAs
+    if (threadIdx.x == 0)
+    {
+        __threadfence();
+        s_last = atomicAdd(&state[3], 1) == nchunk - 1;
+    }
+    __syncthreads();
+    if (!s_last || threadIdx.x != 0) return;
+    __threadfence();
+    const volatile int32_t *st = state;
+    header[DSM_PUB_N_INACTIVE] = size;
+    header[DSM_PUB_PREV] = prev;
+    header[DSM_PUB_CHANGED_FROM] = min(st[1], size);
+    header[DSM_PUB_CHUNKS] = st[2];
+    header[DSM_PUB_ERR_TAG] = res[2];
+    header[DSM_PUB_ERR_FRAME] = res[3];
+    state[0] = size;
+    state[1] = INT_MAX;
+    state[2] = 0;
+    state[3] = 0;
+}
+
+// -------------------------------------------------------------------------------------------
 // parity readback: rebuild the reference's 60-byte Superpixel_seed records for one frame
 // -------------------------------------------------------------------------------------------
 __global__ void k_seeds_export(const __grid_constant__ DsmDev d, int b, dsm_seed_t *out, int raw_md)
@@ -1232,4 +1311,10 @@ void dsm_launch_window_step(const DsmDev &d, const DsmWin &w, int upper, int nr,
 void dsm_launch_inactive_transform(const DsmWin &w, int kf, const float *Wm_dev, cudaStream_t s)
 {
     k_inactive_transform<<<WIN_GRID, 256, 0, s>>>(w, kf, Wm_dev);
+}
+void dsm_launch_cloud_mirror(const dsm_surfel_t *store, const int32_t *size_word, const int32_t *res, int upper, float4 *shadow,
+                             float4 *mirror, int32_t *state, int32_t *header, cudaStream_t s)
+{
+    const int grid = store ? (upper + DSM_PUB_CHUNK - 1) / DSM_PUB_CHUNK : 1;
+    k_cloud_mirror<<<grid > 1 ? grid : 1, DSM_PUB_CHUNK, 0, s>>>(store, size_word, res, shadow, mirror, state, header);
 }

@@ -369,6 +369,42 @@ int dsm_fuse_stream_window(dsm_ctx *ctx, int n_frames, const int32_t *reference_
                            const int32_t *reactivate_kf, const int32_t *reactivate_ofs, /* [n_frames + 1] */
                            int32_t *n_new);
 
+/* ---- publishing from inside the stream: the node's active and inactive clouds after a fused frame ----
+ * What synchronize_msgs publishes after every fuse (surfel_map.cpp:191-198), enqueued in stream order like a fuse, with
+ * one wait (or none, one frame late) and only the changed part of the inactive cloud crossing PCIe.
+ *   dsm_publish_enable    once, on a context with a resident pool (DSM_E_STATE otherwise, and when called twice):
+ *                         allocates pinned host buffers the device writes directly -- max_local_surfels points for the
+ *                         active cloud and, with a store, its reservation for the inactive cloud -- plus a device shadow
+ *                         of the inactive cloud as the host last received it (16 B per reserved surfel).  DSM_E_NOMEM.
+ *                         A later dsm_inactive_reserve rebuilds the inactive buffers with the store (DSM_E_STATE while a
+ *                         snapshot is in flight).
+ *   dsm_publish_enqueue   asynchronous, ordered on the context's stream exactly like dsm_pool_transform: the snapshot is
+ *                         the map after everything enqueued before it (the frame-by-frame stages of the preceding
+ *                         resident call included) and before anything enqueued after it.  Runs the ordered selection of
+ *                         dsm_pool_export_cloud(min_update_times) into the active buffer and one pass over the store that
+ *                         compares each chunk of 256 points with the shadow and forwards the chunks that differ.  Never
+ *                         waits and reads nothing back.  DSM_E_STATE before dsm_publish_enable, and while a snapshot is
+ *                         enqueued and not yet waited for (the host may be reading the buffers).
+ *   dsm_publish_wait      waits for that snapshot only, not for the stream.  *active / *inactive are the context's pinned
+ *                         buffers: valid until the next dsm_publish_enqueue (or dsm_inactive_reserve), never to be freed
+ *                         or written.  active[0 .. *n_active) is what dsm_pool_export_cloud(ctx, min_update_times, ...)
+ *                         would have returned at the snapshot's position in the stream, inactive[0 .. *n_inactive) what
+ *                         dsm_inactive_export_cloud would have, byte for byte (no store: 0 points, *inactive NULL).
+ *                         Points below *inactive_changed_from are bit-identical to the previous snapshot's: it is the
+ *                         lowest index whose point differs from the previous snapshot, an index at or beyond the previous
+ *                         size counting as different, and *n_inactive when there is none.  The first snapshot, and the
+ *                         first after dsm_inactive_reserve, report 0.  Any out-pointer may be NULL.  If a frame of
+ *                         dsm_fuse_stream_window had been rejected before the snapshot, the call returns DSM_E_CAPACITY
+ *                         with the clouds of the last applied frame and does NOT clear the error: the next synchronising
+ *                         call reports and clears it as stated above.  DSM_E_STATE with no snapshot enqueued.
+ *   dsm_debug_publish_chunks   the number of 256-point chunks the last waited snapshot forwarded to the host (0 when the
+ *                         store did not change); DSM_E_STATE while a snapshot is in flight. */
+int dsm_publish_enable(dsm_ctx *ctx);
+int dsm_publish_enqueue(dsm_ctx *ctx, int min_update_times);
+int dsm_publish_wait(dsm_ctx *ctx, const dsm_point_t **active, int *n_active, const dsm_point_t **inactive, int *n_inactive,
+                     int *inactive_changed_from);
+int dsm_debug_publish_chunks(dsm_ctx *ctx, int *count);
+
 /* ---- multi-GPU: frames of a batch sharded across GPUs, ONE gather of the surfel deltas at the end (SURVEY.md 8e) ----
  * One context per GPU (one process or thread each).  The reference has no counterpart (fuse_initialize_map is
  * single-process, fusion_functions.cpp:30-83); what is gathered is what SurfelMap::fuse_map consumes after the call

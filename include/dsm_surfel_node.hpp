@@ -41,6 +41,21 @@
 //     comes back from the next call that reads the map, as dsm_fuse_stream_window specifies.
 //
 // A fused frame never waits for the GPU: the callbacks only enqueue.  The readers (clouds, save_*) synchronise.
+//
+// Publishing after every frame, as synchronize_msgs does (:191-198), through those readers costs several round trips
+// and a copy of the whole inactive cloud per frame.  enable_publishing() makes every fused frame enqueue a snapshot of
+// the active and the inactive cloud right behind its fuse (dsm_publish_enqueue(ctx, 5)), and published_clouds() hands
+// out the snapshot of the latest fused frame: called right after the depth callback it waits for that frame alone;
+// called at the start of the next frame's callback it finds the snapshot finished and waits for nothing, one frame
+// late.  The clouds are the library's pinned buffers, valid until the next frame is fused; the inactive cloud below
+// inactive_changed_from is bit-identical to the one handed out before, so a long-lived copy needs only its tail
+// rewritten.  One snapshot can be in flight: a frame fused while the previous snapshot is unread first waits for that
+// snapshot and drops it (a pose callback may have enqueued loop-closure warps in between, so it cannot be reused).
+// published_clouds() never clears a capacity error: after a frame that did not fit, it and every later call return
+// DSM_E_CAPACITY with the clouds of the last applied frame, and no later frame is applied, until a synchronising reader
+// (local_surfels(), active_points(), ... or dsm_pool_size on context()) has reported and cleared the error.  A node
+// that only ever publishes must call one of them to resume.
+// Without enable_publishing() nothing is enqueued and the node behaves exactly as before.
 // device < 0 builds the node without a context: the callbacks run the whole pose logic (pose database, sync, window
 // bookkeeping) and fuse nothing; any call that reads the map returns DSM_E_STATE.
 #pragma once
@@ -428,6 +443,24 @@ class SurfelMapNode
         if (active_points(points) != DSM_OK) return err_;
         return append_inactive(points, "all_points");
     }
+    // ---- the active and inactive clouds of every fused frame, from inside the stream (see the top of this file) ----
+    int enable_publishing()
+    {
+        if (!ready("enable_publishing")) return err_;
+        if ((err_ = dsm_publish_enable(ctx_)) == DSM_OK) publishing_ = true;
+        return report("enable_publishing");
+    }
+    // active_points() and inactive_points() as they were right after the latest fused frame; DSM_E_STATE when no frame
+    // has been fused since the last call.  A map whose latest frame did not fit returns DSM_E_CAPACITY with the clouds
+    // of the last applied frame.
+    int published_clouds(const dsm_point_t *&active, int &n_active, const dsm_point_t *&inactive, int &n_inactive, int &inactive_changed_from)
+    {
+        if (!ready("published_clouds")) return err_;
+        if (!snapshot_) return fail(DSM_E_STATE, "published_clouds");
+        snapshot_ = false;
+        err_ = dsm_publish_wait(ctx_, &active, &n_active, &inactive, &n_inactive, &inactive_changed_from);
+        return report("published_clouds");
+    }
     // publish_neighbor_pointcloud (:1283-1383): live local points, then the stored points of get_driftfree_poses(ref,
     // 2 * drift_free_poses) in list order
     int neighbor_points(int reference_index, std::vector<dsm_point_t> &points)
@@ -576,6 +609,12 @@ class SurfelMapNode
         const int32_t ref = q.reference_index;
         if (ctx_)
         {
+            if (snapshot_)
+            { // an unread snapshot is retired: its capacity report, if any, stays with the readers
+                const int rc = dsm_publish_wait(ctx_, nullptr, nullptr, nullptr, nullptr, nullptr);
+                snapshot_ = false;
+                if (rc != DSM_OK && rc != DSM_E_CAPACITY) return fail(rc, "fuse");
+            }
             err_ = dsm_fuse_stream_window(ctx_, 1, &ref, image_buffer_.front().second.data(), depth_buffer_.front().second.data(), pose16,
                                           rk.data(), ro, ak.data(), ao, nullptr);
             if (err_ != DSM_OK) return report("fuse");
@@ -586,6 +625,11 @@ class SurfelMapNode
         last_ref_ = q.reference_index;
         fused_ = true;
         pose_buffer_.pop_front();
+        if (publishing_)
+        { // after the bookkeeping: the frame is enqueued, so the host window follows the device whatever this returns
+            snapshot_ = (err_ = dsm_publish_enqueue(ctx_, 5)) == DSM_OK;
+            return report("fuse");
+        }
         return DSM_OK;
     }
 
@@ -679,5 +723,6 @@ class SurfelMapNode
     Pose last_fuse_pose_;
     int last_ref_;
     bool fused_;
+    bool publishing_ = false, snapshot_ = false; // enable_publishing; a snapshot is enqueued and not yet handed out
 };
 } // namespace dsm

@@ -1,0 +1,95 @@
+// Drives include/dsm_surfel_node.hpp through the message script of node_main.cpp (orb / image / depth messages only)
+// with or without enable_publishing(), and dumps what the node publishes.
+// Usage: publish_main W H fx fy cx cy far near drift_free_poses device max_local max_inactive publish in.bin out.bin
+//   out.bin: with publish = 1, after every depth message: int32 rc of published_clouds, int32 inactive_changed_from,
+//            the published active and inactive clouds, then int32 rc and the clouds of active_points() and
+//            inactive_points() read right after (each cloud as int32 n + n points);
+//            at the end, for either value of publish: local_surfels (int32 n + records) and inactive_points.
+// exit code 3 when no usable GPU (the library has no CPU fallback).
+#include <cstdio>
+#include <cstdlib>
+#include <vector>
+#include "dsm_surfel_node.hpp"
+
+static FILE *in_f, *out_f;
+template <class T>
+static bool get(T &v) { return fread(&v, sizeof(T), 1, in_f) == 1; }
+template <class T>
+static bool get_n(std::vector<T> &v, int n)
+{
+    if (n < 0) return false;
+    v.resize((size_t)n);
+    return n == 0 || fread(v.data(), sizeof(T), (size_t)n, in_f) == (size_t)n;
+}
+template <class T>
+static void put(const T &v) { fwrite(&v, sizeof(T), 1, out_f); }
+template <class T>
+static void put_n(const T *p, int n)
+{
+    put(n);
+    if (n > 0) fwrite(p, sizeof(T), (size_t)n, out_f);
+}
+
+int main(int argc, char **argv)
+{
+    if (argc != 16) return 2;
+    const int W = atoi(argv[1]), H = atoi(argv[2]), publish = atoi(argv[13]);
+    dsm::SurfelMapNode node(W, H, atof(argv[3]), atof(argv[4]), atof(argv[5]), atof(argv[6]), atof(argv[7]), atof(argv[8]), atoi(argv[9]),
+                            atoi(argv[10]), atoi(argv[11]), atoi(argv[12]), nullptr);
+    if (node.last_error() != DSM_OK) return node.last_error() == DSM_E_NODEVICE ? 3 : 4;
+    if (publish && node.enable_publishing() != DSM_OK) return 4;
+    in_f = fopen(argv[14], "rb");
+    out_f = fopen(argv[15], "wb");
+    if (!in_f || !out_f) return 5;
+    std::vector<uint8_t> gray;
+    std::vector<float> depth;
+    std::vector<double> path;
+    std::vector<int> pairs;
+    std::vector<dsm_point_t> act, inact;
+    int type = 0;
+    while (get(type))
+    {
+        double stamp = 0;
+        if (type == 0)
+        {
+            int kf = 0, ref = 0, n_path = 0, n_loops = 0;
+            double pose[7];
+            if (!get(stamp) || !get(kf) || !get(ref) || fread(pose, 8, 7, in_f) != 7 || !get(n_path) || !get_n(path, 7 * n_path) ||
+                !get(n_loops) || !get_n(pairs, 2 * n_loops))
+                return 5;
+            if (node.orb_results_input(stamp, pairs.data(), n_loops, path.data(), n_path, pose, kf != 0, ref) != DSM_OK) return 6;
+        }
+        else if (type == 1)
+        {
+            if (!get(stamp) || !get_n(gray, W * H)) return 5;
+            if (node.image_input(stamp, gray.data(), (size_t)W) != DSM_OK) return 6;
+        }
+        else if (type == 2)
+        {
+            if (!get(stamp) || !get_n(depth, W * H)) return 5;
+            if (node.depth_input(stamp, depth.data(), (size_t)W * 4) != DSM_OK) return 6;
+            if (!publish) continue;
+            const dsm_point_t *a = nullptr, *b = nullptr;
+            int na = 0, nb = 0, from = 0;
+            const int rc = node.published_clouds(a, na, b, nb, from);
+            put(rc);
+            put(from);
+            put_n(a, rc == DSM_OK ? na : 0);
+            put_n(b, rc == DSM_OK ? nb : 0);
+            int rr = node.active_points(act);
+            if (rr == DSM_OK) rr = node.inactive_points(inact);
+            put(rr);
+            put_n(act.data(), (int)act.size());
+            put_n(inact.data(), (int)inact.size());
+        }
+        else
+            return 5;
+    }
+    std::vector<dsm_surfel_t> local;
+    if (node.local_surfels(local) != DSM_OK || node.inactive_points(inact) != DSM_OK) return 6;
+    put_n(local.data(), (int)local.size());
+    put_n(inact.data(), (int)inact.size());
+    fclose(in_f);
+    fclose(out_f);
+    return 0;
+}
