@@ -15,20 +15,15 @@
 // ignored silently, so it is reported on stderr and `last_error()` keeps the code (0 = OK).  There is
 // no CPU fallback.
 #pragma once
-#include <cstdio>
-#include <cstring>
 #include <vector>
-#include "dsm.h"
+#include "dsm_context.hpp"
 
 namespace dsm
 {
 class FusionFunctions
 {
   public:
-    FusionFunctions() : ctx_(nullptr), err_(0), device_(0), capacity_(1 << 21) {}
-    ~FusionFunctions() { dsm_destroy(ctx_); }
-    FusionFunctions(const FusionFunctions &) = delete;
-    FusionFunctions &operator=(const FusionFunctions &) = delete;
+    FusionFunctions() : ctx_("dsm::FusionFunctions"), device_(0), capacity_(1 << 21) {}
 
     // optional, before initialize(): CUDA ordinal and the largest local_surfels.size() to expect
     void set_device(int device, int max_local_surfels = 1 << 21)
@@ -40,17 +35,8 @@ class FusionFunctions
     // reference: FusionFunctions::initialize (fusion_functions.cpp:7-28)
     void initialize(int _width, int _height, float _fx, float _fy, float _cx, float _cy, float _fuse_far, float _fuse_near)
     {
-        dsm_destroy(ctx_);
-        ctx_ = nullptr;
-        dsm_params p;
-        std::memset(&p, 0, sizeof(p));
-        p.width = _width, p.height = _height;
-        p.fx = _fx, p.fy = _fy, p.cx = _cx, p.cy = _cy;
-        p.fuse_far = _fuse_far, p.fuse_near = _fuse_near;
-        p.max_batch = 1;
-        p.max_local_surfels = capacity_;
-        err_ = dsm_create(&p, device_, nullptr, &ctx_);
-        if (err_ != DSM_OK) std::fprintf(stderr, "dsm::FusionFunctions::initialize failed: %s\n", dsm_strerror(err_));
+        const dsm_params p = detail::Context::params(_width, _height, _fx, _fy, _cx, _cy, _fuse_far, _fuse_near, 1, capacity_);
+        ctx_.open("initialize", p, device_, false, nullptr, nullptr);
     }
 
     // reference: FusionFunctions::fuse_initialize_map (fusion_functions.cpp:30-83).
@@ -62,26 +48,17 @@ class FusionFunctions
     {
         static_assert(sizeof(Surfel) == sizeof(dsm_surfel_t), "SurfelElement must be the 44-byte reference POD");
         new_surfels.clear();
-        if (!ctx_)
-        {
-            err_ = DSM_E_STATE;
-            std::fprintf(stderr, "dsm::FusionFunctions::fuse_initialize_map: initialize() has not succeeded\n");
-            return;
-        }
-        const int S = dsm_num_seeds(ctx_);
+        if (!ctx_.ready("fuse_initialize_map")) return;
+        const int S = dsm_num_seeds(ctx_.ctx);
         new_surfels.resize((size_t)S);
         int n_new = 0;
-        err_ = dsm_fuse_frame(ctx_, reference_frame_index,
-                              reinterpret_cast<const uint8_t *>(input_image.data), (size_t)input_image.step,
-                              reinterpret_cast<const float *>(input_depth.data), (size_t)input_depth.step,
-                              pose.data(),
-                              reinterpret_cast<dsm_surfel_t *>(local_surfels.data()), (int)local_surfels.size(),
-                              reinterpret_cast<dsm_surfel_t *>(new_surfels.data()), S, &n_new);
-        if (err_ != DSM_OK)
-        {
-            std::fprintf(stderr, "dsm::FusionFunctions::fuse_initialize_map failed: %s (%s)\n", dsm_strerror(err_), dsm_last_error(ctx_));
-            n_new = 0;
-        }
+        const int rc = dsm_fuse_frame(ctx_.ctx, reference_frame_index,
+                                      reinterpret_cast<const uint8_t *>(input_image.data), (size_t)input_image.step,
+                                      reinterpret_cast<const float *>(input_depth.data), (size_t)input_depth.step,
+                                      pose.data(),
+                                      reinterpret_cast<dsm_surfel_t *>(local_surfels.data()), (int)local_surfels.size(),
+                                      reinterpret_cast<dsm_surfel_t *>(new_surfels.data()), S, &n_new);
+        if (ctx_.done(rc, "fuse_initialize_map") != DSM_OK) n_new = 0;
         new_surfels.resize((size_t)n_new);
     }
 
@@ -92,23 +69,14 @@ class FusionFunctions
     template <class Mat>
     int superpixel_image(Mat &image)
     {
-        if (!ctx_)
-        {
-            err_ = DSM_E_STATE;
-            std::fprintf(stderr, "dsm::FusionFunctions::superpixel_image: initialize() has not succeeded\n");
-            return err_;
-        }
-        err_ = dsm_frame_superpixel_image(ctx_, 0, reinterpret_cast<uint8_t *>(image.data), (size_t)image.step);
-        if (err_ != DSM_OK) std::fprintf(stderr, "dsm::FusionFunctions::superpixel_image failed: %s (%s)\n", dsm_strerror(err_), dsm_last_error(ctx_));
-        return err_;
+        return ctx_.run("superpixel_image", [&] { return detail::superpixel_image(ctx_, image); });
     }
 
-    int last_error() const { return err_; }
-    dsm_ctx *context() { return ctx_; }
+    int last_error() const { return ctx_.err; }
+    dsm_ctx *context() { return ctx_.ctx; }
 
   private:
-    dsm_ctx *ctx_;
-    int err_;
+    detail::Context ctx_;
     int device_;
     int capacity_;
 };

@@ -24,22 +24,138 @@
 //
 // Errors: the reference's members return void; here every method returns the C ABI code (0 = OK) and keeps it
 // in last_error().  There is no CPU fallback.
+//
+// The map operations themselves are the functions of dsm::detail below, one per operation; dsm::SurfelMapNode
+// (dsm_surfel_node.hpp) is built on the same ones.
 #pragma once
-#include <cstdio>
 #include <cstring>
 #include <string>
 #include <vector>
-#include "dsm.h"
+#include "dsm_context.hpp"
 
 namespace dsm
 {
+namespace detail
+{
+// Each operation needs a context (Context::ready), returns the C ABI code and appends to the caller's vector, which a
+// failure leaves as it was.
+
+inline int pool_size(Context &c, int &n)
+{
+    n = 0;
+    return dsm_pool_size(c.ctx, &n);
+}
+// the size-then-read of the pool and of the inactive store (read_records)
+template <class Rec, class T, class Read>
+int read_pool(Context &c, std::vector<T> &out, Read read)
+{
+    int n = 0;
+    const int rc = pool_size(c, n);
+    return rc != DSM_OK ? rc : read_records<Rec>(out, n, read);
+}
+template <class Rec, class T, class Read>
+int read_store(Context &c, std::vector<T> &out, Read read)
+{
+    int n = 0;
+    const int rc = dsm_inactive_size(c.ctx, &n, nullptr);
+    return rc != DSM_OK ? rc : read_records<Rec>(out, n, read);
+}
+
+// the local_surfels loop of the cloud publishers: points with update_times >= min_update_times, pool order
+template <class Point>
+int pool_cloud(Context &c, int min_update_times, std::vector<Point> &points)
+{
+    return read_pool<dsm_point_t>(c, points, [&](dsm_point_t *o, int cap, int *got) { return dsm_pool_export_cloud(c.ctx, min_update_times, o, cap, got); });
+}
+// the local surfels with update_times >= min_update_times, pool order
+inline int pool_surfels(Context &c, int min_update_times, std::vector<dsm_surfel_t> &surfels)
+{
+    return read_pool<dsm_surfel_t>(c, surfels, [&](dsm_surfel_t *o, int cap, int *got) { return dsm_pool_export_surfels(c.ctx, min_update_times, o, cap, got); });
+}
+// local_surfels, pool order
+template <class Surfel>
+int whole_pool(Context &c, std::vector<Surfel> &surfels)
+{
+    return read_pool<dsm_surfel_t>(c, surfels, [&](dsm_surfel_t *o, int cap, int *got) { return dsm_pool_download(c.ctx, o, cap, got); });
+}
+// move_add_surfels(), removal: the live surfels last updated by `keyframe` leave the pool, in pool order
+template <class Surfel>
+int retire(Context &c, int keyframe, std::vector<Surfel> &surfels)
+{
+    return read_pool<dsm_surfel_t>(c, surfels, [&](dsm_surfel_t *o, int cap, int *got) { return dsm_pool_retire(c.ctx, keyframe, o, cap, got); });
+}
+// inactive_pointcloud: the inactive store, store order
+template <class Point>
+int inactive_cloud(Context &c, std::vector<Point> &points)
+{
+    return read_store<dsm_point_t>(c, points, [&](dsm_point_t *o, int cap, int *got) { return dsm_inactive_export_cloud(c.ctx, o, cap, got); });
+}
+// publish_neighbor_pointcloud (surfel_map.cpp:1283-1383): the live local points (update_times != 0), then the stored
+// points of `keyframes` in list order
+template <class Point>
+int neighbourhood(Context &c, const std::vector<int> &keyframes, std::vector<Point> &points)
+{
+    const std::vector<int32_t> kf(keyframes.begin(), keyframes.end());
+    const int rc = pool_cloud(c, 1, points);
+    return rc != DSM_OK ? rc : read_store<dsm_point_t>(c, points, [&](dsm_point_t *o, int cap, int *got) {
+        return dsm_inactive_export_poses(c.ctx, kf.data(), (int)kf.size(), o, cap, got);
+    });
+}
+// PoseElement::attached_surfels of one keyframe, or the whole store in store order for keyframe -1
+template <class Surfel>
+int attached(Context &c, int keyframe, std::vector<Surfel> &surfels)
+{
+    int n = 0;
+    const int rc = dsm_inactive_download(c.ctx, keyframe, nullptr, 0, &n);
+    return rc != DSM_OK ? rc : read_records<dsm_surfel_t>(surfels, n, [&](dsm_surfel_t *o, int cap, int *got) {
+        return dsm_inactive_download(c.ctx, keyframe, o, cap, got);
+    });
+}
+// publish_raw_pointcloud (surfel_map.cpp:1115-1151) of the last fused frame: every pixel (n_pixels = width * height) in
+// the world frame at pose7 = {px, py, pz, qx, qy, qz, qw}, column-major, holes included
+template <class Point>
+int raw_cloud(Context &c, const double pose7[7], int n_pixels, std::vector<Point> &points)
+{
+    return read_records<dsm_point_t>(points, n_pixels, [&](dsm_point_t *o, int cap, int *got) { return dsm_frame_raw_cloud(c.ctx, 0, pose7, o, cap, got); });
+}
+
+// save_mesh: `surfels` (the attached surfels of every pose) followed by the local surfels with update_times >= 5, one
+// hexagon each, ASCII PLY
+inline int save_mesh(Context &c, const std::string &name, std::vector<dsm_surfel_t> surfels)
+{
+    int rc = pool_surfels(c, 5, surfels);
+    if (rc == DSM_OK) rc = dsm_write_ply_mesh(name.c_str(), surfels.data(), surfels.size());
+    return rc;
+}
+// save_cloud: the local points with update_times >= 5 followed by the inactive cloud, PCD v0.7 ASCII.  The inactive
+// cloud is the caller's `inactive` points, or the device store's when it is null.
+template <class Point>
+int save_cloud(Context &c, const std::string &name, const std::vector<Point> *inactive)
+{
+    std::vector<dsm_point_t> points;
+    int rc = pool_cloud(c, 5, points);
+    if (rc == DSM_OK && !inactive) rc = inactive_cloud(c, points);
+    if (rc != DSM_OK) return rc;
+    if (inactive) append_points(points, *inactive);
+    return dsm_write_pcd(name.c_str(), points.data(), points.size(), 0);
+}
+
+// synchronize_msgs (surfel_map.cpp:154-161) for one frame: move_add_surfels with the two lists, then fuse_map, all on
+// the device; tightly packed images
+inline int fuse_window(Context &c, int reference_index, const uint8_t *gray, const float *depth, const float pose16[16],
+                       const std::vector<int> &poses_to_remove, const std::vector<int> &poses_to_add)
+{
+    const std::vector<int32_t> rk(poses_to_remove.begin(), poses_to_remove.end()), ak(poses_to_add.begin(), poses_to_add.end());
+    const int32_t ro[2] = {0, (int32_t)rk.size()}, ao[2] = {0, (int32_t)ak.size()};
+    const int32_t ref = reference_index;
+    return dsm_fuse_stream_window(c.ctx, 1, &ref, gray, depth, pose16, rk.data(), ro, ak.data(), ao, nullptr);
+}
+} // namespace detail
+
 class ResidentSurfelPool
 {
   public:
-    ResidentSurfelPool() : ctx_(nullptr), err_(0), device_(0), capacity_(1 << 21), width_(0), height_(0) {}
-    ~ResidentSurfelPool() { dsm_destroy(ctx_); }
-    ResidentSurfelPool(const ResidentSurfelPool &) = delete;
-    ResidentSurfelPool &operator=(const ResidentSurfelPool &) = delete;
+    ResidentSurfelPool() : ctx_("dsm::ResidentSurfelPool"), device_(0), capacity_(1 << 21), width_(0), height_(0) {}
 
     void set_device(int device, int max_local_surfels = 1 << 21)
     {
@@ -49,19 +165,10 @@ class ResidentSurfelPool
 
     int initialize(int width, int height, float fx, float fy, float cx, float cy, float fuse_far, float fuse_near)
     {
-        dsm_destroy(ctx_);
-        ctx_ = nullptr;
-        dsm_params p;
-        std::memset(&p, 0, sizeof(p));
-        p.width = width, p.height = height;
-        p.fx = fx, p.fy = fy, p.cx = cx, p.cy = cy;
-        p.fuse_far = fuse_far, p.fuse_near = fuse_near;
-        p.max_batch = 2; // two frame slots: the copy of frame t+1 overlaps the kernels of frame t
-        p.max_local_surfels = capacity_;
         width_ = width, height_ = height;
-        err_ = dsm_create(&p, device_, nullptr, &ctx_);
-        if (err_ == DSM_OK) err_ = dsm_pool_upload(ctx_, nullptr, 0); // local_surfels starts empty
-        return report("initialize");
+        // two frame slots: the copy of frame t+1 overlaps the kernels of frame t; local_surfels starts empty
+        const dsm_params p = detail::Context::params(width, height, fx, fy, cx, cy, fuse_far, fuse_near, 2, capacity_);
+        return ctx_.open("initialize", p, device_, true, nullptr, nullptr);
     }
 
     // SurfelMap::fuse_map: the hot-path call plus the post-step (slot recycling as the reference), all on the device.
@@ -69,10 +176,10 @@ class ResidentSurfelPool
     template <class Mat, class Mat4f>
     int fuse_map(Mat &image, Mat &depth, Mat4f &pose, int reference_index)
     {
-        if (!ready("fuse_map")) return err_;
-        err_ = dsm_fuse_frame_resident(ctx_, reference_index, reinterpret_cast<const uint8_t *>(image.data), (size_t)image.step,
-                                       reinterpret_cast<const float *>(depth.data), (size_t)depth.step, pose.data(), nullptr);
-        return report("fuse_map");
+        return ctx_.run("fuse_map", [&] {
+            return dsm_fuse_frame_resident(ctx_.ctx, reference_index, reinterpret_cast<const uint8_t *>(image.data), (size_t)image.step,
+                                           reinterpret_cast<const float *>(depth.data), (size_t)depth.step, pose.data(), nullptr);
+        });
     }
 
     // synchronize_msgs (surfel_map.cpp:154-161) in one call: move_add_surfels with the lists get_add_remove_poses hands
@@ -83,7 +190,7 @@ class ResidentSurfelPool
     int fuse_map(Mat &image, Mat &depth, Mat4f &pose, int reference_index, const std::vector<int> &poses_to_remove,
                  const std::vector<int> &poses_to_add)
     {
-        if (!ready("fuse_map")) return err_;
+        if (!ctx_.ready("fuse_map")) return ctx_.err;
         const uint8_t *g = reinterpret_cast<const uint8_t *>(image.data);
         const float *d = reinterpret_cast<const float *>(depth.data);
         if ((size_t)image.step != (size_t)width_ || (size_t)depth.step != (size_t)width_ * 4)
@@ -98,20 +205,14 @@ class ResidentSurfelPool
             }
             g = packed_gray_.data(), d = packed_depth_.data();
         }
-        const std::vector<int32_t> rk(poses_to_remove.begin(), poses_to_remove.end()), ak(poses_to_add.begin(), poses_to_add.end());
-        const int32_t ro[2] = {0, (int32_t)rk.size()}, ao[2] = {0, (int32_t)ak.size()};
-        const int32_t ref = reference_index;
-        err_ = dsm_fuse_stream_window(ctx_, 1, &ref, g, d, pose.data(), rk.data(), ro, ak.data(), ao, nullptr);
-        return report("fuse_map");
+        return ctx_.done(detail::fuse_window(ctx_, reference_index, g, d, pose.data(), poses_to_remove, poses_to_add), "fuse_map");
     }
 
     // warp_surfels(): p <- W p, n <- R_W n for every local surfel; W = T_loop * T_cam^-1 as float, column-major
     template <class Mat4f>
     int warp_active_surfels(Mat4f &warp_pose)
     {
-        if (!ready("warp_active_surfels")) return err_;
-        err_ = dsm_pool_transform(ctx_, warp_pose.data());
-        return report("warp_active_surfels");
+        return ctx_.run("warp_active_surfels", [&] { return dsm_pool_transform(ctx_.ctx, warp_pose.data()); });
     }
 
     // move_add_surfels(), removal: the live surfels last updated by keyframe `inactive_index` leave the pool
@@ -119,19 +220,8 @@ class ResidentSurfelPool
     template <class Surfel>
     int retire_surfels(int inactive_index, std::vector<Surfel> &attached_surfels)
     {
-        static_assert(sizeof(Surfel) == sizeof(dsm_surfel_t), "SurfelElement must be the 44-byte reference POD");
         attached_surfels.clear();
-        if (!ready("retire_surfels")) return err_;
-        int n = 0;
-        err_ = dsm_pool_size(ctx_, &n);
-        if (err_ == DSM_OK)
-        {
-            attached_surfels.resize((size_t)n);
-            int got = 0;
-            err_ = dsm_pool_retire(ctx_, inactive_index, reinterpret_cast<dsm_surfel_t *>(attached_surfels.data()), n, &got);
-            attached_surfels.resize(err_ == DSM_OK ? (size_t)got : 0);
-        }
-        return report("retire_surfels");
+        return ctx_.run("retire_surfels", [&] { return detail::retire(ctx_, inactive_index, attached_surfels); });
     }
 
     // move_add_surfels(), insertion: a pose re-enters the drift-free set
@@ -139,9 +229,9 @@ class ResidentSurfelPool
     int add_surfels(const std::vector<Surfel> &attached_surfels)
     {
         static_assert(sizeof(Surfel) == sizeof(dsm_surfel_t), "SurfelElement must be the 44-byte reference POD");
-        if (!ready("add_surfels")) return err_;
-        err_ = dsm_pool_append(ctx_, reinterpret_cast<const dsm_surfel_t *>(attached_surfels.data()), (int)attached_surfels.size());
-        return report("add_surfels");
+        return ctx_.run("add_surfels", [&] {
+            return dsm_pool_append(ctx_.ctx, reinterpret_cast<const dsm_surfel_t *>(attached_surfels.data()), (int)attached_surfels.size());
+        });
     }
 
     // the local_surfels loop of the cloud publishers: points with update_times >= min_update_times, pool order.
@@ -149,34 +239,14 @@ class ResidentSurfelPool
     template <class Point>
     int active_points(std::vector<Point> &points, int min_update_times = 5)
     {
-        if (!ready("active_points")) return err_;
-        int n = 0;
-        err_ = dsm_pool_size(ctx_, &n);
-        if (err_ != DSM_OK) return report("active_points");
-        scratch_.resize((size_t)(n > 0 ? n : 1));
-        int got = 0;
-        err_ = dsm_pool_export_cloud(ctx_, min_update_times, scratch_.data(), n, &got);
-        if (err_ != DSM_OK) return report("active_points");
-        append(points, got);
-        return DSM_OK;
+        return ctx_.run("active_points", [&] { return detail::pool_cloud(ctx_, min_update_times, points); });
     }
 
     // save_cloud: active points (update_times >= 5) followed by the caller's inactive cloud, PCD v0.7 ASCII
     template <class Point>
     int save_cloud(const std::string &save_path_name, const std::vector<Point> &inactive_points)
     {
-        std::vector<dsm_point_t> all;
-        if (active_points(all, 5) != DSM_OK) return err_;
-        all.reserve(all.size() + inactive_points.size());
-        for (size_t i = 0; i < inactive_points.size(); i++)
-        {
-            dsm_point_t q;
-            q.x = inactive_points[i].x, q.y = inactive_points[i].y, q.z = inactive_points[i].z;
-            q.intensity = inactive_points[i].intensity;
-            all.push_back(q);
-        }
-        err_ = dsm_write_pcd(save_path_name.c_str(), all.data(), all.size(), 0);
-        return report("save_cloud");
+        return ctx_.run("save_cloud", [&] { return detail::save_cloud(ctx_, save_path_name, &inactive_points); });
     }
 
     // save_mesh: the attached surfels of every pose (no filter) followed by the local surfels with
@@ -185,17 +255,10 @@ class ResidentSurfelPool
     int save_mesh(const std::string &save_path_name, const std::vector<Surfel> &attached_surfels_of_all_poses)
     {
         static_assert(sizeof(Surfel) == sizeof(dsm_surfel_t), "SurfelElement must be the 44-byte reference POD");
-        if (!ready("save_mesh")) return err_;
-        int n = 0;
-        err_ = dsm_pool_size(ctx_, &n);
-        if (err_ != DSM_OK) return report("save_mesh");
-        const size_t na = attached_surfels_of_all_poses.size();
-        std::vector<dsm_surfel_t> all(na + (size_t)(n > 0 ? n : 1));
-        if (na) std::memcpy(all.data(), attached_surfels_of_all_poses.data(), na * sizeof(dsm_surfel_t));
-        int got = 0;
-        err_ = dsm_pool_export_surfels(ctx_, 5, all.data() + na, n, &got);
-        if (err_ == DSM_OK) err_ = dsm_write_ply_mesh(save_path_name.c_str(), all.data(), na + (size_t)got);
-        return report("save_mesh");
+        if (!ctx_.ready("save_mesh")) return ctx_.err;
+        const dsm_surfel_t *a = reinterpret_cast<const dsm_surfel_t *>(attached_surfels_of_all_poses.data());
+        return ctx_.done(detail::save_mesh(ctx_, save_path_name, std::vector<dsm_surfel_t>(a, a + attached_surfels_of_all_poses.size())),
+                         "save_mesh");
     }
 
     // ---- device-resident attached_surfels / inactive_pointcloud (see include/dsm.h "inactive store") ----
@@ -203,48 +266,38 @@ class ResidentSurfelPool
     // per-pose inactive warp never move surfels across PCIe.
     int reserve_inactive(int max_inactive_surfels)
     {
-        if (!ready("reserve_inactive")) return err_;
-        err_ = dsm_inactive_reserve(ctx_, max_inactive_surfels);
-        return report("reserve_inactive");
+        return ctx_.run("reserve_inactive", [&] { return dsm_inactive_reserve(ctx_.ctx, max_inactive_surfels); });
     }
     // move_add_surfels(), removal (surfel_map.cpp:1479-1497) without the host copy; returns the surfel count or -1
     int retire_surfels_resident(int inactive_index)
     {
-        if (!ready("retire_surfels_resident")) return -1;
         int n = 0;
-        err_ = dsm_inactive_retire(ctx_, inactive_index, &n);
-        return report("retire_surfels_resident") == DSM_OK ? n : -1;
+        return ctx_.run("retire_surfels_resident", [&] { return dsm_inactive_retire(ctx_.ctx, inactive_index, &n); }) == DSM_OK ? n : -1;
     }
     // move_add_surfels(), insertion (surfel_map.cpp:1583-1587)
     int add_surfels_resident(int pose_index)
     {
-        if (!ready("add_surfels_resident")) return -1;
         int n = 0;
-        err_ = dsm_inactive_reactivate(ctx_, pose_index, &n);
-        return report("add_surfels_resident") == DSM_OK ? n : -1;
+        return ctx_.run("add_surfels_resident", [&] { return dsm_inactive_reactivate(ctx_.ctx, pose_index, &n); }) == DSM_OK ? n : -1;
     }
     // warp_inactive_surfels_cpu_kernel for one pose (surfel_map.cpp:704-733): warp_matrix = (after * pre^-1).cast<float>()
     template <class Mat4f>
     int warp_inactive_surfels(int pose_index, Mat4f &warp_matrix)
     {
-        if (!ready("warp_inactive_surfels")) return err_;
-        err_ = dsm_inactive_transform(ctx_, pose_index, warp_matrix.data());
-        return report("warp_inactive_surfels");
+        return ctx_.run("warp_inactive_surfels", [&] { return dsm_inactive_transform(ctx_.ctx, pose_index, warp_matrix.data()); });
+    }
+    // PoseElement::attached_surfels of pose_index as stored on the device, or every pose's in store order for -1
+    template <class Surfel>
+    int attached_surfels(int pose_index, std::vector<Surfel> &out)
+    {
+        out.clear();
+        return ctx_.run("attached_surfels", [&] { return detail::attached(ctx_, pose_index, out); });
     }
     // inactive_pointcloud appended to `points` (publish_inactive_pointcloud / publish_all_pointcloud / save_cloud)
     template <class Point>
     int inactive_points(std::vector<Point> &points)
     {
-        if (!ready("inactive_points")) return err_;
-        int n = 0;
-        err_ = dsm_inactive_size(ctx_, &n, nullptr);
-        if (err_ != DSM_OK) return report("inactive_points");
-        scratch_.resize((size_t)(n > 0 ? n : 1));
-        int got = 0;
-        err_ = dsm_inactive_export_cloud(ctx_, scratch_.data(), n, &got);
-        if (err_ != DSM_OK) return report("inactive_points");
-        append(points, got);
-        return DSM_OK;
+        return ctx_.run("inactive_points", [&] { return detail::inactive_cloud(ctx_, points); });
     }
 
     // publish_neighbor_pointcloud (surfel_map.cpp:1283-1383): the live local points (update_times != 0) followed by the
@@ -253,17 +306,7 @@ class ResidentSurfelPool
     template <class Point>
     int neighbor_points(std::vector<Point> &points, const std::vector<int> &neighbor_indexs)
     {
-        if (active_points(points, 1) != DSM_OK) return err_;
-        int n = 0;
-        err_ = dsm_inactive_size(ctx_, &n, nullptr);
-        if (err_ != DSM_OK) return report("neighbor_points");
-        scratch_.resize((size_t)(n > 0 ? n : 1));
-        std::vector<int32_t> kf(neighbor_indexs.begin(), neighbor_indexs.end());
-        int got = 0;
-        err_ = dsm_inactive_export_poses(ctx_, kf.data(), (int)kf.size(), scratch_.data(), n, &got);
-        if (err_ != DSM_OK) return report("neighbor_points");
-        append(points, got);
-        return DSM_OK;
+        return ctx_.run("neighbor_points", [&] { return detail::neighbourhood(ctx_, neighbor_indexs, points); });
     }
 
     // publish_raw_pointcloud (surfel_map.cpp:1115-1151) of the frame of the last fuse_map: every pixel in the world frame,
@@ -272,15 +315,10 @@ class ResidentSurfelPool
     template <class Point, class Pose>
     int raw_points(std::vector<Point> &points, const Pose &pose)
     {
-        if (!ready("raw_points")) return err_;
+        if (!ctx_.ready("raw_points")) return ctx_.err;
         const double p7[7] = {pose.position.x, pose.position.y, pose.position.z, pose.orientation.x, pose.orientation.y,
                               pose.orientation.z, pose.orientation.w};
-        scratch_.resize((size_t)width_ * (size_t)height_);
-        int got = 0;
-        err_ = dsm_frame_raw_cloud(ctx_, 0, p7, scratch_.data(), (int)scratch_.size(), &got);
-        if (err_ != DSM_OK) return report("raw_points");
-        append(points, got);
-        return DSM_OK;
+        return ctx_.done(detail::raw_cloud(ctx_, p7, width_ * height_, points), "raw_points");
     }
 
     // FusionFunctions::debug_show (fusion_functions.cpp:977-1006) of the frame of the last fuse_map: the superpixel normal
@@ -289,71 +327,31 @@ class ResidentSurfelPool
     template <class Mat>
     int superpixel_image(Mat &image)
     {
-        if (!ready("superpixel_image")) return err_;
-        err_ = dsm_frame_superpixel_image(ctx_, 0, reinterpret_cast<uint8_t *>(image.data), (size_t)image.step);
-        return report("superpixel_image");
+        return ctx_.run("superpixel_image", [&] { return detail::superpixel_image(ctx_, image); });
     }
 
     // local_surfels as a host vector (debugging, or a caller that still wants the whole pool)
     template <class Surfel>
     int download(std::vector<Surfel> &local_surfels)
     {
-        static_assert(sizeof(Surfel) == sizeof(dsm_surfel_t), "SurfelElement must be the 44-byte reference POD");
         local_surfels.clear();
-        if (!ready("download")) return err_;
-        int n = 0;
-        err_ = dsm_pool_size(ctx_, &n);
-        if (err_ == DSM_OK)
-        {
-            local_surfels.resize((size_t)n);
-            int got = 0;
-            err_ = dsm_pool_download(ctx_, reinterpret_cast<dsm_surfel_t *>(local_surfels.data()), n, &got);
-        }
-        return report("download");
+        return ctx_.run("download", [&] { return detail::whole_pool(ctx_, local_surfels); });
     }
 
     int size()
     {
         int n = 0;
-        if (!ctx_ || dsm_pool_size(ctx_, &n) != DSM_OK) return 0;
+        if (!ctx_.ctx || detail::pool_size(ctx_, n) != DSM_OK) return 0;
         return n;
     }
-    int last_error() const { return err_; }
-    dsm_ctx *context() { return ctx_; }
+    int last_error() const { return ctx_.err; }
+    dsm_ctx *context() { return ctx_.ctx; }
 
   private:
-    bool ready(const char *what)
-    {
-        if (ctx_) return true;
-        err_ = DSM_E_STATE;
-        std::fprintf(stderr, "dsm::ResidentSurfelPool::%s: initialize() has not succeeded\n", what);
-        return false;
-    }
-    // the first `got` points of scratch_, converted field by field, appended to `points`
-    template <class Point>
-    void append(std::vector<Point> &points, int got)
-    {
-        points.reserve(points.size() + (size_t)got);
-        for (int i = 0; i < got; i++)
-        {
-            Point p;
-            p.x = scratch_[(size_t)i].x, p.y = scratch_[(size_t)i].y, p.z = scratch_[(size_t)i].z;
-            p.intensity = scratch_[(size_t)i].intensity;
-            points.push_back(p);
-        }
-    }
-    int report(const char *what)
-    {
-        if (err_ != DSM_OK)
-            std::fprintf(stderr, "dsm::ResidentSurfelPool::%s failed: %s (%s)\n", what, dsm_strerror(err_), ctx_ ? dsm_last_error(ctx_) : "no context");
-        return err_;
-    }
-    dsm_ctx *ctx_;
-    int err_;
+    detail::Context ctx_;
     int device_;
     int capacity_;
     int width_, height_;
-    std::vector<dsm_point_t> scratch_;
     std::vector<uint8_t> packed_gray_;
     std::vector<float> packed_depth_;
 };

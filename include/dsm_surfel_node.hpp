@@ -1,8 +1,8 @@
 // dsm_surfel_node.hpp — header-only dsm::SurfelMapNode: the reference's whole SurfelMap node (surfel_fusion/src/
-// surfel_map.cpp) with the map resident on the GPU, callback for callback, built on the C ABI of dsm.h alone.  Like
-// dsm_surfel_map.hpp it needs neither ROS, Eigen, OpenCV nor PCL: poses are 7 doubles in geometry_msgs::Pose order
-// {px, py, pz, qx, qy, qz, qw}, images are a pointer and a row pitch, clouds are vectors of dsm_point_t.  A ROS node on
-// top of it is topic glue only (INTEGRATION.md §4).
+// surfel_map.cpp) with the map resident on the GPU, callback for callback, built on the C ABI of dsm.h and the map
+// operations of dsm_surfel_map.hpp.  Like dsm_surfel_map.hpp it needs neither ROS, Eigen, OpenCV nor PCL: poses are 7
+// doubles in geometry_msgs::Pose order {px, py, pz, qx, qy, qz, qw}, images are a pointer and a row pitch, clouds are
+// vectors of dsm_point_t.  A ROS node on top of it is topic glue only (INTEGRATION.md §4).
 //
 //   SurfelMap member (surfel_map.cpp)                     here
 //   ---------------------------------------------------   ---------------------------------------------------------
@@ -61,14 +61,13 @@
 #pragma once
 #include <algorithm>
 #include <cmath>
-#include <cstdio>
 #include <cstring>
 #include <deque>
 #include <set>
 #include <string>
 #include <utility>
 #include <vector>
-#include "dsm.h"
+#include "dsm_surfel_map.hpp"
 
 namespace dsm
 {
@@ -229,33 +228,17 @@ class SurfelMapNode
     SurfelMapNode(int cam_width, int cam_height, double cam_fx, double cam_fy, double cam_cx, double cam_cy, double far_dist,
                   double near_dist, int drift_free_poses, int device = 0, int max_local_surfels = 1 << 21,
                   int max_inactive_surfels = 1 << 22, const dsm_constants *constants = nullptr)
-        : ctx_(nullptr), err_(DSM_OK), width_(cam_width), height_(cam_height), drift_free_poses_(drift_free_poses),
-          last_ref_(-1), fused_(false)
+        : ctx_("dsm::SurfelMapNode"), width_(cam_width), height_(cam_height), drift_free_poses_(drift_free_poses), last_ref_(-1),
+          fused_(false)
     {
         std::memset(transform_kitti_.d, 0, sizeof(transform_kitti_.d));
         std::memset(&last_fuse_pose_, 0, sizeof(last_fuse_pose_));
         if (device < 0) return;
-        dsm_params p;
-        std::memset(&p, 0, sizeof(p));
-        p.width = cam_width, p.height = cam_height;
-        p.fx = (float)cam_fx, p.fy = (float)cam_fy, p.cx = (float)cam_cx, p.cy = (float)cam_cy;
-        p.fuse_far = (float)far_dist, p.fuse_near = (float)near_dist;
-        p.max_batch = 2; // two frame slots: the copy of frame t+1 overlaps the kernels of frame t
-        p.max_local_surfels = max_local_surfels;
-        err_ = dsm_create(&p, device, nullptr, &ctx_);
-        if (err_ == DSM_OK) err_ = dsm_pool_upload(ctx_, nullptr, 0);
-        if (err_ == DSM_OK) err_ = dsm_inactive_reserve(ctx_, max_inactive_surfels);
-        if (err_ == DSM_OK && constants) err_ = dsm_set_constants(ctx_, constants);
-        if (err_ != DSM_OK)
-        {
-            report("SurfelMapNode");
-            dsm_destroy(ctx_);
-            ctx_ = nullptr;
-        }
+        // two frame slots: the copy of frame t+1 overlaps the kernels of frame t
+        const dsm_params p = detail::Context::params(cam_width, cam_height, (float)cam_fx, (float)cam_fy, (float)cam_cx, (float)cam_cy,
+                                                     (float)far_dist, (float)near_dist, 2, max_local_surfels);
+        ctx_.open("SurfelMapNode", p, device, true, &max_inactive_surfels, constants);
     }
-    ~SurfelMapNode() { dsm_destroy(ctx_); }
-    SurfelMapNode(const SurfelMapNode &) = delete;
-    SurfelMapNode &operator=(const SurfelMapNode &) = delete;
 
     // ---- the three callbacks of ros_node.cpp ----
 
@@ -267,13 +250,13 @@ class SurfelMapNode
     {
         using namespace node_math;
         const int n_poses = (int)poses_.size();
-        if (!this_pose7 || n_loops < 0 || n_path < 0 || (n_loops && !loop_pairs) || (n_path && !loop_path7)) return fail(DSM_E_INVALID, "orb_results_input");
+        if (!this_pose7 || n_loops < 0 || n_path < 0 || (n_loops && !loop_pairs) || (n_path && !loop_path7)) return ctx_.done(DSM_E_INVALID, "orb_results_input");
         const bool new_kf = is_keyframe || n_poses == 0;
         // a new keyframe links to its reference, which must exist already; any other frame refers to an existing pose
         const int n_after = n_poses + (new_kf ? 1 : 0);
-        if (reference_index < 0 || reference_index >= (new_kf && n_poses > 0 ? n_poses : n_after)) return fail(DSM_E_INVALID, "orb_results_input");
+        if (reference_index < 0 || reference_index >= (new_kf && n_poses > 0 ? n_poses : n_after)) return ctx_.done(DSM_E_INVALID, "orb_results_input");
         for (int i = 0; i < 2 * n_loops; i++)
-            if (loop_pairs[i] < 0) return fail(DSM_E_INVALID, "orb_results_input");
+            if (loop_pairs[i] < 0) return ctx_.done(DSM_E_INVALID, "orb_results_input");
 
         last_warp_.clear();
         // the KITTI axis fix-up, fixed by the first pose (:214-232)
@@ -342,14 +325,14 @@ class SurfelMapNode
     // image_input / depth_input (surfel_map.cpp:83-101): the frame is copied (row pitch in bytes), then the sync runs
     int image_input(double stamp, const uint8_t *gray, size_t pitch)
     {
-        if (!gray || pitch < (size_t)width_) return fail(DSM_E_INVALID, "image_input");
+        if (!gray || pitch < (size_t)width_) return ctx_.done(DSM_E_INVALID, "image_input");
         image_buffer_.push_back(std::make_pair(stamp, std::vector<uint8_t>((size_t)width_ * height_)));
         for (int y = 0; y < height_; y++) std::memcpy(&image_buffer_.back().second[(size_t)y * width_], gray + (size_t)y * pitch, (size_t)width_);
         return synchronize();
     }
     int depth_input(double stamp, const float *depth, size_t pitch)
     {
-        if (!depth || pitch < (size_t)width_ * 4) return fail(DSM_E_INVALID, "depth_input");
+        if (!depth || pitch < (size_t)width_ * 4) return ctx_.done(DSM_E_INVALID, "depth_input");
         depth_buffer_.push_back(std::make_pair(stamp, std::vector<float>((size_t)width_ * height_)));
         const uint8_t *src = reinterpret_cast<const uint8_t *>(depth);
         for (int y = 0; y < height_; y++)
@@ -430,91 +413,71 @@ class SurfelMapNode
 
     // ---- the clouds the node publishes; each replaces `points` ----
     // publish_active_pointcloud (:1398-1417): local surfels with update_times >= 5, pool order
-    int active_points(std::vector<dsm_point_t> &points) { return read_pool_cloud(points, 5, "active_points"); }
+    int active_points(std::vector<dsm_point_t> &points)
+    {
+        points.clear();
+        return ctx_.run("active_points", [&] { return detail::pool_cloud(ctx_, 5, points); });
+    }
     // publish_inactive_pointcloud (:1385-1396): the inactive store, store order, every warped point warped
     int inactive_points(std::vector<dsm_point_t> &points)
     {
         points.clear();
-        return append_inactive(points, "inactive_points");
+        return ctx_.run("inactive_points", [&] { return detail::inactive_cloud(ctx_, points); });
     }
     // publish_all_pointcloud (:1419-1454)
     int all_points(std::vector<dsm_point_t> &points)
     {
-        if (active_points(points) != DSM_OK) return err_;
-        return append_inactive(points, "all_points");
+        points.clear();
+        if (!ctx_.ready("all_points")) return ctx_.err;
+        int rc = detail::pool_cloud(ctx_, 5, points);
+        if (rc == DSM_OK) rc = detail::inactive_cloud(ctx_, points);
+        return ctx_.done(rc, "all_points");
     }
     // ---- the active and inactive clouds of every fused frame, from inside the stream (see the top of this file) ----
     int enable_publishing()
     {
-        if (!ready("enable_publishing")) return err_;
-        if ((err_ = dsm_publish_enable(ctx_)) == DSM_OK) publishing_ = true;
-        return report("enable_publishing");
+        if (ctx_.run("enable_publishing", [&] { return dsm_publish_enable(ctx_.ctx); }) == DSM_OK) publishing_ = true;
+        return ctx_.err;
     }
     // active_points() and inactive_points() as they were right after the latest fused frame; DSM_E_STATE when no frame
     // has been fused since the last call.  A map whose latest frame did not fit returns DSM_E_CAPACITY with the clouds
     // of the last applied frame.
     int published_clouds(const dsm_point_t *&active, int &n_active, const dsm_point_t *&inactive, int &n_inactive, int &inactive_changed_from)
     {
-        if (!ready("published_clouds")) return err_;
-        if (!snapshot_) return fail(DSM_E_STATE, "published_clouds");
+        if (!ctx_.ready("published_clouds")) return ctx_.err;
+        if (!snapshot_) return ctx_.done(DSM_E_STATE, "published_clouds");
         snapshot_ = false;
-        err_ = dsm_publish_wait(ctx_, &active, &n_active, &inactive, &n_inactive, &inactive_changed_from);
-        return report("published_clouds");
+        return ctx_.done(dsm_publish_wait(ctx_.ctx, &active, &n_active, &inactive, &n_inactive, &inactive_changed_from), "published_clouds");
     }
     // publish_neighbor_pointcloud (:1283-1383): live local points, then the stored points of get_driftfree_poses(ref,
     // 2 * drift_free_poses) in list order
     int neighbor_points(int reference_index, std::vector<dsm_point_t> &points)
     {
-        if (read_pool_cloud(points, 1, "neighbor_points") != DSM_OK) return err_;
-        const std::vector<int> df = driftfree_poses(reference_index, 2 * drift_free_poses_);
-        const std::vector<int32_t> kf(df.begin(), df.end());
-        int n = 0;
-        if ((err_ = dsm_inactive_size(ctx_, &n, nullptr)) != DSM_OK) return report("neighbor_points");
-        const size_t base = points.size();
-        points.resize(base + (size_t)n + 1);
-        int got = 0;
-        err_ = dsm_inactive_export_poses(ctx_, kf.data(), (int)kf.size(), points.data() + base, n, &got);
-        points.resize(err_ == DSM_OK ? base + (size_t)got : base);
-        return report("neighbor_points");
+        points.clear();
+        return ctx_.run("neighbor_points",
+                        [&] { return detail::neighbourhood(ctx_, driftfree_poses(reference_index, 2 * drift_free_poses_), points); });
     }
     // publish_raw_pointcloud (:1115-1151) of the last fused frame at its fuse pose
     int raw_points(std::vector<dsm_point_t> &points)
     {
         points.clear();
-        if (!ready("raw_points")) return err_;
-        if (!fused_) return fail(DSM_E_STATE, "raw_points");
+        if (!ctx_.ready("raw_points")) return ctx_.err;
+        if (!fused_) return ctx_.done(DSM_E_STATE, "raw_points");
         const double p7[7] = {last_fuse_pose_.x, last_fuse_pose_.y, last_fuse_pose_.z, last_fuse_pose_.qx,
                               last_fuse_pose_.qy, last_fuse_pose_.qz, last_fuse_pose_.qw};
-        points.resize((size_t)width_ * height_);
-        int got = 0;
-        err_ = dsm_frame_raw_cloud(ctx_, 0, p7, points.data(), (int)points.size(), &got);
-        points.resize(err_ == DSM_OK ? (size_t)got : 0);
-        return report("raw_points");
+        return ctx_.done(detail::raw_cloud(ctx_, p7, width_ * height_, points), "raw_points");
     }
     // local_surfels, pool order
     int local_surfels(std::vector<dsm_surfel_t> &out)
     {
         out.clear();
-        if (!ready("local_surfels")) return err_;
-        int n = 0;
-        if ((err_ = dsm_pool_size(ctx_, &n)) != DSM_OK) return report("local_surfels");
-        out.resize((size_t)n + 1);
-        int got = 0;
-        err_ = dsm_pool_download(ctx_, out.data(), n, &got);
-        out.resize(err_ == DSM_OK ? (size_t)got : 0);
-        return report("local_surfels");
+        return ctx_.run("local_surfels", [&] { return detail::whole_pool(ctx_, out); });
     }
     // PoseElement::attached_surfels of one keyframe
     int attached_surfels(int pose_index, std::vector<dsm_surfel_t> &out)
     {
         out.clear();
-        if (!ready("attached_surfels")) return err_;
-        int n = 0;
-        if ((err_ = dsm_inactive_download(ctx_, pose_index, nullptr, 0, &n)) != DSM_OK) return report("attached_surfels");
-        out.resize((size_t)n + 1);
-        err_ = dsm_inactive_download(ctx_, pose_index, out.data(), n, &n);
-        out.resize(err_ == DSM_OK ? (size_t)n : 0);
-        return report("attached_surfels");
+        return ctx_.run("attached_surfels", [&] { return detail::attached(ctx_, pose_index, out); });
     }
 
     // ---- files ----
@@ -524,34 +487,24 @@ class SurfelMapNode
     // update_times >= 5; one hexagon each, ASCII PLY
     int save_mesh(const std::string &save_path_name)
     {
-        std::vector<dsm_surfel_t> all, part;
+        if (!ctx_.ready("save_mesh")) return ctx_.err;
+        std::vector<dsm_surfel_t> all;
         for (size_t i = 0; i < poses_.size(); i++)
         {
             if (local_.count((int)i)) continue; // a pose in the window has nothing stored
-            if (attached_surfels((int)i, part) != DSM_OK) return err_;
-            all.insert(all.end(), part.begin(), part.end());
+            const int rc = detail::attached(ctx_, (int)i, all);
+            if (rc != DSM_OK) return ctx_.done(rc, "save_mesh");
         }
-        if (!ready("save_mesh")) return err_;
-        int n = 0;
-        if ((err_ = dsm_pool_size(ctx_, &n)) != DSM_OK) return report("save_mesh");
-        const size_t base = all.size();
-        all.resize(base + (size_t)n + 1);
-        int got = 0;
-        err_ = dsm_pool_export_surfels(ctx_, 5, all.data() + base, n, &got);
-        if (err_ == DSM_OK) err_ = dsm_write_ply_mesh(save_path_name.c_str(), all.data(), base + (size_t)got);
-        return report("save_mesh");
+        return ctx_.done(detail::save_mesh(ctx_, save_path_name, std::move(all)), "save_mesh");
     }
     // save_cloud (:1153-1173): local points with update_times >= 5, then the inactive cloud; PCD v0.7 ASCII
     int save_cloud(const std::string &save_path_name)
     {
-        std::vector<dsm_point_t> points;
-        if (all_points(points) != DSM_OK) return err_;
-        err_ = dsm_write_pcd(save_path_name.c_str(), points.data(), points.size(), 0);
-        return report("save_cloud");
+        return ctx_.run("save_cloud", [&] { return detail::save_cloud<dsm_point_t>(ctx_, save_path_name, nullptr); });
     }
 
-    int last_error() const { return err_; }
-    dsm_ctx *context() { return ctx_; }
+    int last_error() const { return ctx_.err; }
+    dsm_ctx *context() { return ctx_.ctx; }
 
   private:
     struct PendingPose
@@ -604,20 +557,17 @@ class SurfelMapNode
         node_math::to_float(fuse, pose16);
         std::vector<int> remove, add;
         window_lists(q.reference_index, remove, add);
-        const std::vector<int32_t> rk(remove.begin(), remove.end()), ak(add.begin(), add.end());
-        const int32_t ro[2] = {0, (int32_t)rk.size()}, ao[2] = {0, (int32_t)ak.size()};
-        const int32_t ref = q.reference_index;
-        if (ctx_)
+        if (ctx_.ctx)
         {
             if (snapshot_)
             { // an unread snapshot is retired: its capacity report, if any, stays with the readers
-                const int rc = dsm_publish_wait(ctx_, nullptr, nullptr, nullptr, nullptr, nullptr);
+                const int rc = dsm_publish_wait(ctx_.ctx, nullptr, nullptr, nullptr, nullptr, nullptr);
                 snapshot_ = false;
-                if (rc != DSM_OK && rc != DSM_E_CAPACITY) return fail(rc, "fuse");
+                if (rc != DSM_OK && rc != DSM_E_CAPACITY) return ctx_.done(rc, "fuse");
             }
-            err_ = dsm_fuse_stream_window(ctx_, 1, &ref, image_buffer_.front().second.data(), depth_buffer_.front().second.data(), pose16,
-                                          rk.data(), ro, ak.data(), ao, nullptr);
-            if (err_ != DSM_OK) return report("fuse");
+            const int rc = detail::fuse_window(ctx_, q.reference_index, image_buffer_.front().second.data(),
+                                               depth_buffer_.front().second.data(), pose16, remove, add);
+            if (ctx_.done(rc, "fuse") != DSM_OK) return rc;
         }
         for (size_t i = 0; i < remove.size(); i++) local_.erase(remove[i]);
         local_.insert(add.begin(), add.end());
@@ -627,8 +577,8 @@ class SurfelMapNode
         pose_buffer_.pop_front();
         if (publishing_)
         { // after the bookkeeping: the frame is enqueued, so the host window follows the device whatever this returns
-            snapshot_ = (err_ = dsm_publish_enqueue(ctx_, 5)) == DSM_OK;
-            return report("fuse");
+            snapshot_ = ctx_.done(dsm_publish_enqueue(ctx_.ctx, 5), "fuse") == DSM_OK;
+            return ctx_.err;
         }
         return DSM_OK;
     }
@@ -655,63 +605,16 @@ class SurfelMapNode
             }
             p.cam_pose = p.loop_pose;
         }
-        if (!ctx_) return;
+        if (!ctx_.ctx) return;
         for (size_t i = 0; i < last_warp_.size(); i++)
         {
             const NodeWarp &x = last_warp_[i];
-            const int rc = x.pose < 0 ? dsm_pool_transform(ctx_, x.W) : dsm_inactive_transform(ctx_, x.pose, x.W);
-            if (rc != DSM_OK && err_ == DSM_OK)
-            {
-                err_ = rc;
-                report("warp_surfels");
-            }
+            const int rc = x.pose < 0 ? dsm_pool_transform(ctx_.ctx, x.W) : dsm_inactive_transform(ctx_.ctx, x.pose, x.W);
+            if (rc != DSM_OK && ctx_.err == DSM_OK) ctx_.done(rc, "warp_surfels");
         }
     }
 
-    int read_pool_cloud(std::vector<dsm_point_t> &points, int min_update_times, const char *what)
-    {
-        points.clear();
-        if (!ready(what)) return err_;
-        int n = 0;
-        if ((err_ = dsm_pool_size(ctx_, &n)) != DSM_OK) return report(what);
-        points.resize((size_t)n + 1);
-        int got = 0;
-        err_ = dsm_pool_export_cloud(ctx_, min_update_times, points.data(), n, &got);
-        points.resize(err_ == DSM_OK ? (size_t)got : 0);
-        return report(what);
-    }
-    int append_inactive(std::vector<dsm_point_t> &points, const char *what)
-    {
-        if (!ready(what)) return err_;
-        int n = 0;
-        if ((err_ = dsm_inactive_size(ctx_, &n, nullptr)) != DSM_OK) return report(what);
-        const size_t base = points.size();
-        points.resize(base + (size_t)n + 1);
-        int got = 0;
-        err_ = dsm_inactive_export_cloud(ctx_, points.data() + base, n, &got);
-        points.resize(err_ == DSM_OK ? base + (size_t)got : base);
-        return report(what);
-    }
-    bool ready(const char *what)
-    {
-        if (ctx_) return true;
-        fail(DSM_E_STATE, what);
-        return false;
-    }
-    int fail(int code, const char *what)
-    {
-        err_ = code;
-        return report(what);
-    }
-    int report(const char *what)
-    {
-        if (err_ != DSM_OK)
-            std::fprintf(stderr, "dsm::SurfelMapNode::%s failed: %s (%s)\n", what, dsm_strerror(err_), ctx_ ? dsm_last_error(ctx_) : "no context");
-        return err_;
-    }
-
-    dsm_ctx *ctx_;
-    int err_;
+    detail::Context ctx_;
     int width_, height_, drift_free_poses_;
     node_math::M4 transform_kitti_;
     std::vector<NodePose> poses_;

@@ -4,23 +4,9 @@
 //   in.bin : int32 ref_idx, float pose[16], int32 n_local, uint8 gray[H*W], float depth[H*W], surfel local[n_local]
 //   out.bin: int32 n_local, surfel local[n_local], int32 n_new, surfel new[n_new]
 // exit code 3 when no usable GPU (the library has no CPU fallback).
-#include <cstdio>
-#include <cstdlib>
-#include <vector>
-#include <opencv2/opencv.hpp> // oracle/shim
-#include <Eigen/Eigen>        // oracle/shim
+#include <Eigen/Eigen> // oracle/shim
 #include "dsm_fusion_functions.hpp"
-
-struct SurfelElement // reference elements.h:22-31
-{
-    float px, py, pz, nx, ny, nz, size, color, weight;
-    int update_times, last_update;
-};
-struct Pose4f
-{
-    float m[16];
-    float *data() { return m; }
-};
+#include "driver_io.hpp"
 
 int main(int argc, char **argv)
 {
@@ -30,26 +16,19 @@ int main(int argc, char **argv)
     fusion_functions.initialize(W, H, (float)atof(argv[3]), (float)atof(argv[4]), (float)atof(argv[5]), (float)atof(argv[6]),
                                 (float)atof(argv[7]), (float)atof(argv[8]));
     if (fusion_functions.last_error() != DSM_OK) return fusion_functions.last_error() == DSM_E_NODEVICE ? 3 : 4;
-    FILE *f = fopen(argv[9], "rb");
-    if (!f) return 5;
-    int ref = 0, n_local = 0;
-    Pose4f pose;
-    if (fread(&ref, 4, 1, f) != 1 || fread(pose.m, 4, 16, f) != 16 || fread(&n_local, 4, 1, f) != 1) return 5;
-    std::vector<unsigned char> gray((size_t)W * H);
-    std::vector<float> depth((size_t)W * H);
-    std::vector<SurfelElement> local_surfels((size_t)n_local), new_surfels;
-    if (fread(gray.data(), 1, gray.size(), f) != gray.size() || fread(depth.data(), 4, depth.size(), f) != depth.size()) return 5;
-    if (n_local && fread(local_surfels.data(), sizeof(SurfelElement), (size_t)n_local, f) != (size_t)n_local) return 5;
-    fclose(f);
-    cv::Mat image(H, W, CV_8UC1, gray.data(), (size_t)W), dmap(H, W, CV_32FC1, depth.data(), (size_t)W * 4);
-    fusion_functions.fuse_initialize_map(ref, image, dmap, pose, local_surfels, new_surfels);
+    in_f = fopen(argv[9], "rb");
+    if (!in_f) return 5;
+    FrameRecord fr(W, H);
+    int n_local = 0;
+    std::vector<SurfelElement> local_surfels, new_surfels;
+    if (!fr.get_head() || !get(n_local) || !fr.get_images() || !get_n(local_surfels, n_local)) return 5;
+    fclose(in_f);
+    cv::Mat image = fr.image(), dmap = fr.depth_map();
+    fusion_functions.fuse_initialize_map(fr.ref, image, dmap, fr.pose, local_surfels, new_surfels);
     if (fusion_functions.last_error() != DSM_OK) return 6;
-    f = fopen(argv[10], "wb");
-    int n_new = (int)new_surfels.size();
-    fwrite(&n_local, 4, 1, f);
-    fwrite(local_surfels.data(), sizeof(SurfelElement), (size_t)n_local, f);
-    fwrite(&n_new, 4, 1, f);
-    fwrite(new_surfels.data(), sizeof(SurfelElement), (size_t)n_new, f);
-    fclose(f);
+    out_f = fopen(argv[10], "wb");
+    put_list(local_surfels);
+    put_list(new_surfels);
+    fclose(out_f);
     return 0;
 }

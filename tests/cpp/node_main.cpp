@@ -17,30 +17,10 @@
 //     map:   int32 rc, then local surfels, attached surfels of every pose, active, inactive, all and neighbour points,
 //            each as int32 n + records
 // exit code 3 when no usable GPU (the library has no CPU fallback).
-#include <cstdio>
-#include <cstdlib>
 #include <string>
-#include <vector>
 #include "dsm_surfel_node.hpp"
+#include "driver_io.hpp"
 
-static FILE *in_f, *out_f;
-template <class T>
-static bool get(T &v) { return fread(&v, sizeof(T), 1, in_f) == 1; }
-template <class T>
-static bool get_n(std::vector<T> &v, int n)
-{
-    if (n < 0) return false;
-    v.resize((size_t)n);
-    return n == 0 || fread(v.data(), sizeof(T), (size_t)n, in_f) == (size_t)n;
-}
-template <class T>
-static void put(const T &v) { fwrite(&v, sizeof(T), 1, out_f); }
-template <class T>
-static void put_list(const std::vector<T> &v)
-{
-    put((int)v.size());
-    if (!v.empty()) fwrite(v.data(), sizeof(T), v.size(), out_f);
-}
 static void put_pose(const dsm::Pose &p)
 {
     const double d[7] = {p.x, p.y, p.z, p.qx, p.qy, p.qz, p.qw};
@@ -58,33 +38,14 @@ int main(int argc, char **argv)
     in_f = fopen(argv[14], "rb");
     out_f = fopen(argv[15], "wb");
     if (!in_f || !out_f) return 5;
-    std::vector<uint8_t> gray;
-    std::vector<float> depth;
-    std::vector<double> path;
-    std::vector<int> pairs;
+    NodeMessages msg;
     int rc = DSM_OK, type = 0;
     while (get(type))
     {
         int r = DSM_OK;
-        double stamp = 0;
-        if (type == 0)
+        if (type <= 2)
         {
-            int kf = 0, ref = 0, n_path = 0, n_loops = 0;
-            double pose[7];
-            if (!get(stamp) || !get(kf) || !get(ref) || fread(pose, 8, 7, in_f) != 7 || !get(n_path) || !get_n(path, 7 * n_path) ||
-                !get(n_loops) || !get_n(pairs, 2 * n_loops))
-                return 5;
-            r = node.orb_results_input(stamp, pairs.data(), n_loops, path.data(), n_path, pose, kf != 0, ref);
-        }
-        else if (type == 1)
-        {
-            if (!get(stamp) || !get_n(gray, W * H)) return 5;
-            r = node.image_input(stamp, gray.data(), (size_t)W);
-        }
-        else if (type == 2)
-        {
-            if (!get(stamp) || !get_n(depth, W * H)) return 5;
-            r = node.depth_input(stamp, depth.data(), (size_t)W * 4);
+            if (!msg.feed(node, type, W, H, r)) return 5;
         }
         else if (type == 3)
         {

@@ -6,29 +6,8 @@
 //            inactive_points() read right after (each cloud as int32 n + n points);
 //            at the end, for either value of publish: local_surfels (int32 n + records) and inactive_points.
 // exit code 3 when no usable GPU (the library has no CPU fallback).
-#include <cstdio>
-#include <cstdlib>
-#include <vector>
 #include "dsm_surfel_node.hpp"
-
-static FILE *in_f, *out_f;
-template <class T>
-static bool get(T &v) { return fread(&v, sizeof(T), 1, in_f) == 1; }
-template <class T>
-static bool get_n(std::vector<T> &v, int n)
-{
-    if (n < 0) return false;
-    v.resize((size_t)n);
-    return n == 0 || fread(v.data(), sizeof(T), (size_t)n, in_f) == (size_t)n;
-}
-template <class T>
-static void put(const T &v) { fwrite(&v, sizeof(T), 1, out_f); }
-template <class T>
-static void put_n(const T *p, int n)
-{
-    put(n);
-    if (n > 0) fwrite(p, sizeof(T), (size_t)n, out_f);
-}
+#include "driver_io.hpp"
 
 int main(int argc, char **argv)
 {
@@ -41,54 +20,31 @@ int main(int argc, char **argv)
     in_f = fopen(argv[14], "rb");
     out_f = fopen(argv[15], "wb");
     if (!in_f || !out_f) return 5;
-    std::vector<uint8_t> gray;
-    std::vector<float> depth;
-    std::vector<double> path;
-    std::vector<int> pairs;
+    NodeMessages msg;
     std::vector<dsm_point_t> act, inact;
-    int type = 0;
+    int type = 0, r = DSM_OK;
     while (get(type))
     {
-        double stamp = 0;
-        if (type == 0)
-        {
-            int kf = 0, ref = 0, n_path = 0, n_loops = 0;
-            double pose[7];
-            if (!get(stamp) || !get(kf) || !get(ref) || fread(pose, 8, 7, in_f) != 7 || !get(n_path) || !get_n(path, 7 * n_path) ||
-                !get(n_loops) || !get_n(pairs, 2 * n_loops))
-                return 5;
-            if (node.orb_results_input(stamp, pairs.data(), n_loops, path.data(), n_path, pose, kf != 0, ref) != DSM_OK) return 6;
-        }
-        else if (type == 1)
-        {
-            if (!get(stamp) || !get_n(gray, W * H)) return 5;
-            if (node.image_input(stamp, gray.data(), (size_t)W) != DSM_OK) return 6;
-        }
-        else if (type == 2)
-        {
-            if (!get(stamp) || !get_n(depth, W * H)) return 5;
-            if (node.depth_input(stamp, depth.data(), (size_t)W * 4) != DSM_OK) return 6;
-            if (!publish) continue;
-            const dsm_point_t *a = nullptr, *b = nullptr;
-            int na = 0, nb = 0, from = 0;
-            const int rc = node.published_clouds(a, na, b, nb, from);
-            put(rc);
-            put(from);
-            put_n(a, rc == DSM_OK ? na : 0);
-            put_n(b, rc == DSM_OK ? nb : 0);
-            int rr = node.active_points(act);
-            if (rr == DSM_OK) rr = node.inactive_points(inact);
-            put(rr);
-            put_n(act.data(), (int)act.size());
-            put_n(inact.data(), (int)inact.size());
-        }
-        else
-            return 5;
+        if (!msg.feed(node, type, W, H, r)) return 5;
+        if (r != DSM_OK) return 6;
+        if (type != 2 || !publish) continue;
+        const dsm_point_t *a = nullptr, *b = nullptr;
+        int na = 0, nb = 0, from = 0;
+        const int rc = node.published_clouds(a, na, b, nb, from);
+        put(rc);
+        put(from);
+        put_n(a, rc == DSM_OK ? na : 0);
+        put_n(b, rc == DSM_OK ? nb : 0);
+        int rr = node.active_points(act);
+        if (rr == DSM_OK) rr = node.inactive_points(inact);
+        put(rr);
+        put_list(act);
+        put_list(inact);
     }
     std::vector<dsm_surfel_t> local;
     if (node.local_surfels(local) != DSM_OK || node.inactive_points(inact) != DSM_OK) return 6;
-    put_n(local.data(), (int)local.size());
-    put_n(inact.data(), (int)inact.size());
+    put_list(local);
+    put_list(inact);
     fclose(in_f);
     fclose(out_f);
     return 0;

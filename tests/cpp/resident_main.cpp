@@ -7,34 +7,8 @@
 //   out.bin: int32 n_pool_after_stream, surfel pool[], int32 n_retired, surfel retired[], int32 n_final, surfel final[],
 //            int32 n_points, point points[]
 // exit code 3 when no usable GPU (the library has no CPU fallback).
-#include <cstdio>
-#include <cstdlib>
-#include <vector>
-#include <opencv2/opencv.hpp> // oracle/shim
 #include "dsm_surfel_map.hpp"
-
-struct SurfelElement // reference elements.h:22-31
-{
-    float px, py, pz, nx, ny, nz, size, color, weight;
-    int update_times, last_update;
-};
-struct PointXYZI // the four named fields of pcl::PointXYZI
-{
-    float x, y, z, intensity;
-};
-struct Pose4f
-{
-    float m[16];
-    float *data() { return m; }
-};
-
-template <class T>
-static void put(FILE *f, const std::vector<T> &v)
-{
-    const int n = (int)v.size();
-    fwrite(&n, 4, 1, f);
-    if (n) fwrite(v.data(), sizeof(T), (size_t)n, f);
-}
+#include "driver_io.hpp"
 
 int main(int argc, char **argv)
 {
@@ -45,25 +19,21 @@ int main(int argc, char **argv)
     if (map.initialize(W, H, (float)atof(argv[3]), (float)atof(argv[4]), (float)atof(argv[5]), (float)atof(argv[6]), (float)atof(argv[7]),
                        (float)atof(argv[8])) != DSM_OK)
         return map.last_error() == DSM_E_NODEVICE ? 3 : 4;
-    FILE *f = fopen(argv[9], "rb");
-    if (!f) return 5;
+    in_f = fopen(argv[9], "rb");
+    if (!in_f) return 5;
     int T = 0;
-    if (fread(&T, 4, 1, f) != 1) return 5;
-    std::vector<unsigned char> gray((size_t)W * H);
-    std::vector<float> depth((size_t)W * H);
+    if (!get(T)) return 5;
+    FrameRecord fr(W, H);
     for (int t = 0; t < T; t++)
     {
-        int ref = 0;
-        Pose4f pose;
-        if (fread(&ref, 4, 1, f) != 1 || fread(pose.m, 4, 16, f) != 16) return 5;
-        if (fread(gray.data(), 1, gray.size(), f) != gray.size() || fread(depth.data(), 4, depth.size(), f) != depth.size()) return 5;
-        cv::Mat image(H, W, CV_8UC1, gray.data(), (size_t)W), dmap(H, W, CV_32FC1, depth.data(), (size_t)W * 4);
-        if (map.fuse_map(image, dmap, pose, ref) != DSM_OK) return 6;
+        if (!fr.get_head() || !fr.get_images()) return 5;
+        cv::Mat image = fr.image(), dmap = fr.depth_map();
+        if (map.fuse_map(image, dmap, fr.pose, fr.ref) != DSM_OK) return 6;
     }
     Pose4f warp;
     int retire_kf = 0;
-    if (fread(warp.m, 4, 16, f) != 16 || fread(&retire_kf, 4, 1, f) != 1) return 5;
-    fclose(f);
+    if (!get(warp) || !get(retire_kf)) return 5;
+    fclose(in_f);
     std::vector<SurfelElement> pool, retired, final_pool;
     std::vector<PointXYZI> points, no_inactive;
     if (map.download(pool) != DSM_OK) return 7;
@@ -74,12 +44,12 @@ int main(int argc, char **argv)
     if (map.save_cloud(argv[11], no_inactive) != DSM_OK) return 12;
     if (map.save_mesh(argv[12], retired) != DSM_OK) return 13;
     if (map.download(final_pool) != DSM_OK) return 14;
-    f = fopen(argv[10], "wb");
-    if (!f) return 5;
-    put(f, pool);
-    put(f, retired);
-    put(f, final_pool);
-    put(f, points);
-    fclose(f);
+    out_f = fopen(argv[10], "wb");
+    if (!out_f) return 5;
+    put_list(pool);
+    put_list(retired);
+    put_list(final_pool);
+    put_list(points);
+    fclose(out_f);
     return 0;
 }

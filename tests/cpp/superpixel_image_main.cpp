@@ -7,23 +7,9 @@
 //   out.bin: T x uint8 resident[H][W*3 + 5] (pitched, the 5 padding bytes of each row as the caller filled them),
 //            uint8 adapter[H][W*3]
 // exit code 3 when no usable GPU (the library has no CPU fallback).
-#include <cstdio>
-#include <cstdlib>
-#include <vector>
-#include <opencv2/opencv.hpp> // oracle/shim
 #include "dsm_fusion_functions.hpp"
 #include "dsm_surfel_map.hpp"
-
-struct Pose4f
-{
-    float m[16];
-    float *data() { return m; }
-};
-struct Surfel // SurfelElement (elements.h:22-31)
-{
-    float px, py, pz, nx, ny, nz, size, color, weight;
-    int update_times, last_update;
-};
+#include "driver_io.hpp"
 
 int main(int argc, char **argv)
 {
@@ -34,41 +20,37 @@ int main(int argc, char **argv)
     dsm::ResidentSurfelPool map;
     map.set_device(0, 200000);
     if (map.initialize(W, H, fx, fy, cx, cy, fa, ne) != DSM_OK) return map.last_error() == DSM_E_NODEVICE ? 3 : 4;
-    FILE *f = fopen(argv[9], "rb");
-    if (!f) return 5;
+    in_f = fopen(argv[9], "rb");
+    if (!in_f) return 5;
     int T = 0;
-    if (fread(&T, 4, 1, f) != 1 || T < 1) return 5;
-    std::vector<unsigned char> gray((size_t)W * H);
-    std::vector<float> depth((size_t)W * H);
+    if (!get(T) || T < 1) return 5;
     const size_t pitch = (size_t)W * 3 + 5;
-    FILE *o = fopen(argv[10], "wb");
-    if (!o) return 5;
+    out_f = fopen(argv[10], "wb");
+    if (!out_f) return 5;
     std::vector<unsigned char> shown(pitch * H);
-    Pose4f pose;
-    int ref = 0;
+    FrameRecord fr(W, H);
     for (int t = 0; t < T; t++)
     {
-        if (fread(&ref, 4, 1, f) != 1 || fread(pose.m, 4, 16, f) != 16) return 5;
-        if (fread(gray.data(), 1, gray.size(), f) != gray.size() || fread(depth.data(), 4, depth.size(), f) != depth.size()) return 5;
-        cv::Mat image(H, W, CV_8UC1, gray.data(), (size_t)W), dmap(H, W, CV_32FC1, depth.data(), (size_t)W * 4);
-        if (map.fuse_map(image, dmap, pose, ref) != DSM_OK) return 6;
+        if (!fr.get_head() || !fr.get_images()) return 5;
+        cv::Mat image = fr.image(), dmap = fr.depth_map();
+        if (map.fuse_map(image, dmap, fr.pose, fr.ref) != DSM_OK) return 6;
         for (size_t i = 0; i < shown.size(); i++) shown[i] = (unsigned char)(0xA5 ^ (i * 7));
         cv::Mat sp(H, W, CV_8UC3, shown.data(), pitch);
         if (map.superpixel_image(sp) != DSM_OK) return 7;
-        fwrite(shown.data(), 1, shown.size(), o);
+        fwrite(shown.data(), 1, shown.size(), out_f);
     }
-    fclose(f);
+    fclose(in_f);
     dsm::FusionFunctions ff;
     ff.set_device(0, 1 << 16);
     ff.initialize(W, H, fx, fy, cx, cy, fa, ne);
     if (ff.last_error() != DSM_OK) return 8;
-    cv::Mat image(H, W, CV_8UC1, gray.data(), (size_t)W), dmap(H, W, CV_32FC1, depth.data(), (size_t)W * 4);
-    std::vector<Surfel> local, fresh;
-    ff.fuse_initialize_map(ref, image, dmap, pose, local, fresh);
+    cv::Mat image = fr.image(), dmap = fr.depth_map();
+    std::vector<SurfelElement> local, fresh;
+    ff.fuse_initialize_map(fr.ref, image, dmap, fr.pose, local, fresh);
     if (ff.last_error() != DSM_OK) return 8;
     cv::Mat out(H, W, CV_8UC3);
     if (ff.superpixel_image(out) != DSM_OK) return 9;
-    fwrite(out.data, 1, out.step * (size_t)H, o);
-    fclose(o);
+    fwrite(out.data, 1, out.step * (size_t)H, out_f);
+    fclose(out_f);
     return 0;
 }

@@ -7,41 +7,8 @@
 //   out.bin: int32 n_pool, surfel pool[], int32 n_stored, surfel store[] (every pose's attached surfels, store order),
 //            int32 n_points, point inactive_points[]
 // exit code 3 when no usable GPU (the library has no CPU fallback).
-#include <cstdio>
-#include <cstdlib>
-#include <vector>
-#include <opencv2/opencv.hpp> // oracle/shim
 #include "dsm_surfel_map.hpp"
-
-struct SurfelElement // reference elements.h:22-31
-{
-    float px, py, pz, nx, ny, nz, size, color, weight;
-    int update_times, last_update;
-};
-struct PointXYZI // the four named fields of pcl::PointXYZI
-{
-    float x, y, z, intensity;
-};
-struct Pose4f
-{
-    float m[16];
-    float *data() { return m; }
-};
-
-template <class T>
-static void put(FILE *f, const std::vector<T> &v)
-{
-    const int n = (int)v.size();
-    fwrite(&n, 4, 1, f);
-    if (n) fwrite(v.data(), sizeof(T), (size_t)n, f);
-}
-static bool get_list(FILE *f, std::vector<int> &v)
-{
-    int n = 0;
-    if (fread(&n, 4, 1, f) != 1 || n < 0) return false;
-    v.resize((size_t)n);
-    return n == 0 || fread(v.data(), 4, (size_t)n, f) == (size_t)n;
-}
+#include "driver_io.hpp"
 
 int main(int argc, char **argv)
 {
@@ -53,36 +20,29 @@ int main(int argc, char **argv)
                        (float)atof(argv[8])) != DSM_OK)
         return map.last_error() == DSM_E_NODEVICE ? 3 : 4;
     if (map.reserve_inactive(400000) != DSM_OK) return 4;
-    FILE *f = fopen(argv[9], "rb");
-    if (!f) return 5;
-    int T = 0;
-    if (fread(&T, 4, 1, f) != 1) return 5;
-    std::vector<unsigned char> gray((size_t)W * H);
-    std::vector<float> depth((size_t)W * H);
+    in_f = fopen(argv[9], "rb");
+    if (!in_f) return 5;
+    int T = 0, n = 0;
+    if (!get(T)) return 5;
+    FrameRecord fr(W, H);
     std::vector<int> remove, add;
     for (int t = 0; t < T; t++)
     {
-        int ref = 0;
-        Pose4f pose;
-        if (fread(&ref, 4, 1, f) != 1 || fread(pose.m, 4, 16, f) != 16 || !get_list(f, remove) || !get_list(f, add)) return 5;
-        if (fread(gray.data(), 1, gray.size(), f) != gray.size() || fread(depth.data(), 4, depth.size(), f) != depth.size()) return 5;
-        cv::Mat image(H, W, CV_8UC1, gray.data(), (size_t)W), dmap(H, W, CV_32FC1, depth.data(), (size_t)W * 4);
-        if (map.fuse_map(image, dmap, pose, ref, remove, add) != DSM_OK) return 6;
+        if (!fr.get_head() || !get(n) || !get_n(remove, n) || !get(n) || !get_n(add, n) || !fr.get_images()) return 5;
+        cv::Mat image = fr.image(), dmap = fr.depth_map();
+        if (map.fuse_map(image, dmap, fr.pose, fr.ref, remove, add) != DSM_OK) return 6;
     }
-    fclose(f);
+    fclose(in_f);
     std::vector<SurfelElement> pool, store;
     std::vector<PointXYZI> points;
     if (map.download(pool) != DSM_OK) return 7;
-    int n = 0, got = 0;
-    if (dsm_inactive_size(map.context(), &n, nullptr) != DSM_OK) return 8;
-    store.resize((size_t)n);
-    if (dsm_inactive_download(map.context(), -1, reinterpret_cast<dsm_surfel_t *>(store.data()), n, &got) != DSM_OK) return 8;
+    if (map.attached_surfels(-1, store) != DSM_OK) return 8;
     if (map.inactive_points(points) != DSM_OK) return 9;
-    f = fopen(argv[10], "wb");
-    if (!f) return 5;
-    put(f, pool);
-    put(f, store);
-    put(f, points);
-    fclose(f);
+    out_f = fopen(argv[10], "wb");
+    if (!out_f) return 5;
+    put_list(pool);
+    put_list(store);
+    put_list(points);
+    fclose(out_f);
     return 0;
 }
