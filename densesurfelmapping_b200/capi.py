@@ -32,6 +32,7 @@ EXPORTS = [
     "dsm_inactive_download", "dsm_inactive_size", "dsm_frame_raw_cloud", "dsm_inactive_export_poses",
     "dsm_frame_superpixel_image", "dsm_fuse_stream_window",
     "dsm_publish_enable", "dsm_publish_enqueue", "dsm_publish_wait", "dsm_debug_publish_chunks",
+    "dsm_inactive_segments", "dsm_inactive_load", "dsm_map_save", "dsm_map_load", "dsm_map_peek",
     "dsm_comm_unique_id", "dsm_comm_init", "dsm_comm_destroy", "dsm_gather_deltas", "dsm_gather_wait", "dsm_gathered_device",
     "dsm_gathered_rank_bytes", "dsm_gathered_download", "dsm_set_constants", "dsm_set_concurrency",
 ]
@@ -111,6 +112,11 @@ def load_library():
     L.dsm_frame_raw_cloud.argtypes = [vp, ci, vp, vp, ci, ctypes.POINTER(ci)]
     L.dsm_inactive_download.argtypes = [vp, ci, vp, ci, ctypes.POINTER(ci)]
     L.dsm_inactive_size.argtypes = [vp, ctypes.POINTER(ci), ctypes.POINTER(ci)]
+    L.dsm_inactive_segments.argtypes = [vp, vp, ci, ctypes.POINTER(ci)]
+    L.dsm_inactive_load.argtypes = [vp, vp, ci, vp, ci]
+    L.dsm_map_save.argtypes = [vp, ctypes.c_char_p, vp, cs]
+    L.dsm_map_load.argtypes = [vp, ctypes.c_char_p, vp, cs, ctypes.POINTER(cs)]
+    L.dsm_map_peek.argtypes = [ctypes.c_char_p, vp, cs, ctypes.POINTER(cs), vp, ci, ctypes.POINTER(ci)]
     L.dsm_pool_retire.argtypes = [vp, ci, vp, ci, ctypes.POINTER(ci)]
     L.dsm_pool_append.argtypes = [vp, vp, ci]
     L.dsm_pool_size.argtypes = [vp, ctypes.POINTER(ci)]
@@ -415,6 +421,34 @@ class Context:
         cap = self.inactive_size()[0] if cap is None else cap
         return self._read(self.lib.dsm_inactive_export_poses, POINT_DTYPE, cap, _ptr(kf) if len(kf) else None, len(kf))
 
+    # ---- checkpoint and resume (DESIGN.md §8.4) ----
+    def inactive_segments(self):
+        """The store's segment table in store order: int32 [n, 3] of (keyframe, offset, count)."""
+        return self._read(self.lib.dsm_inactive_segments, np.dtype((np.int32, 3)), self.inactive_size()[1])
+
+    def inactive_load(self, surfels, segments):
+        """Replaces the store's contents (SURFEL_DTYPE, store order) and its table ([n, 3] of (keyframe, offset, count))."""
+        surfels = np.ascontiguousarray(surfels, dtype=SURFEL_DTYPE)
+        seg = np.ascontiguousarray(segments, dtype=np.int32).reshape(-1, 3)
+        self._ck(self.lib.dsm_inactive_load(self.h, _ptr(surfels) if len(surfels) else None, len(surfels),
+                                            _ptr(seg) if len(seg) else None, len(seg)))
+
+    def map_save(self, path, extra=b""):
+        """The pool, the store, its table and the caller's `extra` bytes to one checkpoint file."""
+        buf = ctypes.create_string_buffer(bytes(extra), max(len(extra), 1))
+        self._ck(self.lib.dsm_map_save(self.h, os.fsencode(path), buf if len(extra) else None, len(extra)))
+
+    def map_load(self, path) -> bytes:
+        """Replaces the map by a checkpoint's and returns its extra bytes."""
+        size = ctypes.c_size_t(0)
+        rc = self.lib.dsm_map_load(self.h, os.fsencode(path), None, 0, ctypes.byref(size))
+        if rc == -6 and size.value > 0:  # the size-then-read of the extra section: nothing was loaded yet
+            buf = ctypes.create_string_buffer(size.value)
+            self._ck(self.lib.dsm_map_load(self.h, os.fsencode(path), buf, size.value, ctypes.byref(size)))
+            return buf.raw[:size.value]
+        self._ck(rc)
+        return b""
+
     # ---- publishing from inside the stream ----
     def publish_enable(self):
         self._ck(self.lib.dsm_publish_enable(self.h))
@@ -548,6 +582,17 @@ def write_ply_mesh(path, surfels):
     """SurfelMap::save_mesh (surfel_map.cpp:1229-1280): one hexagon per surfel, ASCII PLY."""
     surfels = np.ascontiguousarray(surfels, dtype=SURFEL_DTYPE)
     _ck_io(load_library().dsm_write_ply_mesh(os.fsencode(path), _ptr(surfels) if len(surfels) else None, len(surfels)), path)
+
+
+def map_peek(path):
+    """(extra bytes, segment table [n, 3]) of a checkpoint file, checked without a context."""
+    L = load_library()
+    ne, ns = ctypes.c_size_t(0), ctypes.c_int(0)
+    _ck_io(L.dsm_map_peek(os.fsencode(path), None, 0, ctypes.byref(ne), None, 0, ctypes.byref(ns)), path)
+    extra = ctypes.create_string_buffer(max(ne.value, 1))
+    seg = np.zeros((max(ns.value, 1), 3), np.int32)
+    _ck_io(L.dsm_map_peek(os.fsencode(path), extra, ne.value, None, _ptr(seg), ns.value, None), path)
+    return extra.raw[:ne.value], seg[:ns.value].copy()
 
 
 def mesh_vertices(surfels):

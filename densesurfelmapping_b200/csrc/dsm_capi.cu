@@ -3,6 +3,7 @@
 // fusion_functions.cpp:30-83, :960-975) and the copies either side of it.
 // No CPU implementation of any phase lives here: if CUDA is unavailable every call fails.
 #include "dsm_ctx.hpp"
+#include "dsm_map_state.h"
 #include <cmath>
 #include <cstdio>
 #include <cstring>
@@ -1253,6 +1254,82 @@ extern "C" int dsm_inactive_export_poses(dsm_ctx *ctx, const int32_t *keyframes,
         for (const auto &sg : ctx->inact->segs)
             if (sg.kf == keyframes[k]) ranges.push_back(sg);
     return inactive_export_ranges(ctx, ranges, out, cap, n_out);
+}
+
+// the segment table in store order, (keyframe, offset, count) per segment, from the mirror res_sync refreshes
+extern "C" int dsm_inactive_segments(dsm_ctx *ctx, int32_t *kf_ofs_cnt, int cap, int *n_out)
+{
+    if (!ctx || !n_out || cap < 0 || (cap > 0 && !kf_ofs_cnt)) return DSM_E_INVALID;
+    const int rc = res_enter(ctx, NEED_STORE);
+    if (rc != DSM_OK) return rc;
+    const std::vector<InactStore::Seg> &segs = ctx->inact->segs;
+    for (int i = 0; i < (int)segs.size() && i < cap; i++)
+    {
+        kf_ofs_cnt[3 * i] = segs[i].kf;
+        kf_ofs_cnt[3 * i + 1] = segs[i].ofs;
+        kf_ofs_cnt[3 * i + 2] = segs[i].cnt;
+    }
+    *n_out = (int)segs.size();
+    return DSM_OK;
+}
+
+int dsm_inactive_load_check(const dsm_ctx *ctx, const dsm_surfel_t *surfels, int n, const int32_t *kf_ofs_cnt, int n_segments)
+{
+    if (!ctx || n < 0 || n_segments < 0 || (n > 0 && !surfels) || (n_segments > 0 && !kf_ofs_cnt)) return DSM_E_INVALID;
+    if (!ctx->inact || ctx->pub_in_flight) return DSM_E_STATE;
+    if (n > ctx->inact->cap) return DSM_E_CAPACITY;
+    // the table: contiguous from 0, every segment at least one surfel, n in all, no negative keyframe
+    int64_t ofs = 0;
+    for (int i = 0; i < n_segments; i++)
+    {
+        const int32_t *g = kf_ofs_cnt + 3 * i;
+        if (g[0] < 0 || g[1] != ofs || g[2] < 1) return DSM_E_INVALID;
+        ofs += g[2];
+        if (ofs > n) return DSM_E_INVALID;
+    }
+    if (ofs != n) return DSM_E_INVALID;
+    // every stored surfel is live and was last updated by its segment's keyframe: retire selects by last_update and
+    // the transforms leave it alone, so every store the library builds satisfies this
+    for (int i = 0; i < n_segments; i++)
+    {
+        const int32_t *g = kf_ofs_cnt + 3 * i;
+        for (int j = g[1]; j < g[1] + g[2]; j++)
+            if (surfels[j].update_times == 0 || surfels[j].last_update != g[0]) return DSM_E_INVALID;
+    }
+    return DSM_OK;
+}
+
+// Replaces the store's contents and table.  Everything is checked before the device is touched.
+extern "C" int dsm_inactive_load(dsm_ctx *ctx, const dsm_surfel_t *surfels, int n, const int32_t *kf_ofs_cnt, int n_segments)
+{
+    int rc = dsm_inactive_load_check(ctx, surfels, n, kf_ofs_cnt, n_segments);
+    if (rc != DSM_OK) return rc;
+    rc = res_enter(ctx, NEED_STORE);
+    if (rc != DSM_OK) return rc;
+    InactStore &s = *ctx->inact;
+    std::vector<int4> table((size_t)n_segments);
+    for (int i = 0; i < n_segments; i++) table[i] = make_int4(kf_ofs_cnt[3 * i], kf_ofs_cnt[3 * i + 1], kf_ofs_cnt[3 * i + 2], 0);
+    const int32_t hdr[4] = {n, n_segments, 0, 0};
+    CK(cudaStreamSynchronize(ctx->stream)); // nothing enqueued earlier may still read or write the store
+    if (n > 0) CK(cudaMemcpyAsync(s.surfels, surfels, (size_t)n * sizeof(dsm_surfel_t), cudaMemcpyHostToDevice, ctx->stream));
+    if (n_segments > 0) CK(cudaMemcpyAsync(s.seg, table.data(), table.size() * sizeof(int4), cudaMemcpyHostToDevice, ctx->stream));
+    CK(cudaMemcpyAsync(ctx->win_hdr, hdr, sizeof(hdr), cudaMemcpyHostToDevice, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream)); // the sources are the caller's and the stack's
+    s.segs.clear();
+    for (int i = 0; i < n_segments; i++) s.segs.push_back(InactStore::Seg{table[i].x, table[i].y, table[i].z});
+    s.size = s.upper = n;
+    if (ctx->pub_on) CK(publish_state_reset(ctx));
+    return DSM_OK;
+}
+
+int dsm_map_info(const dsm_ctx *ctx, DsmMapInfo *info)
+{
+    if (!ctx || !info) return DSM_E_INVALID;
+    info->params = ctx->p;
+    info->constants = dsm_constants{ctx->d.huber, ctx->d.baseline, ctx->d.disparity_error, ctx->d.min_tolerate_diff};
+    info->store_cap = ctx->inact ? ctx->inact->cap : 0;
+    info->publish_in_flight = ctx->pub_in_flight;
+    return DSM_OK;
 }
 
 // ---- publishing from inside the stream (include/dsm.h) ----

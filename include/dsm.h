@@ -49,7 +49,7 @@ extern "C" {
 #define DSM_E_CAPACITY (-6)  /* more surfels than the context was created for */
 #define DSM_E_STATE (-7)     /* call sequence error (e.g. download before run) */
 #define DSM_E_NCCL (-8)      /* NCCL unavailable or a collective failed */
-#define DSM_E_IO (-9)        /* a file could not be opened or written (dsm_write_*) */
+#define DSM_E_IO (-9)        /* a file could not be opened, read or written (dsm_write_*, dsm_map_*) */
 
 /* ---- element types: byte-identical to the reference ---- */
 
@@ -332,6 +332,48 @@ int dsm_inactive_export_cloud(dsm_ctx *ctx, dsm_point_t *out, int cap, int *n_ou
 int dsm_inactive_export_poses(dsm_ctx *ctx, const int32_t *keyframes, int n_keyframes, dsm_point_t *out, int cap, int *n_out);
 int dsm_inactive_download(dsm_ctx *ctx, int keyframe_index, dsm_surfel_t *out, int cap, int *n_out);
 int dsm_inactive_size(dsm_ctx *ctx, int *n_surfels, int *n_segments);
+
+/* ---- checkpoint and resume of the GPU-resident map (DESIGN.md §8.4) ----
+ * Between frames the pool, the inactive store and its segment table are the whole device state of a map, so a drive
+ * resumed from a checkpoint is byte-identical to the same drive run without interruption.
+ *   dsm_inactive_segments  the segment table in store order: kf_ofs_cnt[i] = (keyframe, offset, count) of segment i.
+ *                          min(cap, n) entries written, *n_out = n.  Synchronises (reports a rejected frame as every
+ *                          synchronising reader does).  DSM_E_STATE without dsm_inactive_reserve.
+ *   dsm_inactive_load      replaces the store's contents and table.  Checked on the host, in this order, before the device
+ *                          is touched, so a failure leaves the store as it was: DSM_E_STATE without a reservation or while
+ *                          a publish snapshot is in flight; DSM_E_CAPACITY for n above the reservation; DSM_E_INVALID for a
+ *                          malformed table (offsets not contiguous from 0, a count below 1, counts not summing to n, a
+ *                          negative keyframe) and for a surfel with update_times == 0 or a last_update other than its
+ *                          segment's keyframe (true of every store the library builds).  A keyframe may own several
+ *                          segments.  With publishing enabled the next snapshot reports inactive_changed_from = 0 and
+ *                          forwards every chunk, as after dsm_inactive_reserve.  Synchronises.
+ *   dsm_map_save           writes the pool (slot order), the store (store order), the table and the caller's `extra` bytes
+ *                          (opaque to the library) to one versioned little-endian file with a 64-bit checksum, together
+ *                          with the context's geometry and constants.  Needs a resident pool (DSM_E_STATE); a store is
+ *                          optional.  A synchronising reader: a pending rejected frame is reported as DSM_E_CAPACITY and
+ *                          cleared, and no file is written; the next save writes the map of the last applied frame.  The
+ *                          file is written under a temporary name in the same directory, flushed to the disk and renamed:
+ *                          DSM_E_IO on any I/O failure, with nothing left under `path`.
+ *   dsm_map_load           reads and checks the whole file before the device is touched, so every failure leaves the map
+ *                          as it was: DSM_E_IO if it cannot be read, is truncated or fails its checksum; DSM_E_INVALID for a
+ *                          wrong magic or format version, and for geometry or constants other than the context's (set the
+ *                          constants before loading; max_batch and the capacities may differ); DSM_E_CAPACITY if the pool
+ *                          does not fit max_local_surfels; DSM_E_STATE while a publish snapshot is in flight, or if the file
+ *                          has stored surfels and the context no store; then dsm_inactive_load's checks; DSM_E_CAPACITY if
+ *                          extra_cap is below the extra section, with *extra_bytes (optional) set and nothing loaded.  Then
+ *                          the pool is uploaded (dsm_pool_upload) and the store replaced (dsm_inactive_load; an empty
+ *                          store section empties a reserved store).  A checkpoint holds no frame: dsm_frame_raw_cloud and
+ *                          dsm_frame_superpixel_image still refer to the most recent call that took images.
+ *   dsm_map_peek           the extra section and the segment table of a checkpoint file, checked as dsm_map_load checks
+ *                          the file itself (DSM_E_IO / DSM_E_INVALID), without a context: a caller can decide on the file
+ *                          before it touches its map.  min(cap, size) of each is written; *extra_bytes and *n_segments
+ *                          (optional) receive the sizes. */
+int dsm_inactive_segments(dsm_ctx *ctx, int32_t *kf_ofs_cnt /* [cap][3] */, int cap, int *n_out);
+int dsm_inactive_load(dsm_ctx *ctx, const dsm_surfel_t *surfels, int n, const int32_t *kf_ofs_cnt, int n_segments);
+int dsm_map_save(dsm_ctx *ctx, const char *path, const void *extra, size_t extra_bytes);
+int dsm_map_load(dsm_ctx *ctx, const char *path, void *extra, size_t extra_cap, size_t *extra_bytes);
+int dsm_map_peek(const char *path, void *extra, size_t extra_cap, size_t *extra_bytes, int32_t *kf_ofs_cnt, int seg_cap,
+                 int *n_segments);
 
 /* ---- the node's whole per-frame sequence on the device: move_add_surfels + fuse_map (surfel_map.cpp:154-161) ----
  * dsm_fuse_stream_window is dsm_fuse_stream_resident with each frame's drift-free window step in front of its fuse.

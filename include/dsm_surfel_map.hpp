@@ -150,6 +150,26 @@ inline int fuse_window(Context &c, int reference_index, const uint8_t *gray, con
     const int32_t ref = reference_index;
     return dsm_fuse_stream_window(c.ctx, 1, &ref, gray, depth, pose16, rk.data(), ro, ak.data(), ao, nullptr);
 }
+
+// the checkpoint of the map (dsm_map_save) with the caller's `extra` bytes in it
+inline int save_state(Context &c, const std::string &path, const std::vector<uint8_t> &extra)
+{
+    return dsm_map_save(c.ctx, path.c_str(), extra.data(), extra.size());
+}
+// dsm_map_load: the map replaced by the checkpoint's, whose extra bytes replace `extra`; a failure leaves both as they were
+inline int load_state(Context &c, const std::string &path, std::vector<uint8_t> &extra)
+{
+    size_t n = 0;
+    std::vector<uint8_t> got;
+    int rc = dsm_map_load(c.ctx, path.c_str(), nullptr, 0, &n);
+    if (rc == DSM_E_CAPACITY && n > 0)
+    { // the size-then-read of the extra section: nothing was loaded by the first call
+        got.resize(n);
+        rc = dsm_map_load(c.ctx, path.c_str(), got.data(), got.size(), &n);
+    }
+    if (rc == DSM_OK) extra.swap(got);
+    return rc;
+}
 } // namespace detail
 
 class ResidentSurfelPool
@@ -336,6 +356,19 @@ class ResidentSurfelPool
     {
         local_surfels.clear();
         return ctx_.run("download", [&] { return detail::whole_pool(ctx_, local_surfels); });
+    }
+
+    // ---- checkpoint and resume (DESIGN.md §8.4) ----
+    // local_surfels, the device store and its segment table to one file, with the caller's own state (the pose
+    // database of a SurfelMap that keeps it) as `extra`; load_state replaces the map by the file's and returns that
+    // `extra`.  The constants must be set before loading; a failed load leaves the map as it was.
+    int save_state(const std::string &path, const std::vector<uint8_t> &extra)
+    {
+        return ctx_.run("save_state", [&] { return detail::save_state(ctx_, path, extra); });
+    }
+    int load_state(const std::string &path, std::vector<uint8_t> &extra)
+    {
+        return ctx_.run("load_state", [&] { return detail::load_state(ctx_, path, extra); });
     }
 
     int size()

@@ -231,6 +231,8 @@ class SurfelMapNode
         : ctx_("dsm::SurfelMapNode"), width_(cam_width), height_(cam_height), drift_free_poses_(drift_free_poses), last_ref_(-1),
           fused_(false)
     {
+        const double cam[6] = {cam_fx, cam_fy, cam_cx, cam_cy, far_dist, near_dist};
+        std::memcpy(cam_, cam, sizeof(cam_));
         std::memset(transform_kitti_.d, 0, sizeof(transform_kitti_.d));
         std::memset(&last_fuse_pose_, 0, sizeof(last_fuse_pose_));
         if (device < 0) return;
@@ -503,6 +505,59 @@ class SurfelMapNode
         return ctx_.run("save_cloud", [&] { return detail::save_cloud<dsm_point_t>(ctx_, save_path_name, nullptr); });
     }
 
+    // ---- checkpoint and resume (DESIGN.md §8.4) ----
+    // save_state writes the device map (dsm_map_save) with the node's own section as its extra bytes: the construction
+    // parameters, the KITTI fix-up, every pose, the window, the queued poses, images and depths, the last warp and the
+    // last fuse.  Doubles are stored bit for bit, so a node that loads the file and receives the remaining messages
+    // equals, byte for byte, the node that saved it and received them.  load_state returns DSM_E_INVALID, with the node
+    // unchanged, for a file without a node section, parameters other than this node's, or a stored segment whose
+    // keyframe is outside the pose database or in the window; the file's own errors are dsm_map_load's.  An unread
+    // publish snapshot is retired first; publishing stays as it was.  Both need a context (DSM_E_STATE).
+    int save_state(const std::string &path)
+    {
+        if (!ctx_.ready("save_state")) return ctx_.err;
+        std::vector<uint8_t> section;
+        write_section(section);
+        return ctx_.done(detail::save_state(ctx_, path, section), "save_state");
+    }
+    int load_state(const std::string &path)
+    {
+        if (!ctx_.ready("load_state")) return ctx_.err;
+        size_t n_extra = 0;
+        int n_seg = 0;
+        int rc = dsm_map_peek(path.c_str(), nullptr, 0, &n_extra, nullptr, 0, &n_seg);
+        if (rc != DSM_OK) return ctx_.done(rc, "load_state");
+        std::vector<uint8_t> section(n_extra + 1);
+        std::vector<int32_t> table(3 * (size_t)n_seg + 3);
+        rc = dsm_map_peek(path.c_str(), section.data(), n_extra, nullptr, table.data(), n_seg, nullptr);
+        if (rc != DSM_OK) return ctx_.done(rc, "load_state");
+        section.resize(n_extra);
+        State s;
+        if (!read_section(section, s)) return ctx_.done(DSM_E_INVALID, "load_state");
+        for (int i = 0; i < n_seg; i++)
+            if (table[3 * i] >= (int)s.poses.size() || s.local.count(table[3 * i])) return ctx_.done(DSM_E_INVALID, "load_state");
+        if (snapshot_)
+        { // as fuse_front does: its capacity report, if any, stays with the readers
+            rc = dsm_publish_wait(ctx_.ctx, nullptr, nullptr, nullptr, nullptr, nullptr);
+            snapshot_ = false;
+            if (rc != DSM_OK && rc != DSM_E_CAPACITY) return ctx_.done(rc, "load_state");
+        }
+        std::vector<uint8_t> extra;
+        rc = detail::load_state(ctx_, path, extra);
+        if (rc != DSM_OK) return ctx_.done(rc, "load_state");
+        transform_kitti_ = s.transform_kitti;
+        poses_.swap(s.poses);
+        local_.swap(s.local);
+        pose_buffer_.swap(s.pose_buffer);
+        image_buffer_.swap(s.image_buffer);
+        depth_buffer_.swap(s.depth_buffer);
+        last_warp_.swap(s.last_warp);
+        last_fuse_pose_ = s.last_fuse_pose;
+        last_ref_ = s.last_ref;
+        fused_ = s.fused;
+        return ctx_.done(DSM_OK, "load_state");
+    }
+
     int last_error() const { return ctx_.err; }
     dsm_ctx *context() { return ctx_.ctx; }
 
@@ -513,6 +568,165 @@ class SurfelMapNode
         Pose relative;
         int reference_index;
     };
+
+    // ---- the node's section of a checkpoint, in order; little-endian, doubles bit for bit ----
+    //   char magic[8] "DSMNODE\0", uint32 version, int32 width, height, double fx, fy, cx, cy, far, near (as given),
+    //   int32 drift_free_poses, double transform_kitti[16] (column-major),
+    //   int32 n_poses, per pose: double cam_pose[7], loop_pose[7], cam_stamp, int32 n_links, int32 links[n_links],
+    //   int32 n_local, int32 local[n_local] (ascending),
+    //   int32 n_pose_buffer, per entry: double stamp, double relative[7], int32 reference_index,
+    //   int32 n_images, per image: double stamp, uint8 gray[H*W];  int32 n_depths, per depth: double stamp, float depth[H*W],
+    //   int32 n_warp, per transform: int32 pose, float W[16],
+    //   double last_fuse_pose[7], int32 last_ref, int32 fused
+    enum { kSectionVersion = 1 };
+    struct State
+    {
+        node_math::M4 transform_kitti;
+        std::vector<NodePose> poses;
+        std::set<int> local;
+        std::deque<PendingPose> pose_buffer;
+        std::deque<std::pair<double, std::vector<uint8_t> > > image_buffer;
+        std::deque<std::pair<double, std::vector<float> > > depth_buffer;
+        std::vector<NodeWarp> last_warp;
+        Pose last_fuse_pose;
+        int last_ref;
+        bool fused;
+    };
+    static const char *section_magic() { return "DSMNODE"; } // with its terminating zero: 8 bytes
+    struct Writer
+    {
+        std::vector<uint8_t> &b;
+        void raw(const void *p, size_t n)
+        {
+            const uint8_t *q = static_cast<const uint8_t *>(p);
+            b.insert(b.end(), q, q + n);
+        }
+        template <class T>
+        void put(const T &v)
+        {
+            raw(&v, sizeof(T));
+        }
+    };
+    struct Reader
+    {
+        const std::vector<uint8_t> &b;
+        size_t o;
+        bool raw(void *p, size_t n)
+        {
+            if (n > b.size() - o) return false;
+            if (n) std::memcpy(p, &b[o], n);
+            o += n;
+            return true;
+        }
+        template <class T>
+        bool get(T &v)
+        {
+            return raw(&v, sizeof(T));
+        }
+        // a count that the rest of the section can hold at `each` bytes per element
+        bool count(int32_t &n, size_t each) { return get(n) && n >= 0 && (size_t)n <= (b.size() - o) / each; }
+    };
+    void write_section(std::vector<uint8_t> &out) const
+    {
+        Writer w = {out};
+        w.raw(section_magic(), 8);
+        w.put((uint32_t)kSectionVersion);
+        w.put((int32_t)width_), w.put((int32_t)height_);
+        w.raw(cam_, sizeof(cam_));
+        w.put((int32_t)drift_free_poses_);
+        w.raw(transform_kitti_.d, sizeof(transform_kitti_.d));
+        w.put((int32_t)poses_.size());
+        for (size_t i = 0; i < poses_.size(); i++)
+        {
+            const NodePose &p = poses_[i];
+            w.put(p.cam_pose), w.put(p.loop_pose), w.put(p.cam_stamp);
+            w.put((int32_t)p.linked_pose_index.size());
+            for (size_t j = 0; j < p.linked_pose_index.size(); j++) w.put((int32_t)p.linked_pose_index[j]);
+        }
+        w.put((int32_t)local_.size());
+        for (std::set<int>::const_iterator it = local_.begin(); it != local_.end(); ++it) w.put((int32_t)*it);
+        w.put((int32_t)pose_buffer_.size());
+        for (size_t i = 0; i < pose_buffer_.size(); i++)
+            w.put(pose_buffer_[i].stamp), w.put(pose_buffer_[i].relative), w.put((int32_t)pose_buffer_[i].reference_index);
+        w.put((int32_t)image_buffer_.size());
+        for (size_t i = 0; i < image_buffer_.size(); i++) w.put(image_buffer_[i].first), w.raw(image_buffer_[i].second.data(), image_buffer_[i].second.size());
+        w.put((int32_t)depth_buffer_.size());
+        for (size_t i = 0; i < depth_buffer_.size(); i++)
+            w.put(depth_buffer_[i].first), w.raw(depth_buffer_[i].second.data(), depth_buffer_[i].second.size() * 4);
+        w.put((int32_t)last_warp_.size());
+        for (size_t i = 0; i < last_warp_.size(); i++) w.put((int32_t)last_warp_[i].pose), w.raw(last_warp_[i].W, sizeof(last_warp_[i].W));
+        w.put(last_fuse_pose_), w.put((int32_t)last_ref_), w.put((int32_t)fused_);
+    }
+    // false for anything but a section of this version written by a node with this node's parameters
+    bool read_section(const std::vector<uint8_t> &in, State &s) const
+    {
+        static_assert(sizeof(Pose) == 56, "Pose: 7 doubles");
+        Reader r = {in, 0};
+        char magic[8];
+        uint32_t version = 0;
+        int32_t w = 0, h = 0, dfp = 0, n = 0;
+        double cam[6];
+        if (!r.raw(magic, 8) || std::memcmp(magic, section_magic(), 8) != 0 || !r.get(version) || version != (uint32_t)kSectionVersion) return false;
+        if (!r.get(w) || !r.get(h) || !r.raw(cam, sizeof(cam)) || !r.get(dfp)) return false;
+        if (w != width_ || h != height_ || std::memcmp(cam, cam_, sizeof(cam)) != 0 || dfp != drift_free_poses_) return false;
+        if (!r.raw(s.transform_kitti.d, sizeof(s.transform_kitti.d)) || !r.count(n, 2 * sizeof(Pose) + 12)) return false;
+        s.poses.resize((size_t)n);
+        for (size_t i = 0; i < s.poses.size(); i++)
+        {
+            NodePose &p = s.poses[i];
+            int32_t nl = 0;
+            if (!r.get(p.cam_pose) || !r.get(p.loop_pose) || !r.get(p.cam_stamp) || !r.count(nl, 4)) return false;
+            p.linked_pose_index.resize((size_t)nl);
+            for (int32_t j = 0; j < nl; j++)
+            {
+                int32_t k = 0;
+                if (!r.get(k) || k < 0 || k >= n) return false;
+                p.linked_pose_index[(size_t)j] = k;
+            }
+        }
+        int32_t m = 0;
+        if (!r.count(m, 4)) return false;
+        for (int32_t j = 0; j < m; j++)
+        {
+            int32_t k = 0;
+            if (!r.get(k) || k < 0 || k >= n) return false;
+            s.local.insert(k);
+        }
+        if (!r.count(m, 8 + sizeof(Pose) + 4)) return false;
+        for (int32_t j = 0; j < m; j++)
+        {
+            PendingPose q;
+            int32_t ref = 0;
+            if (!r.get(q.stamp) || !r.get(q.relative) || !r.get(ref) || ref < 0 || ref >= n) return false;
+            q.reference_index = ref;
+            s.pose_buffer.push_back(q);
+        }
+        const size_t px = (size_t)width_ * height_;
+        if (!r.count(m, 8 + px)) return false;
+        for (int32_t j = 0; j < m; j++)
+        {
+            s.image_buffer.push_back(std::make_pair(0.0, std::vector<uint8_t>(px)));
+            if (!r.get(s.image_buffer.back().first) || !r.raw(s.image_buffer.back().second.data(), px)) return false;
+        }
+        if (!r.count(m, 8 + 4 * px)) return false;
+        for (int32_t j = 0; j < m; j++)
+        {
+            s.depth_buffer.push_back(std::make_pair(0.0, std::vector<float>(px)));
+            if (!r.get(s.depth_buffer.back().first) || !r.raw(s.depth_buffer.back().second.data(), 4 * px)) return false;
+        }
+        if (!r.count(m, sizeof(NodeWarp))) return false;
+        s.last_warp.resize((size_t)m);
+        for (size_t j = 0; j < s.last_warp.size(); j++)
+        {
+            int32_t pose = 0;
+            if (!r.get(pose) || !r.raw(s.last_warp[j].W, sizeof(s.last_warp[j].W))) return false;
+            s.last_warp[j].pose = pose;
+        }
+        int32_t ref = 0, fused = 0;
+        if (!r.get(s.last_fuse_pose) || !r.get(ref) || !r.get(fused) || r.o != in.size()) return false;
+        s.last_ref = ref, s.fused = fused != 0;
+        return true;
+    }
 
     static Point3 position(const Pose &p)
     {
@@ -616,6 +830,7 @@ class SurfelMapNode
 
     detail::Context ctx_;
     int width_, height_, drift_free_poses_;
+    double cam_[6]; // fx, fy, cx, cy, far, near as given to the constructor
     node_math::M4 transform_kitti_;
     std::vector<NodePose> poses_;
     std::set<int> local_;
