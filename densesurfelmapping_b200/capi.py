@@ -33,6 +33,7 @@ EXPORTS = [
     "dsm_frame_superpixel_image", "dsm_fuse_stream_window",
     "dsm_publish_enable", "dsm_publish_enqueue", "dsm_publish_wait", "dsm_debug_publish_chunks",
     "dsm_inactive_segments", "dsm_inactive_load", "dsm_map_save", "dsm_map_load", "dsm_map_peek",
+    "dsm_checkpoint_enable", "dsm_checkpoint_enqueue", "dsm_checkpoint_wait", "dsm_debug_checkpoint_drain_ctas",
     "dsm_comm_unique_id", "dsm_comm_init", "dsm_comm_destroy", "dsm_gather_deltas", "dsm_gather_wait", "dsm_gathered_device",
     "dsm_gathered_rank_bytes", "dsm_gathered_download", "dsm_set_constants", "dsm_set_concurrency",
 ]
@@ -117,6 +118,10 @@ def load_library():
     L.dsm_map_save.argtypes = [vp, ctypes.c_char_p, vp, cs]
     L.dsm_map_load.argtypes = [vp, ctypes.c_char_p, vp, cs, ctypes.POINTER(cs)]
     L.dsm_map_peek.argtypes = [ctypes.c_char_p, vp, cs, ctypes.POINTER(cs), vp, ci, ctypes.POINTER(ci)]
+    L.dsm_checkpoint_enable.argtypes = [vp]
+    L.dsm_checkpoint_enqueue.argtypes = [vp, ctypes.c_char_p, vp, cs]
+    L.dsm_checkpoint_wait.argtypes = [vp, ci, ctypes.POINTER(ci)]
+    L.dsm_debug_checkpoint_drain_ctas.argtypes = [vp, ci]
     L.dsm_pool_retire.argtypes = [vp, ci, vp, ci, ctypes.POINTER(ci)]
     L.dsm_pool_append.argtypes = [vp, vp, ci]
     L.dsm_pool_size.argtypes = [vp, ctypes.POINTER(ci)]
@@ -448,6 +453,23 @@ class Context:
             return buf.raw[:size.value]
         self._ck(rc)
         return b""
+
+    # ---- checkpoints that do not stop the stream (DESIGN.md §8.5) ----
+    def checkpoint_enable(self):
+        self._ck(self.lib.dsm_checkpoint_enable(self.h))
+
+    def checkpoint_enqueue(self, path, extra=b""):
+        """Enqueues the file map_save(path, extra) would write at this position in the stream; written by the context's
+        thread while the caller goes on."""
+        buf = ctypes.create_string_buffer(bytes(extra), max(len(extra), 1))
+        self._ck(self.lib.dsm_checkpoint_enqueue(self.h, os.fsencode(path), buf if len(extra) else None, len(extra)))
+
+    def checkpoint_wait(self, block=True):
+        """True once the enqueued checkpoint's file is written (and the checkpoint retired), False while the write runs
+        (block=False only).  A failed write raises DsmError and retires the checkpoint."""
+        fin = ctypes.c_int(0)
+        self._ck(self.lib.dsm_checkpoint_wait(self.h, 1 if block else 0, ctypes.byref(fin)))
+        return bool(fin.value)
 
     # ---- publishing from inside the stream ----
     def publish_enable(self):

@@ -44,6 +44,7 @@ extern "C" void dsm_destroy(dsm_ctx *ctx)
 {
     if (!ctx) return;
     cudaSetDevice(ctx->device);
+    ctx->ckpt.reset(); // a pending checkpoint is written first, then its thread ends
     dsm_comm_destroy(ctx);
     // an asynchronous batch may still be in flight on any of the context's streams: drain them before the buffers go
     for (auto &s : ctx->own.streams) cudaStreamSynchronize(s.get());
@@ -1077,10 +1078,13 @@ static cudaError_t publish_state_reset(dsm_ctx *ctx)
     return e != cudaSuccess ? e : cudaStreamSynchronize(ctx->stream);
 }
 
+static cudaError_t checkpoint_images(dsm_ctx *ctx);
+
 extern "C" int dsm_inactive_reserve(dsm_ctx *ctx, int max_inactive_surfels)
 {
     if (!ctx || max_inactive_surfels < 1) return DSM_E_INVALID;
     if (ctx->pub_in_flight) return DSM_E_STATE; // the snapshot's inactive buffer goes with the old store
+    if (ctx->ckpt && ctx->ckpt->pending) return DSM_E_STATE; // and the checkpoint's images are sized by it
     int rs = res_sync(ctx);
     if (rs != DSM_OK) return rs;
     if (ctx->inact && ctx->inact->size > 0) return DSM_E_STATE;
@@ -1105,6 +1109,11 @@ extern "C" int dsm_inactive_reserve(dsm_ctx *ctx, int max_inactive_surfels)
         return DSM_E_NOMEM;
     }
     ctx->inact = std::move(s);
+    if (ctx->ckpt && checkpoint_images(ctx) != cudaSuccess)
+    {
+        cudaGetLastError();
+        return DSM_E_NOMEM;
+    }
     return DSM_OK;
 }
 
@@ -1404,6 +1413,159 @@ extern "C" int dsm_debug_publish_chunks(dsm_ctx *ctx, int *count)
     if (!ctx || !count) return DSM_E_INVALID;
     if (!ctx->pub_on || ctx->pub_in_flight) return DSM_E_STATE;
     *count = ctx->pub_hdr[DSM_PUB_CHUNKS];
+    return DSM_OK;
+}
+
+// ---- checkpoints that do not stop the stream (include/dsm.h, DESIGN.md §8.5) ----
+// The two images at the context's current capacities; whatever was there before is released first (the old and the new
+// need not fit at once).  On failure the checkpoint has no images and its calls return DSM_E_STATE.
+static cudaError_t checkpoint_images(dsm_ctx *ctx)
+{
+    DsmCheckpoint &k = *ctx->ckpt;
+    k.img.reset();
+    k.dev = k.host = k.host_dev = nullptr;
+    auto own = std::make_unique<CudaOwner>();
+    const DsmSnapLayout lay = dsm_snap_layout(ctx->p.max_local_surfels, ctx->inact ? ctx->inact->cap : 0);
+    uint8_t *dev = nullptr, *host = nullptr, *host_dev = nullptr;
+    // not zeroed: the drain also copies the unused tail of each section's last line, which the writer never reads
+    cudaError_t e = own->device(&dev, lay.bytes);
+    if (e == cudaSuccess) e = own->mapped(&host, &host_dev, lay.bytes);
+    if (e != cudaSuccess) return e;
+    k.img = std::move(own);
+    k.lay = lay;
+    k.dev = dev, k.host = host, k.host_dev = host_dev;
+    return cudaSuccess;
+}
+
+// The write of one enqueued checkpoint, on the checkpoint's thread: waits for the drain, then writes the host image's
+// sections through the file's one writer.  A snapshot that recorded a rejected frame writes nothing.
+static int checkpoint_write(DsmCheckpoint &k)
+{
+    if (cudaEventSynchronize(k.ev_drain) != cudaSuccess) return DSM_E_CUDA;
+    const volatile int32_t *h = reinterpret_cast<const volatile int32_t *>(k.host);
+    if (h[DSM_SNAP_ERR_TAG] != 0)
+    {
+        k.err_frame = h[DSM_SNAP_ERR_FRAME];
+        return DSM_E_CAPACITY;
+    }
+    const DsmMapSections s{reinterpret_cast<const dsm_surfel_t *>(k.host + k.lay.pool), h[DSM_SNAP_N_POOL],
+                           reinterpret_cast<const dsm_surfel_t *>(k.host + k.lay.store), h[DSM_SNAP_N_STORE],
+                           reinterpret_cast<const int32_t *>(k.host + k.lay.table), h[DSM_SNAP_N_SEGMENTS],
+                           k.extra.data(), k.extra.size()};
+    return dsm_map_write(k.path.c_str(), k.info, s);
+}
+
+static void checkpoint_thread(DsmCheckpoint *k, int device)
+{
+    cudaSetDevice(device);
+    std::unique_lock<std::mutex> lk(k->m);
+    for (;;)
+    {
+        k->cv.wait(lk, [k] { return k->queued || k->quit; });
+        if (!k->queued) return;
+        lk.unlock();
+        const int rc = checkpoint_write(*k);
+        lk.lock();
+        k->result = rc;
+        k->queued = false;
+        k->cv.notify_all();
+    }
+}
+
+extern "C" int dsm_checkpoint_enable(dsm_ctx *ctx)
+{
+    if (!ctx) return DSM_E_INVALID;
+    if (!ctx->res_active || ctx->ckpt) return DSM_E_STATE;
+    CK(cudaSetDevice(ctx->device));
+    auto k = std::make_unique<DsmCheckpoint>();
+    int lo = 0, hi = 0;
+    cudaError_t e = cudaDeviceGetStreamPriorityRange(&lo, &hi);
+    if (e == cudaSuccess) e = k->own.stream(&k->s_drain, lo); // the least priority: the stream's kernels come first
+    if (e == cudaSuccess) e = k->own.event(&k->ev_snap);
+    // the thread waits on this event for the whole stream queued before the snapshot: it sleeps instead of spinning a core
+    if (e == cudaSuccess) e = k->own.event(&k->ev_drain, cudaEventDisableTiming | cudaEventBlockingSync);
+    ctx->ckpt = std::move(k);
+    if (e == cudaSuccess) e = checkpoint_images(ctx);
+    if (e != cudaSuccess)
+    {
+        cudaGetLastError();
+        ctx->ckpt.reset();
+        return DSM_E_NOMEM;
+    }
+    try
+    {
+        ctx->ckpt->worker = std::thread(checkpoint_thread, ctx->ckpt.get(), ctx->device);
+    }
+    catch (...)
+    {
+        ctx->ckpt.reset();
+        return DSM_E_NOMEM;
+    }
+    return DSM_OK;
+}
+
+// Enqueue only, like dsm_publish_enqueue: the snapshot on the context's stream, the drain on the checkpoint's stream
+// after it, the write on the checkpoint's thread.  The view of the map has no gate: the snapshot records the error word.
+extern "C" int dsm_checkpoint_enqueue(dsm_ctx *ctx, const char *path, const void *extra, size_t extra_bytes)
+{
+    if (!ctx || !path || (extra_bytes > 0 && !extra)) return DSM_E_INVALID;
+    DsmCheckpoint *k = ctx->ckpt.get();
+    if (!k || k->pending || !k->img) return DSM_E_STATE;
+    // as dsm_map_save (through dsm_pool_size): a batch call since the last dsm_pool_upload left the batch's slices in the
+    // pool buffer and no resident pool to save; an asynchronous batch still in flight runs on streams the snapshot is not
+    // ordered against
+    if (!ctx->res_active || ctx->in_flight) return DSM_E_STATE;
+    CK(cudaSetDevice(ctx->device));
+    DsmMapInfo info;
+    dsm_map_info(ctx, &info);
+    const InactStore *s = ctx->inact.get();
+    // grids from the host bounds, clamped to the capacities: a caller that never synchronises keeps bounds that only grow
+    dsm_launch_map_snapshot(ctx->d.pool, ctx->res_ofs, std::min(ctx->res_upper, ctx->p.max_local_surfels), s ? s->surfels : nullptr,
+                            s ? s->seg : nullptr, ctx->win_hdr, s ? std::min(s->upper, s->cap) : 0, k->dev, k->lay, ctx->stream);
+    CK(cudaGetLastError());
+    CK(cudaEventRecord(k->ev_snap, ctx->stream));
+    CK(cudaStreamWaitEvent(k->s_drain, k->ev_snap, 0));
+    dsm_launch_map_drain(k->dev, k->host_dev, k->lay, k->drain_ctas, k->s_drain);
+    CK(cudaGetLastError());
+    CK(cudaEventRecord(k->ev_drain, k->s_drain));
+    {
+        std::lock_guard<std::mutex> lk(k->m);
+        k->path = path;
+        k->extra.assign(static_cast<const uint8_t *>(extra), static_cast<const uint8_t *>(extra) + extra_bytes);
+        k->info = info;
+        k->queued = true;
+    }
+    k->cv.notify_all();
+    k->pending = true;
+    return DSM_OK;
+}
+
+extern "C" int dsm_checkpoint_wait(dsm_ctx *ctx, int block, int *finished)
+{
+    if (finished) *finished = 0;
+    if (!ctx) return DSM_E_INVALID;
+    DsmCheckpoint *k = ctx->ckpt.get();
+    if (!k || !k->pending) return DSM_E_STATE;
+    std::unique_lock<std::mutex> lk(k->m);
+    if (k->queued && !block) return DSM_OK;
+    k->cv.wait(lk, [k] { return !k->queued; });
+    k->pending = false;
+    if (finished) *finished = 1;
+    if (k->result == DSM_E_CAPACITY)
+        snprintf(ctx->err, sizeof(ctx->err), "dsm_checkpoint_wait: frame %d of a dsm_fuse_stream_window call did not fit the pool or "
+                 "the store before the checkpoint; no file was written", k->err_frame);
+    else if (k->result == DSM_E_IO)
+        snprintf(ctx->err, sizeof(ctx->err), "dsm_checkpoint_wait: %s could not be written", k->path.c_str());
+    else if (k->result == DSM_E_CUDA)
+        snprintf(ctx->err, sizeof(ctx->err), "dsm_checkpoint_wait: the drain of the snapshot failed");
+    return k->result;
+}
+
+extern "C" int dsm_debug_checkpoint_drain_ctas(dsm_ctx *ctx, int ctas)
+{
+    if (!ctx || ctas < 1) return DSM_E_INVALID;
+    if (!ctx->ckpt || ctx->ckpt->pending) return DSM_E_STATE;
+    ctx->ckpt->drain_ctas = ctas;
     return DSM_OK;
 }
 

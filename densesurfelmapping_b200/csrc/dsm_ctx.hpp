@@ -2,8 +2,13 @@
 // translation units (dsm_capi.cu: single-GPU entry points; dsm_comm.cu: multi-GPU gather over NCCL).
 #pragma once
 #include "dsm_device.cuh"
+#include "dsm_map_state.h"
+#include <condition_variable>
 #include <cstdio>
 #include <memory>
+#include <mutex>
+#include <string>
+#include <thread>
 #include <vector>
 
 struct DsmComm; // multi-GPU state (dsm_comm.cu), nullptr until dsm_comm_init
@@ -115,6 +120,40 @@ struct InactStore
     std::vector<Seg> segs;
 };
 
+// dsm_checkpoint_* (DESIGN.md §8.5): the device image k_map_snapshot writes in stream order, its pinned host twin
+// k_map_drain fills on a low-priority stream, and the thread that writes the file.  The thread touches only the host
+// image and the job below; the caller's thread owns everything else.
+struct DsmCheckpoint
+{
+    CudaOwner own;                 // the drain stream and its events
+    std::unique_ptr<CudaOwner> img; // the two images; dsm_inactive_reserve rebuilds them at the store's new size
+    DsmSnapLayout lay{};
+    uint8_t *dev = nullptr, *host = nullptr, *host_dev = nullptr; // device image, host image and its device alias
+    cudaStream_t s_drain = nullptr;
+    cudaEvent_t ev_snap = nullptr, ev_drain = nullptr; // after k_map_snapshot on the context's stream, after k_map_drain
+    int drain_ctas = DSM_DRAIN_CTAS;
+    bool pending = false; // enqueued and not yet retired by dsm_checkpoint_wait (caller's thread only)
+    // the job, guarded by m: queued from dsm_checkpoint_enqueue until the thread has stored its result
+    std::mutex m;
+    std::condition_variable cv;
+    bool queued = false, quit = false;
+    int result = DSM_OK, err_frame = 0;
+    std::string path;
+    std::vector<uint8_t> extra;
+    DsmMapInfo info{};
+    std::thread worker; // last: started once the members above exist
+
+    ~DsmCheckpoint()
+    { // a queued write finishes (its file lands) before the thread ends
+        {
+            std::lock_guard<std::mutex> lk(m);
+            quit = true;
+        }
+        cv.notify_all();
+        if (worker.joinable()) worker.join();
+    }
+};
+
 #define DSM_MAX_CHUNKS 4
 
 struct dsm_ctx
@@ -182,7 +221,8 @@ struct dsm_ctx
     float4 *pub_active_dev = nullptr;
     int32_t *pub_hdr = nullptr, *pub_hdr_dev = nullptr, *pub_state = nullptr;
     cudaEvent_t pub_ev = nullptr;
-    int run_split = 2;           // sub-batches per dsm_batch_run (dsm_set_concurrency)
+    std::unique_ptr<DsmCheckpoint> ckpt; // nullptr until dsm_checkpoint_enable
+    int run_split = 2;          // sub-batches per dsm_batch_run (dsm_set_concurrency)
     // pinned host staging for the small per-batch tables
     float *h_pose = nullptr; // [2B][32]: pose then inverse; first half: the batch calls, second half: the resident stream
     int32_t *h_ofs = nullptr;

@@ -214,3 +214,39 @@ enum
 // grid; state: device [4], {0, INT_MAX, 0, 0} when the shadow is new
 void dsm_launch_cloud_mirror(const dsm_surfel_t *store, const int32_t *size_word, const int32_t *res, int upper, float4 *shadow,
                              float4 *mirror, int32_t *state, int32_t *header, cudaStream_t s);
+
+// Image of dsm_checkpoint_enqueue, written by k_map_snapshot on the context's stream and copied by k_map_drain into its
+// pinned host twin: a 128-byte header line of DSM_SNAP_* words, then the pool (slot order), the store (store order) and
+// the segment table packed to int32 (keyframe, offset, count), each section at a 128-byte aligned offset and sized for
+// its capacity.  The file's writer stitches the sections together (DESIGN.md §8.5).
+enum
+{
+    DSM_SNAP_N_POOL,     // res_ofs[1] at the snapshot
+    DSM_SNAP_N_STORE,    // win_hdr[0] (0 without a store)
+    DSM_SNAP_N_SEGMENTS, // win_hdr[1] (0 without a store)
+    DSM_SNAP_ERR_TAG,    // the sticky error word of dsm_fuse_stream_window, and
+    DSM_SNAP_ERR_FRAME,  // the frame it rejected
+    DSM_SNAP_WORDS
+};
+struct DsmSnapLayout
+{
+    size_t pool, store, table, bytes; // byte offsets of the sections, total size
+};
+inline size_t dsm_line_up(size_t b) { return (b + 127) / 128 * 128; }
+inline DsmSnapLayout dsm_snap_layout(int pool_cap, int store_cap)
+{
+    DsmSnapLayout l;
+    l.pool = 128;
+    l.store = l.pool + dsm_line_up((size_t)pool_cap * sizeof(dsm_surfel_t));
+    l.table = l.store + dsm_line_up((size_t)store_cap * sizeof(dsm_surfel_t));
+    l.bytes = l.table + dsm_line_up((size_t)store_cap * 12);
+    return l;
+}
+// k_map_snapshot: pool_upper / store_upper >= the live sizes size the grid (surplus CTAs exit at once).  store == nullptr:
+// no store, n_store = n_segments = 0.  res: {0, pool size, error tag, rejected frame}; hdr: {store size, segments, ...}
+void dsm_launch_map_snapshot(const dsm_surfel_t *pool, const int32_t *res, int pool_upper, const dsm_surfel_t *store, const int4 *seg,
+                             const int32_t *hdr, int store_upper, uint8_t *image, const DsmSnapLayout &lay, cudaStream_t s);
+// k_map_drain: the image's live lines (as its header gives them) to host_dev, the device alias of the pinned host image,
+// on a fixed grid of `ctas` CTAs
+#define DSM_DRAIN_CTAS 8
+void dsm_launch_map_drain(const uint8_t *image, uint8_t *host_dev, const DsmSnapLayout &lay, int ctas, cudaStream_t s);

@@ -19,6 +19,8 @@
 //                      104  dsm_surfel_t pool[n_pool] (slot order), dsm_surfel_t store[n_store] (store order),
 //                           int32 table[n_segments][3] (keyframe, offset, count), uint8 extra[extra_bytes],
 //                           uint64 FNV-1a 64 of every byte before it
+//                      dsm_map_write is the one writer of that file: dsm_map_save and the checkpoint thread of
+//                      dsm_checkpoint_enqueue (dsm_capi.cu) hand it the header fields and the sections as spans.
 #include <fcntl.h>
 #include <sys/stat.h>
 #include <unistd.h>
@@ -320,6 +322,11 @@ extern "C" int dsm_map_save(dsm_ctx *ctx, const char *path, const void *extra, s
         if (rc == DSM_OK) rc = dsm_inactive_segments(ctx, table.data(), n_seg, &n_seg);
     }
     if (rc != DSM_OK) return rc;
+    return dsm_map_write(path, info, DsmMapSections{pool.data(), n_pool, store.data(), n_store, table.data(), n_seg, extra, extra_bytes});
+}
+
+int dsm_map_write(const char *path, const DsmMapInfo &info, const DsmMapSections &s)
+{
     MapHeader h;
     std::memset(&h, 0, sizeof(h));
     std::memcpy(h.magic, kMapMagic, 8);
@@ -329,14 +336,14 @@ extern "C" int dsm_map_save(dsm_ctx *ctx, const char *path, const void *extra, s
     h.width = p.width, h.height = p.height;
     h.fx = p.fx, h.fy = p.fy, h.cx = p.cx, h.cy = p.cy, h.fuse_far = p.fuse_far, h.fuse_near = p.fuse_near;
     h.constants = info.constants;
-    h.n_pool = n_pool, h.n_store = n_store, h.n_segments = n_seg;
-    h.extra_bytes = extra_bytes;
+    h.n_pool = s.n_pool, h.n_store = s.n_store, h.n_segments = s.n_segments;
+    h.extra_bytes = s.extra_bytes;
     AtomicFile out(path);
     out.put(&h, sizeof(h));
-    out.put(pool.data(), (size_t)n_pool * sizeof(dsm_surfel_t));
-    out.put(store.data(), (size_t)n_store * sizeof(dsm_surfel_t));
-    out.put(table.data(), (size_t)n_seg * 12);
-    out.put(extra, extra_bytes);
+    out.put(s.pool, (size_t)s.n_pool * sizeof(dsm_surfel_t));
+    out.put(s.store, (size_t)s.n_store * sizeof(dsm_surfel_t));
+    out.put(s.table, (size_t)s.n_segments * 12);
+    out.put(s.extra, s.extra_bytes);
     return out.commit() ? DSM_OK : DSM_E_IO;
 }
 

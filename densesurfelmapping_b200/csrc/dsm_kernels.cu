@@ -1068,6 +1068,78 @@ __global__ void __launch_bounds__(DSM_PUB_CHUNK) k_cloud_mirror(const dsm_surfel
 }
 
 // -------------------------------------------------------------------------------------------
+// k_map_snapshot — the map of dsm_checkpoint_enqueue at its position in the stream, into the checkpoint's device image
+// (DsmSnapLayout).  The live sizes exist on the device only (res_ofs[1], win_hdr), so the copy is sized here: CTA c
+// < pool_grid copies pool surfels [256 c, 256 c + 256) below the pool size, CTA pool_grid + c stored surfels
+// [256 c, 256 c + 256) below the store size and the segments with the same indices (a segment holds >= 1 surfel, so
+// every live segment falls to a live CTA), packed from int4 to int32[3].  The surfels are staged like
+// k_pool_transform's: source and destination chunks start 11264 * c bytes from 128-byte aligned bases, so every whole
+// chunk moves as one TMA bulk copy each way and only the ragged last chunk of a section goes word by word.  CTA 0 writes
+// the header, the error word included: the snapshot does not wait on it (it records it, as k_cloud_mirror does).
+// Launched without PDL: it begins after everything enqueued before it has completed.
+// -------------------------------------------------------------------------------------------
+#define SNAP_CHUNK 256
+__global__ void __launch_bounds__(SNAP_CHUNK) k_map_snapshot(const dsm_surfel_t *pool, const int32_t *res, int pool_grid,
+                                                             const dsm_surfel_t *store, const int4 *seg, const int32_t *hdr,
+                                                             uint8_t *image, const DsmSnapLayout lay)
+{
+    __shared__ alignas(128) float sm[SNAP_CHUNK * 11];
+    __shared__ uint64_t bar;
+    const int n_pool = res[1], n_store = store ? hdr[0] : 0, n_seg = store ? hdr[1] : 0;
+    if (blockIdx.x == 0 && threadIdx.x == 0)
+    {
+        int32_t *h = reinterpret_cast<int32_t *>(image);
+        h[DSM_SNAP_N_POOL] = n_pool;
+        h[DSM_SNAP_N_STORE] = n_store;
+        h[DSM_SNAP_N_SEGMENTS] = n_seg;
+        h[DSM_SNAP_ERR_TAG] = res[2];
+        h[DSM_SNAP_ERR_FRAME] = res[3];
+    }
+    const bool in_pool = (int)blockIdx.x < pool_grid;
+    const int first = (in_pool ? blockIdx.x : blockIdx.x - pool_grid) * SNAP_CHUNK;
+    const int n = in_pool ? n_pool : n_store;
+    if (first >= n) return;
+    const int cnt = min(SNAP_CHUNK, n - first);
+    if (!in_pool && first + (int)threadIdx.x < n_seg)
+    {
+        const int i = first + threadIdx.x;
+        const int4 g = seg[i];
+        int32_t *t = reinterpret_cast<int32_t *>(image + lay.table) + 3 * (size_t)i;
+        t[0] = g.x, t[1] = g.y, t[2] = g.z;
+    }
+    const float *src = reinterpret_cast<const float *>((in_pool ? pool : store) + first);
+    float *dst = reinterpret_cast<float *>(image + (in_pool ? lay.pool : lay.store)) + (size_t)first * 11;
+    const bool bulk = stage_in(sm, src, cnt, &bar, SNAP_CHUNK); // dst is 16-byte aligned whenever src is
+    stage_out(dst, sm, cnt, bulk, SNAP_CHUNK);
+}
+
+// -------------------------------------------------------------------------------------------
+// k_map_drain — the live part of the checkpoint image to its pinned host twin through the device alias, on a side
+// stream after k_map_snapshot: the header line and the whole 128-byte lines that hold each section's live bytes (the
+// sections are line-aligned and sized in lines, so the last line of a section stays inside it).  16 bytes per thread,
+// a quarter-warp per line; a small fixed grid, since the copy is bound by PCIe and must leave the SMs to the stream's
+// kernels.
+// -------------------------------------------------------------------------------------------
+#define DRAIN_BLOCK 256
+__global__ void __launch_bounds__(DRAIN_BLOCK) k_map_drain(const uint8_t *image, uint8_t *host, const DsmSnapLayout lay)
+{
+    const int32_t *h = reinterpret_cast<const int32_t *>(image);
+    const size_t lp = ((size_t)h[DSM_SNAP_N_POOL] * 44 + 127) / 128, ls = ((size_t)h[DSM_SNAP_N_STORE] * 44 + 127) / 128;
+    const size_t lt = ((size_t)h[DSM_SNAP_N_SEGMENTS] * 12 + 127) / 128;
+    const size_t words = 8 * (1 + lp + ls + lt);
+    for (size_t w = (size_t)blockIdx.x * DRAIN_BLOCK + threadIdx.x; w < words; w += (size_t)gridDim.x * DRAIN_BLOCK)
+    {
+        size_t line = w >> 3, ofs;
+        if (line == 0) ofs = 0;
+        else if ((line -= 1) < lp) ofs = lay.pool + line * 128;
+        else if ((line -= lp) < ls) ofs = lay.store + line * 128;
+        else ofs = lay.table + (line - ls) * 128;
+        ofs += (w & 7) * 16;
+        *reinterpret_cast<int4 *>(host + ofs) = __ldg(reinterpret_cast<const int4 *>(image + ofs));
+    }
+}
+
+// -------------------------------------------------------------------------------------------
 // parity readback: rebuild the reference's 60-byte Superpixel_seed records for one frame
 // -------------------------------------------------------------------------------------------
 __global__ void k_seeds_export(const __grid_constant__ DsmDev d, int b, dsm_seed_t *out, int raw_md)
@@ -1317,4 +1389,16 @@ void dsm_launch_cloud_mirror(const dsm_surfel_t *store, const int32_t *size_word
 {
     const int grid = store ? (upper + DSM_PUB_CHUNK - 1) / DSM_PUB_CHUNK : 1;
     k_cloud_mirror<<<grid > 1 ? grid : 1, DSM_PUB_CHUNK, 0, s>>>(store, size_word, res, shadow, mirror, state, header);
+}
+void dsm_launch_map_snapshot(const dsm_surfel_t *pool, const int32_t *res, int pool_upper, const dsm_surfel_t *store, const int4 *seg,
+                             const int32_t *hdr, int store_upper, uint8_t *image, const DsmSnapLayout &lay, cudaStream_t s)
+{
+    const int pool_chunks = (pool_upper + SNAP_CHUNK - 1) / SNAP_CHUNK;
+    const int pool_grid = pool_chunks > 1 ? pool_chunks : 1; // CTA 0 exists and writes the header
+    const int store_grid = store ? (store_upper + SNAP_CHUNK - 1) / SNAP_CHUNK : 0;
+    k_map_snapshot<<<pool_grid + store_grid, SNAP_CHUNK, 0, s>>>(pool, res, pool_grid, store, seg, hdr, image, lay);
+}
+void dsm_launch_map_drain(const uint8_t *image, uint8_t *host_dev, const DsmSnapLayout &lay, int ctas, cudaStream_t s)
+{
+    k_map_drain<<<ctas, DRAIN_BLOCK, 0, s>>>(image, host_dev, lay);
 }

@@ -15,3 +15,19 @@ __attribute__((visibility("hidden"))) int dsm_map_info(const dsm_ctx *ctx, DsmMa
 // the host-side checks of dsm_inactive_load, in its order; touches nothing
 __attribute__((visibility("hidden"))) int dsm_inactive_load_check(const dsm_ctx *ctx, const dsm_surfel_t *surfels, int n,
                                                                   const int32_t *kf_ofs_cnt, int n_segments);
+
+// The sections of one checkpoint file, in file order
+struct DsmMapSections
+{
+    const dsm_surfel_t *pool;
+    int n_pool;
+    const dsm_surfel_t *store;
+    int n_store;
+    const int32_t *table; // [n_segments][3]: keyframe, offset, count
+    int n_segments;
+    const void *extra;
+    size_t extra_bytes;
+};
+// The one writer of the file (dsm_io.cpp), for dsm_map_save and the checkpoint thread: header from `info`, the sections,
+// the checksum; under a temporary name, flushed to the disk and renamed over `path`.  DSM_E_IO leaves nothing under path.
+__attribute__((visibility("hidden"))) int dsm_map_write(const char *path, const DsmMapInfo &info, const DsmMapSections &s);

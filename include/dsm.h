@@ -447,6 +447,42 @@ int dsm_publish_wait(dsm_ctx *ctx, const dsm_point_t **active, int *n_active, co
                      int *inactive_changed_from);
 int dsm_debug_publish_chunks(dsm_ctx *ctx, int *count);
 
+/* ---- checkpoints that do not stop the stream (DESIGN.md §8.5) ----
+ * The file of dsm_map_save, taken in stream order like a publish snapshot: the resident stream pays one device-to-device
+ * copy of the live map, the transfer to the host runs on a low-priority stream beside the next frames, and a thread of
+ * the context writes the file.  For a node that wants a checkpoint every N keyframes without stalling.
+ *   dsm_checkpoint_enable   once, on a context with a resident pool (DSM_E_STATE otherwise, and when called twice).
+ *                           Allocates a device image and a pinned, mapped host image of
+ *                           128 + 44 * max_local_surfels + 56 * (store reservation) bytes each (every section rounded up
+ *                           to 128 bytes; 327 MB each at 2 Mi pool + 4 Mi store), a low-priority stream, two events and
+ *                           the writer thread, which dsm_destroy joins.  DSM_E_NOMEM.  A later dsm_inactive_reserve
+ *                           rebuilds the images at the new size (DSM_E_NOMEM if it cannot; the checkpoint calls then
+ *                           return DSM_E_STATE until a reserve succeeds).
+ *   dsm_checkpoint_enqueue  asynchronous, ordered on the context's stream exactly like dsm_publish_enqueue.  Copies path
+ *                           and extra, captures the geometry and the constants, enqueues the snapshot and the drain and
+ *                           hands the write to the thread.  Never waits and reads nothing back.  The file is byte for
+ *                           byte what dsm_map_save(ctx, path, extra, extra_bytes) would have written at this position in
+ *                           the stream.  DSM_E_INVALID for a NULL path, or extra_bytes > 0 with a NULL extra;
+ *                           DSM_E_STATE before dsm_checkpoint_enable, while an earlier checkpoint has not been
+ *                           retired by dsm_checkpoint_wait, and, as dsm_map_save, when the context holds no resident
+ *                           pool (a batch call since the last dsm_pool_upload) or a dsm_fuse_batch_async batch is in
+ *                           flight; nothing is enqueued then and nothing under path changes.  Every other call may run meanwhile (fuses, transforms,
+ *                           dsm_map_load, dsm_inactive_load, publishing), except dsm_inactive_reserve (DSM_E_STATE).
+ *   dsm_checkpoint_wait     block = 0: DSM_OK with *finished = 0 while the write runs.  Once it has finished (block != 0:
+ *                           after waiting for it), returns its result with *finished = 1 and retires the checkpoint:
+ *                           DSM_OK once the file is on the disk (temporary name, checksum, fsync, rename, directory
+ *                           fsync, as dsm_map_save); DSM_E_IO with nothing left under path; DSM_E_CAPACITY, with no
+ *                           file, when a frame of dsm_fuse_stream_window had been rejected before the snapshot -- the
+ *                           error is NOT cleared: the next synchronising call reports and clears it, as after
+ *                           dsm_publish_wait.  finished may be NULL.  DSM_E_STATE with nothing enqueued.
+ * dsm_destroy with a pending checkpoint returns after its file has been written.  A context is still used from one
+ * thread at a time; the writer thread touches only the host image and the copies of path and extra.
+ *   dsm_debug_checkpoint_drain_ctas   the CTA count of the drain kernel (default 8); DSM_E_STATE while one is pending. */
+int dsm_checkpoint_enable(dsm_ctx *ctx);
+int dsm_checkpoint_enqueue(dsm_ctx *ctx, const char *path, const void *extra, size_t extra_bytes);
+int dsm_checkpoint_wait(dsm_ctx *ctx, int block, int *finished);
+int dsm_debug_checkpoint_drain_ctas(dsm_ctx *ctx, int ctas);
+
 /* ---- multi-GPU: frames of a batch sharded across GPUs, ONE gather of the surfel deltas at the end (SURVEY.md 8e) ----
  * One context per GPU (one process or thread each).  The reference has no counterpart (fuse_initialize_map is
  * single-process, fusion_functions.cpp:30-83); what is gathered is what SurfelMap::fuse_map consumes after the call

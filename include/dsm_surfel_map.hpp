@@ -156,6 +156,19 @@ inline int save_state(Context &c, const std::string &path, const std::vector<uin
 {
     return dsm_map_save(c.ctx, path.c_str(), extra.data(), extra.size());
 }
+// the same file, taken in stream order and written by the context's thread (dsm_checkpoint_enqueue)
+inline int save_state_async(Context &c, const std::string &path, const std::vector<uint8_t> &extra)
+{
+    return dsm_checkpoint_enqueue(c.ctx, path.c_str(), extra.data(), extra.size());
+}
+// dsm_checkpoint_wait with a C++ flag
+inline int wait_state_saved(Context &c, bool block, bool *finished)
+{
+    int fin = 0;
+    const int rc = dsm_checkpoint_wait(c.ctx, block ? 1 : 0, &fin);
+    if (finished) *finished = fin != 0;
+    return rc;
+}
 // dsm_map_load: the map replaced by the checkpoint's, whose extra bytes replace `extra`; a failure leaves both as they were
 inline int load_state(Context &c, const std::string &path, std::vector<uint8_t> &extra)
 {
@@ -369,6 +382,22 @@ class ResidentSurfelPool
     int load_state(const std::string &path, std::vector<uint8_t> &extra)
     {
         return ctx_.run("load_state", [&] { return detail::load_state(ctx_, path, extra); });
+    }
+    // The same file without stopping the stream (DESIGN.md §8.5): enable_checkpoints once after initialize;
+    // save_state_async enqueues the file save_state would write at this point of the stream and returns at once;
+    // wait_state_saved(false, &finished) polls it (finished = false while it is written), wait_state_saved(true, ...)
+    // waits, and either returns the write's result once finished.  One checkpoint at a time.
+    int enable_checkpoints()
+    {
+        return ctx_.run("enable_checkpoints", [&] { return dsm_checkpoint_enable(ctx_.ctx); });
+    }
+    int save_state_async(const std::string &path, const std::vector<uint8_t> &extra)
+    {
+        return ctx_.run("save_state_async", [&] { return detail::save_state_async(ctx_, path, extra); });
+    }
+    int wait_state_saved(bool block, bool *finished)
+    {
+        return ctx_.run("wait_state_saved", [&] { return detail::wait_state_saved(ctx_, block, finished); });
     }
 
     int size()

@@ -520,6 +520,28 @@ class SurfelMapNode
         write_section(section);
         return ctx_.done(detail::save_state(ctx_, path, section), "save_state");
     }
+    // The same file without stopping the node (DESIGN.md §8.5, INTEGRATION.md §4).  enable_checkpoints once after
+    // construction.  save_state_async writes the node's section now -- the host state of exactly the fuses enqueued so
+    // far -- and enqueues the device map behind those fuses; a thread of the context writes the file while the node goes
+    // on.  Meant for a checkpoint every N keyframes from the image callback, with wait_state_saved(false, &finished)
+    // polled on the next call (finished = false while the file is written; once finished it returns the write's result
+    // and the next save_state_async may follow).  An unread publish snapshot stays as it is.  The file equals save_state's
+    // at the same message, and load_state resumes from it.
+    int enable_checkpoints()
+    {
+        return ctx_.run("enable_checkpoints", [&] { return dsm_checkpoint_enable(ctx_.ctx); });
+    }
+    int save_state_async(const std::string &path)
+    {
+        if (!ctx_.ready("save_state_async")) return ctx_.err;
+        std::vector<uint8_t> section;
+        write_section(section);
+        return ctx_.done(detail::save_state_async(ctx_, path, section), "save_state_async");
+    }
+    int wait_state_saved(bool block, bool *finished)
+    {
+        return ctx_.run("wait_state_saved", [&] { return detail::wait_state_saved(ctx_, block, finished); });
+    }
     int load_state(const std::string &path)
     {
         if (!ctx_.ready("load_state")) return ctx_.err;
