@@ -34,6 +34,7 @@ EXPORTS = [
     "dsm_publish_enable", "dsm_publish_enqueue", "dsm_publish_wait", "dsm_debug_publish_chunks",
     "dsm_inactive_segments", "dsm_inactive_load", "dsm_map_save", "dsm_map_load", "dsm_map_peek",
     "dsm_checkpoint_enable", "dsm_checkpoint_enqueue", "dsm_checkpoint_wait", "dsm_debug_checkpoint_drain_ctas",
+    "dsm_checkpoint_enqueue_incremental", "dsm_map_load_journal", "dsm_map_peek_journal", "dsm_journal_materialize",
     "dsm_comm_unique_id", "dsm_comm_init", "dsm_comm_destroy", "dsm_gather_deltas", "dsm_gather_wait", "dsm_gathered_device",
     "dsm_gathered_rank_bytes", "dsm_gathered_download", "dsm_set_constants", "dsm_set_concurrency",
 ]
@@ -122,6 +123,10 @@ def load_library():
     L.dsm_checkpoint_enqueue.argtypes = [vp, ctypes.c_char_p, vp, cs]
     L.dsm_checkpoint_wait.argtypes = [vp, ci, ctypes.POINTER(ci)]
     L.dsm_debug_checkpoint_drain_ctas.argtypes = [vp, ci]
+    L.dsm_checkpoint_enqueue_incremental.argtypes = [vp, ctypes.c_char_p, vp, cs]
+    L.dsm_map_load_journal.argtypes = [vp, ctypes.c_char_p, vp, cs, ctypes.POINTER(cs), ctypes.POINTER(ci)]
+    L.dsm_map_peek_journal.argtypes = [ctypes.c_char_p, vp, cs, ctypes.POINTER(cs), vp, ci, ctypes.POINTER(ci), ctypes.POINTER(ci)]
+    L.dsm_journal_materialize.argtypes = [ctypes.c_char_p, ctypes.c_char_p]
     L.dsm_pool_retire.argtypes = [vp, ci, vp, ci, ctypes.POINTER(ci)]
     L.dsm_pool_append.argtypes = [vp, vp, ci]
     L.dsm_pool_size.argtypes = [vp, ctypes.POINTER(ci)]
@@ -471,6 +476,24 @@ class Context:
         self._ck(self.lib.dsm_checkpoint_wait(self.h, 1 if block else 0, ctypes.byref(fin)))
         return bool(fin.value)
 
+    # ---- incremental checkpoints (DESIGN.md §8.6) ----
+    def checkpoint_enqueue_incremental(self, path, extra=b""):
+        """checkpoint_enqueue, but written as one journal record of the changed chunks beside the base at `path`, or as a
+        new base; checkpoint_wait retires it."""
+        buf = ctypes.create_string_buffer(bytes(extra), max(len(extra), 1))
+        self._ck(self.lib.dsm_checkpoint_enqueue_incremental(self.h, os.fsencode(path), buf if len(extra) else None, len(extra)))
+
+    def map_load_journal(self, path):
+        """map_load of the state base + journal resolve to: (extra bytes, records applied)."""
+        size, rec = ctypes.c_size_t(0), ctypes.c_int(0)
+        rc = self.lib.dsm_map_load_journal(self.h, os.fsencode(path), None, 0, ctypes.byref(size), ctypes.byref(rec))
+        if rc == -6 and size.value > 0:  # the size-then-read of the extra section: nothing was loaded yet
+            buf = ctypes.create_string_buffer(size.value)
+            self._ck(self.lib.dsm_map_load_journal(self.h, os.fsencode(path), buf, size.value, ctypes.byref(size), ctypes.byref(rec)))
+            return buf.raw[:size.value], rec.value
+        self._ck(rc)
+        return b"", rec.value
+
     # ---- publishing from inside the stream ----
     def publish_enable(self):
         self._ck(self.lib.dsm_publish_enable(self.h))
@@ -615,6 +638,22 @@ def map_peek(path):
     seg = np.zeros((max(ns.value, 1), 3), np.int32)
     _ck_io(L.dsm_map_peek(os.fsencode(path), extra, ne.value, None, _ptr(seg), ns.value, None), path)
     return extra.raw[:ne.value], seg[:ns.value].copy()
+
+
+def map_peek_journal(path):
+    """(extra bytes, segment table [n, 3], records applied) of the state base + journal resolve to, without a context."""
+    L = load_library()
+    ne, ns, rec = ctypes.c_size_t(0), ctypes.c_int(0), ctypes.c_int(0)
+    _ck_io(L.dsm_map_peek_journal(os.fsencode(path), None, 0, ctypes.byref(ne), None, 0, ctypes.byref(ns), None), path)
+    extra = ctypes.create_string_buffer(max(ne.value, 1))
+    seg = np.zeros((max(ns.value, 1), 3), np.int32)
+    _ck_io(L.dsm_map_peek_journal(os.fsencode(path), extra, ne.value, None, _ptr(seg), ns.value, None, ctypes.byref(rec)), path)
+    return extra.raw[:ne.value], seg[:ns.value].copy(), rec.value
+
+
+def journal_materialize(path, out_path):
+    """The version-1 checkpoint file of the state base + journal resolve to, written to out_path."""
+    _ck_io(load_library().dsm_journal_materialize(os.fsencode(path), os.fsencode(out_path)), path)
 
 
 def mesh_vertices(surfels):

@@ -633,6 +633,7 @@ extern "C" int dsm_set_constants(dsm_ctx *ctx, const dsm_constants *k)
     CK(cudaStreamSynchronize(ctx->stream));
     ctx->graphs.clear(); // captured schedules embed the kernel parameters
     apply_constants(ctx->d, *k);
+    dsm_checkpoint_map_replaced(ctx); // an incremental checkpoint's base carries the constants
     return DSM_OK;
 }
 
@@ -1316,6 +1317,7 @@ extern "C" int dsm_inactive_load(dsm_ctx *ctx, const dsm_surfel_t *surfels, int 
     rc = res_enter(ctx, NEED_STORE);
     if (rc != DSM_OK) return rc;
     InactStore &s = *ctx->inact;
+    dsm_checkpoint_map_replaced(ctx);
     std::vector<int4> table((size_t)n_segments);
     for (int i = 0; i < n_segments; i++) table[i] = make_int4(kf_ofs_cnt[3 * i], kf_ofs_cnt[3 * i + 1], kf_ofs_cnt[3 * i + 2], 0);
     const int32_t hdr[4] = {n, n_segments, 0, 0};
@@ -1424,23 +1426,70 @@ static cudaError_t checkpoint_images(dsm_ctx *ctx)
     DsmCheckpoint &k = *ctx->ckpt;
     k.img.reset();
     k.dev = k.host = k.host_dev = nullptr;
+    k.stale = true;
     auto own = std::make_unique<CudaOwner>();
-    const DsmSnapLayout lay = dsm_snap_layout(ctx->p.max_local_surfels, ctx->inact ? ctx->inact->cap : 0);
+    const int store_cap = ctx->inact ? ctx->inact->cap : 0;
+    const DsmSnapLayout lay = dsm_snap_layout(ctx->p.max_local_surfels, store_cap);
+    const int pool_chunks = std::max(dsm_snap_chunks(ctx->p.max_local_surfels), 1), store_chunks = dsm_snap_chunks(store_cap);
+    const size_t bytes = lay.bytes + dsm_line_up((size_t)pool_chunks + store_chunks); // k_map_delta's flags follow the image
     uint8_t *dev = nullptr, *host = nullptr, *host_dev = nullptr;
-    // not zeroed: the drain also copies the unused tail of each section's last line, which the writer never reads
-    cudaError_t e = own->device(&dev, lay.bytes);
-    if (e == cudaSuccess) e = own->mapped(&host, &host_dev, lay.bytes);
+    // not zeroed but for the header line (k_map_delta's count of finished CTAs): the drain also copies the unused tail of
+    // each section's last line, which the writer never reads
+    cudaError_t e = own->device(&dev, bytes);
+    if (e == cudaSuccess) e = cudaMemsetAsync(dev, 0, 128, ctx->stream); // ordered before the first snapshot
+    if (e == cudaSuccess) e = own->mapped(&host, &host_dev, bytes);
     if (e != cudaSuccess) return e;
     k.img = std::move(own);
     k.lay = lay;
+    k.pool_chunks = pool_chunks, k.store_chunks = store_chunks;
     k.dev = dev, k.host = host, k.host_dev = host_dev;
     return cudaSuccess;
+}
+
+void dsm_checkpoint_map_replaced(dsm_ctx *ctx)
+{
+    if (ctx && ctx->ckpt) ctx->ckpt->stale = true;
+}
+
+// An incremental checkpoint on the checkpoint's thread (DESIGN.md §8.6): a base writes the file and a fresh journal
+// header, a record lists the chunks k_map_delta flagged and appends them with the table and extra.  The chain ends on any
+// failure, so that the next incremental checkpoint writes a base.
+static int checkpoint_write_incremental(DsmCheckpoint &k, const DsmMapSections &s)
+{
+    if (k.kind == DsmCheckpoint::BASE)
+    {
+        uint64_t sum = 0, bytes = 0, jbytes = 0;
+        int rc = dsm_map_write(k.path.c_str(), k.info, s, &sum, &bytes);
+        if (rc == DSM_OK) rc = dsm_journal_start(k.path.c_str(), sum, &jbytes);
+        if (rc != DSM_OK) return rc;
+        k.chain_path = k.path;
+        k.chain_sum = sum, k.sequence = 1, k.base_bytes = bytes, k.journal_bytes = jbytes;
+        return DSM_OK;
+    }
+    const uint8_t *flags = k.host + k.lay.bytes;
+    k.chunks.clear();
+    const int cp = dsm_snap_chunks(s.n_pool), cs = dsm_snap_chunks(s.n_store);
+    for (int c = 0; c < cp; c++)
+        if (flags[c]) k.chunks.push_back(c);
+    const int k_pool = (int)k.chunks.size();
+    for (int c = 0; c < cs; c++)
+        if (flags[k.pool_chunks + c]) k.chunks.push_back(c);
+    const DsmJournalRecord r{k.sequence, k.chain_sum, s.n_pool, s.n_store, s.n_segments, k.chunks.data(), k_pool,
+                             k.chunks.data() + k_pool, (int)k.chunks.size() - k_pool, k.host + k.lay.pool, k.host + k.lay.store,
+                             s.table, s.extra, s.extra_bytes};
+    uint64_t sum = 0, bytes = 0;
+    const int rc = dsm_journal_append(k.path.c_str(), k.journal_bytes, r, &sum, &bytes);
+    if (rc != DSM_OK) return rc;
+    k.chain_path = k.path;
+    k.chain_sum = sum, k.sequence++, k.journal_bytes += bytes;
+    return DSM_OK;
 }
 
 // The write of one enqueued checkpoint, on the checkpoint's thread: waits for the drain, then writes the host image's
 // sections through the file's one writer.  A snapshot that recorded a rejected frame writes nothing.
 static int checkpoint_write(DsmCheckpoint &k)
 {
+    if (k.kind != DsmCheckpoint::FULL) k.chain_path.clear(); // set again once the base or the record is on the disk
     if (cudaEventSynchronize(k.ev_drain) != cudaSuccess) return DSM_E_CUDA;
     const volatile int32_t *h = reinterpret_cast<const volatile int32_t *>(k.host);
     if (h[DSM_SNAP_ERR_TAG] != 0)
@@ -1452,7 +1501,8 @@ static int checkpoint_write(DsmCheckpoint &k)
                            reinterpret_cast<const dsm_surfel_t *>(k.host + k.lay.store), h[DSM_SNAP_N_STORE],
                            reinterpret_cast<const int32_t *>(k.host + k.lay.table), h[DSM_SNAP_N_SEGMENTS],
                            k.extra.data(), k.extra.size()};
-    return dsm_map_write(k.path.c_str(), k.info, s);
+    if (k.kind == DsmCheckpoint::FULL) return dsm_map_write(k.path.c_str(), k.info, s);
+    return checkpoint_write_incremental(k, s);
 }
 
 static void checkpoint_thread(DsmCheckpoint *k, int device)
@@ -1506,7 +1556,7 @@ extern "C" int dsm_checkpoint_enable(dsm_ctx *ctx)
 
 // Enqueue only, like dsm_publish_enqueue: the snapshot on the context's stream, the drain on the checkpoint's stream
 // after it, the write on the checkpoint's thread.  The view of the map has no gate: the snapshot records the error word.
-extern "C" int dsm_checkpoint_enqueue(dsm_ctx *ctx, const char *path, const void *extra, size_t extra_bytes)
+static int checkpoint_enqueue(dsm_ctx *ctx, const char *path, const void *extra, size_t extra_bytes, bool incremental)
 {
     if (!ctx || !path || (extra_bytes > 0 && !extra)) return DSM_E_INVALID;
     DsmCheckpoint *k = ctx->ckpt.get();
@@ -1519,13 +1569,26 @@ extern "C" int dsm_checkpoint_enqueue(dsm_ctx *ctx, const char *path, const void
     DsmMapInfo info;
     dsm_map_info(ctx, &info);
     const InactStore *s = ctx->inact.get();
+    // a record needs the image to hold the chain's last checkpoint, under this path, and a journal no larger than its
+    // base; the thread has retired the previous checkpoint, so its chain state is final here
+    DsmCheckpoint::Kind kind = DsmCheckpoint::FULL;
+    if (incremental)
+        kind = k->stale || k->chain_path != path || k->journal_bytes > k->base_bytes ? DsmCheckpoint::BASE : DsmCheckpoint::RECORD;
     // grids from the host bounds, clamped to the capacities: a caller that never synchronises keeps bounds that only grow
-    dsm_launch_map_snapshot(ctx->d.pool, ctx->res_ofs, std::min(ctx->res_upper, ctx->p.max_local_surfels), s ? s->surfels : nullptr,
-                            s ? s->seg : nullptr, ctx->win_hdr, s ? std::min(s->upper, s->cap) : 0, k->dev, k->lay, ctx->stream);
+    const int pool_upper = std::min(ctx->res_upper, ctx->p.max_local_surfels), store_upper = s ? std::min(s->upper, s->cap) : 0;
+    if (kind == DsmCheckpoint::RECORD)
+        dsm_launch_map_delta(ctx->d.pool, ctx->res_ofs, pool_upper, s ? s->surfels : nullptr, s ? s->seg : nullptr, ctx->win_hdr,
+                             store_upper, k->dev, k->lay, k->pool_chunks, ctx->stream);
+    else
+        dsm_launch_map_snapshot(ctx->d.pool, ctx->res_ofs, pool_upper, s ? s->surfels : nullptr, s ? s->seg : nullptr, ctx->win_hdr,
+                                store_upper, k->dev, k->lay, ctx->stream);
     CK(cudaGetLastError());
     CK(cudaEventRecord(k->ev_snap, ctx->stream));
     CK(cudaStreamWaitEvent(k->s_drain, k->ev_snap, 0));
-    dsm_launch_map_drain(k->dev, k->host_dev, k->lay, k->drain_ctas, k->s_drain);
+    if (kind == DsmCheckpoint::RECORD)
+        dsm_launch_map_drain_delta(k->dev, k->host_dev, k->lay, k->pool_chunks, k->store_chunks, k->drain_ctas, k->s_drain);
+    else
+        dsm_launch_map_drain(k->dev, k->host_dev, k->lay, k->drain_ctas, k->s_drain);
     CK(cudaGetLastError());
     CK(cudaEventRecord(k->ev_drain, k->s_drain));
     {
@@ -1533,11 +1596,24 @@ extern "C" int dsm_checkpoint_enqueue(dsm_ctx *ctx, const char *path, const void
         k->path = path;
         k->extra.assign(static_cast<const uint8_t *>(extra), static_cast<const uint8_t *>(extra) + extra_bytes);
         k->info = info;
+        k->kind = kind;
         k->queued = true;
     }
     k->cv.notify_all();
     k->pending = true;
+    k->stale = kind == DsmCheckpoint::FULL; // k_map_snapshot wrote the image for a file outside the chain
     return DSM_OK;
+}
+
+extern "C" int dsm_checkpoint_enqueue(dsm_ctx *ctx, const char *path, const void *extra, size_t extra_bytes)
+{
+    return checkpoint_enqueue(ctx, path, extra, extra_bytes, false);
+}
+
+// One chunk pass and a drain of the changed lines for a record; the map of k_map_snapshot for a base (DESIGN.md §8.6)
+extern "C" int dsm_checkpoint_enqueue_incremental(dsm_ctx *ctx, const char *path, const void *extra, size_t extra_bytes)
+{
+    return checkpoint_enqueue(ctx, path, extra, extra_bytes, true);
 }
 
 extern "C" int dsm_checkpoint_wait(dsm_ctx *ctx, int block, int *finished)

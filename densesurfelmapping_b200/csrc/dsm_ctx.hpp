@@ -132,15 +132,31 @@ struct DsmCheckpoint
     cudaStream_t s_drain = nullptr;
     cudaEvent_t ev_snap = nullptr, ev_drain = nullptr; // after k_map_snapshot on the context's stream, after k_map_drain
     int drain_ctas = DSM_DRAIN_CTAS;
+    int pool_chunks = 0, store_chunks = 0; // k_map_delta's flags after the image: one per 256-surfel chunk of each capacity
     bool pending = false; // enqueued and not yet retired by dsm_checkpoint_wait (caller's thread only)
+    // dsm_checkpoint_enqueue_incremental (DESIGN.md §8.6), caller's thread: the device image has been written by something
+    // other than the incremental chain since its last checkpoint (a full checkpoint, new images), or the map was replaced
+    // or its constants changed; the next incremental checkpoint is a base
+    bool stale = true;
     // the job, guarded by m: queued from dsm_checkpoint_enqueue until the thread has stored its result
     std::mutex m;
     std::condition_variable cv;
     bool queued = false, quit = false;
     int result = DSM_OK, err_frame = 0;
+    enum Kind
+    {
+        FULL,   // dsm_checkpoint_enqueue: the version-1 file
+        BASE,   // an incremental checkpoint that writes the file and a fresh journal header
+        RECORD, // an incremental checkpoint that appends one record to the journal
+    } kind = FULL;
     std::string path;
     std::vector<uint8_t> extra;
     DsmMapInfo info{};
+    // the incremental chain as the thread left it: the base under chain_path ("" when the last incremental checkpoint
+    // failed), the checksum of its last record (of the base without one), the next sequence number, and the two lengths
+    std::string chain_path;
+    uint64_t chain_sum = 0, sequence = 1, base_bytes = 0, journal_bytes = 0;
+    std::vector<int32_t> chunks; // the thread's list of changed chunks
     std::thread worker; // last: started once the members above exist
 
     ~DsmCheckpoint()

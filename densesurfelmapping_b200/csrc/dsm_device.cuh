@@ -250,3 +250,25 @@ void dsm_launch_map_snapshot(const dsm_surfel_t *pool, const int32_t *res, int p
 // on a fixed grid of `ctas` CTAs
 #define DSM_DRAIN_CTAS 8
 void dsm_launch_map_drain(const uint8_t *image, uint8_t *host_dev, const DsmSnapLayout &lay, int ctas, cudaStream_t s);
+
+// dsm_checkpoint_enqueue_incremental (DESIGN.md §8.6) keeps the same image, with one flag byte per 256-surfel chunk after
+// it: at lay.bytes, pool_chunks flags for the pool, then store_chunks for the store (one per chunk of each capacity).
+// k_map_delta adds these words to the header line; DSM_DELTA_DONE is 0 between passes (the image's header line starts
+// zeroed, and k_map_snapshot leaves these words alone).
+enum
+{
+    DSM_DELTA_PREV_POOL = DSM_SNAP_WORDS, // the image's pool size before the pass, and
+    DSM_DELTA_PREV_STORE,                 // its store size
+    DSM_DELTA_DONE,                       // CTAs of the pass that have finished
+    DSM_DELTA_WORDS
+};
+#define DSM_SNAP_CHUNK 256
+inline int dsm_snap_chunks(int cap) { return (cap + DSM_SNAP_CHUNK - 1) / DSM_SNAP_CHUNK; }
+// k_map_delta: k_map_snapshot's grid and chunks, written only where the live map differs from the image (or reaches beyond
+// the image's size of the section); every live CTA sets its chunk's flag to 1 if it wrote it, else 0.  The table and the
+// header are written whole.
+void dsm_launch_map_delta(const dsm_surfel_t *pool, const int32_t *res, int pool_upper, const dsm_surfel_t *store, const int4 *seg,
+                          const int32_t *hdr, int store_upper, uint8_t *image, const DsmSnapLayout &lay, int pool_chunks, cudaStream_t s);
+// k_map_drain_delta: the header line, the flag lines, the live table lines and the live lines of the flagged chunks only
+void dsm_launch_map_drain_delta(const uint8_t *image, uint8_t *host_dev, const DsmSnapLayout &lay, int pool_chunks, int store_chunks,
+                                int ctas, cudaStream_t s);

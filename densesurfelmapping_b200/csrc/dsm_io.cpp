@@ -207,6 +207,22 @@ struct Fnv1a
     }
 };
 
+// A whole file into `raw`: DSM_E_IO if it cannot be opened or read
+int read_all(const char *path, std::vector<uint8_t> &raw)
+{
+    FILE *f = std::fopen(path, "rb");
+    if (!f) return DSM_E_IO;
+    long len = -1;
+    if (std::fseek(f, 0, SEEK_END) == 0) len = std::ftell(f);
+    if (len >= 0 && std::fseek(f, 0, SEEK_SET) == 0)
+    {
+        raw.resize((size_t)len);
+        if (len > 0 && std::fread(raw.data(), 1, (size_t)len, f) != (size_t)len) len = -1;
+    }
+    std::fclose(f);
+    return len < 0 ? DSM_E_IO : DSM_OK;
+}
+
 // A checkpoint read whole and checked: magic and version (DSM_E_INVALID), then its length and checksum (DSM_E_IO)
 struct MapFile
 {
@@ -218,17 +234,12 @@ struct MapFile
 
     int read(const char *path)
     {
-        FILE *f = std::fopen(path, "rb");
-        if (!f) return DSM_E_IO;
-        long len = -1;
-        if (std::fseek(f, 0, SEEK_END) == 0) len = std::ftell(f);
-        if (len >= 0 && std::fseek(f, 0, SEEK_SET) == 0)
-        {
-            raw.resize((size_t)len);
-            if (len > 0 && std::fread(raw.data(), 1, (size_t)len, f) != (size_t)len) len = -1;
-        }
-        std::fclose(f);
-        if (len < 0) return DSM_E_IO;
+        const int rc = read_all(path, raw);
+        return rc != DSM_OK ? rc : parse();
+    }
+    // the checks of read() on the bytes in `raw`
+    int parse()
+    {
         if (raw.size() < 16) return DSM_E_IO;
         std::memcpy(&hdr, raw.data(), std::min(raw.size(), sizeof(hdr)));
         if (std::memcmp(hdr.magic, kMapMagic, 8) != 0 || hdr.format != kMapFormat) return DSM_E_INVALID;
@@ -256,6 +267,7 @@ struct AtomicFile
     std::string path, tmp;
     FILE *f = nullptr;
     Fnv1a sum;
+    uint64_t bytes = 0; // written so far
     bool ok = true, created = false, renamed = false;
 
     explicit AtomicFile(const char *p) : path(p), tmp(std::string(p) + ".tmp." + std::to_string((long)getpid()))
@@ -276,6 +288,7 @@ struct AtomicFile
         if (!ok || n == 0) return;
         sum.add(p, n);
         ok = std::fwrite(p, 1, n, f) == n;
+        bytes += n;
     }
     bool commit()
     {
@@ -325,7 +338,7 @@ extern "C" int dsm_map_save(dsm_ctx *ctx, const char *path, const void *extra, s
     return dsm_map_write(path, info, DsmMapSections{pool.data(), n_pool, store.data(), n_store, table.data(), n_seg, extra, extra_bytes});
 }
 
-int dsm_map_write(const char *path, const DsmMapInfo &info, const DsmMapSections &s)
+int dsm_map_write(const char *path, const DsmMapInfo &info, const DsmMapSections &s, uint64_t *checksum, uint64_t *bytes)
 {
     MapHeader h;
     std::memset(&h, 0, sizeof(h));
@@ -344,17 +357,19 @@ int dsm_map_write(const char *path, const DsmMapInfo &info, const DsmMapSections
     out.put(s.store, (size_t)s.n_store * sizeof(dsm_surfel_t));
     out.put(s.table, (size_t)s.n_segments * 12);
     out.put(s.extra, s.extra_bytes);
-    return out.commit() ? DSM_OK : DSM_E_IO;
+    const uint64_t sum = out.sum.h;
+    if (!out.commit()) return DSM_E_IO;
+    if (checksum) *checksum = sum;
+    if (bytes) *bytes = out.bytes;
+    return DSM_OK;
 }
 
-extern "C" int dsm_map_load(dsm_ctx *ctx, const char *path, void *extra, size_t extra_cap, size_t *extra_bytes)
+
+namespace
 {
-    if (!ctx || !path || (extra_cap > 0 && !extra)) return DSM_E_INVALID;
-    DsmMapInfo info;
-    int rc = dsm_map_info(ctx, &info);
-    MapFile m;
-    if (rc == DSM_OK) rc = m.read(path);
-    if (rc != DSM_OK) return rc;
+// The checks and the load of dsm_map_load on a file already read and checked
+int load_checked(dsm_ctx *ctx, const DsmMapInfo &info, const MapFile &m, void *extra, size_t extra_cap, size_t *extra_bytes)
+{
     const MapHeader &h = m.hdr;
     const dsm_params &p = info.params;
     const float geo[6] = {p.fx, p.fy, p.cx, p.cy, p.fuse_far, p.fuse_near};
@@ -363,6 +378,7 @@ extern "C" int dsm_map_load(dsm_ctx *ctx, const char *path, void *extra, size_t 
         return DSM_E_INVALID; // the caller sets the constants before loading
     if (h.n_pool > p.max_local_surfels) return DSM_E_CAPACITY;
     if (info.publish_in_flight) return DSM_E_STATE;
+    int rc = DSM_OK;
     if (info.store_cap == 0)
     {
         if (h.n_store > 0) return DSM_E_STATE;
@@ -375,11 +391,34 @@ extern "C" int dsm_map_load(dsm_ctx *ctx, const char *path, void *extra, size_t 
     }
     if (extra_bytes) *extra_bytes = (size_t)h.extra_bytes;
     if (h.extra_bytes > extra_cap) return DSM_E_CAPACITY;
+    dsm_checkpoint_map_replaced(ctx);
     rc = dsm_pool_upload(ctx, m.pool, h.n_pool);
     if (rc == DSM_OK && info.store_cap > 0) rc = dsm_inactive_load(ctx, m.store, h.n_store, m.table, h.n_segments);
     if (rc != DSM_OK) return rc;
     if (h.extra_bytes > 0) std::memcpy(extra, m.extra, (size_t)h.extra_bytes);
     return DSM_OK;
+}
+
+// What dsm_map_peek returns of a file already read and checked
+void peek_checked(const MapFile &m, void *extra, size_t extra_cap, size_t *extra_bytes, int32_t *kf_ofs_cnt, int seg_cap,
+                  int *n_segments)
+{
+    if (extra_bytes) *extra_bytes = (size_t)m.hdr.extra_bytes;
+    if (n_segments) *n_segments = m.hdr.n_segments;
+    if (extra_cap > 0) std::memcpy(extra, m.extra, (size_t)std::min<uint64_t>(extra_cap, m.hdr.extra_bytes));
+    if (seg_cap > 0) std::memcpy(kf_ofs_cnt, m.table, (size_t)std::min(seg_cap, m.hdr.n_segments) * 12);
+}
+} // namespace
+
+extern "C" int dsm_map_load(dsm_ctx *ctx, const char *path, void *extra, size_t extra_cap, size_t *extra_bytes)
+{
+    if (!ctx || !path || (extra_cap > 0 && !extra)) return DSM_E_INVALID;
+    DsmMapInfo info;
+    int rc = dsm_map_info(ctx, &info);
+    MapFile m;
+    if (rc == DSM_OK) rc = m.read(path);
+    if (rc != DSM_OK) return rc;
+    return load_checked(ctx, info, m, extra, extra_cap, extra_bytes);
 }
 
 extern "C" int dsm_map_peek(const char *path, void *extra, size_t extra_cap, size_t *extra_bytes, int32_t *kf_ofs_cnt, int seg_cap,
@@ -389,9 +428,250 @@ extern "C" int dsm_map_peek(const char *path, void *extra, size_t extra_cap, siz
     MapFile m;
     const int rc = m.read(path);
     if (rc != DSM_OK) return rc;
-    if (extra_bytes) *extra_bytes = (size_t)m.hdr.extra_bytes;
-    if (n_segments) *n_segments = m.hdr.n_segments;
-    if (extra_cap > 0) std::memcpy(extra, m.extra, (size_t)std::min<uint64_t>(extra_cap, m.hdr.extra_bytes));
-    if (seg_cap > 0) std::memcpy(kf_ofs_cnt, m.table, (size_t)std::min(seg_cap, m.hdr.n_segments) * 12);
+    peek_checked(m, extra, extra_cap, extra_bytes, kf_ofs_cnt, seg_cap, n_segments);
     return DSM_OK;
+}
+
+// ---- the journal of incremental checkpoints (DESIGN.md §8.6) ----
+// <path> is a version-1 file, the base; <path>.journal holds, all fields little-endian:
+//    0  char magic[8] "DSMJRNL\0"    8  uint32 format version    12  uint32 0    16  uint64 the base's trailing checksum
+//   24  uint64 FNV-1a 64 of the 24 bytes before it
+// then records, each:
+//    0  uint64 sequence (1 for the first record after the base)    8  int32 n_pool, n_store, n_segments
+//   20  int32 k_pool, k_store (chunks listed)    28  uint32 0    32  uint64 extra_bytes
+//   40  int32 pool_chunk[k_pool], int32 store_chunk[k_store]: ascending indices of the 256-surfel chunks that changed
+//       the payloads, in list order: min(256, n - 256 c) dsm_surfel_t of each chunk c (the pool's, then the store's)
+//       int32 table[n_segments][3], uint8 extra[extra_bytes] (both whole)
+//       uint64 the checksum of the previous record (of the base for the first)
+//       uint64 FNV-1a 64 of every byte of the record before it
+// A record holds every chunk that reaches beyond the previous state's size of its section.  The base is written first
+// (temporary name, rename), then a fresh journal header the same way; a record is appended and flushed to the disk.
+namespace
+{
+const char kJournalMagic[8] = {'D', 'S', 'M', 'J', 'R', 'N', 'L', 0};
+const uint32_t kJournalFormat = 1;
+
+struct JournalHeader
+{
+    char magic[8];
+    uint32_t format, zero;
+    uint64_t base_checksum;
+};
+static_assert(sizeof(JournalHeader) == 24, "journal header layout");
+
+struct RecordHeader
+{
+    uint64_t sequence;
+    int32_t n_pool, n_store, n_segments, k_pool, k_store;
+    uint32_t zero;
+    uint64_t extra_bytes;
+};
+static_assert(sizeof(RecordHeader) == 40, "journal record layout");
+
+const int64_t kChunk = 256;
+const size_t kChunkBytes = kChunk * sizeof(dsm_surfel_t);
+
+std::string journal_path(const char *path) { return std::string(path) + ".journal"; }
+int64_t chunks_of(int64_t n) { return (n + kChunk - 1) / kChunk; }
+// surfels of chunk c of a section of n, 0 for a chunk outside it
+int64_t chunk_count(int64_t n, int64_t c) { return c < 0 || c * kChunk >= n ? 0 : std::min(kChunk, n - c * kChunk); }
+
+// A record's chunk list for a section of n surfels that held `prev` before it: ascending, inside the section, and
+// holding every chunk that reaches beyond prev
+bool list_ok(const int32_t *c, int k, int64_t n, int64_t prev)
+{
+    for (int i = 0; i < k; i++)
+        if (c[i] < 0 || c[i] >= chunks_of(n) || (i > 0 && c[i] <= c[i - 1])) return false;
+    if (n <= prev) return true;
+    const int64_t need = chunks_of(n) - prev / kChunk; // chunks prev / 256 .. the last, which the list must end with
+    return k >= need && c[k - need] == prev / kChunk;
+}
+
+// The one resolver: the base read and checked as dsm_map_load reads it, then the records of its journal replayed in
+// order up to the first that is torn, fails its checksum, breaks the chain or is out of sequence.  m holds the version-1
+// file of the resulting state, parsed as a read file is.  A missing journal, or one that names another base, adds no
+// record; a journal of another magic or format is DSM_E_INVALID, and so is a complete record whose chunk lists do not
+// describe its state.
+int resolve(const char *path, MapFile &m, int *records)
+{
+    if (records) *records = 0;
+    int rc = m.read(path);
+    if (rc != DSM_OK) return rc;
+    std::vector<uint8_t> j;
+    if (read_all(journal_path(path).c_str(), j) != DSM_OK || j.size() < sizeof(JournalHeader) + 8) return DSM_OK;
+    JournalHeader jh;
+    std::memcpy(&jh, j.data(), sizeof(jh));
+    if (std::memcmp(jh.magic, kJournalMagic, 8) != 0 || jh.format != kJournalFormat) return DSM_E_INVALID;
+    Fnv1a hs;
+    hs.add(j.data(), sizeof(jh));
+    uint64_t want = 0, chain = 0;
+    std::memcpy(&want, j.data() + sizeof(jh), 8);
+    std::memcpy(&chain, m.raw.data() + m.raw.size() - 8, 8);
+    if (hs.h != want || jh.base_checksum != chain) return DSM_OK;
+
+    MapHeader hdr = m.hdr;
+    const uint8_t *mp = reinterpret_cast<const uint8_t *>(m.pool), *ms = reinterpret_cast<const uint8_t *>(m.store);
+    std::vector<uint8_t> pool(mp, mp + (size_t)hdr.n_pool * sizeof(dsm_surfel_t));
+    std::vector<uint8_t> store(ms, ms + (size_t)hdr.n_store * sizeof(dsm_surfel_t));
+    std::vector<uint8_t> table(reinterpret_cast<const uint8_t *>(m.table), m.extra);
+    std::vector<uint8_t> extra(m.extra, m.extra + hdr.extra_bytes);
+    std::vector<int32_t> list;
+    int applied = 0;
+    size_t pos = sizeof(JournalHeader) + 8;
+    for (uint64_t seq = 1; pos < j.size(); seq++)
+    {
+        const uint8_t *p = j.data() + pos;
+        const uint64_t left = j.size() - pos;
+        RecordHeader r;
+        if (left < sizeof(r)) break;
+        std::memcpy(&r, p, sizeof(r));
+        if (r.n_pool < 0 || r.n_store < 0 || r.n_segments < 0 || r.k_pool < 0 || r.k_store < 0) break;
+        const uint64_t lists = 4 * ((uint64_t)r.k_pool + (uint64_t)r.k_store);
+        if (r.extra_bytes > left || sizeof(r) + lists > left) break;
+        list.resize((size_t)r.k_pool + r.k_store);
+        if (!list.empty()) std::memcpy(list.data(), p + sizeof(r), (size_t)lists);
+        uint64_t payload = 0;
+        for (size_t i = 0; i < list.size(); i++)
+            payload += (uint64_t)chunk_count((int)i < r.k_pool ? r.n_pool : r.n_store, list[i]) * sizeof(dsm_surfel_t);
+        const uint64_t len = sizeof(r) + lists + payload + 12 * (uint64_t)r.n_segments + r.extra_bytes + 16;
+        if (len > left) break; // torn
+        Fnv1a s;
+        s.add(p, (size_t)len - 8);
+        uint64_t own = 0, prev = 0;
+        std::memcpy(&prev, p + len - 16, 8);
+        std::memcpy(&own, p + len - 8, 8);
+        if (s.h != own || prev != chain || r.sequence != seq) break;
+        if (!list_ok(list.data(), r.k_pool, r.n_pool, hdr.n_pool) || !list_ok(list.data() + r.k_pool, r.k_store, r.n_store, hdr.n_store))
+            return DSM_E_INVALID;
+        const uint8_t *q = p + sizeof(r) + lists;
+        pool.resize((size_t)r.n_pool * sizeof(dsm_surfel_t));
+        store.resize((size_t)r.n_store * sizeof(dsm_surfel_t));
+        for (size_t i = 0; i < list.size(); i++)
+        {
+            const bool in_pool = (int)i < r.k_pool;
+            const size_t n = (size_t)chunk_count(in_pool ? r.n_pool : r.n_store, list[i]) * sizeof(dsm_surfel_t);
+            std::memcpy((in_pool ? pool : store).data() + (size_t)list[i] * kChunkBytes, q, n);
+            q += n;
+        }
+        table.assign(q, q + 12 * (size_t)r.n_segments);
+        q += table.size();
+        extra.assign(q, q + r.extra_bytes);
+        hdr.n_pool = r.n_pool, hdr.n_store = r.n_store, hdr.n_segments = r.n_segments, hdr.extra_bytes = r.extra_bytes;
+        chain = own;
+        pos += (size_t)len;
+        applied++;
+    }
+    if (applied == 0) return DSM_OK;
+    std::vector<uint8_t> raw;
+    raw.reserve(sizeof(hdr) + pool.size() + store.size() + table.size() + extra.size() + 8);
+    const uint8_t *hb = reinterpret_cast<const uint8_t *>(&hdr);
+    raw.insert(raw.end(), hb, hb + sizeof(hdr));
+    for (const std::vector<uint8_t> *v : {&pool, &store, &table, &extra}) raw.insert(raw.end(), v->begin(), v->end());
+    Fnv1a sum;
+    sum.add(raw.data(), raw.size());
+    const uint8_t *sb = reinterpret_cast<const uint8_t *>(&sum.h);
+    raw.insert(raw.end(), sb, sb + 8);
+    m.raw = std::move(raw);
+    rc = m.parse();
+    if (rc == DSM_OK && records) *records = applied;
+    return rc;
+}
+} // namespace
+
+int dsm_journal_start(const char *path, uint64_t base_checksum, uint64_t *bytes)
+{
+    JournalHeader h;
+    std::memset(&h, 0, sizeof(h));
+    std::memcpy(h.magic, kJournalMagic, 8);
+    h.format = kJournalFormat;
+    h.base_checksum = base_checksum;
+    AtomicFile out(journal_path(path).c_str());
+    out.put(&h, sizeof(h));
+    if (!out.commit()) return DSM_E_IO;
+    *bytes = out.bytes;
+    return DSM_OK;
+}
+
+int dsm_journal_append(const char *path, uint64_t journal_bytes, const DsmJournalRecord &r, uint64_t *checksum, uint64_t *bytes)
+{
+    const int fd = ::open(journal_path(path).c_str(), O_WRONLY);
+    if (fd < 0) return DSM_E_IO;
+    struct stat st;
+    FILE *f = nullptr;
+    if (fstat(fd, &st) == 0 && (uint64_t)st.st_size == journal_bytes && lseek(fd, 0, SEEK_END) >= 0) f = fdopen(fd, "wb");
+    if (!f)
+    { // the journal is not the one the chain ends with
+        ::close(fd);
+        return DSM_E_IO;
+    }
+    Fnv1a sum;
+    uint64_t n = 0;
+    bool ok = true;
+    auto put = [&](const void *p, size_t len) {
+        if (!ok || len == 0) return;
+        sum.add(p, len);
+        ok = std::fwrite(p, 1, len, f) == len;
+        n += len;
+    };
+    RecordHeader h;
+    std::memset(&h, 0, sizeof(h));
+    h.sequence = r.sequence;
+    h.n_pool = r.n_pool, h.n_store = r.n_store, h.n_segments = r.n_segments, h.k_pool = r.k_pool, h.k_store = r.k_store;
+    h.extra_bytes = r.extra_bytes;
+    put(&h, sizeof(h));
+    put(r.pool_chunks, 4 * (size_t)r.k_pool);
+    put(r.store_chunks, 4 * (size_t)r.k_store);
+    for (int i = 0; i < r.k_pool; i++)
+        put(r.pool + (size_t)r.pool_chunks[i] * kChunkBytes, (size_t)chunk_count(r.n_pool, r.pool_chunks[i]) * sizeof(dsm_surfel_t));
+    for (int i = 0; i < r.k_store; i++)
+        put(r.store + (size_t)r.store_chunks[i] * kChunkBytes, (size_t)chunk_count(r.n_store, r.store_chunks[i]) * sizeof(dsm_surfel_t));
+    put(r.table, 12 * (size_t)r.n_segments);
+    put(r.extra, r.extra_bytes);
+    put(&r.prev_checksum, 8);
+    const uint64_t own = sum.h;
+    put(&own, 8);
+    ok = ok && std::fflush(f) == 0 && fsync(fileno(f)) == 0;
+    if (!ok && ftruncate(fileno(f), (off_t)journal_bytes) == 0) fsync(fileno(f)); // a torn tail would end every replay
+    ok = std::fclose(f) == 0 && ok;
+    if (!ok) return DSM_E_IO;
+    *checksum = own;
+    *bytes = n;
+    return DSM_OK;
+}
+
+extern "C" int dsm_map_load_journal(dsm_ctx *ctx, const char *path, void *extra, size_t extra_cap, size_t *extra_bytes, int *records)
+{
+    if (records) *records = 0;
+    if (!ctx || !path || (extra_cap > 0 && !extra)) return DSM_E_INVALID;
+    DsmMapInfo info;
+    int rc = dsm_map_info(ctx, &info);
+    MapFile m;
+    int n = 0;
+    if (rc == DSM_OK) rc = resolve(path, m, &n);
+    if (rc == DSM_OK) rc = load_checked(ctx, info, m, extra, extra_cap, extra_bytes);
+    if (rc == DSM_OK && records) *records = n;
+    return rc;
+}
+
+extern "C" int dsm_map_peek_journal(const char *path, void *extra, size_t extra_cap, size_t *extra_bytes, int32_t *kf_ofs_cnt,
+                                    int seg_cap, int *n_segments, int *records)
+{
+    if (records) *records = 0;
+    if (!path || (extra_cap > 0 && !extra) || seg_cap < 0 || (seg_cap > 0 && !kf_ofs_cnt)) return DSM_E_INVALID;
+    MapFile m;
+    const int rc = resolve(path, m, records);
+    if (rc != DSM_OK) return rc;
+    peek_checked(m, extra, extra_cap, extra_bytes, kf_ofs_cnt, seg_cap, n_segments);
+    return DSM_OK;
+}
+
+extern "C" int dsm_journal_materialize(const char *path, const char *out_path)
+{
+    if (!path || !out_path) return DSM_E_INVALID;
+    MapFile m;
+    const int rc = resolve(path, m, nullptr);
+    if (rc != DSM_OK) return rc;
+    AtomicFile out(out_path);
+    out.put(m.raw.data(), m.raw.size() - 8); // commit appends the same checksum
+    return out.commit() ? DSM_OK : DSM_E_IO;
 }

@@ -1140,6 +1140,114 @@ __global__ void __launch_bounds__(DRAIN_BLOCK) k_map_drain(const uint8_t *image,
 }
 
 // -------------------------------------------------------------------------------------------
+// k_map_delta — the map of dsm_checkpoint_enqueue_incremental at its position in the stream, into the same device image,
+// which already holds the map of the last checkpoint (DESIGN.md §8.6).  k_map_snapshot's grid and chunks: CTA c <
+// pool_grid stages pool chunk c, CTA pool_grid + c store chunk c (and writes the segments with the same indices), each
+// staged like k_pool_transform's.  A chunk is changed if one of its live words differs from the image's, or if it
+// reaches beyond the image's size of its section (k_map_snapshot writes nothing past the live sizes); only a changed
+// chunk is written into the image.  Each live CTA writes its chunk's flag, so the set of flags depends on the two maps
+// alone.  The image's sizes are read at the start of every CTA; the last CTA to finish rewrites the header (new sizes,
+// previous sizes, error word) once every other has read them.  Launched without PDL, like k_map_snapshot.
+// -------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(SNAP_CHUNK) k_map_delta(const dsm_surfel_t *pool, const int32_t *res, int pool_grid,
+                                                          const dsm_surfel_t *store, const int4 *seg, const int32_t *hdr,
+                                                          uint8_t *image, const DsmSnapLayout lay, int pool_chunks)
+{
+    __shared__ alignas(128) float sm[SNAP_CHUNK * 11];
+    __shared__ uint64_t bar;
+    __shared__ bool s_last;
+    int32_t *h = reinterpret_cast<int32_t *>(image);
+    const int n_pool = res[1], n_store = store ? hdr[0] : 0, n_seg = store ? hdr[1] : 0;
+    const bool in_pool = (int)blockIdx.x < pool_grid;
+    const int c = in_pool ? blockIdx.x : blockIdx.x - pool_grid, first = c * SNAP_CHUNK;
+    const int n = in_pool ? n_pool : n_store;
+    const int prev = h[in_pool ? DSM_SNAP_N_POOL : DSM_SNAP_N_STORE];
+    bool changed = false;
+    if (first < n)
+    {
+        const int cnt = min(SNAP_CHUNK, n - first);
+        if (!in_pool && first + (int)threadIdx.x < n_seg)
+        {
+            const int i = first + threadIdx.x;
+            const int4 g = seg[i];
+            int32_t *t = reinterpret_cast<int32_t *>(image + lay.table) + 3 * (size_t)i;
+            t[0] = g.x, t[1] = g.y, t[2] = g.z;
+        }
+        const float *src = reinterpret_cast<const float *>((in_pool ? pool : store) + first);
+        float *dst = reinterpret_cast<float *>(image + (in_pool ? lay.pool : lay.store)) + (size_t)first * 11;
+        const bool bulk = stage_in(sm, src, cnt, &bar, SNAP_CHUNK);
+        bool differs = first + cnt > prev;
+        if (!differs)
+        {
+            const uint32_t *old = reinterpret_cast<const uint32_t *>(dst);
+            for (int i = threadIdx.x; i < cnt * 11; i += SNAP_CHUNK) differs |= __float_as_uint(sm[i]) != old[i];
+        }
+        changed = __syncthreads_or(differs);
+        if (changed) stage_out(dst, sm, cnt, bulk, SNAP_CHUNK);
+    }
+    if (threadIdx.x == 0) image[lay.bytes + (in_pool ? c : pool_chunks + c)] = changed ? 1 : 0;
+    __syncthreads();
+    if (threadIdx.x == 0)
+    {
+        __threadfence();
+        s_last = atomicAdd(&h[DSM_DELTA_DONE], 1) == (int)gridDim.x - 1;
+    }
+    __syncthreads();
+    if (!s_last || threadIdx.x != 0) return;
+    __threadfence();
+    volatile int32_t *v = h;
+    v[DSM_DELTA_PREV_POOL] = v[DSM_SNAP_N_POOL];
+    v[DSM_DELTA_PREV_STORE] = v[DSM_SNAP_N_STORE];
+    v[DSM_SNAP_N_POOL] = n_pool;
+    v[DSM_SNAP_N_STORE] = n_store;
+    v[DSM_SNAP_N_SEGMENTS] = n_seg;
+    v[DSM_SNAP_ERR_TAG] = res[2];
+    v[DSM_SNAP_ERR_FRAME] = res[3];
+    v[DSM_DELTA_DONE] = 0;
+}
+
+// -------------------------------------------------------------------------------------------
+// k_map_drain_delta — k_map_drain for k_map_delta's image: the header line, the flag lines and the live table lines
+// whole, then one warp per live chunk that copies the chunk's live 128-byte lines if its flag is set (a chunk of 256
+// surfels is 88 lines, and each section starts on a line).  The same small fixed grid as k_map_drain.
+// -------------------------------------------------------------------------------------------
+#define CHUNK_LINES (SNAP_CHUNK * 44 / 128)
+__global__ void __launch_bounds__(DRAIN_BLOCK) k_map_drain_delta(const uint8_t *image, uint8_t *host, const DsmSnapLayout lay,
+                                                                 int pool_chunks, int store_chunks)
+{
+    const int32_t *h = reinterpret_cast<const int32_t *>(image);
+    const int n_pool = h[DSM_SNAP_N_POOL], n_store = h[DSM_SNAP_N_STORE];
+    const size_t lp = ((size_t)n_pool * 44 + 127) / 128, ls = ((size_t)n_store * 44 + 127) / 128;
+    const size_t lt = ((size_t)h[DSM_SNAP_N_SEGMENTS] * 12 + 127) / 128, lf = ((size_t)pool_chunks + store_chunks + 127) / 128;
+    const size_t words = 8 * (1 + lf + lt);
+    for (size_t w = (size_t)blockIdx.x * DRAIN_BLOCK + threadIdx.x; w < words; w += (size_t)gridDim.x * DRAIN_BLOCK)
+    {
+        size_t line = w >> 3, ofs;
+        if (line == 0) ofs = 0;
+        else if ((line -= 1) < lf) ofs = lay.bytes + line * 128;
+        else ofs = lay.table + (line - lf) * 128;
+        ofs += (w & 7) * 16;
+        *reinterpret_cast<int4 *>(host + ofs) = __ldg(reinterpret_cast<const int4 *>(image + ofs));
+    }
+    const uint8_t *flags = image + lay.bytes;
+    const int cp = (n_pool + SNAP_CHUNK - 1) / SNAP_CHUNK, cs = (n_store + SNAP_CHUNK - 1) / SNAP_CHUNK;
+    const int warps = gridDim.x * (DRAIN_BLOCK / 32), lane = threadIdx.x & 31;
+    for (int q = blockIdx.x * (DRAIN_BLOCK / 32) + (threadIdx.x >> 5); q < cp + cs; q += warps)
+    {
+        const bool in_pool = q < cp;
+        const int c = in_pool ? q : q - cp;
+        if (!flags[in_pool ? c : pool_chunks + c]) continue;
+        const size_t base = in_pool ? lay.pool : lay.store, l0 = (size_t)c * CHUNK_LINES;
+        const size_t l1 = min(l0 + CHUNK_LINES, in_pool ? lp : ls);
+        for (size_t w = l0 * 8 + lane; w < l1 * 8; w += 32)
+        {
+            const size_t ofs = base + w * 16;
+            *reinterpret_cast<int4 *>(host + ofs) = __ldg(reinterpret_cast<const int4 *>(image + ofs));
+        }
+    }
+}
+
+// -------------------------------------------------------------------------------------------
 // parity readback: rebuild the reference's 60-byte Superpixel_seed records for one frame
 // -------------------------------------------------------------------------------------------
 __global__ void k_seeds_export(const __grid_constant__ DsmDev d, int b, dsm_seed_t *out, int raw_md)
@@ -1401,4 +1509,17 @@ void dsm_launch_map_snapshot(const dsm_surfel_t *pool, const int32_t *res, int p
 void dsm_launch_map_drain(const uint8_t *image, uint8_t *host_dev, const DsmSnapLayout &lay, int ctas, cudaStream_t s)
 {
     k_map_drain<<<ctas, DRAIN_BLOCK, 0, s>>>(image, host_dev, lay);
+}
+void dsm_launch_map_delta(const dsm_surfel_t *pool, const int32_t *res, int pool_upper, const dsm_surfel_t *store, const int4 *seg,
+                          const int32_t *hdr, int store_upper, uint8_t *image, const DsmSnapLayout &lay, int pool_chunks, cudaStream_t s)
+{
+    static_assert(DSM_SNAP_CHUNK == SNAP_CHUNK && DSM_DELTA_WORDS <= 32, "the image's chunks and header line");
+    const int pool_grid = std::max(dsm_snap_chunks(pool_upper), 1); // as k_map_snapshot's: CTA 0 exists
+    const int store_grid = store ? dsm_snap_chunks(store_upper) : 0;
+    k_map_delta<<<pool_grid + store_grid, SNAP_CHUNK, 0, s>>>(pool, res, pool_grid, store, seg, hdr, image, lay, pool_chunks);
+}
+void dsm_launch_map_drain_delta(const uint8_t *image, uint8_t *host_dev, const DsmSnapLayout &lay, int pool_chunks, int store_chunks,
+                                int ctas, cudaStream_t s)
+{
+    k_map_drain_delta<<<ctas, DRAIN_BLOCK, 0, s>>>(image, host_dev, lay, pool_chunks, store_chunks);
 }

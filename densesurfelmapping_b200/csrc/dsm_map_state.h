@@ -30,4 +30,31 @@ struct DsmMapSections
 };
 // The one writer of the file (dsm_io.cpp), for dsm_map_save and the checkpoint thread: header from `info`, the sections,
 // the checksum; under a temporary name, flushed to the disk and renamed over `path`.  DSM_E_IO leaves nothing under path.
-__attribute__((visibility("hidden"))) int dsm_map_write(const char *path, const DsmMapInfo &info, const DsmMapSections &s);
+// *checksum / *bytes (optional): the file's trailing checksum and its length.
+__attribute__((visibility("hidden"))) int dsm_map_write(const char *path, const DsmMapInfo &info, const DsmMapSections &s,
+                                                        uint64_t *checksum = nullptr, uint64_t *bytes = nullptr);
+
+// The journal beside a base file (dsm_checkpoint_enqueue_incremental, DESIGN.md §8.6).  dsm_journal_start replaces
+// <path>.journal by a header that names the base's checksum (temporary name, fsync, rename); *bytes is its length.
+__attribute__((visibility("hidden"))) int dsm_journal_start(const char *path, uint64_t base_checksum, uint64_t *bytes);
+// One record: the chunks of 256 surfels that changed since the previous state, in ascending order, each section's chunk c
+// read at 11264 * c bytes from its base (the last chunk of a section cut at its size), then the whole table and extra.
+struct DsmJournalRecord
+{
+    uint64_t sequence, prev_checksum;
+    int n_pool, n_store, n_segments;
+    const int32_t *pool_chunks; // [k_pool]
+    int k_pool;
+    const int32_t *store_chunks; // [k_store]
+    int k_store;
+    const uint8_t *pool, *store;
+    const int32_t *table;
+    const void *extra;
+    size_t extra_bytes;
+};
+// Appends the record to <path>.journal, which must be `journal_bytes` long, and flushes it to the disk.  DSM_E_IO leaves
+// the journal at its old length as far as it can.  *checksum / *bytes: the record's own checksum and its length.
+__attribute__((visibility("hidden"))) int dsm_journal_append(const char *path, uint64_t journal_bytes, const DsmJournalRecord &r,
+                                                             uint64_t *checksum, uint64_t *bytes);
+// dsm_map_load and dsm_inactive_load tell the checkpoint that the map was replaced: the next incremental one is a base
+__attribute__((visibility("hidden"))) void dsm_checkpoint_map_replaced(dsm_ctx *ctx);

@@ -483,6 +483,34 @@ int dsm_checkpoint_enqueue(dsm_ctx *ctx, const char *path, const void *extra, si
 int dsm_checkpoint_wait(dsm_ctx *ctx, int block, int *finished);
 int dsm_debug_checkpoint_drain_ctas(dsm_ctx *ctx, int ctas);
 
+/* ---- incremental checkpoints: a journal of changed chunks beside the last full file (DESIGN.md §8.6) ----
+ * <path> stays an ordinary dsm_map_save file, the base; <path>.journal holds records, each with the 256-surfel chunks of
+ * the pool and the store that changed since the previous checkpoint, the whole segment table and the caller's extra bytes.
+ * The chunks are found on the device, by comparing the live map with the checkpoint image of the previous checkpoint, and
+ * only changed chunks cross PCIe and reach the disk.
+ *   dsm_checkpoint_enqueue_incremental  the contract, ordering and errors of dsm_checkpoint_enqueue; dsm_checkpoint_wait
+ *                           retires it.  Writes a base (the file, then a fresh journal header, each under a temporary
+ *                           name, flushed and renamed) when it is the first incremental checkpoint to path on this
+ *                           context or the previous one went to another path; when the previous checkpoint did not write
+ *                           its file or record (DSM_E_CAPACITY, DSM_E_IO); after a dsm_checkpoint_enqueue; after
+ *                           dsm_map_load, dsm_map_load_journal, dsm_inactive_load, dsm_inactive_reserve or
+ *                           dsm_set_constants; and once the journal has grown larger than its base.  Otherwise appends one
+ *                           record and flushes it to the disk.  Either way the state resolved from path afterwards is byte
+ *                           for byte what dsm_map_save would have written at this position in the stream.
+ *   dsm_map_load_journal    dsm_map_load of the resolved state: the base, then the journal's records in order up to the
+ *   dsm_map_peek_journal    first that is torn, fails its checksum, breaks the chain of checksums or is out of sequence.
+ *                           A missing journal, or one that names another base, adds nothing.  DSM_E_INVALID for a journal
+ *                           of another magic or format, and for a complete record whose chunk lists are not ascending, reach
+ *                           past its sizes or miss a chunk that grows a section.  *records (optional): the records applied.
+ *                           Otherwise the errors of dsm_map_load / dsm_map_peek on that state.
+ *   dsm_journal_materialize writes the version-1 file of the resolved state to out_path (temporary name, fsync, rename),
+ *                           without a context: what dsm_map_load reads, for archives and export. */
+int dsm_checkpoint_enqueue_incremental(dsm_ctx *ctx, const char *path, const void *extra, size_t extra_bytes);
+int dsm_map_load_journal(dsm_ctx *ctx, const char *path, void *extra, size_t extra_cap, size_t *extra_bytes, int *records);
+int dsm_map_peek_journal(const char *path, void *extra, size_t extra_cap, size_t *extra_bytes, int32_t *kf_ofs_cnt, int seg_cap,
+                         int *n_segments, int *records);
+int dsm_journal_materialize(const char *path, const char *out_path);
+
 /* ---- multi-GPU: frames of a batch sharded across GPUs, ONE gather of the surfel deltas at the end (SURVEY.md 8e) ----
  * One context per GPU (one process or thread each).  The reference has no counterpart (fuse_initialize_map is
  * single-process, fusion_functions.cpp:30-83); what is gathered is what SurfelMap::fuse_map consumes after the call

@@ -183,6 +183,29 @@ inline int load_state(Context &c, const std::string &path, std::vector<uint8_t> 
     if (rc == DSM_OK) extra.swap(got);
     return rc;
 }
+// save_state_async as one journal record of the changed chunks beside the base at path, or a new base
+// (dsm_checkpoint_enqueue_incremental, DESIGN.md §8.6); wait_state_saved retires it
+inline int save_state_incremental(Context &c, const std::string &path, const std::vector<uint8_t> &extra)
+{
+    return dsm_checkpoint_enqueue_incremental(c.ctx, path.c_str(), extra.data(), extra.size());
+}
+// load_state of the state the base at path and its journal resolve to (dsm_map_load_journal); *records (optional): the
+// journal records applied
+inline int load_state_incremental(Context &c, const std::string &path, std::vector<uint8_t> &extra, int *records = nullptr)
+{
+    size_t n = 0;
+    int applied = 0;
+    std::vector<uint8_t> got;
+    int rc = dsm_map_load_journal(c.ctx, path.c_str(), nullptr, 0, &n, &applied);
+    if (rc == DSM_E_CAPACITY && n > 0)
+    { // the size-then-read of the extra section: nothing was loaded by the first call
+        got.resize(n);
+        rc = dsm_map_load_journal(c.ctx, path.c_str(), got.data(), got.size(), &n, &applied);
+    }
+    if (rc == DSM_OK) extra.swap(got);
+    if (records) *records = rc == DSM_OK ? applied : 0;
+    return rc;
+}
 } // namespace detail
 
 class ResidentSurfelPool
@@ -398,6 +421,18 @@ class ResidentSurfelPool
     int wait_state_saved(bool block, bool *finished)
     {
         return ctx_.run("wait_state_saved", [&] { return detail::wait_state_saved(ctx_, block, finished); });
+    }
+    // Incremental checkpoints (DESIGN.md §8.6): save_state_incremental is save_state_async, written as one record of the
+    // changed chunks appended to <path>.journal, or as a new base file at path when a record cannot be (the first save to
+    // path, a failed save, the map replaced, the journal larger than its base).  load_state_incremental loads the state
+    // base and journal resolve to; *records (optional) receives the records applied.
+    int save_state_incremental(const std::string &path, const std::vector<uint8_t> &extra)
+    {
+        return ctx_.run("save_state_incremental", [&] { return detail::save_state_incremental(ctx_, path, extra); });
+    }
+    int load_state_incremental(const std::string &path, std::vector<uint8_t> &extra, int *records = nullptr)
+    {
+        return ctx_.run("load_state_incremental", [&] { return detail::load_state_incremental(ctx_, path, extra, records); });
     }
 
     int size()

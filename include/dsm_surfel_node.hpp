@@ -542,31 +542,60 @@ class SurfelMapNode
     {
         return ctx_.run("wait_state_saved", [&] { return detail::wait_state_saved(ctx_, block, finished); });
     }
-    int load_state(const std::string &path)
+    int load_state(const std::string &path) { return load_from(path, false, nullptr, "load_state"); }
+    // Incremental checkpoints (DESIGN.md §8.6, INTEGRATION.md §4): save_state_incremental is save_state_async, written as
+    // one record of the changed chunks (and the whole node section) appended to <path>.journal, or as a new base file at
+    // path when a record cannot be (the first save to path, a failed save, the map replaced, the journal larger than its
+    // base).  wait_state_saved retires it.  load_state_incremental is load_state on the state base and journal resolve
+    // to, with the same checks on its node section and table; *records (optional) receives the records applied.
+    int save_state_incremental(const std::string &path)
     {
-        if (!ctx_.ready("load_state")) return ctx_.err;
+        if (!ctx_.ready("save_state_incremental")) return ctx_.err;
+        std::vector<uint8_t> section;
+        write_section(section);
+        return ctx_.done(detail::save_state_incremental(ctx_, path, section), "save_state_incremental");
+    }
+    int load_state_incremental(const std::string &path, int *records = nullptr)
+    {
+        return load_from(path, true, records, "load_state_incremental");
+    }
+
+    int last_error() const { return ctx_.err; }
+    dsm_ctx *context() { return ctx_.ctx; }
+
+  private:
+    // load_state / load_state_incremental: the file (journal = false) or base + journal (true) peeked and checked against
+    // this node before the map is touched, then loaded
+    int load_from(const std::string &path, bool journal, int *records, const char *what)
+    {
+        if (records) *records = 0;
+        if (!ctx_.ready(what)) return ctx_.err;
         size_t n_extra = 0;
         int n_seg = 0;
-        int rc = dsm_map_peek(path.c_str(), nullptr, 0, &n_extra, nullptr, 0, &n_seg);
-        if (rc != DSM_OK) return ctx_.done(rc, "load_state");
+        auto peek = [&](void *extra, size_t cap, size_t *ne, int32_t *table, int seg_cap, int *ns) {
+            return journal ? dsm_map_peek_journal(path.c_str(), extra, cap, ne, table, seg_cap, ns, nullptr)
+                           : dsm_map_peek(path.c_str(), extra, cap, ne, table, seg_cap, ns);
+        };
+        int rc = peek(nullptr, 0, &n_extra, nullptr, 0, &n_seg);
+        if (rc != DSM_OK) return ctx_.done(rc, what);
         std::vector<uint8_t> section(n_extra + 1);
         std::vector<int32_t> table(3 * (size_t)n_seg + 3);
-        rc = dsm_map_peek(path.c_str(), section.data(), n_extra, nullptr, table.data(), n_seg, nullptr);
-        if (rc != DSM_OK) return ctx_.done(rc, "load_state");
+        rc = peek(section.data(), n_extra, nullptr, table.data(), n_seg, nullptr);
+        if (rc != DSM_OK) return ctx_.done(rc, what);
         section.resize(n_extra);
         State s;
-        if (!read_section(section, s)) return ctx_.done(DSM_E_INVALID, "load_state");
+        if (!read_section(section, s)) return ctx_.done(DSM_E_INVALID, what);
         for (int i = 0; i < n_seg; i++)
-            if (table[3 * i] >= (int)s.poses.size() || s.local.count(table[3 * i])) return ctx_.done(DSM_E_INVALID, "load_state");
+            if (table[3 * i] >= (int)s.poses.size() || s.local.count(table[3 * i])) return ctx_.done(DSM_E_INVALID, what);
         if (snapshot_)
         { // as fuse_front does: its capacity report, if any, stays with the readers
             rc = dsm_publish_wait(ctx_.ctx, nullptr, nullptr, nullptr, nullptr, nullptr);
             snapshot_ = false;
-            if (rc != DSM_OK && rc != DSM_E_CAPACITY) return ctx_.done(rc, "load_state");
+            if (rc != DSM_OK && rc != DSM_E_CAPACITY) return ctx_.done(rc, what);
         }
         std::vector<uint8_t> extra;
-        rc = detail::load_state(ctx_, path, extra);
-        if (rc != DSM_OK) return ctx_.done(rc, "load_state");
+        rc = journal ? detail::load_state_incremental(ctx_, path, extra, records) : detail::load_state(ctx_, path, extra);
+        if (rc != DSM_OK) return ctx_.done(rc, what);
         transform_kitti_ = s.transform_kitti;
         poses_.swap(s.poses);
         local_.swap(s.local);
@@ -577,13 +606,9 @@ class SurfelMapNode
         last_fuse_pose_ = s.last_fuse_pose;
         last_ref_ = s.last_ref;
         fused_ = s.fused;
-        return ctx_.done(DSM_OK, "load_state");
+        return ctx_.done(DSM_OK, what);
     }
 
-    int last_error() const { return ctx_.err; }
-    dsm_ctx *context() { return ctx_.ctx; }
-
-  private:
     struct PendingPose
     {
         double stamp;
