@@ -32,6 +32,7 @@ EXPORTS = [
     "dsm_inactive_download", "dsm_inactive_size", "dsm_frame_raw_cloud", "dsm_inactive_export_poses",
     "dsm_frame_superpixel_image", "dsm_fuse_stream_window",
     "dsm_publish_enable", "dsm_publish_enqueue", "dsm_publish_wait", "dsm_debug_publish_chunks",
+    "dsm_field_enable", "dsm_field_enqueue", "dsm_field_wait",
     "dsm_inactive_segments", "dsm_inactive_load", "dsm_map_save", "dsm_map_load", "dsm_map_peek",
     "dsm_checkpoint_enable", "dsm_checkpoint_enqueue", "dsm_checkpoint_wait", "dsm_debug_checkpoint_drain_ctas",
     "dsm_checkpoint_enqueue_incremental", "dsm_map_load_journal", "dsm_map_peek_journal", "dsm_journal_materialize",
@@ -50,6 +51,10 @@ class DsmParams(ctypes.Structure):
 class DsmConstants(ctypes.Structure):
     _fields_ = [("huber_range", ctypes.c_double), ("baseline", ctypes.c_double), ("disparity_error", ctypes.c_double),
                 ("min_tolerate_diff", ctypes.c_double)]
+
+
+class DsmFieldParams(ctypes.Structure):
+    _fields_ = [("voxel", ctypes.c_float), ("nx", ctypes.c_int32), ("ny", ctypes.c_int32), ("nz", ctypes.c_int32)]
 
 
 CONSTANTS_DRIVE = (0.4, 0.5, 4.0, 0.1)    # fusion_functions.h:13-16
@@ -104,6 +109,9 @@ def load_library():
     L.dsm_publish_enqueue.argtypes = [vp, ci]
     L.dsm_publish_wait.argtypes = [vp, ctypes.POINTER(vp), ctypes.POINTER(ci), ctypes.POINTER(vp), ctypes.POINTER(ci), ctypes.POINTER(ci)]
     L.dsm_debug_publish_chunks.argtypes = [vp, ctypes.POINTER(ci)]
+    L.dsm_field_enable.argtypes = [vp, ctypes.POINTER(DsmFieldParams)]
+    L.dsm_field_enqueue.argtypes = [vp, ctypes.POINTER(ctypes.c_double), ci]
+    L.dsm_field_wait.argtypes = [vp, ctypes.POINTER(vp), ctypes.POINTER(ctypes.c_int32), ctypes.POINTER(ci)]
     L.dsm_inactive_reserve.argtypes = [vp, ci]
     L.dsm_inactive_retire.argtypes = [vp, ci, ctypes.POINTER(ci)]
     L.dsm_inactive_reactivate.argtypes = [vp, ci, ctypes.POINTER(ci)]
@@ -529,6 +537,34 @@ class Context:
         n = ctypes.c_int(0)
         self._ck(self.lib.dsm_debug_publish_chunks(self.h, ctypes.byref(n)))
         return n.value
+
+    # ---- the map as a distance field ----
+    def field_enable(self, voxel, nx, ny, nz):
+        p = DsmFieldParams(float(voxel), int(nx), int(ny), int(nz))
+        self._ck(self.lib.dsm_field_enable(self.h, ctypes.byref(p)))
+        self._field_shape = (int(nz), int(ny), int(nx))
+
+    def field_enqueue(self, center, min_update_times=5):
+        c = (ctypes.c_double * 3)(*[float(v) for v in center])
+        self._ck(self.lib.dsm_field_enqueue(self.h, c, int(min_update_times)))
+
+    def field_wait(self):
+        """(dist, origin, n_occupied) of the enqueued field: dist a float32 [nz][ny][nx] copy of the context's pinned
+        buffer, origin an int32 (3,) array (x, y, z).  A field requested after a rejected frame raises
+        DsmError(DSM_E_CAPACITY) carrying the same tuple as `.field` (the map of the last applied frame)."""
+        ptr, org, nocc = ctypes.c_void_p(), (ctypes.c_int32 * 3)(), ctypes.c_int(0)
+        rc = self.lib.dsm_field_wait(self.h, ctypes.byref(ptr), org, ctypes.byref(nocc))
+        if rc not in (DSM_OK, -6):  # DSM_E_CAPACITY still carries the field
+            self._ck(rc)
+        shape = self._field_shape
+        n = shape[0] * shape[1] * shape[2]
+        buf = (ctypes.c_float * n).from_address(ptr.value)
+        field = (np.frombuffer(buf, dtype=np.float32).reshape(shape).copy(), np.array(org[:], dtype=np.int32), nocc.value)
+        if rc != DSM_OK:
+            err = DsmError(rc, self.lib.dsm_last_error(self.h).decode())
+            err.field = field
+            raise err
+        return field
 
     # ---- raw cloud of a frame ----
     def frame_raw_cloud(self, frame, pose7, cap=None):

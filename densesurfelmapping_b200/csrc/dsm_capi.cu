@@ -1085,6 +1085,7 @@ extern "C" int dsm_inactive_reserve(dsm_ctx *ctx, int max_inactive_surfels)
 {
     if (!ctx || max_inactive_surfels < 1) return DSM_E_INVALID;
     if (ctx->pub_in_flight) return DSM_E_STATE; // the snapshot's inactive buffer goes with the old store
+    if (ctx->field && ctx->field->in_flight) return DSM_E_STATE; // as does the store a field request reads
     if (ctx->ckpt && ctx->ckpt->pending) return DSM_E_STATE; // and the checkpoint's images are sized by it
     int rs = res_sync(ctx);
     if (rs != DSM_OK) return rs;
@@ -1286,7 +1287,7 @@ extern "C" int dsm_inactive_segments(dsm_ctx *ctx, int32_t *kf_ofs_cnt, int cap,
 int dsm_inactive_load_check(const dsm_ctx *ctx, const dsm_surfel_t *surfels, int n, const int32_t *kf_ofs_cnt, int n_segments)
 {
     if (!ctx || n < 0 || n_segments < 0 || (n > 0 && !surfels) || (n_segments > 0 && !kf_ofs_cnt)) return DSM_E_INVALID;
-    if (!ctx->inact || ctx->pub_in_flight) return DSM_E_STATE;
+    if (!ctx->inact || ctx->pub_in_flight || (ctx->field && ctx->field->in_flight)) return DSM_E_STATE;
     if (n > ctx->inact->cap) return DSM_E_CAPACITY;
     // the table: contiguous from 0, every segment at least one surfel, n in all, no negative keyframe
     int64_t ofs = 0;
@@ -1340,6 +1341,7 @@ int dsm_map_info(const dsm_ctx *ctx, DsmMapInfo *info)
     info->constants = dsm_constants{ctx->d.huber, ctx->d.baseline, ctx->d.disparity_error, ctx->d.min_tolerate_diff};
     info->store_cap = ctx->inact ? ctx->inact->cap : 0;
     info->publish_in_flight = ctx->pub_in_flight;
+    info->field_in_flight = ctx->field && ctx->field->in_flight;
     return DSM_OK;
 }
 
@@ -1416,6 +1418,91 @@ extern "C" int dsm_debug_publish_chunks(dsm_ctx *ctx, int *count)
     if (!ctx->pub_on || ctx->pub_in_flight) return DSM_E_STATE;
     *count = ctx->pub_hdr[DSM_PUB_CHUNKS];
     return DSM_OK;
+}
+
+// ---- the map as a distance field (include/dsm.h, DESIGN.md §8.7) ----
+extern "C" int dsm_field_enable(dsm_ctx *ctx, const dsm_field_params *params)
+{
+    if (!ctx || !params) return DSM_E_INVALID;
+    const dsm_field_params &p = *params;
+    if (!std::isfinite(p.voxel) || !(p.voxel > 0.f)) return DSM_E_INVALID;
+    for (int n : {p.nx, p.ny, p.nz})
+        if (n < 1 || n > 1024) return DSM_E_INVALID;
+    if (!ctx->res_active || ctx->field) return DSM_E_STATE;
+    CK(cudaSetDevice(ctx->device));
+    auto f = std::make_unique<DsmField>();
+    f->g.voxel = p.voxel;
+    f->g.n[0] = p.nx, f->g.n[1] = p.ny, f->g.n[2] = p.nz;
+    f->voxels = (size_t)p.nx * p.ny * p.nz;
+    f->bytes = (dsm_field_header(f->voxels) + DSM_FIELD_WORDS) * sizeof(int32_t);
+    cudaError_t e = f->own.device(&f->occ, f->voxels);
+    if (e == cudaSuccess) e = f->own.device(&f->dist, f->bytes / sizeof(int32_t));
+    if (e == cudaSuccess) e = f->own.host(&f->host, f->bytes / sizeof(int32_t));
+    if (e == cudaSuccess) e = f->own.event(&f->ev);
+    if (e == cudaSuccess && dsm_field_setup() != 0) e = cudaErrorInvalidValue;
+    if (e != cudaSuccess)
+    {
+        cudaGetLastError();
+        return DSM_E_NOMEM; // nothing is kept: a later call may try again
+    }
+    ctx->field = std::move(f);
+    return DSM_OK;
+}
+
+// Enqueue only, like dsm_publish_enqueue: clear, mark, the three EDT passes and one copy of the grid with its header into
+// the pinned buffer, then the event.  The launches have no gate: after a rejected frame the map is the one of the last
+// applied frame, which is what the field reports.
+extern "C" int dsm_field_enqueue(dsm_ctx *ctx, const double center[3], int min_update_times)
+{
+    if (!ctx || !center || min_update_times < 1) return DSM_E_INVALID;
+    DsmField *f = ctx->field.get();
+    if (!f || f->in_flight) return DSM_E_STATE;
+    DsmFieldGrid g = f->g;
+    const int64_t lim = int64_t(1) << 24;
+    for (int k = 0; k < 3; k++)
+    {
+        if (!std::isfinite(center[k])) return DSM_E_INVALID;
+        const double q = std::floor(center[k] / (double)g.voxel);
+        if (!(std::fabs(q) <= 4.0 * (double)lim)) return DSM_E_INVALID;
+        const int64_t o = (int64_t)q - g.n[k] / 2;
+        if (o < -lim || o > lim || o + g.n[k] < -lim || o + g.n[k] > lim) return DSM_E_INVALID;
+        g.o[k] = (int)o;
+        g.lo[k] = (float)o;
+        g.hi[k] = (float)(o + g.n[k]);
+    }
+    CK(cudaSetDevice(ctx->device));
+    const DsmDev d = resident_view(ctx, 0);
+    const InactStore *s = ctx->inact.get();
+    int32_t *header = f->dist + dsm_field_header(f->voxels);
+    CK(cudaMemsetAsync(f->occ, 0, f->voxels, ctx->stream));
+    CK(cudaMemsetAsync(header, 0, sizeof(int32_t), ctx->stream));
+    dsm_launch_field_mark(ctx->d.pool, ctx->res_ofs, d.max_pool_per_frame, min_update_times, s ? s->surfels : nullptr, ctx->win_hdr,
+                          s ? std::min(s->upper, s->cap) : 0, g, f->occ, header, ctx->stream);
+    dsm_launch_field_edt(g, f->occ, f->dist, header, ctx->stream);
+    CK(cudaGetLastError());
+    CK(cudaMemcpyAsync(f->host, f->dist, f->bytes, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaEventRecord(f->ev, ctx->stream));
+    f->g = g;
+    f->in_flight = true;
+    return DSM_OK;
+}
+
+extern "C" int dsm_field_wait(dsm_ctx *ctx, const float **dist, int32_t origin[3], int *n_occupied)
+{
+    if (!ctx) return DSM_E_INVALID;
+    DsmField *f = ctx->field.get();
+    if (!f || !f->in_flight) return DSM_E_STATE;
+    CK(cudaSetDevice(ctx->device));
+    CK(cudaEventSynchronize(f->ev));
+    f->in_flight = false;
+    const int32_t *h = f->host + dsm_field_header(f->voxels);
+    if (dist) *dist = reinterpret_cast<const float *>(f->host);
+    if (origin) origin[0] = f->g.o[0], origin[1] = f->g.o[1], origin[2] = f->g.o[2];
+    if (n_occupied) *n_occupied = h[DSM_FIELD_N_OCCUPIED];
+    if (h[DSM_FIELD_ERR_TAG] == 0) return DSM_OK;
+    snprintf(ctx->err, sizeof(ctx->err), "dsm_field_wait: frame %d of a dsm_fuse_stream_window call did not fit the pool or the "
+             "store; the field holds the frames before it", h[DSM_FIELD_ERR_FRAME]);
+    return DSM_E_CAPACITY;
 }
 
 // ---- checkpoints that do not stop the stream (include/dsm.h, DESIGN.md §8.5) ----

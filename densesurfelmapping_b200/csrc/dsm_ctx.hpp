@@ -170,6 +170,19 @@ struct DsmCheckpoint
     }
 };
 
+// dsm_field_* (DESIGN.md §8.7): the occupancy grid, the distance grid with its header words, the pinned host copy of
+// both and the event after the copy, all allocated by dsm_field_enable
+struct DsmField
+{
+    CudaOwner own;
+    DsmFieldGrid g{}; // voxel and size; origin and bounds of the latest request
+    size_t voxels = 0, bytes = 0; // voxels of the grid; bytes of the distance grid with its header
+    uint8_t *occ = nullptr;
+    int32_t *dist = nullptr, *host = nullptr; // device grid, pinned copy
+    cudaEvent_t ev = nullptr;
+    bool in_flight = false; // enqueued and not yet waited for
+};
+
 #define DSM_MAX_CHUNKS 4
 
 struct dsm_ctx
@@ -238,6 +251,7 @@ struct dsm_ctx
     int32_t *pub_hdr = nullptr, *pub_hdr_dev = nullptr, *pub_state = nullptr;
     cudaEvent_t pub_ev = nullptr;
     std::unique_ptr<DsmCheckpoint> ckpt; // nullptr until dsm_checkpoint_enable
+    std::unique_ptr<DsmField> field;     // nullptr until dsm_field_enable
     int run_split = 2;          // sub-batches per dsm_batch_run (dsm_set_concurrency)
     // pinned host staging for the small per-batch tables
     float *h_pose = nullptr; // [2B][32]: pose then inverse; first half: the batch calls, second half: the resident stream

@@ -272,3 +272,29 @@ void dsm_launch_map_delta(const dsm_surfel_t *pool, const int32_t *res, int pool
 // k_map_drain_delta: the header line, the flag lines, the live table lines and the live lines of the flagged chunks only
 void dsm_launch_map_drain_delta(const uint8_t *image, uint8_t *host_dev, const DsmSnapLayout &lay, int pool_chunks, int store_chunks,
                                 int ctas, cudaStream_t s);
+
+// dsm_field_* (DESIGN.md §8.7), dsm_field.cu.  The grid of one request: voxel edge, size, integer origin o and its fp32
+// bounds lo = (float)o, hi = (float)(o + n), exact below 2^24.  The distance grid [nz][ny][nx] (int32 squared distances
+// until the last pass, then fp32 distances) is followed, at word dsm_field_header(voxels), by DSM_FIELD_WORDS header
+// words; one copy moves both to the host.
+struct DsmFieldGrid
+{
+    float voxel;
+    int n[3], o[3];
+    float lo[3], hi[3];
+};
+enum
+{
+    DSM_FIELD_N_OCCUPIED, // occupied voxels (zeroed before the request; k_field_rows adds)
+    DSM_FIELD_ERR_TAG,    // the sticky error word of dsm_fuse_stream_window at the request, and
+    DSM_FIELD_ERR_FRAME,  // the frame it rejected
+    DSM_FIELD_WORDS
+};
+inline size_t dsm_field_header(size_t voxels) { return (voxels + 3) / 4 * 4; }
+int dsm_field_setup(); // raises the dynamic shared-memory limit of the envelope passes (lines of up to 1024 voxels)
+// k_field_mark over pool slots [0, res[1]) with update_times >= min_update_times and stored surfels [0, *store_size);
+// pool_upper / store_upper >= the live sizes size the grid.  store == nullptr: no store.  occ must be zeroed.
+void dsm_launch_field_mark(const dsm_surfel_t *pool, const int32_t *res, int pool_upper, int min_update_times, const dsm_surfel_t *store,
+                           const int32_t *store_size, int store_upper, const DsmFieldGrid &g, uint8_t *occ, int32_t *header, cudaStream_t s);
+// the three EDT passes: occ -> dist (in place from the second pass on); header[DSM_FIELD_N_OCCUPIED] must be zeroed
+void dsm_launch_field_edt(const DsmFieldGrid &g, const uint8_t *occ, int32_t *dist, int32_t *header, cudaStream_t s);

@@ -1,0 +1,208 @@
+// The distance field of dsm_field_enqueue (DESIGN.md §8.7): a local voxel grid of the GPU-resident map and its exact
+// Euclidean distance transform, in stream order.
+//
+//   k_field_mark      one pass over the live pool slots (update_times >= min_update_times) and the stored surfels: every
+//                     point inside the grid stores a 1 into the occupancy grid (cleared by the caller).  Idempotent, so
+//                     no atomics; the live sizes come from the device, surplus CTAs exit at once.
+//   k_field_rows      per x-row, the squared 1-D distance to the nearest occupied voxel (a max scan from the left and a
+//                     min scan from the right, one warp per row) into the distance grid; counts the occupied voxels.
+//   k_field_lines     along y, then along z: the lower envelope of the parabolas f(u) + (x - u)^2 of one line
+//                     (Meijster's separable pass) and its minimum at every voxel, in place.  One thread per line, the
+//                     lanes of a warp on consecutive x, so every global access is coalesced; the envelope lives in
+//                     shared memory, one packed word (f << 10 | u) per entry.  The z pass writes the fp32 distances.
+//
+// Squared distances are int32; an empty line holds FIELD_INF.  Every finite value is below 3 * 1023^2 < 2^22, so a site
+// and its value pack into one word and the conversion to float is exact.  The kernels carry no error gate and are
+// launched without PDL: each begins after everything enqueued before it has completed.
+#include "dsm_device.cuh"
+#include <climits>
+
+#define FIELD_INF INT_MAX
+#define FIELD_MARK_BLOCK 256
+#define FIELD_ROW_WARPS 8
+#define FIELD_BATCH 8 // line loads in flight per thread in the envelope pass
+
+__global__ void __launch_bounds__(FIELD_MARK_BLOCK) k_field_mark(const dsm_surfel_t *pool, const int32_t *res, int pool_grid,
+                                                                 int min_update_times, const dsm_surfel_t *store,
+                                                                 const int32_t *store_size, const DsmFieldGrid g, uint8_t *occ,
+                                                                 int32_t *header)
+{
+    if (blockIdx.x == 0 && threadIdx.x == 0)
+    { // the error word at the request, recorded, not waited on (as k_cloud_mirror does)
+        header[DSM_FIELD_ERR_TAG] = res[2];
+        header[DSM_FIELD_ERR_FRAME] = res[3];
+    }
+    const bool in_pool = (int)blockIdx.x < pool_grid;
+    const int first = (in_pool ? blockIdx.x : blockIdx.x - pool_grid) * FIELD_MARK_BLOCK;
+    const int n = in_pool ? res[1] : *store_size;
+    if (first >= n) return; // the grid is sized from the host's upper bounds
+    const int i = first + threadIdx.x;
+    if (i >= n) return;
+    const dsm_surfel_t *e = (in_pool ? pool : store) + i;
+    if (in_pool && e->update_times < min_update_times) return;
+    const float qx = floorf(e->px / g.voxel), qy = floorf(e->py / g.voxel), qz = floorf(e->pz / g.voxel);
+    // fp32 compares against exact bounds: a NaN or infinite coordinate fails them
+    if (!(qx >= g.lo[0] && qx < g.hi[0] && qy >= g.lo[1] && qy < g.hi[1] && qz >= g.lo[2] && qz < g.hi[2])) return;
+    const int x = (int)qx - g.o[0], y = (int)qy - g.o[1], z = (int)qz - g.o[2];
+    occ[((size_t)z * g.n[1] + y) * g.n[0] + x] = 1;
+}
+
+__global__ void __launch_bounds__(32 * FIELD_ROW_WARPS) k_field_rows(const DsmFieldGrid g, const uint8_t *occ, int32_t *dist, int32_t *header)
+{
+    __shared__ int32_t s_left[FIELD_ROW_WARPS][1024]; // nearest occupied x at or left of each x, -1 if none
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int row = blockIdx.x * FIELD_ROW_WARPS + warp, nx = g.n[0];
+    if (row >= g.n[1] * g.n[2]) return;
+    const uint8_t *o = occ + (size_t)row * nx;
+    int32_t *out = dist + (size_t)row * nx;
+    int32_t *left = s_left[warp];
+    int carry = -1, count = 0;
+    for (int base = 0; base < nx; base += 32)
+    {
+        const int x = base + lane;
+        const bool hit = x < nx && o[x];
+        int v = hit ? x : -1;
+        for (int k = 1; k < 32; k <<= 1)
+        {
+            const int t = __shfl_up_sync(0xffffffffu, v, k);
+            if (lane >= k) v = max(v, t);
+        }
+        v = max(v, carry);
+        if (x < nx) left[x] = v;
+        carry = __shfl_sync(0xffffffffu, v, 31);
+        count += __popc(__ballot_sync(0xffffffffu, hit));
+    }
+    carry = INT_MAX;
+    for (int base = (nx - 1) & ~31; base >= 0; base -= 32)
+    {
+        const int x = base + lane;
+        const bool hit = x < nx && o[x];
+        int v = hit ? x : INT_MAX;
+        for (int k = 1; k < 32; k <<= 1)
+        {
+            const int t = __shfl_down_sync(0xffffffffu, v, k);
+            if (lane + k < 32) v = min(v, t);
+        }
+        v = min(v, carry);
+        carry = __shfl_sync(0xffffffffu, v, 0);
+        if (x < nx)
+        {
+            const int l = left[x];
+            const int d = min(l >= 0 ? x - l : INT_MAX, v != INT_MAX ? v - x : INT_MAX);
+            out[x] = d == INT_MAX ? FIELD_INF : d * d;
+        }
+    }
+    if (lane == 0 && count > 0) atomicAdd(&header[DSM_FIELD_N_OCCUPIED], count);
+}
+
+__device__ __forceinline__ uint32_t env_pack(int u, int f) { return ((uint32_t)f << 10) | (uint32_t)u; }
+__device__ __forceinline__ int env_at(uint32_t e, int x)
+{
+    const int d = x - (int)(e & 1023u);
+    return (int)(e >> 10) + d * d;
+}
+// the last x at which site e is at least as close as site (u, fu), u > e's site: floor of the parabolas' intersection
+__device__ __forceinline__ int env_sep(uint32_t e, int u, int fu)
+{
+    const int s = (int)(e & 1023u), fs = (int)(e >> 10);
+    const int num = u * u - s * s + fu - fs, den = 2 * (u - s);
+    const int q = num / den;
+    return (num % den != 0 && num < 0) ? q - 1 : q;
+}
+
+// One line of `len` voxels at stride `step` per thread; line (x, blockIdx.y) starts at dist + blockIdx.y * outer + x.
+// LAST: the minimum becomes sqrtf((float)d2) * voxel (+inf for an empty line) in place of the squared distance.
+template <bool LAST>
+__global__ void __launch_bounds__(32) k_field_lines(int32_t *dist, int nx, int len, int step, int outer, float voxel)
+{
+    extern __shared__ uint32_t s_env[]; // [len][32]: entry k of lane l at k * 32 + l (conflict-free)
+    const int x = blockIdx.x * 32 + threadIdx.x;
+    if (x >= nx) return;
+    int32_t *line = dist + (size_t)blockIdx.y * outer + x;
+    uint32_t *env = s_env + threadIdx.x;
+    int top = -1, t_top = 0; // the envelope's last entry and the first x it is lowest at
+    for (int u0 = 0; u0 < len; u0 += FIELD_BATCH)
+    {
+        int f[FIELD_BATCH];
+#pragma unroll
+        for (int j = 0; j < FIELD_BATCH; j++) f[j] = u0 + j < len ? line[(size_t)(u0 + j) * step] : FIELD_INF;
+#pragma unroll
+        for (int j = 0; j < FIELD_BATCH; j++)
+        {
+            const int u = u0 + j, fu = f[j];
+            if (fu == FIELD_INF) continue;
+            // drop the entries that site u is strictly closer than at the start of their interval
+            while (top >= 0 && env_at(env[top * 32], t_top) > fu + (t_top - u) * (t_top - u))
+            {
+                top--;
+                t_top = top >= 1 ? 1 + env_sep(env[(top - 1) * 32], (int)(env[top * 32] & 1023u), (int)(env[top * 32] >> 10)) : 0;
+            }
+            if (top < 0)
+            {
+                top = 0;
+                t_top = 0;
+                env[0] = env_pack(u, fu);
+            }
+            else
+            {
+                const int w = 1 + env_sep(env[top * 32], u, fu);
+                if (w < len)
+                {
+                    top++;
+                    t_top = w;
+                    env[top * 32] = env_pack(u, fu);
+                }
+            }
+        }
+    }
+    if (top < 0)
+    {
+        for (int u = 0; u < len; u++) line[(size_t)u * step] = LAST ? __float_as_int(INFINITY) : FIELD_INF;
+        return;
+    }
+    // the lowest entry at x only moves right as x grows: advance while the next one is at least as low
+    int k = 0;
+    uint32_t cur = env[0];
+    for (int u = 0; u < len; u++)
+    {
+        int d = env_at(cur, u);
+        while (k < top)
+        {
+            const uint32_t nxt = env[(k + 1) * 32];
+            const int dn = env_at(nxt, u);
+            if (dn > d) break;
+            k++;
+            cur = nxt;
+            d = dn;
+        }
+        line[(size_t)u * step] = LAST ? __float_as_int(sqrtf((float)d) * voxel) : d;
+    }
+}
+
+int dsm_field_setup()
+{
+    const int smem = 1024 * 32 * 4; // the longest line
+    cudaError_t e = cudaFuncSetAttribute(k_field_lines<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(k_field_lines<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    return e == cudaSuccess ? 0 : -1;
+}
+
+void dsm_launch_field_mark(const dsm_surfel_t *pool, const int32_t *res, int pool_upper, int min_update_times, const dsm_surfel_t *store,
+                           const int32_t *store_size, int store_upper, const DsmFieldGrid &g, uint8_t *occ, int32_t *header, cudaStream_t s)
+{
+    const int pool_chunks = (pool_upper + FIELD_MARK_BLOCK - 1) / FIELD_MARK_BLOCK;
+    const int pool_grid = pool_chunks > 1 ? pool_chunks : 1; // CTA 0 exists and records the error word
+    const int store_grid = store ? (store_upper + FIELD_MARK_BLOCK - 1) / FIELD_MARK_BLOCK : 0;
+    k_field_mark<<<pool_grid + store_grid, FIELD_MARK_BLOCK, 0, s>>>(pool, res, pool_grid, min_update_times, store, store_size, g, occ, header);
+}
+
+void dsm_launch_field_edt(const DsmFieldGrid &g, const uint8_t *occ, int32_t *dist, int32_t *header, cudaStream_t s)
+{
+    const int nx = g.n[0], ny = g.n[1], nz = g.n[2];
+    const int rows = ny * nz;
+    k_field_rows<<<(rows + FIELD_ROW_WARPS - 1) / FIELD_ROW_WARPS, 32 * FIELD_ROW_WARPS, 0, s>>>(g, occ, dist, header);
+    const unsigned xb = (unsigned)(nx + 31) / 32;
+    // along y: lines (x, z) at stride nx; along z: lines (x, y) at stride nx * ny
+    k_field_lines<false><<<dim3(xb, nz), 32, (size_t)ny * 32 * 4, s>>>(dist, nx, ny, nx, nx * ny, g.voxel);
+    k_field_lines<true><<<dim3(xb, ny), 32, (size_t)nz * 32 * 4, s>>>(dist, nx, nz, nx * ny, nx, g.voxel);
+}

@@ -377,7 +377,7 @@ int load_checked(dsm_ctx *ctx, const DsmMapInfo &info, const MapFile &m, void *e
         std::memcmp(&h.constants, &info.constants, sizeof(dsm_constants)) != 0)
         return DSM_E_INVALID; // the caller sets the constants before loading
     if (h.n_pool > p.max_local_surfels) return DSM_E_CAPACITY;
-    if (info.publish_in_flight) return DSM_E_STATE;
+    if (info.publish_in_flight || info.field_in_flight) return DSM_E_STATE;
     int rc = DSM_OK;
     if (info.store_cap == 0)
     {

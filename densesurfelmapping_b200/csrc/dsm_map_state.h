@@ -9,6 +9,7 @@ struct DsmMapInfo
     dsm_constants constants; // the set in force (dsm_set_constants)
     int store_cap;           // the inactive store's reservation in surfels, 0 without one
     bool publish_in_flight;  // a dsm_publish_enqueue snapshot has not been waited for
+    bool field_in_flight;    // a dsm_field_enqueue field has not been waited for
 };
 
 __attribute__((visibility("hidden"))) int dsm_map_info(const dsm_ctx *ctx, DsmMapInfo *info);

@@ -447,6 +447,40 @@ int dsm_publish_wait(dsm_ctx *ctx, const dsm_point_t **active, int *n_active, co
                      int *inactive_changed_from);
 int dsm_debug_publish_chunks(dsm_ctx *ctx, int *count);
 
+/* ---- the map as a distance field for planners (DESIGN.md §8.7) ----
+ * A local voxel grid of the resident map and its exact Euclidean distance transform, built in stream order like a publish
+ * snapshot, so that it follows every loop closure the map follows.  Grid: voxel edge v, size (nx, ny, nz).  A request
+ * centred on c has the integer origin o_k = floor(c_k / (double)v) - floor(n_k / 2).  Its obstacle points are those of
+ * dsm_pool_export_cloud(min_update_times) and dsm_inactive_export_cloud at the request's position in the stream; a point p
+ * marks voxel q - o, q_k = floorf(p_k / v) in fp32, when o_k <= q_k < o_k + n_k on every axis (compared in fp32; a NaN
+ * or infinite coordinate marks nothing).  dist[(z * ny + y) * nx + x] = sqrtf((float)d2) * v, d2 the smallest squared
+ * integer distance from voxel (x, y, z) to an occupied voxel (0 on one), +INFINITY everywhere when none is occupied.
+ * Unsigned: every voxel without an obstacle point counts as free.
+ *   dsm_field_enable    once, on a context with a resident pool (DSM_E_STATE otherwise, and when called twice).  v finite
+ *                       and > 0, each size in [1, 1024] (DSM_E_INVALID).  Allocates the occupancy grid (1 B per voxel)
+ *                       and the distance grid (4 B per voxel) on the device, a pinned host copy of the distance grid and
+ *                       an event.  DSM_E_NOMEM, with nothing kept.
+ *   dsm_field_enqueue   asynchronous, ordered on the context's stream exactly like dsm_publish_enqueue; never waits and
+ *                       reads nothing back.  DSM_E_INVALID for min_update_times < 1, a non-finite centre, or an origin with
+ *                       |o_k| or |o_k + n_k| above 2^24; DSM_E_STATE before dsm_field_enable, and while a field is
+ *                       enqueued and not yet waited for.
+ *   dsm_field_wait      waits for that field only.  *dist is the context's pinned buffer of nx * ny * nz floats, valid
+ *                       until the next dsm_field_enqueue, never to be freed or written; origin receives o and
+ *                       *n_occupied the number of occupied voxels.  Any out-pointer may be NULL.  If a frame of
+ *                       dsm_fuse_stream_window had been rejected before the request, returns DSM_E_CAPACITY with the
+ *                       field of the last applied frame and does NOT clear the error, as dsm_publish_wait.  DSM_E_STATE
+ *                       with no field enqueued.
+ * dsm_inactive_reserve, dsm_inactive_load, dsm_map_load and dsm_map_load_journal return DSM_E_STATE while a field is in
+ * flight. */
+typedef struct dsm_field_params
+{
+    float voxel;
+    int32_t nx, ny, nz;
+} dsm_field_params;
+int dsm_field_enable(dsm_ctx *ctx, const dsm_field_params *params);
+int dsm_field_enqueue(dsm_ctx *ctx, const double center[3], int min_update_times);
+int dsm_field_wait(dsm_ctx *ctx, const float **dist, int32_t origin[3], int *n_occupied);
+
 /* ---- checkpoints that do not stop the stream (DESIGN.md §8.5) ----
  * The file of dsm_map_save, taken in stream order like a publish snapshot: the resident stream pays one device-to-device
  * copy of the live map, the transfer to the host runs on a low-priority stream beside the next frames, and a thread of

@@ -56,6 +56,14 @@
 // (local_surfels(), active_points(), ... or dsm_pool_size on context()) has reported and cleared the error.  A node
 // that only ever publishes must call one of them to resume.
 // Without enable_publishing() nothing is enqueued and the node behaves exactly as before.
+//
+// A planner wants a distance field, not clouds.  enable_distance_field(voxel, nx, ny, nz) makes every fused frame
+// enqueue one more job behind its fuse (and behind its snapshot when publishing): the exact Euclidean distance field of
+// the map on an nx x ny x nz grid centred on the frame's camera, the translation of its fuse pose, with the active
+// cloud's threshold of 5 updates (dsm_field_enqueue(ctx, centre, 5), DESIGN.md §8.7).  distance_field() hands it out
+// with the same one-frame-late pattern, lifetime and capacity rule as published_clouds(); an unread field is retired
+// before the next fuse and before load_state*, as an unread snapshot is.  Without enable_distance_field() nothing is
+// enqueued.
 // device < 0 builds the node without a context: the callbacks run the whole pose logic (pose database, sync, window
 // bookkeeping) and fuse nothing; any call that reads the map returns DSM_E_STATE.
 #pragma once
@@ -451,6 +459,23 @@ class SurfelMapNode
         snapshot_ = false;
         return ctx_.done(dsm_publish_wait(ctx_.ctx, &active, &n_active, &inactive, &n_inactive, &inactive_changed_from), "published_clouds");
     }
+    // ---- the map as a distance field around the camera, for a planner (see the top of this file, DESIGN.md §8.7) ----
+    int enable_distance_field(float voxel, int nx, int ny, int nz)
+    {
+        const dsm_field_params p = {voxel, nx, ny, nz};
+        if (ctx_.run("enable_distance_field", [&] { return dsm_field_enable(ctx_.ctx, &p); }) == DSM_OK) distance_field_ = true;
+        return ctx_.err;
+    }
+    // the field of the latest fused frame: dist [nz][ny][nx] in metres (the library's pinned buffer, valid until the next
+    // frame is fused), the grid's origin in voxels and the occupied voxels.  DSM_E_STATE when no frame has been fused
+    // since the last call; DSM_E_CAPACITY with the field of the last applied frame, as published_clouds().
+    int distance_field(const float *&dist, int32_t origin[3], int &n_occupied)
+    {
+        if (!ctx_.ready("distance_field")) return ctx_.err;
+        if (!field_) return ctx_.done(DSM_E_STATE, "distance_field");
+        field_ = false;
+        return ctx_.done(dsm_field_wait(ctx_.ctx, &dist, origin, &n_occupied), "distance_field");
+    }
     // publish_neighbor_pointcloud (:1283-1383): live local points, then the stored points of get_driftfree_poses(ref,
     // 2 * drift_free_poses) in list order
     int neighbor_points(int reference_index, std::vector<dsm_point_t> &points)
@@ -587,12 +612,7 @@ class SurfelMapNode
         if (!read_section(section, s)) return ctx_.done(DSM_E_INVALID, what);
         for (int i = 0; i < n_seg; i++)
             if (table[3 * i] >= (int)s.poses.size() || s.local.count(table[3 * i])) return ctx_.done(DSM_E_INVALID, what);
-        if (snapshot_)
-        { // as fuse_front does: its capacity report, if any, stays with the readers
-            rc = dsm_publish_wait(ctx_.ctx, nullptr, nullptr, nullptr, nullptr, nullptr);
-            snapshot_ = false;
-            if (rc != DSM_OK && rc != DSM_E_CAPACITY) return ctx_.done(rc, what);
-        }
+        if (retire_unread(what) != DSM_OK) return ctx_.err; // as fuse_front does
         std::vector<uint8_t> extra;
         rc = journal ? detail::load_state_incremental(ctx_, path, extra, records) : detail::load_state(ctx_, path, extra);
         if (rc != DSM_OK) return ctx_.done(rc, what);
@@ -820,12 +840,7 @@ class SurfelMapNode
         window_lists(q.reference_index, remove, add);
         if (ctx_.ctx)
         {
-            if (snapshot_)
-            { // an unread snapshot is retired: its capacity report, if any, stays with the readers
-                const int rc = dsm_publish_wait(ctx_.ctx, nullptr, nullptr, nullptr, nullptr, nullptr);
-                snapshot_ = false;
-                if (rc != DSM_OK && rc != DSM_E_CAPACITY) return ctx_.done(rc, "fuse");
-            }
+            if (retire_unread("fuse") != DSM_OK) return ctx_.err;
             const int rc = detail::fuse_window(ctx_, q.reference_index, image_buffer_.front().second.data(),
                                                depth_buffer_.front().second.data(), pose16, remove, add);
             if (ctx_.done(rc, "fuse") != DSM_OK) return rc;
@@ -836,10 +851,30 @@ class SurfelMapNode
         last_ref_ = q.reference_index;
         fused_ = true;
         pose_buffer_.pop_front();
-        if (publishing_)
-        { // after the bookkeeping: the frame is enqueued, so the host window follows the device whatever this returns
-            snapshot_ = ctx_.done(dsm_publish_enqueue(ctx_.ctx, 5), "fuse") == DSM_OK;
-            return ctx_.err;
+        // after the bookkeeping: the frame is enqueued, so the host window follows the device whatever this returns
+        if (publishing_) snapshot_ = ctx_.done(dsm_publish_enqueue(ctx_.ctx, 5), "fuse") == DSM_OK;
+        if (distance_field_ && (!publishing_ || snapshot_))
+        { // centred on the fuse pose's translation, with the threshold of the published active cloud
+            const double c[3] = {last_fuse_pose_.x, last_fuse_pose_.y, last_fuse_pose_.z};
+            field_ = ctx_.done(dsm_field_enqueue(ctx_.ctx, c, 5), "fuse") == DSM_OK;
+        }
+        return publishing_ || distance_field_ ? ctx_.err : DSM_OK;
+    }
+    // the unread snapshot and field of the previous frame are retired (a pose callback may have enqueued loop-closure
+    // warps since, so neither can be reused); a capacity report stays with the readers
+    int retire_unread(const char *what)
+    {
+        if (snapshot_)
+        {
+            const int rc = dsm_publish_wait(ctx_.ctx, nullptr, nullptr, nullptr, nullptr, nullptr);
+            snapshot_ = false;
+            if (rc != DSM_OK && rc != DSM_E_CAPACITY) return ctx_.done(rc, what);
+        }
+        if (field_)
+        {
+            const int rc = dsm_field_wait(ctx_.ctx, nullptr, nullptr, nullptr);
+            field_ = false;
+            if (rc != DSM_OK && rc != DSM_E_CAPACITY) return ctx_.done(rc, what);
         }
         return DSM_OK;
     }
@@ -889,5 +924,6 @@ class SurfelMapNode
     int last_ref_;
     bool fused_;
     bool publishing_ = false, snapshot_ = false; // enable_publishing; a snapshot is enqueued and not yet handed out
+    bool distance_field_ = false, field_ = false; // enable_distance_field; a field is enqueued and not yet handed out
 };
 } // namespace dsm
