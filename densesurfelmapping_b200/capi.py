@@ -33,6 +33,7 @@ EXPORTS = [
     "dsm_frame_superpixel_image", "dsm_fuse_stream_window",
     "dsm_publish_enable", "dsm_publish_enqueue", "dsm_publish_wait", "dsm_debug_publish_chunks",
     "dsm_field_enable", "dsm_field_enqueue", "dsm_field_wait",
+    "dsm_field_enqueue_resident", "dsm_field_query_enable", "dsm_field_query_enqueue", "dsm_field_query_wait",
     "dsm_inactive_segments", "dsm_inactive_load", "dsm_map_save", "dsm_map_load", "dsm_map_peek",
     "dsm_checkpoint_enable", "dsm_checkpoint_enqueue", "dsm_checkpoint_wait", "dsm_debug_checkpoint_drain_ctas",
     "dsm_checkpoint_enqueue_incremental", "dsm_map_load_journal", "dsm_map_peek_journal", "dsm_journal_materialize",
@@ -55,6 +56,11 @@ class DsmConstants(ctypes.Structure):
 
 class DsmFieldParams(ctypes.Structure):
     _fields_ = [("voxel", ctypes.c_float), ("nx", ctypes.c_int32), ("ny", ctypes.c_int32), ("nz", ctypes.c_int32)]
+
+
+# dsm_field_query_wait's result records (include/dsm.h): a point sample and a trajectory clearance
+FIELD_SAMPLE_DTYPE = np.dtype([("dist", "<f4"), ("gx", "<f4"), ("gy", "<f4"), ("gz", "<f4")])
+CLEARANCE_DTYPE = np.dtype([("min_dist", "<f4"), ("argmin", "<i4"), ("first_hit", "<i4"), ("n_outside", "<i4")])
 
 
 CONSTANTS_DRIVE = (0.4, 0.5, 4.0, 0.1)    # fusion_functions.h:13-16
@@ -112,6 +118,10 @@ def load_library():
     L.dsm_field_enable.argtypes = [vp, ctypes.POINTER(DsmFieldParams)]
     L.dsm_field_enqueue.argtypes = [vp, ctypes.POINTER(ctypes.c_double), ci]
     L.dsm_field_wait.argtypes = [vp, ctypes.POINTER(vp), ctypes.POINTER(ctypes.c_int32), ctypes.POINTER(ci)]
+    L.dsm_field_enqueue_resident.argtypes = [vp, ctypes.POINTER(ctypes.c_double), ci]
+    L.dsm_field_query_enable.argtypes = [vp, ci, ci, ci]
+    L.dsm_field_query_enqueue.argtypes = [vp, vp, ci, vp, vp, ci, ctypes.c_float, ctypes.c_float]
+    L.dsm_field_query_wait.argtypes = [vp, ctypes.POINTER(vp), ctypes.POINTER(vp)]
     L.dsm_inactive_reserve.argtypes = [vp, ci]
     L.dsm_inactive_retire.argtypes = [vp, ci, ctypes.POINTER(ci)]
     L.dsm_inactive_reactivate.argtypes = [vp, ci, ctypes.POINTER(ci)]
@@ -544,27 +554,69 @@ class Context:
         self._ck(self.lib.dsm_field_enable(self.h, ctypes.byref(p)))
         self._field_shape = (int(nz), int(ny), int(nx))
 
-    def field_enqueue(self, center, min_update_times=5):
+    def field_enqueue(self, center, min_update_times=5, host_copy=True):
+        """host_copy=False: dsm_field_enqueue_resident, the grid stays on the device for field_query_*."""
         c = (ctypes.c_double * 3)(*[float(v) for v in center])
-        self._ck(self.lib.dsm_field_enqueue(self.h, c, int(min_update_times)))
+        fn = self.lib.dsm_field_enqueue if host_copy else self.lib.dsm_field_enqueue_resident
+        self._ck(fn(self.h, c, int(min_update_times)))
 
     def field_wait(self):
         """(dist, origin, n_occupied) of the enqueued field: dist a float32 [nz][ny][nx] copy of the context's pinned
-        buffer, origin an int32 (3,) array (x, y, z).  A field requested after a rejected frame raises
-        DsmError(DSM_E_CAPACITY) carrying the same tuple as `.field` (the map of the last applied frame)."""
+        buffer (None for a resident field), origin an int32 (3,) array (x, y, z).  A field requested after a rejected
+        frame raises DsmError(DSM_E_CAPACITY) carrying the same tuple as `.field` (the map of the last applied frame)."""
         ptr, org, nocc = ctypes.c_void_p(), (ctypes.c_int32 * 3)(), ctypes.c_int(0)
         rc = self.lib.dsm_field_wait(self.h, ctypes.byref(ptr), org, ctypes.byref(nocc))
         if rc not in (DSM_OK, -6):  # DSM_E_CAPACITY still carries the field
             self._ck(rc)
         shape = self._field_shape
         n = shape[0] * shape[1] * shape[2]
-        buf = (ctypes.c_float * n).from_address(ptr.value)
-        field = (np.frombuffer(buf, dtype=np.float32).reshape(shape).copy(), np.array(org[:], dtype=np.int32), nocc.value)
+        dist = None
+        if ptr.value:
+            buf = (ctypes.c_float * n).from_address(ptr.value)
+            dist = np.frombuffer(buf, dtype=np.float32).reshape(shape).copy()
+        field = (dist, np.array(org[:], dtype=np.int32), nocc.value)
         if rc != DSM_OK:
             err = DsmError(rc, self.lib.dsm_last_error(self.h).decode())
             err.field = field
             raise err
         return field
+
+    # ---- planner queries against the latest field ----
+    def field_query_enable(self, max_points, max_trajectories, max_waypoints):
+        self._ck(self.lib.dsm_field_query_enable(self.h, int(max_points), int(max_trajectories), int(max_waypoints)))
+
+    def field_query_enqueue(self, points=None, waypoints=None, offsets=None, step=1.0, radius=0.0):
+        """points (n, 3) and trajectories (waypoints (w, 3), offsets (t + 1,), int32) as float64 / int32 arrays, either
+        part may be None; step and radius in metres."""
+        pts = np.ascontiguousarray(np.zeros((0, 3)) if points is None else points, np.float64).reshape(-1, 3)
+        wp = np.ascontiguousarray(np.zeros((0, 3)) if waypoints is None else waypoints, np.float64).reshape(-1, 3)
+        ofs = np.ascontiguousarray(np.zeros(1) if offsets is None else offsets, np.int32).reshape(-1)
+        n_traj = max(len(ofs) - 1, 0)
+        self._ck(self.lib.dsm_field_query_enqueue(self.h, pts.ctypes.data if len(pts) else None, len(pts),
+                                                  wp.ctypes.data if len(wp) else None, ofs.ctypes.data if n_traj else None,
+                                                  n_traj, float(step), float(radius)))
+        self._query_counts = (len(pts), n_traj)
+
+    def field_query_wait(self):
+        """(samples, clearance): numpy copies of the context's pinned results, FIELD_SAMPLE_DTYPE (n_points,) and
+        CLEARANCE_DTYPE (n_trajectories,).  A query on a field taken after a rejected frame raises
+        DsmError(DSM_E_CAPACITY) carrying the same tuple as `.query`."""
+        ps, pc = ctypes.c_void_p(), ctypes.c_void_p()
+        rc = self.lib.dsm_field_query_wait(self.h, ctypes.byref(ps), ctypes.byref(pc))
+        if rc not in (DSM_OK, -6):
+            self._ck(rc)
+        n_pts, n_traj = self._query_counts
+
+        def take(ptr, n, dtype):
+            if n == 0:
+                return np.zeros(0, dtype)
+            return np.frombuffer((ctypes.c_uint8 * (n * dtype.itemsize)).from_address(ptr.value), dtype=dtype).copy()
+        out = (take(ps, n_pts, FIELD_SAMPLE_DTYPE), take(pc, n_traj, CLEARANCE_DTYPE))
+        if rc != DSM_OK:
+            err = DsmError(rc, self.lib.dsm_last_error(self.h).decode())
+            err.query = out
+            raise err
+        return out
 
     # ---- raw cloud of a frame ----
     def frame_raw_cloud(self, frame, pose7, cap=None):

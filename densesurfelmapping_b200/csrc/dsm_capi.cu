@@ -1450,9 +1450,9 @@ extern "C" int dsm_field_enable(dsm_ctx *ctx, const dsm_field_params *params)
 }
 
 // Enqueue only, like dsm_publish_enqueue: clear, mark, the three EDT passes and one copy of the grid with its header into
-// the pinned buffer, then the event.  The launches have no gate: after a rejected frame the map is the one of the last
-// applied frame, which is what the field reports.
-extern "C" int dsm_field_enqueue(dsm_ctx *ctx, const double center[3], int min_update_times)
+// the pinned buffer (host_copy), or of the header alone, then the event.  The launches have no gate: after a rejected
+// frame the map is the one of the last applied frame, which is what the field reports.
+static int field_enqueue(dsm_ctx *ctx, const double center[3], int min_update_times, bool host_copy)
 {
     if (!ctx || !center || min_update_times < 1) return DSM_E_INVALID;
     DsmField *f = ctx->field.get();
@@ -1480,11 +1480,26 @@ extern "C" int dsm_field_enqueue(dsm_ctx *ctx, const double center[3], int min_u
                           s ? std::min(s->upper, s->cap) : 0, g, f->occ, header, ctx->stream);
     dsm_launch_field_edt(g, f->occ, f->dist, header, ctx->stream);
     CK(cudaGetLastError());
-    CK(cudaMemcpyAsync(f->host, f->dist, f->bytes, cudaMemcpyDeviceToHost, ctx->stream));
+    if (host_copy)
+        CK(cudaMemcpyAsync(f->host, f->dist, f->bytes, cudaMemcpyDeviceToHost, ctx->stream));
+    else
+        CK(cudaMemcpyAsync(f->host + dsm_field_header(f->voxels), header, DSM_FIELD_WORDS * sizeof(int32_t), cudaMemcpyDeviceToHost,
+                           ctx->stream));
     CK(cudaEventRecord(f->ev, ctx->stream));
     f->g = g;
-    f->in_flight = true;
+    f->in_flight = f->requested = true;
+    f->resident = !host_copy;
     return DSM_OK;
+}
+
+extern "C" int dsm_field_enqueue(dsm_ctx *ctx, const double center[3], int min_update_times)
+{
+    return field_enqueue(ctx, center, min_update_times, true);
+}
+
+extern "C" int dsm_field_enqueue_resident(dsm_ctx *ctx, const double center[3], int min_update_times)
+{
+    return field_enqueue(ctx, center, min_update_times, false);
 }
 
 extern "C" int dsm_field_wait(dsm_ctx *ctx, const float **dist, int32_t origin[3], int *n_occupied)
@@ -1496,12 +1511,129 @@ extern "C" int dsm_field_wait(dsm_ctx *ctx, const float **dist, int32_t origin[3
     CK(cudaEventSynchronize(f->ev));
     f->in_flight = false;
     const int32_t *h = f->host + dsm_field_header(f->voxels);
-    if (dist) *dist = reinterpret_cast<const float *>(f->host);
+    if (dist) *dist = f->resident ? nullptr : reinterpret_cast<const float *>(f->host);
     if (origin) origin[0] = f->g.o[0], origin[1] = f->g.o[1], origin[2] = f->g.o[2];
     if (n_occupied) *n_occupied = h[DSM_FIELD_N_OCCUPIED];
     if (h[DSM_FIELD_ERR_TAG] == 0) return DSM_OK;
     snprintf(ctx->err, sizeof(ctx->err), "dsm_field_wait: frame %d of a dsm_fuse_stream_window call did not fit the pool or the "
              "store; the field holds the frames before it", h[DSM_FIELD_ERR_FRAME]);
+    return DSM_E_CAPACITY;
+}
+
+// ---- planner queries against the latest field (include/dsm.h, DESIGN.md §8.8) ----
+extern "C" int dsm_field_query_enable(dsm_ctx *ctx, int max_points, int max_trajectories, int max_waypoints)
+{
+    if (!ctx) return DSM_E_INVALID;
+    if (!ctx->field || ctx->field_query) return DSM_E_STATE;
+    for (int n : {max_points, max_trajectories, max_waypoints})
+        if (n < 0 || n > DSM_FIELD_QUERY_MAX_SAMPLES) return DSM_E_INVALID;
+    CK(cudaSetDevice(ctx->device));
+    auto q = std::make_unique<DsmFieldQuery>();
+    q->max_points = max_points, q->max_traj = max_trajectories, q->max_wp = max_waypoints;
+    const size_t req = DsmFieldQuery::req_bytes(max_points, max_waypoints, max_trajectories);
+    const size_t res = DsmFieldQuery::res_bytes(max_points, max_trajectories);
+    cudaError_t e = q->own.host(&q->req_host, req);
+    if (e == cudaSuccess) e = q->own.device(&q->req_dev, req);
+    if (e == cudaSuccess) e = q->own.device(&q->res_dev, res);
+    if (e == cudaSuccess) e = q->own.host(&q->res_host, res);
+    if (e == cudaSuccess) e = q->own.event(&q->ev);
+    if (e != cudaSuccess)
+    {
+        cudaGetLastError();
+        return DSM_E_NOMEM; // nothing is kept: a later call may try again
+    }
+    ctx->field_query = std::move(q);
+    return DSM_OK;
+}
+
+// Stages the request on the calling thread (checking it and counting the samples on the way), then enqueues one H2D
+// copy, the two kernels on the grid of the latest field request, one D2H copy of the results and the event.
+extern "C" int dsm_field_query_enqueue(dsm_ctx *ctx, const double *points, int n_points, const double *waypoints, const int32_t *offsets,
+                                       int n_trajectories, float step, float radius)
+{
+    if (!ctx) return DSM_E_INVALID;
+    DsmFieldQuery *q = ctx->field_query.get();
+    const DsmField *f = ctx->field.get();
+    if (!q || !f || !f->requested || q->in_flight) return DSM_E_STATE;
+    if (n_points < 0 || n_points > q->max_points || n_trajectories < 0 || n_trajectories > q->max_traj) return DSM_E_INVALID;
+    if ((n_points > 0 && !points) || (n_trajectories > 0 && (!waypoints || !offsets))) return DSM_E_INVALID;
+    if (!std::isfinite(step) || !(step > 0.f) || !std::isfinite(radius) || !(radius >= 0.f)) return DSM_E_INVALID;
+    const int n_wp = n_trajectories > 0 ? offsets[n_trajectories] : 0;
+    if (n_trajectories > 0)
+    {
+        if (offsets[0] != 0 || n_wp > q->max_wp) return DSM_E_INVALID;
+        for (int j = 0; j < n_trajectories; j++)
+            if (offsets[j + 1] <= offsets[j]) return DSM_E_INVALID;
+    }
+    // the packed request (dsm_device.cuh)
+    uint8_t *h = q->req_host;
+    double *h_pts = reinterpret_cast<double *>(h), *h_wp = h_pts + 3 * (size_t)n_points;
+    int32_t *h_ofs = reinterpret_cast<int32_t *>(h_wp + 3 * (size_t)n_wp), *h_first = h_ofs + n_trajectories + 1;
+    if (n_points > 0) std::memcpy(h_pts, points, 24 * (size_t)n_points);
+    // one pass over the waypoints: copy, check, and count each segment's samples m = max(1, ceil(L / step)).  The
+    // ceil is an integer test, exact once q = L / step is known to be at most 2^26 (a NaN or infinite q fails that).
+    const double dstep = (double)step;
+    int64_t total = 0; // samples of the call so far
+    for (int j = 0; j < n_trajectories; j++)
+    {
+        const int w0 = offsets[j], w1 = offsets[j + 1];
+        int64_t s = 0; // samples of trajectory j so far
+        for (int w = w0; w < w1; w++)
+        {
+            const double *a = waypoints + 3 * (size_t)w;
+            double *c = h_wp + 3 * (size_t)w;
+            c[0] = a[0], c[1] = a[1], c[2] = a[2];
+            if (!std::isfinite(a[0]) || !std::isfinite(a[1]) || !std::isfinite(a[2])) return DSM_E_INVALID;
+            h_first[w] = (int32_t)s;
+            int64_t m = 1; // the last waypoint: one sample
+            if (w + 1 < w1)
+            {
+                const double *b = a + 3;
+                const double dx = b[0] - a[0], dy = b[1] - a[1], dz = b[2] - a[2];
+                const double q = std::sqrt((dx * dx + dy * dy) + dz * dz) / dstep;
+                if (!(q <= (double)DSM_FIELD_QUERY_MAX_SAMPLES)) return DSM_E_INVALID;
+                m = (int64_t)q;
+                m += (double)m < q;
+                m = std::max<int64_t>(m, 1);
+            }
+            if (m > DSM_FIELD_QUERY_MAX_SAMPLES - total - s) return DSM_E_INVALID;
+            s += m;
+        }
+        total += s;
+    }
+    if (n_trajectories > 0) std::memcpy(h_ofs, offsets, 4 * ((size_t)n_trajectories + 1));
+    CK(cudaSetDevice(ctx->device));
+    const size_t req = DsmFieldQuery::req_bytes(n_points, n_wp, n_trajectories);
+    CK(cudaMemcpyAsync(q->req_dev, q->req_host, req, cudaMemcpyHostToDevice, ctx->stream));
+    const double *d_pts = reinterpret_cast<const double *>(q->req_dev), *d_wp = d_pts + 3 * (size_t)n_points;
+    const int32_t *d_ofs = reinterpret_cast<const int32_t *>(d_wp + 3 * (size_t)n_wp), *d_first = d_ofs + n_trajectories + 1;
+    int32_t *r_hdr = reinterpret_cast<int32_t *>(q->res_dev);
+    float4 *r_samples = reinterpret_cast<float4 *>(q->res_dev + 16);
+    dsm_clearance_t *r_clear = reinterpret_cast<dsm_clearance_t *>(q->res_dev + DsmFieldQuery::res_clearance(n_points));
+    dsm_launch_field_query(reinterpret_cast<const float *>(f->dist), f->dist + dsm_field_header(f->voxels), f->g, d_pts, n_points, d_wp,
+                           d_ofs, d_first, n_trajectories, radius, r_hdr, r_samples, r_clear, ctx->stream);
+    CK(cudaGetLastError());
+    CK(cudaMemcpyAsync(q->res_host, q->res_dev, DsmFieldQuery::res_bytes(n_points, n_trajectories), cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaEventRecord(q->ev, ctx->stream));
+    q->n_points = n_points, q->n_traj = n_trajectories;
+    q->in_flight = true;
+    return DSM_OK;
+}
+
+extern "C" int dsm_field_query_wait(dsm_ctx *ctx, const dsm_field_sample_t **samples, const dsm_clearance_t **clearance)
+{
+    if (!ctx) return DSM_E_INVALID;
+    DsmFieldQuery *q = ctx->field_query.get();
+    if (!q || !q->in_flight) return DSM_E_STATE;
+    CK(cudaSetDevice(ctx->device));
+    CK(cudaEventSynchronize(q->ev));
+    q->in_flight = false;
+    const int32_t *h = reinterpret_cast<const int32_t *>(q->res_host);
+    if (samples) *samples = reinterpret_cast<const dsm_field_sample_t *>(q->res_host + 16);
+    if (clearance) *clearance = reinterpret_cast<const dsm_clearance_t *>(q->res_host + DsmFieldQuery::res_clearance(q->n_points));
+    if (h[DSM_QUERY_ERR_TAG] == 0) return DSM_OK;
+    snprintf(ctx->err, sizeof(ctx->err), "dsm_field_query_wait: frame %d of a dsm_fuse_stream_window call did not fit the pool or the "
+             "store; the field the query read holds the frames before it", h[DSM_QUERY_ERR_FRAME]);
     return DSM_E_CAPACITY;
 }
 

@@ -181,6 +181,24 @@ struct DsmField
     int32_t *dist = nullptr, *host = nullptr; // device grid, pinned copy
     cudaEvent_t ev = nullptr;
     bool in_flight = false; // enqueued and not yet waited for
+    bool requested = false; // a field has been enqueued: the device grid is one a query may read
+    bool resident = false;  // the latest request copies only its header words (dsm_field_enqueue_resident)
+};
+
+// dsm_field_query_* (DESIGN.md §8.8): the packed request (pinned staging and its device twin), the packed result
+// (device and its pinned copy) at the capacities of dsm_field_query_enable, and the event after the result's copy
+struct DsmFieldQuery
+{
+    CudaOwner own;
+    int max_points = 0, max_traj = 0, max_wp = 0;
+    uint8_t *req_host = nullptr, *req_dev = nullptr, *res_host = nullptr, *res_dev = nullptr;
+    cudaEvent_t ev = nullptr;
+    int n_points = 0, n_traj = 0; // of the query in flight or last waited for
+    bool in_flight = false;
+    // byte offsets of the packed layouts (dsm_device.cuh) for n_points, n_wp and n_traj
+    static size_t req_bytes(int n_points, int n_wp, int n_traj) { return 24 * ((size_t)n_points + n_wp) + 4 * ((size_t)n_traj + 1 + n_wp); }
+    static size_t res_clearance(int n_points) { return 16 * (1 + (size_t)n_points); }
+    static size_t res_bytes(int n_points, int n_traj) { return res_clearance(n_points) + 16 * (size_t)n_traj; }
 };
 
 #define DSM_MAX_CHUNKS 4
@@ -252,6 +270,7 @@ struct dsm_ctx
     cudaEvent_t pub_ev = nullptr;
     std::unique_ptr<DsmCheckpoint> ckpt; // nullptr until dsm_checkpoint_enable
     std::unique_ptr<DsmField> field;     // nullptr until dsm_field_enable
+    std::unique_ptr<DsmFieldQuery> field_query; // nullptr until dsm_field_query_enable
     int run_split = 2;          // sub-batches per dsm_batch_run (dsm_set_concurrency)
     // pinned host staging for the small per-batch tables
     float *h_pose = nullptr; // [2B][32]: pose then inverse; first half: the batch calls, second half: the resident stream

@@ -298,3 +298,20 @@ void dsm_launch_field_mark(const dsm_surfel_t *pool, const int32_t *res, int poo
                            const int32_t *store_size, int store_upper, const DsmFieldGrid &g, uint8_t *occ, int32_t *header, cudaStream_t s);
 // the three EDT passes: occ -> dist (in place from the second pass on); header[DSM_FIELD_N_OCCUPIED] must be zeroed
 void dsm_launch_field_edt(const DsmFieldGrid &g, const uint8_t *occ, int32_t *dist, int32_t *header, cudaStream_t s);
+
+// dsm_field_query_* (DESIGN.md §8.8), dsm_field.cu.  One packed request (H2D) and one packed result (D2H):
+//   request  double points[n_points][3] | double waypoints[n_wp][3] | int32 offsets[n_traj + 1] | int32 first[n_wp]
+//            (first[w]: the trajectory's index of waypoint w's first sample, staged by the host; the last waypoint's
+//            entry is the index of the final sample)
+//   result   int32 header[DSM_QUERY_WORDS] | float4 samples[n_points] | dsm_clearance_t clearance[n_traj]
+enum
+{
+    DSM_QUERY_ERR_TAG,   // the field header's DSM_FIELD_ERR_TAG / _ERR_FRAME, copied by k_field_query
+    DSM_QUERY_ERR_FRAME,
+    DSM_QUERY_WORDS = 4  // 16 B: the samples stay float4-aligned
+};
+// k_field_query over n_points (CTA 0 also copies the error words; launched with one CTA at least) and
+// k_field_clearance over n_traj trajectories, both on the grid `dist` with its header (at dsm_field_header(voxels))
+void dsm_launch_field_query(const float *dist, const int32_t *field_header, const DsmFieldGrid &g, const double *points, int n_points,
+                            const double *waypoints, const int32_t *offsets, const int32_t *first, int n_traj, float radius,
+                            int32_t *result_header, float4 *samples, dsm_clearance_t *clearance, cudaStream_t s);

@@ -179,6 +179,138 @@ __global__ void __launch_bounds__(32) k_field_lines(int32_t *dist, int nx, int l
     }
 }
 
+// ---- planner queries against the latest field (dsm_field_query_*, DESIGN.md §8.8) ----
+//   k_field_query      one thread per point: fp64 addressing, eight gathers from the grid (L2-resident at planner
+//                      sizes), trilinear distance and gradient in fp32, one float4 store.
+//   k_field_clearance  one warp per trajectory, the lanes on consecutive samples; each lane walks the host-staged
+//                      segment starts, so the device never rounds a sample count.  A shuffle reduction gives the
+//                      minimum (ties to the lower index), the lowest hit and the outside count: the result is the same
+//                      whatever the schedule.
+// Every fp32 step is an explicit _rn intrinsic, so the numpy restatement (oracle/pyoracle_field_query.py) is bit-exact.
+#define FIELD_QUERY_BLOCK 256
+#define FIELD_CLEAR_WARPS 8
+
+__device__ __forceinline__ float q_lerp(float a, float b, float t) { return __fadd_rn(a, __fmul_rn(t, __fsub_rn(b, a))); }
+
+// one axis of the addressing: false outside (NaN included); else the lower and upper corner and the fraction
+__device__ __forceinline__ bool q_axis(double p, double v, int o, int n, int &i, int &j, float &t)
+{
+    const double u = p / v - (double)o - 0.5;
+    if (!(u >= 0.0 && u <= (double)(n - 1))) return false;
+    i = min((int)floor(u), max(n - 2, 0));
+    j = min(i + 1, n - 1);
+    t = (float)(u - (double)i);
+    return true;
+}
+
+// the point query at p: dist (and, with GRAD, the gradient) per include/dsm.h; inside = the point is inside the grid
+template <bool GRAD>
+__device__ __forceinline__ float4 q_sample(const float *__restrict__ dist, const DsmFieldGrid &g, bool empty, double px, double py, double pz,
+                                           bool &inside)
+{
+    const double v = (double)g.voxel;
+    int ix, jx, iy, jy, iz, jz;
+    float tx, ty, tz;
+    inside = q_axis(px, v, g.o[0], g.n[0], ix, jx, tx) && q_axis(py, v, g.o[1], g.n[1], iy, jy, ty) && q_axis(pz, v, g.o[2], g.n[2], iz, jz, tz);
+    if (!inside) return make_float4(__int_as_float(0x7fc00000), 0.f, 0.f, 0.f);
+    if (empty) return make_float4(INFINITY, 0.f, 0.f, 0.f);
+    const size_t nx = (size_t)g.n[0], ny = (size_t)g.n[1];
+    const size_t r00 = (iz * ny + iy) * nx, r10 = (iz * ny + jy) * nx, r01 = (jz * ny + iy) * nx, r11 = (jz * ny + jy) * nx;
+    const float c000 = __ldg(dist + r00 + ix), c100 = __ldg(dist + r00 + jx), c010 = __ldg(dist + r10 + ix), c110 = __ldg(dist + r10 + jx);
+    const float c001 = __ldg(dist + r01 + ix), c101 = __ldg(dist + r01 + jx), c011 = __ldg(dist + r11 + ix), c111 = __ldg(dist + r11 + jx);
+    float4 r;
+    r.x = q_lerp(q_lerp(q_lerp(c000, c100, tx), q_lerp(c010, c110, tx), ty), q_lerp(q_lerp(c001, c101, tx), q_lerp(c011, c111, tx), ty), tz);
+    if (GRAD)
+    {
+        r.y = __fdiv_rn(q_lerp(q_lerp(__fsub_rn(c100, c000), __fsub_rn(c110, c010), ty), q_lerp(__fsub_rn(c101, c001), __fsub_rn(c111, c011), ty), tz), g.voxel);
+        r.z = __fdiv_rn(q_lerp(q_lerp(__fsub_rn(c010, c000), __fsub_rn(c110, c100), tx), q_lerp(__fsub_rn(c011, c001), __fsub_rn(c111, c101), tx), tz), g.voxel);
+        r.w = __fdiv_rn(q_lerp(q_lerp(__fsub_rn(c001, c000), __fsub_rn(c101, c100), tx), q_lerp(__fsub_rn(c011, c010), __fsub_rn(c111, c110), tx), ty), g.voxel);
+    }
+    else
+        r.y = r.z = r.w = 0.f;
+    return r;
+}
+
+__global__ void __launch_bounds__(FIELD_QUERY_BLOCK) k_field_query(const float *__restrict__ dist, const int32_t *__restrict__ fhdr, const DsmFieldGrid g,
+                                                                   const double *__restrict__ pts, int n, float4 *__restrict__ out, int32_t *rhdr)
+{
+    if (blockIdx.x == 0 && threadIdx.x == 0)
+    { // the field's error words at its request travel with the query's results
+        rhdr[DSM_QUERY_ERR_TAG] = fhdr[DSM_FIELD_ERR_TAG];
+        rhdr[DSM_QUERY_ERR_FRAME] = fhdr[DSM_FIELD_ERR_FRAME];
+    }
+    const int i = blockIdx.x * FIELD_QUERY_BLOCK + threadIdx.x;
+    if (i >= n) return;
+    const double *p = pts + 3 * (size_t)i;
+    bool inside;
+    out[i] = q_sample<true>(dist, g, fhdr[DSM_FIELD_N_OCCUPIED] == 0, p[0], p[1], p[2], inside);
+}
+
+__global__ void __launch_bounds__(32 * FIELD_CLEAR_WARPS) k_field_clearance(const float *__restrict__ dist, const int32_t *__restrict__ fhdr,
+                                                                            const DsmFieldGrid g, const double *__restrict__ wp,
+                                                                            const int32_t *__restrict__ offsets, const int32_t *__restrict__ first,
+                                                                            int n_traj, float radius, dsm_clearance_t *__restrict__ out)
+{
+    const int lane = threadIdx.x & 31, traj = blockIdx.x * FIELD_CLEAR_WARPS + (threadIdx.x >> 5);
+    if (traj >= n_traj) return; // whole warps only
+    const bool empty = fhdr[DSM_FIELD_N_OCCUPIED] == 0;
+    const int last = offsets[traj + 1] - 1, total = first[last] + 1;
+    float best = INFINITY;
+    int arg = INT_MAX, hit = INT_MAX, outside = 0; // INT_MAX: none yet
+    int w = offsets[traj]; // the segment of this lane's sample: first[w] <= s < first[w + 1], or w == last
+    for (int s = lane; s < total; s += 32)
+    {
+        while (w < last && first[w + 1] <= s) w++;
+        const double *a = wp + 3 * (size_t)w;
+        double px = a[0], py = a[1], pz = a[2];
+        if (w < last)
+        {
+            const double *b = a + 3;
+            const double f = (double)(s - first[w]) / (double)(first[w + 1] - first[w]);
+            px = __dadd_rn(px, __dmul_rn(f, __dsub_rn(b[0], a[0])));
+            py = __dadd_rn(py, __dmul_rn(f, __dsub_rn(b[1], a[1])));
+            pz = __dadd_rn(pz, __dmul_rn(f, __dsub_rn(b[2], a[2])));
+        }
+        bool inside;
+        const float d = q_sample<false>(dist, g, empty, px, py, pz, inside).x;
+        if (!inside)
+        {
+            outside++;
+            continue;
+        }
+        if (arg == INT_MAX || d < best) best = d, arg = s; // this lane's samples rise: the first minimum stays
+        if (hit == INT_MAX && d < radius) hit = s;
+    }
+    for (int k = 16; k > 0; k >>= 1)
+    {
+        const float ob = __shfl_xor_sync(0xffffffffu, best, k);
+        const int oa = __shfl_xor_sync(0xffffffffu, arg, k);
+        hit = min(hit, __shfl_xor_sync(0xffffffffu, hit, k));
+        outside += __shfl_xor_sync(0xffffffffu, outside, k);
+        if (oa != INT_MAX && (arg == INT_MAX || ob < best || (ob == best && oa < arg))) best = ob, arg = oa;
+    }
+    if (lane == 0)
+    {
+        dsm_clearance_t c;
+        c.min_dist = best;
+        c.argmin = arg == INT_MAX ? -1 : arg;
+        c.first_hit = hit == INT_MAX ? -1 : hit;
+        c.n_outside = outside;
+        out[traj] = c;
+    }
+}
+
+void dsm_launch_field_query(const float *dist, const int32_t *field_header, const DsmFieldGrid &g, const double *points, int n_points,
+                            const double *waypoints, const int32_t *offsets, const int32_t *first, int n_traj, float radius,
+                            int32_t *result_header, float4 *samples, dsm_clearance_t *clearance, cudaStream_t s)
+{
+    const int qb = (n_points + FIELD_QUERY_BLOCK - 1) / FIELD_QUERY_BLOCK;
+    k_field_query<<<qb > 1 ? qb : 1, FIELD_QUERY_BLOCK, 0, s>>>(dist, field_header, g, points, n_points, samples, result_header);
+    if (n_traj > 0)
+        k_field_clearance<<<(n_traj + FIELD_CLEAR_WARPS - 1) / FIELD_CLEAR_WARPS, 32 * FIELD_CLEAR_WARPS, 0, s>>>(
+            dist, field_header, g, waypoints, offsets, first, n_traj, radius, clearance);
+}
+
 int dsm_field_setup()
 {
     const int smem = 1024 * 32 * 4; // the longest line

@@ -480,6 +480,67 @@ typedef struct dsm_field_params
 int dsm_field_enable(dsm_ctx *ctx, const dsm_field_params *params);
 int dsm_field_enqueue(dsm_ctx *ctx, const double center[3], int min_update_times);
 int dsm_field_wait(dsm_ctx *ctx, const float **dist, int32_t origin[3], int *n_occupied);
+/* dsm_field_enqueue_resident: dsm_field_enqueue (same checks, ordering, kernels and grid) that copies only the header
+ * words to the host; the grid stays on the device for dsm_field_query_*.  dsm_field_wait on such a request returns
+ * *dist = NULL with the same origin, n_occupied and DSM_E_CAPACITY contract. */
+int dsm_field_enqueue_resident(dsm_ctx *ctx, const double center[3], int min_update_times);
+
+/* ---- planner queries against the latest distance field, on the device (DESIGN.md §8.8) ----
+ * A query reads the grid of the latest field request (either enqueue call, waited for or not), in stream order behind
+ * it, with that request's origin o and voxel edge v captured at the query's enqueue; a later field request may be
+ * enqueued while a query is in flight and does not change what the query reads.  Only the grid is read, never the map.
+ *
+ * Point query (fp64 addressing, fp32 arithmetic; voxel x covers [(o + x) v, (o + x + 1) v), its value at the centre).
+ * Per axis k: u_k = p_k / (double)v - (double)o_k - 0.5 in fp64.  The point is inside when 0 <= u_k <= n_k - 1 on every
+ * axis (fp64 compares, NaN fails); then i_k = min(floor(u_k), max(n_k - 2, 0)), j_k = min(i_k + 1, n_k - 1) and
+ * t_k = (float)(u_k - i_k).  With lerp(a, b, t) = a + t * (b - a) in fp32 (one rounding per operation) and c_xyz the
+ * corner taking i or j per axis (c100 takes j on x):
+ *   dist = lerp(lerp(lerp(c000, c100, tx), lerp(c010, c110, tx), ty), lerp(lerp(c001, c101, tx), lerp(c011, c111, tx), ty), tz)
+ *   gx   = lerp(lerp(c100 - c000, c110 - c010, ty), lerp(c101 - c001, c111 - c011, ty), tz) / v
+ *   gy   = lerp(lerp(c010 - c000, c110 - c100, tx), lerp(c011 - c001, c111 - c101, tx), tz) / v
+ *   gz   = lerp(lerp(c001 - c000, c101 - c100, tx), lerp(c011 - c010, c111 - c110, tx), ty) / v
+ * Outside: dist is the canonical quiet NaN (unknown, not free) and the gradient 0.  A field with no occupied voxel gives
+ * every inside point dist = +INFINITY and a zero gradient.
+ *
+ * Trajectory clearance.  Trajectory j is the polyline of waypoints offsets[j] .. offsets[j + 1] - 1, sampled in fp64:
+ * each segment a -> b with L = sqrt((dx^2 + dy^2) + dz^2) and m = max(1, ceil(L / (double)step)) (counted on the host)
+ * gives the samples a + ((double)s / m) * (b - a), s in [0, m); the last waypoint is sampled once at the end.  Samples
+ * are numbered along the trajectory from 0; each is a point query (distance only).  Per trajectory: min_dist the minimum
+ * dist over the inside samples (+INFINITY when none is inside), argmin the lowest sample index attaining it (-1),
+ * first_hit the lowest index of an inside sample with dist < radius (-1 when none), n_outside the samples outside.
+ *
+ *   dsm_field_query_enable   once, after dsm_field_enable (DSM_E_STATE otherwise).  Allocates, for these capacities, one
+ *                            packed pinned request buffer and its device twin, one packed device result buffer and its
+ *                            pinned copy, and an event.  DSM_E_INVALID for a negative capacity or one above 2^26;
+ *                            DSM_E_NOMEM with nothing kept.
+ *   dsm_field_query_enqueue  stages points (n_points x 3 doubles), waypoints and offsets (n_trajectories + 1 ints) into
+ *                            pinned memory on the calling thread, then enqueues one H2D copy, the kernels, one D2H copy
+ *                            of the results and the event on the context's stream; never waits.  A pointer may be NULL
+ *                            when its count is 0.  DSM_E_STATE before dsm_field_query_enable, before any field request
+ *                            and while a query is in flight.  DSM_E_INVALID for a negative count or one over capacity
+ *                            (offsets[n_trajectories] counts the waypoints), offsets[0] != 0 or offsets that do not rise
+ *                            strictly, a non-finite waypoint, a step that is not finite and > 0, a radius that is not
+ *                            finite and >= 0, or more than 2^26 trajectory samples in the call (this bounds the work of
+ *                            one call).  Points may be anything: a NaN or infinite point is outside.
+ *   dsm_field_query_wait     waits for that query only.  *samples (n_points) and *clearance (n_trajectories) are the
+ *                            context's pinned result arrays, valid until the next dsm_field_query_enqueue; either
+ *                            out-pointer may be NULL.  If the field the query read was taken after a rejected frame,
+ *                            returns DSM_E_CAPACITY with valid results and does NOT clear the error, as dsm_field_wait.
+ *                            DSM_E_STATE with no query enqueued. */
+typedef struct dsm_field_sample_t
+{
+    float dist, gx, gy, gz; /* metres, per metre */
+} dsm_field_sample_t;
+typedef struct dsm_clearance_t
+{
+    float min_dist;
+    int32_t argmin, first_hit, n_outside;
+} dsm_clearance_t;
+#define DSM_FIELD_QUERY_MAX_SAMPLES (1 << 26)
+int dsm_field_query_enable(dsm_ctx *ctx, int max_points, int max_trajectories, int max_waypoints);
+int dsm_field_query_enqueue(dsm_ctx *ctx, const double *points, int n_points, const double *waypoints, const int32_t *offsets,
+                            int n_trajectories, float step, float radius);
+int dsm_field_query_wait(dsm_ctx *ctx, const dsm_field_sample_t **samples, const dsm_clearance_t **clearance);
 
 /* ---- checkpoints that do not stop the stream (DESIGN.md §8.5) ----
  * The file of dsm_map_save, taken in stream order like a publish snapshot: the resident stream pays one device-to-device

@@ -63,7 +63,11 @@
 // cloud's threshold of 5 updates (dsm_field_enqueue(ctx, centre, 5), DESIGN.md §8.7).  distance_field() hands it out
 // with the same one-frame-late pattern, lifetime and capacity rule as published_clouds(); an unread field is retired
 // before the next fuse and before load_state*, as an unread snapshot is.  Without enable_distance_field() nothing is
-// enqueued.
+// enqueued.  enable_distance_field(..., false) keeps every field on the device (dsm_field_enqueue_resident):
+// distance_field() then hands out dist == nullptr with the origin and the count, and the planner asks the field what it
+// needs instead (DESIGN.md §8.8): after enable_field_queries(), field_samples() (distance and gradient at points) and
+// trajectory_clearance() (the clearance of candidate paths) read the field of the latest fused frame, one enqueue and
+// one wait each, without touching the one-frame-late distance_field() handout.
 // device < 0 builds the node without a context: the callbacks run the whole pose logic (pose database, sync, window
 // bookkeeping) and fuse nothing; any call that reads the map returns DSM_E_STATE.
 #pragma once
@@ -460,14 +464,36 @@ class SurfelMapNode
         return ctx_.done(dsm_publish_wait(ctx_.ctx, &active, &n_active, &inactive, &n_inactive, &inactive_changed_from), "published_clouds");
     }
     // ---- the map as a distance field around the camera, for a planner (see the top of this file, DESIGN.md §8.7) ----
-    int enable_distance_field(float voxel, int nx, int ny, int nz)
+    // host_copy = false: the grid stays on the device; distance_field() hands out dist == nullptr
+    int enable_distance_field(float voxel, int nx, int ny, int nz, bool host_copy = true)
     {
         const dsm_field_params p = {voxel, nx, ny, nz};
-        if (ctx_.run("enable_distance_field", [&] { return dsm_field_enable(ctx_.ctx, &p); }) == DSM_OK) distance_field_ = true;
+        if (ctx_.run("enable_distance_field", [&] { return dsm_field_enable(ctx_.ctx, &p); }) == DSM_OK)
+            distance_field_ = true, field_host_copy_ = host_copy;
         return ctx_.err;
     }
+    // ---- planner queries against the field of the latest fused frame (DESIGN.md §8.8) ----
+    // once, after enable_distance_field: the capacities of one query
+    int enable_field_queries(int max_points, int max_trajectories, int max_waypoints)
+    {
+        return ctx_.run("enable_field_queries", [&] { return dsm_field_query_enable(ctx_.ctx, max_points, max_trajectories, max_waypoints); });
+    }
+    // distance and gradient at n points (xyz doubles); out receives n samples.  DSM_E_STATE when no field exists;
+    // DSM_E_CAPACITY with the samples of the last applied frame's field, as distance_field().
+    int field_samples(const double *points, int n, std::vector<dsm_field_sample_t> &out)
+    {
+        out.clear();
+        return query("field_samples", points, n, nullptr, nullptr, 0, 1.f, 0.f, &out, nullptr);
+    }
+    // the clearance of n trajectories (waypoints xyz doubles, offsets[n + 1]) sampled every `step` metres against
+    // `radius`; out receives n records (include/dsm.h)
+    int trajectory_clearance(const double *waypoints, const int32_t *offsets, int n, float step, float radius, std::vector<dsm_clearance_t> &out)
+    {
+        out.clear();
+        return query("trajectory_clearance", nullptr, 0, waypoints, offsets, n, step, radius, nullptr, &out);
+    }
     // the field of the latest fused frame: dist [nz][ny][nx] in metres (the library's pinned buffer, valid until the next
-    // frame is fused), the grid's origin in voxels and the occupied voxels.  DSM_E_STATE when no frame has been fused
+    // frame is fused; nullptr for a field kept on the device), the grid's origin in voxels and the occupied voxels.  DSM_E_STATE when no frame has been fused
     // since the last call; DSM_E_CAPACITY with the field of the last applied frame, as published_clouds().
     int distance_field(const float *&dist, int32_t origin[3], int &n_occupied)
     {
@@ -589,6 +615,24 @@ class SurfelMapNode
     dsm_ctx *context() { return ctx_.ctx; }
 
   private:
+    int query(const char *what, const double *points, int n_points, const double *waypoints, const int32_t *offsets, int n_traj, float step,
+              float radius, std::vector<dsm_field_sample_t> *samples, std::vector<dsm_clearance_t> *clearance)
+    {
+        if (!ctx_.ready(what)) return ctx_.err;
+        if (!field_exists_) return ctx_.done(DSM_E_STATE, what);
+        int rc = dsm_field_query_enqueue(ctx_.ctx, points, n_points, waypoints, offsets, n_traj, step, radius);
+        if (rc != DSM_OK) return ctx_.done(rc, what);
+        const dsm_field_sample_t *s = nullptr;
+        const dsm_clearance_t *c = nullptr;
+        rc = dsm_field_query_wait(ctx_.ctx, &s, &c);
+        if (rc == DSM_OK || rc == DSM_E_CAPACITY)
+        {
+            if (samples) samples->assign(s, s + n_points);
+            if (clearance) clearance->assign(c, c + n_traj);
+        }
+        return ctx_.done(rc, what);
+    }
+
     // load_state / load_state_incremental: the file (journal = false) or base + journal (true) peeked and checked against
     // this node before the map is touched, then loaded
     int load_from(const std::string &path, bool journal, int *records, const char *what)
@@ -626,6 +670,7 @@ class SurfelMapNode
         last_fuse_pose_ = s.last_fuse_pose;
         last_ref_ = s.last_ref;
         fused_ = s.fused;
+        field_exists_ = false; // the loaded map has no field until its next fused frame
         return ctx_.done(DSM_OK, what);
     }
 
@@ -856,7 +901,8 @@ class SurfelMapNode
         if (distance_field_ && (!publishing_ || snapshot_))
         { // centred on the fuse pose's translation, with the threshold of the published active cloud
             const double c[3] = {last_fuse_pose_.x, last_fuse_pose_.y, last_fuse_pose_.z};
-            field_ = ctx_.done(dsm_field_enqueue(ctx_.ctx, c, 5), "fuse") == DSM_OK;
+            field_ = ctx_.done(field_host_copy_ ? dsm_field_enqueue(ctx_.ctx, c, 5) : dsm_field_enqueue_resident(ctx_.ctx, c, 5), "fuse") == DSM_OK;
+            field_exists_ = field_exists_ || field_;
         }
         return publishing_ || distance_field_ ? ctx_.err : DSM_OK;
     }
@@ -925,5 +971,7 @@ class SurfelMapNode
     bool fused_;
     bool publishing_ = false, snapshot_ = false; // enable_publishing; a snapshot is enqueued and not yet handed out
     bool distance_field_ = false, field_ = false; // enable_distance_field; a field is enqueued and not yet handed out
+    bool field_host_copy_ = true;  // enable_distance_field's host_copy
+    bool field_exists_ = false;    // a fused frame has enqueued a field: the queries have a grid to read
 };
 } // namespace dsm
