@@ -34,6 +34,7 @@ EXPORTS = [
     "dsm_publish_enable", "dsm_publish_enqueue", "dsm_publish_wait", "dsm_debug_publish_chunks",
     "dsm_field_enable", "dsm_field_enqueue", "dsm_field_wait",
     "dsm_field_enqueue_resident", "dsm_field_query_enable", "dsm_field_query_enqueue", "dsm_field_query_wait",
+    "dsm_views_enable", "dsm_views_capture", "dsm_field_enqueue_known", "dsm_field_state",
     "dsm_inactive_segments", "dsm_inactive_load", "dsm_map_save", "dsm_map_load", "dsm_map_peek",
     "dsm_checkpoint_enable", "dsm_checkpoint_enqueue", "dsm_checkpoint_wait", "dsm_debug_checkpoint_drain_ctas",
     "dsm_checkpoint_enqueue_incremental", "dsm_map_load_journal", "dsm_map_peek_journal", "dsm_journal_materialize",
@@ -122,6 +123,10 @@ def load_library():
     L.dsm_field_query_enable.argtypes = [vp, ci, ci, ci]
     L.dsm_field_query_enqueue.argtypes = [vp, vp, ci, vp, vp, ci, ctypes.c_float, ctypes.c_float]
     L.dsm_field_query_wait.argtypes = [vp, ctypes.POINTER(vp), ctypes.POINTER(vp)]
+    L.dsm_views_enable.argtypes = [vp, ci, ctypes.c_float]
+    L.dsm_views_capture.argtypes = [vp, ci, ci]
+    L.dsm_field_enqueue_known.argtypes = [vp, ctypes.POINTER(ctypes.c_double), ci, vp, vp, ci, ci]
+    L.dsm_field_state.argtypes = [vp, ctypes.POINTER(vp), ctypes.POINTER(ci)]
     L.dsm_inactive_reserve.argtypes = [vp, ci]
     L.dsm_inactive_retire.argtypes = [vp, ci, ctypes.POINTER(ci)]
     L.dsm_inactive_reactivate.argtypes = [vp, ci, ctypes.POINTER(ci)]
@@ -580,6 +585,38 @@ class Context:
             err.field = field
             raise err
         return field
+
+    # ---- free versus unknown space ----
+    def views_enable(self, max_views, max_range):
+        self._ck(self.lib.dsm_views_enable(self.h, int(max_views), float(max_range)))
+
+    def views_capture(self, frame, slot):
+        """The rays of frame `frame` of the most recent call that took images into slot `slot` (asynchronous)."""
+        self._ck(self.lib.dsm_views_capture(self.h, int(frame), int(slot)))
+
+    def field_enqueue_known(self, center, min_update_times, slots, poses, host_copy=True):
+        """A known-space field over the captured slots at poses (n, 12) or (n, 3, 4) fp64 [R | t], camera to world;
+        field_wait then returns its distances and field_state its voxel states."""
+        c = (ctypes.c_double * 3)(*[float(v) for v in center])
+        sl = np.ascontiguousarray(slots, np.int32).reshape(-1)
+        ps = np.ascontiguousarray(poses, np.float64).reshape(-1, 12)
+        n = len(sl)
+        if ps.shape[0] != n:   # the library reads n poses
+            raise ValueError(f"{n} slots and {ps.shape[0]} poses")
+        self._ck(self.lib.dsm_field_enqueue_known(self.h, c, int(min_update_times), sl.ctypes.data if n else None,
+                                                  ps.ctypes.data if n else None, n, 1 if host_copy else 0))
+
+    def field_state(self):
+        """(state, n_free) of the last waited known field: state a uint8 [nz][ny][nx] copy (0 unknown, 1 occupied,
+        2 free; None for a field kept on the device)."""
+        ptr, nfree = ctypes.c_void_p(), ctypes.c_int(0)
+        self._ck(self.lib.dsm_field_state(self.h, ctypes.byref(ptr), ctypes.byref(nfree)))
+        state = None
+        if ptr.value:
+            shape = self._field_shape
+            buf = (ctypes.c_uint8 * (shape[0] * shape[1] * shape[2])).from_address(ptr.value)
+            state = np.frombuffer(buf, dtype=np.uint8).reshape(shape).copy()
+        return state, nfree.value
 
     # ---- planner queries against the latest field ----
     def field_query_enable(self, max_points, max_trajectories, max_waypoints):

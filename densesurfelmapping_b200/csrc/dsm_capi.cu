@@ -1449,10 +1449,19 @@ extern "C" int dsm_field_enable(dsm_ctx *ctx, const dsm_field_params *params)
     return DSM_OK;
 }
 
+// The views of a known request (dsm_field_enqueue_known), checked by the caller
+struct KnownViews
+{
+    const int32_t *slots;
+    const double *poses;
+    int n;
+};
+
 // Enqueue only, like dsm_publish_enqueue: clear, mark, the three EDT passes and one copy of the grid with its header into
 // the pinned buffer (host_copy), or of the header alone, then the event.  The launches have no gate: after a rejected
-// frame the map is the one of the last applied frame, which is what the field reports.
-static int field_enqueue(dsm_ctx *ctx, const double center[3], int min_update_times, bool host_copy)
+// frame the map is the one of the last applied frame, which is what the field reports.  With `known` the pose list is
+// staged and copied first, the carve runs between the mark and the EDT, and host_copy copies the state grid as well.
+static int field_enqueue(dsm_ctx *ctx, const double center[3], int min_update_times, bool host_copy, const KnownViews *known = nullptr)
 {
     if (!ctx || !center || min_update_times < 1) return DSM_E_INVALID;
     DsmField *f = ctx->field.get();
@@ -1474,14 +1483,31 @@ static int field_enqueue(dsm_ctx *ctx, const double center[3], int min_update_ti
     const DsmDev d = resident_view(ctx, 0);
     const InactStore *s = ctx->inact.get();
     int32_t *header = f->dist + dsm_field_header(f->voxels);
+    DsmViews *vw = ctx->views.get();
+    if (known && known->n > 0)
+    { // the previous known request's copy out of this staging ended before its wait, which no field in flight implies
+        double *hp = reinterpret_cast<double *>(vw->stage_host);
+        std::memcpy(hp, known->poses, 12 * sizeof(double) * (size_t)known->n);
+        std::memcpy(hp + 12 * (size_t)known->n, known->slots, sizeof(int32_t) * (size_t)known->n);
+        CK(cudaMemcpyAsync(vw->stage_dev, vw->stage_host, DsmViews::stage_bytes(known->n), cudaMemcpyHostToDevice, ctx->stream));
+    }
     CK(cudaMemsetAsync(f->occ, 0, f->voxels, ctx->stream));
-    CK(cudaMemsetAsync(header, 0, sizeof(int32_t), ctx->stream));
+    CK(cudaMemsetAsync(header, 0, (known ? DSM_FIELD_VIEW + 1 : 1) * sizeof(int32_t), ctx->stream));
     dsm_launch_field_mark(ctx->d.pool, ctx->res_ofs, d.max_pool_per_frame, min_update_times, s ? s->surfels : nullptr, ctx->win_hdr,
                           s ? std::min(s->upper, s->cap) : 0, g, f->occ, header, ctx->stream);
-    dsm_launch_field_edt(g, f->occ, f->dist, header, ctx->stream);
+    if (known)
+    {
+        const double *poses = reinterpret_cast<const double *>(vw->stage_dev);
+        dsm_launch_field_carve(g, vw->rays, ctx->d.S, poses, reinterpret_cast<const int32_t *>(poses + 12 * (size_t)known->n), known->n,
+                               vw->max_range, f->occ, ctx->stream);
+    }
+    dsm_launch_field_edt(g, f->occ, known != nullptr, f->dist, header, ctx->stream);
     CK(cudaGetLastError());
     if (host_copy)
+    {
         CK(cudaMemcpyAsync(f->host, f->dist, f->bytes, cudaMemcpyDeviceToHost, ctx->stream));
+        if (known) CK(cudaMemcpyAsync(vw->state, f->occ, f->voxels, cudaMemcpyDeviceToHost, ctx->stream));
+    }
     else
         CK(cudaMemcpyAsync(f->host + dsm_field_header(f->voxels), header, DSM_FIELD_WORDS * sizeof(int32_t), cudaMemcpyDeviceToHost,
                            ctx->stream));
@@ -1489,6 +1515,8 @@ static int field_enqueue(dsm_ctx *ctx, const double center[3], int min_update_ti
     f->g = g;
     f->in_flight = f->requested = true;
     f->resident = !host_copy;
+    f->known = known != nullptr;
+    f->known_waited = false;
     return DSM_OK;
 }
 
@@ -1510,6 +1538,7 @@ extern "C" int dsm_field_wait(dsm_ctx *ctx, const float **dist, int32_t origin[3
     CK(cudaSetDevice(ctx->device));
     CK(cudaEventSynchronize(f->ev));
     f->in_flight = false;
+    f->known_waited = f->known;
     const int32_t *h = f->host + dsm_field_header(f->voxels);
     if (dist) *dist = f->resident ? nullptr : reinterpret_cast<const float *>(f->host);
     if (origin) origin[0] = f->g.o[0], origin[1] = f->g.o[1], origin[2] = f->g.o[2];
@@ -1610,7 +1639,9 @@ extern "C" int dsm_field_query_enqueue(dsm_ctx *ctx, const double *points, int n
     int32_t *r_hdr = reinterpret_cast<int32_t *>(q->res_dev);
     float4 *r_samples = reinterpret_cast<float4 *>(q->res_dev + 16);
     dsm_clearance_t *r_clear = reinterpret_cast<dsm_clearance_t *>(q->res_dev + DsmFieldQuery::res_clearance(n_points));
-    dsm_launch_field_query(reinterpret_cast<const float *>(f->dist), f->dist + dsm_field_header(f->voxels), f->g, d_pts, n_points, d_wp,
+    // a known field's query view holds its site count where a plain field's header holds its occupied count
+    const int32_t *f_hdr = f->dist + dsm_field_header(f->voxels) + (f->known ? DSM_FIELD_VIEW : 0);
+    dsm_launch_field_query(reinterpret_cast<const float *>(f->dist), f_hdr, f->g, d_pts, n_points, d_wp,
                            d_ofs, d_first, n_trajectories, radius, r_hdr, r_samples, r_clear, ctx->stream);
     CK(cudaGetLastError());
     CK(cudaMemcpyAsync(q->res_host, q->res_dev, DsmFieldQuery::res_bytes(n_points, n_trajectories), cudaMemcpyDeviceToHost, ctx->stream));
@@ -1635,6 +1666,81 @@ extern "C" int dsm_field_query_wait(dsm_ctx *ctx, const dsm_field_sample_t **sam
     snprintf(ctx->err, sizeof(ctx->err), "dsm_field_query_wait: frame %d of a dsm_fuse_stream_window call did not fit the pool or the "
              "store; the field the query read holds the frames before it", h[DSM_QUERY_ERR_FRAME]);
     return DSM_E_CAPACITY;
+}
+
+// ---- free versus unknown space: captured views and the known-space field (include/dsm.h, DESIGN.md §8.9) ----
+extern "C" int dsm_views_enable(dsm_ctx *ctx, int max_views, float max_range)
+{
+    if (!ctx || max_views < 1 || max_views > DSM_VIEWS_MAX || !std::isfinite(max_range) || !(max_range > 0.f)) return DSM_E_INVALID;
+    const DsmField *f = ctx->field.get();
+    if (!f || ctx->views) return DSM_E_STATE;
+    // a ray visits at most about 3 * 1024 voxels
+    if (!((double)max_range <= 1024.0 * (double)f->g.voxel)) return DSM_E_INVALID;
+    // k_field_carve's one-dimensional grid over max_views views (only frames of billions of pixels come near it)
+    if ((int64_t)max_views * dsm_carve_ctas_per_view(ctx->d.S) > INT32_MAX) return DSM_E_INVALID;
+    CK(cudaSetDevice(ctx->device));
+    auto v = std::make_unique<DsmViews>();
+    v->max_views = max_views, v->max_range = max_range;
+    v->filled.assign((size_t)max_views, 0);
+    cudaError_t e = v->own.device(&v->rays, (size_t)max_views * ctx->d.S);
+    if (e == cudaSuccess) e = v->own.host(&v->state, f->voxels);
+    if (e == cudaSuccess) e = v->own.host(&v->stage_host, DsmViews::stage_bytes(max_views));
+    if (e == cudaSuccess) e = v->own.device(&v->stage_dev, DsmViews::stage_bytes(max_views));
+    if (e != cudaSuccess)
+    {
+        cudaGetLastError();
+        return DSM_E_NOMEM; // nothing is kept: a later call may try again
+    }
+    ctx->views = std::move(v);
+    return DSM_OK;
+}
+
+// Enqueue only.  The frame's slot is safe to read on the main stream: the call that filled it left its schedule ordered
+// before later work there, and the next call that rewrites the slot is the next-but-one resident run, whose phase 1
+// waits for half_free of this half (recorded on the main stream at the entry of the run in between, so after this
+// capture), or any other call that takes images, which synchronises with the main stream before it stages them.
+extern "C" int dsm_views_capture(dsm_ctx *ctx, int frame, int slot)
+{
+    if (!ctx) return DSM_E_INVALID;
+    DsmViews *v = ctx->views.get();
+    if (!v) return DSM_E_STATE;
+    if (slot < 0 || slot >= v->max_views) return DSM_E_INVALID;
+    if (ctx->img_n == 0) return DSM_E_STATE;
+    if (frame < 0 || frame >= ctx->img_n) return DSM_E_INVALID;
+    if (!ctx->img_fit) return DSM_E_STATE; // uploaded but not run, or run with the plane fit cut off
+    CK(cudaSetDevice(ctx->device));
+    const int S = ctx->d.S;
+    dsm_launch_views_capture(ctx->d.plane + (size_t)(ctx->img_slot0 + frame) * S * 3, S, v->rays + (size_t)slot * S, ctx->stream);
+    CK(cudaGetLastError());
+    v->filled[(size_t)slot] = 1;
+    return DSM_OK;
+}
+
+extern "C" int dsm_field_enqueue_known(dsm_ctx *ctx, const double center[3], int min_update_times, const int32_t *slots,
+                                       const double *poses, int n_views, int host_copy)
+{
+    if (!ctx) return DSM_E_INVALID;
+    const DsmViews *v = ctx->views.get();
+    if (!v) return DSM_E_STATE;
+    if (n_views < 0 || n_views > v->max_views || (n_views > 0 && (!slots || !poses))) return DSM_E_INVALID;
+    for (int j = 0; j < n_views; j++)
+    {
+        if (slots[j] < 0 || slots[j] >= v->max_views || !v->filled[(size_t)slots[j]]) return DSM_E_INVALID;
+        for (int k = 0; k < 12; k++)
+            if (!std::isfinite(poses[12 * (size_t)j + k])) return DSM_E_INVALID;
+    }
+    const KnownViews known{slots, poses, n_views};
+    return field_enqueue(ctx, center, min_update_times, host_copy != 0, &known);
+}
+
+extern "C" int dsm_field_state(dsm_ctx *ctx, const uint8_t **state, int *n_free)
+{
+    if (!ctx) return DSM_E_INVALID;
+    const DsmField *f = ctx->field.get();
+    if (!f || !f->known_waited) return DSM_E_STATE;
+    if (state) *state = f->resident ? nullptr : ctx->views->state;
+    if (n_free) *n_free = f->host[dsm_field_header(f->voxels) + DSM_FIELD_N_FREE];
+    return DSM_OK;
 }
 
 // ---- checkpoints that do not stop the stream (include/dsm.h, DESIGN.md §8.5) ----

@@ -183,6 +183,22 @@ struct DsmField
     bool in_flight = false; // enqueued and not yet waited for
     bool requested = false; // a field has been enqueued: the device grid is one a query may read
     bool resident = false;  // the latest request copies only its header words (dsm_field_enqueue_resident)
+    bool known = false;     // the latest request is a known one (dsm_field_enqueue_known): its query view is DSM_FIELD_VIEW
+    bool known_waited = false; // the last waited request is a known one, and no request has been enqueued since
+};
+
+// dsm_views_* (DESIGN.md §8.9), allocated by dsm_views_enable: the captured rays of max_views slots, which slots hold a
+// capture, the pinned host copy of a known request's state grid, and the pinned and device staging of its pose list
+struct DsmViews
+{
+    CudaOwner own;
+    int max_views = 0;
+    float max_range = 0.f;
+    float4 *rays = nullptr;       // device [max_views][S]: camera-space ray ends, w = 1, or w = 0 for a seed without one
+    std::vector<uint8_t> filled;  // [max_views], caller's thread: the slot has been captured
+    uint8_t *state = nullptr;     // pinned [voxels]
+    uint8_t *stage_host = nullptr, *stage_dev = nullptr; // double poses[max_views][12] | int32 slots[max_views]
+    static size_t stage_bytes(int n) { return 12 * sizeof(double) * (size_t)n + sizeof(int32_t) * (size_t)n; }
 };
 
 // dsm_field_query_* (DESIGN.md §8.8): the packed request (pinned staging and its device twin), the packed result
@@ -271,6 +287,7 @@ struct dsm_ctx
     std::unique_ptr<DsmCheckpoint> ckpt; // nullptr until dsm_checkpoint_enable
     std::unique_ptr<DsmField> field;     // nullptr until dsm_field_enable
     std::unique_ptr<DsmFieldQuery> field_query; // nullptr until dsm_field_query_enable
+    std::unique_ptr<DsmViews> views;             // nullptr until dsm_views_enable
     int run_split = 2;          // sub-batches per dsm_batch_run (dsm_set_concurrency)
     // pinned host staging for the small per-batch tables
     float *h_pose = nullptr; // [2B][32]: pose then inverse; first half: the batch calls, second half: the resident stream

@@ -288,7 +288,18 @@ enum
     DSM_FIELD_N_OCCUPIED, // occupied voxels (zeroed before the request; k_field_rows adds)
     DSM_FIELD_ERR_TAG,    // the sticky error word of dsm_fuse_stream_window at the request, and
     DSM_FIELD_ERR_FRAME,  // the frame it rejected
-    DSM_FIELD_WORDS
+    DSM_FIELD_N_FREE,     // a known request: free voxels (zeroed before it; k_field_rows<true> adds)
+    // a known request's query view: the three words above as a query reads them, with the count of sites (voxels that
+    // are not free) in place of the occupied count, so that a query's "no site" rule holds for either kind of field
+    DSM_FIELD_VIEW,
+    DSM_FIELD_WORDS = DSM_FIELD_VIEW + 3
+};
+// voxel states of a known request's grid (the occupancy grid, carved in place)
+enum
+{
+    DSM_STATE_UNKNOWN = 0,
+    DSM_STATE_OCCUPIED = 1,
+    DSM_STATE_FREE = 2
 };
 inline size_t dsm_field_header(size_t voxels) { return (voxels + 3) / 4 * 4; }
 int dsm_field_setup(); // raises the dynamic shared-memory limit of the envelope passes (lines of up to 1024 voxels)
@@ -296,8 +307,20 @@ int dsm_field_setup(); // raises the dynamic shared-memory limit of the envelope
 // pool_upper / store_upper >= the live sizes size the grid.  store == nullptr: no store.  occ must be zeroed.
 void dsm_launch_field_mark(const dsm_surfel_t *pool, const int32_t *res, int pool_upper, int min_update_times, const dsm_surfel_t *store,
                            const int32_t *store_size, int store_upper, const DsmFieldGrid &g, uint8_t *occ, int32_t *header, cudaStream_t s);
-// the three EDT passes: occ -> dist (in place from the second pass on); header[DSM_FIELD_N_OCCUPIED] must be zeroed
-void dsm_launch_field_edt(const DsmFieldGrid &g, const uint8_t *occ, int32_t *dist, int32_t *header, cudaStream_t s);
+// the three EDT passes: occ -> dist (in place from the second pass on); header[DSM_FIELD_N_OCCUPIED] must be zeroed.
+// known: occ holds voxel states, the sites are the voxels that are not free, and header[DSM_FIELD_N_FREE] and
+// header[DSM_FIELD_VIEW] must be zeroed as well
+void dsm_launch_field_edt(const DsmFieldGrid &g, const uint8_t *occ, bool known, int32_t *dist, int32_t *header, cudaStream_t s);
+// dsm_views_capture: the rays of one frame slot's S seeds from its plane rows (plane = d.plane + slot * S * 3)
+void dsm_launch_views_capture(const float4 *plane, int S, float4 *rays, cudaStream_t s);
+// k_field_carve's CTAs per view, and the most views one launch takes: the grid is one-dimensional, n_views * per_view
+// CTAs, below 2^31
+#define CARVE_BLOCK 128
+inline int dsm_carve_ctas_per_view(int S) { return (S + CARVE_BLOCK - 1) / CARVE_BLOCK; }
+// k_field_carve over n_views views of S rays each: view j reads the rays of slot slots[j] and the pose poses[12 j ..]
+// (row-major [R | t], camera to world); occ must hold the marks of k_field_mark.  No launch for n_views == 0.
+void dsm_launch_field_carve(const DsmFieldGrid &g, const float4 *rays, int S, const double *poses, const int32_t *slots, int n_views,
+                            float max_range, uint8_t *occ, cudaStream_t s);
 
 // dsm_field_query_* (DESIGN.md §8.8), dsm_field.cu.  One packed request (H2D) and one packed result (D2H):
 //   request  double points[n_points][3] | double waypoints[n_wp][3] | int32 offsets[n_traj + 1] | int32 first[n_wp]

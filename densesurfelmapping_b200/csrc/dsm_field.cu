@@ -47,20 +47,35 @@ __global__ void __launch_bounds__(FIELD_MARK_BLOCK) k_field_mark(const dsm_surfe
     occ[((size_t)z * g.n[1] + y) * g.n[0] + x] = 1;
 }
 
+// KNOWN (dsm_field_enqueue_known, DESIGN.md §8.9): the grid holds states 0 unknown, 1 occupied, 2 free, the sites are
+// the voxels that are not free, and the warp counts occupied, free and site voxels; CTA 0 copies the error words into
+// the query view (DSM_FIELD_VIEW).  Otherwise every nonzero byte is a site and an occupied voxel.
+template <bool KNOWN>
 __global__ void __launch_bounds__(32 * FIELD_ROW_WARPS) k_field_rows(const DsmFieldGrid g, const uint8_t *occ, int32_t *dist, int32_t *header)
 {
-    __shared__ int32_t s_left[FIELD_ROW_WARPS][1024]; // nearest occupied x at or left of each x, -1 if none
+    __shared__ int32_t s_left[FIELD_ROW_WARPS][1024]; // nearest site x at or left of each x, -1 if none
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    if (KNOWN && blockIdx.x == 0 && threadIdx.x == 0)
+    { // k_field_mark wrote them before this pass
+        header[DSM_FIELD_VIEW + DSM_FIELD_ERR_TAG] = header[DSM_FIELD_ERR_TAG];
+        header[DSM_FIELD_VIEW + DSM_FIELD_ERR_FRAME] = header[DSM_FIELD_ERR_FRAME];
+    }
     const int row = blockIdx.x * FIELD_ROW_WARPS + warp, nx = g.n[0];
     if (row >= g.n[1] * g.n[2]) return;
     const uint8_t *o = occ + (size_t)row * nx;
     int32_t *out = dist + (size_t)row * nx;
     int32_t *left = s_left[warp];
-    int carry = -1, count = 0;
+    int carry = -1, count = 0, n_free = 0;
     for (int base = 0; base < nx; base += 32)
     {
         const int x = base + lane;
-        const bool hit = x < nx && o[x];
+        const bool hit = x < nx && (KNOWN ? o[x] != DSM_STATE_FREE : o[x] != 0);
+        if (KNOWN)
+        {
+            const int st = x < nx ? o[x] : 0;
+            count += __popc(__ballot_sync(0xffffffffu, st == DSM_STATE_OCCUPIED));
+            n_free += __popc(__ballot_sync(0xffffffffu, st == DSM_STATE_FREE));
+        }
         int v = hit ? x : -1;
         for (int k = 1; k < 32; k <<= 1)
         {
@@ -70,13 +85,13 @@ __global__ void __launch_bounds__(32 * FIELD_ROW_WARPS) k_field_rows(const DsmFi
         v = max(v, carry);
         if (x < nx) left[x] = v;
         carry = __shfl_sync(0xffffffffu, v, 31);
-        count += __popc(__ballot_sync(0xffffffffu, hit));
+        if (!KNOWN) count += __popc(__ballot_sync(0xffffffffu, hit));
     }
     carry = INT_MAX;
     for (int base = (nx - 1) & ~31; base >= 0; base -= 32)
     {
         const int x = base + lane;
-        const bool hit = x < nx && o[x];
+        const bool hit = x < nx && (KNOWN ? o[x] != DSM_STATE_FREE : o[x] != 0);
         int v = hit ? x : INT_MAX;
         for (int k = 1; k < 32; k <<= 1)
         {
@@ -93,6 +108,11 @@ __global__ void __launch_bounds__(32 * FIELD_ROW_WARPS) k_field_rows(const DsmFi
         }
     }
     if (lane == 0 && count > 0) atomicAdd(&header[DSM_FIELD_N_OCCUPIED], count);
+    if (KNOWN && lane == 0)
+    {
+        if (n_free > 0) atomicAdd(&header[DSM_FIELD_N_FREE], n_free);
+        if (n_free < nx) atomicAdd(&header[DSM_FIELD_VIEW + DSM_FIELD_N_OCCUPIED], nx - n_free);
+    }
 }
 
 __device__ __forceinline__ uint32_t env_pack(int u, int f) { return ((uint32_t)f << 10) | (uint32_t)u; }
@@ -328,13 +348,130 @@ void dsm_launch_field_mark(const dsm_surfel_t *pool, const int32_t *res, int poo
     k_field_mark<<<pool_grid + store_grid, FIELD_MARK_BLOCK, 0, s>>>(pool, res, pool_grid, min_update_times, store, store_size, g, occ, header);
 }
 
-void dsm_launch_field_edt(const DsmFieldGrid &g, const uint8_t *occ, int32_t *dist, int32_t *header, cudaStream_t s)
+void dsm_launch_field_edt(const DsmFieldGrid &g, const uint8_t *occ, bool known, int32_t *dist, int32_t *header, cudaStream_t s)
 {
     const int nx = g.n[0], ny = g.n[1], nz = g.n[2];
     const int rows = ny * nz;
-    k_field_rows<<<(rows + FIELD_ROW_WARPS - 1) / FIELD_ROW_WARPS, 32 * FIELD_ROW_WARPS, 0, s>>>(g, occ, dist, header);
+    const unsigned rb = (unsigned)(rows + FIELD_ROW_WARPS - 1) / FIELD_ROW_WARPS;
+    if (known)
+        k_field_rows<true><<<rb, 32 * FIELD_ROW_WARPS, 0, s>>>(g, occ, dist, header);
+    else
+        k_field_rows<false><<<rb, 32 * FIELD_ROW_WARPS, 0, s>>>(g, occ, dist, header);
     const unsigned xb = (unsigned)(nx + 31) / 32;
     // along y: lines (x, z) at stride nx; along z: lines (x, y) at stride nx * ny
     k_field_lines<false><<<dim3(xb, nz), 32, (size_t)ny * 32 * 4, s>>>(dist, nx, ny, nx, nx * ny, g.voxel);
     k_field_lines<true><<<dim3(xb, ny), 32, (size_t)nz * 32 * 4, s>>>(dist, nx, nz, nx * ny, nx, g.voxel);
+}
+
+// ---- known space (dsm_views_*, dsm_field_enqueue_known, DESIGN.md §8.9) ----
+//   k_views_capture  one thread per seed of a frame slot: plane row 1 (posi.xyz, mean_depth) becomes the seed's ray in
+//                    camera coordinates, w = 1, or a ray with w = 0 (none) unless mean_depth > 0 and posi is finite.
+//   k_field_carve    one thread per (view, ray): the fp64 Amanatides-Woo walk of include/dsm.h from the camera to the
+//                    ray's end, which stores DSM_STATE_FREE into every visited grid voxel whose byte is 0.  Runs after
+//                    k_field_mark and before the rows pass; only 2s are stored and only over 0s, so concurrent stores of
+//                    one voxel store the same value and need no atomics.  A one-dimensional grid, view-major (`per_view`
+//                    CTAs per view): gridDim.y would cap the views at 65535.
+#define VIEWS_BLOCK 256
+
+__global__ void __launch_bounds__(VIEWS_BLOCK) k_views_capture(const float4 *__restrict__ plane, int S, float4 *__restrict__ rays)
+{
+    const int s = blockIdx.x * VIEWS_BLOCK + threadIdx.x;
+    if (s >= S) return;
+    const float4 r = plane[(size_t)s * 3 + 1];
+    const bool ok = r.w > 0.f && isfinite(r.x) && isfinite(r.y) && isfinite(r.z);
+    rays[s] = ok ? make_float4(r.x, r.y, r.z, 1.f) : make_float4(0.f, 0.f, 0.f, 0.f);
+}
+
+__global__ void __launch_bounds__(CARVE_BLOCK) k_field_carve(const float4 *__restrict__ rays, int S, int per_view, const double *__restrict__ poses,
+                                                             const int32_t *__restrict__ slots, double max_range, const DsmFieldGrid g,
+                                                             uint8_t *occ)
+{
+    const int j = (int)blockIdx.x / per_view;
+    const int s = ((int)blockIdx.x - j * per_view) * CARVE_BLOCK + threadIdx.x;
+    if (s >= S) return;
+    const float4 r = rays[(size_t)slots[j] * S + s];
+    if (r.w == 0.f) return;
+    const double *P = poses + 12 * (size_t)j; // row-major [R | t], camera to world
+    const double px = (double)r.x, py = (double)r.y, pz = (double)r.z, v = (double)g.voxel;
+    double a[3], b[3], d[3];
+#pragma unroll
+    for (int k = 0; k < 3; k++)
+    {
+        a[k] = P[4 * k + 3];
+        b[k] = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(P[4 * k], px), __dmul_rn(P[4 * k + 1], py)), __dmul_rn(P[4 * k + 2], pz)), a[k]);
+        d[k] = __dsub_rn(b[k], a[k]);
+    }
+    const double L = __dsqrt_rn(__dadd_rn(__dadd_rn(__dmul_rn(d[0], d[0]), __dmul_rn(d[1], d[1])), __dmul_rn(d[2], d[2])));
+    const bool truncated = L > max_range;
+    if (truncated)
+    {
+        const double f = __ddiv_rn(max_range, L);
+#pragma unroll
+        for (int k = 0; k < 3; k++) b[k] = __dadd_rn(a[k], __dmul_rn(f, d[k]));
+    }
+    int i[3], e[3], st[3];
+    double tM[3], tD[3];
+#pragma unroll
+    for (int k = 0; k < 3; k++)
+    {
+        const double wa = __ddiv_rn(a[k], v), wb = __ddiv_rn(b[k], v);
+        // a ray with a non-finite endpoint carves nothing (fmax / fmin below would pass over a NaN); the walk stays
+        // within one voxel of the box of its two end voxels: a segment whose box misses the grid by more than that
+        // visits nothing in it (and this keeps the voxel indices below in int range)
+        if (!(isfinite(wa) && isfinite(wb))) return;
+        if (!(fmax(wa, wb) >= (double)(g.o[k] - 1) && fmin(wa, wb) < (double)(g.o[k] + g.n[k] + 1))) return;
+        i[k] = (int)floor(wa);
+        e[k] = (int)floor(wb);
+        const double delta = __dsub_rn(wb, wa);
+        st[k] = delta > 0.0 ? 1 : (delta < 0.0 ? -1 : 0);
+        tD[k] = st[k] != 0 ? __drcp_rn(fabs(delta)) : INFINITY;
+        tM[k] = st[k] != 0 ? __ddiv_rn(__dsub_rn((double)(st[k] > 0 ? i[k] + 1 : i[k]), wa), delta) : INFINITY;
+    }
+    // scalars from here on: the walk picks an axis per step, and indexing the arrays by it would put them on the stack
+    int ix = i[0], iy = i[1], iz = i[2];
+    double mx = tM[0], my = tM[1], mz = tM[2];
+    const int nx = g.n[0], ny = g.n[1], nz = g.n[2];
+    while (true)
+    {
+        const bool end = ix == e[0] && iy == e[1] && iz == e[2];
+        const int x = ix - g.o[0], y = iy - g.o[1], z = iz - g.o[2];
+        if ((!end || truncated) && (unsigned)x < (unsigned)nx && (unsigned)y < (unsigned)ny && (unsigned)z < (unsigned)nz)
+        {
+            uint8_t *c = occ + ((size_t)z * ny + y) * nx + x;
+            if (*c == DSM_STATE_UNKNOWN) *c = DSM_STATE_FREE;
+        }
+        if (end) break;
+        // argmin, the lowest axis on ties
+        if (mx <= my && mx <= mz)
+        {
+            if (mx > 1.0) break;
+            ix += st[0];
+            mx = __dadd_rn(mx, tD[0]);
+        }
+        else if (my <= mz)
+        {
+            if (my > 1.0) break;
+            iy += st[1];
+            my = __dadd_rn(my, tD[1]);
+        }
+        else
+        {
+            if (mz > 1.0) break;
+            iz += st[2];
+            mz = __dadd_rn(mz, tD[2]);
+        }
+    }
+}
+
+void dsm_launch_views_capture(const float4 *plane, int S, float4 *rays, cudaStream_t s)
+{
+    k_views_capture<<<(S + VIEWS_BLOCK - 1) / VIEWS_BLOCK, VIEWS_BLOCK, 0, s>>>(plane, S, rays);
+}
+
+void dsm_launch_field_carve(const DsmFieldGrid &g, const float4 *rays, int S, const double *poses, const int32_t *slots, int n_views,
+                            float max_range, uint8_t *occ, cudaStream_t s)
+{
+    const int per_view = dsm_carve_ctas_per_view(S);
+    if (n_views > 0)
+        k_field_carve<<<(unsigned)(n_views * per_view), CARVE_BLOCK, 0, s>>>(rays, S, per_view, poses, slots, (double)max_range, g, occ);
 }

@@ -455,7 +455,8 @@ int dsm_debug_publish_chunks(dsm_ctx *ctx, int *count);
  * marks voxel q - o, q_k = floorf(p_k / v) in fp32, when o_k <= q_k < o_k + n_k on every axis (compared in fp32; a NaN
  * or infinite coordinate marks nothing).  dist[(z * ny + y) * nx + x] = sqrtf((float)d2) * v, d2 the smallest squared
  * integer distance from voxel (x, y, z) to an occupied voxel (0 on one), +INFINITY everywhere when none is occupied.
- * Unsigned: every voxel without an obstacle point counts as free.
+ * Unsigned: every voxel without an obstacle point counts as free (dsm_field_enqueue_known, below, measures the distance to
+ * anything not known to be free).
  *   dsm_field_enable    once, on a context with a resident pool (DSM_E_STATE otherwise, and when called twice).  v finite
  *                       and > 0, each size in [1, 1024] (DSM_E_INVALID).  Allocates the occupancy grid (1 B per voxel)
  *                       and the distance grid (4 B per voxel) on the device, a pinned host copy of the distance grid and
@@ -486,7 +487,7 @@ int dsm_field_wait(dsm_ctx *ctx, const float **dist, int32_t origin[3], int *n_o
 int dsm_field_enqueue_resident(dsm_ctx *ctx, const double center[3], int min_update_times);
 
 /* ---- planner queries against the latest distance field, on the device (DESIGN.md §8.8) ----
- * A query reads the grid of the latest field request (either enqueue call, waited for or not), in stream order behind
+ * A query reads the grid of the latest field request (any enqueue call, waited for or not), in stream order behind
  * it, with that request's origin o and voxel edge v captured at the query's enqueue; a later field request may be
  * enqueued while a query is in flight and does not change what the query reads.  Only the grid is read, never the map.
  *
@@ -499,8 +500,8 @@ int dsm_field_enqueue_resident(dsm_ctx *ctx, const double center[3], int min_upd
  *   gx   = lerp(lerp(c100 - c000, c110 - c010, ty), lerp(c101 - c001, c111 - c011, ty), tz) / v
  *   gy   = lerp(lerp(c010 - c000, c110 - c100, tx), lerp(c011 - c001, c111 - c101, tx), tz) / v
  *   gz   = lerp(lerp(c001 - c000, c101 - c100, tx), lerp(c011 - c010, c111 - c110, tx), ty) / v
- * Outside: dist is the canonical quiet NaN (unknown, not free) and the gradient 0.  A field with no occupied voxel gives
- * every inside point dist = +INFINITY and a zero gradient.
+ * Outside: dist is the canonical quiet NaN (unknown, not free) and the gradient 0.  A field with no occupied voxel (a
+ * known field: with every voxel free) gives every inside point dist = +INFINITY and a zero gradient.
  *
  * Trajectory clearance.  Trajectory j is the polyline of waypoints offsets[j] .. offsets[j + 1] - 1, sampled in fp64:
  * each segment a -> b with L = sqrt((dx^2 + dy^2) + dz^2) and m = max(1, ceil(L / (double)step)) (counted on the host)
@@ -541,6 +542,61 @@ int dsm_field_query_enable(dsm_ctx *ctx, int max_points, int max_trajectories, i
 int dsm_field_query_enqueue(dsm_ctx *ctx, const double *points, int n_points, const double *waypoints, const int32_t *offsets,
                             int n_trajectories, float step, float radius);
 int dsm_field_query_wait(dsm_ctx *ctx, const dsm_field_sample_t **samples, const dsm_clearance_t **clearance);
+
+/* ---- free versus unknown space: the distance to anything not known to be free (DESIGN.md §8.9) ----
+ * The field of dsm_field_enqueue counts every voxel without an obstacle point as free, including space no camera has
+ * seen.  A known request carves the voxels the captured views have observed as free with their rays and measures the
+ * distance to the nearest voxel NOT known to be free (unknown is an obstacle).  Rays are kept in camera coordinates, one
+ * set per captured frame, and every request takes each view's current world pose, so the field follows loop closures.
+ *
+ * Rays.  dsm_views_capture stores, in seed index order, the fp32 camera-space plane-fit point posi of every seed of the
+ * frame with mean_depth > 0 and three finite coordinates (the posi and mean_depth of dsm_get_seeds); other seeds give no
+ * ray.  Adjacent rays are one superpixel apart, so beyond the range where that spacing exceeds a voxel some free voxels
+ * between rays stay unknown, which is the safe side.
+ *
+ * Definition (every step fp64, one rounding per operation).  Occupancy is that of dsm_field_enqueue: state 1.  For view j
+ * with pose [R | t] (poses[12 j ..], row-major, camera to world) and each ray p of slot slots[j] (widened to fp64):
+ *   a = t;  b_k = ((R_k0 p_x + R_k1 p_y) + R_k2 p_z) + t_k;  d = b - a;  L = sqrt((d_0^2 + d_1^2) + d_2^2);
+ *   L > (double)max_range: b_k = a_k + ((double)max_range / L) d_k, and the ray is truncated.
+ * Traversal (Amanatides-Woo) in voxel units: w_a = a / (double)v, w_b = b / (double)v, i = floor(w_a), e = floor(w_b),
+ * delta = w_b - w_a; per axis s_k = sign(delta_k), tD_k = 1 / |delta_k|, tM_k = ((i_k + 1) - w_a_k) / delta_k for
+ * delta_k > 0 and (i_k - w_a_k) / delta_k for delta_k < 0, both +inf for delta_k = 0.  Loop: visit i; stop if i == e;
+ * k = argmin tM (the lowest axis on ties); stop if tM_k > 1; i_k += s_k, tM_k += tD_k.
+ * Carving: a visited voxel with o <= i < o + n becomes free (state 2) unless it is occupied; e of a ray that was not
+ * truncated holds the surface and is never carved.  Every other voxel is unknown (state 0).  (A ray whose endpoints
+ * overflow to a non-finite value carves nothing.)
+ * Distance: dist = sqrtf((float)d2) * v, d2 the smallest squared integer distance to a voxel of state 0 or 1; +INFINITY
+ * everywhere when every voxel is free.  With n_views = 0 every voxel that is not occupied is unknown and dist is 0
+ * everywhere.  The known distance never exceeds dsm_field_enqueue's distance of the same request.
+ *
+ *   dsm_views_enable         once, after dsm_field_enable (DSM_E_STATE otherwise, and when called twice).  DSM_E_INVALID
+ *                            unless 1 <= max_views <= DSM_VIEWS_MAX and max_range is finite, > 0 and <= 1024 v (which
+ *                            bounds the voxels one ray visits), or when max_views x ceil(S / 128) reaches 2^31 (frames
+ *                            of billions of pixels).  Allocates 16 B per ray for max_views x S rays on the
+ *                            device, a pinned copy of the state grid (1 B per voxel) and the pinned and device staging
+ *                            of max_views poses.  DSM_E_NOMEM with nothing kept.
+ *   dsm_views_capture        asynchronous on the context's stream, never waits: overwrites slot `slot` with the rays of
+ *                            frame `frame` of the most recent call that took images (as dsm_frame_superpixel_image:
+ *                            DSM_E_STATE with no such call or one whose schedule did not run through the plane fit,
+ *                            DSM_E_INVALID for a frame outside it).  A frame whose fuse was rejected may be captured.
+ *                            DSM_E_INVALID for a slot outside [0, max_views); DSM_E_STATE before dsm_views_enable.
+ *   dsm_field_enqueue_known  dsm_field_enqueue's request (same checks, origin, ordering and DSM_E_CAPACITY rule at
+ *                            dsm_field_wait) over the views slots[0 .. n_views) at poses (n_views x 12 doubles),
+ *                            staged into pinned memory on the calling thread and copied with one H2D copy.  host_copy =
+ *                            0 keeps both grids on the device, as dsm_field_enqueue_resident.  DSM_E_STATE before
+ *                            dsm_views_enable; DSM_E_INVALID for n_views < 0 or > max_views, a slot out of range or never
+ *                            captured, or a non-finite pose entry.  Queries (dsm_field_query_*) read its distance grid
+ *                            like any other field's.
+ *   dsm_field_state          the state grid [z][y][x] of the last waited known request (pinned, valid until the next
+ *                            field enqueue; NULL for host_copy = 0) and its number of free voxels.  DSM_E_STATE when the
+ *                            last waited request was not a known one.  dsm_field_wait returns a known request's dist,
+ *                            origin and n_occupied as any other's. */
+#define DSM_VIEWS_MAX 65536
+int dsm_views_enable(dsm_ctx *ctx, int max_views, float max_range);
+int dsm_views_capture(dsm_ctx *ctx, int frame, int slot);
+int dsm_field_enqueue_known(dsm_ctx *ctx, const double center[3], int min_update_times, const int32_t *slots, const double *poses,
+                            int n_views, int host_copy);
+int dsm_field_state(dsm_ctx *ctx, const uint8_t **state, int *n_free);
 
 /* ---- checkpoints that do not stop the stream (DESIGN.md §8.5) ----
  * The file of dsm_map_save, taken in stream order like a publish snapshot: the resident stream pays one device-to-device

@@ -68,6 +68,13 @@
 // needs instead (DESIGN.md §8.8): after enable_field_queries(), field_samples() (distance and gradient at points) and
 // trajectory_clearance() (the clearance of candidate paths) read the field of the latest fused frame, one enqueue and
 // one wait each, without touching the one-frame-late distance_field() handout.
+// The field counts every voxel without an obstacle point as free, seen or not.  enable_known_space(max_views, max_range),
+// after enable_distance_field, makes it measure the distance to anything not known to be free (DESIGN.md §8.9): the
+// first fused frame of each new reference keyframe is captured into slot captures % max_views (its superpixel rays, in
+// camera coordinates) and the node keeps (reference_index, relative) per slot; every field request then carries every
+// filled slot at its current world pose cam_pose[ref] * relative, in fuse_pose's arithmetic, so a loop closure moves the
+// views with the map.  known_space() returns the state grid of the field distance_field() handed out last.  Views are
+// not part of a checkpoint: load_state* empties the slot table, which refills as keyframes are fused.
 // device < 0 builds the node without a context: the callbacks run the whole pose logic (pose database, sync, window
 // bookkeeping) and fuse nothing; any call that reads the map returns DSM_E_STATE.
 #pragma once
@@ -472,6 +479,39 @@ class SurfelMapNode
             distance_field_ = true, field_host_copy_ = host_copy;
         return ctx_.err;
     }
+    // ---- free versus unknown space (see the top of this file, DESIGN.md §8.9) ----
+    // once, after enable_distance_field: max_views capture slots, rays cut to max_range metres
+    int enable_known_space(int max_views, float max_range)
+    {
+        if (ctx_.run("enable_known_space", [&] { return dsm_views_enable(ctx_.ctx, max_views, max_range); }) == DSM_OK)
+            known_.assign((size_t)max_views, KnownView{-1, Pose()});
+        return ctx_.err;
+    }
+    // the state grid [nz][ny][nx] (0 unknown, 1 occupied, 2 free; the library's pinned buffer, valid until the next frame
+    // is fused; nullptr for a field kept on the device) and the free voxels of the field distance_field() handed out last.
+    // DSM_E_STATE without known space or before distance_field() has handed out a field.
+    int known_space(const uint8_t *&state, int &n_free)
+    {
+        if (!ctx_.ready("known_space")) return ctx_.err;
+        return ctx_.done(dsm_field_state(ctx_.ctx, &state, &n_free), "known_space");
+    }
+    // the views a field request would carry now: the filled slots, ascending, and their world poses (12 doubles each,
+    // row-major [R | t], camera to world); and the number of captures so far (the latest went to slot
+    // (captures - 1) % max_views)
+    int known_views(std::vector<int32_t> &slots, std::vector<double> &poses) const
+    {
+        slots.clear(), poses.clear();
+        for (size_t i = 0; i < known_.size(); i++)
+        {
+            if (known_[i].ref < 0) continue;
+            const node_math::M4 m = node_math::mul(node_math::from_pose(poses_[(size_t)known_[i].ref].cam_pose), node_math::from_pose(known_[i].relative));
+            slots.push_back((int32_t)i);
+            for (int r = 0; r < 3; r++)
+                for (int c = 0; c < 4; c++) poses.push_back(m(r, c));
+        }
+        return captures_;
+    }
+
     // ---- planner queries against the field of the latest fused frame (DESIGN.md §8.8) ----
     // once, after enable_distance_field: the capacities of one query
     int enable_field_queries(int max_points, int max_trajectories, int max_waypoints)
@@ -671,6 +711,8 @@ class SurfelMapNode
         last_ref_ = s.last_ref;
         fused_ = s.fused;
         field_exists_ = false; // the loaded map has no field until its next fused frame
+        for (size_t i = 0; i < known_.size(); i++) known_[i].ref = -1; // views are not part of the checkpoint
+        captures_ = 0, captured_ref_ = -1;
         return ctx_.done(DSM_OK, what);
     }
 
@@ -897,11 +939,31 @@ class SurfelMapNode
         fused_ = true;
         pose_buffer_.pop_front();
         // after the bookkeeping: the frame is enqueued, so the host window follows the device whatever this returns
+        if (!known_.empty() && q.reference_index != captured_ref_)
+        { // the first fused frame of a new reference keyframe: frame 0 of the call just made
+            const int slot = captures_ % (int)known_.size();
+            if (ctx_.done(dsm_views_capture(ctx_.ctx, 0, slot), "fuse") == DSM_OK)
+            {
+                known_[(size_t)slot] = KnownView{q.reference_index, q.relative};
+                captures_++;
+                captured_ref_ = q.reference_index;
+            }
+        }
         if (publishing_) snapshot_ = ctx_.done(dsm_publish_enqueue(ctx_.ctx, 5), "fuse") == DSM_OK;
         if (distance_field_ && (!publishing_ || snapshot_))
         { // centred on the fuse pose's translation, with the threshold of the published active cloud
             const double c[3] = {last_fuse_pose_.x, last_fuse_pose_.y, last_fuse_pose_.z};
-            field_ = ctx_.done(field_host_copy_ ? dsm_field_enqueue(ctx_.ctx, c, 5) : dsm_field_enqueue_resident(ctx_.ctx, c, 5), "fuse") == DSM_OK;
+            int rc;
+            if (!known_.empty())
+            {
+                std::vector<int32_t> slots;
+                std::vector<double> poses;
+                known_views(slots, poses);
+                rc = dsm_field_enqueue_known(ctx_.ctx, c, 5, slots.data(), poses.data(), (int)slots.size(), field_host_copy_ ? 1 : 0);
+            }
+            else
+                rc = field_host_copy_ ? dsm_field_enqueue(ctx_.ctx, c, 5) : dsm_field_enqueue_resident(ctx_.ctx, c, 5);
+            field_ = ctx_.done(rc, "fuse") == DSM_OK;
             field_exists_ = field_exists_ || field_;
         }
         return publishing_ || distance_field_ ? ctx_.err : DSM_OK;
@@ -973,5 +1035,13 @@ class SurfelMapNode
     bool distance_field_ = false, field_ = false; // enable_distance_field; a field is enqueued and not yet handed out
     bool field_host_copy_ = true;  // enable_distance_field's host_copy
     bool field_exists_ = false;    // a fused frame has enqueued a field: the queries have a grid to read
+    // enable_known_space: per capture slot, the reference keyframe (-1: empty) and the pose relative to it
+    struct KnownView
+    {
+        int ref;
+        Pose relative;
+    };
+    std::vector<KnownView> known_; // empty without known space
+    int captures_ = 0, captured_ref_ = -1; // captures so far; the reference keyframe of the latest
 };
 } // namespace dsm
