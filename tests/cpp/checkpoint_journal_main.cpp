@@ -11,60 +11,7 @@
 //            int32 rc of the four files B and T write into dir: b.ply, t.ply (save_mesh), b.pcd, t.pcd (save_cloud).
 //   "equals": every reader agrees byte for byte, as in checkpoint_async_main.cpp.
 // exit code 3 when no usable GPU (the library has no CPU fallback).
-#include <string>
-#include "dsm_surfel_node.hpp"
 #include "driver_io.hpp"
-
-template <class T>
-static void add(std::vector<uint8_t> &d, const T *p, size_t n)
-{
-    const uint8_t *b = reinterpret_cast<const uint8_t *>(p);
-    d.insert(d.end(), b, b + n * sizeof(T));
-}
-template <class T>
-static void add_list(std::vector<uint8_t> &d, const std::vector<T> &v)
-{
-    const int n = (int)v.size();
-    add(d, &n, 1);
-    add(d, v.data(), v.size());
-}
-
-// everything the node reads back, as bytes (checkpoint_main.cpp's digest)
-static std::vector<uint8_t> digest(dsm::SurfelMapNode &node)
-{
-    std::vector<uint8_t> d;
-    std::vector<dsm_surfel_t> s;
-    int rc = node.local_surfels(s);
-    add(d, &rc, 1);
-    add_list(d, s);
-    const std::vector<dsm::NodePose> &p = node.poses();
-    for (size_t i = 0; i < p.size(); i++)
-    {
-        rc = node.attached_surfels((int)i, s);
-        add(d, &rc, 1);
-        add_list(d, s);
-        add(d, &p[i].cam_pose, 1);
-        add(d, &p[i].loop_pose, 1);
-        add(d, &p[i].cam_stamp, 1);
-        add_list(d, p[i].linked_pose_index);
-    }
-    add_list(d, std::vector<int>(node.local_surfels_indexs().begin(), node.local_surfels_indexs().end()));
-    float pose16[16] = {0};
-    std::vector<int> rem, add_;
-    const int pref = node.pending_frame(pose16, rem, add_);
-    add(d, &pref, 1);
-    add(d, pose16, 16);
-    add_list(d, rem);
-    add_list(d, add_);
-    add_list(d, node.last_warp());
-    const dsm::NodePoseGraph g = node.pose_graph();
-    add_list(d, g.path);
-    add_list(d, g.loop_edges);
-    add_list(d, g.driftfree);
-    add_list(d, g.drift);
-    add(d, &g.camera, 1);
-    return d;
-}
 
 // retires A's pending save and reports it with the records the files now resolve with
 static void retire(dsm::SurfelMapNode &a, const std::string &ckpt)
@@ -79,28 +26,22 @@ static void retire(dsm::SurfelMapNode &a, const std::string &ckpt)
 int main(int argc, char **argv)
 {
     if (argc != 16) return 2;
-    const int W = atoi(argv[1]), H = atoi(argv[2]), dfp = atoi(argv[9]), every = atoi(argv[10]), j = atoi(argv[11]);
-    const double fx = atof(argv[3]), fy = atof(argv[4]), cx = atof(argv[5]), cy = atof(argv[6]), fr = atof(argv[7]), nr = atof(argv[8]);
+    const NodeArgs args(argv, false);
+    const int W = args.W, H = args.H, every = atoi(argv[10]), j = atoi(argv[11]);
     const std::string ckpt = argv[12], dir = argv[15];
     if (every < 1) return 2;
-    const int max_local = 1 << 20, max_inactive = 1 << 21;
-    dsm::SurfelMapNode a(W, H, fx, fy, cx, cy, fr, nr, dfp, 0, max_local, max_inactive);
-    if (a.last_error() != DSM_OK) return a.last_error() == DSM_E_NODEVICE ? 3 : 4;
-    dsm::SurfelMapNode t(W, H, fx, fy, cx, cy, fr, nr, dfp, 0, max_local, max_inactive);
-    in_f = fopen(argv[13], "rb");
-    out_f = fopen(argv[14], "wb");
-    if (!in_f || !out_f) return 5;
+    DriverNode a(args);
+    if (const int e = setup_code(a.last_error())) return e;
+    DriverNode t(args);
+    if (!open_io(argv[13], argv[14])) return 5;
     put(a.enable_checkpoints());
     put(t.last_error());
     NodeMessages msg;
-    int type = 0, r = DSM_OK;
+    int type = 0, ra = DSM_OK, rt = DSM_OK;
     bool pending = false;
     for (int m = 1; m <= j; m++)
     {
-        const long at = ftell(in_f);
-        if (!get(type) || !msg.feed(a, type, W, H, r) || r != DSM_OK) return 5;
-        fseek(in_f, at, SEEK_SET);
-        if (!get(type) || !msg.feed(t, type, W, H, r) || r != DSM_OK) return 5;
+        if (!get(type) || !msg.feed_both(a, t, type, W, H, ra, rt) || ra != DSM_OK || rt != DSM_OK) return 5;
         if (m % every != 0 && m != j) continue;
         if (pending) retire(a, ckpt);
         const int rc = a.save_state_incremental(ckpt);
@@ -113,18 +54,15 @@ int main(int argc, char **argv)
     }
     if (pending) retire(a, ckpt);
     // B resumes from A's base and journal; T, held at message j, is the uninterrupted node
-    dsm::SurfelMapNode b(W, H, fx, fy, cx, cy, fr, nr, dfp, 0, max_local, max_inactive);
+    DriverNode b(args);
     int records = -1;
     put(b.load_state_incremental(ckpt, &records));
     put(records);
     put((int)(digest(b) == digest(t)));
     while (get(type))
     {
-        const long at = ftell(in_f);
-        int rb = DSM_OK, rt = DSM_OK;
-        if (!msg.feed(b, type, W, H, rb)) return 5;
-        fseek(in_f, at, SEEK_SET);
-        if (!msg.feed(t, type, W, H, rt)) return 5;
+        int rb = DSM_OK;
+        if (!msg.feed_both(b, t, type, W, H, rb, rt)) return 5;
         put(rb);
         put(rt);
         put((int)(digest(b) == digest(t)));
@@ -134,7 +72,5 @@ int main(int argc, char **argv)
     if (rs == DSM_OK) rs = b.save_cloud(dir + "/b.pcd");
     if (rs == DSM_OK) rs = t.save_cloud(dir + "/t.pcd");
     put(rs);
-    fclose(in_f);
-    fclose(out_f);
-    return 0;
+    return close_io();
 }

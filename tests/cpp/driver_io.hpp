@@ -1,12 +1,14 @@
 // Shared by the C++ test drivers of this directory: the reference's caller types, the binary I/O of a driver's in.bin
-// and out.bin, the frame record of the fuse_map drivers and the message reader of the node drivers.  Every record is
-// read and written in the layout the driver's header comment gives.
+// and out.bin, the frame record of the fuse_map drivers, and the harness of the node drivers (argument prefix, message
+// loop, cloud records and digest).  Every record is read and written in the layout the driver's header comment gives.
 #pragma once
 #include <cstdint>
 #include <cstdio>
 #include <cstdlib>
+#include <string>
 #include <vector>
 #include <opencv2/opencv.hpp> // oracle/shim
+#include "dsm_surfel_node.hpp"
 
 struct SurfelElement // reference elements.h:22-31
 {
@@ -24,6 +26,27 @@ struct Pose4f // Eigen::Matrix4f: a column-major .data()
 };
 
 static FILE *in_f, *out_f; // the driver's in.bin and out.bin
+
+// false (exit code 5) when either file cannot be opened
+inline bool open_io(const char *in, const char *out)
+{
+    in_f = fopen(in, "rb");
+    out_f = fopen(out, "wb");
+    return in_f && out_f;
+}
+inline int close_io()
+{
+    fclose(in_f);
+    fclose(out_f);
+    return 0;
+}
+
+// the exit code of a set-up error (last_error() after construction): 0 for none, 3 when there is no usable GPU (the
+// library has no CPU fallback), 4 for any other
+inline int setup_code(int last_error)
+{
+    return last_error == DSM_OK ? 0 : last_error == DSM_E_NODEVICE ? 3 : 4;
+}
 
 template <class T>
 static bool get(T &v)
@@ -109,4 +132,138 @@ struct NodeMessages
             return false;
         return true;
     }
+    // one message to node a, then the same message to node b
+    template <class Node>
+    bool feed_both(Node &a, Node &b, int type, int W, int H, int &ra, int &rb)
+    {
+        const long at = ftell(in_f);
+        if (!feed(a, type, W, H, ra)) return false;
+        fseek(in_f, at, SEEK_SET);
+        return feed(b, type, W, H, rb);
+    }
 };
+
+// ---- the node drivers ----
+
+// The argument prefix of the node drivers: argv[1..9] = W H fx fy cx cy far near drift_free_poses, then, in the drivers
+// that take them, argv[10..12] = device max_local max_inactive (else device 0, 2^20 pool and 2^21 stored surfels).
+struct NodeArgs
+{
+    int W, H, dfp, device, max_local, max_inactive;
+    double fx, fy, cx, cy, fr, nr;
+    NodeArgs(char **argv, bool sized)
+        : W(atoi(argv[1])), H(atoi(argv[2])), dfp(atoi(argv[9])), device(sized ? atoi(argv[10]) : 0),
+          max_local(sized ? atoi(argv[11]) : 1 << 20), max_inactive(sized ? atoi(argv[12]) : 1 << 21), fx(atof(argv[3])),
+          fy(atof(argv[4])), cx(atof(argv[5])), cy(atof(argv[6])), fr(atof(argv[7])), nr(atof(argv[8]))
+    {
+    }
+};
+
+// a node of the prefix's parameters; check setup_code(last_error())
+struct DriverNode : dsm::SurfelMapNode
+{
+    explicit DriverNode(const NodeArgs &a, const dsm_constants *constants = nullptr)
+        : dsm::SurfelMapNode(a.W, a.H, a.fx, a.fy, a.cx, a.cy, a.fr, a.nr, a.dfp, a.device, a.max_local, a.max_inactive, constants)
+    {
+    }
+};
+
+// Feeds the script's orb / image / depth messages to the node until its end and calls on_depth() after every depth
+// message.  Returns 0 at the end, 5 for a malformed message, 6 when the node refuses one, else the first nonzero code
+// on_depth() returns.
+template <class F>
+static int feed_script(dsm::SurfelMapNode &node, int W, int H, F on_depth)
+{
+    NodeMessages msg;
+    int type = 0, r = DSM_OK;
+    while (get(type))
+    {
+        if (!msg.feed(node, type, W, H, r)) return 5;
+        if (r != DSM_OK) return 6;
+        if (type != 2) continue;
+        const int e = on_depth();
+        if (e) return e;
+    }
+    return 0;
+}
+
+// int32 rc, then the clouds of active_points() and inactive_points() (each int32 n + n points).  inactive_points() is
+// read only after active_points() succeeded; after a failed read the inactive cloud written is the previous one.
+inline void put_clouds(dsm::SurfelMapNode &node)
+{
+    static std::vector<dsm_point_t> act, inact;
+    int rc = node.active_points(act);
+    if (rc == DSM_OK) rc = node.inactive_points(inact);
+    put(rc);
+    put_list(act);
+    put_list(inact);
+}
+
+// the end of a drive: local_surfels (int32 n + records) and inactive_points; false (exit code 6) when a read fails
+inline bool put_final(dsm::SurfelMapNode &node)
+{
+    std::vector<dsm_surfel_t> local;
+    std::vector<dsm_point_t> inact;
+    if (node.local_surfels(local) != DSM_OK || node.inactive_points(inact) != DSM_OK) return false;
+    put_list(local);
+    put_list(inact);
+    return true;
+}
+
+// save_mesh to <prefix>.ply and save_cloud to <prefix>.pcd; false (exit code 6) when either fails
+inline bool save_files(dsm::SurfelMapNode &node, const std::string &prefix)
+{
+    return node.save_mesh(prefix + ".ply") == DSM_OK && node.save_cloud(prefix + ".pcd") == DSM_OK;
+}
+
+template <class T>
+static void add(std::vector<uint8_t> &d, const T *p, size_t n)
+{
+    const uint8_t *b = reinterpret_cast<const uint8_t *>(p);
+    d.insert(d.end(), b, b + n * sizeof(T));
+}
+template <class T>
+static void add_list(std::vector<uint8_t> &d, const std::vector<T> &v)
+{
+    const int n = (int)v.size();
+    add(d, &n, 1);
+    add(d, v.data(), v.size());
+}
+
+// everything the node reads back, as bytes: local_surfels, attached_surfels of every pose, poses() (cam_pose,
+// loop_pose, cam_stamp, links), local_surfels_indexs(), pending_frame(), last_warp() and pose_graph()
+inline std::vector<uint8_t> digest(dsm::SurfelMapNode &node)
+{
+    std::vector<uint8_t> d;
+    std::vector<dsm_surfel_t> s;
+    int rc = node.local_surfels(s);
+    add(d, &rc, 1);
+    add_list(d, s);
+    const std::vector<dsm::NodePose> &p = node.poses();
+    for (size_t i = 0; i < p.size(); i++)
+    {
+        rc = node.attached_surfels((int)i, s);
+        add(d, &rc, 1);
+        add_list(d, s);
+        add(d, &p[i].cam_pose, 1);
+        add(d, &p[i].loop_pose, 1);
+        add(d, &p[i].cam_stamp, 1);
+        add_list(d, p[i].linked_pose_index);
+    }
+    add_list(d, std::vector<int>(node.local_surfels_indexs().begin(), node.local_surfels_indexs().end()));
+    float pose16[16] = {0};
+    std::vector<int> rem, add_;
+    const int pref = node.pending_frame(pose16, rem, add_);
+    add(d, &pref, 1);
+    add(d, pose16, 16);
+    add_list(d, rem);
+    add_list(d, add_);
+    add_list(d, node.last_warp());
+    const dsm::NodePoseGraph g = node.pose_graph();
+    add_list(d, g.path);
+    add_list(d, g.loop_edges);
+    add_list(d, g.driftfree);
+    add_list(d, g.drift);
+    add(d, &g.camera, 1);
+    return d;
+}

@@ -11,38 +11,27 @@
 //            active_points() and inactive_points() (each int32 n + n points); at the end: local_surfels (int32 n +
 //            records), and the node's save_mesh and save_cloud go to <out_prefix>.ply / <out_prefix>.pcd.
 // exit code 3 when no usable GPU (the library has no CPU fallback).
-#include "dsm_surfel_node.hpp"
 #include "driver_io.hpp"
-#include <string>
 
 int main(int argc, char **argv)
 {
     if (argc != 23) return 2;
-    const int W = atoi(argv[1]), H = atoi(argv[2]);
+    const NodeArgs args(argv, true);
     const float voxel = (float)atof(argv[13]);
     const int nx = atoi(argv[14]), ny = atoi(argv[15]), nz = atoi(argv[16]);
     const int max_views = atoi(argv[17]), reload_at = atoi(argv[19]);
-    dsm::SurfelMapNode node(W, H, atof(argv[3]), atof(argv[4]), atof(argv[5]), atof(argv[6]), atof(argv[7]), atof(argv[8]), atoi(argv[9]),
-                            atoi(argv[10]), atoi(argv[11]), atoi(argv[12]), nullptr);
-    if (node.last_error() != DSM_OK) return node.last_error() == DSM_E_NODEVICE ? 3 : 4;
+    DriverNode node(args);
+    if (const int e = setup_code(node.last_error())) return e;
     if (node.enable_distance_field(voxel, nx, ny, nz) != DSM_OK) return 4;
     if (max_views > 0 && node.enable_known_space(max_views, (float)atof(argv[18])) != DSM_OK) return 4;
-    in_f = fopen(argv[20], "rb");
-    out_f = fopen(argv[21], "wb");
-    if (!in_f || !out_f) return 5;
+    if (!open_io(argv[20], argv[21])) return 5;
     const std::string prefix = argv[22];
     const int S = dsm_num_seeds(node.context());
     std::vector<std::vector<dsm_seed_t> > seeds((size_t)(max_views > 0 ? max_views : 0)); // per slot, of its captured frame
     std::vector<int32_t> slots;
     std::vector<double> poses;
-    NodeMessages msg;
-    std::vector<dsm_point_t> act, inact;
-    int type = 0, r = DSM_OK, depth_msgs = 0, fused = 0, captures = 0;
-    while (get(type))
-    {
-        if (!msg.feed(node, type, W, H, r)) return 5;
-        if (r != DSM_OK) return 6;
-        if (type != 2) continue;
+    int depth_msgs = 0, fused = 0, captures = 0;
+    const int e = feed_script(node, args.W, args.H, [&]() -> int {
         const float *dist = nullptr;
         int32_t origin[3] = {0, 0, 0};
         int n_occ = 0;
@@ -77,22 +66,18 @@ int main(int argc, char **argv)
                 put_n(poses.data() + 12 * j, 12);
             }
         }
-        int rr = node.active_points(act);
-        if (rr == DSM_OK) rr = node.inactive_points(inact);
-        put(rr);
-        put_list(act);
-        put_list(inact);
+        put_clouds(node);
         if (++depth_msgs == reload_at)
         {
             if (node.save_state(prefix + ".state") != DSM_OK || node.load_state(prefix + ".state") != DSM_OK) return 6;
             captures = 0; // load_state empties the slot table
         }
-    }
+        return 0;
+    });
+    if (e) return e;
     std::vector<dsm_surfel_t> local;
     if (node.local_surfels(local) != DSM_OK) return 6;
     put_list(local);
-    if (node.save_mesh(prefix + ".ply") != DSM_OK || node.save_cloud(prefix + ".pcd") != DSM_OK) return 6;
-    fclose(in_f);
-    fclose(out_f);
-    return 0;
+    if (!save_files(node, prefix)) return 6;
+    return close_io();
 }

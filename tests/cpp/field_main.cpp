@@ -10,33 +10,21 @@
 //            at the end: local_surfels (int32 n + records) and inactive_points, and the node's save_mesh and save_cloud
 //            go to <out_prefix>.ply / <out_prefix>.pcd.
 // exit code 3 when no usable GPU (the library has no CPU fallback).
-#include "dsm_surfel_node.hpp"
 #include "driver_io.hpp"
-#include <string>
 
 int main(int argc, char **argv)
 {
     if (argc != 21) return 2;
-    const int W = atoi(argv[1]), H = atoi(argv[2]), publish = atoi(argv[13]);
+    const NodeArgs args(argv, true);
+    const int publish = atoi(argv[13]);
     const float voxel = (float)atof(argv[14]);
     const int nx = atoi(argv[15]), ny = atoi(argv[16]), nz = atoi(argv[17]);
-    dsm::SurfelMapNode node(W, H, atof(argv[3]), atof(argv[4]), atof(argv[5]), atof(argv[6]), atof(argv[7]), atof(argv[8]), atoi(argv[9]),
-                            atoi(argv[10]), atoi(argv[11]), atoi(argv[12]), nullptr);
-    if (node.last_error() != DSM_OK) return node.last_error() == DSM_E_NODEVICE ? 3 : 4;
+    DriverNode node(args);
+    if (const int e = setup_code(node.last_error())) return e;
     if (publish && node.enable_publishing() != DSM_OK) return 4;
     if (voxel > 0.f && node.enable_distance_field(voxel, nx, ny, nz) != DSM_OK) return 4;
-    in_f = fopen(argv[18], "rb");
-    out_f = fopen(argv[19], "wb");
-    if (!in_f || !out_f) return 5;
-    const std::string prefix = argv[20];
-    NodeMessages msg;
-    std::vector<dsm_point_t> act, inact;
-    int type = 0, r = DSM_OK;
-    while (get(type))
-    {
-        if (!msg.feed(node, type, W, H, r)) return 5;
-        if (r != DSM_OK) return 6;
-        if (type != 2) continue;
+    if (!open_io(argv[18], argv[19])) return 5;
+    const int e = feed_script(node, args.W, args.H, [&]() -> int {
         if (voxel > 0.f)
         {
             const float *dist = nullptr;
@@ -59,18 +47,10 @@ int main(int argc, char **argv)
             put_n(a, rc == DSM_OK ? na : 0);
             put_n(b, rc == DSM_OK ? nb : 0);
         }
-        int rr = node.active_points(act);
-        if (rr == DSM_OK) rr = node.inactive_points(inact);
-        put(rr);
-        put_list(act);
-        put_list(inact);
-    }
-    std::vector<dsm_surfel_t> local;
-    if (node.local_surfels(local) != DSM_OK || node.inactive_points(inact) != DSM_OK) return 6;
-    put_list(local);
-    put_list(inact);
-    if (node.save_mesh(prefix + ".ply") != DSM_OK || node.save_cloud(prefix + ".pcd") != DSM_OK) return 6;
-    fclose(in_f);
-    fclose(out_f);
-    return 0;
+        put_clouds(node);
+        return 0;
+    });
+    if (e) return e;
+    if (!put_final(node) || !save_files(node, argv[20])) return 6;
+    return close_io();
 }

@@ -14,9 +14,7 @@
 //            go to <out_prefix>.ply / <out_prefix>.pcd.
 // The points and waypoints are drawn from a fixed generator over the grid's box (one voxel beyond it on every side).
 // exit code 3 when no usable GPU (the library has no CPU fallback).
-#include "dsm_surfel_node.hpp"
 #include "driver_io.hpp"
-#include <string>
 
 static uint64_t rng_state = 0x9e3779b97f4a7c15ull;
 static double uniform() // splitmix64, 53 bits
@@ -30,33 +28,23 @@ static double uniform() // splitmix64, 53 bits
 int main(int argc, char **argv)
 {
     if (argc != 21) return 2;
-    const int W = atoi(argv[1]), H = atoi(argv[2]), queries = atoi(argv[13]);
+    const NodeArgs args(argv, true);
+    const int queries = atoi(argv[13]);
     const float voxel = (float)atof(argv[14]);
     const int nx = atoi(argv[15]), ny = atoi(argv[16]), nz = atoi(argv[17]);
     const int n_points = 512, n_traj = 16, per_traj = 8;
     const float step = voxel / 2, radius = 4 * voxel;
-    dsm::SurfelMapNode node(W, H, atof(argv[3]), atof(argv[4]), atof(argv[5]), atof(argv[6]), atof(argv[7]), atof(argv[8]), atoi(argv[9]),
-                            atoi(argv[10]), atoi(argv[11]), atoi(argv[12]), nullptr);
-    if (node.last_error() != DSM_OK) return node.last_error() == DSM_E_NODEVICE ? 3 : 4;
+    DriverNode node(args);
+    if (const int e = setup_code(node.last_error())) return e;
     if (voxel > 0.f && node.enable_distance_field(voxel, nx, ny, nz, !queries) != DSM_OK) return 4;
     if (queries && node.enable_field_queries(n_points, n_traj, n_traj * per_traj) != DSM_OK) return 4;
-    in_f = fopen(argv[18], "rb");
-    out_f = fopen(argv[19], "wb");
-    if (!in_f || !out_f) return 5;
-    const std::string prefix = argv[20];
-    NodeMessages msg;
-    std::vector<dsm_point_t> act, inact;
+    if (!open_io(argv[18], argv[19])) return 5;
     std::vector<dsm_field_sample_t> samples;
     std::vector<dsm_clearance_t> clearance;
     std::vector<double> points((size_t)3 * n_points), waypoints((size_t)3 * n_traj * per_traj);
     std::vector<int32_t> offsets((size_t)n_traj + 1);
     for (int j = 0; j <= n_traj; j++) offsets[(size_t)j] = j * per_traj;
-    int type = 0, r = DSM_OK;
-    while (get(type))
-    {
-        if (!msg.feed(node, type, W, H, r)) return 5;
-        if (r != DSM_OK) return 6;
-        if (type != 2) continue;
+    const int e = feed_script(node, args.W, args.H, [&]() -> int {
         if (voxel > 0.f)
         {
             const float *dist = nullptr;
@@ -89,18 +77,10 @@ int main(int argc, char **argv)
                 put_list(clearance);
             }
         }
-        int rr = node.active_points(act);
-        if (rr == DSM_OK) rr = node.inactive_points(inact);
-        put(rr);
-        put_list(act);
-        put_list(inact);
-    }
-    std::vector<dsm_surfel_t> local;
-    if (node.local_surfels(local) != DSM_OK || node.inactive_points(inact) != DSM_OK) return 6;
-    put_list(local);
-    put_list(inact);
-    if (node.save_mesh(prefix + ".ply") != DSM_OK || node.save_cloud(prefix + ".pcd") != DSM_OK) return 6;
-    fclose(in_f);
-    fclose(out_f);
-    return 0;
+        put_clouds(node);
+        return 0;
+    });
+    if (e) return e;
+    if (!put_final(node) || !save_files(node, argv[20])) return 6;
+    return close_io();
 }

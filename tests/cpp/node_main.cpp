@@ -17,8 +17,6 @@
 //     map:   int32 rc, then local surfels, attached surfels of every pose, active, inactive, all and neighbour points,
 //            each as int32 n + records
 // exit code 3 when no usable GPU (the library has no CPU fallback).
-#include <string>
-#include "dsm_surfel_node.hpp"
 #include "driver_io.hpp"
 
 static void put_pose(const dsm::Pose &p)
@@ -30,14 +28,12 @@ static void put_pose(const dsm::Pose &p)
 int main(int argc, char **argv)
 {
     if (argc != 16) return 2;
-    const int W = atoi(argv[1]), H = atoi(argv[2]), dfp = atoi(argv[9]), device = atoi(argv[10]);
+    const NodeArgs args(argv, true);
+    const int W = args.W, H = args.H, dfp = args.dfp;
     const dsm_constants rgbd = DSM_CONSTANTS_RGBD;
-    dsm::SurfelMapNode node(W, H, atof(argv[3]), atof(argv[4]), atof(argv[5]), atof(argv[6]), atof(argv[7]), atof(argv[8]), dfp, device,
-                            atoi(argv[11]), atoi(argv[12]), atoi(argv[13]) ? &rgbd : nullptr);
-    if (node.last_error() != DSM_OK) return node.last_error() == DSM_E_NODEVICE ? 3 : 4;
-    in_f = fopen(argv[14], "rb");
-    out_f = fopen(argv[15], "wb");
-    if (!in_f || !out_f) return 5;
+    DriverNode node(args, atoi(argv[13]) ? &rgbd : nullptr);
+    if (const int e = setup_code(node.last_error())) return e;
+    if (!open_io(argv[14], argv[15])) return 5;
     NodeMessages msg;
     int rc = DSM_OK, type = 0;
     while (get(type))
@@ -117,7 +113,5 @@ int main(int argc, char **argv)
             return 5;
         if (rc == DSM_OK) rc = r;
     }
-    fclose(in_f);
-    fclose(out_f);
-    return 0;
+    return close_io();
 }

@@ -10,12 +10,9 @@ import pytest
 
 from densesurfelmapping_b200 import capi
 from densesurfelmapping_b200.elements import SURFEL_DTYPE
-from test_checkpoint_format import build, fnv1a64
+from checkpoint_files import CHUNK, JHEADER, RHEADER, build, changed, fnv1a64
 
-JHEADER = np.dtype([("magic", "S8"), ("format", "<u4"), ("zero", "<u4"), ("base", "<u8")])
-RHEADER = np.dtype([("sequence", "<u8"), ("n_pool", "<i4"), ("n_store", "<i4"), ("n_segments", "<i4"), ("k_pool", "<i4"),
-                    ("k_store", "<i4"), ("zero", "<u4"), ("extra_bytes", "<u8")])
-MAGIC, FORMAT, CHUNK = b"DSMJRNL", 1, 256
+MAGIC, FORMAT = b"DSMJRNL", 1
 CALLS = ["dsm_checkpoint_enqueue_incremental", "dsm_map_load_journal", "dsm_map_peek_journal", "dsm_journal_materialize"]
 E_INVALID = -1
 
@@ -32,16 +29,6 @@ def journal_header(base_sum):
     h = np.zeros(1, JHEADER)
     h["magic"], h["format"], h["base"] = MAGIC, FORMAT, base_sum
     return h.tobytes() + u64(fnv1a64(h.tobytes()))
-
-
-def changed(old, new):
-    """Indices of the 256-surfel chunks of `new` that differ from `old` or reach beyond its size (what k_map_delta flags)."""
-    out = []
-    for c in range((len(new) + CHUNK - 1) // CHUNK):
-        a, b = c * CHUNK, min(len(new), c * CHUNK + CHUNK)
-        if b > len(old) or old[a:b].tobytes() != new[a:b].tobytes():
-            out.append(c)
-    return out
 
 
 def record(seq, prev_sum, state, pool_chunks, store_chunks):

@@ -1,41 +1,16 @@
 """The C++ drop-in: include/dsm_fusion_functions.hpp mirrors the reference's FusionFunctions class.
 CPU: it compiles against cv::Mat / Eigen-like caller types and links to the C ABI; without a GPU it
 fails loudly (exit code 3, no fallback).  GPU: its results match the oracle."""
-import atexit
-import functools
 import os
-import shutil
 import struct
 import subprocess
-import tempfile
 
 import numpy as np
 import pytest
 
 from densesurfelmapping_b200 import synth
 from densesurfelmapping_b200.elements import SURFEL_DTYPE
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-PKG = os.path.join(ROOT, "densesurfelmapping_b200")
-
-
-@functools.lru_cache(maxsize=None)
-def _bin_dir():
-    d = tempfile.mkdtemp(prefix="dsm_cpp_adapter_")
-    atexit.register(shutil.rmtree, d, True)
-    return d
-
-
-@functools.lru_cache(maxsize=None)
-def build_adapter(name="adapter_main"):
-    """tests/cpp/<name>.cpp compiled once per session, outside the tree (the checkout may be read-only)."""
-    src = os.path.join(ROOT, "tests", "cpp", name + ".cpp")
-    out = os.path.join(_bin_dir(), name)
-    cmd = ["g++", "-std=c++11", "-O2", "-Wall", "-I", os.path.join(ROOT, "include"), "-I", os.path.join(ROOT, "oracle", "shim"), src,
-           "-o", out, "-L", PKG, "-ldsm_b200", f"-Wl,-rpath,{PKG}"]
-    r = subprocess.run(cmd, capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr
-    return out
+from node_drive import build_adapter, cam_args
 
 
 def run_adapter(tmp, cam, ref, pose, gray, depth, local):
@@ -43,7 +18,7 @@ def run_adapter(tmp, cam, ref, pose, gray, depth, local):
     with open(fin, "wb") as f:
         f.write(struct.pack("<i", ref) + np.asarray(pose, np.float32).tobytes() + struct.pack("<i", len(local)))
         f.write(gray.tobytes() + depth.tobytes() + local.tobytes())
-    args = [build_adapter(), str(cam.width), str(cam.height)] + [repr(float(v)) for v in (cam.fx, cam.fy, cam.cx, cam.cy, cam.far, cam.near)] + [fin, fout]
+    args = [build_adapter()] + cam_args(cam) + [fin, fout]
     r = subprocess.run(args, capture_output=True, text=True)
     return r, fout
 
@@ -94,7 +69,7 @@ def run_resident(tmp, cam, frames, warp, retire_kf):
     fin = os.path.join(tmp, "stream.bin")
     outs = [os.path.join(tmp, n) for n in ("out.bin", "cloud.pcd", "mesh.ply")]
     write_stream(fin, cam, frames, warp, retire_kf)
-    args = [exe, str(cam.width), str(cam.height)] + [repr(float(v)) for v in (cam.fx, cam.fy, cam.cx, cam.cy, cam.far, cam.near)] + [fin] + outs
+    args = [exe] + cam_args(cam) + [fin] + outs
     return subprocess.run(args, capture_output=True, text=True), outs
 
 
@@ -112,7 +87,6 @@ def test_resident_helper_compiles_and_fails_loudly_without_gpu(tmp_path):
 @pytest.mark.gpu
 def test_resident_helper_flow_matches_oracle(tmp_path):
     import pyoracle
-    from test_gpu_resident import match_as_sets
     from util import oracle_for
     cam = synth.VGA
     orc = oracle_for(cam)

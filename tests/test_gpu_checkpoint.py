@@ -6,57 +6,25 @@ as it was; the first snapshot after a load forwards the whole inactive cloud; an
 own checkpoint (tests/cpp/checkpoint_main.cpp)."""
 import ctypes
 import os
-import subprocess
 
 import numpy as np
 import pytest
 
 from densesurfelmapping_b200 import capi, synth
 from densesurfelmapping_b200.elements import SURFEL_DTYPE
-from test_checkpoint_format import parse
-from test_gpu_publish import Mirror, simple_lists, snapshot_equals_readers, warp
-from test_gpu_window_stream import CAM, T, new_ctx, windowed
-from test_surfel_node import Script, drive
+from checkpoint_files import parse
+from node_drive import node_script, run_driver
+from resident_map import (
+    Mirror, SAVES, STORE, T, loop_warp, made, new_ctx, readers, run, simple_lists, snapshot_equals_readers, stored_keyframes,
+    windowed)
+from util import CAM
 
 pytestmark = pytest.mark.gpu
-
-STORE = 1 << 18
-CONSTANTS = {"drive": capi.CONSTANTS_DRIVE, "rgbd": capi.CONSTANTS_RGBD}
-# save point k (frames 0..k-1 fused) of simple_lists(), and a loop-closure warp issued right before the save or right
-# after the load
-SAVES = {"after_retirement": (5, None), "after_reactivation": (14, None), "keyframe0_back": (10, None),
-         "after_transforms": (8, "before"), "warp_after_load": (12, "after")}
-
-
-def readers(ctx):
-    return (ctx.pool_download().tobytes(), ctx.inactive_download(-1).tobytes(), ctx.inactive_segments().tobytes(),
-            ctx.inactive_export_cloud().tobytes(), ctx.pool_export_cloud(5).tobytes())
 
 
 def assert_same(a, b, what):
     for name, x, y in zip(("pool", "store", "segments", "inactive cloud", "active cloud"), readers(a), readers(b)):
         assert x == y, f"{what}: {name} differs"
-
-
-def run(ctx, lists, t0, t1, chunk):
-    for s in range(t0, t1, chunk):
-        windowed(ctx, s, min(t1, s + chunk), lists, want_counts=False)
-
-
-def loop_warp(ctx, kfs):
-    ctx.pool_transform(warp(1))
-    for kf in kfs:
-        ctx.inactive_transform(kf, warp(2))
-
-
-def stored_keyframes(ctx):
-    return sorted(set(ctx.inactive_segments()[:, 0].tolist()))
-
-
-def made(constants="drive", **kw):
-    ctx = new_ctx(**kw)
-    ctx.set_constants(CONSTANTS[constants])
-    return ctx
 
 
 @pytest.mark.parametrize("save", sorted(SAVES))
@@ -305,30 +273,15 @@ def test_publishing_after_a_load(tmp_path, chunk):
 N_NODE = 24
 
 
-def run_checkpoint_main(tmp, cam, script, drift_free_poses, j):
-    from test_cpp_adapter import build_adapter
-    exe = build_adapter("checkpoint_main")
-    fin, fout, ckpt = os.path.join(tmp, "script.bin"), os.path.join(tmp, "out.bin"), os.path.join(tmp, "node.dsm")
-    with open(fin, "wb") as f:
-        f.write(bytes(script.b))
-    args = [exe, str(cam.width), str(cam.height)] + [repr(float(v)) for v in (cam.fx, cam.fy, cam.cx, cam.cy, cam.far, cam.near)]
-    r = subprocess.run(args + [str(drift_free_poses), str(j), ckpt, fin, fout, tmp], capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr
-    return np.frombuffer(open(fout, "rb").read(), np.int32)
-
-
 # j: messages fed before the save (three per frame: orb, image, depth); frame 16's orb message brings the first loop
 # correction that moves every pose, frame 9's a loop edge back to keyframe 0
 @pytest.mark.parametrize("drift_free_poses,j", [(1, 3 * 7 + 1), (1, 3 * 16 + 1), (1, 3 * 11 + 2), (10, 3 * 9 + 2),
                                                 (10, 3 * 16 + 1), (2, 3 * 13 + 3)])
 def test_node_resumes_from_its_checkpoint(tmp_path, drift_free_poses, j):
     cam = synth.KITTI
-    msgs = drive(N_NODE)
-    sc = Script()
-    for t, (stamp, is_kf, ref, p7, path, loops) in enumerate(msgs):
-        sc.orb(stamp, is_kf, ref, p7, path, loops)
-        sc.images(stamp, *synth.make_frame(cam, 3000 + t, synth.pose_stream(t)))
-    out = run_checkpoint_main(str(tmp_path), cam, sc, drift_free_poses, j).tolist()
+    sc = node_script(cam, N_NODE)
+    ckpt = os.path.join(tmp_path, "node.dsm")
+    out = run_driver("checkpoint_main", str(tmp_path), cam, sc, [drift_free_poses, j, ckpt], after=[tmp_path]).take(np.int32, -1).tolist()
     n_rest = 3 * N_NODE - j
     assert len(out) == 3 + 3 * n_rest + 5
     assert out[:3] == [0, 0, 1], "save, load, equal right after the load"

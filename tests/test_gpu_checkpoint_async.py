@@ -6,18 +6,16 @@ snapshot.  Checkpoints leave the map exactly as a drive without them; a fresh co
 and call-sequence contract; and dsm::SurfelMapNode's save_state_async (tests/cpp/checkpoint_async_main.cpp)."""
 import ctypes
 import os
-import subprocess
 
 import numpy as np
 import pytest
 
 from densesurfelmapping_b200 import capi, synth
 from densesurfelmapping_b200.elements import SURFEL_DTYPE
-from test_checkpoint_format import parse
-from test_gpu_checkpoint import SAVES, STORE, loop_warp, made, readers, run, stored_keyframes
-from test_gpu_publish import simple_lists
-from test_gpu_window_stream import CAM, T, frames, new_ctx, windowed
-from test_surfel_node import Script, drive
+from checkpoint_files import parse
+from node_drive import node_script, run_driver
+from resident_map import SAVES, STORE, T, frames, loop_warp, made, new_ctx, readers, run, simple_lists, stored_keyframes, windowed
+from util import CAM
 
 pytestmark = pytest.mark.gpu
 
@@ -302,29 +300,13 @@ def test_a_publish_snapshot_and_a_checkpoint_in_flight_together(tmp_path):
 N_NODE = 24
 
 
-def run_checkpoint_async_main(tmp, cam, script, drift_free_poses, j):
-    from test_cpp_adapter import build_adapter
-    exe = build_adapter("checkpoint_async_main")
-    fin, fout = os.path.join(tmp, "script.bin"), os.path.join(tmp, "out.bin")
-    with open(fin, "wb") as f:
-        f.write(bytes(script.b))
-    args = [exe, str(cam.width), str(cam.height)] + [repr(float(v)) for v in (cam.fx, cam.fy, cam.cx, cam.cy, cam.far, cam.near)]
-    args += [str(drift_free_poses), str(j), os.path.join(tmp, "a.dsm"), os.path.join(tmp, "t.dsm"), fin, fout, tmp]
-    r = subprocess.run(args, capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr
-    return np.frombuffer(open(fout, "rb").read(), np.int32)
-
-
 # j: messages fed before the save (three per frame: orb, image, depth), the save points of test_gpu_checkpoint.py's node
 @pytest.mark.parametrize("drift_free_poses,j", [(1, 3 * 7 + 1), (1, 3 * 16 + 1), (10, 3 * 9 + 2), (2, 3 * 13 + 3)])
 def test_node_save_state_async(tmp_path, drift_free_poses, j):
     cam = synth.KITTI
-    msgs = drive(N_NODE)
-    sc = Script()
-    for t, (stamp, is_kf, ref, p7, path, loops) in enumerate(msgs):
-        sc.orb(stamp, is_kf, ref, p7, path, loops)
-        sc.images(stamp, *synth.make_frame(cam, 3000 + t, synth.pose_stream(t)))
-    out = run_checkpoint_async_main(str(tmp_path), cam, sc, drift_free_poses, j).tolist()
+    sc = node_script(cam, N_NODE)
+    args = [drift_free_poses, j, tmp_path / "a.dsm", tmp_path / "t.dsm"]
+    out = run_driver("checkpoint_async_main", str(tmp_path), cam, sc, args, after=[tmp_path]).take(np.int32, -1).tolist()
     n_rest = 3 * N_NODE - j
     assert len(out) == 3 + n_rest + 4 + 3 * n_rest + 2
     assert out[:3] == [0, 0, 0], "enable, save_state_async, twin's save_state"

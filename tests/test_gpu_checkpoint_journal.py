@@ -6,18 +6,14 @@ position; every record lists exactly the 256-surfel chunks that differ between t
 leave the map as a drive without them; a fresh context resumes from the journal; and dsm::SurfelMapNode's
 save_state_incremental / load_state_incremental (tests/cpp/checkpoint_journal_main.cpp)."""
 import os
-import subprocess
 
 import numpy as np
 import pytest
 
 from densesurfelmapping_b200 import capi, synth
-from test_checkpoint_format import parse
-from test_checkpoint_journal_format import JHEADER, RHEADER, changed
-from test_gpu_checkpoint import SAVES, STORE, loop_warp, made, readers, run, stored_keyframes
-from test_gpu_publish import simple_lists
-from test_gpu_window_stream import T, new_ctx, windowed
-from test_surfel_node import Script, drive
+from checkpoint_files import JHEADER, RHEADER, changed, parse
+from node_drive import node_script, run_driver
+from resident_map import SAVES, STORE, T, loop_warp, made, new_ctx, readers, run, simple_lists, stored_keyframes, windowed
 
 pytestmark = pytest.mark.gpu
 
@@ -261,29 +257,13 @@ def test_resume_from_the_journal(tmp_path, k):
 N_NODE = 24
 
 
-def run_checkpoint_journal_main(tmp, cam, script, drift_free_poses, every, j):
-    from test_cpp_adapter import build_adapter
-    exe = build_adapter("checkpoint_journal_main")
-    fin, fout = os.path.join(tmp, "script.bin"), os.path.join(tmp, "out.bin")
-    with open(fin, "wb") as f:
-        f.write(bytes(script.b))
-    args = [exe, str(cam.width), str(cam.height)] + [repr(float(v)) for v in (cam.fx, cam.fy, cam.cx, cam.cy, cam.far, cam.near)]
-    args += [str(drift_free_poses), str(every), str(j), os.path.join(tmp, "a.dsm"), fin, fout, tmp]
-    r = subprocess.run(args, capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr
-    return np.frombuffer(open(fout, "rb").read(), np.int32)
-
-
 # every: messages between incremental saves; j: messages fed before node B resumes from A's journal
 @pytest.mark.parametrize("drift_free_poses,every,j", [(1, 6, 3 * 16 + 1), (10, 3, 3 * 9 + 2), (2, 9, 3 * 13 + 3)])
 def test_node_save_state_incremental(tmp_path, drift_free_poses, every, j):
     cam = synth.KITTI
-    msgs = drive(N_NODE)
-    sc = Script()
-    for t, (stamp, is_kf, ref, p7, path, loops) in enumerate(msgs):
-        sc.orb(stamp, is_kf, ref, p7, path, loops)
-        sc.images(stamp, *synth.make_frame(cam, 3000 + t, synth.pose_stream(t)))
-    out = run_checkpoint_journal_main(str(tmp_path), cam, sc, drift_free_poses, every, j).tolist()
+    sc = node_script(cam, N_NODE)
+    args = [drift_free_poses, every, j, tmp_path / "a.dsm"]
+    out = run_driver("checkpoint_journal_main", str(tmp_path), cam, sc, args, after=[tmp_path]).take(np.int32, -1).tolist()
     n_rest = 3 * N_NODE - j
     n_saves = -(-j // every)
     assert len(out) == 2 + 2 * n_saves + 3 + 3 * n_rest + 1

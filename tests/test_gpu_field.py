@@ -5,8 +5,6 @@ dsm_inactive_export_cloud) at the same position in the stream, bit for bit, with
 field changes nothing in the map; the rejected-frame and error contracts; and dsm::SurfelMapNode::distance_field
 (tests/cpp/field_main.cpp)."""
 import filecmp
-import os
-import subprocess
 
 import numpy as np
 import pytest
@@ -14,58 +12,21 @@ import pytest
 import pyoracle_field
 from densesurfelmapping_b200 import capi, synth
 from densesurfelmapping_b200.elements import POINT_DTYPE, SURFEL_DTYPE
-from test_gpu_publish import STORE, simple_lists, warp
-from test_gpu_window_stream import CAM, T, frames, new_ctx, windowed
-from test_surfel_node import Reader, Script, drive
+from node_drive import node_script, run_driver
+from resident_map import (
+    COMBOS, SHAPES, STORE, T, assert_field, camera, centres, field_points, map_state, new_ctx, simple_lists, warp, windowed,
+    xyz)
+from util import CAM
 
 pytestmark = pytest.mark.gpu
-
-SHAPES = [(37, 41, 13), (64, 64, 32), (1, 1, 1), (128, 1, 7)]
-COMBOS = [(m, v) for m in (1, 5) for v in (0.125, 0.1, 0.3)]
-
-
-def xyz(*clouds):
-    return np.concatenate([c.view(np.float32).reshape(-1, 4)[:, :3] for c in clouds])
-
-
-def camera(t):
-    return frames()[t][0][12:15].astype(np.float64)
-
-
-def readers(ctx, m):
-    return xyz(ctx.pool_export_cloud(m), ctx.inactive_export_cloud())
-
-
-def assert_field(got, want, what):
-    dist, origin, n_occ = got
-    assert origin.tolist() == want[1].tolist(), f"{what}: origin"
-    assert n_occ == want[2], f"{what}: occupied voxels {n_occ}, want {want[2]}"
-    assert dist.shape == want[0].shape and dist.tobytes() == want[0].tobytes(), \
-        f"{what}: {(dist.view(np.uint32) != want[0].view(np.uint32)).sum()} voxels differ"
 
 
 def field_equals_oracle(ctx, voxel, shape, center, m, what):
     ctx.field_enqueue(center, m)
     got = ctx.field_wait()
-    want = pyoracle_field.field(readers(ctx, m), voxel, shape, center)
+    want = pyoracle_field.field(field_points(ctx, m), voxel, shape, center)
     assert_field(got, want, what)
     return got
-
-
-def centres(ctx, t, voxel, shape, m):
-    """At the camera of frame t; on the edge of the map's bounding box, so that half of the grid lies beyond it; far
-    outside it, so that nothing is occupied; and in the middle of the voxel of an obstacle point, so that even a grid of
-    one voxel is occupied."""
-    pts = readers(ctx, 1)
-    lo, hi = pts.min(0).astype(np.float64), pts.max(0).astype(np.float64)
-    edge = (lo + hi) / 2
-    edge[0] = hi[0]
-    far = hi + np.array(shape) * voxel + 100.0
-    obstacles = readers(ctx, m)   # none before the first surfel reaches m updates
-    cell = None
-    if len(obstacles):
-        cell = (np.floor(obstacles[len(obstacles) // 2] / np.float32(voxel)).astype(np.float64) + 0.5) * float(np.float32(voxel))
-    return [("camera", camera(t)), ("half off the map", edge), ("off the map", far), ("on an obstacle", cell)]
 
 
 @pytest.mark.parametrize("shape", SHAPES, ids=lambda s: "x".join(map(str, s)))
@@ -138,17 +99,13 @@ def test_field_beside_a_publish_snapshot_and_an_asynchronous_checkpoint(tmp_path
     assert ctx.checkpoint_wait(True)
     ref = new_ctx(store=STORE)
     windowed(ref, 0, 10, lists, want_counts=False)
-    assert_field(got, pyoracle_field.field(readers(ref, 5), voxel, shape, camera(9)), "field")
+    assert_field(got, pyoracle_field.field(field_points(ref, 5), voxel, shape, camera(9)), "field")
     assert active.tobytes() == ref.pool_export_cloud(5).tobytes() and inactive.tobytes() == ref.inactive_export_cloud().tobytes()
     ref.map_save(str(tmp_path / "sync.dsm"))
     assert filecmp.cmp(str(tmp_path / "async.dsm"), str(tmp_path / "sync.dsm"), shallow=False)
     assert len(inactive) > 0
     ctx.close()
     ref.close()
-
-
-def map_state(ctx):
-    return (ctx.pool_download().tobytes(), ctx.inactive_download(-1).tobytes(), ctx.inactive_segments().tobytes())
 
 
 @pytest.mark.parametrize("chunk", [1, 4])
@@ -194,7 +151,7 @@ def test_rejected_frame_comes_back_from_wait_and_stays_for_the_next_read():
     with pytest.raises(capi.DsmError) as e:
         b.field_wait()
     assert e.value.code == -6
-    want = pyoracle_field.field(readers(a, 1), voxel, shape, camera(first - 1))
+    want = pyoracle_field.field(field_points(a, 1), voxel, shape, camera(first - 1))
     assert_field(e.value.field, want, "field after the rejected frame")
     assert want[2] > 0
     with pytest.raises(capi.DsmError) as e:
@@ -250,7 +207,7 @@ def test_error_contract(tmp_path):
         ctx.map_load_journal(str(tmp_path / "m.dsm"))
     assert e.value.code == -7
     got = ctx.field_wait()
-    assert_field(got, pyoracle_field.field(readers(ctx, 5), 0.5, (16, 16, 8), camera(7)), "field after the refused calls")
+    assert_field(got, pyoracle_field.field(field_points(ctx, 5), 0.5, (16, 16, 8), camera(7)), "field after the refused calls")
     assert lib.dsm_field_wait(ctx.h, None, None, None) == -7                         # retired
     ctx.inactive_load(surfels, segs)                                                 # nothing in flight: allowed again
     ctx.map_load(str(tmp_path / "m.dsm"))
@@ -261,31 +218,14 @@ def test_error_contract(tmp_path):
 FIELD = (0.2, 96, 96, 32)
 
 
-def run_field_main(tmp, cam, script, voxel_shape, publish, tag):
-    from test_cpp_adapter import build_adapter
-    exe = build_adapter("field_main")
-    fin, fout, prefix = (os.path.join(tmp, f"{x}{tag}") for x in ("script.bin", "out.bin", "map"))
-    with open(fin, "wb") as f:
-        f.write(bytes(script.b))
-    args = [exe, str(cam.width), str(cam.height)] + [repr(float(v)) for v in (cam.fx, cam.fy, cam.cx, cam.cy, cam.far, cam.near)]
-    args += ["2", "0", str(1 << 20), str(1 << 21), str(publish)] + [repr(float(voxel_shape[0]))] + [str(n) for n in voxel_shape[1:]]
-    args += [fin, fout, prefix]
-    r = subprocess.run(args, capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr
-    return Reader(open(fout, "rb").read()), prefix
-
-
 @pytest.mark.parametrize("publish", [0, 1])
 def test_node_field_equals_the_oracle_and_changes_nothing(tmp_path, publish):
     cam, n = synth.KITTI, 24
-    msgs = drive(n)
-    sc = Script()
-    for t, (stamp, is_kf, ref, p7, path, loops) in enumerate(msgs):
-        sc.orb(stamp, is_kf, ref, p7, path, loops)
-        sc.images(stamp, *synth.make_frame(cam, 3000 + t, synth.pose_stream(t)))
+    sc = node_script(cam, n)
     voxel, nx, ny, nz = FIELD
-    r, pa = run_field_main(str(tmp_path), cam, sc, FIELD, publish, "a")
-    q, pb = run_field_main(str(tmp_path), cam, sc, (0.0, 1, 1, 1), publish, "b")
+    pa, pb = str(tmp_path / "mapa"), str(tmp_path / "mapb")
+    r = run_driver("field_main", str(tmp_path), cam, sc, [2, 0, 1 << 20, 1 << 21, publish, *FIELD], tag="a", after=[pa])
+    q = run_driver("field_main", str(tmp_path), cam, sc, [2, 0, 1 << 20, 1 << 21, publish, 0.0, 1, 1, 1], tag="b", after=[pb])
     occupied = 0
     for t in range(n):
         rc = r.i()

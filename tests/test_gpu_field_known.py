@@ -8,8 +8,6 @@ change nothing in the map, the plain fields or the published clouds; a known fie
 asynchronous checkpoint, and a query on it; the rejected-frame and error contracts; and a size a user runs.  The node is
 checked through tests/cpp/field_known_main.cpp."""
 import filecmp
-import os
-import subprocess
 
 import numpy as np
 import pytest
@@ -19,10 +17,8 @@ import pyoracle_field_known
 import pyoracle_field_query
 from densesurfelmapping_b200 import capi, synth
 from densesurfelmapping_b200.elements import POINT_DTYPE, SEED_DTYPE, SURFEL_DTYPE
-from test_gpu_field import SHAPES, camera, map_state, readers, xyz
-from test_gpu_publish import STORE, simple_lists, warp
-from test_gpu_window_stream import CAM, T, frames, new_ctx, windowed
-from test_surfel_node import Reader, Script, drive
+from node_drive import node_script, run_driver
+from resident_map import SHAPES, STORE, T, camera, field_points, frames, map_state, new_ctx, simple_lists, warp, windowed, xyz
 
 pytestmark = pytest.mark.gpu
 
@@ -73,7 +69,7 @@ def known_equals_oracle(ctx, views, voxel, shape, center, m, what, host_copy=Tru
     ctx.field_enqueue_known(center, m, all_slots, poses, host_copy=host_copy)
     dist, origin, n_occ = ctx.field_wait()
     state, n_free = ctx.field_state()
-    want = pyoracle_field_known.known_field(readers(ctx, m), voxel, shape, center, views.oracle_views(all_slots), MAX_RANGE)
+    want = pyoracle_field_known.known_field(field_points(ctx, m), voxel, shape, center, views.oracle_views(all_slots), MAX_RANGE)
     assert origin.tolist() == want[1].tolist(), f"{what}: origin"
     assert (n_occ, n_free) == (want[2], want[4]), f"{what}: occupied / free {n_occ} / {n_free}, want {want[2]} / {want[4]}"
     if host_copy:
@@ -154,7 +150,7 @@ def test_geometry_of_the_synthetic_scene():
     assert [int(at(p)) for p in to_box] == [pyoracle_field_known.FREE] * len(to_box)
     below = [np.array([c[0] + dx, 2.65, c[2] + dz]) for dx in (-2.0, 0.0, 2.0) for dz in (1.0, 3.0, 5.0)]
     assert [int(at(p)) for p in below] == [pyoracle_field_known.UNKNOWN] * len(below)
-    plain = pyoracle_field.field(readers(ctx, 5), voxel, shape, c)
+    plain = pyoracle_field.field(field_points(ctx, 5), voxel, shape, c)
     assert (want[0] <= plain[0]).all() and want[2] == plain[2]
     ctx.close()
 
@@ -232,7 +228,7 @@ def test_known_field_beside_a_snapshot_a_checkpoint_and_a_query(tmp_path):
     ref = new_ctx(store=STORE)
     for t0 in range(0, 10, 2):
         windowed(ref, t0, t0 + 2, lists, want_counts=False)
-    want = pyoracle_field_known.known_field(readers(ref, 5), voxel, shape, camera(9), views.oracle_views(slots), MAX_RANGE)
+    want = pyoracle_field_known.known_field(field_points(ref, 5), voxel, shape, camera(9), views.oracle_views(slots), MAX_RANGE)
     assert dist is None and state is None and (n_occ, n_free) == (want[2], want[4]) and origin.tolist() == want[1].tolist()
     q = pyoracle_field_query.sample(want[0], want[1], voxel, pts)
     assert samples.tobytes() == q.tobytes()
@@ -263,7 +259,7 @@ def test_rejected_frame_comes_back_from_wait():
         b.field_wait()
     assert e.value.code == -6
     state, n_free = b.field_state()
-    want = pyoracle_field_known.known_field(readers(a, 1), voxel, shape, camera(first - 1), views.oracle_views(slots), MAX_RANGE)
+    want = pyoracle_field_known.known_field(field_points(a, 1), voxel, shape, camera(first - 1), views.oracle_views(slots), MAX_RANGE)
     assert e.value.field[0].tobytes() == want[0].tobytes() and e.value.field[2] == want[2] and want[2] > 0
     assert state.tobytes() == want[3].tobytes() and n_free == want[4] > 0
     with pytest.raises(capi.DsmError) as e:
@@ -414,33 +410,17 @@ MAX_VIEWS = 5
 RELOAD = 12   # the node saves and loads its state after this depth message
 
 
-def run_field_known_main(tmp, cam, script, known, tag):
-    from test_cpp_adapter import build_adapter
-    exe = build_adapter("field_known_main")
-    fin, fout, prefix = (os.path.join(tmp, f"{x}{tag}") for x in ("script.bin", "out.bin", "map"))
-    with open(fin, "wb") as f:
-        f.write(bytes(script.b))
-    args = [exe, str(cam.width), str(cam.height)] + [repr(float(v)) for v in (cam.fx, cam.fy, cam.cx, cam.cy, cam.far, cam.near)]
-    args += ["2", "0", str(1 << 20), str(1 << 21), repr(float(FIELD[0]))] + [str(n) for n in FIELD[1:]]
-    args += [str(MAX_VIEWS if known else 0), repr(MAX_RANGE), str(RELOAD), fin, fout, prefix]
-    r = subprocess.run(args, capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr
-    return Reader(open(fout, "rb").read()), prefix
-
-
 def test_node_known_space_equals_the_oracle_and_changes_nothing(tmp_path):
     """The node drive (keyframes, loop closures): every fused frame's known field equals the oracle over the views the
     node carried (the driver dumps their frames' seeds and current poses); clouds, PLY and PCD files equal a twin
     without known space; after load_state the slot table is empty and refills."""
     cam, n = synth.KITTI, 24
-    msgs = drive(n)
-    sc = Script()
-    for t, (stamp, is_kf, ref, p7, path, loops) in enumerate(msgs):
-        sc.orb(stamp, is_kf, ref, p7, path, loops)
-        sc.images(stamp, *synth.make_frame(cam, 3000 + t, synth.pose_stream(t)))
+    sc = node_script(cam, n)
     voxel, nx, ny, nz = FIELD
-    r, pa = run_field_known_main(str(tmp_path), cam, sc, True, "a")
-    q, pb = run_field_known_main(str(tmp_path), cam, sc, False, "b")
+    pa, pb = str(tmp_path / "mapa"), str(tmp_path / "mapb")
+    node = [2, 0, 1 << 20, 1 << 21, *FIELD]
+    r = run_driver("field_known_main", str(tmp_path), cam, sc, node + [MAX_VIEWS, MAX_RANGE, RELOAD], tag="a", after=[pa])
+    q = run_driver("field_known_main", str(tmp_path), cam, sc, node + [0, MAX_RANGE, RELOAD], tag="b", after=[pb])
     free, most = 0, 0
     for t in range(n):
         rc = r.i()

@@ -6,8 +6,6 @@ its host copy does; the query keeps the grid of its own request when the next fi
 beside a snapshot and an asynchronous checkpoint; queries change nothing in the map, the clouds or the fields; the
 rejected-frame and error contracts; planner sizes; and dsm::SurfelMapNode with a resident field
 (tests/cpp/field_query_main.cpp)."""
-import os
-import subprocess
 
 import numpy as np
 import pytest
@@ -16,10 +14,10 @@ import pyoracle_field
 import pyoracle_field_query as fq
 from densesurfelmapping_b200 import capi, synth
 from densesurfelmapping_b200.elements import POINT_DTYPE, SURFEL_DTYPE
-from test_gpu_field import COMBOS, SHAPES, assert_field, camera, centres, map_state, readers, xyz
-from test_gpu_publish import STORE, simple_lists, warp
-from test_gpu_window_stream import T, new_ctx, windowed
-from test_surfel_node import Reader, Script, drive
+from node_drive import node_script, run_driver
+from resident_map import (
+    COMBOS, SHAPES, STORE, T, assert_field, camera, centres, field_points, map_state, new_ctx, simple_lists, warp, windowed,
+    xyz)
 
 pytestmark = pytest.mark.gpu
 
@@ -163,9 +161,9 @@ def test_a_query_keeps_the_grid_of_its_own_request():
     windowed(ctx, 0, 14, lists, want_counts=False)
     ctx.field_enqueue(camera(13), 5, host_copy=False)
     ctx.field_wait()
-    want_a = pyoracle_field.field(readers(ctx, 5), voxel, shape, camera(13))
+    want_a = pyoracle_field.field(field_points(ctx, 5), voxel, shape, camera(13))
     other = camera(13) + np.array([1.3, -0.7, 0.4])
-    want_b = pyoracle_field.field(readers(ctx, 1), voxel, shape, other)
+    want_b = pyoracle_field.field(field_points(ctx, 1), voxel, shape, other)
     pts = np.concatenate([query_points(rng, want_a[1], voxel, shape), query_points(rng, want_b[1], voxel, shape)])
     wp, ofs = query_trajectories(rng, want_a[1], voxel, shape)
     ctx.field_query_enqueue(pts, wp, ofs, voxel / 2, 0.25)
@@ -194,7 +192,7 @@ def test_queries_beside_a_publish_snapshot_and_an_asynchronous_checkpoint(tmp_pa
     windowed(ctx, 0, 10, lists, want_counts=False)
     ref = new_ctx(store=STORE)
     windowed(ref, 0, 10, lists, want_counts=False)
-    want = pyoracle_field.field(readers(ref, 5), voxel, shape, camera(9))
+    want = pyoracle_field.field(field_points(ref, 5), voxel, shape, camera(9))
     pts = query_points(rng, want[1], voxel, shape)
     wp, ofs = query_trajectories(rng, want[1], voxel, shape)
     ctx.publish_enqueue(5)
@@ -266,7 +264,7 @@ def test_rejected_frame_comes_back_from_the_query_wait():
     b.field_query_enable(*CAPS)
     windowed(b, 0, first + 2, lists, want_counts=False)
     b.field_enqueue(camera(first - 1), 1, host_copy=False)
-    want = pyoracle_field.field(readers(a, 1), voxel, shape, camera(first - 1))
+    want = pyoracle_field.field(field_points(a, 1), voxel, shape, camera(first - 1))
     pts = query_points(rng, want[1], voxel, shape)
     wp, ofs = query_trajectories(rng, want[1], voxel, shape)
     b.field_query_enqueue(pts, wp, ofs, voxel / 2, 0.3)
@@ -354,7 +352,7 @@ def test_error_contract():
     assert lib.dsm_field_query_wait(ctx.h, capi.ctypes.byref(s), capi.ctypes.byref(c)) == 0
     ctx.field_query_enqueue(*ok, 0.1, 0.2)
     got = ctx.field_query_wait()
-    dist = pyoracle_field.field(readers(ctx, 5), 0.25, (16, 16, 8), camera(7))
+    dist = pyoracle_field.field(field_points(ctx, 5), 0.25, (16, 16, 8), camera(7))
     assert field[1].tolist() == dist[1].tolist()
     assert_query(got, expected(dist[0], dist[1], 0.25, *ok, 0.1, 0.2), "query after the refused calls")
     ctx.close()
@@ -371,7 +369,7 @@ def test_queries_at_planner_sizes():
     windowed(ctx, 0, T, lists, want_counts=False)
     ctx.field_enqueue(camera(T - 1), 5, host_copy=False)
     _, origin, n_occ = ctx.field_wait()
-    want = pyoracle_field.field(readers(ctx, 5), voxel, shape, camera(T - 1))
+    want = pyoracle_field.field(field_points(ctx, 5), voxel, shape, camera(T - 1))
     assert origin.tolist() == want[1].tolist() and n_occ == want[2] > 0
     o, n3 = origin.astype(np.float64), np.array(shape, np.float64)
     pts = (o - 1 + rng.random((1 << 20, 3)) * (n3 + 2)) * float(np.float32(voxel))
@@ -387,31 +385,14 @@ def test_queries_at_planner_sizes():
 FIELD = (0.2, 96, 96, 32)
 
 
-def run_field_query_main(tmp, cam, script, voxel_shape, queries, tag):
-    from test_cpp_adapter import build_adapter
-    exe = build_adapter("field_query_main")
-    fin, fout, prefix = (os.path.join(tmp, f"{x}{tag}") for x in ("script.bin", "out.bin", "map"))
-    with open(fin, "wb") as f:
-        f.write(bytes(script.b))
-    args = [exe, str(cam.width), str(cam.height)] + [repr(float(v)) for v in (cam.fx, cam.fy, cam.cx, cam.cy, cam.far, cam.near)]
-    args += ["2", "0", str(1 << 20), str(1 << 21), str(queries)] + [repr(float(voxel_shape[0]))] + [str(n) for n in voxel_shape[1:]]
-    args += [fin, fout, prefix]
-    r = subprocess.run(args, capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr
-    return Reader(open(fout, "rb").read()), prefix
-
-
 def test_node_queries_equal_the_oracle_and_change_nothing(tmp_path):
     import filecmp
     cam, n = synth.KITTI, 24
-    msgs = drive(n)
-    sc = Script()
-    for t, (stamp, is_kf, ref, p7, path, loops) in enumerate(msgs):
-        sc.orb(stamp, is_kf, ref, p7, path, loops)
-        sc.images(stamp, *synth.make_frame(cam, 3000 + t, synth.pose_stream(t)))
+    sc = node_script(cam, n)
     voxel, nx, ny, nz = FIELD
-    r, pa = run_field_query_main(str(tmp_path), cam, sc, FIELD, 1, "a")
-    q, pb = run_field_query_main(str(tmp_path), cam, sc, (0.0, 1, 1, 1), 0, "b")
+    pa, pb = str(tmp_path / "mapa"), str(tmp_path / "mapb")
+    r = run_driver("field_query_main", str(tmp_path), cam, sc, [2, 0, 1 << 20, 1 << 21, 1, *FIELD], tag="a", after=[pa])
+    q = run_driver("field_query_main", str(tmp_path), cam, sc, [2, 0, 1 << 20, 1 << 21, 0, 0.0, 1, 1, 1], tag="b", after=[pb])
     hits = 0
     for t in range(n):
         rc = r.i()

@@ -13,8 +13,8 @@ import pytest
 import pyoracle_clouds
 from densesurfelmapping_b200 import capi, synth
 from densesurfelmapping_b200.elements import POINT_DTYPE, SURFEL_DTYPE
-from test_cpp_adapter import build_adapter
-from test_node_clouds import CAM, canon_points, needs_refmap_clouds, neighbor_replay
+from node_drive import build_adapter
+from util import CAM, canon_points, needs_refmap_clouds, neighbor_replay
 
 pytestmark = pytest.mark.gpu
 

@@ -8,7 +8,7 @@ import pytest
 
 from densesurfelmapping_b200 import synth
 from densesurfelmapping_b200.elements import SURFEL_DTYPE
-from util import check_seeds, check_surfels, compact_like_caller, oracle_for, bits_equal_nan
+from util import bits_equal_nan, check_seeds, check_surfels, compact_like_caller, oracle_for
 
 pytestmark = pytest.mark.gpu
 

@@ -8,7 +8,7 @@ import pytest
 import pyoracle
 from densesurfelmapping_b200 import synth
 from densesurfelmapping_b200.elements import SURFEL_DTYPE
-from util import check_surfels
+from util import CAM as RCAM, check_surfels, poststep_frames
 
 pytestmark = pytest.mark.gpu
 
@@ -159,7 +159,6 @@ def test_against_the_reference_node():
     if not pyoracle.have_refmap():
         pytest.skip("the reference node library is not built")
     from densesurfelmapping_b200 import capi
-    from test_refmap import CAM as RCAM, poststep_frames
     m = pyoracle.RefMap(RCAM)
     c = capi.Context(RCAM, max_batch=2, max_local_surfels=100000)
     pool = np.zeros(0, SURFEL_DTYPE)

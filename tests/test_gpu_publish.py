@@ -3,8 +3,6 @@
 The snapshot equals the synchronous readers (dsm_pool_export_cloud, dsm_inactive_export_cloud) byte for byte at its
 position in the stream; inactive_changed_from and the number of forwarded chunks equal the chunk rule restated in
 oracle/pyoracle_publish.py; the error contract; and dsm::SurfelMapNode::published_clouds (tests/cpp/publish_main.cpp)."""
-import os
-import subprocess
 
 import numpy as np
 import pytest
@@ -12,65 +10,12 @@ import pytest
 import pyoracle_publish
 from densesurfelmapping_b200 import capi, synth
 from densesurfelmapping_b200.elements import POINT_DTYPE, SURFEL_DTYPE
-from test_gpu_window_stream import CAM, T, frames, needs_window_oracle, new_ctx, node_lists, windowed
-from test_surfel_node import Reader, Script, drive
+from node_drive import node_script, run_driver
+from resident_map import (
+    Mirror, STORE, T, needs_window_oracle, new_ctx, node_lists, simple_lists, snapshot_equals_readers, warp, windowed)
+from util import CAM
 
 pytestmark = pytest.mark.gpu
-
-STORE = 1 << 18
-
-
-def warp(k=1):
-    ang = np.deg2rad(1.5 * k)
-    Wm = np.eye(4)
-    Wm[:3, :3] = [[np.cos(ang), -np.sin(ang), 0], [np.sin(ang), np.cos(ang), 0], [0, 0, 1]]
-    Wm[:3, 3] = [0.1 * k, -0.2, 0.05]
-    return Wm
-
-
-def simple_lists():
-    """(reference, retire, reactivate) per frame without the reference node: a keyframe every other frame, a window of
-    two keyframes; keyframe 0 comes back at frame 9, leaves at 11, comes back with keyframe 1 at 13, and frame 14
-    retires three keyframes at once."""
-    out = []
-    for t in range(T):
-        ref = t // 2
-        rem = [ref - 2] if t % 2 == 0 and ref >= 2 else []
-        add = []
-        if t == 9:
-            add = [0]
-        if t == 11:
-            rem = [0]
-        if t == 13:
-            add = [0, 1]
-        if t == 14:
-            rem = [5, 0, 1]
-        out.append((ref, rem, add))
-    return tuple(out)
-
-
-class Mirror:
-    """The host's view across snapshots: the model's shadow and the previous size."""
-
-    def __init__(self, cap=STORE):
-        self.shadow, self.prev = np.zeros((cap, 4), np.float32), 0
-
-    def check(self, ctx, inactive, changed_from, what):
-        pts = inactive.view(np.float32).reshape(-1, 4)
-        chunks, want, self.shadow = pyoracle_publish.mirror_step(self.shadow, self.prev, pts)
-        assert changed_from == want, f"{what}: inactive_changed_from {changed_from}, the clouds first differ at {want}"
-        assert ctx.publish_chunks() == len(chunks), f"{what}: forwarded chunks"
-        self.prev = len(pts)
-        return chunks
-
-
-def snapshot_equals_readers(ctx, mirror, what, min_update_times=5):
-    ctx.publish_enqueue(min_update_times)
-    active, inactive, cf = ctx.publish_wait()
-    assert active.tobytes() == ctx.pool_export_cloud(min_update_times).tobytes(), f"{what}: active cloud"
-    assert inactive.tobytes() == ctx.inactive_export_cloud().tobytes(), f"{what}: inactive cloud"
-    mirror.check(ctx, inactive, cf, what)
-    return active, inactive, cf
 
 
 def run_drive(lists, chunk):
@@ -306,28 +251,11 @@ def test_publisher_that_never_synchronises_past_the_capacity():
 
 
 # ---- the node ----
-def run_publish_main(tmp, cam, script, drift_free_poses, publish):
-    from test_cpp_adapter import build_adapter
-    exe = build_adapter("publish_main")
-    fin, fout = os.path.join(tmp, f"script{publish}.bin"), os.path.join(tmp, f"out{publish}.bin")
-    with open(fin, "wb") as f:
-        f.write(bytes(script.b))
-    args = [exe, str(cam.width), str(cam.height)] + [repr(float(v)) for v in (cam.fx, cam.fy, cam.cx, cam.cy, cam.far, cam.near)]
-    args += [str(drift_free_poses), "0", str(1 << 20), str(1 << 21), str(publish), fin, fout]
-    r = subprocess.run(args, capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr
-    return Reader(open(fout, "rb").read())
-
-
 @pytest.mark.parametrize("drift_free_poses", [1, 2])
 def test_node_publishes_what_its_readers_return(tmp_path, drift_free_poses):
     cam, n = synth.KITTI, 30
-    msgs = drive(n)
-    sc = Script()
-    for t, (stamp, is_kf, ref, p7, path, loops) in enumerate(msgs):
-        sc.orb(stamp, is_kf, ref, p7, path, loops)
-        sc.images(stamp, *synth.make_frame(cam, 3000 + t, synth.pose_stream(t)))
-    r = run_publish_main(str(tmp_path), cam, sc, drift_free_poses, 1)
+    sc = node_script(cam, n)
+    r = run_driver("publish_main", str(tmp_path), cam, sc, [drift_free_poses, 0, 1 << 20, 1 << 21, 1], tag=1)
     prev, warped = np.zeros(0, POINT_DTYPE), 0
     for t in range(n):
         rc, cf = r.i(), r.i()
@@ -343,6 +271,6 @@ def test_node_publishes_what_its_readers_return(tmp_path, drift_free_poses):
         prev = inactive.copy()
     end = (r.lst(SURFEL_DTYPE).tobytes(), r.lst(POINT_DTYPE).tobytes())
     assert r.o == len(r.raw) and len(prev) > 0 and warped > 0
-    q = run_publish_main(str(tmp_path), cam, sc, drift_free_poses, 0)
+    q = run_driver("publish_main", str(tmp_path), cam, sc, [drift_free_poses, 0, 1 << 20, 1 << 21, 0], tag=0)
     assert (q.lst(SURFEL_DTYPE).tobytes(), q.lst(POINT_DTYPE).tobytes()) == end, "publishing perturbed the map"
     assert q.o == len(q.raw)

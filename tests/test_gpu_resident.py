@@ -6,35 +6,9 @@ import pytest
 import pyoracle
 from densesurfelmapping_b200 import synth
 from densesurfelmapping_b200.elements import SURFEL_DTYPE
-from util import check_surfels, oracle_for
+from util import check_surfels, match_as_sets, oracle_for
 
 pytestmark = pytest.mark.gpu
-
-
-def match_as_sets(got, want, tol=1e-4):
-    """Pools are equal as sets: same size, and a one-to-one nearest-neighbour matching within tolerance."""
-    assert len(got) == len(want), f"pool size {len(got)} != {len(want)}"
-    if len(got) == 0:
-        return
-    key = lambda a: np.lexsort((a["pz"], a["py"], a["px"], a["last_update"], a["update_times"]))
-    g, w = got[key(got)], want[key(want)]
-    # lexsort on floats can differ in the last bits; repair by nearest neighbour inside equal-integer groups
-    pg = np.stack([g["px"], g["py"], g["pz"]], -1).astype(np.float64)
-    pw = np.stack([w["px"], w["py"], w["pz"]], -1).astype(np.float64)
-    bad = np.nonzero(np.linalg.norm(pg - pw, axis=1) > tol * np.maximum(np.linalg.norm(pw, axis=1), 1.0))[0]
-    if len(bad):
-        used = set()
-        for i in bad:
-            dist = np.linalg.norm(pw[bad] - pg[i], axis=1)
-            j = int(np.argmin(dist))
-            assert dist[j] <= tol * max(np.linalg.norm(pg[i]), 1.0) and j not in used, f"surfel {i} has no partner"
-            used.add(j)
-            g[i], w_i = g[i], w[bad[j]]
-            check_surfels(g[i:i + 1], np.array([w_i]), "set member")
-        ok = np.setdiff1d(np.arange(len(g)), bad)
-        check_surfels(g[ok], w[ok], "pool (sorted)")
-    else:
-        check_surfels(g, w, "pool (sorted)")
 
 
 def test_resident_stream_matches_reference_flow():

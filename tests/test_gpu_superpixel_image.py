@@ -16,8 +16,9 @@ import pyoracle
 import pyoracle_show
 from densesurfelmapping_b200 import capi, synth
 from densesurfelmapping_b200.elements import SURFEL_DTYPE
-from test_cpp_adapter import build_adapter
-from test_refmap import CAM
+from node_drive import build_adapter
+from util import CAM
+
 
 pytestmark = pytest.mark.gpu
 

@@ -13,7 +13,7 @@ import pytest
 import pyoracle
 import pyoracle_window
 from densesurfelmapping_b200 import capi, synth
-from test_surfel_node import Script, drive, read_dumps, run_node
+from node_drive import Script, drive, read_dumps, run_node
 
 pytestmark = pytest.mark.gpu
 needs_b200_node = pytest.mark.skipif(not pyoracle_window.have_refmap_window(b200=True),

@@ -3,7 +3,6 @@
 Checked against (1) the per-call sequence dsm_inactive_retire / dsm_inactive_reactivate / dsm_fuse_frame_resident, byte
 for byte after every call; (2) dsm_fuse_stream_resident when every list is empty; (3) the reference node itself over the
 product (libdsm_refmap_window_b200.so), with the fuse poses and window lists the node used; plus the error contract."""
-import functools
 import os
 import struct
 import subprocess
@@ -13,60 +12,13 @@ import pytest
 
 import pyoracle
 import pyoracle_window
-from densesurfelmapping_b200 import capi, synth
+from densesurfelmapping_b200 import capi
 from densesurfelmapping_b200.elements import POINT_DTYPE, SURFEL_DTYPE
+from node_drive import build_adapter
+from resident_map import T, frames, needs_window_oracle, new_ctx, node_lists, schedule, windowed
+from util import CAM
 
 pytestmark = pytest.mark.gpu
-
-CAM = synth.Camera(320, 240, 262.5, 262.5, 159.5, 119.5, 0.5, 30.0)
-T = 16
-needs_window_oracle = pytest.mark.skipif(not pyoracle_window.have_refmap_window(),
-                                         reason="oracle/_ref/libdsm_refmap_window.so not built (needs the reference sources)")
-
-
-def schedule(t):
-    """(is_keyframe, reference, loops) of frame t: a keyframe every other frame, a loop edge 4 <-> 0 at frame 9, the
-    reference jumping back to keyframe 1 at frames 12-13 (several keyframes leave at once, old ones return)."""
-    return t % 2 == 0, (1 if t in (12, 13) else "new"), ([4, 0] if t == 9 else [])
-
-
-@functools.lru_cache(maxsize=None)
-def frames():
-    out = []
-    for t in range(T):
-        pose = synth.pose_stream(t)
-        gray, depth = synth.make_frame(CAM, 2000 + t, pose)
-        out.append((pose, gray, depth))
-    return out
-
-
-@functools.lru_cache(maxsize=None)
-def node_lists(drift_free_poses=2):
-    """(reference index, poses_to_remove, poses_to_add) per frame, from the reference node's own get_add_remove_poses
-    and move_add_surfels on the pose graph of the drive."""
-    m = pyoracle_window.RefMapWindow(CAM, drift_free_poses=drift_free_poses)
-    path, last_kf, out = [], 0, []
-    for t in range(T):
-        is_kf, ref, loops = schedule(t)
-        p7 = pyoracle.pose_to_ros7(synth.pose_stream(t))
-        root = (last_kf if t else 0) if ref == "new" else ref
-        m.frame(100.0 + 0.1 * t, None, None, p7, is_kf or t == 0, root, path7=np.array(path).reshape(-1, 7), loops=loops)
-        if is_kf or t == 0:
-            path.append(p7)
-            last_kf = m.num_poses() - 1
-        rem, add = m.window_lists(root)
-        m.move_add_surfels(root)
-        out.append((root, rem, add))
-    m.close()
-    return tuple(out)
-
-
-def new_ctx(max_batch=16, cap=1 << 18, store=1 << 18):
-    ctx = capi.Context(CAM, max_batch=max_batch, max_local_surfels=cap)
-    ctx.pool_upload(np.zeros(0, SURFEL_DTYPE))
-    if store:
-        ctx.inactive_reserve(store)
-    return ctx
 
 
 def per_call(ctx, t0, t1, lists):
@@ -81,15 +33,6 @@ def per_call(ctx, t0, t1, lists):
         pose, gray, depth = frames()[t]
         cnt.append(ctx.fuse_frame_resident(ref, gray, depth, pose, want_count=True))
     return np.array(cnt, np.int32)
-
-
-def windowed(ctx, t0, t1, lists, want_counts=True, empty=False):
-    fr = frames()[t0:t1]
-    ref = [lists[t][0] for t in range(t0, t1)]
-    rem = [[] if empty else lists[t][1] for t in range(t0, t1)]
-    add = [[] if empty else lists[t][2] for t in range(t0, t1)]
-    return ctx.fuse_stream_window(ref, np.stack([f[1] for f in fr]), np.stack([f[2] for f in fr]),
-                                  np.stack([capi.pose16(f[0]) for f in fr]), rem, add, want_counts=want_counts)
 
 
 def state(ctx, kfs=range(T)):
@@ -314,7 +257,6 @@ def test_product_equals_the_reference_node(chunk):
 def test_cpp_caller_of_the_windowed_fuse_map(tmp_path):
     """tests/cpp/window_main.cpp: dsm::ResidentSurfelPool::fuse_map with the two lists, one frame per call, never
     synchronising; the map it reads back at the end equals the Python binding's chunk-of-1 run."""
-    from test_cpp_adapter import build_adapter
     exe = build_adapter("window_main")
     lists = node_lists()
     fin, fout = str(tmp_path / "in.bin"), str(tmp_path / "out.bin")

@@ -14,12 +14,8 @@ import pytest
 import pyoracle
 import pyoracle_clouds
 from densesurfelmapping_b200 import synth
-from test_cpp_adapter import build_adapter
-from test_oracle import GOLD, crc
-from test_refmap import CAM
-
-needs_refmap_clouds = pytest.mark.skipif(not pyoracle_clouds.have_refmap_clouds(),
-                                         reason="oracle/_ref/libdsm_refmap_clouds.so not built (needs the reference sources)")
+from node_drive import build_adapter
+from util import CAM, GOLD, canon_points, crc, needs_refmap_clouds, neighbor_replay
 
 
 def raw_cases():
@@ -36,12 +32,6 @@ def raw_cases():
     return {"qvga_holes": (CAM, g0, d0, p0),
             "kitti": (synth.KITTI, g1, d1, p1),
             "qvga_quaternion_qw_negative": (CAM, g2, d2, np.array([1.5, -0.25, 3.0, 0.3, -0.2, 0.1, -0.9]))}
-
-
-def canon_points(p):
-    p = np.array(p, np.float32, copy=True)
-    p[np.isnan(p)] = np.float32(np.nan)
-    return p.tobytes()
 
 
 def golden_raw():
@@ -63,28 +53,6 @@ def test_raw_cloud_restatement_is_pinned(case):
         m = pyoracle_clouds.RefMapClouds(cam)
         assert m.publish_raw(gray, depth, p7).tobytes() == got.tobytes()
         m.close()
-
-
-def neighbor_replay(m, steps=8):
-    """A controlled drive of the reference node with drift_free_poses=1: one keyframe per step, each referencing the
-    previous one, a loop edge 4-0 at step 5 (pose 0 joins the neighbourhood of pose 4) and a return to pose 0 at step 7
-    (pose 0 re-enters the drift-free window).  Yields, per step, after the pose feed: the pool before move_add_surfels,
-    the window before and after it, the BFS list of publish_neighbor_pointcloud and what that publisher sent; then
-    fuses the step's frame (fuse_map) for the next step."""
-    path = []
-    for t in range(steps):
-        pose = synth.pose_stream(t)
-        gray, depth = synth.make_frame(CAM, 1000 + t, pose)
-        p7 = pyoracle.pose_to_ros7(pose)
-        ref = 0 if t == steps - 1 else max(t - 1, 0)
-        m.frame(100.0 + 0.1 * t, None, None, p7, True, ref, path7=np.array(path).reshape(-1, 7), loops=[4, 0] if t == 5 else ())
-        path.append(p7)
-        pool, window_before = m.local(), m.local_pose_indexs()
-        m.move_add_surfels(ref)
-        m.publish_clouds(ref)
-        yield dict(t=t, ref=ref, pool=pool, window_before=window_before, window=m.local_pose_indexs(),
-                   bfs=m.driftfree_poses(ref, 2), published=m.published("neighbor_pointcloud"))
-        m.fuse_map(gray, depth, pose, ref)
 
 
 def find_slice(cloud, part):

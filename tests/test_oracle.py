@@ -2,7 +2,6 @@
 source, and the restatement against the serialised reference build when that library is present."""
 import json
 import os
-import zlib
 
 import numpy as np
 import pytest
@@ -10,25 +9,7 @@ import pytest
 import pyoracle
 from densesurfelmapping_b200 import synth
 from densesurfelmapping_b200.elements import SEED_DTYPE, SURFEL_DTYPE
-from util import bits_equal_nan
-
-GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
-
-
-def canon(a):
-    """field-by-field bytes (struct padding excluded) with every NaN canonicalised: NaN payload/sign
-    and padding bytes are not part of the contract."""
-    parts = []
-    for f in a.dtype.names:
-        v = np.ascontiguousarray(a[f]).copy()
-        if v.dtype.kind == "f":
-            v[np.isnan(v)] = np.float32(np.nan)
-        parts.append(v.tobytes())
-    return b"".join(parts)
-
-
-def crc(x):
-    return zlib.crc32(x if isinstance(x, (bytes, bytearray)) else np.ascontiguousarray(x).tobytes()) & 0xFFFFFFFF
+from util import GOLD, bits_equal_nan, canon, crc
 
 
 def assert_records_equal(a, b, what):

@@ -9,27 +9,7 @@ import pytest
 import pyoracle
 from densesurfelmapping_b200 import capi, synth
 from densesurfelmapping_b200.elements import POINT_DTYPE, SURFEL_DTYPE
-
-
-def random_surfels(n, seed=0):
-    rng = np.random.RandomState(seed)
-    s = np.zeros(n, SURFEL_DTYPE)
-    for f in ("px", "py", "pz"):
-        s[f] = rng.uniform(-40, 40, n)
-    nr = rng.normal(size=(n, 3))
-    nr /= np.linalg.norm(nr, axis=1, keepdims=True)
-    s["nx"], s["ny"], s["nz"] = nr[:, 0], nr[:, 1], nr[:, 2]
-    s["size"] = rng.uniform(0.01, 0.6, n)
-    s["color"] = rng.randint(0, 256, n) + rng.choice([0.0, 0.25, 0.75], n)  # averaged intensities are not integers
-    s["weight"] = rng.uniform(0.01, 30, n)
-    s["update_times"] = rng.randint(0, 12, n)
-    s["last_update"] = rng.randint(0, 9, n)
-    if n >= 4:
-        s["nx"][0], s["ny"][0], s["nz"][0] = 0, 0, 1    # x_dir = 0: normalize() must leave it alone, not make NaN
-        s["nx"][1], s["ny"][1], s["nz"][1] = 1, 0, 0
-        s["px"][2], s["py"][2], s["pz"][2] = 1e-7, -123456.78, 3.0e5  # exponent formats in %g
-        s["size"][3] = 0
-    return s
+from util import random_surfels
 
 
 def test_mesh_vertices_match_push_a_surfel():

@@ -16,15 +16,12 @@ import pytest
 import pyoracle
 from densesurfelmapping_b200 import capi, synth
 from densesurfelmapping_b200.elements import SURFEL_DTYPE
-from test_oracle import GOLD, canon, crc
-from test_output_formats import random_surfels
-from util import oracle_for
+from util import CAM, GOLD, canon, crc, match_as_sets, oracle_for, poststep_frames, random_surfels
+
 
 # the reference's SurfelMap is built into oracle/_ref/ only where the reference sources are; the pinned members below are
 # also checked against CRC32s minted from it (tests/golden/reference_checksums.json), the other tests need it
 needs_refmap = pytest.mark.skipif(not pyoracle.have_refmap(), reason="oracle/_ref/libdsm_refmap.so not built (needs the reference sources)")
-
-CAM = synth.Camera(320, 240, 262.5, 262.5, 159.5, 119.5, 0.5, 30.0)  # quarter-VGA keeps the CPU suite short
 
 
 def drive(m, n_frames, keyframe_every=1, seed0=1000, loops_at=None):
@@ -44,13 +41,6 @@ def drive(m, n_frames, keyframe_every=1, seed0=1000, loops_at=None):
 
 def golden_map(key):
     return json.load(open(os.path.join(GOLD, "reference_checksums.json")))["map"][key]
-
-
-def poststep_frames():
-    for t in range(4):
-        pose = synth.pose_stream(t)
-        gray, depth = synth.make_frame(CAM, 50 + t, pose)
-        yield t + (7 if t == 3 else 0), gray, depth, pose  # the jump kills unstable surfels: slot recycling AND swap-with-back both run
 
 
 def warp_case():
@@ -275,7 +265,6 @@ def test_three_line_patch_compiles_against_the_reference_source():
 def test_reference_node_over_the_product_matches_the_reference_node():
     """The drop-in claim end to end: the same 6-frame drive through the reference's SurfelMap with its own CPU
     FusionFunctions and with the product library underneath.  Maps agree as sets within the surfel tolerance."""
-    from test_gpu_resident import match_as_sets
     if not pyoracle.have_refmap(b200=True):
         pytest.skip("libdsm_refmap_b200.so not built")
     a, b = pyoracle.RefMap(CAM, drift_free_poses=2), pyoracle.RefMap(CAM, drift_free_poses=2, b200=True)
@@ -299,7 +288,6 @@ def test_device_resident_map_tracks_the_reference_node():
     the product with local_surfels AND attached_surfels resident on the device, replaying the node's own window
     decisions (which keyframes leave / re-enter).  After every frame the device's local pool and inactive store
     equal the node's local_surfels / inactive_pointcloud as sets, within the surfel tolerance."""
-    from test_gpu_resident import match_as_sets
     ref = pyoracle.RefMap(CAM, drift_free_poses=2)
     ctx = capi.Context(CAM, max_batch=2, max_local_surfels=60000)
     ctx.pool_upload(np.zeros(0, SURFEL_DTYPE))

@@ -15,9 +15,8 @@ import pyoracle
 import pyoracle_show
 from densesurfelmapping_b200 import synth
 from densesurfelmapping_b200.elements import SEED_DTYPE, num_seeds
-from test_cpp_adapter import build_adapter
-from test_oracle import GOLD, crc
-from test_refmap import CAM
+from node_drive import build_adapter
+from util import CAM, GOLD, crc
 
 needs_ref_show = pytest.mark.skipif(not pyoracle_show.have_ref_show(),
                                     reason="oracle/_ref/libdsm_ref_show.so not built (needs the reference sources)")

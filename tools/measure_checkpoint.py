@@ -15,7 +15,6 @@ Usage: python tools/measure_checkpoint.py [--reps 5] [--dir DIR] [--out DIR]"""
 import argparse
 import json
 import os
-import subprocess
 import sys
 import tempfile
 import time
@@ -24,40 +23,7 @@ import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-from densesurfelmapping_b200 import capi, synth  # noqa: E402
-from densesurfelmapping_b200.elements import SURFEL_DTYPE  # noqa: E402
-
-SIZES = {"node": (81 << 10, 47 << 10, 80), "large": (1 << 20, 4 << 20, 1024)}
-
-
-def card():
-    r = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True)
-    if r.returncode != 0:
-        raise RuntimeError("nvidia-smi failed: no GPU to measure on")
-    name, power = [x.strip() for x in r.stdout.splitlines()[0].split(",")]
-    return name, power
-
-
-def surfels(rng, n):
-    s = np.zeros(n, SURFEL_DTYPE)
-    for f in ("px", "py", "pz", "nx", "ny", "nz", "size", "color", "weight"):
-        s[f] = rng.standard_normal(n).astype(np.float32)
-    s["update_times"] = rng.integers(1, 20, n)
-    return s
-
-
-def make_map(n_pool, n_store, n_seg, seed=7):
-    rng = np.random.default_rng(seed)
-    ctx = capi.Context(synth.KITTI, max_batch=2, max_local_surfels=n_pool)
-    ctx.pool_upload(surfels(rng, n_pool))
-    ctx.inactive_reserve(n_store)
-    store = surfels(rng, n_store)
-    cnt = np.full(n_seg, n_store // n_seg, np.int32)
-    cnt[-1] += n_store - cnt.sum()
-    ofs = np.concatenate([[0], np.cumsum(cnt)[:-1]]).astype(np.int32)
-    store["last_update"] = np.repeat(np.arange(n_seg, dtype=np.int32), cnt)
-    ctx.inactive_load(store, np.stack([np.arange(n_seg, dtype=np.int32), ofs, cnt], 1))
-    return ctx
+from measure_drive import SIZES, card, make_map  # noqa: E402
 
 
 def measure(name, reps, d):

@@ -17,8 +17,6 @@ Usage: python tools/measure_checkpoint_async.py [--reps 5] [--rounds 3] [--out D
 import argparse
 import json
 import os
-import struct
-import subprocess
 import sys
 import tempfile
 import time
@@ -29,28 +27,10 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tools"))
 sys.path.insert(0, os.path.join(ROOT, "tests"))
-from densesurfelmapping_b200 import synth  # noqa: E402
-from measure_checkpoint import SIZES, card, make_map  # noqa: E402
-from measure_node import CAM, K, messages  # noqa: E402
+from measure_drive import SIZES, build_harness, card, images, kernel_us, make_map, messages, run_harness, write_drive  # noqa: E402
 
 HBM_TBPS = 3.35
 DRAIN_CTAS = (4, 8, 16, 32, 66, 132)
-
-
-def kernel_us(fn, names):
-    """Per-launch device time in us of each kernel in `names` over what fn() enqueues."""
-    import torch
-    from torch.profiler import ProfilerActivity, profile
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        fn()
-        torch.cuda.synchronize()
-    out = {n: [] for n in names}
-    for e in prof.events():
-        for n in names:
-            if n in e.name:
-                t = getattr(e, "device_time", None)
-                out[n].append(float(t if t is not None else e.cuda_time))
-    return out
 
 
 def live_bytes(n_pool, n_store, n_seg):
@@ -105,31 +85,13 @@ def measure_size(name, reps, d):
 
 
 def node_drive(tmp, rounds, frames, every=20):
-    exe = os.path.join(tmp, "measure_checkpoint_async")
-    pkg = os.path.join(ROOT, "densesurfelmapping_b200")
-    subprocess.run(["g++", "-std=c++11", "-O2", "-I", os.path.join(ROOT, "include"), os.path.join(ROOT, "tools", "measure_checkpoint_async.cpp"),
-                    "-o", exe, "-L", pkg, "-ldsm_b200", f"-Wl,-rpath,{pkg}"], check=True)
-    imgs = [synth.make_frame(CAM, 5000 + k, synth.pose_stream(k)) for k in range(K)]
-    msgs = messages(frames)
-    ff, fs = os.path.join(tmp, "frames.bin"), os.path.join(tmp, "script.bin")
-    with open(ff, "wb") as f:
-        f.write(struct.pack("<i", K))
-        for g, d in imgs:
-            f.write(g.tobytes() + d.tobytes())
-    with open(fs, "wb") as f:
-        f.write(struct.pack("<i", len(msgs)))
-        for t, (stamp, is_kf, ref, p7, path) in enumerate(msgs):
-            f.write(struct.pack("<diii", stamp, int(is_kf), ref, t % K) + p7.tobytes())
-            f.write(struct.pack("<i", len(path)) + np.asarray(path, np.float64).tobytes() + struct.pack("<ii", 0, 0))
-    args = [exe, str(CAM.width), str(CAM.height)] + [repr(float(v)) for v in (CAM.fx, CAM.fy, CAM.cx, CAM.cy, CAM.far, CAM.near)]
+    exe = build_harness(tmp, "measure_checkpoint_async")
+    ff, fs = write_drive(tmp, images(), messages(frames))
     out = {"none": [], "save_state_async": [], "save_state": [], "save_state_async_waiting": []}
     last, skipped, wait_ms, call_ms = {}, {k: [] for k in out}, {k: [] for k in out}, {k: [] for k in out}
     for _ in range(rounds):
         for mode, key in enumerate(out):
-            r = subprocess.run(args + ["10", ff, fs, str(mode), str(every), tmp], capture_output=True, text=True)
-            if r.returncode != 0:
-                raise RuntimeError(f"measure_checkpoint_async exited {r.returncode}: {r.stderr[-2000:]}")
-            last[key] = json.loads(r.stdout.strip().splitlines()[-1])
+            last[key] = run_harness(exe, ff, fs, [mode, every, tmp])
             out[key].append(last[key]["ms_per_frame"])
             skipped[key].append(last[key]["skipped"])
             wait_ms[key].append(last[key]["wait_ms"])

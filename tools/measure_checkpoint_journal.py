@@ -20,7 +20,6 @@ import argparse
 import json
 import os
 import struct
-import subprocess
 import sys
 import tempfile
 import time
@@ -32,9 +31,7 @@ sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tools"))
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 from densesurfelmapping_b200 import capi, synth  # noqa: E402
-from measure_checkpoint import card, surfels  # noqa: E402
-from measure_checkpoint_async import kernel_us  # noqa: E402
-from measure_node import CAM, K, messages  # noqa: E402
+from measure_drive import build_harness, card, images, kernel_us, messages, run_harness, surfels, write_drive  # noqa: E402
 
 N_POOL, N_STORE, N_SEG, POOL_KEYS = 1 << 20, 4 << 20, 1024, 64
 
@@ -121,31 +118,13 @@ def measure_pattern(pattern, reps, d):
 
 
 def node_drive(tmp, rounds, frames, every=20):
-    exe = os.path.join(tmp, "measure_checkpoint_journal")
-    pkg = os.path.join(ROOT, "densesurfelmapping_b200")
-    subprocess.run(["g++", "-std=c++11", "-O2", "-I", os.path.join(ROOT, "include"), os.path.join(ROOT, "tools", "measure_checkpoint_journal.cpp"),
-                    "-o", exe, "-L", pkg, "-ldsm_b200", f"-Wl,-rpath,{pkg}"], check=True)
-    imgs = [synth.make_frame(CAM, 5000 + k, synth.pose_stream(k)) for k in range(K)]
-    msgs = messages(frames)
-    ff, fs = os.path.join(tmp, "frames.bin"), os.path.join(tmp, "script.bin")
-    with open(ff, "wb") as f:
-        f.write(struct.pack("<i", K))
-        for g, dd in imgs:
-            f.write(g.tobytes() + dd.tobytes())
-    with open(fs, "wb") as f:
-        f.write(struct.pack("<i", len(msgs)))
-        for t, (stamp, is_kf, ref, p7, path) in enumerate(msgs):
-            f.write(struct.pack("<diii", stamp, int(is_kf), ref, t % K) + p7.tobytes())
-            f.write(struct.pack("<i", len(path)) + np.asarray(path, np.float64).tobytes() + struct.pack("<ii", 0, 0))
-    args = [exe, str(CAM.width), str(CAM.height)] + [repr(float(v)) for v in (CAM.fx, CAM.fy, CAM.cx, CAM.cy, CAM.far, CAM.near)]
+    exe = build_harness(tmp, "measure_checkpoint_journal")
+    ff, fs = write_drive(tmp, images(), messages(frames))
     out = {"none": [], "save_state_async": [], "save_state_incremental": []}
     last = {}
     for _ in range(rounds):
         for mode, key in enumerate(out):
-            r = subprocess.run(args + ["10", ff, fs, str(mode), str(every), tmp], capture_output=True, text=True)
-            if r.returncode != 0:
-                raise RuntimeError(f"measure_checkpoint_journal exited {r.returncode}: {r.stderr[-2000:]}")
-            last[key] = json.loads(r.stdout.strip().splitlines()[-1])
+            last[key] = run_harness(exe, ff, fs, [mode, every, tmp])
             out[key].append(last[key]["ms_per_frame"])
     return {"frames": frames, "every": every, "ms_per_frame": out,
             "saves": {k: {"bytes": v["bytes"], "base": v["base"], "skipped": v["skipped"]} for k, v in last.items()}}

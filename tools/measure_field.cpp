@@ -7,55 +7,22 @@
 //         f: distance_field() of frame t-1 at the start of frame t's callbacks (the last one after the drive)
 //         g: distance_field() right after every frame's fuse
 // Prints one JSON object; "occupied" is the sum of n_occupied over the fields handed out.
-#include <chrono>
-#include <cstdio>
-#include <cstdlib>
-#include <vector>
-#include "dsm_surfel_node.hpp"
-
-typedef std::chrono::steady_clock clk;
-static double ms(clk::time_point a, clk::time_point b) { return std::chrono::duration<double, std::milli>(b - a).count(); }
+#include "measure_drive.hpp"
 
 int main(int argc, char **argv)
 {
     if (argc != 17) return 2;
-    const int W = atoi(argv[1]), H = atoi(argv[2]);
+    const int W = atoi(argv[1]);
     const char mode = argv[12][0];
     const float voxel = (float)atof(argv[13]);
     const int nx = atoi(argv[14]), ny = atoi(argv[15]), nz = atoi(argv[16]);
     if (mode != 'a' && mode != 'f' && mode != 'g') return 2;
-    FILE *ff = fopen(argv[10], "rb"), *fs = fopen(argv[11], "rb");
-    if (!ff || !fs) return 5;
-    int K = 0, T = 0;
-    if (fread(&K, 4, 1, ff) != 1 || fread(&T, 4, 1, fs) != 1) return 5;
-    std::vector<std::vector<uint8_t> > gray((size_t)K, std::vector<uint8_t>((size_t)W * H));
-    std::vector<std::vector<float> > depth((size_t)K, std::vector<float>((size_t)W * H));
-    for (int k = 0; k < K; k++)
-        if (fread(gray[k].data(), 1, gray[k].size(), ff) != gray[k].size() || fread(depth[k].data(), 4, depth[k].size(), ff) != depth[k].size())
-            return 5;
-    dsm::SurfelMapNode node(W, H, atof(argv[3]), atof(argv[4]), atof(argv[5]), atof(argv[6]), atof(argv[7]), atof(argv[8]), atoi(argv[9]), 0);
-    if (node.last_error() != DSM_OK) return node.last_error() == DSM_E_NODEVICE ? 3 : 4;
+    Drive d;
+    if (!d.load(argv)) return 5;
+    const int T = (int)d.msgs.size();
+    DriveNode node(argv);
+    if (const int e = node.setup_code()) return e;
     if (mode != 'a' && node.enable_distance_field(voxel, nx, ny, nz) != DSM_OK) return 4;
-    // the script is read before the clock starts
-    struct Msg
-    {
-        double stamp, pose[7];
-        int kf, ref, k;
-        std::vector<double> path;
-    };
-    std::vector<Msg> msgs((size_t)T);
-    for (int t = 0; t < T; t++)
-    {
-        Msg &m = msgs[(size_t)t];
-        int n_path = 0, n_loops = 0, publish = 0;
-        if (fread(&m.stamp, 8, 1, fs) != 1 || fread(&m.kf, 4, 1, fs) != 1 || fread(&m.ref, 4, 1, fs) != 1 || fread(&m.k, 4, 1, fs) != 1 ||
-            fread(m.pose, 8, 7, fs) != 7 || fread(&n_path, 4, 1, fs) != 1)
-            return 5;
-        m.path.resize((size_t)7 * n_path + 1);
-        if (fread(m.path.data(), 8, (size_t)7 * n_path, fs) != (size_t)7 * n_path || fread(&n_loops, 4, 1, fs) != 1 || n_loops != 0 ||
-            fread(&publish, 4, 1, fs) != 1)
-            return 5;
-    }
     const float *dist = nullptr;
     int32_t origin[3];
     int n_occ = 0, rc = DSM_OK, fields = 0;
@@ -64,15 +31,14 @@ int main(int argc, char **argv)
     const clk::time_point t0 = clk::now();
     for (int t = 0; t < T && rc == DSM_OK; t++)
     {
-        const Msg &m = msgs[(size_t)t];
+        const DriveMsg &m = d.msgs[(size_t)t];
         if (mode == 'f' && t > 0)
         {
             rc = node.distance_field(dist, origin, n_occ);
             occupied += n_occ, fields++;
         }
-        if (rc == DSM_OK) rc = node.orb_results_input(m.stamp, nullptr, 0, m.path.data(), (int)(m.path.size() / 7), m.pose, m.kf != 0, m.ref);
-        if (rc == DSM_OK) rc = node.image_input(m.stamp, gray[(size_t)m.k].data(), (size_t)W);
-        if (rc == DSM_OK) rc = node.depth_input(m.stamp, depth[(size_t)m.k].data(), (size_t)W * 4);
+        if (rc == DSM_OK) rc = m.orb(node);
+        if (rc == DSM_OK) rc = d.images(node, m, W);
         if (rc != DSM_OK) break;
         if (mode == 'g')
         {

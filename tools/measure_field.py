@@ -16,7 +16,6 @@ import argparse
 import ctypes
 import json
 import os
-import subprocess
 import sys
 import tempfile
 import time
@@ -28,38 +27,22 @@ sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tools"))
 sys.path.insert(0, os.path.join(ROOT, "oracle"))
 from densesurfelmapping_b200.elements import SURFEL_DTYPE  # noqa: E402
-from measure_publish import CAM, SMALL, card, spread, write_drive  # noqa: E402
+from measure_drive import SMALL, build_harness, card, images, messages, run_harness, spread, write_drive  # noqa: E402
 
 HBM_BYTES_PER_S = 3.35e12   # H100 SXM data sheet
 VOXEL = 0.1
 KERNELS = {"mark": "k_field_mark", "rows": "k_field_rows", "y_pass": "k_field_lines<false>", "z_pass": "k_field_lines<true>"}
 
 
-def build_driver(tmp):
-    exe = os.path.join(tmp, "measure_field")
-    pkg = os.path.join(ROOT, "densesurfelmapping_b200")
-    subprocess.run(["g++", "-std=c++11", "-O2", "-I", os.path.join(ROOT, "include"), os.path.join(ROOT, "tools", "measure_field.cpp"),
-                    "-o", exe, "-L", pkg, "-ldsm_b200", f"-Wl,-rpath,{pkg}"], check=True)
-    return exe
-
-
-def run_mode(exe, ff, fs, mode, grid, voxel):
-    args = [exe, str(CAM.width), str(CAM.height)] + [repr(float(v)) for v in (CAM.fx, CAM.fy, CAM.cx, CAM.cy, CAM.far, CAM.near)]
-    r = subprocess.run(args + ["10", ff, fs, mode, repr(float(voxel))] + [str(n) for n in grid], capture_output=True, text=True)
-    if r.returncode != 0:
-        raise RuntimeError(f"measure_field mode {mode} exited {r.returncode}: {r.stderr[-2000:]}")
-    return json.loads(r.stdout.strip().splitlines()[-1])
-
-
 def node_drive(n_frames, rounds, grid, voxel):
     with tempfile.TemporaryDirectory() as tmp:
-        exe = build_driver(tmp)
-        ff, fs = write_drive(tmp, n_frames)
+        exe = build_harness(tmp, "measure_field")
+        ff, fs = write_drive(tmp, images(), messages(n_frames))
         times = {m: [] for m in "afg"}
         last = {}
         for _ in range(rounds):
             for m in "afg":
-                last[m] = run_mode(exe, ff, fs, m, grid, voxel)
+                last[m] = run_harness(exe, ff, fs, [m, voxel, *grid])
                 times[m].append(last[m]["ms_per_frame"])
     return {"frames": n_frames, "rounds": rounds, "grid": grid, "voxel": voxel, "store_surfels": last["a"]["store_surfels"],
             "pool_surfels": last["a"]["pool_surfels"], "mean_occupied_voxels": last["f"]["occupied"] / max(last["f"]["fields"], 1),

@@ -17,7 +17,6 @@ import argparse
 import ctypes
 import json
 import os
-import subprocess
 import sys
 import tempfile
 import time
@@ -30,7 +29,7 @@ sys.path.insert(0, os.path.join(ROOT, "tools"))
 sys.path.insert(0, os.path.join(ROOT, "oracle"))
 from densesurfelmapping_b200 import capi, synth  # noqa: E402
 from densesurfelmapping_b200.elements import SURFEL_DTYPE  # noqa: E402
-from measure_publish import CAM, card, spread, write_drive  # noqa: E402
+from measure_drive import build_harness, card, images, messages, run_harness, spread, write_drive  # noqa: E402
 import pyoracle_field_known  # noqa: E402
 
 VOXEL, MAX_RANGE, MAX_VIEWS = 0.2, 40.0, 256
@@ -73,32 +72,15 @@ def visits(views):
     return count[0]
 
 
-def build_driver(tmp):
-    exe = os.path.join(tmp, "measure_field_known")
-    pkg = os.path.join(ROOT, "densesurfelmapping_b200")
-    subprocess.run(["g++", "-std=c++11", "-O2", "-I", os.path.join(ROOT, "include"), os.path.join(ROOT, "tools", "measure_field_known.cpp"),
-                    "-o", exe, "-L", pkg, "-ldsm_b200", f"-Wl,-rpath,{pkg}"], check=True)
-    return exe
-
-
-def run_mode(exe, ff, fs, mode, grid):
-    args = [exe, str(CAM.width), str(CAM.height)] + [repr(float(v)) for v in (CAM.fx, CAM.fy, CAM.cx, CAM.cy, CAM.far, CAM.near)]
-    args += ["10", ff, fs, mode, repr(VOXEL)] + [str(n) for n in grid] + [str(MAX_VIEWS), repr(MAX_RANGE)]
-    r = subprocess.run(args, capture_output=True, text=True)
-    if r.returncode != 0:
-        raise RuntimeError(f"measure_field_known mode {mode} exited {r.returncode}: {r.stderr[-2000:]}")
-    return json.loads(r.stdout.strip().splitlines()[-1])
-
-
 def node_drive(n_frames, rounds, grid):
     with tempfile.TemporaryDirectory() as tmp:
-        exe = build_driver(tmp)
-        ff, fs = write_drive(tmp, n_frames)
+        exe = build_harness(tmp, "measure_field_known")
+        ff, fs = write_drive(tmp, images(), messages(n_frames))
         times = {m: [] for m in "pk"}
         last = {}
         for _ in range(rounds):
             for m in "pk":
-                last[m] = run_mode(exe, ff, fs, m, grid)
+                last[m] = run_harness(exe, ff, fs, [m, VOXEL, *grid, MAX_VIEWS, MAX_RANGE])
                 times[m].append(last[m]["ms_per_frame"])
     return {"frames": n_frames, "rounds": rounds, "grid": grid, "voxel": VOXEL, "views_at_end": last["k"]["views"],
             "free_per_field": last["k"]["free"] / max(last["k"]["fields"], 1), "ms_per_frame": {m: spread(times[m]) for m in "pk"}}

@@ -6,50 +6,27 @@
 //               int32 n_path, double path7[n_path][7], int32 n_loops, int32 pairs[2 n_loops], int32 publish }
 //   publish = 1: the frame also builds the active and inactive clouds, as the reference node publishes them per frame.
 // Prints one JSON object.
-#include <chrono>
-#include <cstdio>
-#include <cstdlib>
-#include <vector>
-#include "dsm_surfel_node.hpp"
-
-typedef std::chrono::steady_clock clk;
-static double ms(clk::time_point a, clk::time_point b) { return std::chrono::duration<double, std::milli>(b - a).count(); }
+#include "measure_drive.hpp"
 
 int main(int argc, char **argv)
 {
     if (argc != 12) return 2;
-    const int W = atoi(argv[1]), H = atoi(argv[2]);
-    FILE *ff = fopen(argv[10], "rb"), *fs = fopen(argv[11], "rb");
-    if (!ff || !fs) return 5;
-    int K = 0, T = 0;
-    if (fread(&K, 4, 1, ff) != 1 || fread(&T, 4, 1, fs) != 1) return 5;
-    std::vector<std::vector<uint8_t> > gray((size_t)K, std::vector<uint8_t>((size_t)W * H));
-    std::vector<std::vector<float> > depth((size_t)K, std::vector<float>((size_t)W * H));
-    for (int k = 0; k < K; k++)
-        if (fread(gray[k].data(), 1, gray[k].size(), ff) != gray[k].size() || fread(depth[k].data(), 4, depth[k].size(), ff) != depth[k].size())
-            return 5;
-    dsm::SurfelMapNode node(W, H, atof(argv[3]), atof(argv[4]), atof(argv[5]), atof(argv[6]), atof(argv[7]), atof(argv[8]), atoi(argv[9]), 0);
-    if (node.last_error() != DSM_OK) return node.last_error() == DSM_E_NODEVICE ? 3 : 4;
+    const int W = atoi(argv[1]);
+    Drive d;
+    if (!d.load(argv)) return 5;
+    const int T = (int)d.msgs.size();
+    DriveNode node(argv);
+    if (const int e = node.setup_code()) return e;
     std::vector<dsm_point_t> active, inactive;
     double frames_ms = 0, publish_ms = 0, loop_ms = 0;
     int n_frames = 0, n_publish = 0, n_loops_ev = 0, transforms = 0;
     const clk::time_point t_all = clk::now();
     for (int t = 0; t < T; t++)
     {
-        double stamp, pose[7];
-        int kf, ref, k, n_path, n_loops, publish;
-        std::vector<double> path;
-        std::vector<int> pairs;
-        if (fread(&stamp, 8, 1, fs) != 1 || fread(&kf, 4, 1, fs) != 1 || fread(&ref, 4, 1, fs) != 1 || fread(&k, 4, 1, fs) != 1 ||
-            fread(pose, 8, 7, fs) != 7 || fread(&n_path, 4, 1, fs) != 1)
-            return 5;
-        path.resize((size_t)7 * n_path + 1);
-        if (fread(path.data(), 8, (size_t)7 * n_path, fs) != (size_t)7 * n_path || fread(&n_loops, 4, 1, fs) != 1) return 5;
-        pairs.resize((size_t)2 * n_loops + 1);
-        if (fread(pairs.data(), 4, (size_t)2 * n_loops, fs) != (size_t)2 * n_loops || fread(&publish, 4, 1, fs) != 1) return 5;
+        const DriveMsg &m = d.msgs[(size_t)t];
         dsm_sync(node.context());
         const clk::time_point a = clk::now();
-        int rc = node.orb_results_input(stamp, pairs.data(), n_loops, path.data(), n_path, pose, kf != 0, ref);
+        int rc = m.orb(node);
         if (!node.last_warp().empty())
         { // a loop closure: the orb callback and the transforms it enqueued
             dsm_sync(node.context());
@@ -58,11 +35,10 @@ int main(int argc, char **argv)
             transforms += (int)node.last_warp().size();
         }
         const clk::time_point b = clk::now();
-        if (rc == DSM_OK) rc = node.image_input(stamp, gray[(size_t)k].data(), (size_t)W);
-        if (rc == DSM_OK) rc = node.depth_input(stamp, depth[(size_t)k].data(), (size_t)W * 4);
+        if (rc == DSM_OK) rc = d.images(node, m, W);
         dsm_sync(node.context());
         frames_ms += ms(node.last_warp().empty() ? a : b, clk::now()); // the frame alone: pose, images, fuse
-        if (rc == DSM_OK && publish)
+        if (rc == DSM_OK && m.publish)
         {
             const clk::time_point c = clk::now();
             rc = node.active_points(active);

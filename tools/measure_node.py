@@ -13,8 +13,6 @@ Usage: python tools/measure_node.py [--frames 320] [--out DIR]"""
 import argparse
 import json
 import os
-import struct
-import subprocess
 import sys
 import tempfile
 import time
@@ -24,57 +22,8 @@ import numpy as np
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "oracle"))
-sys.path.insert(0, os.path.join(ROOT, "tests"))
-from densesurfelmapping_b200 import synth  # noqa: E402
-from test_surfel_node import correction, ros7  # noqa: E402
-
-CAM = synth.KITTI
-K = 8
-
-
-def messages(n_frames):
-    out, kf_frames, last_kf = [], [], 0
-    for t in range(n_frames):
-        C = correction(t // 100)
-        P = np.asarray(synth.pose_stream(t), np.float64).reshape(4, 4).T
-        is_kf = t % 4 == 0
-        path = [ros7(C @ np.asarray(synth.pose_stream(f), np.float64).reshape(4, 4).T) for f in kf_frames]
-        out.append((100.0 + 0.1 * t, is_kf, last_kf if t else 0, ros7(C @ P), path))
-        if is_kf:
-            kf_frames.append(t)
-            last_kf = len(kf_frames) - 1
-    return out
-
-
-def card():
-    r = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True)
-    if r.returncode != 0:
-        raise RuntimeError("nvidia-smi failed: no GPU to measure on")
-    name, power = [x.strip() for x in r.stdout.splitlines()[0].split(",")]
-    return name, power
-
-
-def run_node(tmp, frames, msgs, publish):
-    exe = os.path.join(tmp, "measure_node")
-    if not os.path.exists(exe):
-        pkg = os.path.join(ROOT, "densesurfelmapping_b200")
-        subprocess.run(["g++", "-std=c++11", "-O2", "-I", os.path.join(ROOT, "include"), os.path.join(ROOT, "tools", "measure_node.cpp"),
-                        "-o", exe, "-L", pkg, "-ldsm_b200", f"-Wl,-rpath,{pkg}"], check=True)
-    ff, fs = os.path.join(tmp, "frames.bin"), os.path.join(tmp, "script.bin")
-    with open(ff, "wb") as f:
-        f.write(struct.pack("<i", K))
-        for g, d in frames:
-            f.write(g.tobytes() + d.tobytes())
-    with open(fs, "wb") as f:
-        f.write(struct.pack("<i", len(msgs)))
-        for t, (stamp, is_kf, ref, p7, path) in enumerate(msgs):
-            f.write(struct.pack("<diii", stamp, int(is_kf), ref, t % K) + p7.tobytes())
-            f.write(struct.pack("<i", len(path)) + np.asarray(path, np.float64).tobytes() + struct.pack("<ii", 0, int(publish)))
-    args = [exe, str(CAM.width), str(CAM.height)] + [repr(float(v)) for v in (CAM.fx, CAM.fy, CAM.cx, CAM.cy, CAM.far, CAM.near)]
-    r = subprocess.run(args + ["10", ff, fs], capture_output=True, text=True)
-    if r.returncode != 0:
-        raise RuntimeError(f"measure_node exited {r.returncode}: {r.stderr[-2000:]}")
-    return json.loads(r.stdout.strip().splitlines()[-1])
+sys.path.insert(0, os.path.join(ROOT, "tools"))
+from measure_drive import CAM, K, build_harness, card, images, messages, run_harness, write_drive  # noqa: E402
 
 
 def run_reference(frames, msgs):
@@ -99,11 +48,12 @@ def main():
     a = ap.parse_args()
     assert a.frames >= 300
     name, power = card()
-    frames = [synth.make_frame(CAM, 5000 + k, synth.pose_stream(k)) for k in range(K)]
+    frames = images()
     msgs = messages(a.frames)
     with tempfile.TemporaryDirectory() as tmp:
-        bare = run_node(tmp, frames, msgs, publish=False)
-        pub = run_node(tmp, frames, msgs, publish=True)
+        exe = build_harness(tmp, "measure_node")
+        bare = run_harness(exe, *write_drive(tmp, frames, msgs))
+        pub = run_harness(exe, *write_drive(tmp, frames, msgs, publish=True))
     ref_ms, ref_loop = run_reference(frames, msgs)
     res = {"card": name, "power_limit": power, "frames": a.frames, "width": CAM.width, "height": CAM.height,
            "node_ms_per_frame": bare["frame_ms"], "node_publish_ms_per_frame": pub["publish_ms_per_frame"],

@@ -19,7 +19,6 @@ import argparse
 import ctypes
 import json
 import os
-import subprocess
 import sys
 import tempfile
 import time
@@ -30,11 +29,9 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tools"))
 sys.path.insert(0, os.path.join(ROOT, "tests"))
-from densesurfelmapping_b200 import synth  # noqa: E402
 from densesurfelmapping_b200.elements import POINT_DTYPE, SURFEL_DTYPE  # noqa: E402
+from measure_drive import CAM, SMALL, build_harness, card, images, messages, run_harness, spread, write_drive  # noqa: E402
 
-CAM = synth.KITTI
-SMALL = synth.Camera(320, 240, 262.5, 262.5, 159.5, 119.5, 0.5, 30.0)
 HBM_BYTES_PER_S = 3.35e12   # H100 SXM data sheet
 MODES = "abcd"
 
@@ -44,49 +41,11 @@ def mirror_bytes(n, n_changed):
     return 60 * n + 32 * n_changed
 
 
-def build_driver(tmp):
-    exe = os.path.join(tmp, "measure_publish")
-    pkg = os.path.join(ROOT, "densesurfelmapping_b200")
-    subprocess.run(["g++", "-std=c++11", "-O2", "-I", os.path.join(ROOT, "include"), os.path.join(ROOT, "tools", "measure_publish.cpp"),
-                    "-o", exe, "-L", pkg, "-ldsm_b200", f"-Wl,-rpath,{pkg}"], check=True)
-    return exe
-
-
-def write_drive(tmp, n_frames):
-    import struct
-    from measure_node import K, messages
-    frames = [synth.make_frame(CAM, 5000 + k, synth.pose_stream(k)) for k in range(K)]
-    ff, fs = os.path.join(tmp, "frames.bin"), os.path.join(tmp, "script.bin")
-    with open(ff, "wb") as f:
-        f.write(struct.pack("<i", K))
-        for g, d in frames:
-            f.write(g.tobytes() + d.tobytes())
-    msgs = messages(n_frames)
-    with open(fs, "wb") as f:
-        f.write(struct.pack("<i", len(msgs)))
-        for t, (stamp, is_kf, ref, p7, path) in enumerate(msgs):
-            f.write(struct.pack("<diii", stamp, int(is_kf), ref, t % K) + p7.tobytes())
-            f.write(struct.pack("<i", len(path)) + np.asarray(path, np.float64).tobytes() + struct.pack("<ii", 0, 0))
-    return ff, fs
-
-
-def run_mode(exe, ff, fs, mode, check):
-    args = [exe, str(CAM.width), str(CAM.height)] + [repr(float(v)) for v in (CAM.fx, CAM.fy, CAM.cx, CAM.cy, CAM.far, CAM.near)]
-    r = subprocess.run(args + ["10", ff, fs, mode, str(int(check))], capture_output=True, text=True)
-    if r.returncode != 0:
-        raise RuntimeError(f"measure_publish mode {mode} exited {r.returncode}: {r.stderr[-2000:]}")
-    return json.loads(r.stdout.strip().splitlines()[-1])
-
-
-def spread(xs):
-    return {"median": float(np.median(xs)), "min": float(min(xs)), "max": float(max(xs))}
-
-
 def node_drive(n_frames, rounds):
     with tempfile.TemporaryDirectory() as tmp:
-        exe = build_driver(tmp)
-        ff, fs = write_drive(tmp, n_frames)
-        checked = {m: run_mode(exe, ff, fs, m, True) for m in "bcd"}
+        exe = build_harness(tmp, "measure_publish")
+        ff, fs = write_drive(tmp, images(), messages(n_frames))
+        checked = {m: run_harness(exe, ff, fs, [m, 1]) for m in "bcd"}
         hashes = {m: r["hash"] for m, r in checked.items()}
         if len(set(hashes.values())) != 1:
             raise RuntimeError(f"the modes published different clouds: {hashes}")
@@ -94,7 +53,7 @@ def node_drive(n_frames, rounds):
         last = {}
         for _ in range(rounds):
             for m in MODES:
-                last[m] = run_mode(exe, ff, fs, m, False)
+                last[m] = run_harness(exe, ff, fs, [m, 0])
                 times[m].append(last[m]["ms_per_frame"])
     return {"frames": n_frames, "rounds": rounds, "clouds_hash": hashes["b"], "store_surfels": last["a"]["store_surfels"],
             "pool_surfels": last["a"]["pool_surfels"],
@@ -206,17 +165,6 @@ def kernel_alone(n, launches):
     return res
 
 
-def card():
-    try:
-        r = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True)
-    except FileNotFoundError:
-        r = None
-    if r is None or r.returncode != 0 or not r.stdout.strip():
-        raise RuntimeError("nvidia-smi failed: no GPU to measure on")
-    name, power = [x.strip() for x in r.stdout.splitlines()[0].split(",")]
-    return name, power
-
-
 def main():
     ap = argparse.ArgumentParser(description=__doc__.splitlines()[0])
     ap.add_argument("--frames", type=int, default=320)
@@ -231,8 +179,8 @@ def main():
         ap.error("--launches must be at least 200")
     if a.dry_run:
         with tempfile.TemporaryDirectory() as tmp:
-            build_driver(tmp)
-            ff, fs = write_drive(tmp, a.frames)
+            build_harness(tmp, "measure_publish")
+            ff, fs = write_drive(tmp, images(), messages(a.frames))
             print(json.dumps({"dry_run": True, "frames_bytes": os.path.getsize(ff), "script_bytes": os.path.getsize(fs),
                               "model_bytes_1Mi_unchanged": mirror_bytes(1 << 20, 0)}))
         return
