@@ -35,6 +35,7 @@ EXPORTS = [
     "dsm_field_enable", "dsm_field_enqueue", "dsm_field_wait",
     "dsm_field_enqueue_resident", "dsm_field_query_enable", "dsm_field_query_enqueue", "dsm_field_query_wait",
     "dsm_views_enable", "dsm_views_capture", "dsm_field_enqueue_known", "dsm_field_state",
+    "dsm_frontier_enable", "dsm_frontier_enqueue", "dsm_frontier_wait", "dsm_debug_field_load_state",
     "dsm_inactive_segments", "dsm_inactive_load", "dsm_map_save", "dsm_map_load", "dsm_map_peek",
     "dsm_checkpoint_enable", "dsm_checkpoint_enqueue", "dsm_checkpoint_wait", "dsm_debug_checkpoint_drain_ctas",
     "dsm_checkpoint_enqueue_incremental", "dsm_map_load_journal", "dsm_map_peek_journal", "dsm_journal_materialize",
@@ -62,6 +63,10 @@ class DsmFieldParams(ctypes.Structure):
 # dsm_field_query_wait's result records (include/dsm.h): a point sample and a trajectory clearance
 FIELD_SAMPLE_DTYPE = np.dtype([("dist", "<f4"), ("gx", "<f4"), ("gy", "<f4"), ("gz", "<f4")])
 CLEARANCE_DTYPE = np.dtype([("min_dist", "<f4"), ("argmin", "<i4"), ("first_hit", "<i4"), ("n_outside", "<i4")])
+# dsm_frontier_wait's records (include/dsm.h): a cluster (96 B) and the counts
+FRONTIER_CLUSTER_DTYPE = np.dtype([("n_voxels", "<i4"), ("first", "<i4"), ("offset", "<i4"), ("lo", "<i4", 3), ("hi", "<i4", 3),
+                                   ("reserved", "<i4"), ("n_faces", "<i8"), ("open", "<i8", 3), ("centroid", "<f8", 3)])
+FRONTIER_COUNTS_DTYPE = np.dtype([("n_frontier", "<i4"), ("n_components", "<i4"), ("n_clusters", "<i4"), ("n_listed", "<i4")])
 
 
 CONSTANTS_DRIVE = (0.4, 0.5, 4.0, 0.1)    # fusion_functions.h:13-16
@@ -127,6 +132,10 @@ def load_library():
     L.dsm_views_capture.argtypes = [vp, ci, ci]
     L.dsm_field_enqueue_known.argtypes = [vp, ctypes.POINTER(ctypes.c_double), ci, vp, vp, ci, ci]
     L.dsm_field_state.argtypes = [vp, ctypes.POINTER(vp), ctypes.POINTER(ci)]
+    L.dsm_frontier_enable.argtypes = [vp, ci, ci]
+    L.dsm_frontier_enqueue.argtypes = [vp, ci]
+    L.dsm_frontier_wait.argtypes = [vp, ctypes.POINTER(vp), ctypes.POINTER(vp), vp]
+    L.dsm_debug_field_load_state.argtypes = [vp, vp, ctypes.POINTER(ctypes.c_int32)]
     L.dsm_inactive_reserve.argtypes = [vp, ci]
     L.dsm_inactive_retire.argtypes = [vp, ci, ctypes.POINTER(ci)]
     L.dsm_inactive_reactivate.argtypes = [vp, ci, ctypes.POINTER(ci)]
@@ -617,6 +626,46 @@ class Context:
             buf = (ctypes.c_uint8 * (shape[0] * shape[1] * shape[2])).from_address(ptr.value)
             state = np.frombuffer(buf, dtype=np.uint8).reshape(shape).copy()
         return state, nfree.value
+
+    def debug_field_load_state(self, state, origin):
+        """Makes the uint8 state grid [nz][ny][nx] at integer origin (x, y, z) the latest known field request; field_wait
+        and field_state then read it like any other."""
+        st = np.ascontiguousarray(state, np.uint8)
+        if st.shape != self._field_shape:   # the library reads nx * ny * nz bytes
+            raise ValueError(f"state grid {st.shape}, field {self._field_shape}")
+        org = (ctypes.c_int32 * 3)(*[int(v) for v in origin])
+        self._ck(self.lib.dsm_debug_field_load_state(self.h, st.ctypes.data, org))
+
+    # ---- exploration frontiers of the latest known field ----
+    def frontier_enable(self, max_clusters, max_voxels):
+        self._ck(self.lib.dsm_frontier_enable(self.h, int(max_clusters), int(max_voxels)))
+        self._frontier_caps = (int(max_clusters), int(max_voxels))
+
+    def frontier_enqueue(self, min_voxels=1):
+        self._ck(self.lib.dsm_frontier_enqueue(self.h, int(min_voxels)))
+
+    def frontier_wait(self):
+        """(clusters, voxels, counts): numpy copies of the context's pinned results, FRONTIER_CLUSTER_DTYPE
+        (min(n_clusters, max_clusters),), int32 (n_listed,) and a FRONTIER_COUNTS_DTYPE record.  A job on a field taken
+        after a rejected frame raises DsmError(DSM_E_CAPACITY) carrying the same tuple as `.frontier`."""
+        pc, pv = ctypes.c_void_p(), ctypes.c_void_p()
+        counts = np.zeros(1, FRONTIER_COUNTS_DTYPE)
+        rc = self.lib.dsm_frontier_wait(self.h, ctypes.byref(pc), ctypes.byref(pv), counts.ctypes.data)
+        if rc not in (DSM_OK, -6):
+            self._ck(rc)
+        c = counts[0]
+        n_tab = min(int(c["n_clusters"]), self._frontier_caps[0])
+
+        def take(ptr, n, dtype):
+            if n == 0:
+                return np.zeros(0, dtype)
+            return np.frombuffer((ctypes.c_uint8 * (n * dtype.itemsize)).from_address(ptr.value), dtype=dtype).copy()
+        out = (take(pc, n_tab, FRONTIER_CLUSTER_DTYPE), take(pv, int(c["n_listed"]), np.dtype(np.int32)), c)
+        if rc != DSM_OK:
+            err = DsmError(rc, self.lib.dsm_last_error(self.h).decode())
+            err.frontier = out
+            raise err
+        return out
 
     # ---- planner queries against the latest field ----
     def field_query_enable(self, max_points, max_trajectories, max_waypoints):

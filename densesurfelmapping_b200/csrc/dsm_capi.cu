@@ -1743,6 +1743,128 @@ extern "C" int dsm_field_state(dsm_ctx *ctx, const uint8_t **state, int *n_free)
     return DSM_OK;
 }
 
+// A known request without views: the caller's states, the known distance transform and the host copy of dist with its
+// header (the states are already in the pinned state buffer).  The error words stay 0.
+extern "C" int dsm_debug_field_load_state(dsm_ctx *ctx, const uint8_t *state, const int32_t origin[3])
+{
+    if (!ctx || !state || !origin) return DSM_E_INVALID;
+    DsmField *f = ctx->field.get();
+    DsmViews *vw = ctx->views.get();
+    if (!f || !vw || f->in_flight) return DSM_E_STATE;
+    DsmFieldGrid g = f->g;
+    const int64_t lim = int64_t(1) << 24;
+    for (int k = 0; k < 3; k++)
+    {
+        const int64_t o = origin[k];
+        if (o < -lim || o > lim || o + g.n[k] < -lim || o + g.n[k] > lim) return DSM_E_INVALID;
+        g.o[k] = (int)o;
+        g.lo[k] = (float)o;
+        g.hi[k] = (float)(o + g.n[k]);
+    }
+    for (size_t i = 0; i < f->voxels; i++)
+        if (state[i] > DSM_STATE_FREE) return DSM_E_INVALID;
+    CK(cudaSetDevice(ctx->device));
+    std::memcpy(vw->state, state, f->voxels); // no copy out of it is pending: no field is in flight
+    int32_t *header = f->dist + dsm_field_header(f->voxels);
+    CK(cudaMemcpyAsync(f->occ, vw->state, f->voxels, cudaMemcpyHostToDevice, ctx->stream));
+    CK(cudaMemsetAsync(header, 0, (DSM_FIELD_VIEW + 1) * sizeof(int32_t), ctx->stream));
+    dsm_launch_field_edt(g, f->occ, true, f->dist, header, ctx->stream);
+    CK(cudaGetLastError());
+    CK(cudaMemcpyAsync(f->host, f->dist, f->bytes, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaEventRecord(f->ev, ctx->stream));
+    f->g = g;
+    f->in_flight = f->requested = f->known = true;
+    f->resident = f->known_waited = false;
+    return DSM_OK;
+}
+
+// ---- exploration frontiers of the latest known field (include/dsm.h, DESIGN.md §8.10) ----
+extern "C" int dsm_frontier_enable(dsm_ctx *ctx, int max_clusters, int max_voxels)
+{
+    if (!ctx) return DSM_E_INVALID;
+    const DsmField *f = ctx->field.get();
+    if (!f || !ctx->views || ctx->frontier) return DSM_E_STATE;
+    for (int n : {max_clusters, max_voxels})
+        if (n < 0 || n > DSM_FRONTIER_MAX_CAPACITY) return DSM_E_INVALID;
+    CK(cudaSetDevice(ctx->device));
+    auto fr = std::make_unique<DsmFrontier>();
+    DsmFrontierBufs &b = fr->b;
+    const int *n = f->g.n;
+    b.voxels = (int)f->voxels;
+    // every 2x2x2 block of voxels is 26-connected, so it meets at most one component
+    b.max_comp = ((n[0] + 1) / 2) * ((n[1] + 1) / 2) * ((n[2] + 1) / 2);
+    b.max_clusters = max_clusters, b.max_voxels = max_voxels;
+    const size_t cl = (size_t)std::max(max_clusters, 1), vx = (size_t)std::max(max_voxels, 1);
+    const size_t sel = (size_t)dsm_frontier_sel_blocks(b.voxels);
+    const size_t res = DsmFrontierBufs::res_bytes(max_clusters, max_voxels);
+    CudaOwner &o = fr->own;
+    cudaError_t e = o.device(&b.label, f->voxels);
+    for (int32_t **p : {&b.roots, &b.count, &b.cmap, &b.cid})
+        if (e == cudaSuccess) e = o.device(p, (size_t)b.max_comp);
+    for (int32_t **p : {&b.slot_comp, &b.sizes, &b.offs})
+        if (e == cudaSuccess) e = o.device(p, cl);
+    if (e == cudaSuccess) e = o.device(&b.acc, cl);
+    if (e == cudaSuccess) e = o.device(&b.idx, vx);
+    if (e == cudaSuccess) e = o.device(&b.keys, vx);
+    if (e == cudaSuccess) e = o.device(&b.keys_alt, vx);
+    if (e == cudaSuccess) e = o.device(&b.blk, sel);
+    if (e == cudaSuccess) e = o.device(&b.blk_ofs, sel);
+    if (e == cudaSuccess) e = o.device(&b.res, res);
+    if (e == cudaSuccess) e = o.host(&fr->res_host, res);
+    if (e == cudaSuccess) e = o.event(&fr->ev);
+    if (e == cudaSuccess)
+    {
+        b.temp_bytes = dsm_frontier_temp_bytes(b);
+        e = b.temp_bytes ? o.device(reinterpret_cast<uint8_t **>(&b.temp), b.temp_bytes) : cudaErrorInvalidValue;
+    }
+    if (e != cudaSuccess)
+    {
+        cudaGetLastError();
+        return DSM_E_NOMEM; // nothing is kept: a later call may try again
+    }
+    ctx->frontier = std::move(fr);
+    return DSM_OK;
+}
+
+// Enqueue only: the job on the state grid of the latest (known) field request with that request's origin, one D2H copy
+// of the result capacity and the event.  A later field request clears that grid only behind the job, in stream order.
+extern "C" int dsm_frontier_enqueue(dsm_ctx *ctx, int min_voxels)
+{
+    if (!ctx) return DSM_E_INVALID;
+    DsmFrontier *fr = ctx->frontier.get();
+    const DsmField *f = ctx->field.get();
+    if (!fr || !f || !f->requested || !f->known || fr->in_flight) return DSM_E_STATE;
+    if (min_voxels < 1) return DSM_E_INVALID;
+    CK(cudaSetDevice(ctx->device));
+    const DsmFrontierBufs &b = fr->b;
+    CK(cudaMemsetAsync(b.res, 0, 4 * DSM_FRONTIER_WORDS, ctx->stream));
+    CK(dsm_launch_frontier(b, f->g, f->occ, f->dist + dsm_field_header(f->voxels), min_voxels, ctx->stream));
+    CK(cudaMemcpyAsync(fr->res_host, b.res, DsmFrontierBufs::res_bytes(b.max_clusters, b.max_voxels), cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaEventRecord(fr->ev, ctx->stream));
+    fr->in_flight = true;
+    return DSM_OK;
+}
+
+extern "C" int dsm_frontier_wait(dsm_ctx *ctx, const dsm_frontier_cluster_t **clusters, const int32_t **voxels, dsm_frontier_counts_t *counts)
+{
+    if (!ctx) return DSM_E_INVALID;
+    DsmFrontier *fr = ctx->frontier.get();
+    if (!fr || !fr->in_flight) return DSM_E_STATE;
+    CK(cudaSetDevice(ctx->device));
+    CK(cudaEventSynchronize(fr->ev));
+    fr->in_flight = false;
+    const int32_t *h = reinterpret_cast<const int32_t *>(fr->res_host);
+    const size_t table = 4 * DSM_FRONTIER_WORDS;
+    if (clusters) *clusters = reinterpret_cast<const dsm_frontier_cluster_t *>(fr->res_host + table);
+    if (voxels)
+        *voxels = reinterpret_cast<const int32_t *>(fr->res_host + table + sizeof(dsm_frontier_cluster_t) * (size_t)fr->b.max_clusters);
+    if (counts) std::memcpy(counts, h, sizeof(dsm_frontier_counts_t));
+    if (h[DSM_FRONTIER_ERR_TAG] == 0) return DSM_OK;
+    snprintf(ctx->err, sizeof(ctx->err), "dsm_frontier_wait: frame %d of a dsm_fuse_stream_window call did not fit the pool or the "
+             "store; the field the job read holds the frames before it", h[DSM_FRONTIER_ERR_FRAME]);
+    return DSM_E_CAPACITY;
+}
+
 // ---- checkpoints that do not stop the stream (include/dsm.h, DESIGN.md §8.5) ----
 // The two images at the context's current capacities; whatever was there before is released first (the old and the new
 // need not fit at once).  On failure the checkpoint has no images and its calls return DSM_E_STATE.

@@ -217,6 +217,17 @@ struct DsmFieldQuery
     static size_t res_bytes(int n_points, int n_traj) { return res_clearance(n_points) + 16 * (size_t)n_traj; }
 };
 
+// dsm_frontier_* (DESIGN.md §8.10), allocated by dsm_frontier_enable for the field's grid: the job's device buffers
+// (DsmFrontierBufs, the packed result among them), the result's pinned copy and the event after its copy
+struct DsmFrontier
+{
+    CudaOwner own;
+    DsmFrontierBufs b;
+    uint8_t *res_host = nullptr;
+    cudaEvent_t ev = nullptr;
+    bool in_flight = false;
+};
+
 #define DSM_MAX_CHUNKS 4
 
 struct dsm_ctx
@@ -288,6 +299,7 @@ struct dsm_ctx
     std::unique_ptr<DsmField> field;     // nullptr until dsm_field_enable
     std::unique_ptr<DsmFieldQuery> field_query; // nullptr until dsm_field_query_enable
     std::unique_ptr<DsmViews> views;             // nullptr until dsm_views_enable
+    std::unique_ptr<DsmFrontier> frontier;       // nullptr until dsm_frontier_enable
     int run_split = 2;          // sub-batches per dsm_batch_run (dsm_set_concurrency)
     // pinned host staging for the small per-batch tables
     float *h_pose = nullptr; // [2B][32]: pose then inverse; first half: the batch calls, second half: the resident stream

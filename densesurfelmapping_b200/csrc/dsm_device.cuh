@@ -338,3 +338,50 @@ enum
 void dsm_launch_field_query(const float *dist, const int32_t *field_header, const DsmFieldGrid &g, const double *points, int n_points,
                             const double *waypoints, const int32_t *offsets, const int32_t *first, int n_traj, float radius,
                             int32_t *result_header, float4 *samples, dsm_clearance_t *clearance, cudaStream_t s);
+
+// dsm_frontier_* (DESIGN.md §8.10), dsm_frontier.cu.  One packed result (D2H):
+//   int32 header[DSM_FRONTIER_WORDS] | dsm_frontier_cluster_t table[max_clusters] | int32 list[max_voxels]
+enum
+{
+    DSM_FRONTIER_N_FRONTIER, // the four words of dsm_frontier_counts_t, zeroed before the job
+    DSM_FRONTIER_N_COMPONENTS,
+    DSM_FRONTIER_N_CLUSTERS,
+    DSM_FRONTIER_N_LISTED,
+    DSM_FRONTIER_ERR_TAG,    // the field header's DSM_FIELD_ERR_TAG / _ERR_FRAME, copied by k_frontier_mark
+    DSM_FRONTIER_ERR_FRAME,
+    DSM_FRONTIER_N_LISTED_CLUSTERS, // scratch: the table entries whose voxels are in the list
+    DSM_FRONTIER_N_SELECTED,        // scratch: the members the list compaction selected
+    DSM_FRONTIER_WORDS = 8          // 32 B: the table stays 8-byte aligned
+};
+// what dsm_frontier_reduce accumulates per table entry (integer atomics only)
+struct DsmFrontierAcc
+{
+    int32_t lo[3], hi[3];
+    unsigned long long sum[3], faces, open[3]; // two's complement int64
+};
+// The device buffers of one context's frontier jobs, sized by dsm_frontier_enable for the field's grid
+struct DsmFrontierBufs
+{
+    int voxels = 0, max_comp = 0, max_clusters = 0, max_voxels = 0;
+    int32_t *label = nullptr;                                   // [voxels]
+    int32_t *roots = nullptr, *count = nullptr, *cmap = nullptr, *cid = nullptr; // [max_comp]
+    int32_t *slot_comp = nullptr, *sizes = nullptr, *offs = nullptr; // [max_clusters]
+    DsmFrontierAcc *acc = nullptr;                              // [max_clusters]
+    int32_t *idx = nullptr;                                     // [max_voxels]
+    uint32_t *keys = nullptr, *keys_alt = nullptr;              // [max_voxels]
+    int32_t *blk = nullptr, *blk_ofs = nullptr;                 // [dsm_frontier_sel_blocks(voxels)]: the compactions' CTAs
+    uint8_t *res = nullptr;                                     // the packed result
+    void *temp = nullptr;                                       // CUB scratch of dsm_frontier_temp_bytes
+    size_t temp_bytes = 0;
+    static size_t res_bytes(int max_clusters, int max_voxels)
+    {
+        return 4 * (size_t)DSM_FRONTIER_WORDS + sizeof(dsm_frontier_cluster_t) * (size_t)max_clusters + 4 * (size_t)max_voxels;
+    }
+};
+int dsm_frontier_sel_blocks(int voxels);
+// the CUB scratch the job needs for these sizes (the buffers' pointers may still be null); 0 on a CUB error
+size_t dsm_frontier_temp_bytes(const DsmFrontierBufs &b);
+// the whole job on the state grid `state` of grid g, with the field header of that request; the result header must
+// be zeroed by the caller.  Returns the first error of a CUB call or a launch.
+cudaError_t dsm_launch_frontier(const DsmFrontierBufs &b, const DsmFieldGrid &g, const uint8_t *state, const int32_t *field_header,
+                                int min_voxels, cudaStream_t s);

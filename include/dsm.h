@@ -598,6 +598,67 @@ int dsm_field_enqueue_known(dsm_ctx *ctx, const double center[3], int min_update
                             int n_views, int host_copy);
 int dsm_field_state(dsm_ctx *ctx, const uint8_t **state, int *n_free);
 
+/* ---- exploration frontiers: clusters of known-free voxels that border unknown space (DESIGN.md §8.10) ----
+ * A frontier job reads the state grid of the latest field request, which must be a known one (any enqueue call, waited
+ * for or not), in stream order behind it, with that request's origin o and voxel edge v captured at the job's enqueue; a
+ * later field request may be enqueued while a job is in flight and does not change what the job reads.  Only the state
+ * grid is read, never the map.  Voxel (x, y, z) has the linear index (z * ny + y) * nx + x.
+ *
+ * Definition (integer throughout, so the result does not depend on the schedule; the centroid rounds once per step).
+ *   Frontier voxel: state 2 (free) with at least one of its six face neighbours INSIDE the grid of state 0 (unknown);
+ *   neighbours outside the grid do not count, so the box's own faces are no frontier.
+ *   Components: the 26-connected components of the frontier voxels, ordered by ascending `first`, the lowest linear
+ *   index among their voxels (scipy.ndimage.label with a 3x3x3 structure numbers them in this order).
+ *   Clusters: the components of at least min_voxels voxels, in the same order.  Per cluster: n_voxels, first, the
+ *   inclusive grid-coordinate bounds lo / hi, n_faces the number of (frontier voxel, unknown face neighbour) pairs,
+ *   open the sum over those pairs of the unit step toward the unknown neighbour (the direction to look), and
+ *   centroid_k = ((double)sum_k / (double)n_voxels + ((double)o_k + 0.5)) * (double)v in world metres, sum_k the exact
+ *   sum of the members' grid coordinates.
+ *   Capacities: the table holds the first max_clusters clusters.  The voxel list holds the members of listed clusters
+ *   as int32 linear indices, grouped by cluster in table order and ascending within one; a cluster's offset is the
+ *   exclusive prefix sum of n_voxels over the table, or -1 when offset + n_voxels > max_voxels, so the list always holds
+ *   whole clusters, and they are a prefix of the table.
+ *   Counts: n_frontier every frontier voxel, n_components every component, n_clusters every cluster (the table holds
+ *   min(n_clusters, max_clusters)), n_listed the voxels in the list.  No free or no unknown voxel: all counts are 0.
+ *
+ *   dsm_frontier_enable    once, after dsm_views_enable (DSM_E_STATE otherwise, and when called twice).  DSM_E_INVALID
+ *                          for a negative capacity or one above 2^26.  Allocates, for the field's grid and in the worst
+ *                          case (at most ceil(nx/2) ceil(ny/2) ceil(nz/2) components), a label grid (4 B per voxel), the
+ *                          component and cluster scratch, the device result and its pinned copy of
+ *                          32 + 96 max_clusters + 4 max_voxels bytes, and an event.  DSM_E_NOMEM, with nothing kept.
+ *   dsm_frontier_enqueue   asynchronous on the context's stream, never waits: the kernels, one D2H copy of the result
+ *                          capacity and the event.  DSM_E_STATE before dsm_frontier_enable, before any field request,
+ *                          when the latest field request is not a known one, and while a job is in flight;
+ *                          DSM_E_INVALID for min_voxels < 1.
+ *   dsm_frontier_wait      waits for that job only.  *clusters (min(n_clusters, max_clusters) records) and *voxels
+ *                          (n_listed) are the context's pinned results, valid until the next dsm_frontier_enqueue; any
+ *                          out-pointer may be NULL.  If the field the job read was taken after a rejected frame, returns
+ *                          DSM_E_CAPACITY with valid results and does NOT clear the error, as dsm_field_wait.
+ *                          DSM_E_STATE with no job enqueued.
+ *   dsm_debug_field_load_state   test entry: makes the caller's state grid (nx * ny * nz bytes, [z][y][x]) at origin
+ *                          o the latest known field request, as if a known request had produced it: one H2D copy into
+ *                          the grid, the known distance transform and a host copy, waited for with dsm_field_wait and
+ *                          read with dsm_field_state like any known request.  DSM_E_INVALID for a byte above 2 or an
+ *                          origin outside dsm_field_enqueue's bounds; DSM_E_STATE before dsm_views_enable and while a
+ *                          field is in flight. */
+typedef struct dsm_frontier_cluster_t
+{
+    int32_t n_voxels, first, offset; /* offset: into the voxel list, -1 when the cluster is not in it */
+    int32_t lo[3], hi[3];            /* inclusive grid-coordinate bounds */
+    int32_t reserved;                /* 0 */
+    int64_t n_faces, open[3];
+    double centroid[3];              /* metres */
+} dsm_frontier_cluster_t;            /* 96 B */
+typedef struct dsm_frontier_counts_t
+{
+    int32_t n_frontier, n_components, n_clusters, n_listed;
+} dsm_frontier_counts_t;
+#define DSM_FRONTIER_MAX_CAPACITY (1 << 26)
+int dsm_frontier_enable(dsm_ctx *ctx, int max_clusters, int max_voxels);
+int dsm_frontier_enqueue(dsm_ctx *ctx, int min_voxels);
+int dsm_frontier_wait(dsm_ctx *ctx, const dsm_frontier_cluster_t **clusters, const int32_t **voxels, dsm_frontier_counts_t *counts);
+int dsm_debug_field_load_state(dsm_ctx *ctx, const uint8_t *state, const int32_t origin[3]);
+
 /* ---- checkpoints that do not stop the stream (DESIGN.md §8.5) ----
  * The file of dsm_map_save, taken in stream order like a publish snapshot: the resident stream pays one device-to-device
  * copy of the live map, the transfer to the host runs on a low-priority stream beside the next frames, and a thread of

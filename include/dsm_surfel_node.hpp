@@ -75,6 +75,10 @@
 // filled slot at its current world pose cam_pose[ref] * relative, in fuse_pose's arithmetic, so a loop closure moves the
 // views with the map.  known_space() returns the state grid of the field distance_field() handed out last.  Views are
 // not part of a checkpoint: load_state* empties the slot table, which refills as keyframes are fused.
+// An exploring planner asks where to look next.  enable_frontiers(max_clusters, max_voxels), after enable_known_space,
+// lets frontiers() find the exploration frontiers of the latest fused frame's known field on the device (DESIGN.md
+// §8.10): the clusters of free voxels that border unknown space, their statistics and member voxels, one enqueue and one
+// wait, without touching the one-frame-late distance_field() handout.
 // device < 0 builds the node without a context: the callbacks run the whole pose logic (pose database, sync, window
 // bookkeeping) and fuse nothing; any call that reads the map returns DSM_E_STATE.
 #pragma once
@@ -510,6 +514,38 @@ class SurfelMapNode
                 for (int c = 0; c < 4; c++) poses.push_back(m(r, c));
         }
         return captures_;
+    }
+
+    // ---- exploration frontiers of the latest fused frame's known field (DESIGN.md §8.10) ----
+    // once, after enable_known_space: the capacities of the cluster table and the voxel list
+    int enable_frontiers(int max_clusters, int max_voxels)
+    {
+        if (ctx_.run("enable_frontiers", [&] { return dsm_frontier_enable(ctx_.ctx, max_clusters, max_voxels); }) == DSM_OK)
+            frontier_clusters_ = max_clusters;
+        return ctx_.err;
+    }
+    // the clusters of at least min_voxels frontier voxels (include/dsm.h), the voxel list and the counts of the latest
+    // fused frame's known field; clusters receives min(n_clusters, max_clusters) records and voxels n_listed indices.
+    // DSM_E_STATE without known space, before any field, and after load_state* until the next fused frame;
+    // DSM_E_CAPACITY with the frontiers of the last applied frame's field, as distance_field().
+    int frontiers(int min_voxels, std::vector<dsm_frontier_cluster_t> &clusters, std::vector<int32_t> &voxels, dsm_frontier_counts_t &counts)
+    {
+        clusters.clear();
+        voxels.clear();
+        counts = dsm_frontier_counts_t();
+        if (!ctx_.ready("frontiers")) return ctx_.err;
+        if (known_.empty() || !field_exists_) return ctx_.done(DSM_E_STATE, "frontiers");
+        int rc = dsm_frontier_enqueue(ctx_.ctx, min_voxels);
+        if (rc != DSM_OK) return ctx_.done(rc, "frontiers");
+        const dsm_frontier_cluster_t *c = nullptr;
+        const int32_t *v = nullptr;
+        rc = dsm_frontier_wait(ctx_.ctx, &c, &v, &counts);
+        if (rc == DSM_OK || rc == DSM_E_CAPACITY)
+        {
+            clusters.assign(c, c + std::min(counts.n_clusters, frontier_clusters_));
+            voxels.assign(v, v + counts.n_listed);
+        }
+        return ctx_.done(rc, "frontiers");
     }
 
     // ---- planner queries against the field of the latest fused frame (DESIGN.md §8.8) ----
@@ -1043,5 +1079,6 @@ class SurfelMapNode
     };
     std::vector<KnownView> known_; // empty without known space
     int captures_ = 0, captured_ref_ = -1; // captures so far; the reference keyframe of the latest
+    int frontier_clusters_ = 0;            // enable_frontiers' max_clusters
 };
 } // namespace dsm
