@@ -36,6 +36,7 @@ EXPORTS = [
     "dsm_field_enqueue_resident", "dsm_field_query_enable", "dsm_field_query_enqueue", "dsm_field_query_wait",
     "dsm_views_enable", "dsm_views_capture", "dsm_field_enqueue_known", "dsm_field_state",
     "dsm_frontier_enable", "dsm_frontier_enqueue", "dsm_frontier_wait", "dsm_debug_field_load_state",
+    "dsm_reach_enable", "dsm_reach_enqueue", "dsm_reach_wait",
     "dsm_inactive_segments", "dsm_inactive_load", "dsm_map_save", "dsm_map_load", "dsm_map_peek",
     "dsm_checkpoint_enable", "dsm_checkpoint_enqueue", "dsm_checkpoint_wait", "dsm_debug_checkpoint_drain_ctas",
     "dsm_checkpoint_enqueue_incremental", "dsm_map_load_journal", "dsm_map_peek_journal", "dsm_journal_materialize",
@@ -67,6 +68,13 @@ CLEARANCE_DTYPE = np.dtype([("min_dist", "<f4"), ("argmin", "<i4"), ("first_hit"
 FRONTIER_CLUSTER_DTYPE = np.dtype([("n_voxels", "<i4"), ("first", "<i4"), ("offset", "<i4"), ("lo", "<i4", 3), ("hi", "<i4", 3),
                                    ("reserved", "<i4"), ("n_faces", "<i8"), ("open", "<i8", 3), ("centroid", "<f8", 3)])
 FRONTIER_COUNTS_DTYPE = np.dtype([("n_frontier", "<i4"), ("n_components", "<i4"), ("n_clusters", "<i4"), ("n_listed", "<i4")])
+# dsm_reach_wait's records (include/dsm.h): a target (32 B) and the header (64 B)
+REACH_TARGET_DTYPE = np.dtype([("cost", "<u4"), ("approach", "<i4"), ("target", "<i4"), ("viewpoint", "<i4"), ("path_offset", "<i4"),
+                               ("path_len", "<i4"), ("status", "<i4"), ("reserved", "<i4")])
+REACH_INFO_DTYPE = np.dtype([("origin", "<i4", 3), ("start_voxel", "<i4"), ("start_status", "<i4"), ("start_approach", "<i4"),
+                             ("rounds", "<i4"), ("converged", "<i4"), ("n_traversable", "<i4"), ("n_reached", "<i4"),
+                             ("n_goals", "<i4"), ("n_clusters_total", "<i4"), ("n_targets", "<i4"), ("n_path_voxels", "<i4"),
+                             ("reserved", "<i4", 2)])
 
 
 CONSTANTS_DRIVE = (0.4, 0.5, 4.0, 0.1)    # fusion_functions.h:13-16
@@ -136,6 +144,9 @@ def load_library():
     L.dsm_frontier_enqueue.argtypes = [vp, ci]
     L.dsm_frontier_wait.argtypes = [vp, ctypes.POINTER(vp), ctypes.POINTER(vp), vp]
     L.dsm_debug_field_load_state.argtypes = [vp, vp, ctypes.POINTER(ctypes.c_int32)]
+    L.dsm_reach_enable.argtypes = [vp, ci, ci, ci]
+    L.dsm_reach_enqueue.argtypes = [vp, ctypes.POINTER(ctypes.c_double), ctypes.c_float, ci, vp, ci, ci, ci]
+    L.dsm_reach_wait.argtypes = [vp, vp, ctypes.POINTER(vp), ctypes.POINTER(vp), ctypes.POINTER(vp)]
     L.dsm_inactive_reserve.argtypes = [vp, ci]
     L.dsm_inactive_retire.argtypes = [vp, ci, ctypes.POINTER(ci)]
     L.dsm_inactive_reactivate.argtypes = [vp, ci, ctypes.POINTER(ci)]
@@ -664,6 +675,44 @@ class Context:
         if rc != DSM_OK:
             err = DsmError(rc, self.lib.dsm_last_error(self.h).decode())
             err.frontier = out
+            raise err
+        return out
+
+    # ---- paths through known free space of the latest known field ----
+    def reach_enable(self, max_targets, max_path_voxels, max_rounds):
+        self._ck(self.lib.dsm_reach_enable(self.h, int(max_targets), int(max_path_voxels), int(max_rounds)))
+
+    def reach_enqueue(self, start, radius, approach, goals=None, with_frontiers=False, host_copy=False):
+        """start: a world point (x, y, z); goals: world points, an (n, 3) array-like of float64 (None for none)."""
+        st = (ctypes.c_double * 3)(*[float(v) for v in start])
+        g = np.ascontiguousarray(np.zeros((0, 3)) if goals is None else goals, np.float64).reshape(-1, 3)
+        self._ck(self.lib.dsm_reach_enqueue(self.h, st, float(radius), int(approach), g.ctypes.data if len(g) else None, len(g),
+                                            int(bool(with_frontiers)), int(bool(host_copy))))
+
+    def reach_wait(self):
+        """(info, targets, path, cost): numpy copies of the context's pinned results, a REACH_INFO_DTYPE record,
+        REACH_TARGET_DTYPE (n_targets,), int32 (n_path_voxels,) and the uint32 cost grid [nz][ny][nx] (None without
+        host_copy).  A job on a field taken after a rejected frame raises DsmError(DSM_E_CAPACITY) carrying the same
+        tuple as `.reach`."""
+        pt, pp, pc = ctypes.c_void_p(), ctypes.c_void_p(), ctypes.c_void_p()
+        info = np.zeros(1, REACH_INFO_DTYPE)
+        rc = self.lib.dsm_reach_wait(self.h, info.ctypes.data, ctypes.byref(pt), ctypes.byref(pp), ctypes.byref(pc))
+        if rc not in (DSM_OK, -6):
+            self._ck(rc)
+        i = info[0]
+
+        def take(ptr, n, dtype):
+            if n == 0 or not ptr.value:
+                return np.zeros(0, dtype)
+            return np.frombuffer((ctypes.c_uint8 * (n * dtype.itemsize)).from_address(ptr.value), dtype=dtype).copy()
+        cost = None
+        if pc.value:
+            nz, ny, nx = self._field_shape
+            cost = take(pc, nx * ny * nz, np.dtype(np.uint32)).reshape(nz, ny, nx)
+        out = (i, take(pt, int(i["n_targets"]), REACH_TARGET_DTYPE), take(pp, int(i["n_path_voxels"]), np.dtype(np.int32)), cost)
+        if rc != DSM_OK:
+            err = DsmError(rc, self.lib.dsm_last_error(self.h).decode())
+            err.reach = out
             raise err
         return out
 

@@ -1517,6 +1517,7 @@ static int field_enqueue(dsm_ctx *ctx, const double center[3], int min_update_ti
     f->resident = !host_copy;
     f->known = known != nullptr;
     f->known_waited = false;
+    f->requests++;
     return DSM_OK;
 }
 
@@ -1775,6 +1776,7 @@ extern "C" int dsm_debug_field_load_state(dsm_ctx *ctx, const uint8_t *state, co
     f->g = g;
     f->in_flight = f->requested = f->known = true;
     f->resident = f->known_waited = false;
+    f->requests++;
     return DSM_OK;
 }
 
@@ -1842,6 +1844,7 @@ extern "C" int dsm_frontier_enqueue(dsm_ctx *ctx, int min_voxels)
     CK(cudaMemcpyAsync(fr->res_host, b.res, DsmFrontierBufs::res_bytes(b.max_clusters, b.max_voxels), cudaMemcpyDeviceToHost, ctx->stream));
     CK(cudaEventRecord(fr->ev, ctx->stream));
     fr->in_flight = true;
+    fr->request = f->requests;
     return DSM_OK;
 }
 
@@ -1862,6 +1865,126 @@ extern "C" int dsm_frontier_wait(dsm_ctx *ctx, const dsm_frontier_cluster_t **cl
     if (h[DSM_FRONTIER_ERR_TAG] == 0) return DSM_OK;
     snprintf(ctx->err, sizeof(ctx->err), "dsm_frontier_wait: frame %d of a dsm_fuse_stream_window call did not fit the pool or the "
              "store; the field the job read holds the frames before it", h[DSM_FRONTIER_ERR_FRAME]);
+    return DSM_E_CAPACITY;
+}
+
+// ---- paths through known free space (include/dsm.h, DESIGN.md §8.11) ----
+extern "C" int dsm_reach_enable(dsm_ctx *ctx, int max_targets, int max_path_voxels, int max_rounds)
+{
+    if (!ctx) return DSM_E_INVALID;
+    const DsmField *f = ctx->field.get();
+    if (!f || !ctx->views || ctx->reach) return DSM_E_STATE;
+    for (int n : {max_targets, max_path_voxels})
+        if (n < 0 || n > DSM_REACH_MAX_CAPACITY) return DSM_E_INVALID;
+    if (max_rounds < 1 || max_rounds > DSM_REACH_MAX_ROUNDS || f->voxels > (size_t)DSM_REACH_MAX_VOXELS) return DSM_E_INVALID;
+    CK(cudaSetDevice(ctx->device));
+    auto re = std::make_unique<DsmReach>();
+    DsmReachBufs &b = re->b;
+    b.voxels = (int)f->voxels;
+    for (int k = 0; k < 3; k++) b.tn[k] = (f->g.n[k] + DSM_REACH_TILE - 1) / DSM_REACH_TILE;
+    b.tiles = b.tn[0] * b.tn[1] * b.tn[2];
+    b.max_targets = max_targets, b.max_path = max_path_voxels, b.max_rounds = max_rounds;
+    b.ctas = dsm_reach_ctas();
+    const size_t tg = (size_t)std::max(max_targets, 1);
+    const size_t res = DsmReachBufs::res_bytes(max_targets, max_path_voxels);
+    CudaOwner &o = re->own;
+    cudaError_t e = b.ctas > 0 ? o.device(&b.trav, f->voxels) : cudaErrorInvalidValue;
+    for (uint32_t **p : {&b.cost[0], &b.cost[1]})
+        if (e == cudaSuccess) e = o.device(p, f->voxels);
+    for (int32_t **p : {&b.stamp, &b.sched[0], &b.sched[1]})
+        if (e == cudaSuccess) e = o.device(p, (size_t)b.tiles);
+    if (e == cudaSuccess) e = o.device(&b.count, 3);
+    if (e == cudaSuccess) e = o.device(&b.goals, 3 * tg);
+    if (e == cudaSuccess) e = o.device(&b.best, tg);
+    if (e == cudaSuccess) e = o.device(&b.member, tg);
+    if (e == cudaSuccess) e = o.device(&b.len, tg);
+    if (e == cudaSuccess) e = o.device(&b.ofs, tg);
+    if (e == cudaSuccess) e = o.device(&b.res, res);
+    if (e == cudaSuccess) e = o.host(&re->goals_host, 3 * tg);
+    if (e == cudaSuccess) e = o.host(&re->res_host, res);
+    if (e == cudaSuccess) e = o.host(&re->cost_host, f->voxels);
+    if (e == cudaSuccess) e = o.event(&re->ev);
+    if (e == cudaSuccess)
+    {
+        b.temp_bytes = dsm_reach_temp_bytes(b);
+        e = b.temp_bytes ? o.device(reinterpret_cast<uint8_t **>(&b.temp), b.temp_bytes) : cudaErrorInvalidValue;
+    }
+    if (e != cudaSuccess)
+    {
+        cudaGetLastError();
+        return DSM_E_NOMEM; // nothing is kept: a later call may try again
+    }
+    ctx->reach = std::move(re);
+    return DSM_OK;
+}
+
+// floor(p / (double)v) - o, clamped to [-1, n]: outside the grid stays outside
+static int reach_voxel(double p, float v, int o, int n)
+{
+    const double q = std::floor(p / (double)v) - (double)o;
+    return q < 0.0 ? -1 : q >= (double)n ? n : (int)q;
+}
+
+// Enqueue only: the goal voxels staged and copied, the job on the grids of the latest (known) field request and, with
+// frontiers, on the latest frontier job's device result, one D2H copy of the result capacity (and of the cost grid with
+// host_copy) and the event.  Later field and frontier requests overwrite those buffers only behind the job.
+extern "C" int dsm_reach_enqueue(dsm_ctx *ctx, const double start[3], float radius, int approach, const double *goals, int n_goals,
+                                 int with_frontiers, int host_copy)
+{
+    if (!ctx) return DSM_E_INVALID;
+    DsmReach *re = ctx->reach.get();
+    const DsmField *f = ctx->field.get();
+    if (!re || !f || !f->requested || !f->known || re->in_flight) return DSM_E_STATE;
+    const DsmFrontier *fr = ctx->frontier.get();
+    if (with_frontiers && (!fr || fr->request != f->requests)) return DSM_E_STATE;
+    DsmReachBufs &b = re->b;
+    if (!start || !std::isfinite(radius) || !(radius >= 0.f) || approach < 0 || approach > DSM_REACH_MAX_APPROACH || n_goals < 0 ||
+        n_goals > b.max_targets || (n_goals > 0 && !goals))
+        return DSM_E_INVALID;
+    for (int k = 0; k < 3; k++)
+        if (!std::isfinite(start[k])) return DSM_E_INVALID;
+    for (size_t i = 0; i < 3 * (size_t)n_goals; i++)
+        if (!std::isfinite(goals[i])) return DSM_E_INVALID;
+    const DsmFieldGrid &g = f->g;
+    CK(cudaSetDevice(ctx->device));
+    // the previous job's copy out of this staging ended before its wait, which no job in flight implies
+    for (size_t i = 0; i < 3 * (size_t)n_goals; i++) re->goals_host[i] = reach_voxel(goals[i], g.voxel, g.o[i % 3], g.n[i % 3]);
+    if (n_goals > 0) CK(cudaMemcpyAsync(b.goals, re->goals_host, 12 * (size_t)n_goals, cudaMemcpyHostToDevice, ctx->stream));
+    const int3 s = make_int3(reach_voxel(start[0], g.voxel, g.o[0], g.n[0]), reach_voxel(start[1], g.voxel, g.o[1], g.n[1]),
+                             reach_voxel(start[2], g.voxel, g.o[2], g.n[2]));
+    CK(cudaMemsetAsync(b.res, 0, 4 * DSM_REACH_WORDS, ctx->stream));
+    CK(dsm_launch_reach(b, g, f->occ, f->dist, s, radius, approach, n_goals, with_frontiers ? fr->b.res : nullptr,
+                        with_frontiers ? fr->b.max_clusters : 0, ctx->stream));
+    CK(cudaMemcpyAsync(re->res_host, b.res, DsmReachBufs::res_bytes(b.max_targets, b.max_path), cudaMemcpyDeviceToHost, ctx->stream));
+    if (host_copy) CK(cudaMemcpyAsync(re->cost_host, b.cost[0], 4 * (size_t)b.voxels, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaEventRecord(re->ev, ctx->stream));
+    re->in_flight = true;
+    re->host_copy = host_copy != 0;
+    return DSM_OK;
+}
+
+extern "C" int dsm_reach_wait(dsm_ctx *ctx, dsm_reach_info_t *info, const dsm_reach_target_t **targets, const int32_t **path,
+                              const uint32_t **cost)
+{
+    if (!ctx) return DSM_E_INVALID;
+    DsmReach *re = ctx->reach.get();
+    if (!re || !re->in_flight) return DSM_E_STATE;
+    CK(cudaSetDevice(ctx->device));
+    CK(cudaEventSynchronize(re->ev));
+    re->in_flight = false;
+    const int32_t *h = reinterpret_cast<const int32_t *>(re->res_host);
+    const size_t table = 4 * DSM_REACH_WORDS;
+    if (info)
+    {
+        std::memcpy(info, h, sizeof(dsm_reach_info_t));
+        info->reserved[0] = info->reserved[1] = 0;
+    }
+    if (targets) *targets = reinterpret_cast<const dsm_reach_target_t *>(re->res_host + table);
+    if (path) *path = reinterpret_cast<const int32_t *>(re->res_host + table + sizeof(dsm_reach_target_t) * (size_t)re->b.max_targets);
+    if (cost) *cost = re->host_copy ? re->cost_host : nullptr;
+    if (h[DSM_REACH_ERR_TAG] == 0) return DSM_OK;
+    snprintf(ctx->err, sizeof(ctx->err), "dsm_reach_wait: frame %d of a dsm_fuse_stream_window call did not fit the pool or the "
+             "store; the field the job read holds the frames before it", h[DSM_REACH_ERR_FRAME]);
     return DSM_E_CAPACITY;
 }
 

@@ -185,6 +185,7 @@ struct DsmField
     bool resident = false;  // the latest request copies only its header words (dsm_field_enqueue_resident)
     bool known = false;     // the latest request is a known one (dsm_field_enqueue_known): its query view is DSM_FIELD_VIEW
     bool known_waited = false; // the last waited request is a known one, and no request has been enqueued since
+    uint64_t requests = 0;     // field requests enqueued so far (dsm_reach_enqueue pairs a frontier job with its field)
 };
 
 // dsm_views_* (DESIGN.md §8.9), allocated by dsm_views_enable: the captured rays of max_views slots, which slots hold a
@@ -226,6 +227,21 @@ struct DsmFrontier
     uint8_t *res_host = nullptr;
     cudaEvent_t ev = nullptr;
     bool in_flight = false;
+    uint64_t request = 0; // the DsmField::requests of the field the latest job read (0: no job yet)
+};
+
+// dsm_reach_* (DESIGN.md §8.11), allocated by dsm_reach_enable for the field's grid: the job's device buffers
+// (DsmReachBufs, the packed result among them), the goal staging, the result's and the cost grid's pinned copies and the
+// event after them
+struct DsmReach
+{
+    CudaOwner own;
+    DsmReachBufs b;
+    int32_t *goals_host = nullptr; // pinned [max_targets][3]
+    uint8_t *res_host = nullptr;
+    uint32_t *cost_host = nullptr; // pinned [voxels]
+    cudaEvent_t ev = nullptr;
+    bool in_flight = false, host_copy = false;
 };
 
 #define DSM_MAX_CHUNKS 4
@@ -300,6 +316,7 @@ struct dsm_ctx
     std::unique_ptr<DsmFieldQuery> field_query; // nullptr until dsm_field_query_enable
     std::unique_ptr<DsmViews> views;             // nullptr until dsm_views_enable
     std::unique_ptr<DsmFrontier> frontier;       // nullptr until dsm_frontier_enable
+    std::unique_ptr<DsmReach> reach;             // nullptr until dsm_reach_enable
     int run_split = 2;          // sub-batches per dsm_batch_run (dsm_set_concurrency)
     // pinned host staging for the small per-batch tables
     float *h_pose = nullptr; // [2B][32]: pose then inverse; first half: the batch calls, second half: the resident stream

@@ -385,3 +385,58 @@ size_t dsm_frontier_temp_bytes(const DsmFrontierBufs &b);
 // be zeroed by the caller.  Returns the first error of a CUB call or a launch.
 cudaError_t dsm_launch_frontier(const DsmFrontierBufs &b, const DsmFieldGrid &g, const uint8_t *state, const int32_t *field_header,
                                 int min_voxels, cudaStream_t s);
+
+// dsm_reach_* (DESIGN.md §8.11), dsm_reach.cu.  One packed result (D2H):
+//   int32 header[DSM_REACH_WORDS] | dsm_reach_target_t targets[max_targets] | int32 path[max_path_voxels]
+// The header's first 14 words are those of dsm_reach_info_t; the last two carry the field's error words.
+enum
+{
+    DSM_REACH_ORIGIN = 0, // 3 words
+    DSM_REACH_START_VOXEL = 3,
+    DSM_REACH_START_STATUS,
+    DSM_REACH_START_APPROACH,
+    DSM_REACH_ROUNDS,
+    DSM_REACH_CONVERGED,
+    DSM_REACH_N_TRAVERSABLE,
+    DSM_REACH_N_REACHED,
+    DSM_REACH_N_GOALS,
+    DSM_REACH_N_CLUSTERS_TOTAL,
+    DSM_REACH_N_TARGETS,
+    DSM_REACH_N_PATH_VOXELS,
+    DSM_REACH_ERR_TAG, // the field header's DSM_FIELD_ERR_TAG / _ERR_FRAME, copied by k_reach_start
+    DSM_REACH_ERR_FRAME,
+    DSM_REACH_WORDS = 16 // 64 B
+};
+#define DSM_REACH_TILE 8 // tiles of 8 x 8 x 8 voxels, one CTA of 512 threads each
+// The device buffers of one context's reach jobs, sized by dsm_reach_enable for the field's grid and capacities
+struct DsmReachBufs
+{
+    int voxels = 0, tiles = 0, tn[3] = {0, 0, 0}; // tn: tiles per axis
+    int max_targets = 0, max_path = 0, max_rounds = 0, ctas = 0; // ctas: the persistent CTAs of a round
+    uint8_t *trav = nullptr;                      // [voxels]
+    uint32_t *cost[2] = {nullptr, nullptr};       // [voxels] each
+    int32_t *stamp = nullptr;                     // [tiles]: the latest round a tile was scheduled for
+    int32_t *sched[2] = {nullptr, nullptr};       // [tiles] each: round r's schedule is sched[r % 2]
+    int32_t *count = nullptr;                     // [3]: round r's schedule length is count[r % 3]
+    int32_t *goals = nullptr;                     // device [max_targets][3] goal voxels, staged from goals_host
+    unsigned long long *best = nullptr;           // [max_targets] (cost << 32 | viewpoint)
+    int32_t *member = nullptr;                    // [max_targets] the cluster member attaining best
+    long long *len = nullptr, *ofs = nullptr;     // [max_targets] path lengths and their exclusive prefix sums
+    uint8_t *res = nullptr;                       // the packed result
+    void *temp = nullptr;                         // CUB scratch of dsm_reach_temp_bytes
+    size_t temp_bytes = 0;
+    static size_t res_bytes(int max_targets, int max_path)
+    {
+        return 4 * (size_t)DSM_REACH_WORDS + sizeof(dsm_reach_target_t) * (size_t)max_targets + 4 * (size_t)max_path;
+    }
+};
+// the CUB scratch of the path-length scan; 0 on a CUB error
+size_t dsm_reach_temp_bytes(const DsmReachBufs &b);
+// the persistent CTAs of k_reach_round on this device
+int dsm_reach_ctas();
+// The whole job on the grids of the latest known request (state, distance and header at dsm_field_header(voxels)),
+// from start voxel s (each axis clamped to [-1, n]) with the n_goals goal voxels already in b.goals; frontier_res is the
+// frontier job's device result (nullptr without frontiers).  The result header must be zeroed by the caller.
+cudaError_t dsm_launch_reach(const DsmReachBufs &b, const DsmFieldGrid &g, const uint8_t *state, const int32_t *dist,
+                             const int3 s, float radius, int approach, int n_goals, const uint8_t *frontier_res, int frontier_max_clusters,
+                             cudaStream_t st);

@@ -1,0 +1,468 @@
+// Travel cost through known free space (dsm_reach_*, DESIGN.md §8.11): the cost to go from a start voxel to every
+// traversable voxel of the latest known field, the viewpoints of goals and frontier clusters, and their paths.
+//
+//   k_reach_start    one warp: snaps the start into its approach window, fills the header's start and target counts,
+//                    copies the field's error words and schedules the start's tile for round 0.
+//   k_reach_init     one thread per voxel: the traversable grid (free and dist >= radius), both cost buffers at
+//                    UINT32_MAX but the start at 0, and the traversable count.
+//   k_reach_round    launched max_rounds times; a fixed set of persistent CTAs walks round r's schedule, one 8x8x8 tile
+//                    per CTA of 512 threads, one voxel per thread.  The tile and its one-voxel halo are staged in shared
+//                    memory from buffer r % 2; Bellman-Ford sweeps in place run until __syncthreads_or reports no change
+//                    (the tile-local fixed point with the halo frozen, unique whatever the interleaving); the tile is
+//                    written to buffer (r + 1) % 2, and a tile that changed schedules itself and its 26 neighbours for
+//                    round r + 1, a stamp per tile keeping each listed once; round 0's tile, the start's, counts as changed.  A round with an empty schedule exits at once.
+//   k_reach_settle   copies the tiles of the pending schedule (non-empty only when max_rounds cut the job) into the other
+//                    buffer, so both hold the latest cost of every voxel and the kernels below read buffer 0.
+//   k_reach_reached  the reached count and the converged flag.
+//   k_reach_targets  one warp per goal and per member of the frontier list: the window's best (cost + chamfer, voxel)
+//                    by a 64-bit atomicMin; a second pass picks the lowest member attaining a cluster's minimum.
+//   k_reach_records  one thread per target record.
+//   k_reach_paths    one warp per reached target, lanes on the 26 neighbours and a shuffle argmin per step: a counting
+//                    walk, a cub exclusive scan of the lengths, then the writing walk.
+// The kernels carry no error gate and are launched without PDL, as the other field kernels.
+#include "dsm_device.cuh"
+#include <algorithm>
+#include <cub/device/device_scan.cuh>
+
+#define RC_BLOCK 256
+#define RC_T DSM_REACH_TILE
+#define RC_TILE (RC_T * RC_T * RC_T) // 512 threads
+#define RC_H (RC_T + 2)              // the staged tile with its halo
+#define RC_INF 0xffffffffu
+
+static_assert(sizeof(dsm_reach_target_t) == 32 && sizeof(dsm_reach_info_t) == 64, "dsm_reach layouts");
+static_assert(DSM_REACH_N_PATH_VOXELS == 13 && DSM_REACH_WORDS * 4 == sizeof(dsm_reach_info_t), "the header starts with the info");
+static_assert(DSM_FRONTIER_N_LISTED == 3 && DSM_FRONTIER_N_CLUSTERS == 2, "frontier header words");
+
+// the cost of a move or an offset: 10 a + 4 b + 3 c for the sorted absolute components a >= b >= c
+__host__ __device__ __forceinline__ int reach_chamfer(int dx, int dy, int dz)
+{
+    dx = abs(dx), dy = abs(dy), dz = abs(dz);
+    const int a = max(dx, max(dy, dz)), c = min(dx, min(dy, dz)), b = dx + dy + dz - a - c;
+    return 10 * a + 4 * b + 3 * c;
+}
+
+__device__ __forceinline__ bool reach_inside(const DsmFieldGrid &g, int x, int y, int z)
+{
+    return (unsigned)x < (unsigned)g.n[0] && (unsigned)y < (unsigned)g.n[1] && (unsigned)z < (unsigned)g.n[2];
+}
+__device__ __forceinline__ int reach_index(const DsmFieldGrid &g, int x, int y, int z) { return (z * g.n[1] + y) * g.n[0] + x; }
+
+__device__ __forceinline__ unsigned long long warp_min64(unsigned long long v)
+{
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1)
+    {
+        const unsigned long long w = __shfl_xor_sync(0xffffffffu, v, o);
+        v = w < v ? w : v;
+    }
+    return v;
+}
+
+__device__ __forceinline__ bool traversable(const uint8_t *state, const int32_t *dist, int i, float radius)
+{
+    return state[i] == DSM_STATE_FREE && __int_as_float(dist[i]) >= radius;
+}
+
+__global__ void __launch_bounds__(32) k_reach_start(const DsmFieldGrid g, const uint8_t *__restrict__ state, const int32_t *__restrict__ dist,
+                                                    const int32_t *__restrict__ fhdr, const int3 s, float radius, int k, int n_goals,
+                                                    int max_targets, const int32_t *__restrict__ frontier_hdr, int frontier_max_clusters,
+                                                    const int3 tn, int32_t *__restrict__ sched0, int32_t *__restrict__ stamp,
+                                                    int32_t *__restrict__ count, int32_t *__restrict__ hdr)
+{
+    const int lane = threadIdx.x;
+    const int w = 2 * k + 1;
+    unsigned long long key = ~0ull;
+    const bool in = reach_inside(g, s.x, s.y, s.z);
+    if (in)
+        for (int q = lane; q < w * w * w; q += 32)
+        {
+            const int dx = q % w - k, dy = q / w % w - k, dz = q / (w * w) - k;
+            const int x = s.x + dx, y = s.y + dy, z = s.z + dz;
+            if (!reach_inside(g, x, y, z)) continue;
+            const int i = reach_index(g, x, y, z);
+            if (!traversable(state, dist, i, radius)) continue;
+            const unsigned long long c = ((unsigned long long)reach_chamfer(dx, dy, dz) << 32) | (unsigned)i;
+            key = c < key ? c : key;
+        }
+    key = warp_min64(key);
+    if (lane != 0) return;
+    const int u = key == ~0ull ? -1 : (int)(unsigned)key;
+    for (int d = 0; d < 3; d++) hdr[DSM_REACH_ORIGIN + d] = g.o[d];
+    hdr[DSM_REACH_START_VOXEL] = u;
+    hdr[DSM_REACH_START_STATUS] = !in ? 1 : u < 0 ? 2 : 0;
+    hdr[DSM_REACH_START_APPROACH] = u < 0 ? 0 : (int)(key >> 32);
+    const int n_clusters = frontier_hdr ? min(frontier_hdr[DSM_FRONTIER_N_CLUSTERS], frontier_max_clusters) : 0;
+    hdr[DSM_REACH_N_GOALS] = n_goals;
+    hdr[DSM_REACH_N_CLUSTERS_TOTAL] = n_clusters;
+    hdr[DSM_REACH_N_TARGETS] = n_goals + min(n_clusters, max_targets - n_goals);
+    hdr[DSM_REACH_ERR_TAG] = fhdr[DSM_FIELD_ERR_TAG];
+    hdr[DSM_REACH_ERR_FRAME] = fhdr[DSM_FIELD_ERR_FRAME];
+    count[1] = count[2] = 0;
+    count[0] = u >= 0;
+    if (u >= 0)
+    {
+        const int x = u % g.n[0], y = u / g.n[0] % g.n[1], z = u / (g.n[0] * g.n[1]);
+        const int t = ((z / RC_T) * tn.y + y / RC_T) * tn.x + x / RC_T;
+        sched0[0] = t;
+        stamp[t] = 0;
+    }
+}
+
+__global__ void __launch_bounds__(RC_BLOCK) k_reach_init(const uint8_t *__restrict__ state, const int32_t *__restrict__ dist, int voxels,
+                                                         float radius, uint8_t *__restrict__ trav, uint32_t *__restrict__ c0,
+                                                         uint32_t *__restrict__ c1, int32_t *hdr)
+{
+    const int i = blockIdx.x * RC_BLOCK + threadIdx.x;
+    const bool t = i < voxels && traversable(state, dist, i, radius);
+    if (i < voxels)
+    {
+        const uint32_t c = i == hdr[DSM_REACH_START_VOXEL] ? 0u : RC_INF;
+        trav[i] = t;
+        c0[i] = c;
+        c1[i] = c;
+    }
+    const int n = __syncthreads_count(t);
+    if (threadIdx.x == 0 && n > 0) atomicAdd(&hdr[DSM_REACH_N_TRAVERSABLE], n);
+}
+
+__global__ void __launch_bounds__(RC_TILE) k_reach_round(const DsmFieldGrid g, const int3 tn, const uint8_t *__restrict__ trav,
+                                                         const uint32_t *__restrict__ cin, uint32_t *__restrict__ cout,
+                                                         const int32_t *__restrict__ sched_in, int32_t *__restrict__ sched_out,
+                                                         int32_t *__restrict__ stamp, int32_t *count, int32_t *hdr, int r)
+{
+    __shared__ uint32_t s[RC_H * RC_H * RC_H];
+    const int n = count[r % 3];
+    if (blockIdx.x == 0 && threadIdx.x == 0)
+    {
+        count[(r + 2) % 3] = 0; // round r - 1's count; round r + 1 adds to it
+        if (n > 0) hdr[DSM_REACH_ROUNDS] = r + 1;
+    }
+    if (n == 0) return;
+    const int t = threadIdx.x, lx = t % RC_T, ly = t / RC_T % RC_T, lz = t / (RC_T * RC_T);
+    const int si = ((lz + 1) * RC_H + ly + 1) * RC_H + lx + 1;
+    volatile uint32_t *vs = s;
+    for (int q = blockIdx.x; q < n; q += gridDim.x)
+    {
+        const int tile = sched_in[q];
+        const int tx = tile % tn.x, ty = tile / tn.x % tn.y, tz = tile / (tn.x * tn.y);
+        const int x0 = tx * RC_T - 1, y0 = ty * RC_T - 1, z0 = tz * RC_T - 1;
+        for (int h = t; h < RC_H * RC_H * RC_H; h += RC_TILE)
+        {
+            const int x = x0 + h % RC_H, y = y0 + h / RC_H % RC_H, z = z0 + h / (RC_H * RC_H);
+            s[h] = reach_inside(g, x, y, z) ? cin[reach_index(g, x, y, z)] : RC_INF;
+        }
+        const int x = x0 + 1 + lx, y = y0 + 1 + ly, z = z0 + 1 + lz;
+        const bool inside = reach_inside(g, x, y, z);
+        const int i = inside ? reach_index(g, x, y, z) : 0;
+        const bool tv = inside && trav[i];
+        __syncthreads();
+        const uint32_t c0 = s[si];
+        uint32_t c = c0;
+        while (true)
+        { // only traversable voxels ever hold a finite cost, so a finite neighbour is a traversable one
+            bool changed = false;
+            if (tv)
+            {
+                uint32_t best = c;
+#pragma unroll
+                for (int dz = -1; dz <= 1; dz++)
+#pragma unroll
+                    for (int dy = -1; dy <= 1; dy++)
+#pragma unroll
+                        for (int dx = -1; dx <= 1; dx++)
+                        {
+                            if (dx == 0 && dy == 0 && dz == 0) continue;
+                            const uint32_t v = vs[si + (dz * RC_H + dy) * RC_H + dx];
+                            const uint32_t w = (uint32_t)reach_chamfer(dx, dy, dz);
+                            if (v != RC_INF && v + w < best) best = v + w;
+                        }
+                if (best < c)
+                {
+                    c = best;
+                    vs[si] = c;
+                    changed = true;
+                }
+            }
+            if (!__syncthreads_or(changed)) break;
+        }
+        if (inside) cout[i] = c;
+        // round 0's only tile holds the seeded start: it counts as changed even when none of its other voxels is reached,
+        // or a start cut off from the rest of its tile would end the job after one round
+        if ((__syncthreads_or(c != c0) || r == 0) && t < 27)
+        {
+            const int ax = tx + t % 3 - 1, ay = ty + t / 3 % 3 - 1, az = tz + t / 9 - 1;
+            if ((unsigned)ax < (unsigned)tn.x && (unsigned)ay < (unsigned)tn.y && (unsigned)az < (unsigned)tn.z)
+            {
+                const int a = (az * tn.y + ay) * tn.x + ax;
+                if (atomicMax(&stamp[a], r + 1) < r + 1) sched_out[atomicAdd(&count[(r + 1) % 3], 1)] = a;
+            }
+        }
+        __syncthreads(); // the next tile overwrites s
+    }
+}
+
+__global__ void __launch_bounds__(RC_TILE) k_reach_settle(const DsmFieldGrid g, const int3 tn, const uint32_t *__restrict__ src,
+                                                          uint32_t *__restrict__ dst, const int32_t *__restrict__ sched, const int32_t *count, int r)
+{
+    const int n = count[r % 3];
+    const int t = threadIdx.x, lx = t % RC_T, ly = t / RC_T % RC_T, lz = t / (RC_T * RC_T);
+    for (int q = blockIdx.x; q < n; q += gridDim.x)
+    {
+        const int tile = sched[q];
+        const int x = tile % tn.x * RC_T + lx, y = tile / tn.x % tn.y * RC_T + ly, z = tile / (tn.x * tn.y) * RC_T + lz;
+        if (reach_inside(g, x, y, z))
+        {
+            const int i = reach_index(g, x, y, z);
+            dst[i] = src[i];
+        }
+    }
+}
+
+__global__ void __launch_bounds__(RC_BLOCK) k_reach_reached(const uint32_t *__restrict__ cost, int voxels, const int32_t *count, int max_rounds, int32_t *hdr)
+{
+    const int i = blockIdx.x * RC_BLOCK + threadIdx.x;
+    if (blockIdx.x == 0 && threadIdx.x == 0) hdr[DSM_REACH_CONVERGED] = count[max_rounds % 3] == 0;
+    const int n = __syncthreads_count(i < voxels && cost[i] != RC_INF);
+    if (threadIdx.x == 0 && n > 0) atomicAdd(&hdr[DSM_REACH_N_REACHED], n);
+}
+
+// the frontier table's cluster whose listed members hold list entry j (the listed clusters are a prefix of the table
+// with rising offsets), or -1
+__device__ __forceinline__ int reach_cluster_of(const dsm_frontier_cluster_t *table, int n, int j)
+{
+    int lo = 0, hi = n; // the last c with offset in [0, j]
+    while (lo < hi)
+    {
+        const int m = (lo + hi) / 2;
+        const int o = table[m].offset;
+        if (o >= 0 && o <= j)
+            lo = m + 1;
+        else
+            hi = m;
+    }
+    const int c = lo - 1;
+    return c >= 0 && j < table[c].offset + table[c].n_voxels ? c : -1;
+}
+
+// the window's least (cost[u] + chamfer(g - u)) << 32 | u over reached voxels u, on the whole warp
+__device__ __forceinline__ unsigned long long reach_window(const DsmFieldGrid &g, const uint8_t *trav, const uint32_t *cost, int gx, int gy,
+                                                           int gz, int k, int lane)
+{
+    const int w = 2 * k + 1;
+    unsigned long long key = ~0ull;
+    for (int q = lane; q < w * w * w; q += 32)
+    {
+        const int dx = q % w - k, dy = q / w % w - k, dz = q / (w * w) - k;
+        const int x = gx + dx, y = gy + dy, z = gz + dz;
+        if (!reach_inside(g, x, y, z)) continue;
+        const int i = reach_index(g, x, y, z);
+        const uint32_t c = cost[i];
+        if (!trav[i] || c == RC_INF) continue;
+        const unsigned long long v = ((unsigned long long)(c + (uint32_t)reach_chamfer(dx, dy, dz)) << 32) | (unsigned)i;
+        key = v < key ? v : key;
+    }
+    return warp_min64(key);
+}
+
+template <int PASS>
+__global__ void __launch_bounds__(RC_BLOCK) k_reach_targets(const DsmFieldGrid g, const uint8_t *__restrict__ trav, const uint32_t *__restrict__ cost,
+                                                            const int32_t *__restrict__ goals, const int32_t *__restrict__ fhdr,
+                                                            const dsm_frontier_cluster_t *__restrict__ table, const int32_t *__restrict__ list,
+                                                            int k, const int32_t *__restrict__ hdr, unsigned long long *best, int32_t *member)
+{
+    const int lane = threadIdx.x & 31;
+    const int n_goals = hdr[DSM_REACH_N_GOALS], n_cl = hdr[DSM_REACH_N_TARGETS] - n_goals;
+    const int n_members = n_cl > 0 ? fhdr[DSM_FRONTIER_N_LISTED] : 0;
+    const int warps = gridDim.x * (RC_BLOCK / 32);
+    for (int item = blockIdx.x * (RC_BLOCK / 32) + (threadIdx.x >> 5); item < n_goals + n_members; item += warps)
+    {
+        int tg, gx, gy, gz, gi = 0;
+        if (item < n_goals)
+        {
+            if (PASS == 1) continue; // a goal is its own target voxel
+            tg = item;
+            gx = goals[3 * item], gy = goals[3 * item + 1], gz = goals[3 * item + 2];
+            if (!reach_inside(g, gx, gy, gz)) continue;
+        }
+        else
+        {
+            const int j = item - n_goals;
+            const int c = reach_cluster_of(table, n_cl, j);
+            if (c < 0) continue; // a member of a cluster past max_targets
+            tg = n_goals + c;
+            gi = list[j];
+            gx = gi % g.n[0], gy = gi / g.n[0] % g.n[1], gz = gi / (g.n[0] * g.n[1]);
+        }
+        const unsigned long long key = reach_window(g, trav, cost, gx, gy, gz, k, lane);
+        if (lane != 0 || key == ~0ull) continue;
+        if (PASS == 0)
+            atomicMin(&best[tg], key);
+        else if (key == best[tg])
+            atomicMin(&member[tg], gi);
+    }
+}
+
+__global__ void __launch_bounds__(RC_BLOCK) k_reach_records(const DsmFieldGrid g, const uint32_t *__restrict__ cost, const int32_t *__restrict__ goals,
+                                                            const dsm_frontier_cluster_t *__restrict__ table, const unsigned long long *__restrict__ best,
+                                                            const int32_t *__restrict__ member, const int32_t *__restrict__ hdr,
+                                                            dsm_reach_target_t *__restrict__ out)
+{
+    const int t = blockIdx.x * RC_BLOCK + threadIdx.x;
+    const int n_goals = hdr[DSM_REACH_N_GOALS];
+    if (t >= hdr[DSM_REACH_N_TARGETS]) return;
+    dsm_reach_target_t r;
+    int status;
+    const unsigned long long b = best[t];
+    if (t < n_goals)
+    {
+        const int x = goals[3 * t], y = goals[3 * t + 1], z = goals[3 * t + 2];
+        const bool in = reach_inside(g, x, y, z);
+        r.target = in ? reach_index(g, x, y, z) : -1;
+        status = !in ? 1 : b == ~0ull ? 2 : 0;
+    }
+    else
+    {
+        const dsm_frontier_cluster_t &c = table[t - n_goals];
+        status = c.offset < 0 ? 3 : b == ~0ull ? 2 : 0;
+        r.target = status == 0 ? member[t] : c.first;
+    }
+    const int u = (int)(unsigned)b;
+    r.cost = status == 0 ? (uint32_t)(b >> 32) : RC_INF;
+    r.approach = status == 0 ? (int)(r.cost - cost[u]) : -1;
+    r.viewpoint = status == 0 ? u : -1;
+    r.path_offset = -1;
+    r.path_len = 0;
+    r.status = status;
+    r.reserved = 0;
+    out[t] = r;
+}
+
+// the walk's next voxel from x (cost cx > 0): the traversable neighbour p minimising (cost[p] + w(p, x), p), on the
+// whole warp (lane l < 26 takes the l-th neighbour); -1 when none has a lower cost (a walk never meets that)
+__device__ __forceinline__ int reach_step(const DsmFieldGrid &g, const uint8_t *trav, const uint32_t *cost, int x, uint32_t cx, int lane)
+{
+    const int d = lane < 13 ? lane : lane + 1; // 0 .. 26 without the centre, 13
+    const int dx = d % 3 - 1, dy = d / 3 % 3 - 1, dz = d / 9 - 1;
+    const int px = x % g.n[0] + dx, py = x / g.n[0] % g.n[1] + dy, pz = x / (g.n[0] * g.n[1]) + dz;
+    unsigned long long key = ~0ull;
+    if (lane < 26 && reach_inside(g, px, py, pz))
+    {
+        const int p = reach_index(g, px, py, pz);
+        const uint32_t c = cost[p];
+        if (trav[p] && c != RC_INF) key = ((unsigned long long)c + (unsigned)reach_chamfer(dx, dy, dz)) << 32 | (unsigned)p;
+    }
+    key = warp_min64(key);
+    if (key == ~0ull) return -1;
+    const int p = (int)(unsigned)key;
+    return cost[p] < cx ? p : -1;
+}
+
+// WRITE == false: len[t] = the walk's voxel count (0 unless status 0) for every t < max_targets.  WRITE: the record's
+// path fields, and the path start -> viewpoint at ofs[t] when it fits.
+template <bool WRITE>
+__global__ void __launch_bounds__(RC_BLOCK) k_reach_paths(const DsmFieldGrid g, const uint8_t *__restrict__ trav, const uint32_t *__restrict__ cost,
+                                                          int max_targets, int max_path, long long *len, const long long *__restrict__ ofs,
+                                                          dsm_reach_target_t *rec, int32_t *__restrict__ path, int32_t *hdr)
+{
+    const int lane = threadIdx.x & 31;
+    const int warps = gridDim.x * (RC_BLOCK / 32), n_targets = hdr[DSM_REACH_N_TARGETS];
+    for (int t = blockIdx.x * (RC_BLOCK / 32) + (threadIdx.x >> 5); t < max_targets; t += warps)
+    {
+        const bool reached = t < n_targets && rec[t].status == 0;
+        if (!WRITE && !reached)
+        {
+            if (lane == 0) len[t] = 0;
+            continue;
+        }
+        if (!reached) continue;
+        long long n = 0, at = 0;
+        bool listed = false;
+        if (WRITE)
+        {
+            n = len[t], at = ofs[t];
+            listed = at + n <= (long long)max_path;
+            if (lane == 0)
+            {
+                rec[t].path_len = (int)n;
+                rec[t].path_offset = listed ? (int)at : -1;
+                if (listed) atomicMax(&hdr[DSM_REACH_N_PATH_VOXELS], (int)(at + n));
+            }
+            if (!listed) continue;
+        }
+        int x = rec[t].viewpoint;
+        long long step = 0;
+        while (true)
+        {
+            if (WRITE && lane == 0) path[at + n - 1 - step] = x;
+            step++;
+            const uint32_t cx = cost[x];
+            if (cx == 0) break;
+            x = reach_step(g, trav, cost, x, cx, lane);
+            if (x < 0) break;
+            if (WRITE && step == n) break; // the counting walk stopped here
+        }
+        if (!WRITE && lane == 0) len[t] = step;
+    }
+}
+
+static unsigned rc_blocks(long long n) { return n > 0 ? (unsigned)((n + RC_BLOCK - 1) / RC_BLOCK) : 1u; }
+
+int dsm_reach_ctas()
+{
+    int dev = 0, sms = 0, per = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess ||
+        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per, k_reach_round, RC_TILE, 0) != cudaSuccess)
+        return 0;
+    return sms * per;
+}
+
+size_t dsm_reach_temp_bytes(const DsmReachBufs &b)
+{
+    size_t n = 0;
+    if (cub::DeviceScan::ExclusiveSum(nullptr, n, b.len, b.ofs, std::max(b.max_targets, 1), (cudaStream_t)0) != cudaSuccess) return 0;
+    return std::max(n, (size_t)1);
+}
+
+cudaError_t dsm_launch_reach(const DsmReachBufs &b, const DsmFieldGrid &g, const uint8_t *state, const int32_t *dist,
+                             const int3 s, float radius, int approach, int n_goals, const uint8_t *frontier_res, int frontier_max_clusters,
+                             cudaStream_t st)
+{
+    int32_t *hdr = reinterpret_cast<int32_t *>(b.res);
+    auto *rec = reinterpret_cast<dsm_reach_target_t *>(b.res + 4 * DSM_REACH_WORDS);
+    int32_t *path = reinterpret_cast<int32_t *>(b.res + 4 * DSM_REACH_WORDS + sizeof(dsm_reach_target_t) * (size_t)b.max_targets);
+    const int32_t *fhdr = reinterpret_cast<const int32_t *>(frontier_res);
+    const auto *table = frontier_res ? reinterpret_cast<const dsm_frontier_cluster_t *>(frontier_res + 4 * DSM_FRONTIER_WORDS) : nullptr;
+    const int32_t *list = frontier_res ? reinterpret_cast<const int32_t *>(frontier_res + 4 * DSM_FRONTIER_WORDS +
+                                                                         sizeof(dsm_frontier_cluster_t) * (size_t)frontier_max_clusters)
+                                       : nullptr;
+    const int3 tn = make_int3(b.tn[0], b.tn[1], b.tn[2]);
+    const int32_t *fieldhdr = dist + dsm_field_header((size_t)b.voxels);
+    cudaError_t e = cudaMemsetAsync(b.stamp, 0xff, 4 * (size_t)b.tiles, st);
+    if (e == cudaSuccess && b.max_targets > 0) e = cudaMemsetAsync(b.best, 0xff, 8 * (size_t)b.max_targets, st);
+    if (e == cudaSuccess && b.max_targets > 0) e = cudaMemsetAsync(b.member, 0x7f, 4 * (size_t)b.max_targets, st);
+    if (e != cudaSuccess) return e;
+    k_reach_start<<<1, 32, 0, st>>>(g, state, dist, fieldhdr, s, radius, approach, n_goals, b.max_targets, fhdr, frontier_max_clusters, tn,
+                                    b.sched[0], b.stamp, b.count, hdr);
+    k_reach_init<<<rc_blocks(b.voxels), RC_BLOCK, 0, st>>>(state, dist, b.voxels, radius, b.trav, b.cost[0], b.cost[1], hdr);
+    for (int r = 0; r < b.max_rounds; r++)
+        k_reach_round<<<b.ctas, RC_TILE, 0, st>>>(g, tn, b.trav, b.cost[r % 2], b.cost[(r + 1) % 2], b.sched[r % 2], b.sched[(r + 1) % 2],
+                                                  b.stamp, b.count, hdr, r);
+    const int r = b.max_rounds;
+    k_reach_settle<<<b.ctas, RC_TILE, 0, st>>>(g, tn, b.cost[r % 2], b.cost[(r + 1) % 2], b.sched[r % 2], b.count, r);
+    k_reach_reached<<<rc_blocks(b.voxels), RC_BLOCK, 0, st>>>(b.cost[0], b.voxels, b.count, r, hdr);
+    e = cudaGetLastError();
+    if (e != cudaSuccess || b.max_targets == 0) return e;
+    const unsigned warp_blocks = 2 * (unsigned)b.ctas; // the target and path kernels' warps walk their work
+    k_reach_targets<0><<<warp_blocks, RC_BLOCK, 0, st>>>(g, b.trav, b.cost[0], b.goals, fhdr, table, list, approach, hdr, b.best, b.member);
+    if (frontier_res)
+        k_reach_targets<1><<<warp_blocks, RC_BLOCK, 0, st>>>(g, b.trav, b.cost[0], b.goals, fhdr, table, list, approach, hdr, b.best, b.member);
+    k_reach_records<<<rc_blocks(b.max_targets), RC_BLOCK, 0, st>>>(g, b.cost[0], b.goals, table, b.best, b.member, hdr, rec);
+    k_reach_paths<false><<<warp_blocks, RC_BLOCK, 0, st>>>(g, b.trav, b.cost[0], b.max_targets, b.max_path, b.len, b.ofs, rec, path, hdr);
+    e = cudaGetLastError();
+    size_t n = b.temp_bytes;
+    if (e == cudaSuccess) e = cub::DeviceScan::ExclusiveSum(b.temp, n, b.len, b.ofs, b.max_targets, st);
+    if (e != cudaSuccess) return e;
+    k_reach_paths<true><<<warp_blocks, RC_BLOCK, 0, st>>>(g, b.trav, b.cost[0], b.max_targets, b.max_path, b.len, b.ofs, rec, path, hdr);
+    return cudaGetLastError();
+}

@@ -659,6 +659,96 @@ int dsm_frontier_enqueue(dsm_ctx *ctx, int min_voxels);
 int dsm_frontier_wait(dsm_ctx *ctx, const dsm_frontier_cluster_t **clusters, const int32_t **voxels, dsm_frontier_counts_t *counts);
 int dsm_debug_field_load_state(dsm_ctx *ctx, const uint8_t *state, const int32_t origin[3]);
 
+/* ---- paths through known free space: travel cost from a start to every voxel, goals and frontiers (DESIGN.md §8.11) ----
+ * A reach job reads the state grid and the distance grid of the latest field request, which must be a known one, in
+ * stream order behind it, with that request's origin o and voxel edge v captured at the job's enqueue, and (with
+ * with_frontiers) the result of the latest frontier job.  A later field or frontier request may be enqueued while a job
+ * is in flight and does not change what the job reads.  The map is never read.  Linear index (z * ny + y) * nx + x.
+ *
+ * Definition (integer costs, so a converged result does not depend on the schedule, and the round rule below fixes an
+ * unconverged one as well).
+ *   Traversable: state 2 (free) and dist >= radius, compared in fp32 on the stored distance (metres).  The known
+ *   distance measures to the nearest unknown or occupied voxel inside the grid; voxels outside the grid are not seen by
+ *   the field, so clearance near the box's faces counts only what is inside.
+ *   Moves: the 26-connected moves between traversable voxels, in units of v / 10: face 10, edge 14, corner 17.  In free
+ *   space an offset with sorted absolute components a >= b >= c costs chamfer = 10 a + 4 b + 3 c, between 0.98 and 1.12
+ *   times its length.  Costs are uint32; UINT32_MAX is "not reached".
+ *   Window of voxel g: the Chebyshev box of radius approach (an integer k in [0, 4]) around g, clipped to the grid.
+ *   Start: s_k = floor(p_k / (double)v) - o_k of the fp64 start point p.  The job starts from the traversable voxel u
+ *   in the window of s minimising (chamfer(u - s), u), which gets cost 0.  start_status 0 such a voxel, 1 s outside the
+ *   grid, 2 no traversable voxel in the window; with 1 or 2 nothing is reached.
+ *   Cost to go: cost[x] is the least sum of move weights over paths of traversable voxels from u to x (Dijkstra's).
+ *   Rounds: the grid is cut into 8x8x8 tiles from voxel (0, 0, 0), edge tiles clipped.  Round 0 schedules u's tile.  In
+ *   round r every scheduled tile reads its voxels and its one-voxel halo from buffer r % 2, relaxes to the tile-local
+ *   fixed point with the halo frozen and writes its voxels to buffer (r + 1) % 2; a tile that changed a voxel schedules
+ *   itself and its 26 neighbour tiles for round r + 1.  The seeded start is round 0's change: u's tile schedules its
+ *   neighbours even when no other voxel of it is reached, since u may reach the grid only across the tile's faces.  rounds counts the rounds with a non-empty schedule; the job is
+ *   converged when the last of them changed nothing, and stops after max_rounds.  A converged job's costs are
+ *   Dijkstra's; an unconverged one's are the latest value of every voxel, each >= the exact cost.
+ *   Targets: the goals, then (with_frontiers) the clusters of the latest frontier job's table in table order; the table
+ *   holds the first max_targets of them.  For a target voxel g (a goal's voxel, or every member of a cluster) the
+ *   viewpoint is the traversable, reached voxel u in the window of g minimising (cost[u] + chamfer(g - u), u); for a
+ *   cluster the minimum runs over its members too, ties going to the lowest member.  A record holds cost = cost[u] +
+ *   approach, approach = chamfer(g - u), target g, the viewpoint u and the path's offset and length.  status 0 reached,
+ *   1 goal outside the grid, 2 nothing reached in the window, 3 a cluster without members in the frontier list (its
+ *   offset is -1).  A record of status != 0 has cost UINT32_MAX, approach, viewpoint and path_offset -1 and path_len 0;
+ *   its target is the goal's voxel (-1 outside the grid) or the cluster's first voxel.
+ *   Paths: from the viewpoint, step to the traversable neighbour p minimising (cost[p] + w(p, x), p) until the start;
+ *   on a converged grid that is a tight predecessor.  Every finite cost was written as a neighbour's earlier cost plus a
+ *   weight and costs only fall, so the cost falls at every step of an unconverged grid too and the walk ends, with a
+ *   weight sum between the exact cost and the reported one.  The list holds the paths start -> viewpoint as linear
+ *   indices, in table order; path_offset is the exclusive prefix sum of path_len, or -1 once offset + path_len would pass
+ *   max_path_voxels, so the listed paths are a prefix of the reached targets.
+ *   Header: the origin; start_voxel u (-1 without one), start_status, start_approach chamfer(u - s) (0 without one);
+ *   rounds and converged; n_traversable voxels and n_reached voxels of finite cost; n_goals, n_clusters_total the
+ *   frontier table's entries (0 without with_frontiers; those past max_targets are dropped), n_targets the records and
+ *   n_path_voxels the listed path voxels.
+ *
+ *   dsm_reach_enable    once, after dsm_views_enable (DSM_E_STATE otherwise, and when called twice).  DSM_E_INVALID for
+ *                       a capacity that is negative or above 2^26, max_rounds outside [1, 65536], or a grid above 2^27
+ *                       voxels (so that 17 (N - 1) plus an approach fits in 32 bits).  Allocates a traversable byte grid,
+ *                       two cost grids (4 B per voxel each), the tile stamps and schedules, the device result and its
+ *                       pinned copy of 64 + 32 max_targets + 4 max_path_voxels bytes, a pinned cost-grid copy, the goal
+ *                       staging and an event.  DSM_E_NOMEM with nothing kept.
+ *   dsm_reach_enqueue   asynchronous on the context's stream, never waits: the goals (n_goals x 3 doubles, may be NULL
+ *                       for 0) staged into pinned memory and copied with one H2D copy, the kernels (max_rounds round
+ *                       launches; a round with an empty schedule exits at once), one D2H copy of the result capacity,
+ *                       with host_copy the cost grid as well, and the event.  DSM_E_STATE before dsm_reach_enable, before
+ *                       any field request, when the latest field request is not a known one, while a job is in flight,
+ *                       and with with_frontiers when the latest frontier job was not enqueued on the latest field
+ *                       request (or there is none).  DSM_E_INVALID for a non-finite start or goal, a radius that is not
+ *                       finite and >= 0, an approach outside [0, 4], or n_goals outside [0, max_targets].
+ *   dsm_reach_wait      waits for that job only.  *targets (n_targets records), *path (n_path_voxels) and *cost (the
+ *                       grid [z][y][x], NULL without host_copy) are the context's pinned results, valid until the next
+ *                       dsm_reach_enqueue; any out-pointer may be NULL.  If the field the job read was taken after a
+ *                       rejected frame, returns DSM_E_CAPACITY with valid results and does NOT clear the error, as
+ *                       dsm_field_wait.  DSM_E_STATE with no job enqueued. */
+typedef struct dsm_reach_target_t
+{
+    uint32_t cost;                   /* cost[viewpoint] + approach, units of v / 10; UINT32_MAX unless status 0 */
+    int32_t approach, target, viewpoint;
+    int32_t path_offset, path_len;   /* into the path list, -1 when the path is not in it */
+    int32_t status, reserved;        /* reserved 0 */
+} dsm_reach_target_t;                /* 32 B */
+typedef struct dsm_reach_info_t
+{
+    int32_t origin[3];
+    int32_t start_voxel, start_status, start_approach;
+    int32_t rounds, converged;
+    int32_t n_traversable, n_reached;
+    int32_t n_goals, n_clusters_total, n_targets, n_path_voxels;
+    int32_t reserved[2];
+} dsm_reach_info_t;                  /* 64 B */
+#define DSM_REACH_MAX_CAPACITY (1 << 26)
+#define DSM_REACH_MAX_ROUNDS 65536
+#define DSM_REACH_MAX_VOXELS (1 << 27)
+#define DSM_REACH_MAX_APPROACH 4
+int dsm_reach_enable(dsm_ctx *ctx, int max_targets, int max_path_voxels, int max_rounds);
+int dsm_reach_enqueue(dsm_ctx *ctx, const double start[3], float radius, int approach, const double *goals, int n_goals,
+                      int with_frontiers, int host_copy);
+int dsm_reach_wait(dsm_ctx *ctx, dsm_reach_info_t *info, const dsm_reach_target_t **targets, const int32_t **path,
+                   const uint32_t **cost);
+
 /* ---- checkpoints that do not stop the stream (DESIGN.md §8.5) ----
  * The file of dsm_map_save, taken in stream order like a publish snapshot: the resident stream pays one device-to-device
  * copy of the live map, the transfer to the host runs on a low-priority stream beside the next frames, and a thread of

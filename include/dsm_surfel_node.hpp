@@ -79,6 +79,10 @@
 // lets frontiers() find the exploration frontiers of the latest fused frame's known field on the device (DESIGN.md
 // §8.10): the clusters of free voxels that border unknown space, their statistics and member voxels, one enqueue and one
 // wait, without touching the one-frame-late distance_field() handout.
+// Which frontier is worth the trip?  enable_reach(max_targets, max_path_voxels, max_rounds), after enable_known_space,
+// lets reach() find paths through the known free space of the latest fused frame's field on the device (DESIGN.md
+// §8.11): the travel cost from a start point to goal points and, after a frontiers() call on that frame, to every
+// frontier cluster, with each target's viewpoint and path, one enqueue and one wait.
 // device < 0 builds the node without a context: the callbacks run the whole pose logic (pose database, sync, window
 // bookkeeping) and fuse nothing; any call that reads the map returns DSM_E_STATE.
 #pragma once
@@ -546,6 +550,42 @@ class SurfelMapNode
             voxels.assign(v, v + counts.n_listed);
         }
         return ctx_.done(rc, "frontiers");
+    }
+
+    // ---- paths through the known free space of the latest fused frame's field (DESIGN.md §8.11) ----
+    // once, after enable_known_space: the capacities of the target table and the path list, and the rounds of a job
+    int enable_reach(int max_targets, int max_path_voxels, int max_rounds)
+    {
+        if (ctx_.run("enable_reach", [&] { return dsm_reach_enable(ctx_.ctx, max_targets, max_path_voxels, max_rounds); }) == DSM_OK)
+            reach_targets_ = max_targets;
+        return ctx_.err;
+    }
+    // the travel cost from `start` through voxels free and at least `radius` from anything not known to be free, to the
+    // goals (xyz doubles, goals.size() / 3 of them) and, with with_frontiers, to the clusters the frontiers() call on
+    // this frame found (include/dsm.h): targets receives info.n_targets records and path info.n_path_voxels indices.
+    // DSM_E_STATE without known space, before any field, after load_state* until the next fused frame, and with
+    // with_frontiers without a frontiers() call since the frame was fused; DSM_E_CAPACITY with the paths of the last
+    // applied frame's field, as distance_field().
+    int reach(const double start[3], float radius, int approach, const std::vector<double> &goals, bool with_frontiers, dsm_reach_info_t &info,
+              std::vector<dsm_reach_target_t> &targets, std::vector<int32_t> &path)
+    {
+        targets.clear();
+        path.clear();
+        info = dsm_reach_info_t();
+        if (!ctx_.ready("reach")) return ctx_.err;
+        if (known_.empty() || !field_exists_) return ctx_.done(DSM_E_STATE, "reach");
+        if (goals.size() % 3 != 0) return ctx_.done(DSM_E_INVALID, "reach");
+        int rc = dsm_reach_enqueue(ctx_.ctx, start, radius, approach, goals.data(), (int)(goals.size() / 3), with_frontiers, 0);
+        if (rc != DSM_OK) return ctx_.done(rc, "reach");
+        const dsm_reach_target_t *t = nullptr;
+        const int32_t *p = nullptr;
+        rc = dsm_reach_wait(ctx_.ctx, &info, &t, &p, nullptr);
+        if (rc == DSM_OK || rc == DSM_E_CAPACITY)
+        {
+            targets.assign(t, t + std::min(info.n_targets, reach_targets_));
+            path.assign(p, p + info.n_path_voxels);
+        }
+        return ctx_.done(rc, "reach");
     }
 
     // ---- planner queries against the field of the latest fused frame (DESIGN.md §8.8) ----
@@ -1080,5 +1120,6 @@ class SurfelMapNode
     std::vector<KnownView> known_; // empty without known space
     int captures_ = 0, captured_ref_ = -1; // captures so far; the reference keyframe of the latest
     int frontier_clusters_ = 0;            // enable_frontiers' max_clusters
+    int reach_targets_ = 0;                // enable_reach's max_targets
 };
 } // namespace dsm
