@@ -36,7 +36,7 @@ EXPORTS = [
     "dsm_field_enqueue_resident", "dsm_field_query_enable", "dsm_field_query_enqueue", "dsm_field_query_wait",
     "dsm_views_enable", "dsm_views_capture", "dsm_field_enqueue_known", "dsm_field_state",
     "dsm_frontier_enable", "dsm_frontier_enqueue", "dsm_frontier_wait", "dsm_debug_field_load_state",
-    "dsm_reach_enable", "dsm_reach_enqueue", "dsm_reach_wait",
+    "dsm_reach_enable", "dsm_reach_enqueue", "dsm_reach_wait", "dsm_gain_enable", "dsm_gain_enqueue", "dsm_gain_wait",
     "dsm_inactive_segments", "dsm_inactive_load", "dsm_map_save", "dsm_map_load", "dsm_map_peek",
     "dsm_checkpoint_enable", "dsm_checkpoint_enqueue", "dsm_checkpoint_wait", "dsm_debug_checkpoint_drain_ctas",
     "dsm_checkpoint_enqueue_incremental", "dsm_map_load_journal", "dsm_map_peek_journal", "dsm_journal_materialize",
@@ -75,6 +75,17 @@ REACH_INFO_DTYPE = np.dtype([("origin", "<i4", 3), ("start_voxel", "<i4"), ("sta
                              ("rounds", "<i4"), ("converged", "<i4"), ("n_traversable", "<i4"), ("n_reached", "<i4"),
                              ("n_goals", "<i4"), ("n_clusters_total", "<i4"), ("n_targets", "<i4"), ("n_path_voxels", "<i4"),
                              ("reserved", "<i4", 2)])
+# dsm_gain_wait's records (include/dsm.h): a view's gain (32 B) and the header (32 B)
+VIEW_GAIN_DTYPE = np.dtype([("n_frustum", "<i4"), ("n_free", "<i4"), ("n_unknown", "<i4"), ("n_occupied", "<i4"), ("n_frontier", "<i4"),
+                            ("n_cluster", "<i4"), ("status", "<i4"), ("reserved", "<i4")])
+GAIN_INFO_DTYPE = np.dtype([("origin", "<i4", 3), ("n_views", "<i4"), ("n_clusters_table", "<i4"), ("unknown_blocks", "<i4"),
+                            ("reserved", "<i4", 2)])
+
+
+class DsmGainCamera(ctypes.Structure):
+    """dsm_gain_camera_t (48 B): pinhole intrinsics, image size, range and the blocking rule of a gain job."""
+    _fields_ = [("fx", ctypes.c_double), ("fy", ctypes.c_double), ("cx", ctypes.c_double), ("cy", ctypes.c_double),
+                ("width", ctypes.c_int32), ("height", ctypes.c_int32), ("max_range", ctypes.c_float), ("unknown_blocks", ctypes.c_int32)]
 
 
 CONSTANTS_DRIVE = (0.4, 0.5, 4.0, 0.1)    # fusion_functions.h:13-16
@@ -147,6 +158,9 @@ def load_library():
     L.dsm_reach_enable.argtypes = [vp, ci, ci, ci]
     L.dsm_reach_enqueue.argtypes = [vp, ctypes.POINTER(ctypes.c_double), ctypes.c_float, ci, vp, ci, ci, ci]
     L.dsm_reach_wait.argtypes = [vp, vp, ctypes.POINTER(vp), ctypes.POINTER(vp), ctypes.POINTER(vp)]
+    L.dsm_gain_enable.argtypes = [vp, ci]
+    L.dsm_gain_enqueue.argtypes = [vp, ctypes.POINTER(DsmGainCamera), vp, vp, ci]
+    L.dsm_gain_wait.argtypes = [vp, vp, ctypes.POINTER(vp)]
     L.dsm_inactive_reserve.argtypes = [vp, ci]
     L.dsm_inactive_retire.argtypes = [vp, ci, ctypes.POINTER(ci)]
     L.dsm_inactive_reactivate.argtypes = [vp, ci, ctypes.POINTER(ci)]
@@ -715,6 +729,40 @@ class Context:
             err.reach = out
             raise err
         return out
+
+    # ---- view gain against the latest known field ----
+    def gain_enable(self, max_views):
+        self._ck(self.lib.dsm_gain_enable(self.h, int(max_views)))
+
+    def gain_enqueue(self, camera, poses, clusters=None):
+        """camera: (fx, fy, cx, cy, width, height, max_range, unknown_blocks); poses: (n, 12) row-major [R | t], camera to
+        world; clusters: n frontier-table indices (-1: none), or None when no view names a cluster."""
+        cam = DsmGainCamera(*[float(x) for x in camera[:4]], int(camera[4]), int(camera[5]), float(camera[6]), int(camera[7]))
+        P = np.ascontiguousarray(poses, np.float64).reshape(-1, 12)
+        c = None if clusters is None else np.ascontiguousarray(clusters, np.int32).reshape(-1)
+        if c is not None and len(c) != len(P):
+            raise ValueError(f"{len(c)} clusters for {len(P)} views")
+        self._ck(self.lib.dsm_gain_enqueue(self.h, ctypes.byref(cam), P.ctypes.data if len(P) else None,
+                                           None if c is None else c.ctypes.data, len(P)))
+
+    def gain_wait(self):
+        """(info, gains): numpy copies of the context's pinned results, a GAIN_INFO_DTYPE record and VIEW_GAIN_DTYPE
+        (n_views,).  A job on a field taken after a rejected frame raises DsmError(DSM_E_CAPACITY) carrying the same tuple
+        as `.gain`."""
+        pg = ctypes.c_void_p()
+        info = np.zeros(1, GAIN_INFO_DTYPE)
+        rc = self.lib.dsm_gain_wait(self.h, info.ctypes.data, ctypes.byref(pg))
+        if rc not in (DSM_OK, -6):
+            self._ck(rc)
+        i = info[0]
+        n = int(i["n_views"])
+        g = np.zeros(0, VIEW_GAIN_DTYPE) if n == 0 else np.frombuffer(
+            (ctypes.c_uint8 * (n * VIEW_GAIN_DTYPE.itemsize)).from_address(pg.value), dtype=VIEW_GAIN_DTYPE).copy()
+        if rc != DSM_OK:
+            err = DsmError(rc, self.lib.dsm_last_error(self.h).decode())
+            err.gain = (i, g)
+            raise err
+        return i, g
 
     # ---- planner queries against the latest field ----
     def field_query_enable(self, max_points, max_trajectories, max_waypoints):

@@ -1988,6 +1988,139 @@ extern "C" int dsm_reach_wait(dsm_ctx *ctx, dsm_reach_info_t *info, const dsm_re
     return DSM_E_CAPACITY;
 }
 
+// ---- view gain against the latest known field (include/dsm.h, DESIGN.md §8.12) ----
+extern "C" int dsm_gain_enable(dsm_ctx *ctx, int max_views)
+{
+    if (!ctx) return DSM_E_INVALID;
+    const DsmField *f = ctx->field.get();
+    if (!f || !ctx->views || ctx->gain) return DSM_E_STATE;
+    if (max_views < 1 || max_views > DSM_GAIN_MAX_VIEWS) return DSM_E_INVALID;
+    CK(cudaSetDevice(ctx->device));
+    auto ga = std::make_unique<DsmGain>();
+    ga->max_views = max_views;
+    const size_t res = DsmGain::res_bytes(max_views);
+    CudaOwner &o = ga->own;
+    cudaError_t e = o.device(&ga->views_dev, (size_t)max_views);
+    if (e == cudaSuccess) e = o.host(&ga->views_host, (size_t)max_views);
+    if (e == cudaSuccess) e = o.device(&ga->slot, f->voxels);
+    if (e == cudaSuccess) e = o.device(&ga->res, res);
+    if (e == cudaSuccess) e = o.host(&ga->res_host, res);
+    if (e == cudaSuccess) e = o.event(&ga->ev);
+    if (e != cudaSuccess)
+    {
+        cudaGetLastError();
+        return DSM_E_NOMEM; // nothing is kept: a later call may try again
+    }
+    ctx->gain = std::move(ga);
+    return DSM_OK;
+}
+
+// The grid voxels of view P's box: the bounding box of the image pyramid cut at depth max_range (the apex t and the
+// four image corners (0 | width, 0 | height) at depth max_range) met with the cube around the range sphere, one voxel
+// of padding, clipped to the grid.  Every centre that passes the frustum test lies in the truncated pyramid and in the
+// sphere, so the box sizes the work and cannot change a count.  The pyramid holds them only for a rotation: a pose whose
+// 3x3 part is not orthonormal within 1e-6 per entry of R^T R - I, or a corner that does not come out finite, leaves
+// the cube alone (within that tolerance the pyramid moves by far less than the padding).
+static void gain_box(const double *P, const dsm_gain_camera_t &c, const DsmFieldGrid &g, DsmGainView &V)
+{
+    const double R = (double)c.max_range, v = (double)g.voxel;
+    double plo[3], phi[3];
+    bool finite = true;
+    for (int a = 0; a < 3; a++)
+        for (int b = 0; b < 3; b++)
+            finite = finite && std::fabs(((P[a] * P[b] + P[4 + a] * P[4 + b]) + P[8 + a] * P[8 + b]) - (a == b ? 1.0 : 0.0)) <= 1e-6;
+    for (int k = 0; k < 3; k++) plo[k] = phi[k] = P[4 * k + 3];
+    for (int cu = 0; cu < 2; cu++)
+        for (int cw = 0; cw < 2; cw++)
+        {
+            const double qx = ((cu ? (double)c.width : 0.0) - c.cx) / c.fx * R, qy = ((cw ? (double)c.height : 0.0) - c.cy) / c.fy * R;
+            for (int k = 0; k < 3; k++)
+            {
+                const double p = ((P[4 * k] * qx + P[4 * k + 1] * qy) + P[4 * k + 2] * R) + P[4 * k + 3];
+                finite = finite && std::isfinite(p);
+                plo[k] = std::min(plo[k], p);
+                phi[k] = std::max(phi[k], p);
+            }
+        }
+    for (int k = 0; k < 3; k++)
+    {
+        double lo = P[4 * k + 3] - R, hi = P[4 * k + 3] + R;
+        if (finite) lo = std::max(lo, plo[k]), hi = std::min(hi, phi[k]);
+        const double a = std::max(std::floor(lo / v) - 1.0 - (double)g.o[k], 0.0);
+        const double b = std::min(std::floor(hi / v) + 1.0 - (double)g.o[k], (double)(g.n[k] - 1));
+        V.lo[k] = a <= b ? (int)a : 0;
+        V.size[k] = a <= b ? (int)(b - a) + 1 : 0;
+    }
+}
+
+// Enqueue only: the views staged (pose, box, cluster and first brick) and copied, the kernels on the state grid of the
+// latest (known) field request and, with clusters, on the latest frontier job's device result, one D2H copy of the used
+// result and the event.  Later field and frontier requests overwrite those buffers only behind the job.
+extern "C" int dsm_gain_enqueue(dsm_ctx *ctx, const dsm_gain_camera_t *camera, const double *poses, const int32_t *clusters, int n_views)
+{
+    if (!ctx) return DSM_E_INVALID;
+    DsmGain *ga = ctx->gain.get();
+    const DsmField *f = ctx->field.get();
+    if (!ga || !f || !f->requested || !f->known || ga->in_flight) return DSM_E_STATE;
+    const DsmFrontier *fr = ctx->frontier.get();
+    if (clusters && (!fr || fr->request != f->requests)) return DSM_E_STATE;
+    if (!camera || n_views < 0 || n_views > ga->max_views || (n_views > 0 && !poses)) return DSM_E_INVALID;
+    const dsm_gain_camera_t &c = *camera;
+    const double v = (double)f->g.voxel, R = (double)c.max_range;
+    if (!(std::isfinite(c.fx) && c.fx > 0.0 && std::isfinite(c.fy) && c.fy > 0.0 && std::isfinite(c.cx) && std::isfinite(c.cy)))
+        return DSM_E_INVALID;
+    if (c.width < 1 || c.width > 65536 || c.height < 1 || c.height > 65536 || (c.unknown_blocks != 0 && c.unknown_blocks != 1))
+        return DSM_E_INVALID;
+    if (!std::isfinite(R) || !(R > 0.0) || R > DSM_GAIN_MAX_RANGE_VOXELS * v) return DSM_E_INVALID;
+    const long long m = 2 * (long long)std::ceil(R / v) + 3;
+    if ((long long)n_views * m * m * m > DSM_GAIN_MAX_WORK) return DSM_E_INVALID;
+    for (size_t i = 0; i < 12 * (size_t)n_views; i++)
+        if (!std::isfinite(poses[i])) return DSM_E_INVALID;
+    if (clusters)
+        for (int j = 0; j < n_views; j++)
+            if (clusters[j] < -1) return DSM_E_INVALID;
+    CK(cudaSetDevice(ctx->device));
+    // the previous job's copy out of this staging ended before its wait, which no job in flight implies
+    long long bricks = 0;
+    for (int j = 0; j < n_views; j++)
+    {
+        DsmGainView &V = ga->views_host[j];
+        std::memcpy(V.P, poses + 12 * (size_t)j, sizeof(V.P));
+        gain_box(V.P, c, f->g, V);
+        V.cluster = clusters ? clusters[j] : -1;
+        V.brick0 = (int)bricks; // below 2^31: the work bound caps the bricks far lower
+        bricks += dsm_gain_bricks(V.size);
+    }
+    if (n_views > 0) CK(cudaMemcpyAsync(ga->views_dev, ga->views_host, sizeof(DsmGainView) * (size_t)n_views, cudaMemcpyHostToDevice, ctx->stream));
+    CK(dsm_launch_gain(f->g, f->occ, f->dist, c, ga->views_dev, n_views, bricks, clusters ? fr->b.res : nullptr,
+                       clusters ? fr->b.max_clusters : 0, ga->slot, ga->res, ctx->stream));
+    CK(cudaMemcpyAsync(ga->res_host, ga->res, DsmGain::res_bytes(n_views), cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaEventRecord(ga->ev, ctx->stream));
+    ga->in_flight = true;
+    return DSM_OK;
+}
+
+extern "C" int dsm_gain_wait(dsm_ctx *ctx, dsm_gain_info_t *info, const dsm_view_gain_t **gains)
+{
+    if (!ctx) return DSM_E_INVALID;
+    DsmGain *ga = ctx->gain.get();
+    if (!ga || !ga->in_flight) return DSM_E_STATE;
+    CK(cudaSetDevice(ctx->device));
+    CK(cudaEventSynchronize(ga->ev));
+    ga->in_flight = false;
+    const int32_t *h = reinterpret_cast<const int32_t *>(ga->res_host);
+    if (info)
+    {
+        std::memcpy(info, h, sizeof(dsm_gain_info_t));
+        info->reserved[0] = info->reserved[1] = 0;
+    }
+    if (gains) *gains = reinterpret_cast<const dsm_view_gain_t *>(ga->res_host + 4 * DSM_GAIN_WORDS);
+    if (h[DSM_GAIN_ERR_TAG] == 0) return DSM_OK;
+    snprintf(ctx->err, sizeof(ctx->err), "dsm_gain_wait: frame %d of a dsm_fuse_stream_window call did not fit the pool or the "
+             "store; the field the job read holds the frames before it", h[DSM_GAIN_ERR_FRAME]);
+    return DSM_E_CAPACITY;
+}
+
 // ---- checkpoints that do not stop the stream (include/dsm.h, DESIGN.md §8.5) ----
 // The two images at the context's current capacities; whatever was there before is released first (the old and the new
 // need not fit at once).  On failure the checkpoint has no images and its calls return DSM_E_STATE.

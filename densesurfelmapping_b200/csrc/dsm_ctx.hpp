@@ -244,6 +244,20 @@ struct DsmReach
     bool in_flight = false, host_copy = false;
 };
 
+// dsm_gain_* (DESIGN.md §8.12), allocated by dsm_gain_enable for the field's grid: the pinned and device staging of
+// max_views views, the cluster-slot grid, the device result and its pinned copy, and the event after the copy
+struct DsmGain
+{
+    CudaOwner own;
+    int max_views = 0;
+    DsmGainView *views_host = nullptr, *views_dev = nullptr; // [max_views]
+    int32_t *slot = nullptr;                                  // device [voxels]
+    uint8_t *res = nullptr, *res_host = nullptr;              // 4 DSM_GAIN_WORDS + 32 max_views bytes each
+    cudaEvent_t ev = nullptr;
+    bool in_flight = false;
+    static size_t res_bytes(int n_views) { return 4 * (size_t)DSM_GAIN_WORDS + sizeof(dsm_view_gain_t) * (size_t)n_views; }
+};
+
 #define DSM_MAX_CHUNKS 4
 
 struct dsm_ctx
@@ -317,6 +331,7 @@ struct dsm_ctx
     std::unique_ptr<DsmViews> views;             // nullptr until dsm_views_enable
     std::unique_ptr<DsmFrontier> frontier;       // nullptr until dsm_frontier_enable
     std::unique_ptr<DsmReach> reach;             // nullptr until dsm_reach_enable
+    std::unique_ptr<DsmGain> gain;               // nullptr until dsm_gain_enable
     int run_split = 2;          // sub-batches per dsm_batch_run (dsm_set_concurrency)
     // pinned host staging for the small per-batch tables
     float *h_pose = nullptr; // [2B][32]: pose then inverse; first half: the batch calls, second half: the resident stream

@@ -385,6 +385,23 @@ size_t dsm_frontier_temp_bytes(const DsmFrontierBufs &b);
 // be zeroed by the caller.  Returns the first error of a CUB call or a launch.
 cudaError_t dsm_launch_frontier(const DsmFrontierBufs &b, const DsmFieldGrid &g, const uint8_t *state, const int32_t *field_header,
                                 int min_voxels, cudaStream_t s);
+// the frontier table's cluster among the first n whose listed members hold list entry j, or -1 (a binary search over
+// the offsets: the listed clusters are a prefix of the table with rising offsets)
+__device__ __forceinline__ int dsm_frontier_cluster_of(const dsm_frontier_cluster_t *table, int n, int j)
+{
+    int lo = 0, hi = n; // the last c with offset in [0, j]
+    while (lo < hi)
+    {
+        const int m = (lo + hi) / 2;
+        const int o = table[m].offset;
+        if (o >= 0 && o <= j)
+            lo = m + 1;
+        else
+            hi = m;
+    }
+    const int c = lo - 1;
+    return c >= 0 && j < table[c].offset + table[c].n_voxels ? c : -1;
+}
 
 // dsm_reach_* (DESIGN.md §8.11), dsm_reach.cu.  One packed result (D2H):
 //   int32 header[DSM_REACH_WORDS] | dsm_reach_target_t targets[max_targets] | int32 path[max_path_voxels]
@@ -440,3 +457,38 @@ int dsm_reach_ctas();
 cudaError_t dsm_launch_reach(const DsmReachBufs &b, const DsmFieldGrid &g, const uint8_t *state, const int32_t *dist,
                              const int3 s, float radius, int approach, int n_goals, const uint8_t *frontier_res, int frontier_max_clusters,
                              cudaStream_t st);
+
+// dsm_gain_* (DESIGN.md §8.12), dsm_gain.cu.  One staged request (H2D), DsmGainView views[n_views], and one packed
+// result (D2H): int32 header[DSM_GAIN_WORDS] | dsm_view_gain_t gains[max_views].  The header's first six words are
+// those of dsm_gain_info_t; its padding carries the field's error words, cleared by dsm_gain_wait.
+enum
+{
+    DSM_GAIN_ORIGIN = 0, // 3 words
+    DSM_GAIN_N_VIEWS = 3,
+    DSM_GAIN_N_CLUSTERS_TABLE,
+    DSM_GAIN_UNKNOWN_BLOCKS,
+    DSM_GAIN_ERR_TAG, // the field header's DSM_FIELD_ERR_TAG / _ERR_FRAME, copied by k_gain_init
+    DSM_GAIN_ERR_FRAME,
+    DSM_GAIN_WORDS = 8 // 32 B
+};
+// one view as the host stages it: the pose, its box of grid voxels (lo, size; size 0 on an axis: empty), the named
+// cluster (-1) and the view's first brick in the launch
+struct DsmGainView
+{
+    double P[12];
+    int32_t lo[3], size[3], cluster, brick0;
+}; // 128 B
+#define DSM_GAIN_BX 8 // bricks of 8 x 8 x 4 voxels, one CTA of 256 threads each
+#define DSM_GAIN_BY 8
+#define DSM_GAIN_BZ 4
+inline long long dsm_gain_bricks(const int32_t size[3])
+{
+    return (long long)((size[0] + DSM_GAIN_BX - 1) / DSM_GAIN_BX) * ((size[1] + DSM_GAIN_BY - 1) / DSM_GAIN_BY) *
+           ((size[2] + DSM_GAIN_BZ - 1) / DSM_GAIN_BZ);
+}
+// The whole job on the state grid of the latest known request (header at dsm_field_header(voxels) of dist) for the
+// n_views views already in `views` (bricks in all); frontier_res is the frontier job's device result (nullptr without
+// clusters) and slot a grid of voxels ints.  Writes the whole used result; returns the first launch or memset error.
+cudaError_t dsm_launch_gain(const DsmFieldGrid &g, const uint8_t *state, const int32_t *dist, const dsm_gain_camera_t &cam,
+                            const DsmGainView *views, int n_views, long long bricks, const uint8_t *frontier_res,
+                            int frontier_max_clusters, int32_t *slot, uint8_t *res, cudaStream_t st);

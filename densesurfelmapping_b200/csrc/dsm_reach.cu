@@ -227,24 +227,6 @@ __global__ void __launch_bounds__(RC_BLOCK) k_reach_reached(const uint32_t *__re
     if (threadIdx.x == 0 && n > 0) atomicAdd(&hdr[DSM_REACH_N_REACHED], n);
 }
 
-// the frontier table's cluster whose listed members hold list entry j (the listed clusters are a prefix of the table
-// with rising offsets), or -1
-__device__ __forceinline__ int reach_cluster_of(const dsm_frontier_cluster_t *table, int n, int j)
-{
-    int lo = 0, hi = n; // the last c with offset in [0, j]
-    while (lo < hi)
-    {
-        const int m = (lo + hi) / 2;
-        const int o = table[m].offset;
-        if (o >= 0 && o <= j)
-            lo = m + 1;
-        else
-            hi = m;
-    }
-    const int c = lo - 1;
-    return c >= 0 && j < table[c].offset + table[c].n_voxels ? c : -1;
-}
-
 // the window's least (cost[u] + chamfer(g - u)) << 32 | u over reached voxels u, on the whole warp
 __device__ __forceinline__ unsigned long long reach_window(const DsmFieldGrid &g, const uint8_t *trav, const uint32_t *cost, int gx, int gy,
                                                            int gz, int k, int lane)
@@ -288,7 +270,7 @@ __global__ void __launch_bounds__(RC_BLOCK) k_reach_targets(const DsmFieldGrid g
         else
         {
             const int j = item - n_goals;
-            const int c = reach_cluster_of(table, n_cl, j);
+            const int c = dsm_frontier_cluster_of(table, n_cl, j);
             if (c < 0) continue; // a member of a cluster past max_targets
             tg = n_goals + c;
             gi = list[j];

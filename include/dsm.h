@@ -749,6 +749,78 @@ int dsm_reach_enqueue(dsm_ctx *ctx, const double start[3], float radius, int app
 int dsm_reach_wait(dsm_ctx *ctx, dsm_reach_info_t *info, const dsm_reach_target_t **targets, const int32_t **path,
                    const uint32_t **cost);
 
+/* ---- view gain: the unknown, frontier and cluster voxels a camera pose would see (DESIGN.md §8.12) ----
+ * A gain job reads the state grid of the latest field request, which must be a known one, in stream order behind it,
+ * with that request's origin o and voxel edge v (widened to fp64) captured at the job's enqueue, and (with clusters)
+ * the result of the latest frontier job.  A later field or frontier request may be enqueued while a job is in flight and
+ * does not change what the job reads.  The map is never read.  Linear index (z * ny + y) * nx + x.
+ *
+ * Definition (every step fp64, one rounding per operation; integer counts, so the result does not depend on the
+ * schedule).  The camera is a pinhole in the convention of the frames (x right, y down, z forward); view j has the pose
+ * [R | t] poses[12 j ..] (row-major, camera to world) and, with clusters, names clusters[j] (an index into the latest
+ * frontier job's table, or -1 for none).  For every grid voxel x:
+ *   Centre: c_k = ((double)(o_k + x_k) + 0.5) * v and d = c - t.
+ *   Frustum: (d_0^2 + d_1^2) + d_2^2 <= Rm * Rm with Rm = (double)max_range; q_z > 0 where q_m = (R_0m d_0 + R_1m d_1)
+ *   + R_2m d_2 (R^T d); u = fx (q_x / q_z) + cx with 0 <= u < width; w = fy (q_y / q_z) + cy with 0 <= w < height.
+ *   Seen: a frustum voxel whose walk from a = t to b = c, the Amanatides-Woo walk of dsm_field_enqueue_known literally
+ *   (w_a = a / v, e = floor(b / v), the same tM and tD, the lowest axis on ties, the same stop when tM > 1), reaches e,
+ *   every voxel it visits before e lying inside the grid and, with unknown_blocks = 1 (pessimistic), being free, or,
+ *   with unknown_blocks = 0 (optimistic), not being occupied.  For every voxel x of the grid e is o + x (c / v lies
+ *   within a few ulp of o + x + 0.5), so e is x itself.  A camera whose voxel floor(t / v) - o lies outside the grid
+ *   sees nothing.
+ *   Frontier voxel: that of dsm_frontier_enqueue (free, with a face neighbour of state 0 inside the grid), taken from
+ *   the state grid itself, so it does not depend on a frontier job.
+ *   Record: n_frustum the frustum voxels; n_free, n_unknown, n_occupied the seen voxels of each state; n_frontier the
+ *   seen frontier voxels; n_cluster the seen members (voxels of the frontier list) of the named cluster, -1 when no
+ *   cluster is named or it has no members in the list; status 0 ok, 1 the camera's voxel lies outside the grid, then
+ *   (only with a camera inside) 3 the named cluster is past the table's entries, 2 it is in the table but not in the
+ *   voxel list (offset -1).
+ *   Header: the origin, n_views, n_clusters_table the frontier table's entries (min(n_clusters, max_clusters); 0
+ *   without clusters) and unknown_blocks.
+ *
+ *   dsm_gain_enable    once, after dsm_views_enable (DSM_E_STATE otherwise, and when called twice).  DSM_E_INVALID for
+ *                      max_views outside [1, 2^20].  Allocates the pinned and device staging of max_views poses, boxes
+ *                      and clusters, a cluster-slot grid (4 B per voxel), the device result and its pinned copy of
+ *                      32 + 32 max_views bytes, and an event.  DSM_E_NOMEM with nothing kept.
+ *   dsm_gain_enqueue   asynchronous on the context's stream, never waits: per view a box is computed and staged with the
+ *                      pose and the cluster on the calling thread (the box only sizes the work: see DESIGN.md §8.12),
+ *                      then one H2D copy, the kernels, one D2H copy of 32 + 32 n_views bytes and the event.  clusters
+ *                      may be NULL (no view names a cluster).  DSM_E_STATE before dsm_gain_enable, before any field
+ *                      request, when the latest field request is not a known one, while a job is in flight, and with
+ *                      clusters when the latest frontier job was not enqueued on the latest field request (or there is
+ *                      none).  DSM_E_INVALID for fx, fy not finite and > 0, cx, cy not finite, width or height outside
+ *                      [1, 65536], max_range not finite and > 0 or above 128 v, unknown_blocks not 0 or 1, a non-finite
+ *                      pose entry, a cluster index below -1, n_views outside [0, max_views], or a work bound
+ *                      n_views (2 ceil(max_range / v) + 3)^3 above 2^31 voxels (this bounds the work of one call).
+ *   dsm_gain_wait      waits for that job only.  *gains (n_views records) are the context's pinned results, valid until
+ *                      the next dsm_gain_enqueue; either out-pointer may be NULL.  If the field the job read was taken
+ *                      after a rejected frame, returns DSM_E_CAPACITY with valid results and does NOT clear the error, as
+ *                      dsm_field_wait.  DSM_E_STATE with no job enqueued. */
+typedef struct dsm_gain_camera_t
+{
+    double fx, fy, cx, cy;
+    int32_t width, height;
+    float max_range;                 /* metres */
+    int32_t unknown_blocks;          /* 1: only free voxels pass a line of sight; 0: every voxel but occupied ones */
+} dsm_gain_camera_t;                 /* 48 B */
+typedef struct dsm_view_gain_t
+{
+    int32_t n_frustum, n_free, n_unknown, n_occupied, n_frontier, n_cluster;
+    int32_t status, reserved;        /* reserved 0 */
+} dsm_view_gain_t;                   /* 32 B */
+typedef struct dsm_gain_info_t
+{
+    int32_t origin[3];
+    int32_t n_views, n_clusters_table, unknown_blocks;
+    int32_t reserved[2];
+} dsm_gain_info_t;                   /* 32 B */
+#define DSM_GAIN_MAX_VIEWS (1 << 20)
+#define DSM_GAIN_MAX_RANGE_VOXELS 128
+#define DSM_GAIN_MAX_WORK (1ll << 31)
+int dsm_gain_enable(dsm_ctx *ctx, int max_views);
+int dsm_gain_enqueue(dsm_ctx *ctx, const dsm_gain_camera_t *camera, const double *poses, const int32_t *clusters, int n_views);
+int dsm_gain_wait(dsm_ctx *ctx, dsm_gain_info_t *info, const dsm_view_gain_t **gains);
+
 /* ---- checkpoints that do not stop the stream (DESIGN.md §8.5) ----
  * The file of dsm_map_save, taken in stream order like a publish snapshot: the resident stream pays one device-to-device
  * copy of the live map, the transfer to the host runs on a low-priority stream beside the next frames, and a thread of

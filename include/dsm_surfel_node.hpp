@@ -83,6 +83,10 @@
 // lets reach() find paths through the known free space of the latest fused frame's field on the device (DESIGN.md
 // §8.11): the travel cost from a start point to goal points and, after a frontiers() call on that frame, to every
 // frontier cluster, with each target's viewpoint and path, one enqueue and one wait.
+// What would the robot see from there?  enable_view_gain(max_views), after enable_known_space, lets view_gain() score
+// candidate camera poses against the latest fused frame's known field on the device (DESIGN.md §8.12): per pose, with
+// the node's own intrinsics, the frustum voxels and the free, unknown, occupied, frontier and (after a frontiers() call
+// on that frame) cluster voxels it would see, one enqueue and one wait.
 // device < 0 builds the node without a context: the callbacks run the whole pose logic (pose database, sync, window
 // bookkeeping) and fuse nothing; any call that reads the map returns DSM_E_STATE.
 #pragma once
@@ -586,6 +590,38 @@ class SurfelMapNode
             path.assign(p, p + info.n_path_voxels);
         }
         return ctx_.done(rc, "reach");
+    }
+
+    // ---- view gain against the known field of the latest fused frame (DESIGN.md §8.12) ----
+    // once, after enable_known_space: the most views one view_gain() call scores
+    int enable_view_gain(int max_views)
+    {
+        return ctx_.run("enable_view_gain", [&] { return dsm_gain_enable(ctx_.ctx, max_views); });
+    }
+    // the gain of n_views camera poses (poses: 12 doubles each, row-major [R | t], camera to world) seen with the node's
+    // intrinsics out to max_range (include/dsm.h): gains receives n_views records.  clusters is empty or names, per
+    // view, a cluster of the frontiers() call on this frame (-1: none).  DSM_E_STATE without known space, before any
+    // field, after load_state* until the next fused frame, and with clusters without a frontiers() call since the frame
+    // was fused; DSM_E_CAPACITY with the gains of the last applied frame's field, as distance_field().
+    int view_gain(const double *poses, int n_views, float max_range, int unknown_blocks, const std::vector<int32_t> &clusters,
+                  dsm_gain_info_t &info, std::vector<dsm_view_gain_t> &gains)
+    {
+        gains.clear();
+        info = dsm_gain_info_t();
+        if (!ctx_.ready("view_gain")) return ctx_.err;
+        if (known_.empty() || !field_exists_) return ctx_.done(DSM_E_STATE, "view_gain");
+        if (!clusters.empty() && (int)clusters.size() != n_views) return ctx_.done(DSM_E_INVALID, "view_gain");
+        dsm_gain_camera_t cam;
+        cam.fx = cam_[0], cam.fy = cam_[1], cam.cx = cam_[2], cam.cy = cam_[3];
+        cam.width = width_, cam.height = height_;
+        cam.max_range = max_range;
+        cam.unknown_blocks = unknown_blocks;
+        int rc = dsm_gain_enqueue(ctx_.ctx, &cam, poses, clusters.empty() ? nullptr : clusters.data(), n_views);
+        if (rc != DSM_OK) return ctx_.done(rc, "view_gain");
+        const dsm_view_gain_t *g = nullptr;
+        rc = dsm_gain_wait(ctx_.ctx, &info, &g);
+        if (rc == DSM_OK || rc == DSM_E_CAPACITY) gains.assign(g, g + info.n_views);
+        return ctx_.done(rc, "view_gain");
     }
 
     // ---- planner queries against the field of the latest fused frame (DESIGN.md §8.8) ----
