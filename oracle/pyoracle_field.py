@@ -40,8 +40,13 @@ def squared_distances(occ):
     if not occ.any():
         return None
     _, ind = ndimage.distance_transform_edt(~occ, return_indices=True)
-    diff = ind.astype(np.int64) - np.indices(occ.shape, dtype=np.int64)
-    return (diff * diff).sum(axis=0)
+    d2 = np.zeros(occ.shape, np.int64)
+    for k, n in enumerate(occ.shape):   # one axis at a time: the peak stays near the index array's size
+        shape = [1] * occ.ndim
+        shape[k] = n
+        diff = ind[k].astype(np.int64) - np.arange(n, dtype=np.int64).reshape(shape)
+        d2 += diff * diff
+    return d2
 
 
 def field(points, voxel, shape, center):

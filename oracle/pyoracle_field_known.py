@@ -133,10 +133,16 @@ def known_field(points, voxel, shape, center, views, max_range):
     pts = pts.reshape(len(pts), -1)[:, :3] if pts.size else np.zeros((0, 3), np.float32)
     state = pyoracle_field.occupancy(pts, voxel, shape, o).astype(np.uint8)
     carve(state, views, voxel, o, max_range)
+    dist, n_occupied, n_free = state_field(state, voxel)
+    return dist, o.astype(np.int32), n_occupied, state, n_free
+
+
+def state_field(state, voxel):
+    """(dist, n_occupied, n_free) of the state grid [nz][ny][nx] (uint8): the distance to the nearest voxel that is not
+    free (float32, +inf when every voxel is free), the occupied and the free voxels."""
     d2 = pyoracle_field.squared_distances(state != FREE)
     if d2 is None:
         dist = np.full(state.shape, np.inf, np.float32)
     else:
         dist = np.sqrt(d2.astype(np.float32)) * np.float32(voxel)
-    return (dist.astype(np.float32), o.astype(np.int32), int((state == OCCUPIED).sum()), state,
-            int((state == FREE).sum()))
+    return dist.astype(np.float32), int((state == OCCUPIED).sum()), int((state == FREE).sum())

@@ -7,6 +7,7 @@ import numpy as np
 import pytest
 
 import pyoracle
+import pyoracle_field_known
 import pyoracle_publish
 import pyoracle_window
 from densesurfelmapping_b200 import capi, synth
@@ -183,6 +184,21 @@ def assert_field(got, want, what):
     assert n_occ == want[2], f"{what}: occupied voxels {n_occ}, want {want[2]}"
     assert dist.shape == want[0].shape and dist.tobytes() == want[0].tobytes(), \
         f"{what}: {(dist.view(np.uint32) != want[0].view(np.uint32)).sum()} voxels differ"
+
+
+def load_known(ctx, state, origin, voxel, what=""):
+    """Loads the state grid [nz][ny][nx] at `origin` as the latest known field, waits for it and holds it to
+    oracle/pyoracle_field_known bit for bit: distances, origin, n_occupied, the states read back and n_free.  Returns
+    the distances."""
+    state = np.ascontiguousarray(state, np.uint8)
+    ctx.debug_field_load_state(state, origin)
+    got = ctx.field_wait()
+    dist, n_occ, n_free = pyoracle_field_known.state_field(state, voxel)
+    assert_field(got, (dist, np.asarray(origin, np.int32), n_occ), f"{what} (loaded)")
+    st, nf = ctx.field_state()
+    assert st.tobytes() == state.tobytes(), f"{what} (loaded): {(st != state).sum()} states differ"
+    assert nf == n_free, f"{what} (loaded): free voxels {nf}, want {n_free}"
+    return got[0]
 
 
 def centres(ctx, t, voxel, shape, m):

@@ -4,7 +4,8 @@ The device equals oracle/pyoracle_frontier bit for bit, in the cluster table, th
 known field of the windowed drive (the model runs on the device's own field_state, which tests/test_gpu_field_known.py
 pins to the known-space oracle), a resident request equal to its host-copy twin; on state grids loaded through
 dsm_debug_field_load_state (hand cases, random grids over a sweep of densities, a serpentine of about a million voxels,
-the checkerboard at 512x512x64), at several min_voxels and both capacity cuts; twice the same request gives the same
+the checkerboard at 512x512x64; each load's distances, counts and states are held to the known-space oracle first,
+through resident_map.load_known), at several min_voxels and both capacity cuts; twice the same request gives the same
 bytes; the stream order against later field requests, a publish snapshot and an asynchronous checkpoint; the
 rejected-frame and error contracts; and a drive with frontier jobs leaves the map, the clouds and the fields as a twin
 without them.  The node is checked through tests/cpp/frontier_main.cpp."""
@@ -17,7 +18,7 @@ import pyoracle_frontier
 from densesurfelmapping_b200 import capi, synth
 from densesurfelmapping_b200.elements import POINT_DTYPE, SURFEL_DTYPE
 from node_drive import node_script, run_driver
-from resident_map import SHAPES, STORE, T, camera, map_state, new_ctx, simple_lists, warp, windowed
+from resident_map import SHAPES, STORE, T, camera, load_known, map_state, new_ctx, simple_lists, warp, windowed
 from test_frontier_model import serpentine
 from test_gpu_field_known import MAX_RANGE, Views
 
@@ -47,9 +48,8 @@ def loader(shape, voxel=0.2, caps=CAPS):
     return ctx
 
 
-def load_and_run(ctx, state, origin, m):
-    ctx.debug_field_load_state(state, origin)
-    ctx.field_wait()
+def load_and_run(ctx, state, origin, voxel, m):
+    load_known(ctx, state, origin, voxel)
     ctx.frontier_enqueue(m)
     return ctx.frontier_wait()
 
@@ -57,7 +57,7 @@ def load_and_run(ctx, state, origin, m):
 def check_grid(ctx, state, origin, voxel, ms=(1, 2, 50), what=""):
     mc, mv = ctx._frontier_caps
     for m in ms:
-        same(load_and_run(ctx, state, origin, m), pyoracle_frontier.frontiers(state, origin, voxel, m, mc, mv), f"{what} m={m}")
+        same(load_and_run(ctx, state, origin, voxel, m), pyoracle_frontier.frontiers(state, origin, voxel, m, mc, mv), f"{what} m={m}")
 
 
 def checkerboard(nz, ny, nx):
@@ -105,8 +105,8 @@ def test_random_grids_at_a_size_a_user_runs():
     for p in [(0.5, 0.0, 0.5), (0.2, 0.1, 0.7), (0.7, 0.1, 0.2), (0.05, 0.05, 0.9), (0.9, 0.0, 0.1), (0.33, 0.33, 0.34)]:
         st = rng.choice(3, size=shape[::-1], p=p).astype(np.uint8)
         check_grid(ctx, st, (-160, -160, -5), voxel, what=f"density {p}")
-        a = load_and_run(ctx, st, (-160, -160, -5), 1)
-        b = load_and_run(ctx, st, (-160, -160, -5), 1)
+        a = load_and_run(ctx, st, (-160, -160, -5), voxel, 1)
+        b = load_and_run(ctx, st, (-160, -160, -5), voxel, 1)
         assert all(x.tobytes() == y.tobytes() for x, y in zip(a, b)), "the same request twice"
     ctx.close()
 
@@ -118,7 +118,7 @@ def test_serpentine_and_checkerboard():
     st = serpentine(320, 320, 40)
     assert 900_000 < int((st == FREE).sum()) < 1_200_000
     check_grid(ctx, st, (3, -7, 0), 0.2, ms=(1, 50), what="serpentine")
-    c, v, n = load_and_run(ctx, st, (3, -7, 0), 1)
+    c, v, n = load_and_run(ctx, st, (3, -7, 0), 0.2, 1)
     assert n["n_components"] == 1 and len(v) == n["n_frontier"]
     ctx.close()
     ctx = loader((512, 512, 64), 0.1, (4, 1 << 24))
@@ -161,7 +161,7 @@ def test_stream_order():
     got = ctx.frontier_wait()
     ctx.field_wait()
     same(got, pyoracle_frontier.frontiers(a, (0, 0, 0), 0.2, 1, *CAPS), "the old grid")
-    same(load_and_run(ctx, b, (5, 5, 5), 1), pyoracle_frontier.frontiers(b, (5, 5, 5), 0.2, 1, *CAPS), "the new grid")
+    same(load_and_run(ctx, b, (5, 5, 5), 0.2, 1), pyoracle_frontier.frontiers(b, (5, 5, 5), 0.2, 1, *CAPS), "the new grid")
     ctx.field_enqueue((0, 0, 0), 1)         # a plain request
     with pytest.raises(capi.DsmError) as e:
         ctx.frontier_enqueue(1)

@@ -5,7 +5,8 @@ The device equals oracle/pyoracle_gain bit for bit in every record and header: o
 drive (views at eight yaws around each viewpoint of a reach job and random poses, both blocking rules, with and without
 clusters; the model runs on the device's own field_state, which tests/test_gpu_field_known.py pins to the known-space
 oracle); on grids loaded through dsm_debug_field_load_state (hand cases, a density sweep, 320x320x40 at the longest
-range, a request of max_views views against the model on a subset and against smaller requests); a resident field
+range, a request of max_views views against the model on a subset and against smaller requests; each load's distances,
+counts and states are held to the known-space oracle first, through resident_map.load_known); a resident field
 against its host-copy twin; the stream order against the next field request and the next frontier job; a drive with gain
 jobs beside publish snapshots and asynchronous checkpoints leaves everything as a twin without them; the rejected-frame
 and error contracts.  The node is checked through tests/cpp/gain_main.cpp."""
@@ -20,7 +21,7 @@ import pyoracle_gain as G
 from densesurfelmapping_b200 import capi, synth
 from densesurfelmapping_b200.elements import POINT_DTYPE, SURFEL_DTYPE
 from node_drive import node_script, run_driver
-from resident_map import SHAPES, STORE, T, camera, map_state, new_ctx, simple_lists, warp, windowed
+from resident_map import SHAPES, STORE, T, camera, load_known, map_state, new_ctx, simple_lists, warp, windowed
 from test_gain_model import random_pose, symmetric_scene, symmetric_views, wall_scene, yaw_pose
 from test_gpu_field_known import MAX_RANGE, Views
 
@@ -65,8 +66,7 @@ def job(ctx, state, origin, voxel, cam, poses, clusters=None, m=1):
 
 
 def loaded(ctx, state, origin, voxel, cam, poses, clusters=None, m=1, what=""):
-    ctx.debug_field_load_state(state, origin)
-    ctx.field_wait()
+    load_known(ctx, state, origin, voxel, what)
     got, want = job(ctx, state, origin, voxel, cam, poses, clusters, m)
     same(got, want, what)
     return got
@@ -157,8 +157,7 @@ def test_the_most_views_one_request_takes():
     rng = np.random.default_rng(14)
     st = rng.choice(3, size=shape[::-1], p=(0.2, 0.05, 0.75)).astype(np.uint8)
     ctx = loader(shape, voxel, max_views=max_views)
-    ctx.debug_field_load_state(st, o)
-    ctx.field_wait()
+    load_known(ctx, st, o, voxel)
     ctx.frontier_enqueue(1)
     fr = ctx.frontier_wait()[:2]
     centre = G.centres([(48, 40, 12)], o, voxel)[0]
@@ -429,8 +428,7 @@ def test_error_contract():
     ctx.field_enqueue((0, 0, 0), 1)                                       # a plain request
     ctx.field_wait()
     assert lib.dsm_gain_enqueue(ctx.h, ctypes.byref(ok), P, None, 1) == -7
-    ctx.debug_field_load_state(st, (0, 0, 0))
-    ctx.field_wait()
+    load_known(ctx, st, (0, 0, 0), 0.2)
     cl = np.zeros(1, np.int32)
     assert lib.dsm_gain_enqueue(ctx.h, ctypes.byref(ok), P, cl.ctypes.data, 1) == -7   # clusters without a frontier job
     nan, inf = float("nan"), float("inf")

@@ -4,7 +4,8 @@ The device equals oracle/pyoracle_reach bit for bit in the whole header (rounds 
 records, the path list and the cost grid: on every known field of the windowed drive, with frontier targets (the model
 runs on the device's own field_wait / field_state, which tests/test_gpu_field_known.py pins to the known-space oracle);
 on grids loaded through dsm_debug_field_load_state (hand cases, random grids over a sweep of densities, a maze, a
-serpentine cut short by max_rounds against the round emulator, a grid of over a million voxels against Dijkstra); a
+serpentine cut short by max_rounds against the round emulator, a grid of over a million voxels against Dijkstra; each
+load's distances, counts and states are held to the known-space oracle first, through resident_map.load_known); a
 resident job equals its host-copy twin; the stream order against the next field request and the next frontier job; a
 drive with reach jobs beside publish snapshots and asynchronous checkpoints leaves everything as a twin without them;
 the rejected-frame and error contracts.  The node is checked through tests/cpp/reach_main.cpp."""
@@ -19,7 +20,7 @@ import pyoracle_reach as R
 from densesurfelmapping_b200 import capi, synth
 from densesurfelmapping_b200.elements import POINT_DTYPE, SURFEL_DTYPE
 from node_drive import node_script, run_driver
-from resident_map import SHAPES, STORE, T, camera, map_state, new_ctx, simple_lists, warp, windowed
+from resident_map import SHAPES, STORE, T, camera, load_known, map_state, new_ctx, simple_lists, warp, windowed
 from test_frontier_model import serpentine
 from test_gpu_field_known import MAX_RANGE, Views
 
@@ -71,8 +72,7 @@ def job(ctx, dist, state, origin, voxel, start, radius, k, goals=(), with_fronti
 
 
 def loaded(ctx, state, origin, voxel, start, radius, k, goals=(), with_frontiers=False, m=1, exact=False, what=""):
-    ctx.debug_field_load_state(state, origin)
-    dist = ctx.field_wait()[0]
+    dist = load_known(ctx, state, origin, voxel, what)
     got, want = job(ctx, dist, state, origin, voxel, start, radius, k, goals, with_frontiers, m, exact=exact)
     same(got, want, what, rounds=not exact)
     return got
@@ -223,8 +223,7 @@ def test_resident_job_equals_its_host_copy_twin_and_repeats():
     ctx = loader(shape, 0.2)
     rng = np.random.default_rng(4)
     st = rng.choice(3, size=shape[::-1], p=(0.15, 0.1, 0.75)).astype(np.uint8)
-    ctx.debug_field_load_state(st, (0, 0, 0))
-    ctx.field_wait()
+    load_known(ctx, st, (0, 0, 0), 0.2)
     goals = rng.uniform(0, 6, size=(30, 3))
     outs = []
     for host_copy in (False, True, False):
@@ -443,8 +442,7 @@ def test_error_contract():
     ctx.field_enqueue((0, 0, 0), 1)                                       # a plain request
     ctx.field_wait()
     assert lib.dsm_reach_enqueue(ctx.h, s, 0.0, 0, None, 0, 0, 0) == -7
-    ctx.debug_field_load_state(st, (0, 0, 0))
-    ctx.field_wait()
+    load_known(ctx, st, (0, 0, 0), 0.2)
     assert lib.dsm_reach_enqueue(ctx.h, s, 0.0, 0, None, 0, 1, 0) == -7   # with frontiers, without a frontier job
     nan, inf = float("nan"), float("inf")
     for args in [(D3(nan, 0, 0), 0.0, 0, None, 0), (D3(0, inf, 0), 0.0, 0, None, 0), (s, -0.1, 0, None, 0), (s, nan, 0, None, 0),
