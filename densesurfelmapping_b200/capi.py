@@ -36,7 +36,8 @@ EXPORTS = [
     "dsm_field_enqueue_resident", "dsm_field_query_enable", "dsm_field_query_enqueue", "dsm_field_query_wait",
     "dsm_views_enable", "dsm_views_capture", "dsm_field_enqueue_known", "dsm_field_state",
     "dsm_frontier_enable", "dsm_frontier_enqueue", "dsm_frontier_wait", "dsm_debug_field_load_state",
-    "dsm_reach_enable", "dsm_reach_enqueue", "dsm_reach_wait", "dsm_gain_enable", "dsm_gain_enqueue", "dsm_gain_wait",
+    "dsm_reach_enable", "dsm_reach_enqueue", "dsm_reach_wait", "dsm_reach_matrix_enable", "dsm_reach_matrix_enqueue",
+    "dsm_reach_matrix_wait", "dsm_gain_enable", "dsm_gain_enqueue", "dsm_gain_wait",
     "dsm_inactive_segments", "dsm_inactive_load", "dsm_map_save", "dsm_map_load", "dsm_map_peek",
     "dsm_checkpoint_enable", "dsm_checkpoint_enqueue", "dsm_checkpoint_wait", "dsm_debug_checkpoint_drain_ctas",
     "dsm_checkpoint_enqueue_incremental", "dsm_map_load_journal", "dsm_map_peek_journal", "dsm_journal_materialize",
@@ -75,6 +76,11 @@ REACH_INFO_DTYPE = np.dtype([("origin", "<i4", 3), ("start_voxel", "<i4"), ("sta
                              ("rounds", "<i4"), ("converged", "<i4"), ("n_traversable", "<i4"), ("n_reached", "<i4"),
                              ("n_goals", "<i4"), ("n_clusters_total", "<i4"), ("n_targets", "<i4"), ("n_path_voxels", "<i4"),
                              ("reserved", "<i4", 2)])
+# dsm_reach_matrix_wait's records (include/dsm.h): a site (32 B) and the header (64 B)
+REACH_SITE_DTYPE = np.dtype([("voxel", "<i4"), ("status", "<i4"), ("approach", "<i4"), ("rounds", "<i4"), ("converged", "<i4"),
+                             ("n_reached", "<i4"), ("reserved", "<i4", 2)])
+REACH_MATRIX_INFO_DTYPE = np.dtype([("origin", "<i4", 3), ("n_sites", "<i4"), ("status", "<i4"), ("n_traversable", "<i4"),
+                                    ("n_active_tiles", "<i4"), ("max_tiles", "<i4"), ("rounds", "<i4"), ("reserved", "<i4", 7)])
 # dsm_gain_wait's records (include/dsm.h): a view's gain (32 B) and the header (32 B)
 VIEW_GAIN_DTYPE = np.dtype([("n_frustum", "<i4"), ("n_free", "<i4"), ("n_unknown", "<i4"), ("n_occupied", "<i4"), ("n_frontier", "<i4"),
                             ("n_cluster", "<i4"), ("status", "<i4"), ("reserved", "<i4")])
@@ -158,6 +164,9 @@ def load_library():
     L.dsm_reach_enable.argtypes = [vp, ci, ci, ci]
     L.dsm_reach_enqueue.argtypes = [vp, ctypes.POINTER(ctypes.c_double), ctypes.c_float, ci, vp, ci, ci, ci]
     L.dsm_reach_wait.argtypes = [vp, vp, ctypes.POINTER(vp), ctypes.POINTER(vp), ctypes.POINTER(vp)]
+    L.dsm_reach_matrix_enable.argtypes = [vp, ci, ci, ci]
+    L.dsm_reach_matrix_enqueue.argtypes = [vp, vp, ci, ctypes.c_float, ci]
+    L.dsm_reach_matrix_wait.argtypes = [vp, vp, ctypes.POINTER(vp), ctypes.POINTER(vp)]
     L.dsm_gain_enable.argtypes = [vp, ci]
     L.dsm_gain_enqueue.argtypes = [vp, ctypes.POINTER(DsmGainCamera), vp, vp, ci]
     L.dsm_gain_wait.argtypes = [vp, vp, ctypes.POINTER(vp)]
@@ -727,6 +736,35 @@ class Context:
         if rc != DSM_OK:
             err = DsmError(rc, self.lib.dsm_last_error(self.h).decode())
             err.reach = out
+            raise err
+        return out
+
+    # ---- travel costs between many sites through the known free space of the latest known field ----
+    def reach_matrix_enable(self, max_sites, max_tiles, max_rounds):
+        self._ck(self.lib.dsm_reach_matrix_enable(self.h, int(max_sites), int(max_tiles), int(max_rounds)))
+
+    def reach_matrix_enqueue(self, points, radius, approach):
+        """points: world points, an (n, 3) array-like of float64, n >= 1."""
+        p = np.ascontiguousarray(points, np.float64).reshape(-1, 3)
+        self._ck(self.lib.dsm_reach_matrix_enqueue(self.h, p.ctypes.data if len(p) else None, len(p), float(radius), int(approach)))
+
+    def reach_matrix_wait(self):
+        """(info, sites, matrix): numpy copies of the context's pinned results, a REACH_MATRIX_INFO_DTYPE record,
+        REACH_SITE_DTYPE (n_sites,) and the uint32 matrix (n_sites, n_sites), row i from site i.  A job on a field taken
+        after a rejected frame raises DsmError(DSM_E_CAPACITY) carrying the same tuple as `.reach_matrix`."""
+        ps, pm = ctypes.c_void_p(), ctypes.c_void_p()
+        info = np.zeros(1, REACH_MATRIX_INFO_DTYPE)
+        rc = self.lib.dsm_reach_matrix_wait(self.h, info.ctypes.data, ctypes.byref(ps), ctypes.byref(pm))
+        if rc not in (DSM_OK, -6):
+            self._ck(rc)
+        i = info[0]
+        n = int(i["n_sites"])
+        sites = np.frombuffer((ctypes.c_uint8 * (n * REACH_SITE_DTYPE.itemsize)).from_address(ps.value), dtype=REACH_SITE_DTYPE).copy()
+        m = np.frombuffer((ctypes.c_uint8 * (4 * n * n)).from_address(pm.value), dtype=np.uint32).reshape(n, n).copy()
+        out = (i, sites, m)
+        if rc != DSM_OK:
+            err = DsmError(rc, self.lib.dsm_last_error(self.h).decode())
+            err.reach_matrix = out
             raise err
         return out
 

@@ -1988,6 +1988,112 @@ extern "C" int dsm_reach_wait(dsm_ctx *ctx, dsm_reach_info_t *info, const dsm_re
     return DSM_E_CAPACITY;
 }
 
+// ---- travel costs between many sites (include/dsm.h, DESIGN.md §8.13) ----
+extern "C" int dsm_reach_matrix_enable(dsm_ctx *ctx, int max_sites, int max_tiles, int max_rounds)
+{
+    if (!ctx) return DSM_E_INVALID;
+    const DsmField *f = ctx->field.get();
+    if (!f || !ctx->views || ctx->reach_matrix) return DSM_E_STATE;
+    int tn[3];
+    for (int k = 0; k < 3; k++) tn[k] = (f->g.n[k] + DSM_REACH_TILE - 1) / DSM_REACH_TILE;
+    const long long tiles = (long long)tn[0] * tn[1] * tn[2];
+    if (max_sites < 1 || max_sites > DSM_REACH_MATRIX_MAX_SITES || max_tiles < 1 || max_tiles > tiles || max_rounds < 1 ||
+        max_rounds > DSM_REACH_MAX_ROUNDS || f->voxels > (size_t)DSM_REACH_MAX_VOXELS ||
+        4096ull * (unsigned long long)max_sites * (unsigned long long)max_tiles > DSM_REACH_MATRIX_MAX_COST_BYTES)
+        return DSM_E_INVALID;
+    CK(cudaSetDevice(ctx->device));
+    auto rm = std::make_unique<DsmReachMatrix>();
+    DsmReachMatrixBufs &b = rm->b;
+    b.voxels = (int)f->voxels;
+    for (int k = 0; k < 3; k++) b.tn[k] = tn[k];
+    b.tiles = (int)tiles;
+    b.max_sites = max_sites, b.max_tiles = max_tiles, b.max_rounds = max_rounds;
+    b.ctas = dsm_reach_matrix_ctas();
+    const size_t items = (size_t)max_sites * max_tiles, res = DsmReachMatrixBufs::res_bytes(max_sites);
+    CudaOwner &o = rm->own;
+    cudaError_t e = b.ctas > 0 ? cudaSuccess : cudaErrorInvalidValue;
+    for (int32_t **p : {&b.flag, &b.scan, &b.slot})
+        if (e == cudaSuccess) e = o.device(p, (size_t)b.tiles);
+    if (e == cudaSuccess) e = o.device(&b.mask, 16 * (size_t)b.tiles);
+    if (e == cudaSuccess) e = o.device(&b.tile_of, (size_t)max_tiles);
+    for (uint32_t **p : {&b.cost[0], &b.cost[1]})
+        if (e == cudaSuccess) e = o.device(p, items * 512);
+    for (int32_t **p : {&b.stamp, &b.sched[0], &b.sched[1]})
+        if (e == cudaSuccess) e = o.device(p, items);
+    if (e == cudaSuccess) e = o.device(&b.count, 3 * (size_t)max_sites);
+    for (int32_t **p : {&b.rounds, &b.reached})
+        if (e == cudaSuccess) e = o.device(p, (size_t)max_sites);
+    if (e == cudaSuccess) e = o.device(&b.sites, 3 * (size_t)max_sites);
+    if (e == cudaSuccess) e = o.device(&b.res, res);
+    if (e == cudaSuccess) e = o.host(&rm->sites_host, 3 * (size_t)max_sites);
+    if (e == cudaSuccess) e = o.host(&rm->res_host, res);
+    if (e == cudaSuccess) e = o.event(&rm->ev);
+    if (e == cudaSuccess)
+    {
+        b.temp_bytes = dsm_reach_matrix_temp_bytes(b);
+        e = b.temp_bytes ? o.device(reinterpret_cast<uint8_t **>(&b.temp), b.temp_bytes) : cudaErrorInvalidValue;
+    }
+    if (e != cudaSuccess)
+    {
+        cudaGetLastError();
+        return DSM_E_NOMEM; // nothing is kept: a later call may try again
+    }
+    ctx->reach_matrix = std::move(rm);
+    return DSM_OK;
+}
+
+// Enqueue only: the points' voxels staged and copied, the job on the grids of the latest (known) field request, one D2H
+// copy of the n-site result and the event.  A later field request overwrites those grids only behind the job.
+extern "C" int dsm_reach_matrix_enqueue(dsm_ctx *ctx, const double *points, int n_points, float radius, int approach)
+{
+    if (!ctx) return DSM_E_INVALID;
+    DsmReachMatrix *rm = ctx->reach_matrix.get();
+    const DsmField *f = ctx->field.get();
+    if (!rm || !f || !f->requested || !f->known || rm->in_flight) return DSM_E_STATE;
+    DsmReachMatrixBufs &b = rm->b;
+    if (!points || !std::isfinite(radius) || !(radius >= 0.f) || approach < 0 || approach > DSM_REACH_MAX_APPROACH || n_points < 1 ||
+        n_points > b.max_sites ||
+        (unsigned long long)n_points * (unsigned long long)b.max_tiles * (unsigned long long)b.max_rounds > DSM_REACH_MATRIX_MAX_WORK)
+        return DSM_E_INVALID;
+    for (size_t i = 0; i < 3 * (size_t)n_points; i++)
+        if (!std::isfinite(points[i])) return DSM_E_INVALID;
+    const DsmFieldGrid &g = f->g;
+    CK(cudaSetDevice(ctx->device));
+    // the previous job's copy out of this staging ended before its wait, which no job in flight implies
+    for (size_t i = 0; i < 3 * (size_t)n_points; i++) rm->sites_host[i] = reach_voxel(points[i], g.voxel, g.o[i % 3], g.n[i % 3]);
+    CK(cudaMemcpyAsync(b.sites, rm->sites_host, 12 * (size_t)n_points, cudaMemcpyHostToDevice, ctx->stream));
+    CK(cudaMemsetAsync(b.res, 0, 4 * DSM_RM_WORDS, ctx->stream));
+    CK(dsm_launch_reach_matrix(b, g, f->occ, f->dist, n_points, radius, approach, ctx->stream));
+    CK(cudaMemcpyAsync(rm->res_host, b.res, DsmReachMatrixBufs::res_bytes(n_points), cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaEventRecord(rm->ev, ctx->stream));
+    rm->in_flight = true;
+    rm->n_sites = n_points;
+    return DSM_OK;
+}
+
+extern "C" int dsm_reach_matrix_wait(dsm_ctx *ctx, dsm_reach_matrix_info_t *info, const dsm_reach_site_t **sites, const uint32_t **matrix)
+{
+    if (!ctx) return DSM_E_INVALID;
+    DsmReachMatrix *rm = ctx->reach_matrix.get();
+    if (!rm || !rm->in_flight) return DSM_E_STATE;
+    CK(cudaSetDevice(ctx->device));
+    CK(cudaEventSynchronize(rm->ev));
+    rm->in_flight = false;
+    const int32_t *h = reinterpret_cast<const int32_t *>(rm->res_host);
+    const size_t table = 4 * DSM_RM_WORDS;
+    if (info)
+    {
+        std::memcpy(info, h, sizeof(dsm_reach_matrix_info_t));
+        for (int32_t &w : info->reserved) w = 0;
+    }
+    if (sites) *sites = reinterpret_cast<const dsm_reach_site_t *>(rm->res_host + table);
+    if (matrix) *matrix = reinterpret_cast<const uint32_t *>(rm->res_host + table + sizeof(dsm_reach_site_t) * (size_t)rm->n_sites);
+    if (h[DSM_RM_ERR_TAG] == 0) return DSM_OK;
+    snprintf(ctx->err, sizeof(ctx->err), "dsm_reach_matrix_wait: frame %d of a dsm_fuse_stream_window call did not fit the pool or "
+             "the store; the field the job read holds the frames before it", h[DSM_RM_ERR_FRAME]);
+    return DSM_E_CAPACITY;
+}
+
 // ---- view gain against the latest known field (include/dsm.h, DESIGN.md §8.12) ----
 extern "C" int dsm_gain_enable(dsm_ctx *ctx, int max_views)
 {

@@ -244,6 +244,20 @@ struct DsmReach
     bool in_flight = false, host_copy = false;
 };
 
+// dsm_reach_matrix_* (DESIGN.md §8.13), allocated by dsm_reach_matrix_enable for the field's grid: the job's device
+// buffers (DsmReachMatrixBufs, the packed result among them), the site staging, the result's pinned copy and the event
+// after it
+struct DsmReachMatrix
+{
+    CudaOwner own;
+    DsmReachMatrixBufs b;
+    int32_t *sites_host = nullptr; // pinned [max_sites][3]
+    uint8_t *res_host = nullptr;
+    cudaEvent_t ev = nullptr;
+    int n_sites = 0; // of the job in flight or last waited for
+    bool in_flight = false;
+};
+
 // dsm_gain_* (DESIGN.md §8.12), allocated by dsm_gain_enable for the field's grid: the pinned and device staging of
 // max_views views, the cluster-slot grid, the device result and its pinned copy, and the event after the copy
 struct DsmGain
@@ -331,6 +345,7 @@ struct dsm_ctx
     std::unique_ptr<DsmViews> views;             // nullptr until dsm_views_enable
     std::unique_ptr<DsmFrontier> frontier;       // nullptr until dsm_frontier_enable
     std::unique_ptr<DsmReach> reach;             // nullptr until dsm_reach_enable
+    std::unique_ptr<DsmReachMatrix> reach_matrix; // nullptr until dsm_reach_matrix_enable
     std::unique_ptr<DsmGain> gain;               // nullptr until dsm_gain_enable
     int run_split = 2;          // sub-batches per dsm_batch_run (dsm_set_concurrency)
     // pinned host staging for the small per-batch tables

@@ -458,6 +458,53 @@ cudaError_t dsm_launch_reach(const DsmReachBufs &b, const DsmFieldGrid &g, const
                              const int3 s, float radius, int approach, int n_goals, const uint8_t *frontier_res, int frontier_max_clusters,
                              cudaStream_t st);
 
+// dsm_reach_matrix_* (DESIGN.md §8.13), dsm_reach.cu.  One packed result of a job on n sites (D2H, 64 + 32 n + 4 n^2 B):
+//   int32 header[DSM_RM_WORDS] | dsm_reach_site_t sites[n] | uint32 matrix[n][n]
+// The header's first nine words are those of dsm_reach_matrix_info_t; its last two carry the field's error words,
+// cleared by dsm_reach_matrix_wait.
+enum
+{
+    DSM_RM_ORIGIN = 0, // 3 words
+    DSM_RM_N_SITES = 3,
+    DSM_RM_STATUS,
+    DSM_RM_N_TRAVERSABLE,
+    DSM_RM_N_ACTIVE_TILES,
+    DSM_RM_MAX_TILES,
+    DSM_RM_ROUNDS,
+    DSM_RM_ERR_TAG = 14, // the field header's DSM_FIELD_ERR_TAG / _ERR_FRAME, copied by k_rm_slots
+    DSM_RM_ERR_FRAME,
+    DSM_RM_WORDS = 16 // 64 B
+};
+// The device buffers of one context's matrix jobs, sized by dsm_reach_matrix_enable.  Per (site, slot) the costs are a
+// tile's 512 voxels in tile-local order (x fastest), at ((size_t)site * max_tiles + slot) * 512 of each buffer.
+struct DsmReachMatrixBufs
+{
+    int voxels = 0, tiles = 0, tn[3] = {0, 0, 0};
+    int max_sites = 0, max_tiles = 0, max_rounds = 0, ctas = 0;
+    int32_t *flag = nullptr, *scan = nullptr;     // [tiles]: the tile is active, and the exclusive sum of the flags
+    int32_t *slot = nullptr;                      // [tiles]: the tile's slot, -1 when inactive
+    uint32_t *mask = nullptr;                     // [tiles][16]: the tile's traversable voxels, bit t of word t / 32
+    int32_t *tile_of = nullptr;                   // [max_tiles]: the tile of a slot
+    uint32_t *cost[2] = {nullptr, nullptr};       // [max_sites][max_tiles][512] each
+    int32_t *stamp = nullptr;                     // [max_sites][max_tiles]: the latest round a slot was scheduled for
+    int32_t *sched[2] = {nullptr, nullptr};       // [max_sites][max_tiles] each: round r's schedule is sched[r % 2]
+    int32_t *count = nullptr;                     // [max_sites][3]: site i's round-r schedule length is count[3 i + r % 3]
+    int32_t *rounds = nullptr, *reached = nullptr; // [max_sites]: the rounds with a non-empty schedule, the reached voxels
+    int32_t *sites = nullptr;                     // device [max_sites][3] the points' voxels, staged by the host
+    uint8_t *res = nullptr;                       // the packed result, room for max_sites
+    void *temp = nullptr;                         // CUB scratch of dsm_reach_matrix_temp_bytes
+    size_t temp_bytes = 0;
+    static size_t res_bytes(int n) { return 4 * (size_t)DSM_RM_WORDS + sizeof(dsm_reach_site_t) * (size_t)n + 4 * (size_t)n * n; }
+};
+// the CUB scratch of the tile scan; 0 on a CUB error
+size_t dsm_reach_matrix_temp_bytes(const DsmReachMatrixBufs &b);
+// the persistent CTAs of k_rm_round on this device
+int dsm_reach_matrix_ctas();
+// The whole job on the grids of the latest known request for the n sites' voxels already in b.sites (each axis clamped
+// to [-1, n]).  The result header must be zeroed by the caller.
+cudaError_t dsm_launch_reach_matrix(const DsmReachMatrixBufs &b, const DsmFieldGrid &g, const uint8_t *state, const int32_t *dist,
+                                    int n, float radius, int approach, cudaStream_t st);
+
 // dsm_gain_* (DESIGN.md §8.12), dsm_gain.cu.  One staged request (H2D), DsmGainView views[n_views], and one packed
 // result (D2H): int32 header[DSM_GAIN_WORDS] | dsm_view_gain_t gains[max_views].  The header's first six words are
 // those of dsm_gain_info_t; its padding carries the field's error words, cleared by dsm_gain_wait.

@@ -19,9 +19,12 @@
 //   k_reach_records  one thread per target record.
 //   k_reach_paths    one warp per reached target, lanes on the 26 neighbours and a shuffle argmin per step: a counting
 //                    walk, a cub exclusive scan of the lengths, then the writing walk.
+// The matrix job (dsm_reach_matrix_*, DESIGN.md §8.13) runs the same rounds from many sites at once; its kernels follow
+// dsm_launch_reach below and share reach_snap and reach_relax with k_reach_start and k_reach_round.
 // The kernels carry no error gate and are launched without PDL, as the other field kernels.
 #include "dsm_device.cuh"
 #include <algorithm>
+#include <cub/block/block_scan.cuh>
 #include <cub/device/device_scan.cuh>
 
 #define RC_BLOCK 256
@@ -64,17 +67,14 @@ __device__ __forceinline__ bool traversable(const uint8_t *state, const int32_t 
     return state[i] == DSM_STATE_FREE && __int_as_float(dist[i]) >= radius;
 }
 
-__global__ void __launch_bounds__(32) k_reach_start(const DsmFieldGrid g, const uint8_t *__restrict__ state, const int32_t *__restrict__ dist,
-                                                    const int32_t *__restrict__ fhdr, const int3 s, float radius, int k, int n_goals,
-                                                    int max_targets, const int32_t *__restrict__ frontier_hdr, int frontier_max_clusters,
-                                                    const int3 tn, int32_t *__restrict__ sched0, int32_t *__restrict__ stamp,
-                                                    int32_t *__restrict__ count, int32_t *__restrict__ hdr)
+// the snap of voxel s into its window (include/dsm.h): the least chamfer(u - s) << 32 | u over the window's traversable
+// voxels u, on the whole warp; ~0 when s lies outside the grid or no voxel of the window is traversable
+__device__ __forceinline__ unsigned long long reach_snap(const DsmFieldGrid &g, const uint8_t *state, const int32_t *dist, const int3 s,
+                                                         float radius, int k, int lane)
 {
-    const int lane = threadIdx.x;
     const int w = 2 * k + 1;
     unsigned long long key = ~0ull;
-    const bool in = reach_inside(g, s.x, s.y, s.z);
-    if (in)
+    if (reach_inside(g, s.x, s.y, s.z))
         for (int q = lane; q < w * w * w; q += 32)
         {
             const int dx = q % w - k, dy = q / w % w - k, dz = q / (w * w) - k;
@@ -85,7 +85,53 @@ __global__ void __launch_bounds__(32) k_reach_start(const DsmFieldGrid g, const 
             const unsigned long long c = ((unsigned long long)reach_chamfer(dx, dy, dz) << 32) | (unsigned)i;
             key = c < key ? c : key;
         }
-    key = warp_min64(key);
+    return warp_min64(key);
+}
+
+// The tile-local fixed point of the staged tile (vs: the tile and its halo, RC_H^3, voxel si of this thread, tv its
+// traversable flag, c its cost): Bellman-Ford sweeps in place until __syncthreads_or reports no change, with the halo
+// frozen; unique whatever the interleaving.  Every thread of the CTA calls it.  Returns the voxel's cost.
+__device__ __forceinline__ uint32_t reach_relax(volatile uint32_t *vs, int si, bool tv, uint32_t c)
+{
+    while (true)
+    { // only traversable voxels ever hold a finite cost, so a finite neighbour is a traversable one
+        bool changed = false;
+        if (tv)
+        {
+            uint32_t best = c;
+#pragma unroll
+            for (int dz = -1; dz <= 1; dz++)
+#pragma unroll
+                for (int dy = -1; dy <= 1; dy++)
+#pragma unroll
+                    for (int dx = -1; dx <= 1; dx++)
+                    {
+                        if (dx == 0 && dy == 0 && dz == 0) continue;
+                        const uint32_t v = vs[si + (dz * RC_H + dy) * RC_H + dx];
+                        const uint32_t w = (uint32_t)reach_chamfer(dx, dy, dz);
+                        if (v != RC_INF && v + w < best) best = v + w;
+                    }
+            if (best < c)
+            {
+                c = best;
+                vs[si] = c;
+                changed = true;
+            }
+        }
+        if (!__syncthreads_or(changed)) break;
+    }
+    return c;
+}
+
+__global__ void __launch_bounds__(32) k_reach_start(const DsmFieldGrid g, const uint8_t *__restrict__ state, const int32_t *__restrict__ dist,
+                                                    const int32_t *__restrict__ fhdr, const int3 s, float radius, int k, int n_goals,
+                                                    int max_targets, const int32_t *__restrict__ frontier_hdr, int frontier_max_clusters,
+                                                    const int3 tn, int32_t *__restrict__ sched0, int32_t *__restrict__ stamp,
+                                                    int32_t *__restrict__ count, int32_t *__restrict__ hdr)
+{
+    const int lane = threadIdx.x;
+    const bool in = reach_inside(g, s.x, s.y, s.z);
+    const unsigned long long key = reach_snap(g, state, dist, s, radius, k, lane);
     if (lane != 0) return;
     const int u = key == ~0ull ? -1 : (int)(unsigned)key;
     for (int d = 0; d < 3; d++) hdr[DSM_REACH_ORIGIN + d] = g.o[d];
@@ -158,34 +204,7 @@ __global__ void __launch_bounds__(RC_TILE) k_reach_round(const DsmFieldGrid g, c
         const bool tv = inside && trav[i];
         __syncthreads();
         const uint32_t c0 = s[si];
-        uint32_t c = c0;
-        while (true)
-        { // only traversable voxels ever hold a finite cost, so a finite neighbour is a traversable one
-            bool changed = false;
-            if (tv)
-            {
-                uint32_t best = c;
-#pragma unroll
-                for (int dz = -1; dz <= 1; dz++)
-#pragma unroll
-                    for (int dy = -1; dy <= 1; dy++)
-#pragma unroll
-                        for (int dx = -1; dx <= 1; dx++)
-                        {
-                            if (dx == 0 && dy == 0 && dz == 0) continue;
-                            const uint32_t v = vs[si + (dz * RC_H + dy) * RC_H + dx];
-                            const uint32_t w = (uint32_t)reach_chamfer(dx, dy, dz);
-                            if (v != RC_INF && v + w < best) best = v + w;
-                        }
-                if (best < c)
-                {
-                    c = best;
-                    vs[si] = c;
-                    changed = true;
-                }
-            }
-            if (!__syncthreads_or(changed)) break;
-        }
+        const uint32_t c = reach_relax(vs, si, tv, c0);
         if (inside) cout[i] = c;
         // round 0's only tile holds the seeded start: it counts as changed even when none of its other voxels is reached,
         // or a start cut off from the rest of its tile would end the job after one round
@@ -446,5 +465,290 @@ cudaError_t dsm_launch_reach(const DsmReachBufs &b, const DsmFieldGrid &g, const
     if (e == cudaSuccess) e = cub::DeviceScan::ExclusiveSum(b.temp, n, b.len, b.ofs, b.max_targets, st);
     if (e != cudaSuccess) return e;
     k_reach_paths<true><<<warp_blocks, RC_BLOCK, 0, st>>>(g, b.trav, b.cost[0], b.max_targets, b.max_path, b.len, b.ofs, rec, path, hdr);
+    return cudaGetLastError();
+}
+
+// ---- the matrix job (dsm_reach_matrix_*, DESIGN.md §8.13): the reach job's rounds from many sites at once, on the
+// active tiles only ----
+//   k_rm_tiles    one CTA per tile, one voxel per thread: the tile's traversable mask (a ballot per warp), its active
+//                 flag (__syncthreads_count) and the traversable count.
+//   (a cub exclusive scan of the flags)
+//   k_rm_slots    one thread per tile: slot[tile] (-1 inactive), tile_of[slot] for slots below max_tiles, and the header.
+//   k_rm_sites    one warp per site: the snap, the site record's first words, and round 0's schedule, u's slot.
+//   k_rm_init     one CTA per (site, slot): both cost buffers at UINT32_MAX but the site's own voxel at 0.
+//   k_rm_round    launched max_rounds times on persistent CTAs; each forms the exclusive prefix of the sites' round-r
+//                 schedule lengths and walks the (site, slot) items, one per CTA, exactly as k_reach_round walks tiles:
+//                 stage, reach_relax, write, and a changed tile schedules itself and its active neighbours per site.
+//   k_rm_reached  one CTA per (site, slot): the site's reached count.
+//   k_rm_gather   one thread per matrix entry; thread (i, 0) finishes site i's record.
+// No settle step: every tile a round leaves out holds equal buffers (a tile that changed schedules itself), so buffer
+// max_rounds % 2 holds the latest cost of every voxel, and the last two kernels read it.
+#define RM_SITES DSM_REACH_MATRIX_MAX_SITES
+#define RM_WORDS (RC_TILE / 32) // mask words per tile
+static_assert(sizeof(dsm_reach_site_t) == 32 && sizeof(dsm_reach_matrix_info_t) == 64, "dsm_reach_matrix layouts");
+static_assert(DSM_RM_WORDS * 4 == sizeof(dsm_reach_matrix_info_t) && DSM_RM_ROUNDS == 8, "the header starts with the info");
+static_assert(RM_SITES == 2 * RC_TILE, "k_rm_round scans two sites per thread");
+
+__device__ __forceinline__ int3 rm_tile_xyz(const int3 tn, int tile) { return make_int3(tile % tn.x, tile / tn.x % tn.y, tile / (tn.x * tn.y)); }
+// the tile of voxel u and u's tile-local index
+__device__ __forceinline__ int rm_tile_of_voxel(const DsmFieldGrid &g, const int3 tn, int u, int &local)
+{
+    const int x = u % g.n[0], y = u / g.n[0] % g.n[1], z = u / (g.n[0] * g.n[1]);
+    local = ((z % RC_T) * RC_T + y % RC_T) * RC_T + x % RC_T;
+    return ((z / RC_T) * tn.y + y / RC_T) * tn.x + x / RC_T;
+}
+
+__global__ void __launch_bounds__(RC_TILE) k_rm_tiles(const DsmFieldGrid g, const int3 tn, const uint8_t *__restrict__ state,
+                                                      const int32_t *__restrict__ dist, float radius, int32_t *__restrict__ flag,
+                                                      uint32_t *__restrict__ mask, int32_t *hdr)
+{
+    const int tile = blockIdx.x, t = threadIdx.x;
+    const int3 tc = rm_tile_xyz(tn, tile);
+    const int x = tc.x * RC_T + t % RC_T, y = tc.y * RC_T + t / RC_T % RC_T, z = tc.z * RC_T + t / (RC_T * RC_T);
+    const bool tv = reach_inside(g, x, y, z) && traversable(state, dist, reach_index(g, x, y, z), radius);
+    const unsigned b = __ballot_sync(0xffffffffu, tv);
+    if ((t & 31) == 0) mask[(size_t)tile * RM_WORDS + t / 32] = b;
+    const int n = __syncthreads_count(tv);
+    if (t == 0)
+    {
+        flag[tile] = n > 0;
+        if (n > 0) atomicAdd(&hdr[DSM_RM_N_TRAVERSABLE], n);
+    }
+}
+
+__global__ void __launch_bounds__(RC_BLOCK) k_rm_slots(const DsmFieldGrid g, int tiles, int max_tiles, int n_sites, const int32_t *__restrict__ flag,
+                                                       const int32_t *__restrict__ scan, const int32_t *__restrict__ fhdr,
+                                                       int32_t *__restrict__ slot, int32_t *__restrict__ tile_of, int32_t *hdr)
+{
+    const int tile = blockIdx.x * RC_BLOCK + threadIdx.x;
+    if (tile >= tiles) return;
+    const int s = scan[tile];
+    slot[tile] = flag[tile] ? s : -1;
+    if (flag[tile] && s < max_tiles) tile_of[s] = tile;
+    if (tile == tiles - 1)
+    {
+        const int n_active = s + flag[tile];
+        for (int d = 0; d < 3; d++) hdr[DSM_RM_ORIGIN + d] = g.o[d];
+        hdr[DSM_RM_N_SITES] = n_sites;
+        hdr[DSM_RM_STATUS] = n_active > max_tiles;
+        hdr[DSM_RM_N_ACTIVE_TILES] = n_active;
+        hdr[DSM_RM_MAX_TILES] = max_tiles;
+        hdr[DSM_RM_ERR_TAG] = fhdr[DSM_FIELD_ERR_TAG];
+        hdr[DSM_RM_ERR_FRAME] = fhdr[DSM_FIELD_ERR_FRAME];
+    }
+}
+
+__global__ void __launch_bounds__(RC_BLOCK) k_rm_sites(const DsmFieldGrid g, const int3 tn, const uint8_t *__restrict__ state,
+                                                       const int32_t *__restrict__ dist, const int32_t *__restrict__ sites, int n_sites,
+                                                       float radius, int k, int max_tiles, const int32_t *__restrict__ slot,
+                                                       int32_t *__restrict__ sched0, int32_t *__restrict__ stamp, int32_t *__restrict__ count,
+                                                       const int32_t *hdr, dsm_reach_site_t *__restrict__ rec)
+{
+    const int i = blockIdx.x * (RC_BLOCK / 32) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+    if (i >= n_sites) return;
+    const int3 s = make_int3(sites[3 * i], sites[3 * i + 1], sites[3 * i + 2]);
+    const unsigned long long key = reach_snap(g, state, dist, s, radius, k, lane);
+    if (lane != 0) return;
+    const int u = key == ~0ull ? -1 : (int)(unsigned)key;
+    dsm_reach_site_t r;
+    r.voxel = u;
+    r.status = !reach_inside(g, s.x, s.y, s.z) ? 1 : u < 0 ? 2 : 0;
+    r.approach = u < 0 ? 0 : (int)(key >> 32);
+    r.rounds = r.converged = r.n_reached = 0; // k_rm_gather fills them
+    r.reserved[0] = r.reserved[1] = 0;
+    rec[i] = r;
+    const bool seeded = u >= 0 && hdr[DSM_RM_STATUS] == 0;
+    count[3 * i + 1] = count[3 * i + 2] = 0;
+    count[3 * i] = seeded;
+    if (seeded)
+    {
+        int local;
+        const int a = slot[rm_tile_of_voxel(g, tn, u, local)];
+        sched0[(size_t)i * max_tiles] = a;
+        stamp[(size_t)i * max_tiles + a] = 0;
+    }
+}
+
+__global__ void __launch_bounds__(RC_TILE) k_rm_init(const DsmFieldGrid g, const int3 tn, int n_sites, int max_tiles, const int32_t *__restrict__ slot,
+                                                     const dsm_reach_site_t *__restrict__ rec, const int32_t *__restrict__ hdr,
+                                                     uint32_t *__restrict__ c0, uint32_t *__restrict__ c1)
+{
+    if (hdr[DSM_RM_STATUS] != 0) return;
+    const int n_active = hdr[DSM_RM_N_ACTIVE_TILES], t = threadIdx.x;
+    for (long long q = blockIdx.x; q < (long long)n_sites * n_active; q += gridDim.x)
+    {
+        const int i = (int)(q / n_active), a = (int)(q % n_active);
+        const int u = rec[i].voxel;
+        int local = -1;
+        const bool own = u >= 0 && slot[rm_tile_of_voxel(g, tn, u, local)] == a;
+        const uint32_t c = own && local == t ? 0u : RC_INF;
+        const size_t at = ((size_t)i * max_tiles + a) * RC_TILE + t;
+        c0[at] = c;
+        c1[at] = c;
+    }
+}
+
+__global__ void __launch_bounds__(RC_TILE) k_rm_round(const int3 tn, int n_sites, int max_tiles, const int32_t *__restrict__ slot,
+                                                      const int32_t *__restrict__ tile_of, const uint32_t *__restrict__ mask,
+                                                      const uint32_t *__restrict__ cin, uint32_t *__restrict__ cout,
+                                                      const int32_t *__restrict__ sched_in, int32_t *__restrict__ sched_out,
+                                                      int32_t *__restrict__ stamp, int32_t *count, int32_t *__restrict__ rounds, int32_t *hdr, int r)
+{
+    typedef cub::BlockScan<int, RC_TILE> Scan;
+    __shared__ uint32_t s[RC_H * RC_H * RC_H];
+    __shared__ int pre[RM_SITES + 1]; // the exclusive prefix of the sites' schedule lengths; pre[n_sites] the total
+    __shared__ int nb[27];            // the item's neighbour slots (-1 inactive or outside), 13 its own
+    __shared__ typename Scan::TempStorage scan_tmp;
+    const int t = threadIdx.x;
+    int len[2];
+    for (int e = 0; e < 2; e++) len[e] = 2 * t + e < n_sites ? count[3 * (2 * t + e) + r % 3] : 0;
+    int total;
+    Scan(scan_tmp).ExclusiveSum(len, len, total);
+    for (int e = 0; e < 2; e++)
+        if (2 * t + e < n_sites) pre[2 * t + e] = len[e];
+    if (t == 0) pre[n_sites] = total;
+    if (blockIdx.x == 0)
+    {
+        for (int i = t; i < n_sites; i += RC_TILE)
+        {
+            count[3 * i + (r + 2) % 3] = 0; // round r - 1's count; round r + 1 adds to it
+            if (count[3 * i + r % 3] > 0) rounds[i] = r + 1;
+        }
+        if (t == 0 && total > 0) hdr[DSM_RM_ROUNDS] = r + 1;
+    }
+    if (total == 0) return;
+    __syncthreads();
+    const int lx = t % RC_T, ly = t / RC_T % RC_T, lz = t / (RC_T * RC_T);
+    const int si = ((lz + 1) * RC_H + ly + 1) * RC_H + lx + 1;
+    volatile uint32_t *vs = s;
+    for (int q = blockIdx.x; q < total; q += gridDim.x)
+    {
+        int lo = 0, hi = n_sites - 1; // the last site i with pre[i] <= q: the one whose schedule holds item q
+        while (lo < hi)
+        {
+            const int mid = (lo + hi + 1) / 2;
+            if (pre[mid] <= q) lo = mid;
+            else hi = mid - 1;
+        }
+        const int i = lo;
+        const size_t row = (size_t)i * max_tiles;
+        const int a = sched_in[row + q - pre[i]], tile = tile_of[a];
+        const int3 tc = rm_tile_xyz(tn, tile);
+        if (t < 27)
+        {
+            const int ax = tc.x + t % 3 - 1, ay = tc.y + t / 3 % 3 - 1, az = tc.z + t / 9 - 1;
+            nb[t] = (unsigned)ax < (unsigned)tn.x && (unsigned)ay < (unsigned)tn.y && (unsigned)az < (unsigned)tn.z
+                        ? slot[(az * tn.y + ay) * tn.x + ax]
+                        : -1;
+        }
+        __syncthreads();
+        for (int h = t; h < RC_H * RC_H * RC_H; h += RC_TILE)
+        { // halo coordinate 0 is the lower neighbour's voxel 7, RC_H - 1 the upper neighbour's voxel 0
+            const int hx = h % RC_H, hy = h / RC_H % RC_H, hz = h / (RC_H * RC_H);
+            const int d = (hx > 0) + (hx == RC_H - 1) + 3 * ((hy > 0) + (hy == RC_H - 1)) + 9 * ((hz > 0) + (hz == RC_H - 1));
+            const int local = (((hz + RC_T - 1) & (RC_T - 1)) * RC_T + ((hy + RC_T - 1) & (RC_T - 1))) * RC_T + ((hx + RC_T - 1) & (RC_T - 1));
+            const int b = nb[d];
+            s[h] = b < 0 ? RC_INF : cin[(row + b) * RC_TILE + local];
+        }
+        const bool tv = (mask[(size_t)tile * RM_WORDS + t / 32] >> (t % 32)) & 1u;
+        __syncthreads();
+        const uint32_t c0 = s[si];
+        const uint32_t c = reach_relax(vs, si, tv, c0);
+        cout[(row + a) * RC_TILE + t] = c;
+        // as k_reach_round, round 0's tile is the seeded start's and counts as changed; only active tiles are listed,
+        // since an inactive one holds UINT32_MAX for good
+        if ((__syncthreads_or(c != c0) || r == 0) && t < 27)
+        {
+            const int b = nb[t];
+            if (b >= 0 && atomicMax(&stamp[row + b], r + 1) < r + 1) sched_out[row + atomicAdd(&count[3 * i + (r + 1) % 3], 1)] = b;
+        }
+        __syncthreads(); // the next item overwrites s and nb
+    }
+}
+
+__global__ void __launch_bounds__(RC_TILE) k_rm_reached(int n_sites, int max_tiles, const uint32_t *__restrict__ cost, const int32_t *__restrict__ hdr,
+                                                        int32_t *reached)
+{
+    if (hdr[DSM_RM_STATUS] != 0) return;
+    const int n_active = hdr[DSM_RM_N_ACTIVE_TILES];
+    for (long long q = blockIdx.x; q < (long long)n_sites * n_active; q += gridDim.x)
+    {
+        const int i = (int)(q / n_active), a = (int)(q % n_active);
+        const int n = __syncthreads_count(cost[((size_t)i * max_tiles + a) * RC_TILE + threadIdx.x] != RC_INF);
+        if (threadIdx.x == 0 && n > 0) atomicAdd(&reached[i], n);
+    }
+}
+
+__global__ void __launch_bounds__(RC_BLOCK) k_rm_gather(const DsmFieldGrid g, const int3 tn, int n_sites, int max_tiles, int max_rounds,
+                                                        const int32_t *__restrict__ slot, const uint32_t *__restrict__ cost,
+                                                        const int32_t *__restrict__ count, const int32_t *__restrict__ rounds,
+                                                        const int32_t *__restrict__ reached, const int32_t *__restrict__ hdr,
+                                                        dsm_reach_site_t *rec, uint32_t *__restrict__ matrix)
+{
+    const long long e = (long long)blockIdx.x * RC_BLOCK + threadIdx.x;
+    if (e >= (long long)n_sites * n_sites) return;
+    const int i = (int)(e / n_sites), j = (int)(e % n_sites);
+    const bool ok = hdr[DSM_RM_STATUS] == 0;
+    const int ui = rec[i].voxel, uj = rec[j].voxel; // -1 unless the site's status is 0
+    uint32_t m = RC_INF;
+    if (ok && ui >= 0 && uj >= 0)
+    {
+        int local;
+        const int a = slot[rm_tile_of_voxel(g, tn, uj, local)];
+        m = cost[((size_t)i * max_tiles + a) * RC_TILE + local];
+    }
+    matrix[e] = m;
+    if (j == 0)
+    { // a site without a start is a reach job that reaches nothing: converged after 0 rounds; a cut job ran no round
+        rec[i].rounds = ok ? rounds[i] : 0;
+        rec[i].converged = ok && count[3 * i + max_rounds % 3] == 0;
+        rec[i].n_reached = ok ? reached[i] : 0;
+    }
+}
+
+int dsm_reach_matrix_ctas()
+{
+    int dev = 0, sms = 0, per = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess ||
+        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per, k_rm_round, RC_TILE, 0) != cudaSuccess)
+        return 0;
+    return sms * per;
+}
+
+size_t dsm_reach_matrix_temp_bytes(const DsmReachMatrixBufs &b)
+{
+    size_t n = 0;
+    if (cub::DeviceScan::ExclusiveSum(nullptr, n, b.flag, b.scan, b.tiles, (cudaStream_t)0) != cudaSuccess) return 0;
+    return std::max(n, (size_t)1);
+}
+
+cudaError_t dsm_launch_reach_matrix(const DsmReachMatrixBufs &b, const DsmFieldGrid &g, const uint8_t *state, const int32_t *dist,
+                                    int n, float radius, int approach, cudaStream_t st)
+{
+    int32_t *hdr = reinterpret_cast<int32_t *>(b.res);
+    auto *rec = reinterpret_cast<dsm_reach_site_t *>(b.res + 4 * DSM_RM_WORDS);
+    auto *matrix = reinterpret_cast<uint32_t *>(b.res + 4 * DSM_RM_WORDS + sizeof(dsm_reach_site_t) * (size_t)n);
+    const int3 tn = make_int3(b.tn[0], b.tn[1], b.tn[2]);
+    const int32_t *fieldhdr = dist + dsm_field_header((size_t)b.voxels);
+    cudaError_t e = cudaMemsetAsync(b.stamp, 0xff, 4 * (size_t)n * b.max_tiles, st);
+    if (e == cudaSuccess) e = cudaMemsetAsync(b.rounds, 0, 4 * (size_t)n, st);
+    if (e == cudaSuccess) e = cudaMemsetAsync(b.reached, 0, 4 * (size_t)n, st);
+    if (e != cudaSuccess) return e;
+    k_rm_tiles<<<b.tiles, RC_TILE, 0, st>>>(g, tn, state, dist, radius, b.flag, b.mask, hdr);
+    e = cudaGetLastError();
+    size_t tb = b.temp_bytes;
+    if (e == cudaSuccess) e = cub::DeviceScan::ExclusiveSum(b.temp, tb, b.flag, b.scan, b.tiles, st);
+    if (e != cudaSuccess) return e;
+    k_rm_slots<<<rc_blocks(b.tiles), RC_BLOCK, 0, st>>>(g, b.tiles, b.max_tiles, n, b.flag, b.scan, fieldhdr, b.slot, b.tile_of, hdr);
+    k_rm_sites<<<rc_blocks(32ll * n), RC_BLOCK, 0, st>>>(g, tn, state, dist, b.sites, n, radius, approach, b.max_tiles, b.slot, b.sched[0],
+                                                         b.stamp, b.count, hdr, rec);
+    k_rm_init<<<b.ctas, RC_TILE, 0, st>>>(g, tn, n, b.max_tiles, b.slot, rec, hdr, b.cost[0], b.cost[1]);
+    for (int r = 0; r < b.max_rounds; r++)
+        k_rm_round<<<b.ctas, RC_TILE, 0, st>>>(tn, n, b.max_tiles, b.slot, b.tile_of, b.mask, b.cost[r % 2], b.cost[(r + 1) % 2],
+                                               b.sched[r % 2], b.sched[(r + 1) % 2], b.stamp, b.count, b.rounds, hdr, r);
+    const uint32_t *last = b.cost[b.max_rounds % 2];
+    k_rm_reached<<<b.ctas, RC_TILE, 0, st>>>(n, b.max_tiles, last, hdr, b.reached);
+    k_rm_gather<<<rc_blocks((long long)n * n), RC_BLOCK, 0, st>>>(g, tn, n, b.max_tiles, b.max_rounds, b.slot, last, b.count, b.rounds,
+                                                                  b.reached, hdr, rec, matrix);
     return cudaGetLastError();
 }

@@ -749,6 +749,61 @@ int dsm_reach_enqueue(dsm_ctx *ctx, const double start[3], float radius, int app
 int dsm_reach_wait(dsm_ctx *ctx, dsm_reach_info_t *info, const dsm_reach_target_t **targets, const int32_t **path,
                    const uint32_t **cost);
 
+/* ---- travel costs between many sites: the cost matrix of an exploration tour (DESIGN.md §8.13) ----
+ * A matrix job reads the state and distance grids of the latest field request, which must be a known one, in stream
+ * order behind it, with that request's origin o and voxel edge v captured at the job's enqueue, as a reach job does.
+ * It shares no buffer with the reach job.  Everything not restated here is §8.11's: traversable, the moves and their
+ * weights, the approach window, the 8x8x8 tiles and the round rule with round 0's seeded start tile.
+ *   Sites: site i is the fp64 point points[3i..3i+2], snapped exactly as a reach job snaps its start: voxel u_i,
+ *   status_i (0 ok, 1 outside the grid, 2 no traversable voxel in the window) and approach_i = chamfer(u_i - s_i).  A
+ *   traversable voxel's centre ((o + x) + 0.5) v snaps to itself.  Points may repeat.
+ *   Active tiles: the tiles holding a traversable voxel, numbered in tile order; n_active_tiles of them.  With
+ *   n_active_tiles > max_tiles the job has status 1 (capacity): every matrix entry is UINT32_MAX and every site record
+ *   holds its snap with rounds = converged = n_reached = 0.  The cut depends on the grid and the radius only.
+ *   Costs: for a site of status 0, cost_i is the cost grid of a reach job started at u_i with the same radius, approach
+ *   and max_rounds, bit for bit, unconverged values included; its rounds, converged and n_reached are that job's.  A
+ *   site of status 1 or 2 reaches nothing, with rounds 0 and converged 1, as such a reach job.
+ *   Matrix: M[i][j] = cost_i[u_j] when the job and both sites have status 0, UINT32_MAX otherwise; M[i][i] = 0, and M
+ *   is symmetric between converged sites.  The approaches are not added.
+ *   Header: the origin, n_sites, status, n_traversable, n_active_tiles, max_tiles and rounds (the launches whose
+ *   schedule was non-empty for some site).
+ *
+ *   dsm_reach_matrix_enable   once, after dsm_views_enable (DSM_E_STATE otherwise, and when called twice).
+ *                             DSM_E_INVALID for max_sites outside [1, 1024], max_tiles outside [1, tiles of the grid],
+ *                             max_rounds outside [1, 65536], a grid above 2^27 voxels, or cost buffers (4 KB per site
+ *                             and tile) above 2^34 bytes.  DSM_E_NOMEM with nothing kept.
+ *   dsm_reach_matrix_enqueue  asynchronous on the context's stream, never waits: the points' voxels staged into pinned
+ *                             memory and copied with one H2D copy, the kernels (max_rounds round launches; a round with
+ *                             an empty schedule exits at once), one D2H copy of 64 + 32 n + 4 n^2 bytes and the event.
+ *                             DSM_E_STATE before dsm_reach_matrix_enable, before any field request, when the latest
+ *                             field request is not a known one, and while a job is in flight.  DSM_E_INVALID for a
+ *                             non-finite point, a radius that is not finite and >= 0, an approach outside [0, 4],
+ *                             n_points outside [1, max_sites], or n_points x max_tiles x max_rounds above 2^32.
+ *   dsm_reach_matrix_wait     waits for that job only.  *sites (n_sites records) and *matrix (n_sites x n_sites, row i
+ *                             from site i) are the context's pinned results, valid until the next
+ *                             dsm_reach_matrix_enqueue; any out-pointer may be NULL.  DSM_E_CAPACITY with valid results
+ *                             after a rejected frame, without clearing the error, as dsm_reach_wait.  DSM_E_STATE with
+ *                             no job enqueued. */
+typedef struct dsm_reach_site_t
+{
+    int32_t voxel, status, approach;   /* voxel -1 and approach 0 unless status 0 */
+    int32_t rounds, converged, n_reached;
+    int32_t reserved[2];               /* 0 */
+} dsm_reach_site_t;                    /* 32 B */
+typedef struct dsm_reach_matrix_info_t
+{
+    int32_t origin[3];
+    int32_t n_sites, status;
+    int32_t n_traversable, n_active_tiles, max_tiles, rounds;
+    int32_t reserved[7];               /* 0 */
+} dsm_reach_matrix_info_t;             /* 64 B */
+#define DSM_REACH_MATRIX_MAX_SITES 1024
+#define DSM_REACH_MATRIX_MAX_COST_BYTES (1ull << 34)
+#define DSM_REACH_MATRIX_MAX_WORK (1ull << 32)
+int dsm_reach_matrix_enable(dsm_ctx *ctx, int max_sites, int max_tiles, int max_rounds);
+int dsm_reach_matrix_enqueue(dsm_ctx *ctx, const double *points, int n_points, float radius, int approach);
+int dsm_reach_matrix_wait(dsm_ctx *ctx, dsm_reach_matrix_info_t *info, const dsm_reach_site_t **sites, const uint32_t **matrix);
+
 /* ---- view gain: the unknown, frontier and cluster voxels a camera pose would see (DESIGN.md §8.12) ----
  * A gain job reads the state grid of the latest field request, which must be a known one, in stream order behind it,
  * with that request's origin o and voxel edge v (widened to fp64) captured at the job's enqueue, and (with clusters)

@@ -83,6 +83,11 @@
 // lets reach() find paths through the known free space of the latest fused frame's field on the device (DESIGN.md
 // §8.11): the travel cost from a start point to goal points and, after a frontiers() call on that frame, to every
 // frontier cluster, with each target's viewpoint and path, one enqueue and one wait.
+// In which order should the viewpoints be visited?  enable_reach_matrix(max_sites, max_tiles, max_rounds), after
+// enable_known_space, lets reach_matrix() price an exploration tour on the device (DESIGN.md §8.13): the travel costs
+// between every pair of up to max_sites points through the known free space of the latest fused frame's field, one
+// enqueue and one wait.  A planner chains frontiers(), then reach(with_frontiers) from the robot for each cluster's
+// viewpoint, then reach_matrix over the robot's position and those viewpoints, and hands the matrix to its tour solver.
 // What would the robot see from there?  enable_view_gain(max_views), after enable_known_space, lets view_gain() score
 // candidate camera poses against the latest fused frame's known field on the device (DESIGN.md §8.12): per pose, with
 // the node's own intrinsics, the frustum voxels and the free, unknown, occupied, frontier and (after a frontiers() call
@@ -590,6 +595,40 @@ class SurfelMapNode
             path.assign(p, p + info.n_path_voxels);
         }
         return ctx_.done(rc, "reach");
+    }
+
+    // ---- travel costs between many points of the latest fused frame's field (DESIGN.md §8.13) ----
+    // once, after enable_known_space: the most sites of one call, the most active tiles of a field, and the rounds
+    int enable_reach_matrix(int max_sites, int max_tiles, int max_rounds)
+    {
+        return ctx_.run("enable_reach_matrix", [&] { return dsm_reach_matrix_enable(ctx_.ctx, max_sites, max_tiles, max_rounds); });
+    }
+    // the travel costs between the points (xyz doubles, points.size() / 3 of them) through voxels free and at least
+    // `radius` from anything not known to be free (include/dsm.h): sites receives one record per point and matrix the
+    // n x n costs, row i from point i.  Chained after reach(with_frontiers), the points are the robot and the targets'
+    // viewpoints (their voxel centres ((origin + x) + 0.5) * voxel snap to themselves).  DSM_E_STATE without known
+    // space, before any field and after load_state* until the next fused frame; DSM_E_CAPACITY with the costs of the
+    // last applied frame's field, as distance_field().
+    int reach_matrix(const std::vector<double> &points, float radius, int approach, dsm_reach_matrix_info_t &info,
+                     std::vector<dsm_reach_site_t> &sites, std::vector<uint32_t> &matrix)
+    {
+        sites.clear();
+        matrix.clear();
+        info = dsm_reach_matrix_info_t();
+        if (!ctx_.ready("reach_matrix")) return ctx_.err;
+        if (known_.empty() || !field_exists_) return ctx_.done(DSM_E_STATE, "reach_matrix");
+        if (points.size() % 3 != 0) return ctx_.done(DSM_E_INVALID, "reach_matrix");
+        int rc = dsm_reach_matrix_enqueue(ctx_.ctx, points.data(), (int)(points.size() / 3), radius, approach);
+        if (rc != DSM_OK) return ctx_.done(rc, "reach_matrix");
+        const dsm_reach_site_t *s = nullptr;
+        const uint32_t *m = nullptr;
+        rc = dsm_reach_matrix_wait(ctx_.ctx, &info, &s, &m);
+        if (rc == DSM_OK || rc == DSM_E_CAPACITY)
+        {
+            sites.assign(s, s + info.n_sites);
+            matrix.assign(m, m + (size_t)info.n_sites * info.n_sites);
+        }
+        return ctx_.done(rc, "reach_matrix");
     }
 
     // ---- view gain against the known field of the latest fused frame (DESIGN.md §8.12) ----
