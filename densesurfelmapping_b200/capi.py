@@ -38,6 +38,7 @@ EXPORTS = [
     "dsm_frontier_enable", "dsm_frontier_enqueue", "dsm_frontier_wait", "dsm_debug_field_load_state",
     "dsm_reach_enable", "dsm_reach_enqueue", "dsm_reach_wait", "dsm_reach_matrix_enable", "dsm_reach_matrix_enqueue",
     "dsm_reach_matrix_wait", "dsm_gain_enable", "dsm_gain_enqueue", "dsm_gain_wait",
+    "dsm_tour_enable", "dsm_tour_enqueue", "dsm_tour_wait",
     "dsm_inactive_segments", "dsm_inactive_load", "dsm_map_save", "dsm_map_load", "dsm_map_peek",
     "dsm_checkpoint_enable", "dsm_checkpoint_enqueue", "dsm_checkpoint_wait", "dsm_debug_checkpoint_drain_ctas",
     "dsm_checkpoint_enqueue_incremental", "dsm_map_load_journal", "dsm_map_peek_journal", "dsm_journal_materialize",
@@ -86,6 +87,10 @@ VIEW_GAIN_DTYPE = np.dtype([("n_frustum", "<i4"), ("n_free", "<i4"), ("n_unknown
                             ("n_cluster", "<i4"), ("status", "<i4"), ("reserved", "<i4")])
 GAIN_INFO_DTYPE = np.dtype([("origin", "<i4", 3), ("n_views", "<i4"), ("n_clusters_table", "<i4"), ("unknown_blocks", "<i4"),
                             ("reserved", "<i4", 2)])
+# dsm_tour_wait's records (include/dsm.h): the header (64 B) and a start (16 B)
+TOUR_INFO_DTYPE = np.dtype([("n_sites", "<i4"), ("n_included", "<i4"), ("open", "<i4"), ("n_starts", "<i4"), ("max_passes", "<i4"),
+                            ("best_start", "<i4"), ("best_cost", "<i8"), ("seed", "<u8"), ("n_infinite", "<i4"), ("reserved", "<i4", 5)])
+TOUR_START_DTYPE = np.dtype([("cost", "<i8"), ("passes", "<i4"), ("converged", "<i4")])
 
 
 class DsmGainCamera(ctypes.Structure):
@@ -170,6 +175,9 @@ def load_library():
     L.dsm_gain_enable.argtypes = [vp, ci]
     L.dsm_gain_enqueue.argtypes = [vp, ctypes.POINTER(DsmGainCamera), vp, vp, ci]
     L.dsm_gain_wait.argtypes = [vp, vp, ctypes.POINTER(vp)]
+    L.dsm_tour_enable.argtypes = [vp, ci, ci]
+    L.dsm_tour_enqueue.argtypes = [vp, vp, ci, ci, ci, ci, ctypes.c_uint64]
+    L.dsm_tour_wait.argtypes = [vp, vp, ctypes.POINTER(vp), ctypes.POINTER(vp)]
     L.dsm_inactive_reserve.argtypes = [vp, ci]
     L.dsm_inactive_retire.argtypes = [vp, ci, ctypes.POINTER(ci)]
     L.dsm_inactive_reactivate.argtypes = [vp, ci, ctypes.POINTER(ci)]
@@ -801,6 +809,30 @@ class Context:
             err.gain = (i, g)
             raise err
         return i, g
+
+    # ---- the order of an exploration tour over a travel-cost matrix ----
+    def tour_enable(self, max_sites, max_starts):
+        self._ck(self.lib.dsm_tour_enable(self.h, int(max_sites), int(max_starts)))
+
+    def tour_enqueue(self, matrix, open_, n_starts, max_passes, seed):
+        """matrix: (n, n) uint32 costs, row i from site i (UINT32_MAX: no path), such as reach_matrix_wait's."""
+        m = np.ascontiguousarray(matrix, np.uint32)
+        if m.ndim != 2 or m.shape[0] != m.shape[1]:
+            raise ValueError(f"a square matrix, not {m.shape}")
+        self._ck(self.lib.dsm_tour_enqueue(self.h, m.ctypes.data if m.size else None, m.shape[0], int(open_), int(n_starts),
+                                           int(max_passes), int(seed)))
+
+    def tour_wait(self):
+        """(info, starts, order): numpy copies of the context's pinned results, a TOUR_INFO_DTYPE record,
+        TOUR_START_DTYPE (n_starts,) and the int32 order (n_sites,), -1 past n_included."""
+        ps, po = ctypes.c_void_p(), ctypes.c_void_p()
+        info = np.zeros(1, TOUR_INFO_DTYPE)
+        self._ck(self.lib.dsm_tour_wait(self.h, info.ctypes.data, ctypes.byref(ps), ctypes.byref(po)))
+        i = info[0]
+        k, n = int(i["n_starts"]), int(i["n_sites"])
+        starts = np.frombuffer((ctypes.c_uint8 * (k * TOUR_START_DTYPE.itemsize)).from_address(ps.value), dtype=TOUR_START_DTYPE).copy()
+        order = np.frombuffer((ctypes.c_uint8 * (4 * n)).from_address(po.value), dtype=np.int32).copy()
+        return i, starts, order
 
     # ---- planner queries against the latest field ----
     def field_query_enable(self, max_points, max_trajectories, max_waypoints):

@@ -2227,6 +2227,69 @@ extern "C" int dsm_gain_wait(dsm_ctx *ctx, dsm_gain_info_t *info, const dsm_view
     return DSM_E_CAPACITY;
 }
 
+// ---- the order of an exploration tour (include/dsm.h, DESIGN.md §8.14) ----
+extern "C" int dsm_tour_enable(dsm_ctx *ctx, int max_sites, int max_starts)
+{
+    if (!ctx) return DSM_E_INVALID;
+    if (ctx->tour) return DSM_E_STATE;
+    if (max_sites < 1 || max_sites > DSM_TOUR_MAX_SITES || max_starts < 1 || max_starts > DSM_TOUR_MAX_STARTS) return DSM_E_INVALID;
+    CK(cudaSetDevice(ctx->device));
+    auto tr = std::make_unique<DsmTour>();
+    tr->max_sites = max_sites, tr->max_starts = max_starts;
+    const size_t entries = (size_t)max_sites * max_sites, res = dsm_tour_res_bytes(max_starts, max_sites);
+    CudaOwner &o = tr->own;
+    cudaError_t e = o.host(&tr->matrix_host, entries);
+    if (e == cudaSuccess) e = o.device(&tr->matrix, entries);
+    if (e == cudaSuccess) e = o.device(&tr->tours, (size_t)max_starts * max_sites);
+    if (e == cudaSuccess) e = o.device(&tr->res, res);
+    if (e == cudaSuccess) e = o.host(&tr->res_host, res);
+    if (e == cudaSuccess) e = o.event(&tr->ev);
+    if (e != cudaSuccess)
+    {
+        cudaGetLastError();
+        return DSM_E_NOMEM; // nothing is kept: a later call may try again
+    }
+    ctx->tour = std::move(tr);
+    return DSM_OK;
+}
+
+// Enqueue only: the matrix staged and copied, the kernels, one D2H copy of the used result and the event.
+extern "C" int dsm_tour_enqueue(dsm_ctx *ctx, const uint32_t *matrix, int n, int open, int n_starts, int max_passes, uint64_t seed)
+{
+    if (!ctx) return DSM_E_INVALID;
+    DsmTour *tr = ctx->tour.get();
+    if (!tr || tr->in_flight) return DSM_E_STATE;
+    if (!matrix || n < 1 || n > tr->max_sites || n_starts < 1 || n_starts > tr->max_starts || (open != 0 && open != 1) ||
+        max_passes < 0 || max_passes > DSM_TOUR_MAX_PASSES ||
+        (unsigned long long)n_starts * (unsigned long long)max_passes * (unsigned long long)n * (unsigned long long)n > DSM_TOUR_MAX_WORK)
+        return DSM_E_INVALID;
+    CK(cudaSetDevice(ctx->device));
+    // the previous job's copy out of this staging ended before its wait, which no job in flight implies
+    const size_t bytes = 4 * (size_t)n * n;
+    std::memcpy(tr->matrix_host, matrix, bytes);
+    CK(cudaMemcpyAsync(tr->matrix, tr->matrix_host, bytes, cudaMemcpyHostToDevice, ctx->stream));
+    CK(dsm_launch_tour(tr->matrix, n, open, n_starts, max_passes, seed, tr->tours, tr->res, ctx->stream));
+    CK(cudaMemcpyAsync(tr->res_host, tr->res, dsm_tour_res_bytes(n_starts, n), cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaEventRecord(tr->ev, ctx->stream));
+    tr->in_flight = true;
+    tr->n = n, tr->n_starts = n_starts;
+    return DSM_OK;
+}
+
+extern "C" int dsm_tour_wait(dsm_ctx *ctx, dsm_tour_info_t *info, const dsm_tour_start_t **starts, const int32_t **order)
+{
+    if (!ctx) return DSM_E_INVALID;
+    DsmTour *tr = ctx->tour.get();
+    if (!tr || !tr->in_flight) return DSM_E_STATE;
+    CK(cudaSetDevice(ctx->device));
+    CK(cudaEventSynchronize(tr->ev));
+    tr->in_flight = false;
+    if (info) std::memcpy(info, tr->res_host, sizeof(dsm_tour_info_t));
+    if (starts) *starts = reinterpret_cast<const dsm_tour_start_t *>(tr->res_host + sizeof(dsm_tour_info_t));
+    if (order) *order = reinterpret_cast<const int32_t *>(tr->res_host + sizeof(dsm_tour_info_t) + sizeof(dsm_tour_start_t) * (size_t)tr->n_starts);
+    return DSM_OK;
+}
+
 // ---- checkpoints that do not stop the stream (include/dsm.h, DESIGN.md §8.5) ----
 // The two images at the context's current capacities; whatever was there before is released first (the old and the new
 // need not fit at once).  On failure the checkpoint has no images and its calls return DSM_E_STATE.

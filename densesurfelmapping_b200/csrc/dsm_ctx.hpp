@@ -272,6 +272,20 @@ struct DsmGain
     static size_t res_bytes(int n_views) { return 4 * (size_t)DSM_GAIN_WORDS + sizeof(dsm_view_gain_t) * (size_t)n_views; }
 };
 
+// dsm_tour_* (DESIGN.md §8.14), allocated by dsm_tour_enable: the pinned and device matrix of max_sites^2 entries, the
+// starts' tours, the device result and its pinned copy, and the event after the copy
+struct DsmTour
+{
+    CudaOwner own;
+    int max_sites = 0, max_starts = 0;
+    uint32_t *matrix_host = nullptr, *matrix = nullptr; // [max_sites^2] each
+    int32_t *tours = nullptr;                           // device [max_starts][max_sites]
+    uint8_t *res = nullptr, *res_host = nullptr;        // dsm_tour_res_bytes(max_starts, max_sites) each
+    cudaEvent_t ev = nullptr;
+    int n = 0, n_starts = 0; // of the job in flight or last waited for
+    bool in_flight = false;
+};
+
 #define DSM_MAX_CHUNKS 4
 
 struct dsm_ctx
@@ -347,6 +361,7 @@ struct dsm_ctx
     std::unique_ptr<DsmReach> reach;             // nullptr until dsm_reach_enable
     std::unique_ptr<DsmReachMatrix> reach_matrix; // nullptr until dsm_reach_matrix_enable
     std::unique_ptr<DsmGain> gain;               // nullptr until dsm_gain_enable
+    std::unique_ptr<DsmTour> tour;               // nullptr until dsm_tour_enable
     int run_split = 2;          // sub-batches per dsm_batch_run (dsm_set_concurrency)
     // pinned host staging for the small per-batch tables
     float *h_pose = nullptr; // [2B][32]: pose then inverse; first half: the batch calls, second half: the resident stream

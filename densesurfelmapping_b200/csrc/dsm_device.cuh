@@ -539,3 +539,10 @@ inline long long dsm_gain_bricks(const int32_t size[3])
 cudaError_t dsm_launch_gain(const DsmFieldGrid &g, const uint8_t *state, const int32_t *dist, const dsm_gain_camera_t &cam,
                             const DsmGainView *views, int n_views, long long bricks, const uint8_t *frontier_res,
                             int frontier_max_clusters, int32_t *slot, uint8_t *res, cudaStream_t st);
+
+// dsm_tour_* (DESIGN.md §8.14), dsm_tour.cu.  The whole job on the n x n matrix already on the device: the starts'
+// tours go to tours [n_starts][n], and res receives the packed result of 64 + 16 n_starts + 4 n bytes,
+// dsm_tour_info_t | dsm_tour_start_t starts[n_starts] | int32 order[n].  Returns the first launch error.
+cudaError_t dsm_launch_tour(const uint32_t *matrix, int n, int open, int n_starts, int max_passes, uint64_t seed, int32_t *tours,
+                            uint8_t *res, cudaStream_t st);
+inline size_t dsm_tour_res_bytes(int n_starts, int n) { return 64 + 16 * (size_t)n_starts + 4 * (size_t)n; }

@@ -804,6 +804,63 @@ int dsm_reach_matrix_enable(dsm_ctx *ctx, int max_sites, int max_tiles, int max_
 int dsm_reach_matrix_enqueue(dsm_ctx *ctx, const double *points, int n_points, float radius, int approach);
 int dsm_reach_matrix_wait(dsm_ctx *ctx, dsm_reach_matrix_info_t *info, const dsm_reach_site_t **sites, const uint32_t **matrix);
 
+/* ---- the order of an exploration tour: multi-start local search over a travel-cost matrix (DESIGN.md §8.14) ----
+ * A tour job orders n sites by a deterministic multi-start local search for the asymmetric TSP over a row-major uint32
+ * matrix M[i][j] (the cost from i to j, UINT32_MAX: no path), such as the matrix of dsm_reach_matrix_wait as it stands.
+ * It reads no field and no map: it has no pairing rule with a field request and no DSM_E_CAPACITY after a rejected
+ * frame.  All arithmetic is int64, so the result does not depend on the schedule.
+ *   Included sites: site 0 (the robot) and every j >= 1 with M[0][j] != UINT32_MAX, n_included = m of them; the others
+ *   are left out of the tour.  A matrix job's sites of status != 0 fall out, their row and column being UINT32_MAX.
+ *   Weights: w(i, i) = 0 (the diagonal is ignored), w(i, 0) = 0 when open, else w(i, j) = M[i][j], or P = 2^42 for
+ *   UINT32_MAX.  P exceeds any sum of 1024 finite entries, so a tour with fewer unreachable legs always costs less.
+ *   Tour: positions 0..m-1, t_0 = 0 and t_m = t_0; cost C = sum over k < m of w(t_k, t_{k+1}) (open: the path from the
+ *   robot, the leg back being free; closed: a tour back to site 0); n_infinite counts the legs priced P.
+ *   Construction of start s: positions k = 1..m-1 in turn, among the c = min(3, unvisited) unvisited included sites of
+ *   least (w(t_{k-1}, j), j): start 0 takes the first (nearest neighbour), start s >= 1 candidate
+ *   splitmix64(seed ^ ((uint64)s << 32) ^ k) % c, splitmix64(x) being the splitmix64 generator's output for state x
+ *   (x += 0x9e3779b97f4a7c15, then its finaliser).
+ *   Passes: up to max_passes, each over the whole neighbourhood: 2-opt reverses positions [i, j], 1 <= i < j <= m-1;
+ *   Or-opt moves positions [i, i+L-1], L in {1, 2, 3}, i >= 1, i+L-1 <= m-1, unreversed into the gap after position q,
+ *   q in [0, m-1] outside [i-1, i+L-1].  A pass applies the move of least (delta, type (2-opt 0, Or-opt 1), i, L (2-opt
+ *   0), j or q) when its delta is negative; otherwise the start has converged.  passes counts the applied moves, so a
+ *   start converged exactly when passes < max_passes.
+ *   Result: the best start is the least (C, s).  The header, one record per start and the best tour's order (order[0] =
+ *   0, -1 past n_included): 64 + 16 n_starts + 4 n bytes.
+ *
+ *   dsm_tour_enable   once per context (DSM_E_STATE when called twice).  DSM_E_INVALID for max_sites outside [1, 1024]
+ *                     or max_starts outside [1, 1024].  Allocates the pinned and device matrix (4 max_sites^2 bytes
+ *                     each), the starts' tours (4 max_sites max_starts bytes), the device result and its pinned copy and
+ *                     an event.  DSM_E_NOMEM with nothing kept.
+ *   dsm_tour_enqueue  asynchronous on the context's stream, never waits: the matrix staged into pinned memory on the
+ *                     calling thread, one H2D copy of 4 n^2 bytes, the kernels, one D2H copy of the used result and the
+ *                     event.  DSM_E_STATE before dsm_tour_enable and while a job is in flight.  DSM_E_INVALID for a NULL
+ *                     matrix, n outside [1, max_sites], n_starts outside [1, max_starts], open not 0 or 1, max_passes
+ *                     outside [0, 65536], or n_starts x max_passes x n^2 above 2^32 (this bounds the work of one call).
+ *   dsm_tour_wait     waits for that job only.  *starts (n_starts records) and *order (n entries) are the context's
+ *                     pinned results, valid until the next dsm_tour_enqueue; any out-pointer may be NULL.  DSM_E_STATE
+ *                     with no job enqueued. */
+typedef struct dsm_tour_info_t
+{
+    int32_t n_sites, n_included, open, n_starts, max_passes, best_start;
+    int64_t best_cost;
+    uint64_t seed;
+    int32_t n_infinite;
+    int32_t reserved[5];               /* 0 */
+} dsm_tour_info_t;                     /* 64 B */
+typedef struct dsm_tour_start_t
+{
+    int64_t cost;
+    int32_t passes, converged;
+} dsm_tour_start_t;                    /* 16 B */
+#define DSM_TOUR_MAX_SITES 1024
+#define DSM_TOUR_MAX_STARTS 1024
+#define DSM_TOUR_MAX_PASSES 65536
+#define DSM_TOUR_MAX_WORK (1ull << 32)
+#define DSM_TOUR_P (1ll << 42)
+int dsm_tour_enable(dsm_ctx *ctx, int max_sites, int max_starts);
+int dsm_tour_enqueue(dsm_ctx *ctx, const uint32_t *matrix, int n, int open, int n_starts, int max_passes, uint64_t seed);
+int dsm_tour_wait(dsm_ctx *ctx, dsm_tour_info_t *info, const dsm_tour_start_t **starts, const int32_t **order);
+
 /* ---- view gain: the unknown, frontier and cluster voxels a camera pose would see (DESIGN.md §8.12) ----
  * A gain job reads the state grid of the latest field request, which must be a known one, in stream order behind it,
  * with that request's origin o and voxel edge v (widened to fp64) captured at the job's enqueue, and (with clusters)

@@ -87,7 +87,10 @@
 // enable_known_space, lets reach_matrix() price an exploration tour on the device (DESIGN.md §8.13): the travel costs
 // between every pair of up to max_sites points through the known free space of the latest fused frame's field, one
 // enqueue and one wait.  A planner chains frontiers(), then reach(with_frontiers) from the robot for each cluster's
-// viewpoint, then reach_matrix over the robot's position and those viewpoints, and hands the matrix to its tour solver.
+// viewpoint, then reach_matrix over the robot's position and those viewpoints, and hands the matrix to its tour solver:
+// enable_tour(max_sites, max_starts) lets tour() order the sites on the device (DESIGN.md §8.14), a deterministic
+// multi-start local search over the matrix as it stands, one enqueue and one wait; it reads no field, so it needs
+// neither known space nor a fused frame.
 // What would the robot see from there?  enable_view_gain(max_views), after enable_known_space, lets view_gain() score
 // candidate camera poses against the latest fused frame's known field on the device (DESIGN.md §8.12): per pose, with
 // the node's own intrinsics, the frustum voxels and the free, unknown, occupied, frontier and (after a frontiers() call
@@ -629,6 +632,37 @@ class SurfelMapNode
             matrix.assign(m, m + (size_t)info.n_sites * info.n_sites);
         }
         return ctx_.done(rc, "reach_matrix");
+    }
+
+    // ---- the order of an exploration tour over a travel-cost matrix (DESIGN.md §8.14) ----
+    // once: the most sites and starts of one tour() call
+    int enable_tour(int max_sites, int max_starts)
+    {
+        return ctx_.run("enable_tour", [&] { return dsm_tour_enable(ctx_.ctx, max_sites, max_starts); });
+    }
+    // the best of n_starts local searches over the n x n matrix (row-major, row i from site i, UINT32_MAX: no path; the
+    // matrix of reach_matrix() as it stands), site 0 being the robot (include/dsm.h): starts receives one record per start
+    // and order the best tour's sites, order[0] = 0 and -1 past info.n_included.  open = 1: a path from the robot; 0: a
+    // tour back to it.  Reads no field, so load_state* does not affect it.
+    int tour(const std::vector<uint32_t> &matrix, int n, int open, int n_starts, int max_passes, uint64_t seed, dsm_tour_info_t &info,
+             std::vector<dsm_tour_start_t> &starts, std::vector<int32_t> &order)
+    {
+        starts.clear();
+        order.clear();
+        info = dsm_tour_info_t();
+        if (!ctx_.ready("tour")) return ctx_.err;
+        if (n < 0 || matrix.size() != (size_t)n * n) return ctx_.done(DSM_E_INVALID, "tour");
+        int rc = dsm_tour_enqueue(ctx_.ctx, matrix.data(), n, open, n_starts, max_passes, seed);
+        if (rc != DSM_OK) return ctx_.done(rc, "tour");
+        const dsm_tour_start_t *s = nullptr;
+        const int32_t *o = nullptr;
+        rc = dsm_tour_wait(ctx_.ctx, &info, &s, &o);
+        if (rc == DSM_OK)
+        {
+            starts.assign(s, s + info.n_starts);
+            order.assign(o, o + info.n_sites);
+        }
+        return ctx_.done(rc, "tour");
     }
 
     // ---- view gain against the known field of the latest fused frame (DESIGN.md §8.12) ----
