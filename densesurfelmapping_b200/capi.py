@@ -38,7 +38,7 @@ EXPORTS = [
     "dsm_frontier_enable", "dsm_frontier_enqueue", "dsm_frontier_wait", "dsm_debug_field_load_state",
     "dsm_reach_enable", "dsm_reach_enqueue", "dsm_reach_wait", "dsm_reach_matrix_enable", "dsm_reach_matrix_enqueue",
     "dsm_reach_matrix_wait", "dsm_gain_enable", "dsm_gain_enqueue", "dsm_gain_wait",
-    "dsm_tour_enable", "dsm_tour_enqueue", "dsm_tour_wait",
+    "dsm_tour_enable", "dsm_tour_enqueue", "dsm_tour_wait", "dsm_viewpoint_enable", "dsm_viewpoint_enqueue", "dsm_viewpoint_wait",
     "dsm_inactive_segments", "dsm_inactive_load", "dsm_map_save", "dsm_map_load", "dsm_map_peek",
     "dsm_checkpoint_enable", "dsm_checkpoint_enqueue", "dsm_checkpoint_wait", "dsm_debug_checkpoint_drain_ctas",
     "dsm_checkpoint_enqueue_incremental", "dsm_map_load_journal", "dsm_map_peek_journal", "dsm_journal_materialize",
@@ -91,12 +91,27 @@ GAIN_INFO_DTYPE = np.dtype([("origin", "<i4", 3), ("n_views", "<i4"), ("n_cluste
 TOUR_INFO_DTYPE = np.dtype([("n_sites", "<i4"), ("n_included", "<i4"), ("open", "<i4"), ("n_starts", "<i4"), ("max_passes", "<i4"),
                             ("best_start", "<i4"), ("best_cost", "<i8"), ("seed", "<u8"), ("n_infinite", "<i4"), ("reserved", "<i4", 5)])
 TOUR_START_DTYPE = np.dtype([("cost", "<i8"), ("passes", "<i4"), ("converged", "<i4")])
+# dsm_viewpoint_wait's records (include/dsm.h): a cluster (32 B), a viewpoint slot (32 B) and the header (64 B)
+VIEWPOINT_CLUSTER_DTYPE = np.dtype([("cluster", "<i4"), ("status", "<i4"), ("n_samples", "<i4"), ("n_inside", "<i4"),
+                                    ("n_traversable", "<i4"), ("n_reached", "<i4"), ("n_viewpoints", "<i4"), ("reserved", "<i4")])
+VIEWPOINT_DTYPE = np.dtype([("voxel", "<i4"), ("offset", "<i4"), ("rotation", "<i4"), ("n_seen", "<i4"), ("cost", "<u4"),
+                            ("reserved", "<i4", 3)])
+VIEWPOINT_INFO_DTYPE = np.dtype([("origin", "<i4", 3), ("n_clusters", "<i4"), ("n_offsets", "<i4"), ("n_rotations", "<i4"),
+                                 ("top_k", "<i4"), ("unknown_blocks", "<i4"), ("with_reach", "<i4"), ("n_clusters_table", "<i4"),
+                                 ("reserved", "<i4", 6)])
 
 
 class DsmGainCamera(ctypes.Structure):
     """dsm_gain_camera_t (48 B): pinhole intrinsics, image size, range and the blocking rule of a gain job."""
     _fields_ = [("fx", ctypes.c_double), ("fy", ctypes.c_double), ("cx", ctypes.c_double), ("cy", ctypes.c_double),
                 ("width", ctypes.c_int32), ("height", ctypes.c_int32), ("max_range", ctypes.c_float), ("unknown_blocks", ctypes.c_int32)]
+
+
+class DsmViewpointParams(ctypes.Structure):
+    """dsm_viewpoint_params_t (40 B): the candidate ring, sampling, selection and traversability of a viewpoint job."""
+    _fields_ = [("r_min", ctypes.c_int32), ("r_max", ctypes.c_int32), ("dz_max", ctypes.c_int32), ("stride", ctypes.c_int32),
+                ("max_samples", ctypes.c_int32), ("min_seen", ctypes.c_int32), ("top_k", ctypes.c_int32), ("with_reach", ctypes.c_int32),
+                ("radius", ctypes.c_float), ("reserved", ctypes.c_int32)]
 
 
 CONSTANTS_DRIVE = (0.4, 0.5, 4.0, 0.1)    # fusion_functions.h:13-16
@@ -178,6 +193,9 @@ def load_library():
     L.dsm_tour_enable.argtypes = [vp, ci, ci]
     L.dsm_tour_enqueue.argtypes = [vp, vp, ci, ci, ci, ci, ctypes.c_uint64]
     L.dsm_tour_wait.argtypes = [vp, vp, ctypes.POINTER(vp), ctypes.POINTER(vp)]
+    L.dsm_viewpoint_enable.argtypes = [vp, ci, ci]
+    L.dsm_viewpoint_enqueue.argtypes = [vp, ctypes.POINTER(DsmGainCamera), vp, ci, vp, ci, ctypes.POINTER(DsmViewpointParams)]
+    L.dsm_viewpoint_wait.argtypes = [vp, vp, ctypes.POINTER(vp), ctypes.POINTER(vp)]
     L.dsm_inactive_reserve.argtypes = [vp, ci]
     L.dsm_inactive_retire.argtypes = [vp, ci, ctypes.POINTER(ci)]
     L.dsm_inactive_reactivate.argtypes = [vp, ci, ctypes.POINTER(ci)]
@@ -809,6 +827,44 @@ class Context:
             err.gain = (i, g)
             raise err
         return i, g
+
+    # ---- viewpoints of frontier clusters against the latest known field ----
+    def viewpoint_enable(self, max_clusters, max_candidates):
+        self._ck(self.lib.dsm_viewpoint_enable(self.h, int(max_clusters), int(max_candidates)))
+
+    def viewpoint_enqueue(self, camera, rotations, clusters, params):
+        """camera: (fx, fy, cx, cy, width, height, max_range, unknown_blocks); rotations: (n, 9) row-major camera-to-world
+        3x3 matrices; clusters: frontier-table indices; params: (r_min, r_max, dz_max, stride, max_samples, min_seen,
+        top_k, with_reach, radius)."""
+        cam = DsmGainCamera(*[float(x) for x in camera[:4]], int(camera[4]), int(camera[5]), float(camera[6]), int(camera[7]))
+        R = np.ascontiguousarray(rotations, np.float64).reshape(-1, 9)
+        c = np.ascontiguousarray(clusters, np.int32).reshape(-1)
+        p = DsmViewpointParams(*[int(x) for x in params[:8]], float(params[8]), 0)
+        self._ck(self.lib.dsm_viewpoint_enqueue(self.h, ctypes.byref(cam), R.ctypes.data if len(R) else None, len(R),
+                                                c.ctypes.data if len(c) else None, len(c), ctypes.byref(p)))
+
+    def viewpoint_wait(self):
+        """(info, clusters, viewpoints): numpy copies of the context's pinned results, a VIEWPOINT_INFO_DTYPE record,
+        VIEWPOINT_CLUSTER_DTYPE (n_clusters,) and VIEWPOINT_DTYPE (n_clusters, top_k).  A job on a field taken after a
+        rejected frame raises DsmError(DSM_E_CAPACITY) carrying the same tuple as `.viewpoint`."""
+        pc, pv = ctypes.c_void_p(), ctypes.c_void_p()
+        info = np.zeros(1, VIEWPOINT_INFO_DTYPE)
+        rc = self.lib.dsm_viewpoint_wait(self.h, info.ctypes.data, ctypes.byref(pc), ctypes.byref(pv))
+        if rc not in (DSM_OK, -6):
+            self._ck(rc)
+        i = info[0]
+        n, k = int(i["n_clusters"]), int(i["top_k"])
+
+        def take(ptr, m, dtype):
+            if m == 0:
+                return np.zeros(0, dtype)
+            return np.frombuffer((ctypes.c_uint8 * (m * dtype.itemsize)).from_address(ptr.value), dtype=dtype).copy()
+        out = (i, take(pc, n, VIEWPOINT_CLUSTER_DTYPE), take(pv, n * k, VIEWPOINT_DTYPE).reshape(n, k))
+        if rc != DSM_OK:
+            err = DsmError(rc, self.lib.dsm_last_error(self.h).decode())
+            err.viewpoint = out
+            raise err
+        return out
 
     # ---- the order of an exploration tour over a travel-cost matrix ----
     def tour_enable(self, max_sites, max_starts):

@@ -1960,6 +1960,7 @@ extern "C" int dsm_reach_enqueue(dsm_ctx *ctx, const double start[3], float radi
     CK(cudaEventRecord(re->ev, ctx->stream));
     re->in_flight = true;
     re->host_copy = host_copy != 0;
+    re->request = f->requests;
     return DSM_OK;
 }
 
@@ -2159,6 +2160,15 @@ static void gain_box(const double *P, const dsm_gain_camera_t &c, const DsmField
     }
 }
 
+// gain's camera checks (include/dsm.h): intrinsics, image size, the blocking rule and a range of at most 128 voxels
+static bool gain_camera_ok(const dsm_gain_camera_t &c, double v)
+{
+    const double R = (double)c.max_range;
+    return std::isfinite(c.fx) && c.fx > 0.0 && std::isfinite(c.fy) && c.fy > 0.0 && std::isfinite(c.cx) && std::isfinite(c.cy) &&
+           c.width >= 1 && c.width <= 65536 && c.height >= 1 && c.height <= 65536 && (c.unknown_blocks == 0 || c.unknown_blocks == 1) &&
+           std::isfinite(R) && R > 0.0 && R <= DSM_GAIN_MAX_RANGE_VOXELS * v;
+}
+
 // Enqueue only: the views staged (pose, box, cluster and first brick) and copied, the kernels on the state grid of the
 // latest (known) field request and, with clusters, on the latest frontier job's device result, one D2H copy of the used
 // result and the event.  Later field and frontier requests overwrite those buffers only behind the job.
@@ -2173,11 +2183,7 @@ extern "C" int dsm_gain_enqueue(dsm_ctx *ctx, const dsm_gain_camera_t *camera, c
     if (!camera || n_views < 0 || n_views > ga->max_views || (n_views > 0 && !poses)) return DSM_E_INVALID;
     const dsm_gain_camera_t &c = *camera;
     const double v = (double)f->g.voxel, R = (double)c.max_range;
-    if (!(std::isfinite(c.fx) && c.fx > 0.0 && std::isfinite(c.fy) && c.fy > 0.0 && std::isfinite(c.cx) && std::isfinite(c.cy)))
-        return DSM_E_INVALID;
-    if (c.width < 1 || c.width > 65536 || c.height < 1 || c.height > 65536 || (c.unknown_blocks != 0 && c.unknown_blocks != 1))
-        return DSM_E_INVALID;
-    if (!std::isfinite(R) || !(R > 0.0) || R > DSM_GAIN_MAX_RANGE_VOXELS * v) return DSM_E_INVALID;
+    if (!gain_camera_ok(c, v)) return DSM_E_INVALID;
     const long long m = 2 * (long long)std::ceil(R / v) + 3;
     if ((long long)n_views * m * m * m > DSM_GAIN_MAX_WORK) return DSM_E_INVALID;
     for (size_t i = 0; i < 12 * (size_t)n_views; i++)
@@ -2224,6 +2230,132 @@ extern "C" int dsm_gain_wait(dsm_ctx *ctx, dsm_gain_info_t *info, const dsm_view
     if (h[DSM_GAIN_ERR_TAG] == 0) return DSM_OK;
     snprintf(ctx->err, sizeof(ctx->err), "dsm_gain_wait: frame %d of a dsm_fuse_stream_window call did not fit the pool or the "
              "store; the field the job read holds the frames before it", h[DSM_GAIN_ERR_FRAME]);
+    return DSM_E_CAPACITY;
+}
+
+// ---- viewpoints of frontier clusters (include/dsm.h, DESIGN.md §8.15) ----
+extern "C" int dsm_viewpoint_enable(dsm_ctx *ctx, int max_clusters, int max_candidates)
+{
+    if (!ctx) return DSM_E_INVALID;
+    const DsmField *f = ctx->field.get();
+    if (!f || !ctx->views || ctx->viewpoint) return DSM_E_STATE;
+    if (max_clusters < 1 || max_clusters > DSM_VIEWPOINT_MAX_CLUSTERS || max_candidates < 1 || max_candidates > DSM_VIEWPOINT_MAX_CANDIDATES)
+        return DSM_E_INVALID;
+    CK(cudaSetDevice(ctx->device));
+    auto vp = std::make_unique<DsmViewpoint>();
+    DsmViewpointBufs &b = vp->b;
+    b.max_clusters = max_clusters, b.max_candidates = max_candidates;
+    b.ctas = dsm_viewpoint_ctas();
+    const size_t stage = DsmViewpointBufs::stage_bytes(max_clusters), res = DsmViewpointBufs::res_bytes(max_clusters, DSM_VIEWPOINT_MAX_TOP_K);
+    CudaOwner &o = vp->own;
+    cudaError_t e = b.ctas > 0 ? o.device(&b.stage, stage) : cudaErrorInvalidValue;
+    if (e == cudaSuccess) e = o.host(&vp->stage_host, stage);
+    if (e == cudaSuccess) e = o.device(&b.cl, (size_t)max_clusters);
+    if (e == cudaSuccess) e = o.device(&b.key, (size_t)max_candidates);
+    if (e == cudaSuccess) e = o.device(&b.list, (size_t)max_candidates);
+    if (e == cudaSuccess) e = o.device(&b.count, 1);
+    if (e == cudaSuccess) e = o.device(&b.res, res);
+    if (e == cudaSuccess) e = o.host(&vp->res_host, res);
+    if (e == cudaSuccess) e = o.event(&vp->ev);
+    if (e != cudaSuccess)
+    {
+        cudaGetLastError();
+        return DSM_E_NOMEM; // nothing is kept: a later call may try again
+    }
+    ctx->viewpoint = std::move(vp);
+    return DSM_OK;
+}
+
+// The offsets of include/dsm.h in their order, written as (dx, dy, dz) triples to out (room for
+// DSM_VIEWPOINT_MAX_OFFSETS); returns their number, or -1 past that room.
+static int viewpoint_offsets(const dsm_viewpoint_params_t &p, int32_t *out)
+{
+    int n = 0;
+    const int r = p.r_max / p.stride * p.stride, h = p.dz_max / p.stride * p.stride;
+    for (int dz = -h; dz <= h; dz += p.stride)
+        for (int dy = -r; dy <= r; dy += p.stride)
+            for (int dx = -r; dx <= r; dx += p.stride)
+            {
+                const int q = dx * dx + dy * dy;
+                if (q < p.r_min * p.r_min || q > p.r_max * p.r_max) continue;
+                if (n == DSM_VIEWPOINT_MAX_OFFSETS) return -1;
+                out[3 * n] = dx, out[3 * n + 1] = dy, out[3 * n + 2] = dz;
+                n++;
+            }
+    return n;
+}
+
+// Enqueue only: the rotations, offsets and clusters staged and copied, the kernels on the grids of the latest (known)
+// field request, the latest frontier job's device result and (with_reach) the latest reach job's cost grid, one D2H copy
+// of the used result and the event.  Later field, frontier and reach requests overwrite those buffers only behind the
+// job.
+extern "C" int dsm_viewpoint_enqueue(dsm_ctx *ctx, const dsm_gain_camera_t *camera, const double *rotations, int n_rotations,
+                                     const int32_t *clusters, int n_clusters, const dsm_viewpoint_params_t *params)
+{
+    if (!ctx) return DSM_E_INVALID;
+    DsmViewpoint *vp = ctx->viewpoint.get();
+    const DsmField *f = ctx->field.get();
+    if (!vp || !f || !f->requested || !f->known || vp->in_flight) return DSM_E_STATE;
+    const DsmFrontier *fr = ctx->frontier.get();
+    if (!fr || fr->request != f->requests) return DSM_E_STATE;
+    if (!camera || !params || !rotations || n_rotations < 1 || n_rotations > DSM_VIEWPOINT_MAX_ROTATIONS || n_clusters < 0 ||
+        n_clusters > vp->b.max_clusters || (n_clusters > 0 && !clusters))
+        return DSM_E_INVALID;
+    const dsm_gain_camera_t &c = *camera;
+    const dsm_viewpoint_params_t &p = *params;
+    if (!gain_camera_ok(c, (double)f->g.voxel)) return DSM_E_INVALID;
+    if (p.r_min < 0 || p.r_min > p.r_max || p.r_max > DSM_VIEWPOINT_MAX_RADIUS || p.dz_max < 0 || p.dz_max > DSM_VIEWPOINT_MAX_DZ ||
+        p.stride < 1 || p.stride > DSM_VIEWPOINT_MAX_STRIDE || p.max_samples < 1 || p.max_samples > DSM_VIEWPOINT_MAX_SAMPLES ||
+        p.min_seen < 0 || p.top_k < 1 || p.top_k > DSM_VIEWPOINT_MAX_TOP_K || (p.with_reach != 0 && p.with_reach != 1) ||
+        !std::isfinite(p.radius) || !(p.radius >= 0.f))
+        return DSM_E_INVALID;
+    for (size_t i = 0; i < 9 * (size_t)n_rotations; i++)
+        if (!std::isfinite(rotations[i])) return DSM_E_INVALID;
+    for (int i = 0; i < n_clusters; i++)
+        if (clusters[i] < 0) return DSM_E_INVALID;
+    // the previous job's copy out of this staging ended before its wait, which no job in flight implies
+    int32_t *offsets = reinterpret_cast<int32_t *>(vp->stage_host + DsmViewpointBufs::stage_off());
+    const int n_offsets = viewpoint_offsets(p, offsets);
+    if (n_offsets < 1 || (long long)n_clusters * n_offsets > vp->b.max_candidates ||
+        (long long)n_clusters * n_offsets * p.max_samples > DSM_VIEWPOINT_MAX_WORK)
+        return DSM_E_INVALID;
+    const DsmReach *re = ctx->reach.get();
+    if (p.with_reach && (!re || re->request != f->requests)) return DSM_E_STATE;
+    CK(cudaSetDevice(ctx->device));
+    std::memcpy(vp->stage_host, rotations, 72 * (size_t)n_rotations);
+    if (n_clusters > 0) std::memcpy(vp->stage_host + DsmViewpointBufs::stage_clusters(), clusters, 4 * (size_t)n_clusters);
+    CK(cudaMemcpyAsync(vp->b.stage, vp->stage_host, DsmViewpointBufs::stage_bytes(n_clusters), cudaMemcpyHostToDevice, ctx->stream));
+    CK(dsm_launch_viewpoint(vp->b, f->g, f->occ, f->dist, c, p, n_rotations, n_clusters, n_offsets, fr->b.res, fr->b.max_clusters,
+                            p.with_reach ? re->b.cost[0] : nullptr, ctx->stream));
+    CK(cudaMemcpyAsync(vp->res_host, vp->b.res, DsmViewpointBufs::res_bytes(n_clusters, p.top_k), cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaEventRecord(vp->ev, ctx->stream));
+    vp->in_flight = true;
+    vp->n_clusters = n_clusters, vp->top_k = p.top_k;
+    return DSM_OK;
+}
+
+extern "C" int dsm_viewpoint_wait(dsm_ctx *ctx, dsm_viewpoint_info_t *info, const dsm_viewpoint_cluster_t **clusters,
+                                  const dsm_viewpoint_t **viewpoints)
+{
+    if (!ctx) return DSM_E_INVALID;
+    DsmViewpoint *vp = ctx->viewpoint.get();
+    if (!vp || !vp->in_flight) return DSM_E_STATE;
+    CK(cudaSetDevice(ctx->device));
+    CK(cudaEventSynchronize(vp->ev));
+    vp->in_flight = false;
+    const int32_t *h = reinterpret_cast<const int32_t *>(vp->res_host);
+    const size_t table = 4 * DSM_VP_WORDS;
+    if (info)
+    {
+        std::memcpy(info, h, sizeof(dsm_viewpoint_info_t));
+        for (int32_t &w : info->reserved) w = 0;
+    }
+    if (clusters) *clusters = reinterpret_cast<const dsm_viewpoint_cluster_t *>(vp->res_host + table);
+    if (viewpoints)
+        *viewpoints = reinterpret_cast<const dsm_viewpoint_t *>(vp->res_host + table + sizeof(dsm_viewpoint_cluster_t) * (size_t)vp->n_clusters);
+    if (h[DSM_VP_ERR_TAG] == 0) return DSM_OK;
+    snprintf(ctx->err, sizeof(ctx->err), "dsm_viewpoint_wait: frame %d of a dsm_fuse_stream_window call did not fit the pool or "
+             "the store; the field the job read holds the frames before it", h[DSM_VP_ERR_FRAME]);
     return DSM_E_CAPACITY;
 }
 

@@ -242,6 +242,7 @@ struct DsmReach
     uint32_t *cost_host = nullptr; // pinned [voxels]
     cudaEvent_t ev = nullptr;
     bool in_flight = false, host_copy = false;
+    uint64_t request = 0; // the DsmField::requests of the field the latest job read (0: no job yet)
 };
 
 // dsm_reach_matrix_* (DESIGN.md §8.13), allocated by dsm_reach_matrix_enable for the field's grid: the job's device
@@ -270,6 +271,18 @@ struct DsmGain
     cudaEvent_t ev = nullptr;
     bool in_flight = false;
     static size_t res_bytes(int n_views) { return 4 * (size_t)DSM_GAIN_WORDS + sizeof(dsm_view_gain_t) * (size_t)n_views; }
+};
+
+// dsm_viewpoint_* (DESIGN.md §8.15), allocated by dsm_viewpoint_enable: the job's device buffers (DsmViewpointBufs, the
+// packed result among them), the pinned staging and the result's pinned copy, and the event after the copy
+struct DsmViewpoint
+{
+    CudaOwner own;
+    DsmViewpointBufs b;
+    uint8_t *stage_host = nullptr, *res_host = nullptr;
+    cudaEvent_t ev = nullptr;
+    int n_clusters = 0, top_k = 0; // of the job in flight or last waited for
+    bool in_flight = false;
 };
 
 // dsm_tour_* (DESIGN.md §8.14), allocated by dsm_tour_enable: the pinned and device matrix of max_sites^2 entries, the
@@ -362,6 +375,7 @@ struct dsm_ctx
     std::unique_ptr<DsmReachMatrix> reach_matrix; // nullptr until dsm_reach_matrix_enable
     std::unique_ptr<DsmGain> gain;               // nullptr until dsm_gain_enable
     std::unique_ptr<DsmTour> tour;               // nullptr until dsm_tour_enable
+    std::unique_ptr<DsmViewpoint> viewpoint;     // nullptr until dsm_viewpoint_enable
     int run_split = 2;          // sub-batches per dsm_batch_run (dsm_set_concurrency)
     // pinned host staging for the small per-batch tables
     float *h_pose = nullptr; // [2B][32]: pose then inverse; first half: the batch calls, second half: the resident stream

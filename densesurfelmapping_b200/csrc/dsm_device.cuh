@@ -302,6 +302,11 @@ enum
     DSM_STATE_FREE = 2
 };
 inline size_t dsm_field_header(size_t voxels) { return (voxels + 3) / 4 * 4; }
+// traversable (DESIGN.md §8.11): free, and the stored fp32 distance at least radius
+__device__ __forceinline__ bool dsm_traversable(const uint8_t *state, const int32_t *dist, int i, float radius)
+{
+    return state[i] == DSM_STATE_FREE && __int_as_float(dist[i]) >= radius;
+}
 int dsm_field_setup(); // raises the dynamic shared-memory limit of the envelope passes (lines of up to 1024 voxels)
 // k_field_mark over pool slots [0, res[1]) with update_times >= min_update_times and stored surfels [0, *store_size);
 // pool_upper / store_upper >= the live sizes size the grid.  store == nullptr: no store.  occ must be zeroed.
@@ -533,12 +538,126 @@ inline long long dsm_gain_bricks(const int32_t size[3])
     return (long long)((size[0] + DSM_GAIN_BX - 1) / DSM_GAIN_BX) * ((size[1] + DSM_GAIN_BY - 1) / DSM_GAIN_BY) *
            ((size[2] + DSM_GAIN_BZ - 1) / DSM_GAIN_BZ);
 }
+// Gain's frustum test (include/dsm.h) of d = c - t for the camera-to-world rotation R_km = R[S k + m] (S = 4: a
+// pose's 3x4 rows, S = 3: a bare rotation); every step fp64 with one rounding.  Shared by k_gain_views and
+// k_vp_score.
+template <int S>
+__device__ __forceinline__ bool dsm_gain_frustum(const double *R, double d0, double d1, double d2, double fx, double fy, double cx,
+                                                 double cy, double width, double height, double range2)
+{
+    const double r2 = __dadd_rn(__dadd_rn(__dmul_rn(d0, d0), __dmul_rn(d1, d1)), __dmul_rn(d2, d2));
+    const double qz = __dadd_rn(__dadd_rn(__dmul_rn(R[2], d0), __dmul_rn(R[S + 2], d1)), __dmul_rn(R[2 * S + 2], d2));
+    if (!(r2 <= range2 && qz > 0.0)) return false;
+    const double qx = __dadd_rn(__dadd_rn(__dmul_rn(R[0], d0), __dmul_rn(R[S], d1)), __dmul_rn(R[2 * S], d2));
+    const double qy = __dadd_rn(__dadd_rn(__dmul_rn(R[1], d0), __dmul_rn(R[S + 1], d1)), __dmul_rn(R[2 * S + 1], d2));
+    const double u = __dadd_rn(__dmul_rn(fx, __ddiv_rn(qx, qz)), cx), w = __dadd_rn(__dmul_rn(fy, __ddiv_rn(qy, qz)), cy);
+    return u >= 0.0 && u < width && w >= 0.0 && w < height;
+}
+// Gain's line of sight (include/dsm.h): the walk from a = t to b = c (both fp64 world points within max_range of each
+// other, so every index stays within int) reaches floor(c / v), each voxel before it inside the grid and passing the
+// blocking rule; it leaves at the first voxel that does not.  Shared by k_gain_views and k_vp_score.
+__device__ __forceinline__ bool dsm_gain_walk(const DsmFieldGrid &g, const uint8_t *__restrict__ state, int unknown_blocks, double tx,
+                                              double ty, double tz, double c0, double c1, double c2)
+{
+    const int nx = g.n[0], ny = g.n[1], nz = g.n[2];
+    const double v = (double)g.voxel;
+    const double wa0 = __ddiv_rn(tx, v), wa1 = __ddiv_rn(ty, v), wa2 = __ddiv_rn(tz, v);
+    const double wb0 = __ddiv_rn(c0, v), wb1 = __ddiv_rn(c1, v), wb2 = __ddiv_rn(c2, v);
+    int ix = (int)floor(wa0), iy = (int)floor(wa1), iz = (int)floor(wa2);
+    const int ex = (int)floor(wb0), ey = (int)floor(wb1), ez = (int)floor(wb2);
+    const double e0 = __dsub_rn(wb0, wa0), e1 = __dsub_rn(wb1, wa1), e2 = __dsub_rn(wb2, wa2);
+    const int s0 = e0 > 0.0 ? 1 : (e0 < 0.0 ? -1 : 0), s1 = e1 > 0.0 ? 1 : (e1 < 0.0 ? -1 : 0), s2 = e2 > 0.0 ? 1 : (e2 < 0.0 ? -1 : 0);
+    const double D0 = s0 != 0 ? __drcp_rn(fabs(e0)) : INFINITY, D1 = s1 != 0 ? __drcp_rn(fabs(e1)) : INFINITY,
+                 D2 = s2 != 0 ? __drcp_rn(fabs(e2)) : INFINITY;
+    double mx = s0 != 0 ? __ddiv_rn(__dsub_rn((double)(s0 > 0 ? ix + 1 : ix), wa0), e0) : INFINITY;
+    double my = s1 != 0 ? __ddiv_rn(__dsub_rn((double)(s1 > 0 ? iy + 1 : iy), wa1), e1) : INFINITY;
+    double mz = s2 != 0 ? __ddiv_rn(__dsub_rn((double)(s2 > 0 ? iz + 1 : iz), wa2), e2) : INFINITY;
+    while (true)
+    {
+        if (ix == ex && iy == ey && iz == ez) return true;
+        const int px = ix - g.o[0], py = iy - g.o[1], pz = iz - g.o[2];
+        if (!((unsigned)px < (unsigned)nx && (unsigned)py < (unsigned)ny && (unsigned)pz < (unsigned)nz)) return false;
+        const uint8_t s = __ldg(state + ((size_t)pz * ny + py) * nx + px);
+        if (unknown_blocks ? s != DSM_STATE_FREE : s == DSM_STATE_OCCUPIED) return false;
+        // argmin, the lowest axis on ties
+        if (mx <= my && mx <= mz)
+        {
+            if (mx > 1.0) return false;
+            ix += s0;
+            mx = __dadd_rn(mx, D0);
+        }
+        else if (my <= mz)
+        {
+            if (my > 1.0) return false;
+            iy += s1;
+            my = __dadd_rn(my, D1);
+        }
+        else
+        {
+            if (mz > 1.0) return false;
+            iz += s2;
+            mz = __dadd_rn(mz, D2);
+        }
+    }
+}
 // The whole job on the state grid of the latest known request (header at dsm_field_header(voxels) of dist) for the
 // n_views views already in `views` (bricks in all); frontier_res is the frontier job's device result (nullptr without
 // clusters) and slot a grid of voxels ints.  Writes the whole used result; returns the first launch or memset error.
 cudaError_t dsm_launch_gain(const DsmFieldGrid &g, const uint8_t *state, const int32_t *dist, const dsm_gain_camera_t &cam,
                             const DsmGainView *views, int n_views, long long bricks, const uint8_t *frontier_res,
                             int frontier_max_clusters, int32_t *slot, uint8_t *res, cudaStream_t st);
+
+// dsm_viewpoint_* (DESIGN.md §8.15), dsm_viewpoint.cu.  One staged request (H2D, DsmViewpointBufs::stage_bytes):
+//   double rotations[64][9] | int32 offsets[4096][3] | int32 clusters[n_clusters]
+// and one packed result (D2H, 64 + 32 n (1 + top_k) B):
+//   int32 header[DSM_VP_WORDS] | dsm_viewpoint_cluster_t records[n] | dsm_viewpoint_t slots[n][top_k]
+// The header's first ten words are those of dsm_viewpoint_info_t; its last two carry the field's error words, cleared
+// by dsm_viewpoint_wait.
+enum
+{
+    DSM_VP_ORIGIN = 0, // 3 words
+    DSM_VP_N_CLUSTERS = 3,
+    DSM_VP_N_OFFSETS,
+    DSM_VP_N_ROTATIONS,
+    DSM_VP_TOP_K,
+    DSM_VP_UNKNOWN_BLOCKS,
+    DSM_VP_WITH_REACH,
+    DSM_VP_N_CLUSTERS_TABLE,
+    DSM_VP_ERR_TAG = 14, // the field header's DSM_FIELD_ERR_TAG / _ERR_FRAME, copied by k_vp_clusters
+    DSM_VP_ERR_FRAME,
+    DSM_VP_WORDS = 16 // 64 B
+};
+// what k_vp_clusters leaves per requested cluster for the later kernels
+struct DsmVpCluster
+{
+    int32_t g[3];   // the centre voxel
+    int32_t status; // of the record
+    int32_t base, n, n_s, pad; // the members' list offset and count, the samples
+};
+// The device buffers of one context's viewpoint jobs, sized by dsm_viewpoint_enable
+struct DsmViewpointBufs
+{
+    int max_clusters = 0, max_candidates = 0, ctas = 0; // ctas: the persistent CTAs of k_vp_score
+    uint8_t *stage = nullptr;                 // device twin of the staged request
+    DsmVpCluster *cl = nullptr;               // [max_clusters]
+    unsigned long long *key = nullptr;        // [max_candidates]: the candidate's ranking key, ~0 when it is no viewpoint
+    int32_t *list = nullptr;                  // [max_candidates]: the reached candidates, cluster * n_offsets + offset
+    int32_t *count = nullptr;                 // [1]: their number
+    uint8_t *res = nullptr;                   // the packed result, room for max_clusters at top_k 16
+    static size_t stage_off() { return 8 * 9 * (size_t)DSM_VIEWPOINT_MAX_ROTATIONS; }
+    static size_t stage_clusters() { return stage_off() + 12 * (size_t)DSM_VIEWPOINT_MAX_OFFSETS; }
+    static size_t stage_bytes(int n_clusters) { return stage_clusters() + 4 * (size_t)n_clusters; }
+    static size_t res_bytes(int n, int top_k) { return 4 * (size_t)DSM_VP_WORDS + 32 * (size_t)n * (1 + (size_t)top_k); }
+};
+// the persistent CTAs of k_vp_score on this device
+int dsm_viewpoint_ctas();
+// The whole job on the grids of the latest known request (state, distance and header at dsm_field_header(voxels)), the
+// frontier job's device result and (with_reach) the reach job's settled cost grid, for the request already in b.stage.
+// Writes the whole used result; returns the first launch error.
+cudaError_t dsm_launch_viewpoint(const DsmViewpointBufs &b, const DsmFieldGrid &g, const uint8_t *state, const int32_t *dist,
+                                 const dsm_gain_camera_t &cam, const dsm_viewpoint_params_t &p, int n_rotations, int n_clusters,
+                                 int n_offsets, const uint8_t *frontier_res, int frontier_max_clusters, const uint32_t *reach_cost,
+                                 cudaStream_t st);
 
 // dsm_tour_* (DESIGN.md §8.14), dsm_tour.cu.  The whole job on the n x n matrix already on the device: the starts'
 // tours go to tours [n_starts][n], and res receives the packed result of 64 + 16 n_starts + 4 n bytes,

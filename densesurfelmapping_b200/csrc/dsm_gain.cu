@@ -10,9 +10,10 @@
 //                  binary search over the views' first bricks.  Each thread runs the fp64 frustum test, and only then the
 //                  walk of include/dsm.h from the camera to the voxel's centre, leaving at the first blocking voxel.  The
 //                  counts go through __reduce_add_sync, shared memory and one atomicAdd per counter per CTA.
-// The walk is restated here rather than shared with k_field_carve: carving visits every voxel and stores into the grid,
-// the gain walk reads and stops at the first blocking voxel, so a shared helper would branch on its caller.  The kernels
-// carry no error gate and are launched without PDL, as the other field kernels.
+// The frustum test and the walk are dsm_gain_frustum and dsm_gain_walk (dsm_device.cuh), shared with k_vp_score.  The
+// walk is not shared with k_field_carve: carving visits every voxel and stores into the grid, the gain walk reads and
+// stops at the first blocking voxel, so a shared helper would branch on its caller.  The kernels carry no error gate and
+// are launched without PDL, as the other field kernels.
 #include "dsm_device.cuh"
 #include <algorithm>
 
@@ -121,61 +122,8 @@ __global__ void __launch_bounds__(GAIN_BLOCK) k_gain_views(const DsmFieldGrid g,
         const double c0 = __dmul_rn(__dadd_rn((double)(g.o[0] + x), 0.5), v), c1 = __dmul_rn(__dadd_rn((double)(g.o[1] + y), 0.5), v),
                      c2 = __dmul_rn(__dadd_rn((double)(g.o[2] + z), 0.5), v);
         const double d0 = __dsub_rn(c0, tx), d1 = __dsub_rn(c1, ty), d2 = __dsub_rn(c2, tz);
-        const double r2 = __dadd_rn(__dadd_rn(__dmul_rn(d0, d0), __dmul_rn(d1, d1)), __dmul_rn(d2, d2));
-        const double qz = __dadd_rn(__dadd_rn(__dmul_rn(sv.P[2], d0), __dmul_rn(sv.P[6], d1)), __dmul_rn(sv.P[10], d2));
-        if (r2 <= range2 && qz > 0.0)
-        {
-            const double qx = __dadd_rn(__dadd_rn(__dmul_rn(sv.P[0], d0), __dmul_rn(sv.P[4], d1)), __dmul_rn(sv.P[8], d2));
-            const double qy = __dadd_rn(__dadd_rn(__dmul_rn(sv.P[1], d0), __dmul_rn(sv.P[5], d1)), __dmul_rn(sv.P[9], d2));
-            const double u = __dadd_rn(__dmul_rn(fx, __ddiv_rn(qx, qz)), cx), w = __dadd_rn(__dmul_rn(fy, __ddiv_rn(qy, qz)), cy);
-            frustum = u >= 0.0 && u < width && w >= 0.0 && w < height;
-        }
-        if (frustum)
-        {
-            // the walk from a = t to b = c; |d| <= max_range, so every index below is within the grid's reach of int
-            const double wa0 = __ddiv_rn(tx, v), wa1 = __ddiv_rn(ty, v), wa2 = __ddiv_rn(tz, v);
-            const double wb0 = __ddiv_rn(c0, v), wb1 = __ddiv_rn(c1, v), wb2 = __ddiv_rn(c2, v);
-            int ix = (int)floor(wa0), iy = (int)floor(wa1), iz = (int)floor(wa2);
-            const int ex = (int)floor(wb0), ey = (int)floor(wb1), ez = (int)floor(wb2);
-            const double e0 = __dsub_rn(wb0, wa0), e1 = __dsub_rn(wb1, wa1), e2 = __dsub_rn(wb2, wa2);
-            const int s0 = e0 > 0.0 ? 1 : (e0 < 0.0 ? -1 : 0), s1 = e1 > 0.0 ? 1 : (e1 < 0.0 ? -1 : 0), s2 = e2 > 0.0 ? 1 : (e2 < 0.0 ? -1 : 0);
-            const double D0 = s0 != 0 ? __drcp_rn(fabs(e0)) : INFINITY, D1 = s1 != 0 ? __drcp_rn(fabs(e1)) : INFINITY,
-                         D2 = s2 != 0 ? __drcp_rn(fabs(e2)) : INFINITY;
-            double mx = s0 != 0 ? __ddiv_rn(__dsub_rn((double)(s0 > 0 ? ix + 1 : ix), wa0), e0) : INFINITY;
-            double my = s1 != 0 ? __ddiv_rn(__dsub_rn((double)(s1 > 0 ? iy + 1 : iy), wa1), e1) : INFINITY;
-            double mz = s2 != 0 ? __ddiv_rn(__dsub_rn((double)(s2 > 0 ? iz + 1 : iz), wa2), e2) : INFINITY;
-            while (true)
-            {
-                if (ix == ex && iy == ey && iz == ez)
-                {
-                    seen = true;
-                    break;
-                }
-                const int px = ix - g.o[0], py = iy - g.o[1], pz = iz - g.o[2];
-                if (!((unsigned)px < (unsigned)nx && (unsigned)py < (unsigned)ny && (unsigned)pz < (unsigned)nz)) break;
-                const uint8_t s = __ldg(state + ((size_t)pz * ny + py) * nx + px);
-                if (unknown_blocks ? s != DSM_STATE_FREE : s == DSM_STATE_OCCUPIED) break;
-                // argmin, the lowest axis on ties
-                if (mx <= my && mx <= mz)
-                {
-                    if (mx > 1.0) break;
-                    ix += s0;
-                    mx = __dadd_rn(mx, D0);
-                }
-                else if (my <= mz)
-                {
-                    if (my > 1.0) break;
-                    iy += s1;
-                    my = __dadd_rn(my, D1);
-                }
-                else
-                {
-                    if (mz > 1.0) break;
-                    iz += s2;
-                    mz = __dadd_rn(mz, D2);
-                }
-            }
-        }
+        frustum = dsm_gain_frustum<4>(sv.P, d0, d1, d2, fx, fy, cx, cy, width, height, range2);
+        if (frustum) seen = dsm_gain_walk(g, state, unknown_blocks, tx, ty, tz, c0, c1, c2);
     }
     unsigned st = 0, front = 0, member = 0;
     if (seen)

@@ -62,11 +62,6 @@ __device__ __forceinline__ unsigned long long warp_min64(unsigned long long v)
     return v;
 }
 
-__device__ __forceinline__ bool traversable(const uint8_t *state, const int32_t *dist, int i, float radius)
-{
-    return state[i] == DSM_STATE_FREE && __int_as_float(dist[i]) >= radius;
-}
-
 // the snap of voxel s into its window (include/dsm.h): the least chamfer(u - s) << 32 | u over the window's traversable
 // voxels u, on the whole warp; ~0 when s lies outside the grid or no voxel of the window is traversable
 __device__ __forceinline__ unsigned long long reach_snap(const DsmFieldGrid &g, const uint8_t *state, const int32_t *dist, const int3 s,
@@ -81,7 +76,7 @@ __device__ __forceinline__ unsigned long long reach_snap(const DsmFieldGrid &g, 
             const int x = s.x + dx, y = s.y + dy, z = s.z + dz;
             if (!reach_inside(g, x, y, z)) continue;
             const int i = reach_index(g, x, y, z);
-            if (!traversable(state, dist, i, radius)) continue;
+            if (!dsm_traversable(state, dist, i, radius)) continue;
             const unsigned long long c = ((unsigned long long)reach_chamfer(dx, dy, dz) << 32) | (unsigned)i;
             key = c < key ? c : key;
         }
@@ -160,7 +155,7 @@ __global__ void __launch_bounds__(RC_BLOCK) k_reach_init(const uint8_t *__restri
                                                          uint32_t *__restrict__ c1, int32_t *hdr)
 {
     const int i = blockIdx.x * RC_BLOCK + threadIdx.x;
-    const bool t = i < voxels && traversable(state, dist, i, radius);
+    const bool t = i < voxels && dsm_traversable(state, dist, i, radius);
     if (i < voxels)
     {
         const uint32_t c = i == hdr[DSM_REACH_START_VOXEL] ? 0u : RC_INF;
@@ -505,7 +500,7 @@ __global__ void __launch_bounds__(RC_TILE) k_rm_tiles(const DsmFieldGrid g, cons
     const int tile = blockIdx.x, t = threadIdx.x;
     const int3 tc = rm_tile_xyz(tn, tile);
     const int x = tc.x * RC_T + t % RC_T, y = tc.y * RC_T + t / RC_T % RC_T, z = tc.z * RC_T + t / (RC_T * RC_T);
-    const bool tv = reach_inside(g, x, y, z) && traversable(state, dist, reach_index(g, x, y, z), radius);
+    const bool tv = reach_inside(g, x, y, z) && dsm_traversable(state, dist, reach_index(g, x, y, z), radius);
     const unsigned b = __ballot_sync(0xffffffffu, tv);
     if ((t & 31) == 0) mask[(size_t)tile * RM_WORDS + t / 32] = b;
     const int n = __syncthreads_count(tv);

@@ -1,0 +1,288 @@
+// Viewpoints of frontier clusters (dsm_viewpoint_*, DESIGN.md §8.15): clear candidate positions around each cluster of
+// the latest frontier job, each scored at its best heading by the sampled cluster voxels it would see.
+//
+//   k_vp_clusters    one thread per requested cluster: its status, centre voxel and samples (DsmVpCluster) and its
+//                    record with zero counts; thread 0 writes the header and copies the field's error words.
+//   k_vp_candidates  one thread per (cluster, offset), one cluster per gridDim.y row: the key set to ~0, the inside,
+//                    traversable and reached tests, the counts by __syncthreads_count and one atomicAdd per CTA, and the
+//                    reached candidates appended to a list by warp-aggregated atomics (the list's order does not matter:
+//                    each candidate writes its own key).
+//   k_vp_score       persistent CTAs walking the list, one candidate per CTA at a time and one sample per thread: the
+//                    mask of rotations whose frustum holds the sample (dsm_gain_frustum), then, for a non-empty mask,
+//                    the line of sight (dsm_gain_walk); ballots and popcounts add the seen samples to per-rotation
+//                    counts in shared memory, and thread 0 takes the arg-max and writes the candidate's key.
+//   k_vp_select      one CTA per cluster: top_k rounds of a block minimum over the cluster's keys above the last one.
+// A key packs the ranking (-n_seen, cost, offset index) and the rotation into 63 bits, so the least keys are the
+// viewpoints in order and ~0 is no viewpoint.  The kernels carry no error gate and are launched without PDL, as the
+// other field kernels.
+#include "dsm_device.cuh"
+#include <algorithm>
+
+#define VP_BLOCK 256
+#define VP_NONE 0xffffffffffffffffull
+
+static_assert(sizeof(dsm_viewpoint_params_t) == 40 && sizeof(dsm_viewpoint_cluster_t) == 32 && sizeof(dsm_viewpoint_t) == 32 &&
+                  sizeof(dsm_viewpoint_info_t) == 64, "dsm_viewpoint layouts");
+static_assert(DSM_VP_WORDS * 4 == sizeof(dsm_viewpoint_info_t) && DSM_VP_N_CLUSTERS_TABLE == 9, "the header starts with the info");
+static_assert(DSM_FRONTIER_N_CLUSTERS == 2, "frontier header words");
+static_assert(DSM_VIEWPOINT_MAX_SAMPLES < 8192 && DSM_VIEWPOINT_MAX_OFFSETS <= 4096 && DSM_VIEWPOINT_MAX_ROTATIONS <= 64,
+              "the key's fields: 13 bits of 8191 - n_seen, 32 of cost, 12 of offset, 6 of rotation");
+
+__device__ __forceinline__ unsigned long long vp_key(int n_seen, uint32_t cost, int offset, int rotation)
+{
+    return (unsigned long long)(8191 - n_seen) << 50 | (unsigned long long)cost << 18 | (unsigned long long)offset << 6 |
+           (unsigned long long)rotation;
+}
+
+__global__ void __launch_bounds__(VP_BLOCK) k_vp_clusters(const DsmFieldGrid g, const int32_t *__restrict__ fhdr,
+                                                          const int32_t *__restrict__ frontier_hdr,
+                                                          const dsm_frontier_cluster_t *__restrict__ table, int frontier_max_clusters,
+                                                          const int32_t *__restrict__ clusters, int n_clusters, int n_offsets,
+                                                          int n_rotations, int top_k, int unknown_blocks, int with_reach, int max_samples,
+                                                          int32_t *__restrict__ hdr, dsm_viewpoint_cluster_t *__restrict__ rec,
+                                                          DsmVpCluster *__restrict__ cl, int32_t *__restrict__ count)
+{
+    const int i = blockIdx.x * VP_BLOCK + threadIdx.x;
+    const int n_table = min(frontier_hdr[DSM_FRONTIER_N_CLUSTERS], frontier_max_clusters);
+    if (i == 0)
+    {
+        for (int k = 0; k < 3; k++) hdr[DSM_VP_ORIGIN + k] = g.o[k];
+        hdr[DSM_VP_N_CLUSTERS] = n_clusters;
+        hdr[DSM_VP_N_OFFSETS] = n_offsets;
+        hdr[DSM_VP_N_ROTATIONS] = n_rotations;
+        hdr[DSM_VP_TOP_K] = top_k;
+        hdr[DSM_VP_UNKNOWN_BLOCKS] = unknown_blocks;
+        hdr[DSM_VP_WITH_REACH] = with_reach;
+        hdr[DSM_VP_N_CLUSTERS_TABLE] = n_table;
+        for (int k = DSM_VP_N_CLUSTERS_TABLE + 1; k < DSM_VP_ERR_TAG; k++) hdr[k] = 0;
+        hdr[DSM_VP_ERR_TAG] = fhdr[DSM_FIELD_ERR_TAG];
+        hdr[DSM_VP_ERR_FRAME] = fhdr[DSM_FIELD_ERR_FRAME];
+        *count = 0;
+    }
+    if (i >= n_clusters) return;
+    const int c = clusters[i];
+    const bool past = c >= n_table, unlisted = !past && table[c].offset < 0;
+    DsmVpCluster q;
+    q.status = past ? 3 : unlisted ? 2 : 0;
+    q.base = q.n = q.n_s = q.pad = 0;
+    const double v = (double)g.voxel;
+    for (int k = 0; k < 3; k++) q.g[k] = 0;
+    if (q.status == 0)
+    {
+        const dsm_frontier_cluster_t &T = table[c];
+        for (int k = 0; k < 3; k++) q.g[k] = (int)(floor(__ddiv_rn(T.centroid[k], v)) - (double)g.o[k]);
+        q.base = T.offset;
+        q.n = T.n_voxels;
+        q.n_s = min(T.n_voxels, max_samples);
+    }
+    cl[i] = q;
+    dsm_viewpoint_cluster_t r;
+    r.cluster = c;
+    r.status = q.status;
+    r.n_samples = q.n_s;
+    r.n_inside = r.n_traversable = r.n_reached = r.n_viewpoints = r.reserved = 0;
+    rec[i] = r;
+}
+
+__global__ void __launch_bounds__(VP_BLOCK) k_vp_candidates(const DsmFieldGrid g, const uint8_t *__restrict__ state,
+                                                            const int32_t *__restrict__ dist, const int32_t *__restrict__ offsets,
+                                                            int n_offsets, float radius, const uint32_t *__restrict__ reach_cost,
+                                                            const DsmVpCluster *__restrict__ cl, dsm_viewpoint_cluster_t *__restrict__ rec,
+                                                            unsigned long long *__restrict__ key, int32_t *__restrict__ list,
+                                                            int32_t *__restrict__ count)
+{
+    const int i = blockIdx.y, j = blockIdx.x * VP_BLOCK + threadIdx.x;
+    const DsmVpCluster q = cl[i];
+    const int item = i * n_offsets + j;
+    bool inside = false, trav = false, reached = false;
+    if (j < n_offsets)
+    {
+        key[item] = VP_NONE;
+        if (q.status == 0)
+        {
+            const int x = q.g[0] + offsets[3 * j], y = q.g[1] + offsets[3 * j + 1], z = q.g[2] + offsets[3 * j + 2];
+            inside = (unsigned)x < (unsigned)g.n[0] && (unsigned)y < (unsigned)g.n[1] && (unsigned)z < (unsigned)g.n[2];
+            if (inside)
+            {
+                const int c = (z * g.n[1] + y) * g.n[0] + x;
+                trav = dsm_traversable(state, dist, c, radius);
+                reached = trav && (!reach_cost || reach_cost[c] != 0xffffffffu);
+            }
+        }
+    }
+    const unsigned lane = threadIdx.x & 31, ballot = __ballot_sync(0xffffffffu, reached);
+    int at = 0;
+    if (lane == 0 && ballot) at = atomicAdd(count, __popc(ballot));
+    at = __shfl_sync(0xffffffffu, at, 0);
+    if (reached) list[at + __popc(ballot & ((1u << lane) - 1))] = item;
+    const int n_inside = __syncthreads_count(inside), n_trav = __syncthreads_count(trav), n_reached = __syncthreads_count(reached);
+    if (threadIdx.x == 0 && n_inside)
+    {
+        atomicAdd(&rec[i].n_inside, n_inside);
+        if (n_trav) atomicAdd(&rec[i].n_traversable, n_trav);
+        if (n_reached) atomicAdd(&rec[i].n_reached, n_reached);
+    }
+}
+
+__global__ void __launch_bounds__(VP_BLOCK) k_vp_score(const DsmFieldGrid g, const uint8_t *__restrict__ state,
+                                                       const double *__restrict__ rotations, int n_rotations,
+                                                       const int32_t *__restrict__ offsets, int n_offsets, const DsmVpCluster *__restrict__ cl,
+                                                       const int32_t *__restrict__ members, const int32_t *__restrict__ list,
+                                                       const int32_t *__restrict__ count, const uint32_t *__restrict__ reach_cost,
+                                                       double fx, double fy, double cx, double cy, double width, double height,
+                                                       double range2, int unknown_blocks, int min_seen, unsigned long long *__restrict__ key)
+{
+    __shared__ double s_rot[9 * DSM_VIEWPOINT_MAX_ROTATIONS];
+    __shared__ unsigned s_cnt[DSM_VIEWPOINT_MAX_ROTATIONS];
+    const int tid = threadIdx.x, lane = tid & 31;
+    for (int k = tid; k < 9 * n_rotations; k += VP_BLOCK) s_rot[k] = rotations[k];
+    const int n_items = *count;
+    const int nx = g.n[0], ny = g.n[1];
+    const double v = (double)g.voxel;
+    for (int it = blockIdx.x; it < n_items; it += gridDim.x)
+    {
+        if (tid < DSM_VIEWPOINT_MAX_ROTATIONS) s_cnt[tid] = 0;
+        __syncthreads();
+        const int item = list[it], i = item / n_offsets, j = item % n_offsets;
+        const DsmVpCluster q = cl[i];
+        const int x = q.g[0] + offsets[3 * j], y = q.g[1] + offsets[3 * j + 1], z = q.g[2] + offsets[3 * j + 2];
+        const double tx = __dmul_rn(__dadd_rn((double)(g.o[0] + x), 0.5), v), ty = __dmul_rn(__dadd_rn((double)(g.o[1] + y), 0.5), v),
+                     tz = __dmul_rn(__dadd_rn((double)(g.o[2] + z), 0.5), v);
+        for (int k0 = 0; k0 < q.n_s; k0 += VP_BLOCK)
+        {
+            const int k = k0 + tid;
+            unsigned long long mask = 0;
+            bool seen = false;
+            if (k < q.n_s)
+            {
+                const int m = __ldg(members + q.base + (int)((long long)k * q.n / q.n_s));
+                const int mx = m % nx, my = m / nx % ny, mz = m / (nx * ny);
+                const double c0 = __dmul_rn(__dadd_rn((double)(g.o[0] + mx), 0.5), v), c1 = __dmul_rn(__dadd_rn((double)(g.o[1] + my), 0.5), v),
+                             c2 = __dmul_rn(__dadd_rn((double)(g.o[2] + mz), 0.5), v);
+                const double d0 = __dsub_rn(c0, tx), d1 = __dsub_rn(c1, ty), d2 = __dsub_rn(c2, tz);
+                for (int r = 0; r < n_rotations; r++)
+                    if (dsm_gain_frustum<3>(s_rot + 9 * r, d0, d1, d2, fx, fy, cx, cy, width, height, range2)) mask |= 1ull << r;
+                seen = mask && dsm_gain_walk(g, state, unknown_blocks, tx, ty, tz, c0, c1, c2);
+            }
+            if (__any_sync(0xffffffffu, seen))
+                for (int r = 0; r < n_rotations; r++)
+                {
+                    const unsigned b = __ballot_sync(0xffffffffu, seen && (mask >> r & 1));
+                    if (lane == 0 && b) atomicAdd(&s_cnt[r], __popc(b));
+                }
+        }
+        __syncthreads();
+        if (tid == 0)
+        {
+            int best = 0;
+            for (int r = 1; r < n_rotations; r++)
+                if (s_cnt[r] > s_cnt[best]) best = r;
+            const int n_seen = (int)s_cnt[best];
+            if (n_seen >= max(1, min_seen))
+            {
+                const uint32_t cost = reach_cost ? reach_cost[(z * ny + y) * nx + x] : 0xffffffffu;
+                key[item] = vp_key(n_seen, cost, j, best);
+            }
+        }
+        __syncthreads();
+    }
+}
+
+__global__ void __launch_bounds__(VP_BLOCK) k_vp_select(const DsmFieldGrid g, const int32_t *__restrict__ offsets, int n_offsets, int top_k,
+                                                        const DsmVpCluster *__restrict__ cl, const unsigned long long *__restrict__ key,
+                                                        dsm_viewpoint_cluster_t *__restrict__ rec, dsm_viewpoint_t *__restrict__ out)
+{
+    __shared__ unsigned long long s_min[VP_BLOCK / 32];
+    const int i = blockIdx.x, tid = threadIdx.x;
+    const unsigned long long *k_i = key + (size_t)i * n_offsets;
+    unsigned long long last = 0; // every key is above 0: its top field 8191 - n_seen is at least 4095
+    int n_vp = 0;
+    for (int s = 0; s < top_k; s++)
+    {
+        unsigned long long m = VP_NONE;
+        for (int j = tid; j < n_offsets; j += VP_BLOCK)
+        {
+            const unsigned long long k = k_i[j];
+            if (k > last && k < m) m = k;
+        }
+        for (int o = 16; o > 0; o >>= 1)
+        {
+            const unsigned long long w = __shfl_xor_sync(0xffffffffu, m, o);
+            m = w < m ? w : m;
+        }
+        if ((tid & 31) == 0) s_min[tid >> 5] = m;
+        __syncthreads();
+        m = s_min[0];
+        for (int w = 1; w < VP_BLOCK / 32; w++) m = s_min[w] < m ? s_min[w] : m;
+        __syncthreads();
+        if (tid == 0)
+        {
+            dsm_viewpoint_t r;
+            r.reserved[0] = r.reserved[1] = r.reserved[2] = 0;
+            if (m == VP_NONE)
+            {
+                r.voxel = r.offset = r.rotation = -1;
+                r.n_seen = 0;
+                r.cost = 0xffffffffu;
+            }
+            else
+            {
+                const DsmVpCluster q = cl[i];
+                const int j = (int)(m >> 6 & 4095);
+                const int x = q.g[0] + offsets[3 * j], y = q.g[1] + offsets[3 * j + 1], z = q.g[2] + offsets[3 * j + 2];
+                r.voxel = (z * g.n[1] + y) * g.n[0] + x;
+                r.offset = j;
+                r.rotation = (int)(m & 63);
+                r.n_seen = 8191 - (int)(m >> 50);
+                r.cost = (uint32_t)(m >> 18);
+                n_vp++;
+            }
+            out[(size_t)i * top_k + s] = r;
+        }
+        if (m != VP_NONE) last = m;
+    }
+    if (tid == 0) rec[i].n_viewpoints = n_vp;
+}
+
+int dsm_viewpoint_ctas()
+{
+    int dev = 0, sms = 0, per = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess ||
+        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per, k_vp_score, VP_BLOCK, 0) != cudaSuccess)
+        return 0;
+    return sms * per;
+}
+
+cudaError_t dsm_launch_viewpoint(const DsmViewpointBufs &b, const DsmFieldGrid &g, const uint8_t *state, const int32_t *dist,
+                                 const dsm_gain_camera_t &cam, const dsm_viewpoint_params_t &p, int n_rotations, int n_clusters,
+                                 int n_offsets, const uint8_t *frontier_res, int frontier_max_clusters, const uint32_t *reach_cost,
+                                 cudaStream_t st)
+{
+    const size_t voxels = (size_t)g.n[0] * g.n[1] * g.n[2];
+    int32_t *hdr = reinterpret_cast<int32_t *>(b.res);
+    auto *rec = reinterpret_cast<dsm_viewpoint_cluster_t *>(b.res + 4 * DSM_VP_WORDS);
+    auto *out = reinterpret_cast<dsm_viewpoint_t *>(b.res + 4 * DSM_VP_WORDS + sizeof(dsm_viewpoint_cluster_t) * (size_t)n_clusters);
+    const int32_t *fieldhdr = dist + dsm_field_header(voxels);
+    const int32_t *fhdr = reinterpret_cast<const int32_t *>(frontier_res);
+    const auto *table = reinterpret_cast<const dsm_frontier_cluster_t *>(frontier_res + 4 * DSM_FRONTIER_WORDS);
+    const int32_t *members = reinterpret_cast<const int32_t *>(frontier_res + 4 * DSM_FRONTIER_WORDS +
+                                                               sizeof(dsm_frontier_cluster_t) * (size_t)frontier_max_clusters);
+    const double *rot = reinterpret_cast<const double *>(b.stage);
+    const int32_t *offsets = reinterpret_cast<const int32_t *>(b.stage + DsmViewpointBufs::stage_off());
+    const int32_t *clusters = reinterpret_cast<const int32_t *>(b.stage + DsmViewpointBufs::stage_clusters());
+    const uint32_t *cost = p.with_reach ? reach_cost : nullptr;
+    k_vp_clusters<<<(unsigned)std::max((n_clusters + VP_BLOCK - 1) / VP_BLOCK, 1), VP_BLOCK, 0, st>>>(
+        g, fieldhdr, fhdr, table, frontier_max_clusters, clusters, n_clusters, n_offsets, n_rotations, p.top_k, cam.unknown_blocks,
+        p.with_reach, p.max_samples, hdr, rec, b.cl, b.count);
+    if (n_clusters > 0)
+    {
+        k_vp_candidates<<<dim3((unsigned)((n_offsets + VP_BLOCK - 1) / VP_BLOCK), (unsigned)n_clusters), VP_BLOCK, 0, st>>>(
+            g, state, dist, offsets, n_offsets, p.radius, cost, b.cl, rec, b.key, b.list, b.count);
+        const double R = (double)cam.max_range;
+        k_vp_score<<<(unsigned)b.ctas, VP_BLOCK, 0, st>>>(g, state, rot, n_rotations, offsets, n_offsets, b.cl, members, b.list, b.count, cost,
+                                                          cam.fx, cam.fy, cam.cx, cam.cy, (double)cam.width, (double)cam.height, R * R,
+                                                          cam.unknown_blocks, p.min_seen, b.key);
+        k_vp_select<<<(unsigned)n_clusters, VP_BLOCK, 0, st>>>(g, offsets, n_offsets, p.top_k, b.cl, b.key, rec, out);
+    }
+    return cudaGetLastError();
+}

@@ -933,6 +933,104 @@ int dsm_gain_enable(dsm_ctx *ctx, int max_views);
 int dsm_gain_enqueue(dsm_ctx *ctx, const dsm_gain_camera_t *camera, const double *poses, const int32_t *clusters, int n_views);
 int dsm_gain_wait(dsm_ctx *ctx, dsm_gain_info_t *info, const dsm_view_gain_t **gains);
 
+/* ---- viewpoints of frontier clusters: clear candidate positions scored at their best heading (DESIGN.md §8.15) ----
+ * A viewpoint job reads the state and distance grids of the latest field request, which must be a known one, in stream
+ * order behind it, with that request's origin o and voxel edge v (widened to fp64) captured at the job's enqueue; the
+ * result of the latest frontier job, which must have read that request; and with with_reach the cost grid of the latest
+ * reach job, which must have read it too.  Later field, frontier and reach requests may be enqueued while a job is in
+ * flight and do not change what the job reads.  The map is never read.  Linear index (z * ny + y) * nx + x.
+ *
+ * Definition (integer counts and gain's fp64 steps, one rounding per operation, so the result does not depend on the
+ * schedule).  The camera is dsm_gain_camera_t with gain's meaning; rotation r is rotations[9 r ..], a row-major 3x3
+ * camera-to-world matrix.  clusters[i] names an entry of the frontier table.  Per cluster:
+ *   Status: 3 the cluster is past the table's entries, 2 it is in the table but not in the voxel list (offset -1), 0
+ *   otherwise.  A cluster of status 2 or 3 has no candidates, no samples and no viewpoints.
+ *   Centre voxel: g_k = floor(centroid_k / v) - o_k of the table's fp64 centroid (reach's start snap); it lies within
+ *   the cluster's lo / hi bounds.
+ *   Offsets: every (dx, dy, dz) with all three components multiples of stride, |dz| <= dz_max and r_min^2 <= dx^2 + dy^2
+ *   <= r_max^2, enumerated dz outermost, then dy, then dx, each ascending; the offset index is the position in that
+ *   list, n_offsets its length.
+ *   Candidates: c = g + offset inside the grid and traversable (state free, stored fp32 distance >= radius); with
+ *   with_reach also of finite cost in the reach job, that cost being recorded (UINT32_MAX without with_reach).  The
+ *   camera sits at the centre t_k = ((double)(o_k + c_k) + 0.5) v.
+ *   Samples: with n listed members and n_s = min(n, max_samples), sample k is the member at list position
+ *   floor(k n / n_s) (int64); with n <= max_samples every member.
+ *   Score: seen[r] counts the samples m whose centre passes gain's frustum test for the pose [R_r | t] and whose walk
+ *   from t under unknown_blocks reaches it; n_seen = max_r seen[r], the lowest r on ties.  With every member sampled
+ *   seen[r] equals the n_cluster of a gain job on the pose [R_r | t] naming the cluster.
+ *   Viewpoints: the candidates with n_seen >= max(1, min_seen), ranked by (-n_seen, cost, offset index); the first top_k.
+ *   Records: per cluster the table index, status, n_samples, n_inside (offsets inside the grid), n_traversable, n_reached
+ *   (n_traversable without with_reach) and n_viewpoints; then top_k slots per cluster of voxel (linear index), offset
+ *   index, rotation, n_seen and cost, an empty slot holding voxel = offset = rotation = -1, n_seen 0 and cost
+ *   UINT32_MAX.
+ *   Header: the origin, n_clusters, n_offsets, n_rotations, top_k, unknown_blocks, with_reach and n_clusters_table the
+ *   frontier table's entries.  The result is 64 + 32 n_clusters (1 + top_k) bytes.
+ *
+ *   dsm_viewpoint_enable    once, after dsm_views_enable (DSM_E_STATE otherwise, and when called twice).
+ *                           DSM_E_INVALID for max_clusters outside [1, 4096] or max_candidates outside [1, 2^22].
+ *                           Allocates the pinned and device staging, the per-candidate keys and list, the device result
+ *                           and its pinned copy of 64 + 32 max_clusters (1 + 16) bytes, and an event.  DSM_E_NOMEM with
+ *                           nothing kept.
+ *   dsm_viewpoint_enqueue   asynchronous on the context's stream, never waits: the offsets, rotations and clusters staged
+ *                           and copied with one H2D copy, the kernels, one D2H copy of the used result and the event.
+ *                           DSM_E_STATE before dsm_viewpoint_enable, before any field request, when the latest field
+ *                           request is not a known one, while a job is in flight, when the latest frontier job was not
+ *                           enqueued on the latest field request (or there is none), and with with_reach when the latest
+ *                           reach job was not either.  DSM_E_INVALID for a NULL camera, params or rotations, NULL
+ *                           clusters with n_clusters > 0, gain's camera checks, n_rotations outside [1, 64], a non-finite
+ *                           rotation entry, n_clusters outside [0, max_clusters], a cluster index below 0, r_min, r_max
+ *                           outside 0 <= r_min <= r_max <= 64, dz_max outside [0, 16], stride outside [1, 8],
+ *                           max_samples outside [1, 4096], min_seen < 0, top_k outside [1, 16], with_reach not 0 or 1, a
+ *                           radius that is not finite and >= 0, n_offsets outside [1, 4096], n_clusters n_offsets above
+ *                           max_candidates, or n_clusters n_offsets max_samples above 2^31 walks (this bounds the work
+ *                           of one call).
+ *   dsm_viewpoint_wait      waits for that job only.  *clusters (n_clusters records) and *viewpoints (n_clusters x
+ *                           top_k slots) are the context's pinned results, valid until the next dsm_viewpoint_enqueue;
+ *                           any out-pointer may be NULL.  If the field the job read was taken after a rejected frame,
+ *                           returns DSM_E_CAPACITY with valid results and does NOT clear the error, as dsm_field_wait.
+ *                           DSM_E_STATE with no job enqueued. */
+typedef struct dsm_viewpoint_params_t
+{
+    int32_t r_min, r_max;            /* horizontal ring, voxels */
+    int32_t dz_max, stride;          /* voxels */
+    int32_t max_samples, min_seen, top_k, with_reach;
+    float radius;                    /* metres: the traversable rule of DESIGN.md §8.11 */
+    int32_t reserved;                /* ignored */
+} dsm_viewpoint_params_t;            /* 40 B */
+typedef struct dsm_viewpoint_cluster_t
+{
+    int32_t cluster, status, n_samples;
+    int32_t n_inside, n_traversable, n_reached, n_viewpoints;
+    int32_t reserved;                /* 0 */
+} dsm_viewpoint_cluster_t;           /* 32 B */
+typedef struct dsm_viewpoint_t
+{
+    int32_t voxel, offset, rotation, n_seen;   /* voxel -1: an empty slot */
+    uint32_t cost;                   /* the reach job's cost at the voxel, UINT32_MAX without with_reach */
+    int32_t reserved[3];             /* 0 */
+} dsm_viewpoint_t;                   /* 32 B */
+typedef struct dsm_viewpoint_info_t
+{
+    int32_t origin[3];
+    int32_t n_clusters, n_offsets, n_rotations, top_k, unknown_blocks, with_reach, n_clusters_table;
+    int32_t reserved[6];             /* 0 */
+} dsm_viewpoint_info_t;              /* 64 B */
+#define DSM_VIEWPOINT_MAX_CLUSTERS 4096
+#define DSM_VIEWPOINT_MAX_CANDIDATES (1 << 22)
+#define DSM_VIEWPOINT_MAX_OFFSETS 4096
+#define DSM_VIEWPOINT_MAX_ROTATIONS 64
+#define DSM_VIEWPOINT_MAX_RADIUS 64
+#define DSM_VIEWPOINT_MAX_DZ 16
+#define DSM_VIEWPOINT_MAX_STRIDE 8
+#define DSM_VIEWPOINT_MAX_SAMPLES 4096
+#define DSM_VIEWPOINT_MAX_TOP_K 16
+#define DSM_VIEWPOINT_MAX_WORK (1ll << 31)
+int dsm_viewpoint_enable(dsm_ctx *ctx, int max_clusters, int max_candidates);
+int dsm_viewpoint_enqueue(dsm_ctx *ctx, const dsm_gain_camera_t *camera, const double *rotations, int n_rotations,
+                          const int32_t *clusters, int n_clusters, const dsm_viewpoint_params_t *params);
+int dsm_viewpoint_wait(dsm_ctx *ctx, dsm_viewpoint_info_t *info, const dsm_viewpoint_cluster_t **clusters,
+                       const dsm_viewpoint_t **viewpoints);
+
 /* ---- checkpoints that do not stop the stream (DESIGN.md §8.5) ----
  * The file of dsm_map_save, taken in stream order like a publish snapshot: the resident stream pays one device-to-device
  * copy of the live map, the transfer to the host runs on a low-priority stream beside the next frames, and a thread of

@@ -697,6 +697,48 @@ class SurfelMapNode
         return ctx_.done(rc, "view_gain");
     }
 
+    // ---- viewpoints of frontier clusters against the known field of the latest fused frame (DESIGN.md §8.15) ----
+    // once, after enable_known_space: the most clusters of one viewpoints() call and the most (cluster, offset) pairs
+    int enable_viewpoints(int max_clusters, int max_candidates)
+    {
+        return ctx_.run("enable_viewpoints", [&] { return dsm_viewpoint_enable(ctx_.ctx, max_clusters, max_candidates); });
+    }
+    // clear candidate positions around each named cluster of the frontiers() call on this frame, each scored at the best
+    // of n_rotations rotations (9 doubles each, row-major camera to world) with the node's intrinsics out to max_range
+    // (include/dsm.h); params.with_reach is taken from with_reach, which ranks by the costs of the reach() call on this
+    // frame.  cluster_records receives one record per cluster and viewpoints params.top_k slots per cluster; their voxel
+    // centres ((origin + x) + 0.5) * voxel are the sites for reach_matrix().  DSM_E_STATE without known space, before
+    // any field, after load_state* until the next fused frame, without a frontiers() call since the frame was fused,
+    // and with with_reach without a reach() call since then; DSM_E_CAPACITY with the viewpoints of the last applied
+    // frame's field, as distance_field().
+    int viewpoints(dsm_viewpoint_params_t params, const double *rotations, int n_rotations, float max_range, int unknown_blocks,
+                   const std::vector<int32_t> &clusters, int with_reach, dsm_viewpoint_info_t &info,
+                   std::vector<dsm_viewpoint_cluster_t> &cluster_records, std::vector<dsm_viewpoint_t> &viewpoints)
+    {
+        cluster_records.clear();
+        viewpoints.clear();
+        info = dsm_viewpoint_info_t();
+        if (!ctx_.ready("viewpoints")) return ctx_.err;
+        if (known_.empty() || !field_exists_) return ctx_.done(DSM_E_STATE, "viewpoints");
+        dsm_gain_camera_t cam;
+        cam.fx = cam_[0], cam.fy = cam_[1], cam.cx = cam_[2], cam.cy = cam_[3];
+        cam.width = width_, cam.height = height_;
+        cam.max_range = max_range;
+        cam.unknown_blocks = unknown_blocks;
+        params.with_reach = with_reach;
+        int rc = dsm_viewpoint_enqueue(ctx_.ctx, &cam, rotations, n_rotations, clusters.data(), (int)clusters.size(), &params);
+        if (rc != DSM_OK) return ctx_.done(rc, "viewpoints");
+        const dsm_viewpoint_cluster_t *c = nullptr;
+        const dsm_viewpoint_t *v = nullptr;
+        rc = dsm_viewpoint_wait(ctx_.ctx, &info, &c, &v);
+        if (rc == DSM_OK || rc == DSM_E_CAPACITY)
+        {
+            cluster_records.assign(c, c + info.n_clusters);
+            viewpoints.assign(v, v + (size_t)info.n_clusters * info.top_k);
+        }
+        return ctx_.done(rc, "viewpoints");
+    }
+
     // ---- planner queries against the field of the latest fused frame (DESIGN.md §8.8) ----
     // once, after enable_distance_field: the capacities of one query
     int enable_field_queries(int max_points, int max_trajectories, int max_waypoints)
