@@ -15,6 +15,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libdsm_b200.so")
 
 DSM_OK = 0
+DSM_E_CAPACITY = -6  # a wait that returns it still carries its results (the map of the last applied frame)
 ERRORS = {-1: "DSM_E_INVALID", -2: "DSM_E_SHAPE", -3: "DSM_E_NODEVICE", -4: "DSM_E_CUDA",
           -5: "DSM_E_NOMEM", -6: "DSM_E_CAPACITY", -7: "DSM_E_STATE", -8: "DSM_E_NCCL", -9: "DSM_E_IO"}
 NUM_KERNELS = 10
@@ -269,6 +270,19 @@ def _ptr(a):
     return None if a is None else a.ctypes.data
 
 
+def _take(ptr, n, dtype):
+    """A numpy copy of n records of dtype at the address in ptr (a c_void_p); empty for n == 0 or a null pointer."""
+    dtype = np.dtype(dtype)
+    if n == 0 or not ptr.value:
+        return np.zeros(0, dtype)
+    return np.frombuffer((ctypes.c_uint8 * (n * dtype.itemsize)).from_address(ptr.value), dtype=dtype).copy()
+
+
+def _camera(camera):
+    """The DsmGainCamera of (fx, fy, cx, cy, width, height, max_range, unknown_blocks)."""
+    return DsmGainCamera(*[float(x) for x in camera[:4]], int(camera[4]), int(camera[5]), float(camera[6]), int(camera[7]))
+
+
 def window_lists(per_frame):
     """One list of keyframes per frame -> (keys, offsets[n + 1]) as dsm_fuse_stream_window takes them."""
     lens = [len(x) for x in per_frame]
@@ -309,6 +323,18 @@ class Context:
     def _ck(self, rc):
         if rc != DSM_OK:
             raise DsmError(rc, self.lib.dsm_last_error(self.h).decode() or self.lib.dsm_strerror(rc).decode())
+
+    def _waited(self, rc, name, results):
+        """The results of a wait that returned rc: results() builds them once rc is DSM_OK or DSM_E_CAPACITY (any other
+        code raises first); DSM_E_CAPACITY raises DsmError carrying them as attribute `name`."""
+        if rc not in (DSM_OK, DSM_E_CAPACITY):
+            self._ck(rc)
+        out = results()
+        if rc != DSM_OK:
+            err = DsmError(rc, self.lib.dsm_last_error(self.h).decode())
+            setattr(err, name, out)
+            raise err
+        return out
 
     def close(self):
         if getattr(self, "h", None):
@@ -600,21 +626,7 @@ class Context:
         pa, pi = ctypes.c_void_p(), ctypes.c_void_p()
         na, ni, cf = ctypes.c_int(0), ctypes.c_int(0), ctypes.c_int(0)
         rc = self.lib.dsm_publish_wait(self.h, ctypes.byref(pa), ctypes.byref(na), ctypes.byref(pi), ctypes.byref(ni), ctypes.byref(cf))
-        if rc not in (DSM_OK, -6):  # DSM_E_CAPACITY still carries the clouds
-            self._ck(rc)
-
-        def cloud(ptr, n):
-            if n == 0:
-                return np.zeros(0, dtype=POINT_DTYPE)
-            buf = (ctypes.c_char * (n * POINT_DTYPE.itemsize)).from_address(ptr.value)
-            return np.frombuffer(buf, dtype=POINT_DTYPE).copy()
-
-        clouds = (cloud(pa, na.value), cloud(pi, ni.value), cf.value)
-        if rc != DSM_OK:
-            err = DsmError(rc, self.lib.dsm_last_error(self.h).decode())
-            err.clouds = clouds
-            raise err
-        return clouds
+        return self._waited(rc, "clouds", lambda: (_take(pa, na.value, POINT_DTYPE), _take(pi, ni.value, POINT_DTYPE), cf.value))
 
     def publish_chunks(self):
         """256-point chunks of the inactive cloud the last waited snapshot forwarded to the host."""
@@ -640,20 +652,12 @@ class Context:
         frame raises DsmError(DSM_E_CAPACITY) carrying the same tuple as `.field` (the map of the last applied frame)."""
         ptr, org, nocc = ctypes.c_void_p(), (ctypes.c_int32 * 3)(), ctypes.c_int(0)
         rc = self.lib.dsm_field_wait(self.h, ctypes.byref(ptr), org, ctypes.byref(nocc))
-        if rc not in (DSM_OK, -6):  # DSM_E_CAPACITY still carries the field
-            self._ck(rc)
-        shape = self._field_shape
-        n = shape[0] * shape[1] * shape[2]
-        dist = None
-        if ptr.value:
-            buf = (ctypes.c_float * n).from_address(ptr.value)
-            dist = np.frombuffer(buf, dtype=np.float32).reshape(shape).copy()
-        field = (dist, np.array(org[:], dtype=np.int32), nocc.value)
-        if rc != DSM_OK:
-            err = DsmError(rc, self.lib.dsm_last_error(self.h).decode())
-            err.field = field
-            raise err
-        return field
+
+        def field():
+            shape = self._field_shape
+            dist = _take(ptr, shape[0] * shape[1] * shape[2], np.float32).reshape(shape) if ptr.value else None
+            return dist, np.array(org[:], dtype=np.int32), nocc.value
+        return self._waited(rc, "field", field)
 
     # ---- free versus unknown space ----
     def views_enable(self, max_views, max_range):
@@ -711,21 +715,12 @@ class Context:
         pc, pv = ctypes.c_void_p(), ctypes.c_void_p()
         counts = np.zeros(1, FRONTIER_COUNTS_DTYPE)
         rc = self.lib.dsm_frontier_wait(self.h, ctypes.byref(pc), ctypes.byref(pv), counts.ctypes.data)
-        if rc not in (DSM_OK, -6):
-            self._ck(rc)
         c = counts[0]
-        n_tab = min(int(c["n_clusters"]), self._frontier_caps[0])
 
-        def take(ptr, n, dtype):
-            if n == 0:
-                return np.zeros(0, dtype)
-            return np.frombuffer((ctypes.c_uint8 * (n * dtype.itemsize)).from_address(ptr.value), dtype=dtype).copy()
-        out = (take(pc, n_tab, FRONTIER_CLUSTER_DTYPE), take(pv, int(c["n_listed"]), np.dtype(np.int32)), c)
-        if rc != DSM_OK:
-            err = DsmError(rc, self.lib.dsm_last_error(self.h).decode())
-            err.frontier = out
-            raise err
-        return out
+        def frontier():
+            n_tab = min(int(c["n_clusters"]), self._frontier_caps[0])
+            return _take(pc, n_tab, FRONTIER_CLUSTER_DTYPE), _take(pv, int(c["n_listed"]), np.int32), c
+        return self._waited(rc, "frontier", frontier)
 
     # ---- paths through known free space of the latest known field ----
     def reach_enable(self, max_targets, max_path_voxels, max_rounds):
@@ -746,24 +741,13 @@ class Context:
         pt, pp, pc = ctypes.c_void_p(), ctypes.c_void_p(), ctypes.c_void_p()
         info = np.zeros(1, REACH_INFO_DTYPE)
         rc = self.lib.dsm_reach_wait(self.h, info.ctypes.data, ctypes.byref(pt), ctypes.byref(pp), ctypes.byref(pc))
-        if rc not in (DSM_OK, -6):
-            self._ck(rc)
         i = info[0]
 
-        def take(ptr, n, dtype):
-            if n == 0 or not ptr.value:
-                return np.zeros(0, dtype)
-            return np.frombuffer((ctypes.c_uint8 * (n * dtype.itemsize)).from_address(ptr.value), dtype=dtype).copy()
-        cost = None
-        if pc.value:
-            nz, ny, nx = self._field_shape
-            cost = take(pc, nx * ny * nz, np.dtype(np.uint32)).reshape(nz, ny, nx)
-        out = (i, take(pt, int(i["n_targets"]), REACH_TARGET_DTYPE), take(pp, int(i["n_path_voxels"]), np.dtype(np.int32)), cost)
-        if rc != DSM_OK:
-            err = DsmError(rc, self.lib.dsm_last_error(self.h).decode())
-            err.reach = out
-            raise err
-        return out
+        def reach():
+            shape = self._field_shape
+            cost = _take(pc, shape[0] * shape[1] * shape[2], np.uint32).reshape(shape) if pc.value else None
+            return i, _take(pt, int(i["n_targets"]), REACH_TARGET_DTYPE), _take(pp, int(i["n_path_voxels"]), np.int32), cost
+        return self._waited(rc, "reach", reach)
 
     # ---- travel costs between many sites through the known free space of the latest known field ----
     def reach_matrix_enable(self, max_sites, max_tiles, max_rounds):
@@ -781,18 +765,9 @@ class Context:
         ps, pm = ctypes.c_void_p(), ctypes.c_void_p()
         info = np.zeros(1, REACH_MATRIX_INFO_DTYPE)
         rc = self.lib.dsm_reach_matrix_wait(self.h, info.ctypes.data, ctypes.byref(ps), ctypes.byref(pm))
-        if rc not in (DSM_OK, -6):
-            self._ck(rc)
         i = info[0]
         n = int(i["n_sites"])
-        sites = np.frombuffer((ctypes.c_uint8 * (n * REACH_SITE_DTYPE.itemsize)).from_address(ps.value), dtype=REACH_SITE_DTYPE).copy()
-        m = np.frombuffer((ctypes.c_uint8 * (4 * n * n)).from_address(pm.value), dtype=np.uint32).reshape(n, n).copy()
-        out = (i, sites, m)
-        if rc != DSM_OK:
-            err = DsmError(rc, self.lib.dsm_last_error(self.h).decode())
-            err.reach_matrix = out
-            raise err
-        return out
+        return self._waited(rc, "reach_matrix", lambda: (i, _take(ps, n, REACH_SITE_DTYPE), _take(pm, n * n, np.uint32).reshape(n, n)))
 
     # ---- view gain against the latest known field ----
     def gain_enable(self, max_views):
@@ -801,7 +776,7 @@ class Context:
     def gain_enqueue(self, camera, poses, clusters=None):
         """camera: (fx, fy, cx, cy, width, height, max_range, unknown_blocks); poses: (n, 12) row-major [R | t], camera to
         world; clusters: n frontier-table indices (-1: none), or None when no view names a cluster."""
-        cam = DsmGainCamera(*[float(x) for x in camera[:4]], int(camera[4]), int(camera[5]), float(camera[6]), int(camera[7]))
+        cam = _camera(camera)
         P = np.ascontiguousarray(poses, np.float64).reshape(-1, 12)
         c = None if clusters is None else np.ascontiguousarray(clusters, np.int32).reshape(-1)
         if c is not None and len(c) != len(P):
@@ -816,17 +791,8 @@ class Context:
         pg = ctypes.c_void_p()
         info = np.zeros(1, GAIN_INFO_DTYPE)
         rc = self.lib.dsm_gain_wait(self.h, info.ctypes.data, ctypes.byref(pg))
-        if rc not in (DSM_OK, -6):
-            self._ck(rc)
         i = info[0]
-        n = int(i["n_views"])
-        g = np.zeros(0, VIEW_GAIN_DTYPE) if n == 0 else np.frombuffer(
-            (ctypes.c_uint8 * (n * VIEW_GAIN_DTYPE.itemsize)).from_address(pg.value), dtype=VIEW_GAIN_DTYPE).copy()
-        if rc != DSM_OK:
-            err = DsmError(rc, self.lib.dsm_last_error(self.h).decode())
-            err.gain = (i, g)
-            raise err
-        return i, g
+        return self._waited(rc, "gain", lambda: (i, _take(pg, int(i["n_views"]), VIEW_GAIN_DTYPE)))
 
     # ---- viewpoints of frontier clusters against the latest known field ----
     def viewpoint_enable(self, max_clusters, max_candidates):
@@ -836,7 +802,7 @@ class Context:
         """camera: (fx, fy, cx, cy, width, height, max_range, unknown_blocks); rotations: (n, 9) row-major camera-to-world
         3x3 matrices; clusters: frontier-table indices; params: (r_min, r_max, dz_max, stride, max_samples, min_seen,
         top_k, with_reach, radius)."""
-        cam = DsmGainCamera(*[float(x) for x in camera[:4]], int(camera[4]), int(camera[5]), float(camera[6]), int(camera[7]))
+        cam = _camera(camera)
         R = np.ascontiguousarray(rotations, np.float64).reshape(-1, 9)
         c = np.ascontiguousarray(clusters, np.int32).reshape(-1)
         p = DsmViewpointParams(*[int(x) for x in params[:8]], float(params[8]), 0)
@@ -850,21 +816,10 @@ class Context:
         pc, pv = ctypes.c_void_p(), ctypes.c_void_p()
         info = np.zeros(1, VIEWPOINT_INFO_DTYPE)
         rc = self.lib.dsm_viewpoint_wait(self.h, info.ctypes.data, ctypes.byref(pc), ctypes.byref(pv))
-        if rc not in (DSM_OK, -6):
-            self._ck(rc)
         i = info[0]
         n, k = int(i["n_clusters"]), int(i["top_k"])
-
-        def take(ptr, m, dtype):
-            if m == 0:
-                return np.zeros(0, dtype)
-            return np.frombuffer((ctypes.c_uint8 * (m * dtype.itemsize)).from_address(ptr.value), dtype=dtype).copy()
-        out = (i, take(pc, n, VIEWPOINT_CLUSTER_DTYPE), take(pv, n * k, VIEWPOINT_DTYPE).reshape(n, k))
-        if rc != DSM_OK:
-            err = DsmError(rc, self.lib.dsm_last_error(self.h).decode())
-            err.viewpoint = out
-            raise err
-        return out
+        return self._waited(rc, "viewpoint",
+                            lambda: (i, _take(pc, n, VIEWPOINT_CLUSTER_DTYPE), _take(pv, n * k, VIEWPOINT_DTYPE).reshape(n, k)))
 
     # ---- the order of an exploration tour over a travel-cost matrix ----
     def tour_enable(self, max_sites, max_starts):
@@ -885,10 +840,7 @@ class Context:
         info = np.zeros(1, TOUR_INFO_DTYPE)
         self._ck(self.lib.dsm_tour_wait(self.h, info.ctypes.data, ctypes.byref(ps), ctypes.byref(po)))
         i = info[0]
-        k, n = int(i["n_starts"]), int(i["n_sites"])
-        starts = np.frombuffer((ctypes.c_uint8 * (k * TOUR_START_DTYPE.itemsize)).from_address(ps.value), dtype=TOUR_START_DTYPE).copy()
-        order = np.frombuffer((ctypes.c_uint8 * (4 * n)).from_address(po.value), dtype=np.int32).copy()
-        return i, starts, order
+        return i, _take(ps, int(i["n_starts"]), TOUR_START_DTYPE), _take(po, int(i["n_sites"]), np.int32)
 
     # ---- planner queries against the latest field ----
     def field_query_enable(self, max_points, max_trajectories, max_waypoints):
@@ -912,20 +864,11 @@ class Context:
         DsmError(DSM_E_CAPACITY) carrying the same tuple as `.query`."""
         ps, pc = ctypes.c_void_p(), ctypes.c_void_p()
         rc = self.lib.dsm_field_query_wait(self.h, ctypes.byref(ps), ctypes.byref(pc))
-        if rc not in (DSM_OK, -6):
-            self._ck(rc)
-        n_pts, n_traj = self._query_counts
 
-        def take(ptr, n, dtype):
-            if n == 0:
-                return np.zeros(0, dtype)
-            return np.frombuffer((ctypes.c_uint8 * (n * dtype.itemsize)).from_address(ptr.value), dtype=dtype).copy()
-        out = (take(ps, n_pts, FIELD_SAMPLE_DTYPE), take(pc, n_traj, CLEARANCE_DTYPE))
-        if rc != DSM_OK:
-            err = DsmError(rc, self.lib.dsm_last_error(self.h).decode())
-            err.query = out
-            raise err
-        return out
+        def query():
+            n_pts, n_traj = self._query_counts
+            return _take(ps, n_pts, FIELD_SAMPLE_DTYPE), _take(pc, n_traj, CLEARANCE_DTYPE)
+        return self._waited(rc, "query", query)
 
     # ---- raw cloud of a frame ----
     def frame_raw_cloud(self, frame, pose7, cap=None):

@@ -295,6 +295,7 @@ static cudaEvent_t prof_event(dsm_ctx *ctx)
     }
     cudaEvent_t e = nullptr;
     ctx->own.event(&e, cudaEventDefault); // recycled through ev_free, released with the context
+    ctx->own.take();                       // a failure leaves e null; the next call tries again
     return e;
 }
 struct ProfScope
@@ -1066,9 +1067,9 @@ static DsmDev inactive_view(dsm_ctx *ctx)
 // (what an earlier, failed attempt allocated is kept and used)
 static cudaError_t store_publish_alloc(InactStore &s)
 {
-    cudaError_t e = s.shadow ? cudaSuccess : s.own.device(&s.shadow, (size_t)s.cap);
-    if (e == cudaSuccess && !s.mirror) e = s.own.mapped(&s.mirror, &s.mirror_dev, (size_t)s.cap);
-    return e;
+    if (!s.shadow) s.own.device(&s.shadow, (size_t)s.cap);
+    if (!s.mirror) s.own.mapped(&s.mirror, &s.mirror_dev, (size_t)s.cap);
+    return s.own.take();
 }
 // k_cloud_mirror's state for a shadow that holds nothing: the next snapshot forwards the whole cloud.  Ordered on the
 // context's stream, like the kernels that read it, and waited for (the source is on the stack).
@@ -1345,6 +1346,74 @@ int dsm_map_info(const dsm_ctx *ctx, DsmMapInfo *info)
     return DSM_OK;
 }
 
+// ---- the lifecycle every snapshot, field and planner job shares ----
+// The end of an enable: the new state is kept when every call of its owner succeeded and `ok`, else nothing is kept and
+// a later call may try again
+template <typename T>
+static int keep(std::unique_ptr<T> &slot, std::unique_ptr<T> &fresh, bool ok = true)
+{
+    if (fresh->own.take() != cudaSuccess || !ok)
+    {
+        cudaGetLastError();
+        return DSM_E_NOMEM; // nothing is kept: a later call may try again
+    }
+    slot = std::move(fresh);
+    return DSM_OK;
+}
+
+// The latest field request if it is a known one (what every job on the known field reads), else nullptr
+static const DsmField *known_field(const dsm_ctx *ctx)
+{
+    const DsmField *f = ctx->field.get();
+    return f && f->requested && f->known ? f : nullptr;
+}
+
+// The pairing rule: the latest job of a kind (frontier, reach) read the latest field request
+static bool read_latest(const DsmJob *j, const DsmField *f) { return j && j->request == f->requests; }
+
+// The tail of an enqueue: one D2H copy of the used result bytes, the job's event, and the job in flight with the field
+// request it read (0 for none)
+static int submit(dsm_ctx *ctx, DsmJob &j, const void *res, size_t bytes, uint64_t request)
+{
+    CK(cudaMemcpyAsync(j.res_host, res, bytes, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaEventRecord(j.ev, ctx->stream));
+    j.in_flight = true;
+    j.request = request;
+    return DSM_OK;
+}
+
+// The head of a wait (a job's or the field's): DSM_E_STATE without a request in flight, else its event waited for and
+// the request retired
+template <typename T>
+static int wait_head(dsm_ctx *ctx, T *j)
+{
+    if (!j || !j->in_flight) return DSM_E_STATE;
+    CK(cudaSetDevice(ctx->device));
+    CK(cudaEventSynchronize(j->ev));
+    j->in_flight = false;
+    return DSM_OK;
+}
+
+// The result of a wait whose header h holds the sticky error word of dsm_fuse_stream_window at h[tag] and the frame it
+// rejected after it: DSM_OK without an error, else DSM_E_CAPACITY with the message that `call`'s `what` holds the frames
+// before that one
+static int capacity(dsm_ctx *ctx, const int32_t *h, int tag, const char *call, const char *what)
+{
+    if (h[tag] == 0) return DSM_OK;
+    snprintf(ctx->err, sizeof(ctx->err), "%s: frame %d of a dsm_fuse_stream_window call did not fit the pool or the store; %s holds "
+             "the frames before it", call, h[tag + 1], what);
+    return DSM_E_CAPACITY;
+}
+
+// An info struct copied out of a result header, its reserved words zeroed
+template <typename Info>
+static void copy_info(Info *info, const int32_t *h)
+{
+    if (!info) return;
+    std::memcpy(info, h, sizeof(Info));
+    for (int32_t &w : info->reserved) w = 0;
+}
+
 // ---- publishing from inside the stream (include/dsm.h) ----
 extern "C" int dsm_publish_enable(dsm_ctx *ctx)
 {
@@ -1352,11 +1421,11 @@ extern "C" int dsm_publish_enable(dsm_ctx *ctx)
     if (!ctx->res_active || ctx->pub_on) return DSM_E_STATE;
     CK(cudaSetDevice(ctx->device));
     // a call that failed half-way keeps what it allocated; the next one allocates only what is missing
-    cudaError_t e = cudaSuccess;
-    if (!ctx->pub_active) e = ctx->own.mapped(&ctx->pub_active, &ctx->pub_active_dev, (size_t)std::max(ctx->p.max_local_surfels, 1));
-    if (e == cudaSuccess && !ctx->pub_hdr) e = ctx->own.mapped(&ctx->pub_hdr, &ctx->pub_hdr_dev, DSM_PUB_WORDS);
-    if (e == cudaSuccess && !ctx->pub_state) e = ctx->own.device(&ctx->pub_state, 4);
-    if (e == cudaSuccess && !ctx->pub_ev) e = ctx->own.event(&ctx->pub_ev);
+    if (!ctx->pub_active) ctx->own.mapped(&ctx->pub_active, &ctx->pub_active_dev, (size_t)std::max(ctx->p.max_local_surfels, 1));
+    if (!ctx->pub_hdr) ctx->own.mapped(&ctx->pub_hdr, &ctx->pub_hdr_dev, DSM_PUB_WORDS);
+    if (!ctx->pub_state) ctx->own.device(&ctx->pub_state, 4);
+    if (!ctx->pub_ev) ctx->own.event(&ctx->pub_ev);
+    cudaError_t e = ctx->own.take();
     if (e == cudaSuccess) e = publish_state_reset(ctx);
     if (e == cudaSuccess && ctx->inact) e = store_publish_alloc(*ctx->inact);
     if (e != cudaSuccess)
@@ -1406,10 +1475,7 @@ extern "C" int dsm_publish_wait(dsm_ctx *ctx, const dsm_point_t **active, int *n
     if (inactive) *inactive = ctx->inact ? ctx->inact->mirror : nullptr;
     if (n_inactive) *n_inactive = h[DSM_PUB_N_INACTIVE];
     if (inactive_changed_from) *inactive_changed_from = h[DSM_PUB_CHANGED_FROM];
-    if (h[DSM_PUB_ERR_TAG] == 0) return DSM_OK;
-    snprintf(ctx->err, sizeof(ctx->err), "dsm_publish_wait: frame %d of a dsm_fuse_stream_window call did not fit the pool or the "
-             "store; the snapshot holds the frames before it", h[DSM_PUB_ERR_FRAME]);
-    return DSM_E_CAPACITY;
+    return capacity(ctx, h, DSM_PUB_ERR_TAG, "dsm_publish_wait", "the snapshot");
 }
 
 extern "C" int dsm_debug_publish_chunks(dsm_ctx *ctx, int *count)
@@ -1435,18 +1501,11 @@ extern "C" int dsm_field_enable(dsm_ctx *ctx, const dsm_field_params *params)
     f->g.n[0] = p.nx, f->g.n[1] = p.ny, f->g.n[2] = p.nz;
     f->voxels = (size_t)p.nx * p.ny * p.nz;
     f->bytes = (dsm_field_header(f->voxels) + DSM_FIELD_WORDS) * sizeof(int32_t);
-    cudaError_t e = f->own.device(&f->occ, f->voxels);
-    if (e == cudaSuccess) e = f->own.device(&f->dist, f->bytes / sizeof(int32_t));
-    if (e == cudaSuccess) e = f->own.host(&f->host, f->bytes / sizeof(int32_t));
-    if (e == cudaSuccess) e = f->own.event(&f->ev);
-    if (e == cudaSuccess && dsm_field_setup() != 0) e = cudaErrorInvalidValue;
-    if (e != cudaSuccess)
-    {
-        cudaGetLastError();
-        return DSM_E_NOMEM; // nothing is kept: a later call may try again
-    }
-    ctx->field = std::move(f);
-    return DSM_OK;
+    f->own.device(&f->occ, f->voxels);
+    f->own.device(&f->dist, f->bytes / sizeof(int32_t));
+    f->own.host(&f->host, f->bytes / sizeof(int32_t));
+    f->own.event(&f->ev);
+    return keep(ctx->field, f, dsm_field_setup() == 0);
 }
 
 // The views of a known request (dsm_field_enqueue_known), checked by the caller
@@ -1535,19 +1594,14 @@ extern "C" int dsm_field_wait(dsm_ctx *ctx, const float **dist, int32_t origin[3
 {
     if (!ctx) return DSM_E_INVALID;
     DsmField *f = ctx->field.get();
-    if (!f || !f->in_flight) return DSM_E_STATE;
-    CK(cudaSetDevice(ctx->device));
-    CK(cudaEventSynchronize(f->ev));
-    f->in_flight = false;
+    const int rc = wait_head(ctx, f);
+    if (rc != DSM_OK) return rc;
     f->known_waited = f->known;
     const int32_t *h = f->host + dsm_field_header(f->voxels);
     if (dist) *dist = f->resident ? nullptr : reinterpret_cast<const float *>(f->host);
     if (origin) origin[0] = f->g.o[0], origin[1] = f->g.o[1], origin[2] = f->g.o[2];
     if (n_occupied) *n_occupied = h[DSM_FIELD_N_OCCUPIED];
-    if (h[DSM_FIELD_ERR_TAG] == 0) return DSM_OK;
-    snprintf(ctx->err, sizeof(ctx->err), "dsm_field_wait: frame %d of a dsm_fuse_stream_window call did not fit the pool or the "
-             "store; the field holds the frames before it", h[DSM_FIELD_ERR_FRAME]);
-    return DSM_E_CAPACITY;
+    return capacity(ctx, h, DSM_FIELD_ERR_TAG, "dsm_field_wait", "the field");
 }
 
 // ---- planner queries against the latest field (include/dsm.h, DESIGN.md §8.8) ----
@@ -1562,18 +1616,12 @@ extern "C" int dsm_field_query_enable(dsm_ctx *ctx, int max_points, int max_traj
     q->max_points = max_points, q->max_traj = max_trajectories, q->max_wp = max_waypoints;
     const size_t req = DsmFieldQuery::req_bytes(max_points, max_waypoints, max_trajectories);
     const size_t res = DsmFieldQuery::res_bytes(max_points, max_trajectories);
-    cudaError_t e = q->own.host(&q->req_host, req);
-    if (e == cudaSuccess) e = q->own.device(&q->req_dev, req);
-    if (e == cudaSuccess) e = q->own.device(&q->res_dev, res);
-    if (e == cudaSuccess) e = q->own.host(&q->res_host, res);
-    if (e == cudaSuccess) e = q->own.event(&q->ev);
-    if (e != cudaSuccess)
-    {
-        cudaGetLastError();
-        return DSM_E_NOMEM; // nothing is kept: a later call may try again
-    }
-    ctx->field_query = std::move(q);
-    return DSM_OK;
+    q->own.host(&q->req_host, req);
+    q->own.device(&q->req_dev, req);
+    q->own.device(&q->res_dev, res);
+    q->own.host(&q->res_host, res);
+    q->own.event(&q->ev);
+    return keep(ctx->field_query, q);
 }
 
 // Stages the request on the calling thread (checking it and counting the samples on the way), then enqueues one H2D
@@ -1645,28 +1693,19 @@ extern "C" int dsm_field_query_enqueue(dsm_ctx *ctx, const double *points, int n
     dsm_launch_field_query(reinterpret_cast<const float *>(f->dist), f_hdr, f->g, d_pts, n_points, d_wp,
                            d_ofs, d_first, n_trajectories, radius, r_hdr, r_samples, r_clear, ctx->stream);
     CK(cudaGetLastError());
-    CK(cudaMemcpyAsync(q->res_host, q->res_dev, DsmFieldQuery::res_bytes(n_points, n_trajectories), cudaMemcpyDeviceToHost, ctx->stream));
-    CK(cudaEventRecord(q->ev, ctx->stream));
     q->n_points = n_points, q->n_traj = n_trajectories;
-    q->in_flight = true;
-    return DSM_OK;
+    return submit(ctx, *q, q->res_dev, DsmFieldQuery::res_bytes(n_points, n_trajectories), f->requests);
 }
 
 extern "C" int dsm_field_query_wait(dsm_ctx *ctx, const dsm_field_sample_t **samples, const dsm_clearance_t **clearance)
 {
     if (!ctx) return DSM_E_INVALID;
     DsmFieldQuery *q = ctx->field_query.get();
-    if (!q || !q->in_flight) return DSM_E_STATE;
-    CK(cudaSetDevice(ctx->device));
-    CK(cudaEventSynchronize(q->ev));
-    q->in_flight = false;
-    const int32_t *h = reinterpret_cast<const int32_t *>(q->res_host);
+    const int rc = wait_head(ctx, q);
+    if (rc != DSM_OK) return rc;
     if (samples) *samples = reinterpret_cast<const dsm_field_sample_t *>(q->res_host + 16);
     if (clearance) *clearance = reinterpret_cast<const dsm_clearance_t *>(q->res_host + DsmFieldQuery::res_clearance(q->n_points));
-    if (h[DSM_QUERY_ERR_TAG] == 0) return DSM_OK;
-    snprintf(ctx->err, sizeof(ctx->err), "dsm_field_query_wait: frame %d of a dsm_fuse_stream_window call did not fit the pool or the "
-             "store; the field the query read holds the frames before it", h[DSM_QUERY_ERR_FRAME]);
-    return DSM_E_CAPACITY;
+    return capacity(ctx, q->words(), DSM_QUERY_ERR_TAG, "dsm_field_query_wait", "the field the query read");
 }
 
 // ---- free versus unknown space: captured views and the known-space field (include/dsm.h, DESIGN.md §8.9) ----
@@ -1683,17 +1722,11 @@ extern "C" int dsm_views_enable(dsm_ctx *ctx, int max_views, float max_range)
     auto v = std::make_unique<DsmViews>();
     v->max_views = max_views, v->max_range = max_range;
     v->filled.assign((size_t)max_views, 0);
-    cudaError_t e = v->own.device(&v->rays, (size_t)max_views * ctx->d.S);
-    if (e == cudaSuccess) e = v->own.host(&v->state, f->voxels);
-    if (e == cudaSuccess) e = v->own.host(&v->stage_host, DsmViews::stage_bytes(max_views));
-    if (e == cudaSuccess) e = v->own.device(&v->stage_dev, DsmViews::stage_bytes(max_views));
-    if (e != cudaSuccess)
-    {
-        cudaGetLastError();
-        return DSM_E_NOMEM; // nothing is kept: a later call may try again
-    }
-    ctx->views = std::move(v);
-    return DSM_OK;
+    v->own.device(&v->rays, (size_t)max_views * ctx->d.S);
+    v->own.host(&v->state, f->voxels);
+    v->own.host(&v->stage_host, DsmViews::stage_bytes(max_views));
+    v->own.device(&v->stage_dev, DsmViews::stage_bytes(max_views));
+    return keep(ctx->views, v);
 }
 
 // Enqueue only.  The frame's slot is safe to read on the main stream: the call that filled it left its schedule ordered
@@ -1800,32 +1833,21 @@ extern "C" int dsm_frontier_enable(dsm_ctx *ctx, int max_clusters, int max_voxel
     const size_t sel = (size_t)dsm_frontier_sel_blocks(b.voxels);
     const size_t res = DsmFrontierBufs::res_bytes(max_clusters, max_voxels);
     CudaOwner &o = fr->own;
-    cudaError_t e = o.device(&b.label, f->voxels);
-    for (int32_t **p : {&b.roots, &b.count, &b.cmap, &b.cid})
-        if (e == cudaSuccess) e = o.device(p, (size_t)b.max_comp);
-    for (int32_t **p : {&b.slot_comp, &b.sizes, &b.offs})
-        if (e == cudaSuccess) e = o.device(p, cl);
-    if (e == cudaSuccess) e = o.device(&b.acc, cl);
-    if (e == cudaSuccess) e = o.device(&b.idx, vx);
-    if (e == cudaSuccess) e = o.device(&b.keys, vx);
-    if (e == cudaSuccess) e = o.device(&b.keys_alt, vx);
-    if (e == cudaSuccess) e = o.device(&b.blk, sel);
-    if (e == cudaSuccess) e = o.device(&b.blk_ofs, sel);
-    if (e == cudaSuccess) e = o.device(&b.res, res);
-    if (e == cudaSuccess) e = o.host(&fr->res_host, res);
-    if (e == cudaSuccess) e = o.event(&fr->ev);
-    if (e == cudaSuccess)
-    {
-        b.temp_bytes = dsm_frontier_temp_bytes(b);
-        e = b.temp_bytes ? o.device(reinterpret_cast<uint8_t **>(&b.temp), b.temp_bytes) : cudaErrorInvalidValue;
-    }
-    if (e != cudaSuccess)
-    {
-        cudaGetLastError();
-        return DSM_E_NOMEM; // nothing is kept: a later call may try again
-    }
-    ctx->frontier = std::move(fr);
-    return DSM_OK;
+    o.device(&b.label, f->voxels);
+    for (int32_t **p : {&b.roots, &b.count, &b.cmap, &b.cid}) o.device(p, (size_t)b.max_comp);
+    for (int32_t **p : {&b.slot_comp, &b.sizes, &b.offs}) o.device(p, cl);
+    o.device(&b.acc, cl);
+    o.device(&b.idx, vx);
+    o.device(&b.keys, vx);
+    o.device(&b.keys_alt, vx);
+    o.device(&b.blk, sel);
+    o.device(&b.blk_ofs, sel);
+    o.device(&b.res, res);
+    o.host(&fr->res_host, res);
+    o.event(&fr->ev);
+    b.temp_bytes = dsm_frontier_temp_bytes(b);
+    if (b.temp_bytes) o.device(reinterpret_cast<uint8_t **>(&b.temp), b.temp_bytes);
+    return keep(ctx->frontier, fr, b.temp_bytes != 0);
 }
 
 // Enqueue only: the job on the state grid of the latest (known) field request with that request's origin, one D2H copy
@@ -1834,38 +1856,29 @@ extern "C" int dsm_frontier_enqueue(dsm_ctx *ctx, int min_voxels)
 {
     if (!ctx) return DSM_E_INVALID;
     DsmFrontier *fr = ctx->frontier.get();
-    const DsmField *f = ctx->field.get();
-    if (!fr || !f || !f->requested || !f->known || fr->in_flight) return DSM_E_STATE;
+    const DsmField *f = known_field(ctx);
+    if (!fr || !f || fr->in_flight) return DSM_E_STATE;
     if (min_voxels < 1) return DSM_E_INVALID;
     CK(cudaSetDevice(ctx->device));
     const DsmFrontierBufs &b = fr->b;
     CK(cudaMemsetAsync(b.res, 0, 4 * DSM_FRONTIER_WORDS, ctx->stream));
     CK(dsm_launch_frontier(b, f->g, f->occ, f->dist + dsm_field_header(f->voxels), min_voxels, ctx->stream));
-    CK(cudaMemcpyAsync(fr->res_host, b.res, DsmFrontierBufs::res_bytes(b.max_clusters, b.max_voxels), cudaMemcpyDeviceToHost, ctx->stream));
-    CK(cudaEventRecord(fr->ev, ctx->stream));
-    fr->in_flight = true;
-    fr->request = f->requests;
-    return DSM_OK;
+    return submit(ctx, *fr, b.res, DsmFrontierBufs::res_bytes(b.max_clusters, b.max_voxels), f->requests);
 }
 
 extern "C" int dsm_frontier_wait(dsm_ctx *ctx, const dsm_frontier_cluster_t **clusters, const int32_t **voxels, dsm_frontier_counts_t *counts)
 {
     if (!ctx) return DSM_E_INVALID;
     DsmFrontier *fr = ctx->frontier.get();
-    if (!fr || !fr->in_flight) return DSM_E_STATE;
-    CK(cudaSetDevice(ctx->device));
-    CK(cudaEventSynchronize(fr->ev));
-    fr->in_flight = false;
-    const int32_t *h = reinterpret_cast<const int32_t *>(fr->res_host);
+    const int rc = wait_head(ctx, fr);
+    if (rc != DSM_OK) return rc;
+    const int32_t *h = fr->words();
     const size_t table = 4 * DSM_FRONTIER_WORDS;
     if (clusters) *clusters = reinterpret_cast<const dsm_frontier_cluster_t *>(fr->res_host + table);
     if (voxels)
         *voxels = reinterpret_cast<const int32_t *>(fr->res_host + table + sizeof(dsm_frontier_cluster_t) * (size_t)fr->b.max_clusters);
     if (counts) std::memcpy(counts, h, sizeof(dsm_frontier_counts_t));
-    if (h[DSM_FRONTIER_ERR_TAG] == 0) return DSM_OK;
-    snprintf(ctx->err, sizeof(ctx->err), "dsm_frontier_wait: frame %d of a dsm_fuse_stream_window call did not fit the pool or the "
-             "store; the field the job read holds the frames before it", h[DSM_FRONTIER_ERR_FRAME]);
-    return DSM_E_CAPACITY;
+    return capacity(ctx, h, DSM_FRONTIER_ERR_TAG, "dsm_frontier_wait", "the field the job read");
 }
 
 // ---- paths through known free space (include/dsm.h, DESIGN.md §8.11) ----
@@ -1888,34 +1901,23 @@ extern "C" int dsm_reach_enable(dsm_ctx *ctx, int max_targets, int max_path_voxe
     const size_t tg = (size_t)std::max(max_targets, 1);
     const size_t res = DsmReachBufs::res_bytes(max_targets, max_path_voxels);
     CudaOwner &o = re->own;
-    cudaError_t e = b.ctas > 0 ? o.device(&b.trav, f->voxels) : cudaErrorInvalidValue;
-    for (uint32_t **p : {&b.cost[0], &b.cost[1]})
-        if (e == cudaSuccess) e = o.device(p, f->voxels);
-    for (int32_t **p : {&b.stamp, &b.sched[0], &b.sched[1]})
-        if (e == cudaSuccess) e = o.device(p, (size_t)b.tiles);
-    if (e == cudaSuccess) e = o.device(&b.count, 3);
-    if (e == cudaSuccess) e = o.device(&b.goals, 3 * tg);
-    if (e == cudaSuccess) e = o.device(&b.best, tg);
-    if (e == cudaSuccess) e = o.device(&b.member, tg);
-    if (e == cudaSuccess) e = o.device(&b.len, tg);
-    if (e == cudaSuccess) e = o.device(&b.ofs, tg);
-    if (e == cudaSuccess) e = o.device(&b.res, res);
-    if (e == cudaSuccess) e = o.host(&re->goals_host, 3 * tg);
-    if (e == cudaSuccess) e = o.host(&re->res_host, res);
-    if (e == cudaSuccess) e = o.host(&re->cost_host, f->voxels);
-    if (e == cudaSuccess) e = o.event(&re->ev);
-    if (e == cudaSuccess)
-    {
-        b.temp_bytes = dsm_reach_temp_bytes(b);
-        e = b.temp_bytes ? o.device(reinterpret_cast<uint8_t **>(&b.temp), b.temp_bytes) : cudaErrorInvalidValue;
-    }
-    if (e != cudaSuccess)
-    {
-        cudaGetLastError();
-        return DSM_E_NOMEM; // nothing is kept: a later call may try again
-    }
-    ctx->reach = std::move(re);
-    return DSM_OK;
+    o.device(&b.trav, f->voxels);
+    for (uint32_t **p : {&b.cost[0], &b.cost[1]}) o.device(p, f->voxels);
+    for (int32_t **p : {&b.stamp, &b.sched[0], &b.sched[1]}) o.device(p, (size_t)b.tiles);
+    o.device(&b.count, 3);
+    o.device(&b.goals, 3 * tg);
+    o.device(&b.best, tg);
+    o.device(&b.member, tg);
+    o.device(&b.len, tg);
+    o.device(&b.ofs, tg);
+    o.device(&b.res, res);
+    o.host(&re->goals_host, 3 * tg);
+    o.host(&re->res_host, res);
+    o.host(&re->cost_host, f->voxels);
+    o.event(&re->ev);
+    b.temp_bytes = dsm_reach_temp_bytes(b);
+    if (b.temp_bytes) o.device(reinterpret_cast<uint8_t **>(&b.temp), b.temp_bytes);
+    return keep(ctx->reach, re, b.ctas > 0 && b.temp_bytes != 0);
 }
 
 // floor(p / (double)v) - o, clamped to [-1, n]: outside the grid stays outside
@@ -1933,10 +1935,10 @@ extern "C" int dsm_reach_enqueue(dsm_ctx *ctx, const double start[3], float radi
 {
     if (!ctx) return DSM_E_INVALID;
     DsmReach *re = ctx->reach.get();
-    const DsmField *f = ctx->field.get();
-    if (!re || !f || !f->requested || !f->known || re->in_flight) return DSM_E_STATE;
+    const DsmField *f = known_field(ctx);
+    if (!re || !f || re->in_flight) return DSM_E_STATE;
     const DsmFrontier *fr = ctx->frontier.get();
-    if (with_frontiers && (!fr || fr->request != f->requests)) return DSM_E_STATE;
+    if (with_frontiers && !read_latest(fr, f)) return DSM_E_STATE;
     DsmReachBufs &b = re->b;
     if (!start || !std::isfinite(radius) || !(radius >= 0.f) || approach < 0 || approach > DSM_REACH_MAX_APPROACH || n_goals < 0 ||
         n_goals > b.max_targets || (n_goals > 0 && !goals))
@@ -1955,13 +1957,9 @@ extern "C" int dsm_reach_enqueue(dsm_ctx *ctx, const double start[3], float radi
     CK(cudaMemsetAsync(b.res, 0, 4 * DSM_REACH_WORDS, ctx->stream));
     CK(dsm_launch_reach(b, g, f->occ, f->dist, s, radius, approach, n_goals, with_frontiers ? fr->b.res : nullptr,
                         with_frontiers ? fr->b.max_clusters : 0, ctx->stream));
-    CK(cudaMemcpyAsync(re->res_host, b.res, DsmReachBufs::res_bytes(b.max_targets, b.max_path), cudaMemcpyDeviceToHost, ctx->stream));
     if (host_copy) CK(cudaMemcpyAsync(re->cost_host, b.cost[0], 4 * (size_t)b.voxels, cudaMemcpyDeviceToHost, ctx->stream));
-    CK(cudaEventRecord(re->ev, ctx->stream));
-    re->in_flight = true;
     re->host_copy = host_copy != 0;
-    re->request = f->requests;
-    return DSM_OK;
+    return submit(ctx, *re, b.res, DsmReachBufs::res_bytes(b.max_targets, b.max_path), f->requests);
 }
 
 extern "C" int dsm_reach_wait(dsm_ctx *ctx, dsm_reach_info_t *info, const dsm_reach_target_t **targets, const int32_t **path,
@@ -1969,24 +1967,14 @@ extern "C" int dsm_reach_wait(dsm_ctx *ctx, dsm_reach_info_t *info, const dsm_re
 {
     if (!ctx) return DSM_E_INVALID;
     DsmReach *re = ctx->reach.get();
-    if (!re || !re->in_flight) return DSM_E_STATE;
-    CK(cudaSetDevice(ctx->device));
-    CK(cudaEventSynchronize(re->ev));
-    re->in_flight = false;
-    const int32_t *h = reinterpret_cast<const int32_t *>(re->res_host);
+    const int rc = wait_head(ctx, re);
+    if (rc != DSM_OK) return rc;
     const size_t table = 4 * DSM_REACH_WORDS;
-    if (info)
-    {
-        std::memcpy(info, h, sizeof(dsm_reach_info_t));
-        info->reserved[0] = info->reserved[1] = 0;
-    }
+    copy_info(info, re->words());
     if (targets) *targets = reinterpret_cast<const dsm_reach_target_t *>(re->res_host + table);
     if (path) *path = reinterpret_cast<const int32_t *>(re->res_host + table + sizeof(dsm_reach_target_t) * (size_t)re->b.max_targets);
     if (cost) *cost = re->host_copy ? re->cost_host : nullptr;
-    if (h[DSM_REACH_ERR_TAG] == 0) return DSM_OK;
-    snprintf(ctx->err, sizeof(ctx->err), "dsm_reach_wait: frame %d of a dsm_fuse_stream_window call did not fit the pool or the "
-             "store; the field the job read holds the frames before it", h[DSM_REACH_ERR_FRAME]);
-    return DSM_E_CAPACITY;
+    return capacity(ctx, re->words(), DSM_REACH_ERR_TAG, "dsm_reach_wait", "the field the job read");
 }
 
 // ---- travel costs between many sites (include/dsm.h, DESIGN.md §8.13) ----
@@ -2012,35 +2000,21 @@ extern "C" int dsm_reach_matrix_enable(dsm_ctx *ctx, int max_sites, int max_tile
     b.ctas = dsm_reach_matrix_ctas();
     const size_t items = (size_t)max_sites * max_tiles, res = DsmReachMatrixBufs::res_bytes(max_sites);
     CudaOwner &o = rm->own;
-    cudaError_t e = b.ctas > 0 ? cudaSuccess : cudaErrorInvalidValue;
-    for (int32_t **p : {&b.flag, &b.scan, &b.slot})
-        if (e == cudaSuccess) e = o.device(p, (size_t)b.tiles);
-    if (e == cudaSuccess) e = o.device(&b.mask, 16 * (size_t)b.tiles);
-    if (e == cudaSuccess) e = o.device(&b.tile_of, (size_t)max_tiles);
-    for (uint32_t **p : {&b.cost[0], &b.cost[1]})
-        if (e == cudaSuccess) e = o.device(p, items * 512);
-    for (int32_t **p : {&b.stamp, &b.sched[0], &b.sched[1]})
-        if (e == cudaSuccess) e = o.device(p, items);
-    if (e == cudaSuccess) e = o.device(&b.count, 3 * (size_t)max_sites);
-    for (int32_t **p : {&b.rounds, &b.reached})
-        if (e == cudaSuccess) e = o.device(p, (size_t)max_sites);
-    if (e == cudaSuccess) e = o.device(&b.sites, 3 * (size_t)max_sites);
-    if (e == cudaSuccess) e = o.device(&b.res, res);
-    if (e == cudaSuccess) e = o.host(&rm->sites_host, 3 * (size_t)max_sites);
-    if (e == cudaSuccess) e = o.host(&rm->res_host, res);
-    if (e == cudaSuccess) e = o.event(&rm->ev);
-    if (e == cudaSuccess)
-    {
-        b.temp_bytes = dsm_reach_matrix_temp_bytes(b);
-        e = b.temp_bytes ? o.device(reinterpret_cast<uint8_t **>(&b.temp), b.temp_bytes) : cudaErrorInvalidValue;
-    }
-    if (e != cudaSuccess)
-    {
-        cudaGetLastError();
-        return DSM_E_NOMEM; // nothing is kept: a later call may try again
-    }
-    ctx->reach_matrix = std::move(rm);
-    return DSM_OK;
+    for (int32_t **p : {&b.flag, &b.scan, &b.slot}) o.device(p, (size_t)b.tiles);
+    o.device(&b.mask, 16 * (size_t)b.tiles);
+    o.device(&b.tile_of, (size_t)max_tiles);
+    for (uint32_t **p : {&b.cost[0], &b.cost[1]}) o.device(p, items * 512);
+    for (int32_t **p : {&b.stamp, &b.sched[0], &b.sched[1]}) o.device(p, items);
+    o.device(&b.count, 3 * (size_t)max_sites);
+    for (int32_t **p : {&b.rounds, &b.reached}) o.device(p, (size_t)max_sites);
+    o.device(&b.sites, 3 * (size_t)max_sites);
+    o.device(&b.res, res);
+    o.host(&rm->sites_host, 3 * (size_t)max_sites);
+    o.host(&rm->res_host, res);
+    o.event(&rm->ev);
+    b.temp_bytes = dsm_reach_matrix_temp_bytes(b);
+    if (b.temp_bytes) o.device(reinterpret_cast<uint8_t **>(&b.temp), b.temp_bytes);
+    return keep(ctx->reach_matrix, rm, b.ctas > 0 && b.temp_bytes != 0);
 }
 
 // Enqueue only: the points' voxels staged and copied, the job on the grids of the latest (known) field request, one D2H
@@ -2049,8 +2023,8 @@ extern "C" int dsm_reach_matrix_enqueue(dsm_ctx *ctx, const double *points, int 
 {
     if (!ctx) return DSM_E_INVALID;
     DsmReachMatrix *rm = ctx->reach_matrix.get();
-    const DsmField *f = ctx->field.get();
-    if (!rm || !f || !f->requested || !f->known || rm->in_flight) return DSM_E_STATE;
+    const DsmField *f = known_field(ctx);
+    if (!rm || !f || rm->in_flight) return DSM_E_STATE;
     DsmReachMatrixBufs &b = rm->b;
     if (!points || !std::isfinite(radius) || !(radius >= 0.f) || approach < 0 || approach > DSM_REACH_MAX_APPROACH || n_points < 1 ||
         n_points > b.max_sites ||
@@ -2065,34 +2039,21 @@ extern "C" int dsm_reach_matrix_enqueue(dsm_ctx *ctx, const double *points, int 
     CK(cudaMemcpyAsync(b.sites, rm->sites_host, 12 * (size_t)n_points, cudaMemcpyHostToDevice, ctx->stream));
     CK(cudaMemsetAsync(b.res, 0, 4 * DSM_RM_WORDS, ctx->stream));
     CK(dsm_launch_reach_matrix(b, g, f->occ, f->dist, n_points, radius, approach, ctx->stream));
-    CK(cudaMemcpyAsync(rm->res_host, b.res, DsmReachMatrixBufs::res_bytes(n_points), cudaMemcpyDeviceToHost, ctx->stream));
-    CK(cudaEventRecord(rm->ev, ctx->stream));
-    rm->in_flight = true;
     rm->n_sites = n_points;
-    return DSM_OK;
+    return submit(ctx, *rm, b.res, DsmReachMatrixBufs::res_bytes(n_points), f->requests);
 }
 
 extern "C" int dsm_reach_matrix_wait(dsm_ctx *ctx, dsm_reach_matrix_info_t *info, const dsm_reach_site_t **sites, const uint32_t **matrix)
 {
     if (!ctx) return DSM_E_INVALID;
     DsmReachMatrix *rm = ctx->reach_matrix.get();
-    if (!rm || !rm->in_flight) return DSM_E_STATE;
-    CK(cudaSetDevice(ctx->device));
-    CK(cudaEventSynchronize(rm->ev));
-    rm->in_flight = false;
-    const int32_t *h = reinterpret_cast<const int32_t *>(rm->res_host);
+    const int rc = wait_head(ctx, rm);
+    if (rc != DSM_OK) return rc;
     const size_t table = 4 * DSM_RM_WORDS;
-    if (info)
-    {
-        std::memcpy(info, h, sizeof(dsm_reach_matrix_info_t));
-        for (int32_t &w : info->reserved) w = 0;
-    }
+    copy_info(info, rm->words());
     if (sites) *sites = reinterpret_cast<const dsm_reach_site_t *>(rm->res_host + table);
     if (matrix) *matrix = reinterpret_cast<const uint32_t *>(rm->res_host + table + sizeof(dsm_reach_site_t) * (size_t)rm->n_sites);
-    if (h[DSM_RM_ERR_TAG] == 0) return DSM_OK;
-    snprintf(ctx->err, sizeof(ctx->err), "dsm_reach_matrix_wait: frame %d of a dsm_fuse_stream_window call did not fit the pool or "
-             "the store; the field the job read holds the frames before it", h[DSM_RM_ERR_FRAME]);
-    return DSM_E_CAPACITY;
+    return capacity(ctx, rm->words(), DSM_RM_ERR_TAG, "dsm_reach_matrix_wait", "the field the job read");
 }
 
 // ---- view gain against the latest known field (include/dsm.h, DESIGN.md §8.12) ----
@@ -2107,19 +2068,13 @@ extern "C" int dsm_gain_enable(dsm_ctx *ctx, int max_views)
     ga->max_views = max_views;
     const size_t res = DsmGain::res_bytes(max_views);
     CudaOwner &o = ga->own;
-    cudaError_t e = o.device(&ga->views_dev, (size_t)max_views);
-    if (e == cudaSuccess) e = o.host(&ga->views_host, (size_t)max_views);
-    if (e == cudaSuccess) e = o.device(&ga->slot, f->voxels);
-    if (e == cudaSuccess) e = o.device(&ga->res, res);
-    if (e == cudaSuccess) e = o.host(&ga->res_host, res);
-    if (e == cudaSuccess) e = o.event(&ga->ev);
-    if (e != cudaSuccess)
-    {
-        cudaGetLastError();
-        return DSM_E_NOMEM; // nothing is kept: a later call may try again
-    }
-    ctx->gain = std::move(ga);
-    return DSM_OK;
+    o.device(&ga->views_dev, (size_t)max_views);
+    o.host(&ga->views_host, (size_t)max_views);
+    o.device(&ga->slot, f->voxels);
+    o.device(&ga->res, res);
+    o.host(&ga->res_host, res);
+    o.event(&ga->ev);
+    return keep(ctx->gain, ga);
 }
 
 // The grid voxels of view P's box: the bounding box of the image pyramid cut at depth max_range (the apex t and the
@@ -2176,10 +2131,10 @@ extern "C" int dsm_gain_enqueue(dsm_ctx *ctx, const dsm_gain_camera_t *camera, c
 {
     if (!ctx) return DSM_E_INVALID;
     DsmGain *ga = ctx->gain.get();
-    const DsmField *f = ctx->field.get();
-    if (!ga || !f || !f->requested || !f->known || ga->in_flight) return DSM_E_STATE;
+    const DsmField *f = known_field(ctx);
+    if (!ga || !f || ga->in_flight) return DSM_E_STATE;
     const DsmFrontier *fr = ctx->frontier.get();
-    if (clusters && (!fr || fr->request != f->requests)) return DSM_E_STATE;
+    if (clusters && !read_latest(fr, f)) return DSM_E_STATE;
     if (!camera || n_views < 0 || n_views > ga->max_views || (n_views > 0 && !poses)) return DSM_E_INVALID;
     const dsm_gain_camera_t &c = *camera;
     const double v = (double)f->g.voxel, R = (double)c.max_range;
@@ -2206,31 +2161,18 @@ extern "C" int dsm_gain_enqueue(dsm_ctx *ctx, const dsm_gain_camera_t *camera, c
     if (n_views > 0) CK(cudaMemcpyAsync(ga->views_dev, ga->views_host, sizeof(DsmGainView) * (size_t)n_views, cudaMemcpyHostToDevice, ctx->stream));
     CK(dsm_launch_gain(f->g, f->occ, f->dist, c, ga->views_dev, n_views, bricks, clusters ? fr->b.res : nullptr,
                        clusters ? fr->b.max_clusters : 0, ga->slot, ga->res, ctx->stream));
-    CK(cudaMemcpyAsync(ga->res_host, ga->res, DsmGain::res_bytes(n_views), cudaMemcpyDeviceToHost, ctx->stream));
-    CK(cudaEventRecord(ga->ev, ctx->stream));
-    ga->in_flight = true;
-    return DSM_OK;
+    return submit(ctx, *ga, ga->res, DsmGain::res_bytes(n_views), f->requests);
 }
 
 extern "C" int dsm_gain_wait(dsm_ctx *ctx, dsm_gain_info_t *info, const dsm_view_gain_t **gains)
 {
     if (!ctx) return DSM_E_INVALID;
     DsmGain *ga = ctx->gain.get();
-    if (!ga || !ga->in_flight) return DSM_E_STATE;
-    CK(cudaSetDevice(ctx->device));
-    CK(cudaEventSynchronize(ga->ev));
-    ga->in_flight = false;
-    const int32_t *h = reinterpret_cast<const int32_t *>(ga->res_host);
-    if (info)
-    {
-        std::memcpy(info, h, sizeof(dsm_gain_info_t));
-        info->reserved[0] = info->reserved[1] = 0;
-    }
+    const int rc = wait_head(ctx, ga);
+    if (rc != DSM_OK) return rc;
+    copy_info(info, ga->words());
     if (gains) *gains = reinterpret_cast<const dsm_view_gain_t *>(ga->res_host + 4 * DSM_GAIN_WORDS);
-    if (h[DSM_GAIN_ERR_TAG] == 0) return DSM_OK;
-    snprintf(ctx->err, sizeof(ctx->err), "dsm_gain_wait: frame %d of a dsm_fuse_stream_window call did not fit the pool or the "
-             "store; the field the job read holds the frames before it", h[DSM_GAIN_ERR_FRAME]);
-    return DSM_E_CAPACITY;
+    return capacity(ctx, ga->words(), DSM_GAIN_ERR_TAG, "dsm_gain_wait", "the field the job read");
 }
 
 // ---- viewpoints of frontier clusters (include/dsm.h, DESIGN.md §8.15) ----
@@ -2248,22 +2190,16 @@ extern "C" int dsm_viewpoint_enable(dsm_ctx *ctx, int max_clusters, int max_cand
     b.ctas = dsm_viewpoint_ctas();
     const size_t stage = DsmViewpointBufs::stage_bytes(max_clusters), res = DsmViewpointBufs::res_bytes(max_clusters, DSM_VIEWPOINT_MAX_TOP_K);
     CudaOwner &o = vp->own;
-    cudaError_t e = b.ctas > 0 ? o.device(&b.stage, stage) : cudaErrorInvalidValue;
-    if (e == cudaSuccess) e = o.host(&vp->stage_host, stage);
-    if (e == cudaSuccess) e = o.device(&b.cl, (size_t)max_clusters);
-    if (e == cudaSuccess) e = o.device(&b.key, (size_t)max_candidates);
-    if (e == cudaSuccess) e = o.device(&b.list, (size_t)max_candidates);
-    if (e == cudaSuccess) e = o.device(&b.count, 1);
-    if (e == cudaSuccess) e = o.device(&b.res, res);
-    if (e == cudaSuccess) e = o.host(&vp->res_host, res);
-    if (e == cudaSuccess) e = o.event(&vp->ev);
-    if (e != cudaSuccess)
-    {
-        cudaGetLastError();
-        return DSM_E_NOMEM; // nothing is kept: a later call may try again
-    }
-    ctx->viewpoint = std::move(vp);
-    return DSM_OK;
+    o.device(&b.stage, stage);
+    o.host(&vp->stage_host, stage);
+    o.device(&b.cl, (size_t)max_clusters);
+    o.device(&b.key, (size_t)max_candidates);
+    o.device(&b.list, (size_t)max_candidates);
+    o.device(&b.count, 1);
+    o.device(&b.res, res);
+    o.host(&vp->res_host, res);
+    o.event(&vp->ev);
+    return keep(ctx->viewpoint, vp, b.ctas > 0);
 }
 
 // The offsets of include/dsm.h in their order, written as (dx, dy, dz) triples to out (room for
@@ -2294,10 +2230,10 @@ extern "C" int dsm_viewpoint_enqueue(dsm_ctx *ctx, const dsm_gain_camera_t *came
 {
     if (!ctx) return DSM_E_INVALID;
     DsmViewpoint *vp = ctx->viewpoint.get();
-    const DsmField *f = ctx->field.get();
-    if (!vp || !f || !f->requested || !f->known || vp->in_flight) return DSM_E_STATE;
+    const DsmField *f = known_field(ctx);
+    if (!vp || !f || vp->in_flight) return DSM_E_STATE;
     const DsmFrontier *fr = ctx->frontier.get();
-    if (!fr || fr->request != f->requests) return DSM_E_STATE;
+    if (!read_latest(fr, f)) return DSM_E_STATE;
     if (!camera || !params || !rotations || n_rotations < 1 || n_rotations > DSM_VIEWPOINT_MAX_ROTATIONS || n_clusters < 0 ||
         n_clusters > vp->b.max_clusters || (n_clusters > 0 && !clusters))
         return DSM_E_INVALID;
@@ -2320,18 +2256,15 @@ extern "C" int dsm_viewpoint_enqueue(dsm_ctx *ctx, const dsm_gain_camera_t *came
         (long long)n_clusters * n_offsets * p.max_samples > DSM_VIEWPOINT_MAX_WORK)
         return DSM_E_INVALID;
     const DsmReach *re = ctx->reach.get();
-    if (p.with_reach && (!re || re->request != f->requests)) return DSM_E_STATE;
+    if (p.with_reach && !read_latest(re, f)) return DSM_E_STATE;
     CK(cudaSetDevice(ctx->device));
     std::memcpy(vp->stage_host, rotations, 72 * (size_t)n_rotations);
     if (n_clusters > 0) std::memcpy(vp->stage_host + DsmViewpointBufs::stage_clusters(), clusters, 4 * (size_t)n_clusters);
     CK(cudaMemcpyAsync(vp->b.stage, vp->stage_host, DsmViewpointBufs::stage_bytes(n_clusters), cudaMemcpyHostToDevice, ctx->stream));
     CK(dsm_launch_viewpoint(vp->b, f->g, f->occ, f->dist, c, p, n_rotations, n_clusters, n_offsets, fr->b.res, fr->b.max_clusters,
                             p.with_reach ? re->b.cost[0] : nullptr, ctx->stream));
-    CK(cudaMemcpyAsync(vp->res_host, vp->b.res, DsmViewpointBufs::res_bytes(n_clusters, p.top_k), cudaMemcpyDeviceToHost, ctx->stream));
-    CK(cudaEventRecord(vp->ev, ctx->stream));
-    vp->in_flight = true;
     vp->n_clusters = n_clusters, vp->top_k = p.top_k;
-    return DSM_OK;
+    return submit(ctx, *vp, vp->b.res, DsmViewpointBufs::res_bytes(n_clusters, p.top_k), f->requests);
 }
 
 extern "C" int dsm_viewpoint_wait(dsm_ctx *ctx, dsm_viewpoint_info_t *info, const dsm_viewpoint_cluster_t **clusters,
@@ -2339,24 +2272,14 @@ extern "C" int dsm_viewpoint_wait(dsm_ctx *ctx, dsm_viewpoint_info_t *info, cons
 {
     if (!ctx) return DSM_E_INVALID;
     DsmViewpoint *vp = ctx->viewpoint.get();
-    if (!vp || !vp->in_flight) return DSM_E_STATE;
-    CK(cudaSetDevice(ctx->device));
-    CK(cudaEventSynchronize(vp->ev));
-    vp->in_flight = false;
-    const int32_t *h = reinterpret_cast<const int32_t *>(vp->res_host);
+    const int rc = wait_head(ctx, vp);
+    if (rc != DSM_OK) return rc;
     const size_t table = 4 * DSM_VP_WORDS;
-    if (info)
-    {
-        std::memcpy(info, h, sizeof(dsm_viewpoint_info_t));
-        for (int32_t &w : info->reserved) w = 0;
-    }
+    copy_info(info, vp->words());
     if (clusters) *clusters = reinterpret_cast<const dsm_viewpoint_cluster_t *>(vp->res_host + table);
     if (viewpoints)
         *viewpoints = reinterpret_cast<const dsm_viewpoint_t *>(vp->res_host + table + sizeof(dsm_viewpoint_cluster_t) * (size_t)vp->n_clusters);
-    if (h[DSM_VP_ERR_TAG] == 0) return DSM_OK;
-    snprintf(ctx->err, sizeof(ctx->err), "dsm_viewpoint_wait: frame %d of a dsm_fuse_stream_window call did not fit the pool or "
-             "the store; the field the job read holds the frames before it", h[DSM_VP_ERR_FRAME]);
-    return DSM_E_CAPACITY;
+    return capacity(ctx, vp->words(), DSM_VP_ERR_TAG, "dsm_viewpoint_wait", "the field the job read");
 }
 
 // ---- the order of an exploration tour (include/dsm.h, DESIGN.md §8.14) ----
@@ -2370,19 +2293,13 @@ extern "C" int dsm_tour_enable(dsm_ctx *ctx, int max_sites, int max_starts)
     tr->max_sites = max_sites, tr->max_starts = max_starts;
     const size_t entries = (size_t)max_sites * max_sites, res = dsm_tour_res_bytes(max_starts, max_sites);
     CudaOwner &o = tr->own;
-    cudaError_t e = o.host(&tr->matrix_host, entries);
-    if (e == cudaSuccess) e = o.device(&tr->matrix, entries);
-    if (e == cudaSuccess) e = o.device(&tr->tours, (size_t)max_starts * max_sites);
-    if (e == cudaSuccess) e = o.device(&tr->res, res);
-    if (e == cudaSuccess) e = o.host(&tr->res_host, res);
-    if (e == cudaSuccess) e = o.event(&tr->ev);
-    if (e != cudaSuccess)
-    {
-        cudaGetLastError();
-        return DSM_E_NOMEM; // nothing is kept: a later call may try again
-    }
-    ctx->tour = std::move(tr);
-    return DSM_OK;
+    o.host(&tr->matrix_host, entries);
+    o.device(&tr->matrix, entries);
+    o.device(&tr->tours, (size_t)max_starts * max_sites);
+    o.device(&tr->res, res);
+    o.host(&tr->res_host, res);
+    o.event(&tr->ev);
+    return keep(ctx->tour, tr);
 }
 
 // Enqueue only: the matrix staged and copied, the kernels, one D2H copy of the used result and the event.
@@ -2401,21 +2318,16 @@ extern "C" int dsm_tour_enqueue(dsm_ctx *ctx, const uint32_t *matrix, int n, int
     std::memcpy(tr->matrix_host, matrix, bytes);
     CK(cudaMemcpyAsync(tr->matrix, tr->matrix_host, bytes, cudaMemcpyHostToDevice, ctx->stream));
     CK(dsm_launch_tour(tr->matrix, n, open, n_starts, max_passes, seed, tr->tours, tr->res, ctx->stream));
-    CK(cudaMemcpyAsync(tr->res_host, tr->res, dsm_tour_res_bytes(n_starts, n), cudaMemcpyDeviceToHost, ctx->stream));
-    CK(cudaEventRecord(tr->ev, ctx->stream));
-    tr->in_flight = true;
     tr->n = n, tr->n_starts = n_starts;
-    return DSM_OK;
+    return submit(ctx, *tr, tr->res, dsm_tour_res_bytes(n_starts, n), 0);
 }
 
 extern "C" int dsm_tour_wait(dsm_ctx *ctx, dsm_tour_info_t *info, const dsm_tour_start_t **starts, const int32_t **order)
 {
     if (!ctx) return DSM_E_INVALID;
     DsmTour *tr = ctx->tour.get();
-    if (!tr || !tr->in_flight) return DSM_E_STATE;
-    CK(cudaSetDevice(ctx->device));
-    CK(cudaEventSynchronize(tr->ev));
-    tr->in_flight = false;
+    const int rc = wait_head(ctx, tr);
+    if (rc != DSM_OK) return rc;
     if (info) std::memcpy(info, tr->res_host, sizeof(dsm_tour_info_t));
     if (starts) *starts = reinterpret_cast<const dsm_tour_start_t *>(tr->res_host + sizeof(dsm_tour_info_t));
     if (order) *order = reinterpret_cast<const int32_t *>(tr->res_host + sizeof(dsm_tour_info_t) + sizeof(dsm_tour_start_t) * (size_t)tr->n_starts);
@@ -2880,6 +2792,7 @@ extern "C" int dsm_frame_raw_cloud(dsm_ctx *ctx, int frame, const double pose7[7
     if (!ctx->raw_out && ctx->own.device(&ctx->raw_out, npx) != cudaSuccess)
     {
         cudaGetLastError();
+        ctx->own.take();
         ctx->raw_out = nullptr;
         return DSM_E_NOMEM;
     }
@@ -2908,6 +2821,7 @@ extern "C" int dsm_frame_superpixel_image(dsm_ctx *ctx, int frame, uint8_t *bgr,
     if (!ctx->spimg_out && ctx->own.device(&ctx->spimg_out, row * H) != cudaSuccess)
     {
         cudaGetLastError();
+        ctx->own.take();
         ctx->spimg_out = nullptr;
         return DSM_E_NOMEM;
     }

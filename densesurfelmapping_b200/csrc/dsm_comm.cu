@@ -269,14 +269,15 @@ extern "C" int dsm_comm_init(dsm_ctx *ctx, const void *id, int rank, int nranks)
     ncclUniqueId uid;
     memcpy(&uid, id, DSM_COMM_ID_BYTES);
     NK(api->CommInitRank(&c->comm, nranks, uid, rank));
-    CK(c->own.stream(&c->stream));
-    CK(c->own.event(&c->ev_kernels));
-    CK(c->own.event(&c->ev_packed));
+    c->own.stream(&c->stream);
+    c->own.event(&c->ev_kernels);
+    c->own.event(&c->ev_packed);
     c->pack_cap = payload_cap(ctx);
-    CK(c->own.device(&c->pack, c->pack_cap));
-    CK(c->own.device(&c->d_bytes, (size_t)nranks));
-    CK(c->own.host(&c->h_bytes, (size_t)nranks));
-    CK(c->own.host(&c->h_cnt, (size_t)ctx->p.max_batch));
+    c->own.device(&c->pack, c->pack_cap);
+    c->own.device(&c->d_bytes, (size_t)nranks);
+    c->own.host(&c->h_bytes, (size_t)nranks);
+    c->own.host(&c->h_cnt, (size_t)ctx->p.max_batch);
+    CK(c->own.take());
     c->ofs.assign((size_t)nranks + 1, 0);
     return DSM_OK;
 }
@@ -302,14 +303,15 @@ static int peer_setup(dsm_ctx *ctx, int root)
     c->slot_bytes = (c->pack_cap + 255) / 256 * 256;
     if (!c->slots)
     {
-        CK(c->own.device(&c->slots, (size_t)c->nranks * c->slot_bytes));
-        CK(c->own.device(&c->ctrl, 1));
+        c->own.device(&c->slots, (size_t)c->nranks * c->slot_bytes);
+        c->own.device(&c->ctrl, 1);
     }
     if (!c->poll)
     {
-        CK(c->own.stream(&c->poll));
-        CK(c->own.host(&c->h_arrived, DSM_MAX_RANKS));
+        c->own.stream(&c->poll);
+        c->own.host(&c->h_arrived, DSM_MAX_RANKS);
     }
+    CK(c->own.take());
     c->done_seq = 0;
     CK(cudaMemsetAsync(c->ctrl, 0, sizeof(DsmPeerCtrl), cs));
     CK(cudaStreamSynchronize(cs)); // zeroed before any peer can hold the handle
@@ -326,7 +328,8 @@ static int peer_setup(dsm_ctx *ctx, int root)
     cudaGetLastError();
     memcpy(mine, &h_slots, 64);
     memcpy(mine + 64, &h_ctrl, 64);
-    if (!c->d_handles) CK(c->own.device(&c->d_handles, (size_t)c->nranks * 128));
+    if (!c->d_handles) c->own.device(&c->d_handles, (size_t)c->nranks * 128);
+    CK(c->own.take());
     CK(cudaMemcpyAsync(c->d_handles + (size_t)c->rank * 128, mine, 128, cudaMemcpyHostToDevice, cs));
     NK(api->AllGather(c->d_handles + (size_t)c->rank * 128, c->d_handles, 128, ncclInt8, c->comm, cs));
     std::vector<unsigned char> all((size_t)c->nranks * 128);

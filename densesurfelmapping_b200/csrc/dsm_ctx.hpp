@@ -31,48 +31,64 @@ using GraphExecPtr = std::unique_ptr<CUgraphExec_st, Release<cudaGraphExec_t, cu
 // Every allocation, stream and event a context or communicator makes once and keeps for its lifetime.  The raw pointers
 // and handles the code works with (and the DsmDev the kernels receive) are views; the owner releases them when its
 // holder is deleted.  The holder's streams must be drained before that.
+//
+// The owner keeps its first failed call until take(): every call after it is a no-op that returns that failure, so a
+// list of calls needs one check at its end.  An owner that outlives a failure takes it before its next call.
 struct CudaOwner
 {
     std::vector<DevPtr<void>> dev;
     std::vector<HostPtr> pinned;
     std::vector<StreamPtr> streams;
     std::vector<EventPtr> events;
+    cudaError_t failed = cudaSuccess;
 
+    // the first failure since the last take() (cudaSuccess: none), cleared
+    cudaError_t take()
+    {
+        const cudaError_t e = failed;
+        failed = cudaSuccess;
+        return e;
+    }
     template <typename T>
     cudaError_t device(T **p, size_t n, bool zero = false)
     {
+        if (failed != cudaSuccess) return failed;
         cudaError_t e = cudaMalloc((void **)p, n * sizeof(T));
         if (e == cudaSuccess) dev.emplace_back(*p);
         if (e == cudaSuccess && zero) e = cudaMemset(*p, 0, n * sizeof(T));
-        return e;
+        return failed = e;
     }
     template <typename T>
     cudaError_t host(T **p, size_t n)
     {
+        if (failed != cudaSuccess) return failed;
         cudaError_t e = cudaMallocHost((void **)p, n * sizeof(T));
         if (e == cudaSuccess) pinned.emplace_back(*p);
-        return e;
+        return failed = e;
     }
     // pinned host memory the device writes directly: *dev is its device alias
     template <typename T, typename D>
     cudaError_t mapped(T **p, D **dev, size_t n)
     {
+        if (failed != cudaSuccess) return failed;
         cudaError_t e = cudaHostAlloc((void **)p, n * sizeof(T), cudaHostAllocMapped);
-        if (e != cudaSuccess) return e;
+        if (e != cudaSuccess) return failed = e;
         pinned.emplace_back(*p);
-        return cudaHostGetDevicePointer((void **)dev, *p, 0);
+        return failed = cudaHostGetDevicePointer((void **)dev, *p, 0);
     }
     cudaError_t stream(cudaStream_t *s, int priority = 0)
     {
+        if (failed != cudaSuccess) return failed;
         cudaError_t e = cudaStreamCreateWithPriority(s, cudaStreamNonBlocking, priority);
         if (e == cudaSuccess) streams.emplace_back(*s);
-        return e;
+        return failed = e;
     }
     cudaError_t event(cudaEvent_t *ev, unsigned flags = cudaEventDisableTiming)
     {
+        if (failed != cudaSuccess) return failed;
         cudaError_t e = cudaEventCreateWithFlags(ev, flags);
         if (e == cudaSuccess) events.emplace_back(*ev);
-        return e;
+        return failed = e;
     }
 };
 #pragma GCC visibility pop
@@ -202,16 +218,25 @@ struct DsmViews
     static size_t stage_bytes(int n) { return 12 * sizeof(double) * (size_t)n + sizeof(int32_t) * (size_t)n; }
 };
 
-// dsm_field_query_* (DESIGN.md §8.8): the packed request (pinned staging and its device twin), the packed result
-// (device and its pinned copy) at the capacities of dsm_field_query_enable, and the event after the result's copy
-struct DsmFieldQuery
+// What every planner job (dsm_field_query_* and the jobs on the known field, DESIGN.md §8.8-8.15) holds besides its
+// own buffers: their owner, the pinned copy of its packed result, and the event after that copy
+struct DsmJob
 {
     CudaOwner own;
-    int max_points = 0, max_traj = 0, max_wp = 0;
-    uint8_t *req_host = nullptr, *req_dev = nullptr, *res_host = nullptr, *res_dev = nullptr;
+    uint8_t *res_host = nullptr;
     cudaEvent_t ev = nullptr;
+    bool in_flight = false; // enqueued and not yet waited for
+    uint64_t request = 0;   // the DsmField::requests of the field the latest job read (0: no job yet, or a tour)
+    const int32_t *words() const { return reinterpret_cast<const int32_t *>(res_host); } // the result's header
+};
+
+// dsm_field_query_* (DESIGN.md §8.8): the packed request (pinned staging and its device twin) and the device result at
+// the capacities of dsm_field_query_enable
+struct DsmFieldQuery : DsmJob
+{
+    int max_points = 0, max_traj = 0, max_wp = 0;
+    uint8_t *req_host = nullptr, *req_dev = nullptr, *res_dev = nullptr;
     int n_points = 0, n_traj = 0; // of the query in flight or last waited for
-    bool in_flight = false;
     // byte offsets of the packed layouts (dsm_device.cuh) for n_points, n_wp and n_traj
     static size_t req_bytes(int n_points, int n_wp, int n_traj) { return 24 * ((size_t)n_points + n_wp) + 4 * ((size_t)n_traj + 1 + n_wp); }
     static size_t res_clearance(int n_points) { return 16 * (1 + (size_t)n_points); }
@@ -219,84 +244,60 @@ struct DsmFieldQuery
 };
 
 // dsm_frontier_* (DESIGN.md §8.10), allocated by dsm_frontier_enable for the field's grid: the job's device buffers
-// (DsmFrontierBufs, the packed result among them), the result's pinned copy and the event after its copy
-struct DsmFrontier
+// (DsmFrontierBufs, the packed result among them)
+struct DsmFrontier : DsmJob
 {
-    CudaOwner own;
     DsmFrontierBufs b;
-    uint8_t *res_host = nullptr;
-    cudaEvent_t ev = nullptr;
-    bool in_flight = false;
-    uint64_t request = 0; // the DsmField::requests of the field the latest job read (0: no job yet)
 };
 
 // dsm_reach_* (DESIGN.md §8.11), allocated by dsm_reach_enable for the field's grid: the job's device buffers
-// (DsmReachBufs, the packed result among them), the goal staging, the result's and the cost grid's pinned copies and the
-// event after them
-struct DsmReach
+// (DsmReachBufs, the packed result among them), the goal staging and the cost grid's pinned copy
+struct DsmReach : DsmJob
 {
-    CudaOwner own;
     DsmReachBufs b;
     int32_t *goals_host = nullptr; // pinned [max_targets][3]
-    uint8_t *res_host = nullptr;
     uint32_t *cost_host = nullptr; // pinned [voxels]
-    cudaEvent_t ev = nullptr;
-    bool in_flight = false, host_copy = false;
-    uint64_t request = 0; // the DsmField::requests of the field the latest job read (0: no job yet)
+    bool host_copy = false;
 };
 
 // dsm_reach_matrix_* (DESIGN.md §8.13), allocated by dsm_reach_matrix_enable for the field's grid: the job's device
-// buffers (DsmReachMatrixBufs, the packed result among them), the site staging, the result's pinned copy and the event
-// after it
-struct DsmReachMatrix
+// buffers (DsmReachMatrixBufs, the packed result among them) and the site staging
+struct DsmReachMatrix : DsmJob
 {
-    CudaOwner own;
     DsmReachMatrixBufs b;
     int32_t *sites_host = nullptr; // pinned [max_sites][3]
-    uint8_t *res_host = nullptr;
-    cudaEvent_t ev = nullptr;
     int n_sites = 0; // of the job in flight or last waited for
-    bool in_flight = false;
 };
 
 // dsm_gain_* (DESIGN.md §8.12), allocated by dsm_gain_enable for the field's grid: the pinned and device staging of
-// max_views views, the cluster-slot grid, the device result and its pinned copy, and the event after the copy
-struct DsmGain
+// max_views views, the cluster-slot grid and the device result
+struct DsmGain : DsmJob
 {
-    CudaOwner own;
     int max_views = 0;
     DsmGainView *views_host = nullptr, *views_dev = nullptr; // [max_views]
     int32_t *slot = nullptr;                                  // device [voxels]
-    uint8_t *res = nullptr, *res_host = nullptr;              // 4 DSM_GAIN_WORDS + 32 max_views bytes each
-    cudaEvent_t ev = nullptr;
-    bool in_flight = false;
+    uint8_t *res = nullptr;                                   // 4 DSM_GAIN_WORDS + 32 max_views bytes
     static size_t res_bytes(int n_views) { return 4 * (size_t)DSM_GAIN_WORDS + sizeof(dsm_view_gain_t) * (size_t)n_views; }
 };
 
 // dsm_viewpoint_* (DESIGN.md §8.15), allocated by dsm_viewpoint_enable: the job's device buffers (DsmViewpointBufs, the
-// packed result among them), the pinned staging and the result's pinned copy, and the event after the copy
-struct DsmViewpoint
+// packed result among them) and the pinned staging
+struct DsmViewpoint : DsmJob
 {
-    CudaOwner own;
     DsmViewpointBufs b;
-    uint8_t *stage_host = nullptr, *res_host = nullptr;
-    cudaEvent_t ev = nullptr;
+    uint8_t *stage_host = nullptr;
     int n_clusters = 0, top_k = 0; // of the job in flight or last waited for
-    bool in_flight = false;
 };
 
 // dsm_tour_* (DESIGN.md §8.14), allocated by dsm_tour_enable: the pinned and device matrix of max_sites^2 entries, the
-// starts' tours, the device result and its pinned copy, and the event after the copy
-struct DsmTour
+// starts' tours and the device result
+struct DsmTour : DsmJob
 {
-    CudaOwner own;
     int max_sites = 0, max_starts = 0;
     uint32_t *matrix_host = nullptr, *matrix = nullptr; // [max_sites^2] each
     int32_t *tours = nullptr;                           // device [max_starts][max_sites]
-    uint8_t *res = nullptr, *res_host = nullptr;        // dsm_tour_res_bytes(max_starts, max_sites) each
-    cudaEvent_t ev = nullptr;
+    uint8_t *res = nullptr;                             // dsm_tour_res_bytes(max_starts, max_sites)
     int n = 0, n_starts = 0; // of the job in flight or last waited for
-    bool in_flight = false;
 };
 
 #define DSM_MAX_CHUNKS 4

@@ -549,19 +549,14 @@ class SurfelMapNode
         clusters.clear();
         voxels.clear();
         counts = dsm_frontier_counts_t();
-        if (!ctx_.ready("frontiers")) return ctx_.err;
-        if (known_.empty() || !field_exists_) return ctx_.done(DSM_E_STATE, "frontiers");
-        int rc = dsm_frontier_enqueue(ctx_.ctx, min_voxels);
-        if (rc != DSM_OK) return ctx_.done(rc, "frontiers");
         const dsm_frontier_cluster_t *c = nullptr;
         const int32_t *v = nullptr;
-        rc = dsm_frontier_wait(ctx_.ctx, &c, &v, &counts);
-        if (rc == DSM_OK || rc == DSM_E_CAPACITY)
-        {
-            clusters.assign(c, c + std::min(counts.n_clusters, frontier_clusters_));
-            voxels.assign(v, v + counts.n_listed);
-        }
-        return ctx_.done(rc, "frontiers");
+        return job("frontiers", KNOWN_FIELD, true, [&] { return dsm_frontier_enqueue(ctx_.ctx, min_voxels); },
+                   [&] { return dsm_frontier_wait(ctx_.ctx, &c, &v, &counts); },
+                   [&] {
+                       clusters.assign(c, c + std::min(counts.n_clusters, frontier_clusters_));
+                       voxels.assign(v, v + counts.n_listed);
+                   });
     }
 
     // ---- paths through the known free space of the latest fused frame's field (DESIGN.md §8.11) ----
@@ -584,20 +579,16 @@ class SurfelMapNode
         targets.clear();
         path.clear();
         info = dsm_reach_info_t();
-        if (!ctx_.ready("reach")) return ctx_.err;
-        if (known_.empty() || !field_exists_) return ctx_.done(DSM_E_STATE, "reach");
-        if (goals.size() % 3 != 0) return ctx_.done(DSM_E_INVALID, "reach");
-        int rc = dsm_reach_enqueue(ctx_.ctx, start, radius, approach, goals.data(), (int)(goals.size() / 3), with_frontiers, 0);
-        if (rc != DSM_OK) return ctx_.done(rc, "reach");
         const dsm_reach_target_t *t = nullptr;
         const int32_t *p = nullptr;
-        rc = dsm_reach_wait(ctx_.ctx, &info, &t, &p, nullptr);
-        if (rc == DSM_OK || rc == DSM_E_CAPACITY)
-        {
-            targets.assign(t, t + std::min(info.n_targets, reach_targets_));
-            path.assign(p, p + info.n_path_voxels);
-        }
-        return ctx_.done(rc, "reach");
+        return job(
+            "reach", KNOWN_FIELD, goals.size() % 3 == 0,
+            [&] { return dsm_reach_enqueue(ctx_.ctx, start, radius, approach, goals.data(), (int)(goals.size() / 3), with_frontiers, 0); },
+            [&] { return dsm_reach_wait(ctx_.ctx, &info, &t, &p, nullptr); },
+            [&] {
+                targets.assign(t, t + std::min(info.n_targets, reach_targets_));
+                path.assign(p, p + info.n_path_voxels);
+            });
     }
 
     // ---- travel costs between many points of the latest fused frame's field (DESIGN.md §8.13) ----
@@ -618,20 +609,15 @@ class SurfelMapNode
         sites.clear();
         matrix.clear();
         info = dsm_reach_matrix_info_t();
-        if (!ctx_.ready("reach_matrix")) return ctx_.err;
-        if (known_.empty() || !field_exists_) return ctx_.done(DSM_E_STATE, "reach_matrix");
-        if (points.size() % 3 != 0) return ctx_.done(DSM_E_INVALID, "reach_matrix");
-        int rc = dsm_reach_matrix_enqueue(ctx_.ctx, points.data(), (int)(points.size() / 3), radius, approach);
-        if (rc != DSM_OK) return ctx_.done(rc, "reach_matrix");
         const dsm_reach_site_t *s = nullptr;
         const uint32_t *m = nullptr;
-        rc = dsm_reach_matrix_wait(ctx_.ctx, &info, &s, &m);
-        if (rc == DSM_OK || rc == DSM_E_CAPACITY)
-        {
-            sites.assign(s, s + info.n_sites);
-            matrix.assign(m, m + (size_t)info.n_sites * info.n_sites);
-        }
-        return ctx_.done(rc, "reach_matrix");
+        return job("reach_matrix", KNOWN_FIELD, points.size() % 3 == 0,
+                   [&] { return dsm_reach_matrix_enqueue(ctx_.ctx, points.data(), (int)(points.size() / 3), radius, approach); },
+                   [&] { return dsm_reach_matrix_wait(ctx_.ctx, &info, &s, &m); },
+                   [&] {
+                       sites.assign(s, s + info.n_sites);
+                       matrix.assign(m, m + (size_t)info.n_sites * info.n_sites);
+                   });
     }
 
     // ---- the order of an exploration tour over a travel-cost matrix (DESIGN.md §8.14) ----
@@ -650,19 +636,15 @@ class SurfelMapNode
         starts.clear();
         order.clear();
         info = dsm_tour_info_t();
-        if (!ctx_.ready("tour")) return ctx_.err;
-        if (n < 0 || matrix.size() != (size_t)n * n) return ctx_.done(DSM_E_INVALID, "tour");
-        int rc = dsm_tour_enqueue(ctx_.ctx, matrix.data(), n, open, n_starts, max_passes, seed);
-        if (rc != DSM_OK) return ctx_.done(rc, "tour");
         const dsm_tour_start_t *s = nullptr;
         const int32_t *o = nullptr;
-        rc = dsm_tour_wait(ctx_.ctx, &info, &s, &o);
-        if (rc == DSM_OK)
-        {
-            starts.assign(s, s + info.n_starts);
-            order.assign(o, o + info.n_sites);
-        }
-        return ctx_.done(rc, "tour");
+        return job("tour", NO_FIELD, n >= 0 && matrix.size() == (size_t)n * n,
+                   [&] { return dsm_tour_enqueue(ctx_.ctx, matrix.data(), n, open, n_starts, max_passes, seed); },
+                   [&] { return dsm_tour_wait(ctx_.ctx, &info, &s, &o); },
+                   [&] {
+                       starts.assign(s, s + info.n_starts);
+                       order.assign(o, o + info.n_sites);
+                   });
     }
 
     // ---- view gain against the known field of the latest fused frame (DESIGN.md §8.12) ----
@@ -681,20 +663,11 @@ class SurfelMapNode
     {
         gains.clear();
         info = dsm_gain_info_t();
-        if (!ctx_.ready("view_gain")) return ctx_.err;
-        if (known_.empty() || !field_exists_) return ctx_.done(DSM_E_STATE, "view_gain");
-        if (!clusters.empty() && (int)clusters.size() != n_views) return ctx_.done(DSM_E_INVALID, "view_gain");
-        dsm_gain_camera_t cam;
-        cam.fx = cam_[0], cam.fy = cam_[1], cam.cx = cam_[2], cam.cy = cam_[3];
-        cam.width = width_, cam.height = height_;
-        cam.max_range = max_range;
-        cam.unknown_blocks = unknown_blocks;
-        int rc = dsm_gain_enqueue(ctx_.ctx, &cam, poses, clusters.empty() ? nullptr : clusters.data(), n_views);
-        if (rc != DSM_OK) return ctx_.done(rc, "view_gain");
+        const dsm_gain_camera_t cam = gain_camera(max_range, unknown_blocks);
         const dsm_view_gain_t *g = nullptr;
-        rc = dsm_gain_wait(ctx_.ctx, &info, &g);
-        if (rc == DSM_OK || rc == DSM_E_CAPACITY) gains.assign(g, g + info.n_views);
-        return ctx_.done(rc, "view_gain");
+        return job("view_gain", KNOWN_FIELD, clusters.empty() || (int)clusters.size() == n_views,
+                   [&] { return dsm_gain_enqueue(ctx_.ctx, &cam, poses, clusters.empty() ? nullptr : clusters.data(), n_views); },
+                   [&] { return dsm_gain_wait(ctx_.ctx, &info, &g); }, [&] { gains.assign(g, g + info.n_views); });
     }
 
     // ---- viewpoints of frontier clusters against the known field of the latest fused frame (DESIGN.md §8.15) ----
@@ -718,25 +691,18 @@ class SurfelMapNode
         cluster_records.clear();
         viewpoints.clear();
         info = dsm_viewpoint_info_t();
-        if (!ctx_.ready("viewpoints")) return ctx_.err;
-        if (known_.empty() || !field_exists_) return ctx_.done(DSM_E_STATE, "viewpoints");
-        dsm_gain_camera_t cam;
-        cam.fx = cam_[0], cam.fy = cam_[1], cam.cx = cam_[2], cam.cy = cam_[3];
-        cam.width = width_, cam.height = height_;
-        cam.max_range = max_range;
-        cam.unknown_blocks = unknown_blocks;
+        const dsm_gain_camera_t cam = gain_camera(max_range, unknown_blocks);
         params.with_reach = with_reach;
-        int rc = dsm_viewpoint_enqueue(ctx_.ctx, &cam, rotations, n_rotations, clusters.data(), (int)clusters.size(), &params);
-        if (rc != DSM_OK) return ctx_.done(rc, "viewpoints");
         const dsm_viewpoint_cluster_t *c = nullptr;
         const dsm_viewpoint_t *v = nullptr;
-        rc = dsm_viewpoint_wait(ctx_.ctx, &info, &c, &v);
-        if (rc == DSM_OK || rc == DSM_E_CAPACITY)
-        {
-            cluster_records.assign(c, c + info.n_clusters);
-            viewpoints.assign(v, v + (size_t)info.n_clusters * info.top_k);
-        }
-        return ctx_.done(rc, "viewpoints");
+        return job(
+            "viewpoints", KNOWN_FIELD, true,
+            [&] { return dsm_viewpoint_enqueue(ctx_.ctx, &cam, rotations, n_rotations, clusters.data(), (int)clusters.size(), &params); },
+            [&] { return dsm_viewpoint_wait(ctx_.ctx, &info, &c, &v); },
+            [&] {
+                cluster_records.assign(c, c + info.n_clusters);
+                viewpoints.assign(v, v + (size_t)info.n_clusters * info.top_k);
+            });
     }
 
     // ---- planner queries against the field of the latest fused frame (DESIGN.md §8.8) ----
@@ -882,22 +848,50 @@ class SurfelMapNode
     dsm_ctx *context() { return ctx_.ctx; }
 
   private:
+    // what a planner job reads: nothing, the latest fused frame's field, or its known field
+    enum JobField
+    {
+        NO_FIELD,
+        ANY_FIELD,
+        KNOWN_FIELD,
+    };
+    // One synchronous planner job: the context ready, DSM_E_STATE without the field it reads, DSM_E_INVALID unless
+    // `valid` (the caller's own argument check), then enqueue and wait, and assign takes the results of a job that
+    // returned DSM_OK or DSM_E_CAPACITY (the results of the last applied frame's field, as distance_field())
+    template <typename Enqueue, typename Wait, typename Assign>
+    int job(const char *what, JobField reads, bool valid, Enqueue enqueue, Wait wait, Assign assign)
+    {
+        if (!ctx_.ready(what)) return ctx_.err;
+        if ((reads == KNOWN_FIELD && known_.empty()) || (reads != NO_FIELD && !field_exists_)) return ctx_.done(DSM_E_STATE, what);
+        if (!valid) return ctx_.done(DSM_E_INVALID, what);
+        int rc = enqueue();
+        if (rc != DSM_OK) return ctx_.done(rc, what);
+        rc = wait();
+        if (rc == DSM_OK || rc == DSM_E_CAPACITY) assign();
+        return ctx_.done(rc, what);
+    }
+    // the camera of view_gain() and viewpoints(): the node's intrinsics and image size
+    dsm_gain_camera_t gain_camera(float max_range, int unknown_blocks) const
+    {
+        dsm_gain_camera_t cam;
+        cam.fx = cam_[0], cam.fy = cam_[1], cam.cx = cam_[2], cam.cy = cam_[3];
+        cam.width = width_, cam.height = height_;
+        cam.max_range = max_range;
+        cam.unknown_blocks = unknown_blocks;
+        return cam;
+    }
     int query(const char *what, const double *points, int n_points, const double *waypoints, const int32_t *offsets, int n_traj, float step,
               float radius, std::vector<dsm_field_sample_t> *samples, std::vector<dsm_clearance_t> *clearance)
     {
-        if (!ctx_.ready(what)) return ctx_.err;
-        if (!field_exists_) return ctx_.done(DSM_E_STATE, what);
-        int rc = dsm_field_query_enqueue(ctx_.ctx, points, n_points, waypoints, offsets, n_traj, step, radius);
-        if (rc != DSM_OK) return ctx_.done(rc, what);
         const dsm_field_sample_t *s = nullptr;
         const dsm_clearance_t *c = nullptr;
-        rc = dsm_field_query_wait(ctx_.ctx, &s, &c);
-        if (rc == DSM_OK || rc == DSM_E_CAPACITY)
-        {
-            if (samples) samples->assign(s, s + n_points);
-            if (clearance) clearance->assign(c, c + n_traj);
-        }
-        return ctx_.done(rc, what);
+        return job(what, ANY_FIELD, true,
+                   [&] { return dsm_field_query_enqueue(ctx_.ctx, points, n_points, waypoints, offsets, n_traj, step, radius); },
+                   [&] { return dsm_field_query_wait(ctx_.ctx, &s, &c); },
+                   [&] {
+                       if (samples) samples->assign(s, s + n_points);
+                       if (clearance) clearance->assign(c, c + n_traj);
+                   });
     }
 
     // load_state / load_state_incremental: the file (journal = false) or base + journal (true) peeked and checked against
