@@ -37,6 +37,7 @@ EXPORTS = [
     "dsm_field_enqueue_resident", "dsm_field_query_enable", "dsm_field_query_enqueue", "dsm_field_query_wait",
     "dsm_views_enable", "dsm_views_capture", "dsm_field_enqueue_known", "dsm_field_state",
     "dsm_frontier_enable", "dsm_frontier_enqueue", "dsm_frontier_wait", "dsm_debug_field_load_state",
+    "dsm_field_signed_enable", "dsm_field_signed", "dsm_field_query_enqueue_signed",
     "dsm_reach_enable", "dsm_reach_enqueue", "dsm_reach_wait", "dsm_reach_matrix_enable", "dsm_reach_matrix_enqueue",
     "dsm_reach_matrix_wait", "dsm_gain_enable", "dsm_gain_enqueue", "dsm_gain_wait",
     "dsm_tour_enable", "dsm_tour_enqueue", "dsm_tour_wait", "dsm_viewpoint_enable", "dsm_viewpoint_enqueue", "dsm_viewpoint_wait",
@@ -182,6 +183,9 @@ def load_library():
     L.dsm_frontier_enqueue.argtypes = [vp, ci]
     L.dsm_frontier_wait.argtypes = [vp, ctypes.POINTER(vp), ctypes.POINTER(vp), vp]
     L.dsm_debug_field_load_state.argtypes = [vp, vp, ctypes.POINTER(ctypes.c_int32)]
+    L.dsm_field_signed_enable.argtypes = [vp]
+    L.dsm_field_signed.argtypes = [vp, ctypes.POINTER(vp)]
+    L.dsm_field_query_enqueue_signed.argtypes = [vp, vp, ci, vp, vp, ci, ctypes.c_float, ctypes.c_float]
     L.dsm_reach_enable.argtypes = [vp, ci, ci, ci]
     L.dsm_reach_enqueue.argtypes = [vp, ctypes.POINTER(ctypes.c_double), ctypes.c_float, ci, vp, ci, ci, ci]
     L.dsm_reach_wait.argtypes = [vp, vp, ctypes.POINTER(vp), ctypes.POINTER(vp), ctypes.POINTER(vp)]
@@ -659,6 +663,23 @@ class Context:
             return dist, np.array(org[:], dtype=np.int32), nocc.value
         return self._waited(rc, "field", field)
 
+    # ---- the signed distance field ----
+    def field_signed_enable(self):
+        """Every field request from now on also builds the signed grid (negative depth inside the sites)."""
+        self._ck(self.lib.dsm_field_signed_enable(self.h))
+
+    def field_signed(self):
+        """The signed grid of the last waited field: a float32 [nz][ny][nx] copy of the context's pinned buffer, or None
+        for a resident field.  A field requested after a rejected frame raises DsmError(DSM_E_CAPACITY) carrying the
+        same value as `.signed` (the grid of the last applied frame)."""
+        ptr = ctypes.c_void_p()
+        rc = self.lib.dsm_field_signed(self.h, ctypes.byref(ptr))
+
+        def grid():
+            shape = self._field_shape
+            return _take(ptr, shape[0] * shape[1] * shape[2], np.float32).reshape(shape) if ptr.value else None
+        return self._waited(rc, "signed", grid)
+
     # ---- free versus unknown space ----
     def views_enable(self, max_views, max_range):
         self._ck(self.lib.dsm_views_enable(self.h, int(max_views), float(max_range)))
@@ -846,16 +867,16 @@ class Context:
     def field_query_enable(self, max_points, max_trajectories, max_waypoints):
         self._ck(self.lib.dsm_field_query_enable(self.h, int(max_points), int(max_trajectories), int(max_waypoints)))
 
-    def field_query_enqueue(self, points=None, waypoints=None, offsets=None, step=1.0, radius=0.0):
+    def field_query_enqueue(self, points=None, waypoints=None, offsets=None, step=1.0, radius=0.0, signed=False):
         """points (n, 3) and trajectories (waypoints (w, 3), offsets (t + 1,), int32) as float64 / int32 arrays, either
-        part may be None; step and radius in metres."""
+        part may be None; step and radius in metres.  signed=True: dsm_field_query_enqueue_signed, on the signed grid."""
         pts = np.ascontiguousarray(np.zeros((0, 3)) if points is None else points, np.float64).reshape(-1, 3)
         wp = np.ascontiguousarray(np.zeros((0, 3)) if waypoints is None else waypoints, np.float64).reshape(-1, 3)
         ofs = np.ascontiguousarray(np.zeros(1) if offsets is None else offsets, np.int32).reshape(-1)
         n_traj = max(len(ofs) - 1, 0)
-        self._ck(self.lib.dsm_field_query_enqueue(self.h, pts.ctypes.data if len(pts) else None, len(pts),
-                                                  wp.ctypes.data if len(wp) else None, ofs.ctypes.data if n_traj else None,
-                                                  n_traj, float(step), float(radius)))
+        fn = self.lib.dsm_field_query_enqueue_signed if signed else self.lib.dsm_field_query_enqueue
+        self._ck(fn(self.h, pts.ctypes.data if len(pts) else None, len(pts), wp.ctypes.data if len(wp) else None,
+                    ofs.ctypes.data if n_traj else None, n_traj, float(step), float(radius)))
         self._query_counts = (len(pts), n_traj)
 
     def field_query_wait(self):

@@ -1508,6 +1508,28 @@ extern "C" int dsm_field_enable(dsm_ctx *ctx, const dsm_field_params *params)
     return keep(ctx->field, f, dsm_field_setup() == 0);
 }
 
+// ---- the signed distance field (include/dsm.h, DESIGN.md §8.16) ----
+extern "C" int dsm_field_signed_enable(dsm_ctx *ctx)
+{
+    if (!ctx) return DSM_E_INVALID;
+    DsmField *f = ctx->field.get();
+    if (!f || f->sgn || f->in_flight) return DSM_E_STATE;
+    CK(cudaSetDevice(ctx->device));
+    auto s = std::make_unique<DsmSignedField>();
+    s->own.device(&s->grid, dsm_field_header(f->voxels) + DSM_SIGNED_WORDS);
+    s->own.host(&s->host, f->voxels);
+    return keep(f->sgn, s);
+}
+
+extern "C" int dsm_field_signed(dsm_ctx *ctx, const float **sdist)
+{
+    if (!ctx) return DSM_E_INVALID;
+    const DsmField *f = ctx->field.get();
+    if (!f || !f->signed_waited) return DSM_E_STATE;
+    if (sdist) *sdist = f->resident ? nullptr : f->sgn->host;
+    return capacity(ctx, f->host + dsm_field_header(f->voxels), DSM_FIELD_ERR_TAG, "dsm_field_signed", "the field");
+}
+
 // The views of a known request (dsm_field_enqueue_known), checked by the caller
 struct KnownViews
 {
@@ -1552,6 +1574,8 @@ static int field_enqueue(dsm_ctx *ctx, const double center[3], int min_update_ti
     }
     CK(cudaMemsetAsync(f->occ, 0, f->voxels, ctx->stream));
     CK(cudaMemsetAsync(header, 0, (known ? DSM_FIELD_VIEW + 1 : 1) * sizeof(int32_t), ctx->stream));
+    int32_t *sgrid = f->sgn ? f->sgn->grid : nullptr; // every request after dsm_field_signed_enable builds the signed grid
+    if (sgrid) CK(cudaMemsetAsync(sgrid + dsm_field_header(f->voxels) + DSM_SIGNED_N_F, 0, sizeof(int32_t), ctx->stream));
     dsm_launch_field_mark(ctx->d.pool, ctx->res_ofs, d.max_pool_per_frame, min_update_times, s ? s->surfels : nullptr, ctx->win_hdr,
                           s ? std::min(s->upper, s->cap) : 0, g, f->occ, header, ctx->stream);
     if (known)
@@ -1560,12 +1584,13 @@ static int field_enqueue(dsm_ctx *ctx, const double center[3], int min_update_ti
         dsm_launch_field_carve(g, vw->rays, ctx->d.S, poses, reinterpret_cast<const int32_t *>(poses + 12 * (size_t)known->n), known->n,
                                vw->max_range, f->occ, ctx->stream);
     }
-    dsm_launch_field_edt(g, f->occ, known != nullptr, f->dist, header, ctx->stream);
+    dsm_launch_field_edt(g, f->occ, known != nullptr, f->dist, header, sgrid, ctx->stream);
     CK(cudaGetLastError());
     if (host_copy)
     {
         CK(cudaMemcpyAsync(f->host, f->dist, f->bytes, cudaMemcpyDeviceToHost, ctx->stream));
         if (known) CK(cudaMemcpyAsync(vw->state, f->occ, f->voxels, cudaMemcpyDeviceToHost, ctx->stream));
+        if (sgrid) CK(cudaMemcpyAsync(f->sgn->host, sgrid, f->voxels * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));
     }
     else
         CK(cudaMemcpyAsync(f->host + dsm_field_header(f->voxels), header, DSM_FIELD_WORDS * sizeof(int32_t), cudaMemcpyDeviceToHost,
@@ -1576,6 +1601,8 @@ static int field_enqueue(dsm_ctx *ctx, const double center[3], int min_update_ti
     f->resident = !host_copy;
     f->known = known != nullptr;
     f->known_waited = false;
+    f->signed_latest = sgrid != nullptr;
+    f->signed_waited = false;
     f->requests++;
     return DSM_OK;
 }
@@ -1597,6 +1624,7 @@ extern "C" int dsm_field_wait(dsm_ctx *ctx, const float **dist, int32_t origin[3
     const int rc = wait_head(ctx, f);
     if (rc != DSM_OK) return rc;
     f->known_waited = f->known;
+    f->signed_waited = f->signed_latest;
     const int32_t *h = f->host + dsm_field_header(f->voxels);
     if (dist) *dist = f->resident ? nullptr : reinterpret_cast<const float *>(f->host);
     if (origin) origin[0] = f->g.o[0], origin[1] = f->g.o[1], origin[2] = f->g.o[2];
@@ -1625,14 +1653,16 @@ extern "C" int dsm_field_query_enable(dsm_ctx *ctx, int max_points, int max_traj
 }
 
 // Stages the request on the calling thread (checking it and counting the samples on the way), then enqueues one H2D
-// copy, the two kernels on the grid of the latest field request, one D2H copy of the results and the event.
-extern "C" int dsm_field_query_enqueue(dsm_ctx *ctx, const double *points, int n_points, const double *waypoints, const int32_t *offsets,
-                                       int n_trajectories, float step, float radius)
+// copy, the two kernels on the grid of the latest field request (sgn: on its signed grid), one D2H copy of the results
+// and the event.
+static int field_query_enqueue(dsm_ctx *ctx, bool sgn, const double *points, int n_points, const double *waypoints, const int32_t *offsets,
+                               int n_trajectories, float step, float radius)
 {
     if (!ctx) return DSM_E_INVALID;
     DsmFieldQuery *q = ctx->field_query.get();
     const DsmField *f = ctx->field.get();
     if (!q || !f || !f->requested || q->in_flight) return DSM_E_STATE;
+    if (sgn && !f->signed_latest) return DSM_E_STATE;
     if (n_points < 0 || n_points > q->max_points || n_trajectories < 0 || n_trajectories > q->max_traj) return DSM_E_INVALID;
     if ((n_points > 0 && !points) || (n_trajectories > 0 && (!waypoints || !offsets))) return DSM_E_INVALID;
     if (!std::isfinite(step) || !(step > 0.f) || !std::isfinite(radius) || !(radius >= 0.f)) return DSM_E_INVALID;
@@ -1688,13 +1718,27 @@ extern "C" int dsm_field_query_enqueue(dsm_ctx *ctx, const double *points, int n
     int32_t *r_hdr = reinterpret_cast<int32_t *>(q->res_dev);
     float4 *r_samples = reinterpret_cast<float4 *>(q->res_dev + 16);
     dsm_clearance_t *r_clear = reinterpret_cast<dsm_clearance_t *>(q->res_dev + DsmFieldQuery::res_clearance(n_points));
-    // a known field's query view holds its site count where a plain field's header holds its occupied count
-    const int32_t *f_hdr = f->dist + dsm_field_header(f->voxels) + (f->known ? DSM_FIELD_VIEW : 0);
-    dsm_launch_field_query(reinterpret_cast<const float *>(f->dist), f_hdr, f->g, d_pts, n_points, d_wp,
-                           d_ofs, d_first, n_trajectories, radius, r_hdr, r_samples, r_clear, ctx->stream);
+    // a known field's query view holds its site count where a plain field's header holds its occupied count; the signed
+    // grid's header holds it in the same word
+    const int32_t *grid = sgn ? f->sgn->grid : f->dist;
+    const int32_t *f_hdr = grid + dsm_field_header(f->voxels) + (!sgn && f->known ? DSM_FIELD_VIEW : 0);
+    dsm_launch_field_query(sgn, reinterpret_cast<const float *>(grid), f_hdr, f->g, d_pts, n_points, d_wp, d_ofs, d_first, n_trajectories,
+                           radius, r_hdr, r_samples, r_clear, ctx->stream);
     CK(cudaGetLastError());
     q->n_points = n_points, q->n_traj = n_trajectories;
     return submit(ctx, *q, q->res_dev, DsmFieldQuery::res_bytes(n_points, n_trajectories), f->requests);
+}
+
+extern "C" int dsm_field_query_enqueue(dsm_ctx *ctx, const double *points, int n_points, const double *waypoints, const int32_t *offsets,
+                                       int n_trajectories, float step, float radius)
+{
+    return field_query_enqueue(ctx, false, points, n_points, waypoints, offsets, n_trajectories, step, radius);
+}
+
+extern "C" int dsm_field_query_enqueue_signed(dsm_ctx *ctx, const double *points, int n_points, const double *waypoints,
+                                              const int32_t *offsets, int n_trajectories, float step, float radius)
+{
+    return field_query_enqueue(ctx, true, points, n_points, waypoints, offsets, n_trajectories, step, radius);
 }
 
 extern "C" int dsm_field_query_wait(dsm_ctx *ctx, const dsm_field_sample_t **samples, const dsm_clearance_t **clearance)
@@ -1802,13 +1846,17 @@ extern "C" int dsm_debug_field_load_state(dsm_ctx *ctx, const uint8_t *state, co
     int32_t *header = f->dist + dsm_field_header(f->voxels);
     CK(cudaMemcpyAsync(f->occ, vw->state, f->voxels, cudaMemcpyHostToDevice, ctx->stream));
     CK(cudaMemsetAsync(header, 0, (DSM_FIELD_VIEW + 1) * sizeof(int32_t), ctx->stream));
-    dsm_launch_field_edt(g, f->occ, true, f->dist, header, ctx->stream);
+    int32_t *sgrid = f->sgn ? f->sgn->grid : nullptr; // every request after dsm_field_signed_enable builds the signed grid
+    if (sgrid) CK(cudaMemsetAsync(sgrid + dsm_field_header(f->voxels) + DSM_SIGNED_N_F, 0, sizeof(int32_t), ctx->stream));
+    dsm_launch_field_edt(g, f->occ, true, f->dist, header, sgrid, ctx->stream);
     CK(cudaGetLastError());
     CK(cudaMemcpyAsync(f->host, f->dist, f->bytes, cudaMemcpyDeviceToHost, ctx->stream));
+    if (sgrid) CK(cudaMemcpyAsync(f->sgn->host, sgrid, f->voxels * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));
     CK(cudaEventRecord(f->ev, ctx->stream));
     f->g = g;
     f->in_flight = f->requested = f->known = true;
-    f->resident = f->known_waited = false;
+    f->resident = f->known_waited = f->signed_waited = false;
+    f->signed_latest = sgrid != nullptr;
     f->requests++;
     return DSM_OK;
 }

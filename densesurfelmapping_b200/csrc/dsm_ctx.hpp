@@ -186,6 +186,14 @@ struct DsmCheckpoint
     }
 };
 
+// dsm_field_signed_enable (DESIGN.md §8.16): the signed grid with its header words (dsm_device.cuh) and its pinned copy
+struct DsmSignedField
+{
+    CudaOwner own;
+    int32_t *grid = nullptr; // device
+    float *host = nullptr;   // pinned [voxels]
+};
+
 // dsm_field_* (DESIGN.md §8.7): the occupancy grid, the distance grid with its header words, the pinned host copy of
 // both and the event after the copy, all allocated by dsm_field_enable
 struct DsmField
@@ -202,6 +210,9 @@ struct DsmField
     bool known = false;     // the latest request is a known one (dsm_field_enqueue_known): its query view is DSM_FIELD_VIEW
     bool known_waited = false; // the last waited request is a known one, and no request has been enqueued since
     uint64_t requests = 0;     // field requests enqueued so far (dsm_reach_enqueue pairs a frontier job with its field)
+    std::unique_ptr<DsmSignedField> sgn; // nullptr until dsm_field_signed_enable: every request from then on builds it
+    bool signed_latest = false;          // the latest request built the signed grid
+    bool signed_waited = false;          // the last waited request built it, and no request has been enqueued since
 };
 
 // dsm_views_* (DESIGN.md §8.9), allocated by dsm_views_enable: the captured rays of max_views slots, which slots hold a

@@ -301,6 +301,19 @@ enum
     DSM_STATE_OCCUPIED = 1,
     DSM_STATE_FREE = 2
 };
+// The signed grid (dsm_field_signed_enable, DESIGN.md §8.16): [nz][ny][nx] like the distance grid, with its own header
+// words at dsm_field_header(voxels), laid out as a query reads a field header, and the count of F after them
+enum
+{
+    DSM_SIGNED_N_SITES,   // the request's sites (its query view's count; k_field_lines_signed copies it)
+    DSM_SIGNED_ERR_TAG,   // the request's error words, copied by k_field_lines_signed
+    DSM_SIGNED_ERR_FRAME,
+    DSM_SIGNED_N_F,       // the voxels that are not sites (zeroed before the request; k_field_rows<KNOWN, true> adds)
+    DSM_SIGNED_WORDS
+};
+static_assert(DSM_SIGNED_N_SITES == DSM_FIELD_N_OCCUPIED && DSM_SIGNED_ERR_TAG == DSM_FIELD_ERR_TAG &&
+                  DSM_SIGNED_ERR_FRAME == DSM_FIELD_ERR_FRAME,
+              "a query reads the signed header as a field header");
 inline size_t dsm_field_header(size_t voxels) { return (voxels + 3) / 4 * 4; }
 // traversable (DESIGN.md §8.11): free, and the stored fp32 distance at least radius
 __device__ __forceinline__ bool dsm_traversable(const uint8_t *state, const int32_t *dist, int i, float radius)
@@ -314,8 +327,9 @@ void dsm_launch_field_mark(const dsm_surfel_t *pool, const int32_t *res, int poo
                            const int32_t *store_size, int store_upper, const DsmFieldGrid &g, uint8_t *occ, int32_t *header, cudaStream_t s);
 // the three EDT passes: occ -> dist (in place from the second pass on); header[DSM_FIELD_N_OCCUPIED] must be zeroed.
 // known: occ holds voxel states, the sites are the voxels that are not free, and header[DSM_FIELD_N_FREE] and
-// header[DSM_FIELD_VIEW] must be zeroed as well
-void dsm_launch_field_edt(const DsmFieldGrid &g, const uint8_t *occ, bool known, int32_t *dist, int32_t *header, cudaStream_t s);
+// header[DSM_FIELD_VIEW] must be zeroed as well.  sdist != nullptr: then the signed grid's three passes into sdist, whose
+// header (at dsm_field_header(voxels)) must have DSM_SIGNED_N_F zeroed
+void dsm_launch_field_edt(const DsmFieldGrid &g, const uint8_t *occ, bool known, int32_t *dist, int32_t *header, int32_t *sdist, cudaStream_t s);
 // dsm_views_capture: the rays of one frame slot's S seeds from its plane rows (plane = d.plane + slot * S * 3)
 void dsm_launch_views_capture(const float4 *plane, int S, float4 *rays, cudaStream_t s);
 // k_field_carve's CTAs per view, and the most views one launch takes: the grid is one-dimensional, n_views * per_view
@@ -339,8 +353,9 @@ enum
     DSM_QUERY_WORDS = 4  // 16 B: the samples stay float4-aligned
 };
 // k_field_query over n_points (CTA 0 also copies the error words; launched with one CTA at least) and
-// k_field_clearance over n_traj trajectories, both on the grid `dist` with its header (at dsm_field_header(voxels))
-void dsm_launch_field_query(const float *dist, const int32_t *field_header, const DsmFieldGrid &g, const double *points, int n_points,
+// k_field_clearance over n_traj trajectories, both on the grid `dist` with its header (at dsm_field_header(voxels)); sgn:
+// the instantiations for a signed grid and its header
+void dsm_launch_field_query(bool sgn, const float *dist, const int32_t *field_header, const DsmFieldGrid &g, const double *points, int n_points,
                             const double *waypoints, const int32_t *offsets, const int32_t *first, int n_traj, float radius,
                             int32_t *result_header, float4 *samples, dsm_clearance_t *clearance, cudaStream_t s);
 

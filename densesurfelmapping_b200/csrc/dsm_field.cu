@@ -10,6 +10,9 @@
 //                     (Meijster's separable pass) and its minimum at every voxel, in place.  One thread per line, the
 //                     lanes of a warp on consecutive x, so every global access is coalesced; the envelope lives in
 //                     shared memory, one packed word (f << 10 | u) per entry.  The z pass writes the fp32 distances.
+// With a signed grid (DESIGN.md §8.16) the same three passes run again, after the first three, over the complement F of
+// the sites: k_field_rows<KNOWN, true>, k_field_lines<false>, and k_field_lines_signed, which writes the signed distance
+// of every site and copies the finished distance of every voxel of F from the first z pass.
 //
 // Squared distances are int32; an empty line holds FIELD_INF.  Every finite value is below 3 * 1023^2 < 2^22, so a site
 // and its value pack into one word and the conversion to float is exact.  The kernels carry no error gate and are
@@ -50,12 +53,14 @@ __global__ void __launch_bounds__(FIELD_MARK_BLOCK) k_field_mark(const dsm_surfe
 // KNOWN (dsm_field_enqueue_known, DESIGN.md §8.9): the grid holds states 0 unknown, 1 occupied, 2 free, the sites are
 // the voxels that are not free, and the warp counts occupied, free and site voxels; CTA 0 copies the error words into
 // the query view (DSM_FIELD_VIEW).  Otherwise every nonzero byte is a site and an occupied voxel.
-template <bool KNOWN>
+// COMPLEMENT (the signed grid, DESIGN.md §8.16): the distance to the nearest voxel of F, the voxels that are not sites,
+// into the signed grid, and the count of F into header[DSM_SIGNED_N_F] of the signed grid's header.
+template <bool KNOWN, bool COMPLEMENT = false>
 __global__ void __launch_bounds__(32 * FIELD_ROW_WARPS) k_field_rows(const DsmFieldGrid g, const uint8_t *occ, int32_t *dist, int32_t *header)
 {
     __shared__ int32_t s_left[FIELD_ROW_WARPS][1024]; // nearest site x at or left of each x, -1 if none
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    if (KNOWN && blockIdx.x == 0 && threadIdx.x == 0)
+    if (KNOWN && !COMPLEMENT && blockIdx.x == 0 && threadIdx.x == 0)
     { // k_field_mark wrote them before this pass
         header[DSM_FIELD_VIEW + DSM_FIELD_ERR_TAG] = header[DSM_FIELD_ERR_TAG];
         header[DSM_FIELD_VIEW + DSM_FIELD_ERR_FRAME] = header[DSM_FIELD_ERR_FRAME];
@@ -69,8 +74,8 @@ __global__ void __launch_bounds__(32 * FIELD_ROW_WARPS) k_field_rows(const DsmFi
     for (int base = 0; base < nx; base += 32)
     {
         const int x = base + lane;
-        const bool hit = x < nx && (KNOWN ? o[x] != DSM_STATE_FREE : o[x] != 0);
-        if (KNOWN)
+        const bool hit = x < nx && ((KNOWN ? o[x] != DSM_STATE_FREE : o[x] != 0) != COMPLEMENT);
+        if (KNOWN && !COMPLEMENT)
         {
             const int st = x < nx ? o[x] : 0;
             count += __popc(__ballot_sync(0xffffffffu, st == DSM_STATE_OCCUPIED));
@@ -85,13 +90,13 @@ __global__ void __launch_bounds__(32 * FIELD_ROW_WARPS) k_field_rows(const DsmFi
         v = max(v, carry);
         if (x < nx) left[x] = v;
         carry = __shfl_sync(0xffffffffu, v, 31);
-        if (!KNOWN) count += __popc(__ballot_sync(0xffffffffu, hit));
+        if (!KNOWN || COMPLEMENT) count += __popc(__ballot_sync(0xffffffffu, hit));
     }
     carry = INT_MAX;
     for (int base = (nx - 1) & ~31; base >= 0; base -= 32)
     {
         const int x = base + lane;
-        const bool hit = x < nx && (KNOWN ? o[x] != DSM_STATE_FREE : o[x] != 0);
+        const bool hit = x < nx && ((KNOWN ? o[x] != DSM_STATE_FREE : o[x] != 0) != COMPLEMENT);
         int v = hit ? x : INT_MAX;
         for (int k = 1; k < 32; k <<= 1)
         {
@@ -107,8 +112,8 @@ __global__ void __launch_bounds__(32 * FIELD_ROW_WARPS) k_field_rows(const DsmFi
             out[x] = d == INT_MAX ? FIELD_INF : d * d;
         }
     }
-    if (lane == 0 && count > 0) atomicAdd(&header[DSM_FIELD_N_OCCUPIED], count);
-    if (KNOWN && lane == 0)
+    if (lane == 0 && count > 0) atomicAdd(&header[COMPLEMENT ? DSM_SIGNED_N_F : DSM_FIELD_N_OCCUPIED], count);
+    if (KNOWN && !COMPLEMENT && lane == 0)
     {
         if (n_free > 0) atomicAdd(&header[DSM_FIELD_N_FREE], n_free);
         if (n_free < nx) atomicAdd(&header[DSM_FIELD_VIEW + DSM_FIELD_N_OCCUPIED], nx - n_free);
@@ -130,10 +135,20 @@ __device__ __forceinline__ int env_sep(uint32_t e, int u, int fu)
     return (num % den != 0 && num < 0) ? q - 1 : q;
 }
 
+// What an envelope pass writes at each voxel of its line: the squared distance d2, the distance sqrtf((float)d2) * voxel
+// (+inf for an empty line), or the signed distance (include/dsm.h): for a site (d2 > 0, the squared distance to F) the
+// negative depth (1 - sqrtf((float)d2)) * voxel, for a voxel of F (d2 == 0) the finished distance at the same index of
+// `pos`, and -inf for an empty line (F is empty)
+enum
+{
+    LINES_SQUARED,
+    LINES_DIST,
+    LINES_SIGNED,
+};
+
 // One line of `len` voxels at stride `step` per thread; line (x, blockIdx.y) starts at dist + blockIdx.y * outer + x.
-// LAST: the minimum becomes sqrtf((float)d2) * voxel (+inf for an empty line) in place of the squared distance.
-template <bool LAST>
-__global__ void __launch_bounds__(32) k_field_lines(int32_t *dist, int nx, int len, int step, int outer, float voxel)
+template <int OUT>
+__device__ __forceinline__ void field_lines(int32_t *dist, const int32_t *pos, int nx, int len, int step, int outer, float voxel)
 {
     extern __shared__ uint32_t s_env[]; // [len][32]: entry k of lane l at k * 32 + l (conflict-free)
     const int x = blockIdx.x * 32 + threadIdx.x;
@@ -177,7 +192,8 @@ __global__ void __launch_bounds__(32) k_field_lines(int32_t *dist, int nx, int l
     }
     if (top < 0)
     {
-        for (int u = 0; u < len; u++) line[(size_t)u * step] = LAST ? __float_as_int(INFINITY) : FIELD_INF;
+        const int32_t none = OUT == LINES_SIGNED ? __float_as_int(-INFINITY) : (OUT == LINES_DIST ? __float_as_int(INFINITY) : FIELD_INF);
+        for (int u = 0; u < len; u++) line[(size_t)u * step] = none;
         return;
     }
     // the lowest entry at x only moves right as x grows: advance while the next one is at least as low
@@ -195,8 +211,38 @@ __global__ void __launch_bounds__(32) k_field_lines(int32_t *dist, int nx, int l
             cur = nxt;
             d = dn;
         }
-        line[(size_t)u * step] = LAST ? __float_as_int(sqrtf((float)d) * voxel) : d;
+        if (OUT == LINES_SQUARED)
+            line[(size_t)u * step] = d;
+        else if (OUT == LINES_DIST)
+            line[(size_t)u * step] = __float_as_int(sqrtf((float)d) * voxel);
+        else
+        {
+            const size_t i = (size_t)blockIdx.y * outer + x + (size_t)u * step;
+            line[(size_t)u * step] = d == 0 ? pos[i] : __float_as_int(__fmul_rn(__fsub_rn(1.f, sqrtf((float)d)), voxel));
+        }
     }
+}
+
+// LAST: the minimum becomes sqrtf((float)d2) * voxel (+inf for an empty line) in place of the squared distance.
+template <bool LAST>
+__global__ void __launch_bounds__(32) k_field_lines(int32_t *dist, int nx, int len, int step, int outer, float voxel)
+{
+    field_lines<LAST ? LINES_DIST : LINES_SQUARED>(dist, nullptr, nx, len, step, outer, voxel);
+}
+
+// The signed grid's last pass, along z: sdist holds the squared distances to F of the y pass, dist the finished distance
+// grid of the same request (its z pass has completed: both run in order on one stream), and one thread copies the site
+// count and the error words of the request's query view `hdr` into the signed grid's header `shdr`.
+__global__ void __launch_bounds__(32) k_field_lines_signed(int32_t *sdist, const int32_t *__restrict__ dist, const int32_t *__restrict__ hdr,
+                                                           int32_t *shdr, int nx, int len, int step, int outer, float voxel)
+{
+    if (blockIdx.x == 0 && blockIdx.y == 0 && threadIdx.x == 0)
+    {
+        shdr[DSM_SIGNED_N_SITES] = hdr[DSM_FIELD_N_OCCUPIED];
+        shdr[DSM_SIGNED_ERR_TAG] = hdr[DSM_FIELD_ERR_TAG];
+        shdr[DSM_SIGNED_ERR_FRAME] = hdr[DSM_FIELD_ERR_FRAME];
+    }
+    field_lines<LINES_SIGNED>(sdist, dist, nx, len, step, outer, voxel);
 }
 
 // ---- planner queries against the latest field (dsm_field_query_*, DESIGN.md §8.8) ----
@@ -207,6 +253,8 @@ __global__ void __launch_bounds__(32) k_field_lines(int32_t *dist, int nx, int l
 //                      minimum (ties to the lower index), the lowest hit and the outside count: the result is the same
 //                      whatever the schedule.
 // Every fp32 step is an explicit _rn intrinsic, so the numpy restatement (oracle/pyoracle_field_query.py) is bit-exact.
+// SIGNED (DESIGN.md §8.16): the same on the signed grid, whose header gives two rules in place of the "no site" one: no
+// site, +inf; no voxel of F, -inf (an interpolation of infinities of one sign would be NaN).
 #define FIELD_QUERY_BLOCK 256
 #define FIELD_CLEAR_WARPS 8
 
@@ -223,17 +271,18 @@ __device__ __forceinline__ bool q_axis(double p, double v, int o, int n, int &i,
     return true;
 }
 
-// the point query at p: dist (and, with GRAD, the gradient) per include/dsm.h; inside = the point is inside the grid
+// the point query at p: dist (and, with GRAD, the gradient) per include/dsm.h; inside = the point is inside the grid;
+// empty: every inside point gets dist = fill and a zero gradient
 template <bool GRAD>
-__device__ __forceinline__ float4 q_sample(const float *__restrict__ dist, const DsmFieldGrid &g, bool empty, double px, double py, double pz,
-                                           bool &inside)
+__device__ __forceinline__ float4 q_sample(const float *__restrict__ dist, const DsmFieldGrid &g, bool empty, float fill, double px, double py,
+                                           double pz, bool &inside)
 {
     const double v = (double)g.voxel;
     int ix, jx, iy, jy, iz, jz;
     float tx, ty, tz;
     inside = q_axis(px, v, g.o[0], g.n[0], ix, jx, tx) && q_axis(py, v, g.o[1], g.n[1], iy, jy, ty) && q_axis(pz, v, g.o[2], g.n[2], iz, jz, tz);
     if (!inside) return make_float4(__int_as_float(0x7fc00000), 0.f, 0.f, 0.f);
-    if (empty) return make_float4(INFINITY, 0.f, 0.f, 0.f);
+    if (empty) return make_float4(fill, 0.f, 0.f, 0.f);
     const size_t nx = (size_t)g.n[0], ny = (size_t)g.n[1];
     const size_t r00 = (iz * ny + iy) * nx, r10 = (iz * ny + jy) * nx, r01 = (jz * ny + iy) * nx, r11 = (jz * ny + jy) * nx;
     const float c000 = __ldg(dist + r00 + ix), c100 = __ldg(dist + r00 + jx), c010 = __ldg(dist + r10 + ix), c110 = __ldg(dist + r10 + jx);
@@ -251,6 +300,17 @@ __device__ __forceinline__ float4 q_sample(const float *__restrict__ dist, const
     return r;
 }
 
+// the rules of a field without a site (+inf) and, SIGNED, of one without a voxel of F (-inf): whether one applies, and
+// the distance it gives
+template <bool SIGNED>
+__device__ __forceinline__ bool q_empty(const int32_t *__restrict__ fhdr, float &fill)
+{
+    const bool no_site = fhdr[DSM_FIELD_N_OCCUPIED] == 0;
+    fill = SIGNED && !no_site ? -INFINITY : INFINITY;
+    return no_site || (SIGNED && fhdr[DSM_SIGNED_N_F] == 0);
+}
+
+template <bool SIGNED>
 __global__ void __launch_bounds__(FIELD_QUERY_BLOCK) k_field_query(const float *__restrict__ dist, const int32_t *__restrict__ fhdr, const DsmFieldGrid g,
                                                                    const double *__restrict__ pts, int n, float4 *__restrict__ out, int32_t *rhdr)
 {
@@ -263,9 +323,12 @@ __global__ void __launch_bounds__(FIELD_QUERY_BLOCK) k_field_query(const float *
     if (i >= n) return;
     const double *p = pts + 3 * (size_t)i;
     bool inside;
-    out[i] = q_sample<true>(dist, g, fhdr[DSM_FIELD_N_OCCUPIED] == 0, p[0], p[1], p[2], inside);
+    float fill;
+    const bool empty = q_empty<SIGNED>(fhdr, fill);
+    out[i] = q_sample<true>(dist, g, empty, fill, p[0], p[1], p[2], inside);
 }
 
+template <bool SIGNED>
 __global__ void __launch_bounds__(32 * FIELD_CLEAR_WARPS) k_field_clearance(const float *__restrict__ dist, const int32_t *__restrict__ fhdr,
                                                                             const DsmFieldGrid g, const double *__restrict__ wp,
                                                                             const int32_t *__restrict__ offsets, const int32_t *__restrict__ first,
@@ -273,7 +336,8 @@ __global__ void __launch_bounds__(32 * FIELD_CLEAR_WARPS) k_field_clearance(cons
 {
     const int lane = threadIdx.x & 31, traj = blockIdx.x * FIELD_CLEAR_WARPS + (threadIdx.x >> 5);
     if (traj >= n_traj) return; // whole warps only
-    const bool empty = fhdr[DSM_FIELD_N_OCCUPIED] == 0;
+    float fill;
+    const bool empty = q_empty<SIGNED>(fhdr, fill);
     const int last = offsets[traj + 1] - 1, total = first[last] + 1;
     float best = INFINITY;
     int arg = INT_MAX, hit = INT_MAX, outside = 0; // INT_MAX: none yet
@@ -292,7 +356,7 @@ __global__ void __launch_bounds__(32 * FIELD_CLEAR_WARPS) k_field_clearance(cons
             pz = __dadd_rn(pz, __dmul_rn(f, __dsub_rn(b[2], a[2])));
         }
         bool inside;
-        const float d = q_sample<false>(dist, g, empty, px, py, pz, inside).x;
+        const float d = q_sample<false>(dist, g, empty, fill, px, py, pz, inside).x;
         if (!inside)
         {
             outside++;
@@ -320,15 +384,24 @@ __global__ void __launch_bounds__(32 * FIELD_CLEAR_WARPS) k_field_clearance(cons
     }
 }
 
-void dsm_launch_field_query(const float *dist, const int32_t *field_header, const DsmFieldGrid &g, const double *points, int n_points,
-                            const double *waypoints, const int32_t *offsets, const int32_t *first, int n_traj, float radius,
-                            int32_t *result_header, float4 *samples, dsm_clearance_t *clearance, cudaStream_t s)
+template <bool SIGNED>
+static void launch_field_query(const float *dist, const int32_t *field_header, const DsmFieldGrid &g, const double *points, int n_points,
+                               const double *waypoints, const int32_t *offsets, const int32_t *first, int n_traj, float radius,
+                               int32_t *result_header, float4 *samples, dsm_clearance_t *clearance, cudaStream_t s)
 {
     const int qb = (n_points + FIELD_QUERY_BLOCK - 1) / FIELD_QUERY_BLOCK;
-    k_field_query<<<qb > 1 ? qb : 1, FIELD_QUERY_BLOCK, 0, s>>>(dist, field_header, g, points, n_points, samples, result_header);
+    k_field_query<SIGNED><<<qb > 1 ? qb : 1, FIELD_QUERY_BLOCK, 0, s>>>(dist, field_header, g, points, n_points, samples, result_header);
     if (n_traj > 0)
-        k_field_clearance<<<(n_traj + FIELD_CLEAR_WARPS - 1) / FIELD_CLEAR_WARPS, 32 * FIELD_CLEAR_WARPS, 0, s>>>(
+        k_field_clearance<SIGNED><<<(n_traj + FIELD_CLEAR_WARPS - 1) / FIELD_CLEAR_WARPS, 32 * FIELD_CLEAR_WARPS, 0, s>>>(
             dist, field_header, g, waypoints, offsets, first, n_traj, radius, clearance);
+}
+
+void dsm_launch_field_query(bool sgn, const float *dist, const int32_t *field_header, const DsmFieldGrid &g, const double *points,
+                            int n_points, const double *waypoints, const int32_t *offsets, const int32_t *first, int n_traj, float radius,
+                            int32_t *result_header, float4 *samples, dsm_clearance_t *clearance, cudaStream_t s)
+{
+    (sgn ? launch_field_query<true> : launch_field_query<false>)(dist, field_header, g, points, n_points, waypoints, offsets, first, n_traj,
+                                                                 radius, result_header, samples, clearance, s);
 }
 
 int dsm_field_setup()
@@ -336,6 +409,7 @@ int dsm_field_setup()
     const int smem = 1024 * 32 * 4; // the longest line
     cudaError_t e = cudaFuncSetAttribute(k_field_lines<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     if (e == cudaSuccess) e = cudaFuncSetAttribute(k_field_lines<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(k_field_lines_signed, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     return e == cudaSuccess ? 0 : -1;
 }
 
@@ -348,7 +422,7 @@ void dsm_launch_field_mark(const dsm_surfel_t *pool, const int32_t *res, int poo
     k_field_mark<<<pool_grid + store_grid, FIELD_MARK_BLOCK, 0, s>>>(pool, res, pool_grid, min_update_times, store, store_size, g, occ, header);
 }
 
-void dsm_launch_field_edt(const DsmFieldGrid &g, const uint8_t *occ, bool known, int32_t *dist, int32_t *header, cudaStream_t s)
+void dsm_launch_field_edt(const DsmFieldGrid &g, const uint8_t *occ, bool known, int32_t *dist, int32_t *header, int32_t *sdist, cudaStream_t s)
 {
     const int nx = g.n[0], ny = g.n[1], nz = g.n[2];
     const int rows = ny * nz;
@@ -361,6 +435,16 @@ void dsm_launch_field_edt(const DsmFieldGrid &g, const uint8_t *occ, bool known,
     // along y: lines (x, z) at stride nx; along z: lines (x, y) at stride nx * ny
     k_field_lines<false><<<dim3(xb, nz), 32, (size_t)ny * 32 * 4, s>>>(dist, nx, ny, nx, nx * ny, g.voxel);
     k_field_lines<true><<<dim3(xb, ny), 32, (size_t)nz * 32 * 4, s>>>(dist, nx, nz, nx * ny, nx, g.voxel);
+    if (!sdist) return;
+    // the signed grid: the same passes over the complement; its last pass reads the finished grid above
+    int32_t *sheader = sdist + dsm_field_header((size_t)nx * ny * nz);
+    if (known)
+        k_field_rows<true, true><<<rb, 32 * FIELD_ROW_WARPS, 0, s>>>(g, occ, sdist, sheader);
+    else
+        k_field_rows<false, true><<<rb, 32 * FIELD_ROW_WARPS, 0, s>>>(g, occ, sdist, sheader);
+    k_field_lines<false><<<dim3(xb, nz), 32, (size_t)ny * 32 * 4, s>>>(sdist, nx, ny, nx, nx * ny, g.voxel);
+    k_field_lines_signed<<<dim3(xb, ny), 32, (size_t)nz * 32 * 4, s>>>(sdist, dist, header + (known ? DSM_FIELD_VIEW : 0), sheader, nx, nz,
+                                                                       nx * ny, nx, g.voxel);
 }
 
 // ---- known space (dsm_views_*, dsm_field_enqueue_known, DESIGN.md §8.9) ----

@@ -659,6 +659,41 @@ int dsm_frontier_enqueue(dsm_ctx *ctx, int min_voxels);
 int dsm_frontier_wait(dsm_ctx *ctx, const dsm_frontier_cluster_t **clusters, const int32_t **voxels, dsm_frontier_counts_t *counts);
 int dsm_debug_field_load_state(dsm_ctx *ctx, const uint8_t *state, const int32_t origin[3]);
 
+/* ---- the signed distance field: how deep a point lies inside the sites, and a gradient out of them (DESIGN.md §8.16) ----
+ * The distance grid is 0 on every site, so a point among sites has dist = 0 and a zero gradient: an optimiser whose path
+ * crosses an obstacle or unknown space has no direction to move in.  The signed grid of a request measures that depth.
+ *
+ * Definition.  S is the request's sites, those its dist measures to: the occupied voxels of a plain (or resident)
+ * request, the voxels of state 0 or 1 of a known one (dsm_field_enqueue_known, dsm_debug_field_load_state).  F is every
+ * other voxel.  A voxel of F has sdist = dist, bit for bit.  A voxel of S has sdist = (1 - sqrtf((float)e2)) * v in fp32,
+ * one rounding per operation, e2 the smallest squared integer distance to a voxel of F (e2 <= 3 * 1023^2, so (float)e2
+ * is exact): a site with a face neighbour in F reads 0, as dist does, and the value falls by one voxel edge per voxel of
+ * depth, so the slope across the boundary is 1 on both sides.  F empty: -INFINITY everywhere; S empty: +INFINITY
+ * everywhere (dist's rule).  So sdist <= dist everywhere, equal off S and on sites with e2 = 1, and sdist < 0 exactly on
+ * sites with e2 >= 2.
+ *
+ * Signed queries.  dsm_field_query_enqueue_signed samples the signed grid with dsm_field_query_enqueue's addressing,
+ * interpolation, gradient and clearance, with two rules in place of its "no site" rule: no site gives every inside
+ * point +INFINITY and a zero gradient; no voxel of F gives -INFINITY and a zero gradient.  min_dist may be negative (the
+ * penetration depth of the path's deepest sample); first_hit is the first inside sample with dist < radius.
+ *
+ *   dsm_field_signed_enable        once, after dsm_field_enable (DSM_E_STATE before it, when called twice, and while a
+ *                                  field is in flight).  Allocates the signed grid (4 B per voxel and 16 B of header) on
+ *                                  the device and a pinned host copy of it.  DSM_E_NOMEM with nothing kept.  Every field
+ *                                  request enqueued after it, of any kind, also builds the signed grid, in stream order
+ *                                  after its distance grid; a request with a host copy also copies the signed grid.
+ *   dsm_field_signed               the signed grid [z][y][x] of the last waited request (the context's pinned buffer,
+ *                                  valid until the next field enqueue; NULL for a resident request); sdist may be NULL.
+ *                                  DSM_E_STATE when that request has no signed grid, or a request has been enqueued since.
+ *                                  DSM_E_CAPACITY as dsm_field_wait, with the grid of the last applied frame.
+ *   dsm_field_query_enqueue_signed dsm_field_query_enqueue (same arguments, checks, staging and ordering; waited for
+ *                                  with dsm_field_query_wait) on the signed grid of the latest field request.  DSM_E_STATE
+ *                                  also when that request was enqueued without a signed grid. */
+int dsm_field_signed_enable(dsm_ctx *ctx);
+int dsm_field_signed(dsm_ctx *ctx, const float **sdist);
+int dsm_field_query_enqueue_signed(dsm_ctx *ctx, const double *points, int n_points, const double *waypoints, const int32_t *offsets,
+                                   int n_trajectories, float step, float radius);
+
 /* ---- paths through known free space: travel cost from a start to every voxel, goals and frontiers (DESIGN.md §8.11) ----
  * A reach job reads the state grid and the distance grid of the latest field request, which must be a known one, in
  * stream order behind it, with that request's origin o and voxel edge v captured at the job's enqueue, and (with

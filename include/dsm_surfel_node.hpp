@@ -68,6 +68,10 @@
 // needs instead (DESIGN.md §8.8): after enable_field_queries(), field_samples() (distance and gradient at points) and
 // trajectory_clearance() (the clearance of candidate paths) read the field of the latest fused frame, one enqueue and
 // one wait each, without touching the one-frame-late distance_field() handout.
+// enable_signed_distance(), after enable_distance_field, makes every field also build the signed grid (DESIGN.md §8.16):
+// negative inside obstacles (and, with known space, inside unknown space), so that a gradient points out of them.
+// signed_distance_field() hands out the signed grid of the field distance_field() handed out last, and field_samples()
+// and trajectory_clearance() read it with signed_field = true.
 // The field counts every voxel without an obstacle point as free, seen or not.  enable_known_space(max_views, max_range),
 // after enable_distance_field, makes it measure the distance to anything not known to be free (DESIGN.md §8.9): the
 // first fused frame of each new reference keyframe is captured into slot captures % max_views (its superpixel rays, in
@@ -499,6 +503,21 @@ class SurfelMapNode
             distance_field_ = true, field_host_copy_ = host_copy;
         return ctx_.err;
     }
+    // ---- the signed distance field (DESIGN.md §8.16) ----
+    // once, after enable_distance_field: every field from then on also builds the signed grid (negative depth inside
+    // obstacles, and inside unknown space with known space)
+    int enable_signed_distance()
+    {
+        return ctx_.run("enable_signed_distance", [&] { return dsm_field_signed_enable(ctx_.ctx); });
+    }
+    // the signed grid [nz][ny][nx] in metres of the field distance_field() handed out last (the library's pinned buffer,
+    // valid until the next frame is fused; nullptr for a field kept on the device).  DSM_E_STATE without
+    // enable_signed_distance() before that field, or before distance_field() has handed out a field.
+    int signed_distance_field(const float *&sdist)
+    {
+        if (!ctx_.ready("signed_distance_field")) return ctx_.err;
+        return ctx_.done(dsm_field_signed(ctx_.ctx, &sdist), "signed_distance_field");
+    }
     // ---- free versus unknown space (see the top of this file, DESIGN.md §8.9) ----
     // once, after enable_distance_field: max_views capture slots, rays cut to max_range metres
     int enable_known_space(int max_views, float max_range)
@@ -712,18 +731,20 @@ class SurfelMapNode
         return ctx_.run("enable_field_queries", [&] { return dsm_field_query_enable(ctx_.ctx, max_points, max_trajectories, max_waypoints); });
     }
     // distance and gradient at n points (xyz doubles); out receives n samples.  DSM_E_STATE when no field exists;
-    // DSM_E_CAPACITY with the samples of the last applied frame's field, as distance_field().
-    int field_samples(const double *points, int n, std::vector<dsm_field_sample_t> &out)
+    // DSM_E_CAPACITY with the samples of the last applied frame's field, as distance_field().  signed_field: on the
+    // signed grid (dsm_field_query_enqueue_signed); DSM_E_STATE also when that field was requested without it.
+    int field_samples(const double *points, int n, std::vector<dsm_field_sample_t> &out, bool signed_field = false)
     {
         out.clear();
-        return query("field_samples", points, n, nullptr, nullptr, 0, 1.f, 0.f, &out, nullptr);
+        return query("field_samples", signed_field, points, n, nullptr, nullptr, 0, 1.f, 0.f, &out, nullptr);
     }
     // the clearance of n trajectories (waypoints xyz doubles, offsets[n + 1]) sampled every `step` metres against
-    // `radius`; out receives n records (include/dsm.h)
-    int trajectory_clearance(const double *waypoints, const int32_t *offsets, int n, float step, float radius, std::vector<dsm_clearance_t> &out)
+    // `radius`; out receives n records (include/dsm.h); signed_field as field_samples()
+    int trajectory_clearance(const double *waypoints, const int32_t *offsets, int n, float step, float radius, std::vector<dsm_clearance_t> &out,
+                             bool signed_field = false)
     {
         out.clear();
-        return query("trajectory_clearance", nullptr, 0, waypoints, offsets, n, step, radius, nullptr, &out);
+        return query("trajectory_clearance", signed_field, nullptr, 0, waypoints, offsets, n, step, radius, nullptr, &out);
     }
     // the field of the latest fused frame: dist [nz][ny][nx] in metres (the library's pinned buffer, valid until the next
     // frame is fused; nullptr for a field kept on the device), the grid's origin in voxels and the occupied voxels.  DSM_E_STATE when no frame has been fused
@@ -880,13 +901,16 @@ class SurfelMapNode
         cam.unknown_blocks = unknown_blocks;
         return cam;
     }
-    int query(const char *what, const double *points, int n_points, const double *waypoints, const int32_t *offsets, int n_traj, float step,
-              float radius, std::vector<dsm_field_sample_t> *samples, std::vector<dsm_clearance_t> *clearance)
+    int query(const char *what, bool signed_field, const double *points, int n_points, const double *waypoints, const int32_t *offsets,
+              int n_traj, float step, float radius, std::vector<dsm_field_sample_t> *samples, std::vector<dsm_clearance_t> *clearance)
     {
         const dsm_field_sample_t *s = nullptr;
         const dsm_clearance_t *c = nullptr;
         return job(what, ANY_FIELD, true,
-                   [&] { return dsm_field_query_enqueue(ctx_.ctx, points, n_points, waypoints, offsets, n_traj, step, radius); },
+                   [&] {
+                       return (signed_field ? dsm_field_query_enqueue_signed : dsm_field_query_enqueue)(ctx_.ctx, points, n_points, waypoints,
+                                                                                                         offsets, n_traj, step, radius);
+                   },
                    [&] { return dsm_field_query_wait(ctx_.ctx, &s, &c); },
                    [&] {
                        if (samples) samples->assign(s, s + n_points);
