@@ -41,6 +41,7 @@ EXPORTS = [
     "dsm_reach_enable", "dsm_reach_enqueue", "dsm_reach_wait", "dsm_reach_matrix_enable", "dsm_reach_matrix_enqueue",
     "dsm_reach_matrix_wait", "dsm_gain_enable", "dsm_gain_enqueue", "dsm_gain_wait",
     "dsm_tour_enable", "dsm_tour_enqueue", "dsm_tour_wait", "dsm_viewpoint_enable", "dsm_viewpoint_enqueue", "dsm_viewpoint_wait",
+    "dsm_trajectory_enable", "dsm_trajectory_enqueue", "dsm_trajectory_wait",
     "dsm_inactive_segments", "dsm_inactive_load", "dsm_map_save", "dsm_map_load", "dsm_map_peek",
     "dsm_checkpoint_enable", "dsm_checkpoint_enqueue", "dsm_checkpoint_wait", "dsm_debug_checkpoint_drain_ctas",
     "dsm_checkpoint_enqueue_incremental", "dsm_map_load_journal", "dsm_map_peek_journal", "dsm_journal_materialize",
@@ -102,6 +103,14 @@ VIEWPOINT_INFO_DTYPE = np.dtype([("origin", "<i4", 3), ("n_clusters", "<i4"), ("
                                  ("top_k", "<i4"), ("unknown_blocks", "<i4"), ("with_reach", "<i4"), ("n_clusters_table", "<i4"),
                                  ("reserved", "<i4", 6)])
 
+# dsm_trajectory_wait's records (include/dsm.h): a trajectory (96 B) and the header (64 B)
+TRAJECTORY_DTYPE = np.dtype([("status", "<i4"), ("iterations", "<i4"), ("evaluations", "<i4"), ("n_free_outside", "<i4"),
+                             ("cost_start", "<f8"), ("cost", "<f8"), ("smoothness", "<f8"), ("clearance", "<f8"),
+                             ("feasibility", "<f8"), ("max_v", "<f8"), ("max_a", "<f8"), ("min_dist", "<f4"), ("argmin", "<i4"),
+                             ("first_hit", "<i4"), ("n_outside", "<i4"), ("reserved", "<i4", 2)])
+TRAJECTORY_INFO_DTYPE = np.dtype([("origin", "<i4", 3), ("n_trajectories", "<i4"), ("n_points", "<i4"), ("n_status", "<i4", 4),
+                                  ("reserved", "<i4", 7)])
+
 
 class DsmGainCamera(ctypes.Structure):
     """dsm_gain_camera_t (48 B): pinhole intrinsics, image size, range and the blocking rule of a gain job."""
@@ -114,6 +123,15 @@ class DsmViewpointParams(ctypes.Structure):
     _fields_ = [("r_min", ctypes.c_int32), ("r_max", ctypes.c_int32), ("dz_max", ctypes.c_int32), ("stride", ctypes.c_int32),
                 ("max_samples", ctypes.c_int32), ("min_seen", ctypes.c_int32), ("top_k", ctypes.c_int32), ("with_reach", ctypes.c_int32),
                 ("radius", ctypes.c_float), ("reserved", ctypes.c_int32)]
+
+
+class DsmTrajectoryParams(ctypes.Structure):
+    """dsm_trajectory_params_t (88 B): the weights, limits and stopping rules of a trajectory job, shared by its
+    trajectories."""
+    _fields_ = [("w_smooth", ctypes.c_double), ("w_clear", ctypes.c_double), ("w_feas", ctypes.c_double),
+                ("margin", ctypes.c_double), ("v_max", ctypes.c_double), ("a_max", ctypes.c_double), ("g_tol", ctypes.c_double),
+                ("max_iter", ctypes.c_int32), ("memory", ctypes.c_int32), ("max_ls", ctypes.c_int32), ("samples", ctypes.c_int32),
+                ("radius", ctypes.c_float), ("reserved", ctypes.c_int32 * 3)]
 
 
 CONSTANTS_DRIVE = (0.4, 0.5, 4.0, 0.1)    # fusion_functions.h:13-16
@@ -201,6 +219,9 @@ def load_library():
     L.dsm_viewpoint_enable.argtypes = [vp, ci, ci]
     L.dsm_viewpoint_enqueue.argtypes = [vp, ctypes.POINTER(DsmGainCamera), vp, ci, vp, ci, ctypes.POINTER(DsmViewpointParams)]
     L.dsm_viewpoint_wait.argtypes = [vp, vp, ctypes.POINTER(vp), ctypes.POINTER(vp)]
+    L.dsm_trajectory_enable.argtypes = [vp, ci, ci, ci]
+    L.dsm_trajectory_enqueue.argtypes = [vp, vp, vp, vp, ci, ctypes.POINTER(DsmTrajectoryParams)]
+    L.dsm_trajectory_wait.argtypes = [vp, vp, ctypes.POINTER(vp), ctypes.POINTER(vp)]
     L.dsm_inactive_reserve.argtypes = [vp, ci]
     L.dsm_inactive_retire.argtypes = [vp, ci, ctypes.POINTER(ci)]
     L.dsm_inactive_reactivate.argtypes = [vp, ci, ctypes.POINTER(ci)]
@@ -862,6 +883,36 @@ class Context:
         self._ck(self.lib.dsm_tour_wait(self.h, info.ctypes.data, ctypes.byref(ps), ctypes.byref(po)))
         i = info[0]
         return i, _take(ps, int(i["n_starts"]), TOUR_START_DTYPE), _take(po, int(i["n_sites"]), np.int32)
+
+    # ---- trajectory optimisation on the signed grid of the latest field ----
+    def trajectory_enable(self, max_trajectories, max_points, max_memory):
+        self._ck(self.lib.dsm_trajectory_enable(self.h, int(max_trajectories), int(max_points), int(max_memory)))
+
+    def trajectory_enqueue(self, points, offsets, dt, params):
+        """points (P, 3) float64 control points, offsets (n + 1,) int32, dt (n,) knot intervals; params a dict with the
+        fields of DsmTrajectoryParams (reserved aside), such as oracle/pyoracle_trajectory.params() returns."""
+        pts = np.ascontiguousarray(points, np.float64).reshape(-1, 3)
+        ofs = np.ascontiguousarray(offsets, np.int32).reshape(-1)
+        dts = np.ascontiguousarray(dt, np.float64).reshape(-1)
+        if len(ofs) < 2 or len(dts) != len(ofs) - 1:
+            raise ValueError(f"{len(dts)} knot intervals for {max(len(ofs) - 1, 0)} trajectories")
+        if not 0 <= ofs[-1] <= len(pts):
+            raise ValueError(f"offsets end at {ofs[-1]}, beyond the {len(pts)} points")
+        p = DsmTrajectoryParams(**{k: params[k] for k, _ in DsmTrajectoryParams._fields_ if k != "reserved"})
+        self._ck(self.lib.dsm_trajectory_enqueue(self.h, pts.ctypes.data if len(pts) else None, ofs.ctypes.data if len(ofs) else None,
+                                                 dts.ctypes.data if len(dts) else None, max(len(ofs) - 1, 0), ctypes.byref(p)))
+
+    def trajectory_wait(self):
+        """(info, records, points): numpy copies of the context's pinned results, a TRAJECTORY_INFO_DTYPE record,
+        TRAJECTORY_DTYPE (n_trajectories,) and the optimised control points (n_points, 3).  A job on a field taken after a
+        rejected frame raises DsmError(DSM_E_CAPACITY) carrying the same tuple as `.trajectory`."""
+        pr, pp = ctypes.c_void_p(), ctypes.c_void_p()
+        info = np.zeros(1, TRAJECTORY_INFO_DTYPE)
+        rc = self.lib.dsm_trajectory_wait(self.h, info.ctypes.data, ctypes.byref(pr), ctypes.byref(pp))
+        i = info[0]
+        n, n_pts = int(i["n_trajectories"]), int(i["n_points"])
+        return self._waited(rc, "trajectory",
+                            lambda: (i, _take(pr, n, TRAJECTORY_DTYPE), _take(pp, 3 * n_pts, np.float64).reshape(n_pts, 3)))
 
     # ---- planner queries against the latest field ----
     def field_query_enable(self, max_points, max_trajectories, max_waypoints):

@@ -2382,6 +2382,96 @@ extern "C" int dsm_tour_wait(dsm_ctx *ctx, dsm_tour_info_t *info, const dsm_tour
     return DSM_OK;
 }
 
+// ---- trajectory optimisation on the signed grid (include/dsm.h, DESIGN.md §8.17) ----
+extern "C" int dsm_trajectory_enable(dsm_ctx *ctx, int max_trajectories, int max_points, int max_memory)
+{
+    if (!ctx) return DSM_E_INVALID;
+    const DsmField *f = ctx->field.get();
+    if (!f || !f->sgn || ctx->trajectory) return DSM_E_STATE;
+    if (max_trajectories < 1 || max_trajectories > DSM_TRAJECTORY_MAX_CAPACITY || max_points < 1 || max_points > DSM_TRAJECTORY_MAX_CAPACITY ||
+        max_memory < 1 || max_memory > DSM_TRAJECTORY_MAX_MEMORY)
+        return DSM_E_INVALID;
+    CK(cudaSetDevice(ctx->device));
+    auto tr = std::make_unique<DsmTrajectory>();
+    tr->max_traj = max_trajectories, tr->max_points = max_points, tr->max_memory = max_memory;
+    const size_t stage = dsm_trajectory_stage_bytes(max_points, max_trajectories), res = dsm_trajectory_res_bytes(max_points, max_trajectories);
+    CudaOwner &o = tr->own;
+    o.host(&tr->stage_host, stage);
+    o.device(&tr->stage_dev, stage);
+    o.device(&tr->hist, 6 * (size_t)max_memory * max_points);
+    o.device(&tr->res, res);
+    o.host(&tr->res_host, res);
+    o.event(&tr->ev);
+    return keep(ctx->trajectory, tr);
+}
+
+static bool traj_params_ok(const dsm_trajectory_params_t &p, int max_memory)
+{
+    for (double w : {p.w_smooth, p.w_clear, p.w_feas, p.margin, p.v_max, p.a_max, p.g_tol})
+        if (!std::isfinite(w) || !(w >= 0.0)) return false;
+    return p.max_iter >= 0 && p.max_iter <= DSM_TRAJECTORY_MAX_ITER && p.memory >= 1 && p.memory <= max_memory && p.max_ls >= 1 &&
+           p.max_ls <= DSM_TRAJECTORY_MAX_LS && p.samples >= 1 && p.samples <= DSM_TRAJECTORY_MAX_SAMPLES_PER_SEGMENT &&
+           std::isfinite(p.radius) && p.radius >= 0.f;
+}
+
+// Stages the request on the calling thread (checking it on the way), then enqueues one H2D copy, the kernel on the
+// signed grid of the latest field request, one D2H copy of the used result and the event.
+extern "C" int dsm_trajectory_enqueue(dsm_ctx *ctx, const double *points, const int32_t *offsets, const double *dt, int n_trajectories,
+                                      const dsm_trajectory_params_t *params)
+{
+    if (!ctx) return DSM_E_INVALID;
+    DsmTrajectory *tr = ctx->trajectory.get();
+    const DsmField *f = ctx->field.get();
+    if (!tr || !f || !f->requested || !f->signed_latest || tr->in_flight) return DSM_E_STATE;
+    if (!points || !offsets || !dt || !params || n_trajectories < 1 || n_trajectories > tr->max_traj) return DSM_E_INVALID;
+    const dsm_trajectory_params_t p = *params;
+    if (!traj_params_ok(p, tr->max_memory) || offsets[0] != 0) return DSM_E_INVALID;
+    int nmax = 0;
+    unsigned long long samples = 0;
+    for (int j = 0; j < n_trajectories; j++)
+    {
+        const int n = offsets[j + 1] - offsets[j];
+        if (offsets[j + 1] < offsets[j] || n < 7 || n > DSM_TRAJECTORY_MAX_POINTS || offsets[j + 1] > tr->max_points) return DSM_E_INVALID;
+        if (!std::isfinite(dt[j]) || !(dt[j] > 0.0)) return DSM_E_INVALID;
+        nmax = std::max(nmax, n);
+        samples += (unsigned long long)(n - 3) * (unsigned long long)p.samples + 1;
+    }
+    const int n_points = offsets[n_trajectories];
+    if ((unsigned long long)n_points * (unsigned long long)p.max_iter * (unsigned long long)(p.max_ls + 1) > DSM_TRAJECTORY_MAX_WORK ||
+        samples > DSM_TRAJECTORY_MAX_SAMPLES)
+        return DSM_E_INVALID;
+    for (size_t c = 0; c < 3 * (size_t)n_points; c++)
+        if (!std::isfinite(points[c])) return DSM_E_INVALID;
+    // the packed request (dsm_device.cuh); the previous job's copy out of this staging ended before its wait, which no
+    // job in flight implies
+    uint8_t *h = tr->stage_host;
+    std::memcpy(h, points, 24 * (size_t)n_points);
+    std::memcpy(h + 24 * (size_t)n_points, dt, 8 * (size_t)n_trajectories);
+    std::memcpy(h + 24 * (size_t)n_points + 8 * (size_t)n_trajectories, offsets, 4 * ((size_t)n_trajectories + 1));
+    CK(cudaSetDevice(ctx->device));
+    CK(cudaMemcpyAsync(tr->stage_dev, h, dsm_trajectory_stage_bytes(n_points, n_trajectories), cudaMemcpyHostToDevice, ctx->stream));
+    const double *d_pts = reinterpret_cast<const double *>(tr->stage_dev), *d_dt = d_pts + 3 * (size_t)n_points;
+    const int32_t *d_ofs = reinterpret_cast<const int32_t *>(d_dt + n_trajectories);
+    const int32_t *grid = f->sgn->grid;
+    CK(dsm_launch_trajectory(d_pts, d_dt, d_ofs, n_trajectories, nmax, reinterpret_cast<const float *>(grid), grid + dsm_field_header(f->voxels),
+                             f->g, p, tr->hist, tr->res, ctx->stream));
+    tr->n = n_trajectories, tr->n_points = n_points;
+    return submit(ctx, *tr, tr->res, dsm_trajectory_res_bytes(n_points, n_trajectories), f->requests);
+}
+
+extern "C" int dsm_trajectory_wait(dsm_ctx *ctx, dsm_trajectory_info_t *info, const dsm_trajectory_t **records, const double **points)
+{
+    if (!ctx) return DSM_E_INVALID;
+    DsmTrajectory *tr = ctx->trajectory.get();
+    const int rc = wait_head(ctx, tr);
+    if (rc != DSM_OK) return rc;
+    copy_info(info, tr->words());
+    const uint8_t *r = tr->res_host + 4 * DSM_TRAJ_WORDS;
+    if (records) *records = reinterpret_cast<const dsm_trajectory_t *>(r);
+    if (points) *points = reinterpret_cast<const double *>(r + sizeof(dsm_trajectory_t) * (size_t)tr->n);
+    return capacity(ctx, tr->words(), DSM_TRAJ_ERR_TAG, "dsm_trajectory_wait", "the field the job read");
+}
+
 // ---- checkpoints that do not stop the stream (include/dsm.h, DESIGN.md §8.5) ----
 // The two images at the context's current capacities; whatever was there before is released first (the old and the new
 // need not fit at once).  On failure the checkpoint has no images and its calls return DSM_E_STATE.

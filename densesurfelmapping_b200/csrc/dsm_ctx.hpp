@@ -311,6 +311,17 @@ struct DsmTour : DsmJob
     int n = 0, n_starts = 0; // of the job in flight or last waited for
 };
 
+// dsm_trajectory_* (DESIGN.md §8.17), allocated by dsm_trajectory_enable: the pinned and device staging of the request,
+// the L-BFGS history (6 max_memory doubles per point) and the device result
+struct DsmTrajectory : DsmJob
+{
+    int max_traj = 0, max_points = 0, max_memory = 0;
+    uint8_t *stage_host = nullptr, *stage_dev = nullptr; // dsm_trajectory_stage_bytes(max_points, max_traj)
+    double *hist = nullptr;
+    uint8_t *res = nullptr;                              // dsm_trajectory_res_bytes(max_points, max_traj)
+    int n = 0, n_points = 0; // of the job in flight or last waited for
+};
+
 #define DSM_MAX_CHUNKS 4
 
 struct dsm_ctx
@@ -388,6 +399,7 @@ struct dsm_ctx
     std::unique_ptr<DsmGain> gain;               // nullptr until dsm_gain_enable
     std::unique_ptr<DsmTour> tour;               // nullptr until dsm_tour_enable
     std::unique_ptr<DsmViewpoint> viewpoint;     // nullptr until dsm_viewpoint_enable
+    std::unique_ptr<DsmTrajectory> trajectory;   // nullptr until dsm_trajectory_enable
     int run_split = 2;          // sub-batches per dsm_batch_run (dsm_set_concurrency)
     // pinned host staging for the small per-batch tables
     float *h_pose = nullptr; // [2B][32]: pose then inverse; first half: the batch calls, second half: the resident stream

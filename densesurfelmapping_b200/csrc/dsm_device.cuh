@@ -320,6 +320,59 @@ __device__ __forceinline__ bool dsm_traversable(const uint8_t *state, const int3
 {
     return state[i] == DSM_STATE_FREE && __int_as_float(dist[i]) >= radius;
 }
+// The point query of include/dsm.h on a distance or signed grid (DESIGN.md §8.8, §8.16): fp64 addressing, fp32
+// interpolation with one rounding per operation.  Shared by k_field_query, k_field_clearance and k_trajectory.
+__device__ __forceinline__ float q_lerp(float a, float b, float t) { return __fadd_rn(a, __fmul_rn(t, __fsub_rn(b, a))); }
+
+// one axis of the addressing: false outside (NaN included); else the lower and upper corner and the fraction
+__device__ __forceinline__ bool q_axis(double p, double v, int o, int n, int &i, int &j, float &t)
+{
+    const double u = p / v - (double)o - 0.5;
+    if (!(u >= 0.0 && u <= (double)(n - 1))) return false;
+    i = min((int)floor(u), max(n - 2, 0));
+    j = min(i + 1, n - 1);
+    t = (float)(u - (double)i);
+    return true;
+}
+
+// the point query at p: dist (and, with GRAD, the gradient) per include/dsm.h; inside = the point is inside the grid;
+// empty: every inside point gets dist = fill and a zero gradient
+template <bool GRAD>
+__device__ __forceinline__ float4 q_sample(const float *__restrict__ dist, const DsmFieldGrid &g, bool empty, float fill, double px, double py,
+                                           double pz, bool &inside)
+{
+    const double v = (double)g.voxel;
+    int ix, jx, iy, jy, iz, jz;
+    float tx, ty, tz;
+    inside = q_axis(px, v, g.o[0], g.n[0], ix, jx, tx) && q_axis(py, v, g.o[1], g.n[1], iy, jy, ty) && q_axis(pz, v, g.o[2], g.n[2], iz, jz, tz);
+    if (!inside) return make_float4(__int_as_float(0x7fc00000), 0.f, 0.f, 0.f);
+    if (empty) return make_float4(fill, 0.f, 0.f, 0.f);
+    const size_t nx = (size_t)g.n[0], ny = (size_t)g.n[1];
+    const size_t r00 = (iz * ny + iy) * nx, r10 = (iz * ny + jy) * nx, r01 = (jz * ny + iy) * nx, r11 = (jz * ny + jy) * nx;
+    const float c000 = __ldg(dist + r00 + ix), c100 = __ldg(dist + r00 + jx), c010 = __ldg(dist + r10 + ix), c110 = __ldg(dist + r10 + jx);
+    const float c001 = __ldg(dist + r01 + ix), c101 = __ldg(dist + r01 + jx), c011 = __ldg(dist + r11 + ix), c111 = __ldg(dist + r11 + jx);
+    float4 r;
+    r.x = q_lerp(q_lerp(q_lerp(c000, c100, tx), q_lerp(c010, c110, tx), ty), q_lerp(q_lerp(c001, c101, tx), q_lerp(c011, c111, tx), ty), tz);
+    if (GRAD)
+    {
+        r.y = __fdiv_rn(q_lerp(q_lerp(__fsub_rn(c100, c000), __fsub_rn(c110, c010), ty), q_lerp(__fsub_rn(c101, c001), __fsub_rn(c111, c011), ty), tz), g.voxel);
+        r.z = __fdiv_rn(q_lerp(q_lerp(__fsub_rn(c010, c000), __fsub_rn(c110, c100), tx), q_lerp(__fsub_rn(c011, c001), __fsub_rn(c111, c101), tx), tz), g.voxel);
+        r.w = __fdiv_rn(q_lerp(q_lerp(__fsub_rn(c001, c000), __fsub_rn(c101, c100), tx), q_lerp(__fsub_rn(c011, c010), __fsub_rn(c111, c110), tx), ty), g.voxel);
+    }
+    else
+        r.y = r.z = r.w = 0.f;
+    return r;
+}
+
+// the rules of a field without a site (+inf) and, SIGNED, of one without a voxel of F (-inf): whether one applies, and
+// the distance it gives
+template <bool SIGNED>
+__device__ __forceinline__ bool q_empty(const int32_t *__restrict__ fhdr, float &fill)
+{
+    const bool no_site = fhdr[DSM_FIELD_N_OCCUPIED] == 0;
+    fill = SIGNED && !no_site ? -INFINITY : INFINITY;
+    return no_site || (SIGNED && fhdr[DSM_SIGNED_N_F] == 0);
+}
 int dsm_field_setup(); // raises the dynamic shared-memory limit of the envelope passes (lines of up to 1024 voxels)
 // k_field_mark over pool slots [0, res[1]) with update_times >= min_update_times and stored surfels [0, *store_size);
 // pool_upper / store_upper >= the live sizes size the grid.  store == nullptr: no store.  occ must be zeroed.
@@ -680,3 +733,33 @@ cudaError_t dsm_launch_viewpoint(const DsmViewpointBufs &b, const DsmFieldGrid &
 cudaError_t dsm_launch_tour(const uint32_t *matrix, int n, int open, int n_starts, int max_passes, uint64_t seed, int32_t *tours,
                             uint8_t *res, cudaStream_t st);
 inline size_t dsm_tour_res_bytes(int n_starts, int n) { return 64 + 16 * (size_t)n_starts + 4 * (size_t)n; }
+
+// dsm_trajectory_* (DESIGN.md §8.17), dsm_trajectory.cu.  One staged request (H2D):
+//   double points[n_points][3] | double dt[n] | int32 offsets[n + 1]
+// and one packed result (D2H, 64 + 96 n + 24 n_points B):
+//   int32 header[DSM_TRAJ_WORDS] | dsm_trajectory_t records[n] | double points[n_points][3]
+// The header's first nine words are those of dsm_trajectory_info_t; its last two carry the signed grid's error words,
+// cleared by dsm_trajectory_wait.
+enum
+{
+    DSM_TRAJ_ORIGIN = 0, // 3 words
+    DSM_TRAJ_N = 3,
+    DSM_TRAJ_N_POINTS,
+    DSM_TRAJ_N_STATUS,   // 4 words: trajectories per status (zeroed before the launch; k_trajectory adds)
+    DSM_TRAJ_ERR_TAG = 14, // the signed grid header's DSM_SIGNED_ERR_TAG / _ERR_FRAME, copied by k_trajectory
+    DSM_TRAJ_ERR_FRAME,
+    DSM_TRAJ_WORDS = 16 // 64 B
+};
+inline size_t dsm_trajectory_stage_bytes(int n_points, int n) { return 24 * (size_t)n_points + 8 * (size_t)n + 4 * ((size_t)n + 1); }
+inline size_t dsm_trajectory_res_bytes(int n_points, int n)
+{
+    return 4 * (size_t)DSM_TRAJ_WORDS + sizeof(dsm_trajectory_t) * (size_t)n + 24 * (size_t)n_points;
+}
+// k_trajectory's shared memory for trajectories of at most nmax points: x, xt, g, gt and d, nmax x 3 doubles each
+inline size_t dsm_trajectory_smem(int nmax) { return 5 * 3 * sizeof(double) * (size_t)nmax; }
+// The whole job on the signed grid sdist with its header (at dsm_field_header(voxels)) for the request already on the
+// device (points, dt, offsets; nmax the most points of one of its n_traj trajectories), with the history scratch hist of
+// 6 p.memory doubles per point.  Writes the whole used result; returns the first launch or memset error.
+cudaError_t dsm_launch_trajectory(const double *points, const double *dt, const int32_t *offsets, int n_traj, int nmax, const float *sdist,
+                                  const int32_t *field_header, const DsmFieldGrid &g, const dsm_trajectory_params_t &p, double *hist,
+                                  uint8_t *res, cudaStream_t st);

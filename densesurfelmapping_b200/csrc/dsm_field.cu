@@ -253,62 +253,11 @@ __global__ void __launch_bounds__(32) k_field_lines_signed(int32_t *sdist, const
 //                      minimum (ties to the lower index), the lowest hit and the outside count: the result is the same
 //                      whatever the schedule.
 // Every fp32 step is an explicit _rn intrinsic, so the numpy restatement (oracle/pyoracle_field_query.py) is bit-exact.
+// The point query itself (q_sample, q_empty) lives in dsm_device.cuh, shared with the trajectory job.
 // SIGNED (DESIGN.md §8.16): the same on the signed grid, whose header gives two rules in place of the "no site" one: no
 // site, +inf; no voxel of F, -inf (an interpolation of infinities of one sign would be NaN).
 #define FIELD_QUERY_BLOCK 256
 #define FIELD_CLEAR_WARPS 8
-
-__device__ __forceinline__ float q_lerp(float a, float b, float t) { return __fadd_rn(a, __fmul_rn(t, __fsub_rn(b, a))); }
-
-// one axis of the addressing: false outside (NaN included); else the lower and upper corner and the fraction
-__device__ __forceinline__ bool q_axis(double p, double v, int o, int n, int &i, int &j, float &t)
-{
-    const double u = p / v - (double)o - 0.5;
-    if (!(u >= 0.0 && u <= (double)(n - 1))) return false;
-    i = min((int)floor(u), max(n - 2, 0));
-    j = min(i + 1, n - 1);
-    t = (float)(u - (double)i);
-    return true;
-}
-
-// the point query at p: dist (and, with GRAD, the gradient) per include/dsm.h; inside = the point is inside the grid;
-// empty: every inside point gets dist = fill and a zero gradient
-template <bool GRAD>
-__device__ __forceinline__ float4 q_sample(const float *__restrict__ dist, const DsmFieldGrid &g, bool empty, float fill, double px, double py,
-                                           double pz, bool &inside)
-{
-    const double v = (double)g.voxel;
-    int ix, jx, iy, jy, iz, jz;
-    float tx, ty, tz;
-    inside = q_axis(px, v, g.o[0], g.n[0], ix, jx, tx) && q_axis(py, v, g.o[1], g.n[1], iy, jy, ty) && q_axis(pz, v, g.o[2], g.n[2], iz, jz, tz);
-    if (!inside) return make_float4(__int_as_float(0x7fc00000), 0.f, 0.f, 0.f);
-    if (empty) return make_float4(fill, 0.f, 0.f, 0.f);
-    const size_t nx = (size_t)g.n[0], ny = (size_t)g.n[1];
-    const size_t r00 = (iz * ny + iy) * nx, r10 = (iz * ny + jy) * nx, r01 = (jz * ny + iy) * nx, r11 = (jz * ny + jy) * nx;
-    const float c000 = __ldg(dist + r00 + ix), c100 = __ldg(dist + r00 + jx), c010 = __ldg(dist + r10 + ix), c110 = __ldg(dist + r10 + jx);
-    const float c001 = __ldg(dist + r01 + ix), c101 = __ldg(dist + r01 + jx), c011 = __ldg(dist + r11 + ix), c111 = __ldg(dist + r11 + jx);
-    float4 r;
-    r.x = q_lerp(q_lerp(q_lerp(c000, c100, tx), q_lerp(c010, c110, tx), ty), q_lerp(q_lerp(c001, c101, tx), q_lerp(c011, c111, tx), ty), tz);
-    if (GRAD)
-    {
-        r.y = __fdiv_rn(q_lerp(q_lerp(__fsub_rn(c100, c000), __fsub_rn(c110, c010), ty), q_lerp(__fsub_rn(c101, c001), __fsub_rn(c111, c011), ty), tz), g.voxel);
-        r.z = __fdiv_rn(q_lerp(q_lerp(__fsub_rn(c010, c000), __fsub_rn(c110, c100), tx), q_lerp(__fsub_rn(c011, c001), __fsub_rn(c111, c101), tx), tz), g.voxel);
-        r.w = __fdiv_rn(q_lerp(q_lerp(__fsub_rn(c001, c000), __fsub_rn(c101, c100), tx), q_lerp(__fsub_rn(c011, c010), __fsub_rn(c111, c110), tx), ty), g.voxel);
-    }
-    else
-        r.y = r.z = r.w = 0.f;
-    return r;
-}
-
-// the rules of a field without a site (+inf) and, SIGNED, of one without a voxel of F (-inf): whether one applies, and
-// the distance it gives
-template <bool SIGNED>
-__device__ __forceinline__ bool q_empty(const int32_t *__restrict__ fhdr, float &fill)
-{
-    const bool no_site = fhdr[DSM_FIELD_N_OCCUPIED] == 0;
-    fill = SIGNED && !no_site ? -INFINITY : INFINITY;
-    return no_site || (SIGNED && fhdr[DSM_SIGNED_N_F] == 0);
-}
 
 template <bool SIGNED>
 __global__ void __launch_bounds__(FIELD_QUERY_BLOCK) k_field_query(const float *__restrict__ dist, const int32_t *__restrict__ fhdr, const DsmFieldGrid g,

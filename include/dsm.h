@@ -694,6 +694,109 @@ int dsm_field_signed(dsm_ctx *ctx, const float **sdist);
 int dsm_field_query_enqueue_signed(dsm_ctx *ctx, const double *points, int n_points, const double *waypoints, const int32_t *offsets,
                                    int n_trajectories, float step, float radius);
 
+/* ---- trajectory optimisation on the signed grid: smoothness, clearance and feasibility of B-splines (DESIGN.md §8.17) ----
+ * A trajectory job optimises many uniform cubic B-splines, each given by its control points and knot interval, against
+ * the signed grid of the latest field request (any kind: plain, resident, known or loaded), in stream order behind it,
+ * with that request's origin o and voxel edge v captured at the enqueue.  Like a query it reads only the grid; a later
+ * field request may be enqueued while a job is in flight and does not change what the job reads.
+ *
+ * Definition (every step fp64 with one rounding per operation, except the field samples).
+ *   Trajectory j: control points Q_0 .. Q_{N-1} = points[offsets[j] .. offsets[j+1] - 1] (xyz, world metres), 7 <= N <=
+ *   256, and knot interval dt = dt[j] > 0.  Q_0..Q_2 and Q_{N-3}..Q_{N-1} are fixed (the start and end state); the free
+ *   points are Q_3 .. Q_{N-4}, M = N - 6 of them.
+ *   Field term at a free point: d, (gx, gy, gz) the signed point query (dsm_field_query_enqueue_signed) at Q_i in fp32,
+ *   widened.  A point outside the grid contributes nothing and is counted; the "no site" rule (+INFINITY) contributes
+ *   nothing; a field without a voxel of F (-INFINITY) is not optimised (status 3, the points returned unchanged, every
+ *   cost word 0).
+ *   Sum: every sum over an index k (a term or a free point, k = i - 3 for free point i) is lane-ordered: lane l = k mod 32
+ *   adds its values in ascending k to 0.0, then each lane adds lane l ^ m for m = 16, 8, 4, 2, 1 (the same bits on every
+ *   lane).  A product of two per-point vectors sums ((a_x b_x + a_y b_y) + a_z b_z) per point this way.
+ *   Cost J = (w_smooth J_s + w_clear J_c) + w_feas J_f:
+ *     J_s = sum over m = 0..N-4 of (j_x^2 + j_y^2) + j_z^2, j = (Q_{m+3} - Q_m) + 3 (Q_{m+1} - Q_{m+2}) per axis;
+ *     J_c = sum over free points inside the grid with e = margin - d > 0 of e^2;
+ *     J_f = F_v + F_a, F_v the sum over m = 0..N-2 of (p_x + p_y) + p_z, p = max(0, V^2 - v_max^2)^2 (zero unless the
+ *     difference is > 0) with V = (Q_{m+1} - Q_m) / dt, F_a likewise over m = 0..N-3 with A = ((Q_{m+2} - Q_{m+1}) -
+ *     (Q_{m+1} - Q_m)) / dt^2 (dt^2 = dt dt) against a_max^2.
+ *   Gradient at free point i, per axis, with D(q) = 4 t q for t = q^2 - lim^2 > 0, else 0:
+ *     g_s = 2 (((j_{i-3} - 3 j_{i-2}) + 3 j_{i-1}) - j_i);  g_c = (-2 e) g_axis for a point with a clearance term, else 0;
+ *     g_f = (D(V_{i-1}) - D(V_i)) / dt + ((D(A_{i-2}) - 2 D(A_{i-1})) + D(A_i)) / dt^2;
+ *     g = (w_smooth g_s + w_clear g_c) + w_feas g_f.
+ *   L-BFGS: evaluate at the initial points (evaluations = 1, cost_start = J).  Each iteration: stop with status 0 when
+ *   max |g| (from 0.0, fmax) <= g_tol, with status 1 when iterations == max_iter.  Direction: with stored pairs the
+ *   two-loop recursion, q = g, for pairs newest to oldest alpha_k = (1 / s_k^T y_k) (s_k^T q), q = q - alpha_k y_k; r =
+ *   ((s^T y) / (y^T y) of the newest pair) q; oldest to newest beta = (1 / s_k^T y_k) (y_k^T r), r = r + s_k (alpha_k -
+ *   beta); d = -r; if not g^T d < 0 the pairs are dropped.  Without pairs d = -g and the first step is v / sqrt(g^T g),
+ *   else 1.  Armijo backtracking: up to max_ls trials x_t = x + step d on the free points, accepted when J_t <= J +
+ *   (1e-4 step) g^T d, else step = step 0.5; no accepted trial stops with status 2 at the last accepted point.  After
+ *   an accepted trial s = x_t - x, y = g_t - g; the pair is kept (dropping the oldest beyond `memory`) when s^T y > 0.
+ *   n_free_outside counts the free points outside the grid at the returned points.
+ *   Final check of the returned points: segment m = 0..N-4 at u = (double)s / K, s < K, then the end point (segment
+ *   N-4 at u = 1), sample index m K + s; the point ((b0 Q_m + b1 Q_{m+1}) + b2 Q_{m+2}) + b3 Q_{m+3} per axis with
+ *   u2 = u u, u3 = u2 u, w = 1 - u, b0 = ((w w) w) / 6, b1 = ((3 u3 - 6 u2) + 4) / 6, b2 = (((3 u2 - 3 u3) + 3 u) + 1) / 6,
+ *   b3 = u3 / 6.  Each sample is a signed point query, distance only; min_dist, argmin, first_hit (d < radius) and
+ *   n_outside as the trajectory clearance of dsm_field_query_enqueue.  max_v and max_a are the largest per-axis |V| and
+ *   |A| of the returned control points, which bound the curve's velocity and acceleration (its convex-hull property).
+ *
+ *   dsm_trajectory_enable   once, after dsm_field_signed_enable (DSM_E_STATE otherwise).  DSM_E_INVALID for
+ *                           max_trajectories or max_points outside [1, 2^24] or max_memory outside [1, 16].  Allocates the
+ *                           pinned and device staging, the L-BFGS history (48 max_memory bytes per point), the device
+ *                           result and its pinned copy and an event.  DSM_E_NOMEM with nothing kept.
+ *   dsm_trajectory_enqueue  stages the request on the calling thread, then enqueues one H2D copy, the kernels, one D2H
+ *                           copy of the used result and the event; never waits.  DSM_E_STATE before dsm_trajectory_enable,
+ *                           before any field request, when the latest request was enqueued without the signed grid, and
+ *                           while a job is in flight.  DSM_E_INVALID for a NULL pointer or params, n_trajectories outside
+ *                           [1, max_trajectories], offsets[0] != 0, a trajectory of fewer than 7 or more than 256 points,
+ *                           more than max_points points, a non-finite control point or dt, dt <= 0, a weight, margin,
+ *                           v_max, a_max or g_tol that is not finite and >= 0, max_iter outside [0, 1024], memory outside
+ *                           [1, max_memory], max_ls outside [1, 32], samples outside [1, 64], a radius that is not finite
+ *                           and >= 0, more than 2^32 field samples of optimisation (sum of N_j max_iter (max_ls + 1)), or
+ *                           more than 2^26 final samples.
+ *   dsm_trajectory_wait     waits for that job only.  *records (n_trajectories) and *points (the optimised control points,
+ *                           laid out as the request's) are the context's pinned results, valid until the next
+ *                           dsm_trajectory_enqueue; any out-pointer may be NULL.  DSM_E_CAPACITY as dsm_field_query_wait
+ *                           for a field taken after a rejected frame, with valid results.  DSM_E_STATE with no job
+ *                           enqueued. */
+typedef struct dsm_trajectory_params_t
+{
+    double w_smooth, w_clear, w_feas;  /* weights of J_s, J_c and J_f */
+    double margin, v_max, a_max;       /* metres, metres per second, metres per second squared */
+    double g_tol;                      /* stop when max |g| <= g_tol */
+    int32_t max_iter, memory, max_ls;  /* iterations, L-BFGS pairs, Armijo trials */
+    int32_t samples;                   /* K: final samples per segment */
+    float radius;                      /* first_hit: a final sample with d < radius */
+    int32_t reserved[3];               /* 0 */
+} dsm_trajectory_params_t;             /* 88 B */
+typedef struct dsm_trajectory_t
+{
+    int32_t status;                    /* 0 converged, 1 max_iter, 2 line search failed, 3 no voxel of F */
+    int32_t iterations, evaluations, n_free_outside;
+    double cost_start, cost;           /* J at the initial and the returned points */
+    double smoothness, clearance, feasibility; /* J_s, J_c, J_f at the returned points, unweighted */
+    double max_v, max_a;
+    float min_dist;
+    int32_t argmin, first_hit, n_outside;
+    int32_t reserved[2];               /* 0 */
+} dsm_trajectory_t;                    /* 96 B */
+typedef struct dsm_trajectory_info_t
+{
+    int32_t origin[3];                 /* of the field the job read, in voxels */
+    int32_t n_trajectories, n_points;
+    int32_t n_status[4];               /* trajectories per status */
+    int32_t reserved[7];               /* 0 */
+} dsm_trajectory_info_t;               /* 64 B */
+#define DSM_TRAJECTORY_MAX_POINTS 256
+#define DSM_TRAJECTORY_MAX_MEMORY 16
+#define DSM_TRAJECTORY_MAX_CAPACITY (1 << 24)
+#define DSM_TRAJECTORY_MAX_ITER 1024
+#define DSM_TRAJECTORY_MAX_LS 32
+#define DSM_TRAJECTORY_MAX_SAMPLES_PER_SEGMENT 64
+#define DSM_TRAJECTORY_MAX_WORK (1ull << 32)
+#define DSM_TRAJECTORY_MAX_SAMPLES (1 << 26)
+int dsm_trajectory_enable(dsm_ctx *ctx, int max_trajectories, int max_points, int max_memory);
+int dsm_trajectory_enqueue(dsm_ctx *ctx, const double *points, const int32_t *offsets, const double *dt, int n_trajectories,
+                           const dsm_trajectory_params_t *params);
+int dsm_trajectory_wait(dsm_ctx *ctx, dsm_trajectory_info_t *info, const dsm_trajectory_t **records, const double **points);
+
 /* ---- paths through known free space: travel cost from a start to every voxel, goals and frontiers (DESIGN.md §8.11) ----
  * A reach job reads the state grid and the distance grid of the latest field request, which must be a known one, in
  * stream order behind it, with that request's origin o and voxel edge v captured at the job's enqueue, and (with

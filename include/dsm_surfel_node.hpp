@@ -746,6 +746,32 @@ class SurfelMapNode
         out.clear();
         return query("trajectory_clearance", signed_field, nullptr, 0, waypoints, offsets, n, step, radius, nullptr, &out);
     }
+    // ---- trajectory optimisation on the signed grid of the latest fused frame (DESIGN.md §8.17) ----
+    // once, after enable_signed_distance: the most trajectories, control points and L-BFGS pairs of one trajectories()
+    int enable_trajectories(int max_trajectories, int max_points, int max_memory)
+    {
+        return ctx_.run("enable_trajectories", [&] { return dsm_trajectory_enable(ctx_.ctx, max_trajectories, max_points, max_memory); });
+    }
+    // n uniform cubic B-splines (control points xyz doubles, offsets[n + 1], knot intervals dt[n]) optimised against the
+    // signed grid of the latest fused frame's field (include/dsm.h): records receives n records and optimised the
+    // control points, laid out as the request's.  DSM_E_STATE without enable_signed_distance() before that field, before
+    // any field, and after load_state* until the next fused frame; DSM_E_CAPACITY with the results of the last applied
+    // frame's field, as distance_field().
+    int trajectories(const double *points, const int32_t *offsets, const double *dt, int n, const dsm_trajectory_params_t &params,
+                     dsm_trajectory_info_t &info, std::vector<dsm_trajectory_t> &records, std::vector<double> &optimised)
+    {
+        records.clear();
+        optimised.clear();
+        info = dsm_trajectory_info_t();
+        const dsm_trajectory_t *r = nullptr;
+        const double *q = nullptr;
+        return job("trajectories", ANY_FIELD, true, [&] { return dsm_trajectory_enqueue(ctx_.ctx, points, offsets, dt, n, &params); },
+                   [&] { return dsm_trajectory_wait(ctx_.ctx, &info, &r, &q); },
+                   [&] {
+                       records.assign(r, r + info.n_trajectories);
+                       optimised.assign(q, q + 3 * (size_t)info.n_points);
+                   });
+    }
     // the field of the latest fused frame: dist [nz][ny][nx] in metres (the library's pinned buffer, valid until the next
     // frame is fused; nullptr for a field kept on the device), the grid's origin in voxels and the occupied voxels.  DSM_E_STATE when no frame has been fused
     // since the last call; DSM_E_CAPACITY with the field of the last applied frame, as published_clouds().
