@@ -1,10 +1,13 @@
 // Shared by the C++ test drivers of this directory: the reference's caller types, the binary I/O of a driver's in.bin
-// and out.bin, the frame record of the fuse_map drivers, and the harness of the node drivers (argument prefix, message
-// loop, cloud records and digest).  Every record is read and written in the layout the driver's header comment gives.
+// and out.bin, the frame record of the fuse_map drivers, the harness of the node drivers (argument prefix, message loop,
+// cloud records and digest), and the pieces of the known-field node drivers (field arguments, the field handout of each
+// depth message, the reload step and the end of a drive).  Every record is read and written in the layout the driver's
+// header comment gives.
 #pragma once
 #include <cstdint>
 #include <cstdio>
 #include <cstdlib>
+#include <initializer_list>
 #include <string>
 #include <vector>
 #include <opencv2/opencv.hpp> // oracle/shim
@@ -214,6 +217,80 @@ inline bool put_final(dsm::SurfelMapNode &node)
 inline bool save_files(dsm::SurfelMapNode &node, const std::string &prefix)
 {
     return node.save_mesh(prefix + ".ply") == DSM_OK && node.save_cloud(prefix + ".pcd") == DSM_OK;
+}
+
+// ---- the known-field node drivers ----
+
+// The field block of their arguments, argv[13..18] = voxel nx ny nz max_views max_range, after the sized prefix.
+struct FieldArgs
+{
+    float voxel, max_range;
+    int nx, ny, nz, max_views;
+    explicit FieldArgs(char **argv)
+        : voxel((float)atof(argv[13])), max_range((float)atof(argv[18])), nx(atoi(argv[14])), ny(atoi(argv[15])), nz(atoi(argv[16])),
+          max_views(atoi(argv[17]))
+    {
+    }
+    int cells() const { return nx * ny * nz; }
+    // enable_distance_field, then enable_known_space unless max_views is 0; 4 when either fails
+    int enable(dsm::SurfelMapNode &node) const
+    {
+        if (node.enable_distance_field(voxel, nx, ny, nz) != DSM_OK) return 4;
+        if (max_views > 0 && node.enable_known_space(max_views, max_range) != DSM_OK) return 4;
+        return 0;
+    }
+    // the centre of the grid's middle voxel, ((origin + n / 2) + 0.5) * voxel per axis
+    void middle(const int32_t origin[3], double c[3]) const
+    {
+        const int n[3] = {nx, ny, nz};
+        for (int a = 0; a < 3; a++) c[a] = ((double)(origin[a] + n[a] / 2) + 0.5) * (double)voxel;
+    }
+};
+
+// The field of the frame just fused: distance_field(), then, with `known`, known_space() when distance_field() handed
+// out a field (DSM_OK, and with `capacity` DSM_E_CAPACITY too).  rs is rc when known_space() was not called.
+struct FieldHandout
+{
+    const float *dist;
+    const uint8_t *state;
+    int32_t origin[3];
+    int n_occ, n_free, rc, rs;
+    FieldHandout(dsm::SurfelMapNode &node, bool known, bool capacity = false) : dist(nullptr), state(nullptr), n_occ(0), n_free(0)
+    {
+        origin[0] = origin[1] = origin[2] = 0;
+        rc = node.distance_field(dist, origin, n_occ);
+        rs = known && (rc == DSM_OK || (capacity && rc == DSM_E_CAPACITY)) ? node.known_space(state, n_free) : rc;
+    }
+    bool ok() const { return rc == DSM_OK && rs == DSM_OK; }
+    void put_origin() const { put(origin[0]), put(origin[1]), put(origin[2]); }
+    // the grids (int32 n + n values), empty unless ok()
+    void put_state(const FieldArgs &f) const { put_n(state, ok() ? f.cells() : 0); }
+    void put_dist(const FieldArgs &f) const { put_n(dist, ok() ? f.cells() : 0); }
+};
+
+// the first code of a chain of calls that is not DSM_OK, else DSM_OK
+inline int first_error(std::initializer_list<int> rcs)
+{
+    for (int rc : rcs)
+        if (rc != DSM_OK) return rc;
+    return DSM_OK;
+}
+
+// save_state and load_state through <prefix>.state; false (exit code 6) when either fails
+inline bool reload(dsm::SurfelMapNode &node, const std::string &prefix)
+{
+    return node.save_state(prefix + ".state") == DSM_OK && node.load_state(prefix + ".state") == DSM_OK;
+}
+
+// the end of a drive: local_surfels (int32 n + records), save_mesh and save_cloud to <prefix>.ply / .pcd, then the
+// files closed; 6 when a read or a save fails, else 0
+inline int end_drive(dsm::SurfelMapNode &node, const std::string &prefix)
+{
+    std::vector<dsm_surfel_t> local;
+    if (node.local_surfels(local) != DSM_OK) return 6;
+    put_list(local);
+    if (!save_files(node, prefix)) return 6;
+    return close_io();
 }
 
 template <class T>

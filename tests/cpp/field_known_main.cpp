@@ -17,13 +17,11 @@ int main(int argc, char **argv)
 {
     if (argc != 23) return 2;
     const NodeArgs args(argv, true);
-    const float voxel = (float)atof(argv[13]);
-    const int nx = atoi(argv[14]), ny = atoi(argv[15]), nz = atoi(argv[16]);
-    const int max_views = atoi(argv[17]), reload_at = atoi(argv[19]);
+    const FieldArgs field(argv);
+    const int max_views = field.max_views, reload_at = atoi(argv[19]);
     DriverNode node(args);
     if (const int e = setup_code(node.last_error())) return e;
-    if (node.enable_distance_field(voxel, nx, ny, nz) != DSM_OK) return 4;
-    if (max_views > 0 && node.enable_known_space(max_views, (float)atof(argv[18])) != DSM_OK) return 4;
+    if (const int e = field.enable(node)) return e;
     if (!open_io(argv[20], argv[21])) return 5;
     const std::string prefix = argv[22];
     const int S = dsm_num_seeds(node.context());
@@ -32,11 +30,8 @@ int main(int argc, char **argv)
     std::vector<double> poses;
     int depth_msgs = 0, fused = 0, captures = 0;
     const int e = feed_script(node, args.W, args.H, [&]() -> int {
-        const float *dist = nullptr;
-        int32_t origin[3] = {0, 0, 0};
-        int n_occ = 0;
-        const int rc = node.distance_field(dist, origin, n_occ);
-        fused += rc != DSM_E_STATE; // every fused frame requests a field
+        const FieldHandout h(node, max_views > 0, true);
+        fused += h.rc != DSM_E_STATE; // every fused frame requests a field
         if (max_views > 0)
         {
             const int now = node.known_views(slots, poses);
@@ -48,17 +43,14 @@ int main(int argc, char **argv)
                 if (dsm_get_seeds(node.context(), (fused - 1) & 1, s.data()) != DSM_OK) return 6;
                 captures = now;
             }
-            const uint8_t *state = nullptr;
-            int n_free = 0;
-            const int rs = rc == DSM_OK || rc == DSM_E_CAPACITY ? node.known_space(state, n_free) : rc;
             const dsm::Pose cam = node.pose_graph().camera;
-            put(rc != DSM_OK ? rc : rs);
+            put(first_error({h.rc, h.rs}));
             put(cam.x), put(cam.y), put(cam.z);
-            put(origin[0]), put(origin[1]), put(origin[2]);
-            put(n_occ);
-            put_n(dist, rc == DSM_OK ? nx * ny * nz : 0);
-            put_n(state, rc == DSM_OK && rs == DSM_OK ? nx * ny * nz : 0);
-            put(n_free);
+            h.put_origin();
+            put(h.n_occ);
+            put_n(h.dist, h.rc == DSM_OK ? field.cells() : 0);
+            h.put_state(field);
+            put(h.n_free);
             put((int32_t)slots.size());
             for (size_t j = 0; j < slots.size(); j++)
             {
@@ -69,15 +61,10 @@ int main(int argc, char **argv)
         put_clouds(node);
         if (++depth_msgs == reload_at)
         {
-            if (node.save_state(prefix + ".state") != DSM_OK || node.load_state(prefix + ".state") != DSM_OK) return 6;
+            if (!reload(node, prefix)) return 6;
             captures = 0; // load_state empties the slot table
         }
         return 0;
     });
-    if (e) return e;
-    std::vector<dsm_surfel_t> local;
-    if (node.local_surfels(local) != DSM_OK) return 6;
-    put_list(local);
-    if (!save_files(node, prefix)) return 6;
-    return close_io();
+    return e ? e : end_drive(node, prefix);
 }

@@ -18,14 +18,12 @@ int main(int argc, char **argv)
 {
     if (argc != 25) return 2;
     const NodeArgs args(argv, true);
-    const float voxel = (float)atof(argv[13]);
-    const int nx = atoi(argv[14]), ny = atoi(argv[15]), nz = atoi(argv[16]);
-    const int max_views = atoi(argv[17]), max_clusters = atoi(argv[19]), max_voxels = atoi(argv[20]), reload_at = atoi(argv[21]);
+    const FieldArgs field(argv);
+    const int max_clusters = atoi(argv[19]), max_voxels = atoi(argv[20]), reload_at = atoi(argv[21]);
     const bool frontiers = max_clusters > 0 || max_voxels > 0;
     DriverNode node(args);
     if (const int e = setup_code(node.last_error())) return e;
-    if (node.enable_distance_field(voxel, nx, ny, nz) != DSM_OK) return 4;
-    if (node.enable_known_space(max_views, (float)atof(argv[18])) != DSM_OK) return 4;
+    if (const int e = field.enable(node)) return e;
     if (frontiers && node.enable_frontiers(max_clusters, max_voxels) != DSM_OK) return 4;
     if (!open_io(argv[22], argv[23])) return 5;
     const std::string prefix = argv[24];
@@ -38,19 +36,13 @@ int main(int argc, char **argv)
         dsm_frontier_counts_t counts = dsm_frontier_counts_t();
         // the job is enqueued behind the field request of the frame just fused, before that field is handed out
         const int rf = frontiers ? node.frontiers(m, clusters, voxels, counts) : DSM_OK;
-        const float *dist = nullptr;
-        int32_t origin[3] = {0, 0, 0};
-        int n_occ = 0;
-        const int rc = node.distance_field(dist, origin, n_occ);
-        const uint8_t *state = nullptr;
-        int n_free = 0;
-        const int rs = rc == DSM_OK ? node.known_space(state, n_free) : rc;
+        const FieldHandout h(node, true);
         if (frontiers)
         {
-            put(rc != DSM_OK ? rc : rs != DSM_OK ? rs : rf);
+            put(first_error({h.rc, h.rs, rf}));
             put(m);
-            put(origin[0]), put(origin[1]), put(origin[2]);
-            put_n(state, rc == DSM_OK && rs == DSM_OK ? nx * ny * nz : 0);
+            h.put_origin();
+            h.put_state(field);
             put_list(clusters);
             put_list(voxels);
             put(counts);
@@ -58,17 +50,12 @@ int main(int argc, char **argv)
         int after_load = 1;
         if (++depth_msgs == reload_at)
         {
-            if (node.save_state(prefix + ".state") != DSM_OK || node.load_state(prefix + ".state") != DSM_OK) return 6;
+            if (!reload(node, prefix)) return 6;
             if (frontiers) after_load = node.frontiers(1, clusters, voxels, counts);
         }
         if (frontiers) put(after_load);
         put_clouds(node);
         return 0;
     });
-    if (e) return e;
-    std::vector<dsm_surfel_t> local;
-    if (node.local_surfels(local) != DSM_OK) return 6;
-    put_list(local);
-    if (!save_files(node, prefix)) return 6;
-    return close_io();
+    return e ? e : end_drive(node, prefix);
 }

@@ -25,14 +25,12 @@ int main(int argc, char **argv)
 {
     if (argc != 24) return 2;
     const NodeArgs args(argv, true);
-    const float voxel = (float)atof(argv[13]);
-    const int nx = atoi(argv[14]), ny = atoi(argv[15]), nz = atoi(argv[16]);
-    const int max_views = atoi(argv[17]), max_gain_views = atoi(argv[19]), reload_at = atoi(argv[20]);
+    const FieldArgs field(argv);
+    const int max_gain_views = atoi(argv[19]), reload_at = atoi(argv[20]);
     const bool gain = max_gain_views > 0;
     DriverNode node(args);
     if (const int e = setup_code(node.last_error())) return e;
-    if (node.enable_distance_field(voxel, nx, ny, nz) != DSM_OK) return 4;
-    if (node.enable_known_space(max_views, (float)atof(argv[18])) != DSM_OK) return 4;
+    if (const int e = field.enable(node)) return e;
     if (gain && (node.enable_frontiers(64, 1 << 16) != DSM_OK || node.enable_view_gain(max_gain_views) != DSM_OK)) return 4;
     if (!open_io(argv[21], argv[22])) return 5;
     const std::string prefix = argv[23];
@@ -45,21 +43,16 @@ int main(int argc, char **argv)
     int depth_msgs = 0;
     const int e = feed_script(node, args.W, args.H, [&]() -> int {
         const int ub = depth_msgs % 2;
-        const float max_range = voxel * (float)(10 + 5 * (depth_msgs % 3));
+        const float max_range = field.voxel * (float)(10 + 5 * (depth_msgs % 3));
         dsm_frontier_counts_t counts = dsm_frontier_counts_t();
         dsm_gain_info_t info = dsm_gain_info_t();
         int before = 1, rg = DSM_OK;
         // the jobs are enqueued behind the field request of the frame just fused, before that field is handed out
         if (gain) before = node.view_gain(poses.data(), n_yaws, max_range, ub, named, info, gains);
         const int rf = gain ? node.frontiers(1, clusters, voxels, counts) : DSM_OK;
-        const float *dist = nullptr;
-        int32_t origin[3] = {0, 0, 0};
-        int n_occ = 0;
-        const int rc = node.distance_field(dist, origin, n_occ);
-        const uint8_t *state = nullptr;
-        int n_free = 0;
-        const int rs = rc == DSM_OK ? node.known_space(state, n_free) : rc;
-        const int n[3] = {nx, ny, nz};
+        const FieldHandout h(node, true);
+        double centre[3];
+        field.middle(h.origin, centre);
         for (int k = 0; k < n_yaws; k++)
         {
             const double a = 0.25 * M_PI * k, f[3] = {std::cos(a), std::sin(a), 0.0}, r[3] = {std::sin(a), -std::cos(a), 0.0},
@@ -68,19 +61,18 @@ int main(int argc, char **argv)
             {
                 double *row = &poses[12 * k + 4 * i];
                 row[0] = r[i], row[1] = d[i], row[2] = f[i];
-                row[3] = ((double)(origin[i] + n[i] / 2) + 0.5) * (double)voxel;
+                row[3] = centre[i];
             }
             named[k] = k % ((int)clusters.size() + 2) - 1;
         }
-        if (gain && rc == DSM_OK && rs == DSM_OK && rf == DSM_OK) rg = node.view_gain(poses.data(), n_yaws, max_range, ub, named, info, gains);
+        if (gain && h.ok() && rf == DSM_OK) rg = node.view_gain(poses.data(), n_yaws, max_range, ub, named, info, gains);
         if (gain)
         {
-            const bool ok = rc == DSM_OK && rs == DSM_OK;
-            put(rc != DSM_OK ? rc : rs != DSM_OK ? rs : rf != DSM_OK ? rf : rg);
+            put(first_error({h.rc, h.rs, rf, rg}));
             put(ub);
             put(max_range);
-            put(origin[0]), put(origin[1]), put(origin[2]);
-            put_n(state, ok ? nx * ny * nz : 0);
+            h.put_origin();
+            h.put_state(field);
             put_list(clusters);
             put_list(voxels);
             put_list(poses);
@@ -92,17 +84,12 @@ int main(int argc, char **argv)
         int after_load = 1;
         if (++depth_msgs == reload_at)
         {
-            if (node.save_state(prefix + ".state") != DSM_OK || node.load_state(prefix + ".state") != DSM_OK) return 6;
+            if (!reload(node, prefix)) return 6;
             if (gain) after_load = node.view_gain(poses.data(), n_yaws, max_range, ub, std::vector<int32_t>(), info, gains);
         }
         if (gain) put(after_load);
         put_clouds(node);
         return 0;
     });
-    if (e) return e;
-    std::vector<dsm_surfel_t> local;
-    if (node.local_surfels(local) != DSM_OK) return 6;
-    put_list(local);
-    if (!save_files(node, prefix)) return 6;
-    return close_io();
+    return e ? e : end_drive(node, prefix);
 }

@@ -23,15 +23,12 @@ int main(int argc, char **argv)
 {
     if (argc != 26) return 2;
     const NodeArgs args(argv, true);
-    const float voxel = (float)atof(argv[13]);
-    const int nx = atoi(argv[14]), ny = atoi(argv[15]), nz = atoi(argv[16]);
-    const int max_views = atoi(argv[17]), max_targets = atoi(argv[19]), max_path = atoi(argv[20]), max_rounds = atoi(argv[21]);
-    const int reload_at = atoi(argv[22]);
+    const FieldArgs field(argv);
+    const int max_targets = atoi(argv[19]), max_path = atoi(argv[20]), max_rounds = atoi(argv[21]), reload_at = atoi(argv[22]);
     const bool paths = max_targets > 0 || max_path > 0 || max_rounds > 0;
     DriverNode node(args);
     if (const int e = setup_code(node.last_error())) return e;
-    if (node.enable_distance_field(voxel, nx, ny, nz) != DSM_OK) return 4;
-    if (node.enable_known_space(max_views, (float)atof(argv[18])) != DSM_OK) return 4;
+    if (const int e = field.enable(node)) return e;
     if (paths && (node.enable_frontiers(max_targets, 1 << 16) != DSM_OK || node.enable_reach(max_targets, max_path, max_rounds) != DSM_OK))
         return 4;
     if (!open_io(argv[23], argv[24])) return 5;
@@ -43,7 +40,7 @@ int main(int argc, char **argv)
     int depth_msgs = 0;
     const int e = feed_script(node, args.W, args.H, [&]() -> int {
         const int k = depth_msgs % 5;
-        const float radius = voxel * (float)(depth_msgs % 3) / 2.f;
+        const float radius = field.voxel * (float)(depth_msgs % 3) / 2.f;
         dsm_frontier_counts_t counts = dsm_frontier_counts_t();
         dsm_reach_info_t info = dsm_reach_info_t();
         double start[3] = {0.0, 0.0, 0.0};
@@ -51,26 +48,18 @@ int main(int argc, char **argv)
         // the jobs are enqueued behind the field request of the frame just fused, before that field is handed out
         if (paths) before = node.reach(start, radius, k, no_goals, true, info, targets, path);
         const int rf = paths ? node.frontiers(1, clusters, voxels, counts) : DSM_OK;
-        const float *dist = nullptr;
-        int32_t origin[3] = {0, 0, 0};
-        int n_occ = 0;
-        const int rc = node.distance_field(dist, origin, n_occ);
-        const uint8_t *state = nullptr;
-        int n_free = 0;
-        const int rs = rc == DSM_OK ? node.known_space(state, n_free) : rc;
-        const int n[3] = {nx, ny, nz};
-        for (int a = 0; a < 3; a++) start[a] = ((double)(origin[a] + n[a] / 2) + 0.5) * (double)voxel;
-        if (paths && rc == DSM_OK && rs == DSM_OK && rf == DSM_OK) rr = node.reach(start, radius, k, no_goals, true, info, targets, path);
+        const FieldHandout h(node, true);
+        field.middle(h.origin, start);
+        if (paths && h.ok() && rf == DSM_OK) rr = node.reach(start, radius, k, no_goals, true, info, targets, path);
         if (paths)
         {
-            const bool ok = rc == DSM_OK && rs == DSM_OK;
-            put(rc != DSM_OK ? rc : rs != DSM_OK ? rs : rf != DSM_OK ? rf : rr);
+            put(first_error({h.rc, h.rs, rf, rr}));
             put(k);
             put(start[0]), put(start[1]), put(start[2]);
             put(radius);
-            put(origin[0]), put(origin[1]), put(origin[2]);
-            put_n(state, ok ? nx * ny * nz : 0);
-            put_n(dist, ok ? nx * ny * nz : 0);
+            h.put_origin();
+            h.put_state(field);
+            h.put_dist(field);
             put_list(clusters);
             put_list(voxels);
             put(info);
@@ -81,17 +70,12 @@ int main(int argc, char **argv)
         int after_load = 1;
         if (++depth_msgs == reload_at)
         {
-            if (node.save_state(prefix + ".state") != DSM_OK || node.load_state(prefix + ".state") != DSM_OK) return 6;
+            if (!reload(node, prefix)) return 6;
             if (paths) after_load = node.reach(start, radius, k, no_goals, false, info, targets, path);
         }
         if (paths) put(after_load);
         put_clouds(node);
         return 0;
     });
-    if (e) return e;
-    std::vector<dsm_surfel_t> local;
-    if (node.local_surfels(local) != DSM_OK) return 6;
-    put_list(local);
-    if (!save_files(node, prefix)) return 6;
-    return close_io();
+    return e ? e : end_drive(node, prefix);
 }

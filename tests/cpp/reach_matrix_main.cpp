@@ -23,15 +23,13 @@ int main(int argc, char **argv)
 {
     if (argc != 26) return 2;
     const NodeArgs args(argv, true);
-    const float voxel = (float)atof(argv[13]);
-    const int nx = atoi(argv[14]), ny = atoi(argv[15]), nz = atoi(argv[16]);
-    const int max_views = atoi(argv[17]), max_sites = atoi(argv[19]), max_tiles = atoi(argv[20]), max_rounds = atoi(argv[21]);
-    const int reload_at = atoi(argv[22]);
+    const FieldArgs field(argv);
+    const int nx = field.nx, ny = field.ny;
+    const int max_sites = atoi(argv[19]), max_tiles = atoi(argv[20]), max_rounds = atoi(argv[21]), reload_at = atoi(argv[22]);
     const bool matrices = max_sites > 0 || max_tiles > 0 || max_rounds > 0;
     DriverNode node(args);
     if (const int e = setup_code(node.last_error())) return e;
-    if (node.enable_distance_field(voxel, nx, ny, nz) != DSM_OK) return 4;
-    if (node.enable_known_space(max_views, (float)atof(argv[18])) != DSM_OK) return 4;
+    if (const int e = field.enable(node)) return e;
     if (matrices && (node.enable_frontiers(64, 1 << 16) != DSM_OK || node.enable_reach(max_sites - 1, 1 << 16, max_rounds) != DSM_OK ||
                      node.enable_reach_matrix(max_sites, max_tiles, max_rounds) != DSM_OK))
         return 4;
@@ -47,44 +45,36 @@ int main(int argc, char **argv)
     int depth_msgs = 0;
     const int e = feed_script(node, args.W, args.H, [&]() -> int {
         const int k = depth_msgs % 5;
-        const float radius = voxel * (float)(depth_msgs % 3) / 2.f;
+        const float radius = field.voxel * (float)(depth_msgs % 3) / 2.f;
         dsm_frontier_counts_t counts = dsm_frontier_counts_t();
         dsm_reach_info_t rinfo = dsm_reach_info_t();
         dsm_reach_matrix_info_t info = dsm_reach_matrix_info_t();
         // the jobs are enqueued behind the field request of the frame just fused, before that field is handed out
         const int rf = matrices ? node.frontiers(1, clusters, voxels, counts) : DSM_OK;
-        const float *dist = nullptr;
-        int32_t origin[3] = {0, 0, 0};
-        int n_occ = 0;
-        const int rc = node.distance_field(dist, origin, n_occ);
-        const uint8_t *state = nullptr;
-        int n_free = 0;
-        const int rs = rc == DSM_OK ? node.known_space(state, n_free) : rc;
-        const int n[3] = {nx, ny, nz};
+        const FieldHandout h(node, true);
         double start[3];
-        for (int a = 0; a < 3; a++) start[a] = ((double)(origin[a] + n[a] / 2) + 0.5) * (double)voxel;
+        field.middle(h.origin, start);
         int rr = DSM_OK, rm = DSM_OK;
         points.assign(start, start + 3);
-        if (matrices && rc == DSM_OK && rs == DSM_OK && rf == DSM_OK)
+        if (matrices && h.ok() && rf == DSM_OK)
         {
             rr = node.reach(start, radius, k, no_goals, true, rinfo, targets, path);
             for (const dsm_reach_target_t &t : targets)
                 if (t.status == 0)
                 {
                     const int v = t.viewpoint, c[3] = {v % nx, v / nx % ny, v / (nx * ny)};
-                    for (int a = 0; a < 3; a++) points.push_back(((double)(origin[a] + c[a]) + 0.5) * (double)voxel);
+                    for (int a = 0; a < 3; a++) points.push_back(((double)(h.origin[a] + c[a]) + 0.5) * (double)field.voxel);
                 }
             if (rr == DSM_OK) rm = node.reach_matrix(points, radius, k, info, sites, matrix);
         }
         if (matrices)
         {
-            const bool ok = rc == DSM_OK && rs == DSM_OK;
-            put(rc != DSM_OK ? rc : rs != DSM_OK ? rs : rf != DSM_OK ? rf : rr != DSM_OK ? rr : rm);
+            put(first_error({h.rc, h.rs, rf, rr, rm}));
             put(k);
             put(radius);
-            put(origin[0]), put(origin[1]), put(origin[2]);
-            put_n(state, ok ? nx * ny * nz : 0);
-            put_n(dist, ok ? nx * ny * nz : 0);
+            h.put_origin();
+            h.put_state(field);
+            h.put_dist(field);
             put_list(points);
             put(info);
             put_list(sites);
@@ -93,17 +83,12 @@ int main(int argc, char **argv)
         int after_load = 1;
         if (++depth_msgs == reload_at)
         {
-            if (node.save_state(prefix + ".state") != DSM_OK || node.load_state(prefix + ".state") != DSM_OK) return 6;
+            if (!reload(node, prefix)) return 6;
             if (matrices) after_load = node.reach_matrix(points, radius, k, info, sites, matrix);
         }
         if (matrices) put(after_load);
         put_clouds(node);
         return 0;
     });
-    if (e) return e;
-    std::vector<dsm_surfel_t> local;
-    if (node.local_surfels(local) != DSM_OK) return 6;
-    put_list(local);
-    if (!save_files(node, prefix)) return 6;
-    return close_io();
+    return e ? e : end_drive(node, prefix);
 }

@@ -14,14 +14,13 @@ int main(int argc, char **argv)
 {
     if (argc != 26) return 2;
     const NodeArgs args(argv, true);
-    const float voxel = (float)atof(argv[13]);
-    const int nx = atoi(argv[14]), ny = atoi(argv[15]), nz = atoi(argv[16]);
-    const int max_views = atoi(argv[17]), max_sites = atoi(argv[19]), max_tiles = atoi(argv[20]), max_rounds = atoi(argv[21]);
+    const FieldArgs field(argv);
+    const int nx = field.nx, ny = field.ny;
+    const int max_sites = atoi(argv[19]), max_tiles = atoi(argv[20]), max_rounds = atoi(argv[21]);
     const int n_starts = atoi(argv[22]), max_passes = atoi(argv[23]);
     DriverNode node(args);
     if (const int e = setup_code(node.last_error())) return e;
-    if (node.enable_distance_field(voxel, nx, ny, nz) != DSM_OK) return 4;
-    if (node.enable_known_space(max_views, (float)atof(argv[18])) != DSM_OK) return 4;
+    if (const int e = field.enable(node)) return e;
     if (node.enable_frontiers(64, 1 << 16) != DSM_OK || node.enable_reach(max_sites - 1, 1 << 16, max_rounds) != DSM_OK ||
         node.enable_reach_matrix(max_sites, max_tiles, max_rounds) != DSM_OK || node.enable_tour(max_sites, n_starts) != DSM_OK)
         return 4;
@@ -48,9 +47,9 @@ int main(int argc, char **argv)
         int32_t origin[3] = {0, 0, 0};
         int n_occ = 0;
         if (rc == DSM_OK) rc = node.distance_field(dist, origin, n_occ);
-        const int n[3] = {nx, ny, nz};
-        points.clear();
-        for (int a = 0; a < 3; a++) points.push_back(((double)(origin[a] + n[a] / 2) + 0.5) * (double)voxel);
+        double start[3];
+        field.middle(origin, start);
+        points.assign(start, start + 3);
         if (rc == DSM_OK) rc = node.reach(points.data(), 0.f, 1, no_goals, true, rinfo, targets, path);
         if (rc == DSM_OK)
         {
@@ -58,7 +57,7 @@ int main(int argc, char **argv)
                 if (t.status == 0)
                 {
                     const int v = t.viewpoint, c[3] = {v % nx, v / nx % ny, v / (nx * ny)};
-                    for (int a = 0; a < 3; a++) points.push_back(((double)(origin[a] + c[a]) + 0.5) * (double)voxel);
+                    for (int a = 0; a < 3; a++) points.push_back(((double)(origin[a] + c[a]) + 0.5) * (double)field.voxel);
                 }
             rc = node.reach_matrix(points, 0.f, 1, minfo, sites, matrix);
         }

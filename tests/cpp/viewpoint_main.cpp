@@ -27,14 +27,12 @@ int main(int argc, char **argv)
 {
     if (argc != 24) return 2;
     const NodeArgs args(argv, true);
-    const float voxel = (float)atof(argv[13]);
-    const int nx = atoi(argv[14]), ny = atoi(argv[15]), nz = atoi(argv[16]);
-    const int max_views = atoi(argv[17]), reload_at = atoi(argv[20]);
+    const FieldArgs field(argv);
+    const int reload_at = atoi(argv[20]);
     const bool on = atoi(argv[19]) != 0;
     DriverNode node(args);
     if (const int e = setup_code(node.last_error())) return e;
-    if (node.enable_distance_field(voxel, nx, ny, nz) != DSM_OK) return 4;
-    if (node.enable_known_space(max_views, (float)atof(argv[18])) != DSM_OK) return 4;
+    if (const int e = field.enable(node)) return e;
     if (on && (node.enable_frontiers(64, 1 << 16) != DSM_OK || node.enable_reach(8, 1 << 12, 4096) != DSM_OK ||
                node.enable_viewpoints(66, 1 << 16) != DSM_OK))
         return 4;
@@ -56,38 +54,30 @@ int main(int argc, char **argv)
     int depth_msgs = 0;
     const int e = feed_script(node, args.W, args.H, [&]() -> int {
         const int ub = depth_msgs % 2, with_reach = depth_msgs % 2;
-        const float max_range = voxel * (float)(10 + 5 * (depth_msgs % 3));
+        const float max_range = field.voxel * (float)(10 + 5 * (depth_msgs % 3));
         dsm_viewpoint_params_t prm = {1, 5, 1, 1 + depth_msgs % 2, 64, 1, 4, with_reach, 0.1f, 0};
         dsm_frontier_counts_t counts = dsm_frontier_counts_t();
         dsm_reach_info_t rinfo = dsm_reach_info_t();
         dsm_viewpoint_info_t info = dsm_viewpoint_info_t();
         const int rf = on ? node.frontiers(1, clusters, voxels, counts) : DSM_OK;
-        const float *dist = nullptr;
-        int32_t origin[3] = {0, 0, 0};
-        int n_occ = 0;
-        const int rc = node.distance_field(dist, origin, n_occ);
-        const uint8_t *state = nullptr;
-        int n_free = 0;
-        const int rs = rc == DSM_OK ? node.known_space(state, n_free) : rc;
-        const int n[3] = {nx, ny, nz};
+        const FieldHandout h(node, true);
         double start[3];
-        for (int i = 0; i < 3; i++) start[i] = ((double)(origin[i] + n[i] / 2) + 0.5) * (double)voxel;
+        field.middle(h.origin, start);
         named.clear();
         for (int k = 0; k < (int)clusters.size() + 2; k++) named.push_back(k);
         int rr = DSM_OK, rv = DSM_OK;
-        const bool ok = rc == DSM_OK && rs == DSM_OK && rf == DSM_OK;
+        const bool ok = h.ok() && rf == DSM_OK;
         if (on && ok) rr = node.reach(start, prm.radius, 1, std::vector<double>(), false, rinfo, targets, path);
         if (on && ok && rr == DSM_OK)
             rv = node.viewpoints(prm, rotations.data(), 12, max_range, ub, named, with_reach, info, records, slots);
         if (on)
         {
-            const bool grids = rc == DSM_OK && rs == DSM_OK;
-            put(rc != DSM_OK ? rc : rs != DSM_OK ? rs : rf != DSM_OK ? rf : rr != DSM_OK ? rr : rv);
+            put(first_error({h.rc, h.rs, rf, rr, rv}));
             put(ub);
             put(max_range);
-            put(origin[0]), put(origin[1]), put(origin[2]);
-            put_n(state, grids ? nx * ny * nz : 0);
-            put_n(dist, grids ? nx * ny * nz : 0);
+            h.put_origin();
+            h.put_state(field);
+            h.put_dist(field);
             put_list(clusters);
             put_list(voxels);
             put(rinfo);
@@ -102,17 +92,12 @@ int main(int argc, char **argv)
         int after_load = 1;
         if (++depth_msgs == reload_at)
         {
-            if (node.save_state(prefix + ".state") != DSM_OK || node.load_state(prefix + ".state") != DSM_OK) return 6;
+            if (!reload(node, prefix)) return 6;
             if (on) after_load = node.viewpoints(prm, rotations.data(), 12, max_range, ub, named, 0, info, records, slots);
         }
         if (on) put(after_load);
         put_clouds(node);
         return 0;
     });
-    if (e) return e;
-    std::vector<dsm_surfel_t> local;
-    if (node.local_surfels(local) != DSM_OK) return 6;
-    put_list(local);
-    if (!save_files(node, prefix)) return 6;
-    return close_io();
+    return e ? e : end_drive(node, prefix);
 }

@@ -9,6 +9,7 @@ import numpy as np
 import pytest
 
 from pyoracle_frontier import CLUSTER_DTYPE, FREE, OCCUPIED, UNKNOWN, frontier_mask, frontiers
+from planner_scenes import serpentine
 
 BIG = 1 << 26
 
@@ -132,23 +133,6 @@ def test_checkerboard_is_one_component():
     assert n["n_frontier"] == int((st == FREE).sum()) and n["n_components"] == 1
     assert c["first"].tolist() == [0] and vox.tolist() == np.flatnonzero(st.reshape(-1) == FREE).tolist()
     same(run(st, m=2, mc=1, mv=10), bfs_model(st, (0, 0, 0), 0.2, 2, 1, 10))
-
-
-def serpentine(nx, ny, nz):
-    """Free rows along x on every other (y, z) line, joined at alternating ends into one path through the whole grid;
-    everything else unknown."""
-    st = np.full((nz, ny, nx), UNKNOWN, np.uint8)
-    lines = [(y, z) for z in range(0, nz, 2) for y in (range(0, ny, 2) if z // 2 % 2 == 0 else range(ny - 1 - (ny - 1) % 2, -1, -2))]
-    for k, (y, z) in enumerate(lines):
-        st[z, y, :] = FREE
-        if k + 1 < len(lines):
-            y2, z2 = lines[k + 1]
-            x = nx - 1 if k % 2 == 0 else 0
-            if z2 == z:
-                st[z, y + 1 if y2 > y else y - 1, x] = FREE
-            else:
-                st[z + 1, y, x] = FREE
-    return st
 
 
 def test_serpentine_fills_the_grid():

@@ -11,29 +11,9 @@ import pyoracle_field_known as K
 import pyoracle_frontier
 import pyoracle_gain as G
 from densesurfelmapping_b200 import capi
+from planner_scenes import random_pose, symmetric_scene, symmetric_views, wall_scene, yaw_pose
 
 UNKNOWN, OCCUPIED, FREE = G.UNKNOWN, G.OCCUPIED, G.FREE
-
-
-def yaw_pose(k, t, pitch_down=False):
-    """A camera looking along the k-th horizontal axis direction (+x, +y, -x, -y) from t; R a signed permutation."""
-    f = [(1, 0, 0), (0, 1, 0), (-1, 0, 0), (0, -1, 0)][k]
-    r = [(0, -1, 0), (1, 0, 0), (0, 1, 0), (-1, 0, 0)][k]
-    dn = (0, 0, -1)
-    R = np.array([r, dn, f], np.float64).T
-    if pitch_down:   # looking straight down (z forward = world -z)
-        R = np.array([r, f, dn], np.float64).T * np.array([1, -1, 1])
-    return np.concatenate([R, np.asarray(t, np.float64)[:, None]], axis=1).reshape(12)
-
-
-def random_pose(rng, centre, spread):
-    q = rng.normal(size=4)
-    a, b, c, d = q / np.linalg.norm(q)
-    R = np.array([[a * a + b * b - c * c - d * d, 2 * (b * c - a * d), 2 * (b * d + a * c)],
-                  [2 * (b * c + a * d), a * a - b * b + c * c - d * d, 2 * (c * d - a * b)],
-                  [2 * (b * d - a * c), 2 * (c * d + a * b), a * a - b * b - c * c + d * d]])
-    t = np.asarray(centre, np.float64) + rng.uniform(-spread, spread, 3)
-    return np.concatenate([R, t[:, None]], axis=1).reshape(12)
 
 
 def plain(state, origin, voxel, camera, pose):
@@ -178,12 +158,6 @@ def test_seen_against_exact_geometry(unknown_blocks):
     assert checked > 1000 and disagree <= checked // 100
 
 
-def wall_scene(kind):
-    st = np.full((5, 5, 12), FREE, np.uint8)
-    st[:, :, 6] = kind
-    return st
-
-
 def test_hand_cases():
     voxel, o = 0.5, (0, 0, 0)
     cam = G.Camera(4.0, 4.0, 3.5, 3.5, 8, 8, 5.5, 1)
@@ -262,26 +236,6 @@ def test_axes_of_one_voxel(shape):
     for j, p in enumerate(poses):
         want = plain(st, o, voxel, cam, p)
         assert {k: int(r[j][k]) for k in want} == want
-
-
-def symmetric_scene(n, nz, rng):
-    """A state grid [nz][n][n] (n odd) that depends only on z and on |dx| + |dy| from the centre column: symmetric
-    under 90-degree yaw about the centre voxel, and every tie of the walk between two horizontal axes lands on voxels of
-    one state, so the lowest-axis rule cannot break the symmetry."""
-    h = n // 2
-    table = rng.choice(3, size=(nz, 2 * h + 1), p=(0.25, 0.15, 0.6)).astype(np.uint8)
-    table[:, :3] = FREE
-    y, x = np.mgrid[0:n, 0:n]
-    l1 = np.abs(x - h) + np.abs(y - h)
-    st = table[:, l1]
-    st[:, h, h] = FREE
-    return st
-
-
-def symmetric_views(n, nz, voxel):
-    h = n // 2
-    t = G.centres([(h, h, nz // 2)], (0, 0, 0), voxel)[0]
-    return t, [yaw_pose(k, t) for k in range(4)]
 
 
 def test_yaw_symmetry():

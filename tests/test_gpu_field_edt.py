@@ -15,14 +15,13 @@ import pytest
 import edt_patterns as P
 import pyoracle_field
 import pyoracle_field_query
-from densesurfelmapping_b200 import capi, synth
+from densesurfelmapping_b200 import capi
 from densesurfelmapping_b200.elements import SURFEL_DTYPE
+from known_space import FREE, OCCUPIED, SMALL_CAM, UNKNOWN, small_ctx
 from resident_map import assert_field, load_known
 
 pytestmark = pytest.mark.gpu
 
-SMALL_CAM = synth.Camera(64, 48, 60.0, 60.0, 31.5, 23.5, 0.5, 30.0)
-UNKNOWN, OCCUPIED, FREE = 0, 1, 2
 LIM = 1 << 24
 LENGTHS = [1, 2, 31, 32, 33, 320, 384, 385, 512, 1023, 1024]
 SWEEP = [s for n in LENGTHS for s in ((n, 3, 5), (5, n, 3), (3, 5, n))] + [(33, 385, 1023)]
@@ -34,11 +33,7 @@ def sid(s):
 
 def known_ctx(shape, voxel=0.2):
     """A context whose field has grid `shape` (nx, ny, nz) and views enabled, as the frontier loaders make."""
-    ctx = capi.Context(SMALL_CAM, max_batch=2, max_local_surfels=1 << 12)
-    ctx.pool_upload(np.zeros(0, SURFEL_DTYPE))
-    ctx.field_enable(voxel, *shape)
-    ctx.views_enable(1, 1.0)
-    return ctx
+    return small_ctx(shape, voxel)
 
 
 def states(sites, rng):

@@ -16,50 +16,13 @@ import pyoracle_field
 import pyoracle_field_known
 import pyoracle_field_query
 from densesurfelmapping_b200 import capi, synth
-from densesurfelmapping_b200.elements import POINT_DTYPE, SEED_DTYPE, SURFEL_DTYPE
+from densesurfelmapping_b200.elements import SEED_DTYPE, SURFEL_DTYPE
+from known_space import (K, MAX_RANGE, MAX_VIEWS, NODE_FIELD, RELOAD, SMALL_CAM, Views, assert_error_stays, node_args, pose12,
+                         rejected_known, twin_clouds, twin_node_tail)
 from node_drive import node_script, run_driver
 from resident_map import SHAPES, STORE, T, camera, field_points, frames, map_state, new_ctx, simple_lists, warp, windowed, xyz
 
 pytestmark = pytest.mark.gpu
-
-MAX_RANGE = 30.0
-HALF = 8   # new_ctx's max_batch / 2: a windowed call of n <= 8 frames runs in the staging half of its parity
-
-
-def pose12(p16, W=np.eye(4)):
-    """Row-major [R | t] (camera to world) of a column-major pose, after the warp W."""
-    T4 = np.asarray(p16, np.float64).reshape(4, 4).T
-    return (W @ T4)[:3, :4].reshape(12)
-
-
-class Views:
-    """The test's side of the slot table: per slot, the rays the oracle expects and the view's current pose."""
-
-    def __init__(self, ctx, max_views):
-        self.ctx, self.max = ctx, max_views
-        ctx.views_enable(max_views, MAX_RANGE)
-        self.rays, self.poses, self.n = {}, {}, 0
-
-    def capture_call(self, call, t0, t1):
-        """Captures every frame of windowed call number `call` (frames t0..t1-1) into the next slots."""
-        for f, t in enumerate(range(t0, t1)):
-            slot = self.n % self.max
-            self.ctx.views_capture(f, slot)
-            self.rays[slot] = pyoracle_field_known.capture(self.ctx.seeds((call % 2) * HALF + f))
-            self.poses[slot] = pose12(frames()[t][0])
-            self.n += 1
-
-    def warp(self, W):
-        for s in self.poses:
-            self.poses[s] = pose12(np.eye(4), W @ np.vstack([self.poses[s].reshape(3, 4), [0, 0, 0, 1]]))
-
-    def request(self):
-        slots = sorted(self.rays)
-        return slots, np.array([self.poses[s] for s in slots]).reshape(-1, 12)
-
-    def oracle_views(self, slots):
-        return [(self.rays[s], self.poses[s]) for s in slots]
-
 
 def known_equals_oracle(ctx, views, voxel, shape, center, m, what, host_copy=True, slots=None):
     all_slots, poses = views.request()
@@ -243,30 +206,17 @@ def test_known_field_beside_a_snapshot_a_checkpoint_and_a_query(tmp_path):
 def test_rejected_frame_comes_back_from_wait():
     lists = simple_lists()
     first = next(t for t in range(T) if lists[t][1])
-    shape, voxel = (64, 64, 32), 0.1
     a = new_ctx(store=STORE)
     for t0 in range(0, first, 1):
         windowed(a, t0, t0 + 1, lists, want_counts=False)
-    b = new_ctx(store=1)
-    b.field_enable(voxel, *shape)
-    views = Views(b, 4)
-    for call, t0 in enumerate(range(0, first + 2)):
-        windowed(b, t0, t0 + 1, lists, want_counts=False)
-        views.capture_call(call, t0, t0 + 1)   # the rejected frame's rays are observations too
-    slots, poses = views.request()
-    b.field_enqueue_known(camera(first - 1), 1, slots, poses)
-    with pytest.raises(capi.DsmError) as e:
-        b.field_wait()
-    assert e.value.code == -6
-    state, n_free = b.field_state()
-    want = pyoracle_field_known.known_field(field_points(a, 1), voxel, shape, camera(first - 1), views.oracle_views(slots), MAX_RANGE)
-    assert e.value.field[0].tobytes() == want[0].tobytes() and e.value.field[2] == want[2] and want[2] > 0
-    assert state.tobytes() == want[3].tobytes() and n_free == want[4] > 0
-    with pytest.raises(capi.DsmError) as e:
-        b.pool_size()
-    assert e.value.code == -6                            # wait did not clear it
+    r = rejected_known(lambda ctx: None, lambda ctx, first: None)
+    want = pyoracle_field_known.known_field(field_points(a, 1), r.voxel, r.shape, camera(first - 1), r.views.oracle_views(r.slots),
+                                            MAX_RANGE)
+    assert r.field[0].tobytes() == want[0].tobytes() and r.field[2] == want[2] and want[2] > 0
+    assert r.state.tobytes() == want[3].tobytes() and r.n_free == want[4] > 0
+    assert_error_stays(r.ctx)
     a.close()
-    b.close()
+    r.ctx.close()
 
 
 def test_error_contract():
@@ -330,7 +280,7 @@ def test_the_most_views_one_request_takes():
     poses, the last view alone at the seventh, and one view whose rotation overflows R * p (an infinite ray length
     cuts its rays to zero length; a ray with an infinite or NaN endpoint coordinate carves nothing).  Equal to the
     oracle over the distinct views, and the last view carves voxels no other does."""
-    cam = synth.Camera(64, 48, 60.0, 60.0, 31.5, 23.5, 0.5, 30.0)
+    cam = SMALL_CAM
     ctx = capi.Context(cam, max_batch=2, max_local_surfels=1 << 14)
     ctx.pool_upload(np.zeros(0, SURFEL_DTYPE))
     voxel, shape, max_range = 0.1, (64, 64, 64), 5.0
@@ -373,7 +323,7 @@ def test_the_most_views_one_request_takes():
 def test_a_size_a_user_runs():
     """320x320x40 at 0.2 m over 256 views of 1226x370 frames: eight frames fused once, each captured into 32 slots,
     at 256 poses spread along and across the road."""
-    cam = synth.KITTI
+    cam = K
     ctx = capi.Context(cam, max_batch=16, max_local_surfels=1 << 18)
     ctx.pool_upload(np.zeros(0, SURFEL_DTYPE))
     shape, voxel = (320, 320, 40), 0.2
@@ -405,22 +355,16 @@ def test_a_size_a_user_runs():
 
 
 # ---- the node ----
-FIELD = (0.2, 96, 96, 32)
-MAX_VIEWS = 5
-RELOAD = 12   # the node saves and loads its state after this depth message
-
-
 def test_node_known_space_equals_the_oracle_and_changes_nothing(tmp_path):
     """The node drive (keyframes, loop closures): every fused frame's known field equals the oracle over the views the
     node carried (the driver dumps their frames' seeds and current poses); clouds, PLY and PCD files equal a twin
     without known space; after load_state the slot table is empty and refills."""
-    cam, n = synth.KITTI, 24
+    cam, n = K, 24
     sc = node_script(cam, n)
-    voxel, nx, ny, nz = FIELD
+    voxel, nx, ny, nz = NODE_FIELD
     pa, pb = str(tmp_path / "mapa"), str(tmp_path / "mapb")
-    node = [2, 0, 1 << 20, 1 << 21, *FIELD]
-    r = run_driver("field_known_main", str(tmp_path), cam, sc, node + [MAX_VIEWS, MAX_RANGE, RELOAD], tag="a", after=[pa])
-    q = run_driver("field_known_main", str(tmp_path), cam, sc, node + [0, MAX_RANGE, RELOAD], tag="b", after=[pb])
+    r = run_driver("field_known_main", str(tmp_path), cam, sc, node_args() + [RELOAD], tag="a", after=[pa])
+    q = run_driver("field_known_main", str(tmp_path), cam, sc, node_args(0) + [RELOAD], tag="b", after=[pb])
     free, most = 0, 0
     for t in range(n):
         rc = r.i()
@@ -432,9 +376,8 @@ def test_node_known_space_equals_the_oracle_and_changes_nothing(tmp_path):
         for _ in range(r.i()):
             seeds = r.lst(SEED_DTYPE)
             views.append((pyoracle_field_known.capture(seeds), r.lst(np.float64).copy()))
-        rr, act, inact = r.i(), r.lst(POINT_DTYPE), r.lst(POINT_DTYPE)
-        rq, act_q, inact_q = q.i(), q.lst(POINT_DTYPE), q.lst(POINT_DTYPE)
-        assert rc == 0 and rr == 0 and rq == 0, f"message {t}"
+        act, inact = twin_clouds(r, q, f"message {t}")
+        assert rc == 0, f"message {t}"
         assert 1 <= len(views) <= MAX_VIEWS
         if t == RELOAD:
             assert len(views) == 1, "the slot table refills from empty after load_state"
@@ -443,9 +386,5 @@ def test_node_known_space_equals_the_oracle_and_changes_nothing(tmp_path):
         assert origin.tolist() == want[1].tolist() and (n_occ, n_free) == (want[2], want[4]), f"message {t}"
         assert state.tobytes() == want[3].tobytes() and dist.tobytes() == want[0].tobytes(), f"message {t}"
         free += n_free > 0
-        assert act.tobytes() == act_q.tobytes() and inact.tobytes() == inact_q.tobytes(), f"message {t}: clouds"
     assert free > n // 2 and most > 2
-    assert r.lst(SURFEL_DTYPE).tobytes() == q.lst(SURFEL_DTYPE).tobytes()
-    assert r.o == len(r.raw) and q.o == len(q.raw)
-    for ext in (".ply", ".pcd"):
-        assert filecmp.cmp(pa + ext, pb + ext, shallow=False), ext
+    twin_node_tail(r, q, pa, pb)

@@ -18,14 +18,12 @@ import pyoracle_field_query as fq
 import pyoracle_field_signed as fs
 from densesurfelmapping_b200 import capi, synth
 from densesurfelmapping_b200.elements import POINT_DTYPE, SURFEL_DTYPE
+from known_space import FREE, MAX_RANGE, NODE_FIELD, OCCUPIED, UNKNOWN, Views, small_ctx
 from node_drive import node_script, run_driver
 from resident_map import SHAPES, STORE, T, camera, field_points, map_state, new_ctx, simple_lists, warp, windowed, xyz
-from test_gpu_field_known import MAX_RANGE, Views
 
 pytestmark = pytest.mark.gpu
 
-SMALL_CAM = synth.Camera(64, 48, 60.0, 60.0, 31.5, 23.5, 0.5, 30.0)
-UNKNOWN, OCCUPIED, FREE = 0, 1, 2
 LENGTHS = [1, 2, 31, 32, 33, 320, 384, 385, 512, 1023, 1024]
 SWEEP = [s for n in LENGTHS for s in ((n, 3, 5), (5, n, 3), (3, 5, n))] + [(33, 385, 1023)]
 CAPS = (4096, 64, 512)
@@ -126,10 +124,7 @@ def test_drive_fields_equal_the_oracle(chunk, shape):
 
 # ---- crafted grids ----
 def known_ctx(shape, voxel=0.2):
-    ctx = capi.Context(SMALL_CAM, max_batch=2, max_local_surfels=1 << 12)
-    ctx.pool_upload(np.zeros(0, SURFEL_DTYPE))
-    ctx.field_enable(voxel, *shape)
-    ctx.views_enable(1, 1.0)
+    ctx = small_ctx(shape, voxel)
     ctx.field_signed_enable()
     return ctx
 
@@ -401,7 +396,6 @@ def test_error_contract():
 
 
 # ---- the node ----
-FIELD = (0.2, 96, 96, 32)
 
 
 def test_node_signed_field_equals_the_oracle_and_changes_nothing(tmp_path):
@@ -410,11 +404,11 @@ def test_node_signed_field_equals_the_oracle_and_changes_nothing(tmp_path):
     negative value); distances, clouds, PLY and PCD files equal a twin without the signed grid."""
     cam, n = synth.KITTI, 24
     sc = node_script(cam, n)
-    voxel, nx, ny, nz = FIELD
+    voxel, nx, ny, nz = NODE_FIELD
     pa, pb = str(tmp_path / "mapa"), str(tmp_path / "mapb")
     node = [2, 0, 1 << 20, 1 << 21]
-    r = run_driver("field_signed_main", str(tmp_path), cam, sc, node + [1, *FIELD], tag="a", after=[pa])
-    q = run_driver("field_signed_main", str(tmp_path), cam, sc, node + [0, *FIELD], tag="b", after=[pb])
+    r = run_driver("field_signed_main", str(tmp_path), cam, sc, node + [1, *NODE_FIELD], tag="a", after=[pa])
+    q = run_driver("field_signed_main", str(tmp_path), cam, sc, node + [0, *NODE_FIELD], tag="b", after=[pb])
     for t in range(n):
         rc = r.i()
         c = r.take(np.float64, 3).copy()

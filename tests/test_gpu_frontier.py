@@ -9,41 +9,31 @@ through resident_map.load_known), at several min_voxels and both capacity cuts; 
 bytes; the stream order against later field requests, a publish snapshot and an asynchronous checkpoint; the
 rejected-frame and error contracts; and a drive with frontier jobs leaves the map, the clouds and the fields as a twin
 without them.  The node is checked through tests/cpp/frontier_main.cpp."""
-import filecmp
+from functools import partial
 
 import numpy as np
 import pytest
 
+import known_space
 import pyoracle_frontier
-from densesurfelmapping_b200 import capi, synth
-from densesurfelmapping_b200.elements import POINT_DTYPE, SURFEL_DTYPE
+from densesurfelmapping_b200 import capi
+from densesurfelmapping_b200.elements import SURFEL_DTYPE
+from known_space import (FREE, K, OCCUPIED, RELOAD, SMALL_CAM, UNKNOWN, NODE_FIELD, assert_error_stays, known_drive, node_args,
+                         rejected, rejected_known, small_ctx, twin_clouds, twin_drive, twin_node_tail)
 from node_drive import node_script, run_driver
-from resident_map import SHAPES, STORE, T, camera, load_known, map_state, new_ctx, simple_lists, warp, windowed
-from test_frontier_model import serpentine
-from test_gpu_field_known import MAX_RANGE, Views
+from planner_scenes import serpentine
+from resident_map import SHAPES, load_known
 
 pytestmark = pytest.mark.gpu
 
 BIG = 1 << 26          # DSM_FRONTIER_MAX_CAPACITY
 CAPS = (1 << 14, 1 << 20)   # the loaders' table and list capacities (the result is 5.6 MB)
-SMALL_CAM = synth.Camera(64, 48, 60.0, 60.0, 31.5, 23.5, 0.5, 30.0)
-UNKNOWN, OCCUPIED, FREE = pyoracle_frontier.UNKNOWN, pyoracle_frontier.OCCUPIED, pyoracle_frontier.FREE
-
-
-def same(got, want, what):
-    gc, gv, gn = got
-    wc, wv, wn = want
-    assert gn.tobytes() == wn.tobytes(), f"{what}: counts {gn} want {wn}"
-    assert gc.tobytes() == wc.tobytes(), f"{what}: {len(gc)} / {len(wc)} clusters, first differing {next((i for i in range(min(len(gc), len(wc))) if gc[i].tobytes() != wc[i].tobytes()), None)}"
-    assert gv.tobytes() == wv.tobytes(), f"{what}: voxel list ({len(gv)} / {len(wv)})"
+same = partial(known_space.same, names=("clusters", "voxel list", "counts"))
 
 
 def loader(shape, voxel=0.2, caps=CAPS):
     """A context whose field has grid `shape` (nx, ny, nz), with views and frontiers enabled."""
-    ctx = capi.Context(SMALL_CAM, max_batch=2, max_local_surfels=1 << 12)
-    ctx.pool_upload(np.zeros(0, SURFEL_DTYPE))
-    ctx.field_enable(voxel, *shape)
-    ctx.views_enable(1, 1.0)
+    ctx = small_ctx(shape, voxel)
     ctx.frontier_enable(*caps)
     return ctx
 
@@ -185,123 +175,42 @@ def frontier_of_waited_known(ctx, origin, voxel, m, what):
 def test_known_fields_of_the_drive(chunk, shape):
     """The windowed drive with loop-closure warps between calls (views warped with the map); after every call a
     resident known field with a job, then its host-copy twin with a job: both equal the model on the twin's states."""
-    lists = simple_lists()
-    voxels = (0.125, 0.1, 0.3)
-    ctxs, views = {}, {}
-    for v in voxels:
-        ctxs[v] = new_ctx(store=STORE)
-        ctxs[v].field_enable(v, *shape)
-        views[v] = Views(ctxs[v], 6)
-        ctxs[v].frontier_enable(64, 1 << 16)
-    stored, seen = set(), 0
-    for call, t0 in enumerate(range(0, T, chunk)):
-        t1 = min(T, t0 + chunk)
-        for v in voxels:
-            windowed(ctxs[v], t0, t1, lists, want_counts=False)
-            views[v].capture_call(call, t0, t1)
-        for t in range(t0, t1):
-            stored = (stored | set(lists[t][1])) - set(lists[t][2])
-        if call % 2 == 1 and stored:
-            for v in voxels:
-                ctxs[v].pool_transform(warp(1))
-                ctxs[v].inactive_transform(max(stored), warp(2))
-                views[v].warp(warp(1))
-        v = voxels[call % 3]
-        ctx = ctxs[v]
-        slots, poses = views[v].request()
+    seen = 0
+    drive = known_drive(shape, chunk, (0.125, 0.1, 0.3), lambda c: c.frontier_enable(64, 1 << 16), request=False)
+    for call, t0, t1, ctx, v, cam, slots, poses, _, _ in drive:
         m = (1, 2, 50)[call % 3]
-        ctx.field_enqueue_known(camera(t1 - 1), 5, slots, poses, host_copy=False)
+        ctx.field_enqueue_known(cam, 5, slots, poses, host_copy=False)
         ctx.frontier_enqueue(m)             # before the field is waited for
         ctx.field_wait()
         resident = ctx.frontier_wait()
-        ctx.field_enqueue_known(camera(t1 - 1), 5, slots, poses)
+        ctx.field_enqueue_known(cam, 5, slots, poses)
         origin = ctx.field_wait()[1]
         host = frontier_of_waited_known(ctx, origin, v, m, f"frames {t0}-{t1 - 1}, voxel {v}")
         assert all(x.tobytes() == y.tobytes() for x, y in zip(resident, host)), "resident and host-copy requests"
         seen += int(host[2]["n_clusters"]) > 0
     assert seen > 0 or shape == (1, 1, 1)
-    for c in ctxs.values():
-        c.close()
 
 
 def test_frontiers_change_nothing_else(tmp_path):
     """A drive with frontier jobs, one beside a publish snapshot and an asynchronous checkpoint, leaves the map, both
     published clouds and the fields byte-identical to a twin without them."""
-    lists = simple_lists()
-    shape, voxel = (64, 64, 32), 0.1
-    a, b = new_ctx(store=STORE), new_ctx(store=STORE)
-    va, vb = {}, {}
-    for c, d in ((a, va), (b, vb)):
-        c.field_enable(voxel, *shape)
-        c.publish_enable()
-        c.checkpoint_enable()
-        d["v"] = Views(c, 4)
-    a.frontier_enable(32, 4096)
-    stored = set()
-    for call, t0 in enumerate(range(0, T, 2)):
-        t1 = t0 + 2
-        for c, d in ((a, va), (b, vb)):
-            windowed(c, t0, t1, lists, want_counts=False)
-            d["v"].capture_call(call, t0, t1)
-        for t in range(t0, t1):
-            stored = (stored | set(lists[t][1])) - set(lists[t][2])
-        outs = []
-        for c, d in ((a, va), (b, vb)):
-            slots, poses = d["v"].request()
-            c.field_enqueue_known(camera(t1 - 1), 5, slots, poses)
-            if c is a:
-                a.frontier_enqueue(1 + call % 3)
-            c.publish_enqueue(5)
-            c.checkpoint_enqueue(str(tmp_path / f"{'ab'[c is b]}{call}.dsm"))
-            if call % 2 == 1 and stored:
-                c.pool_transform(warp(1))
-                c.inactive_transform(max(stored), warp(2))
-                d["v"].warp(warp(1))
-            f = c.field_wait()
-            st = c.field_state()
-            p = c.publish_wait()
-            assert c.checkpoint_wait(True)
-            outs.append((f, st, p))
-        got = a.frontier_wait()
-        fa, fb = outs[0][0], outs[1][0]
-        what = f"after frames {t0}-{t1 - 1}"
-        same(got, pyoracle_frontier.frontiers(outs[0][1][0], fa[1], voxel, 1 + call % 3, 32, 4096), what)
-        assert fa[0].tobytes() == fb[0].tobytes() and outs[0][1][0].tobytes() == outs[1][1][0].tobytes(), f"{what}: field"
-        assert outs[0][2][0].tobytes() == outs[1][2][0].tobytes() and outs[0][2][1].tobytes() == outs[1][2][1].tobytes(), f"{what}: clouds"
-        assert map_state(a) == map_state(b), f"{what}: map"
-        assert filecmp.cmp(str(tmp_path / f"a{call}.dsm"), str(tmp_path / f"b{call}.dsm"), shallow=False), f"{what}: checkpoint"
-    a.close()
-    b.close()
+    def enqueue(c, is_a, call, t1):
+        if is_a:
+            c.frontier_enqueue(1 + call % 3)
+
+    def check(a, outs, call, t1, what):
+        same(a.frontier_wait(), pyoracle_frontier.frontiers(outs["state"][0], outs["field"][1], 0.1, 1 + call % 3, 32, 4096), what)
+
+    twin_drive(tmp_path, lambda c: None, lambda a: a.frontier_enable(32, 4096), enqueue, lambda c: {}, check)
 
 
 def test_rejected_frame_comes_back_from_wait():
-    lists = simple_lists()
-    first = next(t for t in range(T) if lists[t][1])
-    shape, voxel = (64, 64, 32), 0.1
-    b = new_ctx(store=1)
-    b.field_enable(voxel, *shape)
-    views = Views(b, 4)
-    b.frontier_enable(64, 1 << 16)
-    for call, t0 in enumerate(range(0, first + 2)):
-        windowed(b, t0, t0 + 1, lists, want_counts=False)
-        views.capture_call(call, t0, t0 + 1)
-    slots, poses = views.request()
-    b.field_enqueue_known(camera(first - 1), 1, slots, poses)
-    b.frontier_enqueue(1)
-    with pytest.raises(capi.DsmError) as e:
-        b.field_wait()
-    assert e.value.code == -6
-    origin = e.value.field[1]
-    state, _ = b.field_state()
-    with pytest.raises(capi.DsmError) as e:
-        b.frontier_wait()
-    assert e.value.code == -6
-    same(e.value.frontier, pyoracle_frontier.frontiers(state, origin, voxel, 1, 64, 1 << 16), "rejected")
-    assert e.value.frontier[2]["n_frontier"] > 0
-    with pytest.raises(capi.DsmError) as e:
-        b.pool_size()
-    assert e.value.code == -6                            # wait did not clear it
-    b.close()
+    r = rejected_known(lambda b: b.frontier_enable(64, 1 << 16), lambda b, first: b.frontier_enqueue(1))
+    e = rejected(r.ctx.frontier_wait)
+    same(e.frontier, pyoracle_frontier.frontiers(r.state, r.field[1], r.voxel, 1, 64, 1 << 16), "rejected")
+    assert e.frontier[2]["n_frontier"] > 0
+    assert_error_stays(r.ctx)
+    r.ctx.close()
 
 
 def test_error_contract():
@@ -352,22 +261,16 @@ def test_error_contract():
 
 
 # ---- the node ----
-FIELD = (0.2, 96, 96, 32)
-MAX_VIEWS = 5
-RELOAD = 12   # the node saves and loads its state after this depth message
-
-
 def test_node_frontiers_equal_the_model_and_change_nothing(tmp_path):
     """The node drive (keyframes, loop closures): after every fused frame, frontiers() equals the model over the state
     grid the driver dumps; clouds, PLY and PCD files equal a twin without frontiers; after load_state, frontiers()
     returns DSM_E_STATE until the next fused frame."""
-    cam, n = synth.KITTI, 24
+    cam, n = K, 24
     sc = node_script(cam, n)
-    voxel, nx, ny, nz = FIELD
+    voxel, nx, ny, nz = NODE_FIELD
     pa, pb = str(tmp_path / "mapa"), str(tmp_path / "mapb")
-    node = [2, 0, 1 << 20, 1 << 21, *FIELD, MAX_VIEWS, MAX_RANGE]
-    r = run_driver("frontier_main", str(tmp_path), cam, sc, node + [64, 1 << 16, RELOAD], tag="a", after=[pa])
-    q = run_driver("frontier_main", str(tmp_path), cam, sc, node + [0, 0, RELOAD], tag="b", after=[pb])
+    r = run_driver("frontier_main", str(tmp_path), cam, sc, node_args() + [64, 1 << 16, RELOAD], tag="a", after=[pa])
+    q = run_driver("frontier_main", str(tmp_path), cam, sc, node_args() + [0, 0, RELOAD], tag="b", after=[pb])
     found = 0
     for t in range(n):
         rc, m = r.i(), r.i()
@@ -376,16 +279,11 @@ def test_node_frontiers_equal_the_model_and_change_nothing(tmp_path):
         clusters, vox = r.lst(pyoracle_frontier.CLUSTER_DTYPE), r.lst(np.int32)
         counts = r.take(np.int32, 4).copy()
         after_load = r.i()
-        rr, act, inact = r.i(), r.lst(POINT_DTYPE), r.lst(POINT_DTYPE)
-        rq, act_q, inact_q = q.i(), q.lst(POINT_DTYPE), q.lst(POINT_DTYPE)
-        assert rc == 0 and rr == 0 and rq == 0, f"message {t}: {rc} {rr} {rq}"
+        twin_clouds(r, q, f"message {t}")
+        assert rc == 0, f"message {t}: {rc}"
         want = pyoracle_frontier.frontiers(state, origin, voxel, m, 64, 1 << 16)
         same((clusters, vox, counts.view(pyoracle_frontier.COUNTS_DTYPE)[0]), want, f"message {t}")
         found += len(clusters) > 0
         assert after_load == (-7 if t == RELOAD - 1 else 1), f"message {t}: frontiers() after load_state"
-        assert act.tobytes() == act_q.tobytes() and inact.tobytes() == inact_q.tobytes(), f"message {t}: clouds"
     assert found > n // 2
-    assert r.lst(SURFEL_DTYPE).tobytes() == q.lst(SURFEL_DTYPE).tobytes()
-    assert r.o == len(r.raw) and q.o == len(q.raw)
-    for ext in (".ply", ".pcd"):
-        assert filecmp.cmp(pa + ext, pb + ext, shallow=False), ext
+    twin_node_tail(r, q, pa, pb)

@@ -11,44 +11,29 @@ against its host-copy twin; the stream order against the next field request and 
 jobs beside publish snapshots and asynchronous checkpoints leaves everything as a twin without them; the rejected-frame
 and error contracts.  The node is checked through tests/cpp/gain_main.cpp."""
 import ctypes
-import filecmp
+from functools import partial
 
 import numpy as np
 import pytest
 
+import known_space
 import pyoracle_frontier
 import pyoracle_gain as G
-from densesurfelmapping_b200 import capi, synth
-from densesurfelmapping_b200.elements import POINT_DTYPE, SURFEL_DTYPE
+from densesurfelmapping_b200 import capi
+from densesurfelmapping_b200.elements import SURFEL_DTYPE
+from known_space import (FREE, K, OCCUPIED, RELOAD, SMALL_CAM, UNKNOWN, NODE_FIELD, assert_error_stays, gcam, known_drive,
+                         node_args, rejected, rejected_known, small_ctx, twin_clouds, twin_drive, twin_node_tail)
 from node_drive import node_script, run_driver
-from resident_map import SHAPES, STORE, T, camera, load_known, map_state, new_ctx, simple_lists, warp, windowed
-from test_gain_model import random_pose, symmetric_scene, symmetric_views, wall_scene, yaw_pose
-from test_gpu_field_known import MAX_RANGE, Views
+from planner_scenes import random_pose, symmetric_scene, symmetric_views, wall_scene, yaw_pose
+from resident_map import SHAPES, camera, load_known
 
 pytestmark = pytest.mark.gpu
 
-SMALL_CAM = synth.Camera(64, 48, 60.0, 60.0, 31.5, 23.5, 0.5, 30.0)
-K = synth.KITTI
-UNKNOWN, OCCUPIED, FREE = G.UNKNOWN, G.OCCUPIED, G.FREE
-
-
-def gcam(cam, max_range, unknown_blocks):
-    return G.Camera(cam.fx, cam.fy, cam.cx, cam.cy, cam.width, cam.height, float(np.float32(max_range)), unknown_blocks)
-
-
-def same(got, want, what):
-    gi, gg = got
-    wi, wg = want
-    assert gi.tobytes() == np.array(wi).tobytes(), f"{what}: header {gi} want {wi}"
-    bad = np.flatnonzero(gg != wg)
-    assert gg.tobytes() == wg.tobytes(), f"{what}: {len(bad)} records differ, first {bad[:4]}\n{gg[bad[:4]]}\nwant\n{wg[bad[:4]]}"
+same = partial(known_space.same, names=("header", "records"))
 
 
 def loader(shape, voxel=0.2, max_views=64, frontier_caps=(256, 1 << 18)):
-    ctx = capi.Context(SMALL_CAM, max_batch=2, max_local_surfels=1 << 12)
-    ctx.pool_upload(np.zeros(0, SURFEL_DTYPE))
-    ctx.field_enable(voxel, *shape)
-    ctx.views_enable(1, 1.0)
+    ctx = small_ctx(shape, voxel)
     ctx.frontier_enable(*frontier_caps)
     ctx.gain_enable(max_views)
     return ctx
@@ -249,37 +234,14 @@ def test_known_fields_of_the_drive(chunk, shape):
     """The windowed drive with loop-closure warps between calls; after every call a known field, its frontiers, a reach
     job from the camera to the clusters, and a gain job over eight yaws at each reached viewpoint and random poses,
     against the model on the field's own state grid; the same job on a resident twin of the request equals it."""
-    lists = simple_lists()
-    voxels = (0.125, 0.1, 0.3)
-    ctxs, views = {}, {}
-    for v in voxels:
-        ctxs[v] = new_ctx(store=STORE)
-        ctxs[v].field_enable(v, *shape)
-        views[v] = Views(ctxs[v], 6)
-        ctxs[v].frontier_enable(64, 1 << 16)
-        ctxs[v].reach_enable(16, 1 << 12, 2048)
-        ctxs[v].gain_enable(256)
+    def enable(c):
+        c.frontier_enable(64, 1 << 16)
+        c.reach_enable(16, 1 << 12, 2048)
+        c.gain_enable(256)
+
     rng = np.random.default_rng(chunk)
-    stored, seen = set(), 0
-    for call, t0 in enumerate(range(0, T, chunk)):
-        t1 = min(T, t0 + chunk)
-        for v in voxels:
-            windowed(ctxs[v], t0, t1, lists, want_counts=False)
-            views[v].capture_call(call, t0, t1)
-        for t in range(t0, t1):
-            stored = (stored | set(lists[t][1])) - set(lists[t][2])
-        if call % 2 == 1 and stored:
-            for v in voxels:
-                ctxs[v].pool_transform(warp(1))
-                ctxs[v].inactive_transform(max(stored), warp(2))
-                views[v].warp(warp(1))
-        v = voxels[call % 3]
-        ctx = ctxs[v]
-        slots, poses = views[v].request()
-        cam = camera(t1 - 1)
-        ctx.field_enqueue_known(cam, 5, slots, poses)
-        _, origin, _ = ctx.field_wait()
-        state, _ = ctx.field_state()
+    seen = 0
+    for call, t0, t1, ctx, v, cam, slots, poses, (_, origin, _), state in known_drive(shape, chunk, (0.125, 0.1, 0.3), enable):
         ctx.frontier_enqueue(1 + call % 3)
         fc, fv, _ = ctx.frontier_wait()
         ctx.reach_enqueue(cam, 0.0, 1, None, True)
@@ -306,102 +268,49 @@ def test_known_fields_of_the_drive(chunk, shape):
         twin = ctx.gain_wait()
         assert twin[0].tobytes() == got[0].tobytes() and twin[1].tobytes() == got[1].tobytes(), "resident twin"
     assert seen > 0 or shape == (1, 1, 1)
-    for c in ctxs.values():
-        c.close()
 
 
 def test_gain_jobs_change_nothing_else(tmp_path):
     """A drive with frontier, reach and gain jobs beside a publish snapshot and an asynchronous checkpoint leaves the
     map, both published clouds, the fields, the state grids, the frontiers, the reach results and the checkpoint files
     byte-identical to a twin without gain jobs."""
-    lists = simple_lists()
-    shape, voxel = (64, 64, 32), 0.1
-    a, b = new_ctx(store=STORE), new_ctx(store=STORE)
-    va, vb = {}, {}
-    for c, d in ((a, va), (b, vb)):
-        c.field_enable(voxel, *shape)
-        c.publish_enable()
-        c.checkpoint_enable()
-        d["v"] = Views(c, 4)
+    rng = np.random.default_rng(5)
+    job = {}
+
+    def enable_both(c):
         c.frontier_enable(32, 4096)
         c.reach_enable(16, 1 << 12, 1024)
-    a.gain_enable(64)
-    rng = np.random.default_rng(5)
-    stored = set()
-    for call, t0 in enumerate(range(0, T, 2)):
-        t1 = t0 + 2
-        for c, d in ((a, va), (b, vb)):
-            windowed(c, t0, t1, lists, want_counts=False)
-            d["v"].capture_call(call, t0, t1)
-        for t in range(t0, t1):
-            stored = (stored | set(lists[t][1])) - set(lists[t][2])
-        outs = []
-        gp = [random_pose(rng, camera(t1 - 1), 1.0) for _ in range(24)]
-        gc = gcam(K, 20 * voxel, call % 2)
-        for c, d in ((a, va), (b, vb)):
-            slots, poses = d["v"].request()
-            c.field_enqueue_known(camera(t1 - 1), 5, slots, poses)
-            c.frontier_enqueue(1)
-            c.reach_enqueue(camera(t1 - 1), 0.1, 2, [camera(0)], True)
-            if c is a:
-                a.gain_enqueue(gc, gp, np.arange(24, dtype=np.int32) - 1)
-            c.publish_enqueue(5)
-            c.checkpoint_enqueue(str(tmp_path / f"{'ab'[c is b]}{call}.dsm"))
-            if call % 2 == 1 and stored:
-                c.pool_transform(warp(1))
-                c.inactive_transform(max(stored), warp(2))
-                d["v"].warp(warp(1))
-            f = c.field_wait()
-            st = c.field_state()
-            fr = c.frontier_wait()
-            re = c.reach_wait()
-            p = c.publish_wait()
-            assert c.checkpoint_wait(True)
-            outs.append((f, st, p, fr, re))
-        got = a.gain_wait()
-        what = f"after frames {t0}-{t1 - 1}"
-        same(got, G.gains(outs[0][1][0], outs[0][0][1], voxel, gc, gp, np.arange(24) - 1, outs[0][3][:2]), what)
-        fa, fb = outs[0][0], outs[1][0]
-        assert fa[0].tobytes() == fb[0].tobytes() and outs[0][1][0].tobytes() == outs[1][1][0].tobytes(), f"{what}: field"
-        assert all(x.tobytes() == y.tobytes() for x, y in zip(outs[0][3], outs[1][3])), f"{what}: frontiers"
-        assert all(x.tobytes() == y.tobytes() for x, y in zip(outs[0][4][:3], outs[1][4][:3])), f"{what}: reach"
-        assert outs[0][2][0].tobytes() == outs[1][2][0].tobytes() and outs[0][2][1].tobytes() == outs[1][2][1].tobytes(), f"{what}: clouds"
-        assert map_state(a) == map_state(b), f"{what}: map"
-        assert filecmp.cmp(str(tmp_path / f"a{call}.dsm"), str(tmp_path / f"b{call}.dsm"), shallow=False), f"{what}: checkpoint"
-    a.close()
-    b.close()
+
+    def enqueue(c, is_a, call, t1):
+        c.frontier_enqueue(1)
+        c.reach_enqueue(camera(t1 - 1), 0.1, 2, [camera(0)], True)
+        if is_a:
+            job["gp"] = [random_pose(rng, camera(t1 - 1), 1.0) for _ in range(24)]
+            job["gc"] = gcam(K, 20 * 0.1, call % 2)
+            c.gain_enqueue(job["gc"], job["gp"], np.arange(24, dtype=np.int32) - 1)
+
+    def check(a, outs, call, t1, what):
+        same(a.gain_wait(), G.gains(outs["state"][0], outs["field"][1], 0.1, job["gc"], job["gp"], np.arange(24) - 1,
+                                    outs["shared"]["frontiers"][:2]), what)
+
+    twin_drive(tmp_path, enable_both, lambda a: a.gain_enable(64), enqueue,
+               lambda c: {"frontiers": c.frontier_wait(), "reach": c.reach_wait()}, check)
 
 
 def test_rejected_frame_comes_back_from_wait():
-    lists = simple_lists()
-    first = next(t for t in range(T) if lists[t][1])
-    shape, voxel = (64, 64, 32), 0.1
-    b = new_ctx(store=1)
-    b.field_enable(voxel, *shape)
-    views = Views(b, 4)
-    b.gain_enable(8)
-    for call, t0 in enumerate(range(0, first + 2)):
-        windowed(b, t0, t0 + 1, lists, want_counts=False)
-        views.capture_call(call, t0, t0 + 1)
-    slots, poses = views.request()
-    b.field_enqueue_known(camera(first - 1), 1, slots, poses)
-    gp = [yaw_pose(k, camera(first - 1)) for k in range(4)]
-    gc = gcam(K, 30 * voxel, 0)
-    b.gain_enqueue(gc, gp)
-    with pytest.raises(capi.DsmError) as e:
-        b.field_wait()
-    assert e.value.code == -6
-    _, origin, _ = e.value.field
-    state, _ = b.field_state()
-    with pytest.raises(capi.DsmError) as e:
-        b.gain_wait()
-    assert e.value.code == -6
-    same(e.value.gain, G.gains(state, origin, voxel, gc, gp), "rejected")
-    assert e.value.gain[1]["n_free"].sum() > 0
-    with pytest.raises(capi.DsmError) as e:
-        b.pool_size()
-    assert e.value.code == -6                            # wait did not clear it
-    b.close()
+    job = {}
+
+    def enqueue(b, first):
+        job["gp"] = [yaw_pose(k, camera(first - 1)) for k in range(4)]
+        job["gc"] = gcam(K, 30 * 0.1, 0)
+        b.gain_enqueue(job["gc"], job["gp"])
+
+    r = rejected_known(lambda b: b.gain_enable(8), enqueue)
+    e = rejected(r.ctx.gain_wait)
+    same(e.gain, G.gains(r.state, r.field[1], r.voxel, job["gc"], job["gp"]), "rejected")
+    assert e.gain[1]["n_free"].sum() > 0
+    assert_error_stays(r.ctx)
+    r.ctx.close()
 
 
 def test_error_contract():
@@ -473,23 +382,17 @@ def test_error_contract():
 
 
 # ---- the node ----
-FIELD = (0.2, 96, 96, 32)
-MAX_VIEWS = 5
-RELOAD = 12   # the node saves and loads its state after this depth message
-
-
 def test_node_view_gain_equals_the_model_and_changes_nothing(tmp_path):
     """The node drive (keyframes, loop closures): after every fused frame, frontiers() and view_gain() at eight yaws
     with named clusters equal the model over the grid, frontiers and poses the driver dumps; clouds, PLY and PCD files
     equal a twin without gain jobs; view_gain() with clusters before a frontiers() call on the frame, and after
     load_state until the next fused frame, returns DSM_E_STATE."""
-    cam, n = synth.KITTI, 24
+    cam, n = K, 24
     sc = node_script(cam, n)
-    voxel, nx, ny, nz = FIELD
+    voxel, nx, ny, nz = NODE_FIELD
     pa, pb = str(tmp_path / "mapa"), str(tmp_path / "mapb")
-    node = [2, 0, 1 << 20, 1 << 21, *FIELD, MAX_VIEWS, MAX_RANGE]
-    r = run_driver("gain_main", str(tmp_path), cam, sc, node + [64, RELOAD], tag="a", after=[pa])
-    q = run_driver("gain_main", str(tmp_path), cam, sc, node + [0, RELOAD], tag="b", after=[pb])
+    r = run_driver("gain_main", str(tmp_path), cam, sc, node_args() + [64, RELOAD], tag="a", after=[pa])
+    q = run_driver("gain_main", str(tmp_path), cam, sc, node_args() + [0, RELOAD], tag="b", after=[pb])
     found = 0
     for t in range(n):
         rc, ub = r.i(), r.i()
@@ -501,17 +404,12 @@ def test_node_view_gain_equals_the_model_and_changes_nothing(tmp_path):
         info = r.take(np.uint8, G.INFO_DTYPE.itemsize).view(G.INFO_DTYPE)[0].copy()
         gains = r.lst(G.GAIN_DTYPE)
         before, after_load = r.i(), r.i()
-        rr, act, inact = r.i(), r.lst(POINT_DTYPE), r.lst(POINT_DTYPE)
-        rq, act_q, inact_q = q.i(), q.lst(POINT_DTYPE), q.lst(POINT_DTYPE)
-        assert rc == 0 and rr == 0 and rq == 0, f"message {t}: {rc} {rr} {rq}"
+        twin_clouds(r, q, f"message {t}")
+        assert rc == 0, f"message {t}: {rc}"
         gc = G.Camera(cam.fx, cam.fy, cam.cx, cam.cy, cam.width, cam.height, max_range, ub)
         same((info, gains), G.gains(state, origin, voxel, gc, poses, named, (clusters, vox)), f"message {t}")
         found += int((gains["n_free"] > 0).sum()) > 0
         assert before == -7, f"message {t}: view_gain() before frontiers()"
         assert after_load == (-7 if t == RELOAD - 1 else 1), f"message {t}: view_gain() after load_state"
-        assert act.tobytes() == act_q.tobytes() and inact.tobytes() == inact_q.tobytes(), f"message {t}: clouds"
     assert found > 0
-    assert r.lst(SURFEL_DTYPE).tobytes() == q.lst(SURFEL_DTYPE).tobytes()
-    assert r.o == len(r.raw) and q.o == len(q.raw)
-    for ext in (".ply", ".pcd"):
-        assert filecmp.cmp(pa + ext, pb + ext, shallow=False), ext
+    twin_node_tail(r, q, pa, pb)

@@ -10,47 +10,31 @@ resident job equals its host-copy twin; the stream order against the next field 
 drive with reach jobs beside publish snapshots and asynchronous checkpoints leaves everything as a twin without them;
 the rejected-frame and error contracts.  The node is checked through tests/cpp/reach_main.cpp."""
 import ctypes
-import filecmp
+from functools import partial
 
 import numpy as np
 import pytest
 
+import known_space
 import pyoracle_frontier
 import pyoracle_reach as R
-from densesurfelmapping_b200 import capi, synth
-from densesurfelmapping_b200.elements import POINT_DTYPE, SURFEL_DTYPE
+from densesurfelmapping_b200 import capi
+from densesurfelmapping_b200.elements import SURFEL_DTYPE
+from known_space import (FREE, K, OCCUPIED, RELOAD, SMALL_CAM, UNKNOWN, NODE_FIELD, assert_error_stays, known_drive, node_args,
+                         rejected, rejected_known, small_ctx, twin_clouds, twin_drive, twin_node_tail)
 from node_drive import node_script, run_driver
-from resident_map import SHAPES, STORE, T, camera, load_known, map_state, new_ctx, simple_lists, warp, windowed
-from test_frontier_model import serpentine
-from test_gpu_field_known import MAX_RANGE, Views
+from planner_scenes import maze, serpentine
+from resident_map import SHAPES, camera, load_known
 
 pytestmark = pytest.mark.gpu
 
-SMALL_CAM = synth.Camera(64, 48, 60.0, 60.0, 31.5, 23.5, 0.5, 30.0)
 FRONTIER_CAPS = (256, 1 << 18)
-UNKNOWN, OCCUPIED, FREE = R.UNKNOWN, R.OCCUPIED, R.FREE
-
-
-def same(got, want, what, rounds=True):
-    gi, gt, gp, gc = got
-    wi, wt, wp, wc = want
-    gi, wi = gi.copy(), np.array(wi)
-    if not rounds:   # an exact oracle has no round count; the device's must say converged
-        assert gi["converged"] == 1, f"{what}: not converged in {gi['rounds']} rounds"
-        gi["rounds"], gi["converged"] = wi["rounds"], wi["converged"]
-    assert gi.tobytes() == wi.tobytes(), f"{what}: header {gi} want {wi}"
-    if gc is not None:
-        assert gc.tobytes() == wc.tobytes(), f"{what}: {(gc != wc).sum()} costs differ"
-    assert gt.tobytes() == wt.tobytes(), f"{what}: targets\n{gt}\nwant\n{wt}"
-    assert gp.tobytes() == wp.tobytes(), f"{what}: path list ({len(gp)} / {len(wp)})"
+same = partial(known_space.same, names=("header", "targets", "path list", "cost grid"))
 
 
 def loader(shape, voxel=0.2, caps=(64, 1 << 16), max_rounds=4096, frontier_caps=FRONTIER_CAPS):
     """A context whose field has grid `shape` (nx, ny, nz), with views, frontiers and reach jobs enabled."""
-    ctx = capi.Context(SMALL_CAM, max_batch=2, max_local_surfels=1 << 12)
-    ctx.pool_upload(np.zeros(0, SURFEL_DTYPE))
-    ctx.field_enable(voxel, *shape)
-    ctx.views_enable(1, 1.0)
+    ctx = small_ctx(shape, voxel)
     ctx.frontier_enable(*frontier_caps)
     ctx.reach_enable(*caps, max_rounds)
     ctx.caps = (caps, max_rounds, frontier_caps)
@@ -133,28 +117,6 @@ def test_random_grids_over_a_density_sweep():
             goals = [world(rng.integers(-2, np.array(shape) + 2), o, voxel) for _ in range(20)]
             loaded(ctx, st, o, voxel, start, radius, k, goals, with_frontiers=True, m=1 + k, what=f"density {p} r={radius} k={k}")
     ctx.close()
-
-
-def maze(n, seed):
-    """A perfect maze on an n x n lattice of cells, two voxels per cell, two voxels tall: one path between any two cells."""
-    rng = np.random.default_rng(seed)
-    st = np.full((2, 2 * n + 1, 2 * n + 1), OCCUPIED, np.uint8)
-    seen = np.zeros((n, n), bool)
-    stack = [(0, 0)]
-    seen[0, 0] = True
-    st[:, 1, 1] = FREE
-    while stack:
-        x, y = stack[-1]
-        nb = [(x + dx, y + dy) for dx, dy in ((1, 0), (-1, 0), (0, 1), (0, -1)) if 0 <= x + dx < n and 0 <= y + dy < n and not seen[y + dy, x + dx]]
-        if not nb:
-            stack.pop()
-            continue
-        a, b = nb[rng.integers(len(nb))]
-        seen[b, a] = True
-        st[:, 2 * b + 1, 2 * a + 1] = FREE
-        st[:, y + b + 1, x + a + 1] = FREE
-        stack.append((a, b))
-    return st
 
 
 def test_maze():
@@ -290,35 +252,12 @@ def test_stream_order():
 def test_known_fields_of_the_drive(chunk, shape):
     """The windowed drive with loop-closure warps between calls; after every call a known field, its frontiers and a
     reach job from the camera to the clusters and a few goals, against the model on the field's own grids."""
-    lists = simple_lists()
-    voxels = (0.125, 0.1, 0.3)
-    ctxs, views = {}, {}
-    for v in voxels:
-        ctxs[v] = new_ctx(store=STORE)
-        ctxs[v].field_enable(v, *shape)
-        views[v] = Views(ctxs[v], 6)
-        ctxs[v].frontier_enable(64, 1 << 16)
-        ctxs[v].reach_enable(96, 1 << 16, 2048)
-    stored, seen = set(), 0
-    for call, t0 in enumerate(range(0, T, chunk)):
-        t1 = min(T, t0 + chunk)
-        for v in voxels:
-            windowed(ctxs[v], t0, t1, lists, want_counts=False)
-            views[v].capture_call(call, t0, t1)
-        for t in range(t0, t1):
-            stored = (stored | set(lists[t][1])) - set(lists[t][2])
-        if call % 2 == 1 and stored:
-            for v in voxels:
-                ctxs[v].pool_transform(warp(1))
-                ctxs[v].inactive_transform(max(stored), warp(2))
-                views[v].warp(warp(1))
-        v = voxels[call % 3]
-        ctx = ctxs[v]
-        slots, poses = views[v].request()
-        ctx.field_enqueue_known(camera(t1 - 1), 5, slots, poses)
-        dist, origin, _ = ctx.field_wait()
-        state, _ = ctx.field_state()
-        cam = camera(t1 - 1)
+    def enable(c):
+        c.frontier_enable(64, 1 << 16)
+        c.reach_enable(96, 1 << 16, 2048)
+
+    seen = 0
+    for call, t0, t1, ctx, v, cam, _, _, (dist, origin, _), state in known_drive(shape, chunk, (0.125, 0.1, 0.3), enable):
         goals = [cam + d for d in ([1.0, 0, 0], [0, 1.0, 0.5], [-2.0, 0.3, 1.0], [0, 0, 0])]
         k, radius = call % 5, (0.0, v, 2 * v)[call % 3]
         ctx.caps = ((96, 1 << 16), 2048, (64, 1 << 16))
@@ -326,95 +265,40 @@ def test_known_fields_of_the_drive(chunk, shape):
         same(got, want, f"frames {t0}-{t1 - 1}, voxel {v}")
         seen += int((got[1]["status"] == 0).sum()) > 1
     assert seen > 0 or shape == (1, 1, 1)
-    for c in ctxs.values():
-        c.close()
 
 
 def test_reach_jobs_change_nothing_else(tmp_path):
     """A drive with frontier and reach jobs beside a publish snapshot and an asynchronous checkpoint leaves the map,
     both published clouds, the fields, the state grids, the frontiers and the checkpoint files byte-identical to a twin
     without reach jobs."""
-    lists = simple_lists()
-    shape, voxel = (64, 64, 32), 0.1
-    a, b = new_ctx(store=STORE), new_ctx(store=STORE)
-    va, vb = {}, {}
-    for c, d in ((a, va), (b, vb)):
-        c.field_enable(voxel, *shape)
-        c.publish_enable()
-        c.checkpoint_enable()
-        d["v"] = Views(c, 4)
-        c.frontier_enable(32, 4096)
-    a.reach_enable(64, 1 << 14, 1024)
-    stored = set()
-    for call, t0 in enumerate(range(0, T, 2)):
-        t1 = t0 + 2
-        for c, d in ((a, va), (b, vb)):
-            windowed(c, t0, t1, lists, want_counts=False)
-            d["v"].capture_call(call, t0, t1)
-        for t in range(t0, t1):
-            stored = (stored | set(lists[t][1])) - set(lists[t][2])
-        outs = []
-        for c, d in ((a, va), (b, vb)):
-            slots, poses = d["v"].request()
-            c.field_enqueue_known(camera(t1 - 1), 5, slots, poses)
-            c.frontier_enqueue(1)
-            if c is a:
-                a.reach_enqueue(camera(t1 - 1), 0.1, 2, [camera(0)], True, call % 2 == 0)
-            c.publish_enqueue(5)
-            c.checkpoint_enqueue(str(tmp_path / f"{'ab'[c is b]}{call}.dsm"))
-            if call % 2 == 1 and stored:
-                c.pool_transform(warp(1))
-                c.inactive_transform(max(stored), warp(2))
-                d["v"].warp(warp(1))
-            f = c.field_wait()
-            st = c.field_state()
-            fr = c.frontier_wait()
-            p = c.publish_wait()
-            assert c.checkpoint_wait(True)
-            outs.append((f, st, p, fr))
-        got = a.reach_wait()
-        fa, fb = outs[0][0], outs[1][0]
-        what = f"after frames {t0}-{t1 - 1}"
-        want = R.reach(outs[0][1][0], fa[0], fa[1], voxel, camera(t1 - 1), 0.1, 2, [camera(0)], outs[0][3][:2], 64, 1 << 14, 1024)
-        same(got, want, what)
-        assert fa[0].tobytes() == fb[0].tobytes() and outs[0][1][0].tobytes() == outs[1][1][0].tobytes(), f"{what}: field"
-        assert all(x.tobytes() == y.tobytes() for x, y in zip(outs[0][3], outs[1][3])), f"{what}: frontiers"
-        assert outs[0][2][0].tobytes() == outs[1][2][0].tobytes() and outs[0][2][1].tobytes() == outs[1][2][1].tobytes(), f"{what}: clouds"
-        assert map_state(a) == map_state(b), f"{what}: map"
-        assert filecmp.cmp(str(tmp_path / f"a{call}.dsm"), str(tmp_path / f"b{call}.dsm"), shallow=False), f"{what}: checkpoint"
-    a.close()
-    b.close()
+    def enqueue(c, is_a, call, t1):
+        c.frontier_enqueue(1)
+        if is_a:
+            c.reach_enqueue(camera(t1 - 1), 0.1, 2, [camera(0)], True, call % 2 == 0)
+
+    def check(a, outs, call, t1, what):
+        want = R.reach(outs["state"][0], outs["field"][0], outs["field"][1], 0.1, camera(t1 - 1), 0.1, 2, [camera(0)],
+                       outs["shared"]["frontiers"][:2], 64, 1 << 14, 1024)
+        same(a.reach_wait(), want, what)
+
+    twin_drive(tmp_path, lambda c: c.frontier_enable(32, 4096), lambda a: a.reach_enable(64, 1 << 14, 1024), enqueue,
+               lambda c: {"frontiers": c.frontier_wait()}, check)
 
 
 def test_rejected_frame_comes_back_from_wait():
-    lists = simple_lists()
-    first = next(t for t in range(T) if lists[t][1])
-    shape, voxel = (64, 64, 32), 0.1
-    b = new_ctx(store=1)
-    b.field_enable(voxel, *shape)
-    views = Views(b, 4)
-    b.reach_enable(8, 1 << 12, 512)
-    for call, t0 in enumerate(range(0, first + 2)):
-        windowed(b, t0, t0 + 1, lists, want_counts=False)
-        views.capture_call(call, t0, t0 + 1)
-    slots, poses = views.request()
-    b.field_enqueue_known(camera(first - 1), 1, slots, poses)
-    goals = [camera(0), camera(first - 1) + 1.0]
-    b.reach_enqueue(camera(first - 1), 0.0, 1, goals, False, True)
-    with pytest.raises(capi.DsmError) as e:
-        b.field_wait()
-    assert e.value.code == -6
-    dist, origin, _ = e.value.field
-    state, _ = b.field_state()
-    with pytest.raises(capi.DsmError) as e:
-        b.reach_wait()
-    assert e.value.code == -6
-    same(e.value.reach, R.reach(state, dist, origin, voxel, camera(first - 1), 0.0, 1, goals, None, 8, 1 << 12, 512), "rejected")
-    assert e.value.reach[0]["n_reached"] > 0
-    with pytest.raises(capi.DsmError) as e:
-        b.pool_size()
-    assert e.value.code == -6                            # wait did not clear it
-    b.close()
+    goals = []
+
+    def enqueue(b, first):
+        goals.extend([camera(0), camera(first - 1) + 1.0])
+        b.reach_enqueue(camera(first - 1), 0.0, 1, goals, False, True)
+
+    r = rejected_known(lambda b: b.reach_enable(8, 1 << 12, 512), enqueue)
+    dist, origin, _ = r.field
+    e = rejected(r.ctx.reach_wait)
+    same(e.reach, R.reach(r.state, dist, origin, r.voxel, camera(r.first - 1), 0.0, 1, goals, None, 8, 1 << 12, 512), "rejected")
+    assert e.reach[0]["n_reached"] > 0
+    assert_error_stays(r.ctx)
+    r.ctx.close()
 
 
 def test_error_contract():
@@ -462,23 +346,17 @@ def test_error_contract():
 
 
 # ---- the node ----
-FIELD = (0.2, 96, 96, 32)
-MAX_VIEWS = 5
-RELOAD = 12   # the node saves and loads its state after this depth message
-
-
 def test_node_reach_equals_the_model_and_changes_nothing(tmp_path):
     """The node drive (keyframes, loop closures): after every fused frame, frontiers() and reach(with_frontiers) from
     the camera equal the model over the grids the driver dumps; clouds, PLY and PCD files equal a twin without reach
     jobs; reach() without a frontiers() call on the frame, and after load_state until the next fused frame, returns
     DSM_E_STATE."""
-    cam, n = synth.KITTI, 24
+    cam, n = K, 24
     sc = node_script(cam, n)
-    voxel, nx, ny, nz = FIELD
+    voxel, nx, ny, nz = NODE_FIELD
     pa, pb = str(tmp_path / "mapa"), str(tmp_path / "mapb")
-    node = [2, 0, 1 << 20, 1 << 21, *FIELD, MAX_VIEWS, MAX_RANGE]
-    r = run_driver("reach_main", str(tmp_path), cam, sc, node + [64, 1 << 16, 2048, RELOAD], tag="a", after=[pa])
-    q = run_driver("reach_main", str(tmp_path), cam, sc, node + [0, 0, 0, RELOAD], tag="b", after=[pb])
+    r = run_driver("reach_main", str(tmp_path), cam, sc, node_args() + [64, 1 << 16, 2048, RELOAD], tag="a", after=[pa])
+    q = run_driver("reach_main", str(tmp_path), cam, sc, node_args() + [0, 0, 0, RELOAD], tag="b", after=[pb])
     found = 0
     for t in range(n):
         rc, k = r.i(), r.i()
@@ -491,17 +369,12 @@ def test_node_reach_equals_the_model_and_changes_nothing(tmp_path):
         info = r.take(np.uint8, R.INFO_DTYPE.itemsize).view(R.INFO_DTYPE)[0].copy()
         targets, path = r.lst(R.TARGET_DTYPE), r.lst(np.int32)
         before, after_load = r.i(), r.i()
-        rr, act, inact = r.i(), r.lst(POINT_DTYPE), r.lst(POINT_DTYPE)
-        rq, act_q, inact_q = q.i(), q.lst(POINT_DTYPE), q.lst(POINT_DTYPE)
-        assert rc == 0 and rr == 0 and rq == 0, f"message {t}: {rc} {rr} {rq}"
+        twin_clouds(r, q, f"message {t}")
+        assert rc == 0, f"message {t}: {rc}"
         want = R.reach(state, dist, origin, voxel, start, radius, k, (), (clusters, vox), 64, 1 << 16, 2048)
         same((info, targets, path, None), want, f"message {t}")
         found += int((targets["status"] == 0).sum()) > 0
         assert before == -7, f"message {t}: reach() before frontiers()"
         assert after_load == (-7 if t == RELOAD - 1 else 1), f"message {t}: reach() after load_state"
-        assert act.tobytes() == act_q.tobytes() and inact.tobytes() == inact_q.tobytes(), f"message {t}: clouds"
     assert found > 0
-    assert r.lst(SURFEL_DTYPE).tobytes() == q.lst(SURFEL_DTYPE).tobytes()
-    assert r.o == len(r.raw) and q.o == len(q.raw)
-    for ext in (".ply", ".pcd"):
-        assert filecmp.cmp(pa + ext, pb + ext, shallow=False), ext
+    twin_node_tail(r, q, pa, pb)

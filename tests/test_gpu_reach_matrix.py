@@ -9,44 +9,32 @@ host-copy cost grid of a dsm_reach job started at site i, read at the sites, wit
 n_reached, converged and unconverged.  Both sides of the capacity cut, stream order against the next field request, a
 drive with matrix jobs beside publish snapshots, checkpoints and reach jobs against a twin without them, the rejected
 frame and every error code.  The node is checked through tests/cpp/reach_matrix_main.cpp."""
-import ctypes
-import filecmp
+from functools import partial
 
 import numpy as np
 import pytest
 from scipy.sparse import csgraph
 
+import known_space
 import pyoracle_reach as R
 import pyoracle_reach_matrix as RM
-from densesurfelmapping_b200 import capi, synth
-from densesurfelmapping_b200.elements import POINT_DTYPE, SURFEL_DTYPE
+from densesurfelmapping_b200 import capi
+from densesurfelmapping_b200.elements import SURFEL_DTYPE
+from known_space import (FREE, K, OCCUPIED, RELOAD, SMALL_CAM, NODE_FIELD, assert_error_stays, known_drive, node_args, rejected,
+                         rejected_known, small_ctx, twin_clouds, twin_drive, twin_node_tail)
 from node_drive import node_script, run_driver
-from resident_map import SHAPES, STORE, T, camera, load_known, map_state, new_ctx, simple_lists, warp, windowed
-from test_frontier_model import serpentine
-from test_gpu_field_known import MAX_RANGE, Views
-from test_gpu_reach import maze
+from planner_scenes import maze, serpentine
+from resident_map import SHAPES, camera, load_known
 
 pytestmark = pytest.mark.gpu
 
-SMALL_CAM = synth.Camera(64, 48, 60.0, 60.0, 31.5, 23.5, 0.5, 30.0)
-UNKNOWN, OCCUPIED, FREE = R.UNKNOWN, R.OCCUPIED, R.FREE
-
-
-def same(got, want, what):
-    gi, gs, gm = got
-    wi, ws, wm = want
-    assert gi.tobytes() == np.array(wi).tobytes(), f"{what}: header {gi} want {wi}"
-    assert gs.tobytes() == ws.tobytes(), f"{what}: sites\n{gs}\nwant\n{ws}"
-    assert gm.tobytes() == wm.tobytes(), f"{what}: {(gm != wm).sum()} of {gm.size} matrix entries differ"
+same = partial(known_space.same, names=("header", "sites", "matrix"))
 
 
 def loader(shape, voxel=0.2, max_sites=64, max_tiles=None, max_rounds=4096, reach=None):
     """A context whose field has grid `shape` (nx, ny, nz), with views and matrix jobs enabled (max_tiles: every tile),
     and reach jobs with `reach` = (max_targets, max_path, max_rounds) capacities."""
-    ctx = capi.Context(SMALL_CAM, max_batch=2, max_local_surfels=1 << 12)
-    ctx.pool_upload(np.zeros(0, SURFEL_DTYPE))
-    ctx.field_enable(voxel, *shape)
-    ctx.views_enable(1, 1.0)
+    ctx = small_ctx(shape, voxel)
     tiles = int(np.prod([(n + 7) // 8 for n in shape]))
     ctx.reach_matrix_enable(max_sites, tiles if max_tiles is None else max_tiles, max_rounds)
     if reach:
@@ -232,38 +220,16 @@ def test_known_fields_of_the_drive(chunk, shape):
     """The windowed drive with loop-closure warps between calls; after every call a known field, its frontiers, a reach
     job from the camera to the clusters, and a matrix job over the field's centre, the reached viewpoints and random
     points, against the model on the field's own grids; the same job on a resident twin of the request equals it."""
-    lists = simple_lists()
-    voxels = (0.125, 0.1, 0.3)
-    ctxs, views = {}, {}
     tiles = int(np.prod([(n + 7) // 8 for n in shape]))
-    for v in voxels:
-        ctxs[v] = new_ctx(store=STORE)
-        ctxs[v].field_enable(v, *shape)
-        views[v] = Views(ctxs[v], 6)
-        ctxs[v].frontier_enable(64, 1 << 16)
-        ctxs[v].reach_enable(16, 1 << 12, 2048)
-        ctxs[v].reach_matrix_enable(16, tiles, 2048)
+
+    def enable(c):
+        c.frontier_enable(64, 1 << 16)
+        c.reach_enable(16, 1 << 12, 2048)
+        c.reach_matrix_enable(16, tiles, 2048)
+
     rng = np.random.default_rng(chunk)
-    stored, seen = set(), 0
-    for call, t0 in enumerate(range(0, T, chunk)):
-        t1 = min(T, t0 + chunk)
-        for v in voxels:
-            windowed(ctxs[v], t0, t1, lists, want_counts=False)
-            views[v].capture_call(call, t0, t1)
-        for t in range(t0, t1):
-            stored = (stored | set(lists[t][1])) - set(lists[t][2])
-        if call % 2 == 1 and stored:
-            for v in voxels:
-                ctxs[v].pool_transform(warp(1))
-                ctxs[v].inactive_transform(max(stored), warp(2))
-                views[v].warp(warp(1))
-        v = voxels[call % 3]
-        ctx = ctxs[v]
-        slots, poses = views[v].request()
-        cam = camera(t1 - 1)
-        ctx.field_enqueue_known(cam, 5, slots, poses)
-        dist, origin, _ = ctx.field_wait()
-        state, _ = ctx.field_state()
+    seen = 0
+    for call, t0, t1, ctx, v, cam, slots, poses, (dist, origin, _), state in known_drive(shape, chunk, (0.125, 0.1, 0.3), enable):
         ctx.frontier_enqueue(1 + call % 3)
         ctx.frontier_wait()
         ctx.reach_enqueue(cam, 0.0, 1, None, True)
@@ -283,99 +249,44 @@ def test_known_fields_of_the_drive(chunk, shape):
         twin = ctx.reach_matrix_wait()
         assert all(x.tobytes() == y.tobytes() for x, y in zip(twin, got)), "resident twin"
     assert seen > 0 or shape == (1, 1, 1)
-    for c in ctxs.values():
-        c.close()
 
 
 def test_matrix_jobs_change_nothing_else(tmp_path):
     """A drive with frontier, reach and matrix jobs beside a publish snapshot and an asynchronous checkpoint leaves the
     map, both published clouds, the fields, the state grids, the frontiers, the reach results and the checkpoint files
     byte-identical to a twin without matrix jobs."""
-    lists = simple_lists()
-    shape, voxel = (64, 64, 32), 0.1
-    a, b = new_ctx(store=STORE), new_ctx(store=STORE)
-    va, vb = {}, {}
-    for c, d in ((a, va), (b, vb)):
-        c.field_enable(voxel, *shape)
-        c.publish_enable()
-        c.checkpoint_enable()
-        d["v"] = Views(c, 4)
+    def enable_both(c):
         c.frontier_enable(32, 4096)
         c.reach_enable(64, 1 << 14, 1024)
-    a.reach_matrix_enable(8, 8 * 8 * 4, 1024)
-    stored = set()
-    for call, t0 in enumerate(range(0, T, 2)):
-        t1 = t0 + 2
-        for c, d in ((a, va), (b, vb)):
-            windowed(c, t0, t1, lists, want_counts=False)
-            d["v"].capture_call(call, t0, t1)
-        for t in range(t0, t1):
-            stored = (stored | set(lists[t][1])) - set(lists[t][2])
-        outs = []
+
+    def enqueue(c, is_a, call, t1):
+        c.frontier_enqueue(1)
+        if is_a:
+            c.reach_matrix_enqueue([camera(t) for t in range(t1)][-8:], 0.1, 2)
+        c.reach_enqueue(camera(t1 - 1), 0.1, 2, [camera(0)], True, True)
+
+    def check(a, outs, call, t1, what):
         pts = [camera(t) for t in range(t1)][-8:]
-        for c, d in ((a, va), (b, vb)):
-            slots, poses = d["v"].request()
-            c.field_enqueue_known(camera(t1 - 1), 5, slots, poses)
-            c.frontier_enqueue(1)
-            if c is a:
-                a.reach_matrix_enqueue(pts, 0.1, 2)
-            c.reach_enqueue(camera(t1 - 1), 0.1, 2, [camera(0)], True, True)
-            c.publish_enqueue(5)
-            c.checkpoint_enqueue(str(tmp_path / f"{'ab'[c is b]}{call}.dsm"))
-            if call % 2 == 1 and stored:
-                c.pool_transform(warp(1))
-                c.inactive_transform(max(stored), warp(2))
-                d["v"].warp(warp(1))
-            f = c.field_wait()
-            st = c.field_state()
-            fr = c.frontier_wait()
-            re = c.reach_wait()
-            p = c.publish_wait()
-            assert c.checkpoint_wait(True)
-            outs.append((f, st, p, fr, re))
-        got = a.reach_matrix_wait()
-        fa, fb = outs[0][0], outs[1][0]
-        what = f"after frames {t0}-{t1 - 1}"
-        same(got, RM.matrix(outs[0][1][0], fa[0], fa[1], voxel, pts, 0.1, 2, 8 * 8 * 4, 1024), what)
-        assert fa[0].tobytes() == fb[0].tobytes() and outs[0][1][0].tobytes() == outs[1][1][0].tobytes(), f"{what}: field"
-        assert all(x.tobytes() == y.tobytes() for x, y in zip(outs[0][3], outs[1][3])), f"{what}: frontiers"
-        assert all(x.tobytes() == y.tobytes() for x, y in zip(outs[0][4], outs[1][4])), f"{what}: reach"
-        assert outs[0][2][0].tobytes() == outs[1][2][0].tobytes() and outs[0][2][1].tobytes() == outs[1][2][1].tobytes(), f"{what}: clouds"
-        assert map_state(a) == map_state(b), f"{what}: map"
-        assert filecmp.cmp(str(tmp_path / f"a{call}.dsm"), str(tmp_path / f"b{call}.dsm"), shallow=False), f"{what}: checkpoint"
-    a.close()
-    b.close()
+        same(a.reach_matrix_wait(), RM.matrix(outs["state"][0], outs["field"][0], outs["field"][1], 0.1, pts, 0.1, 2, 8 * 8 * 4, 1024), what)
+
+    twin_drive(tmp_path, enable_both, lambda a: a.reach_matrix_enable(8, 8 * 8 * 4, 1024), enqueue,
+               lambda c: {"frontiers": c.frontier_wait(), "reach": c.reach_wait()}, check)
 
 
 def test_rejected_frame_comes_back_from_wait():
-    lists = simple_lists()
-    first = next(t for t in range(T) if lists[t][1])
-    shape, voxel = (64, 64, 32), 0.1
-    b = new_ctx(store=1)
-    b.field_enable(voxel, *shape)
-    views = Views(b, 4)
-    b.reach_matrix_enable(4, 8 * 8 * 4, 512)
-    for call, t0 in enumerate(range(0, first + 2)):
-        windowed(b, t0, t0 + 1, lists, want_counts=False)
-        views.capture_call(call, t0, t0 + 1)
-    slots, poses = views.request()
-    b.field_enqueue_known(camera(first - 1), 1, slots, poses)
-    pts = [camera(0), camera(first - 1), camera(first - 1) + 1.0]
-    b.reach_matrix_enqueue(pts, 0.0, 1)
-    with pytest.raises(capi.DsmError) as e:
-        b.field_wait()
-    assert e.value.code == -6
-    dist, origin, _ = e.value.field
-    state, _ = b.field_state()
-    with pytest.raises(capi.DsmError) as e:
-        b.reach_matrix_wait()
-    assert e.value.code == -6
-    same(e.value.reach_matrix, RM.matrix(state, dist, origin, voxel, pts, 0.0, 1, 8 * 8 * 4, 512), "rejected")
-    assert (e.value.reach_matrix[1]["n_reached"] > 0).any()
-    with pytest.raises(capi.DsmError) as e:
-        b.pool_size()
-    assert e.value.code == -6                            # wait did not clear it
-    b.close()
+    pts = []
+
+    def enqueue(b, first):
+        pts.extend([camera(0), camera(first - 1), camera(first - 1) + 1.0])
+        b.reach_matrix_enqueue(pts, 0.0, 1)
+
+    r = rejected_known(lambda b: b.reach_matrix_enable(4, 8 * 8 * 4, 512), enqueue)
+    dist, origin, _ = r.field
+    e = rejected(r.ctx.reach_matrix_wait)
+    same(e.reach_matrix, RM.matrix(r.state, dist, origin, r.voxel, pts, 0.0, 1, 8 * 8 * 4, 512), "rejected")
+    assert (e.reach_matrix[1]["n_reached"] > 0).any()
+    assert_error_stays(r.ctx)
+    r.ctx.close()
 
 
 def test_error_contract():
@@ -438,24 +349,18 @@ def test_error_contract():
 
 
 # ---- the node ----
-FIELD = (0.2, 96, 96, 32)
-MAX_VIEWS = 5
-RELOAD = 12   # the node saves and loads its state after this depth message
-
-
 def test_node_reach_matrix_equals_the_model_and_changes_nothing(tmp_path):
     """The node drive (keyframes, loop closures): after every fused frame, frontiers(), reach(with_frontiers) from the
     field's centre and reach_matrix over that point and the reached viewpoints: the snaps equal the model's and the
     converged matrix equals Dijkstra's over the grids the driver dumps; clouds, PLY and PCD files equal a twin without matrix jobs; reach_matrix after load_state until the
     next fused frame returns DSM_E_STATE."""
-    cam, n = synth.KITTI, 24
+    cam, n = K, 24
     sc = node_script(cam, n)
-    voxel, nx, ny, nz = FIELD
+    voxel, nx, ny, nz = NODE_FIELD
     pa, pb = str(tmp_path / "mapa"), str(tmp_path / "mapb")
-    node = [2, 0, 1 << 20, 1 << 21, *FIELD, MAX_VIEWS, MAX_RANGE]
     tiles = 12 * 12 * 4
-    r = run_driver("reach_matrix_main", str(tmp_path), cam, sc, node + [32, tiles, 2048, RELOAD], tag="a", after=[pa])
-    q = run_driver("reach_matrix_main", str(tmp_path), cam, sc, node + [0, 0, 0, RELOAD], tag="b", after=[pb])
+    r = run_driver("reach_matrix_main", str(tmp_path), cam, sc, node_args() + [32, tiles, 2048, RELOAD], tag="a", after=[pa])
+    q = run_driver("reach_matrix_main", str(tmp_path), cam, sc, node_args() + [0, 0, 0, RELOAD], tag="b", after=[pb])
     found = 0
     for t in range(n):
         rc, k = r.i(), r.i()
@@ -468,9 +373,8 @@ def test_node_reach_matrix_equals_the_model_and_changes_nothing(tmp_path):
         sites = r.lst(RM.SITE_DTYPE)
         m = r.lst(np.uint32)
         after_load = r.i()
-        rr, act, inact = r.i(), r.lst(POINT_DTYPE), r.lst(POINT_DTYPE)
-        rq, act_q, inact_q = q.i(), q.lst(POINT_DTYPE), q.lst(POINT_DTYPE)
-        assert rc == 0 and rr == 0 and rq == 0, f"message {t}: {rc} {rr} {rq}"
+        twin_clouds(r, q, f"message {t}")
+        assert rc == 0, f"message {t}: {rc}"
         # every job converges well within 2048 rounds here, so the model's rows are Dijkstra's (emulating each row on the
         # host would take minutes per drive)
         what = f"message {t}"
@@ -485,9 +389,5 @@ def test_node_reach_matrix_equals_the_model_and_changes_nothing(tmp_path):
         assert m.tobytes() == want.tobytes(), f"{what}: {(m.reshape(want.shape) != want).sum()} entries differ"
         found += int((m != R.INF).sum()) > len(sites)
         assert after_load == (-7 if t == RELOAD - 1 else 1), f"message {t}: reach_matrix() after load_state"
-        assert act.tobytes() == act_q.tobytes() and inact.tobytes() == inact_q.tobytes(), f"message {t}: clouds"
     assert found > 0
-    assert r.lst(SURFEL_DTYPE).tobytes() == q.lst(SURFEL_DTYPE).tobytes()
-    assert r.o == len(r.raw) and q.o == len(q.raw)
-    for ext in (".ply", ".pcd"):
-        assert filecmp.cmp(pa + ext, pb + ext, shallow=False), ext
+    twin_node_tail(r, q, pa, pb)

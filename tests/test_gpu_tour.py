@@ -7,24 +7,21 @@ without UINT32_MAX entries, open and closed; on symmetric and stretched metric m
 max_starts; on the matrices of matrix jobs over the windowed drive's known fields.  One job in flight, a wait that
 waits for its own job only, a drive with tour jobs beside publish snapshots, checkpoints and matrix jobs against a twin
 without them, and every error code.  The node is checked through tests/cpp/tour_main.cpp."""
-import filecmp
+from functools import partial
 
 import numpy as np
 import pytest
 
+import known_space
 import pyoracle_reach_matrix as RM
 import pyoracle_tour as TM
-from densesurfelmapping_b200 import capi, synth
-from densesurfelmapping_b200.elements import SURFEL_DTYPE
+from densesurfelmapping_b200 import capi
+from known_space import K, SMALL_CAM, known_drive, node_args, small_ctx, twin_drive
 from node_drive import node_script, run_driver
-from resident_map import STORE, T, camera, map_state, new_ctx, simple_lists, warp, windowed
-from test_gpu_field_known import MAX_RANGE, Views
-from test_tour_model import metric_matrix, random_matrix
+from planner_scenes import metric_matrix, random_matrix
+from resident_map import camera
 
 pytestmark = pytest.mark.gpu
-
-SMALL_CAM = synth.Camera(64, 48, 60.0, 60.0, 31.5, 23.5, 0.5, 30.0)
-
 
 def context(max_sites, max_starts):
     ctx = capi.Context(SMALL_CAM, max_batch=2, max_local_surfels=1 << 12)
@@ -32,12 +29,7 @@ def context(max_sites, max_starts):
     return ctx
 
 
-def same(got, want, what):
-    gi, gs, go = got
-    wi, ws, wo = want
-    assert gi.tobytes() == np.array(wi).tobytes(), f"{what}: header {gi} want {wi}"
-    assert gs.tobytes() == ws.tobytes(), f"{what}: starts\n{gs}\nwant\n{ws}"
-    assert go.tobytes() == wo.tobytes(), f"{what}: order\n{go}\nwant\n{wo}"
+same = partial(known_space.same, names=("header", "starts", "order"))
 
 
 def job(ctx, M, open_, n_starts, max_passes, seed, what=""):
@@ -94,28 +86,16 @@ def test_matrices_of_the_drive():
     """The windowed drive with loop-closure warps: after every call a known field, its frontiers, a reach job from the
     camera to the clusters and a matrix job over the camera, the field's centre and the reached viewpoints; the tour
     over that matrix as it stands equals the model, open and closed."""
-    lists = simple_lists()
     shape, v = (64, 64, 32), 0.1
-    ctx = new_ctx(store=STORE)
-    ctx.field_enable(v, *shape)
-    views = Views(ctx, 6)
-    ctx.frontier_enable(64, 1 << 16)
-    ctx.reach_enable(31, 1 << 12, 2048)
-    ctx.reach_matrix_enable(32, 8 * 8 * 4, 2048)
-    ctx.tour_enable(32, 64)
-    stored, seen = set(), 0
-    for call, t0 in enumerate(range(0, T, 2)):
-        t1 = t0 + 2
-        windowed(ctx, t0, t1, lists, want_counts=False)
-        views.capture_call(call, t0, t1)
-        for t in range(t0, t1):
-            stored = (stored | set(lists[t][1])) - set(lists[t][2])
-        if call % 2 == 1 and stored:
-            ctx.pool_transform(warp(1))
-            ctx.inactive_transform(max(stored), warp(2))
-            views.warp(warp(1))
-        slots, poses = views.request()
-        cam = camera(t1 - 1)
+
+    def enable(c):
+        c.frontier_enable(64, 1 << 16)
+        c.reach_enable(31, 1 << 12, 2048)
+        c.reach_matrix_enable(32, 8 * 8 * 4, 2048)
+        c.tour_enable(32, 64)
+
+    seen = 0
+    for call, _, _, ctx, _, cam, slots, poses, _, _ in known_drive(shape, 2, (v,), enable, request=False):
         ctx.field_enqueue_known(cam, 5, slots, poses)
         _, origin, _ = ctx.field_wait()
         ctx.frontier_enqueue(1)
@@ -132,14 +112,10 @@ def test_matrices_of_the_drive():
             got = job(ctx, M, open_, 64, 256, call, f"call {call} open={open_}")
             seen += int(got[0]["n_included"]) > 3
     assert seen > 0
-    ctx.close()
 
 
 def test_one_job_in_flight_and_its_own_wait():
-    ctx = capi.Context(SMALL_CAM, max_batch=2, max_local_surfels=1 << 12)
-    ctx.pool_upload(np.zeros(0, SURFEL_DTYPE))
-    ctx.field_enable(0.2, 40, 30, 20)
-    ctx.views_enable(1, 1.0)
+    ctx = small_ctx((40, 30, 20), 0.2)
     ctx.reach_matrix_enable(8, 5 * 4 * 3, 256)
     ctx.tour_enable(64, 8)
     rng = np.random.default_rng(2)
@@ -169,64 +145,27 @@ def test_tour_jobs_change_nothing_else(tmp_path):
     """A drive with frontier, reach and matrix jobs beside a publish snapshot and an asynchronous checkpoint, with tour
     jobs enqueued among them, leaves the map, the clouds, the fields, the frontiers, the reach and matrix results and the
     checkpoint files byte-identical to a twin without tour jobs."""
-    lists = simple_lists()
-    shape, voxel = (64, 64, 32), 0.1
-    a, b = new_ctx(store=STORE), new_ctx(store=STORE)
-    va, vb = {}, {}
-    for c, d in ((a, va), (b, vb)):
-        c.field_enable(voxel, *shape)
-        c.publish_enable()
-        c.checkpoint_enable()
-        d["v"] = Views(c, 4)
+    rng = np.random.default_rng(4)
+    job = {}
+
+    def enable_both(c):
         c.frontier_enable(32, 4096)
         c.reach_enable(64, 1 << 14, 1024)
         c.reach_matrix_enable(8, 8 * 8 * 4, 1024)
-    a.tour_enable(256, 16)
-    rng = np.random.default_rng(4)
-    stored = set()
-    for call, t0 in enumerate(range(0, T, 2)):
-        t1 = t0 + 2
-        for c, d in ((a, va), (b, vb)):
-            windowed(c, t0, t1, lists, want_counts=False)
-            d["v"].capture_call(call, t0, t1)
-        for t in range(t0, t1):
-            stored = (stored | set(lists[t][1])) - set(lists[t][2])
-        outs = []
-        pts = [camera(t) for t in range(t1)][-8:]
-        M = random_matrix(256, rng, 0.01)
-        for c, d in ((a, va), (b, vb)):
-            slots, poses = d["v"].request()
-            c.field_enqueue_known(camera(t1 - 1), 5, slots, poses)
-            c.frontier_enqueue(1)
-            c.reach_matrix_enqueue(pts, 0.1, 2)
-            if c is a:
-                a.tour_enqueue(M, call % 2, 16, 64, call)
-            c.reach_enqueue(camera(t1 - 1), 0.1, 2, [camera(0)], True, True)
-            c.publish_enqueue(5)
-            c.checkpoint_enqueue(str(tmp_path / f"{'ab'[c is b]}{call}.dsm"))
-            if call % 2 == 1 and stored:
-                c.pool_transform(warp(1))
-                c.inactive_transform(max(stored), warp(2))
-                d["v"].warp(warp(1))
-            f = c.field_wait()
-            st = c.field_state()
-            fr = c.frontier_wait()
-            rm = c.reach_matrix_wait()
-            re = c.reach_wait()
-            p = c.publish_wait()
-            assert c.checkpoint_wait(True)
-            outs.append((f, st, p, fr, re, rm))
-        what = f"after frames {t0}-{t1 - 1}"
-        same(a.tour_wait(), TM.tour(M, call % 2, 16, 64, call), what)
-        (fa, sa, pa, fra, rea, rma), (fb, sb, pb, frb, reb, rmb) = outs
-        assert fa[0].tobytes() == fb[0].tobytes() and sa[0].tobytes() == sb[0].tobytes(), f"{what}: field"
-        for x, y, name in ((fra, frb, "frontiers"), (rea, reb, "reach"), (rma, rmb, "matrix")):
-            assert all(np.asarray(u).tobytes() == np.asarray(w).tobytes() for u, w in zip(x, y)), f"{what}: {name}"
-        assert pa[0].tobytes() == pb[0].tobytes() and pa[1].tobytes() == pb[1].tobytes(), f"{what}: clouds"
-        assert map_state(a) == map_state(b), f"{what}: map"
-        assert filecmp.cmp(str(tmp_path / f"a{call}.dsm"), str(tmp_path / f"b{call}.dsm"), shallow=False), f"{what}: checkpoint"
-    a.close()
-    b.close()
+
+    def enqueue(c, is_a, call, t1):
+        c.frontier_enqueue(1)
+        c.reach_matrix_enqueue([camera(t) for t in range(t1)][-8:], 0.1, 2)
+        if is_a:
+            job["M"] = random_matrix(256, rng, 0.01)
+            c.tour_enqueue(job["M"], call % 2, 16, 64, call)
+        c.reach_enqueue(camera(t1 - 1), 0.1, 2, [camera(0)], True, True)
+
+    def check(a, outs, call, t1, what):
+        same(a.tour_wait(), TM.tour(job["M"], call % 2, 16, 64, call), what)
+
+    twin_drive(tmp_path, enable_both, lambda a: a.tour_enable(256, 16), enqueue,
+               lambda c: {"frontiers": c.frontier_wait(), "matrix": c.reach_matrix_wait(), "reach": c.reach_wait()}, check)
 
 
 def test_error_contract():
@@ -263,18 +202,13 @@ def test_error_contract():
 
 
 # ---- the node ----
-FIELD = (0.2, 96, 96, 32)
-MAX_VIEWS = 5
-
-
 def test_node_tour_equals_the_model(tmp_path):
     """The node drive (keyframes, loop closures): after every fused frame, frontiers(), reach(with_frontiers) from the
     field's centre, reach_matrix over that point and the reached viewpoints, and tour() over that matrix; every dumped
     tour equals the model on the dumped matrix."""
-    cam, n = synth.KITTI, 24
+    cam, n = K, 24
     sc = node_script(cam, n)
-    node = [2, 0, 1 << 20, 1 << 21, *FIELD, MAX_VIEWS, MAX_RANGE]
-    r = run_driver("tour_main", str(tmp_path), cam, sc, node + [32, 12 * 12 * 4, 2048, 32, 512])
+    r = run_driver("tour_main", str(tmp_path), cam, sc, node_args() + [32, 12 * 12 * 4, 2048, 32, 512])
     found = 0
     for t in range(n):
         rc, open_ = r.i(), r.i()

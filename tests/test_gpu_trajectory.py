@@ -16,22 +16,17 @@ import pyoracle_trajectory as tj
 from densesurfelmapping_b200 import capi, synth
 from densesurfelmapping_b200.elements import SURFEL_DTYPE
 from densesurfelmapping_b200.elements import POINT_DTYPE
+from known_space import FREE, MAX_RANGE, NODE_FIELD, OCCUPIED, SMALL_CAM, UNKNOWN, Views, small_ctx
 from node_drive import node_script, run_driver
 from resident_map import STORE, T, camera, field_points, map_state, new_ctx, simple_lists, warp, windowed, xyz
-from test_gpu_field_known import MAX_RANGE, Views
 
 pytestmark = pytest.mark.gpu
 
-SMALL_CAM = synth.Camera(64, 48, 60.0, 60.0, 31.5, 23.5, 0.5, 30.0)
-UNKNOWN, OCCUPIED, FREE = 0, 1, 2
 CAPS = (64, 1 << 14, 16)
 
 
 def known_ctx(shape, voxel):
-    ctx = capi.Context(SMALL_CAM, max_batch=2, max_local_surfels=1 << 12)
-    ctx.pool_upload(np.zeros(0, SURFEL_DTYPE))
-    ctx.field_enable(voxel, *shape)
-    ctx.views_enable(1, 1.0)
+    ctx = small_ctx(shape, voxel)
     ctx.field_signed_enable()
     ctx.trajectory_enable(*CAPS)
     ctx.field_query_enable(1 << 16, 1, 2)
@@ -391,7 +386,6 @@ def test_error_contract():
 
 
 # ---- the node ----
-FIELD = (0.2, 96, 96, 32)
 RELOAD = 10
 PARAMS_DTYPE = np.dtype([(k, "<f8") for k in ("w_smooth", "w_clear", "w_feas", "margin", "v_max", "a_max", "g_tol")] +
                         [(k, "<i4") for k in ("max_iter", "memory", "max_ls", "samples")] + [("radius", "<f4"), ("reserved", "<i4", 3)])
@@ -403,8 +397,8 @@ def test_node_trajectories_equal_the_model(tmp_path):
     its results equal the model on the signed grid, which equals the oracle over the node's own clouds."""
     cam, n = synth.KITTI, 16
     sc = node_script(cam, n)
-    voxel, nx, ny, nz = FIELD
-    r = run_driver("trajectory_main", str(tmp_path), cam, sc, [2, 0, 1 << 20, 1 << 21, *FIELD, RELOAD], after=[str(tmp_path / "map")])
+    voxel, nx, ny, nz = NODE_FIELD
+    r = run_driver("trajectory_main", str(tmp_path), cam, sc, [2, 0, 1 << 20, 1 << 21, *NODE_FIELD, RELOAD], after=[str(tmp_path / "map")])
     assert r.i() == -7 and r.i() == 0 and r.i() == -7
     pr = r.take(PARAMS_DTYPE, 1)[0]
     p = {k: pr[k].item() for k in tj.PARAM_NAMES}

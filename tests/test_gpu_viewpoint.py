@@ -10,48 +10,36 @@ job at its pose naming its cluster, gives n_cluster == n_seen; with reach each c
 Stream order, a drive beside publish snapshots and asynchronous checkpoints against a twin without viewpoint jobs, the
 rejected frame and every error code are checked too.  The node is checked through tests/cpp/viewpoint_main.cpp."""
 import ctypes
-import filecmp
+from functools import partial
 
 import numpy as np
 import pytest
 
+import known_space
 import pyoracle_frontier
 import pyoracle_gain as G
 import pyoracle_reach
 import pyoracle_viewpoint as V
-from densesurfelmapping_b200 import capi, synth
-from densesurfelmapping_b200.elements import POINT_DTYPE, SURFEL_DTYPE
+from densesurfelmapping_b200 import capi
+from densesurfelmapping_b200.elements import SURFEL_DTYPE
+from known_space import (FREE, K, OCCUPIED, RELOAD, SMALL_CAM, UNKNOWN, NODE_FIELD, assert_error_stays, gcam, known_drive,
+                         node_args, rejected, rejected_known, small_ctx, twin_clouds, twin_drive, twin_node_tail)
 from node_drive import node_script, run_driver
-from resident_map import SHAPES, STORE, T, camera, load_known, map_state, new_ctx, simple_lists, warp, windowed
-from test_gpu_field_known import MAX_RANGE, Views
-from test_viewpoint_model import open_room, params, rotations, scene
+from planner_scenes import open_room, params, rotations, scene
+from resident_map import SHAPES, camera, load_known
 
 pytestmark = pytest.mark.gpu
 
-SMALL_CAM = synth.Camera(64, 48, 60.0, 60.0, 31.5, 23.5, 0.5, 30.0)
-K = synth.KITTI
-UNKNOWN, OCCUPIED, FREE = G.UNKNOWN, G.OCCUPIED, G.FREE
 INF = V.INF
 ROT8 = np.concatenate([rotations(4), rotations(2, (0.35, -0.35))])
 ROT64 = rotations(16, (0.0, 0.3, -0.3, 0.6))
 
 
-def gcam(cam, max_range, unknown_blocks):
-    return G.Camera(cam.fx, cam.fy, cam.cx, cam.cy, cam.width, cam.height, float(np.float32(max_range)), unknown_blocks)
-
-
-def same(got, want, what):
-    for k, name in enumerate(("header", "clusters", "viewpoints")):
-        g, w = got[k], np.asarray(want[k])
-        bad = np.flatnonzero((g != w).reshape(-1)) if g.shape == w.shape else []
-        assert g.tobytes() == w.tobytes(), f"{what}: {name} differ at {bad[:4]}\n{g.reshape(-1)[bad[:4]]}\nwant\n{w.reshape(-1)[bad[:4]]}"
+same = partial(known_space.same, names=("header", "clusters", "viewpoints"))
 
 
 def loader(shape, voxel=0.2, max_clusters=64, max_candidates=1 << 16, reach=False, gain=0):
-    ctx = capi.Context(SMALL_CAM, max_batch=2, max_local_surfels=1 << 12)
-    ctx.pool_upload(np.zeros(0, SURFEL_DTYPE))
-    ctx.field_enable(voxel, *shape)
-    ctx.views_enable(1, 1.0)
+    ctx = small_ctx(shape, voxel)
     ctx.frontier_enable(256, 1 << 18)
     if reach:
         ctx.reach_enable(16, 1 << 12, 4096)
@@ -238,37 +226,14 @@ def test_known_fields_of_the_drive(chunk, shape):
     """The windowed drive with loop-closure warps between calls; after every call a known field, its frontiers, a reach
     job from the camera with its host copy, and a viewpoint job over the clusters, against the model on the field's
     own grids; the viewpoints re-scored by gain jobs; the same job on a resident twin of the request equals it."""
-    lists = simple_lists()
-    voxels = (0.125, 0.1, 0.3)
-    ctxs, views = {}, {}
-    for v in voxels:
-        ctxs[v] = new_ctx(store=STORE)
-        ctxs[v].field_enable(v, *shape)
-        views[v] = Views(ctxs[v], 6)
-        ctxs[v].frontier_enable(64, 1 << 16)
-        ctxs[v].reach_enable(16, 1 << 12, 2048)
-        ctxs[v].gain_enable(2048)
-        ctxs[v].viewpoint_enable(64, 1 << 18)
-    stored, found = set(), 0
-    for call, t0 in enumerate(range(0, T, chunk)):
-        t1 = min(T, t0 + chunk)
-        for v in voxels:
-            windowed(ctxs[v], t0, t1, lists, want_counts=False)
-            views[v].capture_call(call, t0, t1)
-        for t in range(t0, t1):
-            stored = (stored | set(lists[t][1])) - set(lists[t][2])
-        if call % 2 == 1 and stored:
-            for v in voxels:
-                ctxs[v].pool_transform(warp(1))
-                ctxs[v].inactive_transform(max(stored), warp(2))
-                views[v].warp(warp(1))
-        v = voxels[call % 3]
-        ctx = ctxs[v]
-        slots, poses = views[v].request()
-        cam = camera(t1 - 1)
-        ctx.field_enqueue_known(cam, 5, slots, poses)
-        dist, origin, _ = ctx.field_wait()
-        state, _ = ctx.field_state()
+    def enable(c):
+        c.frontier_enable(64, 1 << 16)
+        c.reach_enable(16, 1 << 12, 2048)
+        c.gain_enable(2048)
+        c.viewpoint_enable(64, 1 << 18)
+
+    found = 0
+    for call, t0, t1, ctx, v, cam, slots, poses, (dist, origin, _), state in known_drive(shape, chunk, (0.125, 0.1, 0.3), enable):
         ctx.frontier_enqueue(1 + call % 3)
         fc, fv, _ = ctx.frontier_wait()
         with_reach = call % 2
@@ -300,107 +265,52 @@ def test_known_fields_of_the_drive(chunk, shape):
         twin = ctx.viewpoint_wait()
         assert all(a.tobytes() == b.tobytes() for a, b in zip(twin, got)), f"{what}: resident twin"
     assert found > 0 or shape == (1, 1, 1)
-    for c in ctxs.values():
-        c.close()
 
 
 def test_viewpoint_jobs_change_nothing_else(tmp_path):
     """A drive with frontier, reach and viewpoint jobs beside a publish snapshot and an asynchronous checkpoint leaves
     the map, both published clouds, the fields, the state grids, the frontiers, the reach results and the checkpoint
     files byte-identical to a twin without viewpoint jobs."""
-    lists = simple_lists()
-    shape, voxel = (64, 64, 32), 0.1
-    a, b = new_ctx(store=STORE), new_ctx(store=STORE)
-    va, vb = {}, {}
-    for c, d in ((a, va), (b, vb)):
-        c.field_enable(voxel, *shape)
-        c.publish_enable()
-        c.checkpoint_enable()
-        d["v"] = Views(c, 4)
+    prm = params(1, 5, 1, 1, top_k=3, with_reach=1)
+
+    def enable_both(c):
         c.frontier_enable(32, 4096)
         c.reach_enable(16, 1 << 12, 1024)
-    a.viewpoint_enable(32, 1 << 16)
-    stored = set()
-    for call, t0 in enumerate(range(0, T, 2)):
-        t1 = t0 + 2
-        for c, d in ((a, va), (b, vb)):
-            windowed(c, t0, t1, lists, want_counts=False)
-            d["v"].capture_call(call, t0, t1)
-        for t in range(t0, t1):
-            stored = (stored | set(lists[t][1])) - set(lists[t][2])
-        outs = []
-        gc = gcam(K, 20 * voxel, call % 2)
-        prm = params(1, 5, 1, 1, top_k=3, with_reach=1)
-        for c, d in ((a, va), (b, vb)):
-            slots, poses = d["v"].request()
-            c.field_enqueue_known(camera(t1 - 1), 5, slots, poses)
-            c.frontier_enqueue(1)
-            c.reach_enqueue(camera(t1 - 1), 0.1, 2, [camera(0)], True, True)
-            if c is a:
-                a.viewpoint_enqueue(gc, ROT8, np.arange(8), prm)
-            c.publish_enqueue(5)
-            c.checkpoint_enqueue(str(tmp_path / f"{'ab'[c is b]}{call}.dsm"))
-            if call % 2 == 1 and stored:
-                c.pool_transform(warp(1))
-                c.inactive_transform(max(stored), warp(2))
-                d["v"].warp(warp(1))
-            f = c.field_wait()
-            st = c.field_state()
-            fr = c.frontier_wait()
-            re = c.reach_wait()
-            p = c.publish_wait()
-            assert c.checkpoint_wait(True)
-            outs.append((f, st, p, fr, re))
-        got = a.viewpoint_wait()
-        what = f"after frames {t0}-{t1 - 1}"
-        same(got, V.viewpoints(outs[0][1][0], outs[0][0][0], outs[0][0][1], voxel, gc, ROT8, np.arange(8), prm, outs[0][3][:2],
-                               outs[0][4][3]), what)
-        fa, fb = outs[0][0], outs[1][0]
-        assert fa[0].tobytes() == fb[0].tobytes() and outs[0][1][0].tobytes() == outs[1][1][0].tobytes(), f"{what}: field"
-        assert all(x.tobytes() == y.tobytes() for x, y in zip(outs[0][3], outs[1][3])), f"{what}: frontiers"
-        assert all(x.tobytes() == y.tobytes() for x, y in zip(outs[0][4], outs[1][4])), f"{what}: reach"
-        assert outs[0][2][0].tobytes() == outs[1][2][0].tobytes() and outs[0][2][1].tobytes() == outs[1][2][1].tobytes(), f"{what}: clouds"
-        assert map_state(a) == map_state(b), f"{what}: map"
-        assert filecmp.cmp(str(tmp_path / f"a{call}.dsm"), str(tmp_path / f"b{call}.dsm"), shallow=False), f"{what}: checkpoint"
-    a.close()
-    b.close()
+
+    def enqueue(c, is_a, call, t1):
+        c.frontier_enqueue(1)
+        c.reach_enqueue(camera(t1 - 1), 0.1, 2, [camera(0)], True, True)
+        if is_a:
+            c.viewpoint_enqueue(gcam(K, 20 * 0.1, call % 2), ROT8, np.arange(8), prm)
+
+    def check(a, outs, call, t1, what):
+        want = V.viewpoints(outs["state"][0], outs["field"][0], outs["field"][1], 0.1, gcam(K, 20 * 0.1, call % 2), ROT8, np.arange(8),
+                            prm, outs["shared"]["frontiers"][:2], outs["shared"]["reach"][3])
+        same(a.viewpoint_wait(), want, what)
+
+    twin_drive(tmp_path, enable_both, lambda a: a.viewpoint_enable(32, 1 << 16), enqueue,
+               lambda c: {"frontiers": c.frontier_wait(), "reach": c.reach_wait()}, check)
 
 
 def test_rejected_frame_comes_back_from_wait():
-    lists = simple_lists()
-    first = next(t for t in range(T) if lists[t][1])
-    shape, voxel = (64, 64, 32), 0.1
-    b = new_ctx(store=1)
-    b.field_enable(voxel, *shape)
-    views = Views(b, 4)
-    b.frontier_enable(32, 1 << 14)
-    b.viewpoint_enable(32, 1 << 16)
-    for call, t0 in enumerate(range(0, first + 2)):
-        windowed(b, t0, t0 + 1, lists, want_counts=False)
-        views.capture_call(call, t0, t0 + 1)
-    slots, poses = views.request()
-    b.field_enqueue_known(camera(first - 1), 1, slots, poses)
-    b.frontier_enqueue(1)
-    gc = gcam(K, 30 * voxel, 0)
-    prm = params(1, 6, 1, 1, top_k=2)
-    b.viewpoint_enqueue(gc, ROT8, np.arange(8), prm)
-    with pytest.raises(capi.DsmError) as e:
-        b.field_wait()
-    assert e.value.code == -6
-    dist, origin, _ = e.value.field
-    state, _ = b.field_state()
-    with pytest.raises(capi.DsmError) as e:
-        b.frontier_wait()
-    fr = e.value.frontier
-    with pytest.raises(capi.DsmError) as e:
-        b.viewpoint_wait()
-    assert e.value.code == -6
-    same(e.value.viewpoint, V.viewpoints(state, dist, origin, voxel, gc, ROT8, np.arange(8), prm, fr[:2]), "rejected")
-    assert e.value.viewpoint[1]["n_traversable"].sum() > 0
-    with pytest.raises(capi.DsmError) as e:
-        b.pool_size()
-    assert e.value.code == -6                            # wait did not clear it
-    b.close()
+    gc, prm = gcam(K, 30 * 0.1, 0), params(1, 6, 1, 1, top_k=2)
+
+    def enable(b):
+        b.frontier_enable(32, 1 << 14)
+        b.viewpoint_enable(32, 1 << 16)
+
+    def enqueue(b, first):
+        b.frontier_enqueue(1)
+        b.viewpoint_enqueue(gc, ROT8, np.arange(8), prm)
+
+    r = rejected_known(enable, enqueue)
+    dist, origin, _ = r.field
+    fr = rejected(r.ctx.frontier_wait).frontier
+    e = rejected(r.ctx.viewpoint_wait)
+    same(e.viewpoint, V.viewpoints(r.state, dist, origin, r.voxel, gc, ROT8, np.arange(8), prm, fr[:2]), "rejected")
+    assert e.viewpoint[1]["n_traversable"].sum() > 0
+    assert_error_stays(r.ctx)
+    r.ctx.close()
 
 
 def test_error_contract():
@@ -503,24 +413,18 @@ def test_error_contract():
 
 
 # ---- the node ----
-FIELD = (0.2, 96, 96, 32)
-MAX_VIEWS = 5
-RELOAD = 12   # the node saves and loads its state after this depth message
-
-
 def test_node_viewpoints_equal_the_model_and_change_nothing(tmp_path):
     """The node drive (keyframes, loop closures): after every fused frame, frontiers(), reach() and viewpoints() over
     every cluster, with reach on every other frame, equal the model over the grids, frontiers, reach start and rotations
     the driver dumps (the reach job's costs being Dijkstra's from its start); clouds,
     PLY and PCD files equal a twin without viewpoint jobs; viewpoints() after load_state until the next fused frame
     returns DSM_E_STATE."""
-    cam, n = synth.KITTI, 24
+    cam, n = K, 24
     sc = node_script(cam, n)
-    voxel, nx, ny, nz = FIELD
+    voxel, nx, ny, nz = NODE_FIELD
     pa, pb = str(tmp_path / "mapa"), str(tmp_path / "mapb")
-    node = [2, 0, 1 << 20, 1 << 21, *FIELD, MAX_VIEWS, MAX_RANGE]
-    r = run_driver("viewpoint_main", str(tmp_path), cam, sc, node + [1, RELOAD], tag="a", after=[pa])
-    q = run_driver("viewpoint_main", str(tmp_path), cam, sc, node + [0, RELOAD], tag="b", after=[pb])
+    r = run_driver("viewpoint_main", str(tmp_path), cam, sc, node_args() + [1, RELOAD], tag="a", after=[pa])
+    q = run_driver("viewpoint_main", str(tmp_path), cam, sc, node_args() + [0, RELOAD], tag="b", after=[pb])
     found = 0
     for t in range(n):
         rc, ub = r.i(), r.i()
@@ -537,9 +441,8 @@ def test_node_viewpoints_equal_the_model_and_change_nothing(tmp_path):
         recs = r.lst(V.CLUSTER_DTYPE)
         slots = r.lst(V.VIEWPOINT_DTYPE).reshape(len(recs), -1)
         after_load = r.i()
-        rr, act, inact = r.i(), r.lst(POINT_DTYPE), r.lst(POINT_DTYPE)
-        rq, act_q, inact_q = q.i(), q.lst(POINT_DTYPE), q.lst(POINT_DTYPE)
-        assert rc == 0 and rr == 0 and rq == 0, f"message {t}: {rc} {rr} {rq}"
+        twin_clouds(r, q, f"message {t}")
+        assert rc == 0, f"message {t}: {rc}"
         gc = G.Camera(cam.fx, cam.fy, cam.cx, cam.cy, cam.width, cam.height, max_range, ub)
         cost = None
         if prm.with_reach:     # the reach job from the middle voxel converged, so its costs are Dijkstra's
@@ -549,9 +452,5 @@ def test_node_viewpoints_equal_the_model_and_change_nothing(tmp_path):
         same((info, recs, slots), want, f"message {t}")
         found += int((recs["n_viewpoints"] > 0).sum()) > 0
         assert after_load == (-7 if t == RELOAD - 1 else 1), f"message {t}: viewpoints() after load_state"
-        assert act.tobytes() == act_q.tobytes() and inact.tobytes() == inact_q.tobytes(), f"message {t}: clouds"
     assert found > 0
-    assert r.lst(SURFEL_DTYPE).tobytes() == q.lst(SURFEL_DTYPE).tobytes()
-    assert r.o == len(r.raw) and q.o == len(q.raw)
-    for ext in (".ply", ".pcd"):
-        assert filecmp.cmp(pa + ext, pb + ext, shallow=False), ext
+    twin_node_tail(r, q, pa, pb)

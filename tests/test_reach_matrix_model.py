@@ -12,7 +12,7 @@ from scipy.sparse import csgraph
 import pyoracle_reach as R
 import pyoracle_reach_matrix as RM
 from densesurfelmapping_b200 import capi
-from test_frontier_model import serpentine
+from planner_scenes import serpentine
 
 FREE, UNKNOWN, OCCUPIED = R.FREE, R.UNKNOWN, R.OCCUPIED
 

@@ -9,26 +9,9 @@ import pyoracle_reach as R
 import pyoracle_reach_matrix as RM
 import pyoracle_tour as T
 from densesurfelmapping_b200 import capi
+from planner_scenes import metric_matrix, random_matrix
 
 INF = T.INF
-
-
-def random_matrix(n, rng, p_inf=0.0, symmetric=False, hi=1000):
-    M = rng.integers(0, hi, (n, n)).astype(np.uint32)
-    if symmetric:
-        M = np.minimum(M, M.T)
-    if p_inf:
-        M[rng.random((n, n)) < p_inf] = INF
-    np.fill_diagonal(M, 0)
-    return M
-
-
-def metric_matrix(n, rng, stretch=1.3):
-    """Euclidean distances between random points, each entry stretched by a factor in [1, stretch]: asymmetric, close
-    to metric, as travel costs through free space are."""
-    p = rng.uniform(0, 100, (n, 2))
-    d = np.linalg.norm(p[:, None] - p[None], axis=-1)
-    return np.round(d * rng.uniform(1.0, stretch, (n, n)) * 10).astype(np.uint32)
 
 
 def recost(M, open_, order):

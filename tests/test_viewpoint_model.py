@@ -12,38 +12,10 @@ import pyoracle_gain as G
 import pyoracle_reach
 import pyoracle_viewpoint as V
 from densesurfelmapping_b200 import capi
+from planner_scenes import open_room, params, rotation, rotations, scene
 
 UNKNOWN, OCCUPIED, FREE = G.UNKNOWN, G.OCCUPIED, G.FREE
 INF = V.INF
-
-
-def rotation(yaw, pitch=0.0):
-    """The row-major camera-to-world 3x3 of a camera looking along yaw (from +x toward +y) and pitch (up), x right, y
-    down, z forward."""
-    f = np.array([np.cos(pitch) * np.cos(yaw), np.cos(pitch) * np.sin(yaw), np.sin(pitch)])
-    r = np.array([np.sin(yaw), -np.cos(yaw), 0.0])
-    return np.stack([r, np.cross(f, r), f], axis=1).reshape(9)
-
-
-def rotations(n_yaw, pitches=(0.0,)):
-    """A yaw sweep of n_yaw headings at each pitch, (n_yaw len(pitches), 9)."""
-    return np.stack([rotation(2 * np.pi * k / n_yaw, p) for p in pitches for k in range(n_yaw)])
-
-
-def params(r_min=1, r_max=3, dz_max=1, stride=1, max_samples=4096, min_seen=0, top_k=4, with_reach=0, radius=0.0):
-    return V.Params(r_min, r_max, dz_max, stride, max_samples, min_seen, top_k, with_reach, radius)
-
-
-def scene(rng, shape, n_blobs=6, p_occupied=0.04):
-    """A state grid [nz][ny][nx]: free space with scattered occupied voxels and n_blobs unknown boxes, each bordered by
-    its own frontier clusters."""
-    nx, ny, nz = shape
-    st = np.where(rng.random((nz, ny, nx)) < p_occupied, OCCUPIED, FREE).astype(np.uint8)
-    for _ in range(n_blobs):
-        a = [int(rng.integers(0, n)) for n in (nx, ny, nz)]
-        b = [min(n, x + int(rng.integers(1, 4))) for x, n in zip(a, (nx, ny, nz))]
-        st[a[2]:b[2], a[1]:b[1], a[0]:b[0]] = UNKNOWN
-    return st
 
 
 def job(st, o, voxel, cam, rot, cl, prm, min_voxels=1, max_voxels=1 << 20, reach_cost=None):
@@ -195,13 +167,6 @@ def test_sampling_cut():
             c = np.array([s0["voxel"] % nx, s0["voxel"] // nx % ny, s0["voxel"] // (nx * ny)])
             assert V.seen_counts(st, o, voxel, cam, rot, G.centres([c], o, voxel)[0], mc).max() == s0["n_seen"]
     assert rng is not None
-
-
-def open_room():
-    """A free room 12x12x3 whose +y wall is unknown: one flat cluster along the wall."""
-    st = np.full((3, 13, 12), FREE, np.uint8)
-    st[:, 12, :] = UNKNOWN
-    return st
 
 
 def test_ties():
