@@ -45,6 +45,7 @@ EXPORTS = [
     "dsm_inactive_segments", "dsm_inactive_load", "dsm_map_save", "dsm_map_load", "dsm_map_peek",
     "dsm_checkpoint_enable", "dsm_checkpoint_enqueue", "dsm_checkpoint_wait", "dsm_debug_checkpoint_drain_ctas",
     "dsm_checkpoint_enqueue_incremental", "dsm_map_load_journal", "dsm_map_peek_journal", "dsm_journal_materialize",
+    "dsm_checkpoint_views_enable",
     "dsm_comm_unique_id", "dsm_comm_init", "dsm_comm_destroy", "dsm_gather_deltas", "dsm_gather_wait", "dsm_gathered_device",
     "dsm_gathered_rank_bytes", "dsm_gathered_download", "dsm_set_constants", "dsm_set_concurrency",
 ]
@@ -238,6 +239,7 @@ def load_library():
     L.dsm_map_load.argtypes = [vp, ctypes.c_char_p, vp, cs, ctypes.POINTER(cs)]
     L.dsm_map_peek.argtypes = [ctypes.c_char_p, vp, cs, ctypes.POINTER(cs), vp, ci, ctypes.POINTER(ci)]
     L.dsm_checkpoint_enable.argtypes = [vp]
+    L.dsm_checkpoint_views_enable.argtypes = [vp]
     L.dsm_checkpoint_enqueue.argtypes = [vp, ctypes.c_char_p, vp, cs]
     L.dsm_checkpoint_wait.argtypes = [vp, ci, ctypes.POINTER(ci)]
     L.dsm_debug_checkpoint_drain_ctas.argtypes = [vp, ci]
@@ -625,6 +627,10 @@ class Context:
         new base; checkpoint_wait retires it."""
         buf = ctypes.create_string_buffer(bytes(extra), max(len(extra), 1))
         self._ck(self.lib.dsm_checkpoint_enqueue_incremental(self.h, os.fsencode(path), buf if len(extra) else None, len(extra)))
+
+    def checkpoint_views_enable(self):
+        """Every checkpoint from now on carries the captured views, and every load replaces them (DESIGN.md §8.18)."""
+        self._ck(self.lib.dsm_checkpoint_views_enable(self.h))
 
     def map_load_journal(self, path):
         """map_load of the state base + journal resolve to: (extra bytes, records applied)."""

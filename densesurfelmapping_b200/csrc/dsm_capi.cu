@@ -1343,6 +1343,7 @@ int dsm_map_info(const dsm_ctx *ctx, DsmMapInfo *info)
     info->store_cap = ctx->inact ? ctx->inact->cap : 0;
     info->publish_in_flight = ctx->pub_in_flight;
     info->field_in_flight = ctx->field && ctx->field->in_flight;
+    info->view_rays = ctx->views && ctx->views->checkpointed ? ctx->d.S : 0;
     return DSM_OK;
 }
 
@@ -1766,6 +1767,7 @@ extern "C" int dsm_views_enable(dsm_ctx *ctx, int max_views, float max_range)
     auto v = std::make_unique<DsmViews>();
     v->max_views = max_views, v->max_range = max_range;
     v->filled.assign((size_t)max_views, 0);
+    v->gen.assign((size_t)max_views, 0);
     v->own.device(&v->rays, (size_t)max_views * ctx->d.S);
     v->own.host(&v->state, f->voxels);
     v->own.host(&v->stage_host, DsmViews::stage_bytes(max_views));
@@ -1791,6 +1793,91 @@ extern "C" int dsm_views_capture(dsm_ctx *ctx, int frame, int slot)
     dsm_launch_views_capture(ctx->d.plane + (size_t)(ctx->img_slot0 + frame) * S * 3, S, v->rays + (size_t)slot * S, ctx->stream);
     CK(cudaGetLastError());
     v->filled[(size_t)slot] = 1;
+    v->gen[(size_t)slot] = ++v->gens;
+    return DSM_OK;
+}
+
+// ---- views in the checkpoint (include/dsm.h, DESIGN.md §8.18) ----
+// Calls f(first, count) for each run of consecutive slots in an ascending list
+template <typename F>
+static cudaError_t slot_runs(const int32_t *slots, int n, F f)
+{
+    for (int i = 0; i < n;)
+    {
+        int j = i + 1;
+        while (j < n && slots[j] == slots[j - 1] + 1) j++;
+        const cudaError_t e = f(i, j - i);
+        if (e != cudaSuccess) return e;
+        i = j;
+    }
+    return cudaSuccess;
+}
+
+int dsm_views_load_check(const dsm_ctx *ctx, const int32_t *slots, int n, const void *rays)
+{
+    const DsmViews *v = ctx->views.get();
+    for (int i = 0; i < n; i++)
+        if (slots[i] >= v->max_views) return DSM_E_CAPACITY;
+    // what k_views_capture writes: finite coordinates with w = 1, or all 16 bytes zero
+    const uint8_t *b = static_cast<const uint8_t *>(rays);
+    static const uint8_t zero[16] = {};
+    for (size_t r = 0; r < (size_t)n * ctx->d.S; r++)
+    {
+        float4 q;
+        std::memcpy(&q, b + 16 * r, 16);
+        const bool ray = q.w == 1.f && std::isfinite(q.x) && std::isfinite(q.y) && std::isfinite(q.z);
+        if (!ray && std::memcmp(&q, zero, 16) != 0) return DSM_E_INVALID;
+    }
+    return DSM_OK;
+}
+
+int dsm_views_load(dsm_ctx *ctx, const int32_t *slots, int n, const void *rays)
+{
+    DsmViews &v = *ctx->views;
+    const size_t S = (size_t)ctx->d.S;
+    const uint8_t *b = static_cast<const uint8_t *>(rays);
+    CK(cudaSetDevice(ctx->device));
+    CK(slot_runs(slots, n, [&](int i, int c) {
+        return cudaMemcpyAsync(v.rays + (size_t)slots[i] * S, b + 16 * S * i, 16 * S * c, cudaMemcpyHostToDevice, ctx->stream);
+    }));
+    CK(cudaStreamSynchronize(ctx->stream)); // the source is the file's buffer
+    std::fill(v.filled.begin(), v.filled.end(), 0);
+    for (int i = 0; i < n; i++) v.filled[(size_t)slots[i]] = 1;
+    for (uint64_t &g : v.gen) g = ++v.gens; // every slot differs from the checkpoint image
+    return DSM_OK;
+}
+
+int dsm_views_download(dsm_ctx *ctx, std::vector<int32_t> &slots, std::vector<uint8_t> &rays)
+{
+    const DsmViews &v = *ctx->views;
+    const size_t S = (size_t)ctx->d.S;
+    slots.clear();
+    for (int s = 0; s < v.max_views; s++)
+        if (v.filled[(size_t)s]) slots.push_back(s);
+    rays.resize(16 * S * slots.size());
+    CK(cudaSetDevice(ctx->device));
+    CK(slot_runs(slots.data(), (int)slots.size(), [&](int i, int c) {
+        return cudaMemcpyAsync(rays.data() + 16 * S * i, v.rays + (size_t)slots[i] * S, 16 * S * c, cudaMemcpyDeviceToHost, ctx->stream);
+    }));
+    CK(cudaStreamSynchronize(ctx->stream));
+    return DSM_OK;
+}
+
+static cudaError_t checkpoint_view_image(dsm_ctx *ctx);
+
+extern "C" int dsm_checkpoint_views_enable(dsm_ctx *ctx)
+{
+    if (!ctx) return DSM_E_INVALID;
+    DsmViews *v = ctx->views.get();
+    if (!v || v->checkpointed) return DSM_E_STATE;
+    CK(cudaSetDevice(ctx->device));
+    v->checkpointed = true;
+    if (ctx->ckpt && checkpoint_view_image(ctx) != cudaSuccess)
+    {
+        cudaGetLastError();
+        v->checkpointed = false;
+        return DSM_E_NOMEM;
+    }
     return DSM_OK;
 }
 
@@ -2500,6 +2587,26 @@ static cudaError_t checkpoint_images(dsm_ctx *ctx)
     return cudaSuccess;
 }
 
+// The views section of the image (DESIGN.md §8.18), once both dsm_checkpoint_enable and dsm_checkpoint_views_enable have
+// run: it holds no slot yet, so the next snapshot copies every filled one, and the next incremental checkpoint is a base.
+// On failure nothing is kept.
+static cudaError_t checkpoint_view_image(dsm_ctx *ctx)
+{
+    DsmCheckpoint &k = *ctx->ckpt;
+    const DsmViews &v = *ctx->views;
+    const size_t rays = (size_t)v.max_views * ctx->d.S;
+    auto own = std::make_unique<CudaOwner>();
+    float4 *dev = nullptr, *host = nullptr;
+    cudaError_t e = own->device(&dev, rays);
+    if (e == cudaSuccess) e = own->host(&host, rays);
+    if (e != cudaSuccess) return e;
+    k.vimg = std::move(own);
+    k.vdev = dev, k.vhost = host;
+    k.vgen.assign((size_t)v.max_views, 0);
+    k.stale = true;
+    return cudaSuccess;
+}
+
 void dsm_checkpoint_map_replaced(dsm_ctx *ctx)
 {
     if (ctx && ctx->ckpt) ctx->ckpt->stale = true;
@@ -2514,7 +2621,7 @@ static int checkpoint_write_incremental(DsmCheckpoint &k, const DsmMapSections &
     {
         uint64_t sum = 0, bytes = 0, jbytes = 0;
         int rc = dsm_map_write(k.path.c_str(), k.info, s, &sum, &bytes);
-        if (rc == DSM_OK) rc = dsm_journal_start(k.path.c_str(), sum, &jbytes);
+        if (rc == DSM_OK) rc = dsm_journal_start(k.path.c_str(), sum, s.rays_per_view, &jbytes);
         if (rc != DSM_OK) return rc;
         k.chain_path = k.path;
         k.chain_sum = sum, k.sequence = 1, k.base_bytes = bytes, k.journal_bytes = jbytes;
@@ -2530,7 +2637,7 @@ static int checkpoint_write_incremental(DsmCheckpoint &k, const DsmMapSections &
         if (flags[k.pool_chunks + c]) k.chunks.push_back(c);
     const DsmJournalRecord r{k.sequence, k.chain_sum, s.n_pool, s.n_store, s.n_segments, k.chunks.data(), k_pool,
                              k.chunks.data() + k_pool, (int)k.chunks.size() - k_pool, k.host + k.lay.pool, k.host + k.lay.store,
-                             s.table, s.extra, s.extra_bytes};
+                             s.table, s.extra, s.extra_bytes, s.view_slots, s.n_views, s.view_rays, s.rays_per_view};
     uint64_t sum = 0, bytes = 0;
     const int rc = dsm_journal_append(k.path.c_str(), k.journal_bytes, r, &sum, &bytes);
     if (rc != DSM_OK) return rc;
@@ -2551,10 +2658,14 @@ static int checkpoint_write(DsmCheckpoint &k)
         k.err_frame = h[DSM_SNAP_ERR_FRAME];
         return DSM_E_CAPACITY;
     }
+    // the views the drain brought over, by slot: every filled one for a file or a base, the snapshot's for a record
+    const int S = k.info.view_rays;
+    std::vector<const void *> views(k.view_slots.size());
+    for (size_t i = 0; i < views.size(); i++) views[i] = k.vhost + (size_t)k.view_slots[i] * S;
     const DsmMapSections s{reinterpret_cast<const dsm_surfel_t *>(k.host + k.lay.pool), h[DSM_SNAP_N_POOL],
                            reinterpret_cast<const dsm_surfel_t *>(k.host + k.lay.store), h[DSM_SNAP_N_STORE],
                            reinterpret_cast<const int32_t *>(k.host + k.lay.table), h[DSM_SNAP_N_SEGMENTS],
-                           k.extra.data(), k.extra.size()};
+                           k.extra.data(), k.extra.size(), k.view_slots.data(), (int)k.view_slots.size(), views.data(), S};
     if (k.kind == DsmCheckpoint::FULL) return dsm_map_write(k.path.c_str(), k.info, s);
     return checkpoint_write_incremental(k, s);
 }
@@ -2590,6 +2701,7 @@ extern "C" int dsm_checkpoint_enable(dsm_ctx *ctx)
     if (e == cudaSuccess) e = k->own.event(&k->ev_drain, cudaEventDisableTiming | cudaEventBlockingSync);
     ctx->ckpt = std::move(k);
     if (e == cudaSuccess) e = checkpoint_images(ctx);
+    if (e == cudaSuccess && ctx->views && ctx->views->checkpointed) e = checkpoint_view_image(ctx);
     if (e != cudaSuccess)
     {
         cudaGetLastError();
@@ -2637,6 +2749,24 @@ static int checkpoint_enqueue(dsm_ctx *ctx, const char *path, const void *extra,
         dsm_launch_map_snapshot(ctx->d.pool, ctx->res_ofs, pool_upper, s ? s->surfels : nullptr, s ? s->seg : nullptr, ctx->win_hdr,
                                 store_upper, k->dev, k->lay, ctx->stream);
     CK(cudaGetLastError());
+    // views (DESIGN.md §8.18): the slots captured or loaded since the previous snapshot into the image, at the same
+    // stream position; then, after the snapshot, every filled slot of the image to the host, or for a record the copied ones
+    const DsmViews *v = info.view_rays > 0 ? ctx->views.get() : nullptr;
+    const size_t S = (size_t)ctx->d.S;
+    std::vector<int32_t> &snap = k->snap_slots, filled;
+    snap.clear();
+    if (v)
+    {
+        for (int i = 0; i < v->max_views; i++)
+            if (v->filled[(size_t)i])
+            {
+                filled.push_back(i);
+                if (v->gen[(size_t)i] != k->vgen[(size_t)i]) snap.push_back(i);
+            }
+        CK(slot_runs(snap.data(), (int)snap.size(), [&](int i, int c) {
+            return cudaMemcpyAsync(k->vdev + snap[i] * S, v->rays + snap[i] * S, 16 * S * c, cudaMemcpyDeviceToDevice, ctx->stream);
+        }));
+    }
     CK(cudaEventRecord(k->ev_snap, ctx->stream));
     CK(cudaStreamWaitEvent(k->s_drain, k->ev_snap, 0));
     if (kind == DsmCheckpoint::RECORD)
@@ -2644,9 +2774,18 @@ static int checkpoint_enqueue(dsm_ctx *ctx, const char *path, const void *extra,
     else
         dsm_launch_map_drain(k->dev, k->host_dev, k->lay, k->drain_ctas, k->s_drain);
     CK(cudaGetLastError());
+    const std::vector<int32_t> &drained = kind == DsmCheckpoint::RECORD ? snap : filled;
+    if (v)
+        CK(slot_runs(drained.data(), (int)drained.size(), [&](int i, int c) {
+            return cudaMemcpyAsync(k->vhost + drained[i] * S, k->vdev + drained[i] * S, 16 * S * c, cudaMemcpyDeviceToHost, k->s_drain);
+        }));
     CK(cudaEventRecord(k->ev_drain, k->s_drain));
+    // the image now holds these slots, whether or not the write succeeds: a failed write ends the chain, and the base
+    // that follows drains every filled slot of the image
+    for (int32_t i : snap) k->vgen[(size_t)i] = v->gen[(size_t)i];
     {
         std::lock_guard<std::mutex> lk(k->m);
+        k->view_slots = drained;
         k->path = path;
         k->extra.assign(static_cast<const uint8_t *>(extra), static_cast<const uint8_t *>(extra) + extra_bytes);
         k->info = info;

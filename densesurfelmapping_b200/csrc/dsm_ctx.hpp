@@ -173,6 +173,14 @@ struct DsmCheckpoint
     std::string chain_path;
     uint64_t chain_sum = 0, sequence = 1, base_bytes = 0, journal_bytes = 0;
     std::vector<int32_t> chunks; // the thread's list of changed chunks
+    // dsm_checkpoint_views_enable (DESIGN.md §8.18): the views section of the image, device and pinned [max_views][S],
+    // allocated once both enables have run.  Caller's thread: vgen[s] the capture generation (DsmViews::gen) the
+    // section holds for slot s, 0 for none; snap_slots the slots the last snapshot copied.  The job: view_slots, the
+    // slots its file or record lists, read from vhost by slot.
+    std::unique_ptr<CudaOwner> vimg;
+    float4 *vdev = nullptr, *vhost = nullptr;
+    std::vector<uint64_t> vgen;
+    std::vector<int32_t> snap_slots, view_slots;
     std::thread worker; // last: started once the members above exist
 
     ~DsmCheckpoint()
@@ -224,6 +232,9 @@ struct DsmViews
     float max_range = 0.f;
     float4 *rays = nullptr;       // device [max_views][S]: camera-space ray ends, w = 1, or w = 0 for a seed without one
     std::vector<uint8_t> filled;  // [max_views], caller's thread: the slot has been captured
+    bool checkpointed = false;    // dsm_checkpoint_views_enable: every checkpoint carries the filled slots
+    std::vector<uint64_t> gen;    // [max_views], caller's thread: a fresh number at every capture or load of the slot
+    uint64_t gens = 0;            // the last number handed out
     uint8_t *state = nullptr;     // pinned [voxels]
     uint8_t *stage_host = nullptr, *stage_dev = nullptr; // double poses[max_views][12] | int32 slots[max_views]
     static size_t stage_bytes(int n) { return 12 * sizeof(double) * (size_t)n + sizeof(int32_t) * (size_t)n; }

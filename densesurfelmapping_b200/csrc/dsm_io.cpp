@@ -21,6 +21,10 @@
 //                           uint64 FNV-1a 64 of every byte before it
 //                      dsm_map_write is the one writer of that file: dsm_map_save and the checkpoint thread of
 //                      dsm_checkpoint_enqueue (dsm_capi.cu) hand it the header fields and the sections as spans.
+//                      Version 2, of a context after dsm_checkpoint_views_enable (DESIGN.md §8.18): the word at 92 holds
+//                      S, the rays per view, which must be (W/8)·(H/8); after the table come int32 n_views,
+//                      int32 slots[n_views] (strictly ascending, >= 0) and float4 rays[n_views][S], then extra and the
+//                      checksum as in version 1.
 #include <fcntl.h>
 #include <sys/stat.h>
 #include <unistd.h>
@@ -29,6 +33,7 @@
 #include <cmath>
 #include <cstdio>
 #include <cstring>
+#include <map>
 #include <string>
 #include <vector>
 
@@ -182,7 +187,7 @@ extern "C" int dsm_write_ply_mesh(const char *path, const dsm_surfel_t *surfels,
 namespace
 {
 const char kMapMagic[8] = {'D', 'S', 'M', 'M', 'A', 'P', 0, 0};
-const uint32_t kMapFormat = 1;
+const uint32_t kMapFormat = 1, kMapFormatViews = 2;
 
 struct MapHeader // the first 104 bytes of the file, in file order
 {
@@ -192,7 +197,7 @@ struct MapHeader // the first 104 bytes of the file, in file order
     int32_t width, height;
     float fx, fy, cx, cy, fuse_far, fuse_near;
     dsm_constants constants;
-    int32_t n_pool, n_store, n_segments, zero;
+    int32_t n_pool, n_store, n_segments, rays_per_view; // rays_per_view: 0 in version 1
     uint64_t extra_bytes;
 };
 static_assert(sizeof(MapHeader) == 104, "checkpoint header layout");
@@ -223,7 +228,18 @@ int read_all(const char *path, std::vector<uint8_t> &raw)
     return len < 0 ? DSM_E_IO : DSM_OK;
 }
 
-// A checkpoint read whole and checked: magic and version (DSM_E_INVALID), then its length and checksum (DSM_E_IO)
+// The rays per view of a version-2 header: dsm_num_seeds of its frame size
+int64_t seeds_of(const MapHeader &h) { return (int64_t)(h.width / 8) * (h.height / 8); }
+
+bool ascending(const int32_t *slots, int64_t n)
+{
+    for (int64_t i = 0; i < n; i++)
+        if (slots[i] < 0 || (i > 0 && slots[i] <= slots[i - 1])) return false;
+    return true;
+}
+
+// A checkpoint read whole and checked: magic, version and, in version 2, the rays-per-view word (DSM_E_INVALID), then
+// its length and checksum (DSM_E_IO), then the views section's slot list (DSM_E_INVALID)
 struct MapFile
 {
     std::vector<uint8_t> raw;
@@ -231,6 +247,9 @@ struct MapFile
     const dsm_surfel_t *pool = nullptr, *store = nullptr;
     const int32_t *table = nullptr;
     const uint8_t *extra = nullptr;
+    int rays_per_view = 0, n_views = 0; // 0 and 0 in version 1
+    const int32_t *view_slots = nullptr;
+    const uint8_t *view_rays = nullptr; // [n_views][rays_per_view] float4
 
     int read(const char *path)
     {
@@ -242,11 +261,22 @@ struct MapFile
     {
         if (raw.size() < 16) return DSM_E_IO;
         std::memcpy(&hdr, raw.data(), std::min(raw.size(), sizeof(hdr)));
-        if (std::memcmp(hdr.magic, kMapMagic, 8) != 0 || hdr.format != kMapFormat) return DSM_E_INVALID;
+        if (std::memcmp(hdr.magic, kMapMagic, 8) != 0 || (hdr.format != kMapFormat && hdr.format != kMapFormatViews))
+            return DSM_E_INVALID;
         if (raw.size() < sizeof(hdr) + 8) return DSM_E_IO;
+        const bool views = hdr.format == kMapFormatViews;
+        if (views && (hdr.rays_per_view < 1 || hdr.rays_per_view != seeds_of(hdr))) return DSM_E_INVALID;
         if (hdr.n_pool < 0 || hdr.n_store < 0 || hdr.n_segments < 0) return DSM_E_IO;
-        const uint64_t body = (uint64_t)(hdr.n_pool + (uint64_t)hdr.n_store) * sizeof(dsm_surfel_t) + (uint64_t)hdr.n_segments * 12;
-        if (hdr.extra_bytes > raw.size() || sizeof(hdr) + body + hdr.extra_bytes + 8 != raw.size()) return DSM_E_IO;
+        uint64_t body = (uint64_t)(hdr.n_pool + (uint64_t)hdr.n_store) * sizeof(dsm_surfel_t) + (uint64_t)hdr.n_segments * 12;
+        int32_t nv = 0;
+        if (views)
+        {
+            if (body > raw.size() || sizeof(hdr) + body + 4 + 8 > raw.size()) return DSM_E_IO;
+            std::memcpy(&nv, raw.data() + sizeof(hdr) + body, 4);
+            if (nv < 0 || (nv > 0 && (uint64_t)hdr.rays_per_view > raw.size() / 16 / (uint64_t)nv)) return DSM_E_IO;
+            body += 4 + 4 * (uint64_t)nv + 16 * (uint64_t)hdr.rays_per_view * (uint64_t)nv;
+        }
+        if (hdr.extra_bytes > raw.size() || body > raw.size() || sizeof(hdr) + body + hdr.extra_bytes + 8 != raw.size()) return DSM_E_IO;
         Fnv1a sum;
         sum.add(raw.data(), raw.size() - 8);
         uint64_t want = 0;
@@ -257,6 +287,15 @@ struct MapFile
         store = pool + hdr.n_pool;
         table = reinterpret_cast<const int32_t *>(store + hdr.n_store);
         extra = reinterpret_cast<const uint8_t *>(table + 3 * (size_t)hdr.n_segments);
+        rays_per_view = views ? hdr.rays_per_view : 0;
+        n_views = nv;
+        if (views)
+        {
+            view_slots = reinterpret_cast<const int32_t *>(extra) + 1;
+            view_rays = reinterpret_cast<const uint8_t *>(view_slots + nv);
+            extra = view_rays + 16 * (size_t)hdr.rays_per_view * nv;
+            if (!ascending(view_slots, nv)) return DSM_E_INVALID;
+        }
         return DSM_OK;
     }
 };
@@ -324,7 +363,8 @@ extern "C" int dsm_map_save(dsm_ctx *ctx, const char *path, const void *extra, s
     int n_pool = 0, n_store = 0, n_seg = 0;
     if (rc == DSM_OK) rc = dsm_pool_size(ctx, &n_pool); // DSM_E_STATE without a pool; reports a rejected frame
     std::vector<dsm_surfel_t> pool((size_t)n_pool + 1), store(1);
-    std::vector<int32_t> table(3);
+    std::vector<int32_t> table(3), slots;
+    std::vector<uint8_t> rays;
     if (rc == DSM_OK) rc = dsm_pool_download(ctx, pool.data(), n_pool, &n_pool);
     if (rc == DSM_OK && info.store_cap > 0)
     {
@@ -334,8 +374,12 @@ extern "C" int dsm_map_save(dsm_ctx *ctx, const char *path, const void *extra, s
         if (rc == DSM_OK) rc = dsm_inactive_download(ctx, -1, store.data(), n_store, &n_store);
         if (rc == DSM_OK) rc = dsm_inactive_segments(ctx, table.data(), n_seg, &n_seg);
     }
+    if (rc == DSM_OK && info.view_rays > 0) rc = dsm_views_download(ctx, slots, rays);
     if (rc != DSM_OK) return rc;
-    return dsm_map_write(path, info, DsmMapSections{pool.data(), n_pool, store.data(), n_store, table.data(), n_seg, extra, extra_bytes});
+    std::vector<const void *> views(slots.size());
+    for (size_t i = 0; i < slots.size(); i++) views[i] = rays.data() + 16 * (size_t)info.view_rays * i;
+    return dsm_map_write(path, info, DsmMapSections{pool.data(), n_pool, store.data(), n_store, table.data(), n_seg, extra, extra_bytes,
+                                                    slots.data(), (int)slots.size(), views.data(), info.view_rays});
 }
 
 int dsm_map_write(const char *path, const DsmMapInfo &info, const DsmMapSections &s, uint64_t *checksum, uint64_t *bytes)
@@ -343,19 +387,25 @@ int dsm_map_write(const char *path, const DsmMapInfo &info, const DsmMapSections
     MapHeader h;
     std::memset(&h, 0, sizeof(h));
     std::memcpy(h.magic, kMapMagic, 8);
-    h.format = kMapFormat;
+    h.format = s.rays_per_view > 0 ? kMapFormatViews : kMapFormat;
     h.version = dsm_version();
     const dsm_params &p = info.params;
     h.width = p.width, h.height = p.height;
     h.fx = p.fx, h.fy = p.fy, h.cx = p.cx, h.cy = p.cy, h.fuse_far = p.fuse_far, h.fuse_near = p.fuse_near;
     h.constants = info.constants;
-    h.n_pool = s.n_pool, h.n_store = s.n_store, h.n_segments = s.n_segments;
+    h.n_pool = s.n_pool, h.n_store = s.n_store, h.n_segments = s.n_segments, h.rays_per_view = s.rays_per_view;
     h.extra_bytes = s.extra_bytes;
     AtomicFile out(path);
     out.put(&h, sizeof(h));
     out.put(s.pool, (size_t)s.n_pool * sizeof(dsm_surfel_t));
     out.put(s.store, (size_t)s.n_store * sizeof(dsm_surfel_t));
     out.put(s.table, (size_t)s.n_segments * 12);
+    if (s.rays_per_view > 0)
+    {
+        out.put(&s.n_views, 4);
+        out.put(s.view_slots, 4 * (size_t)s.n_views);
+        for (int i = 0; i < s.n_views; i++) out.put(s.view_rays[i], 16 * (size_t)s.rays_per_view);
+    }
     out.put(s.extra, s.extra_bytes);
     const uint64_t sum = out.sum.h;
     if (!out.commit()) return DSM_E_IO;
@@ -389,11 +439,20 @@ int load_checked(dsm_ctx *ctx, const DsmMapInfo &info, const MapFile &m, void *e
         rc = dsm_inactive_load_check(ctx, m.store, h.n_store, m.table, h.n_segments);
         if (rc != DSM_OK) return rc;
     }
+    // views: a context that did not opt in refuses a views section, as a context without a store refuses stored surfels
+    if (m.rays_per_view > 0 && info.view_rays == 0) return DSM_E_STATE;
+    if (m.rays_per_view > 0)
+    {
+        rc = dsm_views_load_check(ctx, m.view_slots, m.n_views, m.view_rays);
+        if (rc != DSM_OK) return rc;
+    }
     if (extra_bytes) *extra_bytes = (size_t)h.extra_bytes;
     if (h.extra_bytes > extra_cap) return DSM_E_CAPACITY;
     dsm_checkpoint_map_replaced(ctx);
     rc = dsm_pool_upload(ctx, m.pool, h.n_pool);
     if (rc == DSM_OK && info.store_cap > 0) rc = dsm_inactive_load(ctx, m.store, h.n_store, m.table, h.n_segments);
+    // a file without a views section leaves no slot filled
+    if (rc == DSM_OK && info.view_rays > 0) rc = dsm_views_load(ctx, m.view_slots, m.n_views, m.view_rays);
     if (rc != DSM_OK) return rc;
     if (h.extra_bytes > 0) std::memcpy(extra, m.extra, (size_t)h.extra_bytes);
     return DSM_OK;
@@ -433,12 +492,12 @@ extern "C" int dsm_map_peek(const char *path, void *extra, size_t extra_cap, siz
 }
 
 // ---- the journal of incremental checkpoints (DESIGN.md §8.6) ----
-// <path> is a version-1 file, the base; <path>.journal holds, all fields little-endian:
-//    0  char magic[8] "DSMJRNL\0"    8  uint32 format version    12  uint32 0    16  uint64 the base's trailing checksum
+// <path> is a version-1 or version-2 file, the base; <path>.journal holds, all fields little-endian:
+//    0  char magic[8] "DSMJRNL\0"    8  uint32 format version    12  uint32 0 (S)    16  uint64 the base's trailing checksum
 //   24  uint64 FNV-1a 64 of the 24 bytes before it
 // then records, each:
 //    0  uint64 sequence (1 for the first record after the base)    8  int32 n_pool, n_store, n_segments
-//   20  int32 k_pool, k_store (chunks listed)    28  uint32 0    32  uint64 extra_bytes
+//   20  int32 k_pool, k_store (chunks listed)    28  uint32 0 (k_views)    32  uint64 extra_bytes
 //   40  int32 pool_chunk[k_pool], int32 store_chunk[k_store]: ascending indices of the 256-surfel chunks that changed
 //       the payloads, in list order: min(256, n - 256 c) dsm_surfel_t of each chunk c (the pool's, then the store's)
 //       int32 table[n_segments][3], uint8 extra[extra_bytes] (both whole)
@@ -446,15 +505,19 @@ extern "C" int dsm_map_peek(const char *path, void *extra, size_t extra_cap, siz
 //       uint64 FNV-1a 64 of every byte of the record before it
 // A record holds every chunk that reaches beyond the previous state's size of its section.  The base is written first
 // (temporary name, rename), then a fresh journal header the same way; a record is appended and flushed to the disk.
+// Version 2 goes beside a version-2 base (DESIGN.md §8.18): the header word at 12 holds the base's rays per view S; a
+// record's word at 28 is k_views, int32 view_slot[k_views] (strictly ascending, the slots captured since the previous
+// state) follows the store's chunk list, and float4 rays[k_views][S] follow the store's payloads.  The resolved views
+// are the base's with every record's slots put in, each replacing the slot's rays.
 namespace
 {
 const char kJournalMagic[8] = {'D', 'S', 'M', 'J', 'R', 'N', 'L', 0};
-const uint32_t kJournalFormat = 1;
+const uint32_t kJournalFormat = 1, kJournalFormatViews = 2;
 
 struct JournalHeader
 {
     char magic[8];
-    uint32_t format, zero;
+    uint32_t format, rays_per_view; // rays_per_view: 0 in version 1
     uint64_t base_checksum;
 };
 static_assert(sizeof(JournalHeader) == 24, "journal header layout");
@@ -463,7 +526,7 @@ struct RecordHeader
 {
     uint64_t sequence;
     int32_t n_pool, n_store, n_segments, k_pool, k_store;
-    uint32_t zero;
+    int32_t k_views; // 0 in version 1
     uint64_t extra_bytes;
 };
 static_assert(sizeof(RecordHeader) == 40, "journal record layout");
@@ -488,10 +551,11 @@ bool list_ok(const int32_t *c, int k, int64_t n, int64_t prev)
 }
 
 // The one resolver: the base read and checked as dsm_map_load reads it, then the records of its journal replayed in
-// order up to the first that is torn, fails its checksum, breaks the chain or is out of sequence.  m holds the version-1
-// file of the resulting state, parsed as a read file is.  A missing journal, or one that names another base, adds no
-// record; a journal of another magic or format is DSM_E_INVALID, and so is a complete record whose chunk lists do not
-// describe its state.
+// order up to the first that is torn, fails its checksum, breaks the chain or is out of sequence.  m holds the file of
+// the resulting state, in the base's version, parsed as a read file is.  A missing journal, or one that names another
+// base, adds no record; a journal of another magic or format is DSM_E_INVALID, and so are a version-2 journal whose rays
+// per view are not the base's, a journal of this base in the other version, and a complete record whose chunk or view
+// lists do not describe its state.
 int resolve(const char *path, MapFile &m, int *records)
 {
     if (records) *records = 0;
@@ -501,13 +565,18 @@ int resolve(const char *path, MapFile &m, int *records)
     if (read_all(journal_path(path).c_str(), j) != DSM_OK || j.size() < sizeof(JournalHeader) + 8) return DSM_OK;
     JournalHeader jh;
     std::memcpy(&jh, j.data(), sizeof(jh));
-    if (std::memcmp(jh.magic, kJournalMagic, 8) != 0 || jh.format != kJournalFormat) return DSM_E_INVALID;
+    if (std::memcmp(jh.magic, kJournalMagic, 8) != 0 || (jh.format != kJournalFormat && jh.format != kJournalFormatViews))
+        return DSM_E_INVALID;
+    const bool views = jh.format == kJournalFormatViews;
+    if (views && (int64_t)jh.rays_per_view != seeds_of(m.hdr)) return DSM_E_INVALID; // never 0
     Fnv1a hs;
     hs.add(j.data(), sizeof(jh));
     uint64_t want = 0, chain = 0;
     std::memcpy(&want, j.data() + sizeof(jh), 8);
     std::memcpy(&chain, m.raw.data() + m.raw.size() - 8, 8);
     if (hs.h != want || jh.base_checksum != chain) return DSM_OK;
+    if (views != (m.rays_per_view > 0)) return DSM_E_INVALID; // the journal of this base, but not of its version
+    const size_t ray_bytes = 16 * (size_t)m.rays_per_view;
 
     MapHeader hdr = m.hdr;
     const uint8_t *mp = reinterpret_cast<const uint8_t *>(m.pool), *ms = reinterpret_cast<const uint8_t *>(m.store);
@@ -515,6 +584,8 @@ int resolve(const char *path, MapFile &m, int *records)
     std::vector<uint8_t> store(ms, ms + (size_t)hdr.n_store * sizeof(dsm_surfel_t));
     std::vector<uint8_t> table(reinterpret_cast<const uint8_t *>(m.table), m.extra);
     std::vector<uint8_t> extra(m.extra, m.extra + hdr.extra_bytes);
+    std::map<int32_t, const uint8_t *> rays; // slot -> its latest rays, in m.raw or j
+    for (int i = 0; i < m.n_views; i++) rays[m.view_slots[i]] = m.view_rays + ray_bytes * i;
     std::vector<int32_t> list;
     int applied = 0;
     size_t pos = sizeof(JournalHeader) + 8;
@@ -525,13 +596,17 @@ int resolve(const char *path, MapFile &m, int *records)
         RecordHeader r;
         if (left < sizeof(r)) break;
         std::memcpy(&r, p, sizeof(r));
-        if (r.n_pool < 0 || r.n_store < 0 || r.n_segments < 0 || r.k_pool < 0 || r.k_store < 0) break;
-        const uint64_t lists = 4 * ((uint64_t)r.k_pool + (uint64_t)r.k_store);
+        if (!views) r.k_views = 0;
+        if (r.n_pool < 0 || r.n_store < 0 || r.n_segments < 0 || r.k_pool < 0 || r.k_store < 0 || r.k_views < 0) break;
+        const uint64_t chunk_lists = 4 * ((uint64_t)r.k_pool + (uint64_t)r.k_store), lists = chunk_lists + 4 * (uint64_t)r.k_views;
         if (r.extra_bytes > left || sizeof(r) + lists > left) break;
-        list.resize((size_t)r.k_pool + r.k_store);
+        if (r.k_views > 0 && ray_bytes > left / (uint64_t)r.k_views) break; // torn
+        const size_t k_chunks = (size_t)r.k_pool + r.k_store;
+        list.resize(k_chunks + r.k_views);
         if (!list.empty()) std::memcpy(list.data(), p + sizeof(r), (size_t)lists);
-        uint64_t payload = 0;
-        for (size_t i = 0; i < list.size(); i++)
+        const int32_t *vslots = list.data() + k_chunks;
+        uint64_t payload = ray_bytes * (uint64_t)r.k_views;
+        for (size_t i = 0; i < k_chunks; i++)
             payload += (uint64_t)chunk_count((int)i < r.k_pool ? r.n_pool : r.n_store, list[i]) * sizeof(dsm_surfel_t);
         const uint64_t len = sizeof(r) + lists + payload + 12 * (uint64_t)r.n_segments + r.extra_bytes + 16;
         if (len > left) break; // torn
@@ -541,18 +616,20 @@ int resolve(const char *path, MapFile &m, int *records)
         std::memcpy(&prev, p + len - 16, 8);
         std::memcpy(&own, p + len - 8, 8);
         if (s.h != own || prev != chain || r.sequence != seq) break;
-        if (!list_ok(list.data(), r.k_pool, r.n_pool, hdr.n_pool) || !list_ok(list.data() + r.k_pool, r.k_store, r.n_store, hdr.n_store))
+        if (!list_ok(list.data(), r.k_pool, r.n_pool, hdr.n_pool) || !list_ok(list.data() + r.k_pool, r.k_store, r.n_store, hdr.n_store) ||
+            !ascending(vslots, r.k_views))
             return DSM_E_INVALID;
         const uint8_t *q = p + sizeof(r) + lists;
         pool.resize((size_t)r.n_pool * sizeof(dsm_surfel_t));
         store.resize((size_t)r.n_store * sizeof(dsm_surfel_t));
-        for (size_t i = 0; i < list.size(); i++)
+        for (size_t i = 0; i < k_chunks; i++)
         {
             const bool in_pool = (int)i < r.k_pool;
             const size_t n = (size_t)chunk_count(in_pool ? r.n_pool : r.n_store, list[i]) * sizeof(dsm_surfel_t);
             std::memcpy((in_pool ? pool : store).data() + (size_t)list[i] * kChunkBytes, q, n);
             q += n;
         }
+        for (int i = 0; i < r.k_views; i++, q += ray_bytes) rays[vslots[i]] = q;
         table.assign(q, q + 12 * (size_t)r.n_segments);
         q += table.size();
         extra.assign(q, q + r.extra_bytes);
@@ -563,10 +640,24 @@ int resolve(const char *path, MapFile &m, int *records)
     }
     if (applied == 0) return DSM_OK;
     std::vector<uint8_t> raw;
-    raw.reserve(sizeof(hdr) + pool.size() + store.size() + table.size() + extra.size() + 8);
+    raw.reserve(sizeof(hdr) + pool.size() + store.size() + table.size() + extra.size() + 8 +
+                (views ? 4 + (4 + ray_bytes) * rays.size() : 0));
     const uint8_t *hb = reinterpret_cast<const uint8_t *>(&hdr);
     raw.insert(raw.end(), hb, hb + sizeof(hdr));
-    for (const std::vector<uint8_t> *v : {&pool, &store, &table, &extra}) raw.insert(raw.end(), v->begin(), v->end());
+    for (const std::vector<uint8_t> *v : {&pool, &store, &table}) raw.insert(raw.end(), v->begin(), v->end());
+    if (views)
+    {
+        const int32_t n = (int32_t)rays.size();
+        const uint8_t *nb = reinterpret_cast<const uint8_t *>(&n);
+        raw.insert(raw.end(), nb, nb + 4);
+        for (const auto &v : rays)
+        {
+            const uint8_t *sb = reinterpret_cast<const uint8_t *>(&v.first);
+            raw.insert(raw.end(), sb, sb + 4);
+        }
+        for (const auto &v : rays) raw.insert(raw.end(), v.second, v.second + ray_bytes);
+    }
+    raw.insert(raw.end(), extra.begin(), extra.end());
     Fnv1a sum;
     sum.add(raw.data(), raw.size());
     const uint8_t *sb = reinterpret_cast<const uint8_t *>(&sum.h);
@@ -578,12 +669,13 @@ int resolve(const char *path, MapFile &m, int *records)
 }
 } // namespace
 
-int dsm_journal_start(const char *path, uint64_t base_checksum, uint64_t *bytes)
+int dsm_journal_start(const char *path, uint64_t base_checksum, int rays_per_view, uint64_t *bytes)
 {
     JournalHeader h;
     std::memset(&h, 0, sizeof(h));
     std::memcpy(h.magic, kJournalMagic, 8);
-    h.format = kJournalFormat;
+    h.format = rays_per_view > 0 ? kJournalFormatViews : kJournalFormat;
+    h.rays_per_view = (uint32_t)std::max(rays_per_view, 0);
     h.base_checksum = base_checksum;
     AtomicFile out(journal_path(path).c_str());
     out.put(&h, sizeof(h));
@@ -617,14 +709,17 @@ int dsm_journal_append(const char *path, uint64_t journal_bytes, const DsmJourna
     std::memset(&h, 0, sizeof(h));
     h.sequence = r.sequence;
     h.n_pool = r.n_pool, h.n_store = r.n_store, h.n_segments = r.n_segments, h.k_pool = r.k_pool, h.k_store = r.k_store;
+    h.k_views = r.k_views;
     h.extra_bytes = r.extra_bytes;
     put(&h, sizeof(h));
     put(r.pool_chunks, 4 * (size_t)r.k_pool);
     put(r.store_chunks, 4 * (size_t)r.k_store);
+    put(r.view_slots, 4 * (size_t)r.k_views);
     for (int i = 0; i < r.k_pool; i++)
         put(r.pool + (size_t)r.pool_chunks[i] * kChunkBytes, (size_t)chunk_count(r.n_pool, r.pool_chunks[i]) * sizeof(dsm_surfel_t));
     for (int i = 0; i < r.k_store; i++)
         put(r.store + (size_t)r.store_chunks[i] * kChunkBytes, (size_t)chunk_count(r.n_store, r.store_chunks[i]) * sizeof(dsm_surfel_t));
+    for (int i = 0; i < r.k_views; i++) put(r.view_rays[i], 16 * (size_t)r.rays_per_view);
     put(r.table, 12 * (size_t)r.n_segments);
     put(r.extra, r.extra_bytes);
     put(&r.prev_checksum, 8);

@@ -1,6 +1,8 @@
 // Private to the library: what the checkpoint file of dsm_io.cpp (dsm_map_save / dsm_map_load) needs to know about a
 // context beyond the C ABI.  Defined in dsm_capi.cu; hidden, so neither is exported.
 #pragma once
+#include <vector>
+
 #include "../../include/dsm.h"
 
 struct DsmMapInfo
@@ -10,6 +12,7 @@ struct DsmMapInfo
     int store_cap;           // the inactive store's reservation in surfels, 0 without one
     bool publish_in_flight;  // a dsm_publish_enqueue snapshot has not been waited for
     bool field_in_flight;    // a dsm_field_enqueue field has not been waited for
+    int view_rays;           // rays per view (dsm_num_seeds) after dsm_checkpoint_views_enable, else 0
 };
 
 __attribute__((visibility("hidden"))) int dsm_map_info(const dsm_ctx *ctx, DsmMapInfo *info);
@@ -17,7 +20,17 @@ __attribute__((visibility("hidden"))) int dsm_map_info(const dsm_ctx *ctx, DsmMa
 __attribute__((visibility("hidden"))) int dsm_inactive_load_check(const dsm_ctx *ctx, const dsm_surfel_t *surfels, int n,
                                                                   const int32_t *kf_ofs_cnt, int n_segments);
 
-// The sections of one checkpoint file, in file order
+// the host-side checks of a views section (DESIGN.md §8.18) in its load order, touching nothing: DSM_E_CAPACITY for a
+// slot >= max_views, DSM_E_INVALID for a ray dsm_views_capture cannot have written
+__attribute__((visibility("hidden"))) int dsm_views_load_check(const dsm_ctx *ctx, const int32_t *slots, int n, const void *rays);
+// Replaces the captured views by slots[0 .. n) with their rays ([n][dsm_num_seeds] float4, packed); every other slot
+// becomes unfilled.  Synchronises.
+__attribute__((visibility("hidden"))) int dsm_views_load(dsm_ctx *ctx, const int32_t *slots, int n, const void *rays);
+// The filled slots, ascending, and their rays packed in that order, read in stream order.  Synchronises.
+__attribute__((visibility("hidden"))) int dsm_views_download(dsm_ctx *ctx, std::vector<int32_t> &slots, std::vector<uint8_t> &rays);
+
+// The sections of one checkpoint file, in file order.  rays_per_view > 0 makes it a version-2 file with a views section
+// of n_views slots (ascending) after the table, view_rays[i] pointing at the rays_per_view float4 of view_slots[i].
 struct DsmMapSections
 {
     const dsm_surfel_t *pool;
@@ -28,6 +41,10 @@ struct DsmMapSections
     int n_segments;
     const void *extra;
     size_t extra_bytes;
+    const int32_t *view_slots;
+    int n_views;
+    const void *const *view_rays;
+    int rays_per_view;
 };
 // The one writer of the file (dsm_io.cpp), for dsm_map_save and the checkpoint thread: header from `info`, the sections,
 // the checksum; under a temporary name, flushed to the disk and renamed over `path`.  DSM_E_IO leaves nothing under path.
@@ -37,9 +54,12 @@ __attribute__((visibility("hidden"))) int dsm_map_write(const char *path, const 
 
 // The journal beside a base file (dsm_checkpoint_enqueue_incremental, DESIGN.md §8.6).  dsm_journal_start replaces
 // <path>.journal by a header that names the base's checksum (temporary name, fsync, rename); *bytes is its length.
-__attribute__((visibility("hidden"))) int dsm_journal_start(const char *path, uint64_t base_checksum, uint64_t *bytes);
+// rays_per_view > 0: the journal of a version-2 base, whose records carry views.
+__attribute__((visibility("hidden"))) int dsm_journal_start(const char *path, uint64_t base_checksum, int rays_per_view, uint64_t *bytes);
 // One record: the chunks of 256 surfels that changed since the previous state, in ascending order, each section's chunk c
 // read at 11264 * c bytes from its base (the last chunk of a section cut at its size), then the whole table and extra.
+// In the journal of a version-2 base, the views captured since the previous state: view_rays[i] points at the
+// rays_per_view float4 of view_slots[i] (ascending).
 struct DsmJournalRecord
 {
     uint64_t sequence, prev_checksum;
@@ -52,6 +72,10 @@ struct DsmJournalRecord
     const int32_t *table;
     const void *extra;
     size_t extra_bytes;
+    const int32_t *view_slots;
+    int k_views;
+    const void *const *view_rays;
+    int rays_per_view;
 };
 // Appends the record to <path>.journal, which must be `journal_bytes` long, and flushes it to the disk.  DSM_E_IO leaves
 // the journal at its old length as far as it can.  *checksum / *bytes: the record's own checksum and its length.

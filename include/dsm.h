@@ -598,6 +598,27 @@ int dsm_field_enqueue_known(dsm_ctx *ctx, const double center[3], int min_update
                             int n_views, int host_copy);
 int dsm_field_state(dsm_ctx *ctx, const uint8_t **state, int *n_free);
 
+/* ---- views in the checkpoint: resume known space (DESIGN.md §8.18) ----
+ * Without this call, checkpoints carry no views and a load leaves the slot table empty, so every known request after a
+ * restart carves nothing.  With it, every checkpoint of the context (dsm_map_save, dsm_checkpoint_enqueue, both kinds of
+ * dsm_checkpoint_enqueue_incremental) carries the ascending list of filled slots and, for each, its S = dsm_num_seeds
+ * rays exactly as dsm_views_capture wrote them (float4, w = 1, or all zero for a seed without a ray).  Poses are the
+ * caller's: it passes them with every known request and keeps them in its own extra section.
+ *   dsm_checkpoint_views_enable  once, after dsm_views_enable (DSM_E_STATE before it and when called twice).  From
+ *                       then on every file is version 2 (a views section, even with no slot filled) and every journal
+ *                       beside such a base carries, per record, exactly the slots captured since the previous checkpoint.
+ *                       Enabling in the middle of an incremental chain makes the next incremental checkpoint a base.
+ *                       With dsm_checkpoint_enable (either order: the second call allocates it) the checkpoint gains a
+ *                       device and a pinned views image of 16 B per ray for max_views x S rays each (28.8 MB each for
+ *                       256 views of 1226x370).  DSM_E_NOMEM with nothing kept.
+ * Loading (dsm_map_load, dsm_map_load_journal) on a context that opted in replaces its views by the file's: slots not in
+ * the file, and every slot for a version-1 file, become unfilled.  Checked before the device is touched: DSM_E_CAPACITY
+ * for a slot >= max_views; DSM_E_INVALID for a ray dsm_views_capture cannot have written (w not 0 or 1, w = 0 with a
+ * non-zero byte, a non-finite coordinate).  On a context that did not opt in, a file with a views section is DSM_E_STATE
+ * and nothing is loaded; views are untouched by a version-1 file.  dsm_map_peek, dsm_map_peek_journal and
+ * dsm_journal_materialize read both versions; materialising a version-2 chain writes the version-2 file of its state. */
+int dsm_checkpoint_views_enable(dsm_ctx *ctx);
+
 /* ---- exploration frontiers: clusters of known-free voxels that border unknown space (DESIGN.md §8.10) ----
  * A frontier job reads the state grid of the latest field request, which must be a known one (any enqueue call, waited
  * for or not), in stream order behind it, with that request's origin o and voxel edge v captured at the job's enqueue; a
@@ -1225,7 +1246,7 @@ int dsm_debug_checkpoint_drain_ctas(dsm_ctx *ctx, int ctas);
  *                           of another magic or format, and for a complete record whose chunk lists are not ascending, reach
  *                           past its sizes or miss a chunk that grows a section.  *records (optional): the records applied.
  *                           Otherwise the errors of dsm_map_load / dsm_map_peek on that state.
- *   dsm_journal_materialize writes the version-1 file of the resolved state to out_path (temporary name, fsync, rename),
+ *   dsm_journal_materialize writes the file of the resolved state, in its base's version, to out_path (temporary name, fsync, rename),
  *                           without a context: what dsm_map_load reads, for archives and export. */
 int dsm_checkpoint_enqueue_incremental(dsm_ctx *ctx, const char *path, const void *extra, size_t extra_bytes);
 int dsm_map_load_journal(dsm_ctx *ctx, const char *path, void *extra, size_t extra_cap, size_t *extra_bytes, int *records);

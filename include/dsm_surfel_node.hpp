@@ -77,8 +77,11 @@
 // first fused frame of each new reference keyframe is captured into slot captures % max_views (its superpixel rays, in
 // camera coordinates) and the node keeps (reference_index, relative) per slot; every field request then carries every
 // filled slot at its current world pose cam_pose[ref] * relative, in fuse_pose's arithmetic, so a loop closure moves the
-// views with the map.  known_space() returns the state grid of the field distance_field() handed out last.  Views are
-// not part of a checkpoint: load_state* empties the slot table, which refills as keyframes are fused.
+// views with the map.  known_space() returns the state grid of the field distance_field() handed out last.  Without
+// enable_view_checkpoints() views are not part of a checkpoint: load_state* empties the slot table, which refills as
+// keyframes are fused.  enable_view_checkpoints(), after enable_known_space, makes every save_state* carry the views
+// (the library's rays, DESIGN.md §8.18, and the node's slot table in its section) and load_state* restore them, so a
+// resumed node carves the same free space as one that never stopped.
 // An exploring planner asks where to look next.  enable_frontiers(max_clusters, max_voxels), after enable_known_space,
 // lets frontiers() find the exploration frontiers of the latest fused frame's known field on the device (DESIGN.md
 // §8.10): the clusters of free voxels that border unknown space, their statistics and member voxels, one enqueue and one
@@ -523,7 +526,19 @@ class SurfelMapNode
     int enable_known_space(int max_views, float max_range)
     {
         if (ctx_.run("enable_known_space", [&] { return dsm_views_enable(ctx_.ctx, max_views, max_range); }) == DSM_OK)
+        {
             known_.assign((size_t)max_views, KnownView{-1, Pose()});
+            known_range_ = max_range;
+        }
+        return ctx_.err;
+    }
+    // once, after enable_known_space (DSM_E_STATE before it): every checkpoint from now on carries the captured views and
+    // the slot table (node section version 2), and every load restores them (DESIGN.md §8.18).  A version-1 section
+    // still loads, with an empty table; a node without this call refuses a version-2 section with DSM_E_INVALID.
+    int enable_view_checkpoints()
+    {
+        if (known_.empty()) return ctx_.done(DSM_E_STATE, "enable_view_checkpoints");
+        if (ctx_.run("enable_view_checkpoints", [&] { return dsm_checkpoint_views_enable(ctx_.ctx); }) == DSM_OK) view_checkpoints_ = true;
         return ctx_.err;
     }
     // the state grid [nz][ny][nx] (0 unknown, 1 occupied, 2 free; the library's pinned buffer, valid until the next frame
@@ -982,8 +997,10 @@ class SurfelMapNode
         last_ref_ = s.last_ref;
         fused_ = s.fused;
         field_exists_ = false; // the loaded map has no field until its next fused frame
-        for (size_t i = 0; i < known_.size(); i++) known_[i].ref = -1; // views are not part of the checkpoint
-        captures_ = 0, captured_ref_ = -1;
+        // a version-2 section restores the slot table the library's views match; without one the table starts empty
+        for (size_t i = 0; i < known_.size(); i++)
+            known_[i] = s.views ? KnownView{s.view_ref[i], s.view_rel[i]} : KnownView{-1, Pose()};
+        captures_ = s.views ? s.captures : 0, captured_ref_ = s.views ? s.captured_ref : -1;
         return ctx_.done(DSM_OK, what);
     }
 
@@ -1003,7 +1020,9 @@ class SurfelMapNode
     //   int32 n_images, per image: double stamp, uint8 gray[H*W];  int32 n_depths, per depth: double stamp, float depth[H*W],
     //   int32 n_warp, per transform: int32 pose, float W[16],
     //   double last_fuse_pose[7], int32 last_ref, int32 fused
-    enum { kSectionVersion = 1 };
+    // version 2 (enable_view_checkpoints) appends: int32 max_views, float max_range, int32 captures, captured_ref,
+    //   per slot: int32 reference_index (-1: empty), double relative[7]
+    enum { kSectionVersion = 1, kSectionVersionViews = 2 };
     struct State
     {
         node_math::M4 transform_kitti;
@@ -1016,6 +1035,10 @@ class SurfelMapNode
         Pose last_fuse_pose;
         int last_ref;
         bool fused;
+        bool views = false; // a version-2 section: the slot table below
+        int captures = 0, captured_ref = -1;
+        std::vector<int> view_ref;
+        std::vector<Pose> view_rel;
     };
     static const char *section_magic() { return "DSMNODE"; } // with its terminating zero: 8 bytes
     struct Writer
@@ -1055,7 +1078,7 @@ class SurfelMapNode
     {
         Writer w = {out};
         w.raw(section_magic(), 8);
-        w.put((uint32_t)kSectionVersion);
+        w.put((uint32_t)(view_checkpoints_ ? kSectionVersionViews : kSectionVersion));
         w.put((int32_t)width_), w.put((int32_t)height_);
         w.raw(cam_, sizeof(cam_));
         w.put((int32_t)drift_free_poses_);
@@ -1081,8 +1104,12 @@ class SurfelMapNode
         w.put((int32_t)last_warp_.size());
         for (size_t i = 0; i < last_warp_.size(); i++) w.put((int32_t)last_warp_[i].pose), w.raw(last_warp_[i].W, sizeof(last_warp_[i].W));
         w.put(last_fuse_pose_), w.put((int32_t)last_ref_), w.put((int32_t)fused_);
+        if (!view_checkpoints_) return;
+        w.put((int32_t)known_.size()), w.put(known_range_), w.put((int32_t)captures_), w.put((int32_t)captured_ref_);
+        for (size_t i = 0; i < known_.size(); i++) w.put((int32_t)known_[i].ref), w.put(known_[i].relative);
     }
-    // false for anything but a section of this version written by a node with this node's parameters
+    // false for anything but a section of version 1, or of version 2 on a node with view checkpoints, written by a node
+    // with this node's parameters (and, in version 2, its max_views and max_range, every slot's keyframe in the database)
     bool read_section(const std::vector<uint8_t> &in, State &s) const
     {
         static_assert(sizeof(Pose) == 56, "Pose: 7 doubles");
@@ -1091,7 +1118,9 @@ class SurfelMapNode
         uint32_t version = 0;
         int32_t w = 0, h = 0, dfp = 0, n = 0;
         double cam[6];
-        if (!r.raw(magic, 8) || std::memcmp(magic, section_magic(), 8) != 0 || !r.get(version) || version != (uint32_t)kSectionVersion) return false;
+        if (!r.raw(magic, 8) || std::memcmp(magic, section_magic(), 8) != 0 || !r.get(version)) return false;
+        s.views = version == (uint32_t)kSectionVersionViews;
+        if (version != (uint32_t)kSectionVersion && !(s.views && view_checkpoints_)) return false;
         if (!r.get(w) || !r.get(h) || !r.raw(cam, sizeof(cam)) || !r.get(dfp)) return false;
         if (w != width_ || h != height_ || std::memcmp(cam, cam_, sizeof(cam)) != 0 || dfp != drift_free_poses_) return false;
         if (!r.raw(s.transform_kitti.d, sizeof(s.transform_kitti.d)) || !r.count(n, 2 * sizeof(Pose) + 12)) return false;
@@ -1148,9 +1177,26 @@ class SurfelMapNode
             s.last_warp[j].pose = pose;
         }
         int32_t ref = 0, fused = 0;
-        if (!r.get(s.last_fuse_pose) || !r.get(ref) || !r.get(fused) || r.o != in.size()) return false;
+        if (!r.get(s.last_fuse_pose) || !r.get(ref) || !r.get(fused)) return false;
         s.last_ref = ref, s.fused = fused != 0;
-        return true;
+        if (s.views)
+        {
+            int32_t max_views = 0, captures = 0, captured_ref = 0;
+            float max_range = 0.f;
+            if (!r.get(max_views) || !r.get(max_range) || !r.get(captures) || !r.get(captured_ref)) return false;
+            if (max_views != (int32_t)known_.size() || std::memcmp(&max_range, &known_range_, 4) != 0 || captures < 0) return false;
+            if (captured_ref < -1 || captured_ref >= n) return false;
+            s.captures = captures, s.captured_ref = captured_ref;
+            s.view_ref.resize((size_t)max_views);
+            s.view_rel.resize((size_t)max_views);
+            for (int32_t j = 0; j < max_views; j++)
+            {
+                int32_t k = 0;
+                if (!r.get(k) || k < -1 || k >= n || !r.get(s.view_rel[(size_t)j])) return false;
+                s.view_ref[(size_t)j] = k;
+            }
+        }
+        return r.o == in.size();
     }
 
     static Point3 position(const Pose &p)
@@ -1314,6 +1360,8 @@ class SurfelMapNode
     };
     std::vector<KnownView> known_; // empty without known space
     int captures_ = 0, captured_ref_ = -1; // captures so far; the reference keyframe of the latest
+    float known_range_ = 0.f;              // enable_known_space's max_range
+    bool view_checkpoints_ = false;        // enable_view_checkpoints: section version 2
     int frontier_clusters_ = 0;            // enable_frontiers' max_clusters
     int reach_targets_ = 0;                // enable_reach's max_targets
 };
