@@ -42,6 +42,7 @@ EXPORTS = [
     "dsm_reach_matrix_wait", "dsm_gain_enable", "dsm_gain_enqueue", "dsm_gain_wait",
     "dsm_tour_enable", "dsm_tour_enqueue", "dsm_tour_wait", "dsm_viewpoint_enable", "dsm_viewpoint_enqueue", "dsm_viewpoint_wait",
     "dsm_trajectory_enable", "dsm_trajectory_enqueue", "dsm_trajectory_wait",
+    "dsm_heading_enable", "dsm_heading_enqueue", "dsm_heading_wait",
     "dsm_inactive_segments", "dsm_inactive_load", "dsm_map_save", "dsm_map_load", "dsm_map_peek",
     "dsm_checkpoint_enable", "dsm_checkpoint_enqueue", "dsm_checkpoint_wait", "dsm_debug_checkpoint_drain_ctas",
     "dsm_checkpoint_enqueue_incremental", "dsm_map_load_journal", "dsm_map_peek_journal", "dsm_journal_materialize",
@@ -111,6 +112,16 @@ TRAJECTORY_DTYPE = np.dtype([("status", "<i4"), ("iterations", "<i4"), ("evaluat
                              ("first_hit", "<i4"), ("n_outside", "<i4"), ("reserved", "<i4", 2)])
 TRAJECTORY_INFO_DTYPE = np.dtype([("origin", "<i4", 3), ("n_trajectories", "<i4"), ("n_points", "<i4"), ("n_status", "<i4", 4),
                                   ("reserved", "<i4", 7)])
+
+# dsm_heading_enqueue's per-trajectory request (16 B) and dsm_heading_wait's records (include/dsm.h): a trajectory (32 B),
+# a sample (32 B), the counts of one (sample, rotation) (8 B) and the header (64 B)
+HEADING_REQUEST_DTYPE = np.dtype([("start", "<i4"), ("end", "<i4"), ("max_step", "<i4"), ("reserved", "<i4")])
+HEADING_DTYPE = np.dtype([("status", "<i4"), ("n_samples", "<i4"), ("sample_offset", "<i4"), ("n_outside", "<i4"), ("score", "<i8"),
+                          ("steps", "<i4"), ("reserved", "<i4")])
+HEADING_SAMPLE_DTYPE = np.dtype([("p", "<f8", 3), ("rotation", "<i4"), ("turn", "<i4")])
+HEADING_COUNT_DTYPE = np.dtype([("n_unknown", "<i4"), ("n_frontier", "<i4")])
+HEADING_INFO_DTYPE = np.dtype([("origin", "<i4", 3), ("n_trajectories", "<i4"), ("n_samples", "<i4"), ("n_rot", "<i4"),
+                               ("unknown_blocks", "<i4"), ("n_status", "<i4", 2), ("reserved", "<i4", 7)])
 
 
 class DsmGainCamera(ctypes.Structure):
@@ -223,6 +234,9 @@ def load_library():
     L.dsm_trajectory_enable.argtypes = [vp, ci, ci, ci]
     L.dsm_trajectory_enqueue.argtypes = [vp, vp, vp, vp, ci, ctypes.POINTER(DsmTrajectoryParams)]
     L.dsm_trajectory_wait.argtypes = [vp, vp, ctypes.POINTER(vp), ctypes.POINTER(vp)]
+    L.dsm_heading_enable.argtypes = [vp, ci, ci]
+    L.dsm_heading_enqueue.argtypes = [vp, vp, vp, ci, ctypes.POINTER(DsmGainCamera), vp, ci, ci, vp, ctypes.c_int32, ctypes.c_int32]
+    L.dsm_heading_wait.argtypes = [vp, vp, ctypes.POINTER(vp), ctypes.POINTER(vp), ctypes.POINTER(vp)]
     L.dsm_inactive_reserve.argtypes = [vp, ci]
     L.dsm_inactive_retire.argtypes = [vp, ci, ctypes.POINTER(ci)]
     L.dsm_inactive_reactivate.argtypes = [vp, ci, ctypes.POINTER(ci)]
@@ -919,6 +933,45 @@ class Context:
         n, n_pts = int(i["n_trajectories"]), int(i["n_points"])
         return self._waited(rc, "trajectory",
                             lambda: (i, _take(pr, n, TRAJECTORY_DTYPE), _take(pp, 3 * n_pts, np.float64).reshape(n_pts, 3)))
+
+    # ---- headings along trajectories against the latest known field ----
+    def heading_enable(self, max_trajectories, max_samples):
+        self._ck(self.lib.dsm_heading_enable(self.h, int(max_trajectories), int(max_samples)))
+
+    def heading_enqueue(self, points, offsets, camera, rotations, samples, requests, w_unknown, w_frontier):
+        """points (P, 3) float64 control points and offsets (n + 1,) int32 as trajectory_enqueue takes them; camera:
+        (fx, fy, cx, cy, width, height, max_range, unknown_blocks); rotations: (n_rot, 9) row-major camera-to-world 3x3
+        matrices, neighbouring headings next to each other, cyclically; samples: K per segment; requests: n
+        HEADING_REQUEST_DTYPE records or (start, end, max_step) rows; integer weights of the unknown and frontier counts."""
+        pts = np.ascontiguousarray(points, np.float64).reshape(-1, 3)
+        ofs = np.ascontiguousarray(offsets, np.int32).reshape(-1)
+        R = np.ascontiguousarray(rotations, np.float64).reshape(-1, 9)
+        req = np.asarray(requests)
+        if req.dtype != HEADING_REQUEST_DTYPE:
+            rows = np.asarray(requests, np.int32).reshape(-1, 3)
+            req = np.zeros(len(rows), HEADING_REQUEST_DTYPE)
+            req["start"], req["end"], req["max_step"] = rows[:, 0], rows[:, 1], rows[:, 2]
+        req = np.ascontiguousarray(req.reshape(-1))
+        if len(ofs) < 2 or len(req) != len(ofs) - 1:
+            raise ValueError(f"{len(req)} requests for {max(len(ofs) - 1, 0)} trajectories")
+        if not 0 <= ofs[-1] <= len(pts):
+            raise ValueError(f"offsets end at {ofs[-1]}, beyond the {len(pts)} points")
+        cam = _camera(camera)
+        self._ck(self.lib.dsm_heading_enqueue(self.h, pts.ctypes.data if len(pts) else None, ofs.ctypes.data, len(ofs) - 1,
+                                              ctypes.byref(cam), R.ctypes.data if len(R) else None, len(R), int(samples),
+                                              req.ctypes.data, int(w_unknown), int(w_frontier)))
+
+    def heading_wait(self):
+        """(info, records, samples, counts): numpy copies of the context's pinned results, a HEADING_INFO_DTYPE record,
+        HEADING_DTYPE (n_trajectories,), HEADING_SAMPLE_DTYPE (n_samples,) and HEADING_COUNT_DTYPE (n_samples, n_rot).  A
+        job on a field taken after a rejected frame raises DsmError(DSM_E_CAPACITY) carrying the same tuple as `.heading`."""
+        pr, ps, pc = ctypes.c_void_p(), ctypes.c_void_p(), ctypes.c_void_p()
+        info = np.zeros(1, HEADING_INFO_DTYPE)
+        rc = self.lib.dsm_heading_wait(self.h, info.ctypes.data, ctypes.byref(pr), ctypes.byref(ps), ctypes.byref(pc))
+        i = info[0]
+        n, S, R = int(i["n_trajectories"]), int(i["n_samples"]), int(i["n_rot"])
+        return self._waited(rc, "heading", lambda: (i, _take(pr, n, HEADING_DTYPE), _take(ps, S, HEADING_SAMPLE_DTYPE),
+                                                    _take(pc, S * R, HEADING_COUNT_DTYPE).reshape(S, R)))
 
     # ---- planner queries against the latest field ----
     def field_query_enable(self, max_points, max_trajectories, max_waypoints):

@@ -2492,6 +2492,22 @@ extern "C" int dsm_trajectory_enable(dsm_ctx *ctx, int max_trajectories, int max
     return keep(ctx->trajectory, tr);
 }
 
+// The control points of n uniform cubic B-splines as the trajectory and heading jobs take them (include/dsm.h):
+// offsets[0] = 0, 7 to 256 points per trajectory, at most max_points in all, every coordinate finite
+static bool spline_points_ok(const double *points, const int32_t *offsets, int n, int max_points)
+{
+    if (offsets[0] != 0) return false;
+    for (int j = 0; j < n; j++)
+    {
+        if (offsets[j + 1] < offsets[j]) return false;
+        const int m = offsets[j + 1] - offsets[j];
+        if (m < 7 || m > DSM_TRAJECTORY_MAX_POINTS || offsets[j + 1] > max_points) return false;
+    }
+    for (size_t c = 0; c < 3 * (size_t)offsets[n]; c++)
+        if (!std::isfinite(points[c])) return false;
+    return true;
+}
+
 static bool traj_params_ok(const dsm_trajectory_params_t &p, int max_memory)
 {
     for (double w : {p.w_smooth, p.w_clear, p.w_feas, p.margin, p.v_max, p.a_max, p.g_tol})
@@ -2512,13 +2528,12 @@ extern "C" int dsm_trajectory_enqueue(dsm_ctx *ctx, const double *points, const 
     if (!tr || !f || !f->requested || !f->signed_latest || tr->in_flight) return DSM_E_STATE;
     if (!points || !offsets || !dt || !params || n_trajectories < 1 || n_trajectories > tr->max_traj) return DSM_E_INVALID;
     const dsm_trajectory_params_t p = *params;
-    if (!traj_params_ok(p, tr->max_memory) || offsets[0] != 0) return DSM_E_INVALID;
+    if (!traj_params_ok(p, tr->max_memory) || !spline_points_ok(points, offsets, n_trajectories, tr->max_points)) return DSM_E_INVALID;
     int nmax = 0;
     unsigned long long samples = 0;
     for (int j = 0; j < n_trajectories; j++)
     {
         const int n = offsets[j + 1] - offsets[j];
-        if (offsets[j + 1] < offsets[j] || n < 7 || n > DSM_TRAJECTORY_MAX_POINTS || offsets[j + 1] > tr->max_points) return DSM_E_INVALID;
         if (!std::isfinite(dt[j]) || !(dt[j] > 0.0)) return DSM_E_INVALID;
         nmax = std::max(nmax, n);
         samples += (unsigned long long)(n - 3) * (unsigned long long)p.samples + 1;
@@ -2527,8 +2542,6 @@ extern "C" int dsm_trajectory_enqueue(dsm_ctx *ctx, const double *points, const 
     if ((unsigned long long)n_points * (unsigned long long)p.max_iter * (unsigned long long)(p.max_ls + 1) > DSM_TRAJECTORY_MAX_WORK ||
         samples > DSM_TRAJECTORY_MAX_SAMPLES)
         return DSM_E_INVALID;
-    for (size_t c = 0; c < 3 * (size_t)n_points; c++)
-        if (!std::isfinite(points[c])) return DSM_E_INVALID;
     // the packed request (dsm_device.cuh); the previous job's copy out of this staging ended before its wait, which no
     // job in flight implies
     uint8_t *h = tr->stage_host;
@@ -2557,6 +2570,143 @@ extern "C" int dsm_trajectory_wait(dsm_ctx *ctx, dsm_trajectory_info_t *info, co
     if (records) *records = reinterpret_cast<const dsm_trajectory_t *>(r);
     if (points) *points = reinterpret_cast<const double *>(r + sizeof(dsm_trajectory_t) * (size_t)tr->n);
     return capacity(ctx, tr->words(), DSM_TRAJ_ERR_TAG, "dsm_trajectory_wait", "the field the job read");
+}
+
+// ---- headings along trajectories against the latest known field (include/dsm.h, DESIGN.md §8.19) ----
+extern "C" int dsm_heading_enable(dsm_ctx *ctx, int max_trajectories, int max_samples)
+{
+    if (!ctx) return DSM_E_INVALID;
+    const DsmField *f = ctx->field.get();
+    if (!f || !ctx->views || ctx->heading) return DSM_E_STATE;
+    if (max_trajectories < 1 || max_trajectories > DSM_HEADING_MAX_CAPACITY || max_samples < 1 || max_samples > DSM_HEADING_MAX_CAPACITY)
+        return DSM_E_INVALID;
+    CK(cudaSetDevice(ctx->device));
+    auto hd = std::make_unique<DsmHeading>();
+    hd->max_traj = max_trajectories, hd->max_samples = max_samples;
+    const size_t stage = dsm_heading_stage_bytes(max_trajectories, max_samples),
+                 res = dsm_heading_res_bytes(max_trajectories, max_samples, DSM_HEADING_MAX_ROTATIONS);
+    CudaOwner &o = hd->own;
+    o.host(&hd->stage_host, stage);
+    o.device(&hd->stage_dev, stage);
+    o.device(&hd->succ, (size_t)DSM_HEADING_MAX_ROTATIONS * max_samples);
+    o.device(&hd->res, res);
+    o.host(&hd->res_host, res);
+    o.event(&hd->ev);
+    return keep(ctx->heading, hd);
+}
+
+// Sample s of the uniform cubic B-spline Q[N][3] at K samples per segment (include/dsm.h: the final-check samples of a
+// trajectory job), each operation rounded once (the host code is built without contraction)
+static void spline_sample(const double *Q, int N, int K, int s, double p[3])
+{
+    const int m = std::min(s / K, N - 4);
+    const double u = (double)(s - m * K) / (double)K, u2 = u * u, u3 = u2 * u, w = 1.0 - u;
+    const double b0 = ((w * w) * w) / 6.0, b1 = ((3.0 * u3 - 6.0 * u2) + 4.0) / 6.0, b2 = (((3.0 * u2 - 3.0 * u3) + 3.0 * u) + 1.0) / 6.0,
+                 b3 = u3 / 6.0;
+    const double *q = Q + 3 * (size_t)m;
+    for (int k = 0; k < 3; k++) p[k] = ((b0 * q[k] + b1 * q[3 + k]) + b2 * q[6 + k]) + b3 * q[9 + k];
+}
+
+// Stages the request on the calling thread (checking it on the way): per sample its position and the hull of gain's
+// boxes over the rotations, then enqueues one H2D copy, the kernels on the state grid of the latest (known) field
+// request, one D2H copy of the used result and the event.  Later field requests overwrite that grid only behind the job.
+extern "C" int dsm_heading_enqueue(dsm_ctx *ctx, const double *points, const int32_t *offsets, int n_trajectories, const dsm_gain_camera_t *camera,
+                                   const double *rotations, int n_rot, int samples, const dsm_heading_request_t *requests, int32_t w_unknown,
+                                   int32_t w_frontier)
+{
+    if (!ctx) return DSM_E_INVALID;
+    DsmHeading *hd = ctx->heading.get();
+    const DsmField *f = known_field(ctx);
+    if (!hd || !f || hd->in_flight) return DSM_E_STATE;
+    if (!points || !offsets || !camera || !rotations || !requests || n_trajectories < 1 || n_trajectories > hd->max_traj) return DSM_E_INVALID;
+    const dsm_gain_camera_t &c = *camera;
+    const double v = (double)f->g.voxel;
+    if (!gain_camera_ok(c, v) || n_rot < 1 || n_rot > DSM_HEADING_MAX_ROTATIONS || samples < 1 || samples > DSM_HEADING_MAX_SAMPLES_PER_SEGMENT ||
+        w_unknown < 0 || w_unknown > DSM_HEADING_MAX_WEIGHT || w_frontier < 0 || w_frontier > DSM_HEADING_MAX_WEIGHT)
+        return DSM_E_INVALID;
+    for (size_t i = 0; i < 9 * (size_t)n_rot; i++)
+        if (!std::isfinite(rotations[i])) return DSM_E_INVALID;
+    if (!spline_points_ok(points, offsets, n_trajectories, INT32_MAX)) return DSM_E_INVALID;
+    long long n_samples = 0;
+    for (int j = 0; j < n_trajectories; j++)
+    {
+        const dsm_heading_request_t &q = requests[j];
+        if (q.start < 0 || q.start >= n_rot || q.end < -1 || q.end >= n_rot || q.max_step < 0 || q.max_step > n_rot) return DSM_E_INVALID;
+        n_samples += (long long)samples * (offsets[j + 1] - offsets[j] - 3) + 1;
+    }
+    const long long m = 2 * (long long)std::ceil((double)c.max_range / v) + 3;
+    if (n_samples > hd->max_samples || n_samples * m * m * m > DSM_HEADING_MAX_WORK) return DSM_E_INVALID;
+    // the packed request (dsm_device.cuh); the previous job's copy out of this staging ended before its wait, which no
+    // job in flight implies
+    uint8_t *h = hd->stage_host;
+    std::memcpy(h, rotations, 72 * (size_t)n_rot);
+    auto *traj = reinterpret_cast<DsmHeadingTraj *>(h + 72 * (size_t)DSM_HEADING_MAX_ROTATIONS);
+    auto *smp = reinterpret_cast<DsmHeadingSample *>(traj + n_trajectories);
+    long long bricks = 0;
+    int s0 = 0;
+    for (int j = 0; j < n_trajectories; j++)
+    {
+        const int N = offsets[j + 1] - offsets[j], S = samples * (N - 3) + 1;
+        DsmHeadingTraj &T = traj[j];
+        T.sample0 = s0, T.n_samples = S, T.start = requests[j].start, T.end = requests[j].end, T.max_step = requests[j].max_step;
+        T.n_outside = 0;
+        for (int s = 0; s < S; s++)
+        {
+            DsmHeadingSample &Z = smp[s0 + s];
+            spline_sample(points + 3 * (size_t)offsets[j], N, samples, s, Z.p);
+            Z.pad = 0;
+            bool inside = true;
+            for (int k = 0; k < 3; k++)
+            {
+                const double q = std::floor(Z.p[k] / v) - (double)f->g.o[k];
+                inside = inside && q >= 0.0 && q < (double)f->g.n[k];
+            }
+            int lo[3] = {INT32_MAX, INT32_MAX, INT32_MAX}, hi[3] = {-1, -1, -1}; // the hull, exclusive of hi
+            for (int r = 0; inside && r < n_rot; r++)
+            {
+                DsmGainView V;
+                for (int a = 0; a < 3; a++)
+                {
+                    for (int b = 0; b < 3; b++) V.P[4 * a + b] = rotations[9 * r + 3 * a + b];
+                    V.P[4 * a + 3] = Z.p[a];
+                }
+                gain_box(V.P, c, f->g, V);
+                if (V.size[0] == 0 || V.size[1] == 0 || V.size[2] == 0) continue;
+                for (int k = 0; k < 3; k++) lo[k] = std::min(lo[k], V.lo[k]), hi[k] = std::max(hi[k], V.lo[k] + V.size[k]);
+            }
+            T.n_outside += !inside;
+            for (int k = 0; k < 3; k++)
+            {
+                Z.lo[k] = hi[k] < 0 ? 0 : lo[k];
+                Z.size[k] = hi[k] < 0 ? 0 : hi[k] - lo[k];
+            }
+            Z.brick0 = (int)bricks; // below 2^31: the work bound caps the bricks far lower
+            bricks += dsm_gain_bricks(Z.size);
+        }
+        s0 += S;
+    }
+    CK(cudaSetDevice(ctx->device));
+    CK(cudaMemcpyAsync(hd->stage_dev, h, dsm_heading_stage_bytes(n_trajectories, s0), cudaMemcpyHostToDevice, ctx->stream));
+    CK(dsm_launch_heading(f->g, f->occ, f->dist, c, hd->stage_dev, n_trajectories, s0, n_rot, bricks, w_unknown, w_frontier, hd->succ,
+                          hd->res, ctx->stream));
+    hd->n = n_trajectories, hd->n_samples = s0, hd->n_rot = n_rot;
+    return submit(ctx, *hd, hd->res, dsm_heading_res_bytes(n_trajectories, s0, n_rot), f->requests);
+}
+
+extern "C" int dsm_heading_wait(dsm_ctx *ctx, dsm_heading_info_t *info, const dsm_heading_t **records, const dsm_heading_sample_t **samples,
+                                const dsm_heading_count_t **counts)
+{
+    if (!ctx) return DSM_E_INVALID;
+    DsmHeading *hd = ctx->heading.get();
+    const int rc = wait_head(ctx, hd);
+    if (rc != DSM_OK) return rc;
+    copy_info(info, hd->words());
+    const auto *r = reinterpret_cast<const dsm_heading_t *>(hd->res_host + 4 * DSM_HEAD_WORDS);
+    const auto *p = reinterpret_cast<const dsm_heading_sample_t *>(r + hd->n);
+    if (records) *records = r;
+    if (samples) *samples = p;
+    if (counts) *counts = reinterpret_cast<const dsm_heading_count_t *>(p + hd->n_samples);
+    return capacity(ctx, hd->words(), DSM_HEAD_ERR_TAG, "dsm_heading_wait", "the field the job read");
 }
 
 // ---- checkpoints that do not stop the stream (include/dsm.h, DESIGN.md §8.5) ----

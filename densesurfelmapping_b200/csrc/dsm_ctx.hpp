@@ -333,6 +333,17 @@ struct DsmTrajectory : DsmJob
     int n = 0, n_points = 0; // of the job in flight or last waited for
 };
 
+// dsm_heading_* (DESIGN.md §8.19), allocated by dsm_heading_enable: the pinned and device staging of the request, the
+// successor table (64 int8 per sample) and the device result
+struct DsmHeading : DsmJob
+{
+    int max_traj = 0, max_samples = 0;
+    uint8_t *stage_host = nullptr, *stage_dev = nullptr; // dsm_heading_stage_bytes(max_traj, max_samples)
+    int8_t *succ = nullptr;
+    uint8_t *res = nullptr;                              // dsm_heading_res_bytes(max_traj, max_samples, 64)
+    int n = 0, n_samples = 0, n_rot = 0; // of the job in flight or last waited for
+};
+
 #define DSM_MAX_CHUNKS 4
 
 struct dsm_ctx
@@ -411,6 +422,7 @@ struct dsm_ctx
     std::unique_ptr<DsmTour> tour;               // nullptr until dsm_tour_enable
     std::unique_ptr<DsmViewpoint> viewpoint;     // nullptr until dsm_viewpoint_enable
     std::unique_ptr<DsmTrajectory> trajectory;   // nullptr until dsm_trajectory_enable
+    std::unique_ptr<DsmHeading> heading;         // nullptr until dsm_heading_enable
     int run_split = 2;          // sub-batches per dsm_batch_run (dsm_set_concurrency)
     // pinned host staging for the small per-batch tables
     float *h_pose = nullptr; // [2B][32]: pose then inverse; first half: the batch calls, second half: the resident stream

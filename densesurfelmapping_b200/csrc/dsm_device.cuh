@@ -763,3 +763,49 @@ inline size_t dsm_trajectory_smem(int nmax) { return 5 * 3 * sizeof(double) * (s
 cudaError_t dsm_launch_trajectory(const double *points, const double *dt, const int32_t *offsets, int n_traj, int nmax, const float *sdist,
                                   const int32_t *field_header, const DsmFieldGrid &g, const dsm_trajectory_params_t &p, double *hist,
                                   uint8_t *res, cudaStream_t st);
+
+// dsm_heading_* (DESIGN.md §8.19), dsm_heading.cu.  One staged request (H2D, dsm_heading_stage_bytes(n, S)):
+//   double rotations[64][9] | DsmHeadingTraj trajectories[n] | DsmHeadingSample samples[S]
+// and one packed result (D2H, dsm_heading_res_bytes(n, S, n_rot)):
+//   int32 header[DSM_HEAD_WORDS] | dsm_heading_t records[n] | dsm_heading_sample_t samples[S] | dsm_heading_count_t counts[S][n_rot]
+// The header's first eleven words are those of dsm_heading_info_t; its last two carry the field's error words, cleared
+// by dsm_heading_wait.
+enum
+{
+    DSM_HEAD_ORIGIN = 0, // 3 words
+    DSM_HEAD_N = 3,
+    DSM_HEAD_N_SAMPLES,
+    DSM_HEAD_N_ROT,
+    DSM_HEAD_UNKNOWN_BLOCKS,
+    DSM_HEAD_N_STATUS,     // 2 words: trajectories per status (k_heading_plan adds)
+    DSM_HEAD_ERR_TAG = 14, // the field header's DSM_FIELD_ERR_TAG / _ERR_FRAME, copied by k_heading_plan
+    DSM_HEAD_ERR_FRAME,
+    DSM_HEAD_WORDS = 16 // 64 B
+};
+// one trajectory as the host stages it: its first sample and samples, the request, and its samples outside the grid
+struct DsmHeadingTraj
+{
+    int32_t sample0, n_samples, start, end, max_step, n_outside;
+}; // 24 B
+// one sample as the host stages it: the camera position, the hull of its gain boxes over the rotations (lo, size; size
+// 0 on an axis: empty, as for a camera outside the grid) and its first brick in the launch
+struct DsmHeadingSample
+{
+    double p[3];
+    int32_t lo[3], size[3], brick0, pad;
+}; // 56 B
+inline size_t dsm_heading_stage_bytes(int n, int n_samples)
+{
+    return 72 * (size_t)DSM_HEADING_MAX_ROTATIONS + sizeof(DsmHeadingTraj) * (size_t)n + sizeof(DsmHeadingSample) * (size_t)n_samples;
+}
+inline size_t dsm_heading_res_bytes(int n, int n_samples, int n_rot)
+{
+    return 4 * (size_t)DSM_HEAD_WORDS + sizeof(dsm_heading_t) * (size_t)n + (sizeof(dsm_heading_sample_t) + sizeof(dsm_heading_count_t) * (size_t)n_rot) * n_samples;
+}
+// The whole job on the state grid of the latest known request (header at dsm_field_header(voxels) of dist) for the
+// request already in `stage` on the device (n trajectories, n_samples samples, n_rot rotations, bricks in all), with
+// the successor table succ of 64 bytes per sample.  Zeroes and writes the whole used result; returns the first launch
+// or memset error.
+cudaError_t dsm_launch_heading(const DsmFieldGrid &g, const uint8_t *state, const int32_t *dist, const dsm_gain_camera_t &cam,
+                               const uint8_t *stage, int n, int n_samples, int n_rot, long long bricks, int w_unknown, int w_frontier,
+                               int8_t *succ, uint8_t *res, cudaStream_t st);

@@ -1190,6 +1190,108 @@ int dsm_viewpoint_enqueue(dsm_ctx *ctx, const dsm_gain_camera_t *camera, const d
 int dsm_viewpoint_wait(dsm_ctx *ctx, dsm_viewpoint_info_t *info, const dsm_viewpoint_cluster_t **clusters,
                        const dsm_viewpoint_t **viewpoints);
 
+/* ---- headings along trajectories: view gain per sample and rotation, then the best rate-limited sequence (DESIGN.md §8.19) ----
+ * A heading job reads the state grid of the latest field request, which must be a known one, in stream order behind
+ * it, with that request's origin o and voxel edge v (widened to fp64) captured at the job's enqueue.  It needs no
+ * frontier job.  A later field request may be enqueued while a job is in flight and does not change what the job reads.
+ * The map is never read.
+ *
+ * Definition (integer counts and int64 scores, so the result does not depend on the schedule; the sample positions fp64
+ * with one rounding per operation).
+ *   Trajectories: the layout of dsm_trajectory_enqueue, control points Q_0 .. Q_{N-1} = points[offsets[j] ..
+ *   offsets[j+1] - 1] of uniform cubic B-splines, 7 <= N <= 256 (dsm_trajectory_wait's optimised points can be passed
+ *   unchanged).
+ *   Samples: the final-check samples of dsm_trajectory_enqueue at K = samples per segment: segment m = 0..N-4 at u =
+ *   (double)s / K, s < K, then the end point (segment N-4 at u = 1); S_j = K (N - 3) + 1 per trajectory, numbered
+ *   from sample_offset in trajectory order; the point ((b0 Q_m + b1 Q_{m+1}) + b2 Q_{m+2}) + b3 Q_{m+3} per axis with
+ *   that entry's basis, evaluated on the host in that order without contraction.
+ *   Rotations: rotations[9 r ..], r < n_rot, row-major 3x3 camera to world as dsm_viewpoint_enqueue takes them.  The list
+ *   is a cycle: r and (r +- 1) mod n_rot are neighbouring headings.
+ *   Counts: n_unknown[s][r] and n_frontier[s][r] are, by definition, the n_unknown and n_frontier of a gain job with
+ *   `camera` on the pose [R_r | p_s]; a sample whose camera voxel floor(p_s / v) - o lies outside the grid counts 0
+ *   and adds to n_outside.  score[s][r] = w_unknown n_unknown + w_frontier n_frontier in int64.  Scores add up per
+ *   sample: a voxel seen from several samples counts once per sample.
+ *   Sequence: r_0 = start; r_{s+1} = (r_s + d_s) mod n_rot with steps d_s in [-max_step, max_step]; with end >= 0,
+ *   r_{S-1} = end.  The plan maximises sum_s score[s][r_s], then minimises sum_s |d_s|; remaining ties go to the first
+ *   d in the order 0, -1, +1, -2, +2, ... taken sample by sample from s = 0 (distinct d count as distinct even when
+ *   they land on the same rotation).  It is a backward pass that keeps the first best successor per (s, r) in that
+ *   order, then a forward trace from start.  Status 0 planned; 1 end cannot be reached from start within the limit:
+ *   every rotation -1, every turn 0, score and steps 0.
+ *   Result: the header; per trajectory its status, n_samples, sample_offset, n_outside, the planned score and steps =
+ *   sum |d_s|; per sample its position, rotation and turn, the cumulative signed steps sum_{k<s} d_k from start (for
+ *   evenly spaced yaws, yaw_s = yaw_start + turn 2 pi / n_rot, unwrapped); per (sample, rotation) the two counts,
+ *   counts[(sample_offset + s) n_rot + r].  The result is 64 + 32 n + 32 S + 8 S n_rot bytes for S samples in all.
+ *   Feasibility: the unwrapped yaws, taken as control points of a uniform cubic B-spline with the ends held at knot
+ *   interval dt / K (dt the position spline's knot interval), change by at most max_step 2 pi / n_rot between
+ *   neighbours, so by the convex-hull property the yaw spline's rate is at most max_step (2 pi / n_rot) K / dt.  That
+ *   is why max_step counts list steps per sample interval.  An end that cannot be reached asks for a longer dt or a
+ *   free end.
+ *
+ *   dsm_heading_enable    once, after dsm_views_enable (DSM_E_STATE otherwise, and when called twice).  DSM_E_INVALID
+ *                         for max_trajectories or max_samples outside [1, 2^22].  Allocates the pinned and device
+ *                         staging, the device successor table (64 B per sample), the device result and its pinned copy
+ *                         of 64 + 32 max_trajectories + 544 max_samples bytes, and an event.  DSM_E_NOMEM with nothing
+ *                         kept.
+ *   dsm_heading_enqueue   stages the request on the calling thread (the samples and, per sample, a box of grid voxels:
+ *                         the hull of gain's boxes over the rotations), then enqueues one H2D copy, the kernels, one D2H
+ *                         copy of the used result and the event; never waits.  DSM_E_STATE before dsm_heading_enable,
+ *                         before any field request, when the latest field request is not a known one, and while a job
+ *                         is in flight.  DSM_E_INVALID for a NULL pointer, n_trajectories outside [1, max_trajectories],
+ *                         offsets[0] != 0, a trajectory of fewer than 7 or more than 256 points, a non-finite control
+ *                         point, gain's camera checks (with its 128 v range cap), n_rot outside [1, 64], a non-finite
+ *                         rotation entry, samples outside [1, 64], a start outside [0, n_rot), an end outside [-1,
+ *                         n_rot), a max_step outside [0, n_rot], a weight outside [0, 2^16], more than max_samples
+ *                         samples, or more than 2^31 voxel visits, sum_s (2 ceil(max_range / v) + 3)^3 (this bounds the
+ *                         work of one call).
+ *   dsm_heading_wait      waits for that job only.  *records (n_trajectories), *samples (n_samples) and *counts
+ *                         (n_samples x n_rot) are the context's pinned results, valid until the next
+ *                         dsm_heading_enqueue; any out-pointer may be NULL.  If the field the job read was taken after a
+ *                         rejected frame, returns DSM_E_CAPACITY with valid results and does NOT clear the error, as
+ *                         dsm_field_wait.  DSM_E_STATE with no job enqueued. */
+typedef struct dsm_heading_request_t
+{
+    int32_t start;                   /* r_0, in [0, n_rot) */
+    int32_t end;                     /* r_{S-1}, in [0, n_rot), or -1: free */
+    int32_t max_step;                /* list steps per sample interval, in [0, n_rot] */
+    int32_t reserved;                /* ignored */
+} dsm_heading_request_t;             /* 16 B */
+typedef struct dsm_heading_t
+{
+    int32_t status;                  /* 0 planned, 1 end unreachable */
+    int32_t n_samples, sample_offset, n_outside;
+    int64_t score;                   /* sum of the planned rotations' scores */
+    int32_t steps;                   /* sum |d_s| */
+    int32_t reserved;                /* 0 */
+} dsm_heading_t;                     /* 32 B */
+typedef struct dsm_heading_sample_t
+{
+    double p[3];                     /* the sample's position, world metres */
+    int32_t rotation;                /* r_s, -1 for status 1 */
+    int32_t turn;                    /* sum of the signed steps before s */
+} dsm_heading_sample_t;              /* 32 B */
+typedef struct dsm_heading_count_t
+{
+    int32_t n_unknown, n_frontier;
+} dsm_heading_count_t;               /* 8 B */
+typedef struct dsm_heading_info_t
+{
+    int32_t origin[3];
+    int32_t n_trajectories, n_samples, n_rot, unknown_blocks;
+    int32_t n_status[2];             /* trajectories per status */
+    int32_t reserved[7];             /* 0 */
+} dsm_heading_info_t;                /* 64 B */
+#define DSM_HEADING_MAX_CAPACITY (1 << 22)
+#define DSM_HEADING_MAX_ROTATIONS 64
+#define DSM_HEADING_MAX_SAMPLES_PER_SEGMENT 64
+#define DSM_HEADING_MAX_WEIGHT (1 << 16)
+#define DSM_HEADING_MAX_WORK (1ll << 31)
+int dsm_heading_enable(dsm_ctx *ctx, int max_trajectories, int max_samples);
+int dsm_heading_enqueue(dsm_ctx *ctx, const double *points, const int32_t *offsets, int n_trajectories, const dsm_gain_camera_t *camera,
+                        const double *rotations, int n_rot, int samples, const dsm_heading_request_t *requests, int32_t w_unknown,
+                        int32_t w_frontier);
+int dsm_heading_wait(dsm_ctx *ctx, dsm_heading_info_t *info, const dsm_heading_t **records, const dsm_heading_sample_t **samples,
+                     const dsm_heading_count_t **counts);
+
 /* ---- checkpoints that do not stop the stream (DESIGN.md §8.5) ----
  * The file of dsm_map_save, taken in stream order like a publish snapshot: the resident stream pays one device-to-device
  * copy of the live map, the transfer to the host runs on a low-priority stream beside the next frames, and a thread of

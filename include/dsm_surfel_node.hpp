@@ -102,6 +102,10 @@
 // candidate camera poses against the latest fused frame's known field on the device (DESIGN.md §8.12): per pose, with
 // the node's own intrinsics, the frustum voxels and the free, unknown, occupied, frontier and (after a frontiers() call
 // on that frame) cluster voxels it would see, one enqueue and one wait.
+// Where should the camera look along the way?  enable_headings(max_trajectories, max_samples), after
+// enable_known_space, lets headings() plan the camera's heading along trajectories on the device (DESIGN.md §8.19): the
+// unknown and frontier voxels seen at every sample and rotation, then the best rate-limited rotation sequence per
+// trajectory, one enqueue and one wait.
 // device < 0 builds the node without a context: the callbacks run the whole pose logic (pose database, sync, window
 // bookkeeping) and fuse nothing; any call that reads the map returns DSM_E_STATE.
 #pragma once
@@ -786,6 +790,42 @@ class SurfelMapNode
                        records.assign(r, r + info.n_trajectories);
                        optimised.assign(q, q + 3 * (size_t)info.n_points);
                    });
+    }
+    // ---- headings along trajectories against the known field of the latest fused frame (DESIGN.md §8.19) ----
+    // once, after enable_known_space: the most trajectories and samples of one headings() call
+    int enable_headings(int max_trajectories, int max_samples)
+    {
+        return ctx_.run("enable_headings", [&] { return dsm_heading_enable(ctx_.ctx, max_trajectories, max_samples); });
+    }
+    // the camera heading along n uniform cubic B-splines (control points xyz doubles and offsets[n + 1], as
+    // trajectories() takes and returns them), sampled `samples` times per segment and scored at n_rot rotations (9
+    // doubles each, row-major camera to world, neighbouring headings next to each other, cyclically) with the node's
+    // intrinsics out to max_range (include/dsm.h): records receives n records, samples_out one position, rotation and
+    // turn per sample, and counts n_rot counts per sample.  DSM_E_STATE without known space, before any field and after
+    // load_state* until the next fused frame; DSM_E_CAPACITY with the results of the last applied frame's field, as
+    // distance_field().
+    int headings(const double *points, const int32_t *offsets, int n, const double *rotations, int n_rot, int samples,
+                 const dsm_heading_request_t *requests, float max_range, int unknown_blocks, int32_t w_unknown, int32_t w_frontier,
+                 dsm_heading_info_t &info, std::vector<dsm_heading_t> &records, std::vector<dsm_heading_sample_t> &samples_out,
+                 std::vector<dsm_heading_count_t> &counts)
+    {
+        records.clear();
+        samples_out.clear();
+        counts.clear();
+        info = dsm_heading_info_t();
+        const dsm_gain_camera_t cam = gain_camera(max_range, unknown_blocks);
+        const dsm_heading_t *r = nullptr;
+        const dsm_heading_sample_t *s = nullptr;
+        const dsm_heading_count_t *c = nullptr;
+        return job(
+            "headings", KNOWN_FIELD, true,
+            [&] { return dsm_heading_enqueue(ctx_.ctx, points, offsets, n, &cam, rotations, n_rot, samples, requests, w_unknown, w_frontier); },
+            [&] { return dsm_heading_wait(ctx_.ctx, &info, &r, &s, &c); },
+            [&] {
+                records.assign(r, r + info.n_trajectories);
+                samples_out.assign(s, s + info.n_samples);
+                counts.assign(c, c + (size_t)info.n_samples * info.n_rot);
+            });
     }
     // the field of the latest fused frame: dist [nz][ny][nx] in metres (the library's pinned buffer, valid until the next
     // frame is fused; nullptr for a field kept on the device), the grid's origin in voxels and the occupied voxels.  DSM_E_STATE when no frame has been fused
