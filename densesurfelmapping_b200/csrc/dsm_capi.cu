@@ -1,6 +1,8 @@
 // Host side of the C ABI declared in include/dsm.h: context, HBM allocation, the per-frame
 // kernel schedule (mirrors FusionFunctions::fuse_initialize_map / generate_super_pixels,
-// fusion_functions.cpp:30-83, :960-975) and the copies either side of it.
+// fusion_functions.cpp:30-83, :960-975) and the copies either side of it; the batch and stream paths, the resident pool
+// and the inactive store, publishing, the distance field with its captured views, checkpoints and the debug readers.
+// Each planner job's entry points live beside its kernels (dsm_field.cu for the queries, dsm_frontier.cu, ...).
 // No CPU implementation of any phase lives here: if CUDA is unavailable every call fails.
 #include "dsm_ctx.hpp"
 #include "dsm_map_state.h"
@@ -1347,74 +1349,6 @@ int dsm_map_info(const dsm_ctx *ctx, DsmMapInfo *info)
     return DSM_OK;
 }
 
-// ---- the lifecycle every snapshot, field and planner job shares ----
-// The end of an enable: the new state is kept when every call of its owner succeeded and `ok`, else nothing is kept and
-// a later call may try again
-template <typename T>
-static int keep(std::unique_ptr<T> &slot, std::unique_ptr<T> &fresh, bool ok = true)
-{
-    if (fresh->own.take() != cudaSuccess || !ok)
-    {
-        cudaGetLastError();
-        return DSM_E_NOMEM; // nothing is kept: a later call may try again
-    }
-    slot = std::move(fresh);
-    return DSM_OK;
-}
-
-// The latest field request if it is a known one (what every job on the known field reads), else nullptr
-static const DsmField *known_field(const dsm_ctx *ctx)
-{
-    const DsmField *f = ctx->field.get();
-    return f && f->requested && f->known ? f : nullptr;
-}
-
-// The pairing rule: the latest job of a kind (frontier, reach) read the latest field request
-static bool read_latest(const DsmJob *j, const DsmField *f) { return j && j->request == f->requests; }
-
-// The tail of an enqueue: one D2H copy of the used result bytes, the job's event, and the job in flight with the field
-// request it read (0 for none)
-static int submit(dsm_ctx *ctx, DsmJob &j, const void *res, size_t bytes, uint64_t request)
-{
-    CK(cudaMemcpyAsync(j.res_host, res, bytes, cudaMemcpyDeviceToHost, ctx->stream));
-    CK(cudaEventRecord(j.ev, ctx->stream));
-    j.in_flight = true;
-    j.request = request;
-    return DSM_OK;
-}
-
-// The head of a wait (a job's or the field's): DSM_E_STATE without a request in flight, else its event waited for and
-// the request retired
-template <typename T>
-static int wait_head(dsm_ctx *ctx, T *j)
-{
-    if (!j || !j->in_flight) return DSM_E_STATE;
-    CK(cudaSetDevice(ctx->device));
-    CK(cudaEventSynchronize(j->ev));
-    j->in_flight = false;
-    return DSM_OK;
-}
-
-// The result of a wait whose header h holds the sticky error word of dsm_fuse_stream_window at h[tag] and the frame it
-// rejected after it: DSM_OK without an error, else DSM_E_CAPACITY with the message that `call`'s `what` holds the frames
-// before that one
-static int capacity(dsm_ctx *ctx, const int32_t *h, int tag, const char *call, const char *what)
-{
-    if (h[tag] == 0) return DSM_OK;
-    snprintf(ctx->err, sizeof(ctx->err), "%s: frame %d of a dsm_fuse_stream_window call did not fit the pool or the store; %s holds "
-             "the frames before it", call, h[tag + 1], what);
-    return DSM_E_CAPACITY;
-}
-
-// An info struct copied out of a result header, its reserved words zeroed
-template <typename Info>
-static void copy_info(Info *info, const int32_t *h)
-{
-    if (!info) return;
-    std::memcpy(info, h, sizeof(Info));
-    for (int32_t &w : info->reserved) w = 0;
-}
-
 // ---- publishing from inside the stream (include/dsm.h) ----
 extern "C" int dsm_publish_enable(dsm_ctx *ctx)
 {
@@ -1633,126 +1567,6 @@ extern "C" int dsm_field_wait(dsm_ctx *ctx, const float **dist, int32_t origin[3
     return capacity(ctx, h, DSM_FIELD_ERR_TAG, "dsm_field_wait", "the field");
 }
 
-// ---- planner queries against the latest field (include/dsm.h, DESIGN.md §8.8) ----
-extern "C" int dsm_field_query_enable(dsm_ctx *ctx, int max_points, int max_trajectories, int max_waypoints)
-{
-    if (!ctx) return DSM_E_INVALID;
-    if (!ctx->field || ctx->field_query) return DSM_E_STATE;
-    for (int n : {max_points, max_trajectories, max_waypoints})
-        if (n < 0 || n > DSM_FIELD_QUERY_MAX_SAMPLES) return DSM_E_INVALID;
-    CK(cudaSetDevice(ctx->device));
-    auto q = std::make_unique<DsmFieldQuery>();
-    q->max_points = max_points, q->max_traj = max_trajectories, q->max_wp = max_waypoints;
-    const size_t req = DsmFieldQuery::req_bytes(max_points, max_waypoints, max_trajectories);
-    const size_t res = DsmFieldQuery::res_bytes(max_points, max_trajectories);
-    q->own.host(&q->req_host, req);
-    q->own.device(&q->req_dev, req);
-    q->own.device(&q->res_dev, res);
-    q->own.host(&q->res_host, res);
-    q->own.event(&q->ev);
-    return keep(ctx->field_query, q);
-}
-
-// Stages the request on the calling thread (checking it and counting the samples on the way), then enqueues one H2D
-// copy, the two kernels on the grid of the latest field request (sgn: on its signed grid), one D2H copy of the results
-// and the event.
-static int field_query_enqueue(dsm_ctx *ctx, bool sgn, const double *points, int n_points, const double *waypoints, const int32_t *offsets,
-                               int n_trajectories, float step, float radius)
-{
-    if (!ctx) return DSM_E_INVALID;
-    DsmFieldQuery *q = ctx->field_query.get();
-    const DsmField *f = ctx->field.get();
-    if (!q || !f || !f->requested || q->in_flight) return DSM_E_STATE;
-    if (sgn && !f->signed_latest) return DSM_E_STATE;
-    if (n_points < 0 || n_points > q->max_points || n_trajectories < 0 || n_trajectories > q->max_traj) return DSM_E_INVALID;
-    if ((n_points > 0 && !points) || (n_trajectories > 0 && (!waypoints || !offsets))) return DSM_E_INVALID;
-    if (!std::isfinite(step) || !(step > 0.f) || !std::isfinite(radius) || !(radius >= 0.f)) return DSM_E_INVALID;
-    const int n_wp = n_trajectories > 0 ? offsets[n_trajectories] : 0;
-    if (n_trajectories > 0)
-    {
-        if (offsets[0] != 0 || n_wp > q->max_wp) return DSM_E_INVALID;
-        for (int j = 0; j < n_trajectories; j++)
-            if (offsets[j + 1] <= offsets[j]) return DSM_E_INVALID;
-    }
-    // the packed request (dsm_device.cuh)
-    uint8_t *h = q->req_host;
-    double *h_pts = reinterpret_cast<double *>(h), *h_wp = h_pts + 3 * (size_t)n_points;
-    int32_t *h_ofs = reinterpret_cast<int32_t *>(h_wp + 3 * (size_t)n_wp), *h_first = h_ofs + n_trajectories + 1;
-    if (n_points > 0) std::memcpy(h_pts, points, 24 * (size_t)n_points);
-    // one pass over the waypoints: copy, check, and count each segment's samples m = max(1, ceil(L / step)).  The
-    // ceil is an integer test, exact once q = L / step is known to be at most 2^26 (a NaN or infinite q fails that).
-    const double dstep = (double)step;
-    int64_t total = 0; // samples of the call so far
-    for (int j = 0; j < n_trajectories; j++)
-    {
-        const int w0 = offsets[j], w1 = offsets[j + 1];
-        int64_t s = 0; // samples of trajectory j so far
-        for (int w = w0; w < w1; w++)
-        {
-            const double *a = waypoints + 3 * (size_t)w;
-            double *c = h_wp + 3 * (size_t)w;
-            c[0] = a[0], c[1] = a[1], c[2] = a[2];
-            if (!std::isfinite(a[0]) || !std::isfinite(a[1]) || !std::isfinite(a[2])) return DSM_E_INVALID;
-            h_first[w] = (int32_t)s;
-            int64_t m = 1; // the last waypoint: one sample
-            if (w + 1 < w1)
-            {
-                const double *b = a + 3;
-                const double dx = b[0] - a[0], dy = b[1] - a[1], dz = b[2] - a[2];
-                const double q = std::sqrt((dx * dx + dy * dy) + dz * dz) / dstep;
-                if (!(q <= (double)DSM_FIELD_QUERY_MAX_SAMPLES)) return DSM_E_INVALID;
-                m = (int64_t)q;
-                m += (double)m < q;
-                m = std::max<int64_t>(m, 1);
-            }
-            if (m > DSM_FIELD_QUERY_MAX_SAMPLES - total - s) return DSM_E_INVALID;
-            s += m;
-        }
-        total += s;
-    }
-    if (n_trajectories > 0) std::memcpy(h_ofs, offsets, 4 * ((size_t)n_trajectories + 1));
-    CK(cudaSetDevice(ctx->device));
-    const size_t req = DsmFieldQuery::req_bytes(n_points, n_wp, n_trajectories);
-    CK(cudaMemcpyAsync(q->req_dev, q->req_host, req, cudaMemcpyHostToDevice, ctx->stream));
-    const double *d_pts = reinterpret_cast<const double *>(q->req_dev), *d_wp = d_pts + 3 * (size_t)n_points;
-    const int32_t *d_ofs = reinterpret_cast<const int32_t *>(d_wp + 3 * (size_t)n_wp), *d_first = d_ofs + n_trajectories + 1;
-    int32_t *r_hdr = reinterpret_cast<int32_t *>(q->res_dev);
-    float4 *r_samples = reinterpret_cast<float4 *>(q->res_dev + 16);
-    dsm_clearance_t *r_clear = reinterpret_cast<dsm_clearance_t *>(q->res_dev + DsmFieldQuery::res_clearance(n_points));
-    // a known field's query view holds its site count where a plain field's header holds its occupied count; the signed
-    // grid's header holds it in the same word
-    const int32_t *grid = sgn ? f->sgn->grid : f->dist;
-    const int32_t *f_hdr = grid + dsm_field_header(f->voxels) + (!sgn && f->known ? DSM_FIELD_VIEW : 0);
-    dsm_launch_field_query(sgn, reinterpret_cast<const float *>(grid), f_hdr, f->g, d_pts, n_points, d_wp, d_ofs, d_first, n_trajectories,
-                           radius, r_hdr, r_samples, r_clear, ctx->stream);
-    CK(cudaGetLastError());
-    q->n_points = n_points, q->n_traj = n_trajectories;
-    return submit(ctx, *q, q->res_dev, DsmFieldQuery::res_bytes(n_points, n_trajectories), f->requests);
-}
-
-extern "C" int dsm_field_query_enqueue(dsm_ctx *ctx, const double *points, int n_points, const double *waypoints, const int32_t *offsets,
-                                       int n_trajectories, float step, float radius)
-{
-    return field_query_enqueue(ctx, false, points, n_points, waypoints, offsets, n_trajectories, step, radius);
-}
-
-extern "C" int dsm_field_query_enqueue_signed(dsm_ctx *ctx, const double *points, int n_points, const double *waypoints,
-                                              const int32_t *offsets, int n_trajectories, float step, float radius)
-{
-    return field_query_enqueue(ctx, true, points, n_points, waypoints, offsets, n_trajectories, step, radius);
-}
-
-extern "C" int dsm_field_query_wait(dsm_ctx *ctx, const dsm_field_sample_t **samples, const dsm_clearance_t **clearance)
-{
-    if (!ctx) return DSM_E_INVALID;
-    DsmFieldQuery *q = ctx->field_query.get();
-    const int rc = wait_head(ctx, q);
-    if (rc != DSM_OK) return rc;
-    if (samples) *samples = reinterpret_cast<const dsm_field_sample_t *>(q->res_host + 16);
-    if (clearance) *clearance = reinterpret_cast<const dsm_clearance_t *>(q->res_host + DsmFieldQuery::res_clearance(q->n_points));
-    return capacity(ctx, q->words(), DSM_QUERY_ERR_TAG, "dsm_field_query_wait", "the field the query read");
-}
-
 // ---- free versus unknown space: captured views and the known-space field (include/dsm.h, DESIGN.md §8.9) ----
 extern "C" int dsm_views_enable(dsm_ctx *ctx, int max_views, float max_range)
 {
@@ -1946,767 +1760,6 @@ extern "C" int dsm_debug_field_load_state(dsm_ctx *ctx, const uint8_t *state, co
     f->signed_latest = sgrid != nullptr;
     f->requests++;
     return DSM_OK;
-}
-
-// ---- exploration frontiers of the latest known field (include/dsm.h, DESIGN.md §8.10) ----
-extern "C" int dsm_frontier_enable(dsm_ctx *ctx, int max_clusters, int max_voxels)
-{
-    if (!ctx) return DSM_E_INVALID;
-    const DsmField *f = ctx->field.get();
-    if (!f || !ctx->views || ctx->frontier) return DSM_E_STATE;
-    for (int n : {max_clusters, max_voxels})
-        if (n < 0 || n > DSM_FRONTIER_MAX_CAPACITY) return DSM_E_INVALID;
-    CK(cudaSetDevice(ctx->device));
-    auto fr = std::make_unique<DsmFrontier>();
-    DsmFrontierBufs &b = fr->b;
-    const int *n = f->g.n;
-    b.voxels = (int)f->voxels;
-    // every 2x2x2 block of voxels is 26-connected, so it meets at most one component
-    b.max_comp = ((n[0] + 1) / 2) * ((n[1] + 1) / 2) * ((n[2] + 1) / 2);
-    b.max_clusters = max_clusters, b.max_voxels = max_voxels;
-    const size_t cl = (size_t)std::max(max_clusters, 1), vx = (size_t)std::max(max_voxels, 1);
-    const size_t sel = (size_t)dsm_frontier_sel_blocks(b.voxels);
-    const size_t res = DsmFrontierBufs::res_bytes(max_clusters, max_voxels);
-    CudaOwner &o = fr->own;
-    o.device(&b.label, f->voxels);
-    for (int32_t **p : {&b.roots, &b.count, &b.cmap, &b.cid}) o.device(p, (size_t)b.max_comp);
-    for (int32_t **p : {&b.slot_comp, &b.sizes, &b.offs}) o.device(p, cl);
-    o.device(&b.acc, cl);
-    o.device(&b.idx, vx);
-    o.device(&b.keys, vx);
-    o.device(&b.keys_alt, vx);
-    o.device(&b.blk, sel);
-    o.device(&b.blk_ofs, sel);
-    o.device(&b.res, res);
-    o.host(&fr->res_host, res);
-    o.event(&fr->ev);
-    b.temp_bytes = dsm_frontier_temp_bytes(b);
-    if (b.temp_bytes) o.device(reinterpret_cast<uint8_t **>(&b.temp), b.temp_bytes);
-    return keep(ctx->frontier, fr, b.temp_bytes != 0);
-}
-
-// Enqueue only: the job on the state grid of the latest (known) field request with that request's origin, one D2H copy
-// of the result capacity and the event.  A later field request clears that grid only behind the job, in stream order.
-extern "C" int dsm_frontier_enqueue(dsm_ctx *ctx, int min_voxels)
-{
-    if (!ctx) return DSM_E_INVALID;
-    DsmFrontier *fr = ctx->frontier.get();
-    const DsmField *f = known_field(ctx);
-    if (!fr || !f || fr->in_flight) return DSM_E_STATE;
-    if (min_voxels < 1) return DSM_E_INVALID;
-    CK(cudaSetDevice(ctx->device));
-    const DsmFrontierBufs &b = fr->b;
-    CK(cudaMemsetAsync(b.res, 0, 4 * DSM_FRONTIER_WORDS, ctx->stream));
-    CK(dsm_launch_frontier(b, f->g, f->occ, f->dist + dsm_field_header(f->voxels), min_voxels, ctx->stream));
-    return submit(ctx, *fr, b.res, DsmFrontierBufs::res_bytes(b.max_clusters, b.max_voxels), f->requests);
-}
-
-extern "C" int dsm_frontier_wait(dsm_ctx *ctx, const dsm_frontier_cluster_t **clusters, const int32_t **voxels, dsm_frontier_counts_t *counts)
-{
-    if (!ctx) return DSM_E_INVALID;
-    DsmFrontier *fr = ctx->frontier.get();
-    const int rc = wait_head(ctx, fr);
-    if (rc != DSM_OK) return rc;
-    const int32_t *h = fr->words();
-    const size_t table = 4 * DSM_FRONTIER_WORDS;
-    if (clusters) *clusters = reinterpret_cast<const dsm_frontier_cluster_t *>(fr->res_host + table);
-    if (voxels)
-        *voxels = reinterpret_cast<const int32_t *>(fr->res_host + table + sizeof(dsm_frontier_cluster_t) * (size_t)fr->b.max_clusters);
-    if (counts) std::memcpy(counts, h, sizeof(dsm_frontier_counts_t));
-    return capacity(ctx, h, DSM_FRONTIER_ERR_TAG, "dsm_frontier_wait", "the field the job read");
-}
-
-// ---- paths through known free space (include/dsm.h, DESIGN.md §8.11) ----
-extern "C" int dsm_reach_enable(dsm_ctx *ctx, int max_targets, int max_path_voxels, int max_rounds)
-{
-    if (!ctx) return DSM_E_INVALID;
-    const DsmField *f = ctx->field.get();
-    if (!f || !ctx->views || ctx->reach) return DSM_E_STATE;
-    for (int n : {max_targets, max_path_voxels})
-        if (n < 0 || n > DSM_REACH_MAX_CAPACITY) return DSM_E_INVALID;
-    if (max_rounds < 1 || max_rounds > DSM_REACH_MAX_ROUNDS || f->voxels > (size_t)DSM_REACH_MAX_VOXELS) return DSM_E_INVALID;
-    CK(cudaSetDevice(ctx->device));
-    auto re = std::make_unique<DsmReach>();
-    DsmReachBufs &b = re->b;
-    b.voxels = (int)f->voxels;
-    for (int k = 0; k < 3; k++) b.tn[k] = (f->g.n[k] + DSM_REACH_TILE - 1) / DSM_REACH_TILE;
-    b.tiles = b.tn[0] * b.tn[1] * b.tn[2];
-    b.max_targets = max_targets, b.max_path = max_path_voxels, b.max_rounds = max_rounds;
-    b.ctas = dsm_reach_ctas();
-    const size_t tg = (size_t)std::max(max_targets, 1);
-    const size_t res = DsmReachBufs::res_bytes(max_targets, max_path_voxels);
-    CudaOwner &o = re->own;
-    o.device(&b.trav, f->voxels);
-    for (uint32_t **p : {&b.cost[0], &b.cost[1]}) o.device(p, f->voxels);
-    for (int32_t **p : {&b.stamp, &b.sched[0], &b.sched[1]}) o.device(p, (size_t)b.tiles);
-    o.device(&b.count, 3);
-    o.device(&b.goals, 3 * tg);
-    o.device(&b.best, tg);
-    o.device(&b.member, tg);
-    o.device(&b.len, tg);
-    o.device(&b.ofs, tg);
-    o.device(&b.res, res);
-    o.host(&re->goals_host, 3 * tg);
-    o.host(&re->res_host, res);
-    o.host(&re->cost_host, f->voxels);
-    o.event(&re->ev);
-    b.temp_bytes = dsm_reach_temp_bytes(b);
-    if (b.temp_bytes) o.device(reinterpret_cast<uint8_t **>(&b.temp), b.temp_bytes);
-    return keep(ctx->reach, re, b.ctas > 0 && b.temp_bytes != 0);
-}
-
-// floor(p / (double)v) - o, clamped to [-1, n]: outside the grid stays outside
-static int reach_voxel(double p, float v, int o, int n)
-{
-    const double q = std::floor(p / (double)v) - (double)o;
-    return q < 0.0 ? -1 : q >= (double)n ? n : (int)q;
-}
-
-// Enqueue only: the goal voxels staged and copied, the job on the grids of the latest (known) field request and, with
-// frontiers, on the latest frontier job's device result, one D2H copy of the result capacity (and of the cost grid with
-// host_copy) and the event.  Later field and frontier requests overwrite those buffers only behind the job.
-extern "C" int dsm_reach_enqueue(dsm_ctx *ctx, const double start[3], float radius, int approach, const double *goals, int n_goals,
-                                 int with_frontiers, int host_copy)
-{
-    if (!ctx) return DSM_E_INVALID;
-    DsmReach *re = ctx->reach.get();
-    const DsmField *f = known_field(ctx);
-    if (!re || !f || re->in_flight) return DSM_E_STATE;
-    const DsmFrontier *fr = ctx->frontier.get();
-    if (with_frontiers && !read_latest(fr, f)) return DSM_E_STATE;
-    DsmReachBufs &b = re->b;
-    if (!start || !std::isfinite(radius) || !(radius >= 0.f) || approach < 0 || approach > DSM_REACH_MAX_APPROACH || n_goals < 0 ||
-        n_goals > b.max_targets || (n_goals > 0 && !goals))
-        return DSM_E_INVALID;
-    for (int k = 0; k < 3; k++)
-        if (!std::isfinite(start[k])) return DSM_E_INVALID;
-    for (size_t i = 0; i < 3 * (size_t)n_goals; i++)
-        if (!std::isfinite(goals[i])) return DSM_E_INVALID;
-    const DsmFieldGrid &g = f->g;
-    CK(cudaSetDevice(ctx->device));
-    // the previous job's copy out of this staging ended before its wait, which no job in flight implies
-    for (size_t i = 0; i < 3 * (size_t)n_goals; i++) re->goals_host[i] = reach_voxel(goals[i], g.voxel, g.o[i % 3], g.n[i % 3]);
-    if (n_goals > 0) CK(cudaMemcpyAsync(b.goals, re->goals_host, 12 * (size_t)n_goals, cudaMemcpyHostToDevice, ctx->stream));
-    const int3 s = make_int3(reach_voxel(start[0], g.voxel, g.o[0], g.n[0]), reach_voxel(start[1], g.voxel, g.o[1], g.n[1]),
-                             reach_voxel(start[2], g.voxel, g.o[2], g.n[2]));
-    CK(cudaMemsetAsync(b.res, 0, 4 * DSM_REACH_WORDS, ctx->stream));
-    CK(dsm_launch_reach(b, g, f->occ, f->dist, s, radius, approach, n_goals, with_frontiers ? fr->b.res : nullptr,
-                        with_frontiers ? fr->b.max_clusters : 0, ctx->stream));
-    if (host_copy) CK(cudaMemcpyAsync(re->cost_host, b.cost[0], 4 * (size_t)b.voxels, cudaMemcpyDeviceToHost, ctx->stream));
-    re->host_copy = host_copy != 0;
-    return submit(ctx, *re, b.res, DsmReachBufs::res_bytes(b.max_targets, b.max_path), f->requests);
-}
-
-extern "C" int dsm_reach_wait(dsm_ctx *ctx, dsm_reach_info_t *info, const dsm_reach_target_t **targets, const int32_t **path,
-                              const uint32_t **cost)
-{
-    if (!ctx) return DSM_E_INVALID;
-    DsmReach *re = ctx->reach.get();
-    const int rc = wait_head(ctx, re);
-    if (rc != DSM_OK) return rc;
-    const size_t table = 4 * DSM_REACH_WORDS;
-    copy_info(info, re->words());
-    if (targets) *targets = reinterpret_cast<const dsm_reach_target_t *>(re->res_host + table);
-    if (path) *path = reinterpret_cast<const int32_t *>(re->res_host + table + sizeof(dsm_reach_target_t) * (size_t)re->b.max_targets);
-    if (cost) *cost = re->host_copy ? re->cost_host : nullptr;
-    return capacity(ctx, re->words(), DSM_REACH_ERR_TAG, "dsm_reach_wait", "the field the job read");
-}
-
-// ---- travel costs between many sites (include/dsm.h, DESIGN.md §8.13) ----
-extern "C" int dsm_reach_matrix_enable(dsm_ctx *ctx, int max_sites, int max_tiles, int max_rounds)
-{
-    if (!ctx) return DSM_E_INVALID;
-    const DsmField *f = ctx->field.get();
-    if (!f || !ctx->views || ctx->reach_matrix) return DSM_E_STATE;
-    int tn[3];
-    for (int k = 0; k < 3; k++) tn[k] = (f->g.n[k] + DSM_REACH_TILE - 1) / DSM_REACH_TILE;
-    const long long tiles = (long long)tn[0] * tn[1] * tn[2];
-    if (max_sites < 1 || max_sites > DSM_REACH_MATRIX_MAX_SITES || max_tiles < 1 || max_tiles > tiles || max_rounds < 1 ||
-        max_rounds > DSM_REACH_MAX_ROUNDS || f->voxels > (size_t)DSM_REACH_MAX_VOXELS ||
-        4096ull * (unsigned long long)max_sites * (unsigned long long)max_tiles > DSM_REACH_MATRIX_MAX_COST_BYTES)
-        return DSM_E_INVALID;
-    CK(cudaSetDevice(ctx->device));
-    auto rm = std::make_unique<DsmReachMatrix>();
-    DsmReachMatrixBufs &b = rm->b;
-    b.voxels = (int)f->voxels;
-    for (int k = 0; k < 3; k++) b.tn[k] = tn[k];
-    b.tiles = (int)tiles;
-    b.max_sites = max_sites, b.max_tiles = max_tiles, b.max_rounds = max_rounds;
-    b.ctas = dsm_reach_matrix_ctas();
-    const size_t items = (size_t)max_sites * max_tiles, res = DsmReachMatrixBufs::res_bytes(max_sites);
-    CudaOwner &o = rm->own;
-    for (int32_t **p : {&b.flag, &b.scan, &b.slot}) o.device(p, (size_t)b.tiles);
-    o.device(&b.mask, 16 * (size_t)b.tiles);
-    o.device(&b.tile_of, (size_t)max_tiles);
-    for (uint32_t **p : {&b.cost[0], &b.cost[1]}) o.device(p, items * 512);
-    for (int32_t **p : {&b.stamp, &b.sched[0], &b.sched[1]}) o.device(p, items);
-    o.device(&b.count, 3 * (size_t)max_sites);
-    for (int32_t **p : {&b.rounds, &b.reached}) o.device(p, (size_t)max_sites);
-    o.device(&b.sites, 3 * (size_t)max_sites);
-    o.device(&b.res, res);
-    o.host(&rm->sites_host, 3 * (size_t)max_sites);
-    o.host(&rm->res_host, res);
-    o.event(&rm->ev);
-    b.temp_bytes = dsm_reach_matrix_temp_bytes(b);
-    if (b.temp_bytes) o.device(reinterpret_cast<uint8_t **>(&b.temp), b.temp_bytes);
-    return keep(ctx->reach_matrix, rm, b.ctas > 0 && b.temp_bytes != 0);
-}
-
-// Enqueue only: the points' voxels staged and copied, the job on the grids of the latest (known) field request, one D2H
-// copy of the n-site result and the event.  A later field request overwrites those grids only behind the job.
-extern "C" int dsm_reach_matrix_enqueue(dsm_ctx *ctx, const double *points, int n_points, float radius, int approach)
-{
-    if (!ctx) return DSM_E_INVALID;
-    DsmReachMatrix *rm = ctx->reach_matrix.get();
-    const DsmField *f = known_field(ctx);
-    if (!rm || !f || rm->in_flight) return DSM_E_STATE;
-    DsmReachMatrixBufs &b = rm->b;
-    if (!points || !std::isfinite(radius) || !(radius >= 0.f) || approach < 0 || approach > DSM_REACH_MAX_APPROACH || n_points < 1 ||
-        n_points > b.max_sites ||
-        (unsigned long long)n_points * (unsigned long long)b.max_tiles * (unsigned long long)b.max_rounds > DSM_REACH_MATRIX_MAX_WORK)
-        return DSM_E_INVALID;
-    for (size_t i = 0; i < 3 * (size_t)n_points; i++)
-        if (!std::isfinite(points[i])) return DSM_E_INVALID;
-    const DsmFieldGrid &g = f->g;
-    CK(cudaSetDevice(ctx->device));
-    // the previous job's copy out of this staging ended before its wait, which no job in flight implies
-    for (size_t i = 0; i < 3 * (size_t)n_points; i++) rm->sites_host[i] = reach_voxel(points[i], g.voxel, g.o[i % 3], g.n[i % 3]);
-    CK(cudaMemcpyAsync(b.sites, rm->sites_host, 12 * (size_t)n_points, cudaMemcpyHostToDevice, ctx->stream));
-    CK(cudaMemsetAsync(b.res, 0, 4 * DSM_RM_WORDS, ctx->stream));
-    CK(dsm_launch_reach_matrix(b, g, f->occ, f->dist, n_points, radius, approach, ctx->stream));
-    rm->n_sites = n_points;
-    return submit(ctx, *rm, b.res, DsmReachMatrixBufs::res_bytes(n_points), f->requests);
-}
-
-extern "C" int dsm_reach_matrix_wait(dsm_ctx *ctx, dsm_reach_matrix_info_t *info, const dsm_reach_site_t **sites, const uint32_t **matrix)
-{
-    if (!ctx) return DSM_E_INVALID;
-    DsmReachMatrix *rm = ctx->reach_matrix.get();
-    const int rc = wait_head(ctx, rm);
-    if (rc != DSM_OK) return rc;
-    const size_t table = 4 * DSM_RM_WORDS;
-    copy_info(info, rm->words());
-    if (sites) *sites = reinterpret_cast<const dsm_reach_site_t *>(rm->res_host + table);
-    if (matrix) *matrix = reinterpret_cast<const uint32_t *>(rm->res_host + table + sizeof(dsm_reach_site_t) * (size_t)rm->n_sites);
-    return capacity(ctx, rm->words(), DSM_RM_ERR_TAG, "dsm_reach_matrix_wait", "the field the job read");
-}
-
-// ---- view gain against the latest known field (include/dsm.h, DESIGN.md §8.12) ----
-extern "C" int dsm_gain_enable(dsm_ctx *ctx, int max_views)
-{
-    if (!ctx) return DSM_E_INVALID;
-    const DsmField *f = ctx->field.get();
-    if (!f || !ctx->views || ctx->gain) return DSM_E_STATE;
-    if (max_views < 1 || max_views > DSM_GAIN_MAX_VIEWS) return DSM_E_INVALID;
-    CK(cudaSetDevice(ctx->device));
-    auto ga = std::make_unique<DsmGain>();
-    ga->max_views = max_views;
-    const size_t res = DsmGain::res_bytes(max_views);
-    CudaOwner &o = ga->own;
-    o.device(&ga->views_dev, (size_t)max_views);
-    o.host(&ga->views_host, (size_t)max_views);
-    o.device(&ga->slot, f->voxels);
-    o.device(&ga->res, res);
-    o.host(&ga->res_host, res);
-    o.event(&ga->ev);
-    return keep(ctx->gain, ga);
-}
-
-// The grid voxels of view P's box: the bounding box of the image pyramid cut at depth max_range (the apex t and the
-// four image corners (0 | width, 0 | height) at depth max_range) met with the cube around the range sphere, one voxel
-// of padding, clipped to the grid.  Every centre that passes the frustum test lies in the truncated pyramid and in the
-// sphere, so the box sizes the work and cannot change a count.  The pyramid holds them only for a rotation: a pose whose
-// 3x3 part is not orthonormal within 1e-6 per entry of R^T R - I, or a corner that does not come out finite, leaves
-// the cube alone (within that tolerance the pyramid moves by far less than the padding).
-static void gain_box(const double *P, const dsm_gain_camera_t &c, const DsmFieldGrid &g, DsmGainView &V)
-{
-    const double R = (double)c.max_range, v = (double)g.voxel;
-    double plo[3], phi[3];
-    bool finite = true;
-    for (int a = 0; a < 3; a++)
-        for (int b = 0; b < 3; b++)
-            finite = finite && std::fabs(((P[a] * P[b] + P[4 + a] * P[4 + b]) + P[8 + a] * P[8 + b]) - (a == b ? 1.0 : 0.0)) <= 1e-6;
-    for (int k = 0; k < 3; k++) plo[k] = phi[k] = P[4 * k + 3];
-    for (int cu = 0; cu < 2; cu++)
-        for (int cw = 0; cw < 2; cw++)
-        {
-            const double qx = ((cu ? (double)c.width : 0.0) - c.cx) / c.fx * R, qy = ((cw ? (double)c.height : 0.0) - c.cy) / c.fy * R;
-            for (int k = 0; k < 3; k++)
-            {
-                const double p = ((P[4 * k] * qx + P[4 * k + 1] * qy) + P[4 * k + 2] * R) + P[4 * k + 3];
-                finite = finite && std::isfinite(p);
-                plo[k] = std::min(plo[k], p);
-                phi[k] = std::max(phi[k], p);
-            }
-        }
-    for (int k = 0; k < 3; k++)
-    {
-        double lo = P[4 * k + 3] - R, hi = P[4 * k + 3] + R;
-        if (finite) lo = std::max(lo, plo[k]), hi = std::min(hi, phi[k]);
-        const double a = std::max(std::floor(lo / v) - 1.0 - (double)g.o[k], 0.0);
-        const double b = std::min(std::floor(hi / v) + 1.0 - (double)g.o[k], (double)(g.n[k] - 1));
-        V.lo[k] = a <= b ? (int)a : 0;
-        V.size[k] = a <= b ? (int)(b - a) + 1 : 0;
-    }
-}
-
-// gain's camera checks (include/dsm.h): intrinsics, image size, the blocking rule and a range of at most 128 voxels
-static bool gain_camera_ok(const dsm_gain_camera_t &c, double v)
-{
-    const double R = (double)c.max_range;
-    return std::isfinite(c.fx) && c.fx > 0.0 && std::isfinite(c.fy) && c.fy > 0.0 && std::isfinite(c.cx) && std::isfinite(c.cy) &&
-           c.width >= 1 && c.width <= 65536 && c.height >= 1 && c.height <= 65536 && (c.unknown_blocks == 0 || c.unknown_blocks == 1) &&
-           std::isfinite(R) && R > 0.0 && R <= DSM_GAIN_MAX_RANGE_VOXELS * v;
-}
-
-// Enqueue only: the views staged (pose, box, cluster and first brick) and copied, the kernels on the state grid of the
-// latest (known) field request and, with clusters, on the latest frontier job's device result, one D2H copy of the used
-// result and the event.  Later field and frontier requests overwrite those buffers only behind the job.
-extern "C" int dsm_gain_enqueue(dsm_ctx *ctx, const dsm_gain_camera_t *camera, const double *poses, const int32_t *clusters, int n_views)
-{
-    if (!ctx) return DSM_E_INVALID;
-    DsmGain *ga = ctx->gain.get();
-    const DsmField *f = known_field(ctx);
-    if (!ga || !f || ga->in_flight) return DSM_E_STATE;
-    const DsmFrontier *fr = ctx->frontier.get();
-    if (clusters && !read_latest(fr, f)) return DSM_E_STATE;
-    if (!camera || n_views < 0 || n_views > ga->max_views || (n_views > 0 && !poses)) return DSM_E_INVALID;
-    const dsm_gain_camera_t &c = *camera;
-    const double v = (double)f->g.voxel, R = (double)c.max_range;
-    if (!gain_camera_ok(c, v)) return DSM_E_INVALID;
-    const long long m = 2 * (long long)std::ceil(R / v) + 3;
-    if ((long long)n_views * m * m * m > DSM_GAIN_MAX_WORK) return DSM_E_INVALID;
-    for (size_t i = 0; i < 12 * (size_t)n_views; i++)
-        if (!std::isfinite(poses[i])) return DSM_E_INVALID;
-    if (clusters)
-        for (int j = 0; j < n_views; j++)
-            if (clusters[j] < -1) return DSM_E_INVALID;
-    CK(cudaSetDevice(ctx->device));
-    // the previous job's copy out of this staging ended before its wait, which no job in flight implies
-    long long bricks = 0;
-    for (int j = 0; j < n_views; j++)
-    {
-        DsmGainView &V = ga->views_host[j];
-        std::memcpy(V.P, poses + 12 * (size_t)j, sizeof(V.P));
-        gain_box(V.P, c, f->g, V);
-        V.cluster = clusters ? clusters[j] : -1;
-        V.brick0 = (int)bricks; // below 2^31: the work bound caps the bricks far lower
-        bricks += dsm_gain_bricks(V.size);
-    }
-    if (n_views > 0) CK(cudaMemcpyAsync(ga->views_dev, ga->views_host, sizeof(DsmGainView) * (size_t)n_views, cudaMemcpyHostToDevice, ctx->stream));
-    CK(dsm_launch_gain(f->g, f->occ, f->dist, c, ga->views_dev, n_views, bricks, clusters ? fr->b.res : nullptr,
-                       clusters ? fr->b.max_clusters : 0, ga->slot, ga->res, ctx->stream));
-    return submit(ctx, *ga, ga->res, DsmGain::res_bytes(n_views), f->requests);
-}
-
-extern "C" int dsm_gain_wait(dsm_ctx *ctx, dsm_gain_info_t *info, const dsm_view_gain_t **gains)
-{
-    if (!ctx) return DSM_E_INVALID;
-    DsmGain *ga = ctx->gain.get();
-    const int rc = wait_head(ctx, ga);
-    if (rc != DSM_OK) return rc;
-    copy_info(info, ga->words());
-    if (gains) *gains = reinterpret_cast<const dsm_view_gain_t *>(ga->res_host + 4 * DSM_GAIN_WORDS);
-    return capacity(ctx, ga->words(), DSM_GAIN_ERR_TAG, "dsm_gain_wait", "the field the job read");
-}
-
-// ---- viewpoints of frontier clusters (include/dsm.h, DESIGN.md §8.15) ----
-extern "C" int dsm_viewpoint_enable(dsm_ctx *ctx, int max_clusters, int max_candidates)
-{
-    if (!ctx) return DSM_E_INVALID;
-    const DsmField *f = ctx->field.get();
-    if (!f || !ctx->views || ctx->viewpoint) return DSM_E_STATE;
-    if (max_clusters < 1 || max_clusters > DSM_VIEWPOINT_MAX_CLUSTERS || max_candidates < 1 || max_candidates > DSM_VIEWPOINT_MAX_CANDIDATES)
-        return DSM_E_INVALID;
-    CK(cudaSetDevice(ctx->device));
-    auto vp = std::make_unique<DsmViewpoint>();
-    DsmViewpointBufs &b = vp->b;
-    b.max_clusters = max_clusters, b.max_candidates = max_candidates;
-    b.ctas = dsm_viewpoint_ctas();
-    const size_t stage = DsmViewpointBufs::stage_bytes(max_clusters), res = DsmViewpointBufs::res_bytes(max_clusters, DSM_VIEWPOINT_MAX_TOP_K);
-    CudaOwner &o = vp->own;
-    o.device(&b.stage, stage);
-    o.host(&vp->stage_host, stage);
-    o.device(&b.cl, (size_t)max_clusters);
-    o.device(&b.key, (size_t)max_candidates);
-    o.device(&b.list, (size_t)max_candidates);
-    o.device(&b.count, 1);
-    o.device(&b.res, res);
-    o.host(&vp->res_host, res);
-    o.event(&vp->ev);
-    return keep(ctx->viewpoint, vp, b.ctas > 0);
-}
-
-// The offsets of include/dsm.h in their order, written as (dx, dy, dz) triples to out (room for
-// DSM_VIEWPOINT_MAX_OFFSETS); returns their number, or -1 past that room.
-static int viewpoint_offsets(const dsm_viewpoint_params_t &p, int32_t *out)
-{
-    int n = 0;
-    const int r = p.r_max / p.stride * p.stride, h = p.dz_max / p.stride * p.stride;
-    for (int dz = -h; dz <= h; dz += p.stride)
-        for (int dy = -r; dy <= r; dy += p.stride)
-            for (int dx = -r; dx <= r; dx += p.stride)
-            {
-                const int q = dx * dx + dy * dy;
-                if (q < p.r_min * p.r_min || q > p.r_max * p.r_max) continue;
-                if (n == DSM_VIEWPOINT_MAX_OFFSETS) return -1;
-                out[3 * n] = dx, out[3 * n + 1] = dy, out[3 * n + 2] = dz;
-                n++;
-            }
-    return n;
-}
-
-// Enqueue only: the rotations, offsets and clusters staged and copied, the kernels on the grids of the latest (known)
-// field request, the latest frontier job's device result and (with_reach) the latest reach job's cost grid, one D2H copy
-// of the used result and the event.  Later field, frontier and reach requests overwrite those buffers only behind the
-// job.
-extern "C" int dsm_viewpoint_enqueue(dsm_ctx *ctx, const dsm_gain_camera_t *camera, const double *rotations, int n_rotations,
-                                     const int32_t *clusters, int n_clusters, const dsm_viewpoint_params_t *params)
-{
-    if (!ctx) return DSM_E_INVALID;
-    DsmViewpoint *vp = ctx->viewpoint.get();
-    const DsmField *f = known_field(ctx);
-    if (!vp || !f || vp->in_flight) return DSM_E_STATE;
-    const DsmFrontier *fr = ctx->frontier.get();
-    if (!read_latest(fr, f)) return DSM_E_STATE;
-    if (!camera || !params || !rotations || n_rotations < 1 || n_rotations > DSM_VIEWPOINT_MAX_ROTATIONS || n_clusters < 0 ||
-        n_clusters > vp->b.max_clusters || (n_clusters > 0 && !clusters))
-        return DSM_E_INVALID;
-    const dsm_gain_camera_t &c = *camera;
-    const dsm_viewpoint_params_t &p = *params;
-    if (!gain_camera_ok(c, (double)f->g.voxel)) return DSM_E_INVALID;
-    if (p.r_min < 0 || p.r_min > p.r_max || p.r_max > DSM_VIEWPOINT_MAX_RADIUS || p.dz_max < 0 || p.dz_max > DSM_VIEWPOINT_MAX_DZ ||
-        p.stride < 1 || p.stride > DSM_VIEWPOINT_MAX_STRIDE || p.max_samples < 1 || p.max_samples > DSM_VIEWPOINT_MAX_SAMPLES ||
-        p.min_seen < 0 || p.top_k < 1 || p.top_k > DSM_VIEWPOINT_MAX_TOP_K || (p.with_reach != 0 && p.with_reach != 1) ||
-        !std::isfinite(p.radius) || !(p.radius >= 0.f))
-        return DSM_E_INVALID;
-    for (size_t i = 0; i < 9 * (size_t)n_rotations; i++)
-        if (!std::isfinite(rotations[i])) return DSM_E_INVALID;
-    for (int i = 0; i < n_clusters; i++)
-        if (clusters[i] < 0) return DSM_E_INVALID;
-    // the previous job's copy out of this staging ended before its wait, which no job in flight implies
-    int32_t *offsets = reinterpret_cast<int32_t *>(vp->stage_host + DsmViewpointBufs::stage_off());
-    const int n_offsets = viewpoint_offsets(p, offsets);
-    if (n_offsets < 1 || (long long)n_clusters * n_offsets > vp->b.max_candidates ||
-        (long long)n_clusters * n_offsets * p.max_samples > DSM_VIEWPOINT_MAX_WORK)
-        return DSM_E_INVALID;
-    const DsmReach *re = ctx->reach.get();
-    if (p.with_reach && !read_latest(re, f)) return DSM_E_STATE;
-    CK(cudaSetDevice(ctx->device));
-    std::memcpy(vp->stage_host, rotations, 72 * (size_t)n_rotations);
-    if (n_clusters > 0) std::memcpy(vp->stage_host + DsmViewpointBufs::stage_clusters(), clusters, 4 * (size_t)n_clusters);
-    CK(cudaMemcpyAsync(vp->b.stage, vp->stage_host, DsmViewpointBufs::stage_bytes(n_clusters), cudaMemcpyHostToDevice, ctx->stream));
-    CK(dsm_launch_viewpoint(vp->b, f->g, f->occ, f->dist, c, p, n_rotations, n_clusters, n_offsets, fr->b.res, fr->b.max_clusters,
-                            p.with_reach ? re->b.cost[0] : nullptr, ctx->stream));
-    vp->n_clusters = n_clusters, vp->top_k = p.top_k;
-    return submit(ctx, *vp, vp->b.res, DsmViewpointBufs::res_bytes(n_clusters, p.top_k), f->requests);
-}
-
-extern "C" int dsm_viewpoint_wait(dsm_ctx *ctx, dsm_viewpoint_info_t *info, const dsm_viewpoint_cluster_t **clusters,
-                                  const dsm_viewpoint_t **viewpoints)
-{
-    if (!ctx) return DSM_E_INVALID;
-    DsmViewpoint *vp = ctx->viewpoint.get();
-    const int rc = wait_head(ctx, vp);
-    if (rc != DSM_OK) return rc;
-    const size_t table = 4 * DSM_VP_WORDS;
-    copy_info(info, vp->words());
-    if (clusters) *clusters = reinterpret_cast<const dsm_viewpoint_cluster_t *>(vp->res_host + table);
-    if (viewpoints)
-        *viewpoints = reinterpret_cast<const dsm_viewpoint_t *>(vp->res_host + table + sizeof(dsm_viewpoint_cluster_t) * (size_t)vp->n_clusters);
-    return capacity(ctx, vp->words(), DSM_VP_ERR_TAG, "dsm_viewpoint_wait", "the field the job read");
-}
-
-// ---- the order of an exploration tour (include/dsm.h, DESIGN.md §8.14) ----
-extern "C" int dsm_tour_enable(dsm_ctx *ctx, int max_sites, int max_starts)
-{
-    if (!ctx) return DSM_E_INVALID;
-    if (ctx->tour) return DSM_E_STATE;
-    if (max_sites < 1 || max_sites > DSM_TOUR_MAX_SITES || max_starts < 1 || max_starts > DSM_TOUR_MAX_STARTS) return DSM_E_INVALID;
-    CK(cudaSetDevice(ctx->device));
-    auto tr = std::make_unique<DsmTour>();
-    tr->max_sites = max_sites, tr->max_starts = max_starts;
-    const size_t entries = (size_t)max_sites * max_sites, res = dsm_tour_res_bytes(max_starts, max_sites);
-    CudaOwner &o = tr->own;
-    o.host(&tr->matrix_host, entries);
-    o.device(&tr->matrix, entries);
-    o.device(&tr->tours, (size_t)max_starts * max_sites);
-    o.device(&tr->res, res);
-    o.host(&tr->res_host, res);
-    o.event(&tr->ev);
-    return keep(ctx->tour, tr);
-}
-
-// Enqueue only: the matrix staged and copied, the kernels, one D2H copy of the used result and the event.
-extern "C" int dsm_tour_enqueue(dsm_ctx *ctx, const uint32_t *matrix, int n, int open, int n_starts, int max_passes, uint64_t seed)
-{
-    if (!ctx) return DSM_E_INVALID;
-    DsmTour *tr = ctx->tour.get();
-    if (!tr || tr->in_flight) return DSM_E_STATE;
-    if (!matrix || n < 1 || n > tr->max_sites || n_starts < 1 || n_starts > tr->max_starts || (open != 0 && open != 1) ||
-        max_passes < 0 || max_passes > DSM_TOUR_MAX_PASSES ||
-        (unsigned long long)n_starts * (unsigned long long)max_passes * (unsigned long long)n * (unsigned long long)n > DSM_TOUR_MAX_WORK)
-        return DSM_E_INVALID;
-    CK(cudaSetDevice(ctx->device));
-    // the previous job's copy out of this staging ended before its wait, which no job in flight implies
-    const size_t bytes = 4 * (size_t)n * n;
-    std::memcpy(tr->matrix_host, matrix, bytes);
-    CK(cudaMemcpyAsync(tr->matrix, tr->matrix_host, bytes, cudaMemcpyHostToDevice, ctx->stream));
-    CK(dsm_launch_tour(tr->matrix, n, open, n_starts, max_passes, seed, tr->tours, tr->res, ctx->stream));
-    tr->n = n, tr->n_starts = n_starts;
-    return submit(ctx, *tr, tr->res, dsm_tour_res_bytes(n_starts, n), 0);
-}
-
-extern "C" int dsm_tour_wait(dsm_ctx *ctx, dsm_tour_info_t *info, const dsm_tour_start_t **starts, const int32_t **order)
-{
-    if (!ctx) return DSM_E_INVALID;
-    DsmTour *tr = ctx->tour.get();
-    const int rc = wait_head(ctx, tr);
-    if (rc != DSM_OK) return rc;
-    if (info) std::memcpy(info, tr->res_host, sizeof(dsm_tour_info_t));
-    if (starts) *starts = reinterpret_cast<const dsm_tour_start_t *>(tr->res_host + sizeof(dsm_tour_info_t));
-    if (order) *order = reinterpret_cast<const int32_t *>(tr->res_host + sizeof(dsm_tour_info_t) + sizeof(dsm_tour_start_t) * (size_t)tr->n_starts);
-    return DSM_OK;
-}
-
-// ---- trajectory optimisation on the signed grid (include/dsm.h, DESIGN.md §8.17) ----
-extern "C" int dsm_trajectory_enable(dsm_ctx *ctx, int max_trajectories, int max_points, int max_memory)
-{
-    if (!ctx) return DSM_E_INVALID;
-    const DsmField *f = ctx->field.get();
-    if (!f || !f->sgn || ctx->trajectory) return DSM_E_STATE;
-    if (max_trajectories < 1 || max_trajectories > DSM_TRAJECTORY_MAX_CAPACITY || max_points < 1 || max_points > DSM_TRAJECTORY_MAX_CAPACITY ||
-        max_memory < 1 || max_memory > DSM_TRAJECTORY_MAX_MEMORY)
-        return DSM_E_INVALID;
-    CK(cudaSetDevice(ctx->device));
-    auto tr = std::make_unique<DsmTrajectory>();
-    tr->max_traj = max_trajectories, tr->max_points = max_points, tr->max_memory = max_memory;
-    const size_t stage = dsm_trajectory_stage_bytes(max_points, max_trajectories), res = dsm_trajectory_res_bytes(max_points, max_trajectories);
-    CudaOwner &o = tr->own;
-    o.host(&tr->stage_host, stage);
-    o.device(&tr->stage_dev, stage);
-    o.device(&tr->hist, 6 * (size_t)max_memory * max_points);
-    o.device(&tr->res, res);
-    o.host(&tr->res_host, res);
-    o.event(&tr->ev);
-    return keep(ctx->trajectory, tr);
-}
-
-// The control points of n uniform cubic B-splines as the trajectory and heading jobs take them (include/dsm.h):
-// offsets[0] = 0, 7 to 256 points per trajectory, at most max_points in all, every coordinate finite
-static bool spline_points_ok(const double *points, const int32_t *offsets, int n, int max_points)
-{
-    if (offsets[0] != 0) return false;
-    for (int j = 0; j < n; j++)
-    {
-        if (offsets[j + 1] < offsets[j]) return false;
-        const int m = offsets[j + 1] - offsets[j];
-        if (m < 7 || m > DSM_TRAJECTORY_MAX_POINTS || offsets[j + 1] > max_points) return false;
-    }
-    for (size_t c = 0; c < 3 * (size_t)offsets[n]; c++)
-        if (!std::isfinite(points[c])) return false;
-    return true;
-}
-
-static bool traj_params_ok(const dsm_trajectory_params_t &p, int max_memory)
-{
-    for (double w : {p.w_smooth, p.w_clear, p.w_feas, p.margin, p.v_max, p.a_max, p.g_tol})
-        if (!std::isfinite(w) || !(w >= 0.0)) return false;
-    return p.max_iter >= 0 && p.max_iter <= DSM_TRAJECTORY_MAX_ITER && p.memory >= 1 && p.memory <= max_memory && p.max_ls >= 1 &&
-           p.max_ls <= DSM_TRAJECTORY_MAX_LS && p.samples >= 1 && p.samples <= DSM_TRAJECTORY_MAX_SAMPLES_PER_SEGMENT &&
-           std::isfinite(p.radius) && p.radius >= 0.f;
-}
-
-// Stages the request on the calling thread (checking it on the way), then enqueues one H2D copy, the kernel on the
-// signed grid of the latest field request, one D2H copy of the used result and the event.
-extern "C" int dsm_trajectory_enqueue(dsm_ctx *ctx, const double *points, const int32_t *offsets, const double *dt, int n_trajectories,
-                                      const dsm_trajectory_params_t *params)
-{
-    if (!ctx) return DSM_E_INVALID;
-    DsmTrajectory *tr = ctx->trajectory.get();
-    const DsmField *f = ctx->field.get();
-    if (!tr || !f || !f->requested || !f->signed_latest || tr->in_flight) return DSM_E_STATE;
-    if (!points || !offsets || !dt || !params || n_trajectories < 1 || n_trajectories > tr->max_traj) return DSM_E_INVALID;
-    const dsm_trajectory_params_t p = *params;
-    if (!traj_params_ok(p, tr->max_memory) || !spline_points_ok(points, offsets, n_trajectories, tr->max_points)) return DSM_E_INVALID;
-    int nmax = 0;
-    unsigned long long samples = 0;
-    for (int j = 0; j < n_trajectories; j++)
-    {
-        const int n = offsets[j + 1] - offsets[j];
-        if (!std::isfinite(dt[j]) || !(dt[j] > 0.0)) return DSM_E_INVALID;
-        nmax = std::max(nmax, n);
-        samples += (unsigned long long)(n - 3) * (unsigned long long)p.samples + 1;
-    }
-    const int n_points = offsets[n_trajectories];
-    if ((unsigned long long)n_points * (unsigned long long)p.max_iter * (unsigned long long)(p.max_ls + 1) > DSM_TRAJECTORY_MAX_WORK ||
-        samples > DSM_TRAJECTORY_MAX_SAMPLES)
-        return DSM_E_INVALID;
-    // the packed request (dsm_device.cuh); the previous job's copy out of this staging ended before its wait, which no
-    // job in flight implies
-    uint8_t *h = tr->stage_host;
-    std::memcpy(h, points, 24 * (size_t)n_points);
-    std::memcpy(h + 24 * (size_t)n_points, dt, 8 * (size_t)n_trajectories);
-    std::memcpy(h + 24 * (size_t)n_points + 8 * (size_t)n_trajectories, offsets, 4 * ((size_t)n_trajectories + 1));
-    CK(cudaSetDevice(ctx->device));
-    CK(cudaMemcpyAsync(tr->stage_dev, h, dsm_trajectory_stage_bytes(n_points, n_trajectories), cudaMemcpyHostToDevice, ctx->stream));
-    const double *d_pts = reinterpret_cast<const double *>(tr->stage_dev), *d_dt = d_pts + 3 * (size_t)n_points;
-    const int32_t *d_ofs = reinterpret_cast<const int32_t *>(d_dt + n_trajectories);
-    const int32_t *grid = f->sgn->grid;
-    CK(dsm_launch_trajectory(d_pts, d_dt, d_ofs, n_trajectories, nmax, reinterpret_cast<const float *>(grid), grid + dsm_field_header(f->voxels),
-                             f->g, p, tr->hist, tr->res, ctx->stream));
-    tr->n = n_trajectories, tr->n_points = n_points;
-    return submit(ctx, *tr, tr->res, dsm_trajectory_res_bytes(n_points, n_trajectories), f->requests);
-}
-
-extern "C" int dsm_trajectory_wait(dsm_ctx *ctx, dsm_trajectory_info_t *info, const dsm_trajectory_t **records, const double **points)
-{
-    if (!ctx) return DSM_E_INVALID;
-    DsmTrajectory *tr = ctx->trajectory.get();
-    const int rc = wait_head(ctx, tr);
-    if (rc != DSM_OK) return rc;
-    copy_info(info, tr->words());
-    const uint8_t *r = tr->res_host + 4 * DSM_TRAJ_WORDS;
-    if (records) *records = reinterpret_cast<const dsm_trajectory_t *>(r);
-    if (points) *points = reinterpret_cast<const double *>(r + sizeof(dsm_trajectory_t) * (size_t)tr->n);
-    return capacity(ctx, tr->words(), DSM_TRAJ_ERR_TAG, "dsm_trajectory_wait", "the field the job read");
-}
-
-// ---- headings along trajectories against the latest known field (include/dsm.h, DESIGN.md §8.19) ----
-extern "C" int dsm_heading_enable(dsm_ctx *ctx, int max_trajectories, int max_samples)
-{
-    if (!ctx) return DSM_E_INVALID;
-    const DsmField *f = ctx->field.get();
-    if (!f || !ctx->views || ctx->heading) return DSM_E_STATE;
-    if (max_trajectories < 1 || max_trajectories > DSM_HEADING_MAX_CAPACITY || max_samples < 1 || max_samples > DSM_HEADING_MAX_CAPACITY)
-        return DSM_E_INVALID;
-    CK(cudaSetDevice(ctx->device));
-    auto hd = std::make_unique<DsmHeading>();
-    hd->max_traj = max_trajectories, hd->max_samples = max_samples;
-    const size_t stage = dsm_heading_stage_bytes(max_trajectories, max_samples),
-                 res = dsm_heading_res_bytes(max_trajectories, max_samples, DSM_HEADING_MAX_ROTATIONS);
-    CudaOwner &o = hd->own;
-    o.host(&hd->stage_host, stage);
-    o.device(&hd->stage_dev, stage);
-    o.device(&hd->succ, (size_t)DSM_HEADING_MAX_ROTATIONS * max_samples);
-    o.device(&hd->res, res);
-    o.host(&hd->res_host, res);
-    o.event(&hd->ev);
-    return keep(ctx->heading, hd);
-}
-
-// Sample s of the uniform cubic B-spline Q[N][3] at K samples per segment (include/dsm.h: the final-check samples of a
-// trajectory job), each operation rounded once (the host code is built without contraction)
-static void spline_sample(const double *Q, int N, int K, int s, double p[3])
-{
-    const int m = std::min(s / K, N - 4);
-    const double u = (double)(s - m * K) / (double)K, u2 = u * u, u3 = u2 * u, w = 1.0 - u;
-    const double b0 = ((w * w) * w) / 6.0, b1 = ((3.0 * u3 - 6.0 * u2) + 4.0) / 6.0, b2 = (((3.0 * u2 - 3.0 * u3) + 3.0 * u) + 1.0) / 6.0,
-                 b3 = u3 / 6.0;
-    const double *q = Q + 3 * (size_t)m;
-    for (int k = 0; k < 3; k++) p[k] = ((b0 * q[k] + b1 * q[3 + k]) + b2 * q[6 + k]) + b3 * q[9 + k];
-}
-
-// Stages the request on the calling thread (checking it on the way): per sample its position and the hull of gain's
-// boxes over the rotations, then enqueues one H2D copy, the kernels on the state grid of the latest (known) field
-// request, one D2H copy of the used result and the event.  Later field requests overwrite that grid only behind the job.
-extern "C" int dsm_heading_enqueue(dsm_ctx *ctx, const double *points, const int32_t *offsets, int n_trajectories, const dsm_gain_camera_t *camera,
-                                   const double *rotations, int n_rot, int samples, const dsm_heading_request_t *requests, int32_t w_unknown,
-                                   int32_t w_frontier)
-{
-    if (!ctx) return DSM_E_INVALID;
-    DsmHeading *hd = ctx->heading.get();
-    const DsmField *f = known_field(ctx);
-    if (!hd || !f || hd->in_flight) return DSM_E_STATE;
-    if (!points || !offsets || !camera || !rotations || !requests || n_trajectories < 1 || n_trajectories > hd->max_traj) return DSM_E_INVALID;
-    const dsm_gain_camera_t &c = *camera;
-    const double v = (double)f->g.voxel;
-    if (!gain_camera_ok(c, v) || n_rot < 1 || n_rot > DSM_HEADING_MAX_ROTATIONS || samples < 1 || samples > DSM_HEADING_MAX_SAMPLES_PER_SEGMENT ||
-        w_unknown < 0 || w_unknown > DSM_HEADING_MAX_WEIGHT || w_frontier < 0 || w_frontier > DSM_HEADING_MAX_WEIGHT)
-        return DSM_E_INVALID;
-    for (size_t i = 0; i < 9 * (size_t)n_rot; i++)
-        if (!std::isfinite(rotations[i])) return DSM_E_INVALID;
-    if (!spline_points_ok(points, offsets, n_trajectories, INT32_MAX)) return DSM_E_INVALID;
-    long long n_samples = 0;
-    for (int j = 0; j < n_trajectories; j++)
-    {
-        const dsm_heading_request_t &q = requests[j];
-        if (q.start < 0 || q.start >= n_rot || q.end < -1 || q.end >= n_rot || q.max_step < 0 || q.max_step > n_rot) return DSM_E_INVALID;
-        n_samples += (long long)samples * (offsets[j + 1] - offsets[j] - 3) + 1;
-    }
-    const long long m = 2 * (long long)std::ceil((double)c.max_range / v) + 3;
-    if (n_samples > hd->max_samples || n_samples * m * m * m > DSM_HEADING_MAX_WORK) return DSM_E_INVALID;
-    // the packed request (dsm_device.cuh); the previous job's copy out of this staging ended before its wait, which no
-    // job in flight implies
-    uint8_t *h = hd->stage_host;
-    std::memcpy(h, rotations, 72 * (size_t)n_rot);
-    auto *traj = reinterpret_cast<DsmHeadingTraj *>(h + 72 * (size_t)DSM_HEADING_MAX_ROTATIONS);
-    auto *smp = reinterpret_cast<DsmHeadingSample *>(traj + n_trajectories);
-    long long bricks = 0;
-    int s0 = 0;
-    for (int j = 0; j < n_trajectories; j++)
-    {
-        const int N = offsets[j + 1] - offsets[j], S = samples * (N - 3) + 1;
-        DsmHeadingTraj &T = traj[j];
-        T.sample0 = s0, T.n_samples = S, T.start = requests[j].start, T.end = requests[j].end, T.max_step = requests[j].max_step;
-        T.n_outside = 0;
-        for (int s = 0; s < S; s++)
-        {
-            DsmHeadingSample &Z = smp[s0 + s];
-            spline_sample(points + 3 * (size_t)offsets[j], N, samples, s, Z.p);
-            Z.pad = 0;
-            bool inside = true;
-            for (int k = 0; k < 3; k++)
-            {
-                const double q = std::floor(Z.p[k] / v) - (double)f->g.o[k];
-                inside = inside && q >= 0.0 && q < (double)f->g.n[k];
-            }
-            int lo[3] = {INT32_MAX, INT32_MAX, INT32_MAX}, hi[3] = {-1, -1, -1}; // the hull, exclusive of hi
-            for (int r = 0; inside && r < n_rot; r++)
-            {
-                DsmGainView V;
-                for (int a = 0; a < 3; a++)
-                {
-                    for (int b = 0; b < 3; b++) V.P[4 * a + b] = rotations[9 * r + 3 * a + b];
-                    V.P[4 * a + 3] = Z.p[a];
-                }
-                gain_box(V.P, c, f->g, V);
-                if (V.size[0] == 0 || V.size[1] == 0 || V.size[2] == 0) continue;
-                for (int k = 0; k < 3; k++) lo[k] = std::min(lo[k], V.lo[k]), hi[k] = std::max(hi[k], V.lo[k] + V.size[k]);
-            }
-            T.n_outside += !inside;
-            for (int k = 0; k < 3; k++)
-            {
-                Z.lo[k] = hi[k] < 0 ? 0 : lo[k];
-                Z.size[k] = hi[k] < 0 ? 0 : hi[k] - lo[k];
-            }
-            Z.brick0 = (int)bricks; // below 2^31: the work bound caps the bricks far lower
-            bricks += dsm_gain_bricks(Z.size);
-        }
-        s0 += S;
-    }
-    CK(cudaSetDevice(ctx->device));
-    CK(cudaMemcpyAsync(hd->stage_dev, h, dsm_heading_stage_bytes(n_trajectories, s0), cudaMemcpyHostToDevice, ctx->stream));
-    CK(dsm_launch_heading(f->g, f->occ, f->dist, c, hd->stage_dev, n_trajectories, s0, n_rot, bricks, w_unknown, w_frontier, hd->succ,
-                          hd->res, ctx->stream));
-    hd->n = n_trajectories, hd->n_samples = s0, hd->n_rot = n_rot;
-    return submit(ctx, *hd, hd->res, dsm_heading_res_bytes(n_trajectories, s0, n_rot), f->requests);
-}
-
-extern "C" int dsm_heading_wait(dsm_ctx *ctx, dsm_heading_info_t *info, const dsm_heading_t **records, const dsm_heading_sample_t **samples,
-                                const dsm_heading_count_t **counts)
-{
-    if (!ctx) return DSM_E_INVALID;
-    DsmHeading *hd = ctx->heading.get();
-    const int rc = wait_head(ctx, hd);
-    if (rc != DSM_OK) return rc;
-    copy_info(info, hd->words());
-    const auto *r = reinterpret_cast<const dsm_heading_t *>(hd->res_host + 4 * DSM_HEAD_WORDS);
-    const auto *p = reinterpret_cast<const dsm_heading_sample_t *>(r + hd->n);
-    if (records) *records = r;
-    if (samples) *samples = p;
-    if (counts) *counts = reinterpret_cast<const dsm_heading_count_t *>(p + hd->n_samples);
-    return capacity(ctx, hd->words(), DSM_HEAD_ERR_TAG, "dsm_heading_wait", "the field the job read");
 }
 
 // ---- checkpoints that do not stop the stream (include/dsm.h, DESIGN.md §8.5) ----

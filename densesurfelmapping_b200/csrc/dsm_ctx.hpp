@@ -1,10 +1,15 @@
-// Private to the library: the context behind the opaque `dsm_ctx` of include/dsm.h, shared by the host-side
-// translation units (dsm_capi.cu: single-GPU entry points; dsm_comm.cu: multi-GPU gather over NCCL).
+// Private to the library: the context behind the opaque `dsm_ctx` of include/dsm.h, shared by the translation units
+// that hold its entry points (dsm_capi.cu: the map, the field and checkpoints; dsm_comm.cu: multi-GPU gather over NCCL;
+// dsm_field.cu, dsm_frontier.cu, dsm_reach.cu, dsm_gain.cu, dsm_viewpoint.cu, dsm_tour.cu, dsm_trajectory.cu and
+// dsm_heading.cu: the planner jobs, each beside its kernels), and the lifecycle those jobs share.
 #pragma once
 #include "dsm_device.cuh"
 #include "dsm_map_state.h"
+#include <algorithm>
+#include <cmath>
 #include <condition_variable>
 #include <cstdio>
+#include <cstring>
 #include <memory>
 #include <mutex>
 #include <string>
@@ -253,94 +258,139 @@ struct DsmJob
 };
 
 // dsm_field_query_* (DESIGN.md §8.8): the packed request (pinned staging and its device twin) and the device result at
-// the capacities of dsm_field_query_enable
+// the capacities of dsm_field_query_enable; both layouts live in dsm_field.cu
 struct DsmFieldQuery : DsmJob
 {
     int max_points = 0, max_traj = 0, max_wp = 0;
     uint8_t *req_host = nullptr, *req_dev = nullptr, *res_dev = nullptr;
     int n_points = 0, n_traj = 0; // of the query in flight or last waited for
-    // byte offsets of the packed layouts (dsm_device.cuh) for n_points, n_wp and n_traj
-    static size_t req_bytes(int n_points, int n_wp, int n_traj) { return 24 * ((size_t)n_points + n_wp) + 4 * ((size_t)n_traj + 1 + n_wp); }
-    static size_t res_clearance(int n_points) { return 16 * (1 + (size_t)n_points); }
-    static size_t res_bytes(int n_points, int n_traj) { return res_clearance(n_points) + 16 * (size_t)n_traj; }
 };
 
-// dsm_frontier_* (DESIGN.md §8.10), allocated by dsm_frontier_enable for the field's grid: the job's device buffers
-// (DsmFrontierBufs, the packed result among them)
+struct DsmFrontierAcc; // what k_frontier_reduce accumulates per table entry (dsm_frontier.cu)
+
+// dsm_frontier_* (DESIGN.md §8.10), allocated by dsm_frontier_enable for the field's grid: the job's device buffers and
+// its packed result, which the gain, viewpoint and reach jobs read as well
 struct DsmFrontier : DsmJob
 {
-    DsmFrontierBufs b;
+    int voxels = 0, max_comp = 0, max_clusters = 0, max_voxels = 0;
+    int32_t *label = nullptr;                                   // [voxels]
+    int32_t *roots = nullptr, *count = nullptr, *cmap = nullptr, *cid = nullptr; // [max_comp]
+    int32_t *slot_comp = nullptr, *sizes = nullptr, *offs = nullptr; // [max_clusters]
+    DsmFrontierAcc *acc = nullptr;                              // [max_clusters]
+    int32_t *idx = nullptr;                                     // [max_voxels]
+    uint32_t *keys = nullptr, *keys_alt = nullptr;              // [max_voxels]
+    int32_t *blk = nullptr, *blk_ofs = nullptr;                 // one per CTA of the compactions
+    uint8_t *res = nullptr;                                     // the packed result (dsm_device.cuh)
+    void *temp = nullptr;                                       // CUB scratch
+    size_t temp_bytes = 0;
+    // byte offsets of the result's cluster table and member list
+    static size_t table_at() { return 4 * (size_t)DSM_FRONTIER_WORDS; }
+    size_t list_at() const { return table_at() + sizeof(dsm_frontier_cluster_t) * (size_t)max_clusters; }
 };
 
-// dsm_reach_* (DESIGN.md §8.11), allocated by dsm_reach_enable for the field's grid: the job's device buffers
-// (DsmReachBufs, the packed result among them), the goal staging and the cost grid's pinned copy
+// dsm_reach_* (DESIGN.md §8.11), allocated by dsm_reach_enable for the field's grid: the job's device buffers, the packed
+// result (dsm_reach.cu), the goal staging and the cost grid's pinned copy
 struct DsmReach : DsmJob
 {
-    DsmReachBufs b;
+    int voxels = 0, tiles = 0, tn[3] = {0, 0, 0}; // tn: tiles per axis
+    int max_targets = 0, max_path = 0, max_rounds = 0, ctas = 0; // ctas: the persistent CTAs of a round
+    uint8_t *trav = nullptr;                      // [voxels]
+    uint32_t *cost[2] = {nullptr, nullptr};       // [voxels] each
+    int32_t *stamp = nullptr;                     // [tiles]: the latest round a tile was scheduled for
+    int32_t *sched[2] = {nullptr, nullptr};       // [tiles] each: round r's schedule is sched[r % 2]
+    int32_t *count = nullptr;                     // [3]: round r's schedule length is count[r % 3]
+    int32_t *goals = nullptr;                     // device [max_targets][3] goal voxels, staged from goals_host
+    unsigned long long *best = nullptr;           // [max_targets] (cost << 32 | viewpoint)
+    int32_t *member = nullptr;                    // [max_targets] the cluster member attaining best
+    long long *len = nullptr, *ofs = nullptr;     // [max_targets] path lengths and their exclusive prefix sums
+    uint8_t *res = nullptr;                       // the packed result
+    void *temp = nullptr;                         // CUB scratch of the path-length scan
+    size_t temp_bytes = 0;
     int32_t *goals_host = nullptr; // pinned [max_targets][3]
     uint32_t *cost_host = nullptr; // pinned [voxels]
     bool host_copy = false;
 };
 
 // dsm_reach_matrix_* (DESIGN.md §8.13), allocated by dsm_reach_matrix_enable for the field's grid: the job's device
-// buffers (DsmReachMatrixBufs, the packed result among them) and the site staging
+// buffers, the packed result (dsm_reach.cu) and the site staging.  Per (site, slot) the costs are a tile's 512 voxels in
+// tile-local order (x fastest), at ((size_t)site * max_tiles + slot) * 512 of each buffer.
 struct DsmReachMatrix : DsmJob
 {
-    DsmReachMatrixBufs b;
+    int voxels = 0, tiles = 0, tn[3] = {0, 0, 0};
+    int max_sites = 0, max_tiles = 0, max_rounds = 0, ctas = 0;
+    int32_t *flag = nullptr, *scan = nullptr;     // [tiles]: the tile is active, and the exclusive sum of the flags
+    int32_t *slot = nullptr;                      // [tiles]: the tile's slot, -1 when inactive
+    uint32_t *mask = nullptr;                     // [tiles][16]: the tile's traversable voxels, bit t of word t / 32
+    int32_t *tile_of = nullptr;                   // [max_tiles]: the tile of a slot
+    uint32_t *cost[2] = {nullptr, nullptr};       // [max_sites][max_tiles][512] each
+    int32_t *stamp = nullptr;                     // [max_sites][max_tiles]: the latest round a slot was scheduled for
+    int32_t *sched[2] = {nullptr, nullptr};       // [max_sites][max_tiles] each: round r's schedule is sched[r % 2]
+    int32_t *count = nullptr;                     // [max_sites][3]: site i's round-r schedule length is count[3 i + r % 3]
+    int32_t *rounds = nullptr, *reached = nullptr; // [max_sites]: the rounds with a non-empty schedule, the reached voxels
+    int32_t *sites = nullptr;                     // device [max_sites][3] the points' voxels, staged from sites_host
+    uint8_t *res = nullptr;                       // the packed result, room for max_sites
+    void *temp = nullptr;                         // CUB scratch of the tile scan
+    size_t temp_bytes = 0;
     int32_t *sites_host = nullptr; // pinned [max_sites][3]
     int n_sites = 0; // of the job in flight or last waited for
 };
 
 // dsm_gain_* (DESIGN.md §8.12), allocated by dsm_gain_enable for the field's grid: the pinned and device staging of
-// max_views views, the cluster-slot grid and the device result
+// max_views views, the cluster-slot grid and the device result (dsm_gain.cu)
 struct DsmGain : DsmJob
 {
     int max_views = 0;
     DsmGainView *views_host = nullptr, *views_dev = nullptr; // [max_views]
     int32_t *slot = nullptr;                                  // device [voxels]
-    uint8_t *res = nullptr;                                   // 4 DSM_GAIN_WORDS + 32 max_views bytes
-    static size_t res_bytes(int n_views) { return 4 * (size_t)DSM_GAIN_WORDS + sizeof(dsm_view_gain_t) * (size_t)n_views; }
+    uint8_t *res = nullptr;
 };
 
-// dsm_viewpoint_* (DESIGN.md §8.15), allocated by dsm_viewpoint_enable: the job's device buffers (DsmViewpointBufs, the
-// packed result among them) and the pinned staging
+struct DsmVpCluster; // what k_vp_clusters leaves per requested cluster (dsm_viewpoint.cu)
+
+// dsm_viewpoint_* (DESIGN.md §8.15), allocated by dsm_viewpoint_enable: the job's device buffers, the pinned staging of
+// the request and its device twin, and the packed result (both layouts in dsm_viewpoint.cu)
 struct DsmViewpoint : DsmJob
 {
-    DsmViewpointBufs b;
-    uint8_t *stage_host = nullptr;
+    int max_clusters = 0, max_candidates = 0, ctas = 0; // ctas: the persistent CTAs of k_vp_score
+    uint8_t *stage_host = nullptr, *stage_dev = nullptr;
+    DsmVpCluster *cl = nullptr;               // [max_clusters]
+    unsigned long long *key = nullptr;        // [max_candidates]: the candidate's ranking key, ~0 when it is no viewpoint
+    int32_t *list = nullptr;                  // [max_candidates]: the reached candidates, cluster * n_offsets + offset
+    int32_t *count = nullptr;                 // [1]: their number
+    uint8_t *res = nullptr;                   // the packed result, room for max_clusters at top_k 16
     int n_clusters = 0, top_k = 0; // of the job in flight or last waited for
 };
 
 // dsm_tour_* (DESIGN.md §8.14), allocated by dsm_tour_enable: the pinned and device matrix of max_sites^2 entries, the
-// starts' tours and the device result
+// starts' tours and the device result (dsm_tour.cu)
 struct DsmTour : DsmJob
 {
     int max_sites = 0, max_starts = 0;
     uint32_t *matrix_host = nullptr, *matrix = nullptr; // [max_sites^2] each
     int32_t *tours = nullptr;                           // device [max_starts][max_sites]
-    uint8_t *res = nullptr;                             // dsm_tour_res_bytes(max_starts, max_sites)
+    uint8_t *res = nullptr;
     int n = 0, n_starts = 0; // of the job in flight or last waited for
 };
 
 // dsm_trajectory_* (DESIGN.md §8.17), allocated by dsm_trajectory_enable: the pinned and device staging of the request,
-// the L-BFGS history (6 max_memory doubles per point) and the device result
+// the L-BFGS history (6 max_memory doubles per point) and the device result (both layouts in dsm_trajectory.cu)
 struct DsmTrajectory : DsmJob
 {
     int max_traj = 0, max_points = 0, max_memory = 0;
-    uint8_t *stage_host = nullptr, *stage_dev = nullptr; // dsm_trajectory_stage_bytes(max_points, max_traj)
+    uint8_t *stage_host = nullptr, *stage_dev = nullptr;
     double *hist = nullptr;
-    uint8_t *res = nullptr;                              // dsm_trajectory_res_bytes(max_points, max_traj)
+    uint8_t *res = nullptr;
     int n = 0, n_points = 0; // of the job in flight or last waited for
 };
 
 // dsm_heading_* (DESIGN.md §8.19), allocated by dsm_heading_enable: the pinned and device staging of the request, the
-// successor table (64 int8 per sample) and the device result
+// successor table (64 int8 per sample) and the device result (both layouts in dsm_heading.cu)
 struct DsmHeading : DsmJob
 {
     int max_traj = 0, max_samples = 0;
-    uint8_t *stage_host = nullptr, *stage_dev = nullptr; // dsm_heading_stage_bytes(max_traj, max_samples)
+    uint8_t *stage_host = nullptr, *stage_dev = nullptr;
     int8_t *succ = nullptr;
-    uint8_t *res = nullptr;                              // dsm_heading_res_bytes(max_traj, max_samples, 64)
+    uint8_t *res = nullptr;
     int n = 0, n_samples = 0, n_rot = 0; // of the job in flight or last waited for
 };
 
@@ -449,3 +499,135 @@ struct dsm_ctx
         }                                                                                                \
     } while (0)
 
+// ---- the lifecycle every snapshot, field and planner job shares ----
+// The end of an enable: the new state is kept when every call of its owner succeeded and `ok`, else nothing is kept and
+// a later call may try again
+template <typename T>
+static inline int keep(std::unique_ptr<T> &slot, std::unique_ptr<T> &fresh, bool ok = true)
+{
+    if (fresh->own.take() != cudaSuccess || !ok)
+    {
+        cudaGetLastError();
+        return DSM_E_NOMEM; // nothing is kept: a later call may try again
+    }
+    slot = std::move(fresh);
+    return DSM_OK;
+}
+
+// The latest field request if it is a known one (what every job on the known field reads), else nullptr
+static inline const DsmField *known_field(const dsm_ctx *ctx)
+{
+    const DsmField *f = ctx->field.get();
+    return f && f->requested && f->known ? f : nullptr;
+}
+
+// The pairing rule: the latest job of a kind (frontier, reach) read the latest field request
+static inline bool read_latest(const DsmJob *j, const DsmField *f) { return j && j->request == f->requests; }
+
+// The tail of an enqueue: one D2H copy of the used result bytes, the job's event, and the job in flight with the field
+// request it read (0 for none)
+static inline int submit(dsm_ctx *ctx, DsmJob &j, const void *res, size_t bytes, uint64_t request)
+{
+    CK(cudaMemcpyAsync(j.res_host, res, bytes, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaEventRecord(j.ev, ctx->stream));
+    j.in_flight = true;
+    j.request = request;
+    return DSM_OK;
+}
+
+// The head of a wait (a job's or the field's): DSM_E_STATE without a request in flight, else its event waited for and
+// the request retired
+template <typename T>
+static inline int wait_head(dsm_ctx *ctx, T *j)
+{
+    if (!j || !j->in_flight) return DSM_E_STATE;
+    CK(cudaSetDevice(ctx->device));
+    CK(cudaEventSynchronize(j->ev));
+    j->in_flight = false;
+    return DSM_OK;
+}
+
+// The result of a wait whose header h holds the sticky error word of dsm_fuse_stream_window at h[tag] and the frame it
+// rejected after it: DSM_OK without an error, else DSM_E_CAPACITY with the message that `call`'s `what` holds the frames
+// before that one
+static inline int capacity(dsm_ctx *ctx, const int32_t *h, int tag, const char *call, const char *what)
+{
+    if (h[tag] == 0) return DSM_OK;
+    snprintf(ctx->err, sizeof(ctx->err), "%s: frame %d of a dsm_fuse_stream_window call did not fit the pool or the store; %s holds "
+             "the frames before it", call, h[tag + 1], what);
+    return DSM_E_CAPACITY;
+}
+
+// An info struct copied out of a result header, its reserved words zeroed
+template <typename Info>
+static inline void copy_info(Info *info, const int32_t *h)
+{
+    if (!info) return;
+    std::memcpy(info, h, sizeof(Info));
+    for (int32_t &w : info->reserved) w = 0;
+}
+
+// ---- host checks and staging shared by the jobs on a camera (gain, viewpoints, headings) or on splines (trajectories,
+// headings) ----
+// gain's camera checks (include/dsm.h): intrinsics, image size, the blocking rule and a range of at most 128 voxels
+static inline bool gain_camera_ok(const dsm_gain_camera_t &c, double v)
+{
+    const double R = (double)c.max_range;
+    return std::isfinite(c.fx) && c.fx > 0.0 && std::isfinite(c.fy) && c.fy > 0.0 && std::isfinite(c.cx) && std::isfinite(c.cy) &&
+           c.width >= 1 && c.width <= 65536 && c.height >= 1 && c.height <= 65536 && (c.unknown_blocks == 0 || c.unknown_blocks == 1) &&
+           std::isfinite(R) && R > 0.0 && R <= DSM_GAIN_MAX_RANGE_VOXELS * v;
+}
+
+// The grid voxels of view P's box: the bounding box of the image pyramid cut at depth max_range (the apex t and the
+// four image corners (0 | width, 0 | height) at depth max_range) met with the cube around the range sphere, one voxel
+// of padding, clipped to the grid.  Every centre that passes the frustum test lies in the truncated pyramid and in the
+// sphere, so the box sizes the work and cannot change a count.  The pyramid holds them only for a rotation: a pose whose
+// 3x3 part is not orthonormal within 1e-6 per entry of R^T R - I, or a corner that does not come out finite, leaves
+// the cube alone (within that tolerance the pyramid moves by far less than the padding).
+static inline void gain_box(const double *P, const dsm_gain_camera_t &c, const DsmFieldGrid &g, DsmGainView &V)
+{
+    const double R = (double)c.max_range, v = (double)g.voxel;
+    double plo[3], phi[3];
+    bool finite = true;
+    for (int a = 0; a < 3; a++)
+        for (int b = 0; b < 3; b++)
+            finite = finite && std::fabs(((P[a] * P[b] + P[4 + a] * P[4 + b]) + P[8 + a] * P[8 + b]) - (a == b ? 1.0 : 0.0)) <= 1e-6;
+    for (int k = 0; k < 3; k++) plo[k] = phi[k] = P[4 * k + 3];
+    for (int cu = 0; cu < 2; cu++)
+        for (int cw = 0; cw < 2; cw++)
+        {
+            const double qx = ((cu ? (double)c.width : 0.0) - c.cx) / c.fx * R, qy = ((cw ? (double)c.height : 0.0) - c.cy) / c.fy * R;
+            for (int k = 0; k < 3; k++)
+            {
+                const double p = ((P[4 * k] * qx + P[4 * k + 1] * qy) + P[4 * k + 2] * R) + P[4 * k + 3];
+                finite = finite && std::isfinite(p);
+                plo[k] = std::min(plo[k], p);
+                phi[k] = std::max(phi[k], p);
+            }
+        }
+    for (int k = 0; k < 3; k++)
+    {
+        double lo = P[4 * k + 3] - R, hi = P[4 * k + 3] + R;
+        if (finite) lo = std::max(lo, plo[k]), hi = std::min(hi, phi[k]);
+        const double a = std::max(std::floor(lo / v) - 1.0 - (double)g.o[k], 0.0);
+        const double b = std::min(std::floor(hi / v) + 1.0 - (double)g.o[k], (double)(g.n[k] - 1));
+        V.lo[k] = a <= b ? (int)a : 0;
+        V.size[k] = a <= b ? (int)(b - a) + 1 : 0;
+    }
+}
+
+// The control points of n uniform cubic B-splines as the trajectory and heading jobs take them (include/dsm.h):
+// offsets[0] = 0, 7 to 256 points per trajectory, at most max_points in all, every coordinate finite
+static inline bool spline_points_ok(const double *points, const int32_t *offsets, int n, int max_points)
+{
+    if (offsets[0] != 0) return false;
+    for (int j = 0; j < n; j++)
+    {
+        if (offsets[j + 1] < offsets[j]) return false;
+        const int m = offsets[j + 1] - offsets[j];
+        if (m < 7 || m > DSM_TRAJECTORY_MAX_POINTS || offsets[j + 1] > max_points) return false;
+    }
+    for (size_t c = 0; c < 3 * (size_t)offsets[n]; c++)
+        if (!std::isfinite(points[c])) return false;
+    return true;
+}

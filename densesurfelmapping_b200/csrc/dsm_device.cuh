@@ -394,25 +394,8 @@ inline int dsm_carve_ctas_per_view(int S) { return (S + CARVE_BLOCK - 1) / CARVE
 void dsm_launch_field_carve(const DsmFieldGrid &g, const float4 *rays, int S, const double *poses, const int32_t *slots, int n_views,
                             float max_range, uint8_t *occ, cudaStream_t s);
 
-// dsm_field_query_* (DESIGN.md §8.8), dsm_field.cu.  One packed request (H2D) and one packed result (D2H):
-//   request  double points[n_points][3] | double waypoints[n_wp][3] | int32 offsets[n_traj + 1] | int32 first[n_wp]
-//            (first[w]: the trajectory's index of waypoint w's first sample, staged by the host; the last waypoint's
-//            entry is the index of the final sample)
-//   result   int32 header[DSM_QUERY_WORDS] | float4 samples[n_points] | dsm_clearance_t clearance[n_traj]
-enum
-{
-    DSM_QUERY_ERR_TAG,   // the field header's DSM_FIELD_ERR_TAG / _ERR_FRAME, copied by k_field_query
-    DSM_QUERY_ERR_FRAME,
-    DSM_QUERY_WORDS = 4  // 16 B: the samples stay float4-aligned
-};
-// k_field_query over n_points (CTA 0 also copies the error words; launched with one CTA at least) and
-// k_field_clearance over n_traj trajectories, both on the grid `dist` with its header (at dsm_field_header(voxels)); sgn:
-// the instantiations for a signed grid and its header
-void dsm_launch_field_query(bool sgn, const float *dist, const int32_t *field_header, const DsmFieldGrid &g, const double *points, int n_points,
-                            const double *waypoints, const int32_t *offsets, const int32_t *first, int n_traj, float radius,
-                            int32_t *result_header, float4 *samples, dsm_clearance_t *clearance, cudaStream_t s);
-
-// dsm_frontier_* (DESIGN.md §8.10), dsm_frontier.cu.  One packed result (D2H):
+// dsm_frontier_* (DESIGN.md §8.10), dsm_frontier.cu.  One packed result (D2H), which the reach, gain and viewpoint jobs
+// read on the device as well (DsmFrontier::table_at, list_at):
 //   int32 header[DSM_FRONTIER_WORDS] | dsm_frontier_cluster_t table[max_clusters] | int32 list[max_voxels]
 enum
 {
@@ -426,38 +409,6 @@ enum
     DSM_FRONTIER_N_SELECTED,        // scratch: the members the list compaction selected
     DSM_FRONTIER_WORDS = 8          // 32 B: the table stays 8-byte aligned
 };
-// what dsm_frontier_reduce accumulates per table entry (integer atomics only)
-struct DsmFrontierAcc
-{
-    int32_t lo[3], hi[3];
-    unsigned long long sum[3], faces, open[3]; // two's complement int64
-};
-// The device buffers of one context's frontier jobs, sized by dsm_frontier_enable for the field's grid
-struct DsmFrontierBufs
-{
-    int voxels = 0, max_comp = 0, max_clusters = 0, max_voxels = 0;
-    int32_t *label = nullptr;                                   // [voxels]
-    int32_t *roots = nullptr, *count = nullptr, *cmap = nullptr, *cid = nullptr; // [max_comp]
-    int32_t *slot_comp = nullptr, *sizes = nullptr, *offs = nullptr; // [max_clusters]
-    DsmFrontierAcc *acc = nullptr;                              // [max_clusters]
-    int32_t *idx = nullptr;                                     // [max_voxels]
-    uint32_t *keys = nullptr, *keys_alt = nullptr;              // [max_voxels]
-    int32_t *blk = nullptr, *blk_ofs = nullptr;                 // [dsm_frontier_sel_blocks(voxels)]: the compactions' CTAs
-    uint8_t *res = nullptr;                                     // the packed result
-    void *temp = nullptr;                                       // CUB scratch of dsm_frontier_temp_bytes
-    size_t temp_bytes = 0;
-    static size_t res_bytes(int max_clusters, int max_voxels)
-    {
-        return 4 * (size_t)DSM_FRONTIER_WORDS + sizeof(dsm_frontier_cluster_t) * (size_t)max_clusters + 4 * (size_t)max_voxels;
-    }
-};
-int dsm_frontier_sel_blocks(int voxels);
-// the CUB scratch the job needs for these sizes (the buffers' pointers may still be null); 0 on a CUB error
-size_t dsm_frontier_temp_bytes(const DsmFrontierBufs &b);
-// the whole job on the state grid `state` of grid g, with the field header of that request; the result header must
-// be zeroed by the caller.  Returns the first error of a CUB call or a launch.
-cudaError_t dsm_launch_frontier(const DsmFrontierBufs &b, const DsmFieldGrid &g, const uint8_t *state, const int32_t *field_header,
-                                int min_voxels, cudaStream_t s);
 // the frontier table's cluster among the first n whose listed members hold list entry j, or -1 (a binary search over
 // the offsets: the listed clusters are a prefix of the table with rising offsets)
 __device__ __forceinline__ int dsm_frontier_cluster_of(const dsm_frontier_cluster_t *table, int n, int j)
@@ -476,123 +427,9 @@ __device__ __forceinline__ int dsm_frontier_cluster_of(const dsm_frontier_cluste
     return c >= 0 && j < table[c].offset + table[c].n_voxels ? c : -1;
 }
 
-// dsm_reach_* (DESIGN.md §8.11), dsm_reach.cu.  One packed result (D2H):
-//   int32 header[DSM_REACH_WORDS] | dsm_reach_target_t targets[max_targets] | int32 path[max_path_voxels]
-// The header's first 14 words are those of dsm_reach_info_t; the last two carry the field's error words.
-enum
-{
-    DSM_REACH_ORIGIN = 0, // 3 words
-    DSM_REACH_START_VOXEL = 3,
-    DSM_REACH_START_STATUS,
-    DSM_REACH_START_APPROACH,
-    DSM_REACH_ROUNDS,
-    DSM_REACH_CONVERGED,
-    DSM_REACH_N_TRAVERSABLE,
-    DSM_REACH_N_REACHED,
-    DSM_REACH_N_GOALS,
-    DSM_REACH_N_CLUSTERS_TOTAL,
-    DSM_REACH_N_TARGETS,
-    DSM_REACH_N_PATH_VOXELS,
-    DSM_REACH_ERR_TAG, // the field header's DSM_FIELD_ERR_TAG / _ERR_FRAME, copied by k_reach_start
-    DSM_REACH_ERR_FRAME,
-    DSM_REACH_WORDS = 16 // 64 B
-};
-#define DSM_REACH_TILE 8 // tiles of 8 x 8 x 8 voxels, one CTA of 512 threads each
-// The device buffers of one context's reach jobs, sized by dsm_reach_enable for the field's grid and capacities
-struct DsmReachBufs
-{
-    int voxels = 0, tiles = 0, tn[3] = {0, 0, 0}; // tn: tiles per axis
-    int max_targets = 0, max_path = 0, max_rounds = 0, ctas = 0; // ctas: the persistent CTAs of a round
-    uint8_t *trav = nullptr;                      // [voxels]
-    uint32_t *cost[2] = {nullptr, nullptr};       // [voxels] each
-    int32_t *stamp = nullptr;                     // [tiles]: the latest round a tile was scheduled for
-    int32_t *sched[2] = {nullptr, nullptr};       // [tiles] each: round r's schedule is sched[r % 2]
-    int32_t *count = nullptr;                     // [3]: round r's schedule length is count[r % 3]
-    int32_t *goals = nullptr;                     // device [max_targets][3] goal voxels, staged from goals_host
-    unsigned long long *best = nullptr;           // [max_targets] (cost << 32 | viewpoint)
-    int32_t *member = nullptr;                    // [max_targets] the cluster member attaining best
-    long long *len = nullptr, *ofs = nullptr;     // [max_targets] path lengths and their exclusive prefix sums
-    uint8_t *res = nullptr;                       // the packed result
-    void *temp = nullptr;                         // CUB scratch of dsm_reach_temp_bytes
-    size_t temp_bytes = 0;
-    static size_t res_bytes(int max_targets, int max_path)
-    {
-        return 4 * (size_t)DSM_REACH_WORDS + sizeof(dsm_reach_target_t) * (size_t)max_targets + 4 * (size_t)max_path;
-    }
-};
-// the CUB scratch of the path-length scan; 0 on a CUB error
-size_t dsm_reach_temp_bytes(const DsmReachBufs &b);
-// the persistent CTAs of k_reach_round on this device
-int dsm_reach_ctas();
-// The whole job on the grids of the latest known request (state, distance and header at dsm_field_header(voxels)),
-// from start voxel s (each axis clamped to [-1, n]) with the n_goals goal voxels already in b.goals; frontier_res is the
-// frontier job's device result (nullptr without frontiers).  The result header must be zeroed by the caller.
-cudaError_t dsm_launch_reach(const DsmReachBufs &b, const DsmFieldGrid &g, const uint8_t *state, const int32_t *dist,
-                             const int3 s, float radius, int approach, int n_goals, const uint8_t *frontier_res, int frontier_max_clusters,
-                             cudaStream_t st);
-
-// dsm_reach_matrix_* (DESIGN.md §8.13), dsm_reach.cu.  One packed result of a job on n sites (D2H, 64 + 32 n + 4 n^2 B):
-//   int32 header[DSM_RM_WORDS] | dsm_reach_site_t sites[n] | uint32 matrix[n][n]
-// The header's first nine words are those of dsm_reach_matrix_info_t; its last two carry the field's error words,
-// cleared by dsm_reach_matrix_wait.
-enum
-{
-    DSM_RM_ORIGIN = 0, // 3 words
-    DSM_RM_N_SITES = 3,
-    DSM_RM_STATUS,
-    DSM_RM_N_TRAVERSABLE,
-    DSM_RM_N_ACTIVE_TILES,
-    DSM_RM_MAX_TILES,
-    DSM_RM_ROUNDS,
-    DSM_RM_ERR_TAG = 14, // the field header's DSM_FIELD_ERR_TAG / _ERR_FRAME, copied by k_rm_slots
-    DSM_RM_ERR_FRAME,
-    DSM_RM_WORDS = 16 // 64 B
-};
-// The device buffers of one context's matrix jobs, sized by dsm_reach_matrix_enable.  Per (site, slot) the costs are a
-// tile's 512 voxels in tile-local order (x fastest), at ((size_t)site * max_tiles + slot) * 512 of each buffer.
-struct DsmReachMatrixBufs
-{
-    int voxels = 0, tiles = 0, tn[3] = {0, 0, 0};
-    int max_sites = 0, max_tiles = 0, max_rounds = 0, ctas = 0;
-    int32_t *flag = nullptr, *scan = nullptr;     // [tiles]: the tile is active, and the exclusive sum of the flags
-    int32_t *slot = nullptr;                      // [tiles]: the tile's slot, -1 when inactive
-    uint32_t *mask = nullptr;                     // [tiles][16]: the tile's traversable voxels, bit t of word t / 32
-    int32_t *tile_of = nullptr;                   // [max_tiles]: the tile of a slot
-    uint32_t *cost[2] = {nullptr, nullptr};       // [max_sites][max_tiles][512] each
-    int32_t *stamp = nullptr;                     // [max_sites][max_tiles]: the latest round a slot was scheduled for
-    int32_t *sched[2] = {nullptr, nullptr};       // [max_sites][max_tiles] each: round r's schedule is sched[r % 2]
-    int32_t *count = nullptr;                     // [max_sites][3]: site i's round-r schedule length is count[3 i + r % 3]
-    int32_t *rounds = nullptr, *reached = nullptr; // [max_sites]: the rounds with a non-empty schedule, the reached voxels
-    int32_t *sites = nullptr;                     // device [max_sites][3] the points' voxels, staged by the host
-    uint8_t *res = nullptr;                       // the packed result, room for max_sites
-    void *temp = nullptr;                         // CUB scratch of dsm_reach_matrix_temp_bytes
-    size_t temp_bytes = 0;
-    static size_t res_bytes(int n) { return 4 * (size_t)DSM_RM_WORDS + sizeof(dsm_reach_site_t) * (size_t)n + 4 * (size_t)n * n; }
-};
-// the CUB scratch of the tile scan; 0 on a CUB error
-size_t dsm_reach_matrix_temp_bytes(const DsmReachMatrixBufs &b);
-// the persistent CTAs of k_rm_round on this device
-int dsm_reach_matrix_ctas();
-// The whole job on the grids of the latest known request for the n sites' voxels already in b.sites (each axis clamped
-// to [-1, n]).  The result header must be zeroed by the caller.
-cudaError_t dsm_launch_reach_matrix(const DsmReachMatrixBufs &b, const DsmFieldGrid &g, const uint8_t *state, const int32_t *dist,
-                                    int n, float radius, int approach, cudaStream_t st);
-
-// dsm_gain_* (DESIGN.md §8.12), dsm_gain.cu.  One staged request (H2D), DsmGainView views[n_views], and one packed
-// result (D2H): int32 header[DSM_GAIN_WORDS] | dsm_view_gain_t gains[max_views].  The header's first six words are
-// those of dsm_gain_info_t; its padding carries the field's error words, cleared by dsm_gain_wait.
-enum
-{
-    DSM_GAIN_ORIGIN = 0, // 3 words
-    DSM_GAIN_N_VIEWS = 3,
-    DSM_GAIN_N_CLUSTERS_TABLE,
-    DSM_GAIN_UNKNOWN_BLOCKS,
-    DSM_GAIN_ERR_TAG, // the field header's DSM_FIELD_ERR_TAG / _ERR_FRAME, copied by k_gain_init
-    DSM_GAIN_ERR_FRAME,
-    DSM_GAIN_WORDS = 8 // 32 B
-};
-// one view as the host stages it: the pose, its box of grid voxels (lo, size; size 0 on an axis: empty), the named
-// cluster (-1) and the view's first brick in the launch
+// dsm_gain_* (DESIGN.md §8.12), dsm_gain.cu, and what the viewpoint and heading jobs share with it: one view as the host
+// stages it (the pose, its box of grid voxels (lo, size; size 0 on an axis: empty), the named cluster (-1) and the
+// view's first brick in the launch), the bricks, the frustum test and the line of sight
 struct DsmGainView
 {
     double P[12];
@@ -668,144 +505,3 @@ __device__ __forceinline__ bool dsm_gain_walk(const DsmFieldGrid &g, const uint8
         }
     }
 }
-// The whole job on the state grid of the latest known request (header at dsm_field_header(voxels) of dist) for the
-// n_views views already in `views` (bricks in all); frontier_res is the frontier job's device result (nullptr without
-// clusters) and slot a grid of voxels ints.  Writes the whole used result; returns the first launch or memset error.
-cudaError_t dsm_launch_gain(const DsmFieldGrid &g, const uint8_t *state, const int32_t *dist, const dsm_gain_camera_t &cam,
-                            const DsmGainView *views, int n_views, long long bricks, const uint8_t *frontier_res,
-                            int frontier_max_clusters, int32_t *slot, uint8_t *res, cudaStream_t st);
-
-// dsm_viewpoint_* (DESIGN.md §8.15), dsm_viewpoint.cu.  One staged request (H2D, DsmViewpointBufs::stage_bytes):
-//   double rotations[64][9] | int32 offsets[4096][3] | int32 clusters[n_clusters]
-// and one packed result (D2H, 64 + 32 n (1 + top_k) B):
-//   int32 header[DSM_VP_WORDS] | dsm_viewpoint_cluster_t records[n] | dsm_viewpoint_t slots[n][top_k]
-// The header's first ten words are those of dsm_viewpoint_info_t; its last two carry the field's error words, cleared
-// by dsm_viewpoint_wait.
-enum
-{
-    DSM_VP_ORIGIN = 0, // 3 words
-    DSM_VP_N_CLUSTERS = 3,
-    DSM_VP_N_OFFSETS,
-    DSM_VP_N_ROTATIONS,
-    DSM_VP_TOP_K,
-    DSM_VP_UNKNOWN_BLOCKS,
-    DSM_VP_WITH_REACH,
-    DSM_VP_N_CLUSTERS_TABLE,
-    DSM_VP_ERR_TAG = 14, // the field header's DSM_FIELD_ERR_TAG / _ERR_FRAME, copied by k_vp_clusters
-    DSM_VP_ERR_FRAME,
-    DSM_VP_WORDS = 16 // 64 B
-};
-// what k_vp_clusters leaves per requested cluster for the later kernels
-struct DsmVpCluster
-{
-    int32_t g[3];   // the centre voxel
-    int32_t status; // of the record
-    int32_t base, n, n_s, pad; // the members' list offset and count, the samples
-};
-// The device buffers of one context's viewpoint jobs, sized by dsm_viewpoint_enable
-struct DsmViewpointBufs
-{
-    int max_clusters = 0, max_candidates = 0, ctas = 0; // ctas: the persistent CTAs of k_vp_score
-    uint8_t *stage = nullptr;                 // device twin of the staged request
-    DsmVpCluster *cl = nullptr;               // [max_clusters]
-    unsigned long long *key = nullptr;        // [max_candidates]: the candidate's ranking key, ~0 when it is no viewpoint
-    int32_t *list = nullptr;                  // [max_candidates]: the reached candidates, cluster * n_offsets + offset
-    int32_t *count = nullptr;                 // [1]: their number
-    uint8_t *res = nullptr;                   // the packed result, room for max_clusters at top_k 16
-    static size_t stage_off() { return 8 * 9 * (size_t)DSM_VIEWPOINT_MAX_ROTATIONS; }
-    static size_t stage_clusters() { return stage_off() + 12 * (size_t)DSM_VIEWPOINT_MAX_OFFSETS; }
-    static size_t stage_bytes(int n_clusters) { return stage_clusters() + 4 * (size_t)n_clusters; }
-    static size_t res_bytes(int n, int top_k) { return 4 * (size_t)DSM_VP_WORDS + 32 * (size_t)n * (1 + (size_t)top_k); }
-};
-// the persistent CTAs of k_vp_score on this device
-int dsm_viewpoint_ctas();
-// The whole job on the grids of the latest known request (state, distance and header at dsm_field_header(voxels)), the
-// frontier job's device result and (with_reach) the reach job's settled cost grid, for the request already in b.stage.
-// Writes the whole used result; returns the first launch error.
-cudaError_t dsm_launch_viewpoint(const DsmViewpointBufs &b, const DsmFieldGrid &g, const uint8_t *state, const int32_t *dist,
-                                 const dsm_gain_camera_t &cam, const dsm_viewpoint_params_t &p, int n_rotations, int n_clusters,
-                                 int n_offsets, const uint8_t *frontier_res, int frontier_max_clusters, const uint32_t *reach_cost,
-                                 cudaStream_t st);
-
-// dsm_tour_* (DESIGN.md §8.14), dsm_tour.cu.  The whole job on the n x n matrix already on the device: the starts'
-// tours go to tours [n_starts][n], and res receives the packed result of 64 + 16 n_starts + 4 n bytes,
-// dsm_tour_info_t | dsm_tour_start_t starts[n_starts] | int32 order[n].  Returns the first launch error.
-cudaError_t dsm_launch_tour(const uint32_t *matrix, int n, int open, int n_starts, int max_passes, uint64_t seed, int32_t *tours,
-                            uint8_t *res, cudaStream_t st);
-inline size_t dsm_tour_res_bytes(int n_starts, int n) { return 64 + 16 * (size_t)n_starts + 4 * (size_t)n; }
-
-// dsm_trajectory_* (DESIGN.md §8.17), dsm_trajectory.cu.  One staged request (H2D):
-//   double points[n_points][3] | double dt[n] | int32 offsets[n + 1]
-// and one packed result (D2H, 64 + 96 n + 24 n_points B):
-//   int32 header[DSM_TRAJ_WORDS] | dsm_trajectory_t records[n] | double points[n_points][3]
-// The header's first nine words are those of dsm_trajectory_info_t; its last two carry the signed grid's error words,
-// cleared by dsm_trajectory_wait.
-enum
-{
-    DSM_TRAJ_ORIGIN = 0, // 3 words
-    DSM_TRAJ_N = 3,
-    DSM_TRAJ_N_POINTS,
-    DSM_TRAJ_N_STATUS,   // 4 words: trajectories per status (zeroed before the launch; k_trajectory adds)
-    DSM_TRAJ_ERR_TAG = 14, // the signed grid header's DSM_SIGNED_ERR_TAG / _ERR_FRAME, copied by k_trajectory
-    DSM_TRAJ_ERR_FRAME,
-    DSM_TRAJ_WORDS = 16 // 64 B
-};
-inline size_t dsm_trajectory_stage_bytes(int n_points, int n) { return 24 * (size_t)n_points + 8 * (size_t)n + 4 * ((size_t)n + 1); }
-inline size_t dsm_trajectory_res_bytes(int n_points, int n)
-{
-    return 4 * (size_t)DSM_TRAJ_WORDS + sizeof(dsm_trajectory_t) * (size_t)n + 24 * (size_t)n_points;
-}
-// k_trajectory's shared memory for trajectories of at most nmax points: x, xt, g, gt and d, nmax x 3 doubles each
-inline size_t dsm_trajectory_smem(int nmax) { return 5 * 3 * sizeof(double) * (size_t)nmax; }
-// The whole job on the signed grid sdist with its header (at dsm_field_header(voxels)) for the request already on the
-// device (points, dt, offsets; nmax the most points of one of its n_traj trajectories), with the history scratch hist of
-// 6 p.memory doubles per point.  Writes the whole used result; returns the first launch or memset error.
-cudaError_t dsm_launch_trajectory(const double *points, const double *dt, const int32_t *offsets, int n_traj, int nmax, const float *sdist,
-                                  const int32_t *field_header, const DsmFieldGrid &g, const dsm_trajectory_params_t &p, double *hist,
-                                  uint8_t *res, cudaStream_t st);
-
-// dsm_heading_* (DESIGN.md §8.19), dsm_heading.cu.  One staged request (H2D, dsm_heading_stage_bytes(n, S)):
-//   double rotations[64][9] | DsmHeadingTraj trajectories[n] | DsmHeadingSample samples[S]
-// and one packed result (D2H, dsm_heading_res_bytes(n, S, n_rot)):
-//   int32 header[DSM_HEAD_WORDS] | dsm_heading_t records[n] | dsm_heading_sample_t samples[S] | dsm_heading_count_t counts[S][n_rot]
-// The header's first eleven words are those of dsm_heading_info_t; its last two carry the field's error words, cleared
-// by dsm_heading_wait.
-enum
-{
-    DSM_HEAD_ORIGIN = 0, // 3 words
-    DSM_HEAD_N = 3,
-    DSM_HEAD_N_SAMPLES,
-    DSM_HEAD_N_ROT,
-    DSM_HEAD_UNKNOWN_BLOCKS,
-    DSM_HEAD_N_STATUS,     // 2 words: trajectories per status (k_heading_plan adds)
-    DSM_HEAD_ERR_TAG = 14, // the field header's DSM_FIELD_ERR_TAG / _ERR_FRAME, copied by k_heading_plan
-    DSM_HEAD_ERR_FRAME,
-    DSM_HEAD_WORDS = 16 // 64 B
-};
-// one trajectory as the host stages it: its first sample and samples, the request, and its samples outside the grid
-struct DsmHeadingTraj
-{
-    int32_t sample0, n_samples, start, end, max_step, n_outside;
-}; // 24 B
-// one sample as the host stages it: the camera position, the hull of its gain boxes over the rotations (lo, size; size
-// 0 on an axis: empty, as for a camera outside the grid) and its first brick in the launch
-struct DsmHeadingSample
-{
-    double p[3];
-    int32_t lo[3], size[3], brick0, pad;
-}; // 56 B
-inline size_t dsm_heading_stage_bytes(int n, int n_samples)
-{
-    return 72 * (size_t)DSM_HEADING_MAX_ROTATIONS + sizeof(DsmHeadingTraj) * (size_t)n + sizeof(DsmHeadingSample) * (size_t)n_samples;
-}
-inline size_t dsm_heading_res_bytes(int n, int n_samples, int n_rot)
-{
-    return 4 * (size_t)DSM_HEAD_WORDS + sizeof(dsm_heading_t) * (size_t)n + (sizeof(dsm_heading_sample_t) + sizeof(dsm_heading_count_t) * (size_t)n_rot) * n_samples;
-}
-// The whole job on the state grid of the latest known request (header at dsm_field_header(voxels) of dist) for the
-// request already in `stage` on the device (n trajectories, n_samples samples, n_rot rotations, bricks in all), with
-// the successor table succ of 64 bytes per sample.  Zeroes and writes the whole used result; returns the first launch
-// or memset error.
-cudaError_t dsm_launch_heading(const DsmFieldGrid &g, const uint8_t *state, const int32_t *dist, const dsm_gain_camera_t &cam,
-                               const uint8_t *stage, int n, int n_samples, int n_rot, long long bricks, int w_unknown, int w_frontier,
-                               int8_t *succ, uint8_t *res, cudaStream_t st);

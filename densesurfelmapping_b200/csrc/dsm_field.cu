@@ -17,7 +17,10 @@
 // Squared distances are int32; an empty line holds FIELD_INF.  Every finite value is below 3 * 1023^2 < 2^22, so a site
 // and its value pack into one word and the conversion to float is exact.  The kernels carry no error gate and are
 // launched without PDL: each begins after everything enqueued before it has completed.
-#include "dsm_device.cuh"
+//
+// dsm_capi.cu enqueues the field through the launchers at the end of this file; the planner queries' C ABI calls
+// (dsm_field_query_enable, _enqueue, _enqueue_signed and _wait) follow their kernels.
+#include "dsm_ctx.hpp"
 #include <climits>
 
 #define FIELD_INF INT_MAX
@@ -256,6 +259,18 @@ __global__ void __launch_bounds__(32) k_field_lines_signed(int32_t *sdist, const
 // The point query itself (q_sample, q_empty) lives in dsm_device.cuh, shared with the trajectory job.
 // SIGNED (DESIGN.md §8.16): the same on the signed grid, whose header gives two rules in place of the "no site" one: no
 // site, +inf; no voxel of F, -inf (an interpolation of infinities of one sign would be NaN).
+//
+// One packed request (H2D) and one packed result (D2H):
+//   request  double points[n_points][3] | double waypoints[n_wp][3] | int32 offsets[n_traj + 1] | int32 first[n_wp]
+//            (first[w]: the trajectory's index of waypoint w's first sample, staged by the host; the last waypoint's
+//            entry is the index of the final sample)
+//   result   int32 header[DSM_QUERY_WORDS] | float4 samples[n_points] | dsm_clearance_t clearance[n_traj]
+enum
+{
+    DSM_QUERY_ERR_TAG,   // the field header's DSM_FIELD_ERR_TAG / _ERR_FRAME, copied by k_field_query
+    DSM_QUERY_ERR_FRAME,
+    DSM_QUERY_WORDS = 4  // 16 B: the samples stay float4-aligned
+};
 #define FIELD_QUERY_BLOCK 256
 #define FIELD_CLEAR_WARPS 8
 
@@ -333,24 +348,143 @@ __global__ void __launch_bounds__(32 * FIELD_CLEAR_WARPS) k_field_clearance(cons
     }
 }
 
-template <bool SIGNED>
-static void launch_field_query(const float *dist, const int32_t *field_header, const DsmFieldGrid &g, const double *points, int n_points,
-                               const double *waypoints, const int32_t *offsets, const int32_t *first, int n_traj, float radius,
-                               int32_t *result_header, float4 *samples, dsm_clearance_t *clearance, cudaStream_t s)
+// the packed request's sections at `base` (the pinned staging or its device twin), and the byte offsets of both layouts
+struct QueryRequest
 {
-    const int qb = (n_points + FIELD_QUERY_BLOCK - 1) / FIELD_QUERY_BLOCK;
-    k_field_query<SIGNED><<<qb > 1 ? qb : 1, FIELD_QUERY_BLOCK, 0, s>>>(dist, field_header, g, points, n_points, samples, result_header);
-    if (n_traj > 0)
-        k_field_clearance<SIGNED><<<(n_traj + FIELD_CLEAR_WARPS - 1) / FIELD_CLEAR_WARPS, 32 * FIELD_CLEAR_WARPS, 0, s>>>(
-            dist, field_header, g, waypoints, offsets, first, n_traj, radius, clearance);
+    double *points, *waypoints;
+    int32_t *offsets, *first;
+};
+static QueryRequest query_request(uint8_t *base, int n_points, int n_wp, int n_traj)
+{
+    QueryRequest r;
+    r.points = reinterpret_cast<double *>(base);
+    r.waypoints = r.points + 3 * (size_t)n_points;
+    r.offsets = reinterpret_cast<int32_t *>(r.waypoints + 3 * (size_t)n_wp);
+    r.first = r.offsets + n_traj + 1;
+    return r;
+}
+static size_t query_req_bytes(int n_points, int n_wp, int n_traj) { return 24 * ((size_t)n_points + n_wp) + 4 * ((size_t)n_traj + 1 + n_wp); }
+static size_t query_clearance_at(int n_points) { return 16 * (1 + (size_t)n_points); }
+static size_t query_res_bytes(int n_points, int n_traj) { return query_clearance_at(n_points) + 16 * (size_t)n_traj; }
+
+extern "C" int dsm_field_query_enable(dsm_ctx *ctx, int max_points, int max_trajectories, int max_waypoints)
+{
+    if (!ctx) return DSM_E_INVALID;
+    if (!ctx->field || ctx->field_query) return DSM_E_STATE;
+    for (int n : {max_points, max_trajectories, max_waypoints})
+        if (n < 0 || n > DSM_FIELD_QUERY_MAX_SAMPLES) return DSM_E_INVALID;
+    CK(cudaSetDevice(ctx->device));
+    auto q = std::make_unique<DsmFieldQuery>();
+    q->max_points = max_points, q->max_traj = max_trajectories, q->max_wp = max_waypoints;
+    const size_t req = query_req_bytes(max_points, max_waypoints, max_trajectories);
+    const size_t res = query_res_bytes(max_points, max_trajectories);
+    q->own.host(&q->req_host, req);
+    q->own.device(&q->req_dev, req);
+    q->own.device(&q->res_dev, res);
+    q->own.host(&q->res_host, res);
+    q->own.event(&q->ev);
+    return keep(ctx->field_query, q);
 }
 
-void dsm_launch_field_query(bool sgn, const float *dist, const int32_t *field_header, const DsmFieldGrid &g, const double *points,
-                            int n_points, const double *waypoints, const int32_t *offsets, const int32_t *first, int n_traj, float radius,
-                            int32_t *result_header, float4 *samples, dsm_clearance_t *clearance, cudaStream_t s)
+// Stages the request on the calling thread (checking it and counting the samples on the way), then enqueues one H2D
+// copy, the two kernels on the grid of the latest field request (sgn: on its signed grid), one D2H copy of the results
+// and the event.
+static int field_query_enqueue(dsm_ctx *ctx, bool sgn, const double *points, int n_points, const double *waypoints, const int32_t *offsets,
+                               int n_trajectories, float step, float radius)
 {
-    (sgn ? launch_field_query<true> : launch_field_query<false>)(dist, field_header, g, points, n_points, waypoints, offsets, first, n_traj,
-                                                                 radius, result_header, samples, clearance, s);
+    if (!ctx) return DSM_E_INVALID;
+    DsmFieldQuery *q = ctx->field_query.get();
+    const DsmField *f = ctx->field.get();
+    if (!q || !f || !f->requested || q->in_flight) return DSM_E_STATE;
+    if (sgn && !f->signed_latest) return DSM_E_STATE;
+    if (n_points < 0 || n_points > q->max_points || n_trajectories < 0 || n_trajectories > q->max_traj) return DSM_E_INVALID;
+    if ((n_points > 0 && !points) || (n_trajectories > 0 && (!waypoints || !offsets))) return DSM_E_INVALID;
+    if (!std::isfinite(step) || !(step > 0.f) || !std::isfinite(radius) || !(radius >= 0.f)) return DSM_E_INVALID;
+    const int n_wp = n_trajectories > 0 ? offsets[n_trajectories] : 0;
+    if (n_trajectories > 0)
+    {
+        if (offsets[0] != 0 || n_wp > q->max_wp) return DSM_E_INVALID;
+        for (int j = 0; j < n_trajectories; j++)
+            if (offsets[j + 1] <= offsets[j]) return DSM_E_INVALID;
+    }
+    const QueryRequest h = query_request(q->req_host, n_points, n_wp, n_trajectories);
+    if (n_points > 0) std::memcpy(h.points, points, 24 * (size_t)n_points);
+    // one pass over the waypoints: copy, check, and count each segment's samples m = max(1, ceil(L / step)).  The
+    // ceil is an integer test, exact once q = L / step is known to be at most 2^26 (a NaN or infinite q fails that).
+    const double dstep = (double)step;
+    int64_t total = 0; // samples of the call so far
+    for (int j = 0; j < n_trajectories; j++)
+    {
+        const int w0 = offsets[j], w1 = offsets[j + 1];
+        int64_t s = 0; // samples of trajectory j so far
+        for (int w = w0; w < w1; w++)
+        {
+            const double *a = waypoints + 3 * (size_t)w;
+            double *c = h.waypoints + 3 * (size_t)w;
+            c[0] = a[0], c[1] = a[1], c[2] = a[2];
+            if (!std::isfinite(a[0]) || !std::isfinite(a[1]) || !std::isfinite(a[2])) return DSM_E_INVALID;
+            h.first[w] = (int32_t)s;
+            int64_t m = 1; // the last waypoint: one sample
+            if (w + 1 < w1)
+            {
+                const double *b = a + 3;
+                const double dx = b[0] - a[0], dy = b[1] - a[1], dz = b[2] - a[2];
+                const double q = std::sqrt((dx * dx + dy * dy) + dz * dz) / dstep;
+                if (!(q <= (double)DSM_FIELD_QUERY_MAX_SAMPLES)) return DSM_E_INVALID;
+                m = (int64_t)q;
+                m += (double)m < q;
+                m = std::max<int64_t>(m, 1);
+            }
+            if (m > DSM_FIELD_QUERY_MAX_SAMPLES - total - s) return DSM_E_INVALID;
+            s += m;
+        }
+        total += s;
+    }
+    if (n_trajectories > 0) std::memcpy(h.offsets, offsets, 4 * ((size_t)n_trajectories + 1));
+    CK(cudaSetDevice(ctx->device));
+    CK(cudaMemcpyAsync(q->req_dev, q->req_host, query_req_bytes(n_points, n_wp, n_trajectories), cudaMemcpyHostToDevice, ctx->stream));
+    const QueryRequest d = query_request(q->req_dev, n_points, n_wp, n_trajectories);
+    int32_t *r_hdr = reinterpret_cast<int32_t *>(q->res_dev);
+    float4 *r_samples = reinterpret_cast<float4 *>(q->res_dev + 16);
+    dsm_clearance_t *r_clear = reinterpret_cast<dsm_clearance_t *>(q->res_dev + query_clearance_at(n_points));
+    // a known field's query view holds its site count where a plain field's header holds its occupied count; the signed
+    // grid's header holds it in the same word
+    const int32_t *grid = sgn ? f->sgn->grid : f->dist;
+    const int32_t *f_hdr = grid + dsm_field_header(f->voxels) + (!sgn && f->known ? DSM_FIELD_VIEW : 0);
+    const float *dist = reinterpret_cast<const float *>(grid);
+    const int qb = (n_points + FIELD_QUERY_BLOCK - 1) / FIELD_QUERY_BLOCK;
+    (sgn ? k_field_query<true> : k_field_query<false>)<<<qb > 1 ? qb : 1, FIELD_QUERY_BLOCK, 0, ctx->stream>>>(dist, f_hdr, f->g, d.points,
+                                                                                                            n_points, r_samples, r_hdr);
+    if (n_trajectories > 0)
+        (sgn ? k_field_clearance<true> : k_field_clearance<false>)<<<(n_trajectories + FIELD_CLEAR_WARPS - 1) / FIELD_CLEAR_WARPS,
+                                                                     32 * FIELD_CLEAR_WARPS, 0, ctx->stream>>>(
+            dist, f_hdr, f->g, d.waypoints, d.offsets, d.first, n_trajectories, radius, r_clear);
+    CK(cudaGetLastError());
+    q->n_points = n_points, q->n_traj = n_trajectories;
+    return submit(ctx, *q, q->res_dev, query_res_bytes(n_points, n_trajectories), f->requests);
+}
+
+extern "C" int dsm_field_query_enqueue(dsm_ctx *ctx, const double *points, int n_points, const double *waypoints, const int32_t *offsets,
+                                       int n_trajectories, float step, float radius)
+{
+    return field_query_enqueue(ctx, false, points, n_points, waypoints, offsets, n_trajectories, step, radius);
+}
+
+extern "C" int dsm_field_query_enqueue_signed(dsm_ctx *ctx, const double *points, int n_points, const double *waypoints,
+                                              const int32_t *offsets, int n_trajectories, float step, float radius)
+{
+    return field_query_enqueue(ctx, true, points, n_points, waypoints, offsets, n_trajectories, step, radius);
+}
+
+extern "C" int dsm_field_query_wait(dsm_ctx *ctx, const dsm_field_sample_t **samples, const dsm_clearance_t **clearance)
+{
+    if (!ctx) return DSM_E_INVALID;
+    DsmFieldQuery *q = ctx->field_query.get();
+    const int rc = wait_head(ctx, q);
+    if (rc != DSM_OK) return rc;
+    if (samples) *samples = reinterpret_cast<const dsm_field_sample_t *>(q->res_host + 16);
+    if (clearance) *clearance = reinterpret_cast<const dsm_clearance_t *>(q->res_host + query_clearance_at(q->n_points));
+    return capacity(ctx, q->words(), DSM_QUERY_ERR_TAG, "dsm_field_query_wait", "the field the query read");
 }
 
 int dsm_field_setup()

@@ -23,8 +23,9 @@
 //   the list            the listed clusters' members compacted in linear order (fr_select) into the first n_listed
 //                       entries of max_voxels, the rest keyed past every cluster, then cub's stable radix sort by table
 //                       slot: members grouped by cluster in table order, ascending within one.
-// The kernels carry no error gate and are launched without PDL, as the other field kernels.
-#include "dsm_device.cuh"
+// The kernels carry no error gate and are launched without PDL, as the other field kernels.  The job's C ABI calls
+// (dsm_frontier_enable, _enqueue and _wait) follow them.
+#include "dsm_ctx.hpp"
 #include <climits>
 #include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_scan.cuh>
@@ -40,6 +41,13 @@ static_assert(sizeof(dsm_frontier_cluster_t) == 96 && offsetof(dsm_frontier_clus
                   offsetof(dsm_frontier_cluster_t, centroid) == 72, "dsm_frontier_cluster_t layout");
 static_assert(sizeof(dsm_frontier_counts_t) == 16 && offsetof(dsm_frontier_counts_t, n_listed) == 12, "dsm_frontier_counts_t layout");
 static_assert(DSM_FRONTIER_N_LISTED == 3 && 4 * DSM_FRONTIER_WORDS % 8 == 0, "the header starts with the counts");
+
+// what k_frontier_reduce accumulates per table entry (integer atomics only)
+struct DsmFrontierAcc
+{
+    int32_t lo[3], hi[3];
+    unsigned long long sum[3], faces, open[3]; // two's complement int64
+};
 
 // the 13 backward neighbours of the 26-neighbourhood: dz < 0, or dz == 0 and dy < 0, or dz == dy == 0 and dx < 0
 __constant__ int8_t c_back[13][3] = {{-1, -1, -1}, {0, -1, -1}, {1, -1, -1}, {-1, 0, -1}, {0, 0, -1}, {1, 0, -1}, {-1, 1, -1},
@@ -426,12 +434,13 @@ __global__ void __launch_bounds__(FR_BLOCK) k_frontier_sel_write(const P pred, i
 
 static unsigned fr_blocks(int n) { return n > 0 ? (unsigned)((n + FR_BLOCK - 1) / FR_BLOCK) : 1u; }
 static int fr_key_bits(int max_clusters) { return 32 - __builtin_clz((unsigned)max_clusters | 1u); } // the key past every slot fits
-int dsm_frontier_sel_blocks(int voxels) { return (voxels + FR_SEL - 1) / FR_SEL; }
+static int fr_sel_blocks(int voxels) { return (voxels + FR_SEL - 1) / FR_SEL; }
+static size_t fr_res_bytes(const DsmFrontier &b) { return b.list_at() + 4 * (size_t)b.max_voxels; }
 
 template <class P>
-static cudaError_t fr_select(const DsmFrontierBufs &b, const P &pred, int32_t *out, int32_t *count, cudaStream_t s)
+static cudaError_t fr_select(const DsmFrontier &b, const P &pred, int32_t *out, int32_t *count, cudaStream_t s)
 {
-    const int nb = dsm_frontier_sel_blocks(b.voxels);
+    const int nb = fr_sel_blocks(b.voxels);
     k_frontier_sel_count<<<nb, FR_BLOCK, 0, s>>>(pred, b.voxels, b.blk);
     size_t n = b.temp_bytes;
     cudaError_t e = cudaGetLastError();
@@ -443,25 +452,25 @@ static cudaError_t fr_select(const DsmFrontierBufs &b, const P &pred, int32_t *o
 
 // The CUB calls of the job at the sizes fixed at enable (0: the CTA scan of fr_select, 1: the cluster numbering, 2: the
 // list offsets, 3: the list's sort); temp == nullptr only sizes the scratch into *bytes.
-static cudaError_t fr_cub(const DsmFrontierBufs &b, void *temp, size_t *bytes, cudaStream_t s, int which)
+static cudaError_t fr_cub(const DsmFrontier &b, void *temp, size_t *bytes, cudaStream_t s, int which)
 {
     size_t n = temp ? b.temp_bytes : 0;
     cudaError_t e = cudaSuccess;
     switch (which)
     {
-    case 0: e = cub::DeviceScan::ExclusiveSum(temp, n, b.blk, b.blk_ofs, dsm_frontier_sel_blocks(b.voxels), s); break;
+    case 0: e = cub::DeviceScan::ExclusiveSum(temp, n, b.blk, b.blk_ofs, fr_sel_blocks(b.voxels), s); break;
     case 1: e = cub::DeviceScan::ExclusiveSum(temp, n, b.cmap, b.cid, b.max_comp, s); break;
     case 2: e = cub::DeviceScan::ExclusiveSum(temp, n, b.sizes, b.offs, b.max_clusters, s); break;
     default:
-        e = cub::DeviceRadixSort::SortPairs(temp, n, b.keys, b.keys_alt, b.idx,
-                                            reinterpret_cast<int32_t *>(b.res + 4 * DSM_FRONTIER_WORDS + sizeof(dsm_frontier_cluster_t) * (size_t)b.max_clusters),
-                                            b.max_voxels, 0, fr_key_bits(b.max_clusters), s);
+        e = cub::DeviceRadixSort::SortPairs(temp, n, b.keys, b.keys_alt, b.idx, reinterpret_cast<int32_t *>(b.res + b.list_at()), b.max_voxels,
+                                            0, fr_key_bits(b.max_clusters), s);
     }
     if (!temp) *bytes = n;
     return e;
 }
 
-size_t dsm_frontier_temp_bytes(const DsmFrontierBufs &b)
+// the CUB scratch the job needs for its sizes (the buffers' pointers may still be null); 0 on a CUB error
+static size_t fr_temp_bytes(const DsmFrontier &b)
 {
     size_t most = 1;
     for (int which = 0; which < 4; which++)
@@ -475,42 +484,105 @@ size_t dsm_frontier_temp_bytes(const DsmFrontierBufs &b)
     return most;
 }
 
-cudaError_t dsm_launch_frontier(const DsmFrontierBufs &b, const DsmFieldGrid &g, const uint8_t *state, const int32_t *field_header,
-                                int min_voxels, cudaStream_t s)
+extern "C" int dsm_frontier_enable(dsm_ctx *ctx, int max_clusters, int max_voxels)
 {
+    if (!ctx) return DSM_E_INVALID;
+    const DsmField *f = ctx->field.get();
+    if (!f || !ctx->views || ctx->frontier) return DSM_E_STATE;
+    for (int n : {max_clusters, max_voxels})
+        if (n < 0 || n > DSM_FRONTIER_MAX_CAPACITY) return DSM_E_INVALID;
+    CK(cudaSetDevice(ctx->device));
+    auto fr = std::make_unique<DsmFrontier>();
+    DsmFrontier &b = *fr;
+    const int *n = f->g.n;
+    b.voxels = (int)f->voxels;
+    // every 2x2x2 block of voxels is 26-connected, so it meets at most one component
+    b.max_comp = ((n[0] + 1) / 2) * ((n[1] + 1) / 2) * ((n[2] + 1) / 2);
+    b.max_clusters = max_clusters, b.max_voxels = max_voxels;
+    const size_t cl = (size_t)std::max(max_clusters, 1), vx = (size_t)std::max(max_voxels, 1);
+    const size_t sel = (size_t)fr_sel_blocks(b.voxels);
+    const size_t res = fr_res_bytes(b);
+    CudaOwner &o = fr->own;
+    o.device(&b.label, f->voxels);
+    for (int32_t **p : {&b.roots, &b.count, &b.cmap, &b.cid}) o.device(p, (size_t)b.max_comp);
+    for (int32_t **p : {&b.slot_comp, &b.sizes, &b.offs}) o.device(p, cl);
+    o.device(&b.acc, cl);
+    o.device(&b.idx, vx);
+    o.device(&b.keys, vx);
+    o.device(&b.keys_alt, vx);
+    o.device(&b.blk, sel);
+    o.device(&b.blk_ofs, sel);
+    o.device(&b.res, res);
+    o.host(&fr->res_host, res);
+    o.event(&fr->ev);
+    b.temp_bytes = fr_temp_bytes(b);
+    if (b.temp_bytes) o.device(reinterpret_cast<uint8_t **>(&b.temp), b.temp_bytes);
+    return keep(ctx->frontier, fr, b.temp_bytes != 0);
+}
+
+// Enqueue only: the job on the state grid of the latest (known) field request with that request's origin, one D2H copy
+// of the result capacity and the event.  A later field request clears that grid only behind the job, in stream order.
+extern "C" int dsm_frontier_enqueue(dsm_ctx *ctx, int min_voxels)
+{
+    if (!ctx) return DSM_E_INVALID;
+    DsmFrontier *fr = ctx->frontier.get();
+    const DsmField *f = known_field(ctx);
+    if (!fr || !f || fr->in_flight) return DSM_E_STATE;
+    if (min_voxels < 1) return DSM_E_INVALID;
+    CK(cudaSetDevice(ctx->device));
+    const DsmFrontier &b = *fr;
+    const DsmFieldGrid &g = f->g;
+    const uint8_t *state = f->occ;
+    const cudaStream_t s = ctx->stream;
     int32_t *hdr = reinterpret_cast<int32_t *>(b.res);
-    auto *table = reinterpret_cast<dsm_frontier_cluster_t *>(b.res + 4 * DSM_FRONTIER_WORDS);
+    auto *table = reinterpret_cast<dsm_frontier_cluster_t *>(b.res + DsmFrontier::table_at());
+    CK(cudaMemsetAsync(b.res, 0, 4 * DSM_FRONTIER_WORDS, s));
     const int rows = g.n[1] * g.n[2];
-    k_frontier_mark<<<(unsigned)(rows + FR_ROW_WARPS - 1) / FR_ROW_WARPS, 32 * FR_ROW_WARPS, 0, s>>>(g, state, field_header, b.label, hdr);
+    k_frontier_mark<<<(unsigned)(rows + FR_ROW_WARPS - 1) / FR_ROW_WARPS, 32 * FR_ROW_WARPS, 0, s>>>(g, state, f->dist + dsm_field_header(f->voxels),
+                                                                                                 b.label, hdr);
     const dim3 tiles((g.n[0] + FR_TX - 1) / FR_TX, (g.n[1] + FR_TY - 1) / FR_TY, (g.n[2] + FR_TZ - 1) / FR_TZ);
     k_frontier_tile<<<tiles, FR_TILE, 0, s>>>(g, b.label);
     k_frontier_seam<<<tiles, FR_TILE, 0, s>>>(g, b.label);
     k_frontier_flatten<<<fr_blocks(b.voxels), FR_BLOCK, 0, s>>>(b.label, b.voxels);
-    cudaError_t e = cudaGetLastError();
-    if (e == cudaSuccess) e = fr_select(b, FrIsRoot{b.label}, b.roots, hdr + DSM_FRONTIER_N_COMPONENTS, s);
-    if (e != cudaSuccess) return e;
+    CK(cudaGetLastError());
+    CK(fr_select(b, FrIsRoot{b.label}, b.roots, hdr + DSM_FRONTIER_N_COMPONENTS, s));
     k_frontier_number<<<fr_blocks(b.max_comp), FR_BLOCK, 0, s>>>(b.label, b.roots, b.count, hdr);
     k_frontier_count<<<fr_blocks(b.voxels), FR_BLOCK, 0, s>>>(b.label, b.voxels, b.count);
     k_frontier_keep<<<fr_blocks(b.max_comp), FR_BLOCK, 0, s>>>(b.count, b.max_comp, min_voxels, b.cmap, hdr);
-    e = cudaGetLastError();
-    if (e == cudaSuccess) e = fr_cub(b, b.temp, nullptr, s, 1);
-    if (e == cudaSuccess && b.max_clusters > 0) e = cudaMemsetAsync(b.sizes, 0, 4 * (size_t)b.max_clusters, s);
-    if (e != cudaSuccess) return e;
+    CK(cudaGetLastError());
+    CK(fr_cub(b, b.temp, nullptr, s, 1));
+    if (b.max_clusters > 0) CK(cudaMemsetAsync(b.sizes, 0, 4 * (size_t)b.max_clusters, s));
     k_frontier_slot<<<fr_blocks(b.max_comp), FR_BLOCK, 0, s>>>(b.count, b.cmap, b.cid, b.max_clusters, b.slot_comp, b.sizes, b.acc, hdr);
-    e = cudaGetLastError();
-    if (e != cudaSuccess || b.max_clusters == 0) return e;
-    k_frontier_reduce<<<fr_blocks(b.voxels), FR_BLOCK, 0, s>>>(g, state, b.label, b.cmap, b.acc);
-    e = cudaGetLastError();
-    if (e == cudaSuccess) e = fr_cub(b, b.temp, nullptr, s, 2);
-    if (e != cudaSuccess) return e;
-    k_frontier_table<<<fr_blocks(b.max_clusters), FR_BLOCK, 0, s>>>(g, b.roots, b.slot_comp, b.sizes, b.offs, b.acc, b.max_clusters,
-                                                                    b.max_voxels, table, hdr);
-    e = cudaGetLastError();
-    if (e != cudaSuccess || b.max_voxels == 0) return e;
-    e = fr_select(b, FrIsListed{b.label, b.cmap, hdr}, b.idx, hdr + DSM_FRONTIER_N_SELECTED, s);
-    if (e != cudaSuccess) return e;
-    k_frontier_keys<<<fr_blocks(b.max_voxels), FR_BLOCK, 0, s>>>(b.label, b.cmap, b.idx, b.keys, b.max_voxels, (uint32_t)b.max_clusters, hdr);
-    e = cudaGetLastError();
-    if (e == cudaSuccess) e = fr_cub(b, b.temp, nullptr, s, 3);
-    return e;
+    CK(cudaGetLastError());
+    if (b.max_clusters > 0)
+    {
+        k_frontier_reduce<<<fr_blocks(b.voxels), FR_BLOCK, 0, s>>>(g, state, b.label, b.cmap, b.acc);
+        CK(cudaGetLastError());
+        CK(fr_cub(b, b.temp, nullptr, s, 2));
+        k_frontier_table<<<fr_blocks(b.max_clusters), FR_BLOCK, 0, s>>>(g, b.roots, b.slot_comp, b.sizes, b.offs, b.acc, b.max_clusters,
+                                                                        b.max_voxels, table, hdr);
+        CK(cudaGetLastError());
+        if (b.max_voxels > 0)
+        {
+            CK(fr_select(b, FrIsListed{b.label, b.cmap, hdr}, b.idx, hdr + DSM_FRONTIER_N_SELECTED, s));
+            k_frontier_keys<<<fr_blocks(b.max_voxels), FR_BLOCK, 0, s>>>(b.label, b.cmap, b.idx, b.keys, b.max_voxels, (uint32_t)b.max_clusters,
+                                                                         hdr);
+            CK(cudaGetLastError());
+            CK(fr_cub(b, b.temp, nullptr, s, 3));
+        }
+    }
+    return submit(ctx, *fr, b.res, fr_res_bytes(b), f->requests);
+}
+
+extern "C" int dsm_frontier_wait(dsm_ctx *ctx, const dsm_frontier_cluster_t **clusters, const int32_t **voxels, dsm_frontier_counts_t *counts)
+{
+    if (!ctx) return DSM_E_INVALID;
+    DsmFrontier *fr = ctx->frontier.get();
+    const int rc = wait_head(ctx, fr);
+    if (rc != DSM_OK) return rc;
+    const int32_t *h = fr->words();
+    if (clusters) *clusters = reinterpret_cast<const dsm_frontier_cluster_t *>(fr->res_host + DsmFrontier::table_at());
+    if (voxels) *voxels = reinterpret_cast<const int32_t *>(fr->res_host + fr->list_at());
+    if (counts) std::memcpy(counts, h, sizeof(dsm_frontier_counts_t));
+    return capacity(ctx, h, DSM_FRONTIER_ERR_TAG, "dsm_frontier_wait", "the field the job read");
 }

@@ -2,7 +2,7 @@
 // the free, unknown, occupied, frontier and cluster voxels it would see through the known grid.
 //
 //   k_gain_slots   one thread per entry of the frontier list (with clusters only): slot[list[j]] = the table entry that
-//                  lists j, over a slot grid the launcher set to -1.
+//                  lists j, over a slot grid the enqueue set to -1.
 //   k_gain_init    one thread per view: the record's zero counts, its status and n_cluster (0, or -1 without a countable
 //                  cluster); thread 0 writes the header and copies the field's error words.
 //   k_gain_views   one 8x8x4 brick of a view's box per CTA of 256 threads, one voxel per thread, bricks laid out
@@ -13,10 +13,25 @@
 // The frustum test and the walk are dsm_gain_frustum and dsm_gain_walk (dsm_device.cuh), shared with k_vp_score.  The
 // walk is not shared with k_field_carve: carving visits every voxel and stores into the grid, the gain walk reads and
 // stops at the first blocking voxel, so a shared helper would branch on its caller.  The kernels carry no error gate and
-// are launched without PDL, as the other field kernels.
-#include "dsm_device.cuh"
-#include <algorithm>
+// are launched without PDL, as the other field kernels.  The job's C ABI calls (dsm_gain_enable, _enqueue and _wait)
+// follow them.
+//
+// One staged request (H2D), DsmGainView views[n_views] (dsm_device.cuh), and one packed result (D2H):
+//   int32 header[DSM_GAIN_WORDS] | dsm_view_gain_t gains[max_views]
+// The header's first six words are those of dsm_gain_info_t; its padding carries the field's error words, cleared by
+// dsm_gain_wait.
+#include "dsm_ctx.hpp"
 
+enum
+{
+    DSM_GAIN_ORIGIN = 0, // 3 words
+    DSM_GAIN_N_VIEWS = 3,
+    DSM_GAIN_N_CLUSTERS_TABLE,
+    DSM_GAIN_UNKNOWN_BLOCKS,
+    DSM_GAIN_ERR_TAG, // the field header's DSM_FIELD_ERR_TAG / _ERR_FRAME, copied by k_gain_init
+    DSM_GAIN_ERR_FRAME,
+    DSM_GAIN_WORDS = 8 // 32 B
+};
 #define GAIN_BLOCK (DSM_GAIN_BX * DSM_GAIN_BY * DSM_GAIN_BZ) // 256
 
 static_assert(sizeof(dsm_view_gain_t) == 32 && sizeof(dsm_gain_info_t) == 32 && sizeof(dsm_gain_camera_t) == 48, "dsm_gain layouts");
@@ -155,30 +170,93 @@ __global__ void __launch_bounds__(GAIN_BLOCK) k_gain_views(const DsmFieldGrid g,
     if (tid < GAIN_COUNTS && s_cnt[tid]) atomicAdd(reinterpret_cast<int32_t *>(out + j) + tid, (int)s_cnt[tid]);
 }
 
-cudaError_t dsm_launch_gain(const DsmFieldGrid &g, const uint8_t *state, const int32_t *dist, const dsm_gain_camera_t &cam,
-                            const DsmGainView *views, int n_views, long long bricks, const uint8_t *frontier_res,
-                            int frontier_max_clusters, int32_t *slot, uint8_t *res, cudaStream_t st)
+static size_t gain_res_bytes(int n_views) { return 4 * (size_t)DSM_GAIN_WORDS + sizeof(dsm_view_gain_t) * (size_t)n_views; }
+
+extern "C" int dsm_gain_enable(dsm_ctx *ctx, int max_views)
 {
-    const size_t voxels = (size_t)g.n[0] * g.n[1] * g.n[2];
-    int32_t *hdr = reinterpret_cast<int32_t *>(res);
-    auto *out = reinterpret_cast<dsm_view_gain_t *>(res + 4 * DSM_GAIN_WORDS);
-    const int32_t *fieldhdr = dist + dsm_field_header(voxels);
-    const int32_t *fhdr = reinterpret_cast<const int32_t *>(frontier_res);
-    const auto *table = frontier_res ? reinterpret_cast<const dsm_frontier_cluster_t *>(frontier_res + 4 * DSM_FRONTIER_WORDS) : nullptr;
-    if (frontier_res)
+    if (!ctx) return DSM_E_INVALID;
+    const DsmField *f = ctx->field.get();
+    if (!f || !ctx->views || ctx->gain) return DSM_E_STATE;
+    if (max_views < 1 || max_views > DSM_GAIN_MAX_VIEWS) return DSM_E_INVALID;
+    CK(cudaSetDevice(ctx->device));
+    auto ga = std::make_unique<DsmGain>();
+    ga->max_views = max_views;
+    const size_t res = gain_res_bytes(max_views);
+    CudaOwner &o = ga->own;
+    o.device(&ga->views_dev, (size_t)max_views);
+    o.host(&ga->views_host, (size_t)max_views);
+    o.device(&ga->slot, f->voxels);
+    o.device(&ga->res, res);
+    o.host(&ga->res_host, res);
+    o.event(&ga->ev);
+    return keep(ctx->gain, ga);
+}
+
+// Enqueue only: the views staged (pose, box, cluster and first brick) and copied, the kernels on the state grid of the
+// latest (known) field request and, with clusters, on the latest frontier job's device result, one D2H copy of the used
+// result and the event.  Later field and frontier requests overwrite those buffers only behind the job.
+extern "C" int dsm_gain_enqueue(dsm_ctx *ctx, const dsm_gain_camera_t *camera, const double *poses, const int32_t *clusters, int n_views)
+{
+    if (!ctx) return DSM_E_INVALID;
+    DsmGain *ga = ctx->gain.get();
+    const DsmField *f = known_field(ctx);
+    if (!ga || !f || ga->in_flight) return DSM_E_STATE;
+    const DsmFrontier *fr = ctx->frontier.get();
+    if (clusters && !read_latest(fr, f)) return DSM_E_STATE;
+    if (!camera || n_views < 0 || n_views > ga->max_views || (n_views > 0 && !poses)) return DSM_E_INVALID;
+    const dsm_gain_camera_t &c = *camera;
+    const double v = (double)f->g.voxel, R = (double)c.max_range;
+    if (!gain_camera_ok(c, v)) return DSM_E_INVALID;
+    const long long m = 2 * (long long)std::ceil(R / v) + 3;
+    if ((long long)n_views * m * m * m > DSM_GAIN_MAX_WORK) return DSM_E_INVALID;
+    for (size_t i = 0; i < 12 * (size_t)n_views; i++)
+        if (!std::isfinite(poses[i])) return DSM_E_INVALID;
+    if (clusters)
+        for (int j = 0; j < n_views; j++)
+            if (clusters[j] < -1) return DSM_E_INVALID;
+    CK(cudaSetDevice(ctx->device));
+    // the previous job's copy out of this staging ended before its wait, which no job in flight implies
+    long long bricks = 0;
+    for (int j = 0; j < n_views; j++)
     {
-        const int32_t *list = reinterpret_cast<const int32_t *>(frontier_res + 4 * DSM_FRONTIER_WORDS +
-                                                                sizeof(dsm_frontier_cluster_t) * (size_t)frontier_max_clusters);
-        const cudaError_t e = cudaMemsetAsync(slot, 0xff, 4 * voxels, st);
-        if (e != cudaSuccess) return e;
-        k_gain_slots<<<(unsigned)std::min<size_t>((voxels + GAIN_BLOCK - 1) / GAIN_BLOCK, 1024), GAIN_BLOCK, 0, st>>>(table, list, fhdr,
-                                                                                                                   frontier_max_clusters, slot);
+        DsmGainView &V = ga->views_host[j];
+        std::memcpy(V.P, poses + 12 * (size_t)j, sizeof(V.P));
+        gain_box(V.P, c, f->g, V);
+        V.cluster = clusters ? clusters[j] : -1;
+        V.brick0 = (int)bricks; // below 2^31: the work bound caps the bricks far lower
+        bricks += dsm_gain_bricks(V.size);
+    }
+    const cudaStream_t st = ctx->stream;
+    if (n_views > 0) CK(cudaMemcpyAsync(ga->views_dev, ga->views_host, sizeof(DsmGainView) * (size_t)n_views, cudaMemcpyHostToDevice, st));
+    const DsmFieldGrid &g = f->g;
+    int32_t *hdr = reinterpret_cast<int32_t *>(ga->res);
+    auto *out = reinterpret_cast<dsm_view_gain_t *>(ga->res + 4 * DSM_GAIN_WORDS);
+    // the frontier job's result, with clusters
+    const int32_t *fhdr = clusters ? reinterpret_cast<const int32_t *>(fr->res) : nullptr;
+    const auto *table = clusters ? reinterpret_cast<const dsm_frontier_cluster_t *>(fr->res + DsmFrontier::table_at()) : nullptr;
+    const int frontier_max_clusters = clusters ? fr->max_clusters : 0;
+    if (clusters)
+    {
+        CK(cudaMemsetAsync(ga->slot, 0xff, 4 * f->voxels, st));
+        k_gain_slots<<<(unsigned)std::min<size_t>((f->voxels + GAIN_BLOCK - 1) / GAIN_BLOCK, 1024), GAIN_BLOCK, 0, st>>>(
+            table, reinterpret_cast<const int32_t *>(fr->res + fr->list_at()), fhdr, frontier_max_clusters, ga->slot);
     }
     k_gain_init<<<(unsigned)std::max((n_views + GAIN_BLOCK - 1) / GAIN_BLOCK, 1), GAIN_BLOCK, 0, st>>>(
-        g, views, n_views, fieldhdr, fhdr, table, frontier_max_clusters, cam.unknown_blocks, hdr, out);
-    const double R = (double)cam.max_range;
+        g, ga->views_dev, n_views, f->dist + dsm_field_header(f->voxels), fhdr, table, frontier_max_clusters, c.unknown_blocks, hdr, out);
     if (bricks > 0)
-        k_gain_views<<<(unsigned)bricks, GAIN_BLOCK, 0, st>>>(g, state, views, n_views, cam.fx, cam.fy, cam.cx, cam.cy, (double)cam.width,
-                                                              (double)cam.height, R * R, cam.unknown_blocks, frontier_res ? slot : nullptr, out);
-    return cudaGetLastError();
+        k_gain_views<<<(unsigned)bricks, GAIN_BLOCK, 0, st>>>(g, f->occ, ga->views_dev, n_views, c.fx, c.fy, c.cx, c.cy, (double)c.width,
+                                                              (double)c.height, R * R, c.unknown_blocks, clusters ? ga->slot : nullptr, out);
+    CK(cudaGetLastError());
+    return submit(ctx, *ga, ga->res, gain_res_bytes(n_views), f->requests);
+}
+
+extern "C" int dsm_gain_wait(dsm_ctx *ctx, dsm_gain_info_t *info, const dsm_view_gain_t **gains)
+{
+    if (!ctx) return DSM_E_INVALID;
+    DsmGain *ga = ctx->gain.get();
+    const int rc = wait_head(ctx, ga);
+    if (rc != DSM_OK) return rc;
+    copy_info(info, ga->words());
+    if (gains) *gains = reinterpret_cast<const dsm_view_gain_t *>(ga->res_host + 4 * DSM_GAIN_WORDS);
+    return capacity(ctx, ga->words(), DSM_GAIN_ERR_TAG, "dsm_gain_wait", "the field the job read");
 }

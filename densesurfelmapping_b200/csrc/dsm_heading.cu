@@ -14,10 +14,42 @@
 //                    first best step per (sample, rotation) stored as int8 in the successor table; then lane 0 traces
 //                    forward from start and writes the rotations, turns and the record.  Block 0 writes the header.
 // The counts are integers and the plan exact in int64, so the result does not depend on the schedule.  The kernels
-// carry no error gate and are launched without PDL, as the other field kernels.
-#include "dsm_device.cuh"
-#include <algorithm>
+// carry no error gate and are launched without PDL, as the other field kernels.  The job's C ABI calls
+// (dsm_heading_enable, _enqueue and _wait) follow them.
+//
+// One staged request (H2D, head_stage_bytes(n, S)):
+//   double rotations[64][9] | DsmHeadingTraj trajectories[n] | DsmHeadingSample samples[S]
+// and one packed result (D2H, head_res_bytes(n, S, n_rot)):
+//   int32 header[DSM_HEAD_WORDS] | dsm_heading_t records[n] | dsm_heading_sample_t samples[S] | dsm_heading_count_t counts[S][n_rot]
+// The header's first eleven words are those of dsm_heading_info_t; its last two carry the field's error words, cleared
+// by dsm_heading_wait.
+#include "dsm_ctx.hpp"
 #include <climits>
+
+enum
+{
+    DSM_HEAD_ORIGIN = 0, // 3 words
+    DSM_HEAD_N = 3,
+    DSM_HEAD_N_SAMPLES,
+    DSM_HEAD_N_ROT,
+    DSM_HEAD_UNKNOWN_BLOCKS,
+    DSM_HEAD_N_STATUS,     // 2 words: trajectories per status (k_heading_plan adds)
+    DSM_HEAD_ERR_TAG = 14, // the field header's DSM_FIELD_ERR_TAG / _ERR_FRAME, copied by k_heading_plan
+    DSM_HEAD_ERR_FRAME,
+    DSM_HEAD_WORDS = 16 // 64 B
+};
+// one trajectory as the host stages it: its first sample and samples, the request, and its samples outside the grid
+struct DsmHeadingTraj
+{
+    int32_t sample0, n_samples, start, end, max_step, n_outside;
+}; // 24 B
+// one sample as the host stages it: the camera position, the hull of its gain boxes over the rotations (lo, size; size
+// 0 on an axis: empty, as for a camera outside the grid) and its first brick in the launch
+struct DsmHeadingSample
+{
+    double p[3];
+    int32_t lo[3], size[3], brick0, pad;
+}; // 56 B
 
 #define HEAD_BLOCK (DSM_GAIN_BX * DSM_GAIN_BY * DSM_GAIN_BZ) // 256
 #define HEAD_PLAN_WARPS 4
@@ -199,26 +231,186 @@ __global__ void __launch_bounds__(HEAD_PLAN_WARPS * 32) k_heading_plan(const Dsm
     atomicAdd(&hdr[DSM_HEAD_N_STATUS + R.status], 1);
 }
 
-cudaError_t dsm_launch_heading(const DsmFieldGrid &g, const uint8_t *state, const int32_t *dist, const dsm_gain_camera_t &cam,
-                               const uint8_t *stage, int n, int n_samples, int n_rot, long long bricks, int w_unknown, int w_frontier,
-                               int8_t *succ, uint8_t *res, cudaStream_t st)
+// The sections of a staged request at `base` (the pinned staging or its device twin) and of a result at `base` (the
+// device result or its pinned copy), for n trajectories and S samples
+struct HeadStage
 {
-    const size_t voxels = (size_t)g.n[0] * g.n[1] * g.n[2];
-    const cudaError_t e = cudaMemsetAsync(res, 0, dsm_heading_res_bytes(n, n_samples, n_rot), st);
-    if (e != cudaSuccess) return e;
-    int32_t *hdr = reinterpret_cast<int32_t *>(res);
-    auto *rec = reinterpret_cast<dsm_heading_t *>(res + 4 * DSM_HEAD_WORDS);
-    auto *out = reinterpret_cast<dsm_heading_sample_t *>(rec + n);
-    auto *counts = reinterpret_cast<dsm_heading_count_t *>(out + n_samples);
-    const double *rot = reinterpret_cast<const double *>(stage);
-    const auto *traj = reinterpret_cast<const DsmHeadingTraj *>(stage + 72 * (size_t)DSM_HEADING_MAX_ROTATIONS);
-    const auto *smp = reinterpret_cast<const DsmHeadingSample *>(traj + n);
-    const double R = (double)cam.max_range;
+    double *rot;
+    DsmHeadingTraj *traj;
+    DsmHeadingSample *smp;
+};
+static HeadStage head_stage(uint8_t *base, int n)
+{
+    HeadStage h;
+    h.rot = reinterpret_cast<double *>(base);
+    h.traj = reinterpret_cast<DsmHeadingTraj *>(base + 72 * (size_t)DSM_HEADING_MAX_ROTATIONS);
+    h.smp = reinterpret_cast<DsmHeadingSample *>(h.traj + n);
+    return h;
+}
+struct HeadResult
+{
+    int32_t *hdr;
+    dsm_heading_t *rec;
+    dsm_heading_sample_t *out;
+    dsm_heading_count_t *counts;
+};
+static HeadResult head_result(uint8_t *base, int n, int S)
+{
+    HeadResult r;
+    r.hdr = reinterpret_cast<int32_t *>(base);
+    r.rec = reinterpret_cast<dsm_heading_t *>(base + 4 * DSM_HEAD_WORDS);
+    r.out = reinterpret_cast<dsm_heading_sample_t *>(r.rec + n);
+    r.counts = reinterpret_cast<dsm_heading_count_t *>(r.out + S);
+    return r;
+}
+static size_t head_stage_bytes(int n, int S)
+{
+    return 72 * (size_t)DSM_HEADING_MAX_ROTATIONS + sizeof(DsmHeadingTraj) * (size_t)n + sizeof(DsmHeadingSample) * (size_t)S;
+}
+static size_t head_res_bytes(int n, int S, int n_rot)
+{
+    return 4 * (size_t)DSM_HEAD_WORDS + sizeof(dsm_heading_t) * (size_t)n + (sizeof(dsm_heading_sample_t) + sizeof(dsm_heading_count_t) * (size_t)n_rot) * S;
+}
+
+extern "C" int dsm_heading_enable(dsm_ctx *ctx, int max_trajectories, int max_samples)
+{
+    if (!ctx) return DSM_E_INVALID;
+    const DsmField *f = ctx->field.get();
+    if (!f || !ctx->views || ctx->heading) return DSM_E_STATE;
+    if (max_trajectories < 1 || max_trajectories > DSM_HEADING_MAX_CAPACITY || max_samples < 1 || max_samples > DSM_HEADING_MAX_CAPACITY)
+        return DSM_E_INVALID;
+    CK(cudaSetDevice(ctx->device));
+    auto hd = std::make_unique<DsmHeading>();
+    hd->max_traj = max_trajectories, hd->max_samples = max_samples;
+    const size_t stage = head_stage_bytes(max_trajectories, max_samples), res = head_res_bytes(max_trajectories, max_samples, DSM_HEADING_MAX_ROTATIONS);
+    CudaOwner &o = hd->own;
+    o.host(&hd->stage_host, stage);
+    o.device(&hd->stage_dev, stage);
+    o.device(&hd->succ, (size_t)DSM_HEADING_MAX_ROTATIONS * max_samples);
+    o.device(&hd->res, res);
+    o.host(&hd->res_host, res);
+    o.event(&hd->ev);
+    return keep(ctx->heading, hd);
+}
+
+// Sample s of the uniform cubic B-spline Q[N][3] at K samples per segment (include/dsm.h: the final-check samples of a
+// trajectory job), each operation rounded once (the host code is built without contraction)
+static void spline_sample(const double *Q, int N, int K, int s, double p[3])
+{
+    const int m = std::min(s / K, N - 4);
+    const double u = (double)(s - m * K) / (double)K, u2 = u * u, u3 = u2 * u, w = 1.0 - u;
+    const double b0 = ((w * w) * w) / 6.0, b1 = ((3.0 * u3 - 6.0 * u2) + 4.0) / 6.0, b2 = (((3.0 * u2 - 3.0 * u3) + 3.0 * u) + 1.0) / 6.0,
+                 b3 = u3 / 6.0;
+    const double *q = Q + 3 * (size_t)m;
+    for (int k = 0; k < 3; k++) p[k] = ((b0 * q[k] + b1 * q[3 + k]) + b2 * q[6 + k]) + b3 * q[9 + k];
+}
+
+// Stages the request on the calling thread (checking it on the way): per sample its position and the hull of gain's
+// boxes over the rotations, then enqueues one H2D copy, the kernels on the state grid of the latest (known) field
+// request, one D2H copy of the used result and the event.  Later field requests overwrite that grid only behind the job.
+extern "C" int dsm_heading_enqueue(dsm_ctx *ctx, const double *points, const int32_t *offsets, int n_trajectories, const dsm_gain_camera_t *camera,
+                                   const double *rotations, int n_rot, int samples, const dsm_heading_request_t *requests, int32_t w_unknown,
+                                   int32_t w_frontier)
+{
+    if (!ctx) return DSM_E_INVALID;
+    DsmHeading *hd = ctx->heading.get();
+    const DsmField *f = known_field(ctx);
+    if (!hd || !f || hd->in_flight) return DSM_E_STATE;
+    if (!points || !offsets || !camera || !rotations || !requests || n_trajectories < 1 || n_trajectories > hd->max_traj) return DSM_E_INVALID;
+    const dsm_gain_camera_t &c = *camera;
+    const double v = (double)f->g.voxel;
+    if (!gain_camera_ok(c, v) || n_rot < 1 || n_rot > DSM_HEADING_MAX_ROTATIONS || samples < 1 || samples > DSM_HEADING_MAX_SAMPLES_PER_SEGMENT ||
+        w_unknown < 0 || w_unknown > DSM_HEADING_MAX_WEIGHT || w_frontier < 0 || w_frontier > DSM_HEADING_MAX_WEIGHT)
+        return DSM_E_INVALID;
+    for (size_t i = 0; i < 9 * (size_t)n_rot; i++)
+        if (!std::isfinite(rotations[i])) return DSM_E_INVALID;
+    if (!spline_points_ok(points, offsets, n_trajectories, INT32_MAX)) return DSM_E_INVALID;
+    long long n_samples = 0;
+    for (int j = 0; j < n_trajectories; j++)
+    {
+        const dsm_heading_request_t &q = requests[j];
+        if (q.start < 0 || q.start >= n_rot || q.end < -1 || q.end >= n_rot || q.max_step < 0 || q.max_step > n_rot) return DSM_E_INVALID;
+        n_samples += (long long)samples * (offsets[j + 1] - offsets[j] - 3) + 1;
+    }
+    const long long m = 2 * (long long)std::ceil((double)c.max_range / v) + 3;
+    if (n_samples > hd->max_samples || n_samples * m * m * m > DSM_HEADING_MAX_WORK) return DSM_E_INVALID;
+    // the packed request; the previous job's copy out of this staging ended before its wait, which no job in flight
+    // implies
+    const HeadStage h = head_stage(hd->stage_host, n_trajectories);
+    std::memcpy(h.rot, rotations, 72 * (size_t)n_rot);
+    long long bricks = 0;
+    int s0 = 0;
+    for (int j = 0; j < n_trajectories; j++)
+    {
+        const int N = offsets[j + 1] - offsets[j], S = samples * (N - 3) + 1;
+        DsmHeadingTraj &T = h.traj[j];
+        T.sample0 = s0, T.n_samples = S, T.start = requests[j].start, T.end = requests[j].end, T.max_step = requests[j].max_step;
+        T.n_outside = 0;
+        for (int s = 0; s < S; s++)
+        {
+            DsmHeadingSample &Z = h.smp[s0 + s];
+            spline_sample(points + 3 * (size_t)offsets[j], N, samples, s, Z.p);
+            Z.pad = 0;
+            bool inside = true;
+            for (int k = 0; k < 3; k++)
+            {
+                const double q = std::floor(Z.p[k] / v) - (double)f->g.o[k];
+                inside = inside && q >= 0.0 && q < (double)f->g.n[k];
+            }
+            int lo[3] = {INT32_MAX, INT32_MAX, INT32_MAX}, hi[3] = {-1, -1, -1}; // the hull, exclusive of hi
+            for (int r = 0; inside && r < n_rot; r++)
+            {
+                DsmGainView V;
+                for (int a = 0; a < 3; a++)
+                {
+                    for (int b = 0; b < 3; b++) V.P[4 * a + b] = rotations[9 * r + 3 * a + b];
+                    V.P[4 * a + 3] = Z.p[a];
+                }
+                gain_box(V.P, c, f->g, V);
+                if (V.size[0] == 0 || V.size[1] == 0 || V.size[2] == 0) continue;
+                for (int k = 0; k < 3; k++) lo[k] = std::min(lo[k], V.lo[k]), hi[k] = std::max(hi[k], V.lo[k] + V.size[k]);
+            }
+            T.n_outside += !inside;
+            for (int k = 0; k < 3; k++)
+            {
+                Z.lo[k] = hi[k] < 0 ? 0 : lo[k];
+                Z.size[k] = hi[k] < 0 ? 0 : hi[k] - lo[k];
+            }
+            Z.brick0 = (int)bricks; // below 2^31: the work bound caps the bricks far lower
+            bricks += dsm_gain_bricks(Z.size);
+        }
+        s0 += S;
+    }
+    CK(cudaSetDevice(ctx->device));
+    const cudaStream_t st = ctx->stream;
+    const int n = n_trajectories;
+    CK(cudaMemcpyAsync(hd->stage_dev, hd->stage_host, head_stage_bytes(n, s0), cudaMemcpyHostToDevice, st));
+    CK(cudaMemsetAsync(hd->res, 0, head_res_bytes(n, s0, n_rot), st));
+    const HeadStage d = head_stage(hd->stage_dev, n);
+    const HeadResult r = head_result(hd->res, n, s0);
+    const double R = (double)c.max_range;
     if (bricks > 0)
-        k_heading_views<<<(unsigned)bricks, HEAD_BLOCK, 0, st>>>(g, state, smp, n_samples, rot, n_rot, cam.fx, cam.fy, cam.cx, cam.cy,
-                                                                 (double)cam.width, (double)cam.height, R * R, cam.unknown_blocks, counts);
+        k_heading_views<<<(unsigned)bricks, HEAD_BLOCK, 0, st>>>(f->g, f->occ, d.smp, s0, d.rot, n_rot, c.fx, c.fy, c.cx, c.cy, (double)c.width,
+                                                                 (double)c.height, R * R, c.unknown_blocks, r.counts);
     k_heading_plan<<<(unsigned)((n + HEAD_PLAN_WARPS - 1) / HEAD_PLAN_WARPS), HEAD_PLAN_WARPS * 32, 0, st>>>(
-        g, dist + dsm_field_header(voxels), traj, n, smp, n_samples, n_rot, cam.unknown_blocks, w_unknown, w_frontier, counts, succ, hdr,
-        rec, out);
-    return cudaGetLastError();
+        f->g, f->dist + dsm_field_header(f->voxels), d.traj, n, d.smp, s0, n_rot, c.unknown_blocks, w_unknown, w_frontier, r.counts, hd->succ,
+        r.hdr, r.rec, r.out);
+    CK(cudaGetLastError());
+    hd->n = n, hd->n_samples = s0, hd->n_rot = n_rot;
+    return submit(ctx, *hd, hd->res, head_res_bytes(n, s0, n_rot), f->requests);
+}
+
+extern "C" int dsm_heading_wait(dsm_ctx *ctx, dsm_heading_info_t *info, const dsm_heading_t **records, const dsm_heading_sample_t **samples,
+                                const dsm_heading_count_t **counts)
+{
+    if (!ctx) return DSM_E_INVALID;
+    DsmHeading *hd = ctx->heading.get();
+    const int rc = wait_head(ctx, hd);
+    if (rc != DSM_OK) return rc;
+    copy_info(info, hd->words());
+    const HeadResult r = head_result(hd->res_host, hd->n, hd->n_samples);
+    if (records) *records = r.rec;
+    if (samples) *samples = r.out;
+    if (counts) *counts = r.counts;
+    return capacity(ctx, hd->words(), DSM_HEAD_ERR_TAG, "dsm_heading_wait", "the field the job read");
 }

@@ -20,13 +20,35 @@
 //   k_reach_paths    one warp per reached target, lanes on the 26 neighbours and a shuffle argmin per step: a counting
 //                    walk, a cub exclusive scan of the lengths, then the writing walk.
 // The matrix job (dsm_reach_matrix_*, DESIGN.md §8.13) runs the same rounds from many sites at once; its kernels follow
-// dsm_launch_reach below and share reach_snap and reach_relax with k_reach_start and k_reach_round.
+// the reach job's C ABI calls (dsm_reach_enable, _enqueue and _wait) below, share reach_snap and reach_relax with
+// k_reach_start and k_reach_round, and are followed by its own (dsm_reach_matrix_enable, _enqueue and _wait).
 // The kernels carry no error gate and are launched without PDL, as the other field kernels.
-#include "dsm_device.cuh"
-#include <algorithm>
+#include "dsm_ctx.hpp"
 #include <cub/block/block_scan.cuh>
 #include <cub/device/device_scan.cuh>
 
+// One packed result (D2H):
+//   int32 header[DSM_REACH_WORDS] | dsm_reach_target_t targets[max_targets] | int32 path[max_path_voxels]
+// The header's first 14 words are those of dsm_reach_info_t; the last two carry the field's error words.
+enum
+{
+    DSM_REACH_ORIGIN = 0, // 3 words
+    DSM_REACH_START_VOXEL = 3,
+    DSM_REACH_START_STATUS,
+    DSM_REACH_START_APPROACH,
+    DSM_REACH_ROUNDS,
+    DSM_REACH_CONVERGED,
+    DSM_REACH_N_TRAVERSABLE,
+    DSM_REACH_N_REACHED,
+    DSM_REACH_N_GOALS,
+    DSM_REACH_N_CLUSTERS_TOTAL,
+    DSM_REACH_N_TARGETS,
+    DSM_REACH_N_PATH_VOXELS,
+    DSM_REACH_ERR_TAG, // the field header's DSM_FIELD_ERR_TAG / _ERR_FRAME, copied by k_reach_start
+    DSM_REACH_ERR_FRAME,
+    DSM_REACH_WORDS = 16 // 64 B
+};
+#define DSM_REACH_TILE 8 // tiles of 8 x 8 x 8 voxels, one CTA of 512 threads each
 #define RC_BLOCK 256
 #define RC_T DSM_REACH_TILE
 #define RC_TILE (RC_T * RC_T * RC_T) // 512 threads
@@ -404,7 +426,8 @@ __global__ void __launch_bounds__(RC_BLOCK) k_reach_paths(const DsmFieldGrid g, 
 
 static unsigned rc_blocks(long long n) { return n > 0 ? (unsigned)((n + RC_BLOCK - 1) / RC_BLOCK) : 1u; }
 
-int dsm_reach_ctas()
+// the persistent CTAs of k_reach_round on this device
+static int reach_ctas()
 {
     int dev = 0, sms = 0, per = 0;
     if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess ||
@@ -413,33 +436,108 @@ int dsm_reach_ctas()
     return sms * per;
 }
 
-size_t dsm_reach_temp_bytes(const DsmReachBufs &b)
+// the CUB scratch of the path-length scan; 0 on a CUB error
+static size_t reach_temp_bytes(const DsmReach &b)
 {
     size_t n = 0;
     if (cub::DeviceScan::ExclusiveSum(nullptr, n, b.len, b.ofs, std::max(b.max_targets, 1), (cudaStream_t)0) != cudaSuccess) return 0;
     return std::max(n, (size_t)1);
 }
 
-cudaError_t dsm_launch_reach(const DsmReachBufs &b, const DsmFieldGrid &g, const uint8_t *state, const int32_t *dist,
-                             const int3 s, float radius, int approach, int n_goals, const uint8_t *frontier_res, int frontier_max_clusters,
-                             cudaStream_t st)
+// byte offsets of the result's path list and its end
+static size_t reach_path_at(const DsmReach &b) { return 4 * (size_t)DSM_REACH_WORDS + sizeof(dsm_reach_target_t) * (size_t)b.max_targets; }
+static size_t reach_res_bytes(const DsmReach &b) { return reach_path_at(b) + 4 * (size_t)b.max_path; }
+
+extern "C" int dsm_reach_enable(dsm_ctx *ctx, int max_targets, int max_path_voxels, int max_rounds)
 {
+    if (!ctx) return DSM_E_INVALID;
+    const DsmField *f = ctx->field.get();
+    if (!f || !ctx->views || ctx->reach) return DSM_E_STATE;
+    for (int n : {max_targets, max_path_voxels})
+        if (n < 0 || n > DSM_REACH_MAX_CAPACITY) return DSM_E_INVALID;
+    if (max_rounds < 1 || max_rounds > DSM_REACH_MAX_ROUNDS || f->voxels > (size_t)DSM_REACH_MAX_VOXELS) return DSM_E_INVALID;
+    CK(cudaSetDevice(ctx->device));
+    auto re = std::make_unique<DsmReach>();
+    DsmReach &b = *re;
+    b.voxels = (int)f->voxels;
+    for (int k = 0; k < 3; k++) b.tn[k] = (f->g.n[k] + DSM_REACH_TILE - 1) / DSM_REACH_TILE;
+    b.tiles = b.tn[0] * b.tn[1] * b.tn[2];
+    b.max_targets = max_targets, b.max_path = max_path_voxels, b.max_rounds = max_rounds;
+    b.ctas = reach_ctas();
+    const size_t tg = (size_t)std::max(max_targets, 1);
+    const size_t res = reach_res_bytes(b);
+    CudaOwner &o = re->own;
+    o.device(&b.trav, f->voxels);
+    for (uint32_t **p : {&b.cost[0], &b.cost[1]}) o.device(p, f->voxels);
+    for (int32_t **p : {&b.stamp, &b.sched[0], &b.sched[1]}) o.device(p, (size_t)b.tiles);
+    o.device(&b.count, 3);
+    o.device(&b.goals, 3 * tg);
+    o.device(&b.best, tg);
+    o.device(&b.member, tg);
+    o.device(&b.len, tg);
+    o.device(&b.ofs, tg);
+    o.device(&b.res, res);
+    o.host(&re->goals_host, 3 * tg);
+    o.host(&re->res_host, res);
+    o.host(&re->cost_host, f->voxels);
+    o.event(&re->ev);
+    b.temp_bytes = reach_temp_bytes(b);
+    if (b.temp_bytes) o.device(reinterpret_cast<uint8_t **>(&b.temp), b.temp_bytes);
+    return keep(ctx->reach, re, b.ctas > 0 && b.temp_bytes != 0);
+}
+
+// floor(p / (double)v) - o, clamped to [-1, n]: outside the grid stays outside
+static int reach_voxel(double p, float v, int o, int n)
+{
+    const double q = std::floor(p / (double)v) - (double)o;
+    return q < 0.0 ? -1 : q >= (double)n ? n : (int)q;
+}
+
+// Enqueue only: the goal voxels staged and copied, the job on the grids of the latest (known) field request and, with
+// frontiers, on the latest frontier job's device result, one D2H copy of the result capacity (and of the cost grid with
+// host_copy) and the event.  Later field and frontier requests overwrite those buffers only behind the job.
+extern "C" int dsm_reach_enqueue(dsm_ctx *ctx, const double start[3], float radius, int approach, const double *goals, int n_goals,
+                                 int with_frontiers, int host_copy)
+{
+    if (!ctx) return DSM_E_INVALID;
+    DsmReach *re = ctx->reach.get();
+    const DsmField *f = known_field(ctx);
+    if (!re || !f || re->in_flight) return DSM_E_STATE;
+    const DsmFrontier *fr = ctx->frontier.get();
+    if (with_frontiers && !read_latest(fr, f)) return DSM_E_STATE;
+    DsmReach &b = *re;
+    if (!start || !std::isfinite(radius) || !(radius >= 0.f) || approach < 0 || approach > DSM_REACH_MAX_APPROACH || n_goals < 0 ||
+        n_goals > b.max_targets || (n_goals > 0 && !goals))
+        return DSM_E_INVALID;
+    for (int k = 0; k < 3; k++)
+        if (!std::isfinite(start[k])) return DSM_E_INVALID;
+    for (size_t i = 0; i < 3 * (size_t)n_goals; i++)
+        if (!std::isfinite(goals[i])) return DSM_E_INVALID;
+    const DsmFieldGrid &g = f->g;
+    const cudaStream_t st = ctx->stream;
+    CK(cudaSetDevice(ctx->device));
+    // the previous job's copy out of this staging ended before its wait, which no job in flight implies
+    for (size_t i = 0; i < 3 * (size_t)n_goals; i++) re->goals_host[i] = reach_voxel(goals[i], g.voxel, g.o[i % 3], g.n[i % 3]);
+    if (n_goals > 0) CK(cudaMemcpyAsync(b.goals, re->goals_host, 12 * (size_t)n_goals, cudaMemcpyHostToDevice, st));
+    const int3 s = make_int3(reach_voxel(start[0], g.voxel, g.o[0], g.n[0]), reach_voxel(start[1], g.voxel, g.o[1], g.n[1]),
+                             reach_voxel(start[2], g.voxel, g.o[2], g.n[2]));
+    CK(cudaMemsetAsync(b.res, 0, 4 * DSM_REACH_WORDS, st));
     int32_t *hdr = reinterpret_cast<int32_t *>(b.res);
     auto *rec = reinterpret_cast<dsm_reach_target_t *>(b.res + 4 * DSM_REACH_WORDS);
-    int32_t *path = reinterpret_cast<int32_t *>(b.res + 4 * DSM_REACH_WORDS + sizeof(dsm_reach_target_t) * (size_t)b.max_targets);
-    const int32_t *fhdr = reinterpret_cast<const int32_t *>(frontier_res);
-    const auto *table = frontier_res ? reinterpret_cast<const dsm_frontier_cluster_t *>(frontier_res + 4 * DSM_FRONTIER_WORDS) : nullptr;
-    const int32_t *list = frontier_res ? reinterpret_cast<const int32_t *>(frontier_res + 4 * DSM_FRONTIER_WORDS +
-                                                                         sizeof(dsm_frontier_cluster_t) * (size_t)frontier_max_clusters)
-                                       : nullptr;
+    int32_t *path = reinterpret_cast<int32_t *>(b.res + reach_path_at(b));
+    // the frontier job's result, with frontiers
+    const int32_t *fhdr = with_frontiers ? reinterpret_cast<const int32_t *>(fr->res) : nullptr;
+    const auto *table = with_frontiers ? reinterpret_cast<const dsm_frontier_cluster_t *>(fr->res + DsmFrontier::table_at()) : nullptr;
+    const int32_t *list = with_frontiers ? reinterpret_cast<const int32_t *>(fr->res + fr->list_at()) : nullptr;
+    const int frontier_max_clusters = with_frontiers ? fr->max_clusters : 0;
+    const uint8_t *state = f->occ;
+    const int32_t *dist = f->dist;
     const int3 tn = make_int3(b.tn[0], b.tn[1], b.tn[2]);
-    const int32_t *fieldhdr = dist + dsm_field_header((size_t)b.voxels);
-    cudaError_t e = cudaMemsetAsync(b.stamp, 0xff, 4 * (size_t)b.tiles, st);
-    if (e == cudaSuccess && b.max_targets > 0) e = cudaMemsetAsync(b.best, 0xff, 8 * (size_t)b.max_targets, st);
-    if (e == cudaSuccess && b.max_targets > 0) e = cudaMemsetAsync(b.member, 0x7f, 4 * (size_t)b.max_targets, st);
-    if (e != cudaSuccess) return e;
-    k_reach_start<<<1, 32, 0, st>>>(g, state, dist, fieldhdr, s, radius, approach, n_goals, b.max_targets, fhdr, frontier_max_clusters, tn,
-                                    b.sched[0], b.stamp, b.count, hdr);
+    CK(cudaMemsetAsync(b.stamp, 0xff, 4 * (size_t)b.tiles, st));
+    if (b.max_targets > 0) CK(cudaMemsetAsync(b.best, 0xff, 8 * (size_t)b.max_targets, st));
+    if (b.max_targets > 0) CK(cudaMemsetAsync(b.member, 0x7f, 4 * (size_t)b.max_targets, st));
+    k_reach_start<<<1, 32, 0, st>>>(g, state, dist, dist + dsm_field_header(f->voxels), s, radius, approach, n_goals, b.max_targets, fhdr,
+                                    frontier_max_clusters, tn, b.sched[0], b.stamp, b.count, hdr);
     k_reach_init<<<rc_blocks(b.voxels), RC_BLOCK, 0, st>>>(state, dist, b.voxels, radius, b.trav, b.cost[0], b.cost[1], hdr);
     for (int r = 0; r < b.max_rounds; r++)
         k_reach_round<<<b.ctas, RC_TILE, 0, st>>>(g, tn, b.trav, b.cost[r % 2], b.cost[(r + 1) % 2], b.sched[r % 2], b.sched[(r + 1) % 2],
@@ -447,20 +545,38 @@ cudaError_t dsm_launch_reach(const DsmReachBufs &b, const DsmFieldGrid &g, const
     const int r = b.max_rounds;
     k_reach_settle<<<b.ctas, RC_TILE, 0, st>>>(g, tn, b.cost[r % 2], b.cost[(r + 1) % 2], b.sched[r % 2], b.count, r);
     k_reach_reached<<<rc_blocks(b.voxels), RC_BLOCK, 0, st>>>(b.cost[0], b.voxels, b.count, r, hdr);
-    e = cudaGetLastError();
-    if (e != cudaSuccess || b.max_targets == 0) return e;
-    const unsigned warp_blocks = 2 * (unsigned)b.ctas; // the target and path kernels' warps walk their work
-    k_reach_targets<0><<<warp_blocks, RC_BLOCK, 0, st>>>(g, b.trav, b.cost[0], b.goals, fhdr, table, list, approach, hdr, b.best, b.member);
-    if (frontier_res)
-        k_reach_targets<1><<<warp_blocks, RC_BLOCK, 0, st>>>(g, b.trav, b.cost[0], b.goals, fhdr, table, list, approach, hdr, b.best, b.member);
-    k_reach_records<<<rc_blocks(b.max_targets), RC_BLOCK, 0, st>>>(g, b.cost[0], b.goals, table, b.best, b.member, hdr, rec);
-    k_reach_paths<false><<<warp_blocks, RC_BLOCK, 0, st>>>(g, b.trav, b.cost[0], b.max_targets, b.max_path, b.len, b.ofs, rec, path, hdr);
-    e = cudaGetLastError();
-    size_t n = b.temp_bytes;
-    if (e == cudaSuccess) e = cub::DeviceScan::ExclusiveSum(b.temp, n, b.len, b.ofs, b.max_targets, st);
-    if (e != cudaSuccess) return e;
-    k_reach_paths<true><<<warp_blocks, RC_BLOCK, 0, st>>>(g, b.trav, b.cost[0], b.max_targets, b.max_path, b.len, b.ofs, rec, path, hdr);
-    return cudaGetLastError();
+    CK(cudaGetLastError());
+    if (b.max_targets > 0)
+    {
+        const unsigned warp_blocks = 2 * (unsigned)b.ctas; // the target and path kernels' warps walk their work
+        k_reach_targets<0><<<warp_blocks, RC_BLOCK, 0, st>>>(g, b.trav, b.cost[0], b.goals, fhdr, table, list, approach, hdr, b.best, b.member);
+        if (with_frontiers)
+            k_reach_targets<1><<<warp_blocks, RC_BLOCK, 0, st>>>(g, b.trav, b.cost[0], b.goals, fhdr, table, list, approach, hdr, b.best, b.member);
+        k_reach_records<<<rc_blocks(b.max_targets), RC_BLOCK, 0, st>>>(g, b.cost[0], b.goals, table, b.best, b.member, hdr, rec);
+        k_reach_paths<false><<<warp_blocks, RC_BLOCK, 0, st>>>(g, b.trav, b.cost[0], b.max_targets, b.max_path, b.len, b.ofs, rec, path, hdr);
+        CK(cudaGetLastError());
+        size_t n = b.temp_bytes;
+        CK(cub::DeviceScan::ExclusiveSum(b.temp, n, b.len, b.ofs, b.max_targets, st));
+        k_reach_paths<true><<<warp_blocks, RC_BLOCK, 0, st>>>(g, b.trav, b.cost[0], b.max_targets, b.max_path, b.len, b.ofs, rec, path, hdr);
+        CK(cudaGetLastError());
+    }
+    if (host_copy) CK(cudaMemcpyAsync(re->cost_host, b.cost[0], 4 * (size_t)b.voxels, cudaMemcpyDeviceToHost, st));
+    re->host_copy = host_copy != 0;
+    return submit(ctx, *re, b.res, reach_res_bytes(b), f->requests);
+}
+
+extern "C" int dsm_reach_wait(dsm_ctx *ctx, dsm_reach_info_t *info, const dsm_reach_target_t **targets, const int32_t **path,
+                              const uint32_t **cost)
+{
+    if (!ctx) return DSM_E_INVALID;
+    DsmReach *re = ctx->reach.get();
+    const int rc = wait_head(ctx, re);
+    if (rc != DSM_OK) return rc;
+    copy_info(info, re->words());
+    if (targets) *targets = reinterpret_cast<const dsm_reach_target_t *>(re->res_host + 4 * DSM_REACH_WORDS);
+    if (path) *path = reinterpret_cast<const int32_t *>(re->res_host + reach_path_at(*re));
+    if (cost) *cost = re->host_copy ? re->cost_host : nullptr;
+    return capacity(ctx, re->words(), DSM_REACH_ERR_TAG, "dsm_reach_wait", "the field the job read");
 }
 
 // ---- the matrix job (dsm_reach_matrix_*, DESIGN.md §8.13): the reach job's rounds from many sites at once, on the
@@ -478,6 +594,24 @@ cudaError_t dsm_launch_reach(const DsmReachBufs &b, const DsmFieldGrid &g, const
 //   k_rm_gather   one thread per matrix entry; thread (i, 0) finishes site i's record.
 // No settle step: every tile a round leaves out holds equal buffers (a tile that changed schedules itself), so buffer
 // max_rounds % 2 holds the latest cost of every voxel, and the last two kernels read it.
+//
+// One packed result of a job on n sites (D2H, 64 + 32 n + 4 n^2 B):
+//   int32 header[DSM_RM_WORDS] | dsm_reach_site_t sites[n] | uint32 matrix[n][n]
+// The header's first nine words are those of dsm_reach_matrix_info_t; its last two carry the field's error words,
+// cleared by dsm_reach_matrix_wait.
+enum
+{
+    DSM_RM_ORIGIN = 0, // 3 words
+    DSM_RM_N_SITES = 3,
+    DSM_RM_STATUS,
+    DSM_RM_N_TRAVERSABLE,
+    DSM_RM_N_ACTIVE_TILES,
+    DSM_RM_MAX_TILES,
+    DSM_RM_ROUNDS,
+    DSM_RM_ERR_TAG = 14, // the field header's DSM_FIELD_ERR_TAG / _ERR_FRAME, copied by k_rm_slots
+    DSM_RM_ERR_FRAME,
+    DSM_RM_WORDS = 16 // 64 B
+};
 #define RM_SITES DSM_REACH_MATRIX_MAX_SITES
 #define RM_WORDS (RC_TILE / 32) // mask words per tile
 static_assert(sizeof(dsm_reach_site_t) == 32 && sizeof(dsm_reach_matrix_info_t) == 64, "dsm_reach_matrix layouts");
@@ -701,7 +835,8 @@ __global__ void __launch_bounds__(RC_BLOCK) k_rm_gather(const DsmFieldGrid g, co
     }
 }
 
-int dsm_reach_matrix_ctas()
+// the persistent CTAs of k_rm_round on this device
+static int rm_ctas()
 {
     int dev = 0, sms = 0, per = 0;
     if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess ||
@@ -710,31 +845,95 @@ int dsm_reach_matrix_ctas()
     return sms * per;
 }
 
-size_t dsm_reach_matrix_temp_bytes(const DsmReachMatrixBufs &b)
+// the CUB scratch of the tile scan; 0 on a CUB error
+static size_t rm_temp_bytes(const DsmReachMatrix &b)
 {
     size_t n = 0;
     if (cub::DeviceScan::ExclusiveSum(nullptr, n, b.flag, b.scan, b.tiles, (cudaStream_t)0) != cudaSuccess) return 0;
     return std::max(n, (size_t)1);
 }
 
-cudaError_t dsm_launch_reach_matrix(const DsmReachMatrixBufs &b, const DsmFieldGrid &g, const uint8_t *state, const int32_t *dist,
-                                    int n, float radius, int approach, cudaStream_t st)
+// byte offsets of an n-site result's matrix and its end
+static size_t rm_matrix_at(int n) { return 4 * (size_t)DSM_RM_WORDS + sizeof(dsm_reach_site_t) * (size_t)n; }
+static size_t rm_res_bytes(int n) { return rm_matrix_at(n) + 4 * (size_t)n * n; }
+
+extern "C" int dsm_reach_matrix_enable(dsm_ctx *ctx, int max_sites, int max_tiles, int max_rounds)
 {
+    if (!ctx) return DSM_E_INVALID;
+    const DsmField *f = ctx->field.get();
+    if (!f || !ctx->views || ctx->reach_matrix) return DSM_E_STATE;
+    int tn[3];
+    for (int k = 0; k < 3; k++) tn[k] = (f->g.n[k] + DSM_REACH_TILE - 1) / DSM_REACH_TILE;
+    const long long tiles = (long long)tn[0] * tn[1] * tn[2];
+    if (max_sites < 1 || max_sites > DSM_REACH_MATRIX_MAX_SITES || max_tiles < 1 || max_tiles > tiles || max_rounds < 1 ||
+        max_rounds > DSM_REACH_MAX_ROUNDS || f->voxels > (size_t)DSM_REACH_MAX_VOXELS ||
+        4096ull * (unsigned long long)max_sites * (unsigned long long)max_tiles > DSM_REACH_MATRIX_MAX_COST_BYTES)
+        return DSM_E_INVALID;
+    CK(cudaSetDevice(ctx->device));
+    auto rm = std::make_unique<DsmReachMatrix>();
+    DsmReachMatrix &b = *rm;
+    b.voxels = (int)f->voxels;
+    for (int k = 0; k < 3; k++) b.tn[k] = tn[k];
+    b.tiles = (int)tiles;
+    b.max_sites = max_sites, b.max_tiles = max_tiles, b.max_rounds = max_rounds;
+    b.ctas = rm_ctas();
+    const size_t items = (size_t)max_sites * max_tiles, res = rm_res_bytes(max_sites);
+    CudaOwner &o = rm->own;
+    for (int32_t **p : {&b.flag, &b.scan, &b.slot}) o.device(p, (size_t)b.tiles);
+    o.device(&b.mask, 16 * (size_t)b.tiles);
+    o.device(&b.tile_of, (size_t)max_tiles);
+    for (uint32_t **p : {&b.cost[0], &b.cost[1]}) o.device(p, items * 512);
+    for (int32_t **p : {&b.stamp, &b.sched[0], &b.sched[1]}) o.device(p, items);
+    o.device(&b.count, 3 * (size_t)max_sites);
+    for (int32_t **p : {&b.rounds, &b.reached}) o.device(p, (size_t)max_sites);
+    o.device(&b.sites, 3 * (size_t)max_sites);
+    o.device(&b.res, res);
+    o.host(&rm->sites_host, 3 * (size_t)max_sites);
+    o.host(&rm->res_host, res);
+    o.event(&rm->ev);
+    b.temp_bytes = rm_temp_bytes(b);
+    if (b.temp_bytes) o.device(reinterpret_cast<uint8_t **>(&b.temp), b.temp_bytes);
+    return keep(ctx->reach_matrix, rm, b.ctas > 0 && b.temp_bytes != 0);
+}
+
+// Enqueue only: the points' voxels staged and copied, the job on the grids of the latest (known) field request, one D2H
+// copy of the n-site result and the event.  A later field request overwrites those grids only behind the job.
+extern "C" int dsm_reach_matrix_enqueue(dsm_ctx *ctx, const double *points, int n_points, float radius, int approach)
+{
+    if (!ctx) return DSM_E_INVALID;
+    DsmReachMatrix *rm = ctx->reach_matrix.get();
+    const DsmField *f = known_field(ctx);
+    if (!rm || !f || rm->in_flight) return DSM_E_STATE;
+    DsmReachMatrix &b = *rm;
+    if (!points || !std::isfinite(radius) || !(radius >= 0.f) || approach < 0 || approach > DSM_REACH_MAX_APPROACH || n_points < 1 ||
+        n_points > b.max_sites ||
+        (unsigned long long)n_points * (unsigned long long)b.max_tiles * (unsigned long long)b.max_rounds > DSM_REACH_MATRIX_MAX_WORK)
+        return DSM_E_INVALID;
+    for (size_t i = 0; i < 3 * (size_t)n_points; i++)
+        if (!std::isfinite(points[i])) return DSM_E_INVALID;
+    const DsmFieldGrid &g = f->g;
+    const cudaStream_t st = ctx->stream;
+    const int n = n_points;
+    CK(cudaSetDevice(ctx->device));
+    // the previous job's copy out of this staging ended before its wait, which no job in flight implies
+    for (size_t i = 0; i < 3 * (size_t)n; i++) rm->sites_host[i] = reach_voxel(points[i], g.voxel, g.o[i % 3], g.n[i % 3]);
+    CK(cudaMemcpyAsync(b.sites, rm->sites_host, 12 * (size_t)n, cudaMemcpyHostToDevice, st));
+    CK(cudaMemsetAsync(b.res, 0, 4 * DSM_RM_WORDS, st));
     int32_t *hdr = reinterpret_cast<int32_t *>(b.res);
     auto *rec = reinterpret_cast<dsm_reach_site_t *>(b.res + 4 * DSM_RM_WORDS);
-    auto *matrix = reinterpret_cast<uint32_t *>(b.res + 4 * DSM_RM_WORDS + sizeof(dsm_reach_site_t) * (size_t)n);
+    auto *matrix = reinterpret_cast<uint32_t *>(b.res + rm_matrix_at(n));
+    const uint8_t *state = f->occ;
+    const int32_t *dist = f->dist;
     const int3 tn = make_int3(b.tn[0], b.tn[1], b.tn[2]);
-    const int32_t *fieldhdr = dist + dsm_field_header((size_t)b.voxels);
-    cudaError_t e = cudaMemsetAsync(b.stamp, 0xff, 4 * (size_t)n * b.max_tiles, st);
-    if (e == cudaSuccess) e = cudaMemsetAsync(b.rounds, 0, 4 * (size_t)n, st);
-    if (e == cudaSuccess) e = cudaMemsetAsync(b.reached, 0, 4 * (size_t)n, st);
-    if (e != cudaSuccess) return e;
+    CK(cudaMemsetAsync(b.stamp, 0xff, 4 * (size_t)n * b.max_tiles, st));
+    CK(cudaMemsetAsync(b.rounds, 0, 4 * (size_t)n, st));
+    CK(cudaMemsetAsync(b.reached, 0, 4 * (size_t)n, st));
     k_rm_tiles<<<b.tiles, RC_TILE, 0, st>>>(g, tn, state, dist, radius, b.flag, b.mask, hdr);
-    e = cudaGetLastError();
+    CK(cudaGetLastError());
     size_t tb = b.temp_bytes;
-    if (e == cudaSuccess) e = cub::DeviceScan::ExclusiveSum(b.temp, tb, b.flag, b.scan, b.tiles, st);
-    if (e != cudaSuccess) return e;
-    k_rm_slots<<<rc_blocks(b.tiles), RC_BLOCK, 0, st>>>(g, b.tiles, b.max_tiles, n, b.flag, b.scan, fieldhdr, b.slot, b.tile_of, hdr);
+    CK(cub::DeviceScan::ExclusiveSum(b.temp, tb, b.flag, b.scan, b.tiles, st));
+    k_rm_slots<<<rc_blocks(b.tiles), RC_BLOCK, 0, st>>>(g, b.tiles, b.max_tiles, n, b.flag, b.scan, dist + dsm_field_header(f->voxels), b.slot,
+                                                        b.tile_of, hdr);
     k_rm_sites<<<rc_blocks(32ll * n), RC_BLOCK, 0, st>>>(g, tn, state, dist, b.sites, n, radius, approach, b.max_tiles, b.slot, b.sched[0],
                                                          b.stamp, b.count, hdr, rec);
     k_rm_init<<<b.ctas, RC_TILE, 0, st>>>(g, tn, n, b.max_tiles, b.slot, rec, hdr, b.cost[0], b.cost[1]);
@@ -745,5 +944,19 @@ cudaError_t dsm_launch_reach_matrix(const DsmReachMatrixBufs &b, const DsmFieldG
     k_rm_reached<<<b.ctas, RC_TILE, 0, st>>>(n, b.max_tiles, last, hdr, b.reached);
     k_rm_gather<<<rc_blocks((long long)n * n), RC_BLOCK, 0, st>>>(g, tn, n, b.max_tiles, b.max_rounds, b.slot, last, b.count, b.rounds,
                                                                   b.reached, hdr, rec, matrix);
-    return cudaGetLastError();
+    CK(cudaGetLastError());
+    rm->n_sites = n;
+    return submit(ctx, *rm, b.res, rm_res_bytes(n), f->requests);
+}
+
+extern "C" int dsm_reach_matrix_wait(dsm_ctx *ctx, dsm_reach_matrix_info_t *info, const dsm_reach_site_t **sites, const uint32_t **matrix)
+{
+    if (!ctx) return DSM_E_INVALID;
+    DsmReachMatrix *rm = ctx->reach_matrix.get();
+    const int rc = wait_head(ctx, rm);
+    if (rc != DSM_OK) return rc;
+    copy_info(info, rm->words());
+    if (sites) *sites = reinterpret_cast<const dsm_reach_site_t *>(rm->res_host + 4 * DSM_RM_WORDS);
+    if (matrix) *matrix = reinterpret_cast<const uint32_t *>(rm->res_host + rm_matrix_at(rm->n_sites));
+    return capacity(ctx, rm->words(), DSM_RM_ERR_TAG, "dsm_reach_matrix_wait", "the field the job read");
 }

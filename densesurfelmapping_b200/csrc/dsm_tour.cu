@@ -10,8 +10,10 @@
 //                  applies it through the second tour buffer.  The start's tour and record go to global memory.
 //   k_tour_best    one CTA: the least (cost, start), the best tour's order and legs priced P, and the header.
 // The matrix is read through the read-only path: at 4 n^2 bytes (4 MB at n = 1024) it stays in L2.  The kernels carry
-// no error gate and are launched without PDL, as the field jobs' kernels.
-#include "dsm_device.cuh"
+// no error gate and are launched without PDL, as the field jobs' kernels.  The job's C ABI calls (dsm_tour_enable,
+// _enqueue and _wait) follow them; its packed result (D2H) is
+//   dsm_tour_info_t | dsm_tour_start_t starts[n_starts] | int32 order[n]
+#include "dsm_ctx.hpp"
 #include <climits>
 #include <cub/block/block_scan.cuh>
 
@@ -246,10 +248,60 @@ __global__ void __launch_bounds__(TOUR_BLOCK) k_tour_best(const uint32_t *__rest
     }
 }
 
-cudaError_t dsm_launch_tour(const uint32_t *matrix, int n, int open, int n_starts, int max_passes, uint64_t seed, int32_t *tours,
-                            uint8_t *res, cudaStream_t st)
+// byte offsets of the result's order and its end
+static size_t tour_order_at(int n_starts) { return sizeof(dsm_tour_info_t) + sizeof(dsm_tour_start_t) * (size_t)n_starts; }
+static size_t tour_res_bytes(int n_starts, int n) { return tour_order_at(n_starts) + 4 * (size_t)n; }
+
+extern "C" int dsm_tour_enable(dsm_ctx *ctx, int max_sites, int max_starts)
 {
-    k_tour_search<<<n_starts, TOUR_BLOCK, 0, st>>>(matrix, n, open, max_passes, seed, tours, reinterpret_cast<dsm_tour_start_t *>(res + 64));
-    k_tour_best<<<1, TOUR_BLOCK, 0, st>>>(matrix, n, open, n_starts, max_passes, seed, tours, res);
-    return cudaGetLastError();
+    if (!ctx) return DSM_E_INVALID;
+    if (ctx->tour) return DSM_E_STATE;
+    if (max_sites < 1 || max_sites > DSM_TOUR_MAX_SITES || max_starts < 1 || max_starts > DSM_TOUR_MAX_STARTS) return DSM_E_INVALID;
+    CK(cudaSetDevice(ctx->device));
+    auto tr = std::make_unique<DsmTour>();
+    tr->max_sites = max_sites, tr->max_starts = max_starts;
+    const size_t entries = (size_t)max_sites * max_sites, res = tour_res_bytes(max_starts, max_sites);
+    CudaOwner &o = tr->own;
+    o.host(&tr->matrix_host, entries);
+    o.device(&tr->matrix, entries);
+    o.device(&tr->tours, (size_t)max_starts * max_sites);
+    o.device(&tr->res, res);
+    o.host(&tr->res_host, res);
+    o.event(&tr->ev);
+    return keep(ctx->tour, tr);
+}
+
+// Enqueue only: the matrix staged and copied, the kernels, one D2H copy of the used result and the event.
+extern "C" int dsm_tour_enqueue(dsm_ctx *ctx, const uint32_t *matrix, int n, int open, int n_starts, int max_passes, uint64_t seed)
+{
+    if (!ctx) return DSM_E_INVALID;
+    DsmTour *tr = ctx->tour.get();
+    if (!tr || tr->in_flight) return DSM_E_STATE;
+    if (!matrix || n < 1 || n > tr->max_sites || n_starts < 1 || n_starts > tr->max_starts || (open != 0 && open != 1) ||
+        max_passes < 0 || max_passes > DSM_TOUR_MAX_PASSES ||
+        (unsigned long long)n_starts * (unsigned long long)max_passes * (unsigned long long)n * (unsigned long long)n > DSM_TOUR_MAX_WORK)
+        return DSM_E_INVALID;
+    CK(cudaSetDevice(ctx->device));
+    // the previous job's copy out of this staging ended before its wait, which no job in flight implies
+    const size_t bytes = 4 * (size_t)n * n;
+    std::memcpy(tr->matrix_host, matrix, bytes);
+    CK(cudaMemcpyAsync(tr->matrix, tr->matrix_host, bytes, cudaMemcpyHostToDevice, ctx->stream));
+    k_tour_search<<<n_starts, TOUR_BLOCK, 0, ctx->stream>>>(tr->matrix, n, open, max_passes, seed, tr->tours,
+                                                            reinterpret_cast<dsm_tour_start_t *>(tr->res + sizeof(dsm_tour_info_t)));
+    k_tour_best<<<1, TOUR_BLOCK, 0, ctx->stream>>>(tr->matrix, n, open, n_starts, max_passes, seed, tr->tours, tr->res);
+    CK(cudaGetLastError());
+    tr->n = n, tr->n_starts = n_starts;
+    return submit(ctx, *tr, tr->res, tour_res_bytes(n_starts, n), 0);
+}
+
+extern "C" int dsm_tour_wait(dsm_ctx *ctx, dsm_tour_info_t *info, const dsm_tour_start_t **starts, const int32_t **order)
+{
+    if (!ctx) return DSM_E_INVALID;
+    DsmTour *tr = ctx->tour.get();
+    const int rc = wait_head(ctx, tr);
+    if (rc != DSM_OK) return rc;
+    if (info) std::memcpy(info, tr->res_host, sizeof(dsm_tour_info_t));
+    if (starts) *starts = reinterpret_cast<const dsm_tour_start_t *>(tr->res_host + sizeof(dsm_tour_info_t));
+    if (order) *order = reinterpret_cast<const int32_t *>(tr->res_host + tour_order_at(tr->n_starts));
+    return DSM_OK;
 }

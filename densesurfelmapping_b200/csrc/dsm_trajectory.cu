@@ -12,8 +12,27 @@
 //                 depend on the schedule.  Trajectories finish independently.
 // Every fp64 step is an explicit _rn intrinsic (the library is built with -fmad=false), so the numpy restatement
 // (oracle/pyoracle_trajectory.py) is bit-exact; the field samples are the fp32 signed point query of k_field_query<true>.
-#include "dsm_device.cuh"
+// The job's C ABI calls (dsm_trajectory_enable, _enqueue and _wait) follow the kernel.
+//
+// One staged request (H2D):
+//   double points[n_points][3] | double dt[n] | int32 offsets[n + 1]
+// and one packed result (D2H, 64 + 96 n + 24 n_points B):
+//   int32 header[DSM_TRAJ_WORDS] | dsm_trajectory_t records[n] | double points[n_points][3]
+// The header's first nine words are those of dsm_trajectory_info_t; its last two carry the signed grid's error words,
+// cleared by dsm_trajectory_wait.
+#include "dsm_ctx.hpp"
 #include <climits>
+
+enum
+{
+    DSM_TRAJ_ORIGIN = 0, // 3 words
+    DSM_TRAJ_N = 3,
+    DSM_TRAJ_N_POINTS,
+    DSM_TRAJ_N_STATUS,   // 4 words: trajectories per status (zeroed before the launch; k_trajectory adds)
+    DSM_TRAJ_ERR_TAG = 14, // the signed grid header's DSM_SIGNED_ERR_TAG / _ERR_FRAME, copied by k_trajectory
+    DSM_TRAJ_ERR_FRAME,
+    DSM_TRAJ_WORDS = 16 // 64 B
+};
 
 #define TRAJ_C1 1e-4
 // Every per-free-point array (g, gt, d and the history) is touched only by the lane that owns the free point: lane
@@ -350,12 +369,98 @@ __global__ void __launch_bounds__(32, 1) k_trajectory(const double *__restrict__
     }
 }
 
-cudaError_t dsm_launch_trajectory(const double *points, const double *dt, const int32_t *offsets, int n_traj, int nmax, const float *sdist,
-                                  const int32_t *field_header, const DsmFieldGrid &g, const dsm_trajectory_params_t &p, double *hist,
-                                  uint8_t *res, cudaStream_t st)
+// byte offsets of the staged request's dt and offsets and its end, and of the result's points and its end
+static size_t traj_stage_dt(int n_points) { return 24 * (size_t)n_points; }
+static size_t traj_stage_offsets(int n_points, int n) { return traj_stage_dt(n_points) + 8 * (size_t)n; }
+static size_t traj_stage_bytes(int n_points, int n) { return traj_stage_offsets(n_points, n) + 4 * ((size_t)n + 1); }
+static size_t traj_points_at(int n) { return 4 * (size_t)DSM_TRAJ_WORDS + sizeof(dsm_trajectory_t) * (size_t)n; }
+static size_t traj_res_bytes(int n_points, int n) { return traj_points_at(n) + 24 * (size_t)n_points; }
+
+extern "C" int dsm_trajectory_enable(dsm_ctx *ctx, int max_trajectories, int max_points, int max_memory)
 {
-    cudaError_t e = cudaMemsetAsync(res, 0, 4 * DSM_TRAJ_WORDS, st);
-    if (e != cudaSuccess) return e;
-    k_trajectory<<<n_traj, 32, dsm_trajectory_smem(nmax), st>>>(points, dt, offsets, n_traj, nmax, sdist, field_header, g, p, hist, res);
-    return cudaGetLastError();
+    if (!ctx) return DSM_E_INVALID;
+    const DsmField *f = ctx->field.get();
+    if (!f || !f->sgn || ctx->trajectory) return DSM_E_STATE;
+    if (max_trajectories < 1 || max_trajectories > DSM_TRAJECTORY_MAX_CAPACITY || max_points < 1 || max_points > DSM_TRAJECTORY_MAX_CAPACITY ||
+        max_memory < 1 || max_memory > DSM_TRAJECTORY_MAX_MEMORY)
+        return DSM_E_INVALID;
+    CK(cudaSetDevice(ctx->device));
+    auto tr = std::make_unique<DsmTrajectory>();
+    tr->max_traj = max_trajectories, tr->max_points = max_points, tr->max_memory = max_memory;
+    const size_t stage = traj_stage_bytes(max_points, max_trajectories), res = traj_res_bytes(max_points, max_trajectories);
+    CudaOwner &o = tr->own;
+    o.host(&tr->stage_host, stage);
+    o.device(&tr->stage_dev, stage);
+    o.device(&tr->hist, 6 * (size_t)max_memory * max_points);
+    o.device(&tr->res, res);
+    o.host(&tr->res_host, res);
+    o.event(&tr->ev);
+    return keep(ctx->trajectory, tr);
+}
+
+static bool traj_params_ok(const dsm_trajectory_params_t &p, int max_memory)
+{
+    for (double w : {p.w_smooth, p.w_clear, p.w_feas, p.margin, p.v_max, p.a_max, p.g_tol})
+        if (!std::isfinite(w) || !(w >= 0.0)) return false;
+    return p.max_iter >= 0 && p.max_iter <= DSM_TRAJECTORY_MAX_ITER && p.memory >= 1 && p.memory <= max_memory && p.max_ls >= 1 &&
+           p.max_ls <= DSM_TRAJECTORY_MAX_LS && p.samples >= 1 && p.samples <= DSM_TRAJECTORY_MAX_SAMPLES_PER_SEGMENT &&
+           std::isfinite(p.radius) && p.radius >= 0.f;
+}
+
+// Stages the request on the calling thread (checking it on the way), then enqueues one H2D copy, the kernel on the
+// signed grid of the latest field request, one D2H copy of the used result and the event.
+extern "C" int dsm_trajectory_enqueue(dsm_ctx *ctx, const double *points, const int32_t *offsets, const double *dt, int n_trajectories,
+                                      const dsm_trajectory_params_t *params)
+{
+    if (!ctx) return DSM_E_INVALID;
+    DsmTrajectory *tr = ctx->trajectory.get();
+    const DsmField *f = ctx->field.get();
+    if (!tr || !f || !f->requested || !f->signed_latest || tr->in_flight) return DSM_E_STATE;
+    if (!points || !offsets || !dt || !params || n_trajectories < 1 || n_trajectories > tr->max_traj) return DSM_E_INVALID;
+    const dsm_trajectory_params_t p = *params;
+    if (!traj_params_ok(p, tr->max_memory) || !spline_points_ok(points, offsets, n_trajectories, tr->max_points)) return DSM_E_INVALID;
+    int nmax = 0;
+    unsigned long long samples = 0;
+    for (int j = 0; j < n_trajectories; j++)
+    {
+        const int n = offsets[j + 1] - offsets[j];
+        if (!std::isfinite(dt[j]) || !(dt[j] > 0.0)) return DSM_E_INVALID;
+        nmax = std::max(nmax, n);
+        samples += (unsigned long long)(n - 3) * (unsigned long long)p.samples + 1;
+    }
+    const int n_points = offsets[n_trajectories];
+    if ((unsigned long long)n_points * (unsigned long long)p.max_iter * (unsigned long long)(p.max_ls + 1) > DSM_TRAJECTORY_MAX_WORK ||
+        samples > DSM_TRAJECTORY_MAX_SAMPLES)
+        return DSM_E_INVALID;
+    // the packed request; the previous job's copy out of this staging ended before its wait, which no job in flight
+    // implies
+    uint8_t *h = tr->stage_host;
+    std::memcpy(h, points, 24 * (size_t)n_points);
+    std::memcpy(h + traj_stage_dt(n_points), dt, 8 * (size_t)n_trajectories);
+    std::memcpy(h + traj_stage_offsets(n_points, n_trajectories), offsets, 4 * ((size_t)n_trajectories + 1));
+    CK(cudaSetDevice(ctx->device));
+    const cudaStream_t st = ctx->stream;
+    CK(cudaMemcpyAsync(tr->stage_dev, h, traj_stage_bytes(n_points, n_trajectories), cudaMemcpyHostToDevice, st));
+    const int32_t *grid = f->sgn->grid;
+    CK(cudaMemsetAsync(tr->res, 0, 4 * DSM_TRAJ_WORDS, st));
+    // k_trajectory's shared memory: x, xt, g, gt and d, nmax x 3 doubles each
+    k_trajectory<<<n_trajectories, 32, 5 * 3 * sizeof(double) * (size_t)nmax, st>>>(
+        reinterpret_cast<const double *>(tr->stage_dev), reinterpret_cast<const double *>(tr->stage_dev + traj_stage_dt(n_points)),
+        reinterpret_cast<const int32_t *>(tr->stage_dev + traj_stage_offsets(n_points, n_trajectories)), n_trajectories, nmax,
+        reinterpret_cast<const float *>(grid), grid + dsm_field_header(f->voxels), f->g, p, tr->hist, tr->res);
+    CK(cudaGetLastError());
+    tr->n = n_trajectories, tr->n_points = n_points;
+    return submit(ctx, *tr, tr->res, traj_res_bytes(n_points, n_trajectories), f->requests);
+}
+
+extern "C" int dsm_trajectory_wait(dsm_ctx *ctx, dsm_trajectory_info_t *info, const dsm_trajectory_t **records, const double **points)
+{
+    if (!ctx) return DSM_E_INVALID;
+    DsmTrajectory *tr = ctx->trajectory.get();
+    const int rc = wait_head(ctx, tr);
+    if (rc != DSM_OK) return rc;
+    copy_info(info, tr->words());
+    if (records) *records = reinterpret_cast<const dsm_trajectory_t *>(tr->res_host + 4 * DSM_TRAJ_WORDS);
+    if (points) *points = reinterpret_cast<const double *>(tr->res_host + traj_points_at(tr->n));
+    return capacity(ctx, tr->words(), DSM_TRAJ_ERR_TAG, "dsm_trajectory_wait", "the field the job read");
 }

@@ -14,9 +14,37 @@
 //   k_vp_select      one CTA per cluster: top_k rounds of a block minimum over the cluster's keys above the last one.
 // A key packs the ranking (-n_seen, cost, offset index) and the rotation into 63 bits, so the least keys are the
 // viewpoints in order and ~0 is no viewpoint.  The kernels carry no error gate and are launched without PDL, as the
-// other field kernels.
-#include "dsm_device.cuh"
-#include <algorithm>
+// other field kernels.  The job's C ABI calls (dsm_viewpoint_enable, _enqueue and _wait) follow them.
+//
+// One staged request (H2D, vp_stage_bytes):
+//   double rotations[64][9] | int32 offsets[4096][3] | int32 clusters[n_clusters]
+// and one packed result (D2H, 64 + 32 n (1 + top_k) B):
+//   int32 header[DSM_VP_WORDS] | dsm_viewpoint_cluster_t records[n] | dsm_viewpoint_t slots[n][top_k]
+// The header's first ten words are those of dsm_viewpoint_info_t; its last two carry the field's error words, cleared
+// by dsm_viewpoint_wait.
+#include "dsm_ctx.hpp"
+
+enum
+{
+    DSM_VP_ORIGIN = 0, // 3 words
+    DSM_VP_N_CLUSTERS = 3,
+    DSM_VP_N_OFFSETS,
+    DSM_VP_N_ROTATIONS,
+    DSM_VP_TOP_K,
+    DSM_VP_UNKNOWN_BLOCKS,
+    DSM_VP_WITH_REACH,
+    DSM_VP_N_CLUSTERS_TABLE,
+    DSM_VP_ERR_TAG = 14, // the field header's DSM_FIELD_ERR_TAG / _ERR_FRAME, copied by k_vp_clusters
+    DSM_VP_ERR_FRAME,
+    DSM_VP_WORDS = 16 // 64 B
+};
+// what k_vp_clusters leaves per requested cluster for the later kernels
+struct DsmVpCluster
+{
+    int32_t g[3];   // the centre voxel
+    int32_t status; // of the record
+    int32_t base, n, n_s, pad; // the members' list offset and count, the samples
+};
 
 #define VP_BLOCK 256
 #define VP_NONE 0xffffffffffffffffull
@@ -244,7 +272,8 @@ __global__ void __launch_bounds__(VP_BLOCK) k_vp_select(const DsmFieldGrid g, co
     if (tid == 0) rec[i].n_viewpoints = n_vp;
 }
 
-int dsm_viewpoint_ctas()
+// the persistent CTAs of k_vp_score on this device
+static int vp_ctas()
 {
     int dev = 0, sms = 0, per = 0;
     if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess ||
@@ -253,36 +282,134 @@ int dsm_viewpoint_ctas()
     return sms * per;
 }
 
-cudaError_t dsm_launch_viewpoint(const DsmViewpointBufs &b, const DsmFieldGrid &g, const uint8_t *state, const int32_t *dist,
-                                 const dsm_gain_camera_t &cam, const dsm_viewpoint_params_t &p, int n_rotations, int n_clusters,
-                                 int n_offsets, const uint8_t *frontier_res, int frontier_max_clusters, const uint32_t *reach_cost,
-                                 cudaStream_t st)
+// byte offsets of the staged request's offsets and clusters and its end, and of the result's slots and its end
+static size_t vp_stage_offsets() { return 8 * 9 * (size_t)DSM_VIEWPOINT_MAX_ROTATIONS; }
+static size_t vp_stage_clusters() { return vp_stage_offsets() + 12 * (size_t)DSM_VIEWPOINT_MAX_OFFSETS; }
+static size_t vp_stage_bytes(int n_clusters) { return vp_stage_clusters() + 4 * (size_t)n_clusters; }
+static size_t vp_slots_at(int n) { return 4 * (size_t)DSM_VP_WORDS + sizeof(dsm_viewpoint_cluster_t) * (size_t)n; }
+static size_t vp_res_bytes(int n, int top_k) { return vp_slots_at(n) + sizeof(dsm_viewpoint_t) * (size_t)n * top_k; }
+
+extern "C" int dsm_viewpoint_enable(dsm_ctx *ctx, int max_clusters, int max_candidates)
 {
-    const size_t voxels = (size_t)g.n[0] * g.n[1] * g.n[2];
-    int32_t *hdr = reinterpret_cast<int32_t *>(b.res);
-    auto *rec = reinterpret_cast<dsm_viewpoint_cluster_t *>(b.res + 4 * DSM_VP_WORDS);
-    auto *out = reinterpret_cast<dsm_viewpoint_t *>(b.res + 4 * DSM_VP_WORDS + sizeof(dsm_viewpoint_cluster_t) * (size_t)n_clusters);
-    const int32_t *fieldhdr = dist + dsm_field_header(voxels);
-    const int32_t *fhdr = reinterpret_cast<const int32_t *>(frontier_res);
-    const auto *table = reinterpret_cast<const dsm_frontier_cluster_t *>(frontier_res + 4 * DSM_FRONTIER_WORDS);
-    const int32_t *members = reinterpret_cast<const int32_t *>(frontier_res + 4 * DSM_FRONTIER_WORDS +
-                                                               sizeof(dsm_frontier_cluster_t) * (size_t)frontier_max_clusters);
-    const double *rot = reinterpret_cast<const double *>(b.stage);
-    const int32_t *offsets = reinterpret_cast<const int32_t *>(b.stage + DsmViewpointBufs::stage_off());
-    const int32_t *clusters = reinterpret_cast<const int32_t *>(b.stage + DsmViewpointBufs::stage_clusters());
-    const uint32_t *cost = p.with_reach ? reach_cost : nullptr;
+    if (!ctx) return DSM_E_INVALID;
+    const DsmField *f = ctx->field.get();
+    if (!f || !ctx->views || ctx->viewpoint) return DSM_E_STATE;
+    if (max_clusters < 1 || max_clusters > DSM_VIEWPOINT_MAX_CLUSTERS || max_candidates < 1 || max_candidates > DSM_VIEWPOINT_MAX_CANDIDATES)
+        return DSM_E_INVALID;
+    CK(cudaSetDevice(ctx->device));
+    auto vp = std::make_unique<DsmViewpoint>();
+    vp->max_clusters = max_clusters, vp->max_candidates = max_candidates;
+    vp->ctas = vp_ctas();
+    const size_t stage = vp_stage_bytes(max_clusters), res = vp_res_bytes(max_clusters, DSM_VIEWPOINT_MAX_TOP_K);
+    CudaOwner &o = vp->own;
+    o.device(&vp->stage_dev, stage);
+    o.host(&vp->stage_host, stage);
+    o.device(&vp->cl, (size_t)max_clusters);
+    o.device(&vp->key, (size_t)max_candidates);
+    o.device(&vp->list, (size_t)max_candidates);
+    o.device(&vp->count, 1);
+    o.device(&vp->res, res);
+    o.host(&vp->res_host, res);
+    o.event(&vp->ev);
+    return keep(ctx->viewpoint, vp, vp->ctas > 0);
+}
+
+// The offsets of include/dsm.h in their order, written as (dx, dy, dz) triples to out (room for
+// DSM_VIEWPOINT_MAX_OFFSETS); returns their number, or -1 past that room.
+static int viewpoint_offsets(const dsm_viewpoint_params_t &p, int32_t *out)
+{
+    int n = 0;
+    const int r = p.r_max / p.stride * p.stride, h = p.dz_max / p.stride * p.stride;
+    for (int dz = -h; dz <= h; dz += p.stride)
+        for (int dy = -r; dy <= r; dy += p.stride)
+            for (int dx = -r; dx <= r; dx += p.stride)
+            {
+                const int q = dx * dx + dy * dy;
+                if (q < p.r_min * p.r_min || q > p.r_max * p.r_max) continue;
+                if (n == DSM_VIEWPOINT_MAX_OFFSETS) return -1;
+                out[3 * n] = dx, out[3 * n + 1] = dy, out[3 * n + 2] = dz;
+                n++;
+            }
+    return n;
+}
+
+// Enqueue only: the rotations, offsets and clusters staged and copied, the kernels on the grids of the latest (known)
+// field request, the latest frontier job's device result and (with_reach) the latest reach job's cost grid, one D2H copy
+// of the used result and the event.  Later field, frontier and reach requests overwrite those buffers only behind the
+// job.
+extern "C" int dsm_viewpoint_enqueue(dsm_ctx *ctx, const dsm_gain_camera_t *camera, const double *rotations, int n_rotations,
+                                     const int32_t *clusters, int n_clusters, const dsm_viewpoint_params_t *params)
+{
+    if (!ctx) return DSM_E_INVALID;
+    DsmViewpoint *vp = ctx->viewpoint.get();
+    const DsmField *f = known_field(ctx);
+    if (!vp || !f || vp->in_flight) return DSM_E_STATE;
+    const DsmFrontier *fr = ctx->frontier.get();
+    if (!read_latest(fr, f)) return DSM_E_STATE;
+    if (!camera || !params || !rotations || n_rotations < 1 || n_rotations > DSM_VIEWPOINT_MAX_ROTATIONS || n_clusters < 0 ||
+        n_clusters > vp->max_clusters || (n_clusters > 0 && !clusters))
+        return DSM_E_INVALID;
+    const dsm_gain_camera_t &c = *camera;
+    const dsm_viewpoint_params_t &p = *params;
+    if (!gain_camera_ok(c, (double)f->g.voxel)) return DSM_E_INVALID;
+    if (p.r_min < 0 || p.r_min > p.r_max || p.r_max > DSM_VIEWPOINT_MAX_RADIUS || p.dz_max < 0 || p.dz_max > DSM_VIEWPOINT_MAX_DZ ||
+        p.stride < 1 || p.stride > DSM_VIEWPOINT_MAX_STRIDE || p.max_samples < 1 || p.max_samples > DSM_VIEWPOINT_MAX_SAMPLES ||
+        p.min_seen < 0 || p.top_k < 1 || p.top_k > DSM_VIEWPOINT_MAX_TOP_K || (p.with_reach != 0 && p.with_reach != 1) ||
+        !std::isfinite(p.radius) || !(p.radius >= 0.f))
+        return DSM_E_INVALID;
+    for (size_t i = 0; i < 9 * (size_t)n_rotations; i++)
+        if (!std::isfinite(rotations[i])) return DSM_E_INVALID;
+    for (int i = 0; i < n_clusters; i++)
+        if (clusters[i] < 0) return DSM_E_INVALID;
+    // the previous job's copy out of this staging ended before its wait, which no job in flight implies
+    const int n_offsets = viewpoint_offsets(p, reinterpret_cast<int32_t *>(vp->stage_host + vp_stage_offsets()));
+    if (n_offsets < 1 || (long long)n_clusters * n_offsets > vp->max_candidates ||
+        (long long)n_clusters * n_offsets * p.max_samples > DSM_VIEWPOINT_MAX_WORK)
+        return DSM_E_INVALID;
+    const DsmReach *re = ctx->reach.get();
+    if (p.with_reach && !read_latest(re, f)) return DSM_E_STATE;
+    CK(cudaSetDevice(ctx->device));
+    const cudaStream_t st = ctx->stream;
+    std::memcpy(vp->stage_host, rotations, 72 * (size_t)n_rotations);
+    if (n_clusters > 0) std::memcpy(vp->stage_host + vp_stage_clusters(), clusters, 4 * (size_t)n_clusters);
+    CK(cudaMemcpyAsync(vp->stage_dev, vp->stage_host, vp_stage_bytes(n_clusters), cudaMemcpyHostToDevice, st));
+    const DsmFieldGrid &g = f->g;
+    int32_t *hdr = reinterpret_cast<int32_t *>(vp->res);
+    auto *rec = reinterpret_cast<dsm_viewpoint_cluster_t *>(vp->res + 4 * DSM_VP_WORDS);
+    auto *out = reinterpret_cast<dsm_viewpoint_t *>(vp->res + vp_slots_at(n_clusters));
+    const auto *table = reinterpret_cast<const dsm_frontier_cluster_t *>(fr->res + DsmFrontier::table_at());
+    const int32_t *members = reinterpret_cast<const int32_t *>(fr->res + fr->list_at());
+    const double *rot = reinterpret_cast<const double *>(vp->stage_dev);
+    const int32_t *offsets = reinterpret_cast<const int32_t *>(vp->stage_dev + vp_stage_offsets());
+    const uint32_t *cost = p.with_reach ? re->cost[0] : nullptr;
     k_vp_clusters<<<(unsigned)std::max((n_clusters + VP_BLOCK - 1) / VP_BLOCK, 1), VP_BLOCK, 0, st>>>(
-        g, fieldhdr, fhdr, table, frontier_max_clusters, clusters, n_clusters, n_offsets, n_rotations, p.top_k, cam.unknown_blocks,
-        p.with_reach, p.max_samples, hdr, rec, b.cl, b.count);
+        g, f->dist + dsm_field_header(f->voxels), reinterpret_cast<const int32_t *>(fr->res), table, fr->max_clusters,
+        reinterpret_cast<const int32_t *>(vp->stage_dev + vp_stage_clusters()), n_clusters, n_offsets, n_rotations, p.top_k, c.unknown_blocks,
+        p.with_reach, p.max_samples, hdr, rec, vp->cl, vp->count);
     if (n_clusters > 0)
     {
         k_vp_candidates<<<dim3((unsigned)((n_offsets + VP_BLOCK - 1) / VP_BLOCK), (unsigned)n_clusters), VP_BLOCK, 0, st>>>(
-            g, state, dist, offsets, n_offsets, p.radius, cost, b.cl, rec, b.key, b.list, b.count);
-        const double R = (double)cam.max_range;
-        k_vp_score<<<(unsigned)b.ctas, VP_BLOCK, 0, st>>>(g, state, rot, n_rotations, offsets, n_offsets, b.cl, members, b.list, b.count, cost,
-                                                          cam.fx, cam.fy, cam.cx, cam.cy, (double)cam.width, (double)cam.height, R * R,
-                                                          cam.unknown_blocks, p.min_seen, b.key);
-        k_vp_select<<<(unsigned)n_clusters, VP_BLOCK, 0, st>>>(g, offsets, n_offsets, p.top_k, b.cl, b.key, rec, out);
+            g, f->occ, f->dist, offsets, n_offsets, p.radius, cost, vp->cl, rec, vp->key, vp->list, vp->count);
+        const double R = (double)c.max_range;
+        k_vp_score<<<(unsigned)vp->ctas, VP_BLOCK, 0, st>>>(g, f->occ, rot, n_rotations, offsets, n_offsets, vp->cl, members, vp->list, vp->count,
+                                                            cost, c.fx, c.fy, c.cx, c.cy, (double)c.width, (double)c.height, R * R,
+                                                            c.unknown_blocks, p.min_seen, vp->key);
+        k_vp_select<<<(unsigned)n_clusters, VP_BLOCK, 0, st>>>(g, offsets, n_offsets, p.top_k, vp->cl, vp->key, rec, out);
     }
-    return cudaGetLastError();
+    CK(cudaGetLastError());
+    vp->n_clusters = n_clusters, vp->top_k = p.top_k;
+    return submit(ctx, *vp, vp->res, vp_res_bytes(n_clusters, p.top_k), f->requests);
+}
+
+extern "C" int dsm_viewpoint_wait(dsm_ctx *ctx, dsm_viewpoint_info_t *info, const dsm_viewpoint_cluster_t **clusters,
+                                  const dsm_viewpoint_t **viewpoints)
+{
+    if (!ctx) return DSM_E_INVALID;
+    DsmViewpoint *vp = ctx->viewpoint.get();
+    const int rc = wait_head(ctx, vp);
+    if (rc != DSM_OK) return rc;
+    copy_info(info, vp->words());
+    if (clusters) *clusters = reinterpret_cast<const dsm_viewpoint_cluster_t *>(vp->res_host + 4 * DSM_VP_WORDS);
+    if (viewpoints) *viewpoints = reinterpret_cast<const dsm_viewpoint_t *>(vp->res_host + vp_slots_at(vp->n_clusters));
+    return capacity(ctx, vp->words(), DSM_VP_ERR_TAG, "dsm_viewpoint_wait", "the field the job read");
 }
