@@ -7,7 +7,7 @@ import subprocess
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libdsm_b200.so")
-SOURCES = ["dsm_kernels.cu", "dsm_tile.cu", "dsm_capi.cu", "dsm_comm.cu", "dsm_io.cpp", "dsm_field.cu", "dsm_frontier.cu", "dsm_reach.cu", "dsm_gain.cu", "dsm_tour.cu", "dsm_viewpoint.cu", "dsm_trajectory.cu", "dsm_heading.cu"]
+SOURCES = ["dsm_kernels.cu", "dsm_tile.cu", "dsm_capi.cu", "dsm_comm.cu", "dsm_io.cpp", "dsm_field.cu", "dsm_frontier.cu", "dsm_reach.cu", "dsm_gain.cu", "dsm_tour.cu", "dsm_viewpoint.cu", "dsm_trajectory.cu", "dsm_heading.cu", "dsm_terrain.cu"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-fmad=false", "-prec-div=true", "-prec-sqrt=true", "-ftz=false",

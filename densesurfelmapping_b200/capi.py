@@ -43,6 +43,7 @@ EXPORTS = [
     "dsm_tour_enable", "dsm_tour_enqueue", "dsm_tour_wait", "dsm_viewpoint_enable", "dsm_viewpoint_enqueue", "dsm_viewpoint_wait",
     "dsm_trajectory_enable", "dsm_trajectory_enqueue", "dsm_trajectory_wait",
     "dsm_heading_enable", "dsm_heading_enqueue", "dsm_heading_wait",
+    "dsm_terrain_enable", "dsm_terrain_enqueue", "dsm_terrain_wait",
     "dsm_inactive_segments", "dsm_inactive_load", "dsm_map_save", "dsm_map_load", "dsm_map_peek",
     "dsm_checkpoint_enable", "dsm_checkpoint_enqueue", "dsm_checkpoint_wait", "dsm_debug_checkpoint_drain_ctas",
     "dsm_checkpoint_enqueue_incremental", "dsm_map_load_journal", "dsm_map_peek_journal", "dsm_journal_materialize",
@@ -122,6 +123,10 @@ HEADING_SAMPLE_DTYPE = np.dtype([("p", "<f8", 3), ("rotation", "<i4"), ("turn", 
 HEADING_COUNT_DTYPE = np.dtype([("n_unknown", "<i4"), ("n_frontier", "<i4")])
 HEADING_INFO_DTYPE = np.dtype([("origin", "<i4", 3), ("n_trajectories", "<i4"), ("n_samples", "<i4"), ("n_rot", "<i4"),
                                ("unknown_blocks", "<i4"), ("n_status", "<i4", 2), ("reserved", "<i4", 7)])
+
+# dsm_terrain_wait's header (include/dsm.h, 64 B)
+TERRAIN_INFO_DTYPE = np.dtype([("origin", "<i4", 3), ("m", "<i4", 3), ("up", "<i4"), ("headroom", "<i4"), ("max_step", "<i4"),
+                               ("n_support", "<i4"), ("n_blocked", "<i4"), ("n_traversable", "<i4"), ("reserved", "<i4", 4)])
 
 
 class DsmGainCamera(ctypes.Structure):
@@ -237,6 +242,9 @@ def load_library():
     L.dsm_heading_enable.argtypes = [vp, ci, ci]
     L.dsm_heading_enqueue.argtypes = [vp, vp, vp, ci, ctypes.POINTER(DsmGainCamera), vp, ci, ci, vp, ctypes.c_int32, ctypes.c_int32]
     L.dsm_heading_wait.argtypes = [vp, vp, ctypes.POINTER(vp), ctypes.POINTER(vp), ctypes.POINTER(vp)]
+    L.dsm_terrain_enable.argtypes = [vp, ci]
+    L.dsm_terrain_enqueue.argtypes = [vp, ci, ci]
+    L.dsm_terrain_wait.argtypes = [vp, vp, ctypes.POINTER(vp), ctypes.POINTER(vp), ctypes.POINTER(vp), ctypes.POINTER(vp)]
     L.dsm_inactive_reserve.argtypes = [vp, ci]
     L.dsm_inactive_retire.argtypes = [vp, ci, ctypes.POINTER(ci)]
     L.dsm_inactive_reactivate.argtypes = [vp, ci, ctypes.POINTER(ci)]
@@ -972,6 +980,30 @@ class Context:
         n, S, R = int(i["n_trajectories"]), int(i["n_samples"]), int(i["n_rot"])
         return self._waited(rc, "heading", lambda: (i, _take(pr, n, HEADING_DTYPE), _take(ps, S, HEADING_SAMPLE_DTYPE),
                                                     _take(pc, S * R, HEADING_COUNT_DTYPE).reshape(S, R)))
+
+    # ---- the terrain of the latest known field ----
+    def terrain_enable(self, up):
+        """up in {+-1, +-2, +-3}: the field grid's axis |up| - 1, toward + or - (-2 for y-down camera frames)."""
+        self._ck(self.lib.dsm_terrain_enable(self.h, int(up)))
+
+    def terrain_enqueue(self, headroom, max_step):
+        self._ck(self.lib.dsm_terrain_enqueue(self.h, int(headroom), int(max_step)))
+
+    def terrain_wait(self):
+        """(info, level, status, step, clearance): numpy copies of the context's pinned results, a TERRAIN_INFO_DTYPE
+        record and the int16, uint8, uint8 and float32 planes [m2][m1][m0] of the terrain grid.  A job on a field taken
+        after a rejected frame raises DsmError(DSM_E_CAPACITY) carrying the same tuple as `.terrain`."""
+        pl, ps, pt, pc = ctypes.c_void_p(), ctypes.c_void_p(), ctypes.c_void_p(), ctypes.c_void_p()
+        info = np.zeros(1, TERRAIN_INFO_DTYPE)
+        rc = self.lib.dsm_terrain_wait(self.h, info.ctypes.data, ctypes.byref(pl), ctypes.byref(ps), ctypes.byref(pt), ctypes.byref(pc))
+        i = info[0]
+        m0, m1, m2 = (int(x) for x in i["m"])
+        cells = m0 * m1 * m2
+
+        def planes():
+            return (i,) + tuple(_take(p, cells, dt).reshape(m2, m1, m0) for p, dt in ((pl, np.int16), (ps, np.uint8), (pt, np.uint8),
+                                                                                      (pc, np.float32)))
+        return self._waited(rc, "terrain", planes)
 
     # ---- planner queries against the latest field ----
     def field_query_enable(self, max_points, max_trajectories, max_waypoints):

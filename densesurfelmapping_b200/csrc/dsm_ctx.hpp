@@ -1,7 +1,7 @@
 // Private to the library: the context behind the opaque `dsm_ctx` of include/dsm.h, shared by the translation units
 // that hold its entry points (dsm_capi.cu: the map, the field and checkpoints; dsm_comm.cu: multi-GPU gather over NCCL;
-// dsm_field.cu, dsm_frontier.cu, dsm_reach.cu, dsm_gain.cu, dsm_viewpoint.cu, dsm_tour.cu, dsm_trajectory.cu and
-// dsm_heading.cu: the planner jobs, each beside its kernels), and the lifecycle those jobs share.
+// dsm_field.cu, dsm_frontier.cu, dsm_reach.cu, dsm_gain.cu, dsm_viewpoint.cu, dsm_tour.cu, dsm_trajectory.cu,
+// dsm_heading.cu and dsm_terrain.cu: the planner jobs, each beside its kernels), and the lifecycle those jobs share.
 #pragma once
 #include "dsm_device.cuh"
 #include "dsm_map_state.h"
@@ -394,6 +394,16 @@ struct DsmHeading : DsmJob
     int n = 0, n_samples = 0, n_rot = 0; // of the job in flight or last waited for
 };
 
+// dsm_terrain_* (DESIGN.md §8.20), allocated by dsm_terrain_enable for the field's grid collapsed along the up axis: the
+// device result (its layout in dsm_terrain.cu)
+struct DsmTerrain : DsmJob
+{
+    int up = 0, cells = 0;
+    int m[3] = {0, 0, 0};
+    uint8_t *res = nullptr;
+    int origin[3] = {0, 0, 0}, headroom = 0, max_step = 0; // of the job in flight or last waited for
+};
+
 #define DSM_MAX_CHUNKS 4
 
 struct dsm_ctx
@@ -473,6 +483,7 @@ struct dsm_ctx
     std::unique_ptr<DsmViewpoint> viewpoint;     // nullptr until dsm_viewpoint_enable
     std::unique_ptr<DsmTrajectory> trajectory;   // nullptr until dsm_trajectory_enable
     std::unique_ptr<DsmHeading> heading;         // nullptr until dsm_heading_enable
+    std::unique_ptr<DsmTerrain> terrain;         // nullptr until dsm_terrain_enable
     int run_split = 2;          // sub-batches per dsm_batch_run (dsm_set_concurrency)
     // pinned host staging for the small per-batch tables
     float *h_pose = nullptr; // [2B][32]: pose then inverse; first half: the batch calls, second half: the resident stream

@@ -1292,6 +1292,62 @@ int dsm_heading_enqueue(dsm_ctx *ctx, const double *points, const int32_t *offse
 int dsm_heading_wait(dsm_ctx *ctx, dsm_heading_info_t *info, const dsm_heading_t **records, const dsm_heading_sample_t **samples,
                      const dsm_heading_count_t **counts);
 
+/* ---- terrain: where a ground robot can drive on the known field (DESIGN.md §8.20) ----
+ * A terrain job reads the state grid of the latest field request, which must be a known one, in stream order behind it,
+ * with that request's origin o captured at the job's enqueue.  A later field request may be enqueued while a job is in
+ * flight and does not change what the job reads.  The map is never read.
+ *
+ * Definition (integer throughout, so the result does not depend on the schedule; the clearance rounds as a field's).
+ *   Up axis: up in {+-1, +-2, +-3}, fixed at enable: axis a = |up| - 1 of the field grid, pointing toward +a for a
+ *   positive up and -a for a negative one.  "Above voxel k" (k the coordinate along a) is k + 1 for a positive up and
+ *   k - 1 for a negative one.  Camera-frame poses with y down (KITTI, the synthetic world) take up = -2; a z-up world
+ *   takes up = +3.
+ *   Terrain grid: the field grid with axis a collapsed, m_k = n_k except m_a = 1, at the request's origin o (all three
+ *   words).  Cell (x, y, z) has the linear index (z * m1 + y) * m0 + x, as a voxel of a grid of shape m.
+ *   Support: per column, level = the uppermost (in the up sense) k with state[k] == 1 (occupied) whose `headroom`
+ *   voxels above it lie inside the grid and are all of state 2 (free); -1 when no k qualifies.  Unknown space is never
+ *   free: a deck whose top no camera has seen is not chosen, and the road under it is when its headroom was observed;
+ *   a column whose headroom is cut by the grid's top face or holds one unknown voxel has no support.  The surface of
+ *   level k lies at height (o_a + k + 1) v metres along +a for a positive up, and at -(o_a + k) v metres, measured
+ *   along -a, for a negative one.
+ *   Step: for a cell with support, the largest |level(c) - level(n)| over the cell's in-grid 8-neighbours n in the two
+ *   axes other than a that have support, 0 without such a neighbour; 0 for a cell without support.  The result stores
+ *   min(step, 255); the status compares the full step.
+ *   Status: 0 no support, 1 support but step > max_step, 2 traversable: the field's state codes (unknown, occupied,
+ *   free), so "not traversable" is "status != 2".
+ *   Clearance: sqrtf((float)d2) * v, d2 the smallest squared integer distance in cells (over the terrain grid) to a cell
+ *   of status != 2; 0 on such cells, +inf when every cell is traversable.  It is the known field's distance of the
+ *   status plane as a grid of shape m: a caller that keeps clearance >= r keeps a disc of radius r on drivable ground.
+ *   Counts: n_support the cells with support, n_blocked those of status 1, n_traversable those of status 2.
+ *   Result: per cell an int16 level, a uint8 status, a uint8 step and a float clearance, 8 B per cell.
+ *
+ *   dsm_terrain_enable    once, after dsm_views_enable (DSM_E_STATE otherwise, and when called twice).  DSM_E_INVALID
+ *                         for up outside {+-1, +-2, +-3}.  Allocates, for the field's grid collapsed along a, the device
+ *                         result (the four planes, 8 B per cell, and 32 B of header) and its pinned copy, and an event.
+ *                         DSM_E_NOMEM with nothing kept.
+ *   dsm_terrain_enqueue   asynchronous on the context's stream, never waits: the kernels, one D2H copy of the result and
+ *                         the event.  DSM_E_STATE before dsm_terrain_enable, before any field request, when the latest
+ *                         field request is not a known one, and while a job is in flight.  DSM_E_INVALID for headroom
+ *                         outside [1, n_a - 1] or max_step outside [0, 1023].
+ *   dsm_terrain_wait      waits for that job only.  *level, *status, *step and *clearance (m0 m1 m2 cells each) are
+ *                         the context's pinned results, valid until the next dsm_terrain_enqueue; any out-pointer may be
+ *                         NULL.  If the field the job read was taken after a rejected frame, returns DSM_E_CAPACITY with
+ *                         valid results and does NOT clear the error, as dsm_field_wait.  DSM_E_STATE with no job
+ *                         enqueued. */
+typedef struct dsm_terrain_info_t
+{
+    int32_t origin[3];               /* the field request's origin, voxels */
+    int32_t m[3];                    /* the terrain grid: the field grid with m[|up| - 1] = 1 */
+    int32_t up, headroom, max_step;
+    int32_t n_support, n_blocked, n_traversable;
+    int32_t reserved[4];             /* 0 */
+} dsm_terrain_info_t;                /* 64 B */
+#define DSM_TERRAIN_MAX_STEP 1023
+int dsm_terrain_enable(dsm_ctx *ctx, int up);
+int dsm_terrain_enqueue(dsm_ctx *ctx, int headroom, int max_step);
+int dsm_terrain_wait(dsm_ctx *ctx, dsm_terrain_info_t *info, const int16_t **level, const uint8_t **status, const uint8_t **step,
+                     const float **clearance);
+
 /* ---- checkpoints that do not stop the stream (DESIGN.md §8.5) ----
  * The file of dsm_map_save, taken in stream order like a publish snapshot: the resident stream pays one device-to-device
  * copy of the live map, the transfer to the host runs on a low-priority stream beside the next frames, and a thread of

@@ -106,6 +106,10 @@
 // enable_known_space, lets headings() plan the camera's heading along trajectories on the device (DESIGN.md §8.19): the
 // unknown and frontier voxels seen at every sample and rotation, then the best rate-limited rotation sequence per
 // trajectory, one enqueue and one wait.
+// Where can a ground robot drive?  enable_terrain(up), after enable_known_space, lets terrain() find the supporting
+// surface of every column of the latest fused frame's known field along the up axis on the device (DESIGN.md §8.20):
+// its level, the step to its neighbours, whether it is traversable and the clearance to the nearest cell that is not,
+// one enqueue and one wait.
 // device < 0 builds the node without a context: the callbacks run the whole pose logic (pose database, sync, window
 // bookkeeping) and fuse nothing; any call that reads the map returns DSM_E_STATE.
 #pragma once
@@ -826,6 +830,36 @@ class SurfelMapNode
                 samples_out.assign(s, s + info.n_samples);
                 counts.assign(c, c + (size_t)info.n_samples * info.n_rot);
             });
+    }
+    // ---- the terrain of the known field of the latest fused frame (DESIGN.md §8.20) ----
+    // once, after enable_known_space: up in {+-1, +-2, +-3}, the field grid's axis |up| - 1 toward + or - (-2 for the
+    // y-down camera frames of KITTI poses)
+    int enable_terrain(int up) { return ctx_.run("enable_terrain", [&] { return dsm_terrain_enable(ctx_.ctx, up); }); }
+    // per cell of the field grid collapsed along the up axis ([m2][m1][m0], info.m): the support level, status (0 no
+    // support, 1 blocked by the step, 2 traversable), step and clearance in metres (include/dsm.h) for `headroom` free
+    // voxels above the support and steps of at most max_step voxels.  DSM_E_STATE without known space, before any field
+    // and after load_state* until the next fused frame; DSM_E_CAPACITY with the terrain of the last applied frame's
+    // field, as distance_field().
+    int terrain(int headroom, int max_step, dsm_terrain_info_t &info, std::vector<int16_t> &level, std::vector<uint8_t> &status,
+                std::vector<uint8_t> &step, std::vector<float> &clearance)
+    {
+        level.clear();
+        status.clear();
+        step.clear();
+        clearance.clear();
+        info = dsm_terrain_info_t();
+        const int16_t *l = nullptr;
+        const uint8_t *s = nullptr, *t = nullptr;
+        const float *c = nullptr;
+        return job("terrain", KNOWN_FIELD, true, [&] { return dsm_terrain_enqueue(ctx_.ctx, headroom, max_step); },
+                   [&] { return dsm_terrain_wait(ctx_.ctx, &info, &l, &s, &t, &c); },
+                   [&] {
+                       const size_t n = (size_t)info.m[0] * info.m[1] * info.m[2];
+                       level.assign(l, l + n);
+                       status.assign(s, s + n);
+                       step.assign(t, t + n);
+                       clearance.assign(c, c + n);
+                   });
     }
     // the field of the latest fused frame: dist [nz][ny][nx] in metres (the library's pinned buffer, valid until the next
     // frame is fused; nullptr for a field kept on the device), the grid's origin in voxels and the occupied voxels.  DSM_E_STATE when no frame has been fused
