@@ -38,7 +38,7 @@ EXPORTS = [
     "dsm_views_enable", "dsm_views_capture", "dsm_field_enqueue_known", "dsm_field_state",
     "dsm_frontier_enable", "dsm_frontier_enqueue", "dsm_frontier_wait", "dsm_debug_field_load_state",
     "dsm_field_signed_enable", "dsm_field_signed", "dsm_field_query_enqueue_signed",
-    "dsm_reach_enable", "dsm_reach_enqueue", "dsm_reach_wait", "dsm_reach_matrix_enable", "dsm_reach_matrix_enqueue",
+    "dsm_reach_enable", "dsm_reach_enqueue", "dsm_reach_enqueue_terrain", "dsm_reach_wait", "dsm_reach_matrix_enable", "dsm_reach_matrix_enqueue",
     "dsm_reach_matrix_wait", "dsm_gain_enable", "dsm_gain_enqueue", "dsm_gain_wait",
     "dsm_tour_enable", "dsm_tour_enqueue", "dsm_tour_wait", "dsm_viewpoint_enable", "dsm_viewpoint_enqueue", "dsm_viewpoint_wait",
     "dsm_trajectory_enable", "dsm_trajectory_enqueue", "dsm_trajectory_wait",
@@ -223,6 +223,7 @@ def load_library():
     L.dsm_field_query_enqueue_signed.argtypes = [vp, vp, ci, vp, vp, ci, ctypes.c_float, ctypes.c_float]
     L.dsm_reach_enable.argtypes = [vp, ci, ci, ci]
     L.dsm_reach_enqueue.argtypes = [vp, ctypes.POINTER(ctypes.c_double), ctypes.c_float, ci, vp, ci, ci, ci]
+    L.dsm_reach_enqueue_terrain.argtypes = [vp, ctypes.POINTER(ctypes.c_double), ctypes.c_float, ci, vp, ci, ci, ci]
     L.dsm_reach_wait.argtypes = [vp, vp, ctypes.POINTER(vp), ctypes.POINTER(vp), ctypes.POINTER(vp)]
     L.dsm_reach_matrix_enable.argtypes = [vp, ci, ci, ci]
     L.dsm_reach_matrix_enqueue.argtypes = [vp, vp, ci, ctypes.c_float, ci]
@@ -798,16 +799,25 @@ class Context:
 
     def reach_enqueue(self, start, radius, approach, goals=None, with_frontiers=False, host_copy=False):
         """start: a world point (x, y, z); goals: world points, an (n, 3) array-like of float64 (None for none)."""
+        self._reach_enqueue(self.lib.dsm_reach_enqueue, False, start, radius, approach, goals, with_frontiers, host_copy)
+
+    def reach_enqueue_terrain(self, start, radius, approach, goals=None, with_frontiers=False, host_copy=False):
+        """The reach job on the plane of the latest terrain job (DESIGN.md §8.21), arguments as reach_enqueue's; each
+        point stands for its column.  reach_wait then returns the cost grid [m2][m1][m0] of the terrain grid."""
+        self._reach_enqueue(self.lib.dsm_reach_enqueue_terrain, True, start, radius, approach, goals, with_frontiers, host_copy)
+
+    def _reach_enqueue(self, call, terrain, start, radius, approach, goals, with_frontiers, host_copy):
         st = (ctypes.c_double * 3)(*[float(v) for v in start])
         g = np.ascontiguousarray(np.zeros((0, 3)) if goals is None else goals, np.float64).reshape(-1, 3)
-        self._ck(self.lib.dsm_reach_enqueue(self.h, st, float(radius), int(approach), g.ctypes.data if len(g) else None, len(g),
-                                            int(bool(with_frontiers)), int(bool(host_copy))))
+        self._ck(call(self.h, st, float(radius), int(approach), g.ctypes.data if len(g) else None, len(g), int(bool(with_frontiers)),
+                      int(bool(host_copy))))
+        self._reach_terrain = terrain   # which grid reach_wait's cost grid covers
 
     def reach_wait(self):
         """(info, targets, path, cost): numpy copies of the context's pinned results, a REACH_INFO_DTYPE record,
-        REACH_TARGET_DTYPE (n_targets,), int32 (n_path_voxels,) and the uint32 cost grid [nz][ny][nx] (None without
-        host_copy).  A job on a field taken after a rejected frame raises DsmError(DSM_E_CAPACITY) carrying the same
-        tuple as `.reach`."""
+        REACH_TARGET_DTYPE (n_targets,), int32 (n_path_voxels,) and the uint32 cost grid (None without host_copy),
+        [nz][ny][nx] after reach_enqueue and [m2][m1][m0] of the terrain grid after reach_enqueue_terrain.  A job on a
+        field taken after a rejected frame raises DsmError(DSM_E_CAPACITY) carrying the same tuple as `.reach`."""
         pt, pp, pc = ctypes.c_void_p(), ctypes.c_void_p(), ctypes.c_void_p()
         info = np.zeros(1, REACH_INFO_DTYPE)
         rc = self.lib.dsm_reach_wait(self.h, info.ctypes.data, ctypes.byref(pt), ctypes.byref(pp), ctypes.byref(pc))
@@ -815,6 +825,8 @@ class Context:
 
         def reach():
             shape = self._field_shape
+            if getattr(self, "_reach_terrain", False):   # the field grid collapsed along the terrain's up axis
+                shape = tuple(1 if k == 2 - (abs(self._terrain_up) - 1) else n for k, n in enumerate(shape))
             cost = _take(pc, shape[0] * shape[1] * shape[2], np.uint32).reshape(shape) if pc.value else None
             return i, _take(pt, int(i["n_targets"]), REACH_TARGET_DTYPE), _take(pp, int(i["n_path_voxels"]), np.int32), cost
         return self._waited(rc, "reach", reach)
@@ -985,6 +997,7 @@ class Context:
     def terrain_enable(self, up):
         """up in {+-1, +-2, +-3}: the field grid's axis |up| - 1, toward + or - (-2 for y-down camera frames)."""
         self._ck(self.lib.dsm_terrain_enable(self.h, int(up)))
+        self._terrain_up = int(up)
 
     def terrain_enqueue(self, headroom, max_step):
         self._ck(self.lib.dsm_terrain_enqueue(self.h, int(headroom), int(max_step)))

@@ -289,11 +289,13 @@ struct DsmFrontier : DsmJob
 };
 
 // dsm_reach_* (DESIGN.md §8.11), allocated by dsm_reach_enable for the field's grid: the job's device buffers, the packed
-// result (dsm_reach.cu), the goal staging and the cost grid's pinned copy
+// result (dsm_reach.cu), the goal staging and the cost grid's pinned copy.  A terrain job (§8.21) runs in the same
+// buffers: its plane has no more cells than the field has voxels, nor more 32 x 16 tiles than the field has 8^3 ones.
 struct DsmReach : DsmJob
 {
     int voxels = 0, tiles = 0, tn[3] = {0, 0, 0}; // tn: tiles per axis
     int max_targets = 0, max_path = 0, max_rounds = 0, ctas = 0; // ctas: the persistent CTAs of a round
+    int ctas_flat = 0;                            // those of a terrain job's round (dsm_reach_enqueue_terrain)
     uint8_t *trav = nullptr;                      // [voxels]
     uint32_t *cost[2] = {nullptr, nullptr};       // [voxels] each
     int32_t *stamp = nullptr;                     // [tiles]: the latest round a tile was scheduled for
@@ -402,6 +404,15 @@ struct DsmTerrain : DsmJob
     int m[3] = {0, 0, 0};
     uint8_t *res = nullptr;
     int origin[3] = {0, 0, 0}, headroom = 0, max_step = 0; // of the job in flight or last waited for
+    // byte offsets of the result's sections for C cells, which the terrain reach job reads as well:
+    //   float clearance[C] | pad to dsm_field_header(C) words | int32 header[8] (a field header's words, dsm_device.cuh) |
+    //   int16 level[C] | uint8 status[C] | uint8 step[C]
+    static constexpr int HEADER_WORDS = 8;
+    static size_t header_at(int cells) { return 4 * dsm_field_header((size_t)cells); }
+    static size_t level_at(int cells) { return header_at(cells) + 4 * HEADER_WORDS; }
+    static size_t status_at(int cells) { return level_at(cells) + 2 * (size_t)cells; }
+    static size_t step_at(int cells) { return status_at(cells) + (size_t)cells; }
+    static size_t res_bytes(int cells) { return step_at(cells) + (size_t)cells; }
 };
 
 #define DSM_MAX_CHUNKS 4

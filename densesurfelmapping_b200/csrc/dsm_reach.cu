@@ -19,6 +19,10 @@
 //   k_reach_records  one thread per target record.
 //   k_reach_paths    one warp per reached target, lanes on the 26 neighbours and a shuffle argmin per step: a counting
 //                    walk, a cub exclusive scan of the lengths, then the writing walk.
+// The terrain job (dsm_reach_enqueue_terrain, DESIGN.md §8.21) runs the same kernels on the plane (P, Q, 1) of the latest
+// terrain job's status and clearance planes: the rounds on flat 32 x 16 x 1 tiles (k_reach_round<32, 16, 1>: a 34 x 18
+// halo, 8 neighbours per sweep, 9 neighbour tiles), and the target kernels on a ReachTerrainGrid, which maps a frontier
+// member voxel to its column's cell.
 // The matrix job (dsm_reach_matrix_*, DESIGN.md §8.13) runs the same rounds from many sites at once; its kernels follow
 // the reach job's C ABI calls (dsm_reach_enable, _enqueue and _wait) below, share reach_snap and reach_relax with
 // k_reach_start and k_reach_round, and are followed by its own (dsm_reach_matrix_enable, _enqueue and _wait).
@@ -26,6 +30,7 @@
 #include "dsm_ctx.hpp"
 #include <cub/block/block_scan.cuh>
 #include <cub/device/device_scan.cuh>
+#include <type_traits>
 
 // One packed result (D2H):
 //   int32 header[DSM_REACH_WORDS] | dsm_reach_target_t targets[max_targets] | int32 path[max_path_voxels]
@@ -54,6 +59,27 @@ enum
 #define RC_TILE (RC_T * RC_T * RC_T) // 512 threads
 #define RC_H (RC_T + 2)              // the staged tile with its halo
 #define RC_INF 0xffffffffu
+#define RC_FLAT_X 32 // the terrain job's tiles: 32 x 16 x 1 cells of its plane
+#define RC_FLAT_Y 16
+
+// A round's tile of TX x TY x TZ voxels, one per CTA of RC_TILE threads, and the shared-memory halo it is staged with.
+// A flat tile (TZ == 1) runs on a grid one voxel thick: no halo and no moves along z, and 9 neighbour tiles.
+template <int TX, int TY, int TZ>
+struct ReachTile
+{
+    static_assert(TX * TY * TZ == RC_TILE, "one voxel per thread");
+    static constexpr int DZ = TZ == 1 ? 0 : 1; // the moves' z offsets span -DZ .. DZ
+    static constexpr int HX = TX + 2, HY = TY + 2, HZ = TZ + 2 * DZ;
+    static constexpr int HALO = HX * HY * HZ;
+    static constexpr int NB = DZ ? 27 : 9; // the tile and its neighbour tiles
+};
+
+// The terrain job's grid: n the plane (P, Q, 1), o the terrain job's origin; nf the field grid's extents and h0 < h1 its
+// two in-plane axes, which map a field voxel to the cell of its column
+struct ReachTerrainGrid : DsmFieldGrid
+{
+    int nf[3], h0, h1;
+};
 
 static_assert(sizeof(dsm_reach_target_t) == 32 && sizeof(dsm_reach_info_t) == 64, "dsm_reach layouts");
 static_assert(DSM_REACH_N_PATH_VOXELS == 13 && DSM_REACH_WORDS * 4 == sizeof(dsm_reach_info_t), "the header starts with the info");
@@ -105,11 +131,13 @@ __device__ __forceinline__ unsigned long long reach_snap(const DsmFieldGrid &g, 
     return warp_min64(key);
 }
 
-// The tile-local fixed point of the staged tile (vs: the tile and its halo, RC_H^3, voxel si of this thread, tv its
-// traversable flag, c its cost): Bellman-Ford sweeps in place until __syncthreads_or reports no change, with the halo
-// frozen; unique whatever the interleaving.  Every thread of the CTA calls it.  Returns the voxel's cost.
+// The tile-local fixed point of the staged tile (vs: the tile and its halo, ReachTile's HALO words, voxel si of this
+// thread, tv its traversable flag, c its cost): Bellman-Ford sweeps in place until __syncthreads_or reports no change,
+// with the halo frozen; unique whatever the interleaving.  Every thread of the CTA calls it.  Returns the voxel's cost.
+template <int TX, int TY, int TZ>
 __device__ __forceinline__ uint32_t reach_relax(volatile uint32_t *vs, int si, bool tv, uint32_t c)
 {
+    typedef ReachTile<TX, TY, TZ> T;
     while (true)
     { // only traversable voxels ever hold a finite cost, so a finite neighbour is a traversable one
         bool changed = false;
@@ -117,14 +145,14 @@ __device__ __forceinline__ uint32_t reach_relax(volatile uint32_t *vs, int si, b
         {
             uint32_t best = c;
 #pragma unroll
-            for (int dz = -1; dz <= 1; dz++)
+            for (int dz = -T::DZ; dz <= T::DZ; dz++)
 #pragma unroll
                 for (int dy = -1; dy <= 1; dy++)
 #pragma unroll
                     for (int dx = -1; dx <= 1; dx++)
                     {
                         if (dx == 0 && dy == 0 && dz == 0) continue;
-                        const uint32_t v = vs[si + (dz * RC_H + dy) * RC_H + dx];
+                        const uint32_t v = vs[si + (dz * T::HY + dy) * T::HX + dx];
                         const uint32_t w = (uint32_t)reach_chamfer(dx, dy, dz);
                         if (v != RC_INF && v + w < best) best = v + w;
                     }
@@ -140,6 +168,7 @@ __device__ __forceinline__ uint32_t reach_relax(volatile uint32_t *vs, int si, b
     return c;
 }
 
+template <int TX, int TY, int TZ>
 __global__ void __launch_bounds__(32) k_reach_start(const DsmFieldGrid g, const uint8_t *__restrict__ state, const int32_t *__restrict__ dist,
                                                     const int32_t *__restrict__ fhdr, const int3 s, float radius, int k, int n_goals,
                                                     int max_targets, const int32_t *__restrict__ frontier_hdr, int frontier_max_clusters,
@@ -166,7 +195,7 @@ __global__ void __launch_bounds__(32) k_reach_start(const DsmFieldGrid g, const 
     if (u >= 0)
     {
         const int x = u % g.n[0], y = u / g.n[0] % g.n[1], z = u / (g.n[0] * g.n[1]);
-        const int t = ((z / RC_T) * tn.y + y / RC_T) * tn.x + x / RC_T;
+        const int t = ((z / TZ) * tn.y + y / TY) * tn.x + x / TX;
         sched0[0] = t;
         stamp[t] = 0;
     }
@@ -189,12 +218,14 @@ __global__ void __launch_bounds__(RC_BLOCK) k_reach_init(const uint8_t *__restri
     if (threadIdx.x == 0 && n > 0) atomicAdd(&hdr[DSM_REACH_N_TRAVERSABLE], n);
 }
 
+template <int TX, int TY, int TZ>
 __global__ void __launch_bounds__(RC_TILE) k_reach_round(const DsmFieldGrid g, const int3 tn, const uint8_t *__restrict__ trav,
                                                          const uint32_t *__restrict__ cin, uint32_t *__restrict__ cout,
                                                          const int32_t *__restrict__ sched_in, int32_t *__restrict__ sched_out,
                                                          int32_t *__restrict__ stamp, int32_t *count, int32_t *hdr, int r)
 {
-    __shared__ uint32_t s[RC_H * RC_H * RC_H];
+    typedef ReachTile<TX, TY, TZ> T;
+    __shared__ uint32_t s[T::HALO];
     const int n = count[r % 3];
     if (blockIdx.x == 0 && threadIdx.x == 0)
     {
@@ -202,32 +233,32 @@ __global__ void __launch_bounds__(RC_TILE) k_reach_round(const DsmFieldGrid g, c
         if (n > 0) hdr[DSM_REACH_ROUNDS] = r + 1;
     }
     if (n == 0) return;
-    const int t = threadIdx.x, lx = t % RC_T, ly = t / RC_T % RC_T, lz = t / (RC_T * RC_T);
-    const int si = ((lz + 1) * RC_H + ly + 1) * RC_H + lx + 1;
+    const int t = threadIdx.x, lx = t % TX, ly = t / TX % TY, lz = t / (TX * TY);
+    const int si = ((lz + T::DZ) * T::HY + ly + 1) * T::HX + lx + 1;
     volatile uint32_t *vs = s;
     for (int q = blockIdx.x; q < n; q += gridDim.x)
     {
         const int tile = sched_in[q];
         const int tx = tile % tn.x, ty = tile / tn.x % tn.y, tz = tile / (tn.x * tn.y);
-        const int x0 = tx * RC_T - 1, y0 = ty * RC_T - 1, z0 = tz * RC_T - 1;
-        for (int h = t; h < RC_H * RC_H * RC_H; h += RC_TILE)
+        const int x0 = tx * TX - 1, y0 = ty * TY - 1, z0 = tz * TZ - T::DZ;
+        for (int h = t; h < T::HALO; h += RC_TILE)
         {
-            const int x = x0 + h % RC_H, y = y0 + h / RC_H % RC_H, z = z0 + h / (RC_H * RC_H);
+            const int x = x0 + h % T::HX, y = y0 + h / T::HX % T::HY, z = z0 + h / (T::HX * T::HY);
             s[h] = reach_inside(g, x, y, z) ? cin[reach_index(g, x, y, z)] : RC_INF;
         }
-        const int x = x0 + 1 + lx, y = y0 + 1 + ly, z = z0 + 1 + lz;
+        const int x = x0 + 1 + lx, y = y0 + 1 + ly, z = z0 + T::DZ + lz;
         const bool inside = reach_inside(g, x, y, z);
         const int i = inside ? reach_index(g, x, y, z) : 0;
         const bool tv = inside && trav[i];
         __syncthreads();
         const uint32_t c0 = s[si];
-        const uint32_t c = reach_relax(vs, si, tv, c0);
+        const uint32_t c = reach_relax<TX, TY, TZ>(vs, si, tv, c0);
         if (inside) cout[i] = c;
         // round 0's only tile holds the seeded start: it counts as changed even when none of its other voxels is reached,
         // or a start cut off from the rest of its tile would end the job after one round
-        if ((__syncthreads_or(c != c0) || r == 0) && t < 27)
+        if ((__syncthreads_or(c != c0) || r == 0) && t < T::NB)
         {
-            const int ax = tx + t % 3 - 1, ay = ty + t / 3 % 3 - 1, az = tz + t / 9 - 1;
+            const int ax = tx + t % 3 - 1, ay = ty + t / 3 % 3 - 1, az = tz + t / 9 - T::DZ;
             if ((unsigned)ax < (unsigned)tn.x && (unsigned)ay < (unsigned)tn.y && (unsigned)az < (unsigned)tn.z)
             {
                 const int a = (az * tn.y + ay) * tn.x + ax;
@@ -238,15 +269,16 @@ __global__ void __launch_bounds__(RC_TILE) k_reach_round(const DsmFieldGrid g, c
     }
 }
 
+template <int TX, int TY, int TZ>
 __global__ void __launch_bounds__(RC_TILE) k_reach_settle(const DsmFieldGrid g, const int3 tn, const uint32_t *__restrict__ src,
                                                           uint32_t *__restrict__ dst, const int32_t *__restrict__ sched, const int32_t *count, int r)
 {
     const int n = count[r % 3];
-    const int t = threadIdx.x, lx = t % RC_T, ly = t / RC_T % RC_T, lz = t / (RC_T * RC_T);
+    const int t = threadIdx.x, lx = t % TX, ly = t / TX % TY, lz = t / (TX * TY);
     for (int q = blockIdx.x; q < n; q += gridDim.x)
     {
         const int tile = sched[q];
-        const int x = tile % tn.x * RC_T + lx, y = tile / tn.x % tn.y * RC_T + ly, z = tile / (tn.x * tn.y) * RC_T + lz;
+        const int x = tile % tn.x * TX + lx, y = tile / tn.x % tn.y * TY + ly, z = tile / (tn.x * tn.y) * TZ + lz;
         if (reach_inside(g, x, y, z))
         {
             const int i = reach_index(g, x, y, z);
@@ -283,8 +315,22 @@ __device__ __forceinline__ unsigned long long reach_window(const DsmFieldGrid &g
     return warp_min64(key);
 }
 
-template <int PASS>
-__global__ void __launch_bounds__(RC_BLOCK) k_reach_targets(const DsmFieldGrid g, const uint8_t *__restrict__ trav, const uint32_t *__restrict__ cost,
+// A field voxel's target coordinates: the voxel itself on the field grid, the cell of its column on the terrain plane;
+// reach_cell that cell's index
+__device__ __forceinline__ int3 reach_member(const DsmFieldGrid &g, int v) { return make_int3(v % g.n[0], v / g.n[0] % g.n[1], v / (g.n[0] * g.n[1])); }
+__device__ __forceinline__ int3 reach_member(const ReachTerrainGrid &g, int v)
+{
+    const int x = v % g.nf[0], y = v / g.nf[0] % g.nf[1], z = v / (g.nf[0] * g.nf[1]);
+    return make_int3(g.h0 == 0 ? x : y, g.h1 == 1 ? y : z, 0); // h0 is 0 or 1, h1 is 1 or 2
+}
+__device__ __forceinline__ int reach_cell(const ReachTerrainGrid &g, int v)
+{
+    const int3 c = reach_member(g, v);
+    return c.y * g.n[0] + c.x;
+}
+
+template <int PASS, typename Grid>
+__global__ void __launch_bounds__(RC_BLOCK) k_reach_targets(const Grid g, const uint8_t *__restrict__ trav, const uint32_t *__restrict__ cost,
                                                             const int32_t *__restrict__ goals, const int32_t *__restrict__ fhdr,
                                                             const dsm_frontier_cluster_t *__restrict__ table, const int32_t *__restrict__ list,
                                                             int k, const int32_t *__restrict__ hdr, unsigned long long *best, int32_t *member)
@@ -310,7 +356,8 @@ __global__ void __launch_bounds__(RC_BLOCK) k_reach_targets(const DsmFieldGrid g
             if (c < 0) continue; // a member of a cluster past max_targets
             tg = n_goals + c;
             gi = list[j];
-            gx = gi % g.n[0], gy = gi / g.n[0] % g.n[1], gz = gi / (g.n[0] * g.n[1]);
+            const int3 m = reach_member(g, gi);
+            gx = m.x, gy = m.y, gz = m.z;
         }
         const unsigned long long key = reach_window(g, trav, cost, gx, gy, gz, k, lane);
         if (lane != 0 || key == ~0ull) continue;
@@ -321,7 +368,8 @@ __global__ void __launch_bounds__(RC_BLOCK) k_reach_targets(const DsmFieldGrid g
     }
 }
 
-__global__ void __launch_bounds__(RC_BLOCK) k_reach_records(const DsmFieldGrid g, const uint32_t *__restrict__ cost, const int32_t *__restrict__ goals,
+template <typename Grid>
+__global__ void __launch_bounds__(RC_BLOCK) k_reach_records(const Grid g, const uint32_t *__restrict__ cost, const int32_t *__restrict__ goals,
                                                             const dsm_frontier_cluster_t *__restrict__ table, const unsigned long long *__restrict__ best,
                                                             const int32_t *__restrict__ member, const int32_t *__restrict__ hdr,
                                                             dsm_reach_target_t *__restrict__ out)
@@ -344,6 +392,7 @@ __global__ void __launch_bounds__(RC_BLOCK) k_reach_records(const DsmFieldGrid g
         const dsm_frontier_cluster_t &c = table[t - n_goals];
         status = c.offset < 0 ? 3 : b == ~0ull ? 2 : 0;
         r.target = status == 0 ? member[t] : c.first;
+        if constexpr (std::is_same<Grid, ReachTerrainGrid>::value) r.target = reach_cell(g, r.target);
     }
     const int u = (int)(unsigned)b;
     r.cost = status == 0 ? (uint32_t)(b >> 32) : RC_INF;
@@ -426,12 +475,12 @@ __global__ void __launch_bounds__(RC_BLOCK) k_reach_paths(const DsmFieldGrid g, 
 
 static unsigned rc_blocks(long long n) { return n > 0 ? (unsigned)((n + RC_BLOCK - 1) / RC_BLOCK) : 1u; }
 
-// the persistent CTAs of k_reach_round on this device
-static int reach_ctas()
+// the persistent CTAs of a round kernel on this device
+static int reach_ctas(const void *round)
 {
     int dev = 0, sms = 0, per = 0;
     if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess ||
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per, k_reach_round, RC_TILE, 0) != cudaSuccess)
+        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per, round, RC_TILE, 0) != cudaSuccess)
         return 0;
     return sms * per;
 }
@@ -463,7 +512,8 @@ extern "C" int dsm_reach_enable(dsm_ctx *ctx, int max_targets, int max_path_voxe
     for (int k = 0; k < 3; k++) b.tn[k] = (f->g.n[k] + DSM_REACH_TILE - 1) / DSM_REACH_TILE;
     b.tiles = b.tn[0] * b.tn[1] * b.tn[2];
     b.max_targets = max_targets, b.max_path = max_path_voxels, b.max_rounds = max_rounds;
-    b.ctas = reach_ctas();
+    b.ctas = reach_ctas((const void *)k_reach_round<RC_T, RC_T, RC_T>);
+    b.ctas_flat = reach_ctas((const void *)k_reach_round<RC_FLAT_X, RC_FLAT_Y, 1>);
     const size_t tg = (size_t)std::max(max_targets, 1);
     const size_t res = reach_res_bytes(b);
     CudaOwner &o = re->own;
@@ -483,7 +533,7 @@ extern "C" int dsm_reach_enable(dsm_ctx *ctx, int max_targets, int max_path_voxe
     o.event(&re->ev);
     b.temp_bytes = reach_temp_bytes(b);
     if (b.temp_bytes) o.device(reinterpret_cast<uint8_t **>(&b.temp), b.temp_bytes);
-    return keep(ctx->reach, re, b.ctas > 0 && b.temp_bytes != 0);
+    return keep(ctx->reach, re, b.ctas > 0 && b.ctas_flat > 0 && b.temp_bytes != 0);
 }
 
 // floor(p / (double)v) - o, clamped to [-1, n]: outside the grid stays outside
@@ -491,6 +541,73 @@ static int reach_voxel(double p, float v, int o, int n)
 {
     const double q = std::floor(p / (double)v) - (double)o;
     return q < 0.0 ? -1 : q >= (double)n ? n : (int)q;
+}
+
+// the argument checks both enqueues share (include/dsm.h)
+static bool reach_args_ok(const DsmReach &b, const double start[3], float radius, int approach, const double *goals, int n_goals)
+{
+    if (!start || !std::isfinite(radius) || !(radius >= 0.f) || approach < 0 || approach > DSM_REACH_MAX_APPROACH || n_goals < 0 ||
+        n_goals > b.max_targets || (n_goals > 0 && !goals))
+        return false;
+    for (int k = 0; k < 3; k++)
+        if (!std::isfinite(start[k])) return false;
+    for (size_t i = 0; i < 3 * (size_t)n_goals; i++)
+        if (!std::isfinite(goals[i])) return false;
+    return true;
+}
+
+// The job on grid g of `cells` voxels cut into tiles of TX x TY x TZ (tn per axis, `tiles` in all, rounds on `ctas`
+// persistent CTAs), over the traversable test of (state, dist) and with the field error words of fhdr, from start voxel
+// s to the goal voxels already staged in b.goals and, with fr, the clusters of that frontier job; then the D2H copy of
+// the cost grid with host_copy.  The enqueue submits the result.
+template <int TX, int TY, int TZ, typename Grid>
+static int reach_launch(dsm_ctx *ctx, DsmReach &b, const Grid &g, const int3 tn, int tiles, int ctas, int cells, const uint8_t *state,
+                        const int32_t *dist, const int32_t *fhdr, const int3 s, float radius, int approach, int n_goals,
+                        const DsmFrontier *fr, int host_copy)
+{
+    const cudaStream_t st = ctx->stream;
+    const bool with_frontiers = fr != nullptr;
+    CK(cudaMemsetAsync(b.res, 0, 4 * DSM_REACH_WORDS, st));
+    int32_t *hdr = reinterpret_cast<int32_t *>(b.res);
+    auto *rec = reinterpret_cast<dsm_reach_target_t *>(b.res + 4 * DSM_REACH_WORDS);
+    int32_t *path = reinterpret_cast<int32_t *>(b.res + reach_path_at(b));
+    // the frontier job's result, with frontiers
+    const int32_t *frontier_hdr = with_frontiers ? reinterpret_cast<const int32_t *>(fr->res) : nullptr;
+    const auto *table = with_frontiers ? reinterpret_cast<const dsm_frontier_cluster_t *>(fr->res + DsmFrontier::table_at()) : nullptr;
+    const int32_t *list = with_frontiers ? reinterpret_cast<const int32_t *>(fr->res + fr->list_at()) : nullptr;
+    const int frontier_max_clusters = with_frontiers ? fr->max_clusters : 0;
+    CK(cudaMemsetAsync(b.stamp, 0xff, 4 * (size_t)tiles, st));
+    if (b.max_targets > 0) CK(cudaMemsetAsync(b.best, 0xff, 8 * (size_t)b.max_targets, st));
+    if (b.max_targets > 0) CK(cudaMemsetAsync(b.member, 0x7f, 4 * (size_t)b.max_targets, st));
+    k_reach_start<TX, TY, TZ><<<1, 32, 0, st>>>(g, state, dist, fhdr, s, radius, approach, n_goals, b.max_targets, frontier_hdr,
+                                                frontier_max_clusters, tn, b.sched[0], b.stamp, b.count, hdr);
+    k_reach_init<<<rc_blocks(cells), RC_BLOCK, 0, st>>>(state, dist, cells, radius, b.trav, b.cost[0], b.cost[1], hdr);
+    for (int r = 0; r < b.max_rounds; r++)
+        k_reach_round<TX, TY, TZ><<<ctas, RC_TILE, 0, st>>>(g, tn, b.trav, b.cost[r % 2], b.cost[(r + 1) % 2], b.sched[r % 2],
+                                                            b.sched[(r + 1) % 2], b.stamp, b.count, hdr, r);
+    const int r = b.max_rounds;
+    k_reach_settle<TX, TY, TZ><<<ctas, RC_TILE, 0, st>>>(g, tn, b.cost[r % 2], b.cost[(r + 1) % 2], b.sched[r % 2], b.count, r);
+    k_reach_reached<<<rc_blocks(cells), RC_BLOCK, 0, st>>>(b.cost[0], cells, b.count, r, hdr);
+    CK(cudaGetLastError());
+    if (b.max_targets > 0)
+    {
+        const unsigned warp_blocks = 2 * (unsigned)ctas; // the target and path kernels' warps walk their work
+        k_reach_targets<0><<<warp_blocks, RC_BLOCK, 0, st>>>(g, b.trav, b.cost[0], b.goals, frontier_hdr, table, list, approach, hdr, b.best,
+                                                             b.member);
+        if (with_frontiers)
+            k_reach_targets<1><<<warp_blocks, RC_BLOCK, 0, st>>>(g, b.trav, b.cost[0], b.goals, frontier_hdr, table, list, approach, hdr,
+                                                                 b.best, b.member);
+        k_reach_records<<<rc_blocks(b.max_targets), RC_BLOCK, 0, st>>>(g, b.cost[0], b.goals, table, b.best, b.member, hdr, rec);
+        k_reach_paths<false><<<warp_blocks, RC_BLOCK, 0, st>>>(g, b.trav, b.cost[0], b.max_targets, b.max_path, b.len, b.ofs, rec, path, hdr);
+        CK(cudaGetLastError());
+        size_t n = b.temp_bytes;
+        CK(cub::DeviceScan::ExclusiveSum(b.temp, n, b.len, b.ofs, b.max_targets, st));
+        k_reach_paths<true><<<warp_blocks, RC_BLOCK, 0, st>>>(g, b.trav, b.cost[0], b.max_targets, b.max_path, b.len, b.ofs, rec, path, hdr);
+        CK(cudaGetLastError());
+    }
+    if (host_copy) CK(cudaMemcpyAsync(b.cost_host, b.cost[0], 4 * (size_t)cells, cudaMemcpyDeviceToHost, st));
+    b.host_copy = host_copy != 0;
+    return DSM_OK;
 }
 
 // Enqueue only: the goal voxels staged and copied, the job on the grids of the latest (known) field request and, with
@@ -506,63 +623,65 @@ extern "C" int dsm_reach_enqueue(dsm_ctx *ctx, const double start[3], float radi
     const DsmFrontier *fr = ctx->frontier.get();
     if (with_frontiers && !read_latest(fr, f)) return DSM_E_STATE;
     DsmReach &b = *re;
-    if (!start || !std::isfinite(radius) || !(radius >= 0.f) || approach < 0 || approach > DSM_REACH_MAX_APPROACH || n_goals < 0 ||
-        n_goals > b.max_targets || (n_goals > 0 && !goals))
-        return DSM_E_INVALID;
-    for (int k = 0; k < 3; k++)
-        if (!std::isfinite(start[k])) return DSM_E_INVALID;
-    for (size_t i = 0; i < 3 * (size_t)n_goals; i++)
-        if (!std::isfinite(goals[i])) return DSM_E_INVALID;
+    if (!reach_args_ok(b, start, radius, approach, goals, n_goals)) return DSM_E_INVALID;
     const DsmFieldGrid &g = f->g;
-    const cudaStream_t st = ctx->stream;
     CK(cudaSetDevice(ctx->device));
     // the previous job's copy out of this staging ended before its wait, which no job in flight implies
     for (size_t i = 0; i < 3 * (size_t)n_goals; i++) re->goals_host[i] = reach_voxel(goals[i], g.voxel, g.o[i % 3], g.n[i % 3]);
-    if (n_goals > 0) CK(cudaMemcpyAsync(b.goals, re->goals_host, 12 * (size_t)n_goals, cudaMemcpyHostToDevice, st));
+    if (n_goals > 0) CK(cudaMemcpyAsync(b.goals, re->goals_host, 12 * (size_t)n_goals, cudaMemcpyHostToDevice, ctx->stream));
     const int3 s = make_int3(reach_voxel(start[0], g.voxel, g.o[0], g.n[0]), reach_voxel(start[1], g.voxel, g.o[1], g.n[1]),
                              reach_voxel(start[2], g.voxel, g.o[2], g.n[2]));
-    CK(cudaMemsetAsync(b.res, 0, 4 * DSM_REACH_WORDS, st));
-    int32_t *hdr = reinterpret_cast<int32_t *>(b.res);
-    auto *rec = reinterpret_cast<dsm_reach_target_t *>(b.res + 4 * DSM_REACH_WORDS);
-    int32_t *path = reinterpret_cast<int32_t *>(b.res + reach_path_at(b));
-    // the frontier job's result, with frontiers
-    const int32_t *fhdr = with_frontiers ? reinterpret_cast<const int32_t *>(fr->res) : nullptr;
-    const auto *table = with_frontiers ? reinterpret_cast<const dsm_frontier_cluster_t *>(fr->res + DsmFrontier::table_at()) : nullptr;
-    const int32_t *list = with_frontiers ? reinterpret_cast<const int32_t *>(fr->res + fr->list_at()) : nullptr;
-    const int frontier_max_clusters = with_frontiers ? fr->max_clusters : 0;
-    const uint8_t *state = f->occ;
-    const int32_t *dist = f->dist;
     const int3 tn = make_int3(b.tn[0], b.tn[1], b.tn[2]);
-    CK(cudaMemsetAsync(b.stamp, 0xff, 4 * (size_t)b.tiles, st));
-    if (b.max_targets > 0) CK(cudaMemsetAsync(b.best, 0xff, 8 * (size_t)b.max_targets, st));
-    if (b.max_targets > 0) CK(cudaMemsetAsync(b.member, 0x7f, 4 * (size_t)b.max_targets, st));
-    k_reach_start<<<1, 32, 0, st>>>(g, state, dist, dist + dsm_field_header(f->voxels), s, radius, approach, n_goals, b.max_targets, fhdr,
-                                    frontier_max_clusters, tn, b.sched[0], b.stamp, b.count, hdr);
-    k_reach_init<<<rc_blocks(b.voxels), RC_BLOCK, 0, st>>>(state, dist, b.voxels, radius, b.trav, b.cost[0], b.cost[1], hdr);
-    for (int r = 0; r < b.max_rounds; r++)
-        k_reach_round<<<b.ctas, RC_TILE, 0, st>>>(g, tn, b.trav, b.cost[r % 2], b.cost[(r + 1) % 2], b.sched[r % 2], b.sched[(r + 1) % 2],
-                                                  b.stamp, b.count, hdr, r);
-    const int r = b.max_rounds;
-    k_reach_settle<<<b.ctas, RC_TILE, 0, st>>>(g, tn, b.cost[r % 2], b.cost[(r + 1) % 2], b.sched[r % 2], b.count, r);
-    k_reach_reached<<<rc_blocks(b.voxels), RC_BLOCK, 0, st>>>(b.cost[0], b.voxels, b.count, r, hdr);
-    CK(cudaGetLastError());
-    if (b.max_targets > 0)
-    {
-        const unsigned warp_blocks = 2 * (unsigned)b.ctas; // the target and path kernels' warps walk their work
-        k_reach_targets<0><<<warp_blocks, RC_BLOCK, 0, st>>>(g, b.trav, b.cost[0], b.goals, fhdr, table, list, approach, hdr, b.best, b.member);
-        if (with_frontiers)
-            k_reach_targets<1><<<warp_blocks, RC_BLOCK, 0, st>>>(g, b.trav, b.cost[0], b.goals, fhdr, table, list, approach, hdr, b.best, b.member);
-        k_reach_records<<<rc_blocks(b.max_targets), RC_BLOCK, 0, st>>>(g, b.cost[0], b.goals, table, b.best, b.member, hdr, rec);
-        k_reach_paths<false><<<warp_blocks, RC_BLOCK, 0, st>>>(g, b.trav, b.cost[0], b.max_targets, b.max_path, b.len, b.ofs, rec, path, hdr);
-        CK(cudaGetLastError());
-        size_t n = b.temp_bytes;
-        CK(cub::DeviceScan::ExclusiveSum(b.temp, n, b.len, b.ofs, b.max_targets, st));
-        k_reach_paths<true><<<warp_blocks, RC_BLOCK, 0, st>>>(g, b.trav, b.cost[0], b.max_targets, b.max_path, b.len, b.ofs, rec, path, hdr);
-        CK(cudaGetLastError());
-    }
-    if (host_copy) CK(cudaMemcpyAsync(re->cost_host, b.cost[0], 4 * (size_t)b.voxels, cudaMemcpyDeviceToHost, st));
-    re->host_copy = host_copy != 0;
+    const int rc = reach_launch<RC_T, RC_T, RC_T>(ctx, b, g, tn, b.tiles, b.ctas, b.voxels, f->occ, f->dist, f->dist + dsm_field_header(f->voxels),
+                                                  s, radius, approach, n_goals, with_frontiers ? fr : nullptr, host_copy);
+    if (rc != DSM_OK) return rc;
     return submit(ctx, *re, b.res, reach_res_bytes(b), f->requests);
+}
+
+// Enqueue only: the job of dsm_reach_enqueue on the plane of the latest terrain job (DESIGN.md §8.21), the points'
+// columns staged as cells of that plane, in stream order behind that job.  A later terrain, field or frontier request
+// overwrites what the job reads only behind it.  The job pairs with no field request (request 0), so a viewpoint job
+// never reads its cost grid as a field's.
+extern "C" int dsm_reach_enqueue_terrain(dsm_ctx *ctx, const double start[3], float radius, int approach, const double *goals, int n_goals,
+                                         int with_frontiers, int host_copy)
+{
+    if (!ctx) return DSM_E_INVALID;
+    DsmReach *re = ctx->reach.get();
+    const DsmTerrain *tr = ctx->terrain.get();
+    if (!re || !tr || tr->request == 0 || re->in_flight) return DSM_E_STATE;
+    const DsmFrontier *fr = ctx->frontier.get();
+    if (with_frontiers && !(fr && fr->request == tr->request)) return DSM_E_STATE;
+    DsmReach &b = *re;
+    if (!reach_args_ok(b, start, radius, approach, goals, n_goals)) return DSM_E_INVALID;
+    const DsmFieldGrid &fg = ctx->field->g;
+    const int a = std::abs(tr->up) - 1, h0 = a == 0 ? 1 : 0, h1 = a == 2 ? 1 : 2;
+    ReachTerrainGrid g;
+    static_cast<DsmFieldGrid &>(g) = fg;
+    for (int k = 0; k < 3; k++) g.o[k] = tr->origin[k], g.nf[k] = fg.n[k];
+    g.n[0] = fg.n[h0], g.n[1] = fg.n[h1], g.n[2] = 1;
+    g.h0 = h0, g.h1 = h1;
+    const int cells = tr->cells;
+    CK(cudaSetDevice(ctx->device));
+    // a point's column: its two in-plane voxel coordinates, whatever its height
+    auto cell = [&](const double *p, int32_t *out) {
+        out[0] = reach_voxel(p[h0], fg.voxel, g.o[h0], g.n[0]);
+        out[1] = reach_voxel(p[h1], fg.voxel, g.o[h1], g.n[1]);
+        out[2] = 0;
+    };
+    // the previous job's copy out of this staging ended before its wait, which no job in flight implies
+    for (int i = 0; i < n_goals; i++) cell(goals + 3 * i, re->goals_host + 3 * i);
+    if (n_goals > 0) CK(cudaMemcpyAsync(b.goals, re->goals_host, 12 * (size_t)n_goals, cudaMemcpyHostToDevice, ctx->stream));
+    int32_t sc[3];
+    cell(start, sc);
+    const int3 s = make_int3(sc[0], sc[1], sc[2]);
+    const int3 tn = make_int3((g.n[0] + RC_FLAT_X - 1) / RC_FLAT_X, (g.n[1] + RC_FLAT_Y - 1) / RC_FLAT_Y, 1);
+    const uint8_t *status = tr->res + DsmTerrain::status_at(cells);
+    const int32_t *clearance = reinterpret_cast<const int32_t *>(tr->res);
+    const int32_t *thdr = reinterpret_cast<const int32_t *>(tr->res + DsmTerrain::header_at(cells));
+    const int rc = reach_launch<RC_FLAT_X, RC_FLAT_Y, 1>(ctx, b, g, tn, tn.x * tn.y, b.ctas_flat, cells, status, clearance, thdr, s, radius,
+                                                         approach, n_goals, with_frontiers ? fr : nullptr, host_copy);
+    if (rc != DSM_OK) return rc;
+    return submit(ctx, *re, b.res, reach_res_bytes(b), 0);
 }
 
 extern "C" int dsm_reach_wait(dsm_ctx *ctx, dsm_reach_info_t *info, const dsm_reach_target_t **targets, const int32_t **path,
@@ -782,7 +901,7 @@ __global__ void __launch_bounds__(RC_TILE) k_rm_round(const int3 tn, int n_sites
         const bool tv = (mask[(size_t)tile * RM_WORDS + t / 32] >> (t % 32)) & 1u;
         __syncthreads();
         const uint32_t c0 = s[si];
-        const uint32_t c = reach_relax(vs, si, tv, c0);
+        const uint32_t c = reach_relax<RC_T, RC_T, RC_T>(vs, si, tv, c0);
         cout[(row + a) * RC_TILE + t] = c;
         // as k_reach_round, round 0's tile is the seeded start's and counts as changed; only active tiles are listed,
         // since an inactive one holds UINT32_MAX for good

@@ -17,13 +17,12 @@
 // The kernels carry no error gate and are launched without PDL, as the other field kernels.  The job's C ABI calls
 // (dsm_terrain_enable, _enqueue and _wait) follow them.
 //
-// One packed result (D2H), for C cells:
-//   float clearance[C] | pad to dsm_field_header(C) words | int32 header[8] (a field header's words, dsm_device.cuh) |
-//   int16 level[C] | uint8 status[C] | uint8 step[C]
+// One packed result (D2H), its layout in DsmTerrain (dsm_ctx.hpp); the terrain reach job (dsm_reach.cu) reads its status
+// and clearance planes and its header on the device.
 #include "dsm_ctx.hpp"
 
 #define TERRAIN_BLOCK 256
-#define TERRAIN_HEADER_WORDS 8
+#define TERRAIN_HEADER_WORDS DsmTerrain::HEADER_WORDS
 
 static_assert(sizeof(dsm_terrain_info_t) == 64 && offsetof(dsm_terrain_info_t, n_support) == 36, "dsm_terrain_info_t layout");
 static_assert(DSM_FIELD_WORDS <= TERRAIN_HEADER_WORDS, "the terrain header holds a field header");
@@ -83,12 +82,6 @@ __global__ void __launch_bounds__(TERRAIN_BLOCK) k_terrain_step(const int16_t *_
 }
 
 static unsigned tr_blocks(int n) { return (unsigned)((n + TERRAIN_BLOCK - 1) / TERRAIN_BLOCK); }
-// byte offsets of the result's sections
-static size_t tr_header_at(int cells) { return 4 * dsm_field_header((size_t)cells); }
-static size_t tr_level_at(int cells) { return tr_header_at(cells) + 4 * TERRAIN_HEADER_WORDS; }
-static size_t tr_status_at(int cells) { return tr_level_at(cells) + 2 * (size_t)cells; }
-static size_t tr_step_at(int cells) { return tr_status_at(cells) + (size_t)cells; }
-static size_t tr_res_bytes(int cells) { return tr_step_at(cells) + (size_t)cells; }
 
 extern "C" int dsm_terrain_enable(dsm_ctx *ctx, int up)
 {
@@ -101,7 +94,7 @@ extern "C" int dsm_terrain_enable(dsm_ctx *ctx, int up)
     tr->up = up;
     for (int k = 0; k < 3; k++) tr->m[k] = k == std::abs(up) - 1 ? 1 : f->g.n[k];
     tr->cells = tr->m[0] * tr->m[1] * tr->m[2];
-    const size_t res = tr_res_bytes(tr->cells);
+    const size_t res = DsmTerrain::res_bytes(tr->cells);
     tr->own.device(&tr->res, res);
     tr->own.host(&tr->res_host, res);
     tr->own.event(&tr->ev);
@@ -122,9 +115,9 @@ extern "C" int dsm_terrain_enqueue(dsm_ctx *ctx, int headroom, int max_step)
     const cudaStream_t s = ctx->stream;
     const int C = tr->cells, *n = f->g.n, *m = tr->m;
     int32_t *dist = reinterpret_cast<int32_t *>(tr->res);
-    int32_t *hdr = reinterpret_cast<int32_t *>(tr->res + tr_header_at(C));
-    int16_t *level = reinterpret_cast<int16_t *>(tr->res + tr_level_at(C));
-    uint8_t *status = tr->res + tr_status_at(C), *step = tr->res + tr_step_at(C);
+    int32_t *hdr = reinterpret_cast<int32_t *>(tr->res + DsmTerrain::header_at(C));
+    int16_t *level = reinterpret_cast<int16_t *>(tr->res + DsmTerrain::level_at(C));
+    uint8_t *status = tr->res + DsmTerrain::status_at(C), *step = tr->res + DsmTerrain::step_at(C);
     const int strides[3] = {1, n[0], n[0] * n[1]}, cstrides[3] = {1, m[0], m[0] * m[1]};
     const int h0 = a == 0 ? 1 : 0, h1 = a == 2 ? 1 : 2;
     CK(cudaMemsetAsync(hdr, 0, 4 * TERRAIN_HEADER_WORDS, s));
@@ -138,7 +131,7 @@ extern "C" int dsm_terrain_enqueue(dsm_ctx *ctx, int headroom, int max_step)
     CK(cudaGetLastError());
     for (int k = 0; k < 3; k++) tr->origin[k] = f->g.o[k];
     tr->headroom = headroom, tr->max_step = max_step;
-    return submit(ctx, *tr, tr->res, tr_res_bytes(C), f->requests);
+    return submit(ctx, *tr, tr->res, DsmTerrain::res_bytes(C), f->requests);
 }
 
 extern "C" int dsm_terrain_wait(dsm_ctx *ctx, dsm_terrain_info_t *info, const int16_t **level, const uint8_t **status, const uint8_t **step,
@@ -149,7 +142,7 @@ extern "C" int dsm_terrain_wait(dsm_ctx *ctx, dsm_terrain_info_t *info, const in
     const int rc = wait_head(ctx, tr);
     if (rc != DSM_OK) return rc;
     const int C = tr->cells;
-    const int32_t *h = reinterpret_cast<const int32_t *>(tr->res_host + tr_header_at(C));
+    const int32_t *h = reinterpret_cast<const int32_t *>(tr->res_host + DsmTerrain::header_at(C));
     if (info)
     {
         *info = dsm_terrain_info_t();
@@ -159,9 +152,9 @@ extern "C" int dsm_terrain_wait(dsm_ctx *ctx, dsm_terrain_info_t *info, const in
         info->n_traversable = h[DSM_FIELD_N_FREE];
         info->n_support = info->n_blocked + info->n_traversable;
     }
-    if (level) *level = reinterpret_cast<const int16_t *>(tr->res_host + tr_level_at(C));
-    if (status) *status = tr->res_host + tr_status_at(C);
-    if (step) *step = tr->res_host + tr_step_at(C);
+    if (level) *level = reinterpret_cast<const int16_t *>(tr->res_host + DsmTerrain::level_at(C));
+    if (status) *status = tr->res_host + DsmTerrain::status_at(C);
+    if (step) *step = tr->res_host + DsmTerrain::step_at(C);
     if (clearance) *clearance = reinterpret_cast<const float *>(tr->res_host);
     return capacity(ctx, h, DSM_FIELD_ERR_TAG, "dsm_terrain_wait", "the field the job read");
 }

@@ -908,6 +908,34 @@ int dsm_reach_enqueue(dsm_ctx *ctx, const double start[3], float radius, int app
 int dsm_reach_wait(dsm_ctx *ctx, dsm_reach_info_t *info, const dsm_reach_target_t **targets, const int32_t **path,
                    const uint32_t **cost);
 
+/* ---- driving paths on the terrain: the reach job on the latest terrain job's plane (DESIGN.md §8.21) ----
+ * A terrain reach job is the reach job above run on the grid of the latest terrain job (§8.20), in stream order behind
+ * that job, which may still be in flight; a later terrain, field or frontier request overwrites what it reads only behind
+ * it.  It uses the reach job's buffers, records, info and wait.  Everything not restated here is §8.11's, on that grid.
+ *   Grid: the terrain grid m (m[|up| - 1] = 1) at the terrain job's origin, voxel edge v.  Cells in the terrain planes'
+ *   linear order q P + p, P and Q the two in-plane extents, p and q the lower and higher in-plane axes; start_voxel,
+ *   target, viewpoint, the path list and the cost grid are cells.  The header's origin is the terrain job's.
+ *   Traversable: status 2 and clearance >= radius, dsm_traversable on the status and clearance planes.
+ *   Moves: the 8 in-plane moves, face 10 and diagonal 14, in units of v / 10.  The cost is horizontal travel only: every
+ *   traversable cell has step <= max_step, so no move between two of them climbs more than max_step voxels.
+ *   Start and goals: a point's voxel as in §8.11 with its up coordinate replaced by 0, so a point's column is where a
+ *   ground robot stands whatever its height; status 1 is decided by the two in-plane axes.  The window is a square.
+ *   Frontier targets: every member voxel of the latest frontier job stands for its column's cell; ties go to the lowest
+ *   member in the field's voxel order; a record's target is the cell of that member, or of the cluster's first voxel
+ *   for status 2 and 3.  Members sharing a column are allowed.
+ *   Rounds: tiles of 32 x 16 cells from cell (0, 0), 32 along p and 16 along q; a tile that changed schedules itself
+ *   and its 8 in-plane neighbours.  The round-0 rule, rounds and converged are §8.11's; a converged job is Dijkstra's on
+ *   the 8-connected graph.
+ *
+ *   dsm_reach_enqueue_terrain  as dsm_reach_enqueue.  DSM_E_STATE before dsm_reach_enable, with no terrain job yet,
+ *                              while a reach job is in flight, and with with_frontiers unless the latest frontier job
+ *                              read the field request the latest terrain job read.  DSM_E_INVALID exactly as
+ *                              dsm_reach_enqueue.  dsm_reach_wait's *cost then holds m0 m1 m2 cells, and it returns
+ *                              DSM_E_CAPACITY when the terrain job's field was taken after a rejected frame.  The job
+ *                              reads no field request, so a viewpoint job's with_reach refuses its cost grid. */
+int dsm_reach_enqueue_terrain(dsm_ctx *ctx, const double start[3], float radius, int approach, const double *goals, int n_goals,
+                              int with_frontiers, int host_copy);
+
 /* ---- travel costs between many sites: the cost matrix of an exploration tour (DESIGN.md §8.13) ----
  * A matrix job reads the state and distance grids of the latest field request, which must be a known one, in stream
  * order behind it, with that request's origin o and voxel edge v captured at the job's enqueue, as a reach job does.

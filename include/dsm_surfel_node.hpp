@@ -859,7 +859,36 @@ class SurfelMapNode
                        status.assign(s, s + n);
                        step.assign(t, t + n);
                        clearance.assign(c, c + n);
+                       terrain_frame_ = true;
                    });
+    }
+    // ---- driving paths on the terrain of the latest fused frame (DESIGN.md §8.21), after enable_reach ----
+    // reach() on the plane of the terrain() call on this frame: the travel cost from the column of `start` over the
+    // traversable cells at least `radius` from any other, to the columns of the goals (xyz doubles) and, with
+    // with_frontiers, to the clusters of the frontiers() call on this frame.  Cells, viewpoints and path entries are
+    // indices q P + p of the terrain grid; a cell's surface point lies on the level plane of terrain().  DSM_E_STATE
+    // without a terrain() call on this frame, with with_frontiers without a frontiers() call on it, and after
+    // load_state* until the next fused frame; DSM_E_CAPACITY with the paths of the last applied frame's terrain.
+    int reach_terrain(const double start[3], float radius, int approach, const std::vector<double> &goals, bool with_frontiers,
+                      dsm_reach_info_t &info, std::vector<dsm_reach_target_t> &targets, std::vector<int32_t> &path)
+    {
+        targets.clear();
+        path.clear();
+        info = dsm_reach_info_t();
+        const dsm_reach_target_t *t = nullptr;
+        const int32_t *p = nullptr;
+        return job(
+            "reach_terrain", KNOWN_FIELD, goals.size() % 3 == 0,
+            [&] {
+                return terrain_frame_ ? dsm_reach_enqueue_terrain(ctx_.ctx, start, radius, approach, goals.data(), (int)(goals.size() / 3),
+                                                                  with_frontiers, 0)
+                                      : DSM_E_STATE;
+            },
+            [&] { return dsm_reach_wait(ctx_.ctx, &info, &t, &p, nullptr); },
+            [&] {
+                targets.assign(t, t + std::min(info.n_targets, reach_targets_));
+                path.assign(p, p + info.n_path_voxels);
+            });
     }
     // the field of the latest fused frame: dist [nz][ny][nx] in metres (the library's pinned buffer, valid until the next
     // frame is fused; nullptr for a field kept on the device), the grid's origin in voxels and the occupied voxels.  DSM_E_STATE when no frame has been fused
@@ -1071,6 +1100,7 @@ class SurfelMapNode
         last_ref_ = s.last_ref;
         fused_ = s.fused;
         field_exists_ = false; // the loaded map has no field until its next fused frame
+        terrain_frame_ = false;
         // a version-2 section restores the slot table the library's views match; without one the table starts empty
         for (size_t i = 0; i < known_.size(); i++)
             known_[i] = s.views ? KnownView{s.view_ref[i], s.view_rel[i]} : KnownView{-1, Pose()};
@@ -1355,6 +1385,7 @@ class SurfelMapNode
             else
                 rc = field_host_copy_ ? dsm_field_enqueue(ctx_.ctx, c, 5) : dsm_field_enqueue_resident(ctx_.ctx, c, 5);
             field_ = ctx_.done(rc, "fuse") == DSM_OK;
+            terrain_frame_ = false; // a new field: terrain() has not run on it
             field_exists_ = field_exists_ || field_;
         }
         return publishing_ || distance_field_ ? ctx_.err : DSM_OK;
@@ -1426,6 +1457,7 @@ class SurfelMapNode
     bool distance_field_ = false, field_ = false; // enable_distance_field; a field is enqueued and not yet handed out
     bool field_host_copy_ = true;  // enable_distance_field's host_copy
     bool field_exists_ = false;    // a fused frame has enqueued a field: the queries have a grid to read
+    bool terrain_frame_ = false;   // terrain() has run on the latest fused frame's field: reach_terrain() has a plane
     // enable_known_space: per capture slot, the reference keyframe (-1: empty) and the pose relative to it
     struct KnownView
     {
