@@ -39,7 +39,7 @@ EXPORTS = [
     "dsm_frontier_enable", "dsm_frontier_enqueue", "dsm_frontier_wait", "dsm_debug_field_load_state",
     "dsm_field_signed_enable", "dsm_field_signed", "dsm_field_query_enqueue_signed",
     "dsm_reach_enable", "dsm_reach_enqueue", "dsm_reach_enqueue_terrain", "dsm_reach_wait", "dsm_reach_matrix_enable", "dsm_reach_matrix_enqueue",
-    "dsm_reach_matrix_wait", "dsm_gain_enable", "dsm_gain_enqueue", "dsm_gain_wait",
+    "dsm_reach_matrix_enqueue_terrain", "dsm_reach_matrix_wait", "dsm_gain_enable", "dsm_gain_enqueue", "dsm_gain_wait",
     "dsm_tour_enable", "dsm_tour_enqueue", "dsm_tour_wait", "dsm_viewpoint_enable", "dsm_viewpoint_enqueue", "dsm_viewpoint_wait",
     "dsm_trajectory_enable", "dsm_trajectory_enqueue", "dsm_trajectory_wait",
     "dsm_heading_enable", "dsm_heading_enqueue", "dsm_heading_wait",
@@ -227,6 +227,7 @@ def load_library():
     L.dsm_reach_wait.argtypes = [vp, vp, ctypes.POINTER(vp), ctypes.POINTER(vp), ctypes.POINTER(vp)]
     L.dsm_reach_matrix_enable.argtypes = [vp, ci, ci, ci]
     L.dsm_reach_matrix_enqueue.argtypes = [vp, vp, ci, ctypes.c_float, ci]
+    L.dsm_reach_matrix_enqueue_terrain.argtypes = [vp, vp, ci, ctypes.c_float, ci]
     L.dsm_reach_matrix_wait.argtypes = [vp, vp, ctypes.POINTER(vp), ctypes.POINTER(vp)]
     L.dsm_gain_enable.argtypes = [vp, ci]
     L.dsm_gain_enqueue.argtypes = [vp, ctypes.POINTER(DsmGainCamera), vp, vp, ci]
@@ -837,8 +838,16 @@ class Context:
 
     def reach_matrix_enqueue(self, points, radius, approach):
         """points: world points, an (n, 3) array-like of float64, n >= 1."""
+        self._reach_matrix_enqueue(self.lib.dsm_reach_matrix_enqueue, points, radius, approach)
+
+    def reach_matrix_enqueue_terrain(self, points, radius, approach):
+        """The matrix job on the plane of the latest terrain job (DESIGN.md §8.22), arguments as reach_matrix_enqueue's;
+        each point stands for its column, and the site voxels reach_matrix_wait returns are cells q P + p of that plane."""
+        self._reach_matrix_enqueue(self.lib.dsm_reach_matrix_enqueue_terrain, points, radius, approach)
+
+    def _reach_matrix_enqueue(self, call, points, radius, approach):
         p = np.ascontiguousarray(points, np.float64).reshape(-1, 3)
-        self._ck(self.lib.dsm_reach_matrix_enqueue(self.h, p.ctypes.data if len(p) else None, len(p), float(radius), int(approach)))
+        self._ck(call(self.h, p.ctypes.data if len(p) else None, len(p), float(radius), int(approach)))
 
     def reach_matrix_wait(self):
         """(info, sites, matrix): numpy copies of the context's pinned results, a REACH_MATRIX_INFO_DTYPE record,

@@ -315,11 +315,13 @@ struct DsmReach : DsmJob
 
 // dsm_reach_matrix_* (DESIGN.md §8.13), allocated by dsm_reach_matrix_enable for the field's grid: the job's device
 // buffers, the packed result (dsm_reach.cu) and the site staging.  Per (site, slot) the costs are a tile's 512 voxels in
-// tile-local order (x fastest), at ((size_t)site * max_tiles + slot) * 512 of each buffer.
+// tile-local order (x fastest), at ((size_t)site * max_tiles + slot) * 512 of each buffer.  A terrain job (§8.22) runs
+// in the same buffers: a 32 x 16 tile has 512 cells too, and its plane has no more of them than the field has 8^3 tiles.
 struct DsmReachMatrix : DsmJob
 {
     int voxels = 0, tiles = 0, tn[3] = {0, 0, 0};
-    int max_sites = 0, max_tiles = 0, max_rounds = 0, ctas = 0;
+    int max_sites = 0, max_tiles = 0, max_rounds = 0, ctas = 0; // ctas: the persistent CTAs of a round
+    int ctas_flat = 0;                            // those of a terrain job's round (dsm_reach_matrix_enqueue_terrain)
     int32_t *flag = nullptr, *scan = nullptr;     // [tiles]: the tile is active, and the exclusive sum of the flags
     int32_t *slot = nullptr;                      // [tiles]: the tile's slot, -1 when inactive
     uint32_t *mask = nullptr;                     // [tiles][16]: the tile's traversable voxels, bit t of word t / 32
@@ -331,7 +333,7 @@ struct DsmReachMatrix : DsmJob
     int32_t *rounds = nullptr, *reached = nullptr; // [max_sites]: the rounds with a non-empty schedule, the reached voxels
     int32_t *sites = nullptr;                     // device [max_sites][3] the points' voxels, staged from sites_host
     uint8_t *res = nullptr;                       // the packed result, room for max_sites
-    void *temp = nullptr;                         // CUB scratch of the tile scan
+    void *temp = nullptr;                         // CUB scratch of the tile scan, for the field's and every flat count
     size_t temp_bytes = 0;
     int32_t *sites_host = nullptr; // pinned [max_sites][3]
     int n_sites = 0; // of the job in flight or last waited for

@@ -543,6 +543,30 @@ static int reach_voxel(double p, float v, int o, int n)
     return q < 0.0 ? -1 : q >= (double)n ? n : (int)q;
 }
 
+// The plane of terrain job tr on field grid fg as a reach grid (DESIGN.md §8.21): the plane (P, Q, 1) of fg's two axes
+// h0 < h1 other than the up axis, at tr's origin
+static ReachTerrainGrid reach_terrain_grid(const DsmFieldGrid &fg, const DsmTerrain &tr)
+{
+    const int a = std::abs(tr.up) - 1;
+    ReachTerrainGrid g;
+    static_cast<DsmFieldGrid &>(g) = fg;
+    g.h0 = a == 0 ? 1 : 0, g.h1 = a == 2 ? 1 : 2;
+    for (int k = 0; k < 3; k++) g.o[k] = tr.origin[k], g.nf[k] = fg.n[k];
+    g.n[0] = fg.n[g.h0], g.n[1] = fg.n[g.h1], g.n[2] = 1;
+    return g;
+}
+
+// a point's column on that plane: its two in-plane voxel coordinates, whatever its height
+static void reach_terrain_cell(const ReachTerrainGrid &g, const double *p, int32_t out[3])
+{
+    out[0] = reach_voxel(p[g.h0], g.voxel, g.o[g.h0], g.n[0]);
+    out[1] = reach_voxel(p[g.h1], g.voxel, g.o[g.h1], g.n[1]);
+    out[2] = 0;
+}
+
+// the flat 32 x 16 tiles per axis of a plane of n0 x n1 cells
+static int3 reach_flat_tn(int n0, int n1) { return make_int3((n0 + RC_FLAT_X - 1) / RC_FLAT_X, (n1 + RC_FLAT_Y - 1) / RC_FLAT_Y, 1); }
+
 // the argument checks both enqueues share (include/dsm.h)
 static bool reach_args_ok(const DsmReach &b, const double start[3], float radius, int approach, const double *goals, int n_goals)
 {
@@ -653,28 +677,16 @@ extern "C" int dsm_reach_enqueue_terrain(dsm_ctx *ctx, const double start[3], fl
     if (with_frontiers && !(fr && fr->request == tr->request)) return DSM_E_STATE;
     DsmReach &b = *re;
     if (!reach_args_ok(b, start, radius, approach, goals, n_goals)) return DSM_E_INVALID;
-    const DsmFieldGrid &fg = ctx->field->g;
-    const int a = std::abs(tr->up) - 1, h0 = a == 0 ? 1 : 0, h1 = a == 2 ? 1 : 2;
-    ReachTerrainGrid g;
-    static_cast<DsmFieldGrid &>(g) = fg;
-    for (int k = 0; k < 3; k++) g.o[k] = tr->origin[k], g.nf[k] = fg.n[k];
-    g.n[0] = fg.n[h0], g.n[1] = fg.n[h1], g.n[2] = 1;
-    g.h0 = h0, g.h1 = h1;
+    const ReachTerrainGrid g = reach_terrain_grid(ctx->field->g, *tr);
     const int cells = tr->cells;
     CK(cudaSetDevice(ctx->device));
-    // a point's column: its two in-plane voxel coordinates, whatever its height
-    auto cell = [&](const double *p, int32_t *out) {
-        out[0] = reach_voxel(p[h0], fg.voxel, g.o[h0], g.n[0]);
-        out[1] = reach_voxel(p[h1], fg.voxel, g.o[h1], g.n[1]);
-        out[2] = 0;
-    };
     // the previous job's copy out of this staging ended before its wait, which no job in flight implies
-    for (int i = 0; i < n_goals; i++) cell(goals + 3 * i, re->goals_host + 3 * i);
+    for (int i = 0; i < n_goals; i++) reach_terrain_cell(g, goals + 3 * i, re->goals_host + 3 * i);
     if (n_goals > 0) CK(cudaMemcpyAsync(b.goals, re->goals_host, 12 * (size_t)n_goals, cudaMemcpyHostToDevice, ctx->stream));
     int32_t sc[3];
-    cell(start, sc);
+    reach_terrain_cell(g, start, sc);
     const int3 s = make_int3(sc[0], sc[1], sc[2]);
-    const int3 tn = make_int3((g.n[0] + RC_FLAT_X - 1) / RC_FLAT_X, (g.n[1] + RC_FLAT_Y - 1) / RC_FLAT_Y, 1);
+    const int3 tn = reach_flat_tn(g.n[0], g.n[1]);
     const uint8_t *status = tr->res + DsmTerrain::status_at(cells);
     const int32_t *clearance = reinterpret_cast<const int32_t *>(tr->res);
     const int32_t *thdr = reinterpret_cast<const int32_t *>(tr->res + DsmTerrain::header_at(cells));
@@ -713,6 +725,9 @@ extern "C" int dsm_reach_wait(dsm_ctx *ctx, dsm_reach_info_t *info, const dsm_re
 //   k_rm_gather   one thread per matrix entry; thread (i, 0) finishes site i's record.
 // No settle step: every tile a round leaves out holds equal buffers (a tile that changed schedules itself), so buffer
 // max_rounds % 2 holds the latest cost of every voxel, and the last two kernels read it.
+// The terrain matrix job (dsm_reach_matrix_enqueue_terrain, DESIGN.md §8.22) runs the same kernels on the plane of the
+// latest terrain job, as the terrain reach job does: k_rm_tiles, _sites, _init, _round and _gather on flat 32 x 16 x 1
+// tiles (k_rm_round<32, 16, 1>: a 34 x 18 halo, 9 neighbour slots), k_rm_slots and k_rm_reached unchanged.
 //
 // One packed result of a job on n sites (D2H, 64 + 32 n + 4 n^2 B):
 //   int32 header[DSM_RM_WORDS] | dsm_reach_site_t sites[n] | uint32 matrix[n][n]
@@ -738,21 +753,23 @@ static_assert(DSM_RM_WORDS * 4 == sizeof(dsm_reach_matrix_info_t) && DSM_RM_ROUN
 static_assert(RM_SITES == 2 * RC_TILE, "k_rm_round scans two sites per thread");
 
 __device__ __forceinline__ int3 rm_tile_xyz(const int3 tn, int tile) { return make_int3(tile % tn.x, tile / tn.x % tn.y, tile / (tn.x * tn.y)); }
-// the tile of voxel u and u's tile-local index
+// the tile of voxel u and u's tile-local index, on tiles of TX x TY x TZ
+template <int TX, int TY, int TZ>
 __device__ __forceinline__ int rm_tile_of_voxel(const DsmFieldGrid &g, const int3 tn, int u, int &local)
 {
     const int x = u % g.n[0], y = u / g.n[0] % g.n[1], z = u / (g.n[0] * g.n[1]);
-    local = ((z % RC_T) * RC_T + y % RC_T) * RC_T + x % RC_T;
-    return ((z / RC_T) * tn.y + y / RC_T) * tn.x + x / RC_T;
+    local = ((z % TZ) * TY + y % TY) * TX + x % TX;
+    return ((z / TZ) * tn.y + y / TY) * tn.x + x / TX;
 }
 
+template <int TX, int TY, int TZ>
 __global__ void __launch_bounds__(RC_TILE) k_rm_tiles(const DsmFieldGrid g, const int3 tn, const uint8_t *__restrict__ state,
                                                       const int32_t *__restrict__ dist, float radius, int32_t *__restrict__ flag,
                                                       uint32_t *__restrict__ mask, int32_t *hdr)
 {
     const int tile = blockIdx.x, t = threadIdx.x;
     const int3 tc = rm_tile_xyz(tn, tile);
-    const int x = tc.x * RC_T + t % RC_T, y = tc.y * RC_T + t / RC_T % RC_T, z = tc.z * RC_T + t / (RC_T * RC_T);
+    const int x = tc.x * TX + t % TX, y = tc.y * TY + t / TX % TY, z = tc.z * TZ + t / (TX * TY);
     const bool tv = reach_inside(g, x, y, z) && dsm_traversable(state, dist, reach_index(g, x, y, z), radius);
     const unsigned b = __ballot_sync(0xffffffffu, tv);
     if ((t & 31) == 0) mask[(size_t)tile * RM_WORDS + t / 32] = b;
@@ -786,6 +803,7 @@ __global__ void __launch_bounds__(RC_BLOCK) k_rm_slots(const DsmFieldGrid g, int
     }
 }
 
+template <int TX, int TY, int TZ>
 __global__ void __launch_bounds__(RC_BLOCK) k_rm_sites(const DsmFieldGrid g, const int3 tn, const uint8_t *__restrict__ state,
                                                        const int32_t *__restrict__ dist, const int32_t *__restrict__ sites, int n_sites,
                                                        float radius, int k, int max_tiles, const int32_t *__restrict__ slot,
@@ -811,12 +829,13 @@ __global__ void __launch_bounds__(RC_BLOCK) k_rm_sites(const DsmFieldGrid g, con
     if (seeded)
     {
         int local;
-        const int a = slot[rm_tile_of_voxel(g, tn, u, local)];
+        const int a = slot[rm_tile_of_voxel<TX, TY, TZ>(g, tn, u, local)];
         sched0[(size_t)i * max_tiles] = a;
         stamp[(size_t)i * max_tiles + a] = 0;
     }
 }
 
+template <int TX, int TY, int TZ>
 __global__ void __launch_bounds__(RC_TILE) k_rm_init(const DsmFieldGrid g, const int3 tn, int n_sites, int max_tiles, const int32_t *__restrict__ slot,
                                                      const dsm_reach_site_t *__restrict__ rec, const int32_t *__restrict__ hdr,
                                                      uint32_t *__restrict__ c0, uint32_t *__restrict__ c1)
@@ -828,7 +847,7 @@ __global__ void __launch_bounds__(RC_TILE) k_rm_init(const DsmFieldGrid g, const
         const int i = (int)(q / n_active), a = (int)(q % n_active);
         const int u = rec[i].voxel;
         int local = -1;
-        const bool own = u >= 0 && slot[rm_tile_of_voxel(g, tn, u, local)] == a;
+        const bool own = u >= 0 && slot[rm_tile_of_voxel<TX, TY, TZ>(g, tn, u, local)] == a;
         const uint32_t c = own && local == t ? 0u : RC_INF;
         const size_t at = ((size_t)i * max_tiles + a) * RC_TILE + t;
         c0[at] = c;
@@ -836,16 +855,19 @@ __global__ void __launch_bounds__(RC_TILE) k_rm_init(const DsmFieldGrid g, const
     }
 }
 
+template <int TX, int TY, int TZ>
 __global__ void __launch_bounds__(RC_TILE) k_rm_round(const int3 tn, int n_sites, int max_tiles, const int32_t *__restrict__ slot,
                                                       const int32_t *__restrict__ tile_of, const uint32_t *__restrict__ mask,
                                                       const uint32_t *__restrict__ cin, uint32_t *__restrict__ cout,
                                                       const int32_t *__restrict__ sched_in, int32_t *__restrict__ sched_out,
                                                       int32_t *__restrict__ stamp, int32_t *count, int32_t *__restrict__ rounds, int32_t *hdr, int r)
 {
+    typedef ReachTile<TX, TY, TZ> T;
+    static_assert((TX & (TX - 1)) == 0 && (TY & (TY - 1)) == 0 && (TZ & (TZ - 1)) == 0, "the halo's masks");
     typedef cub::BlockScan<int, RC_TILE> Scan;
-    __shared__ uint32_t s[RC_H * RC_H * RC_H];
+    __shared__ uint32_t s[T::HALO];
     __shared__ int pre[RM_SITES + 1]; // the exclusive prefix of the sites' schedule lengths; pre[n_sites] the total
-    __shared__ int nb[27];            // the item's neighbour slots (-1 inactive or outside), 13 its own
+    __shared__ int nb[T::NB];         // the item's neighbour slots (-1 inactive or outside), NB / 2 its own
     __shared__ typename Scan::TempStorage scan_tmp;
     const int t = threadIdx.x;
     int len[2];
@@ -866,8 +888,8 @@ __global__ void __launch_bounds__(RC_TILE) k_rm_round(const int3 tn, int n_sites
     }
     if (total == 0) return;
     __syncthreads();
-    const int lx = t % RC_T, ly = t / RC_T % RC_T, lz = t / (RC_T * RC_T);
-    const int si = ((lz + 1) * RC_H + ly + 1) * RC_H + lx + 1;
+    const int lx = t % TX, ly = t / TX % TY, lz = t / (TX * TY);
+    const int si = ((lz + T::DZ) * T::HY + ly + 1) * T::HX + lx + 1;
     volatile uint32_t *vs = s;
     for (int q = blockIdx.x; q < total; q += gridDim.x)
     {
@@ -882,30 +904,31 @@ __global__ void __launch_bounds__(RC_TILE) k_rm_round(const int3 tn, int n_sites
         const size_t row = (size_t)i * max_tiles;
         const int a = sched_in[row + q - pre[i]], tile = tile_of[a];
         const int3 tc = rm_tile_xyz(tn, tile);
-        if (t < 27)
+        if (t < T::NB)
         {
-            const int ax = tc.x + t % 3 - 1, ay = tc.y + t / 3 % 3 - 1, az = tc.z + t / 9 - 1;
+            const int ax = tc.x + t % 3 - 1, ay = tc.y + t / 3 % 3 - 1, az = tc.z + t / 9 - T::DZ;
             nb[t] = (unsigned)ax < (unsigned)tn.x && (unsigned)ay < (unsigned)tn.y && (unsigned)az < (unsigned)tn.z
                         ? slot[(az * tn.y + ay) * tn.x + ax]
                         : -1;
         }
         __syncthreads();
-        for (int h = t; h < RC_H * RC_H * RC_H; h += RC_TILE)
-        { // halo coordinate 0 is the lower neighbour's voxel 7, RC_H - 1 the upper neighbour's voxel 0
-            const int hx = h % RC_H, hy = h / RC_H % RC_H, hz = h / (RC_H * RC_H);
-            const int d = (hx > 0) + (hx == RC_H - 1) + 3 * ((hy > 0) + (hy == RC_H - 1)) + 9 * ((hz > 0) + (hz == RC_H - 1));
-            const int local = (((hz + RC_T - 1) & (RC_T - 1)) * RC_T + ((hy + RC_T - 1) & (RC_T - 1))) * RC_T + ((hx + RC_T - 1) & (RC_T - 1));
+        for (int h = t; h < T::HALO; h += RC_TILE)
+        { // halo coordinate 0 is the lower neighbour's last voxel, HX - 1 the upper neighbour's voxel 0 (a flat tile's
+          // halo has one layer along z, its own)
+            const int hx = h % T::HX, hy = h / T::HX % T::HY, hz = h / (T::HX * T::HY);
+            const int d = (hx > 0) + (hx == T::HX - 1) + 3 * ((hy > 0) + (hy == T::HY - 1)) + 9 * T::DZ * ((hz > 0) + (hz == T::HZ - 1));
+            const int local = (((hz + TZ - T::DZ) & (TZ - 1)) * TY + ((hy + TY - 1) & (TY - 1))) * TX + ((hx + TX - 1) & (TX - 1));
             const int b = nb[d];
             s[h] = b < 0 ? RC_INF : cin[(row + b) * RC_TILE + local];
         }
         const bool tv = (mask[(size_t)tile * RM_WORDS + t / 32] >> (t % 32)) & 1u;
         __syncthreads();
         const uint32_t c0 = s[si];
-        const uint32_t c = reach_relax<RC_T, RC_T, RC_T>(vs, si, tv, c0);
+        const uint32_t c = reach_relax<TX, TY, TZ>(vs, si, tv, c0);
         cout[(row + a) * RC_TILE + t] = c;
         // as k_reach_round, round 0's tile is the seeded start's and counts as changed; only active tiles are listed,
         // since an inactive one holds UINT32_MAX for good
-        if ((__syncthreads_or(c != c0) || r == 0) && t < 27)
+        if ((__syncthreads_or(c != c0) || r == 0) && t < T::NB)
         {
             const int b = nb[t];
             if (b >= 0 && atomicMax(&stamp[row + b], r + 1) < r + 1) sched_out[row + atomicAdd(&count[3 * i + (r + 1) % 3], 1)] = b;
@@ -927,6 +950,7 @@ __global__ void __launch_bounds__(RC_TILE) k_rm_reached(int n_sites, int max_til
     }
 }
 
+template <int TX, int TY, int TZ>
 __global__ void __launch_bounds__(RC_BLOCK) k_rm_gather(const DsmFieldGrid g, const int3 tn, int n_sites, int max_tiles, int max_rounds,
                                                         const int32_t *__restrict__ slot, const uint32_t *__restrict__ cost,
                                                         const int32_t *__restrict__ count, const int32_t *__restrict__ rounds,
@@ -942,7 +966,7 @@ __global__ void __launch_bounds__(RC_BLOCK) k_rm_gather(const DsmFieldGrid g, co
     if (ok && ui >= 0 && uj >= 0)
     {
         int local;
-        const int a = slot[rm_tile_of_voxel(g, tn, uj, local)];
+        const int a = slot[rm_tile_of_voxel<TX, TY, TZ>(g, tn, uj, local)];
         m = cost[((size_t)i * max_tiles + a) * RC_TILE + local];
     }
     matrix[e] = m;
@@ -954,21 +978,11 @@ __global__ void __launch_bounds__(RC_BLOCK) k_rm_gather(const DsmFieldGrid g, co
     }
 }
 
-// the persistent CTAs of k_rm_round on this device
-static int rm_ctas()
-{
-    int dev = 0, sms = 0, per = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess ||
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per, k_rm_round, RC_TILE, 0) != cudaSuccess)
-        return 0;
-    return sms * per;
-}
-
-// the CUB scratch of the tile scan; 0 on a CUB error
-static size_t rm_temp_bytes(const DsmReachMatrix &b)
+// the CUB scratch of a tile scan over `tiles` flags; 0 on a CUB error
+static size_t rm_temp_bytes(const DsmReachMatrix &b, int tiles)
 {
     size_t n = 0;
-    if (cub::DeviceScan::ExclusiveSum(nullptr, n, b.flag, b.scan, b.tiles, (cudaStream_t)0) != cudaSuccess) return 0;
+    if (cub::DeviceScan::ExclusiveSum(nullptr, n, b.flag, b.scan, tiles, (cudaStream_t)0) != cudaSuccess) return 0;
     return std::max(n, (size_t)1);
 }
 
@@ -995,7 +1009,8 @@ extern "C" int dsm_reach_matrix_enable(dsm_ctx *ctx, int max_sites, int max_tile
     for (int k = 0; k < 3; k++) b.tn[k] = tn[k];
     b.tiles = (int)tiles;
     b.max_sites = max_sites, b.max_tiles = max_tiles, b.max_rounds = max_rounds;
-    b.ctas = rm_ctas();
+    b.ctas = reach_ctas((const void *)k_rm_round<RC_T, RC_T, RC_T>);
+    b.ctas_flat = reach_ctas((const void *)k_rm_round<RC_FLAT_X, RC_FLAT_Y, 1>);
     const size_t items = (size_t)max_sites * max_tiles, res = rm_res_bytes(max_sites);
     CudaOwner &o = rm->own;
     for (int32_t **p : {&b.flag, &b.scan, &b.slot}) o.device(p, (size_t)b.tiles);
@@ -1010,9 +1025,65 @@ extern "C" int dsm_reach_matrix_enable(dsm_ctx *ctx, int max_sites, int max_tile
     o.host(&rm->sites_host, 3 * (size_t)max_sites);
     o.host(&rm->res_host, res);
     o.event(&rm->ev);
-    b.temp_bytes = rm_temp_bytes(b);
+    // the scan runs over the field's tiles or over the flat tiles of a terrain plane, whichever the up axis: scratch
+    // for the field's count need not cover a smaller one
+    b.temp_bytes = rm_temp_bytes(b, b.tiles);
+    for (int a = 0; a < 3 && b.temp_bytes; a++)
+    {
+        const int3 ft = reach_flat_tn(f->g.n[a == 0 ? 1 : 0], f->g.n[a == 2 ? 1 : 2]);
+        const size_t n = rm_temp_bytes(b, ft.x * ft.y);
+        b.temp_bytes = n ? std::max(b.temp_bytes, n) : 0;
+    }
     if (b.temp_bytes) o.device(reinterpret_cast<uint8_t **>(&b.temp), b.temp_bytes);
-    return keep(ctx->reach_matrix, rm, b.ctas > 0 && b.temp_bytes != 0);
+    return keep(ctx->reach_matrix, rm, b.ctas > 0 && b.ctas_flat > 0 && b.temp_bytes != 0);
+}
+
+// the argument checks both matrix enqueues share (include/dsm.h)
+static bool rm_args_ok(const DsmReachMatrix &b, const double *points, int n_points, float radius, int approach)
+{
+    if (!points || !std::isfinite(radius) || !(radius >= 0.f) || approach < 0 || approach > DSM_REACH_MAX_APPROACH || n_points < 1 ||
+        n_points > b.max_sites ||
+        (unsigned long long)n_points * (unsigned long long)b.max_tiles * (unsigned long long)b.max_rounds > DSM_REACH_MATRIX_MAX_WORK)
+        return false;
+    for (size_t i = 0; i < 3 * (size_t)n_points; i++)
+        if (!std::isfinite(points[i])) return false;
+    return true;
+}
+
+// The job of n sites already staged in rm.sites_host on grid g cut into tiles of TX x TY x TZ (tn per axis, `tiles` in
+// all, rounds on `ctas` persistent CTAs), over the traversable test of (state, dist) and with the field error words of
+// fhdr.  The enqueue submits the result.
+template <int TX, int TY, int TZ>
+static int rm_launch(dsm_ctx *ctx, DsmReachMatrix &b, const DsmFieldGrid &g, const int3 tn, int tiles, int ctas, const uint8_t *state,
+                     const int32_t *dist, const int32_t *fhdr, int n, float radius, int approach)
+{
+    const cudaStream_t st = ctx->stream;
+    CK(cudaMemcpyAsync(b.sites, b.sites_host, 12 * (size_t)n, cudaMemcpyHostToDevice, st));
+    CK(cudaMemsetAsync(b.res, 0, 4 * DSM_RM_WORDS, st));
+    int32_t *hdr = reinterpret_cast<int32_t *>(b.res);
+    auto *rec = reinterpret_cast<dsm_reach_site_t *>(b.res + 4 * DSM_RM_WORDS);
+    auto *matrix = reinterpret_cast<uint32_t *>(b.res + rm_matrix_at(n));
+    CK(cudaMemsetAsync(b.stamp, 0xff, 4 * (size_t)n * b.max_tiles, st));
+    CK(cudaMemsetAsync(b.rounds, 0, 4 * (size_t)n, st));
+    CK(cudaMemsetAsync(b.reached, 0, 4 * (size_t)n, st));
+    k_rm_tiles<TX, TY, TZ><<<tiles, RC_TILE, 0, st>>>(g, tn, state, dist, radius, b.flag, b.mask, hdr);
+    CK(cudaGetLastError());
+    size_t tb = b.temp_bytes;
+    CK(cub::DeviceScan::ExclusiveSum(b.temp, tb, b.flag, b.scan, tiles, st));
+    k_rm_slots<<<rc_blocks(tiles), RC_BLOCK, 0, st>>>(g, tiles, b.max_tiles, n, b.flag, b.scan, fhdr, b.slot, b.tile_of, hdr);
+    k_rm_sites<TX, TY, TZ><<<rc_blocks(32ll * n), RC_BLOCK, 0, st>>>(g, tn, state, dist, b.sites, n, radius, approach, b.max_tiles, b.slot,
+                                                                    b.sched[0], b.stamp, b.count, hdr, rec);
+    k_rm_init<TX, TY, TZ><<<ctas, RC_TILE, 0, st>>>(g, tn, n, b.max_tiles, b.slot, rec, hdr, b.cost[0], b.cost[1]);
+    for (int r = 0; r < b.max_rounds; r++)
+        k_rm_round<TX, TY, TZ><<<ctas, RC_TILE, 0, st>>>(tn, n, b.max_tiles, b.slot, b.tile_of, b.mask, b.cost[r % 2], b.cost[(r + 1) % 2],
+                                                         b.sched[r % 2], b.sched[(r + 1) % 2], b.stamp, b.count, b.rounds, hdr, r);
+    const uint32_t *last = b.cost[b.max_rounds % 2];
+    k_rm_reached<<<ctas, RC_TILE, 0, st>>>(n, b.max_tiles, last, hdr, b.reached);
+    k_rm_gather<TX, TY, TZ><<<rc_blocks((long long)n * n), RC_BLOCK, 0, st>>>(g, tn, n, b.max_tiles, b.max_rounds, b.slot, last, b.count,
+                                                                             b.rounds, b.reached, hdr, rec, matrix);
+    CK(cudaGetLastError());
+    b.n_sites = n;
+    return DSM_OK;
 }
 
 // Enqueue only: the points' voxels staged and copied, the job on the grids of the latest (known) field request, one D2H
@@ -1024,48 +1095,42 @@ extern "C" int dsm_reach_matrix_enqueue(dsm_ctx *ctx, const double *points, int 
     const DsmField *f = known_field(ctx);
     if (!rm || !f || rm->in_flight) return DSM_E_STATE;
     DsmReachMatrix &b = *rm;
-    if (!points || !std::isfinite(radius) || !(radius >= 0.f) || approach < 0 || approach > DSM_REACH_MAX_APPROACH || n_points < 1 ||
-        n_points > b.max_sites ||
-        (unsigned long long)n_points * (unsigned long long)b.max_tiles * (unsigned long long)b.max_rounds > DSM_REACH_MATRIX_MAX_WORK)
-        return DSM_E_INVALID;
-    for (size_t i = 0; i < 3 * (size_t)n_points; i++)
-        if (!std::isfinite(points[i])) return DSM_E_INVALID;
+    if (!rm_args_ok(b, points, n_points, radius, approach)) return DSM_E_INVALID;
     const DsmFieldGrid &g = f->g;
-    const cudaStream_t st = ctx->stream;
     const int n = n_points;
     CK(cudaSetDevice(ctx->device));
     // the previous job's copy out of this staging ended before its wait, which no job in flight implies
     for (size_t i = 0; i < 3 * (size_t)n; i++) rm->sites_host[i] = reach_voxel(points[i], g.voxel, g.o[i % 3], g.n[i % 3]);
-    CK(cudaMemcpyAsync(b.sites, rm->sites_host, 12 * (size_t)n, cudaMemcpyHostToDevice, st));
-    CK(cudaMemsetAsync(b.res, 0, 4 * DSM_RM_WORDS, st));
-    int32_t *hdr = reinterpret_cast<int32_t *>(b.res);
-    auto *rec = reinterpret_cast<dsm_reach_site_t *>(b.res + 4 * DSM_RM_WORDS);
-    auto *matrix = reinterpret_cast<uint32_t *>(b.res + rm_matrix_at(n));
-    const uint8_t *state = f->occ;
-    const int32_t *dist = f->dist;
     const int3 tn = make_int3(b.tn[0], b.tn[1], b.tn[2]);
-    CK(cudaMemsetAsync(b.stamp, 0xff, 4 * (size_t)n * b.max_tiles, st));
-    CK(cudaMemsetAsync(b.rounds, 0, 4 * (size_t)n, st));
-    CK(cudaMemsetAsync(b.reached, 0, 4 * (size_t)n, st));
-    k_rm_tiles<<<b.tiles, RC_TILE, 0, st>>>(g, tn, state, dist, radius, b.flag, b.mask, hdr);
-    CK(cudaGetLastError());
-    size_t tb = b.temp_bytes;
-    CK(cub::DeviceScan::ExclusiveSum(b.temp, tb, b.flag, b.scan, b.tiles, st));
-    k_rm_slots<<<rc_blocks(b.tiles), RC_BLOCK, 0, st>>>(g, b.tiles, b.max_tiles, n, b.flag, b.scan, dist + dsm_field_header(f->voxels), b.slot,
-                                                        b.tile_of, hdr);
-    k_rm_sites<<<rc_blocks(32ll * n), RC_BLOCK, 0, st>>>(g, tn, state, dist, b.sites, n, radius, approach, b.max_tiles, b.slot, b.sched[0],
-                                                         b.stamp, b.count, hdr, rec);
-    k_rm_init<<<b.ctas, RC_TILE, 0, st>>>(g, tn, n, b.max_tiles, b.slot, rec, hdr, b.cost[0], b.cost[1]);
-    for (int r = 0; r < b.max_rounds; r++)
-        k_rm_round<<<b.ctas, RC_TILE, 0, st>>>(tn, n, b.max_tiles, b.slot, b.tile_of, b.mask, b.cost[r % 2], b.cost[(r + 1) % 2],
-                                               b.sched[r % 2], b.sched[(r + 1) % 2], b.stamp, b.count, b.rounds, hdr, r);
-    const uint32_t *last = b.cost[b.max_rounds % 2];
-    k_rm_reached<<<b.ctas, RC_TILE, 0, st>>>(n, b.max_tiles, last, hdr, b.reached);
-    k_rm_gather<<<rc_blocks((long long)n * n), RC_BLOCK, 0, st>>>(g, tn, n, b.max_tiles, b.max_rounds, b.slot, last, b.count, b.rounds,
-                                                                  b.reached, hdr, rec, matrix);
-    CK(cudaGetLastError());
-    rm->n_sites = n;
+    const int rc = rm_launch<RC_T, RC_T, RC_T>(ctx, b, g, tn, b.tiles, b.ctas, f->occ, f->dist, f->dist + dsm_field_header(f->voxels), n,
+                                               radius, approach);
+    if (rc != DSM_OK) return rc;
     return submit(ctx, *rm, b.res, rm_res_bytes(n), f->requests);
+}
+
+// Enqueue only: the job of dsm_reach_matrix_enqueue on the plane of the latest terrain job (DESIGN.md §8.22), the
+// points' columns staged as cells of that plane, in stream order behind that job.  A later terrain, field or frontier
+// request overwrites what the job reads only behind it.  The job pairs with no field request (request 0).
+extern "C" int dsm_reach_matrix_enqueue_terrain(dsm_ctx *ctx, const double *points, int n_points, float radius, int approach)
+{
+    if (!ctx) return DSM_E_INVALID;
+    DsmReachMatrix *rm = ctx->reach_matrix.get();
+    const DsmTerrain *tr = ctx->terrain.get();
+    if (!rm || !tr || tr->request == 0 || rm->in_flight) return DSM_E_STATE;
+    DsmReachMatrix &b = *rm;
+    if (!rm_args_ok(b, points, n_points, radius, approach)) return DSM_E_INVALID;
+    const ReachTerrainGrid g = reach_terrain_grid(ctx->field->g, *tr);
+    const int n = n_points, cells = tr->cells;
+    CK(cudaSetDevice(ctx->device));
+    // the previous job's copy out of this staging ended before its wait, which no job in flight implies
+    for (int i = 0; i < n; i++) reach_terrain_cell(g, points + 3 * i, rm->sites_host + 3 * i);
+    const int3 tn = reach_flat_tn(g.n[0], g.n[1]);
+    const uint8_t *status = tr->res + DsmTerrain::status_at(cells);
+    const int32_t *clearance = reinterpret_cast<const int32_t *>(tr->res);
+    const int32_t *thdr = reinterpret_cast<const int32_t *>(tr->res + DsmTerrain::header_at(cells));
+    const int rc = rm_launch<RC_FLAT_X, RC_FLAT_Y, 1>(ctx, b, g, tn, tn.x * tn.y, b.ctas_flat, status, clearance, thdr, n, radius, approach);
+    if (rc != DSM_OK) return rc;
+    return submit(ctx, *rm, b.res, rm_res_bytes(n), 0);
 }
 
 extern "C" int dsm_reach_matrix_wait(dsm_ctx *ctx, dsm_reach_matrix_info_t *info, const dsm_reach_site_t **sites, const uint32_t **matrix)

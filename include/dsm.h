@@ -991,6 +991,32 @@ int dsm_reach_matrix_enable(dsm_ctx *ctx, int max_sites, int max_tiles, int max_
 int dsm_reach_matrix_enqueue(dsm_ctx *ctx, const double *points, int n_points, float radius, int approach);
 int dsm_reach_matrix_wait(dsm_ctx *ctx, dsm_reach_matrix_info_t *info, const dsm_reach_site_t **sites, const uint32_t **matrix);
 
+/* ---- driving costs between many sites: the matrix job on the latest terrain job's plane (DESIGN.md §8.22) ----
+ * A terrain matrix job is the matrix job above run on the plane of the latest terrain job (§8.20), as the terrain reach
+ * job (§8.21) runs the reach job there: in stream order behind that job, which may still be in flight; a later terrain,
+ * field or frontier request overwrites what it reads only behind it.  It uses the matrix job's buffers, enable, info,
+ * site records, result and wait, and allocates nothing.  Everything not restated here is §8.13's, on that plane.
+ *   Grid: §8.21's, the plane (P, Q, 1) at the terrain job's origin and voxel edge v, cells in the linear order q P + p;
+ *   site voxels are cells, and the header's origin is the terrain job's.
+ *   Traversable: status 2 and clearance >= radius, as in §8.21; the 8 in-plane moves, face 10 and diagonal 14.
+ *   Sites: a point is snapped as a terrain reach job's start: its column (its up coordinate replaced by 0), then the
+ *   approach window as a square; status 1 is decided by the two in-plane axes.  A cell centre, in-plane coordinates
+ *   ((o_h + c_h) + 0.5) v and any up coordinate, snaps to itself, so a terrain reach job's viewpoint cells may come back
+ *   as sites.
+ *   Active tiles: the 32 x 16 tiles from cell (0, 0) that hold a traversable cell, in tile order; status 1 (the cut)
+ *   when n_active_tiles > max_tiles.
+ *   Costs: for a site of status 0, its row reads the cost plane of a dsm_reach_enqueue_terrain job started there with
+ *   the same radius, approach and max_rounds, bit for bit, unconverged values included; its rounds, converged and
+ *   n_reached are that job's.  M[i][j] = cost_i[u_j] as in §8.13.
+ *
+ *   dsm_reach_matrix_enqueue_terrain  as dsm_reach_matrix_enqueue.  DSM_E_STATE before dsm_reach_matrix_enable, with no
+ *                                     terrain job yet, and while a matrix job is in flight.  DSM_E_INVALID exactly as
+ *                                     dsm_reach_matrix_enqueue, the n_points x max_tiles x max_rounds <= 2^32 bound
+ *                                     included.  dsm_reach_matrix_wait returns DSM_E_CAPACITY when the terrain job's
+ *                                     field was taken after a rejected frame.  The job reads no field request.  Terrain
+ *                                     and field matrix jobs may alternate on one context. */
+int dsm_reach_matrix_enqueue_terrain(dsm_ctx *ctx, const double *points, int n_points, float radius, int approach);
+
 /* ---- the order of an exploration tour: multi-start local search over a travel-cost matrix (DESIGN.md §8.14) ----
  * A tour job orders n sites by a deterministic multi-start local search for the asymmetric TSP over a row-major uint32
  * matrix M[i][j] (the cost from i to j, UINT32_MAX: no path), such as the matrix of dsm_reach_matrix_wait as it stands.

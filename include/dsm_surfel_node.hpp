@@ -109,7 +109,9 @@
 // Where can a ground robot drive?  enable_terrain(up), after enable_known_space, lets terrain() find the supporting
 // surface of every column of the latest fused frame's known field along the up axis on the device (DESIGN.md §8.20):
 // its level, the step to its neighbours, whether it is traversable and the clearance to the nearest cell that is not,
-// one enqueue and one wait.
+// one enqueue and one wait.  A ground planner's exploration chain runs on that plane: terrain(), then frontiers(), then
+// reach_terrain(with_frontiers) from the robot for each cluster's viewpoint cell (DESIGN.md §8.21), then
+// reach_matrix_terrain over the robot's position and the viewpoint cells' centres (§8.22), then tour() on that matrix.
 // device < 0 builds the node without a context: the callbacks run the whole pose logic (pose database, sync, window
 // bookkeeping) and fuse nothing; any call that reads the map returns DSM_E_STATE.
 #pragma once
@@ -888,6 +890,33 @@ class SurfelMapNode
             [&] {
                 targets.assign(t, t + std::min(info.n_targets, reach_targets_));
                 path.assign(p, p + info.n_path_voxels);
+            });
+    }
+    // ---- driving costs between many points on the terrain of the latest fused frame (DESIGN.md §8.22), after
+    // enable_reach_matrix ----
+    // reach_matrix() on the plane of the terrain() call on this frame: the travel costs between the columns of the points
+    // (xyz doubles) over the traversable cells at least `radius` from any other; site voxels are cells q P + p of the
+    // terrain grid.  Chained after reach_terrain(with_frontiers), the points are the robot and the viewpoint cells'
+    // centres, which snap to themselves at any height.  DSM_E_STATE without a terrain() call on this frame and after
+    // load_state* until the next fused frame; DSM_E_CAPACITY with the costs of the last applied frame's terrain.
+    int reach_matrix_terrain(const std::vector<double> &points, float radius, int approach, dsm_reach_matrix_info_t &info,
+                             std::vector<dsm_reach_site_t> &sites, std::vector<uint32_t> &matrix)
+    {
+        sites.clear();
+        matrix.clear();
+        info = dsm_reach_matrix_info_t();
+        const dsm_reach_site_t *s = nullptr;
+        const uint32_t *m = nullptr;
+        return job(
+            "reach_matrix_terrain", KNOWN_FIELD, points.size() % 3 == 0,
+            [&] {
+                return terrain_frame_ ? dsm_reach_matrix_enqueue_terrain(ctx_.ctx, points.data(), (int)(points.size() / 3), radius, approach)
+                                      : DSM_E_STATE;
+            },
+            [&] { return dsm_reach_matrix_wait(ctx_.ctx, &info, &s, &m); },
+            [&] {
+                sites.assign(s, s + info.n_sites);
+                matrix.assign(m, m + (size_t)info.n_sites * info.n_sites);
             });
     }
     // the field of the latest fused frame: dist [nz][ny][nx] in metres (the library's pinned buffer, valid until the next
