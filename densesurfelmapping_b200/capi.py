@@ -41,6 +41,7 @@ EXPORTS = [
     "dsm_reach_enable", "dsm_reach_enqueue", "dsm_reach_enqueue_terrain", "dsm_reach_wait", "dsm_reach_matrix_enable", "dsm_reach_matrix_enqueue",
     "dsm_reach_matrix_enqueue_terrain", "dsm_reach_matrix_wait", "dsm_gain_enable", "dsm_gain_enqueue", "dsm_gain_wait",
     "dsm_tour_enable", "dsm_tour_enqueue", "dsm_tour_wait", "dsm_viewpoint_enable", "dsm_viewpoint_enqueue", "dsm_viewpoint_wait",
+    "dsm_viewpoint_enqueue_terrain",
     "dsm_trajectory_enable", "dsm_trajectory_enqueue", "dsm_trajectory_wait",
     "dsm_heading_enable", "dsm_heading_enqueue", "dsm_heading_wait",
     "dsm_terrain_enable", "dsm_terrain_enqueue", "dsm_terrain_wait",
@@ -237,6 +238,7 @@ def load_library():
     L.dsm_tour_wait.argtypes = [vp, vp, ctypes.POINTER(vp), ctypes.POINTER(vp)]
     L.dsm_viewpoint_enable.argtypes = [vp, ci, ci]
     L.dsm_viewpoint_enqueue.argtypes = [vp, ctypes.POINTER(DsmGainCamera), vp, ci, vp, ci, ctypes.POINTER(DsmViewpointParams)]
+    L.dsm_viewpoint_enqueue_terrain.argtypes = [vp, ctypes.POINTER(DsmGainCamera), vp, ci, vp, ci, ctypes.POINTER(DsmViewpointParams), ci]
     L.dsm_viewpoint_wait.argtypes = [vp, vp, ctypes.POINTER(vp), ctypes.POINTER(vp)]
     L.dsm_trajectory_enable.argtypes = [vp, ci, ci, ci]
     L.dsm_trajectory_enqueue.argtypes = [vp, vp, vp, vp, ci, ctypes.POINTER(DsmTrajectoryParams)]
@@ -893,12 +895,21 @@ class Context:
         """camera: (fx, fy, cx, cy, width, height, max_range, unknown_blocks); rotations: (n, 9) row-major camera-to-world
         3x3 matrices; clusters: frontier-table indices; params: (r_min, r_max, dz_max, stride, max_samples, min_seen,
         top_k, with_reach, radius)."""
+        self._viewpoint_enqueue(self.lib.dsm_viewpoint_enqueue, camera, rotations, clusters, params)
+
+    def viewpoint_enqueue_terrain(self, camera, rotations, clusters, params, eye):
+        """The viewpoint job on the plane of the latest terrain job (DESIGN.md §8.23), arguments as viewpoint_enqueue's
+        with dz_max 0; the camera stands eye voxels above each candidate cell's support, and the slots' voxels that
+        viewpoint_wait returns are cells q P + p of that plane."""
+        self._viewpoint_enqueue(self.lib.dsm_viewpoint_enqueue_terrain, camera, rotations, clusters, params, int(eye))
+
+    def _viewpoint_enqueue(self, call, camera, rotations, clusters, params, *eye):
         cam = _camera(camera)
         R = np.ascontiguousarray(rotations, np.float64).reshape(-1, 9)
         c = np.ascontiguousarray(clusters, np.int32).reshape(-1)
         p = DsmViewpointParams(*[int(x) for x in params[:8]], float(params[8]), 0)
-        self._ck(self.lib.dsm_viewpoint_enqueue(self.h, ctypes.byref(cam), R.ctypes.data if len(R) else None, len(R),
-                                                c.ctypes.data if len(c) else None, len(c), ctypes.byref(p)))
+        self._ck(call(self.h, ctypes.byref(cam), R.ctypes.data if len(R) else None, len(R), c.ctypes.data if len(c) else None, len(c),
+                      ctypes.byref(p), *eye))
 
     def viewpoint_wait(self):
         """(info, clusters, viewpoints): numpy copies of the context's pinned results, a VIEWPOINT_INFO_DTYPE record,

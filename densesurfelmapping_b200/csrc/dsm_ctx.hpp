@@ -311,6 +311,7 @@ struct DsmReach : DsmJob
     int32_t *goals_host = nullptr; // pinned [max_targets][3]
     uint32_t *cost_host = nullptr; // pinned [voxels]
     bool host_copy = false;
+    uint64_t terrain = 0; // the DsmTerrain::enqueues of the terrain job the latest job ran on (0: a field job, or none)
 };
 
 // dsm_reach_matrix_* (DESIGN.md §8.13), allocated by dsm_reach_matrix_enable for the field's grid: the job's device
@@ -356,6 +357,7 @@ struct DsmVpCluster; // what k_vp_clusters leaves per requested cluster (dsm_vie
 struct DsmViewpoint : DsmJob
 {
     int max_clusters = 0, max_candidates = 0, ctas = 0; // ctas: the persistent CTAs of k_vp_score
+    int ctas_terrain = 0;                               // those of a terrain job's k_vp_score (dsm_viewpoint_enqueue_terrain)
     uint8_t *stage_host = nullptr, *stage_dev = nullptr;
     DsmVpCluster *cl = nullptr;               // [max_clusters]
     unsigned long long *key = nullptr;        // [max_candidates]: the candidate's ranking key, ~0 when it is no viewpoint
@@ -406,6 +408,7 @@ struct DsmTerrain : DsmJob
     int m[3] = {0, 0, 0};
     uint8_t *res = nullptr;
     int origin[3] = {0, 0, 0}, headroom = 0, max_step = 0; // of the job in flight or last waited for
+    uint64_t enqueues = 0; // jobs enqueued so far: tells two terrain jobs on one field request apart (DsmReach::terrain)
     // byte offsets of the result's sections for C cells, which the terrain reach job reads as well:
     //   float clearance[C] | pad to dsm_field_header(C) words | int32 header[8] (a field header's words, dsm_device.cuh) |
     //   int16 level[C] | uint8 status[C] | uint8 step[C]
@@ -416,6 +419,26 @@ struct DsmTerrain : DsmJob
     static size_t step_at(int cells) { return status_at(cells) + (size_t)cells; }
     static size_t res_bytes(int cells) { return step_at(cells) + (size_t)cells; }
 };
+
+// The plane of a terrain job as the jobs on it see it (DESIGN.md §8.21-8.23): n the plane (P, Q, 1), o the terrain job's
+// origin; nf the field grid's extents and h0 < h1 its two in-plane axes, which map a field voxel to the cell of its column
+struct ReachTerrainGrid : DsmFieldGrid
+{
+    int nf[3], h0, h1;
+};
+
+// The plane of terrain job tr on field grid fg: the plane (P, Q, 1) of fg's two axes h0 < h1 other than the up axis, at
+// tr's origin
+static inline ReachTerrainGrid reach_terrain_grid(const DsmFieldGrid &fg, const DsmTerrain &tr)
+{
+    const int a = std::abs(tr.up) - 1;
+    ReachTerrainGrid g;
+    static_cast<DsmFieldGrid &>(g) = fg;
+    g.h0 = a == 0 ? 1 : 0, g.h1 = a == 2 ? 1 : 2;
+    for (int k = 0; k < 3; k++) g.o[k] = tr.origin[k], g.nf[k] = fg.n[k];
+    g.n[0] = fg.n[g.h0], g.n[1] = fg.n[g.h1], g.n[2] = 1;
+    return g;
+}
 
 #define DSM_MAX_CHUNKS 4
 

@@ -74,13 +74,6 @@ struct ReachTile
     static constexpr int NB = DZ ? 27 : 9; // the tile and its neighbour tiles
 };
 
-// The terrain job's grid: n the plane (P, Q, 1), o the terrain job's origin; nf the field grid's extents and h0 < h1 its
-// two in-plane axes, which map a field voxel to the cell of its column
-struct ReachTerrainGrid : DsmFieldGrid
-{
-    int nf[3], h0, h1;
-};
-
 static_assert(sizeof(dsm_reach_target_t) == 32 && sizeof(dsm_reach_info_t) == 64, "dsm_reach layouts");
 static_assert(DSM_REACH_N_PATH_VOXELS == 13 && DSM_REACH_WORDS * 4 == sizeof(dsm_reach_info_t), "the header starts with the info");
 static_assert(DSM_FRONTIER_N_LISTED == 3 && DSM_FRONTIER_N_CLUSTERS == 2, "frontier header words");
@@ -543,19 +536,6 @@ static int reach_voxel(double p, float v, int o, int n)
     return q < 0.0 ? -1 : q >= (double)n ? n : (int)q;
 }
 
-// The plane of terrain job tr on field grid fg as a reach grid (DESIGN.md §8.21): the plane (P, Q, 1) of fg's two axes
-// h0 < h1 other than the up axis, at tr's origin
-static ReachTerrainGrid reach_terrain_grid(const DsmFieldGrid &fg, const DsmTerrain &tr)
-{
-    const int a = std::abs(tr.up) - 1;
-    ReachTerrainGrid g;
-    static_cast<DsmFieldGrid &>(g) = fg;
-    g.h0 = a == 0 ? 1 : 0, g.h1 = a == 2 ? 1 : 2;
-    for (int k = 0; k < 3; k++) g.o[k] = tr.origin[k], g.nf[k] = fg.n[k];
-    g.n[0] = fg.n[g.h0], g.n[1] = fg.n[g.h1], g.n[2] = 1;
-    return g;
-}
-
 // a point's column on that plane: its two in-plane voxel coordinates, whatever its height
 static void reach_terrain_cell(const ReachTerrainGrid &g, const double *p, int32_t out[3])
 {
@@ -659,13 +639,14 @@ extern "C" int dsm_reach_enqueue(dsm_ctx *ctx, const double start[3], float radi
     const int rc = reach_launch<RC_T, RC_T, RC_T>(ctx, b, g, tn, b.tiles, b.ctas, b.voxels, f->occ, f->dist, f->dist + dsm_field_header(f->voxels),
                                                   s, radius, approach, n_goals, with_frontiers ? fr : nullptr, host_copy);
     if (rc != DSM_OK) return rc;
+    re->terrain = 0;
     return submit(ctx, *re, b.res, reach_res_bytes(b), f->requests);
 }
 
 // Enqueue only: the job of dsm_reach_enqueue on the plane of the latest terrain job (DESIGN.md §8.21), the points'
 // columns staged as cells of that plane, in stream order behind that job.  A later terrain, field or frontier request
-// overwrites what the job reads only behind it.  The job pairs with no field request (request 0), so a viewpoint job
-// never reads its cost grid as a field's.
+// overwrites what the job reads only behind it.  The job pairs with no field request (request 0), so a field viewpoint
+// job never reads its cost grid as a field's; it records the terrain job it ran on for a terrain viewpoint job.
 extern "C" int dsm_reach_enqueue_terrain(dsm_ctx *ctx, const double start[3], float radius, int approach, const double *goals, int n_goals,
                                          int with_frontiers, int host_copy)
 {
@@ -693,6 +674,7 @@ extern "C" int dsm_reach_enqueue_terrain(dsm_ctx *ctx, const double start[3], fl
     const int rc = reach_launch<RC_FLAT_X, RC_FLAT_Y, 1>(ctx, b, g, tn, tn.x * tn.y, b.ctas_flat, cells, status, clearance, thdr, s, radius,
                                                          approach, n_goals, with_frontiers ? fr : nullptr, host_copy);
     if (rc != DSM_OK) return rc;
+    re->terrain = tr->enqueues;
     return submit(ctx, *re, b.res, reach_res_bytes(b), 0);
 }
 

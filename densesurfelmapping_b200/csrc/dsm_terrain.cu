@@ -131,6 +131,7 @@ extern "C" int dsm_terrain_enqueue(dsm_ctx *ctx, int headroom, int max_step)
     CK(cudaGetLastError());
     for (int k = 0; k < 3; k++) tr->origin[k] = f->g.o[k];
     tr->headroom = headroom, tr->max_step = max_step;
+    tr->enqueues++;
     return submit(ctx, *tr, tr->res, DsmTerrain::res_bytes(C), f->requests);
 }
 

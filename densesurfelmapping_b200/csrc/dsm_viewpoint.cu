@@ -15,6 +15,10 @@
 // A key packs the ranking (-n_seen, cost, offset index) and the rotation into 63 bits, so the least keys are the
 // viewpoints in order and ~0 is no viewpoint.  The kernels carry no error gate and are launched without PDL, as the
 // other field kernels.  The job's C ABI calls (dsm_viewpoint_enable, _enqueue and _wait) follow them.
+// The terrain job (dsm_viewpoint_enqueue_terrain, DESIGN.md §8.23) runs the same kernels on a VpTerrainGrid: centres,
+// candidates, keys and slots on the plane (P, Q, 1) of the latest terrain job, traversable on its status and clearance
+// planes, and the camera over a candidate cell at the field voxel eye voxels above its support, from which the walk
+// runs through the field's state grid as on the field.
 //
 // One staged request (H2D, vp_stage_bytes):
 //   double rotations[64][9] | int32 offsets[4096][3] | int32 clusters[n_clusters]
@@ -62,7 +66,46 @@ __device__ __forceinline__ unsigned long long vp_key(int n_seen, uint32_t cost, 
            (unsigned long long)rotation;
 }
 
-__global__ void __launch_bounds__(VP_BLOCK) k_vp_clusters(const DsmFieldGrid g, const int32_t *__restrict__ fhdr,
+// The terrain job's grid (DESIGN.md §8.23): the plane of the terrain job (ReachTerrainGrid), its level plane, and du the
+// camera's height above the support in voxels along the field's up axis (eye, negated for a negative up)
+struct VpTerrainGrid : ReachTerrainGrid
+{
+    const int16_t *level;
+    int du;
+};
+
+// What the kernels ask of their grid: the centre voxel of a cluster (reach's start snap of its fp64 centroid, on the
+// plane's two axes), the field grid the walk and the member voxels live on, and the field voxel of the camera over a
+// candidate (x, y, z).  On the field grid the candidate is that voxel.
+__device__ __forceinline__ void vp_centre(const DsmFieldGrid &g, const dsm_frontier_cluster_t &T, int32_t *out)
+{
+    const double v = (double)g.voxel;
+    for (int k = 0; k < 3; k++) out[k] = (int)(floor(__ddiv_rn(T.centroid[k], v)) - (double)g.o[k]);
+}
+__device__ __forceinline__ void vp_centre(const VpTerrainGrid &g, const dsm_frontier_cluster_t &T, int32_t *out)
+{
+    const double v = (double)g.voxel;
+    const int o0 = g.h0 == 0 ? g.o[0] : g.o[1], o1 = g.h1 == 1 ? g.o[1] : g.o[2]; // selects: no local copy of g
+    out[0] = (int)(floor(__ddiv_rn(T.centroid[g.h0], v)) - (double)o0);
+    out[1] = (int)(floor(__ddiv_rn(T.centroid[g.h1], v)) - (double)o1);
+    out[2] = 0;
+}
+__device__ __forceinline__ const DsmFieldGrid &vp_field(const DsmFieldGrid &g) { return g; }
+__device__ __forceinline__ DsmFieldGrid vp_field(const VpTerrainGrid &g)
+{
+    DsmFieldGrid f = g;
+    for (int k = 0; k < 3; k++) f.n[k] = g.nf[k];
+    return f;
+}
+__device__ __forceinline__ int3 vp_camera(const DsmFieldGrid &, int x, int y, int z) { return make_int3(x, y, z); }
+__device__ __forceinline__ int3 vp_camera(const VpTerrainGrid &g, int x, int y, int)
+{ // x along h0 and y along h1; the up axis is the third (h0 is 0 or 1, h1 is 1 or 2)
+    const int u = (int)g.level[y * g.n[0] + x] + g.du;
+    return make_int3(g.h0 == 0 ? x : u, g.h0 == 1 ? x : g.h1 == 1 ? y : u, g.h1 == 2 ? y : u);
+}
+
+template <typename Grid>
+__global__ void __launch_bounds__(VP_BLOCK) k_vp_clusters(const Grid g, const int32_t *__restrict__ fhdr,
                                                           const int32_t *__restrict__ frontier_hdr,
                                                           const dsm_frontier_cluster_t *__restrict__ table, int frontier_max_clusters,
                                                           const int32_t *__restrict__ clusters, int n_clusters, int n_offsets,
@@ -93,12 +136,11 @@ __global__ void __launch_bounds__(VP_BLOCK) k_vp_clusters(const DsmFieldGrid g, 
     DsmVpCluster q;
     q.status = past ? 3 : unlisted ? 2 : 0;
     q.base = q.n = q.n_s = q.pad = 0;
-    const double v = (double)g.voxel;
     for (int k = 0; k < 3; k++) q.g[k] = 0;
     if (q.status == 0)
     {
         const dsm_frontier_cluster_t &T = table[c];
-        for (int k = 0; k < 3; k++) q.g[k] = (int)(floor(__ddiv_rn(T.centroid[k], v)) - (double)g.o[k]);
+        vp_centre(g, T, q.g);
         q.base = T.offset;
         q.n = T.n_voxels;
         q.n_s = min(T.n_voxels, max_samples);
@@ -112,7 +154,8 @@ __global__ void __launch_bounds__(VP_BLOCK) k_vp_clusters(const DsmFieldGrid g, 
     rec[i] = r;
 }
 
-__global__ void __launch_bounds__(VP_BLOCK) k_vp_candidates(const DsmFieldGrid g, const uint8_t *__restrict__ state,
+template <typename Grid>
+__global__ void __launch_bounds__(VP_BLOCK) k_vp_candidates(const Grid g, const uint8_t *__restrict__ state,
                                                             const int32_t *__restrict__ dist, const int32_t *__restrict__ offsets,
                                                             int n_offsets, float radius, const uint32_t *__restrict__ reach_cost,
                                                             const DsmVpCluster *__restrict__ cl, dsm_viewpoint_cluster_t *__restrict__ rec,
@@ -152,7 +195,8 @@ __global__ void __launch_bounds__(VP_BLOCK) k_vp_candidates(const DsmFieldGrid g
     }
 }
 
-__global__ void __launch_bounds__(VP_BLOCK) k_vp_score(const DsmFieldGrid g, const uint8_t *__restrict__ state,
+template <typename Grid>
+__global__ void __launch_bounds__(VP_BLOCK) k_vp_score(const Grid g, const uint8_t *__restrict__ state,
                                                        const double *__restrict__ rotations, int n_rotations,
                                                        const int32_t *__restrict__ offsets, int n_offsets, const DsmVpCluster *__restrict__ cl,
                                                        const int32_t *__restrict__ members, const int32_t *__restrict__ list,
@@ -165,7 +209,8 @@ __global__ void __launch_bounds__(VP_BLOCK) k_vp_score(const DsmFieldGrid g, con
     const int tid = threadIdx.x, lane = tid & 31;
     for (int k = tid; k < 9 * n_rotations; k += VP_BLOCK) s_rot[k] = rotations[k];
     const int n_items = *count;
-    const int nx = g.n[0], ny = g.n[1];
+    const auto &fg = vp_field(g);
+    const int nx = fg.n[0], ny = fg.n[1];
     const double v = (double)g.voxel;
     for (int it = blockIdx.x; it < n_items; it += gridDim.x)
     {
@@ -174,8 +219,9 @@ __global__ void __launch_bounds__(VP_BLOCK) k_vp_score(const DsmFieldGrid g, con
         const int item = list[it], i = item / n_offsets, j = item % n_offsets;
         const DsmVpCluster q = cl[i];
         const int x = q.g[0] + offsets[3 * j], y = q.g[1] + offsets[3 * j + 1], z = q.g[2] + offsets[3 * j + 2];
-        const double tx = __dmul_rn(__dadd_rn((double)(g.o[0] + x), 0.5), v), ty = __dmul_rn(__dadd_rn((double)(g.o[1] + y), 0.5), v),
-                     tz = __dmul_rn(__dadd_rn((double)(g.o[2] + z), 0.5), v);
+        const int3 t = vp_camera(g, x, y, z);
+        const double tx = __dmul_rn(__dadd_rn((double)(g.o[0] + t.x), 0.5), v), ty = __dmul_rn(__dadd_rn((double)(g.o[1] + t.y), 0.5), v),
+                     tz = __dmul_rn(__dadd_rn((double)(g.o[2] + t.z), 0.5), v);
         for (int k0 = 0; k0 < q.n_s; k0 += VP_BLOCK)
         {
             const int k = k0 + tid;
@@ -190,7 +236,7 @@ __global__ void __launch_bounds__(VP_BLOCK) k_vp_score(const DsmFieldGrid g, con
                 const double d0 = __dsub_rn(c0, tx), d1 = __dsub_rn(c1, ty), d2 = __dsub_rn(c2, tz);
                 for (int r = 0; r < n_rotations; r++)
                     if (dsm_gain_frustum<3>(s_rot + 9 * r, d0, d1, d2, fx, fy, cx, cy, width, height, range2)) mask |= 1ull << r;
-                seen = mask && dsm_gain_walk(g, state, unknown_blocks, tx, ty, tz, c0, c1, c2);
+                seen = mask && dsm_gain_walk(fg, state, unknown_blocks, tx, ty, tz, c0, c1, c2);
             }
             if (__any_sync(0xffffffffu, seen))
                 for (int r = 0; r < n_rotations; r++)
@@ -208,7 +254,7 @@ __global__ void __launch_bounds__(VP_BLOCK) k_vp_score(const DsmFieldGrid g, con
             const int n_seen = (int)s_cnt[best];
             if (n_seen >= max(1, min_seen))
             {
-                const uint32_t cost = reach_cost ? reach_cost[(z * ny + y) * nx + x] : 0xffffffffu;
+                const uint32_t cost = reach_cost ? reach_cost[(z * g.n[1] + y) * g.n[0] + x] : 0xffffffffu;
                 key[item] = vp_key(n_seen, cost, j, best);
             }
         }
@@ -216,7 +262,8 @@ __global__ void __launch_bounds__(VP_BLOCK) k_vp_score(const DsmFieldGrid g, con
     }
 }
 
-__global__ void __launch_bounds__(VP_BLOCK) k_vp_select(const DsmFieldGrid g, const int32_t *__restrict__ offsets, int n_offsets, int top_k,
+template <typename Grid>
+__global__ void __launch_bounds__(VP_BLOCK) k_vp_select(const Grid g, const int32_t *__restrict__ offsets, int n_offsets, int top_k,
                                                         const DsmVpCluster *__restrict__ cl, const unsigned long long *__restrict__ key,
                                                         dsm_viewpoint_cluster_t *__restrict__ rec, dsm_viewpoint_t *__restrict__ out)
 {
@@ -272,12 +319,12 @@ __global__ void __launch_bounds__(VP_BLOCK) k_vp_select(const DsmFieldGrid g, co
     if (tid == 0) rec[i].n_viewpoints = n_vp;
 }
 
-// the persistent CTAs of k_vp_score on this device
-static int vp_ctas()
+// the persistent CTAs of a k_vp_score instantiation on this device
+static int vp_ctas(const void *score)
 {
     int dev = 0, sms = 0, per = 0;
     if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess ||
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per, k_vp_score, VP_BLOCK, 0) != cudaSuccess)
+        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per, score, VP_BLOCK, 0) != cudaSuccess)
         return 0;
     return sms * per;
 }
@@ -299,7 +346,8 @@ extern "C" int dsm_viewpoint_enable(dsm_ctx *ctx, int max_clusters, int max_cand
     CK(cudaSetDevice(ctx->device));
     auto vp = std::make_unique<DsmViewpoint>();
     vp->max_clusters = max_clusters, vp->max_candidates = max_candidates;
-    vp->ctas = vp_ctas();
+    vp->ctas = vp_ctas((const void *)k_vp_score<DsmFieldGrid>);
+    vp->ctas_terrain = vp_ctas((const void *)k_vp_score<VpTerrainGrid>);
     const size_t stage = vp_stage_bytes(max_clusters), res = vp_res_bytes(max_clusters, DSM_VIEWPOINT_MAX_TOP_K);
     CudaOwner &o = vp->own;
     o.device(&vp->stage_dev, stage);
@@ -311,7 +359,7 @@ extern "C" int dsm_viewpoint_enable(dsm_ctx *ctx, int max_clusters, int max_cand
     o.device(&vp->res, res);
     o.host(&vp->res_host, res);
     o.event(&vp->ev);
-    return keep(ctx->viewpoint, vp, vp->ctas > 0);
+    return keep(ctx->viewpoint, vp, vp->ctas > 0 && vp->ctas_terrain > 0);
 }
 
 // The offsets of include/dsm.h in their order, written as (dx, dy, dz) triples to out (room for
@@ -333,6 +381,74 @@ static int viewpoint_offsets(const dsm_viewpoint_params_t &p, int32_t *out)
     return n;
 }
 
+// The argument checks both enqueues share (include/dsm.h), on a grid of voxel edge v: the offsets written to the
+// staging and their number returned, or -1 for DSM_E_INVALID
+static int vp_args(const DsmViewpoint &vp, const dsm_gain_camera_t *camera, const double *rotations, int n_rotations,
+                   const int32_t *clusters, int n_clusters, const dsm_viewpoint_params_t *params, float v)
+{
+    if (!camera || !params || !rotations || n_rotations < 1 || n_rotations > DSM_VIEWPOINT_MAX_ROTATIONS || n_clusters < 0 ||
+        n_clusters > vp.max_clusters || (n_clusters > 0 && !clusters))
+        return -1;
+    const dsm_gain_camera_t &c = *camera;
+    const dsm_viewpoint_params_t &p = *params;
+    if (!gain_camera_ok(c, (double)v)) return -1;
+    if (p.r_min < 0 || p.r_min > p.r_max || p.r_max > DSM_VIEWPOINT_MAX_RADIUS || p.dz_max < 0 || p.dz_max > DSM_VIEWPOINT_MAX_DZ ||
+        p.stride < 1 || p.stride > DSM_VIEWPOINT_MAX_STRIDE || p.max_samples < 1 || p.max_samples > DSM_VIEWPOINT_MAX_SAMPLES ||
+        p.min_seen < 0 || p.top_k < 1 || p.top_k > DSM_VIEWPOINT_MAX_TOP_K || (p.with_reach != 0 && p.with_reach != 1) ||
+        !std::isfinite(p.radius) || !(p.radius >= 0.f))
+        return -1;
+    for (size_t i = 0; i < 9 * (size_t)n_rotations; i++)
+        if (!std::isfinite(rotations[i])) return -1;
+    for (int i = 0; i < n_clusters; i++)
+        if (clusters[i] < 0) return -1;
+    // the previous job's copy out of this staging ended before its wait, which no job in flight implies
+    const int n_offsets = viewpoint_offsets(p, reinterpret_cast<int32_t *>(vp.stage_host + vp_stage_offsets()));
+    if (n_offsets < 1 || (long long)n_clusters * n_offsets > vp.max_candidates ||
+        (long long)n_clusters * n_offsets * p.max_samples > DSM_VIEWPOINT_MAX_WORK)
+        return -1;
+    return n_offsets;
+}
+
+// The job on grid g after vp_args: the rotations and clusters staged, one H2D copy, the kernels with the candidates'
+// traversable test on (state, dist), the walk on the field's state grid walk_state, the error words of fhdr and the
+// latest frontier job's device result, then the enqueue's submit of the field request `request`
+template <typename Grid>
+static int vp_launch(dsm_ctx *ctx, DsmViewpoint &vp, const Grid &g, int ctas, const uint8_t *state, const int32_t *dist,
+                     const uint8_t *walk_state, const int32_t *fhdr, const DsmFrontier &fr, const uint32_t *cost, const dsm_gain_camera_t &c,
+                     const double *rotations, int n_rotations, const int32_t *clusters, int n_clusters, const dsm_viewpoint_params_t &p,
+                     int n_offsets, uint64_t request)
+{
+    CK(cudaSetDevice(ctx->device));
+    const cudaStream_t st = ctx->stream;
+    std::memcpy(vp.stage_host, rotations, 72 * (size_t)n_rotations);
+    if (n_clusters > 0) std::memcpy(vp.stage_host + vp_stage_clusters(), clusters, 4 * (size_t)n_clusters);
+    CK(cudaMemcpyAsync(vp.stage_dev, vp.stage_host, vp_stage_bytes(n_clusters), cudaMemcpyHostToDevice, st));
+    int32_t *hdr = reinterpret_cast<int32_t *>(vp.res);
+    auto *rec = reinterpret_cast<dsm_viewpoint_cluster_t *>(vp.res + 4 * DSM_VP_WORDS);
+    auto *out = reinterpret_cast<dsm_viewpoint_t *>(vp.res + vp_slots_at(n_clusters));
+    const auto *table = reinterpret_cast<const dsm_frontier_cluster_t *>(fr.res + DsmFrontier::table_at());
+    const int32_t *members = reinterpret_cast<const int32_t *>(fr.res + fr.list_at());
+    const double *rot = reinterpret_cast<const double *>(vp.stage_dev);
+    const int32_t *offsets = reinterpret_cast<const int32_t *>(vp.stage_dev + vp_stage_offsets());
+    k_vp_clusters<<<(unsigned)std::max((n_clusters + VP_BLOCK - 1) / VP_BLOCK, 1), VP_BLOCK, 0, st>>>(
+        g, fhdr, reinterpret_cast<const int32_t *>(fr.res), table, fr.max_clusters,
+        reinterpret_cast<const int32_t *>(vp.stage_dev + vp_stage_clusters()), n_clusters, n_offsets, n_rotations, p.top_k, c.unknown_blocks,
+        p.with_reach, p.max_samples, hdr, rec, vp.cl, vp.count);
+    if (n_clusters > 0)
+    {
+        k_vp_candidates<<<dim3((unsigned)((n_offsets + VP_BLOCK - 1) / VP_BLOCK), (unsigned)n_clusters), VP_BLOCK, 0, st>>>(
+            g, state, dist, offsets, n_offsets, p.radius, cost, vp.cl, rec, vp.key, vp.list, vp.count);
+        const double R = (double)c.max_range;
+        k_vp_score<<<(unsigned)ctas, VP_BLOCK, 0, st>>>(g, walk_state, rot, n_rotations, offsets, n_offsets, vp.cl, members, vp.list, vp.count,
+                                                        cost, c.fx, c.fy, c.cx, c.cy, (double)c.width, (double)c.height, R * R,
+                                                        c.unknown_blocks, p.min_seen, vp.key);
+        k_vp_select<<<(unsigned)n_clusters, VP_BLOCK, 0, st>>>(g, offsets, n_offsets, p.top_k, vp.cl, vp.key, rec, out);
+    }
+    CK(cudaGetLastError());
+    vp.n_clusters = n_clusters, vp.top_k = p.top_k;
+    return submit(ctx, vp, vp.res, vp_res_bytes(n_clusters, p.top_k), request);
+}
+
 // Enqueue only: the rotations, offsets and clusters staged and copied, the kernels on the grids of the latest (known)
 // field request, the latest frontier job's device result and (with_reach) the latest reach job's cost grid, one D2H copy
 // of the used result and the event.  Later field, frontier and reach requests overwrite those buffers only behind the
@@ -346,59 +462,42 @@ extern "C" int dsm_viewpoint_enqueue(dsm_ctx *ctx, const dsm_gain_camera_t *came
     if (!vp || !f || vp->in_flight) return DSM_E_STATE;
     const DsmFrontier *fr = ctx->frontier.get();
     if (!read_latest(fr, f)) return DSM_E_STATE;
-    if (!camera || !params || !rotations || n_rotations < 1 || n_rotations > DSM_VIEWPOINT_MAX_ROTATIONS || n_clusters < 0 ||
-        n_clusters > vp->max_clusters || (n_clusters > 0 && !clusters))
-        return DSM_E_INVALID;
-    const dsm_gain_camera_t &c = *camera;
-    const dsm_viewpoint_params_t &p = *params;
-    if (!gain_camera_ok(c, (double)f->g.voxel)) return DSM_E_INVALID;
-    if (p.r_min < 0 || p.r_min > p.r_max || p.r_max > DSM_VIEWPOINT_MAX_RADIUS || p.dz_max < 0 || p.dz_max > DSM_VIEWPOINT_MAX_DZ ||
-        p.stride < 1 || p.stride > DSM_VIEWPOINT_MAX_STRIDE || p.max_samples < 1 || p.max_samples > DSM_VIEWPOINT_MAX_SAMPLES ||
-        p.min_seen < 0 || p.top_k < 1 || p.top_k > DSM_VIEWPOINT_MAX_TOP_K || (p.with_reach != 0 && p.with_reach != 1) ||
-        !std::isfinite(p.radius) || !(p.radius >= 0.f))
-        return DSM_E_INVALID;
-    for (size_t i = 0; i < 9 * (size_t)n_rotations; i++)
-        if (!std::isfinite(rotations[i])) return DSM_E_INVALID;
-    for (int i = 0; i < n_clusters; i++)
-        if (clusters[i] < 0) return DSM_E_INVALID;
-    // the previous job's copy out of this staging ended before its wait, which no job in flight implies
-    const int n_offsets = viewpoint_offsets(p, reinterpret_cast<int32_t *>(vp->stage_host + vp_stage_offsets()));
-    if (n_offsets < 1 || (long long)n_clusters * n_offsets > vp->max_candidates ||
-        (long long)n_clusters * n_offsets * p.max_samples > DSM_VIEWPOINT_MAX_WORK)
-        return DSM_E_INVALID;
+    const int n_offsets = vp_args(*vp, camera, rotations, n_rotations, clusters, n_clusters, params, f->g.voxel);
+    if (n_offsets < 0) return DSM_E_INVALID;
     const DsmReach *re = ctx->reach.get();
-    if (p.with_reach && !read_latest(re, f)) return DSM_E_STATE;
-    CK(cudaSetDevice(ctx->device));
-    const cudaStream_t st = ctx->stream;
-    std::memcpy(vp->stage_host, rotations, 72 * (size_t)n_rotations);
-    if (n_clusters > 0) std::memcpy(vp->stage_host + vp_stage_clusters(), clusters, 4 * (size_t)n_clusters);
-    CK(cudaMemcpyAsync(vp->stage_dev, vp->stage_host, vp_stage_bytes(n_clusters), cudaMemcpyHostToDevice, st));
-    const DsmFieldGrid &g = f->g;
-    int32_t *hdr = reinterpret_cast<int32_t *>(vp->res);
-    auto *rec = reinterpret_cast<dsm_viewpoint_cluster_t *>(vp->res + 4 * DSM_VP_WORDS);
-    auto *out = reinterpret_cast<dsm_viewpoint_t *>(vp->res + vp_slots_at(n_clusters));
-    const auto *table = reinterpret_cast<const dsm_frontier_cluster_t *>(fr->res + DsmFrontier::table_at());
-    const int32_t *members = reinterpret_cast<const int32_t *>(fr->res + fr->list_at());
-    const double *rot = reinterpret_cast<const double *>(vp->stage_dev);
-    const int32_t *offsets = reinterpret_cast<const int32_t *>(vp->stage_dev + vp_stage_offsets());
-    const uint32_t *cost = p.with_reach ? re->cost[0] : nullptr;
-    k_vp_clusters<<<(unsigned)std::max((n_clusters + VP_BLOCK - 1) / VP_BLOCK, 1), VP_BLOCK, 0, st>>>(
-        g, f->dist + dsm_field_header(f->voxels), reinterpret_cast<const int32_t *>(fr->res), table, fr->max_clusters,
-        reinterpret_cast<const int32_t *>(vp->stage_dev + vp_stage_clusters()), n_clusters, n_offsets, n_rotations, p.top_k, c.unknown_blocks,
-        p.with_reach, p.max_samples, hdr, rec, vp->cl, vp->count);
-    if (n_clusters > 0)
-    {
-        k_vp_candidates<<<dim3((unsigned)((n_offsets + VP_BLOCK - 1) / VP_BLOCK), (unsigned)n_clusters), VP_BLOCK, 0, st>>>(
-            g, f->occ, f->dist, offsets, n_offsets, p.radius, cost, vp->cl, rec, vp->key, vp->list, vp->count);
-        const double R = (double)c.max_range;
-        k_vp_score<<<(unsigned)vp->ctas, VP_BLOCK, 0, st>>>(g, f->occ, rot, n_rotations, offsets, n_offsets, vp->cl, members, vp->list, vp->count,
-                                                            cost, c.fx, c.fy, c.cx, c.cy, (double)c.width, (double)c.height, R * R,
-                                                            c.unknown_blocks, p.min_seen, vp->key);
-        k_vp_select<<<(unsigned)n_clusters, VP_BLOCK, 0, st>>>(g, offsets, n_offsets, p.top_k, vp->cl, vp->key, rec, out);
-    }
-    CK(cudaGetLastError());
-    vp->n_clusters = n_clusters, vp->top_k = p.top_k;
-    return submit(ctx, *vp, vp->res, vp_res_bytes(n_clusters, p.top_k), f->requests);
+    if (params->with_reach && !read_latest(re, f)) return DSM_E_STATE;
+    return vp_launch(ctx, *vp, f->g, vp->ctas, f->occ, f->dist, f->occ, f->dist + dsm_field_header(f->voxels), *fr,
+                     params->with_reach ? re->cost[0] : nullptr, *camera, rotations, n_rotations, clusters, n_clusters, *params, n_offsets,
+                     f->requests);
+}
+
+// Enqueue only: the job of dsm_viewpoint_enqueue on the plane of the latest terrain job (DESIGN.md §8.23), with the
+// camera eye voxels above each candidate cell's support, in stream order behind that job.  The walk reads the field's
+// state grid, so the latest field request must be the one the terrain job read; later field, terrain, frontier and
+// reach requests overwrite what the job reads only behind it.
+extern "C" int dsm_viewpoint_enqueue_terrain(dsm_ctx *ctx, const dsm_gain_camera_t *camera, const double *rotations, int n_rotations,
+                                             const int32_t *clusters, int n_clusters, const dsm_viewpoint_params_t *params, int eye)
+{
+    if (!ctx) return DSM_E_INVALID;
+    DsmViewpoint *vp = ctx->viewpoint.get();
+    const DsmTerrain *tr = ctx->terrain.get();
+    if (!vp || !tr || tr->request == 0 || tr->request != ctx->field->requests || vp->in_flight) return DSM_E_STATE;
+    const DsmField *f = ctx->field.get();
+    const DsmFrontier *fr = ctx->frontier.get();
+    if (!(fr && fr->request == tr->request)) return DSM_E_STATE;
+    const int n_offsets = vp_args(*vp, camera, rotations, n_rotations, clusters, n_clusters, params, f->g.voxel);
+    if (n_offsets < 0 || params->dz_max != 0 || eye < 1 || eye > tr->headroom) return DSM_E_INVALID;
+    const DsmReach *re = ctx->reach.get();
+    if (params->with_reach && !(re && re->terrain == tr->enqueues)) return DSM_E_STATE;
+    const int cells = tr->cells;
+    VpTerrainGrid g;
+    static_cast<ReachTerrainGrid &>(g) = reach_terrain_grid(f->g, *tr);
+    g.level = reinterpret_cast<const int16_t *>(tr->res + DsmTerrain::level_at(cells));
+    g.du = tr->up > 0 ? eye : -eye;
+    return vp_launch(ctx, *vp, g, vp->ctas_terrain, tr->res + DsmTerrain::status_at(cells), reinterpret_cast<const int32_t *>(tr->res),
+                     f->occ, reinterpret_cast<const int32_t *>(tr->res + DsmTerrain::header_at(cells)), *fr,
+                     params->with_reach ? re->cost[0] : nullptr, *camera, rotations, n_rotations, clusters, n_clusters, *params, n_offsets,
+                     tr->request);
 }
 
 extern "C" int dsm_viewpoint_wait(dsm_ctx *ctx, dsm_viewpoint_info_t *info, const dsm_viewpoint_cluster_t **clusters,

@@ -932,7 +932,8 @@ int dsm_reach_wait(dsm_ctx *ctx, dsm_reach_info_t *info, const dsm_reach_target_
  *                              read the field request the latest terrain job read.  DSM_E_INVALID exactly as
  *                              dsm_reach_enqueue.  dsm_reach_wait's *cost then holds m0 m1 m2 cells, and it returns
  *                              DSM_E_CAPACITY when the terrain job's field was taken after a rejected frame.  The job
- *                              reads no field request, so a viewpoint job's with_reach refuses its cost grid. */
+ *                              reads no field request, so a field viewpoint job's with_reach refuses its cost grid; a
+ *                              terrain viewpoint job's (§8.23) takes it while the job ran on the latest terrain job. */
 int dsm_reach_enqueue_terrain(dsm_ctx *ctx, const double start[3], float radius, int approach, const double *goals, int n_goals,
                               int with_frontiers, int host_copy);
 
@@ -1243,6 +1244,39 @@ int dsm_viewpoint_enqueue(dsm_ctx *ctx, const dsm_gain_camera_t *camera, const d
                           const int32_t *clusters, int n_clusters, const dsm_viewpoint_params_t *params);
 int dsm_viewpoint_wait(dsm_ctx *ctx, dsm_viewpoint_info_t *info, const dsm_viewpoint_cluster_t **clusters,
                        const dsm_viewpoint_t **viewpoints);
+
+/* ---- viewpoints of a ground robot: the viewpoint job on the latest terrain job's plane (DESIGN.md §8.23) ----
+ * A terrain viewpoint job is the viewpoint job above run on the plane of the latest terrain job (§8.20), as the terrain
+ * reach job (§8.21) runs the reach job there: in stream order behind that job, which may still be in flight.  It uses
+ * the viewpoint job's buffers, enable, header, records, slots and wait, and allocates nothing.  Its camera stands on the
+ * ground: eye voxels above the support of each candidate cell.  Everything not restated here is §8.15's; statuses,
+ * samples, scoring, ranking, top_k and the layouts are unchanged.
+ *   Plane: §8.21's, the plane (P, Q, 1) at the terrain job's origin o and voxel edge v, cells in the linear order
+ *   q P + p, p and q the lower and higher in-plane axes h0 < h1.  A slot's voxel is a cell; the header's origin is the
+ *   terrain job's.
+ *   Centre cell: reach's start snap of the table's fp64 centroid on the two in-plane axes, floor(centroid_h / v) - o_h:
+ *   the centroid's column.
+ *   Offsets: §8.15's enumeration with dz_max = 0 (other values are refused); offset (dx, dy) moves along (p, q).
+ *   Candidates: c = g + offset inside the plane and traversable, status 2 and clearance >= radius (dsm_traversable on
+ *   the status and clearance planes, as §8.21); with with_reach also of finite cost in the latest reach job, which must
+ *   be a terrain reach job on the latest terrain job, that cost being recorded.
+ *   Camera: at the field voxel whose in-plane coordinates are the cell's (p, q) and whose coordinate along the up axis
+ *   a is u = level[c] + eye for a positive up and level[c] - eye for a negative one; t_k = ((double)(o_k + voxel_k) +
+ *   0.5) v.  With eye in [1, headroom] of the terrain job, that voxel lies in the grid and is free (the support's
+ *   definition), and the camera is (eye - 1/2) v above the support's top face.
+ *   Score: §8.15's, with gain's frustum test and walk through the state grid of the field request the terrain job read.
+ *   With every member sampled seen[r] equals the n_cluster of a gain job on the pose [R_r | t] naming the cluster.
+ *
+ *   dsm_viewpoint_enqueue_terrain  as dsm_viewpoint_enqueue.  DSM_E_STATE before dsm_viewpoint_enable, with no terrain
+ *                                  job yet, when the latest field request is not the one the latest terrain job read,
+ *                                  while a viewpoint job is in flight, when the latest frontier job did not read that
+ *                                  request, and with with_reach unless the latest reach job is a terrain reach job on
+ *                                  the latest terrain job.  DSM_E_INVALID exactly as dsm_viewpoint_enqueue, and for
+ *                                  dz_max != 0 or eye outside [1, headroom].  dsm_viewpoint_wait returns DSM_E_CAPACITY
+ *                                  when the terrain job's field was taken after a rejected frame.  Terrain and field
+ *                                  viewpoint jobs may alternate on one context. */
+int dsm_viewpoint_enqueue_terrain(dsm_ctx *ctx, const dsm_gain_camera_t *camera, const double *rotations, int n_rotations,
+                                  const int32_t *clusters, int n_clusters, const dsm_viewpoint_params_t *params, int eye);
 
 /* ---- headings along trajectories: view gain per sample and rotation, then the best rate-limited sequence (DESIGN.md §8.19) ----
  * A heading job reads the state grid of the latest field request, which must be a known one, in stream order behind

@@ -110,8 +110,9 @@
 // surface of every column of the latest fused frame's known field along the up axis on the device (DESIGN.md §8.20):
 // its level, the step to its neighbours, whether it is traversable and the clearance to the nearest cell that is not,
 // one enqueue and one wait.  A ground planner's exploration chain runs on that plane: terrain(), then frontiers(), then
-// reach_terrain(with_frontiers) from the robot for each cluster's viewpoint cell (DESIGN.md §8.21), then
-// reach_matrix_terrain over the robot's position and the viewpoint cells' centres (§8.22), then tour() on that matrix.
+// reach_terrain(with_frontiers) from the robot (DESIGN.md §8.21), then viewpoints_terrain(with_reach) for the cells whose
+// camera, eye voxels above the ground, would see each cluster best (§8.23), then reach_matrix_terrain over the robot's
+// position and those cameras (§8.22), then tour() on that matrix.
 // device < 0 builds the node without a context: the callbacks run the whole pose logic (pose database, sync, window
 // bookkeeping) and fuse nothing; any call that reads the map returns DSM_E_STATE.
 #pragma once
@@ -742,6 +743,39 @@ class SurfelMapNode
         return job(
             "viewpoints", KNOWN_FIELD, true,
             [&] { return dsm_viewpoint_enqueue(ctx_.ctx, &cam, rotations, n_rotations, clusters.data(), (int)clusters.size(), &params); },
+            [&] { return dsm_viewpoint_wait(ctx_.ctx, &info, &c, &v); },
+            [&] {
+                cluster_records.assign(c, c + info.n_clusters);
+                viewpoints.assign(v, v + (size_t)info.n_clusters * info.top_k);
+            });
+    }
+    // ---- viewpoints of a ground robot on the terrain of the latest fused frame (DESIGN.md §8.23) ----
+    // viewpoints() on the plane of the terrain() call on this frame, with params.dz_max 0: candidate cells around each
+    // cluster's column, traversable at least `radius` from any other cell, each camera `eye` voxels above the cell's
+    // support (eye in [1, headroom] of that terrain() call); with_reach ranks by the costs of the reach_terrain() call on
+    // that terrain.  Slot voxels are cells q P + p of the terrain grid; the camera's field voxel is the cell's column at
+    // level + eye (up > 0) or level - eye (up < 0), and its centre, snapped to its column, is the cell's site for
+    // reach_matrix_terrain().  DSM_E_STATE without a terrain() call on this frame, without a frontiers() call since the
+    // frame was fused, with with_reach without a reach_terrain() call on that terrain, and after load_state* until the
+    // next fused frame; DSM_E_CAPACITY with the viewpoints of the last applied frame's terrain.
+    int viewpoints_terrain(dsm_viewpoint_params_t params, int eye, const double *rotations, int n_rotations, float max_range,
+                           int unknown_blocks, const std::vector<int32_t> &clusters, int with_reach, dsm_viewpoint_info_t &info,
+                           std::vector<dsm_viewpoint_cluster_t> &cluster_records, std::vector<dsm_viewpoint_t> &viewpoints)
+    {
+        cluster_records.clear();
+        viewpoints.clear();
+        info = dsm_viewpoint_info_t();
+        const dsm_gain_camera_t cam = gain_camera(max_range, unknown_blocks);
+        params.with_reach = with_reach;
+        const dsm_viewpoint_cluster_t *c = nullptr;
+        const dsm_viewpoint_t *v = nullptr;
+        return job(
+            "viewpoints_terrain", KNOWN_FIELD, true,
+            [&] {
+                return terrain_frame_ ? dsm_viewpoint_enqueue_terrain(ctx_.ctx, &cam, rotations, n_rotations, clusters.data(),
+                                                                      (int)clusters.size(), &params, eye)
+                                      : DSM_E_STATE;
+            },
             [&] { return dsm_viewpoint_wait(ctx_.ctx, &info, &c, &v); },
             [&] {
                 cluster_records.assign(c, c + info.n_clusters);
